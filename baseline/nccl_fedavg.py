@@ -1,4 +1,4 @@
-"""NCCL + cuBLAS/cuDNN baseline ("the reference's own NCCL build", BASELINE.json / BASELINE.md).
+"""NCCL + cuBLAS/cuDNN baseline ("the reference's own NCCL build").
 
 A faithful re-expression of the reference ALGORITHM with stock components only -- nothing from
 ``baton_b200`` is imported:

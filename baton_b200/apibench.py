@@ -101,7 +101,7 @@ def main_http(args, emit) -> int:
                                 backend=args.backend, wire_dtype=args.wire, port=wport, heartbeat_time=600,
                                 worker_host="http://127.0.0.1:{}/{}/".format(wport, name),
                                 train_kwargs={"lr": args.lr, "batch_size": args.batch_size},
-                                n_ctas=min(args.n_ctas, 148))     # one CTA per SM: slack for foreign kernels
+                                n_ctas=min(args.n_ctas, 132))     # one CTA per SM: slack for foreign kernels
         runner = web.AppRunner(app)
         await runner.setup()
         await web.TCPSite(runner, "127.0.0.1", wport).start()

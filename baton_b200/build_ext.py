@@ -1,10 +1,11 @@
-"""In-tree build of the sm_100a extension ``baton_b200/_C.so``.
+"""In-tree build of the sm_90a extension ``baton_b200/_C.so``.
 
-``nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo`` per ``.cu`` (the
+``nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo`` per ``.cu`` (the
 kernels include no PyTorch header, so each file compiles in seconds), ``g++`` for
 ``bindings.cpp`` against the PyTorch headers, one shared object linked in-tree
 so it travels to the GPU box with the repo snapshot.  Incremental: a file is
-recompiled only when it (or a header) is newer than its object.
+recompiled only when it (or a header) is newer than its object; everything is rebuilt when the compiler, the
+flags or the PyTorch version differ from those recorded next to the objects.
 
     python -m baton_b200.build_ext [--force] [--verbose]
 """
@@ -26,9 +27,9 @@ if TRACE:
     BUILD = os.path.join(HERE, "csrc", "build_trace")
 TARGET = os.path.join(HERE, "_C_trace.so" if TRACE else "_C.so")
 
-CU_SOURCES = ["gemm_tcgen05.cu", "gemm_fp8.cu", "quant.cu", "attention.cu", "im2col_tma.cu", "gemm_simt.cu", "fedavg.cu", "elementwise.cu", "conv.cu", "norm.cu", "loss.cu"]
+CU_SOURCES = ["gemm_wgmma.cu", "gemm_fp8.cu", "quant.cu", "attention.cu", "im2col_tma.cu", "gemm_simt.cu", "fedavg.cu", "elementwise.cu", "conv.cu", "norm.cu", "loss.cu"]
 HEADERS = ["ptx.cuh", "launch.h", "pdl.cuh", "mx.cuh"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math", "-Xptxas", "-v"]
 if os.environ.get("BATON_BUILD_PHASE_TIMING") == "1":     # in-kernel %globaltimer stamps in the FedAvg collective
     NVCC_FLAGS.append("-DB200_FEDAVG_PHASE_TIMING")
@@ -68,6 +69,12 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     os.makedirs(BUILD, exist_ok=True)
     nvcc = _nvcc()
+    # objects record the compiler and flags they were built with: a tree built for another architecture (or with
+    # other defines) is rebuilt from scratch instead of being relinked because its sources look older
+    stamp = os.path.join(BUILD, "flags.txt")
+    want = "\n".join([nvcc] + NVCC_FLAGS + [torch.__version__]) + "\n"
+    if not force and (not os.path.exists(stamp) or open(stamp).read() != want):
+        force = True
     headers = [os.path.join(CSRC, h) for h in HEADERS]
     t0 = time.time()
     jobs = []
@@ -100,6 +107,8 @@ def build(force: bool = False, verbose: bool = False) -> str:
             "-L" + torch_lib, "-L" + cuda_lib, "-lc10", "-lc10_cuda", "-ltorch_cpu", "-ltorch_cuda", "-ltorch",
             "-ltorch_python", "-lcudart", "-Wl,-rpath," + torch_lib, "-Wl,--no-as-needed"]
         _run(link, verbose)
+    with open(stamp, "w") as fh:
+        fh.write(want)
     if verbose:
         print("built {} in {:.1f}s ({} compile steps)".format(TARGET, time.time() - t0, len(jobs)))
     return TARGET

@@ -4,7 +4,7 @@ The reference has no config system: three positional argv (demo.py:64-66) and
 constructor defaults -- ``client_ttl=300`` (manager.py:22), ``heartbeat_time=60``,
 ``port=8080`` (worker.py:13-14), ``n_epoch=32`` (manager.py:55), ``lr=0.001,
 batch_size=32`` (demo.py:29).  Those defaults are preserved here and extended
-with the knobs the BASELINE.json configs need.
+with the knobs the benchmark configurations need.
 """
 from __future__ import annotations
 

@@ -2,7 +2,7 @@
 
 ``GpuExperimentWorker`` is an :class:`ExperimentWorker` (reference worker.py:12-127: register,
 heartbeat, ``round_start`` -> local training -> ``report_update``) whose model lives in a flat
-parameter arena on one B200 and whose uploads/downloads never touch HTTP: the POSTs carry metadata
+parameter arena on one GPU and whose uploads/downloads never touch HTTP: the POSTs carry metadata
 only and the round-end reduce + broadcast is the fused NVLink kernel, launched on every seat when
 the manager sends the aggregation plan (``POST /{name}/aggregate``).
 

@@ -2,18 +2,16 @@
 // sequence length 128):   P = softmax(scale * Q K^T)   O = P V
 //
 //   TMA   Q [128 x 64], K [128 x 64] (K-major operands), V [128 keys x 64] (MN-major B operand) -> smem
-//   MMA 1 S = Q K^T            tcgen05.mma 128 x 128 x 64  -> TMEM columns [0, 128)
-//   softmax: TMEM lane == query row, so each of the 128 epilogue threads owns one full row -- row max and
-//            row sum need no shuffles.  Three cheap passes over TMEM keep the register count low enough
-//            for several CTAs per SM: (A) max, (B) exp -> un-normalised bf16 P~ written to shared memory in
-//            the 128B-swizzled K-major layout tcgen05 expects for an A operand, row sum; (C) normalised P
-//            to global memory (saved for backward) while MMA 2 already runs.
-//   MMA 2 O~ = P~ V            tcgen05.mma 128 x 64 x 128  -> TMEM columns [128, 192)
+//   MMA 1 S = Q K^T            wgmma, two consumer warpgroups x (64 x 128 x 64)  -> fp32 tile in shared memory
+//   softmax: one thread per query row reads its row of the staged tile -- row max and row sum need no shuffles:
+//            (A) max, (B) exp -> un-normalised bf16 P~ written to shared memory in the 128B-swizzled K-major layout
+//            wgmma expects for an A operand, row sum; (C) normalised P to global memory (saved for backward).
+//   MMA 2 O~ = P~ V            wgmma, two warpgroups x (64 x 64 x 128)  -> fp32 tile in shared memory
 //   epilogue O = O~ / rowsum   -> out[b*S + q, h*64 : h*64+64]
 //
 // The S x S scores never touch HBM and P is written exactly once (the unfused path writes S, reads S,
-// writes P, reads P).  Validated on B200 in round 2 (tests/test_gpu_bert.py, profiles/r2_validate_experimental.txt)
-// and the default since it measured +4.6 % on the BERT-base round (BATON_FUSED_ATTN=0 selects the three-kernel path).
+// writes P, reads P).  The default (BATON_FUSED_ATTN=0 selects the three-kernel path); tests/test_gpu_bert.py
+// checks both against an fp32 reference.
 #define B200_TU_TAG 4
 #include "launch.h"
 #include "pdl.cuh"
@@ -27,10 +25,14 @@ namespace b200 {
 
 constexpr int AT_S = 128;      // queries == keys per CTA
 constexpr int AT_D = 64;       // head dimension
-constexpr int AT_THREADS = 256;
+constexpr int AT_THREADS = 384;                    // warpgroup 0: TMA producer; warpgroups 1, 2: wgmma + softmax
+constexpr int AT_CONSUMERS = 256;
 constexpr int AT_Q_BYTES = AT_S * AT_D * 2;        // 16 KB, K-major, 128 B rows
 constexpr int AT_P_BYTES = AT_S * AT_S * 2;        // 32 KB = two 64-key k-tiles of 16 KB
-constexpr int AT_TMEM_COLS = 256;                  // S: [0,128)  O: [128,192)
+constexpr int AT_SP = AT_S + 4;                    // fp32 pitch of a staged 128-column tile (skews banks)
+constexpr int AT_OP = AT_D + 4;                    // fp32 pitch of a staged 64-column tile
+constexpr int AT_WIDE_BYTES = AT_S * AT_SP * 4;
+constexpr int AT_NARROW_BYTES = AT_S * AT_OP * 4;
 
 struct AttnParams {
   __nv_bfloat16* out;      // [B*S, D]
@@ -39,7 +41,7 @@ struct AttnParams {
   float scale_log2e;       // softmax scale * log2(e)
 };
 
-__global__ void __launch_bounds__(AT_THREADS, 2)
+__global__ void __launch_bounds__(AT_THREADS, 1)
 attention_fwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                           const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -48,11 +50,9 @@ attention_fwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
   uint8_t* sK = sQ + AT_Q_BYTES;
   uint8_t* sV = sK + AT_Q_BYTES;
   uint8_t* sP = sV + AT_Q_BYTES;
-  uint64_t* bar_load = reinterpret_cast<uint64_t*>(sP + AT_P_BYTES);
-  uint64_t* bar_s = bar_load + 1;      // S = Q K^T complete
-  uint64_t* bar_p = bar_load + 2;      // P~ written to shared memory (4 arrivals: one per softmax warp)
-  uint64_t* bar_o = bar_load + 3;      // O~ complete
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_load + 4);
+  float* sS = reinterpret_cast<float*>(sP + AT_P_BYTES);                 // scores, fp32 [128][AT_SP]
+  float* sO = reinterpret_cast<float*>(sP + AT_P_BYTES + AT_WIDE_BYTES); // O~, fp32 [128][AT_OP]
+  uint64_t* bar_load = reinterpret_cast<uint64_t*>(sP + AT_P_BYTES + AT_WIDE_BYTES + AT_NARROW_BYTES);
 
   griddep_launch_dependents();
   const int warp = threadIdx.x >> 5;
@@ -63,22 +63,10 @@ attention_fwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
-  }
-  if (warp == 1 && elect_one()) {
     mbar_init(bar_load, 1);
-    mbar_init(bar_s, 1);
-    mbar_init(bar_p, 4);
-    mbar_init(bar_o, 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, AT_TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   griddep_wait();
 
   if (warp == 0) {
@@ -89,135 +77,139 @@ attention_fwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
       tma_load_4d(sV, &tmV, bar_load, 0, 0, h, b);                 // box [64 d][64 keys]  (MN-major atom 0)
       tma_load_4d(sV + 8192, &tmV, bar_load, 0, 64, h, b);         // keys 64..127
     }
-  } else if (warp == 1) {
+  } else if (warp >= 4) {
+    const int ew = warp - 4, g = ew >> 2;                          // warpgroup g computes query rows 64 g .. 64 g + 63
     mbar_wait(bar_load, 0);
-    tc_fence_after();
-    if (elect_one()) {
-      const uint32_t idesc1 = umma_idesc_bf16(AT_S, AT_S, 0, 0);
-      const uint32_t q = smem_u32(sQ), k = smem_u32(sK);
+    {
+      // MMA 1: S = Q K^T (both K-major)
+      float acc[64];
+#pragma unroll
+      for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+      const uint32_t q = smem_u32(sQ) + g * 8192, k = smem_u32(sK);
+      wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < AT_D / 16; ++kk)
-        tc_mma_f16(tmem_base, umma_smem_desc_sw128(q + kk * 32, 16, 1024), umma_smem_desc_sw128(k + kk * 32, 16, 1024),
-                   idesc1, kk != 0);
-      tc_commit(bar_s);
+        wgmma_bf16_n128<0, 0>(acc, gmma_desc_sw128(q + kk * 32, 16, 1024), gmma_desc_sw128(k + kk * 32, 16, 1024), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_operands(acc);
+      wg_store_acc<128>(acc, sS, AT_SP, 64 * g);
     }
-    __syncwarp();
-    mbar_wait(bar_p, 0);
-    tc_fence_after();
-    if (elect_one()) {
-      const uint32_t idesc2 = umma_idesc_bf16(AT_S, AT_D, 0, 1);       // B = V is MN-major (d contiguous)
-      const uint32_t pp = smem_u32(sP), v = smem_u32(sV);
+    named_bar_sync(1, AT_CONSUMERS);
+    // softmax: thread == query row (warps 4..7), row max and row sum need no shuffles
+    const int lane = static_cast<int>(lane_id());
+    const int r = (ew & 3) * 32 + lane;
+    const float* srow = sS + r * AT_SP;
+    float mb = 0.f, inv = 0.f;
+    if (ew < 4) {
+      // pass A: row maximum
+      float m = -INFINITY;
+#pragma unroll 1
+      for (int c = 0; c < AT_S; c += 32) {
+        uint32_t x[32];
+        acc_ld_row32(srow + c, x);
+#pragma unroll
+        for (int j = 0; j < 32; ++j) m = fmaxf(m, __uint_as_float(x[j]));
+      }
+      mb = m * p.scale_log2e;
+      // pass B: P~ = exp2(scale*log2e*x - mb) -> bf16 -> swizzled shared memory (K-major A operand); row sum
+      float sum = 0.f;
+      uint8_t* prow = sP + r * 128;
+#pragma unroll 1
+      for (int c = 0; c < AT_S; c += 32) {
+        uint32_t x[32];
+        acc_ld_row32(srow + c, x);
+        float e[32];
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          e[j] = exp2f(fmaf(__uint_as_float(x[j]), p.scale_log2e, -mb));
+          sum += e[j];
+        }
+        uint8_t* tile = prow + (c >> 6) * 16384;                     // 64-key k-tile
+#pragma unroll
+        for (int j = 0; j < 32; j += 8) {
+          const int chunk = ((c & 63) + j) >> 3;                     // 16-byte chunk inside the 128-byte row
+          *reinterpret_cast<uint4*>(tile + ((chunk ^ (r & 7)) << 4)) =
+              make_uint4(pack_bf16x2(e[j], e[j + 1]), pack_bf16x2(e[j + 2], e[j + 3]), pack_bf16x2(e[j + 4], e[j + 5]),
+                         pack_bf16x2(e[j + 6], e[j + 7]));
+        }
+      }
+      inv = 1.f / sum;
+      fence_proxy_async();          // generic-proxy smem writes -> visible to the tensor core (async proxy)
+    }
+    named_bar_sync(1, AT_CONSUMERS);
+    {
+      // MMA 2: O~ = P~ V   (A = P~ K-major in two 64-key halves, B = V MN-major: d contiguous)
+      float acc[32];
+#pragma unroll
+      for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+      const uint32_t pp = smem_u32(sP) + g * 8192, v = smem_u32(sV);
+      wgmma_fence();
 #pragma unroll
       for (int kt = 0; kt < 2; ++kt)
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk)
-          tc_mma_f16(tmem_base + AT_S, umma_smem_desc_sw128(pp + kt * 16384 + kk * 32, 16, 1024),
-                     umma_smem_desc_sw128(v + kt * 8192 + kk * 2048, 8192, 1024), idesc2, (kt | kk) != 0);
-      tc_commit(bar_o);
+          wgmma_bf16_n64<0, 1>(acc, gmma_desc_sw128(pp + kt * 16384 + kk * 32, 16, 1024),
+                               gmma_desc_sw128(v + kt * 8192 + kk * 2048, 8192, 1024), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_operands(acc);
+      wg_store_acc<64>(acc, sO, AT_OP, 64 * g);
     }
-    __syncwarp();
-  } else if (warp >= 4) {
-    const int q = warp & 3;
-    const int lane = static_cast<int>(lane_id());
-    const int r = q * 32 + lane;                                   // query row == TMEM lane
-    const uint32_t t_row = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    mbar_wait(bar_s, 0);
-    tc_fence_after();
-    // pass A: row maximum
-    float m = -INFINITY;
+    named_bar_sync(1, AT_CONSUMERS);
+    if (ew < 4) {
+      // normalised probabilities to global memory (saved for backward)
+      __nv_bfloat16* grow = p.probs + (static_cast<size_t>(bh) * AT_S + r) * AT_S;
 #pragma unroll 1
-    for (int c = 0; c < AT_S; c += 32) {
-      uint32_t x[32];
-      tmem_ld_32x32b_x32(t_row + c, x);
-      tmem_ld_wait();
+      for (int c = 0; c < AT_S; c += 32) {
+        uint32_t x[32];
+        acc_ld_row32(srow + c, x);
+        float e[32];
 #pragma unroll
-      for (int j = 0; j < 32; ++j) m = fmaxf(m, __uint_as_float(x[j]));
-    }
-    const float mb = m * p.scale_log2e;
-    // pass B: P~ = exp2(scale*log2e*x - mb) -> bf16 -> swizzled shared memory; row sum
-    float sum = 0.f;
-    uint8_t* prow = sP + r * 128;
-#pragma unroll 1
-    for (int c = 0; c < AT_S; c += 32) {
-      uint32_t x[32];
-      tmem_ld_32x32b_x32(t_row + c, x);
-      tmem_ld_wait();
-      float e[32];
+        for (int j = 0; j < 32; ++j) e[j] = exp2f(fmaf(__uint_as_float(x[j]), p.scale_log2e, -mb)) * inv;
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        e[j] = exp2f(fmaf(__uint_as_float(x[j]), p.scale_log2e, -mb));
-        sum += e[j];
+        for (int j = 0; j < 32; j += 8)
+          *reinterpret_cast<uint4*>(grow + c + j) =
+              make_uint4(pack_bf16x2(e[j], e[j + 1]), pack_bf16x2(e[j + 2], e[j + 3]), pack_bf16x2(e[j + 4], e[j + 5]),
+                         pack_bf16x2(e[j + 6], e[j + 7]));
       }
-      uint8_t* tile = prow + (c >> 6) * 16384;                     // 64-key k-tile
+      // epilogue: O = O~ / rowsum
+      __nv_bfloat16* orow = p.out + (static_cast<size_t>(b) * AT_S + r) * p.D + h * AT_D;
+#pragma unroll 1
+      for (int c = 0; c < AT_D; c += 32) {
+        uint32_t x[32];
+        acc_ld_row32(sO + r * AT_OP + c, x);
 #pragma unroll
-      for (int j = 0; j < 32; j += 8) {
-        const int chunk = ((c & 63) + j) >> 3;                     // 16-byte chunk inside the 128-byte row
-        *reinterpret_cast<uint4*>(tile + ((chunk ^ (r & 7)) << 4)) =
-            make_uint4(pack_bf16x2(e[j], e[j + 1]), pack_bf16x2(e[j + 2], e[j + 3]), pack_bf16x2(e[j + 4], e[j + 5]),
-                       pack_bf16x2(e[j + 6], e[j + 7]));
+        for (int j = 0; j < 32; j += 8)
+          *reinterpret_cast<uint4*>(orow + c + j) =
+              make_uint4(pack_bf16x2(__uint_as_float(x[j]) * inv, __uint_as_float(x[j + 1]) * inv),
+                         pack_bf16x2(__uint_as_float(x[j + 2]) * inv, __uint_as_float(x[j + 3]) * inv),
+                         pack_bf16x2(__uint_as_float(x[j + 4]) * inv, __uint_as_float(x[j + 5]) * inv),
+                         pack_bf16x2(__uint_as_float(x[j + 6]) * inv, __uint_as_float(x[j + 7]) * inv));
       }
-    }
-    fence_proxy_async_all();          // generic-proxy smem writes -> visible to the tensor core (async proxy)
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bar_p);
-    const float inv = 1.f / sum;
-    // pass C: normalised probabilities to global memory (overlaps MMA 2)
-    __nv_bfloat16* grow = p.probs + (static_cast<size_t>(bh) * AT_S + r) * AT_S;
-#pragma unroll 1
-    for (int c = 0; c < AT_S; c += 32) {
-      uint32_t x[32];
-      tmem_ld_32x32b_x32(t_row + c, x);
-      tmem_ld_wait();
-      float e[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) e[j] = exp2f(fmaf(__uint_as_float(x[j]), p.scale_log2e, -mb)) * inv;
-#pragma unroll
-      for (int j = 0; j < 32; j += 8)
-        *reinterpret_cast<uint4*>(grow + c + j) =
-            make_uint4(pack_bf16x2(e[j], e[j + 1]), pack_bf16x2(e[j + 2], e[j + 3]), pack_bf16x2(e[j + 4], e[j + 5]),
-                       pack_bf16x2(e[j + 6], e[j + 7]));
-    }
-    // epilogue: O = O~ / rowsum
-    mbar_wait(bar_o, 0);
-    tc_fence_after();
-    __nv_bfloat16* orow = p.out + (static_cast<size_t>(b) * AT_S + r) * p.D + h * AT_D;
-#pragma unroll 1
-    for (int c = 0; c < AT_D; c += 32) {
-      uint32_t x[32];
-      tmem_ld_32x32b_x32(t_row + AT_S + c, x);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 32; j += 8)
-        *reinterpret_cast<uint4*>(orow + c + j) =
-            make_uint4(pack_bf16x2(__uint_as_float(x[j]) * inv, __uint_as_float(x[j + 1]) * inv),
-                       pack_bf16x2(__uint_as_float(x[j + 2]) * inv, __uint_as_float(x[j + 3]) * inv),
-                       pack_bf16x2(__uint_as_float(x[j + 4]) * inv, __uint_as_float(x[j + 5]) * inv),
-                       pack_bf16x2(__uint_as_float(x[j + 6]) * inv, __uint_as_float(x[j + 7]) * inv));
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, AT_TMEM_COLS);
 }
 
 
 // ---- backward, same tiling: one CTA per (batch, head), S = 128, d = 64 ------------------------------------------
-//   dV = P^T dO          (A = P^T  MN-major view of the K-major P tile, B = dO MN-major)      -> TMEM [128,192)
-//   dP = dO V^T          (A = dO K-major, B = V K-major)                                       -> TMEM [0,128)
+//   dV = P^T dO          (A = P^T  MN-major view of the K-major P tile, B = dO MN-major)
+//   dP = dO V^T          (A = dO K-major, B = V K-major)
 //   dS = P o (dP - rowsum(dP o P))      thread == query row; written IN PLACE over P in shared memory
-//   dQ = scale * dS K    (A = dS K-major, B = K MN-major)                                      -> TMEM [0,64)
-//   dK = scale * dS^T Q  (A = dS^T MN-major view of the same tile, B = Q MN-major)             -> TMEM [64,128)
+//   dQ = scale * dS K    (A = dS K-major, B = K MN-major)
+//   dK = scale * dS^T Q  (A = dS^T MN-major view of the same tile, B = Q MN-major)
 // Every operand tile is a plain [128 rows x 128 B] swizzled block; "K-major" vs "MN-major" is only the descriptor
-// (k-step = 32 B inside a row vs 16 rows = 2048 B, atom stride 16384 B for the two 64-key halves of P / dS).
-// The unfused path reads P twice, writes dP, reads it back, writes dS and reads it twice (all S x S, through HBM);
-// here P is read once and nothing S x S is written.  Validated and on by default together with the forward (BATON_FUSED_ATTN).
+// (k-step = 32 B inside a row vs 16 rows = 2048 B; the two 64-key halves of P / dS are 16384 B apart).  Each
+// consumer warpgroup computes 64 output rows; results are staged in fp32 shared-memory tiles for the row-per-thread
+// passes.  The unfused path reads P twice, writes dP, reads it back, writes dS and reads it twice (all S x S, through
+// HBM); here P is read once and nothing S x S is written.  On by default together with the forward (BATON_FUSED_ATTN).
 struct AttnBwdParams {
   __nv_bfloat16* dqkv;     // [B*S, 3*D]
   int H, D;
   float scale;
 };
 
-__global__ void __launch_bounds__(AT_THREADS, 2)
+__global__ void __launch_bounds__(AT_THREADS, 1)
 attention_bwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                           const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
                           const __grid_constant__ CUtensorMap tmP, const AttnBwdParams p) {
@@ -228,11 +220,9 @@ attention_bwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
   uint8_t* sV = sK + AT_Q_BYTES;
   uint8_t* sdO = sV + AT_Q_BYTES;
   uint8_t* sP = sdO + AT_Q_BYTES;                   // [2 key halves][128 q x 64 keys]; becomes dS in place
-  uint64_t* bar_load = reinterpret_cast<uint64_t*>(sP + AT_P_BYTES);
-  uint64_t* bar_1 = bar_load + 1;      // dV and dP complete (P in shared memory no longer read by the tensor core)
-  uint64_t* bar_2 = bar_load + 2;      // dS written (4 arrivals), dP fully consumed
-  uint64_t* bar_3 = bar_load + 3;      // dQ and dK complete
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_load + 4);
+  float* sW = reinterpret_cast<float*>(sP + AT_P_BYTES);                  // dP, later [dQ | dK], fp32 [128][AT_SP]
+  float* sN = reinterpret_cast<float*>(sP + AT_P_BYTES + AT_WIDE_BYTES);  // dV, fp32 [128][AT_OP]
+  uint64_t* bar_load = reinterpret_cast<uint64_t*>(sP + AT_P_BYTES + AT_WIDE_BYTES + AT_NARROW_BYTES);
 
   griddep_launch_dependents();
   const int warp = threadIdx.x >> 5;
@@ -241,22 +231,10 @@ attention_bwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
   if (warp == 0 && elect_one()) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
     tma_prefetch_desc(&tmdO); tma_prefetch_desc(&tmP);
-  }
-  if (warp == 1 && elect_one()) {
     mbar_init(bar_load, 1);
-    mbar_init(bar_1, 1);
-    mbar_init(bar_2, 4);
-    mbar_init(bar_3, 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, AT_TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   griddep_wait();
 
   if (warp == 0) {
@@ -269,120 +247,128 @@ attention_bwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
       tma_load_2d(sP, &tmP, bar_load, 0, bh * AT_S);                 // keys 0..63   x 128 query rows
       tma_load_2d(sP + 16384, &tmP, bar_load, 64, bh * AT_S);        // keys 64..127
     }
-  } else if (warp == 1) {
-    mbar_wait(bar_load, 0);
-    tc_fence_after();
+  } else if (warp >= 4) {
+    const int ew = warp - 4, g = ew >> 2;
     const uint32_t q = smem_u32(sQ), k = smem_u32(sK), v = smem_u32(sV), d_o = smem_u32(sdO), pp = smem_u32(sP);
-    if (elect_one()) {
-      // dV[key, d] = sum_q P[q, key] dO[q, d]: both operands MN-major, reduction over the 128 query rows
-      const uint32_t id_dv = umma_idesc_bf16(AT_S, AT_D, 1, 1);
+    mbar_wait(bar_load, 0);
+    {
+      // dV[key, d] = sum_q P[q, key] dO[q, d]: both operands MN-major, reduction over the 128 query rows;
+      // warpgroup g owns keys 64 g .. 64 g + 63 = the g-th 64-key half of P
+      float dv[32], dp[64];
+#pragma unroll
+      for (int j = 0; j < 32; ++j) dv[j] = 0.f;
+#pragma unroll
+      for (int j = 0; j < 64; ++j) dp[j] = 0.f;
+      wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < 8; ++kk)
-        tc_mma_f16(tmem_base + AT_S, umma_smem_desc_sw128(pp + kk * 2048, 16384, 1024),
-                   umma_smem_desc_sw128(d_o + kk * 2048, 8192, 1024), id_dv, kk != 0);
+        wgmma_bf16_n64<1, 1>(dv, gmma_desc_sw128(pp + g * 16384 + kk * 2048, 16384, 1024),
+                             gmma_desc_sw128(d_o + kk * 2048, 8192, 1024), 1u);
       // dP[q, key] = sum_d dO[q, d] V[key, d]: both K-major
-      const uint32_t id_dp = umma_idesc_bf16(AT_S, AT_S, 0, 0);
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk)
-        tc_mma_f16(tmem_base, umma_smem_desc_sw128(d_o + kk * 32, 16, 1024), umma_smem_desc_sw128(v + kk * 32, 16, 1024),
-                   id_dp, kk != 0);
-      tc_commit(bar_1);
+        wgmma_bf16_n128<0, 0>(dp, gmma_desc_sw128(d_o + g * 8192 + kk * 32, 16, 1024),
+                              gmma_desc_sw128(v + kk * 32, 16, 1024), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_operands(dv);
+      wgmma_fence_operands(dp);
+      wg_store_acc<64>(dv, sN, AT_OP, 64 * g);
+      wg_store_acc<128>(dp, sW, AT_SP, 64 * g);
     }
-    __syncwarp();
-    mbar_wait(bar_2, 0);
-    tc_fence_after();
-    if (elect_one()) {
+    named_bar_sync(1, AT_CONSUMERS);
+    const int lane = static_cast<int>(lane_id());
+    const int r = (ew & 3) * 32 + lane;                            // query row (dP, dQ) / key row (dV, dK)
+    __nv_bfloat16* grow = p.dqkv + (static_cast<size_t>(b) * AT_S + r) * (3 * static_cast<size_t>(p.D)) + h * AT_D;
+    if (ew < 4) {
+      uint8_t* prow = sP + r * 128;
+      const float* wrow = sW + r * AT_SP;
+      // pass 1: delta = sum_key P[r, key] * dP[r, key]
+      float delta = 0.f;
+#pragma unroll 1
+      for (int c = 0; c < AT_S; c += 32) {
+        uint32_t x[32];
+        acc_ld_row32(wrow + c, x);
+        const uint8_t* tile = prow + (c >> 6) * 16384;
+#pragma unroll
+        for (int j = 0; j < 32; j += 8) {
+          const int chunk = ((c & 63) + j) >> 3;
+          const uint4 pv = *reinterpret_cast<const uint4*>(tile + ((chunk ^ (r & 7)) << 4));
+          const float2 p0 = unpack_bf16x2(pv.x), p1 = unpack_bf16x2(pv.y), p2 = unpack_bf16x2(pv.z), p3 = unpack_bf16x2(pv.w);
+          delta = fmaf(p0.x, __uint_as_float(x[j]), delta);     delta = fmaf(p0.y, __uint_as_float(x[j + 1]), delta);
+          delta = fmaf(p1.x, __uint_as_float(x[j + 2]), delta); delta = fmaf(p1.y, __uint_as_float(x[j + 3]), delta);
+          delta = fmaf(p2.x, __uint_as_float(x[j + 4]), delta); delta = fmaf(p2.y, __uint_as_float(x[j + 5]), delta);
+          delta = fmaf(p3.x, __uint_as_float(x[j + 6]), delta); delta = fmaf(p3.y, __uint_as_float(x[j + 7]), delta);
+        }
+      }
+      // pass 2: dS = P * (dP - delta), bf16, in place over P (this thread owns row r of both halves)
+#pragma unroll 1
+      for (int c = 0; c < AT_S; c += 32) {
+        uint32_t x[32];
+        acc_ld_row32(wrow + c, x);
+        uint8_t* tile = prow + (c >> 6) * 16384;
+#pragma unroll
+        for (int j = 0; j < 32; j += 8) {
+          const int chunk = ((c & 63) + j) >> 3;
+          uint4* slot = reinterpret_cast<uint4*>(tile + ((chunk ^ (r & 7)) << 4));
+          const uint4 pv = *slot;
+          const float2 p0 = unpack_bf16x2(pv.x), p1 = unpack_bf16x2(pv.y), p2 = unpack_bf16x2(pv.z), p3 = unpack_bf16x2(pv.w);
+          *slot = make_uint4(pack_bf16x2(p0.x * (__uint_as_float(x[j]) - delta), p0.y * (__uint_as_float(x[j + 1]) - delta)),
+                             pack_bf16x2(p1.x * (__uint_as_float(x[j + 2]) - delta), p1.y * (__uint_as_float(x[j + 3]) - delta)),
+                             pack_bf16x2(p2.x * (__uint_as_float(x[j + 4]) - delta), p2.y * (__uint_as_float(x[j + 5]) - delta)),
+                             pack_bf16x2(p3.x * (__uint_as_float(x[j + 6]) - delta), p3.y * (__uint_as_float(x[j + 7]) - delta)));
+        }
+      }
+      fence_proxy_async();            // dS (generic-proxy writes) -> visible to the tensor core
+    } else {
+      // dV row r (= key index) is complete: the second warpgroup stores it while the first computes dS
+#pragma unroll 1
+      for (int c = 0; c < AT_D; c += 32) {
+        uint32_t x[32];
+        acc_ld_row32(sN + r * AT_OP + c, x);
+#pragma unroll
+        for (int j = 0; j < 32; j += 8)
+          *reinterpret_cast<uint4*>(grow + 2 * p.D + c + j) =
+              make_uint4(pack_bf16x2(__uint_as_float(x[j]), __uint_as_float(x[j + 1])),
+                         pack_bf16x2(__uint_as_float(x[j + 2]), __uint_as_float(x[j + 3])),
+                         pack_bf16x2(__uint_as_float(x[j + 4]), __uint_as_float(x[j + 5])),
+                         pack_bf16x2(__uint_as_float(x[j + 6]), __uint_as_float(x[j + 7])));
+      }
+    }
+    named_bar_sync(1, AT_CONSUMERS);
+    {
       // dQ[q, d] = sum_key dS[q, key] K[key, d]: A K-major (two 64-key halves), B = K MN-major
-      const uint32_t id_dq = umma_idesc_bf16(AT_S, AT_D, 0, 1);
+      // dK[key, d] = sum_q dS[q, key] Q[q, d]: A = dS^T (MN-major view, key half g), B = Q MN-major
+      float dq[32], dk[32];
+#pragma unroll
+      for (int j = 0; j < 32; ++j) { dq[j] = 0.f; dk[j] = 0.f; }
+      wgmma_fence();
 #pragma unroll
       for (int kt = 0; kt < 2; ++kt)
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk)
-          tc_mma_f16(tmem_base, umma_smem_desc_sw128(pp + kt * 16384 + kk * 32, 16, 1024),
-                     umma_smem_desc_sw128(k + (kt * 4 + kk) * 2048, 8192, 1024), id_dq, (kt | kk) != 0);
-      // dK[key, d] = sum_q dS[q, key] Q[q, d]: A = dS^T (MN-major view), B = Q MN-major
-      const uint32_t id_dk = umma_idesc_bf16(AT_S, AT_D, 1, 1);
+          wgmma_bf16_n64<0, 1>(dq, gmma_desc_sw128(pp + kt * 16384 + g * 8192 + kk * 32, 16, 1024),
+                               gmma_desc_sw128(k + (kt * 4 + kk) * 2048, 8192, 1024), 1u);
 #pragma unroll
       for (int kk = 0; kk < 8; ++kk)
-        tc_mma_f16(tmem_base + AT_D, umma_smem_desc_sw128(pp + kk * 2048, 16384, 1024),
-                   umma_smem_desc_sw128(q + kk * 2048, 8192, 1024), id_dk, kk != 0);
-      tc_commit(bar_3);
+        wgmma_bf16_n64<1, 1>(dk, gmma_desc_sw128(pp + g * 16384 + kk * 2048, 16384, 1024),
+                             gmma_desc_sw128(q + kk * 2048, 8192, 1024), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_operands(dq);
+      wgmma_fence_operands(dk);
+      wg_store_acc<64>(dq, sW, AT_SP, 64 * g);          // dP is consumed: columns [0,64) dQ, [64,128) dK
+      wg_store_acc<64>(dk, sW + AT_D, AT_SP, 64 * g);
     }
-    __syncwarp();
-  } else if (warp >= 4) {
-    const int qd = warp & 3;
-    const int lane = static_cast<int>(lane_id());
-    const int r = qd * 32 + lane;                                   // TMEM lane: query row (dP, dQ) / key row (dV, dK)
-    const uint32_t t_row = tmem_base + (static_cast<uint32_t>(qd * 32) << 16);
-    uint8_t* prow = sP + r * 128;
-    mbar_wait(bar_1, 0);
-    tc_fence_after();
-    // pass 1: delta = sum_key P[r, key] * dP[r, key]
-    float delta = 0.f;
+    named_bar_sync(1, AT_CONSUMERS);
+    // dQ row r (query) from columns [0,64), dK row r (key) from columns [64,128), both scaled by the softmax scale;
+    // the two warpgroups take one half each
+    const int c = (ew < 4 ? 0 : AT_D);
 #pragma unroll 1
-    for (int c = 0; c < AT_S; c += 32) {
+    for (int cc = c; cc < c + AT_D; cc += 32) {
       uint32_t x[32];
-      tmem_ld_32x32b_x32(t_row + c, x);
-      tmem_ld_wait();
-      const uint8_t* tile = prow + (c >> 6) * 16384;
-#pragma unroll
-      for (int j = 0; j < 32; j += 8) {
-        const int chunk = ((c & 63) + j) >> 3;
-        const uint4 pv = *reinterpret_cast<const uint4*>(tile + ((chunk ^ (r & 7)) << 4));
-        const float2 p0 = unpack_bf16x2(pv.x), p1 = unpack_bf16x2(pv.y), p2 = unpack_bf16x2(pv.z), p3 = unpack_bf16x2(pv.w);
-        delta = fmaf(p0.x, __uint_as_float(x[j]), delta);     delta = fmaf(p0.y, __uint_as_float(x[j + 1]), delta);
-        delta = fmaf(p1.x, __uint_as_float(x[j + 2]), delta); delta = fmaf(p1.y, __uint_as_float(x[j + 3]), delta);
-        delta = fmaf(p2.x, __uint_as_float(x[j + 4]), delta); delta = fmaf(p2.y, __uint_as_float(x[j + 5]), delta);
-        delta = fmaf(p3.x, __uint_as_float(x[j + 6]), delta); delta = fmaf(p3.y, __uint_as_float(x[j + 7]), delta);
-      }
-    }
-    // pass 2: dS = P * (dP - delta), bf16, in place over P (this thread owns row r of both halves)
-#pragma unroll 1
-    for (int c = 0; c < AT_S; c += 32) {
-      uint32_t x[32];
-      tmem_ld_32x32b_x32(t_row + c, x);
-      tmem_ld_wait();
-      uint8_t* tile = prow + (c >> 6) * 16384;
-#pragma unroll
-      for (int j = 0; j < 32; j += 8) {
-        const int chunk = ((c & 63) + j) >> 3;
-        uint4* slot = reinterpret_cast<uint4*>(tile + ((chunk ^ (r & 7)) << 4));
-        const uint4 pv = *slot;
-        const float2 p0 = unpack_bf16x2(pv.x), p1 = unpack_bf16x2(pv.y), p2 = unpack_bf16x2(pv.z), p3 = unpack_bf16x2(pv.w);
-        *slot = make_uint4(pack_bf16x2(p0.x * (__uint_as_float(x[j]) - delta), p0.y * (__uint_as_float(x[j + 1]) - delta)),
-                           pack_bf16x2(p1.x * (__uint_as_float(x[j + 2]) - delta), p1.y * (__uint_as_float(x[j + 3]) - delta)),
-                           pack_bf16x2(p2.x * (__uint_as_float(x[j + 4]) - delta), p2.y * (__uint_as_float(x[j + 5]) - delta)),
-                           pack_bf16x2(p3.x * (__uint_as_float(x[j + 6]) - delta), p3.y * (__uint_as_float(x[j + 7]) - delta)));
-      }
-    }
-    tc_fence_before();                // this thread's TMEM reads of dP precede the MMAs that overwrite those columns
-    fence_proxy_async_all();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bar_2);
-    // dV row r (= key index) is complete since bar_1: store it while dQ / dK are being computed
-    __nv_bfloat16* grow = p.dqkv + (static_cast<size_t>(b) * AT_S + r) * (3 * static_cast<size_t>(p.D)) + h * AT_D;
-#pragma unroll 1
-    for (int c = 0; c < AT_D; c += 32) {
-      uint32_t x[32];
-      tmem_ld_32x32b_x32(t_row + AT_S + c, x);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 32; j += 8)
-        *reinterpret_cast<uint4*>(grow + 2 * p.D + c + j) =
-            make_uint4(pack_bf16x2(__uint_as_float(x[j]), __uint_as_float(x[j + 1])),
-                       pack_bf16x2(__uint_as_float(x[j + 2]), __uint_as_float(x[j + 3])),
-                       pack_bf16x2(__uint_as_float(x[j + 4]), __uint_as_float(x[j + 5])),
-                       pack_bf16x2(__uint_as_float(x[j + 6]), __uint_as_float(x[j + 7])));
-    }
-    mbar_wait(bar_3, 0);
-    tc_fence_after();
-    // dQ row r (query) from columns [0,64), dK row r (key) from columns [64,128), both scaled by the softmax scale
-#pragma unroll 1
-    for (int c = 0; c < 2 * AT_D; c += 32) {
-      uint32_t x[32];
-      tmem_ld_32x32b_x32(t_row + c, x);
-      tmem_ld_wait();
-      __nv_bfloat16* dst = grow + (c < AT_D ? c : p.D + (c - AT_D));
+      acc_ld_row32(sW + r * AT_SP + cc, x);
+      __nv_bfloat16* dst = grow + (cc < AT_D ? cc : p.D + (cc - AT_D));
 #pragma unroll
       for (int j = 0; j < 32; j += 8)
         *reinterpret_cast<uint4*>(dst + j) =
@@ -392,9 +378,6 @@ attention_bwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
                        pack_bf16x2(__uint_as_float(x[j + 6]) * p.scale, __uint_as_float(x[j + 7]) * p.scale));
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, AT_TMEM_COLS);
 }
 
 }  // namespace b200
@@ -420,7 +403,7 @@ extern "C" int b200_attention_fwd(const void* qkv, void* out, void* probs, int B
   p.H = H;
   p.D = static_cast<int>(D);
   p.scale_log2e = scale * 1.4426950408889634f;
-  constexpr int smem = 3 * AT_Q_BYTES + AT_P_BYTES + 4 * 8 + 16 + 1024;
+  constexpr int smem = 3 * AT_Q_BYTES + AT_P_BYTES + AT_WIDE_BYTES + AT_NARROW_BYTES + 8 + 1024;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(attention_fwd_s128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
@@ -458,7 +441,7 @@ extern "C" int b200_attention_bwd(const void* qkv, const void* dout, const void*
   p.H = H;
   p.D = static_cast<int>(D);
   p.scale = scale;
-  constexpr int smem = 4 * AT_Q_BYTES + AT_P_BYTES + 4 * 8 + 16 + 1024;
+  constexpr int smem = 4 * AT_Q_BYTES + AT_P_BYTES + AT_WIDE_BYTES + AT_NARROW_BYTES + 8 + 1024;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(attention_bwd_s128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);

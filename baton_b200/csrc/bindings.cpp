@@ -1,4 +1,4 @@
-// PyTorch bindings for the sm_100a kernels.  Thin by design: shape logic lives in Python
+// PyTorch bindings for the sm_90a kernels.  Thin by design: shape logic lives in Python
 // (baton_b200/ops), this file only unwraps tensors, picks the current stream and checks codes.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -26,7 +26,7 @@ inline T* opt_ptr(const std::optional<at::Tensor>& t) {
 
 // ---- in-graph kernel timeline (pdl.cuh): every translation unit owns a copy of the trace pointer
 extern "C" {
-#define B200_TRACE_TUS(X) X(gemm_tcgen05) X(gemm_fp8) X(quant) X(attention) X(im2col_tma) X(gemm_simt) X(fedavg) \
+#define B200_TRACE_TUS(X) X(gemm_wgmma) X(gemm_fp8) X(quant) X(attention) X(im2col_tma) X(gemm_simt) X(fedavg) \
   X(elementwise) X(conv) X(norm) X(loss)
 #define B200_DECL(tu) int b200_trace_set_##tu(unsigned long long* p);
 B200_TRACE_TUS(B200_DECL)
@@ -630,7 +630,7 @@ void mse(const at::Tensor& pred, const at::Tensor& target, const std::optional<a
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "baton_b200 sm_100a kernels";
+  m.doc() = "baton_b200 sm_90a kernels";
   m.attr("MAX_RANKS") = B200_MAX_RANKS;
   m.def("gemm", &gemm);
   m.def("trace_set", &trace_set);

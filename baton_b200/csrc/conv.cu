@@ -1,4 +1,4 @@
-// NHWC convolution plumbing around the tcgen05 GEMM: im2col (forward / wgrad operand), col2im
+// NHWC convolution plumbing around the wgmma GEMM: im2col (forward / wgrad operand), col2im
 // (dgrad scatter written as a gather so it needs no atomics), max / average pooling.
 // A convolution is   Y[N*Ho*Wo, Cout] = col[N*Ho*Wo, KH*KW*Cin] * W[Cout, KH*KW*Cin]^T
 // with K index = (kh*KW + kw)*Cin + c, i.e. weights stored [Cout, KH, KW, Cin] (channels_last).
@@ -10,7 +10,7 @@
 namespace b200 {
 
 constexpr int CV_THREADS = 256;
-static inline int cv_grid(long long n, int max_ctas = 148 * 8) {
+static inline int cv_grid(long long n, int max_ctas = device_sm_count() * 8) {
   long long g = (n + CV_THREADS - 1) / CV_THREADS;
   if (g < 1) g = 1;
   if (g > max_ctas) g = max_ctas;
@@ -94,7 +94,7 @@ im2col_scalar_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restr
 // small-channel path, shared-memory edition: one CTA builds the col rows of ONE output image row (n, ho).  The KH input
 // rows it needs (KH x W x C elements, 1.3 KB for the 7x7x3 stem at 32x32) are fetched once with 16-byte loads, the
 // 16-byte col vectors are then assembled from shared memory -- the scalar kernel above issued eight 2-byte global loads per
-// vector (10.3 us for the ResNet stem inside the captured step).  Needs (W * C) % 8 == 0 (16-byte aligned image rows).
+// vector.  Needs (W * C) % 8 == 0 (16-byte aligned image rows).
 __global__ void __launch_bounds__(128)
 im2col_smallc_smem_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ col, int N, int H, int W, int C,
                           int KH, int KW, int stride, int pad, int Ho, int Wo, int kp) {
@@ -250,8 +250,7 @@ maxpool_bwd_gather_kernel(const __nv_bfloat162* __restrict__ dy, const int2* __r
 
 // ---- 16-byte variants (C % 8 == 0): one thread = 8 channels of one pixel; the winner is remembered as ONE BYTE (the tap
 // index kh * k + kw inside the window) instead of a 4-byte flat position, and the backward optionally sums a two-piece
-// gradient (dy_a + dy_b) while loading.  The scalar kernels above moved 4 bytes per request and took 8.4 / 27.6 us for
-// the 32x32-input ResNet stem inside the captured step (in-graph timeline, profiles/).
+// gradient (dy_a + dy_b) while loading.  The scalar kernels above move 4 bytes per request.
 __global__ void __launch_bounds__(CV_THREADS)
 maxpool_vec_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, uint2* __restrict__ arg, int N, int H, int W, int C8,
                    int k, int stride, int pad, int Ho, int Wo) {

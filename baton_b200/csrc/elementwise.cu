@@ -1,7 +1,7 @@
 // HBM-bound elementwise / reduction kernels over flat buffers: fused arena SGD (K4), multi-source
 // weighted sum (manager-side FedAvg, K1 fallback), casts, batch row gather (K8), column sums
 // (bias gradients), ReLU / GELU pieces.  All use 16-byte vectors and grid-stride loops sized to
-// 148 SMs x a few resident CTAs.
+// the device's SMs x a few resident CTAs.
 #define B200_TU_TAG 8
 #include "launch.h"
 #include "pdl.cuh"
@@ -10,7 +10,7 @@
 namespace b200 {
 
 constexpr int EW_THREADS = 256;
-static inline int ew_grid(long long n_vec, int max_ctas = 148 * 8) {
+static inline int ew_grid(long long n_vec, int max_ctas = device_sm_count() * 8) {
   long long g = (n_vec + EW_THREADS - 1) / EW_THREADS;
   if (g < 1) g = 1;
   if (g > max_ctas) g = max_ctas;
@@ -549,7 +549,7 @@ extern "C" int b200_colsum(const void* x, float* out, long long rows, int cols, 
     const int cols8 = cols / 8;
     const unsigned gx = static_cast<unsigned>((cols8 + 31) / 32);
     // ~2 waves of CTAs over the machine, at least one 32-row pass each
-    long long want = (2 * 148 + gx - 1) / gx;
+    long long want = (2 * device_sm_count() + gx - 1) / gx;
     long long rpc = (rows + want - 1) / want;
     rpc = (rpc + 31) / 32 * 32;
     if (rpc < 32) rpc = 32;

@@ -1,4 +1,4 @@
-// Fused FedAvg collective over NVLink 5 / NVSwitch -- ONE persistent kernel per round that does
+// Fused FedAvg collective over NVLink / NVSwitch -- ONE persistent kernel per round that does
 //
 //   (wire formats: fp32, bf16, or block-scaled fp8 = e4m3 + one UE8M0 scale per 32 elements)
 //   phase 0  pack      wire_r[t]  = cast( s_r * (theta_r[t] - global[t]) )   (delta mode)
@@ -15,7 +15,7 @@
 //   phase 2  apply     global += result ; theta = global ; bf16 shadow = bf16(theta) ; momentum = 0
 //                      (the reference's load_state_dict, worker.py:98, with no extra pass), then
 //                      publish a per-tile arrival flag so the next forward's first GEMM
-//                      (gemm_tcgen05, flag-gated TMA producer) can start on its weight tiles while
+//                      (gemm_wgmma, flag-gated TMA producer) can start on its weight tiles while
 //                      the rest of the arena is still in flight.
 //   barrier  (closing: wire / pads may be reused by the next round)
 //
@@ -317,9 +317,8 @@ __global__ void __maxnreg__(96) fedavg_allreduce_kernel(const __grid_constant__ 
   __syncthreads();
 
   // ---------------------------------------------------------------- phase 1: reduce + broadcast
-  // A remote 16-byte load costs a full NVLink round trip (~2-3 us); with few ranks a thread that handles ONE wire vector
-  // per trip has only A loads in flight and the phase runs at a quarter of the link rate (2 GPUs: 54 us for 11 MB each
-  // way, phase stamps as in profiles/r2_agg_bench_8gpu.txt).  Each trip therefore handles U vectors, U chosen so that
+  // A remote 16-byte load costs a full NVLink round trip (microseconds); with few ranks a thread that handles ONE wire
+  // vector per trip has only A loads in flight and cannot keep the link busy.  Each trip therefore handles U vectors, U chosen so that
   // about eight remote loads per thread are in flight whatever the number of ranks.
   auto reduce_tiles = [&](auto u_tag) {
     constexpr int U = decltype(u_tag)::value;

@@ -1,23 +1,21 @@
-// Block-scaled FP8 (MXFP8) GEMM on the 5th-gen tensor cores.
+// Block-scaled FP8 (MXFP8) GEMM on the Hopper tensor cores.
 //
 //     D[M,N] = act( alpha * (A .* SFA)[M,K] * (B .* SFB)[N,K]^T + bias[N] )
 //
 // A, B: e4m3, both K-major (row-major [rows, K]); SFA / SFB: one UE8M0 scale per 32 consecutive K
-// elements of every row (OCP MX format), accumulate fp32 in TMEM, `tcgen05.mma.kind::mxf8f6f4.block_scale`.
-// The transposed operands that dgrad / wgrad need are produced (already quantised along THEIR
-// reduction dimension) by the fused quantise+transpose kernels in quant.cu, so one K-major kernel
-// serves forward, dgrad and wgrad.
+// elements of every row (OCP MX format), accumulate fp32.  The transposed operands that dgrad / wgrad need are
+// produced (already quantised along THEIR reduction dimension) by the fused quantise+transpose kernels in quant.cu,
+// so one K-major kernel serves forward, dgrad and wgrad.
 //
-// Scale-factor plumbing (the fiddly part): for a 128-row x 128-K tile the 128 x 4 scale bytes are
-// stored in global memory as one contiguous 512-byte ATOM  [row % 32][row / 32][k-block]  (the
-// layout tcgen05 expects); per pipeline stage the producer fetches the A and B atoms with a plain
-// bulk copy next to the TMA tiles, the MMA warp moves them smem -> TMEM with
-// `tcgen05.cp.32x128b.warpx4` (4 TMEM columns per atom) and issues the four K=32 MMAs of the stage
-// with the per-MMA scale byte selected through the instruction descriptor (a_sf_id / b_sf_id).
-// tcgen05.cp and tcgen05.mma execute in issue order, so one TMEM scale buffer is reused every stage.
+// Hopper's FP8 wgmma has no block scaling, so each 32-element K block is one m64 x BN x 32 wgmma into a scratch
+// accumulator, folded into the running one as  acc += sfa[row] * sfb[col] * scratch  (a power-of-two scale per
+// element, exact).  For a 128-row x 128-K tile the 128 x 4 scale bytes are stored in global memory as one contiguous
+// 512-byte ATOM  [row % 32][row / 32][k-block]; per pipeline stage the producer fetches the A and B atoms with a
+// plain bulk copy next to the TMA tiles and the consumer warpgroups read their rows' / columns' bytes from shared
+// memory.
 //
-// `block_scaled = 0` runs the same pipeline with `kind::f8f6f4` (no scale factors; per-tensor scales
-// folded into alpha).
+// `block_scaled = 0` runs the same pipeline with plain e4m3 wgmma accumulating across the whole k-tile (per-tensor
+// scales folded into alpha).
 #define B200_TU_TAG 2
 #include "ptx.cuh"
 #include "launch.h"
@@ -27,8 +25,9 @@ namespace b200 {
 
 constexpr int F8_BM = 128;
 constexpr int F8_BK = 128;      // 128 e4m3 = 128 B = one swizzle row
-constexpr int F8_UMMA_K = 32;   // K per tcgen05.mma for 8-bit operands
-constexpr int F8_THREADS = 256;
+constexpr int F8_WG_K = 32;     // K per wgmma for 8-bit operands
+constexpr int F8_THREADS = 384;    // warpgroup 0: TMA producer, warpgroups 1-2: wgmma + epilogue
+constexpr int F8_CONSUMER_WARPS = 8;
 constexpr int SF_ATOM = 512;    // bytes: 128 rows x 4 k-blocks
 
 struct Fp8Params {
@@ -68,54 +67,26 @@ __device__ __forceinline__ void bulk_load(void* smem_dst, const void* gsrc, uint
                "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-// smem (32 rows x 16 B, no swizzle) -> TMEM, replicated to the four 32-lane quadrants
-__device__ __forceinline__ void tmem_cp_sf(uint32_t taddr, uint32_t smem_addr) {
-  // K-major, SWIZZLE_NONE descriptor: 8-row core matrices 128 B apart (SBO), version 1
-  uint64_t d = static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(16 >> 4) << 16;    // LBO (unused: a single 16 B column)
-  d |= static_cast<uint64_t>(128 >> 4) << 32;   // SBO
-  d |= static_cast<uint64_t>(1) << 46;
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" ::"r"(taddr), "l"(d) : "memory");
-}
-// instruction descriptors
-__device__ __forceinline__ uint32_t idesc_mxf8(int M, int N, uint32_t a_sf, uint32_t b_sf) {
-  // [4,6) b_sf_id  [7,10) a_fmt (0 = E4M3)  [10,13) b_fmt  [17,23) N>>3  [23] scale fmt (1 = UE8M0)
-  // [24,29) M>>4  [29,31) a_sf_id
-  return (b_sf << 4) | (static_cast<uint32_t>(N >> 3) << 17) | (1u << 23) | (static_cast<uint32_t>(M >> 4) << 24) |
-         (a_sf << 29);
-}
-__device__ __forceinline__ uint32_t idesc_f8(int M, int N) {
-  return (1u << 4) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);  // c_format = F32
-}
-__device__ __forceinline__ void mma_mxf8(uint32_t d, uint64_t ad, uint64_t bd, uint32_t idesc, uint32_t acc,
-                                         uint32_t sfa, uint32_t sfb) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t}"
-      ::"r"(d), "l"(ad), "l"(bd), "r"(idesc), "r"(acc), "r"(sfa), "r"(sfb)
-      : "memory");
-}
-__device__ __forceinline__ void mma_f8(uint32_t d, uint64_t ad, uint64_t bd, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d), "l"(ad), "l"(bd), "r"(idesc), "r"(acc)
-      : "memory");
+// position of the scale byte of (row, 32-element K block kb) inside a 512-byte atom [row % 32][row / 32][kb]
+__device__ __forceinline__ int sf_index(int row, int kb) { return (row & 31) * 16 + (row >> 5) * 4 + kb; }
+// UE8M0: a bare biased exponent, 2^(e - 127)
+__device__ __forceinline__ float ue8m0(uint8_t e) { return __uint_as_float(static_cast<uint32_t>(e) << 23); }
+template <int N>
+__device__ __forceinline__ void wgmma_e4m3(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
+  if constexpr (N == 64) wgmma_e4m3_n64(d, da, db, scale_d);
+  else wgmma_e4m3_n128(d, da, db, scale_d);
 }
 
 template <int BN, int STAGES>
 __global__ void __launch_bounds__(F8_THREADS, 1)
 gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Fp8Params p) {
   using L = F8Smem<BN>;
-  constexpr int TCOLS = (BN + 8 * (1 + L::SFB_ATOMS) <= 64) ? 64 : ((BN + 8 * (1 + L::SFB_ATOMS) <= 128) ? 128 : (BN + 8 * (1 + L::SFB_ATOMS) <= 256 ? 256 : 512));
+  constexpr int PITCH = BN + 4;                      // fp32 pitch of the staged accumulator tile
+  static_assert(STAGES * L::STAGE_BYTES >= F8_BM * PITCH * 4, "the drained ring must hold the fp32 accumulator tile");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * L::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
 
   griddep_launch_dependents();
   const int warp = threadIdx.x >> 5;
@@ -131,25 +102,13 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   if (warp == 0 && elect_one()) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1 && elect_one()) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], F8_CONSUMER_WARPS);
     }
-    mbar_init(tmem_full_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, TCOLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_sfa = tmem_base + BN;          // 4 columns
-  const uint32_t tmem_sfb = tmem_base + BN + 4;      // 4 columns per 128 rows of B
   griddep_wait();
 
   if (warp == 0) {
@@ -174,49 +133,66 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
+  } else if (warp >= 4) {
+    const int ew = warp - 4, g = ew >> 2;            // warpgroup g: rows 64 g .. 64 g + 63 of the tile
+    const int lane = static_cast<int>(lane_id());
+    const int fr0 = 64 * g + 16 * (ew & 3) + (lane >> 2);   // fragment rows fr0, fr0 + 8; columns 8 i + 2 (lane % 4) + e
+    float acc[BN / 2];
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
     for (int i = 0; i < num_kt; ++i) {
       const int s = i % STAGES;
       const uint32_t ph = (i / STAGES) & 1;
       mbar_wait(&full_bar[s], ph);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t sa = smem_u32(smem + s * L::STAGE_BYTES);
-        const uint32_t sb = sa + L::A_BYTES;
-        const uint32_t ssf = sb + L::B_BYTES;
-        if (p.block_scaled) {
-          tmem_cp_sf(tmem_sfa, ssf);
+      const uint32_t sa = smem_u32(smem + s * L::STAGE_BYTES) + g * 8192;   // 64 rows x 128 B
+      const uint32_t sb = smem_u32(smem + s * L::STAGE_BYTES + L::A_BYTES);
+      if (p.block_scaled) {
+        // one K = 32 block at a time: tmp = A_kb B_kb^T, then acc += sfa[row, kb] * sfb[col, kb] * tmp
+        const uint8_t* ssf = smem + s * L::STAGE_BYTES + L::A_BYTES + L::B_BYTES;
+#pragma unroll 1
+        for (int kb = 0; kb < F8_BK / F8_WG_K; ++kb) {
+          float tmp[BN / 2];
+          wgmma_fence();
+          wgmma_e4m3<BN>(tmp, gmma_desc_sw128(sa + kb * 32, 16, 1024), gmma_desc_sw128(sb + kb * 32, 16, 1024), 0u);
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_operands(tmp);
+          const float sa0 = ue8m0(ssf[sf_index(fr0, kb)]), sa1 = ue8m0(ssf[sf_index(fr0 + 8, kb)]);
 #pragma unroll
-          for (int j = 0; j < L::SFB_ATOMS; ++j) tmem_cp_sf(tmem_sfb + 4 * j, ssf + SF_ATOM * (1 + j));
+          for (int c8 = 0; c8 < BN / 8; ++c8) {
+            const int col = 8 * c8 + 2 * (lane & 3);
+            const float sb0 = ue8m0(ssf[SF_ATOM + sf_index(col, kb)]), sb1 = ue8m0(ssf[SF_ATOM + sf_index(col + 1, kb)]);
+            acc[4 * c8] = fmaf(sa0 * sb0, tmp[4 * c8], acc[4 * c8]);
+            acc[4 * c8 + 1] = fmaf(sa0 * sb1, tmp[4 * c8 + 1], acc[4 * c8 + 1]);
+            acc[4 * c8 + 2] = fmaf(sa1 * sb0, tmp[4 * c8 + 2], acc[4 * c8 + 2]);
+            acc[4 * c8 + 3] = fmaf(sa1 * sb1, tmp[4 * c8 + 3], acc[4 * c8 + 3]);
+          }
         }
+      } else {
+        wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < F8_BK / F8_UMMA_K; ++k) {
-          const uint64_t ad = umma_smem_desc_sw128(sa + k * 32, 16, 1024);
-          const uint64_t bd = umma_smem_desc_sw128(sb + k * 32, 16, 1024);
-          if (p.block_scaled)
-            mma_mxf8(tmem_base, ad, bd, idesc_mxf8(F8_BM, BN, k, k), (i | k) != 0, tmem_sfa, tmem_sfb);
-          else
-            mma_f8(tmem_base, ad, bd, idesc_f8(F8_BM, BN), (i | k) != 0);
-        }
-        tc_commit(&empty_bar[s]);
-        if (i == num_kt - 1) tc_commit(tmem_full_bar);
+        for (int kb = 0; kb < F8_BK / F8_WG_K; ++kb)
+          wgmma_e4m3<BN>(acc, gmma_desc_sw128(sa + kb * 32, 16, 1024), gmma_desc_sw128(sb + kb * 32, 16, 1024), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_operands(acc);
       }
-      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[s]);
     }
-  } else if (warp >= 4) {
-    const int q = warp & 3;
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-    const int row = m0 + q * 32 + static_cast<int>(lane_id());
+    named_bar_sync(1, F8_CONSUMER_WARPS * 32);       // both warpgroups are done with the ring: stage the accumulator
+    float* part = reinterpret_cast<float*>(smem);
+    wg_store_acc<BN>(acc, part, PITCH, 64 * g);
+    named_bar_sync(1, F8_CONSUMER_WARPS * 32);
+    const int q = ew & 3;
+    const int row = m0 + q * 32 + lane;
     const bool row_ok = row < p.M;
     const size_t elt = p.out_fp32 ? 4 : 2;
     uint8_t* drow = reinterpret_cast<uint8_t*>(p.D) + static_cast<size_t>(row) * p.ldd * elt;
     const bool vec_ok = ((reinterpret_cast<uintptr_t>(p.D) & 15) == 0) && ((p.ldd * elt) % 16 == 0);
 #pragma unroll 1
-    for (int c = 0; c < BN; c += 32) {
+    for (int c = g * 32; c < BN; c += 64) {          // the two warps of a row quarter take alternate 32-column chunks
       uint32_t r[32];
-      tmem_ld_32x32b_x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + c, r);
-      tmem_ld_wait();
+      acc_ld_row32(part + (q * 32 + lane) * PITCH + c, r);
       const int col0 = n0 + c;
       if (!row_ok || col0 >= p.N) continue;
       float v[32];
@@ -260,9 +236,6 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, TCOLS);
 }
 
 typedef CUresult (*EncodeTiledFn8)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,

@@ -8,13 +8,13 @@
 //   traversal strides = conv stride; the instruction takes the base pixel of the 128-pixel column in INPUT
 //   coordinates (w = q*stride - pad, h = p*stride - pad) and the filter tap as 16-bit offsets (s, r);
 //   out-of-image taps are zero-filled.  The result lands as [pixels x 64 channels] rows of 128 B with the 128 B
-//   swizzle, i.e. exactly the K-major A tile gemm_tcgen05.cu already consumes.
+//   swizzle, i.e. exactly the K-major A tile gemm_wgmma.cu already consumes.
 //
 // This file only contains the encoder, the PTX wrapper and a PROBE kernel that dumps such tiles back to global
 // memory in the layout of the explicit im2col kernel, so the semantics can be pinned down against it
 // (tests/test_gpu_kernels.py::test_tma_im2col_probe_matches_explicit_im2col, opt-in: BATON_TMA_IM2COL=1).
-// Semantics probe only (not on any model path): it pinned down the im2col-mode coordinate convention on hardware in
-// round 2 (profiles/r2_validate_experimental.txt) before the implicit-GEMM convolution modes of gemm_tcgen05.cu relied on it.
+// Semantics probe only (not on any model path): it pins down the im2col-mode coordinate convention the implicit-GEMM
+// convolution modes of gemm_wgmma.cu rely on.
 #define B200_TU_TAG 5
 #include <cuda.h>
 

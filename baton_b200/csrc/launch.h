@@ -1,4 +1,4 @@
-// C launch API of the sm_100a kernels (implemented in the .cu files, wrapped for PyTorch in
+// C launch API of the sm_90a kernels (implemented in the .cu files, wrapped for PyTorch in
 // bindings.cpp).  Every launcher takes raw device pointers and a stream and returns 0 or a
 // CUDA error code, so the .cu files do not include any PyTorch header and compile in seconds.
 #pragma once
@@ -9,7 +9,7 @@
 
 extern "C" {
 
-// ---- gemm_tcgen05.cu
+// ---- gemm_wgmma.cu
 int b200_gemm_bf16(const void* a, const void* b, void* d, const float* bias, int M, int N, int K, long long lda,
                    long long ldb, long long ldd, int a_mn, int b_mn, int out_fp32, int act, int split_k, int accumulate,
                    float alpha, const uint32_t* tile_flags, uint32_t flag_epoch, long long flag_elem_off, int flag_tile_elems,
@@ -24,7 +24,7 @@ int b200_attention_fwd(const void* qkv, void* out, void* probs, int B, int S, in
                        cudaStream_t stream);
 int b200_attention_bwd(const void* qkv, const void* dout, const void* probs, void* dqkv, int B, int S, int H, int dh,
                        float scale, cudaStream_t stream);
-// ---- implicit-GEMM convolution (experimental: gemm_tcgen05.cu CONV modes fed by TMA im2col maps)
+// ---- implicit-GEMM convolution (experimental: gemm_wgmma.cu CONV modes fed by TMA im2col maps)
 int b200_conv_igemm_fwd(const void* x, const void* w, void* y, int N, int H, int W, int Cin, int Cout, int KH, int KW,
                         int stride, int pad, int Ho, int Wo, int cluster_k, int force_bn, float* col_stats,
                         cudaStream_t stream);

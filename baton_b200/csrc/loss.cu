@@ -122,8 +122,7 @@ mse_kernel(const void* __restrict__ pred, const float* __restrict__ target, void
 //   dX[r, :] = dlogits[r, :] W          (bf16, feeds the backbone's backward)
 //   dW      += dlogits^T X ,  db += colsum(dlogits)      (fp32 atomics straight into the gradient arena)
 //   loss_acc[0] += mean loss, loss_acc[1] += #correct
-// The separate launches this replaces (tcgen05 GEMM 128x10x512, loss, cast, colsum, two SIMT GEMMs) cost ~18 us of the
-// captured ResNet-18 step for ~4 MFLOP of work.  One CTA handles HEAD_ROWS rows: warp w owns row w for the logits, the
+// It replaces six launches (GEMM 128x10x512, loss, cast, colsum, two SIMT GEMMs) for ~4 MFLOP of work.  One CTA handles HEAD_ROWS rows: warp w owns row w for the logits, the
 // 256 threads then share the dX / dW tiles.  x: bf16 [rows, K], W: bf16 [NC, K] (the arena's shadow), b: fp32.
 constexpr int HEAD_ROWS = 8;
 __global__ void __launch_bounds__(256)
@@ -151,7 +150,7 @@ linear_xent_head_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   {   // logits + loss of row `warp` (8 warps = HEAD_ROWS rows); lane c ends up holding logit c.  Four classes at a time:
       // independent accumulators and interleaved shuffle reductions (the one-class-at-a-time version was a 10-deep
-      // dependent chain of reductions: the kernel took 14 us in the captured step)
+      // dependent chain of reductions)
     const int row = r0 + warp;
     float mine = -INFINITY;
     for (int c0 = 0; c0 < NC; c0 += 4) {
@@ -257,7 +256,7 @@ extern "C" int b200_mse(const void* pred, int pred_fp32, const float* target, vo
                         float* loss_acc, long long n, float grad_scale, cudaStream_t stream) {
   if (n <= 0) return 0;
   long long g = (n + 255) / 256;
-  if (g > 148 * 4) g = 148 * 4;
+  if (g > device_sm_count() * 4) g = device_sm_count() * 4;
   const unsigned grid = static_cast<unsigned>(g);
 #define MSE(A, B) launch_pdl(mse_kernel<A, B>, grid, 256, 0, stream, pred, target, dpred, loss_acc, n, grad_scale)
   if (pred_fp32) { if (dp_fp32) MSE(true, true); else MSE(true, false); }

@@ -697,8 +697,7 @@ static inline int rows_per_block(int C) {   // 8 warps x rows per warp
 // ---- vectorised column reductions (C % 8 == 0, C/8 a power of two <= 256): a thread owns 8 adjacent
 // channels (one 16-byte load per row), TPR = C/8 threads cover a row, 256/TPR rows are in flight per pass and
 // every thread issues 4 independent row loads before it accumulates.  Partials meet in shared memory; one
-// global atomic per channel per CTA.  (The scalar kernels above took 5-8 us on 1 MB tensors: 16 dependent
-// 4-byte loads per thread.)
+// global atomic per channel per CTA.  (The scalar kernels above issue 16 dependent 4-byte loads per thread.)
 __device__ __forceinline__ void unpack8_bn(const uint4& u, float (&f)[8]) {
   const float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), c = unpack_bf16x2(u.z), d = unpack_bf16x2(u.w);
   f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y; f[4] = c.x; f[5] = c.y; f[6] = d.x; f[7] = d.y;
@@ -799,11 +798,11 @@ bn_bwd_reduce_vec_kernel(const uint4* __restrict__ x, const uint4* __restrict__ 
 }
 
 
-// ---- BatchNorm backward in ONE kernel with a device-wide barrier (opt-in: BATON_BN_BWD_FUSED=1; validated on B200,
-// ---- but slower than the cluster kernel below that became the default: 9.5 us vs 7.8 us for two kernels) -------
+// ---- BatchNorm backward in ONE kernel with a device-wide barrier (opt-in: BATON_BN_BWD_FUSED=1;
+// ---- the cluster kernel below is the default) -------
 // phase 1 = bn_bwd_reduce_vec (per-channel sum dy', sum dy' * xhat), device-wide barrier, phase 2 = bn_bwd_apply.
 // The activations of a 32x32-input ResNet layer are <= 1 MB, so the second read hits L2 and the kernel saves a
-// launch (~4-5 us of a ~9 us pair).  The barrier is a generation counter in global memory ({count, generation},
+// launch.  The barrier is a generation counter in global memory ({count, generation},
 // self-resetting, so CUDA-graph replays need no host reset).  Deadlock freedom: the grid is capped at two CTAs
 // per SM (always co-resident on an otherwise idle or draining GPU), and the programmatic-launch trigger for the
 // NEXT kernel is only given AFTER the barrier, so early-launched dependents can never occupy the SM slots that
@@ -917,8 +916,7 @@ bn_bwd_fused_kernel(const uint4* __restrict__ x, const uint4* __restrict__ y, co
 // registers; the per-channel sums (sum dy', sum dy' * xhat) are reduced warp -> CTA (shared memory) -> cluster
 // (distributed shared memory, fixed order: deterministic), and after one cluster barrier the same registers produce
 // dx (and dres = dy').  No device-wide barrier (the channel slices are independent), no second pass over global
-// memory, no workspace: the two-kernel reduce + apply pair (3.1 + 4.7 us in the captured ResNet-18 step, in-graph
-// timeline profiles/r2_trace_resnet18_*.txt) becomes one launch.
+// memory, no workspace: the two-kernel reduce + apply pair becomes one launch.
 // The gradient may arrive in TWO pieces (dy = dy_a + dy_b): a ResNet block input receives the main-branch dgrad and
 // the residual-branch gradient, and summing them here removes the separate add kernel.
 constexpr int BNC_CW = 16;        // channels per cluster
@@ -1095,7 +1093,7 @@ static inline int colred_rows_per_cta(long long rows, int C, int unroll) {
 
 static inline dim3 colred_grid(long long rows, int C) {
   long long gy = (rows + 127) / 128;
-  if (gy > 148) gy = 148;
+  if (gy > device_sm_count()) gy = device_sm_count();
   if (gy < 1) gy = 1;
   return dim3((C / 2 + 31) / 32, static_cast<unsigned>(gy));
 }
@@ -1318,7 +1316,7 @@ bn_maxpool_bwd_apply_kernel(const uint4* __restrict__ z, const uint4* __restrict
 static inline int stream_grid(long long nvec) {
   long long g = (nvec + 255) / 256;
   if (g < 1) g = 1;
-  if (g > 148 * 4) g = 148 * 4;
+  if (g > device_sm_count() * 4) g = device_sm_count() * 4;
   return static_cast<int>(g);
 }
 
@@ -1433,7 +1431,7 @@ extern "C" int b200_bn_bwd_cluster(const void* x, const void* y, const void* dy_
   const int slices = C / BNC_CW;
   int S = 1;
   while (S < max_cluster && (rows + S - 1) / S > BNC_LANES) S <<= 1;             // aim at one row per thread ...
-  while (S > 1 && static_cast<long long>(slices) * S > 2 * 148) S >>= 1;          // ... within two CTAs per SM
+  while (S > 1 && static_cast<long long>(slices) * S > 2 * device_sm_count()) S >>= 1;          // ... within two CTAs per SM
   const int rpc = static_cast<int>((rows + S - 1) / S);
   const int iters = (rpc + BNC_LANES - 1) / BNC_LANES;
   const dim3 grid(static_cast<unsigned>(slices), static_cast<unsigned>(S));
@@ -1447,8 +1445,8 @@ extern "C" int b200_bn_bwd_cluster(const void* x, const void* y, const void* dy_
   if (iters <= 4) BNC_GO(4);
   if (iters <= 8) BNC_GO(8);
   // More rows than the register cache holds (ResNet stem: 32768 rows x 64 channels): the uncached variant (ITER = 0,
-  // second pass re-reads) is correct but a 16-trip latency-bound loop per thread -- measured 45 us against 17 us for the
-  // grid-wide reduce + apply pair (in-graph timeline), so such shapes are handed back to the two-kernel path.
+  // second pass re-reads) is correct but a 16-trip latency-bound loop per thread, slower than the
+  // grid-wide reduce + apply pair, so such shapes are handed back to the two-kernel path.
   if (!allow_uncached) return -2;
   BNC_GO(0);
 #undef BNC_GO
@@ -1462,7 +1460,7 @@ extern "C" int b200_bn_bwd_fused(const void* x, const void* y, const void* dy, v
   if (!colred_vec_ok(C, x, relu ? y : nullptr, dy) || (reinterpret_cast<uintptr_t>(dx) & 15) || C > 2048) return -2;
   if (rows * C * 2 > (32ll << 20)) return -2;
   const int rpp = 256 / (C >> 3);
-  long long rpc = (rows + 2 * 148 - 1) / (2 * 148);          // at most two CTAs per SM: always co-resident
+  long long rpc = (rows + 2 * device_sm_count() - 1) / (2 * device_sm_count());          // at most two CTAs per SM: always co-resident
   rpc = (rpc + rpp - 1) / rpp * rpp;
   if (rpc < rpp) rpc = rpp;
   const unsigned grid = static_cast<unsigned>((rows + rpc - 1) / rpc);
@@ -1505,14 +1503,14 @@ extern "C" int b200_layernorm_bwd(const void* x, const void* dy, void* dx, const
   if (row_vec_ok(C, x, dy, dx) && (reinterpret_cast<uintptr_t>(gamma) & 15) == 0) {
     const int rpb = rows_per_block(C);
     long long gv = (rows + rpb - 1) / rpb;
-    if (gv > 148 * 2) gv = 148 * 2;
+    if (gv > device_sm_count() * 2) gv = device_sm_count() * 2;
 #define LN_BWD(LPR, VPL) launch_pdl(layernorm_bwd_vec_kernel<LPR, VPL>, static_cast<unsigned>(gv), 256, 2 * C * sizeof(float), stream, xp, gp, dp, gamma, mean, rstd, dgamma, dbeta, rows, C)
     ROW_DISPATCH(C, LN_BWD);
 #undef LN_BWD
     RET_LAST();
   }
   long long g = (rows + 7) / 8;
-  if (g > 148 * 2) g = 148 * 2;
+  if (g > device_sm_count() * 2) g = device_sm_count() * 2;
   launch_pdl(layernorm_bwd_kernel, static_cast<unsigned>(g), 256, 2 * C * sizeof(float), stream, xp, gp, dp, gamma, mean,
              rstd, dgamma, dbeta, rows, C);
   RET_LAST();

@@ -1,7 +1,7 @@
 // Programmatic Dependent Launch (PDL) helpers.
 //
 // A local-SGD step is ~200 small kernels in a dependency chain; at ~1 ms per step the per-node
-// launch latency and prologue (barrier init, TMEM alloc, descriptor prefetch, smem tables) is a
+// launch latency and prologue (barrier init, descriptor prefetch, smem tables) is a
 // large share of the time.  Every kernel of this library
 //   1. calls griddep_launch_dependents() first thing  -> the NEXT kernel in the stream / captured
 //      graph may become resident and run its prologue while this one is still executing, and
@@ -84,6 +84,17 @@ __device__ __forceinline__ void griddep_launch_dependents_tagged(long long tag) 
 #define griddep_wait() griddep_wait_tagged(static_cast<long long>(B200_TU_TAG) * 100000 + __LINE__)
 #define griddep_launch_dependents() griddep_launch_dependents_tagged(static_cast<long long>(B200_TU_TAG) * 100000 + __LINE__)
 
+// streaming multiprocessors of the current device (grid caps, one-wave thresholds, co-residency bounds)
+inline int device_sm_count() {
+  static int n = 0;
+  if (n == 0) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    if (n <= 0) n = 1;
+  }
+  return n;
+}
 inline bool pdl_enabled() {
   static int on = -1;
   if (on < 0) {

@@ -6,7 +6,7 @@
 //   quant_mx_cols : x[R, C] bf16  ->  q[C, Rp] e4m3 (TRANSPOSED), scales along R
 //                                                       (operand of a GEMM reducing over R: dgrad / wgrad)
 //
-// Scales are written directly in the 512-byte atom layout tcgen05 consumes (gemm_fp8.cu):
+// Scales are written directly in the 512-byte atom layout gemm_fp8.cu reads:
 //   atom(row_tile, k_tile)[ (row % 32) * 16 + ((row % 128) / 32) * 4 + (k % 128) / 32 ]
 #define B200_TU_TAG 3
 #include <cuda_fp8.h>
@@ -129,7 +129,7 @@ extern "C" int b200_quant_mx_rows(const void* x, void* q, void* sf, long long R,
   const long long Rpad = (R + 127) / 128 * 128;
   const int Cpad = (C + 127) / 128 * 128;
   long long blocks = (Rpad * (Cpad / 8) + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > device_sm_count() * 16) blocks = device_sm_count() * 16;
   launch_pdl(quant_mx_rows_kernel, static_cast<unsigned>(blocks), 256, 0, stream,
              reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<uint8_t*>(q), reinterpret_cast<uint8_t*>(sf), R, C,
              ld_in, Cp, Rpad, Cpad);
@@ -149,7 +149,7 @@ extern "C" int b200_dequant_mx(const void* q, const void* sf, float* out, long l
   if (R <= 0 || C <= 0) return 0;
   const int Cpad = (C + 127) / 128 * 128;
   long long blocks = (R * C + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > device_sm_count() * 8) blocks = device_sm_count() * 8;
   dequant_mx_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
       reinterpret_cast<const uint8_t*>(q), reinterpret_cast<const uint8_t*>(sf), out, R, C, Cp, Cpad);
   return static_cast<int>(cudaGetLastError());

@@ -5,7 +5,7 @@ every round draws ``n in [5, 20]``, ``X ~ N(0,1)`` of shape ``[32n, 10]`` and
 ``y = (p * X).sum(1)`` for a fixed ground-truth ``p`` (demo.py:55); the varying
 ``n_samples = 32n`` is what exercises the FedAvg weighting.
 
-Added for the BASELINE.json configs: class-conditional image shards (32x32) and
+Added for the benchmark configurations: class-conditional image shards (32x32) and
 token shards with three label partitions across K clients -- IID, label-skew
 (each client sees ``classes_per_client`` classes) and Dirichlet(alpha) non-IID
 (the standard FL benchmark partition; alpha=0.1 is highly skewed).

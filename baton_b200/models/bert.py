@@ -1,4 +1,4 @@
-"""BERT-base sequence classifier on the sm_100a layers (BASELINE.json config 3: the large
+"""BERT-base sequence classifier on the sm_90a layers (benchmark configuration: the large
 delta-reduce that stresses the NVLink roofline -- ~109.5 M parameters, 219 MB in bf16).
 
 Standard post-LN encoder (embeddings -> 12 x [self-attention, FFN] -> pooler -> classifier) with
@@ -6,7 +6,7 @@ the usual parameter names (``bert.embeddings.word_embeddings.weight``,
 ``bert.encoder.layer.N.attention.self.query.weight`` ... are folded into one packed
 ``attention.qkv`` projection here for a single GEMM; ``load_hf_state_dict`` / ``hf_state_dict`` map a stock
 Hugging-Face ``BertForSequenceClassification`` state_dict onto it and back, so HF checkpoints load and our
-checkpoints stay loadable by HF -- tests/test_bert_hf_compat.py).  Every matmul is the tcgen05
+checkpoints stay loadable by HF -- tests/test_bert_hf_compat.py).  Every matmul is the wgmma
 GEMM (GELU fused in the epilogue), attention is four strided-batched GEMMs + the softmax kernel on
 the packed QKV buffer, LayerNorm fuses the residual add.  Dropout is omitted (p = 0): the
 reference has none and synthetic-shard benchmarking does not want the noise.

@@ -2,7 +2,7 @@
 
 Parity target: demo ``Model`` = ``nn.Linear(10, 1)`` named "lineartest"
 (reference demo.py:15-24).  ``MLP2`` is the "2-layer MLP FedAvg, 2 workers on
-CPU/gloo via demo.py" plumbing model from BASELINE.json.
+CPU/gloo via demo.py" plumbing model of the benchmark configurations.
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""ResNet-18 / ResNet-50 on the sm_100a layers (BASELINE.json configs 2 and 4).
+"""ResNet-18 / ResNet-50 on the sm_90a layers.
 
 Architecture and ``state_dict`` keys follow the standard ImageNet-style ResNet
 (7x7/2 stem, 3x3/2 max-pool, four stages, global average pool, linear head), so
@@ -7,7 +7,7 @@ a stock PyTorch ResNet ``state_dict`` of the same depth loads unchanged -- the
 ResNet-18 float state is 11,191,242 elements (SURVEY.md section 5.1).
 
 Execution differs from a stock model: activations are bf16 NHWC, every
-convolution is im2col + tcgen05 GEMM, BatchNorm fuses the residual add and the
+convolution is im2col + wgmma GEMM, BatchNorm fuses the residual add and the
 ReLU of the block, parameters live in the flat arena.  The user-model contract
 (``name``, ``__hash__``, ``train(X, y, n_epoch=...)``) comes from
 ``FederatedModule`` (reference demo.py:15-49).
@@ -231,7 +231,7 @@ class ResNet(FederatedModule):
 
     # BATON_SGD_OVERLAP=1: parameters from this prefix on receive their gradients first, their optimizer slice runs beside
     # the rest of the backward pass.  "layer1." = everything but the stem (SGD beside the stem's backward + weight gradient,
-    # which leave most of the GPU idle); "layer3." = the deep layers only (88 % of a ResNet-18; measured neutral)
+    # which leave most of the GPU idle); "layer3." = the deep layers only (88 % of a ResNet-18's parameters)
     tail_split_prefix = __import__("os").environ.get("BATON_SGD_SPLIT", "layer1.")
 
     def explicit_step(self, x, target, loss_acc=None, hooks=None):

@@ -1,6 +1,6 @@
-"""Hand-written sm_100a kernels and the layers built on them.
+"""Hand-written sm_90a kernels and the layers built on them.
 
-``functional`` -- raw kernel wrappers (tcgen05 GEMM, fused SGD, im2col, ...)
+``functional`` -- raw kernel wrappers (wgmma GEMM, fused SGD, im2col, ...)
 ``nn``         -- layers with hand-written backward passes (Linear, Conv2d,
                   BatchNorm2d(+residual+ReLU), LayerNorm, pooling, losses)
 """

@@ -1,4 +1,4 @@
-"""Loader for the in-tree sm_100a extension (``baton_b200/_C.so``).
+"""Loader for the in-tree sm_90a extension (``baton_b200/_C.so``).
 
 The extension is the product: on a machine with a CUDA device every op in
 ``baton_b200.ops`` runs its hand-written kernel and a missing/unloadable
@@ -68,7 +68,7 @@ def load(build_if_missing: bool = False):
             _RAW = importlib.import_module("baton_b200._C")
     except Exception as exc:  # pragma: no cover - exercised only on broken installs
         raise RuntimeError(
-            "baton_b200._C (sm_100a kernels) is not available: {!r}. "
+            "baton_b200._C (sm_90a kernels) is not available: {!r}. "
             "Run `python -m baton_b200.build_ext`.".format(exc)) from exc
     _PROXY = _Counting(_RAW)
     return _PROXY

@@ -1,4 +1,4 @@
-"""Functional wrappers over the sm_100a kernels (shape logic + dispatch).
+"""Functional wrappers over the sm_90a kernels (shape logic + dispatch).
 
 Conventions
 -----------
@@ -18,7 +18,7 @@ import torch
 from ._ext import load
 
 BF16 = torch.bfloat16
-NUM_SMS = 148
+NUM_SMS = 132          # H100 SXM: wave counts of the dispatch heuristics below
 
 
 def _pitch(t: torch.Tensor) -> int:
@@ -31,17 +31,16 @@ def _tma_ok(t: torch.Tensor) -> bool:
 
 
 def pick_bn(M: int, N: int) -> int:
-    """Widest N tile that still yields >= one wave of CTAs; 64 for small problems."""
+    """Widest N tile the GEMM kernels instantiate (128) when it still yields enough CTAs; 64 for small problems.
+    The split-K heuristics below count output tiles with this width, so it must be the width that actually runs."""
     m_tiles = (M + 127) // 128
-    for bn in (256, 128):
-        if N >= bn and m_tiles * ((N + bn - 1) // bn) >= NUM_SMS:
-            return bn
+    if N >= 128 and m_tiles * ((N + 127) // 128) >= NUM_SMS:
+        return 128
     if N > 128 and m_tiles * ((N + 127) // 128) >= NUM_SMS // 2:
         return 128
     return 64
 
 
-# measured on B200 (captured ResNet-18 step, 8 steps): 148 -> 4.538 ms, 96 -> 4.503, 64 -> 4.481, 32 -> 4.557
 _WGRAD_MAX_CTAS = int(__import__("os").environ.get("BATON_WGRAD_MAX_CTAS", "64"))
 
 
@@ -61,11 +60,11 @@ def pick_cluster_k(M: int, N: int, K: int, bn: int) -> int:
     tiles = ((M + 127) // 128) * ((N + bn - 1) // bn)
     k_tiles = (K + 63) // 64
     min_kt = int(os.environ.get("BATON_GEMM_CLUSTER_MIN_KT", "4"))   # k tiles each CTA must keep
-    if min_kt <= 0 or k_tiles < 16:     # short main loops gain nothing (8192x64x576: 5.5 us plain vs 6.7 us split)
+    if min_kt <= 0 or k_tiles < 16:     # short main loops gain nothing from splitting
         return 1
     best = 1
     for s in (2, 4, 8):
-        # measured on B200: clusters of 8 only pay off while they cover at most ~half the SMs
+        # clusters of 8 only pay off while they cover at most ~half the SMs
         # (placement needs 8 free SMs inside one GPC); clusters of <= 4 are fine up to a full wave
         cap = NUM_SMS // 2 if s == 8 else 128
         if tiles * s <= cap and k_tiles >= min_kt * s:
@@ -80,7 +79,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
          flag_elem_off: int = 0, flag_tile_elems: int = 0, flag_bias_off: int = -1, force_bn: int = 0,
          force_simt: bool = False, col_stats: Optional[torch.Tensor] = None,
          flag_epoch_word: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """``out[M,N] = act(alpha * A @ B^T + bias)`` on tcgen05 tensor cores.
+    """``out[M,N] = act(alpha * A @ B^T + bias)`` on the tensor cores (wgmma).
 
     ``n_valid`` limits the written columns (used when B carries zero K-padding
     rows, e.g. the wgrad of a layer whose K was padded to a multiple of 8).
@@ -125,7 +124,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
 
 def gemm_stats_fusable(M: int, N: int, K: int) -> bool:
     """Can :func:`gemm` take column statistics of this problem in its epilogue?  Every bf16-output tensor-core
-    path can: single-pass tiles do it from the TMEM rows (butterfly column sums), cluster split-K in the DSMEM
+    path can: single-pass tiles do it from the staged accumulator rows (butterfly column sums), cluster split-K in the DSMEM
     reduction; only operands that fall back to the SIMT kernel (pitch not a multiple of 8) cannot."""
     return K % 8 == 0
 
@@ -411,7 +410,7 @@ def mse(pred: torch.Tensor, target: torch.Tensor, want_grad: bool = True):
 def gemm_batched(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, *, M: int, N: int, K: int, lda: int, ldb: int,
                  ldd: int, a_mn: bool, b_mn: bool, n_outer: int, n_inner: int, a_strides, b_strides, d_strides,
                  alpha: float = 1.0, act: int = 0, accumulate: bool = False) -> torch.Tensor:
-    """Strided-batched tcgen05 GEMM over a two-level batch (outer, inner) = (batch, head): operands are
+    """Strided-batched wgmma GEMM over a two-level batch (outer, inner) = (batch, head): operands are
     addressed through 4-D TMA tensor maps, so Q/K/V slices of a packed QKV buffer need no copies.
     ``*_strides`` = (outer, inner) element strides; ``a``/``b``/``out`` give the base pointers."""
     load().gemm_batched(a, b, out, M, N, K, lda, ldb, ldd, a_mn, b_mn, act, alpha, n_outer, n_inner,

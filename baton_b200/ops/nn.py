@@ -1,4 +1,4 @@
-"""Layers built on the sm_100a kernels, with hand-written backward passes.
+"""Layers built on the sm_90a kernels, with hand-written backward passes.
 
 Every layer keeps an fp32 master parameter (a view into the flat parameter
 arena once ``ParamArena`` has adopted the model) and consumes a bf16 shadow
@@ -291,7 +291,7 @@ class Linear(nn.Module):
 
 
 # ================================================================================ Conv2d (NHWC, implicit GEMM)
-# implicit-GEMM convolution (TMA im2col operands; validated on B200 in round 2, profiles/r2_validate_experimental.txt).
+# implicit-GEMM convolution (TMA im2col operands).
 # BATON_CONV_IGEMM=0 falls back to explicit im2col / col2im + GEMM.
 _CONV_IGEMM = __import__("os").environ.get("BATON_CONV_IGEMM", "1") == "1"
 _CONV_IGEMM_DGRAD = __import__("os").environ.get("BATON_CONV_IGEMM_DGRAD", "1") == "1"
@@ -732,19 +732,19 @@ def mse_loss(pred: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
 
 
 # ================================================================================ attention / embedding (BERT)
-_FUSED_ATTN = __import__("os").environ.get("BATON_FUSED_ATTN", "1") == "1"   # validated on hardware; +4.5 % on BERT-base (BASELINE.md)
+_FUSED_ATTN = __import__("os").environ.get("BATON_FUSED_ATTN", "1") == "1"
 
 
 class _AttnFn(torch.autograd.Function):
     """Multi-head self-attention core on a packed ``qkv [B*S, 3*H*dh]`` buffer: four strided-batched
-    tcgen05 GEMMs + the row-softmax kernel forward, five GEMMs + softmax backward; Q/K/V and their
+    wgmma GEMMs + the row-softmax kernel forward, five GEMMs + softmax backward; Q/K/V and their
     gradients are addressed in place through 4-D TMA maps (no head split / merge copies)."""
 
     @staticmethod
     def forward(ctx, qkv, B, S, H, dh, mask_bias=None):
         D = H * dh
         if _FUSED_ATTN and S == 128 and dh == 64 and mask_bias is None:
-            # single-kernel forward (csrc/attention.cu): scores stay in TMEM, P is written once
+            # single-kernel forward (csrc/attention.cu): scores stay in shared memory, P is written once
             probs = torch.empty((B * H * S, S), dtype=BF16, device=qkv.device)
             out = torch.empty((B * S, D), dtype=BF16, device=qkv.device)
             if load().attention_fwd(qkv, out, probs, B, S, H, dh, 1.0 / math.sqrt(dh)):

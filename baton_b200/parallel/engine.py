@@ -1,7 +1,7 @@
 """SPMD federated engine: one process per GPU, every rank is a federated client.
 
 This is the in-process counterpart of the HTTP control plane for jobs launched
-with ``torchrun`` on one NVSwitch box (the BASELINE.json ResNet / BERT configs).
+with ``torchrun`` on one NVSwitch box (the ResNet / BERT benchmark configurations).
 A *round* on every rank is
 
     (host -> device copy of this round's private shard, from pinned memory)
@@ -11,7 +11,7 @@ A *round* on every rank is
 
 with no host-side exchange between ranks: the sample counts n_k travel on the
 collective's barrier flags.  Client sampling / logical clients stay in Python
-(BASELINE.json: "client sampling and round bookkeeping stay in Python"): with
+(client sampling and round bookkeeping are host logic): with
 ``logical_clients > world`` each rank time-slices several logical clients and
 folds their sample-weighted deltas locally before the cross-GPU reduce; the
 per-round draw is a seeded ``random.Random`` shared by all ranks, so no
@@ -43,7 +43,7 @@ class RoundResult:
 class FederatedEngine:
     def __init__(self, model, device, *, backend: str = "fused", group=None, loss: str = "ce",
                  lr: float = 0.05, batch_size: int = 128, momentum: float = 0.0, weight_decay: float = 0.0,
-                 wire_dtype: str = "bf16", mode: str = "delta", n_ctas: int = 148, use_graph: bool = True,
+                 wire_dtype: str = "bf16", mode: str = "delta", n_ctas: Optional[int] = None, use_graph: bool = True,
                  logical_clients: int = 0, sample_k: Optional[int] = None, seed: int = 0, name: str = "exp",
                  nvls: "bool | str" = "auto", tile_flags: bool = False):
         self.device = torch.device(device)

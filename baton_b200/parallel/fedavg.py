@@ -23,7 +23,7 @@ from .arena import ParamArena
 from .symm import SymmetricBuffer
 
 MAX_LOSS = 64       # per-epoch loss slots carried through the collective
-MAX_CTAS = 296      # pad slots; the kernel runs one 512-thread CTA per SM (148 on B200), clamped by the launcher
+MAX_CTAS = 296      # pad slots; the kernel runs one 512-thread CTA per SM (132 on H100 SXM), clamped by the launcher
 
 
 def _align(x: int, a: int) -> int:
@@ -32,7 +32,7 @@ def _align(x: int, a: int) -> int:
 
 class FedAvgSession:
     def __init__(self, arena: ParamArena, group=None, *, wire_dtype: str = "bf16", mode: str = "delta",
-                 nvls: "bool | str" = "auto", n_ctas: int = 148, tile_elems: int = 0, timeout_log2: int = 24,
+                 nvls: "bool | str" = "auto", n_ctas: Optional[int] = None, tile_elems: int = 0, timeout_log2: int = 24,
                  reset_momentum: bool = True, tile_flags: bool = False):
         from ..ops._ext import load
         self._C = load()
@@ -44,6 +44,9 @@ class FedAvgSession:
         self.wire_bf16 = wire_dtype == "bf16"
         self.wire_kind = {"fp32": 0, "bf16": 1, "fp8": 2}[wire_dtype]
         self.delta = mode == "delta"
+        if n_ctas is None:   # one CTA per SM: the cooperative launch clamps the grid to what is co-resident
+            dev = torch.device(self.device)
+            n_ctas = torch.cuda.get_device_properties(dev).multi_processor_count if dev.type == "cuda" else 1
         self.n_ctas = max(1, min(int(n_ctas), MAX_CTAS))
         self.tile_elems = int(tile_elems)
         # every cross-GPU spin is BOUNDED by default (2^24 polls, several seconds): a seat that dies between the

@@ -93,11 +93,10 @@ class GraphedLocalSGD:
         self.input_dtype = input_dtype
         import os
         self.explicit = os.environ.get("BATON_EXPLICIT_STEP", "1") != "0"   # models that offer a hand-scheduled step
-        # optimizer slice of the deep layers beside the rest of the backward pass: implemented and validated, but measured
-        # neutral on B200 (the HBM-bound slice slows the latency-bound kernels it runs beside by as much as it
-        # hides: 4.52 vs 4.54 ms per 8 steps, profiles/r2_step_experiments.txt) -> opt-in
+        # optimizer slice of the deep layers beside the rest of the backward pass: opt-in (the HBM-bound slice slows the
+        # latency-bound kernels it runs beside)
         self.tail_overlap = os.environ.get("BATON_SGD_OVERLAP", "0") == "1"
-        self.tail_ctas = int(os.environ.get("BATON_SGD_TAIL_CTAS", "148"))    # grid cap of the overlapped SGD slice
+        self.tail_ctas = int(os.environ.get("BATON_SGD_TAIL_CTAS", "132"))    # grid cap of the overlapped SGD slice
         self.k3_join = None           # set by the engine: callable joining the round-end collective (enables the graph split)
         self._first_gemm_hook = None
         self.pack = None              # set by the engine: FedAvgSession.pack_spec() -> last SGD step emits the upload copy

@@ -10,8 +10,8 @@ done" stamps is the critical-path time of the earlier kernel *as it ran inside t
     tr = KernelTrace(capacity=1 << 16); tr.start(); graph.replay(); torch.cuda.synchronize()
     for row in tr.summary(): print(row)
 
-The reference has no tracing at all (SURVEY.md section 5); this is the "tracing / profiling" subsystem of the
-B200 build together with ``metrics.phase`` (NVTX ranges + CUDA-event timers).
+The reference has no tracing at all (SURVEY.md section 5); this is its "tracing / profiling" subsystem,
+together with ``metrics.phase`` (NVTX ranges + CUDA-event timers).
 """
 from __future__ import annotations
 
@@ -22,7 +22,7 @@ from typing import Dict, List, Tuple
 
 import torch
 
-_TUS = ["?", "gemm_tcgen05", "gemm_fp8", "quant", "attention", "im2col_tma", "gemm_simt", "fedavg", "elementwise",
+_TUS = ["?", "gemm_wgmma", "gemm_fp8", "quant", "attention", "im2col_tma", "gemm_simt", "fedavg", "elementwise",
         "conv", "norm", "loss"]
 _CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "csrc")
 _NAME_CACHE: Dict[int, str] = {}

@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""Flagship benchmark: ResNet-18 FedAvg on B200, one federated client per GPU.
+"""Flagship benchmark: ResNet-18 FedAvg on H100, one federated client per GPU.
 
     python bench.py --gpus N --steps K --warmup W           (N > 1: launched under torchrun)
+    python bench.py ... --dump-outputs DIR                   (also write what the last timed round computed)
 
-One *step* is one federated round (BASELINE.json config 2):
+One *step* is one federated round:
     local SGD over the client's private synthetic non-IID shard (local_epochs=1, bf16)
     -> fused weighted reduce + broadcast + running-mean apply over NVLink (ONE kernel, no NCCL)
 ``value`` = local samples/s summed over all N clients (weak scaling: per-client work is fixed),
@@ -13,7 +14,7 @@ per-epoch loss read back device->host EVERY round.
 
 ``--impl reference`` runs the unmodified reference (baseline/reference_arm.py, nothing of this
 package on that path); ``--impl baseline`` runs the same algorithm on stock PyTorch ops with the
-round-end reduce done by NCCL (the "reference's own NCCL build" of BASELINE.json).
+round-end reduce done by NCCL.
 """
 from __future__ import annotations
 
@@ -26,6 +27,7 @@ import sys
 import time
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
+DUMP_MAX_ELEMS = 16 << 20          # 64 MB of float32
 
 
 def parse_args(argv=None):
@@ -47,7 +49,7 @@ def parse_args(argv=None):
     ap.add_argument("--dtype", default="bf16", choices=["bf16", "fp8"],
                     help="fp8 = block-scaled MXFP8 convolutions (fwd/dgrad/wgrad), everything else bf16/fp32")
     ap.add_argument("--backend", default="fused", choices=["fused", "nccl"])
-    ap.add_argument("--n-ctas", type=int, default=148)
+    ap.add_argument("--n-ctas", type=int, default=132)
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--bcast-gemm", type=int, default=int(os.environ.get("BATON_BCAST_GEMM", "0")),
                     help="1: K3 -- the head of the next round's captured epoch (batch gather, im2col, flag-gated weight staging "
@@ -61,11 +63,15 @@ def parse_args(argv=None):
     ap.add_argument("--logical-clients", type=int, default=0,
                     help="> n_gpus: time-slice this many logical clients over the GPUs (sampling sweep config)")
     ap.add_argument("--sample-k", type=int, default=None, help="logical clients sampled per round")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed rounds, write the global model the last one produced to DIR/*.npy (float32; "
+                         "a fixed seeded sample above %d parameters) so two builds can be compared output for output"
+                         % DUMP_MAX_ELEMS)
     return ap.parse_args(argv)
 
 
 class ClockSampler:
-    """nvidia-smi sampler running DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampler running DURING the timed region (SM clock, power, throttle reasons)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -122,6 +128,23 @@ def _claim_stdout():
 
 def _emit(real_fd: int, obj) -> None:
     os.write(real_fd, (json.dumps(obj) + "\n").encode())
+
+
+def _dump_outputs(out_dir: str, arena) -> None:
+    """The global model after the last timed round -- what ``run_round`` hands the next round and the caller --
+    as float32 .npy.  Models above DUMP_MAX_ELEMS parameters are sampled at fixed positions: an even stride with a
+    seeded offset inside each stride, so the sample costs O(DUMP_MAX_ELEMS) and is the same in every run."""
+    import numpy as np
+    import torch
+    w = (arena.global_w if arena.global_w is not None else arena.theta)[: arena.n_param].detach().float()
+    n = w.numel()
+    if n > DUMP_MAX_ELEMS:
+        stride = n // DUMP_MAX_ELEMS
+        g = torch.Generator().manual_seed(0)
+        idx = torch.arange(DUMP_MAX_ELEMS, dtype=torch.int64) * stride + torch.randint(0, stride, (DUMP_MAX_ELEMS,), generator=g)
+        w = w[idx.to(w.device)]
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "global_weights.npy"), w.cpu().numpy().astype(np.float32))
 
 
 def main(argv=None):
@@ -193,7 +216,7 @@ def main(argv=None):
         resident = lambda cid: dev_shards[cid]      # noqa: E731
         pinned = lambda cid: host_shards[cid]       # noqa: E731
     h2d = FederatedEngine.h2d_bytes(X_host, y_host)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 50 MB L2
 
     def barrier():
         if world > 1:
@@ -240,6 +263,8 @@ def main(argv=None):
     barrier()
     dev_ms = e0.elapsed_time(e1)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        _dump_outputs(args.dump_outputs, eng.arena)
     launches = total_launches() - c_before
     kpe = getattr(eng.trainer, "kernels_per_epoch", 0) or 0
     graph_launches = args.steps * args.local_epochs * kpe     # kernels replayed from the captured epoch graph
@@ -336,17 +361,18 @@ def _roofline(agg_us: float, wire_bytes: int, world: int, link_gbps=None):
     """Fraction of the NVLink roofline achieved by the fused reduce+broadcast: bytes that must cross
     one GPU's links in each direction = (K-1)/K * |wire| (reduce-scatter pull and broadcast push use opposite
     directions), over the per-direction bandwidth measured on THIS box by ``SymmetricBuffer.measure_link_gbps``
-    (fallback: the 770 GB/s of B200_PROFILING.md).  For K = 1 the bound is local HBM."""
+    (fallback: 450 GB/s, half the 900 GB/s NVLink of the H100 SXM data sheet).  For K = 1 the bound is local HBM
+    (3.35 TB/s, H100 SXM data sheet)."""
     if agg_us <= 0:
         return None
     if world <= 1:
         bytes_hbm = wire_bytes * (2 + 2 + 2 + 2 + 1)   # pack r/w, reduce r/w, apply: read wire, write theta/global/bf16
-        floor_us = bytes_hbm / 6482.7e9 * 1e6
+        floor_us = bytes_hbm / 3.35e12 * 1e6
         return {"bound": "hbm", "floor_us": floor_us, "fraction_of_measured": floor_us / agg_us}
     inbound = (world - 1) / world * wire_bytes
-    bw = (link_gbps or 770.0) * 1e9
+    bw = (link_gbps or 450.0) * 1e9
     floor_us = inbound / bw * 1e6             # pull and push use opposite directions concurrently
-    return {"bound": "nvlink {:.0f} GB/s/dir ({})".format(bw / 1e9, "measured in this run" if link_gbps else "B200_PROFILING.md"),
+    return {"bound": "nvlink {:.0f} GB/s/dir ({})".format(bw / 1e9, "measured in this run" if link_gbps else "H100 SXM data sheet"),
             "floor_us": floor_us, "fraction_of_measured": floor_us / agg_us}
 
 

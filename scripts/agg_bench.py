@@ -30,7 +30,7 @@ def main():
         dist.init_process_group("nccl", device_id=dev)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     rows = []
-    ctas_list = [int(x) for x in os.environ.get("AGG_CTAS", "148").split(",")]
+    ctas_list = [int(x) for x in os.environ.get("AGG_CTAS", "132").split(",")]
     models = os.environ.get("AGG_MODELS", ",".join(SIZES)).split(",")
     wires = os.environ.get("AGG_WIRES", "bf16,fp32,fp8").split(",")
     for name, n in SIZES.items():
@@ -75,11 +75,11 @@ def main():
                     dist.all_reduce(t, op=dist.ReduceOp.MAX)
                 wire_bytes = arena.n * (2 if wire == "bf16" else 4) if wire != "fp8" else arena.n + arena.n // 32
                 if world > 1:
-                    floor = (world - 1) / world * wire_bytes / 770e9 * 1e6
-                    bound = "nvlink770"
+                    floor = (world - 1) / world * wire_bytes / 450e9 * 1e6     # H100 SXM NVLink, per direction
+                    bound = "nvlink450"
                 else:
                     fp = arena.n * 4
-                    floor = (2 * fp + wire_bytes + 2 * wire_bytes + wire_bytes + fp + 2 * fp + arena.n * 2) / 6482.7e9 * 1e6
+                    floor = (2 * fp + wire_bytes + 2 * wire_bytes + wire_bytes + fp + 2 * fp + arena.n * 2) / 3.35e12 * 1e6   # H100 SXM HBM3
                     bound = "hbm"
                 rows.append({"model": name, "elems": arena.n, "wire": wire, "variant": label, "ctas": ctas,
                              "us_best": float(t[0]), "us_mean": float(t[1]), "floor_us": floor, "bound": bound,

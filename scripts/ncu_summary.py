@@ -1,4 +1,4 @@
-"""Summarise .ncu-rep files (read on the GPU-less host with `ncu -i`) into profiles/*.txt."""
+"""Summarise .ncu-rep files (read on the GPU-less host with `ncu -i`) into text tables."""
 import csv
 import subprocess
 import sys

@@ -1,7 +1,7 @@
 """Per-kernel SASS comparison between a git revision and the working tree (GPU-less check that a refactor did
 not touch the instruction stream of kernels that were already validated on hardware).
 
-    python scripts/sass_diff.py <git-rev>          # e.g. the last commit that ran on a B200
+    python scripts/sass_diff.py <git-rev>          # e.g. the last commit validated on the GPU
 
 Compiles every csrc/*.cu of <git-rev> into a temp dir, hashes the instruction text of every kernel (addresses and
 encodings stripped) and compares with baton_b200/csrc/build/*.o.  A trailing `, 0` template argument that was
@@ -14,7 +14,7 @@ import sys
 import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--use_fast_math"]
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--use_fast_math"]
 
 
 def kernel_hashes(obj):

@@ -1,5 +1,5 @@
 """Where does a latency-bound conv GEMM spend its ~3-7 us?  Intra-kernel %globaltimer stamps (trace build) of the fixed
-tcgen05 kernel inside a captured chain conv -> bn_apply -> conv ..., printed as offsets from the moment the kernel's
+GEMM kernel inside a captured chain conv -> bn_apply -> conv ..., printed as offsets from the moment the kernel's
 dependencies completed.   BATON_TRACE=1 python scripts/trace_gemm_anatomy.py"""
 import collections
 import os

@@ -177,7 +177,7 @@ def main():
     x = torch.randn(256, 512, device=dev).to(BF16)
     sess.aggregate(my_n=1.0, on_side_stream=True)
     sess.gate_first_layer(net.fc1)
-    y = net.fc1(x)                     # tcgen05 GEMM whose TMA producer acquires the tile flags
+    y = net.fc1(x)                     # wgmma GEMM whose TMA producer acquires the tile flags
     sess.join()
     torch.cuda.synchronize()
     ref = torch.relu(x.float() @ net.fc1.weight.detach().to(BF16).float().t() + net.fc1.bias.detach())

@@ -1,4 +1,4 @@
-"""BERT tier: strided-batched tcgen05 GEMM, fused attention core, embedding, and the BERT encoder
+"""BERT tier: strided-batched wgmma GEMM, fused attention core, embedding, and the BERT encoder
 against fp32 PyTorch references."""
 import math
 import os

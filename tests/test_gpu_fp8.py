@@ -1,4 +1,4 @@
-"""MXFP8 tier: quantisers (rows / fused transpose) and the block-scaled tcgen05 GEMM against a
+"""MXFP8 tier: quantisers (rows / fused transpose) and the block-scaled wgmma GEMM against a
 dequantise-then-fp32-matmul reference (exact up to accumulation order)."""
 import pytest
 import torch
@@ -116,15 +116,33 @@ def test_resnet18_trains_in_mxfp8_under_cuda_graph():
         arena = ParamArena(m, dev, momentum=True)
         m.build_workspace(dev)
         m._graphed_trainer = GraphedLocalSGD(m, arena, loss="ce")
-        return m.train(X, y, n_epoch=6, lr=0.05, batch_size=128, momentum=0.9)
+        return m, m.train(X, y, n_epoch=6, lr=0.05, batch_size=128, momentum=0.9)
 
-    # Typical history: 1.29, 0.07, 0.003, ... (18 / 18 isolated runs, also with a NaN-poisoned allocator:
-    # scripts/poison_fp8.py).  ONE run inside the full suite did not meet the bound and could not be reproduced, so a
-    # failed attempt is reported loudly and repeated once instead of failing the whole run on it (DESIGN.md section 7).
-    hist = attempt()
+    def evidence(m, hist):
+        """What a non-converging run looked like: loss history, non-finite parameters, and the fp8 GEMM of this
+        process at the ResNet-18 layer shapes against the dequantise-then-fp32 reference."""
+        from baton_b200.ops import functional as F
+        bad = [n for n, p in m.named_parameters() if not bool(torch.isfinite(p).all())]
+        errs = {}
+        g = torch.Generator(device=dev).manual_seed(1)
+        for M, N, K in [(8192, 64, 576), (2048, 128, 1152), (512, 256, 2304), (128, 512, 4608)]:
+            a = torch.randn(M, K, device=dev, generator=g).to(BF16)
+            b = torch.randn(N, K, device=dev, generator=g).to(BF16)
+            qa, sa = F.quant_mx_rows(a)
+            qb, sb = F.quant_mx_rows(b)
+            ref = F.dequant_mx(qa, sa, K) @ F.dequant_mx(qb, sb, K).t()
+            errs["{}x{}x{}".format(M, N, K)] = _rel(F.gemm_fp8(qa, sa, qb, sb, K, out_dtype=torch.float32), ref)
+        return "history {} non-finite parameters {} fp8 GEMM rel. error {}".format(hist, bad[:8], errs)
+
+    # Typical history: 1.29, 0.07, 0.003, ...  An intermittent non-converging run inside the full suite is recorded in
+    # DESIGN.md ("Known issue"); a failed attempt reports its evidence and is repeated once, and the assertion message
+    # carries the evidence of both attempts.
+    m, hist = attempt()
+    first = None
     if not (hist[-1] < hist[0] * 0.8):
         import warnings
-        warnings.warn("MXFP8 ResNet-18 training attempt 1 did not converge: {}".format(hist))
+        first = evidence(m, hist)
+        warnings.warn("MXFP8 ResNet-18 training attempt 1 did not converge: " + first)
         torch.cuda.synchronize()
-        hist = attempt()
-    assert hist[-1] < hist[0] * 0.8, hist
+        m, hist = attempt()
+    assert hist[-1] < hist[0] * 0.8, "attempt 1: {}; attempt 2: {}".format(first, evidence(m, hist))

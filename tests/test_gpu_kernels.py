@@ -1,4 +1,4 @@
-"""Kernel-correctness tier: every sm_100a kernel against a plain PyTorch fp32
+"""Kernel-correctness tier: every sm_90a kernel against a plain PyTorch fp32
 reference of the same op (SURVEY.md section 4)."""
 import math
 import os
@@ -113,7 +113,7 @@ def test_gemm_cluster_split_k_dsmem_reduce(F, S, M, N, K, bn):
 @pytest.mark.parametrize("a_mn,b_mn", [(False, False), (False, True), (True, True)])
 @pytest.mark.parametrize("M,N,K", [(4096, 2304, 768), (4104, 2000, 520), (8192, 1024, 256)])
 def test_gemm_persistent_path(F, a_mn, b_mn, M, N, K):
-    """>= 148 output tiles: persistent CTAs, two TMEM accumulator stages (epilogue overlaps the next tile)."""
+    """>= one wave of output tiles: persistent CTAs, the TMA producer runs ahead across tile boundaries."""
     torch.manual_seed(M + N)
     dev = _dev()
     A = torch.randn(M, K, device=dev).to(BF16)
@@ -133,8 +133,8 @@ def test_gemm_persistent_path(F, a_mn, b_mn, M, N, K):
 
 @pytest.mark.parametrize("a_mn,b_mn", [(False, False), (True, True)])
 def test_gemm_two_cta_pairs(F, a_mn, b_mn):
-    """Deep-K, multi-wave problem: dispatched to the cta_group::2 kernel (CTA pairs share 256 x 256 tiles,
-    each CTA loads half of B, one elected thread issues the MMAs for both SMs)."""
+    """Deep-K, multi-wave problem with a ragged N tile (a shape the CTA-pair kernel of the Blackwell build served;
+    on Hopper it runs on the persistent kernel)."""
     torch.manual_seed(5)
     dev = _dev()
     M, N, K = 4096, 2560 - 8, 2048 + 64          # ragged N tile, K not a multiple of the stage count

@@ -1,5 +1,5 @@
 """Host-side dispatch heuristics of the tensor-core GEMM (pure Python, no GPU): pinned to the shapes they were
-tuned on (BASELINE.md, profiles/r1_gemm_variants.md) so a refactor cannot silently change a measured path."""
+tuned on so a refactor cannot silently change a measured path."""
 import torch
 
 from baton_b200.ops import functional as F
@@ -7,9 +7,9 @@ from baton_b200.ops import nn as bnn
 
 
 def test_tile_width_tracks_the_wave_count():
-    assert F.pick_bn(8192, 8192) == 256          # big GEMM: widest tile, still many waves
-    assert F.pick_bn(16384, 2304) == 256         # BERT qkv at batch 128 x seq 128
-    assert F.pick_bn(4096, 768) == 128           # 32 x 6 = 192 tiles of 128 beat 96 tiles of 256
+    assert F.pick_bn(8192, 8192) == 128          # big GEMM: the widest tile the kernels instantiate
+    assert F.pick_bn(16384, 2304) == 128         # BERT qkv at batch 128 x seq 128
+    assert F.pick_bn(4096, 768) == 128           # 32 x 6 = 192 tiles of 128
     assert F.pick_bn(8192, 64) == 64             # ResNet layer1
     assert F.pick_bn(128, 512) == 64             # ResNet layer4 at 32x32 inputs: few rows, keep CTAs many
 
@@ -20,7 +20,7 @@ def test_cluster_split_k_only_for_deep_few_tile_problems():
     assert F.pick_cluster_k(2048, 128, 1152, 64) == 4        # layer2
     assert F.pick_cluster_k(512, 256, 2304, 64) == 4         # layer3
     assert F.pick_cluster_k(128, 512, 4608, 64) == 8         # layer4: 8 tiles x 8 = 64 CTAs <= half the SMs
-    assert F.pick_cluster_k(8192, 8192, 8192, 256) == 1      # never for problems that fill the machine
+    assert F.pick_cluster_k(8192, 8192, 8192, 128) == 1      # never for problems that fill the machine
 
 
 def test_atomic_split_k_for_weight_gradients():
