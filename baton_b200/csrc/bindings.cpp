@@ -24,6 +24,20 @@ inline T* opt_ptr(const std::optional<at::Tensor>& t) {
 }
 #define CHECK_CUDA(x) TORCH_CHECK((x).is_cuda(), #x " must be a CUDA tensor")
 
+// optimizer epilogue of a weight-gradient GEMM: theta / theta_bf16 / momentum start at the element of D[0, 0]
+inline std::optional<B200SgdEpilogue> sgd_epilogue(const std::optional<at::Tensor>& theta,
+                                                   const std::optional<at::Tensor>& theta_bf16,
+                                                   const std::optional<at::Tensor>& mom,
+                                                   const std::optional<at::Tensor>& hyper, bool nesterov) {
+  if (!hyper.has_value() || !hyper->defined()) return std::nullopt;
+  TORCH_CHECK(theta.has_value() && theta->scalar_type() == at::kFloat && hyper->scalar_type() == at::kFloat &&
+                  (!theta_bf16.has_value() || theta_bf16->scalar_type() == at::kBFloat16) &&
+                  (!mom.has_value() || mom->scalar_type() == at::kFloat),
+              "sgd epilogue: fp32 theta / momentum / hyper, bf16 shadow");
+  return B200SgdEpilogue{theta->data_ptr<float>(), opt_ptr<void>(theta_bf16), opt_ptr<float>(mom),
+                         hyper->data_ptr<float>(), nesterov ? 1 : 0};
+}
+
 // ---- in-graph kernel timeline (pdl.cuh): every translation unit owns a copy of the trace pointer
 extern "C" {
 #define B200_TRACE_TUS(X) X(gemm_wgmma) X(gemm_fp8) X(quant) X(attention) X(im2col_tma) X(gemm_simt) X(fedavg) \
@@ -48,11 +62,14 @@ bool trace_set(const std::optional<at::Tensor>& buf) {
   return rc == 0;
 }
 
-void gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor d, const std::optional<at::Tensor>& bias, int64_t M,
+// false: the optimizer epilogue was requested and declined (nothing was written)
+bool gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor d, const std::optional<at::Tensor>& bias, int64_t M,
           int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldd, bool a_mn, bool b_mn, int64_t act,
           int64_t split_k, bool accumulate, double alpha, const std::optional<at::Tensor>& flags, int64_t flag_epoch,
           int64_t flag_elem_off, int64_t flag_tile_elems, int64_t flag_bias_off, int64_t force_bn, bool simt,
-          const std::optional<at::Tensor>& col_stats, const std::optional<at::Tensor>& flag_epoch_word) {
+          const std::optional<at::Tensor>& col_stats, const std::optional<at::Tensor>& flag_epoch_word,
+          const std::optional<at::Tensor>& sgd_theta, const std::optional<at::Tensor>& sgd_theta_bf16,
+          const std::optional<at::Tensor>& sgd_mom, const std::optional<at::Tensor>& sgd_hyper, bool sgd_nesterov) {
   CHECK_CUDA(a); CHECK_CUDA(b); CHECK_CUDA(d);
   TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16, "gemm operands must be bf16");
   TORCH_CHECK(d.scalar_type() == at::kBFloat16 || d.scalar_type() == at::kFloat, "gemm output must be bf16/fp32");
@@ -62,17 +79,21 @@ void gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor d, const std::opt
   TORCH_CHECK(!col_stats.has_value() || (!simt && col_stats->scalar_type() == at::kFloat && col_stats->numel() >= 2 * N),
               "col_stats needs the tensor-core path and a [2N] fp32 buffer");
   if (simt) {
+    TORCH_CHECK(!sgd_hyper.has_value(), "the SIMT GEMM has no optimizer epilogue");
     check(b200_gemm_simt(cptr(a), cptr(b), ptr(d), bp, M, N, K, lda, ldb, ldd, a_mn, b_mn, out_fp32, act, accumulate,
                          static_cast<float>(alpha), cur_stream()),
           "gemm_simt");
-    return;
+    return true;
   }
-  check(b200_gemm_bf16(cptr(a), cptr(b), ptr(d), bp, M, N, K, lda, ldb, ldd, a_mn, b_mn, out_fp32, act, split_k,
-                       accumulate, static_cast<float>(alpha), opt_ptr<const uint32_t>(flags),
-                       static_cast<uint32_t>(flag_epoch), flag_elem_off, static_cast<int>(flag_tile_elems), flag_bias_off,
-                       static_cast<int>(force_bn), opt_ptr<float>(col_stats), opt_ptr<const uint32_t>(flag_epoch_word),
-                       cur_stream()),
-        "gemm_bf16");
+  const std::optional<B200SgdEpilogue> sgd = sgd_epilogue(sgd_theta, sgd_theta_bf16, sgd_mom, sgd_hyper, sgd_nesterov);
+  const int rc = b200_gemm_bf16(cptr(a), cptr(b), ptr(d), bp, M, N, K, lda, ldb, ldd, a_mn, b_mn, out_fp32, act, split_k,
+                                accumulate, static_cast<float>(alpha), opt_ptr<const uint32_t>(flags),
+                                static_cast<uint32_t>(flag_epoch), flag_elem_off, static_cast<int>(flag_tile_elems),
+                                flag_bias_off, static_cast<int>(force_bn), opt_ptr<float>(col_stats),
+                                opt_ptr<const uint32_t>(flag_epoch_word), sgd ? &*sgd : nullptr, cur_stream());
+  if (rc == B200_SGD_EPILOGUE_DECLINED) return false;
+  check(rc, "gemm_bf16");
+  return true;
 }
 
 void gemm_batched(const at::Tensor& a, const at::Tensor& b, at::Tensor d, int64_t M, int64_t N, int64_t K, int64_t lda,
@@ -167,18 +188,22 @@ bool conv_igemm_dgrad(const at::Tensor& dy, const at::Tensor& w, at::Tensor dx, 
   return true;
 }
 bool conv_igemm_wgrad(const at::Tensor& dy, const at::Tensor& x, at::Tensor dw, int64_t cout, int64_t kh, int64_t kw,
-                      int64_t stride, int64_t pad, int64_t ho, int64_t wo, int64_t split_k, int64_t force_bn) {
+                      int64_t stride, int64_t pad, int64_t ho, int64_t wo, int64_t split_k, int64_t force_bn,
+                      const std::optional<at::Tensor>& sgd_theta, const std::optional<at::Tensor>& sgd_theta_bf16,
+                      const std::optional<at::Tensor>& sgd_mom, const std::optional<at::Tensor>& sgd_hyper,
+                      bool sgd_nesterov) {
   CHECK_CUDA(dy); CHECK_CUDA(x); CHECK_CUDA(dw);
   TORCH_CHECK(x.scalar_type() == at::kBFloat16 && dy.scalar_type() == at::kBFloat16 && dw.scalar_type() == at::kFloat &&
               x.dim() == 4 && x.is_contiguous() && dy.is_contiguous());
   const c10::cuda::CUDAGuard guard(x.device());
+  const std::optional<B200SgdEpilogue> sgd = sgd_epilogue(sgd_theta, sgd_theta_bf16, sgd_mom, sgd_hyper, sgd_nesterov);
   const int rc = b200_conv_igemm_wgrad(cptr(dy), cptr(x), dw.data_ptr<float>(), static_cast<int>(x.size(0)),
                                        static_cast<int>(x.size(1)), static_cast<int>(x.size(2)), static_cast<int>(x.size(3)),
                                        static_cast<int>(cout), static_cast<int>(kh), static_cast<int>(kw),
                                        static_cast<int>(stride), static_cast<int>(pad), static_cast<int>(ho),
                                        static_cast<int>(wo), static_cast<int>(split_k), static_cast<int>(force_bn),
-                                       cur_stream());
-  if (rc == -2) return false;
+                                       sgd ? &*sgd : nullptr, cur_stream());
+  if (rc == -2 || rc == B200_SGD_EPILOGUE_DECLINED) return false;
   check(rc, "conv_igemm_wgrad");
   return true;
 }
@@ -223,6 +248,21 @@ void fused_sgd(at::Tensor w, at::Tensor g, const std::optional<at::Tensor>& mom,
                        reinterpret_cast<const unsigned long long*>(opt_ptr<const int64_t>(wire_slot)),
                        opt_ptr<const float>(pack_global), opt_ptr<const float>(pack_scale), n_pack, wire_fp32, cur_stream()),
         "fused_sgd");
+}
+
+// segments: int64 [n][3] device table {offset, length, kind} over the arena (see fused_sgd_segments_kernel)
+void fused_sgd_segments(at::Tensor w, at::Tensor g, const std::optional<at::Tensor>& mom,
+                        const std::optional<at::Tensor>& wb, const at::Tensor& segments, const at::Tensor& hyper,
+                        bool nesterov) {
+  CHECK_CUDA(w); CHECK_CUDA(segments);
+  TORCH_CHECK(w.scalar_type() == at::kFloat && g.scalar_type() == at::kFloat && hyper.scalar_type() == at::kFloat);
+  TORCH_CHECK(segments.scalar_type() == at::kLong && segments.dim() == 2 && segments.size(1) == 3 &&
+              segments.is_contiguous(), "segments: contiguous int64 [n, 3]");
+  const c10::cuda::CUDAGuard guard(w.device());
+  check(b200_fused_sgd_segments(w.data_ptr<float>(), g.data_ptr<float>(), opt_ptr<float>(mom), opt_ptr<void>(wb),
+                                reinterpret_cast<const long long*>(segments.data_ptr<int64_t>()),
+                                static_cast<int>(segments.size(0)), hyper.data_ptr<float>(), nesterov, cur_stream()),
+        "fused_sgd_segments");
 }
 
 void fold_client(at::Tensor acc, at::Tensor theta, const at::Tensor& global_w, const std::optional<at::Tensor>& wb,
@@ -648,6 +688,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("quant_mx_cols", &quant_mx_cols);
   m.def("dequant_mx", &dequant_mx);
   m.def("fused_sgd", &fused_sgd);
+  m.def("fused_sgd_segments", &fused_sgd_segments);
   m.def("weighted_sum", &weighted_sum);
   m.def("fold_client", &fold_client);
   m.def("cast", &cast);

@@ -6,6 +6,7 @@
 #include "launch.h"
 #include "pdl.cuh"
 #include "ptx.cuh"
+#include "sgd.cuh"
 
 namespace b200 {
 
@@ -18,9 +19,8 @@ static inline int ew_grid(long long n_vec, int max_ctas = device_sm_count() * 8)
 }
 
 // ------------------------------------------------------------------ fused SGD over the arena
-// One pass over {w, g, m}: g' = g + wd*w ; m = mu*m + (1-damp)*g' ; step = nesterov ? g' + mu*m : m ;
-// w -= lr*step ; g = 0 (so split-K wgrad GEMMs can red.add into it next step) ; bf16 shadow = bf16(w).
-// Hyper-parameters come from device memory so a captured CUDA graph can be replayed with a new lr.
+// One pass over {w, g, m}: the update of sgd.cuh ; g = 0 (so split-K wgrad GEMMs can red.add into it next step) ;
+// bf16 shadow = bf16(w).
 // K4 "emit the upload copy" (SURVEY 2.6): the LAST step of a local epoch can also write this client's wire copy for the
 // round-end collective -- bf16 / fp32 of (w_new - global) * scale -- while w_new is still in registers, so the
 // collective's own pack phase (one more read of theta + global, ~10 B / element) disappears.  The wire address is
@@ -41,7 +41,7 @@ fused_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict
                  int nesterov, const SgdPack pk) {
   griddep_launch_dependents();
   griddep_wait();
-  const float lr = hyper[0], mu = hyper[1], wd = hyper[2], damp = hyper[3];
+  const SgdHyper h = load_sgd_hyper(hyper);
   const long long nv = n >> 2;
   uint8_t* wire = nullptr;
   float pscale = 1.f;
@@ -51,26 +51,10 @@ fused_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict
   }
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < nv;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    float4 wv = reinterpret_cast<float4*>(w)[i];
-    float4 gv = reinterpret_cast<float4*>(g)[i];
-    gv.x = fmaf(wd, wv.x, gv.x); gv.y = fmaf(wd, wv.y, gv.y);
-    gv.z = fmaf(wd, wv.z, gv.z); gv.w = fmaf(wd, wv.w, gv.w);
-    float4 st = gv;
-    if (mom != nullptr) {
-      float4 mv = reinterpret_cast<float4*>(mom)[i];
-      const float od = 1.f - damp;
-      mv.x = fmaf(mu, mv.x, od * gv.x); mv.y = fmaf(mu, mv.y, od * gv.y);
-      mv.z = fmaf(mu, mv.z, od * gv.z); mv.w = fmaf(mu, mv.w, od * gv.w);
-      reinterpret_cast<float4*>(mom)[i] = mv;
-      if (nesterov) {
-        st.x = fmaf(mu, mv.x, gv.x); st.y = fmaf(mu, mv.y, gv.y);
-        st.z = fmaf(mu, mv.z, gv.z); st.w = fmaf(mu, mv.w, gv.w);
-      } else {
-        st = mv;
-      }
-    }
-    wv.x = fmaf(-lr, st.x, wv.x); wv.y = fmaf(-lr, st.y, wv.y);
-    wv.z = fmaf(-lr, st.z, wv.z); wv.w = fmaf(-lr, st.w, wv.w);
+    float4 mv = mom != nullptr ? reinterpret_cast<float4*>(mom)[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 wv = sgd_update4(h, reinterpret_cast<float4*>(w)[i], reinterpret_cast<float4*>(g)[i], mv,
+                                  mom != nullptr, nesterov);
+    if (mom != nullptr) reinterpret_cast<float4*>(mom)[i] = mv;
     reinterpret_cast<float4*>(w)[i] = wv;
     if (zero_grad) reinterpret_cast<float4*>(g)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     if (wb != nullptr) reinterpret_cast<uint2*>(wb)[i] = make_uint2(pack_bf16x2(wv.x, wv.y), pack_bf16x2(wv.z, wv.w));
@@ -102,17 +86,60 @@ fused_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict
   // scalar tail (n is normally padded to a multiple of 4 by the arena)
   if (blockIdx.x == 0) {
     for (long long i = (nv << 2) + threadIdx.x; i < n; i += blockDim.x) {
-      float gv = fmaf(wd, w[i], g[i]);
-      float st = gv;
-      if (mom != nullptr) {
-        float mv = fmaf(mu, mom[i], (1.f - damp) * gv);
-        mom[i] = mv;
-        st = nesterov ? fmaf(mu, mv, gv) : mv;
-      }
-      float wv = fmaf(-lr, st, w[i]);
+      float mv = mom != nullptr ? mom[i] : 0.f;
+      const float wv = sgd_update(h, w[i], g[i], mv, mom != nullptr, nesterov);
+      if (mom != nullptr) mom[i] = mv;
       w[i] = wv;
       if (zero_grad) g[i] = 0.f;
       if (wb != nullptr) wb[i] = __float2bfloat16_rn(wv);
+    }
+  }
+}
+
+// ------------------------------------------------------------------ leftover SGD of a step with an optimizer epilogue
+// When the weight-gradient GEMMs of a step applied SGD in their epilogue (gemm_wgmma.cu), what is left is a set of
+// arena ranges, given as a device table of chunks {offset, length, kind} -- one chunk per CTA iteration.
+//   kind 0: parameters with a gradient -- the update of fused_sgd_kernel, gradient zeroed afterwards;
+//   kind 1: parameters whose gradient is identically zero (the off-centre taps of a k x k convolution on a 1x1 map) --
+//           the update with g = 0, gradient never read.  With weight decay 0 and no momentum buffer that update is the
+//           identity, and the chunk is skipped; this is decided here from `hyper`, so a captured graph stays exact when
+//           it is replayed with new hyper-parameters.
+__global__ void __launch_bounds__(EW_THREADS)
+fused_sgd_segments_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict__ mom,
+                          __nv_bfloat16* __restrict__ wb, const long long* __restrict__ seg, int n_seg,
+                          const float* __restrict__ hyper, int nesterov) {
+  griddep_launch_dependents();
+  griddep_wait();
+  const SgdHyper h = load_sgd_hyper(hyper);
+  const bool has_mom = mom != nullptr;
+  const bool nograd_is_identity = h.wd == 0.f && !has_mom;
+  for (int s = blockIdx.x; s < n_seg; s += gridDim.x) {
+    const long long off = seg[3 * s], len = seg[3 * s + 1];
+    const bool has_grad = seg[3 * s + 2] == 0;
+    if (!has_grad && nograd_is_identity) continue;      // block-uniform
+    long long done = 0;
+    if ((off & 3) == 0) {
+      const long long nv = len >> 2;
+      for (long long i = threadIdx.x; i < nv; i += blockDim.x) {
+        const long long e = off + (i << 2);
+        float4 mv = has_mom ? *reinterpret_cast<float4*>(mom + e) : make_float4(0.f, 0.f, 0.f, 0.f);
+        const float4 gv = has_grad ? *reinterpret_cast<float4*>(g + e) : make_float4(0.f, 0.f, 0.f, 0.f);
+        const float4 wv = sgd_update4(h, *reinterpret_cast<float4*>(w + e), gv, mv, has_mom, nesterov);
+        if (has_mom) *reinterpret_cast<float4*>(mom + e) = mv;
+        *reinterpret_cast<float4*>(w + e) = wv;
+        if (has_grad) *reinterpret_cast<float4*>(g + e) = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (wb != nullptr) *reinterpret_cast<uint2*>(wb + e) = make_uint2(pack_bf16x2(wv.x, wv.y), pack_bf16x2(wv.z, wv.w));
+      }
+      done = nv << 2;
+    }
+    for (long long i = done + threadIdx.x; i < len; i += blockDim.x) {
+      const long long e = off + i;
+      float mv = has_mom ? mom[e] : 0.f;
+      const float wv = sgd_update(h, w[e], has_grad ? g[e] : 0.f, mv, has_mom, nesterov);
+      if (has_mom) mom[e] = mv;
+      w[e] = wv;
+      if (has_grad) g[e] = 0.f;
+      if (wb != nullptr) wb[e] = __float2bfloat16_rn(wv);
     }
   }
 }
@@ -494,6 +521,16 @@ extern "C" int b200_fused_sgd(float* w, float* g, float* mom, void* w_bf16, long
   if (wire_slot != nullptr && ((n & 7) || (pk.n_pack & 7))) return -2;
   launch_pdl(fused_sgd_kernel, max_ctas > 0 ? ew_grid(n >> 2, max_ctas) : ew_grid(n >> 2), EW_THREADS, 0, stream, w, g, mom, reinterpret_cast<__nv_bfloat16*>(w_bf16), n,
                                                                 hyper, zero_grad, nesterov, pk);
+  RET_LAST();
+}
+extern "C" int b200_fused_sgd_segments(float* w, float* g, float* mom, void* w_bf16, const long long* segments, int n_seg,
+                                       const float* hyper, int nesterov, cudaStream_t stream) {
+  if (n_seg <= 0) return 0;
+  if ((reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(mom)) & 15 ||
+      reinterpret_cast<uintptr_t>(w_bf16) & 7)
+    return -2;
+  launch_pdl(fused_sgd_segments_kernel, ew_grid(n_seg * static_cast<long long>(EW_THREADS)), EW_THREADS, 0, stream, w, g,
+             mom, reinterpret_cast<__nv_bfloat16*>(w_bf16), segments, n_seg, hyper, nesterov);
   RET_LAST();
 }
 extern "C" int b200_fold_client(float* acc, float* theta, const float* global_w, void* w_bf16, float* mom, long long n_mom,

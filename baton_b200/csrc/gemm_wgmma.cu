@@ -29,6 +29,7 @@
 #include "ptx.cuh"
 #include "launch.h"
 #include "pdl.cuh"
+#include "sgd.cuh"
 
 namespace b200 {
 
@@ -74,6 +75,13 @@ struct GemmParams {
   int conv_taps;           // dgrad: KH * KW
   int conv_ncol;           // dgrad: Cin of the convolution (column pitch of one tap inside a weight row)
   const uint32_t* flag_epoch_ptr;   // bcast_gemm inside a captured graph: the required flag value lives in device memory
+  // optimizer epilogue (the SGD instantiation of the fixed-depth kernel, single K pass): SGD on theta instead of
+  // red.add into D; the pointers address the element D[0, 0] would and are indexed like D
+  const float* sgd_hyper = nullptr;
+  float* sgd_theta = nullptr;
+  __nv_bfloat16* sgd_wb = nullptr;
+  float* sgd_mom = nullptr;
+  int sgd_nesterov = 0;
 };
 
 // Wait until every arrival flag covering arena elements [e0, e1] has reached `need` (published by the FedAvg kernel with
@@ -266,6 +274,42 @@ __device__ __forceinline__ void store_row_chunk(const GemmParams& p, int row, in
   }
 }
 
+// Optimizer epilogue of one 32-column row chunk (columns [col0, col0 + 32) of `row`, `e` = its element offset from D[0,0]).
+// The tile holds the complete gradient of these weights (single K pass), so the SGD step runs here and the gradient
+// buffer is never touched.  0 + v is the value a red.add into the zeroed gradient would have left (-0 becomes +0), and
+// sgd_update is the arena optimizer's arithmetic: the result matches accumulate-then-fused_sgd bit for bit.
+__device__ __forceinline__ void sgd_epilogue_chunk(const GemmParams& p, size_t e, int col0, const float (&v)[32],
+                                                   bool vec) {
+  const SgdHyper h = load_sgd_hyper(p.sgd_hyper);
+  float* w = p.sgd_theta + e;
+  float* m = p.sgd_mom != nullptr ? p.sgd_mom + e : nullptr;
+  __nv_bfloat16* wb = p.sgd_wb != nullptr ? p.sgd_wb + e : nullptr;
+  const bool nest = p.sgd_nesterov != 0;
+  if (vec && col0 + 32 <= p.N) {
+#pragma unroll
+    for (int j = 0; j < 32; j += 4) {
+      float4 mv = m != nullptr ? *reinterpret_cast<const float4*>(m + j) : make_float4(0.f, 0.f, 0.f, 0.f);
+      const float4 gv = make_float4(__fadd_rn(0.f, v[j]), __fadd_rn(0.f, v[j + 1]), __fadd_rn(0.f, v[j + 2]),
+                                    __fadd_rn(0.f, v[j + 3]));
+      const float4 wv = sgd_update4(h, *reinterpret_cast<const float4*>(w + j), gv, mv, m != nullptr, nest);
+      *reinterpret_cast<float4*>(w + j) = wv;
+      if (m != nullptr) *reinterpret_cast<float4*>(m + j) = mv;
+      if (wb != nullptr) *reinterpret_cast<uint2*>(wb + j) = make_uint2(pack_bf16x2(wv.x, wv.y), pack_bf16x2(wv.z, wv.w));
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      if (col0 + j < p.N) {
+        float mv = m != nullptr ? m[j] : 0.f;
+        const float wv = sgd_update(h, w[j], __fadd_rn(0.f, v[j]), mv, m != nullptr, nest);
+        w[j] = wv;
+        if (m != nullptr) m[j] = mv;
+        if (wb != nullptr) wb[j] = __float2bfloat16_rn(wv);
+      }
+    }
+  }
+}
+
 // Consumer main loop, shared by every kernel below: warpgroup g (0 or 1) accumulates rows [64 g, 64 g + 64) of the
 // 128 x BN tile in registers over `num_kt` k-tiles of the ring.  A stage is handed back to the producer (one arrival
 // per consumer warp) as soon as the wgmma that read it have retired -- one k-tile of MMAs stays in flight.
@@ -310,7 +354,8 @@ __device__ __forceinline__ void consume_ktiles(float (&acc)[BN / 2], uint8_t* sm
 // im2col(dy) gathered by TMA im2col with pad' = k - 1 - pad (k-tile = one flipped tap x 64 OUTPUT channels), B = the
 // [64 cout] x [BN cin] slab of that tap inside the channels_last weight matrix, loaded MN-major (no weight transpose,
 // no col2im).  See csrc/im2col_tma.cu for the tensor maps.
-template <int BN, int STAGES, int CONV = 0>
+// SGD: optimizer epilogue instantiation (weight gradients only) -- every other GEMM keeps the plain epilogue.
+template <int BN, int STAGES, int CONV = 0, bool SGD = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                          const GemmParams p) {
@@ -464,6 +509,9 @@ gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
                     (static_cast<size_t>(row) * p.ldd + static_cast<size_t>(bz_outer) * p.d_outer +
                      static_cast<size_t>(bz_inner) * p.d_inner) * elt;
     const bool vec_ok = ((reinterpret_cast<uintptr_t>(p.D) & 15) == 0) && ((p.ldd * elt) % 16 == 0);
+    const bool sgd_vec = SGD && (p.ldd % 4 == 0) &&
+                         ((reinterpret_cast<uintptr_t>(p.sgd_theta) | reinterpret_cast<uintptr_t>(p.sgd_mom)) & 15) == 0 &&
+                         (reinterpret_cast<uintptr_t>(p.sgd_wb) & 7) == 0;
     // fused BatchNorm statistics: per row quarter column sums, [4 quarters][2 * BN] floats
     float* sstat = cstat + q * 2 * BN;
     const bool want_stats = p.col_stats != nullptr;
@@ -483,6 +531,10 @@ gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       if (want_stats) stage_col_stats(sstat, BN, c, v);
       if (!row_ok) continue;
       const bool full = (col0 + 32 <= p.N);
+      if constexpr (SGD) {
+        sgd_epilogue_chunk(p, static_cast<size_t>(row) * p.ldd + col0, col0, v, sgd_vec);
+        continue;
+      }
       if (p.atomic_out) {
         float* d = reinterpret_cast<float*>(drow) + col0;
         if (full && vec_ok) {
@@ -976,18 +1028,23 @@ static int make_map4(CUtensorMap* map, const void* base, long long rows, long lo
 // BN wider than 128 is not instantiated (see the top of the file): a requested 256 runs as 128.
 static int clamp_bn(int bn) { return bn > 128 ? 128 : bn; }
 
-template <int BN, int STAGES, int CONV = 0>
+static void set_sgd_epilogue(GemmParams& p, const B200SgdEpilogue& s) {
+  p.sgd_hyper = s.hyper; p.sgd_theta = s.theta; p.sgd_wb = reinterpret_cast<__nv_bfloat16*>(s.theta_bf16);
+  p.sgd_mom = s.mom; p.sgd_nesterov = s.nesterov;
+}
+
+template <int BN, int STAGES, int CONV = 0, bool SGD = false>
 static int launch_fixed(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, dim3 grid,
                       cudaStream_t stream) {
   constexpr int smem = STAGES * SmemLayout<BN>::STAGE_BYTES + 2 * STAGES * 8 + 8 * BN * 4 + 1024;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_fixed_kernel<BN, STAGES, CONV>,
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return static_cast<int>(e);
     configured = true;
   }
-  cudaError_t le = launch_pdl(gemm_bf16_fixed_kernel<BN, STAGES, CONV>, grid, GEMM_THREADS, smem, stream, ta, tb, p);
+  cudaError_t le = launch_pdl(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD>, grid, GEMM_THREADS, smem, stream, ta, tb, p);
   if (le != cudaSuccess) return static_cast<int>(le);
   return static_cast<int>(cudaGetLastError());
 }
@@ -1093,9 +1150,13 @@ extern "C" int b200_gemm_bf16(const void* a, const void* b, void* d, const float
                               int split_k, int accumulate, float alpha, const uint32_t* tile_flags,
                               uint32_t flag_epoch, long long flag_elem_off, int flag_tile_elems,
                               long long flag_bias_off, int force_bn, float* col_stats, const uint32_t* flag_epoch_ptr,
-                              cudaStream_t stream) {
+                              const B200SgdEpilogue* sgd, cudaStream_t stream) {
   using namespace b200;
   if (M <= 0 || N <= 0 || K <= 0) return 0;
+  // optimizer epilogue: only a weight gradient (MN-major operands, plain fp32 accumulation) qualifies
+  if (sgd != nullptr && (!accumulate || !out_fp32 || !a_mn || !b_mn || bias != nullptr || act != 0 || alpha != 1.0f ||
+                         col_stats != nullptr || tile_flags != nullptr))
+    return B200_SGD_EPILOGUE_DECLINED;
   // fused BatchNorm statistics: plain single-pass GEMM only (no split-K partials, no bias / activation / scaling)
   if (col_stats != nullptr && (split_k > 1 || bias != nullptr || act != 0 || alpha != 1.0f || accumulate)) return -3;
   if ((lda % 8) || (ldb % 8) || (reinterpret_cast<uintptr_t>(a) & 15) || (reinterpret_cast<uintptr_t>(b) & 15))
@@ -1148,10 +1209,6 @@ extern "C" int b200_gemm_bf16(const void* a, const void* b, void* d, const float
   const int max_stages = bn == 128 ? 6 : 8;
   p.stages = per < max_stages ? (per < 2 ? 2 : per) : max_stages;
   dim3 grid((N + bn - 1) / bn, (M + BM - 1) / BM, split_k);
-  if (cluster_k > 1) {
-    if (bn == 128) return launch_cfg<128>(ta, tb, p, grid, stream);
-    return launch_cfg<64>(ta, tb, p, grid, stream);
-  }
   // large plain GEMMs (>= one wave of tiles, single K pass): persistent kernel with overlapped epilogue
   static int persistent_on = -1;
   if (persistent_on < 0) {
@@ -1159,11 +1216,26 @@ extern "C" int b200_gemm_bf16(const void* a, const void* b, void* d, const float
     persistent_on = (e != nullptr && e[0] == '0') ? 0 : 1;
   }
   const int num_tiles = static_cast<int>(grid.x * grid.y);
-  if (persistent_on && split_k == 1 && tile_flags == nullptr && num_tiles >= device_sm_count() && bn == 128)
-    return launch_persistent<128, 3>(ta, tb, p, num_tiles, stream);
+  const bool persistent = persistent_on && split_k == 1 && tile_flags == nullptr && num_tiles >= device_sm_count() &&
+                          bn == 128;
+  if (sgd != nullptr) {
+    // the optimizer epilogue lives in the fixed-depth kernel and needs each tile's complete gradient in one CTA
+    if (split_k != 1 || cluster_k != 1 || persistent) return B200_SGD_EPILOGUE_DECLINED;
+    set_sgd_epilogue(p, *sgd);
+  }
+  if (cluster_k > 1) {
+    if (bn == 128) return launch_cfg<128>(ta, tb, p, grid, stream);
+    return launch_cfg<64>(ta, tb, p, grid, stream);
+  }
+  if (persistent) return launch_persistent<128, 3>(ta, tb, p, num_tiles, stream);
   // short K loops (stem convolution: 3 k tiles, 1x1 shortcuts: 1-4) do not need a deep ring: a shallow one asks for
   // little shared memory
   const bool shallow = per <= 4 && !p.batched;
+  if (sgd != nullptr) {
+    if (bn == 128)
+      return shallow ? launch_fixed<128, 3, 0, true>(ta, tb, p, grid, stream) : launch_fixed<128, 6, 0, true>(ta, tb, p, grid, stream);
+    return shallow ? launch_fixed<64, 4, 0, true>(ta, tb, p, grid, stream) : launch_fixed<64, 8, 0, true>(ta, tb, p, grid, stream);
+  }
   if (bn == 128) return shallow ? launch_fixed<128, 3>(ta, tb, p, grid, stream) : launch_fixed<128, 6>(ta, tb, p, grid, stream);
   return shallow ? launch_fixed<64, 4>(ta, tb, p, grid, stream) : launch_fixed<64, 8>(ta, tb, p, grid, stream);
 }
@@ -1322,7 +1394,7 @@ extern "C" int b200_conv_igemm_dgrad(const void* dy, const void* w, void* dx, in
 // weight gradient: dw[Cout, KH*KW*Cin] (fp32, accumulated with red.add) += dy[N*Ho*Wo, Cout]^T im2col(x)
 extern "C" int b200_conv_igemm_wgrad(const void* dy, const void* x, float* dw, int N, int H, int W, int Cin, int Cout,
                                      int KH, int KW, int stride, int pad, int Ho, int Wo, int split_k, int force_bn,
-                                     cudaStream_t stream) {
+                                     const B200SgdEpilogue* sgd, cudaStream_t stream) {
   using namespace b200;
   const long long Mp = static_cast<long long>(N) * Ho * Wo;      // reduction length (output pixels)
   const int Kc = KH * KW * Cin;                                    // GEMM N
@@ -1341,7 +1413,9 @@ extern "C" int b200_conv_igemm_wgrad(const void* dy, const void* x, float* dw, i
   if (split_k > k_tiles) split_k = k_tiles;
   const int per = (k_tiles + split_k - 1) / split_k;
   split_k = (k_tiles + per - 1) / per;
+  if (sgd != nullptr && split_k != 1) return B200_SGD_EPILOGUE_DECLINED;
   GemmParams p;
+  if (sgd != nullptr) set_sgd_epilogue(p, *sgd);
   p.M = Cout; p.N = Kc; p.K = static_cast<int>(Mp); p.D = dw; p.ldd = Kc; p.bias = nullptr; p.out_fp32 = 1; p.act = 0;
   p.a_mn = 1; p.b_mn = 1; p.k_tiles_per_split = per; p.cluster_k = 1; p.atomic_out = 1;
   p.epi_staged = 0; p.col_stats = nullptr;
@@ -1352,6 +1426,10 @@ extern "C" int b200_conv_igemm_wgrad(const void* dy, const void* x, float* dw, i
   p.conv_ho = Ho; p.conv_wo = Wo; p.conv_stride = stride; p.conv_pad = pad; p.conv_kw = KW; p.conv_cin = Cin;
   p.conv_taps = KH * KW; p.conv_ncol = Cin;
   dim3 grid((Kc + bn - 1) / bn, (Cout + BM - 1) / BM, split_k);
+  if (sgd != nullptr) {
+    if (bn == 128) return launch_fixed<128, 6, 2, true>(ta, tb, p, grid, stream);
+    return launch_fixed<64, 8, 2, true>(ta, tb, p, grid, stream);
+  }
   if (bn == 128) return launch_fixed<128, 6, 2>(ta, tb, p, grid, stream);
   return launch_fixed<64, 8, 2>(ta, tb, p, grid, stream);
 }

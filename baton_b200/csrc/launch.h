@@ -9,12 +9,26 @@
 
 extern "C" {
 
+// Optimizer epilogue of a weight-gradient GEMM: instead of accumulating the gradient into D, apply the SGD step to the
+// parameters in place.  theta / theta_bf16 / mom point at the element that D[0, 0] would address and are indexed like
+// D (same ldd).  hyper = device float[4] as for b200_fused_sgd.  A launcher that cannot apply it returns
+// B200_SGD_EPILOGUE_DECLINED and touches nothing; the caller then accumulates the gradient as usual.
+struct B200SgdEpilogue {
+  float* theta;
+  void* theta_bf16;                 // or nullptr
+  float* mom;                       // or nullptr (no momentum buffer)
+  const float* hyper;
+  int nesterov;
+};
+#define B200_SGD_EPILOGUE_DECLINED (-6)
+
 // ---- gemm_wgmma.cu
+// sgd != nullptr: optimizer epilogue (accumulate, fp32 D, MN-major operands, single K pass on the fixed-depth kernel)
 int b200_gemm_bf16(const void* a, const void* b, void* d, const float* bias, int M, int N, int K, long long lda,
                    long long ldb, long long ldd, int a_mn, int b_mn, int out_fp32, int act, int split_k, int accumulate,
                    float alpha, const uint32_t* tile_flags, uint32_t flag_epoch, long long flag_elem_off, int flag_tile_elems,
                    long long flag_bias_off, int force_bn, float* col_stats, const uint32_t* flag_epoch_ptr,
-                   cudaStream_t stream);
+                   const B200SgdEpilogue* sgd, cudaStream_t stream);
 int b200_gemm_bf16_batched(const void* a, const void* b, void* d, int M, int N, int K, long long lda, long long ldb,
                            long long ldd, int a_mn, int b_mn, int out_fp32, int act, float alpha, int n_outer,
                            int n_inner, long long a_outer, long long a_inner, long long b_outer, long long b_inner,
@@ -31,7 +45,8 @@ int b200_conv_igemm_fwd(const void* x, const void* w, void* y, int N, int H, int
 int b200_conv_igemm_dgrad(const void* dy, const void* w, void* dx, int N, int H, int W, int Cin, int Cout, int KH, int KW,
                           int pad, int Ho, int Wo, int cluster_k, int force_bn, cudaStream_t stream);
 int b200_conv_igemm_wgrad(const void* dy, const void* x, float* dw, int N, int H, int W, int Cin, int Cout, int KH, int KW,
-                          int stride, int pad, int Ho, int Wo, int split_k, int force_bn, cudaStream_t stream);
+                          int stride, int pad, int Ho, int Wo, int split_k, int force_bn, const B200SgdEpilogue* sgd,
+                          cudaStream_t stream);
 // ---- im2col_tma.cu (experimental: TMA im2col tensor maps, probe kernel only)
 int b200_im2col_tma_probe(const void* x, void* col, int N, int H, int W, int C, int KH, int KW, int stride, int pad,
                           int Ho, int Wo, cudaStream_t stream);
@@ -53,6 +68,10 @@ int b200_gemm_simt(const void* a, const void* b, void* d, const float* bias, int
 int b200_fused_sgd(float* w, float* g, float* mom, void* w_bf16, long long n, const float* hyper, int zero_grad,
                    int nesterov, int max_ctas, const unsigned long long* wire_slot, const float* pack_global,
                    const float* pack_scale, long long n_pack, int wire_fp32, cudaStream_t stream);
+// the same step over a device table of n_seg arena chunks {offset, length, kind} (int64 [n_seg][3]); kind 0: with a
+// gradient (zeroed afterwards), kind 1: gradient identically zero (never read)
+int b200_fused_sgd_segments(float* w, float* g, float* mom, void* w_bf16, const long long* segments, int n_seg,
+                            const float* hyper, int nesterov, cudaStream_t stream);
 // logical-client fold: acc (+)= nk * (theta - global) [+ reset of the replica]; mode 2: theta = global + acc * nk
 int b200_fold_client(float* acc, float* theta, const float* global_w, void* w_bf16, float* mom, long long n_mom, long long n,
                      float nk, int mode, int reset, cudaStream_t stream);

@@ -11,7 +11,7 @@ Conventions
 """
 from __future__ import annotations
 
-from typing import Optional, Sequence, Tuple
+from typing import List, Optional, Sequence, Tuple
 
 import torch
 
@@ -78,7 +78,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
          n_valid: Optional[int] = None, flags: Optional[torch.Tensor] = None, flag_epoch: int = 0,
          flag_elem_off: int = 0, flag_tile_elems: int = 0, flag_bias_off: int = -1, force_bn: int = 0,
          force_simt: bool = False, col_stats: Optional[torch.Tensor] = None,
-         flag_epoch_word: Optional[torch.Tensor] = None) -> torch.Tensor:
+         flag_epoch_word: Optional[torch.Tensor] = None, sgd: Optional[dict] = None) -> Optional[torch.Tensor]:
     """``out[M,N] = act(alpha * A @ B^T + bias)`` on the tensor cores (wgmma).
 
     ``n_valid`` limits the written columns (used when B carries zero K-padding
@@ -86,7 +86,11 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
 
     ``col_stats`` (fp32 ``[2N]``): the epilogue also accumulates the per-column sum and sum of squares of the
     bf16 output into it -- the BatchNorm batch statistics of a convolution, without a second pass over the
-    activation.  Only legal where :func:`gemm_stats_fusable` says so (single-pass tensor-core GEMM)."""
+    activation.  Only legal where :func:`gemm_stats_fusable` says so (single-pass tensor-core GEMM).
+
+    ``sgd`` (see :func:`sgd_epilogue_args`): on a weight-gradient GEMM (``accumulate`` into fp32 ``out``, MN-major
+    operands) apply the SGD step to the parameters in the epilogue instead of accumulating the gradient into ``out``.
+    Returns ``None`` when this GEMM cannot (split-K, persistent kernel...): nothing was written, accumulate instead."""
     C = load()
     M, K = (a.shape[1], a.shape[0]) if a_mn else (a.shape[0], a.shape[1])
     N, Kb = (b.shape[1], b.shape[0]) if b_mn else (b.shape[0], b.shape[1])
@@ -100,10 +104,12 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
     ldd = out.stride(0) if out.dim() == 2 else N
     lda, ldb = _pitch(a), _pitch(b)
     use_simt = force_simt or not (_tma_ok(a) and _tma_ok(b))
+    if use_simt and sgd is not None:
+        return None
     if use_simt:
         assert col_stats is None, "fused column statistics need the tensor-core path"
         C.gemm(a, b, out, bias, M, N, K, lda, ldb, ldd, a_mn, b_mn, act, 1, accumulate, alpha, None, 0, 0, 0, -1, 0,
-               True, None, None)
+               True, None, None, None, None, None, None, False)
         return out
     bn = force_bn or pick_bn(M, N)
     if col_stats is not None:
@@ -117,8 +123,13 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
                 split_k = 1
     if split_k > 1:
         assert out.dtype == torch.float32 and bias is None and act == 0
-    C.gemm(a, b, out, bias, M, N, K, lda, ldb, ldd, a_mn, b_mn, act, split_k, accumulate, alpha, flags, flag_epoch,
-           flag_elem_off, flag_tile_elems, flag_bias_off, bn, False, col_stats, flag_epoch_word)
+    if sgd is not None and split_k != 1:
+        return None                 # the optimizer epilogue needs every tile's complete gradient in one CTA
+    sg = sgd or {}
+    if not C.gemm(a, b, out, bias, M, N, K, lda, ldb, ldd, a_mn, b_mn, act, split_k, accumulate, alpha, flags, flag_epoch,
+                  flag_elem_off, flag_tile_elems, flag_bias_off, bn, False, col_stats, flag_epoch_word, sg.get("theta"),
+                  sg.get("theta_bf16"), sg.get("momentum"), sg.get("hyper"), bool(sg.get("nesterov", False))):
+        return None
     return out
 
 
@@ -143,6 +154,57 @@ def fused_sgd(w: torch.Tensor, g: torch.Tensor, hyper: torch.Tensor, momentum_bu
     pk = pack or {}
     load().fused_sgd(w, g, momentum_buf, w_bf16, hyper, zero_grad, nesterov, max_ctas, pk.get("wire_slot"),
                      pk.get("global_w"), pk.get("scale"), int(pk.get("n_pack", 0)), bool(pk.get("wire_fp32", False)))
+
+
+def sgd_epilogue_args(theta: torch.Tensor, grad: torch.Tensor, grad_view: torch.Tensor, hyper: torch.Tensor,
+                      momentum: Optional[torch.Tensor] = None, theta_bf16: Optional[torch.Tensor] = None,
+                      nesterov: bool = False) -> dict:
+    """``sgd=`` argument of a weight-gradient GEMM whose output ``grad_view`` is a view of the flat gradient ``grad``:
+    the parameter, bf16 shadow and momentum buffers (same offsets as ``grad``) from the element ``grad_view[0, 0]`` on."""
+    off = (grad_view.data_ptr() - grad.data_ptr()) // grad.element_size()
+    assert 0 <= off < grad.numel(), "the GEMM output is not a view of the gradient arena"
+    return {"theta": theta[off:], "theta_bf16": theta_bf16[off:] if theta_bf16 is not None else None,
+            "momentum": momentum[off:] if momentum is not None else None, "hyper": hyper, "nesterov": nesterov}
+
+
+SGD_CHUNK = 8192       # arena elements per chunk of the leftover optimizer pass (one CTA iteration each)
+
+
+def sgd_segments(n: int, fused: Sequence[Tuple[int, int, int, int]], nograd: Sequence[Tuple[int, int]],
+                 chunk: int = SGD_CHUNK) -> List[Tuple[int, int, int]]:
+    """Chunk table of the leftover optimizer pass of a step whose weight-gradient GEMMs applied SGD in their epilogue.
+
+    ``fused``: ``(offset, rows, cols, ld)`` element blocks the epilogues updated (row ``r`` covers
+    ``[offset + r * ld, offset + r * ld + cols)``); ``nograd``: ``(offset, length)`` parameter ranges whose gradient is
+    identically zero outside the fused blocks.  Returns ``(offset, length, kind)`` chunks of at most ``chunk`` elements
+    that cover ``[0, n)`` minus the fused blocks exactly once, in offset order; kind 1 inside a ``nograd`` range, else
+    0."""
+    pieces = sorted((o + r * ld, o + r * ld + cols) for o, rows, cols, ld in fused for r in range(rows))
+    free, pos = [], 0
+    for s, e in pieces:
+        if s < pos or e > n:
+            raise ValueError("fused blocks overlap or leave the arena: [{}, {})".format(s, e))
+        if s > pos:
+            free.append((pos, s))
+        pos = e
+    if pos < n:
+        free.append((pos, n))
+    ng = sorted((o, o + l) for o, l in nograd)
+    out = []
+    for s, e in free:
+        cuts = sorted({s, e} | {b for r in ng for b in r if s < b < e})
+        for a, b in zip(cuts, cuts[1:]):
+            kind = 1 if any(lo <= a and b <= hi for lo, hi in ng) else 0
+            out.extend((c, min(chunk, b - c), kind) for c in range(a, b, chunk))
+    return out
+
+
+def fused_sgd_segments(w: torch.Tensor, g: torch.Tensor, hyper: torch.Tensor, segments: torch.Tensor,
+                       momentum_buf: Optional[torch.Tensor] = None, w_bf16: Optional[torch.Tensor] = None,
+                       nesterov: bool = False) -> None:
+    """The step of :func:`fused_sgd` over the arena chunks of ``segments`` (device int64 ``[S, 3]`` from
+    :func:`sgd_segments`); chunks of kind 1 never read the gradient."""
+    load().fused_sgd_segments(w, g, momentum_buf, w_bf16, segments, hyper, nesterov)
 
 
 def weighted_sum_(dst: torch.Tensor, srcs: Sequence[torch.Tensor], weights: Sequence[float]) -> torch.Tensor:
@@ -281,9 +343,10 @@ def conv_igemm_dgrad(dy: torch.Tensor, w2d: torch.Tensor, in_shape, kh: int, kw:
 
 
 def conv_igemm_wgrad_(dy2d: torch.Tensor, x: torch.Tensor, dw2d: torch.Tensor, kh: int, kw: int, stride: int,
-                      pad: int) -> bool:
+                      pad: int, sgd: Optional[dict] = None) -> bool:
     """EXPERIMENTAL implicit wgrad: ``dw2d[Cout, kh*kw*Cin] += dy2d^T im2col(x)`` (fp32 atomics, split over
-    pixels) without materialising ``im2col(x)``."""
+    pixels) without materialising ``im2col(x)``.  ``sgd``: optimizer epilogue as in :func:`gemm`.  False: nothing
+    was done (shape not supported, or the optimizer epilogue declined)."""
     n, h, w, c = x.shape
     cout = dy2d.shape[1]
     if c % 64 or not x.is_contiguous() or not dy2d.is_contiguous() or not dw2d.is_contiguous():
@@ -291,7 +354,13 @@ def conv_igemm_wgrad_(dy2d: torch.Tensor, x: torch.Tensor, dw2d: torch.Tensor, k
     ho, wo = conv_out_size(h, kh, stride, pad), conv_out_size(w, kw, stride, pad)
     M, K = n * ho * wo, kh * kw * c
     bn = pick_bn(cout, K)
-    return bool(load().conv_igemm_wgrad(dy2d, x, dw2d, cout, kh, kw, stride, pad, ho, wo, pick_split_k(cout, K, M, bn), bn))
+    split_k = pick_split_k(cout, K, M, bn)
+    if sgd is not None and split_k != 1:
+        return False                # the optimizer epilogue needs every tile's complete gradient in one CTA
+    sg = sgd or {}
+    return bool(load().conv_igemm_wgrad(dy2d, x, dw2d, cout, kh, kw, stride, pad, ho, wo, split_k, bn,
+                                        sg.get("theta"), sg.get("theta_bf16"), sg.get("momentum"), sg.get("hyper"),
+                                        bool(sg.get("nesterov", False))))
 
 
 def col2im(col: torch.Tensor, shape: Tuple[int, int, int, int], kh: int, kw: int, stride: int, pad: int,

@@ -18,6 +18,7 @@ call so the control plane / tests run on a GPU-less host.
 """
 from __future__ import annotations
 
+import contextlib
 import math
 from typing import Optional
 
@@ -175,6 +176,57 @@ class _Branch:
 
 
 BRANCH = _Branch()
+
+
+class _SgdEpilogue:
+    """Optimizer epilogue of the convolution weight gradients.  While a trainer holds it open (:meth:`open`), a conv
+    wgrad GEMM that owns complete gradient tiles (split-K = 1) applies the SGD step to the weights in its epilogue
+    instead of accumulating into the gradient arena, and records what it updated: ``fused`` blocks
+    ``(offset, rows, cols, ld)`` and, for centre-tap convolutions, the ``nograd`` range ``(offset, length)`` of the whole
+    weight (its other taps never receive a gradient).  The trainer's leftover optimizer pass covers the rest of the
+    arena (``F.sgd_segments``).  The gradient of a fused block is never written, so it stays zero for unfused steps."""
+
+    def __init__(self):
+        self.arena = None
+
+    @contextlib.contextmanager
+    def open(self, arena, hyper, nesterov):
+        self.arena, self.hyper, self.nesterov = arena, hyper, nesterov
+        self.fused, self.nograd = [], []
+        try:
+            yield self
+        finally:
+            self.arena = None
+
+    @property
+    def active(self):
+        return self.arena is not None
+
+    def args(self, out2d):
+        """``sgd=`` argument for a wgrad GEMM writing the arena gradient view ``out2d``, or None when closed."""
+        a = self.arena
+        if a is None:
+            return None
+        return F.sgd_epilogue_args(a.theta, a.grad, out2d, self.hyper, a.momentum, a.theta_bf16, self.nesterov)
+
+    def record(self, out2d, nograd_of=None):
+        off = (out2d.data_ptr() - self.arena.grad.data_ptr()) // 4
+        self.fused.append((off, out2d.shape[0], out2d.shape[1], out2d.stride(0)))
+        if nograd_of is not None:
+            self.nograd.append(((nograd_of.data_ptr() - self.arena.grad.data_ptr()) // 4, nograd_of.numel()))
+
+
+SGD_EPI = _SgdEpilogue()
+
+
+def _wgrad(fn, out2d, nograd_of=None):
+    """Run a weight-gradient GEMM ``fn(sgd)`` -- with the optimizer epilogue when it is open and the GEMM accepts it,
+    accumulating into ``out2d`` otherwise."""
+    sgd = SGD_EPI.args(out2d)
+    if sgd is not None and fn(sgd):
+        SGD_EPI.record(out2d, nograd_of)
+    else:
+        fn(None)
 
 
 def _grad_target(p: Optional[torch.Tensor]):
@@ -362,12 +414,16 @@ class _ConvFn(torch.autograd.Function):
                 g2d = full[:, tap, :]
             if tgt is None:
                 F.gemm(dy2, col, a_mn=True, b_mn=True, out=g2d, accumulate=True)
-            else:
-                WGRAD.run(lambda: F.gemm(dy2, col, a_mn=True, b_mn=True, out=g2d, accumulate=True), dy2, col)
+            tok = WGRAD.mark(dy2)
             dx = None
             if ctx.needs_dx:
                 wc = w_bf16.view(cout, kh * kw, c)[:, tap, :]
                 dx = F.gemm(dy2, wc, b_mn=True).view(n, 1, 1, c)
+            if tgt is not None:
+                # an optimizer epilogue rewrites the bf16 weights the dgrad above reads: it must start after it
+                WGRAD.run(lambda: _wgrad(lambda sgd: F.gemm(dy2, col, a_mn=True, b_mn=True, out=g2d, accumulate=True,
+                                                            sgd=sgd) is not None, g2d, nograd_of=tgt),
+                          dy2, col, after=None if SGD_EPI.active else tok)
             return dx, gw, None, None, None, None, None, None, None, None
         igemm = getattr(ctx, "igemm", False)          # col IS x: the weight gradient gathers im2col(x) on the fly
         tok = WGRAD.mark(dy2)      # the weight-gradient branch depends on what is enqueued so far, not on the dgrad below
@@ -388,7 +444,10 @@ class _ConvFn(torch.autograd.Function):
             out2d = tgt.permute(0, 2, 3, 1).reshape(cout, k_true) if tgt.dim() == 4 else tgt.view(cout, k_true)
             assert out2d.data_ptr() == tgt.data_ptr(), "conv weight grad must be channels_last in the arena"
             if igemm:
-                WGRAD.run(lambda: F.conv_igemm_wgrad_(dy2, col, out2d, kh, kw, stride, pad), dy2, col, after=tok)
+                # an optimizer epilogue rewrites the bf16 weights the dgrad above reads: it must start after it
+                WGRAD.run(lambda: _wgrad(lambda sgd: F.conv_igemm_wgrad_(dy2, col, out2d, kh, kw, stride, pad, sgd=sgd),
+                                         out2d),
+                          dy2, col, after=None if SGD_EPI.active else tok)
             else:
                 WGRAD.run(lambda: F.gemm(dy2, col, a_mn=True, b_mn=True, out=out2d, accumulate=True, n_valid=k_true),
                           dy2, col, after=tok)

@@ -97,6 +97,10 @@ class GraphedLocalSGD:
         # latency-bound kernels it runs beside)
         self.tail_overlap = os.environ.get("BATON_SGD_OVERLAP", "0") == "1"
         self.tail_ctas = int(os.environ.get("BATON_SGD_TAIL_CTAS", "132"))    # grid cap of the overlapped SGD slice
+        # SGD in the epilogue of the convolution weight-gradient GEMMs (explicit step, steps that do not emit the upload
+        # copy); 0: one optimizer pass over the whole arena every step
+        self.sgd_fused = os.environ.get("BATON_SGD_FUSED", "1") != "0"
+        self._seg_tables = {}
         self.k3_join = None           # set by the engine: callable joining the round-end collective (enables the graph split)
         self._first_gemm_hook = None
         self.pack = None              # set by the engine: FedAvgSession.pack_spec() -> last SGD step emits the upload copy
@@ -130,9 +134,10 @@ class GraphedLocalSGD:
         yb = F.gather_rows(y, idx) if y.dtype == torch.int64 and y.dim() == 1 else y.index_select(0, idx)
         return xb, yb
 
-    def _step(self, X, y, idx, batch=None, emit_wire=False):
+    def _step(self, X, y, idx, batch=None, emit_wire=False, fuse_sgd=True):
         """One SGD step on ``X[idx], y[idx]`` (or on the already gathered ``batch``).  ``emit_wire``: last step of
-        an epoch -- the optimizer kernel also writes the upload copy for the round-end collective (``self.pack``)."""
+        an epoch -- the optimizer kernel also writes the upload copy for the round-end collective (``self.pack``).
+        ``fuse_sgd=False``: no optimizer epilogue in the weight-gradient GEMMs (one optimizer pass over the arena)."""
         F = self.F
         xb, yb = batch if batch is not None else self._gather(X, y, idx)
         ws = getattr(self.model, "stats_workspace", None)
@@ -152,7 +157,16 @@ class GraphedLocalSGD:
             split = 0 if (emit_wire and self.pack is not None) else self._tail_split()
             self._split_active = split
             self._tail_done = False
-            explicit(xb, yb, loss_acc=self.loss_acc, hooks=self if (split or self._first_gemm_hook is not None) else None)
+            hooks = self if (split or self._first_gemm_hook is not None) else None
+            if self.sgd_fused and fuse_sgd and not split and not emit_wire:
+                # the split-K = 1 convolution weight gradients apply SGD in their GEMM epilogue; one launch covers the rest
+                with self.bnn.SGD_EPI.open(a, self.hyper, self.nesterov) as epi:
+                    explicit(xb, yb, loss_acc=self.loss_acc, hooks=hooks)
+                F.fused_sgd_segments(a.theta, a.grad, self.hyper, self._segment_table(epi.fused, epi.nograd),
+                                     a.momentum, bf, nesterov=self.nesterov)
+                self.emitted_wire = False
+                return
+            explicit(xb, yb, loss_acc=self.loss_acc, hooks=hooks)
             end = split if (split and self._tail_done) else a.n_param
             pack = self.pack if (emit_wire and end == a.n_param) else None
             F.fused_sgd(a.theta[:end], a.grad[:end], self.hyper,
@@ -169,6 +183,16 @@ class GraphedLocalSGD:
                     bf[: a.n_param] if bf is not None else None, zero_grad=True, nesterov=self.nesterov, pack=pack)
         self.emitted_wire = pack is not None
         self.loss_acc.add_(stats)
+
+    def _segment_table(self, fused, nograd):
+        """Device chunk table of the leftover optimizer pass, built once per set of epilogue-updated ranges (they only
+        change with the batch shape, so every step of a captured epoch reuses the table its warm-up built)."""
+        key = (tuple(fused), tuple(nograd))
+        table = self._seg_tables.get(key)
+        if table is None:
+            segs = self.F.sgd_segments(self.arena.n_param, fused, nograd)
+            table = self._seg_tables[key] = torch.tensor(segs, dtype=torch.int64).view(-1, 3).to(self.device)
+        return table
 
     # ---- optimizer / backward overlap (hooks called by ``model.explicit_step``) ----
     def _tail_split(self) -> int:
@@ -333,7 +357,7 @@ class GraphedLocalSGD:
                     ent["graph2"].replay()
                 if tail:
                     with torch.enable_grad():
-                        self._step(X, y, perm_full[n_steps * batch_size:])
+                        self._step(X, y, perm_full[n_steps * batch_size:], fuse_sgd=False)
                     self.before_tail_forward()
                 epoch_losses[e].copy_(self.loss_acc)
         else:

@@ -58,8 +58,8 @@ lines = ["# model {} batch {} steps/epoch {}  kernels/step {}  epoch {:.3f} ms u
     args.model, args.batch_size, args.steps, tr.n_kernels_per_step, untraced_ms, e0.elapsed_time(e1), ok)]
 rows = kt.timeline()
 lines += kt.summary()
-# one steady-state step: from the (steps//2)-th fused_sgd to the next
-sgd = [i for i, r in enumerate(rows) if r["name"] == "fused_sgd_kernel"]
+# one steady-state step: from the (steps//2)-th optimizer kernel to the next
+sgd = [i for i, r in enumerate(rows) if r["name"] in ("fused_sgd_kernel", "fused_sgd_segments_kernel")]
 if len(sgd) >= 3:
     a, b = sgd[len(sgd) // 2 - 1] + 1, sgd[len(sgd) // 2] + 1
     lines.append("# one step ({} kernels, {:.1f} us): t_us since step start | slot us | resident-before-deps us | kernel".format(
