@@ -236,15 +236,15 @@ void dequant_mx(const at::Tensor& q, const at::Tensor& sf, at::Tensor out, int64
 }
 
 void fused_sgd(at::Tensor w, at::Tensor g, const std::optional<at::Tensor>& mom, const std::optional<at::Tensor>& wb,
-               const at::Tensor& hyper, bool zero_grad, bool nesterov, int64_t max_ctas,
-               const std::optional<at::Tensor>& wire_slot, const std::optional<at::Tensor>& pack_global,
-               const std::optional<at::Tensor>& pack_scale, int64_t n_pack, bool wire_fp32) {
+               const at::Tensor& hyper, bool zero_grad, bool nesterov, const std::optional<at::Tensor>& wire_slot,
+               const std::optional<at::Tensor>& pack_global, const std::optional<at::Tensor>& pack_scale, int64_t n_pack,
+               bool wire_fp32) {
   CHECK_CUDA(w);
   TORCH_CHECK(w.scalar_type() == at::kFloat && g.scalar_type() == at::kFloat && hyper.scalar_type() == at::kFloat);
   TORCH_CHECK(w.is_contiguous() && g.is_contiguous() && w.numel() == g.numel());
   const c10::cuda::CUDAGuard guard(w.device());
   check(b200_fused_sgd(w.data_ptr<float>(), g.data_ptr<float>(), opt_ptr<float>(mom), opt_ptr<void>(wb), w.numel(),
-                       hyper.data_ptr<float>(), zero_grad, nesterov, static_cast<int>(max_ctas),
+                       hyper.data_ptr<float>(), zero_grad, nesterov,
                        reinterpret_cast<const unsigned long long*>(opt_ptr<const int64_t>(wire_slot)),
                        opt_ptr<const float>(pack_global), opt_ptr<const float>(pack_scale), n_pack, wire_fp32, cur_stream()),
         "fused_sgd");
@@ -561,22 +561,6 @@ bool bn_maxpool_bwd(const at::Tensor& z, const at::Tensor& p, const at::Tensor& 
   check(rc, "bn_maxpool_bwd");
   return true;
 }
-// single-kernel (grid-barrier) BatchNorm backward, opt-in; false = shape not supported, use reduce + apply
-bool bn_bwd_fused(const at::Tensor& x, const at::Tensor& y, const at::Tensor& dy, at::Tensor dx,
-                  const std::optional<at::Tensor>& dres, const std::optional<at::Tensor>& gamma, const at::Tensor& mean,
-                  const at::Tensor& rstd, at::Tensor sums, const std::optional<at::Tensor>& dgamma,
-                  const std::optional<at::Tensor>& dbeta, int64_t rows, int64_t C, bool relu, at::Tensor barrier) {
-  CHECK_CUDA(x);
-  TORCH_CHECK(barrier.scalar_type() == at::kInt && barrier.numel() >= 2, "barrier: int32[2], zero-initialised");
-  const c10::cuda::CUDAGuard guard(x.device());
-  const int rc = b200_bn_bwd_fused(x.data_ptr(), y.data_ptr(), dy.data_ptr(), dx.data_ptr(), opt_ptr<void>(dres),
-                                   opt_ptr<const float>(gamma), mean.data_ptr<float>(), rstd.data_ptr<float>(),
-                                   sums.data_ptr<float>(), opt_ptr<float>(dgamma), opt_ptr<float>(dbeta), rows, C, relu,
-                                   reinterpret_cast<unsigned int*>(barrier.data_ptr<int>()), cur_stream());
-  if (rc == -2) return false;
-  check(rc, "bn_bwd_fused");
-  return true;
-}
 // single-kernel BatchNorm backward (cluster per channel slice); dy = dy_a (+ dy_b).  False: shape not supported.
 bool bn_bwd_cluster(const at::Tensor& x, const at::Tensor& y, const at::Tensor& dy_a, const std::optional<at::Tensor>& dy_b,
                     at::Tensor dx, const std::optional<at::Tensor>& dres, const std::optional<at::Tensor>& gamma,
@@ -676,7 +660,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("trace_set", &trace_set);
   m.def("attention_fwd", &attention_fwd);
   m.def("attention_bwd", &attention_bwd);
-  m.def("bn_bwd_fused", &bn_bwd_fused);
   m.def("bn_bwd_cluster", &bn_bwd_cluster);
   m.def("im2col_tma_probe", &im2col_tma_probe);
   m.def("conv_igemm_fwd", &conv_igemm_fwd);

@@ -508,10 +508,8 @@ embedding_bwd_kernel(const uint4* __restrict__ dy, const long long* __restrict__
 using namespace b200;
 #define RET_LAST() return static_cast<int>(cudaGetLastError())
 
-// max_ctas > 0 caps the grid (grid-stride kernel): an optimizer slice that runs BESIDE latency-bound compute kernels on
-// another stream must leave SM slots free for them
 extern "C" int b200_fused_sgd(float* w, float* g, float* mom, void* w_bf16, long long n, const float* hyper,
-                              int zero_grad, int nesterov, int max_ctas, const unsigned long long* wire_slot,
+                              int zero_grad, int nesterov, const unsigned long long* wire_slot,
                               const float* pack_global, const float* pack_scale, long long n_pack, int wire_fp32,
                               cudaStream_t stream) {
   if (n <= 0) return 0;
@@ -519,8 +517,8 @@ extern "C" int b200_fused_sgd(float* w, float* g, float* mom, void* w_bf16, long
   pk.wire_slot = wire_slot; pk.global_w = pack_global; pk.scale = pack_scale;
   pk.n_pack = n_pack > n ? n_pack : n; pk.wire_fp32 = wire_fp32;
   if (wire_slot != nullptr && ((n & 7) || (pk.n_pack & 7))) return -2;
-  launch_pdl(fused_sgd_kernel, max_ctas > 0 ? ew_grid(n >> 2, max_ctas) : ew_grid(n >> 2), EW_THREADS, 0, stream, w, g, mom, reinterpret_cast<__nv_bfloat16*>(w_bf16), n,
-                                                                hyper, zero_grad, nesterov, pk);
+  launch_pdl(fused_sgd_kernel, ew_grid(n >> 2), EW_THREADS, 0, stream, w, g, mom, reinterpret_cast<__nv_bfloat16*>(w_bf16),
+             n, hyper, zero_grad, nesterov, pk);
   RET_LAST();
 }
 extern "C" int b200_fused_sgd_segments(float* w, float* g, float* mom, void* w_bf16, const long long* segments, int n_seg,

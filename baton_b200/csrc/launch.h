@@ -66,7 +66,7 @@ int b200_gemm_simt(const void* a, const void* b, void* d, const float* bias, int
 // hyper = device float[4] {lr, momentum, weight_decay, dampening}
 // wire_slot != nullptr: also emit the client's wire copy for the round-end collective (see SgdPack in elementwise.cu)
 int b200_fused_sgd(float* w, float* g, float* mom, void* w_bf16, long long n, const float* hyper, int zero_grad,
-                   int nesterov, int max_ctas, const unsigned long long* wire_slot, const float* pack_global,
+                   int nesterov, const unsigned long long* wire_slot, const float* pack_global,
                    const float* pack_scale, long long n_pack, int wire_fp32, cudaStream_t stream);
 // the same step over a device table of n_seg arena chunks {offset, length, kind} (int64 [n_seg][3]); kind 0: with a
 // gradient (zeroed afterwards), kind 1: gradient identically zero (never read)
@@ -167,9 +167,6 @@ int b200_bn_maxpool_bwd(const void* z, const void* p, const void* argmax, const 
 int b200_bn_bwd_cluster(const void* x, const void* y, const void* dy_a, const void* dy_b, void* dx, void* dres,
                         const float* gamma, const float* save_mean, const float* save_rstd, float* dgamma, float* dbeta,
                         long long rows, int C, int relu, int max_cluster, cudaStream_t stream);
-int b200_bn_bwd_fused(const void* x, const void* y, const void* dy, void* dx, void* dres, const float* gamma,
-                      const float* save_mean, const float* save_rstd, float* sums, float* dgamma, float* dbeta,
-                      long long rows, int C, int relu, unsigned int* barrier, cudaStream_t stream);
 int b200_layernorm_fwd(const void* x, const void* residual, void* y, const float* gamma, const float* beta,
                        float* mean, float* rstd, long long rows, int C, float eps, cudaStream_t stream);
 int b200_layernorm_bwd(const void* x, const void* dy, void* dx, const float* gamma, const float* mean,

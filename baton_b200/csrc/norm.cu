@@ -798,118 +798,6 @@ bn_bwd_reduce_vec_kernel(const uint4* __restrict__ x, const uint4* __restrict__ 
 }
 
 
-// ---- BatchNorm backward in ONE kernel with a device-wide barrier (opt-in: BATON_BN_BWD_FUSED=1;
-// ---- the cluster kernel below is the default) -------
-// phase 1 = bn_bwd_reduce_vec (per-channel sum dy', sum dy' * xhat), device-wide barrier, phase 2 = bn_bwd_apply.
-// The activations of a 32x32-input ResNet layer are <= 1 MB, so the second read hits L2 and the kernel saves a
-// launch.  The barrier is a generation counter in global memory ({count, generation},
-// self-resetting, so CUDA-graph replays need no host reset).  Deadlock freedom: the grid is capped at two CTAs
-// per SM (always co-resident on an otherwise idle or draining GPU), and the programmatic-launch trigger for the
-// NEXT kernel is only given AFTER the barrier, so early-launched dependents can never occupy the SM slots that
-// not-yet-scheduled CTAs of this grid still need.
-__device__ __forceinline__ void grid_barrier_generation(unsigned int* bar) {
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    volatile unsigned int* vb = bar;
-    const unsigned int gen = vb[1];
-    __threadfence();
-    if (atomicAdd(bar, 1u) == gridDim.x - 1) {
-      vb[0] = 0u;                 // reset for the next use (next replay of the graph)
-      __threadfence();
-      atomicAdd(bar + 1, 1u);     // release the others
-    } else {
-      while (vb[1] == gen) {
-      }
-    }
-    __threadfence();
-  }
-  __syncthreads();
-}
-
-__global__ void __launch_bounds__(256, 2)
-bn_bwd_fused_kernel(const uint4* __restrict__ x, const uint4* __restrict__ y, const uint4* __restrict__ dy,
-                    uint4* __restrict__ dx, uint4* __restrict__ dres, const float* __restrict__ gamma,
-                    const float* __restrict__ mean, const float* __restrict__ rstd, float* __restrict__ sums,
-                    float* __restrict__ dgamma, float* __restrict__ dbeta, long long rows, int C, int relu,
-                    int rows_per_cta, unsigned int* __restrict__ bar) {
-  griddep_wait();
-  extern __shared__ float sm[];          // phase 1: [256 threads][16] partials; phase 2: ka, kb, kc, km, kr [C] each
-  const int tpr = C >> 3, rpp = 256 / tpr;
-  const int cg = threadIdx.x % tpr, rg = threadIdx.x / tpr;
-  const long long r0 = static_cast<long long>(blockIdx.x) * rows_per_cta;
-  long long r1 = r0 + rows_per_cta;
-  if (r1 > rows) r1 = rows;
-  {
-    float m[8], rs[8], a[8], q[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { m[j] = mean[cg * 8 + j]; rs[j] = rstd[cg * 8 + j]; a[j] = 0.f; q[j] = 0.f; }
-    for (long long r = r0 + rg; r < r1; r += rpp) {
-      float xf[8], gf[8];
-      unpack8_bn(x[r * tpr + cg], xf);
-      unpack8_bn(dy[r * tpr + cg], gf);
-      if (relu) {
-        float yf[8];
-        unpack8_bn(y[r * tpr + cg], yf);
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          if (!(yf[j] > 0.f)) gf[j] = 0.f;
-      }
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        a[j] += gf[j];
-        q[j] = fmaf(gf[j], (xf[j] - m[j]) * rs[j], q[j]);
-      }
-    }
-    colred_finish(a, q, sm, tpr, cg, rg, sums, C);     // smem reduce + one global atomic per channel per CTA
-  }
-  grid_barrier_generation(bar);                         // every CTA's partial sums are in `sums`
-  griddep_launch_dependents();                          // only now may the next kernel start its prologue
-  float* ka = sm;
-  float* kb = sm + C;
-  float* kc = sm + 2 * C;
-  float* km = sm + 3 * C;
-  float* kr = sm + 4 * C;
-  const float inv_rows = 1.f / static_cast<float>(rows);
-  for (int c = threadIdx.x; c < C; c += 256) {
-    const float s_dy = __ldcg(sums + c), s_dyx = __ldcg(sums + C + c);   // L2: written by other SMs' atomics
-    const float g = gamma != nullptr ? gamma[c] : 1.f;
-    const float r = rstd[c];
-    ka[c] = g * r;
-    kb[c] = s_dy * inv_rows;
-    kc[c] = s_dyx * inv_rows;
-    km[c] = mean[c];
-    kr[c] = r;
-    if (blockIdx.x == 0) {
-      if (dgamma != nullptr) dgamma[c] += s_dyx;
-      if (dbeta != nullptr) dbeta[c] += s_dy;
-    }
-  }
-  __syncthreads();
-  for (long long r = r0 + rg; r < r1; r += rpp) {
-    const long long i = r * tpr + cg;
-    float xf[8], gf[8], o[8];
-    unpack8_bn(x[i], xf);
-    unpack8_bn(dy[i], gf);
-    if (relu) {
-      float yf[8];
-      unpack8_bn(y[i], yf);
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        if (!(yf[j] > 0.f)) gf[j] = 0.f;
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int c = cg * 8 + j;
-      const float xh = (xf[j] - km[c]) * kr[c];
-      o[j] = ka[c] * (gf[j] - kb[c] - xh * kc[c]);
-    }
-    dx[i] = make_uint4(pack_bf16x2(o[0], o[1]), pack_bf16x2(o[2], o[3]), pack_bf16x2(o[4], o[5]), pack_bf16x2(o[6], o[7]));
-    if (dres != nullptr)
-      dres[i] = make_uint4(pack_bf16x2(gf[0], gf[1]), pack_bf16x2(gf[2], gf[3]), pack_bf16x2(gf[4], gf[5]),
-                           pack_bf16x2(gf[6], gf[7]));
-  }
-}
-
 // ---- BatchNorm backward in ONE kernel, cluster edition (default path) ------------------------------------------
 // A thread-block CLUSTER owns a 16-channel slice of the [rows, C] activation (32 B = one sector per row and tensor)
 // and splits the rows between its CTAs.  Every thread reads its (x, y, dy) pieces ONCE and keeps them in
@@ -1376,8 +1264,8 @@ extern "C" int b200_bn_bwd_apply(const void* x, const void* y, const void* dy, v
       rows, C, relu);
   RET_LAST();
 }
-// single-kernel (grid-barrier) BatchNorm backward, opt-in; returns -2 when the shape does not fit the vector layout or the
-// tensor is too large to stay L2-resident between the two phases (the caller then uses the two-kernel path).
+// one launch of the cluster BatchNorm backward with clusters of S CTAs along y; returns -2 when S > 8 and the device
+// does not allow that non-portable cluster size (the caller then uses the two-kernel path).
 template <int ITER>
 static int launch_bn_bwd_cluster(dim3 grid, int S, cudaStream_t stream, const uint4* x, const uint4* y, const uint4* dy_a,
                                  const uint4* dy_b, uint4* dx, uint4* dres, const float* gamma, const float* mean,
@@ -1452,26 +1340,6 @@ extern "C" int b200_bn_bwd_cluster(const void* x, const void* y, const void* dy_
 #undef BNC_GO
 }
 
-extern "C" int b200_bn_bwd_fused(const void* x, const void* y, const void* dy, void* dx, void* dres, const float* gamma,
-                                 const float* save_mean, const float* save_rstd, float* sums, float* dgamma,
-                                 float* dbeta, long long rows, int C, int relu, unsigned int* barrier,
-                                 cudaStream_t stream) {
-  if (rows <= 0) return 0;
-  if (!colred_vec_ok(C, x, relu ? y : nullptr, dy) || (reinterpret_cast<uintptr_t>(dx) & 15) || C > 2048) return -2;
-  if (rows * C * 2 > (32ll << 20)) return -2;
-  const int rpp = 256 / (C >> 3);
-  long long rpc = (rows + 2 * device_sm_count() - 1) / (2 * device_sm_count());          // at most two CTAs per SM: always co-resident
-  rpc = (rpc + rpp - 1) / rpp * rpp;
-  if (rpc < rpp) rpc = rpp;
-  const unsigned grid = static_cast<unsigned>((rows + rpc - 1) / rpc);
-  size_t smem = 256 * 16 * sizeof(float);
-  if (smem < 5 * static_cast<size_t>(C) * sizeof(float)) smem = 5 * static_cast<size_t>(C) * sizeof(float);
-  launch_pdl(bn_bwd_fused_kernel, grid, 256, smem, stream, reinterpret_cast<const uint4*>(x),
-             reinterpret_cast<const uint4*>(y), reinterpret_cast<const uint4*>(dy), reinterpret_cast<uint4*>(dx),
-             reinterpret_cast<uint4*>(dres), gamma, save_mean, save_rstd, sums, dgamma, dbeta, rows, C, relu,
-             static_cast<int>(rpc), barrier);
-  RET_LAST();
-}
 extern "C" int b200_layernorm_fwd(const void* x, const void* residual, void* y, const float* gamma, const float* beta,
                                   float* mean, float* rstd, long long rows, int C, float eps, cudaStream_t stream) {
   if (rows <= 0) return 0;

@@ -229,41 +229,27 @@ class ResNet(FederatedModule):
             return [d, dx_ds]
         return [d, dres]
 
-    # BATON_SGD_OVERLAP=1: parameters from this prefix on receive their gradients first, their optimizer slice runs beside
-    # the rest of the backward pass.  "layer1." = everything but the stem (SGD beside the stem's backward + weight gradient,
-    # which leave most of the GPU idle); "layer3." = the deep layers only (88 % of a ResNet-18's parameters)
-    tail_split_prefix = __import__("os").environ.get("BATON_SGD_SPLIT", "layer1.")
-
-    def explicit_step(self, x, target, loss_acc=None, hooks=None):
+    def explicit_step(self, x, target, loss_acc=None, after_first_gemm=None):
         """Forward + loss + backward of one batch with parameter gradients accumulated into the arena (the same
         contract as ``loss.backward()`` on ``forward``); returns the device ``[mean loss, #correct]`` pair.
         CUDA + arena-adopted training mode only.
 
-        ``hooks`` (optional, from the trainer): ``hooks.tail_grads_ready()`` is called as soon as the gradients of the
-        deep layers (``tail_split_prefix`` onwards: 88 % of a ResNet-18's parameters) are complete, so their optimizer
-        step can run beside the rest of the backward pass; ``hooks.before_tail_forward()`` is called before the first
-        forward use of those weights."""
+        ``after_first_gemm`` (optional, from the trainer) is called right after the GEMM of the first convolution."""
         F = bnn.F
-        pre = self.tail_split_prefix or "layer3."
-        tail_layer = int(pre[5]) - 1 if pre.startswith("layer") and pre[5:6].isdigit() else 2
         if self.stats_workspace is not None:
             self.stats_workspace.zero_()
-        after_first = getattr(hooks, "after_first_gemm", None) if hooks is not None else None
         stem = cp = None
-        fused_stem = _stem_fwd(self.conv1, self.bn1, self.maxpool, x, after_first) if _STEM_FUSED else None
+        fused_stem = _stem_fwd(self.conv1, self.bn1, self.maxpool, x, after_first_gemm) if _STEM_FUSED else None
         if fused_stem is not None:
             h = fused_stem[0]
         else:
-            h, stem = _conv_bn_fwd(self.conv1, self.bn1, x, after_conv=after_first)
+            h, stem = _conv_bn_fwd(self.conv1, self.bn1, x, after_conv=after_first_gemm)
             cp = bnn.Ctx()
             h = bnn._MaxPoolFn.forward(cp, h, self.maxpool.k, self.maxpool.stride, self.maxpool.pad)
         tape = []
-        for li, layer in enumerate((self.layer1, self.layer2, self.layer3, self.layer4)):
-            if li == tail_layer and hooks is not None and getattr(hooks, "_tail_pending", False):
-                hooks.before_tail_forward()
+        for layer in (self.layer1, self.layer2, self.layer3, self.layer4):
             for blk in layer:
                 h = self._block_fwd(blk, h, tape)
-        n_head_blocks = sum(len(l) for l in (self.layer1, self.layer2, self.layer3, self.layer4)[:tail_layer])
         ca = None
         if h.shape[1] == 1 and h.shape[2] == 1:
             feat = h.reshape(h.shape[0], h.shape[3])
@@ -290,8 +276,6 @@ class ResNet(FederatedModule):
         pieces = [d]
         for bi in range(len(tape) - 1, -1, -1):
             pieces = self._block_bwd(tape[bi], pieces)
-            if bi == n_head_blocks and hooks is not None and getattr(hooks, "_split_active", 0):
-                hooks.tail_grads_ready()
         if fused_stem is not None:
             _stem_bwd(fused_stem, self.bn1, self.maxpool, pieces[0], pieces[1] if len(pieces) > 1 else None)
         else:

@@ -143,16 +143,15 @@ def gemm_stats_fusable(M: int, N: int, K: int) -> bool:
 # ---------------------------------------------------------------------------- elementwise / optimizer
 def fused_sgd(w: torch.Tensor, g: torch.Tensor, hyper: torch.Tensor, momentum_buf: Optional[torch.Tensor] = None,
               w_bf16: Optional[torch.Tensor] = None, zero_grad: bool = True, nesterov: bool = False,
-              max_ctas: int = 0, pack: Optional[dict] = None) -> None:
-    """One kernel over the whole flat arena (reference: ``optimizer.step()``, demo.py:47).  ``max_ctas`` caps the
-    grid for a slice that runs concurrently with other work.
+              pack: Optional[dict] = None) -> None:
+    """One kernel over the whole flat arena (reference: ``optimizer.step()``, demo.py:47).
 
     ``pack`` (SURVEY K4, "emits the upload copy"): ``{"wire_slot": int64[1] device word holding the wire address,
     "global_w": fp32 global copy or None, "scale": fp32[1] device scalar or None, "n_pack": elements to pack
     (parameters + float buffers), "wire_fp32": bool}`` -- the step also writes this client's wire copy for the
     round-end collective while the new weights are in registers."""
     pk = pack or {}
-    load().fused_sgd(w, g, momentum_buf, w_bf16, hyper, zero_grad, nesterov, max_ctas, pk.get("wire_slot"),
+    load().fused_sgd(w, g, momentum_buf, w_bf16, hyper, zero_grad, nesterov, pk.get("wire_slot"),
                      pk.get("global_w"), pk.get("scale"), int(pk.get("n_pack", 0)), bool(pk.get("wire_fp32", False)))
 
 

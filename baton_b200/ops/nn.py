@@ -513,21 +513,6 @@ class Conv2d(nn.Module):
 
 
 # ================================================================================ BatchNorm (+residual +ReLU)
-_BN_BWD_FUSED = __import__("os").environ.get("BATON_BN_BWD_FUSED", "0") == "1"   # grid-barrier variant: validated, slower
-# single-kernel BatchNorm backward, one thread-block cluster per 16-channel slice (csrc/norm.cu)
-_BN_BWD_CLUSTER = __import__("os").environ.get("BATON_BN_BWD_CLUSTER", "1") == "1"
-_BN_BWD_MAX_CLUSTER = int(__import__("os").environ.get("BATON_BN_BWD_MAX_CLUSTER", "16"))
-_GRID_BARRIERS = {}
-
-
-def _grid_barrier_words(device):
-    """{count, generation} words of the device-wide barrier used by the single-kernel BatchNorm backward."""
-    buf = _GRID_BARRIERS.get(device)
-    if buf is None:
-        buf = _GRID_BARRIERS[device] = torch.zeros(2, dtype=torch.int32, device=device)
-    return buf
-
-
 class _BNFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, residual, gamma, beta, rmean, rvar, nbt, eps, momentum, relu, training, ws, anchor,
@@ -568,16 +553,10 @@ class _BNFn(torch.autograd.Function):
             gg = tg = torch.zeros(ctx.c, dtype=torch.float32, device=x.device)
         if tb is None:
             gb = tb = torch.zeros(ctx.c, dtype=torch.float32, device=x.device)
-        done = False
-        if _BN_BWD_CLUSTER:
-            done = C_.bn_bwd_cluster(x, y, dy, dy_b, dx, dres, gamma, mean, rstd, tg, tb, ctx.rows, ctx.c, ctx.relu,
-                                     _BN_BWD_MAX_CLUSTER)
-        if not done and dy_b is not None:
-            dy = F.add(dy, dy_b.contiguous())
-        if not done and _BN_BWD_FUSED:       # reduce + device-wide barrier + apply in one kernel
-            done = C_.bn_bwd_fused(x, y, dy, dx, dres, gamma, mean, rstd, ctx.sums_b, tg, tb, ctx.rows, ctx.c, ctx.relu,
-                                   _grid_barrier_words(x.device))
-        if not done:
+        # one launch (a thread-block cluster per 16-channel slice, csrc/norm.cu); shapes it declines take reduce + apply
+        if not C_.bn_bwd_cluster(x, y, dy, dy_b, dx, dres, gamma, mean, rstd, tg, tb, ctx.rows, ctx.c, ctx.relu, 16):
+            if dy_b is not None:
+                dy = F.add(dy, dy_b.contiguous())
             C_.bn_bwd_reduce(x, y, dy, mean, rstd, ctx.sums_b, ctx.rows, ctx.c, ctx.relu)
             C_.bn_bwd_apply(x, y, dy, dx, dres, gamma, mean, rstd, ctx.sums_b, tg, tb, ctx.rows, ctx.c, ctx.relu)
         if ctx.has_res and dres is None:

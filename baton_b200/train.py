@@ -13,8 +13,9 @@ Two executions of the same contract:
 * ``GraphedLocalSGD`` (CUDA) -- the whole step (on-device batch gather, forward,
   loss, backward, fused arena SGD, loss accumulation) is captured once into a
   CUDA graph and replayed per batch; parameters, gradients and momentum live in
-  the flat arena so the optimizer is one kernel (``ops.fused_sgd``) instead of
-  one launch per tensor.  No host synchronisation inside an epoch.
+  the flat arena, so the optimizer takes at most one launch per step beyond the
+  weight-gradient GEMM epilogues instead of one launch per tensor.  No host
+  synchronisation inside an epoch.
 """
 from __future__ import annotations
 
@@ -71,10 +72,17 @@ class GraphedLocalSGD:
     """CUDA local-SGD engine for an arena-adopted model.
 
     One *epoch* -- ``n // batch_size`` steps of {on-device batch gather, forward,
-    fused loss, hand-written backward, ONE fused SGD kernel over the arena, loss
-    accumulation} -- is captured into a single CUDA graph and replayed once per
-    epoch, so the host issues one launch per epoch and never synchronises inside
-    a round: the per-epoch losses are read back together when the round ends.
+    fused loss, hand-written backward, SGD, loss accumulation} -- is captured into
+    a single CUDA graph and replayed once per epoch, so the host issues one launch
+    per epoch and never synchronises inside a round: the per-epoch losses are read
+    back together when the round ends.
+
+    SGD runs in one of two places.  In a hand-scheduled bf16 step
+    (``model.explicit_step``) the split-K = 1 convolution weight-gradient GEMMs
+    apply it in their epilogue and ``fused_sgd_segments`` updates the rest of the
+    arena.  The epoch's last step (it also writes the upload copy), ragged eager
+    steps, ``BATON_SGD_FUSED=0`` and autograd steps run ONE ``fused_sgd`` kernel
+    over the whole arena instead.
 
     ``model`` must already be adopted by a :class:`~baton_b200.parallel.arena.ParamArena`
     (``arena``); the engine is what ``FederatedModule.local_train`` dispatches to
@@ -93,10 +101,6 @@ class GraphedLocalSGD:
         self.input_dtype = input_dtype
         import os
         self.explicit = os.environ.get("BATON_EXPLICIT_STEP", "1") != "0"   # models that offer a hand-scheduled step
-        # optimizer slice of the deep layers beside the rest of the backward pass: opt-in (the HBM-bound slice slows the
-        # latency-bound kernels it runs beside)
-        self.tail_overlap = os.environ.get("BATON_SGD_OVERLAP", "0") == "1"
-        self.tail_ctas = int(os.environ.get("BATON_SGD_TAIL_CTAS", "132"))    # grid cap of the overlapped SGD slice
         # SGD in the epilogue of the convolution weight-gradient GEMMs (explicit step, steps that do not emit the upload
         # copy); 0: one optimizer pass over the whole arena every step
         self.sgd_fused = os.environ.get("BATON_SGD_FUSED", "1") != "0"
@@ -106,11 +110,6 @@ class GraphedLocalSGD:
         self.pack = None              # set by the engine: FedAvgSession.pack_spec() -> last SGD step emits the upload copy
         self.emitted_wire = False
         self.graph_emits_wire = False
-        self._split = None
-        self._split_active = 0
-        self._tail_stream = None
-        self._tail_pending = False
-        self._tail_done = False
         dev = arena.device
         self.device = dev
         self.hyper = torch.zeros(4, dtype=torch.float32, device=dev)
@@ -150,39 +149,29 @@ class GraphedLocalSGD:
         bf = a.theta_bf16
         if explicit is not None and self.loss_kind in ("ce", "cross_entropy"):
             # hand-scheduled forward + loss + backward (no autograd engine): two-piece block gradients, parallel shortcut
-            # branch; the loss kernel accumulates straight into the epoch's running sums.  The optimizer step of the deep
-            # layers (their gradients are complete early in the backward pass) runs on a side stream beside the rest
-            # of the backward pass and the first layers of the NEXT step's forward.
-            # the epoch's last step emits the upload copy from ONE optimizer launch over the whole arena: no split there
-            split = 0 if (emit_wire and self.pack is not None) else self._tail_split()
-            self._split_active = split
-            self._tail_done = False
-            hooks = self if (split or self._first_gemm_hook is not None) else None
-            if self.sgd_fused and fuse_sgd and not split and not emit_wire:
+            # branch; the loss kernel accumulates straight into the epoch's running sums
+            if self.sgd_fused and fuse_sgd and not emit_wire:
                 # the split-K = 1 convolution weight gradients apply SGD in their GEMM epilogue; one launch covers the rest
                 with self.bnn.SGD_EPI.open(a, self.hyper, self.nesterov) as epi:
-                    explicit(xb, yb, loss_acc=self.loss_acc, hooks=hooks)
+                    explicit(xb, yb, loss_acc=self.loss_acc, after_first_gemm=self._first_gemm_hook)
                 F.fused_sgd_segments(a.theta, a.grad, self.hyper, self._segment_table(epi.fused, epi.nograd),
                                      a.momentum, bf, nesterov=self.nesterov)
                 self.emitted_wire = False
                 return
-            explicit(xb, yb, loss_acc=self.loss_acc, hooks=hooks)
-            end = split if (split and self._tail_done) else a.n_param
-            pack = self.pack if (emit_wire and end == a.n_param) else None
-            F.fused_sgd(a.theta[:end], a.grad[:end], self.hyper,
-                        a.momentum[:end] if a.momentum is not None else None,
-                        bf[:end] if bf is not None else None, zero_grad=True, nesterov=self.nesterov, pack=pack)
-            self.emitted_wire = pack is not None
-            return
-        out = self.model(xb)
-        loss, stats = self._loss(out, yb)
-        loss.backward()
-        self.bnn.WGRAD.join()      # weight-gradient GEMMs run on a side stream; they must land before the step
+            explicit(xb, yb, loss_acc=self.loss_acc, after_first_gemm=self._first_gemm_hook)
+            stats = None
+        else:
+            out = self.model(xb)
+            loss, stats = self._loss(out, yb)
+            loss.backward()
+            self.bnn.WGRAD.join()      # weight-gradient GEMMs run on a side stream; they must land before the step
+        # one optimizer pass over the whole arena; the epoch's last step also emits the upload copy
         pack = self.pack if emit_wire else None
         F.fused_sgd(a.theta[: a.n_param], a.grad, self.hyper, a.momentum,
                     bf[: a.n_param] if bf is not None else None, zero_grad=True, nesterov=self.nesterov, pack=pack)
         self.emitted_wire = pack is not None
-        self.loss_acc.add_(stats)
+        if stats is not None:
+            self.loss_acc.add_(stats)
 
     def _segment_table(self, fused, nograd):
         """Device chunk table of the leftover optimizer pass, built once per set of epilogue-updated ranges (they only
@@ -193,51 +182,6 @@ class GraphedLocalSGD:
             segs = self.F.sgd_segments(self.arena.n_param, fused, nograd)
             table = self._seg_tables[key] = torch.tensor(segs, dtype=torch.int64).view(-1, 3).to(self.device)
         return table
-
-    # ---- optimizer / backward overlap (hooks called by ``model.explicit_step``) ----
-    def _tail_split(self) -> int:
-        """Arena offset where the deep layers' parameters start (0: no split)."""
-        if not self.tail_overlap:
-            return 0
-        if self._split is None:
-            prefix = getattr(self.model, "tail_split_prefix", None)
-            self._split = 0
-            if prefix:
-                for name, slot in self.arena.slots.items():
-                    if slot.is_param and name.startswith(prefix):
-                        self._split = slot.offset - slot.offset % 8
-                        break
-        return self._split
-
-    def tail_grads_ready(self):
-        """Gradients of ``theta[split:n_param]`` are complete (once the weight-gradient branch has drained): run their
-        SGD slice on its own stream, on a capped grid, beside the remaining backward pass."""
-        a, dev, split = self.arena, self.device, self._split
-        if self._tail_stream is None:
-            self._tail_stream = torch.cuda.Stream(device=dev)
-        side = self._tail_stream
-        side.wait_stream(torch.cuda.current_stream(dev))
-        wg = self.bnn.WGRAD.streams.get(dev)
-        if wg is not None:
-            side.wait_stream(wg)
-        bf = a.theta_bf16
-        with torch.cuda.stream(side):
-            self.F.fused_sgd(a.theta[split: a.n_param], a.grad[split:], self.hyper,
-                             a.momentum[split:] if a.momentum is not None else None,
-                             bf[split: a.n_param] if bf is not None else None, zero_grad=True, nesterov=self.nesterov,
-                             max_ctas=self.tail_ctas)
-        self._tail_done = True
-        self._tail_pending = True
-
-    def after_first_gemm(self):
-        """Called by ``model.explicit_step`` right after the GEMM of the model's first convolution."""
-        if self._first_gemm_hook is not None:
-            self._first_gemm_hook()
-
-    def before_tail_forward(self):
-        if self._tail_pending:
-            torch.cuda.current_stream(self.device).wait_stream(self._tail_stream)
-            self._tail_pending = False
 
     def _set_hyper(self, lr, momentum, weight_decay, dampening=0.0):
         vals = (float(lr), float(momentum), float(weight_decay), float(dampening))
@@ -258,7 +202,6 @@ class GraphedLocalSGD:
             snap_m = self.arena.momentum.clone() if self.arena.momentum is not None else None
             for _ in range(2):
                 self._step(X, y, perm[:batch_size])
-            self.before_tail_forward()       # drain the overlapped optimizer slice
         torch.cuda.current_stream(self.device).wait_stream(side)
         torch.cuda.synchronize(self.device)
         from .ops._ext import total_launches
@@ -275,7 +218,6 @@ class GraphedLocalSGD:
                                               yp[s * batch_size:(s + 1) * batch_size]),
                            emit_wire=(s == n_steps - 1 and self.pack is not None))
             self.graph_emits_wire = self.pack is not None
-            self.before_tail_forward()       # every forked stream must rejoin before the capture ends
 
         if (self.k3_join is not None and self.explicit and hasattr(self.model, "explicit_step")
                 and getattr(self.model, "compute_dtype", "bf16") == "bf16"):
@@ -358,7 +300,6 @@ class GraphedLocalSGD:
                 if tail:
                     with torch.enable_grad():
                         self._step(X, y, perm_full[n_steps * batch_size:], fuse_sgd=False)
-                    self.before_tail_forward()
                 epoch_losses[e].copy_(self.loss_acc)
         else:
             perm_full = torch.randperm(n, device=self.device)
@@ -369,7 +310,6 @@ class GraphedLocalSGD:
                 for idx in torch.split(perm_full, batch_size):
                     with torch.enable_grad():
                         self._step(X, y, idx)
-                self.before_tail_forward()
                 epoch_losses[e].copy_(self.loss_acc)
         steps = n_steps + (1 if tail else 0)
         self.last_steps = steps

@@ -1,7 +1,6 @@
 """Kernel-correctness tier: every sm_90a kernel against a plain PyTorch fp32
 reference of the same op (SURVEY.md section 4)."""
 import math
-import os
 
 import pytest
 import torch
@@ -400,34 +399,6 @@ def test_batchnorm_fwd_bwd(bnn, relu, with_res, n, h, c):
     assert _rel(bn.bias.grad, ref.bias.grad) < 3e-2
     if with_res:
         assert _rel(res.grad.float() * clear, r32.grad.permute(0, 2, 3, 1) * clear) < 1e-2
-
-
-@pytest.mark.skipif(os.environ.get("BATON_BN_BWD_FUSED") != "1",
-                    reason="experimental single-kernel BatchNorm backward: opt in with BATON_BN_BWD_FUSED=1")
-@pytest.mark.parametrize("n,h,c", [(128, 8, 64), (128, 4, 128), (128, 1, 512), (9, 5, 128)])
-def test_batchnorm_backward_single_kernel_matches_two_kernel_path(bnn, n, h, c):
-    torch.manual_seed(11)
-    dev = _dev()
-    x = (torch.randn(n, h, h, c, device=dev) * 2 + 0.5).to(BF16)
-    res = torch.randn(n, h, h, c, device=dev).to(BF16)
-    dy = None
-    outs = []
-    for fused in (False, True):
-        bnn._BN_BWD_FUSED = fused
-        torch.manual_seed(12)
-        bn = bnn.BatchNorm2d(c, relu=True).to(dev)
-        with torch.no_grad():
-            bn.weight.uniform_(0.5, 1.5)
-        xi, ri = x.clone().requires_grad_(True), res.clone().requires_grad_(True)
-        y = bn(xi, ri)
-        dy = torch.randn_like(y) if dy is None else dy
-        for _ in range(3):                               # the barrier words are reused launch after launch
-            xi.grad = ri.grad = bn.weight.grad = bn.bias.grad = None
-            y.backward(dy, retain_graph=True)
-        outs.append((xi.grad.float(), ri.grad.float(), bn.weight.grad.clone(), bn.bias.grad.clone()))
-    bnn._BN_BWD_FUSED = True
-    for a, b in zip(outs[1], outs[0]):
-        assert _rel(a, b) < 1e-2
 
 
 @pytest.mark.parametrize("n,h,c,relu,two", [(128, 8, 64, True, True), (128, 8, 64, False, False), (128, 4, 128, True, True),

@@ -1,33 +1,10 @@
-"""CPU-side checks of round-2 host logic: the optimizer split point, the collective roofline arithmetic of bench.py and the
-NVLink measurement's degenerate case."""
+"""CPU-side checks of round-2 host logic: the collective roofline arithmetic of bench.py and the NVLink measurement's
+degenerate case."""
 import importlib
 import os
 import sys
 
-import torch
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def test_sgd_split_point_follows_the_model_prefix(monkeypatch):
-    from baton_b200.models import resnet18
-    from baton_b200.parallel.arena import ParamArena
-    from baton_b200.train import GraphedLocalSGD
-    m = resnet18(10)
-    arena = ParamArena(m, torch.device("cpu"))
-    monkeypatch.setenv("BATON_SGD_OVERLAP", "1")
-    tr = GraphedLocalSGD(m, arena, loss="ce", use_graph=False)
-    stem = m.conv1.weight.numel() + m.bn1.weight.numel() + m.bn1.bias.numel()
-    for prefix, want in (("layer1.", arena.slots["layer1.0.conv1.weight"].offset),
-                         ("layer3.", arena.slots["layer3.0.conv1.weight"].offset)):
-        m.tail_split_prefix = prefix
-        tr._split = None
-        split = tr._tail_split()
-        assert split % 8 == 0 and want - 8 < split <= want
-        if prefix == "layer1.":
-            assert split >= stem - 8          # everything but the stem is in the overlapped slice
-    monkeypatch.setenv("BATON_SGD_OVERLAP", "0")
-    assert GraphedLocalSGD(m, arena, loss="ce", use_graph=False)._tail_split() == 0
 
 
 def test_collective_roofline_uses_the_measured_link():
