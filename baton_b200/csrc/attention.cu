@@ -10,8 +10,8 @@
 //   epilogue O = O~ / rowsum   -> out[b*S + q, h*64 : h*64+64]
 //
 // The S x S scores never touch HBM and P is written exactly once (the unfused path writes S, reads S,
-// writes P, reads P).  The default (BATON_FUSED_ATTN=0 selects the three-kernel path); tests/test_gpu_bert.py
-// checks both against an fp32 reference.
+// writes P, reads P).  It runs whenever S = 128, d_head = 64 and there is no mask; tests/test_gpu_bert.py checks it
+// against the multi-kernel path and an fp32 reference.
 #define B200_TU_TAG 4
 #include "launch.h"
 #include "pdl.cuh"
@@ -202,7 +202,7 @@ attention_fwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
 // (k-step = 32 B inside a row vs 16 rows = 2048 B; the two 64-key halves of P / dS are 16384 B apart).  Each
 // consumer warpgroup computes 64 output rows; results are staged in fp32 shared-memory tiles for the row-per-thread
 // passes.  The unfused path reads P twice, writes dP, reads it back, writes dS and reads it twice (all S x S, through
-// HBM); here P is read once and nothing S x S is written.  On by default together with the forward (BATON_FUSED_ATTN).
+// HBM); here P is read once and nothing S x S is written.  It runs wherever the fused forward did.
 struct AttnBwdParams {
   __nv_bfloat16* dqkv;     // [B*S, 3*D]
   int H, D;

@@ -48,7 +48,6 @@ struct GemmParams {
   const float* bias;      // [N] or nullptr
   int out_fp32;           // 1: D is fp32, 0: D is bf16
   int act;                // 0 none, 1 relu, 2 gelu(tanh)
-  int epi_staged;         // persistent kernels: 1 = smem-staged row-coalesced stores, 0 = direct per-lane stores
   float* col_stats;       // optional [2N]: += column sums / sums of squares of the (bf16-rounded) output (BatchNorm)
   int a_mn, b_mn;         // operand majors
   int k_tiles_per_split;  // split-K: k tiles handled by one z-slice
@@ -602,7 +601,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
   const int row = m0 + q * 32 + lane;
   const float* arow = acc_tile + (q * 32 + lane) * L::PART_PITCH;
   const int elt = p.out_fp32 ? 4 : 2;
-  const bool fast = p.epi_staged && vec_ok && !p.atomic_out && (p.N % 8 == 0);
+  const bool fast = vec_ok && !p.atomic_out && (p.N % 8 == 0);
   if (!fast) {
 #pragma unroll 1
     for (int c = half * 32; c < BN; c += 64) {
@@ -1088,12 +1087,7 @@ static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const GemmPa
   if (L::PART_BYTES > ring) ring = L::PART_BYTES;
   int smem = ring + 2 * MAX_STAGES * 8 + 8 * BN * 4 + 1024;
   // occupancy cap: CTAs of this kernel per SM (shared memory is the limiter we control)
-  static int max_ctas = -1;
-  if (max_ctas < 0) {
-    const char* e = std::getenv("BATON_GEMM_CTAS_PER_SM");
-    max_ctas = e != nullptr ? std::atoi(e) : 2;
-    if (max_ctas < 1) max_ctas = 1;
-  }
+  constexpr int max_ctas = 2;
   // atomic epilogues (wgrad): one CTA per SM, co-resident CTAs only contend for the same output lines
   const int ctas_here = p.atomic_out ? 1 : max_ctas;
   const int floor_smem = (227 * 1024) / (ctas_here + 1) + 1024;   // > 1/(ctas+1) of the SM
@@ -1193,12 +1187,6 @@ extern "C" int b200_gemm_bf16(const void* a, const void* b, void* d, const float
   p.a_mn = a_mn; p.b_mn = b_mn; p.k_tiles_per_split = per;
   p.cluster_k = cluster_k;
   p.atomic_out = (accumulate || (split_k > 1 && cluster_k == 1)) ? 1 : 0;
-  static int epi_staged = -1;
-  if (epi_staged < 0) {
-    const char* e = std::getenv("BATON_GEMM_EPI_STAGED");
-    epi_staged = (e != nullptr && e[0] == '0') ? 0 : 1;   // default on: row-coalesced stores
-  }
-  p.epi_staged = epi_staged;
   p.col_stats = col_stats;
   p.tile_flags = tile_flags; p.flag_epoch = flag_epoch; p.alpha = alpha;
   p.flag_elem_off = flag_elem_off; p.flag_tile_elems = flag_tile_elems; p.ldb = ldb;
@@ -1210,14 +1198,8 @@ extern "C" int b200_gemm_bf16(const void* a, const void* b, void* d, const float
   p.stages = per < max_stages ? (per < 2 ? 2 : per) : max_stages;
   dim3 grid((N + bn - 1) / bn, (M + BM - 1) / BM, split_k);
   // large plain GEMMs (>= one wave of tiles, single K pass): persistent kernel with overlapped epilogue
-  static int persistent_on = -1;
-  if (persistent_on < 0) {
-    const char* e = std::getenv("BATON_GEMM_PERSISTENT");
-    persistent_on = (e != nullptr && e[0] == '0') ? 0 : 1;
-  }
   const int num_tiles = static_cast<int>(grid.x * grid.y);
-  const bool persistent = persistent_on && split_k == 1 && tile_flags == nullptr && num_tiles >= device_sm_count() &&
-                          bn == 128;
+  const bool persistent = split_k == 1 && tile_flags == nullptr && num_tiles >= device_sm_count() && bn == 128;
   if (sgd != nullptr) {
     // the optimizer epilogue lives in the fixed-depth kernel and needs each tile's complete gradient in one CTA
     if (split_k != 1 || cluster_k != 1 || persistent) return B200_SGD_EPILOGUE_DECLINED;
@@ -1272,7 +1254,6 @@ extern "C" int b200_gemm_bf16_batched(const void* a, const void* b, void* d, int
   p.M = M; p.N = N; p.K = K; p.D = d; p.ldd = ldd; p.bias = nullptr; p.out_fp32 = out_fp32; p.act = act;
   p.a_mn = a_mn; p.b_mn = b_mn; p.k_tiles_per_split = (K + BK - 1) / BK; p.cluster_k = 1;
   p.atomic_out = accumulate ? 1 : 0;
-  p.epi_staged = 0;
   p.col_stats = nullptr;
   p.tile_flags = nullptr; p.flag_epoch = 0; p.alpha = alpha; p.flag_elem_off = 0; p.flag_tile_elems = 0;
   p.ldb = ldb; p.flag_bias_off = -1; p.flag_epoch_ptr = nullptr; p.stages = 4;
@@ -1283,14 +1264,8 @@ extern "C" int b200_gemm_bf16_batched(const void* a, const void* b, void* d, int
   // attention-sized batches are thousands of one- or two-k-tile problems: a CTA per problem is all
   // prologue (barrier init, first TMA round trip).  Persistent CTAs amortise that and overlap
   // the epilogue of problem i with the loads + MMAs of problem i+1.
-  static int batched_persistent = -1;
-  if (batched_persistent < 0) {
-    const char* e = std::getenv("BATON_GEMM_BATCHED_PERSISTENT");
-    batched_persistent = (e != nullptr && e[0] == '0') ? 0 : 1;
-  }
   const long long total_tiles = static_cast<long long>(grid.x) * grid.y * grid.z;
-  if (batched_persistent && total_tiles >= 2 * device_sm_count() && total_tiles < (1ll << 30)) {
-    p.epi_staged = 1;
+  if (total_tiles >= 2 * device_sm_count() && total_tiles < (1ll << 30)) {
     const int nt = static_cast<int>(total_tiles);
     if (bn == 128) return launch_persistent<128, 3>(ta, tb, p, nt, stream);
     return launch_persistent<64, 5>(ta, tb, p, nt, stream);
@@ -1299,7 +1274,7 @@ extern "C" int b200_gemm_bf16_batched(const void* a, const void* b, void* d, int
   return launch_fixed<64, 8>(ta, tb, p, grid, stream);
 }
 
-// ---- implicit-GEMM convolution (the default; BATON_CONV_IGEMM=0 turns it off) ----
+// ---- implicit-GEMM convolution ----
 extern "C" int b200_encode_map_im2col_bf16(void* map, const void* x, int N, int H, int W, int C, int KH, int KW,
                                             int stride, int pad, int channels, int pixels);
 
@@ -1327,7 +1302,7 @@ extern "C" int b200_conv_igemm_fwd(const void* x, const void* w, void* y, int N,
   GemmParams p;
   p.M = static_cast<int>(M); p.N = Cout; p.K = K; p.D = y; p.ldd = Cout; p.bias = nullptr; p.out_fp32 = 0; p.act = 0;
   p.a_mn = 0; p.b_mn = 0; p.k_tiles_per_split = per; p.cluster_k = cluster_k; p.atomic_out = 0;
-  p.epi_staged = 0; p.col_stats = col_stats;
+  p.col_stats = col_stats;
   p.tile_flags = nullptr; p.flag_epoch = 0; p.alpha = 1.0f; p.flag_elem_off = 0; p.flag_tile_elems = 0; p.ldb = K;
   p.flag_bias_off = -1; p.flag_epoch_ptr = nullptr;
   p.batched = 0; p.batch_inner = 1; p.batch_count = 1; p.d_outer = 0; p.d_inner = 0;
@@ -1373,7 +1348,7 @@ extern "C" int b200_conv_igemm_dgrad(const void* dy, const void* w, void* dx, in
   GemmParams p;
   p.M = static_cast<int>(M); p.N = Cin; p.K = K; p.D = dx; p.ldd = Cin; p.bias = nullptr; p.out_fp32 = 0; p.act = 0;
   p.a_mn = 0; p.b_mn = 1; p.k_tiles_per_split = per; p.cluster_k = cluster_k; p.atomic_out = 0;
-  p.epi_staged = 0; p.col_stats = nullptr;
+  p.col_stats = nullptr;
   p.tile_flags = nullptr; p.flag_epoch = 0; p.alpha = 1.0f; p.flag_elem_off = 0; p.flag_tile_elems = 0;
   p.ldb = static_cast<long long>(KH) * KW * Cin;
   p.flag_bias_off = -1; p.flag_epoch_ptr = nullptr;
@@ -1418,7 +1393,7 @@ extern "C" int b200_conv_igemm_wgrad(const void* dy, const void* x, float* dw, i
   if (sgd != nullptr) set_sgd_epilogue(p, *sgd);
   p.M = Cout; p.N = Kc; p.K = static_cast<int>(Mp); p.D = dw; p.ldd = Kc; p.bias = nullptr; p.out_fp32 = 1; p.act = 0;
   p.a_mn = 1; p.b_mn = 1; p.k_tiles_per_split = per; p.cluster_k = 1; p.atomic_out = 1;
-  p.epi_staged = 0; p.col_stats = nullptr;
+  p.col_stats = nullptr;
   p.tile_flags = nullptr; p.flag_epoch = 0; p.alpha = 1.0f; p.flag_elem_off = 0; p.flag_tile_elems = 0; p.ldb = Kc;
   p.flag_bias_off = -1; p.flag_epoch_ptr = nullptr;
   p.batched = 0; p.batch_inner = 1; p.batch_count = 1; p.d_outer = 0; p.d_inner = 0;

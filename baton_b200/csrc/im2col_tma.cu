@@ -12,7 +12,7 @@
 //
 // This file only contains the encoder, the PTX wrapper and a PROBE kernel that dumps such tiles back to global
 // memory in the layout of the explicit im2col kernel, so the semantics can be pinned down against it
-// (tests/test_gpu_kernels.py::test_tma_im2col_probe_matches_explicit_im2col, opt-in: BATON_TMA_IM2COL=1).
+// (tests/test_gpu_kernels.py::test_tma_im2col_probe_matches_explicit_im2col).
 // Semantics probe only (not on any model path): it pins down the im2col-mode coordinate convention the implicit-GEMM
 // convolution modes of gemm_wgmma.cu rely on.
 #define B200_TU_TAG 5

@@ -95,6 +95,9 @@ inline int device_sm_count() {
   }
   return n;
 }
+// BATON_PDL=0 launches every kernel without the programmatic-serialization attribute.  It selects no separate code:
+// it rules PDL in or out as the cause of an ordering race (DESIGN.md section 6), and scripts/microbench.py measures
+// the per-node cost with and without it.
 inline bool pdl_enabled() {
   static int on = -1;
   if (on < 0) {

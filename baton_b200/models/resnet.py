@@ -7,8 +7,9 @@ a stock PyTorch ResNet ``state_dict`` of the same depth loads unchanged -- the
 ResNet-18 float state is 11,191,242 elements (SURVEY.md section 5.1).
 
 Execution differs from a stock model: activations are bf16 NHWC, every
-convolution is im2col + wgmma GEMM, BatchNorm fuses the residual add and the
-ReLU of the block, parameters live in the flat arena.  The user-model contract
+convolution is a wgmma GEMM (implicit GEMM over TMA im2col loads where the
+shape allows it, explicit im2col otherwise), BatchNorm fuses the residual add
+and the ReLU of the block, parameters live in the flat arena.  The user-model contract
 (``name``, ``__hash__``, ``train(X, y, n_epoch=...)``) comes from
 ``FederatedModule`` (reference demo.py:15-49).
 """
@@ -54,8 +55,7 @@ def _conv_bn_bwd(ctxs, dy_a, dy_b=None, needs_dx=True):
 
 # The stem (conv1 -> bn1 -> relu -> maxpool): BatchNorm + ReLU + max-pool are ONE kernel forward and two backward (the
 # normalised 16x16 activation is never written: the pooled output carries the ReLU mask, BatchNorm's backward sums run
-# over the pooled gradient -- csrc/norm.cu, "ResNet stem").  BATON_STEM_FUSED=0 keeps the separate kernels.
-_STEM_FUSED = __import__("os").environ.get("BATON_STEM_FUSED", "1") != "0"
+# over the pooled gradient -- csrc/norm.cu, "ResNet stem").  Where _stem_fwd declines, the separate kernels run.
 
 
 def _stem_fwd(conv, bn, pool, x, after_conv=None):
@@ -239,7 +239,7 @@ class ResNet(FederatedModule):
         if self.stats_workspace is not None:
             self.stats_workspace.zero_()
         stem = cp = None
-        fused_stem = _stem_fwd(self.conv1, self.bn1, self.maxpool, x, after_first_gemm) if _STEM_FUSED else None
+        fused_stem = _stem_fwd(self.conv1, self.bn1, self.maxpool, x, after_first_gemm)
         if fused_stem is not None:
             h = fused_stem[0]
         else:

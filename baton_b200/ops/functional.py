@@ -41,11 +41,12 @@ def pick_bn(M: int, N: int) -> int:
     return 64
 
 
-_WGRAD_MAX_CTAS = int(__import__("os").environ.get("BATON_WGRAD_MAX_CTAS", "64"))
+_WGRAD_MAX_CTAS = 64        # CTAs of one split-K weight-gradient launch (see pick_split_k)
+_CLUSTER_MIN_KT = 4         # k tiles every CTA of a split-K cluster must keep (see pick_cluster_k)
 
 
 def pick_split_k(M: int, N: int, K: int, bn: int) -> int:
-    """Atomic split-K factor of a weight-gradient GEMM.  ``BATON_WGRAD_MAX_CTAS`` caps the CTAs of one launch: these
+    """Atomic split-K factor of a weight-gradient GEMM.  ``_WGRAD_MAX_CTAS`` caps the CTAs of one launch: these
     GEMMs run as a parallel graph branch beside the dgrad / BatchNorm chain and should leave SMs to it."""
     tiles = ((M + 127) // 128) * ((N + bn - 1) // bn)
     k_tiles = (K + 63) // 64
@@ -56,18 +57,16 @@ def pick_split_k(M: int, N: int, K: int, bn: int) -> int:
 
 def pick_cluster_k(M: int, N: int, K: int, bn: int) -> int:
     """Cluster split-K factor (1, 2, 4 or 8) for GEMMs with few output tiles and a long K."""
-    import os
     tiles = ((M + 127) // 128) * ((N + bn - 1) // bn)
     k_tiles = (K + 63) // 64
-    min_kt = int(os.environ.get("BATON_GEMM_CLUSTER_MIN_KT", "4"))   # k tiles each CTA must keep
-    if min_kt <= 0 or k_tiles < 16:     # short main loops gain nothing from splitting
+    if k_tiles < 16:     # short main loops gain nothing from splitting
         return 1
     best = 1
     for s in (2, 4, 8):
         # clusters of 8 only pay off while they cover at most ~half the SMs
         # (placement needs 8 free SMs inside one GPC); clusters of <= 4 are fine up to a full wave
         cap = NUM_SMS // 2 if s == 8 else 128
-        if tiles * s <= cap and k_tiles >= min_kt * s:
+        if tiles * s <= cap and k_tiles >= _CLUSTER_MIN_KT * s:
             best = s
     return best
 
@@ -310,7 +309,7 @@ def im2col(x: torch.Tensor, kh: int, kw: int, stride: int, pad: int) -> Tuple[to
 
 def conv_igemm_fwd(x: torch.Tensor, w2d: torch.Tensor, kh: int, kw: int, stride: int, pad: int,
                    col_stats: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
-    """EXPERIMENTAL implicit-GEMM convolution forward: ``y[N*Ho*Wo, Cout]`` straight from NHWC ``x`` through TMA
+    """Implicit-GEMM convolution forward: ``y[N*Ho*Wo, Cout]`` straight from NHWC ``x`` through TMA
     im2col loads (no ``col`` buffer).  ``w2d``: ``[Cout, kh*kw*Cin]`` channels_last weights.  Returns ``None``
     when the shape is not supported (Cin % 64 != 0)."""
     n, h, w, c = x.shape
@@ -343,7 +342,7 @@ def conv_igemm_dgrad(dy: torch.Tensor, w2d: torch.Tensor, in_shape, kh: int, kw:
 
 def conv_igemm_wgrad_(dy2d: torch.Tensor, x: torch.Tensor, dw2d: torch.Tensor, kh: int, kw: int, stride: int,
                       pad: int, sgd: Optional[dict] = None) -> bool:
-    """EXPERIMENTAL implicit wgrad: ``dw2d[Cout, kh*kw*Cin] += dy2d^T im2col(x)`` (fp32 atomics, split over
+    """Implicit wgrad: ``dw2d[Cout, kh*kw*Cin] += dy2d^T im2col(x)`` (fp32 atomics, split over
     pixels) without materialising ``im2col(x)``.  ``sgd``: optimizer epilogue as in :func:`gemm`.  False: nothing
     was done (shape not supported, or the optimizer epilogue declined)."""
     n, h, w, c = x.shape

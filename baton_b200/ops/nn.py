@@ -75,6 +75,11 @@ class Ctx:
         pass
 
 
+# dY[M, N] x X[M, K]: a weight-gradient GEMM above this many flops fills the machine on its own, gains nothing from a
+# parallel branch and would only fight the persistent (one CTA per SM) dgrad kernels for SMs, so it runs inline
+_WGRAD_OVERLAP_MAX_FLOPS = 4e9
+
+
 class _WgradOverlap:
     """Weight-gradient GEMMs only feed the optimizer, so they are forked onto a side stream and overlap
     the dgrad -> BatchNorm-backward chain of the layers below (inside a captured graph this becomes a
@@ -83,9 +88,6 @@ class _WgradOverlap:
     is also called by the trainer before the optimizer step."""
 
     def __init__(self):
-        import os
-        self.enabled = os.environ.get("BATON_WGRAD_OVERLAP", "1") != "0"
-        self.max_flops = float(os.environ.get("BATON_WGRAD_OVERLAP_MAX_GFLOP", "4")) * 1e9
         self.streams = {}
         self.keep = []
         self.pending = False
@@ -95,18 +97,14 @@ class _WgradOverlap:
         """Record "the operands are ready" on the current stream.  Calling this BEFORE the dgrad GEMM is enqueued and
         :meth:`run` (with the returned token) AFTER it puts the dgrad kernel -- the one on the critical path -- first
         in the captured graph's launch order while the weight-gradient branch still only depends on what precedes it."""
-        if not self.enabled or not ref.is_cuda:
+        if not ref.is_cuda:
             return None
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(ref.device))
         return ev
 
     def run(self, fn, *keep, after=None):
-        if not self.enabled or not keep[0].is_cuda:
-            return fn()
-        # dY[M, N] x X[M, K]: a GEMM that fills the machine on its own gains nothing from a parallel branch and
-        # would only fight the persistent (one CTA per SM) dgrad kernels for SMs
-        if 2.0 * keep[0].shape[0] * keep[0].shape[-1] * keep[1].shape[-1] > self.max_flops:
+        if not keep[0].is_cuda or 2.0 * keep[0].shape[0] * keep[0].shape[-1] * keep[1].shape[-1] > _WGRAD_OVERLAP_MAX_FLOPS:
             return fn()
         dev = keep[0].device
         side = self.streams.get(dev)
@@ -147,15 +145,12 @@ class _Branch:
     the SMs and are latency bound, so two chains side by side cost the time of the longer one."""
 
     def __init__(self):
-        import os
-        self.enabled = os.environ.get("BATON_BRANCH_OVERLAP", "1") != "0"
         self.streams = {}
         self.keep = []
         self.pending = False
 
     def fork(self, *keep):
-        import contextlib
-        if not self.enabled or not keep[0].is_cuda:
+        if not keep[0].is_cuda:
             return contextlib.nullcontext()
         dev = keep[0].device
         side = self.streams.get(dev)
@@ -343,12 +338,8 @@ class Linear(nn.Module):
 
 
 # ================================================================================ Conv2d (NHWC, implicit GEMM)
-# implicit-GEMM convolution (TMA im2col operands).
-# BATON_CONV_IGEMM=0 falls back to explicit im2col / col2im + GEMM.
-_CONV_IGEMM = __import__("os").environ.get("BATON_CONV_IGEMM", "1") == "1"
-_CONV_IGEMM_DGRAD = __import__("os").environ.get("BATON_CONV_IGEMM_DGRAD", "1") == "1"
-
-
+# implicit-GEMM convolution (TMA im2col operands) wherever the shape allows it; explicit im2col / col2im + GEMM for
+# the shapes it declines (the C = 3 stem, Cin % 64 != 0, stride-2 dgrads, a kernel that reports "unsupported")
 class _ConvFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, w_bf16, kh, kw, stride, pad, anchor, stats=None, gate=None):
@@ -370,7 +361,7 @@ class _ConvFn(torch.autograd.Function):
             ctx.igemm = False
             if kh == 1 and kw == 1 and stride == 1 and pad == 0 and c % 8 == 0:
                 col, ho, wo, kp = x.view(n * h * w, c), h, w, c
-            elif _CONV_IGEMM and c % 64 == 0:
+            elif c % 64 == 0:
                 # A operand gathered by TMA im2col inside the GEMM, no col buffer (backward: implicit
                 # wgrad from x itself)
                 ho, wo, kp = F.conv_out_size(h, kh, stride, pad), F.conv_out_size(w, kw, stride, pad), kh * kw * c
@@ -429,8 +420,7 @@ class _ConvFn(torch.autograd.Function):
         tok = WGRAD.mark(dy2)      # the weight-gradient branch depends on what is enqueued so far, not on the dgrad below
         dx = None
         if ctx.needs_dx:
-            if (_CONV_IGEMM and _CONV_IGEMM_DGRAD and stride == 1 and kh == kw and kh > 1 and kp == k_true
-                    and w_bf16.shape[1] == k_true):
+            if stride == 1 and kh == kw and kh > 1 and kp == k_true and w_bf16.shape[1] == k_true:
                 # implicit dgrad: flipped-filter convolution of dy, no dcol buffer / col2im
                 dx = F.conv_igemm_dgrad(dy2.view(n, ho, wo, cout), w_bf16, (n, h, w, c), kh, kw, pad)
             if dx is None:
@@ -770,9 +760,6 @@ def mse_loss(pred: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
 
 
 # ================================================================================ attention / embedding (BERT)
-_FUSED_ATTN = __import__("os").environ.get("BATON_FUSED_ATTN", "1") == "1"
-
-
 class _AttnFn(torch.autograd.Function):
     """Multi-head self-attention core on a packed ``qkv [B*S, 3*H*dh]`` buffer: four strided-batched
     wgmma GEMMs + the row-softmax kernel forward, five GEMMs + softmax backward; Q/K/V and their
@@ -781,7 +768,7 @@ class _AttnFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, qkv, B, S, H, dh, mask_bias=None):
         D = H * dh
-        if _FUSED_ATTN and S == 128 and dh == 64 and mask_bias is None:
+        if S == 128 and dh == 64 and mask_bias is None:
             # single-kernel forward (csrc/attention.cu): scores stay in shared memory, P is written once
             probs = torch.empty((B * H * S, S), dtype=BF16, device=qkv.device)
             out = torch.empty((B * S, D), dtype=BF16, device=qkv.device)
@@ -814,7 +801,7 @@ class _AttnFn(torch.autograd.Function):
         D = H * dh
         dout = dout.contiguous()
         dqkv = torch.empty_like(qkv)
-        if _FUSED_ATTN and S == 128 and dh == 64 and not getattr(ctx, "masked", False):
+        if S == 128 and dh == 64 and not getattr(ctx, "masked", False):
             # single-kernel backward (csrc/attention.cu): dP / dS never leave the SM
             if load().attention_bwd(qkv, dout, probs, dqkv, B, S, H, dh, 1.0 / math.sqrt(dh)):
                 return dqkv, None, None, None, None, None

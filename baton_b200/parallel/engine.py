@@ -69,14 +69,13 @@ class FederatedEngine:
         self.rank, self.world = self.session.rank, self.session.world
         # K4: the last SGD step of the captured epoch writes the upload copy itself (no pack phase in the collective);
         # only for the plain one-client-per-GPU rounds -- logical clients fold their deltas after training
-        self.prepack = (backend == "fused" and self.device.type == "cuda" and not (logical_clients and logical_clients > self.world)
-                        and __import__("os").environ.get("BATON_PREPACK", "1") != "0")
+        self.prepack = (backend == "fused" and self.device.type == "cuda"
+                        and not (logical_clients and logical_clients > self.world))
         if self.prepack and hasattr(self.session, "pack_spec"):
             self.trainer.pack = self.session.pack_spec()
         # the round-end collective runs on the session's high-priority side stream: the NEXT round's host->device shard
         # copy (and anything else that does not touch the arena) overlaps it; local training joins first
-        self.overlap_collective = (backend == "fused" and self.device.type == "cuda"
-                                   and __import__("os").environ.get("BATON_COLLECTIVE_OVERLAP", "1") != "0")
+        self.overlap_collective = backend == "fused" and self.device.type == "cuda"
         # K3 (bcast_gemm) on the flagship path: the first convolution's weight staging + GEMM acquire the collective's
         # arrival flags, and the head of the next round's captured epoch runs while the collective is still in flight
         self.k3 = bool(self.overlap_collective and tile_flags and hasattr(model, "conv1")

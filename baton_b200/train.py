@@ -77,12 +77,13 @@ class GraphedLocalSGD:
     per epoch and never synchronises inside a round: the per-epoch losses are read
     back together when the round ends.
 
-    SGD runs in one of two places.  In a hand-scheduled bf16 step
-    (``model.explicit_step``) the split-K = 1 convolution weight-gradient GEMMs
-    apply it in their epilogue and ``fused_sgd_segments`` updates the rest of the
-    arena.  The epoch's last step (it also writes the upload copy), ragged eager
-    steps, ``BATON_SGD_FUSED=0`` and autograd steps run ONE ``fused_sgd`` kernel
-    over the whole arena instead.
+    A model that offers ``explicit_step`` trains with it whenever it runs in bf16
+    with the cross-entropy loss; MXFP8, MSE and models without one go through
+    autograd.  SGD runs in one of two places.  In a hand-scheduled step the
+    split-K = 1 convolution weight-gradient GEMMs apply it in their epilogue and
+    ``fused_sgd_segments`` updates the rest of the arena.  The epoch's last step
+    (it also writes the upload copy), ragged eager steps and autograd steps run
+    ONE ``fused_sgd`` kernel over the whole arena instead.
 
     ``model`` must already be adopted by a :class:`~baton_b200.parallel.arena.ParamArena`
     (``arena``); the engine is what ``FederatedModule.local_train`` dispatches to
@@ -99,11 +100,6 @@ class GraphedLocalSGD:
         self.nesterov = nesterov
         self.use_graph = use_graph
         self.input_dtype = input_dtype
-        import os
-        self.explicit = os.environ.get("BATON_EXPLICIT_STEP", "1") != "0"   # models that offer a hand-scheduled step
-        # SGD in the epilogue of the convolution weight-gradient GEMMs (explicit step, steps that do not emit the upload
-        # copy); 0: one optimizer pass over the whole arena every step
-        self.sgd_fused = os.environ.get("BATON_SGD_FUSED", "1") != "0"
         self._seg_tables = {}
         self.k3_join = None           # set by the engine: callable joining the round-end collective (enables the graph split)
         self._first_gemm_hook = None
@@ -142,7 +138,7 @@ class GraphedLocalSGD:
         ws = getattr(self.model, "stats_workspace", None)
         if ws is not None and not getattr(self.model, "zeroes_own_workspace", False):
             ws.zero_()
-        explicit = getattr(self.model, "explicit_step", None) if self.explicit else None
+        explicit = getattr(self.model, "explicit_step", None)
         if getattr(self.model, "compute_dtype", "bf16") != "bf16":
             explicit = None            # the hand-scheduled step drives the bf16 conv kernels; MXFP8 convs go through autograd
         a = self.arena
@@ -150,7 +146,7 @@ class GraphedLocalSGD:
         if explicit is not None and self.loss_kind in ("ce", "cross_entropy"):
             # hand-scheduled forward + loss + backward (no autograd engine): two-piece block gradients, parallel shortcut
             # branch; the loss kernel accumulates straight into the epoch's running sums
-            if self.sgd_fused and fuse_sgd and not emit_wire:
+            if fuse_sgd and not emit_wire:
                 # the split-K = 1 convolution weight gradients apply SGD in their GEMM epilogue; one launch covers the rest
                 with self.bnn.SGD_EPI.open(a, self.hyper, self.nesterov) as epi:
                     explicit(xb, yb, loss_acc=self.loss_acc, after_first_gemm=self._first_gemm_hook)
@@ -219,7 +215,7 @@ class GraphedLocalSGD:
                            emit_wire=(s == n_steps - 1 and self.pack is not None))
             self.graph_emits_wire = self.pack is not None
 
-        if (self.k3_join is not None and self.explicit and hasattr(self.model, "explicit_step")
+        if (self.k3_join is not None and hasattr(self.model, "explicit_step")
                 and getattr(self.model, "compute_dtype", "bf16") == "bf16"):
             # bcast_gemm (K3): the epoch is captured as TWO graphs that share one memory pool.  Graph 1 ends right after
             # the first convolution's GEMM of the first step -- everything in it either does not touch the parameter

@@ -6,7 +6,6 @@ import sys
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-os.environ.setdefault("BATON_WGRAD_OVERLAP", "1")
 from baton_b200.models import bert_tiny, resnet18  # noqa: E402
 from baton_b200.ops import functional as F  # noqa: E402
 from baton_b200.ops import nn as bnn  # noqa: E402
@@ -54,8 +53,6 @@ sess.join()
 sess.aggregate(my_n=16.0)
 # fused attention (S = 128, d = 64)
 qkv = torch.randn(2 * 128, 3 * 2 * 64, device=dev).to(BF16).requires_grad_(True)
-os.environ["BATON_FUSED_ATTN"] = "1"
-bnn._FUSED_ATTN = True
 bnn.attention(qkv, 2, 128, 2, 64).sum().backward()
 b = bert_tiny(3)
 ab = ParamArena(b, dev)

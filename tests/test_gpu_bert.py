@@ -84,7 +84,7 @@ def test_bert_tiny_matches_fp32_reference_and_trains():
     assert hist[-1] < hist[0], hist
 
 
-def test_fused_attention_forward_and_backward_match_multi_kernel_path():
+def test_fused_attention_forward_and_backward_match_masked_multi_kernel_path():
     from baton_b200.ops import nn as bnn
     torch.manual_seed(0)
     dev = torch.device("cuda:0")
@@ -92,14 +92,12 @@ def test_fused_attention_forward_and_backward_match_multi_kernel_path():
     D = H * dh
     qkv = (torch.randn(B * S, 3 * D, device=dev) * 0.5).to(BF16)
     outs = []
-    default = bnn._FUSED_ATTN
-    for fused in (False, True):
-        bnn._FUSED_ATTN = fused
+    # a mask sends forward and backward down the multi-kernel path; adding a bf16 zero to the scores is exact
+    for mask_bias in (torch.zeros(B, S, device=dev), None):
         x = qkv.clone().requires_grad_(True)
-        out = bnn.attention(x, B, S, H, dh)
+        out = bnn.attention(x, B, S, H, dh, mask_bias=mask_bias)
         g = torch.ones_like(out)
         out.backward(g)
         outs.append((out.detach().float(), x.grad.float()))
-    bnn._FUSED_ATTN = default
     assert _rel(outs[1][0], outs[0][0]) < 2e-2
     assert _rel(outs[1][1], outs[0][1]) < 3e-2

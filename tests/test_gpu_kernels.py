@@ -211,23 +211,27 @@ def test_tma_im2col_probe_matches_explicit_im2col(F, c, k, stride, pad, h):
 @pytest.mark.parametrize("cin,cout,k,stride,pad,h,n", [(64, 64, 3, 1, 1, 8, 128), (64, 128, 3, 2, 1, 8, 128),
                                                        (128, 128, 3, 1, 1, 4, 128), (256, 256, 3, 1, 1, 2, 128),
                                                        (64, 128, 1, 2, 0, 8, 128), (64, 64, 3, 1, 1, 5, 7)])
-def test_implicit_gemm_conv_matches_im2col_path(bnn, cin, cout, k, stride, pad, h, n):
+def test_implicit_gemm_conv_matches_im2col_path(F, bnn, cin, cout, k, stride, pad, h, n):
     torch.manual_seed(cin + cout + k)
     dev = _dev()
     x = torch.randn(n, h, h, cin, device=dev).to(BF16)
-    outs = []
-    for igemm in (False, True):
-        bnn._CONV_IGEMM = igemm
-        torch.manual_seed(1)
-        conv = bnn.Conv2d(cin, cout, k, stride, pad).to(dev)
-        xi = x.clone().requires_grad_(True)
-        y = conv(xi)
-        y.backward(torch.ones_like(y) * 0.5)
-        outs.append((y.detach().float(), xi.grad.float(), conv.weight.grad.float()))
-    bnn._CONV_IGEMM = True
-    assert _rel(outs[1][0], outs[0][0]) < 1e-2
-    assert _rel(outs[1][1], outs[0][1]) < 1e-2
-    assert _rel(outs[1][2], outs[0][2]) < 1e-2
+    torch.manual_seed(1)
+    conv = bnn.Conv2d(cin, cout, k, stride, pad).to(dev)
+    xi = x.clone().requires_grad_(True)
+    y = conv(xi)
+    dy = torch.ones_like(y) * 0.5
+    y.backward(dy)
+    # reference: the explicit im2col / col2im + GEMM lowering the layer takes for shapes implicit GEMM declines
+    w2d = conv._w_bf16()
+    col, ho, wo, _ = F.im2col(x, k, k, stride, pad)
+    dy2 = dy.reshape(n * ho * wo, cout)
+    y_ref = F.gemm(col, w2d).view(n, ho, wo, cout)
+    dx_ref = F.col2im(F.gemm(dy2, w2d, b_mn=True), (n, h, h, cin), k, k, stride, pad, ho, wo)
+    dw_ref = F.gemm(dy2, col, a_mn=True, b_mn=True, out_dtype=torch.float32, accumulate=True)
+    dw_ref = dw_ref.view(cout, k, k, cin).permute(0, 3, 1, 2)
+    assert _rel(y.detach(), y_ref) < 1e-2
+    assert _rel(xi.grad, dx_ref) < 1e-2
+    assert _rel(conv.weight.grad, dw_ref) < 1e-2
 
 
 def test_gemm_simt_fallback_small_pitch(F):
