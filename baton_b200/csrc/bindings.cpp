@@ -187,6 +187,26 @@ bool conv_igemm_dgrad(const at::Tensor& dy, const at::Tensor& w, at::Tensor dx, 
   check(rc, "conv_igemm_dgrad");
   return true;
 }
+// stride 2: `ntaps` (4) taps per parity class, `taps` (4 x 4) packed tap words (ops/functional.py conv_s2_dgrad_taps)
+bool conv_igemm_dgrad_s2(const at::Tensor& dy, const at::Tensor& w, at::Tensor dx, int64_t kh, int64_t kw,
+                         const std::vector<int64_t>& ntaps, const std::vector<int64_t>& taps, int64_t force_bn) {
+  CHECK_CUDA(dy); CHECK_CUDA(w); CHECK_CUDA(dx);
+  TORCH_CHECK(dy.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16 && dx.scalar_type() == at::kBFloat16 &&
+              dy.dim() == 4 && dx.dim() == 4 && dy.is_contiguous() && w.is_contiguous() && dx.is_contiguous());
+  TORCH_CHECK(ntaps.size() == 4 && taps.size() == 16, "conv_igemm_dgrad_s2: 4 classes x 4 taps");
+  int nt[4], tw[16];
+  for (int i = 0; i < 4; ++i) nt[i] = static_cast<int>(ntaps[i]);
+  for (int i = 0; i < 16; ++i) tw[i] = static_cast<int>(taps[i]);
+  const c10::cuda::CUDAGuard guard(dy.device());
+  const int rc = b200_conv_igemm_dgrad_s2(cptr(dy), cptr(w), ptr(dx), static_cast<int>(dx.size(0)),
+                                          static_cast<int>(dx.size(1)), static_cast<int>(dx.size(2)),
+                                          static_cast<int>(dx.size(3)), static_cast<int>(dy.size(3)), static_cast<int>(kh),
+                                          static_cast<int>(kw), static_cast<int>(dy.size(1)), static_cast<int>(dy.size(2)),
+                                          nt, tw, static_cast<int>(force_bn), cur_stream());
+  if (rc == -2) return false;
+  check(rc, "conv_igemm_dgrad_s2");
+  return true;
+}
 bool conv_igemm_wgrad(const at::Tensor& dy, const at::Tensor& x, at::Tensor dw, int64_t cout, int64_t kh, int64_t kw,
                       int64_t stride, int64_t pad, int64_t ho, int64_t wo, int64_t split_k, int64_t force_bn,
                       const std::optional<at::Tensor>& sgd_theta, const std::optional<at::Tensor>& sgd_theta_bf16,
@@ -665,6 +685,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("conv_igemm_fwd", &conv_igemm_fwd);
   m.def("conv_igemm_wgrad", &conv_igemm_wgrad);
   m.def("conv_igemm_dgrad", &conv_igemm_dgrad);
+  m.def("conv_igemm_dgrad_s2", &conv_igemm_dgrad_s2);
   m.def("gemm_batched", &gemm_batched);
   m.def("gemm_fp8", &gemm_fp8);
   m.def("quant_mx_rows", &quant_mx_rows);

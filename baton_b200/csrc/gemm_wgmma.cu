@@ -40,6 +40,7 @@ constexpr int GEMM_THREADS = 384;
 constexpr int CONSUMER_WARPS = 8;      // warpgroups 1 and 2
 constexpr int CONSUMER_THREADS = 32 * CONSUMER_WARPS;
 constexpr int MAX_STAGES = 8;
+constexpr int S2_MAX_TAPS = 4;         // taps of one parity class of a stride-2 dgrad (3x3: at most 2 x 2)
 
 struct GemmParams {
   int M, N, K;
@@ -81,6 +82,11 @@ struct GemmParams {
   __nv_bfloat16* sgd_wb = nullptr;
   float* sgd_mom = nullptr;
   int sgd_nesterov = 0;
+  // stride-2 implicit dgrad (CONV == 4): dx pixel (2i + a, 2j + b) of parity class c = 2a + b sums s2_ntaps[c] taps,
+  // each packed as filter tap | dy row offset << 16 | dy column offset << 24: dy pixel (i + dp, j + dq)
+  int conv_h = 0, conv_w = 0;  // dx image size
+  int s2_ntaps[4] = {0, 0, 0, 0};
+  int s2_tap[4][S2_MAX_TAPS] = {};
 };
 
 // Wait until every arrival flag covering arena elements [e0, e1] has reached `need` (published by the FedAvg kernel with
@@ -346,13 +352,63 @@ __device__ __forceinline__ void consume_ktiles(float (&acc)[BN / 2], uint8_t* sm
   if (prev >= 0 && lane_id() == 0) mbar_arrive(&empty_bar[prev]);
 }
 
+// ---- stride-2 implicit dgrad (CONV == 4): sub-pixel decomposition ----
+// The dx pixels of parity class c = 2a + b, (2i + a, 2j + b), form a stride-1 correlation of dy with the taps that land
+// on them.  Every class enumerates the same N x Ho x Wo grid of (n, i, j) as GEMM rows; blockIdx.y = c * m_tiles + m
+// tile.  A class without taps runs no k tile and stores zeros; rows outside dx (odd H or W) are not stored.
+__device__ __forceinline__ int s2_class(const GemmParams& p, int& m0) {
+  const int tiles_m = (p.M + BM - 1) / BM;
+  const int cls = static_cast<int>(blockIdx.y) / tiles_m;
+  m0 = (static_cast<int>(blockIdx.y) - cls * tiles_m) * BM;
+  return cls;
+}
+// selects instead of a dynamic index: a runtime-indexed kernel parameter array would be copied to local memory
+__device__ __forceinline__ int s2_ntaps(const GemmParams& p, int cls) {
+  int n = 0;
+#pragma unroll
+  for (int c = 0; c < 4; ++c) n = c == cls ? p.s2_ntaps[c] : n;
+  return n;
+}
+__device__ __forceinline__ int s2_tap(const GemmParams& p, int cls, int slot) {
+  int w = 0;
+#pragma unroll
+  for (int c = 0; c < 4; ++c)
+#pragma unroll
+    for (int t = 0; t < S2_MAX_TAPS; ++t) w = (c == cls && t == slot) ? p.s2_tap[c][t] : w;
+  return w;
+}
+// dx row of GEMM row m of class cls, or -1 (m >= M, or the pixel lies past the last row / column of an odd-sized dx)
+__device__ __forceinline__ int s2_dx_row(const GemmParams& p, int cls, int m) {
+  if (m >= p.M) return -1;
+  const int hw = p.conv_ho * p.conv_wo;
+  const int n = m / hw, r = m - n * hw;
+  const int i = r / p.conv_wo, j = r - i * p.conv_wo;
+  const int h = 2 * i + (cls >> 1), w = 2 * j + (cls & 1);
+  return (h < p.conv_h && w < p.conv_w) ? (n * p.conv_h + h) * p.conv_w + w : -1;
+}
+// TMA loads of k tile kt of class cls: A = 128 dy pixels (i + dp, j + dq) x 64 output channels (zero outside dy),
+// B = the [64 cout] x [BN cin] slab of the tap inside the channels_last weight matrix, MN-major
+template <int BN>
+__device__ __forceinline__ void s2_load_ktile(const CUtensorMap* tmA, const CUtensorMap* tmB, const GemmParams& p,
+                                              uint8_t* sa, uint8_t* sb, uint64_t* bar, int cls, int kt, int m0, int n0) {
+  const int cblocks = p.conv_cin >> 6;
+  const int slot = kt / cblocks, cb = kt - slot * cblocks;
+  const int tw = s2_tap(p, cls, slot);
+  const int q0 = m0 % p.conv_wo, t0 = m0 / p.conv_wo;
+  tma_load_im2col_4d(sa, tmA, bar, cb * 64, q0, t0 % p.conv_ho, t0 / p.conv_ho, (tw >> 24) & 0xff, (tw >> 16) & 0xff);
+  const int wcol = (tw & 0xffff) * p.conv_ncol + n0;
+#pragma unroll
+  for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * 8192, tmB, bar, wcol + j * 64, cb * 64);
+}
+
 // ---- fixed-depth pipeline: the default path ----
 // CONV: 0 = plain GEMM; 1 = implicit-GEMM conv forward (A = im2col(x) gathered by TMA im2col, k-tile = one filter
 // tap x 64 input channels); 2 = implicit wgrad (B = im2col(x) MN-major, k-tile = 64 output pixels, every 64-wide
 // N atom = one tap x 64 channels); 3 = implicit dgrad of a stride-1 convolution: dx = conv(dy, flipped w) -- A =
 // im2col(dy) gathered by TMA im2col with pad' = k - 1 - pad (k-tile = one flipped tap x 64 OUTPUT channels), B = the
 // [64 cout] x [BN cin] slab of that tap inside the channels_last weight matrix, loaded MN-major (no weight transpose,
-// no col2im).  See csrc/im2col_tma.cu for the tensor maps.
+// no col2im); 4 = implicit dgrad of a stride-2 convolution, one parity class of dx pixels per group of M tiles (see
+// s2_class).  See csrc/im2col_tma.cu for the tensor maps.
 // SGD: optimizer epilogue instantiation (weight gradients only) -- every other GEMM keeps the plain epilogue.
 template <int BN, int STAGES, int CONV = 0, bool SGD = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
@@ -369,15 +425,17 @@ gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 
   griddep_launch_dependents();  // PDL: the next kernel may start its prologue now
   const int warp = threadIdx.x >> 5;
-  const int m0 = blockIdx.y * BM;
+  int m0 = blockIdx.y * BM;
+  const int cls = CONV == 4 ? s2_class(p, m0) : 0;
   const int n0 = blockIdx.x * BN;
-  const int k_tiles_total = (p.K + BK - 1) / BK;
+  const int k_tiles_total = CONV == 4 ? s2_ntaps(p, cls) * (p.conv_cin >> 6) : (p.K + BK - 1) / BK;
   const int bz_outer = p.batched ? static_cast<int>(blockIdx.z) / p.batch_inner : 0;
   const int bz_inner = p.batched ? static_cast<int>(blockIdx.z) % p.batch_inner : 0;
   const int kt_begin = p.batched ? 0 : blockIdx.z * p.k_tiles_per_split;
   int kt_end = kt_begin + p.k_tiles_per_split;
   if (kt_end > k_tiles_total) kt_end = k_tiles_total;
-  const int num_kt = kt_end - kt_begin;  // host guarantees >= 1 for every launched z
+  // host guarantees >= 1 for every launched z, except CONV == 4: a class without taps runs none
+  const int num_kt = kt_end - kt_begin;
 
   if (warp == 0 && elect_one()) {
     tma_prefetch_desc(&tmA);
@@ -436,6 +494,8 @@ gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
             for (int j = 0; j < BN / 64; ++j)
               tma_load_4d(sb + j * 8192, &tmB, &full_bar[s], n0 + j * 64, k0, bz_inner, bz_outer);
           }
+        } else if constexpr (CONV == 4) {
+          s2_load_ktile<BN>(&tmA, &tmB, p, sa, sb, &full_bar[s], cls, kt_begin + i, m0, n0);
         } else {
         if constexpr (CONV == 1 || CONV == 3) {
           // k-tile -> (filter tap, 64-channel block); base pixel of this CTA's 128 output pixels in input coords
@@ -502,10 +562,11 @@ gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     const int c_begin = (ew < 4 ? 0 : (NCHUNK + 1) / 2) * 32, c_end = (ew < 4 ? (NCHUNK + 1) / 2 : NCHUNK) * 32;
     const int lrow = q * 32 + static_cast<int>(lane_id());
     const int row = m0 + lrow;
-    const bool row_ok = row < p.M;
+    const int orow = CONV == 4 ? s2_dx_row(p, cls, row) : row;   // output row (CONV == 4: -1 = not stored)
+    const bool row_ok = CONV == 4 ? orow >= 0 : row < p.M;
     const size_t elt = p.out_fp32 ? 4 : 2;
     uint8_t* drow = reinterpret_cast<uint8_t*>(p.D) +
-                    (static_cast<size_t>(row) * p.ldd + static_cast<size_t>(bz_outer) * p.d_outer +
+                    (static_cast<size_t>(CONV == 4 && orow < 0 ? 0 : orow) * p.ldd + static_cast<size_t>(bz_outer) * p.d_outer +
                      static_cast<size_t>(bz_inner) * p.d_inner) * elt;
     const bool vec_ok = ((reinterpret_cast<uintptr_t>(p.D) & 15) == 0) && ((p.ldd * elt) % 16 == 0);
     const bool sgd_vec = SGD && (p.ldd % 4 == 0) &&
@@ -1364,6 +1425,59 @@ extern "C" int b200_conv_igemm_dgrad(const void* dy, const void* w, void* dx, in
   }
   if (bn == 128) return launch_fixed<128, 6, 3>(ta, tb, p, grid, stream);
   return launch_fixed<64, 8, 3>(ta, tb, p, grid, stream);
+}
+
+// input gradient of a STRIDE-2 convolution by sub-pixel decomposition (see s2_class): dx[N, H, W, Cin] from dy NHWC bf16
+// [N, Ho, Wo, Cout] and w [Cout, KH*KW*Cin] channels_last, both channel counts multiples of 64.  `ntaps[c]` taps of
+// class c are `taps[c * S2_MAX_TAPS + t]` (filter tap | dp << 16 | dq << 24, ops/functional.py conv_s2_dgrad_taps).
+// One launch for all four classes; every element of dx is written.
+extern "C" int b200_conv_igemm_dgrad_s2(const void* dy, const void* w, void* dx, int N, int H, int W, int Cin, int Cout,
+                                        int KH, int KW, int Ho, int Wo, const int* ntaps, const int* taps, int force_bn,
+                                        cudaStream_t stream) {
+  using namespace b200;
+  const long long M = static_cast<long long>(N) * Ho * Wo;   // GEMM rows of one class
+  if (static_cast<long long>(N) * H * W <= 0 || Cin <= 0) return 0;
+  if (Cout % 64 != 0 || Cin % 64 != 0 || M <= 0 || static_cast<long long>(N) * H * W > (1ll << 30) ||
+      (H + 1) / 2 > Ho || (W + 1) / 2 > Wo || (reinterpret_cast<uintptr_t>(dy) & 15) ||
+      (reinterpret_cast<uintptr_t>(w) & 15) || (reinterpret_cast<uintptr_t>(dx) & 15))
+    return -2;
+  const long long tiles_m = (M + BM - 1) / BM;
+  if (4 * tiles_m > 65535) return -2;
+  GemmParams p;
+  int max_taps = 0;
+  for (int c = 0; c < 4; ++c) {
+    if (ntaps[c] < 0 || ntaps[c] > S2_MAX_TAPS) return -2;
+    for (int t = 0; t < ntaps[c]; ++t) {
+      const int tw = taps[c * S2_MAX_TAPS + t];
+      if (tw < 0 || (tw & 0xffff) >= KH * KW) return -2;
+      p.s2_tap[c][t] = tw;
+    }
+    p.s2_ntaps[c] = ntaps[c];
+    max_taps = ntaps[c] > max_taps ? ntaps[c] : max_taps;
+  }
+  if (max_taps == 0) return -2;
+  const int bn = clamp_bn(force_bn > 0 ? force_bn : (Cin > 64 ? 128 : 64));
+  CUtensorMap ta, tb;
+  // dy traversed pixel by pixel over its own extent; the tap offsets (dq, dp) shift each gather, zero outside dy
+  int rc = b200_encode_map_im2col_bf16(&ta, dy, N, Ho, Wo, Cout, 1, 1, 1, 0, 64, BM);
+  if (rc) return rc;
+  rc = make_map(&tb, w, Cout, static_cast<long long>(KH) * KW * Cin, static_cast<long long>(KH) * KW * Cin, 64, BK);
+  if (rc) return rc;
+  // single K pass per CTA: these GEMMs are short (at most 4 taps x Cout / 64 k tiles) and run on the dgrad chain
+  // beside the weight-gradient branch, where a cluster split would take SMs from it
+  const int k_tiles = max_taps * (Cout / 64);
+  p.M = static_cast<int>(M); p.N = Cin; p.K = k_tiles * BK; p.D = dx; p.ldd = Cin; p.bias = nullptr; p.out_fp32 = 0;
+  p.act = 0; p.a_mn = 0; p.b_mn = 1; p.k_tiles_per_split = k_tiles; p.cluster_k = 1; p.atomic_out = 0;
+  p.col_stats = nullptr;
+  p.tile_flags = nullptr; p.flag_epoch = 0; p.alpha = 1.0f; p.flag_elem_off = 0; p.flag_tile_elems = 0;
+  p.ldb = static_cast<long long>(KH) * KW * Cin;
+  p.flag_bias_off = -1; p.flag_epoch_ptr = nullptr;
+  p.batched = 0; p.batch_inner = 1; p.batch_count = 1; p.d_outer = 0; p.d_inner = 0;
+  p.conv_ho = Ho; p.conv_wo = Wo; p.conv_stride = 2; p.conv_pad = 0; p.conv_kw = KW; p.conv_cin = Cout;
+  p.conv_taps = KH * KW; p.conv_ncol = Cin; p.conv_h = H; p.conv_w = W;
+  dim3 grid((Cin + bn - 1) / bn, static_cast<unsigned>(4 * tiles_m), 1);
+  if (bn == 128) return launch_fixed<128, 6, 4>(ta, tb, p, grid, stream);
+  return launch_fixed<64, 8, 4>(ta, tb, p, grid, stream);
 }
 
 // weight gradient: dw[Cout, KH*KW*Cin] (fp32, accumulated with red.add) += dy[N*Ho*Wo, Cout]^T im2col(x)

@@ -44,6 +44,8 @@ int b200_conv_igemm_fwd(const void* x, const void* w, void* y, int N, int H, int
                         cudaStream_t stream);
 int b200_conv_igemm_dgrad(const void* dy, const void* w, void* dx, int N, int H, int W, int Cin, int Cout, int KH, int KW,
                           int pad, int Ho, int Wo, int cluster_k, int force_bn, cudaStream_t stream);
+int b200_conv_igemm_dgrad_s2(const void* dy, const void* w, void* dx, int N, int H, int W, int Cin, int Cout, int KH,
+                             int KW, int Ho, int Wo, const int* ntaps, const int* taps, int force_bn, cudaStream_t stream);
 int b200_conv_igemm_wgrad(const void* dy, const void* x, float* dw, int N, int H, int W, int Cin, int Cout, int KH, int KW,
                           int stride, int pad, int Ho, int Wo, int split_k, int force_bn, const B200SgdEpilogue* sgd,
                           cudaStream_t stream);

@@ -324,19 +324,66 @@ def conv_igemm_fwd(x: torch.Tensor, w2d: torch.Tensor, kh: int, kw: int, stride:
     return y if ok else None
 
 
-def conv_igemm_dgrad(dy: torch.Tensor, w2d: torch.Tensor, in_shape, kh: int, kw: int, pad: int) -> Optional[torch.Tensor]:
-    """Implicit-GEMM input gradient of a STRIDE-1 convolution: ``dx[N, H, W, Cin]`` from NHWC ``dy`` and the
-    channels_last weights ``w2d [Cout, kh*kw*Cin]`` -- the flipped-filter convolution of ``dy``, gathered by TMA
-    im2col, with the weight slab of each tap loaded MN-major in place (no ``dcol`` buffer, no col2im, no weight
-    transpose).  Returns ``None`` when the shape is not supported (channels not multiples of 64)."""
+S2_MAX_TAPS = 4     # taps of one parity class the stride-2 dgrad kernel takes (gemm_wgmma.cu S2_MAX_TAPS)
+
+
+def conv_s2_dgrad_taps(kh: int, kw: int, pad: int, ho: int, wo: int) -> Optional[List[List[Tuple[int, int, int]]]]:
+    """Sub-pixel decomposition of the input gradient of a stride-2 convolution with dy of size ``ho x wo``.
+
+    Class ``c = 2a + b`` holds the dx pixels ``(2i + a, 2j + b)``; its entry lists the taps ``(r * kw + s, dp, dq)``
+    with ``dx[2i + a, 2j + b] = sum dy[i + dp, j + dq] * W[r, s]`` (``2 (i + dp) - pad + r = 2i + a``), terms with
+    ``dy`` outside the image being zero.  Taps whose dy pixel lies past dy for every ``i`` / ``j`` are left out.
+    ``None`` when a class needs a negative offset or more than ``S2_MAX_TAPS`` taps."""
+    classes = []
+    for a in (0, 1):
+        for b in (0, 1):
+            taps = []
+            for r in range(kh):
+                if (a + pad - r) % 2:
+                    continue
+                dp = (a + pad - r) // 2
+                for s in range(kw):
+                    if (b + pad - s) % 2:
+                        continue
+                    dq = (b + pad - s) // 2
+                    if dp < 0 or dq < 0:
+                        return None
+                    if dp < ho and dq < wo:
+                        taps.append((r * kw + s, dp, dq))
+            if len(taps) > S2_MAX_TAPS:
+                return None
+            classes.append(taps)
+    return classes
+
+
+def conv_igemm_dgrad(dy: torch.Tensor, w2d: torch.Tensor, in_shape, kh: int, kw: int, pad: int, stride: int = 1,
+                     out: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
+    """Implicit-GEMM input gradient of a stride-1 or stride-2 convolution: ``dx[N, H, W, Cin]`` from NHWC ``dy`` and
+    the channels_last weights ``w2d [Cout, kh*kw*Cin]``, gathered by TMA im2col, with the weight slab of each tap
+    loaded MN-major in place (no ``dcol`` buffer, no col2im, no weight transpose).  Stride 1: the flipped-filter
+    convolution of ``dy``.  Stride 2: one launch over the four parity classes of :func:`conv_s2_dgrad_taps`.
+    ``out``: contiguous bf16 ``[N, H, W, Cin]`` to write (every element is written).  Returns ``None`` when the shape
+    is not supported (channels not multiples of 64, other strides)."""
     n, h, w, c = in_shape
     cout = dy.shape[-1]
     if c % 64 or cout % 64 or w2d.shape[1] != kh * kw * c or not dy.is_contiguous() or not w2d.is_contiguous():
         return None
-    M, K = n * h * w, kh * kw * cout
-    bn = pick_bn(M, c)
-    dx = torch.empty((n, h, w, c), dtype=BF16, device=dy.device)
-    ok = load().conv_igemm_dgrad(dy, w2d, dx, kh, kw, pad, pick_cluster_k(M, c, K, bn), bn)
+    if stride == 1:
+        M, K = n * h * w, kh * kw * cout
+        bn = pick_bn(M, c)
+        dx = out if out is not None else torch.empty((n, h, w, c), dtype=BF16, device=dy.device)
+        ok = load().conv_igemm_dgrad(dy, w2d, dx, kh, kw, pad, pick_cluster_k(M, c, K, bn), bn)
+        return dx if ok else None
+    if stride != 2:
+        return None
+    ho, wo = dy.shape[1], dy.shape[2]
+    classes = conv_s2_dgrad_taps(kh, kw, pad, ho, wo)
+    if classes is None:
+        return None
+    bn = pick_bn(4 * n * ho * wo, c)       # rows of all four classes
+    words = [[t | dp << 16 | dq << 24 for t, dp, dq in taps] + [0] * (S2_MAX_TAPS - len(taps)) for taps in classes]
+    dx = out if out is not None else torch.empty((n, h, w, c), dtype=BF16, device=dy.device)
+    ok = load().conv_igemm_dgrad_s2(dy, w2d, dx, kh, kw, [len(t) for t in classes], [x for ws in words for x in ws], bn)
     return dx if ok else None
 
 

@@ -339,7 +339,8 @@ class Linear(nn.Module):
 
 # ================================================================================ Conv2d (NHWC, implicit GEMM)
 # implicit-GEMM convolution (TMA im2col operands) wherever the shape allows it; explicit im2col / col2im + GEMM for
-# the shapes it declines (the C = 3 stem, Cin % 64 != 0, stride-2 dgrads, a kernel that reports "unsupported")
+# the shapes it declines (the C = 3 stem, Cin % 64 != 0, strides other than 1 and 2, stride-2 filters whose parity
+# classes need negative dy offsets or more than four taps, a kernel that reports "unsupported")
 class _ConvFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, w_bf16, kh, kw, stride, pad, anchor, stats=None, gate=None):
@@ -420,9 +421,10 @@ class _ConvFn(torch.autograd.Function):
         tok = WGRAD.mark(dy2)      # the weight-gradient branch depends on what is enqueued so far, not on the dgrad below
         dx = None
         if ctx.needs_dx:
-            if stride == 1 and kh == kw and kh > 1 and kp == k_true and w_bf16.shape[1] == k_true:
-                # implicit dgrad: flipped-filter convolution of dy, no dcol buffer / col2im
-                dx = F.conv_igemm_dgrad(dy2.view(n, ho, wo, cout), w_bf16, (n, h, w, c), kh, kw, pad)
+            if kp == k_true and w_bf16.shape[1] == k_true and (stride == 2 or (stride == 1 and kh == kw and kh > 1)):
+                # implicit dgrad, no dcol buffer / col2im: stride 1 = flipped-filter convolution of dy, stride 2 = its
+                # four parity classes of dx pixels in one launch
+                dx = F.conv_igemm_dgrad(dy2.view(n, ho, wo, cout), w_bf16, (n, h, w, c), kh, kw, pad, stride=stride)
             if dx is None:
                 dcol = F.gemm(dy2, w_bf16, b_mn=True)  # [M, kp]
                 if kh == 1 and kw == 1 and stride == 1 and pad == 0 and c % 8 == 0:
