@@ -11,21 +11,53 @@ bootstrap the symmetric-memory rendezvous.
 """
 from __future__ import annotations
 
-from typing import Callable, Tuple
+from typing import Callable, Optional, Tuple
 
 import torch
+from aiohttp import web
 
 from ..parallel.arena import ParamArena
 from ..parallel.fedavg import FedAvgSession, NcclSession
 from ..train import GraphedLocalSGD
+from ..utils.aio import run_blocking
 from .worker import ExperimentWorker
 
 
-class GpuExperimentWorker(ExperimentWorker):
+class EvaluatingSeat:
+    """``POST /{name}/evaluate`` of a seat that holds the global model: evaluates it on the seat's held-out shard
+    (``eval_shard_fn() -> (X, y)``) with ``self.trainer.evaluate`` on the training thread, off the event loop, and
+    answers JSON ``{n_samples, loss_sum, correct}``.  501 when the seat has no held-out data."""
+
+    eval_shard_fn: Optional[Callable[[], Tuple[torch.Tensor, torch.Tensor]]] = None
+    eval_batch_size = 512
+
+    def register_handlers(self) -> None:
+        super().register_handlers()
+        self.app.router.add_post("/{}/evaluate".format(self.name), self.evaluate)
+
+    async def evaluate(self, request: web.Request) -> web.Response:
+        if not self._credentials_ok(request):
+            return web.json_response({"err": "Wrong Client"}, status=404)
+        if self.eval_shard_fn is None:
+            return web.json_response({"err": "No Evaluation Data"}, status=501)
+        loss_sum, correct, n = await run_blocking(self._evaluate_blocking, executor=self._executor)
+        return web.json_response({"n_samples": n, "loss_sum": loss_sum, "correct": correct})
+
+    def _evaluate_blocking(self):
+        X, y = self.eval_shard_fn()
+        return self.trainer.evaluate(X, y, batch_size=self.eval_batch_size)
+
+
+class GpuExperimentWorker(EvaluatingSeat, ExperimentWorker):
     def __init__(self, app, model, manager: str, *, device, shard_fn: Callable[[], Tuple[torch.Tensor, torch.Tensor]],
                  backend: str = "fused", group=None, loss: str = "ce", wire_dtype: str = "bf16",
-                 momentum: float = 0.0, use_graph: bool = True, n_ctas: int = 64, **kwargs):
+                 momentum: float = 0.0, use_graph: bool = True, n_ctas: int = 64,
+                 eval_shard_fn: Optional[Callable[[], Tuple[torch.Tensor, torch.Tensor]]] = None,
+                 eval_batch_size: int = 512, **kwargs):
+        """``eval_shard_fn`` (optional): ``() -> (X, y)``, this seat's held-out shard for ``POST /{name}/evaluate``."""
         self.device = torch.device(device)
+        self.eval_shard_fn, self.eval_batch_size = eval_shard_fn, eval_batch_size
+        self._eval_stage = None
         torch.cuda.set_device(self.device)          # the constructing thread (usually the event-loop thread)
         self.arena = ParamArena(model, self.device, momentum=momentum > 0)
         if hasattr(model, "build_workspace"):
@@ -54,3 +86,16 @@ class GpuExperimentWorker(ExperimentWorker):
             self._stage[1].copy_(y, non_blocking=True)
             X, y = self._stage
         return (X, y), int(X.shape[0])
+
+    def _evaluate_blocking(self):
+        """Held-out shards from the host are copied into their own persistent buffers (the captured evaluation
+        graph keeps their addresses; the training buffers are left alone)."""
+        X, y = self.eval_shard_fn()
+        if not X.is_cuda:
+            if self._eval_stage is None or self._eval_stage[0].shape != X.shape:
+                self._eval_stage = (torch.empty(X.shape, dtype=X.dtype, device=self.device),
+                                    torch.empty(y.shape, dtype=y.dtype, device=self.device))
+            self._eval_stage[0].copy_(X, non_blocking=True)
+            self._eval_stage[1].copy_(y, non_blocking=True)
+            X, y = self._eval_stage
+        return self.trainer.evaluate(X, y, batch_size=self.eval_batch_size)

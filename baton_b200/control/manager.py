@@ -20,8 +20,9 @@ the round).
 
 New capabilities: client sampling (``sample_k`` / ``sample_fraction`` /
 ``?sample_k=``), pluggable data planes (``http`` | ``fused`` | ``nccl``),
-checkpoint at ``end_round`` + resume, structured metrics (``/metrics``), and
-``/state``.
+checkpoint at ``end_round`` + resume, structured metrics (``/metrics``),
+``/state``, and ``GET /{name}/evaluate`` (held-out loss and accuracy of the global
+model, computed on the GPU seats of a seated data plane).
 """
 from __future__ import annotations
 
@@ -120,6 +121,7 @@ class Experiment:
         r.add_get("/{}/state".format(self.name), self.get_state)
         r.add_get("/{}/metrics".format(self.name), self.get_metrics)
         r.add_get("/{}/state_dict".format(self.name), self.get_state_dict)
+        r.add_get("/{}/evaluate".format(self.name), self.trigger_evaluate)
 
     async def _on_cleanup(self, app) -> None:
         self._cancel_timeout()
@@ -141,6 +143,52 @@ class Experiment:
         body = wire.dumps({"state_dict": ckpt._cpu_state_dict(self.model),
                            "n_updates": self.update_manager.n_updates})
         return web.Response(body=body, content_type="application/octet-stream")
+
+    # -- evaluation ----------------------------------------------------------
+    async def trigger_evaluate(self, request: web.Request) -> web.Response:
+        """Sample-weighted held-out loss and accuracy of the global model over the live seats that hold it.  Each seat
+        evaluates its own held-out shard on its GPU (``POST /{name}/evaluate``); seats without held-out data answer
+        501 and are left out.  423 while a round is open -- also when one opened or closed while the seats were
+        evaluating, since they may then have evaluated different models (nothing is recorded) -- and 501 on the
+        ``http`` plane (no seat holds the model)."""
+        if self.plane.carries_tensors:
+            return web.json_response({"err": "Evaluation needs a GPU-seated data plane"}, status=501)
+        if self.update_manager.in_progress:
+            return web.json_response({"err": "Update in progress"}, status=423)
+        cm = self.client_manager
+        n_updates = self.update_manager.n_updates
+        seats = [cid for cid, rec in cm.clients.items() if rec.get("rank") is not None and rec.get("model_synced")]
+        replies = await asyncio.gather(*(self._evaluate_seat(cid) for cid in seats))
+        if self.update_manager.in_progress or self.update_manager.n_updates != n_updates:
+            return web.json_response({"err": "Update in progress"}, status=423)
+        got = [r for r in replies if r is not None]
+        n = sum(r["n_samples"] for r in got)
+        rec = self.metrics.add_eval(
+            n_updates=self.update_manager.n_updates, n_seats=len(got), n_samples=n,
+            loss=sum(r["loss_sum"] for r in got) / n if n else None,
+            accuracy=sum(r["correct"] for r in got) / n if n else None)
+        return web.json_response(json_clean(rec))
+
+    async def _evaluate_seat(self, client_id: str) -> Optional[dict]:
+        rec = self.client_manager.clients.get(client_id)
+        if rec is None:
+            return None
+        url = "{}evaluate?client_id={}&key={}".format(rec["url"], client_id, rec["key"])
+        try:
+            async with self.client_manager._get_session().post(url) as resp:
+                if resp.status != 200:
+                    return None
+                body = await resp.json()
+        except Exception as exc:
+            log.warning("evaluation on %s failed: %r", client_id, exc)
+            return None
+        try:
+            out = {k: float(body[k]) for k in ("n_samples", "loss_sum", "correct")}
+        except (KeyError, TypeError, ValueError):
+            return None
+        if any(v != v or v in (float("inf"), float("-inf")) for v in out.values()) or out["n_samples"] < 0:
+            return None
+        return out
 
     # -- round start -------------------------------------------------------
     async def trigger_start_round(self, request: web.Request) -> web.Response:

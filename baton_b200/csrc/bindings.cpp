@@ -38,6 +38,29 @@ inline std::optional<B200SgdEpilogue> sgd_epilogue(const std::optional<at::Tenso
                          hyper->data_ptr<float>(), nesterov ? 1 : 0};
 }
 
+// eval-mode BatchNorm epilogue of a forward GEMM: fp32 [N] scale and shift, optional bf16 residual rows
+inline std::optional<B200AffineEpilogue> affine_epilogue(const std::optional<at::Tensor>& scale,
+                                                         const std::optional<at::Tensor>& shift,
+                                                         const std::optional<at::Tensor>& residual, bool relu,
+                                                         int64_t rows, int64_t N) {
+  if (!scale.has_value() || !scale->defined()) return std::nullopt;
+  TORCH_CHECK(shift.has_value() && shift->defined(), "affine epilogue: scale without shift");
+  CHECK_CUDA(*scale); CHECK_CUDA(*shift);
+  TORCH_CHECK(scale->scalar_type() == at::kFloat && shift->scalar_type() == at::kFloat &&
+                  scale->is_contiguous() && shift->is_contiguous() && scale->numel() >= N && shift->numel() >= N,
+              "affine epilogue: fp32 [N] scale / shift");
+  long long ldr = 0;
+  if (residual.has_value() && residual->defined()) {
+    CHECK_CUDA(*residual);
+    TORCH_CHECK(residual->scalar_type() == at::kBFloat16 && residual->stride(-1) == 1 && residual->size(-1) == N &&
+                    residual->numel() >= rows * N,
+                "affine epilogue: bf16 [rows, N] residual with unit inner stride");
+    ldr = residual->dim() >= 2 ? residual->stride(-2) : N;
+  }
+  return B200AffineEpilogue{scale->data_ptr<float>(), shift->data_ptr<float>(), opt_ptr<const void>(residual), ldr,
+                            relu ? 1 : 0};
+}
+
 // ---- in-graph kernel timeline (pdl.cuh): every translation unit owns a copy of the trace pointer
 extern "C" {
 #define B200_TRACE_TUS(X) X(gemm_wgmma) X(gemm_fp8) X(quant) X(attention) X(im2col_tma) X(gemm_simt) X(fedavg) \
@@ -62,14 +85,16 @@ bool trace_set(const std::optional<at::Tensor>& buf) {
   return rc == 0;
 }
 
-// false: the optimizer epilogue was requested and declined (nothing was written)
+// false: the optimizer or BatchNorm epilogue was requested and declined (nothing was written)
 bool gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor d, const std::optional<at::Tensor>& bias, int64_t M,
           int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldd, bool a_mn, bool b_mn, int64_t act,
           int64_t split_k, bool accumulate, double alpha, const std::optional<at::Tensor>& flags, int64_t flag_epoch,
           int64_t flag_elem_off, int64_t flag_tile_elems, int64_t flag_bias_off, int64_t force_bn, bool simt,
           const std::optional<at::Tensor>& col_stats, const std::optional<at::Tensor>& flag_epoch_word,
           const std::optional<at::Tensor>& sgd_theta, const std::optional<at::Tensor>& sgd_theta_bf16,
-          const std::optional<at::Tensor>& sgd_mom, const std::optional<at::Tensor>& sgd_hyper, bool sgd_nesterov) {
+          const std::optional<at::Tensor>& sgd_mom, const std::optional<at::Tensor>& sgd_hyper, bool sgd_nesterov,
+          const std::optional<at::Tensor>& bn_scale, const std::optional<at::Tensor>& bn_shift,
+          const std::optional<at::Tensor>& residual, bool bn_relu) {
   CHECK_CUDA(a); CHECK_CUDA(b); CHECK_CUDA(d);
   TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16, "gemm operands must be bf16");
   TORCH_CHECK(d.scalar_type() == at::kBFloat16 || d.scalar_type() == at::kFloat, "gemm output must be bf16/fp32");
@@ -80,18 +105,21 @@ bool gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor d, const std::opt
               "col_stats needs the tensor-core path and a [2N] fp32 buffer");
   if (simt) {
     TORCH_CHECK(!sgd_hyper.has_value(), "the SIMT GEMM has no optimizer epilogue");
+    TORCH_CHECK(!bn_scale.has_value(), "the SIMT GEMM has no BatchNorm epilogue");
     check(b200_gemm_simt(cptr(a), cptr(b), ptr(d), bp, M, N, K, lda, ldb, ldd, a_mn, b_mn, out_fp32, act, accumulate,
                          static_cast<float>(alpha), cur_stream()),
           "gemm_simt");
     return true;
   }
   const std::optional<B200SgdEpilogue> sgd = sgd_epilogue(sgd_theta, sgd_theta_bf16, sgd_mom, sgd_hyper, sgd_nesterov);
+  const std::optional<B200AffineEpilogue> affine = affine_epilogue(bn_scale, bn_shift, residual, bn_relu, M, N);
   const int rc = b200_gemm_bf16(cptr(a), cptr(b), ptr(d), bp, M, N, K, lda, ldb, ldd, a_mn, b_mn, out_fp32, act, split_k,
                                 accumulate, static_cast<float>(alpha), opt_ptr<const uint32_t>(flags),
                                 static_cast<uint32_t>(flag_epoch), flag_elem_off, static_cast<int>(flag_tile_elems),
                                 flag_bias_off, static_cast<int>(force_bn), opt_ptr<float>(col_stats),
-                                opt_ptr<const uint32_t>(flag_epoch_word), sgd ? &*sgd : nullptr, cur_stream());
-  if (rc == B200_SGD_EPILOGUE_DECLINED) return false;
+                                opt_ptr<const uint32_t>(flag_epoch_word), sgd ? &*sgd : nullptr,
+                                affine ? &*affine : nullptr, cur_stream());
+  if (rc == B200_SGD_EPILOGUE_DECLINED || rc == B200_AFFINE_EPILOGUE_DECLINED) return false;
   check(rc, "gemm_bf16");
   return true;
 }
@@ -156,18 +184,22 @@ bool attention_bwd(const at::Tensor& qkv, const at::Tensor& dout, const at::Tens
 // implicit-GEMM convolution; false = shape not supported (caller falls back to im2col + GEMM)
 bool conv_igemm_fwd(const at::Tensor& x, const at::Tensor& w, at::Tensor y, int64_t kh, int64_t kw, int64_t stride,
                     int64_t pad, int64_t ho, int64_t wo, int64_t cluster_k, int64_t force_bn,
-                    const std::optional<at::Tensor>& col_stats) {
+                    const std::optional<at::Tensor>& col_stats, const std::optional<at::Tensor>& bn_scale,
+                    const std::optional<at::Tensor>& bn_shift, const std::optional<at::Tensor>& residual, bool bn_relu) {
   CHECK_CUDA(x); CHECK_CUDA(w); CHECK_CUDA(y);
   TORCH_CHECK(x.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16 && y.scalar_type() == at::kBFloat16 &&
               x.dim() == 4 && x.is_contiguous() && w.is_contiguous() && y.is_contiguous());
+  TORCH_CHECK(y.numel() == x.size(0) * ho * wo * w.size(0), "conv_igemm_fwd: y must hold [N*Ho*Wo, Cout] elements");
   const c10::cuda::CUDAGuard guard(x.device());
+  const std::optional<B200AffineEpilogue> affine =
+      affine_epilogue(bn_scale, bn_shift, residual, bn_relu, x.size(0) * ho * wo, w.size(0));
   const int rc = b200_conv_igemm_fwd(cptr(x), cptr(w), ptr(y), static_cast<int>(x.size(0)), static_cast<int>(x.size(1)),
                                      static_cast<int>(x.size(2)), static_cast<int>(x.size(3)), static_cast<int>(w.size(0)),
                                      static_cast<int>(kh), static_cast<int>(kw), static_cast<int>(stride),
                                      static_cast<int>(pad), static_cast<int>(ho), static_cast<int>(wo),
                                      static_cast<int>(cluster_k), static_cast<int>(force_bn), opt_ptr<float>(col_stats),
-                                     cur_stream());
-  if (rc == -2) return false;
+                                     affine ? &*affine : nullptr, cur_stream());
+  if (rc == -2 || rc == B200_AFFINE_EPILOGUE_DECLINED) return false;
   check(rc, "conv_igemm_fwd");
   return true;
 }
@@ -596,6 +628,17 @@ bool bn_bwd_cluster(const at::Tensor& x, const at::Tensor& y, const at::Tensor& 
   check(rc, "bn_bwd_cluster");
   return true;
 }
+// eval-mode BatchNorm folding of every BatchNorm in `table` (int64 [n_bn, 7], see launch.h) into `out`
+void bn_fold_eval(const at::Tensor& arena, const at::Tensor& table, at::Tensor out) {
+  CHECK_CUDA(arena); CHECK_CUDA(table); CHECK_CUDA(out);
+  TORCH_CHECK(arena.scalar_type() == at::kFloat && out.scalar_type() == at::kFloat && table.scalar_type() == at::kLong &&
+                  table.dim() == 2 && table.size(1) == 7 && table.is_contiguous() && out.is_contiguous(),
+              "bn_fold_eval: fp32 arena / out, int64 [n, 7] table");
+  const c10::cuda::CUDAGuard guard(arena.device());
+  check(b200_bn_fold_eval(arena.data_ptr<float>(), reinterpret_cast<const long long*>(table.data_ptr<int64_t>()),
+                          static_cast<int>(table.size(0)), out.data_ptr<float>(), cur_stream()),
+        "bn_fold_eval");
+}
 void layernorm_fwd(const at::Tensor& x, const std::optional<at::Tensor>& res, at::Tensor y, const at::Tensor& gamma,
                    const at::Tensor& beta, at::Tensor mean, at::Tensor rstd, int64_t rows, int64_t C, double eps) {
   CHECK_CUDA(x);
@@ -657,6 +700,26 @@ bool linear_xent_head(const at::Tensor& x, const at::Tensor& w, const std::optio
                                        static_cast<int>(w.size(0)), static_cast<float>(grad_scale), cur_stream());
   if (rc == -2) return false;
   check(rc, "linear_xent_head");
+  return true;
+}
+// forward-only classifier head (evaluation); false: shape not supported
+bool linear_xent_eval(const at::Tensor& x, const at::Tensor& w, const std::optional<at::Tensor>& bias, const at::Tensor& target,
+                      at::Tensor loss_acc, const std::optional<at::Tensor>& logits_out) {
+  CHECK_CUDA(x);
+  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16 && x.dim() == 2 && w.dim() == 2 &&
+              x.is_contiguous() && w.is_contiguous() && x.size(1) == w.size(1));
+  TORCH_CHECK(target.scalar_type() == at::kLong && target.numel() >= x.size(0) && loss_acc.scalar_type() == at::kFloat &&
+              loss_acc.numel() >= 2);
+  TORCH_CHECK(!bias.has_value() || (bias->scalar_type() == at::kFloat && bias->numel() == w.size(0)));
+  TORCH_CHECK(!logits_out.has_value() || (logits_out->scalar_type() == at::kFloat && logits_out->is_contiguous() &&
+                                          logits_out->numel() == x.size(0) * w.size(0)));
+  const c10::cuda::CUDAGuard guard(x.device());
+  const int rc = b200_linear_xent_eval(x.data_ptr(), w.data_ptr(), opt_ptr<const float>(bias),
+                                       reinterpret_cast<const long long*>(target.data_ptr<int64_t>()),
+                                       loss_acc.data_ptr<float>(), opt_ptr<float>(logits_out), static_cast<int>(x.size(0)),
+                                       static_cast<int>(x.size(1)), static_cast<int>(w.size(0)), cur_stream());
+  if (rc == -2) return false;
+  check(rc, "linear_xent_eval");
   return true;
 }
 void mse(const at::Tensor& pred, const at::Tensor& target, const std::optional<at::Tensor>& dpred, at::Tensor loss_acc,
@@ -725,4 +788,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("softmax_xent", &softmax_xent);
   m.def("mse", &mse);
   m.def("linear_xent_head", &linear_xent_head);
+  m.def("linear_xent_eval", &linear_xent_eval);
+  m.def("bn_fold_eval", &bn_fold_eval);
 }

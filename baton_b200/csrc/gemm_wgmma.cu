@@ -87,6 +87,12 @@ struct GemmParams {
   int conv_h = 0, conv_w = 0;  // dx image size
   int s2_ntaps[4] = {0, 0, 0, 0};
   int s2_tap[4][S2_MAX_TAPS] = {};
+  // eval-mode BatchNorm epilogue (the AFFINE instantiations): D = act(acc * bn_scale[c] + bn_shift[c] + residual[r, c]),
+  // bf16 out; act is 0 or 1 (ReLU)
+  const float* bn_scale = nullptr;
+  const float* bn_shift = nullptr;
+  const __nv_bfloat16* residual = nullptr;   // optional, [M, ldr]
+  long long ldr = 0;
 };
 
 // Wait until every arrival flag covering arena elements [e0, e1] has reached `need` (published by the FedAvg kernel with
@@ -238,10 +244,51 @@ __device__ __forceinline__ void transform_chunk(const GemmParams& p, int col0, f
   }
 }
 
+// Eval-mode BatchNorm of one row chunk (columns [col0, col0 + NV) of `row` < M): bn_apply's eval arithmetic,
+// fmaf(z, scale, shift) + residual, then ReLU, on the fp32 accumulator instead of a bf16-rounded z.  The host
+// guarantees N % 8 == 0, 16-byte aligned scale / shift / residual rows and ldr % 8 == 0, so every group of 8 columns
+// is either wholly inside N or wholly past it and loads as vectors.
 template <int NV>
+__device__ __forceinline__ void affine_chunk(const GemmParams& p, int row, int col0, float (&v)[NV]) {
+  static_assert(NV % 8 == 0, "affine epilogue works on groups of 8 columns");
+  const bool relu = p.act == 1;
+  const __nv_bfloat16* res = p.residual != nullptr ? p.residual + static_cast<size_t>(row) * p.ldr + col0 : nullptr;
+#pragma unroll
+  for (int j = 0; j < NV; j += 8) {
+    if (col0 + j >= p.N) break;
+    // every lane of a warp reads the same scale / shift addresses: one broadcast request each
+    const float4 s0 = __ldg(reinterpret_cast<const float4*>(p.bn_scale + col0 + j));
+    const float4 s1 = __ldg(reinterpret_cast<const float4*>(p.bn_scale + col0 + j + 4));
+    const float4 h0 = __ldg(reinterpret_cast<const float4*>(p.bn_shift + col0 + j));
+    const float4 h1 = __ldg(reinterpret_cast<const float4*>(p.bn_shift + col0 + j + 4));
+    const float sc[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+    const float sh[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
+    float r[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (res != nullptr) {
+      const uint4 rv = *reinterpret_cast<const uint4*>(res + j);
+      const uint32_t rw[4] = {rv.x, rv.y, rv.z, rv.w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float2 f = unpack_bf16x2(rw[i]);
+        r[2 * i] = f.x;
+        r[2 * i + 1] = f.y;
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float x = fmaf(v[j + i], sc[i], sh[i]) + r[i];
+      v[j + i] = relu ? fmaxf(x, 0.f) : x;
+    }
+  }
+}
+
+template <int NV, bool AFFINE = false>
 __device__ __forceinline__ void store_row_chunk(const GemmParams& p, int row, int col0, float (&v)[NV], bool vec_ok,
                                                 size_t d_off = 0) {
-  transform_chunk<NV>(p, col0, v);
+  if constexpr (AFFINE)
+    affine_chunk<NV>(p, row, col0, v);
+  else
+    transform_chunk<NV>(p, col0, v);
   const bool full = (col0 + NV <= p.N);
   if (p.out_fp32) {
     float* d = reinterpret_cast<float*>(p.D) + d_off + static_cast<size_t>(row) * p.ldd + col0;
@@ -410,7 +457,8 @@ __device__ __forceinline__ void s2_load_ktile(const CUtensorMap* tmA, const CUte
 // no col2im); 4 = implicit dgrad of a stride-2 convolution, one parity class of dx pixels per group of M tiles (see
 // s2_class).  See csrc/im2col_tma.cu for the tensor maps.
 // SGD: optimizer epilogue instantiation (weight gradients only) -- every other GEMM keeps the plain epilogue.
-template <int BN, int STAGES, int CONV = 0, bool SGD = false>
+// AFFINE: eval-mode BatchNorm epilogue instantiation (affine_chunk, forward convolutions in evaluation).
+template <int BN, int STAGES, int CONV = 0, bool SGD = false, bool AFFINE = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                          const GemmParams p) {
@@ -587,9 +635,14 @@ gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
         if (want_stats) { sstat[c + lane_id()] = 0.f; sstat[BN + c + lane_id()] = 0.f; }
         continue;
       }
-      transform_chunk<32>(p, col0, v);
-      if (want_stats) stage_col_stats(sstat, BN, c, v);
-      if (!row_ok) continue;
+      if constexpr (AFFINE) {
+        if (!row_ok) continue;
+        affine_chunk<32>(p, row, col0, v);
+      } else {
+        transform_chunk<32>(p, col0, v);
+        if (want_stats) stage_col_stats(sstat, BN, c, v);
+        if (!row_ok) continue;
+      }
       const bool full = (col0 + 32 <= p.N);
       if constexpr (SGD) {
         sgd_epilogue_chunk(p, static_cast<size_t>(row) * p.ldd + col0, col0, v, sgd_vec);
@@ -830,7 +883,8 @@ gemm_bf16_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
 
 
 // ---- runtime-depth pipeline + cluster split-K (DSMEM reduce) ----
-template <int BN, bool CLUSTER, int CONV = 0>
+// AFFINE: eval-mode BatchNorm epilogue (affine_chunk), applied by the CTA that stores the reduced rows
+template <int BN, bool CLUSTER, int CONV = 0, bool AFFINE = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                         const GemmParams p) {
@@ -950,7 +1004,7 @@ gemm_bf16_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
         float v[32];
 #pragma unroll
         for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-        store_row_chunk<32>(p, row, col0, v, vec_ok);
+        store_row_chunk<32, AFFINE>(p, row, col0, v, vec_ok);
       }
     }
   }
@@ -988,7 +1042,7 @@ gemm_bf16_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
             cq[j] = fmaf(rnd, rnd, cq[j]);
           }
         }
-        if (row < p.M && col0 < p.N) store_row_chunk<8>(p, row, col0, v, vec_ok);
+        if (row < p.M && col0 < p.N) store_row_chunk<8, AFFINE>(p, row, col0, v, vec_ok);
       }
       if (want_stats) {
         // threads t, t + CG, t + 2 CG ... own the same 8 columns: fold the lanes of a warp with shuffles, park one
@@ -1093,18 +1147,32 @@ static void set_sgd_epilogue(GemmParams& p, const B200SgdEpilogue& s) {
   p.sgd_mom = s.mom; p.sgd_nesterov = s.nesterov;
 }
 
-template <int BN, int STAGES, int CONV = 0, bool SGD = false>
+static void set_affine_epilogue(GemmParams& p, const B200AffineEpilogue& a) {
+  p.bn_scale = a.scale; p.bn_shift = a.shift; p.residual = reinterpret_cast<const __nv_bfloat16*>(a.residual);
+  p.ldr = a.ldr; p.act = a.relu ? 1 : 0;
+}
+
+// what the affine epilogue needs of its output and operands (see affine_chunk)
+static bool affine_ok(const B200AffineEpilogue& a, int N) {
+  return a.scale != nullptr && a.shift != nullptr && N % 8 == 0 &&
+         ((reinterpret_cast<uintptr_t>(a.scale) | reinterpret_cast<uintptr_t>(a.shift) |
+           reinterpret_cast<uintptr_t>(a.residual)) & 15) == 0 &&
+         (a.residual == nullptr || (a.ldr % 8 == 0 && a.ldr >= N));
+}
+
+template <int BN, int STAGES, int CONV = 0, bool SGD = false, bool AFFINE = false>
 static int launch_fixed(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, dim3 grid,
                       cudaStream_t stream) {
   constexpr int smem = STAGES * SmemLayout<BN>::STAGE_BYTES + 2 * STAGES * 8 + 8 * BN * 4 + 1024;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD>,
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD, AFFINE>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return static_cast<int>(e);
     configured = true;
   }
-  cudaError_t le = launch_pdl(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD>, grid, GEMM_THREADS, smem, stream, ta, tb, p);
+  cudaError_t le = launch_pdl(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD, AFFINE>, grid, GEMM_THREADS, smem, stream,
+                              ta, tb, p);
   if (le != cudaSuccess) return static_cast<int>(le);
   return static_cast<int>(cudaGetLastError());
 }
@@ -1128,7 +1196,7 @@ static int launch_persistent(const CUtensorMap& ta, const CUtensorMap& tb, const
   return static_cast<int>(cudaGetLastError());
 }
 
-template <int BN, int CONV = 0>
+template <int BN, int CONV = 0, bool AFFINE = false>
 static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, dim3 grid,
                       cudaStream_t stream) {
   using L = SmemLayout<BN>;
@@ -1137,10 +1205,11 @@ static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const GemmPa
   static bool configured = false;
   if (!configured) {
     const int cap = max_smem > L::PART_BYTES + 4096 ? max_smem : L::PART_BYTES + 4096;
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_splitk_kernel<BN, false, CONV>,
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_splitk_kernel<BN, false, CONV, AFFINE>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
     if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(gemm_bf16_splitk_kernel<BN, true, CONV>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
+      e = cudaFuncSetAttribute(gemm_bf16_splitk_kernel<BN, true, CONV, AFFINE>,
+                               cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
     if (e != cudaSuccess) return static_cast<int>(e);
     configured = true;
   }
@@ -1174,8 +1243,8 @@ static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const GemmPa
   }
   cfg.attrs = attr;
   cfg.numAttrs = na;
-  cudaError_t le = p.cluster_k > 1 ? cudaLaunchKernelEx(&cfg, gemm_bf16_splitk_kernel<BN, true, CONV>, ta, tb, p)
-                                   : cudaLaunchKernelEx(&cfg, gemm_bf16_splitk_kernel<BN, false, CONV>, ta, tb, p);
+  cudaError_t le = p.cluster_k > 1 ? cudaLaunchKernelEx(&cfg, gemm_bf16_splitk_kernel<BN, true, CONV, AFFINE>, ta, tb, p)
+                                   : cudaLaunchKernelEx(&cfg, gemm_bf16_splitk_kernel<BN, false, CONV, AFFINE>, ta, tb, p);
   if (le != cudaSuccess) return static_cast<int>(le);
   return static_cast<int>(cudaGetLastError());
 }
@@ -1205,13 +1274,17 @@ extern "C" int b200_gemm_bf16(const void* a, const void* b, void* d, const float
                               int split_k, int accumulate, float alpha, const uint32_t* tile_flags,
                               uint32_t flag_epoch, long long flag_elem_off, int flag_tile_elems,
                               long long flag_bias_off, int force_bn, float* col_stats, const uint32_t* flag_epoch_ptr,
-                              const B200SgdEpilogue* sgd, cudaStream_t stream) {
+                              const B200SgdEpilogue* sgd, const B200AffineEpilogue* affine, cudaStream_t stream) {
   using namespace b200;
   if (M <= 0 || N <= 0 || K <= 0) return 0;
   // optimizer epilogue: only a weight gradient (MN-major operands, plain fp32 accumulation) qualifies
   if (sgd != nullptr && (!accumulate || !out_fp32 || !a_mn || !b_mn || bias != nullptr || act != 0 || alpha != 1.0f ||
                          col_stats != nullptr || tile_flags != nullptr))
     return B200_SGD_EPILOGUE_DECLINED;
+  // eval-mode BatchNorm epilogue: a plain bf16 forward GEMM, one K pass per CTA or a cluster split-K
+  if (affine != nullptr && (sgd != nullptr || accumulate || out_fp32 || bias != nullptr || act != 0 || alpha != 1.0f ||
+                            col_stats != nullptr || tile_flags != nullptr || split_k > 1 || !affine_ok(*affine, N)))
+    return B200_AFFINE_EPILOGUE_DECLINED;
   // fused BatchNorm statistics: plain single-pass GEMM only (no split-K partials, no bias / activation / scaling)
   if (col_stats != nullptr && (split_k > 1 || bias != nullptr || act != 0 || alpha != 1.0f || accumulate)) return -3;
   if ((lda % 8) || (ldb % 8) || (reinterpret_cast<uintptr_t>(a) & 15) || (reinterpret_cast<uintptr_t>(b) & 15))
@@ -1260,11 +1333,24 @@ extern "C" int b200_gemm_bf16(const void* a, const void* b, void* d, const float
   dim3 grid((N + bn - 1) / bn, (M + BM - 1) / BM, split_k);
   // large plain GEMMs (>= one wave of tiles, single K pass): persistent kernel with overlapped epilogue
   const int num_tiles = static_cast<int>(grid.x * grid.y);
-  const bool persistent = split_k == 1 && tile_flags == nullptr && num_tiles >= device_sm_count() && bn == 128;
+  // the affine epilogue runs on the fixed-depth kernel where the persistent one would be picked
+  const bool persistent = split_k == 1 && tile_flags == nullptr && num_tiles >= device_sm_count() && bn == 128 &&
+                          affine == nullptr;
   if (sgd != nullptr) {
     // the optimizer epilogue lives in the fixed-depth kernel and needs each tile's complete gradient in one CTA
     if (split_k != 1 || cluster_k != 1 || persistent) return B200_SGD_EPILOGUE_DECLINED;
     set_sgd_epilogue(p, *sgd);
+  }
+  const bool shallow = per <= 4 && !p.batched;
+  if (affine != nullptr) {
+    set_affine_epilogue(p, *affine);
+    if (cluster_k > 1)
+      return bn == 128 ? launch_cfg<128, 0, true>(ta, tb, p, grid, stream) : launch_cfg<64, 0, true>(ta, tb, p, grid, stream);
+    if (bn == 128)
+      return shallow ? launch_fixed<128, 3, 0, false, true>(ta, tb, p, grid, stream)
+                     : launch_fixed<128, 6, 0, false, true>(ta, tb, p, grid, stream);
+    return shallow ? launch_fixed<64, 4, 0, false, true>(ta, tb, p, grid, stream)
+                   : launch_fixed<64, 8, 0, false, true>(ta, tb, p, grid, stream);
   }
   if (cluster_k > 1) {
     if (bn == 128) return launch_cfg<128>(ta, tb, p, grid, stream);
@@ -1273,7 +1359,6 @@ extern "C" int b200_gemm_bf16(const void* a, const void* b, void* d, const float
   if (persistent) return launch_persistent<128, 3>(ta, tb, p, num_tiles, stream);
   // short K loops (stem convolution: 3 k tiles, 1x1 shortcuts: 1-4) do not need a deep ring: a shallow one asks for
   // little shared memory
-  const bool shallow = per <= 4 && !p.batched;
   if (sgd != nullptr) {
     if (bn == 128)
       return shallow ? launch_fixed<128, 3, 0, true>(ta, tb, p, grid, stream) : launch_fixed<128, 6, 0, true>(ta, tb, p, grid, stream);
@@ -1342,7 +1427,7 @@ extern "C" int b200_encode_map_im2col_bf16(void* map, const void* x, int N, int 
 // forward: y[N*Ho*Wo, Cout] = im2col(x) w^T with x NHWC bf16 (Cin % 64 == 0), w [Cout, KH*KW*Cin] (channels_last)
 extern "C" int b200_conv_igemm_fwd(const void* x, const void* w, void* y, int N, int H, int W, int Cin, int Cout, int KH,
                                    int KW, int stride, int pad, int Ho, int Wo, int cluster_k, int force_bn,
-                                   float* col_stats, cudaStream_t stream) {
+                                   float* col_stats, const B200AffineEpilogue* affine, cudaStream_t stream) {
   using namespace b200;
   const long long M = static_cast<long long>(N) * Ho * Wo;
   const int K = KH * KW * Cin;
@@ -1350,6 +1435,7 @@ extern "C" int b200_conv_igemm_fwd(const void* x, const void* w, void* y, int N,
   if (Cin % 64 != 0 || Cout % 8 != 0 || M > (1ll << 30) || (reinterpret_cast<uintptr_t>(x) & 15) ||
       (reinterpret_cast<uintptr_t>(w) & 15) || (reinterpret_cast<uintptr_t>(y) & 15))
     return -2;
+  if (affine != nullptr && (col_stats != nullptr || !affine_ok(*affine, Cout))) return B200_AFFINE_EPILOGUE_DECLINED;
   const int bn = clamp_bn(force_bn > 0 ? force_bn : (Cout > 64 ? 128 : 64));
   CUtensorMap ta, tb;
   int rc = b200_encode_map_im2col_bf16(&ta, x, N, H, W, Cin, KH, KW, stride, pad, 64, BM);
@@ -1372,11 +1458,21 @@ extern "C" int b200_conv_igemm_fwd(const void* x, const void* w, void* y, int N,
   p.conv_ho = Ho; p.conv_wo = Wo; p.conv_stride = stride; p.conv_pad = pad; p.conv_kw = KW; p.conv_cin = Cin;
   p.conv_taps = KH * KW; p.conv_ncol = Cin;
   dim3 grid((Cout + bn - 1) / bn, static_cast<unsigned>((M + BM - 1) / BM), cluster_k);
+  const bool shallow = per <= 4;
+  if (affine != nullptr) {
+    set_affine_epilogue(p, *affine);
+    if (cluster_k > 1)
+      return bn == 128 ? launch_cfg<128, 1, true>(ta, tb, p, grid, stream) : launch_cfg<64, 1, true>(ta, tb, p, grid, stream);
+    if (bn == 128)
+      return shallow ? launch_fixed<128, 3, 1, false, true>(ta, tb, p, grid, stream)
+                     : launch_fixed<128, 6, 1, false, true>(ta, tb, p, grid, stream);
+    return shallow ? launch_fixed<64, 4, 1, false, true>(ta, tb, p, grid, stream)
+                   : launch_fixed<64, 8, 1, false, true>(ta, tb, p, grid, stream);
+  }
   if (cluster_k > 1) {
     if (bn == 128) return launch_cfg<128, 1>(ta, tb, p, grid, stream);
     return launch_cfg<64, 1>(ta, tb, p, grid, stream);
   }
-  const bool shallow = per <= 4;
   if (bn == 128) return shallow ? launch_fixed<128, 3, 1>(ta, tb, p, grid, stream) : launch_fixed<128, 6, 1>(ta, tb, p, grid, stream);
   return shallow ? launch_fixed<64, 4, 1>(ta, tb, p, grid, stream) : launch_fixed<64, 8, 1>(ta, tb, p, grid, stream);
 }

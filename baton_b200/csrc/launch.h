@@ -22,13 +22,27 @@ struct B200SgdEpilogue {
 };
 #define B200_SGD_EPILOGUE_DECLINED (-6)
 
+// Eval-mode BatchNorm epilogue of a forward convolution GEMM: D = relu?(acc * scale[c] + shift[c] + residual[r, c]) in
+// bf16, with the per-column scale / shift that bn_fold_eval derives from the running statistics.  residual is optional
+// (bf16, row pitch ldr).  Needs N % 8 == 0, 16-byte aligned scale / shift / residual and ldr % 8 == 0.  A launcher that
+// cannot apply it returns B200_AFFINE_EPILOGUE_DECLINED and touches nothing; the caller then runs the GEMM and bn_apply.
+struct B200AffineEpilogue {
+  const float* scale;
+  const float* shift;
+  const void* residual;             // or nullptr
+  long long ldr;
+  int relu;
+};
+#define B200_AFFINE_EPILOGUE_DECLINED (-7)
+
 // ---- gemm_wgmma.cu
 // sgd != nullptr: optimizer epilogue (accumulate, fp32 D, MN-major operands, single K pass on the fixed-depth kernel)
+// affine != nullptr: eval-mode BatchNorm epilogue (bf16 D, act 0, no bias / split-K partials; fixed or cluster kernel)
 int b200_gemm_bf16(const void* a, const void* b, void* d, const float* bias, int M, int N, int K, long long lda,
                    long long ldb, long long ldd, int a_mn, int b_mn, int out_fp32, int act, int split_k, int accumulate,
                    float alpha, const uint32_t* tile_flags, uint32_t flag_epoch, long long flag_elem_off, int flag_tile_elems,
                    long long flag_bias_off, int force_bn, float* col_stats, const uint32_t* flag_epoch_ptr,
-                   const B200SgdEpilogue* sgd, cudaStream_t stream);
+                   const B200SgdEpilogue* sgd, const B200AffineEpilogue* affine, cudaStream_t stream);
 int b200_gemm_bf16_batched(const void* a, const void* b, void* d, int M, int N, int K, long long lda, long long ldb,
                            long long ldd, int a_mn, int b_mn, int out_fp32, int act, float alpha, int n_outer,
                            int n_inner, long long a_outer, long long a_inner, long long b_outer, long long b_inner,
@@ -41,7 +55,7 @@ int b200_attention_bwd(const void* qkv, const void* dout, const void* probs, voi
 // ---- implicit-GEMM convolution (experimental: gemm_wgmma.cu CONV modes fed by TMA im2col maps)
 int b200_conv_igemm_fwd(const void* x, const void* w, void* y, int N, int H, int W, int Cin, int Cout, int KH, int KW,
                         int stride, int pad, int Ho, int Wo, int cluster_k, int force_bn, float* col_stats,
-                        cudaStream_t stream);
+                        const B200AffineEpilogue* affine, cudaStream_t stream);
 int b200_conv_igemm_dgrad(const void* dy, const void* w, void* dx, int N, int H, int W, int Cin, int Cout, int KH, int KW,
                           int pad, int Ho, int Wo, int cluster_k, int force_bn, cudaStream_t stream);
 int b200_conv_igemm_dgrad_s2(const void* dy, const void* w, void* dx, int N, int H, int W, int Cin, int Cout, int KH,
@@ -169,6 +183,9 @@ int b200_bn_maxpool_bwd(const void* z, const void* p, const void* argmax, const 
 int b200_bn_bwd_cluster(const void* x, const void* y, const void* dy_a, const void* dy_b, void* dx, void* dres,
                         const float* gamma, const float* save_mean, const float* save_rstd, float* dgamma, float* dbeta,
                         long long rows, int C, int relu, int max_cluster, cudaStream_t stream);
+// eval-mode BatchNorm folding: one block per BatchNorm; table = int64 [n_bn][7] {gamma, beta, running_mean,
+// running_var (element offsets into arena; gamma / beta -1 = none), output offset, C, eps as float bits}
+int b200_bn_fold_eval(const float* arena, const long long* table, int n_bn, float* out, cudaStream_t stream);
 int b200_layernorm_fwd(const void* x, const void* residual, void* y, const float* gamma, const float* beta,
                        float* mean, float* rstd, long long rows, int C, float eps, cudaStream_t stream);
 int b200_layernorm_bwd(const void* x, const void* dy, void* dx, const float* gamma, const float* mean,
@@ -184,6 +201,9 @@ int b200_softmax_xent(const void* logits, int logits_fp32, const long long* targ
 int b200_linear_xent_head(const void* x, const void* w, const float* bias, const long long* target, void* dx, float* dw,
                           float* db, float* loss_acc, float* logits_out, int rows, int K, int NC, float grad_scale,
                           cudaStream_t stream);
+// forward-only head (evaluation): loss_acc[0] += sum of the row losses, loss_acc[1] += #correct
+int b200_linear_xent_eval(const void* x, const void* w, const float* bias, const long long* target, float* loss_acc,
+                          float* logits_out, int rows, int K, int NC, cudaStream_t stream);
 int b200_mse(const void* pred, int pred_fp32, const float* target, void* dpred, int dp_fp32, float* loss_acc,
              long long n, float grad_scale, cudaStream_t stream);
 }

@@ -124,7 +124,9 @@ mse_kernel(const void* __restrict__ pred, const float* __restrict__ target, void
 //   loss_acc[0] += mean loss, loss_acc[1] += #correct
 // It replaces six launches (GEMM 128x10x512, loss, cast, colsum, two SIMT GEMMs) for ~4 MFLOP of work.  One CTA handles HEAD_ROWS rows: warp w owns row w for the logits, the
 // 256 threads then share the dX / dW tiles.  x: bf16 [rows, K], W: bf16 [NC, K] (the arena's shadow), b: fp32.
+// BACKWARD = false: the evaluation instantiation -- logits, loss and #correct only (no dX / dW / db; grid.y = 1).
 constexpr int HEAD_ROWS = 8;
+template <bool BACKWARD>
 __global__ void __launch_bounds__(256)
 linear_xent_head_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ w, const float* __restrict__ bias,
                         const long long* __restrict__ target, __nv_bfloat16* __restrict__ dx, float* __restrict__ dw,
@@ -202,6 +204,7 @@ linear_xent_head_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16
     atomicAdd(loss_acc, l * grad_scale);
     atomicAdd(loss_acc + 1, h);
   }
+  if constexpr (!BACKWARD) return;
   // the backward outputs are split over blockIdx.y: slice s owns columns [k_lo, k_hi) of dX and dW (the logits above are
   // recomputed by every slice -- 8 x NC x K FMAs -- which is cheaper than the 16-CTA serial tail it replaces)
   const int kslice = K / static_cast<int>(gridDim.y);
@@ -277,17 +280,42 @@ extern "C" int b200_linear_xent_head(const void* x, const void* w, const float* 
     return -2;
   static size_t configured = 0;
   if (smem > 48 * 1024 && smem > configured) {
-    cudaError_t e = cudaFuncSetAttribute(linear_xent_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(linear_xent_head_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          static_cast<int>(smem));
     if (e != cudaSuccess) return static_cast<int>(e);
     configured = smem;
   }
   int ks = 8;                                   // column slices of the backward outputs (grid.y); each a multiple of 8 columns
   while (ks > 1 && (K % (ks * 8))) ks >>= 1;
-  cudaError_t le = launch_pdl(linear_xent_head_kernel, dim3((rows + HEAD_ROWS - 1) / HEAD_ROWS, ks), dim3(256), smem, stream,
+  cudaError_t le = launch_pdl(linear_xent_head_kernel<true>, dim3((rows + HEAD_ROWS - 1) / HEAD_ROWS, ks), dim3(256), smem, stream,
                               reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<const __nv_bfloat16*>(w), bias,
                               target, reinterpret_cast<__nv_bfloat16*>(dx), dw, db, loss_acc, logits_out, rows, K, NC,
                               grad_scale);
+  if (le != cudaSuccess) return static_cast<int>(le);
+  return static_cast<int>(cudaGetLastError());
+}
+
+// forward-only classifier head (evaluation): loss_acc[0] += sum of the row losses, loss_acc[1] += #correct, optional fp32
+// logits.  Same shape limits as b200_linear_xent_head.
+extern "C" int b200_linear_xent_eval(const void* x, const void* w, const float* bias, const long long* target,
+                                     float* loss_acc, float* logits_out, int rows, int K, int NC, cudaStream_t stream) {
+  using namespace b200;
+  if (rows <= 0) return 0;
+  const size_t smem = static_cast<size_t>(K) * (NC + HEAD_ROWS) * 2 + HEAD_ROWS * 34 * 4;
+  if (NC < 1 || NC > 32 || (K % 8) || smem > 200 * 1024 || (reinterpret_cast<uintptr_t>(x) & 15) ||
+      (reinterpret_cast<uintptr_t>(w) & 15))
+    return -2;
+  static size_t configured = 0;
+  if (smem > 48 * 1024 && smem > configured) {
+    cudaError_t e = cudaFuncSetAttribute(linear_xent_head_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         static_cast<int>(smem));
+    if (e != cudaSuccess) return static_cast<int>(e);
+    configured = smem;
+  }
+  cudaError_t le = launch_pdl(linear_xent_head_kernel<false>, dim3((rows + HEAD_ROWS - 1) / HEAD_ROWS, 1), dim3(256), smem,
+                              stream, reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<const __nv_bfloat16*>(w),
+                              bias, target, static_cast<__nv_bfloat16*>(nullptr), static_cast<float*>(nullptr),
+                              static_cast<float*>(nullptr), loss_acc, logits_out, rows, K, NC, 1.0f);
   if (le != cudaSuccess) return static_cast<int>(le);
   return static_cast<int>(cudaGetLastError());
 }

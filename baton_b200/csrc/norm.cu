@@ -1201,6 +1201,28 @@ bn_maxpool_bwd_apply_kernel(const uint4* __restrict__ z, const uint4* __restrict
   }
 }
 
+// Eval-mode BatchNorm folding: block b turns BatchNorm b into the per-channel scale / shift of bn_apply_kernel's eval
+// branch (same expressions), read from the parameter arena.  table[b] = {gamma, beta, running_mean, running_var,
+// output offset, C, eps bits}; the first four are element offsets into `arena`, gamma / beta may be -1 (affine=False).
+// out[off .. off + C) = scale, out[off + C .. off + 2C) = shift.
+__global__ void __launch_bounds__(256)
+bn_fold_eval_kernel(const float* __restrict__ arena, const long long* __restrict__ table, float* __restrict__ out) {
+  griddep_launch_dependents();
+  griddep_wait();
+  const long long* t = table + static_cast<size_t>(blockIdx.x) * 7;
+  const long long go = t[0], bo = t[1], mo = t[2], vo = t[3], oo = t[4];
+  const int C = static_cast<int>(t[5]);
+  const float eps = __int_as_float(static_cast<int>(t[6]));
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const float mean = arena[mo + c];
+    const float var = arena[vo + c];
+    const float rstd = rsqrtf(var + eps);
+    const float g = go >= 0 ? arena[go + c] : 1.f;
+    out[oo + c] = g * rstd;
+    out[oo + C + c] = (bo >= 0 ? arena[bo + c] : 0.f) - mean * g * rstd;
+  }
+}
+
 static inline int stream_grid(long long nvec) {
   long long g = (nvec + 255) / 256;
   if (g < 1) g = 1;
@@ -1212,6 +1234,12 @@ static inline int stream_grid(long long nvec) {
 
 using namespace b200;
 #define RET_LAST() return static_cast<int>(cudaGetLastError())
+
+extern "C" int b200_bn_fold_eval(const float* arena, const long long* table, int n_bn, float* out, cudaStream_t stream) {
+  if (n_bn <= 0) return 0;
+  launch_pdl(bn_fold_eval_kernel, n_bn, 256, 0, stream, arena, table, out);
+  RET_LAST();
+}
 
 extern "C" int b200_bn_stats(const void* x, float* sums, long long rows, int C, cudaStream_t stream) {
   if (rows <= 0) return 0;

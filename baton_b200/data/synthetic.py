@@ -9,6 +9,11 @@ Added for the benchmark configurations: class-conditional image shards (32x32) a
 token shards with three label partitions across K clients -- IID, label-skew
 (each client sees ``classes_per_client`` classes) and Dirichlet(alpha) non-IID
 (the standard FL benchmark partition; alpha=0.1 is highly skewed).
+
+Held-out data for evaluating the global model: ``holdout_image_shard`` /
+``holdout_token_shard`` draw IID, class-balanced samples of the same classes
+(the same image class means, the same vocabulary bands) from a random stream
+that no training client uses, so accuracy on them measures generalisation.
 """
 from __future__ import annotations
 
@@ -77,21 +82,72 @@ def _labels_for(spec: ShardSpec, generator: Optional[torch.Generator]) -> torch.
     return torch.multinomial(spec.class_probs, spec.n_samples, replacement=True, generator=generator)
 
 
+# seed offset of the held-out stream: client k trains on seed * mult + 1000003 * (k + 1) and the class means use ``seed``
+# itself; seed * mult + 500009 equals neither for any seed >= 0
+_HOLDOUT_OFFSET = 500009
+
+
+def _stream(seed: int, mult: int, client: int) -> torch.Generator:
+    """Sample generator of training client ``client``."""
+    return torch.Generator().manual_seed(seed * mult + 1000003 * (client + 1))
+
+
+def _holdout_stream(seed: int, mult: int) -> torch.Generator:
+    """Sample generator of the held-out data: a stream no training client and no class-mean draw uses."""
+    return torch.Generator().manual_seed(seed * mult + _HOLDOUT_OFFSET)
+
+
+def class_means(num_classes: int, *, channels: int = 3, size: int = 32, seed: int = 0) -> torch.Tensor:
+    """The per-class mean images ``[num_classes, size, size, channels]`` behind :func:`image_shard`."""
+    gm = torch.Generator().manual_seed(seed)
+    return torch.randn(num_classes, size, size, channels, generator=gm) * 0.5
+
+
+def _images(means, y, g, noise, dtype, channels_last, pin):
+    X = means[y] + noise * torch.randn(y.numel(), *means.shape[1:], generator=g)
+    if not channels_last:
+        X = X.permute(0, 3, 1, 2).contiguous()
+    X = X.to(dtype)
+    if pin and torch.cuda.is_available():
+        X, y = X.pin_memory(), y.pin_memory()
+    return X, y
+
+
+def _balanced_labels(num_classes: int, n: int, g: torch.Generator) -> torch.Tensor:
+    """``n`` labels, every class ``n // num_classes`` or one more times, in random order."""
+    return (torch.arange(n) % num_classes)[torch.randperm(n, generator=g)]
+
+
 def image_shard(spec: ShardSpec, *, channels: int = 3, size: int = 32, seed: int = 0,
                 dtype=torch.float32, channels_last: bool = True, pin: bool = False,
                 noise: float = 1.0) -> Tuple[torch.Tensor, torch.Tensor]:
     """Class-conditional Gaussian images: each class has a fixed random mean
     pattern (shared across clients through ``seed``), samples are mean + noise.
     Returned as NHWC when ``channels_last`` (the layout the conv kernels use)."""
-    num_classes = spec.class_probs.numel()
-    gm = torch.Generator().manual_seed(seed)
-    means = torch.randn(num_classes, size, size, channels, generator=gm) * 0.5
-    g = torch.Generator().manual_seed(seed * 7919 + 1000003 * (spec.client + 1))
+    means = class_means(spec.class_probs.numel(), channels=channels, size=size, seed=seed)
+    g = _stream(seed, 7919, spec.client)
     y = _labels_for(spec, g)
-    X = means[y] + noise * torch.randn(spec.n_samples, size, size, channels, generator=g)
-    if not channels_last:
-        X = X.permute(0, 3, 1, 2).contiguous()
-    X = X.to(dtype)
+    return _images(means, y, g, noise, dtype, channels_last, pin)
+
+
+def holdout_image_shard(num_classes: int, n: int, *, channels: int = 3, size: int = 32, seed: int = 0,
+                        dtype=torch.float32, channels_last: bool = True, pin: bool = False,
+                        noise: float = 1.0) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Held-out images for evaluation: class-balanced labels, the class means of :func:`image_shard` with the same
+    ``seed``, and noise from a random stream no training client draws from."""
+    means = class_means(num_classes, channels=channels, size=size, seed=seed)
+    g = _holdout_stream(seed, 7919)
+    y = _balanced_labels(num_classes, n, g)
+    return _images(means, y, g, noise, dtype, channels_last, pin)
+
+
+def _tokens(y, seq_len, vocab, num_classes, g, pin):
+    n = y.numel()
+    base = torch.randint(0, vocab, (n, seq_len), generator=g)
+    band = max(1, vocab // (num_classes * 4))
+    hot = torch.randint(0, band, (n, seq_len), generator=g) + (y.view(-1, 1) * band)
+    use_hot = torch.rand(n, seq_len, generator=g) < 0.3
+    X = torch.where(use_hot, hot, base)
     if pin and torch.cuda.is_available():
         X, y = X.pin_memory(), y.pin_memory()
     return X, y
@@ -101,14 +157,15 @@ def token_shard(spec: ShardSpec, *, seq_len: int = 128, vocab: int = 30522, seed
                 pin: bool = False) -> Tuple[torch.Tensor, torch.Tensor]:
     """Class-conditional token sequences for the BERT config: each class
     over-samples a class-specific slice of the vocabulary."""
-    num_classes = spec.class_probs.numel()
-    g = torch.Generator().manual_seed(seed * 104729 + 1000003 * (spec.client + 1))
+    g = _stream(seed, 104729, spec.client)
     y = _labels_for(spec, g)
-    base = torch.randint(0, vocab, (spec.n_samples, seq_len), generator=g)
-    band = max(1, vocab // (num_classes * 4))
-    hot = torch.randint(0, band, (spec.n_samples, seq_len), generator=g) + (y.view(-1, 1) * band)
-    use_hot = torch.rand(spec.n_samples, seq_len, generator=g) < 0.3
-    X = torch.where(use_hot, hot, base)
-    if pin and torch.cuda.is_available():
-        X, y = X.pin_memory(), y.pin_memory()
-    return X, y
+    return _tokens(y, seq_len, vocab, spec.class_probs.numel(), g, pin)
+
+
+def holdout_token_shard(num_classes: int, n: int, *, seq_len: int = 128, vocab: int = 30522, seed: int = 0,
+                        pin: bool = False) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Held-out token sequences for evaluation: class-balanced labels, the vocabulary bands of :func:`token_shard`,
+    from a random stream no training client draws from."""
+    g = _holdout_stream(seed, 104729)
+    y = _balanced_labels(num_classes, n, g)
+    return _tokens(y, seq_len, vocab, num_classes, g, pin)

@@ -4,8 +4,8 @@ The reference's observability is 23 ``print`` calls (e.g. manager.py:73,117,
 131-132).  This module provides:
 
   * ``RoundMetrics`` -- an in-memory JSON-able log of round records (wall time,
-    participants, samples, bytes moved, device-timed phases) served by the
-    manager at ``GET /{name}/metrics``;
+    participants, samples, bytes moved, device-timed phases) and of evaluations of
+    the global model, served by the manager at ``GET /{name}/metrics``;
   * ``phase`` -- a context manager that opens an NVTX range (when CUDA is
     present) and records host wall time, used around broadcast / local-train /
     upload-reduce;
@@ -27,6 +27,7 @@ class RoundMetrics:
     def __init__(self, name: str, max_records: int = 4096):
         self.name = name
         self.records: List[dict] = []
+        self.evals: List[dict] = []         # held-out loss / accuracy of the global model, oldest first
         self.max_records = max_records
         self.counters: Dict[str, float] = {}
 
@@ -41,6 +42,14 @@ class RoundMetrics:
         log.info("round %s", json.dumps(record, default=str))
         return record
 
+    def add_eval(self, **record) -> dict:
+        record.setdefault("t", time.time())
+        self.evals.append(record)
+        if len(self.evals) > self.max_records:
+            del self.evals[: len(self.evals) - self.max_records]
+        log.info("eval %s", json.dumps(record, default=str))
+        return record
+
     def summary(self) -> dict:
         walls = [r["wall_s"] for r in self.records if "wall_s" in r]
         samples = sum(r.get("n_samples", 0) for r in self.records)
@@ -52,6 +61,7 @@ class RoundMetrics:
             "samples_per_s": (samples / total) if total > 0 else None,
             "counters": dict(self.counters),
             "last": self.records[-1] if self.records else None,
+            "evals": list(self.evals),
         }
 
 

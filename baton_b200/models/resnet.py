@@ -91,6 +91,34 @@ def _stem_bwd(saved, bn, pool, dy_a, dy_b=None):
     bnn._ConvFn.backward(cc, dz)
 
 
+# Evaluation (``ResNet.explicit_eval``): every conv + BatchNorm pair is ONE GEMM whose epilogue applies the eval-mode
+# BatchNorm -- the per-channel scale / shift that ``F.bn_fold_eval`` wrote into ``model.eval_bn_table`` at the
+# BatchNorm's ``eval_off`` -- plus the block's shortcut and the ReLU.  Where a GEMM declines the epilogue, the plain
+# GEMM and ``bn_apply(training=0)`` run instead.  The bf16 weights come from ``ResNet.prepare_eval`` (once per pass).
+def _conv_bn_eval(conv, bn, x, table, residual=None):
+    F = bnn.F
+    n, h, w, c = x.shape
+    k, s, p = conv.kernel_size, conv.stride, conv.padding
+    cout = conv.out_channels
+    ho, wo = F.conv_out_size(h, k, s, p), F.conv_out_size(w, k, s, p)
+    wt = conv.eval_weight
+    af = F.affine_epilogue_args(table, bn.eval_off, cout, bn.relu, residual)
+    centre = h == 1 and w == 1 and k % 2 == 1 and p == k // 2 and c % 8 == 0 and k > 1
+    if centre:                  # a k x k "same" convolution of a 1x1 map sees only its centre tap (see _ConvFn)
+        y = F.gemm(x.view(n, c), wt.view(cout, k * k, c)[:, (k // 2) * k + k // 2, :], affine=af)
+    elif k == 1 and s == 1 and p == 0 and c % 8 == 0:
+        y = F.gemm(x.view(n * h * w, c), wt, affine=af)
+    elif c % 64 == 0:
+        y = F.conv_igemm_fwd(x, wt, k, k, s, p, affine=af)
+    else:
+        y = F.gemm(F.im2col(x, k, k, s, p)[0], wt, affine=af)
+    if y is None:
+        z = bnn._ConvFn.forward(bnn.Ctx(), x, conv.weight, wt, k, k, s, p, None)
+        y = bnn._BNFn.forward(bnn.Ctx(), z, residual, bn.weight, bn.bias, bn.running_mean, bn.running_var, None, bn.eps,
+                              bn.momentum, bn.relu, False, None, None)
+    return y.view(n, ho, wo, cout)
+
+
 class BasicBlock(nn.Module):
     expansion = 1
 
@@ -283,6 +311,53 @@ class ResNet(FederatedModule):
             _conv_bn_bwd(stem, d, needs_dx=False)
         bnn.WGRAD.join()
         return stats
+
+    # ------------------------------------------------------------------ evaluation
+    def _block_eval(self, blk, x, table):
+        identity = x
+        if blk.downsample is not None:
+            with bnn.BRANCH.fork(x):                      # parallel graph branch: 1x1 conv + BN of the shortcut
+                identity = _conv_bn_eval(blk.downsample[0], blk.downsample[1], x, table)
+        out = x
+        n = len(blk.units)
+        for i, (cn, bn_name) in enumerate(blk.units):
+            last = i == n - 1
+            if last:
+                bnn.BRANCH.join()
+            out = _conv_bn_eval(getattr(blk, cn), getattr(blk, bn_name), out, table, identity if last else None)
+        return out
+
+    def prepare_eval(self):
+        """Head of an evaluation pass: the bf16 weights every ``explicit_eval`` of the pass reads (the stem's
+        zero-padded copy is made here, once, instead of per batch; the others are views of the arena shadow)."""
+        for m in self.modules():
+            if isinstance(m, bnn.Conv2d):
+                m.eval_weight = m._w_bf16(gated=False)   # evaluation runs after the collective has been joined
+
+    def explicit_eval(self, x, target, acc, want_logits: bool = False):
+        """Forward-only pass of one batch in eval mode (running statistics): adds the SUM of the row cross-entropies
+        and the number of correct predictions into ``acc`` (fp32 ``[2]``); returns the fp32 logits when
+        ``want_logits``, else ``None``.  Every BatchNorm runs in the epilogue of its
+        convolution GEMM, reading the scale / shift that ``F.bn_fold_eval`` wrote into ``self.eval_bn_table`` and the
+        weights of :meth:`prepare_eval` (both run at the head of the pass).  Saves
+        nothing for a backward pass and writes no model state.  CUDA, bf16 only."""
+        F = bnn.F
+        table = self.eval_bn_table
+        h = _conv_bn_eval(self.conv1, self.bn1, x, table)
+        h = F.maxpool(h, self.maxpool.k, self.maxpool.stride, self.maxpool.pad)[0]
+        for layer in (self.layer1, self.layer2, self.layer3, self.layer4):
+            for blk in layer:
+                h = self._block_eval(blk, h, table)
+        feat = h.reshape(h.shape[0], h.shape[3]) if h.shape[1] == 1 and h.shape[2] == 1 else F.avgpool(h)
+        fc = self.fc
+        w = bnn._shadow(fc, "weight", fc.weight)
+        if fc.act == 0:
+            head = F.linear_xent_eval(feat.contiguous(), w, fc.bias, target, acc, want_logits=want_logits)
+            if head is not None:
+                return head[1]
+        logits = F.gemm(feat.contiguous(), w, bias=fc.bias, act=fc.act, out_dtype=torch.float32)
+        F.softmax_xent(logits, target, want_grad=False, acc=acc, loss_scale=1.0)
+        return logits if want_logits else None
 
     # ------------------------------------------------------------------
     def build_workspace(self, device) -> torch.Tensor:

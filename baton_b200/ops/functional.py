@@ -77,7 +77,8 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
          n_valid: Optional[int] = None, flags: Optional[torch.Tensor] = None, flag_epoch: int = 0,
          flag_elem_off: int = 0, flag_tile_elems: int = 0, flag_bias_off: int = -1, force_bn: int = 0,
          force_simt: bool = False, col_stats: Optional[torch.Tensor] = None,
-         flag_epoch_word: Optional[torch.Tensor] = None, sgd: Optional[dict] = None) -> Optional[torch.Tensor]:
+         flag_epoch_word: Optional[torch.Tensor] = None, sgd: Optional[dict] = None,
+         affine: Optional[dict] = None) -> Optional[torch.Tensor]:
     """``out[M,N] = act(alpha * A @ B^T + bias)`` on the tensor cores (wgmma).
 
     ``n_valid`` limits the written columns (used when B carries zero K-padding
@@ -89,7 +90,11 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
 
     ``sgd`` (see :func:`sgd_epilogue_args`): on a weight-gradient GEMM (``accumulate`` into fp32 ``out``, MN-major
     operands) apply the SGD step to the parameters in the epilogue instead of accumulating the gradient into ``out``.
-    Returns ``None`` when this GEMM cannot (split-K, persistent kernel...): nothing was written, accumulate instead."""
+    Returns ``None`` when this GEMM cannot (split-K, persistent kernel...): nothing was written, accumulate instead.
+
+    ``affine`` (see :func:`affine_epilogue_args`): eval-mode BatchNorm in the epilogue of a bf16 forward GEMM,
+    ``out = relu?(A @ B^T * scale + shift + residual)``.  Returns ``None`` when this GEMM cannot apply it: nothing was
+    written, run the GEMM and ``bn_apply`` instead."""
     C = load()
     M, K = (a.shape[1], a.shape[0]) if a_mn else (a.shape[0], a.shape[1])
     N, Kb = (b.shape[1], b.shape[0]) if b_mn else (b.shape[0], b.shape[1])
@@ -103,12 +108,12 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
     ldd = out.stride(0) if out.dim() == 2 else N
     lda, ldb = _pitch(a), _pitch(b)
     use_simt = force_simt or not (_tma_ok(a) and _tma_ok(b))
-    if use_simt and sgd is not None:
+    if use_simt and (sgd is not None or affine is not None):
         return None
     if use_simt:
         assert col_stats is None, "fused column statistics need the tensor-core path"
         C.gemm(a, b, out, bias, M, N, K, lda, ldb, ldd, a_mn, b_mn, act, 1, accumulate, alpha, None, 0, 0, 0, -1, 0,
-               True, None, None, None, None, None, None, False)
+               True, None, None, None, None, None, None, False, None, None, None, False)
         return out
     bn = force_bn or pick_bn(M, N)
     if col_stats is not None:
@@ -124,11 +129,32 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
         assert out.dtype == torch.float32 and bias is None and act == 0
     if sgd is not None and split_k != 1:
         return None                 # the optimizer epilogue needs every tile's complete gradient in one CTA
-    sg = sgd or {}
+    if affine is not None and split_k > 1:
+        return None                 # atomic split-K partials cannot take a per-element epilogue
+    sg, af = sgd or {}, affine or {}
     if not C.gemm(a, b, out, bias, M, N, K, lda, ldb, ldd, a_mn, b_mn, act, split_k, accumulate, alpha, flags, flag_epoch,
                   flag_elem_off, flag_tile_elems, flag_bias_off, bn, False, col_stats, flag_epoch_word, sg.get("theta"),
-                  sg.get("theta_bf16"), sg.get("momentum"), sg.get("hyper"), bool(sg.get("nesterov", False))):
+                  sg.get("theta_bf16"), sg.get("momentum"), sg.get("hyper"), bool(sg.get("nesterov", False)),
+                  af.get("scale"), af.get("shift"), af.get("residual"), bool(af.get("relu", False))):
         return None
+    return out
+
+
+def affine_epilogue_args(table: torch.Tensor, offset: int, channels: int, relu: bool,
+                         residual: Optional[torch.Tensor] = None) -> dict:
+    """``affine=`` argument of :func:`gemm` / :func:`conv_igemm_fwd` for the BatchNorm whose eval scale / shift
+    :func:`bn_fold_eval` wrote at ``offset`` of ``table``; ``residual``: optional bf16 ``[rows, channels]`` (or NHWC)
+    tensor added before the ReLU."""
+    return {"scale": table[offset: offset + channels], "shift": table[offset + channels: offset + 2 * channels],
+            "relu": relu, "residual": residual}
+
+
+def bn_fold_eval(arena: torch.Tensor, table: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """Eval-mode scale / shift of every BatchNorm of ``table`` (int64 ``[n_bn, 7]``: element offsets of gamma, beta,
+    running_mean, running_var in the fp32 ``arena``, output offset, C, eps as float32 bits) into ``out``, one launch:
+    ``scale = gamma * rsqrt(var + eps)``, ``shift = beta - mean * gamma * rsqrt(var + eps)`` -- ``bn_apply``'s eval
+    arithmetic."""
+    load().bn_fold_eval(arena, table, out)
     return out
 
 
@@ -308,19 +334,26 @@ def im2col(x: torch.Tensor, kh: int, kw: int, stride: int, pad: int) -> Tuple[to
 
 
 def conv_igemm_fwd(x: torch.Tensor, w2d: torch.Tensor, kh: int, kw: int, stride: int, pad: int,
-                   col_stats: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
+                   col_stats: Optional[torch.Tensor] = None, affine: Optional[dict] = None,
+                   cluster_k: Optional[int] = None, force_bn: int = 0,
+                   out: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
     """Implicit-GEMM convolution forward: ``y[N*Ho*Wo, Cout]`` straight from NHWC ``x`` through TMA
-    im2col loads (no ``col`` buffer).  ``w2d``: ``[Cout, kh*kw*Cin]`` channels_last weights.  Returns ``None``
-    when the shape is not supported (Cin % 64 != 0)."""
+    im2col loads (no ``col`` buffer).  ``w2d``: ``[Cout, kh*kw*Cin]`` channels_last weights.  ``affine``: eval-mode
+    BatchNorm epilogue as in :func:`gemm`.  ``out``: contiguous bf16 ``[N*Ho*Wo, Cout]`` to write.  Returns ``None``
+    when the shape (or the epilogue) is not supported (Cin % 64 != 0)."""
     n, h, w, c = x.shape
     cout = w2d.shape[0]
     if c % 64 or w2d.shape[1] != kh * kw * c or not x.is_contiguous() or not w2d.is_contiguous():
         return None
     ho, wo = conv_out_size(h, kh, stride, pad), conv_out_size(w, kw, stride, pad)
     M, K = n * ho * wo, kh * kw * c
-    bn = pick_bn(M, cout)
-    y = torch.empty((M, cout), dtype=BF16, device=x.device)
-    ok = load().conv_igemm_fwd(x, w2d, y, kh, kw, stride, pad, ho, wo, pick_cluster_k(M, cout, K, bn), bn, col_stats)
+    bn = force_bn or pick_bn(M, cout)
+    if cluster_k is None:
+        cluster_k = pick_cluster_k(M, cout, K, bn)
+    y = out if out is not None else torch.empty((M, cout), dtype=BF16, device=x.device)
+    af = affine or {}
+    ok = load().conv_igemm_fwd(x, w2d, y, kh, kw, stride, pad, ho, wo, cluster_k, bn, col_stats, af.get("scale"),
+                               af.get("shift"), af.get("residual"), bool(af.get("relu", False)))
     return y if ok else None
 
 
@@ -486,15 +519,17 @@ def avgpool_bwd(dy: torch.Tensor, in_shape) -> torch.Tensor:
 
 # ---------------------------------------------------------------------------- losses
 def softmax_xent(logits: torch.Tensor, target: torch.Tensor, want_grad: bool = True,
-                 grad_dtype: Optional[torch.dtype] = None, acc: Optional[torch.Tensor] = None):
+                 grad_dtype: Optional[torch.dtype] = None, acc: Optional[torch.Tensor] = None,
+                 loss_scale: Optional[float] = None):
     """Fused softmax cross-entropy: returns ``(acc, dlogits)`` where ``acc[0]`` is the
     batch-mean loss and ``acc[1]`` the number of correct predictions.  ``acc`` (fp32 ``[2]``) may be supplied: the
-    kernel ADDS into it (a device-side running sum over the steps of an epoch, no extra kernels)."""
+    kernel ADDS into it (a device-side running sum over the steps of an epoch, no extra kernels).  ``loss_scale``
+    replaces the ``1 / rows`` that scales the loss and the gradient (1.0: the sum of the row losses)."""
     rows, c = logits.shape
     if acc is None:
         acc = torch.zeros(2, dtype=torch.float32, device=logits.device)
     dl = torch.empty_like(logits, dtype=grad_dtype or logits.dtype) if want_grad else None
-    load().softmax_xent(logits, target, dl, acc, rows, c, logits.stride(0), 1.0 / rows)
+    load().softmax_xent(logits, target, dl, acc, rows, c, logits.stride(0), 1.0 / rows if loss_scale is None else loss_scale)
     return acc, dl
 
 
@@ -511,6 +546,16 @@ def linear_xent_head(x: torch.Tensor, w_bf16: torch.Tensor, bias: Optional[torch
     logits = torch.empty((rows, w_bf16.shape[0]), dtype=torch.float32, device=x.device) if want_logits else None
     ok = load().linear_xent_head(x, w_bf16, bias, target, dx, dw, db, acc, logits, 1.0 / rows)
     return (acc, dx, logits) if ok else None
+
+
+def linear_xent_eval(x: torch.Tensor, w_bf16: torch.Tensor, bias: Optional[torch.Tensor], target: torch.Tensor,
+                     acc: torch.Tensor, want_logits: bool = False):
+    """Forward-only classifier head (evaluation), one launch: ``logits = x w^T + b`` (<= 32 classes), then ``acc[0]``
+    += the SUM of the row cross-entropies and ``acc[1]`` += #correct.  Returns ``(acc, logits or None)`` or ``None``
+    when the shape is not supported."""
+    logits = torch.empty((x.shape[0], w_bf16.shape[0]), dtype=torch.float32, device=x.device) if want_logits else None
+    ok = load().linear_xent_eval(x, w_bf16, bias, target, acc, logits)
+    return (acc, logits) if ok else None
 
 
 def mse(pred: torch.Tensor, target: torch.Tensor, want_grad: bool = True):

@@ -467,13 +467,15 @@ class Conv2d(nn.Module):
         self.kp = F.round_up(self.k_true, 8)
         self.flags_cfg = None   # bcast_gemm: set by FedAvgSession.gate_first_conv for the first conv of the model
 
-    def _w_bf16(self):
+    def _w_bf16(self, gated: bool = True):
+        """bf16 ``[Cout, kp]`` weights.  ``gated=False``: the zero-padded copy does not wait on the first layer's
+        arrival flags (callers that run after the round-end collective has been joined)."""
         sh = getattr(self, "weight_bf16", None)
         if sh is None:
             sh = _shadow(self, "weight", self.weight)
         sh = sh.view(self.out_channels, self.k_true)
         if self.kp != self.k_true:  # K not a multiple of 8 (7x7x3 stem): zero-padded copy for TMA
-            sh = F.pad_rows(sh, self.kp, gate=self.flags_cfg)
+            sh = F.pad_rows(sh, self.kp, gate=self.flags_cfg if gated else None)
         return sh
 
     def forward(self, x):

@@ -40,6 +40,23 @@ class RoundResult:
     global_loss: Optional[List[float]] = None
 
 
+@dataclass
+class EvalResult:
+    """Sample-weighted loss and accuracy of the global model on held-out data: ``loss`` / ``accuracy`` / ``n_samples``
+    over every rank's shards, ``local_*`` over this rank's.  ``loss`` is the mean per-sample cross-entropy (or mean
+    squared error); ``accuracy`` is 0 for regression; both are ``nan`` when no sample was evaluated."""
+    loss: float
+    accuracy: float
+    n_samples: int
+    local_loss: float
+    local_accuracy: float
+    local_n_samples: int
+
+
+def _mean(total: float, n: float) -> float:
+    return total / n if n > 0 else float("nan")
+
+
 class FederatedEngine:
     def __init__(self, model, device, *, backend: str = "fused", group=None, loss: str = "ce",
                  lr: float = 0.05, batch_size: int = 128, momentum: float = 0.0, weight_decay: float = 0.0,
@@ -90,6 +107,7 @@ class FederatedEngine:
         self.sample_k = sample_k
         self._rng = random.Random(seed)            # identical stream on every rank
         self._stage: Dict[Tuple, Tuple[torch.Tensor, torch.Tensor]] = {}
+        self._eval_stage: Dict[Tuple, Tuple[torch.Tensor, torch.Tensor]] = {}
         self._acc = None
         self.last_losses_dev = None
         self.samples_trained = 0          # samples this rank pushed through local SGD (per epoch)
@@ -100,12 +118,15 @@ class FederatedEngine:
         """Asynchronous host->device copy of a shard into persistent staging buffers (so the
         captured epoch graph keeps pointing at the same addresses).  ``X_host``/``y_host`` should
         be pinned.  Returns the device views."""
+        return self._copy_in(self._stage, X_host, y_host, slot)
+
+    def _copy_in(self, stage: dict, X_host: torch.Tensor, y_host: torch.Tensor, slot: int):
         key = (slot, tuple(X_host.shape), X_host.dtype, tuple(y_host.shape), y_host.dtype)
-        bufs = self._stage.get(key)
+        bufs = stage.get(key)
         if bufs is None:
             bufs = (torch.empty(X_host.shape, dtype=X_host.dtype, device=self.device),
                     torch.empty(y_host.shape, dtype=y_host.dtype, device=self.device))
-            self._stage[key] = bufs
+            stage[key] = bufs
         bufs[0].copy_(X_host, non_blocking=True)
         bufs[1].copy_(y_host, non_blocking=True)
         return bufs
@@ -223,6 +244,42 @@ class FederatedEngine:
 
     def global_loss(self, n_epoch: int) -> List[float]:
         return self.session.reduced_loss(n_epoch)
+
+    # ------------------------------------------------------------------ evaluation
+    def evaluate(self, shards, batch_size: Optional[int] = None) -> EvalResult:
+        """Loss and accuracy of the global model on held-out data.  ``shards`` takes the forms of :meth:`run_round`:
+        an ``(X, y)`` pair for this rank, a callable ``rank -> (X, y)``, or with logical clients a callable
+        ``client_id -> (X, y)`` (every client this rank hosts is evaluated and the results are summed); ``None`` or
+        an empty shard contributes nothing.  Host shards are staged into their own buffers, never the training ones.
+        Nothing of the model, the arena or the training state changes.  Every rank must call it: the global numbers
+        come from one all-reduce of ``[loss sum, #correct, n]`` over the session's process group."""
+        self.sync()          # the round-end collective may still be writing the arena on its side stream
+        batch = int(batch_size or self.hp["batch_size"])
+        if self.logical_clients:
+            ids = [c for c in range(self.logical_clients) if self.hosted(c)]
+            pairs = [shards(c) for c in ids] if shards is not None else []
+        elif shards is None:
+            pairs = []
+        else:
+            pairs = [shards(self.rank) if callable(shards) else shards]
+        loss = correct = n = 0.0
+        for pair in pairs:
+            if pair is None or pair[0].shape[0] == 0:
+                continue
+            X, y = pair
+            if self.device.type == "cuda" and not X.is_cuda:
+                # one staging buffer per shape: a pass ends with a host read, so the next shard may overwrite it
+                X, y = self._copy_in(self._eval_stage, X, y, 0)
+            ls, c, k = self.trainer.evaluate(X, y, batch_size=batch)
+            loss, correct, n = loss + ls, correct + c, n + k
+        tot = [loss, correct, n]
+        group = getattr(self.session, "group", None)
+        if self.world > 1 and torch.distributed.is_available() and torch.distributed.is_initialized():
+            t = torch.tensor(tot, dtype=torch.float64, device=self.device)
+            torch.distributed.all_reduce(t, group=group)
+            tot = t.tolist()
+        return EvalResult(loss=_mean(tot[0], tot[2]), accuracy=_mean(tot[1], tot[2]), n_samples=int(tot[2]),
+                          local_loss=_mean(loss, n), local_accuracy=_mean(correct, n), local_n_samples=int(n))
 
     def state_dict(self):
         self.sync()

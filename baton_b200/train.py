@@ -19,6 +19,7 @@ Two executions of the same contract:
 """
 from __future__ import annotations
 
+from collections import OrderedDict
 from typing import Callable, List, Optional
 
 import torch
@@ -68,6 +69,43 @@ def run_local_sgd(model: nn.Module, X: torch.Tensor, y: torch.Tensor, *, n_epoch
     return loss_history
 
 
+def bn_fold_table(model: nn.Module, arena):
+    """``(table, n_floats)``: the descriptor table of ``F.bn_fold_eval`` for every BatchNorm of an arena-adopted model
+    (int64 ``[n_bn, 7]`` on the arena's device) and the size of its output, or ``None`` when the model has none.
+    Sets each BatchNorm's ``eval_off``: where its eval scale (``C`` floats) and shift (the next ``C``) land in the
+    output buffer, 8-float aligned."""
+    import struct
+    from .ops import nn as bnn
+    rows, off = [], 0
+    for name, m in model.named_modules():
+        if not isinstance(m, bnn.BatchNorm2d):
+            continue
+        pre = name + "." if name else ""
+        slot = lambda leaf: arena.slots[pre + leaf].offset if (pre + leaf) in arena.slots else -1   # noqa: E731
+        eps_bits = struct.unpack("<i", struct.pack("<f", float(m.eps)))[0]
+        rows.append([slot("weight"), slot("bias"), slot("running_mean"), slot("running_var"), off, m.num_features,
+                     eps_bits])
+        m.eval_off = off
+        off += (2 * m.num_features + 7) // 8 * 8
+    if not rows:
+        return None
+    return torch.tensor(rows, dtype=torch.int64).to(arena.device), off
+
+
+def _eval_batch_generic(model, xb, yb, acc, loss_kind, F):
+    """``model.eval()`` forward of one batch, then the summed loss (and #correct for classification) into ``acc``."""
+    with torch.no_grad():
+        out = model(xb)
+    if loss_kind in ("ce", "cross_entropy"):
+        out2 = out.reshape(-1, out.shape[-1])
+        F.softmax_xent(out2 if out2.stride(-1) == 1 else out2.contiguous(), yb, want_grad=False, acc=acc,
+                       loss_scale=1.0)
+    else:
+        # per-sample mean squared error, summed over the batch: the mean over samples is mse_loss of the whole shard
+        per_row = max(1, out.numel() // max(1, out.shape[0]))
+        F.load().mse(out.contiguous(), yb.reshape(out.shape).contiguous().float(), None, acc, 1.0 / per_row)
+
+
 class GraphedLocalSGD:
     """CUDA local-SGD engine for an arena-adopted model.
 
@@ -89,6 +127,8 @@ class GraphedLocalSGD:
     (``arena``); the engine is what ``FederatedModule.local_train`` dispatches to
     for CUDA shards (``model._graphed_trainer``).
     """
+
+    EVAL_GRAPHS_MAX = 4      # captured evaluation passes kept (each holds its activations in a private pool)
 
     def __init__(self, model: nn.Module, arena, *, loss: str = "ce", nesterov: bool = False,
                  use_graph: bool = True, input_dtype=torch.bfloat16):
@@ -114,6 +154,10 @@ class GraphedLocalSGD:
         self._hyper_host = None
         self.n_kernels_per_step = None
         self.last_stats = {}
+        self.eval_acc = torch.zeros(2, dtype=torch.float32, device=dev)   # evaluation only: [loss sum, #correct]
+        self._eval_graphs = OrderedDict()    # captured evaluation passes, least recently used first
+        self._fold = None
+        self.eval_launches = None     # Counter of the kernels in the last captured evaluation pass
 
     # -------------------------------------------------------------- one SGD step (capturable)
     def _loss(self, out, yb):
@@ -260,6 +304,86 @@ class GraphedLocalSGD:
         self.loss_acc.zero_()
         return {"graph": graph, "graph2": graph2, "perm": perm, "X": X, "y": y}
 
+    # -------------------------------------------------------------- evaluation
+    def _eval_pass(self, X, y, batch_size, explicit):
+        """One pass over ``X, y``: the BatchNorm fold at its head (the running statistics of this round), every full
+        batch and the ragged last one.  Capturable; writes only ``eval_acc`` and the fold table."""
+        self.eval_acc.zero_()
+        if explicit:
+            self._eval_head()
+        n = X.shape[0]
+        for s in range(0, n, batch_size):
+            xb, yb = X[s: s + batch_size], y[s: s + batch_size]
+            if explicit:
+                self.model.explicit_eval(xb, yb, self.eval_acc)
+            else:
+                _eval_batch_generic(self.model, xb, yb, self.eval_acc, self.loss_kind, self.F)
+
+    def _eval_head(self):
+        """What an ``explicit_eval`` pass reads and the arena determines: the BatchNorm fold, the pass's weights."""
+        table, out = self._fold
+        self.F.bn_fold_eval(self.arena.theta, table, out)
+        self.model.prepare_eval()
+
+    def evaluate(self, X, y, batch_size: int = 512):
+        """Loss and accuracy of the model as it stands (in eval mode) on a device-resident shard, without touching the
+        arena, the training accumulators or the BatchNorm state.  Returns ``(loss_sum, correct, n)`` as floats: the
+        summed per-sample loss (cross-entropy, or the per-sample mean squared error) and the number of correct
+        predictions (0 for regression).  The whole pass is captured into ONE CUDA graph per shard (shape and
+        address); a replay re-folds the BatchNorms from the current running statistics."""
+        assert X.is_cuda, "GraphedLocalSGD.evaluate needs a device-resident shard"
+        n = X.shape[0]
+        if n == 0:
+            return 0.0, 0.0, 0.0
+        batch_size = max(1, min(batch_size, n))
+        explicit = (hasattr(self.model, "explicit_eval") and hasattr(self.model, "prepare_eval")
+                    and getattr(self.model, "compute_dtype", "bf16") == "bf16" and self.loss_kind in ("ce", "cross_entropy"))
+        if explicit and self._fold is None:
+            fold = bn_fold_table(self.model, self.arena)
+            if fold is None:
+                explicit = False
+            else:
+                table, size = fold
+                out = torch.zeros(size, dtype=torch.float32, device=self.device)
+                self._fold = (table, out)
+                self.model.eval_bn_table = out
+        was_training = self.model.training
+        nn.Module.train(self.model, False)
+        try:
+            if self.use_graph:
+                key = (n, batch_size, tuple(X.shape[1:]), tuple(y.shape[1:]), X.dtype, y.dtype, X.data_ptr(),
+                       y.data_ptr(), explicit)
+                graph = self._eval_graphs.get(key)
+                if graph is None:
+                    while len(self._eval_graphs) >= self.EVAL_GRAPHS_MAX:
+                        self._eval_graphs.popitem(last=False)       # frees that graph and its memory pool
+                    graph = self._eval_graphs[key] = self._capture_eval(X, y, batch_size, explicit)
+                self._eval_graphs.move_to_end(key)
+                graph.replay()
+            else:
+                self._eval_pass(X, y, batch_size, explicit)
+            loss_sum, correct = self.eval_acc.tolist()
+        finally:
+            nn.Module.train(self.model, was_training)
+        return float(loss_sum), float(correct), float(n)
+
+    def _capture_eval(self, X, y, batch_size, explicit):
+        from .ops._ext import launch_counts
+        cur = torch.cuda.current_stream(self.device)
+        side = torch.cuda.Stream(device=self.device)
+        side.wait_stream(cur)
+        with torch.cuda.stream(side):   # warm-up outside capture (lazy init, kernel attributes); no state is written
+            self._eval_pass(X, y, batch_size, explicit)
+        cur.wait_stream(side)
+        torch.cuda.synchronize(self.device)
+        graph = torch.cuda.CUDAGraph()
+        c0 = launch_counts()
+        with torch.cuda.graph(graph):
+            self._eval_pass(X, y, batch_size, explicit)
+        self.eval_launches = launch_counts() - c0
+        self.eval_captures = getattr(self, "eval_captures", 0) + 1
+        return graph
+
     # -------------------------------------------------------------- public
     @torch.no_grad()
     def _shuffle_into(self, perm, n, generator=None):
@@ -368,3 +492,23 @@ class PortableLocalSGD:
         host = out.tolist()
         self.last_stats = {"accuracy": [h[1] / n for h in host], "steps_per_epoch": steps}
         return [h[0] / steps for h in host]
+
+    def evaluate(self, X, y, batch_size: int = 512):
+        """Same contract as :meth:`GraphedLocalSGD.evaluate` on plain PyTorch ops."""
+        n = X.shape[0]
+        was_training = self.model.training
+        nn.Module.train(self.model, False)
+        loss_sum = correct = 0.0
+        try:
+            with torch.no_grad():
+                for xb, yb in zip(torch.split(X, max(1, batch_size)), torch.split(y, max(1, batch_size))):
+                    pred = self.model(xb)
+                    if yb.dtype.is_floating_point:
+                        per_row = max(1, pred.numel() // max(1, pred.shape[0]))
+                        loss_sum += float(((pred.float() - yb.reshape(pred.shape).float()) ** 2).sum()) / per_row
+                    else:
+                        loss_sum += float(nn.functional.cross_entropy(pred.float(), yb, reduction="sum"))
+                        correct += float((pred.argmax(-1) == yb).sum())
+        finally:
+            nn.Module.train(self.model, was_training)
+        return loss_sum, correct, float(n)

@@ -4,8 +4,10 @@ not touch the instruction stream of kernels that were already validated on hardw
     python scripts/sass_diff.py <git-rev>          # e.g. the last commit validated on the GPU
 
 Compiles every csrc/*.cu of <git-rev> into a temp dir, hashes the instruction text of every kernel (addresses and
-encodings stripped) and compares with baton_b200/csrc/build/*.o.  A trailing `, 0` template argument that was
-added to an existing kernel (e.g. the CONV mode) is normalised away; new kernels are listed separately."""
+encodings stripped) and compares with baton_b200/csrc/build/*.o.  Kernels are matched by demangled name, with
+template arguments appended at their default value normalised away: trailing `, 0` / `, false` arguments (e.g. the
+CONV mode, the SGD and AFFINE epilogue flags) on both sides, and `<true>` on a kernel that was not a template before
+(a new `false` instantiation beside it).  New kernels are listed separately."""
 import hashlib
 import os
 import re
@@ -24,6 +26,31 @@ def kernel_hashes(obj):
         name = fn.split("\n", 1)[0].strip()
         ins = re.findall(r"/\*[0-9a-f]{4,6}\*/\s+(.*?);", fn)
         out[name] = (hashlib.md5("\n".join(ins).encode()).hexdigest(), len(ins))
+    return out
+
+
+def demangle(names):
+    out = subprocess.run(["c++filt"], input="\n".join(names), stdout=subprocess.PIPE, text=True).stdout.splitlines()
+    return dict(zip(names, out))
+
+
+def canonical(hashes, old_plain=()):
+    """demangled name -> hash, appended default-valued template arguments stripped (see the module docstring)"""
+    dm = demangle(list(hashes))
+    out = {}
+    for k, v in hashes.items():
+        name = dm[k]
+        if name.startswith("void "):
+            name = name[5:]
+        prev = None
+        while prev != name:
+            prev = name
+            name = re.sub(r", (?:0|false)>\(", ">(", name)
+        plain = name.replace("<true>(", "(", 1)
+        if plain != name and plain in old_plain:
+            name = plain
+        assert name not in out, "two kernels normalise to " + name
+        out[name] = v
     return out
 
 
@@ -47,16 +74,15 @@ def main():
         if not os.path.exists(new_obj):
             print("MISSING OBJECT", f)
             continue
-        old, new = kernel_hashes(os.path.join(old_dir, f)), kernel_hashes(new_obj)
-        norm = {k.replace("ELi0EEEv14", "EEEv14"): v for k, v in new.items()
-                if "ELi1EEEv14" not in k and "ELi2EEEv14" not in k}
+        old = canonical(kernel_hashes(os.path.join(old_dir, f)))
+        new = norm = canonical(kernel_hashes(new_obj), old_plain=set(old))
         for k, v in old.items():
             total += 1
             if norm.get(k) == v:
                 same += 1
             else:
                 print("DIFF  {:14s} {:5d} -> {:5d}  {}".format(f, v[1], norm.get(k, (0, 0))[1], k[:90]))
-        fresh = [k for k in new if k not in old and k.replace("ELi0EEEv14", "EEEv14") not in old]
+        fresh = [k for k in new if k not in old]
         if fresh:
             print("NEW   {:14s} {}".format(f, len(fresh)))
     print("kernels in {}: {}   byte-identical instruction stream now: {}".format(rev[:10], total, same))
