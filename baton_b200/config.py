@@ -27,6 +27,7 @@ class FederationConfig:
     batch_size: int = 32               # demo.py:29
     momentum: float = 0.0
     weight_decay: float = 0.0
+    prox_mu: float = 0.0               # FedProx proximal coefficient (0: FedAvg's plain local SGD)
     partition: str = "iid"             # iid | label_skew | dirichlet
     alpha: float = 0.1                 # Dirichlet concentration
     samples_per_client: int = 4096
@@ -37,6 +38,10 @@ class FederationConfig:
     wire_dtype: str = "bf16"           # precision of the upload over NVLink: fp32 | bf16
     checkpoint_dir: Optional[str] = None
     seed: int = 0
+
+    def __post_init__(self):
+        if not (0.0 <= float(self.prox_mu) < float("inf")):
+            raise ValueError("prox_mu must be a finite number >= 0, got {!r}".format(self.prox_mu))
 
     def to_json(self) -> str:
         return json.dumps(asdict(self), sort_keys=True)

@@ -24,18 +24,29 @@ inline T* opt_ptr(const std::optional<at::Tensor>& t) {
 }
 #define CHECK_CUDA(x) TORCH_CHECK((x).is_cuda(), #x " must be a CUDA tensor")
 
-// optimizer epilogue of a weight-gradient GEMM: theta / theta_bf16 / momentum start at the element of D[0, 0]
+// FedProx anchor of an SGD step: fp32, contiguous, at least as long as the parameters it anchors, with a 5-float hyper
+inline const float* prox_anchor(const std::optional<at::Tensor>& anchor, int64_t numel, const at::Tensor& hyper) {
+  if (!anchor.has_value() || !anchor->defined()) return nullptr;
+  CHECK_CUDA(*anchor);
+  TORCH_CHECK(anchor->scalar_type() == at::kFloat && anchor->is_contiguous() && anchor->numel() >= numel,
+              "prox anchor: contiguous fp32 covering the parameters");
+  TORCH_CHECK(hyper.numel() >= 5, "prox anchor: hyper needs 5 floats {lr, momentum, weight_decay, dampening, prox_mu}");
+  return anchor->data_ptr<float>();
+}
+
+// optimizer epilogue of a weight-gradient GEMM: theta / theta_bf16 / momentum / anchor start at the element of D[0, 0]
 inline std::optional<B200SgdEpilogue> sgd_epilogue(const std::optional<at::Tensor>& theta,
                                                    const std::optional<at::Tensor>& theta_bf16,
                                                    const std::optional<at::Tensor>& mom,
-                                                   const std::optional<at::Tensor>& hyper, bool nesterov) {
+                                                   const std::optional<at::Tensor>& hyper, bool nesterov,
+                                                   const std::optional<at::Tensor>& anchor) {
   if (!hyper.has_value() || !hyper->defined()) return std::nullopt;
   TORCH_CHECK(theta.has_value() && theta->scalar_type() == at::kFloat && hyper->scalar_type() == at::kFloat &&
                   (!theta_bf16.has_value() || theta_bf16->scalar_type() == at::kBFloat16) &&
                   (!mom.has_value() || mom->scalar_type() == at::kFloat),
               "sgd epilogue: fp32 theta / momentum / hyper, bf16 shadow");
   return B200SgdEpilogue{theta->data_ptr<float>(), opt_ptr<void>(theta_bf16), opt_ptr<float>(mom),
-                         hyper->data_ptr<float>(), nesterov ? 1 : 0};
+                         hyper->data_ptr<float>(), nesterov ? 1 : 0, prox_anchor(anchor, theta->numel(), *hyper)};
 }
 
 // eval-mode BatchNorm epilogue of a forward GEMM: fp32 [N] scale and shift, optional bf16 residual rows
@@ -93,7 +104,7 @@ bool gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor d, const std::opt
           const std::optional<at::Tensor>& col_stats, const std::optional<at::Tensor>& flag_epoch_word,
           const std::optional<at::Tensor>& sgd_theta, const std::optional<at::Tensor>& sgd_theta_bf16,
           const std::optional<at::Tensor>& sgd_mom, const std::optional<at::Tensor>& sgd_hyper, bool sgd_nesterov,
-          const std::optional<at::Tensor>& bn_scale, const std::optional<at::Tensor>& bn_shift,
+          const std::optional<at::Tensor>& sgd_anchor, const std::optional<at::Tensor>& bn_scale, const std::optional<at::Tensor>& bn_shift,
           const std::optional<at::Tensor>& residual, bool bn_relu) {
   CHECK_CUDA(a); CHECK_CUDA(b); CHECK_CUDA(d);
   TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16, "gemm operands must be bf16");
@@ -111,7 +122,8 @@ bool gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor d, const std::opt
           "gemm_simt");
     return true;
   }
-  const std::optional<B200SgdEpilogue> sgd = sgd_epilogue(sgd_theta, sgd_theta_bf16, sgd_mom, sgd_hyper, sgd_nesterov);
+  const std::optional<B200SgdEpilogue> sgd =
+      sgd_epilogue(sgd_theta, sgd_theta_bf16, sgd_mom, sgd_hyper, sgd_nesterov, sgd_anchor);
   const std::optional<B200AffineEpilogue> affine = affine_epilogue(bn_scale, bn_shift, residual, bn_relu, M, N);
   const int rc = b200_gemm_bf16(cptr(a), cptr(b), ptr(d), bp, M, N, K, lda, ldb, ldd, a_mn, b_mn, out_fp32, act, split_k,
                                 accumulate, static_cast<float>(alpha), opt_ptr<const uint32_t>(flags),
@@ -243,12 +255,13 @@ bool conv_igemm_wgrad(const at::Tensor& dy, const at::Tensor& x, at::Tensor dw, 
                       int64_t stride, int64_t pad, int64_t ho, int64_t wo, int64_t split_k, int64_t force_bn,
                       const std::optional<at::Tensor>& sgd_theta, const std::optional<at::Tensor>& sgd_theta_bf16,
                       const std::optional<at::Tensor>& sgd_mom, const std::optional<at::Tensor>& sgd_hyper,
-                      bool sgd_nesterov) {
+                      bool sgd_nesterov, const std::optional<at::Tensor>& sgd_anchor) {
   CHECK_CUDA(dy); CHECK_CUDA(x); CHECK_CUDA(dw);
   TORCH_CHECK(x.scalar_type() == at::kBFloat16 && dy.scalar_type() == at::kBFloat16 && dw.scalar_type() == at::kFloat &&
               x.dim() == 4 && x.is_contiguous() && dy.is_contiguous());
   const c10::cuda::CUDAGuard guard(x.device());
-  const std::optional<B200SgdEpilogue> sgd = sgd_epilogue(sgd_theta, sgd_theta_bf16, sgd_mom, sgd_hyper, sgd_nesterov);
+  const std::optional<B200SgdEpilogue> sgd =
+      sgd_epilogue(sgd_theta, sgd_theta_bf16, sgd_mom, sgd_hyper, sgd_nesterov, sgd_anchor);
   const int rc = b200_conv_igemm_wgrad(cptr(dy), cptr(x), dw.data_ptr<float>(), static_cast<int>(x.size(0)),
                                        static_cast<int>(x.size(1)), static_cast<int>(x.size(2)), static_cast<int>(x.size(3)),
                                        static_cast<int>(cout), static_cast<int>(kh), static_cast<int>(kw),
@@ -290,7 +303,7 @@ void dequant_mx(const at::Tensor& q, const at::Tensor& sf, at::Tensor out, int64
 void fused_sgd(at::Tensor w, at::Tensor g, const std::optional<at::Tensor>& mom, const std::optional<at::Tensor>& wb,
                const at::Tensor& hyper, bool zero_grad, bool nesterov, const std::optional<at::Tensor>& wire_slot,
                const std::optional<at::Tensor>& pack_global, const std::optional<at::Tensor>& pack_scale, int64_t n_pack,
-               bool wire_fp32) {
+               bool wire_fp32, const std::optional<at::Tensor>& prox_anchor_) {
   CHECK_CUDA(w);
   TORCH_CHECK(w.scalar_type() == at::kFloat && g.scalar_type() == at::kFloat && hyper.scalar_type() == at::kFloat);
   TORCH_CHECK(w.is_contiguous() && g.is_contiguous() && w.numel() == g.numel());
@@ -298,14 +311,15 @@ void fused_sgd(at::Tensor w, at::Tensor g, const std::optional<at::Tensor>& mom,
   check(b200_fused_sgd(w.data_ptr<float>(), g.data_ptr<float>(), opt_ptr<float>(mom), opt_ptr<void>(wb), w.numel(),
                        hyper.data_ptr<float>(), zero_grad, nesterov,
                        reinterpret_cast<const unsigned long long*>(opt_ptr<const int64_t>(wire_slot)),
-                       opt_ptr<const float>(pack_global), opt_ptr<const float>(pack_scale), n_pack, wire_fp32, cur_stream()),
+                       opt_ptr<const float>(pack_global), opt_ptr<const float>(pack_scale), n_pack, wire_fp32,
+                       prox_anchor(prox_anchor_, w.numel(), hyper), cur_stream()),
         "fused_sgd");
 }
 
 // segments: int64 [n][3] device table {offset, length, kind} over the arena (see fused_sgd_segments_kernel)
 void fused_sgd_segments(at::Tensor w, at::Tensor g, const std::optional<at::Tensor>& mom,
                         const std::optional<at::Tensor>& wb, const at::Tensor& segments, const at::Tensor& hyper,
-                        bool nesterov) {
+                        bool nesterov, const std::optional<at::Tensor>& prox_anchor_) {
   CHECK_CUDA(w); CHECK_CUDA(segments);
   TORCH_CHECK(w.scalar_type() == at::kFloat && g.scalar_type() == at::kFloat && hyper.scalar_type() == at::kFloat);
   TORCH_CHECK(segments.scalar_type() == at::kLong && segments.dim() == 2 && segments.size(1) == 3 &&
@@ -313,7 +327,8 @@ void fused_sgd_segments(at::Tensor w, at::Tensor g, const std::optional<at::Tens
   const c10::cuda::CUDAGuard guard(w.device());
   check(b200_fused_sgd_segments(w.data_ptr<float>(), g.data_ptr<float>(), opt_ptr<float>(mom), opt_ptr<void>(wb),
                                 reinterpret_cast<const long long*>(segments.data_ptr<int64_t>()),
-                                static_cast<int>(segments.size(0)), hyper.data_ptr<float>(), nesterov, cur_stream()),
+                                static_cast<int>(segments.size(0)), hyper.data_ptr<float>(), nesterov,
+                                prox_anchor(prox_anchor_, w.numel(), hyper), cur_stream()),
         "fused_sgd_segments");
 }
 

@@ -35,13 +35,15 @@ struct SgdPack {
   int wire_fp32;                         // 0: bf16 wire, 1: fp32 wire
 };
 
+// PROX: FedProx step toward `anchor` (indexed like w); otherwise `anchor` is not read.
+template <bool PROX>
 __global__ void __launch_bounds__(EW_THREADS)
 fused_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict__ mom,
                  __nv_bfloat16* __restrict__ wb, long long n, const float* __restrict__ hyper, int zero_grad,
-                 int nesterov, const SgdPack pk) {
+                 int nesterov, const SgdPack pk, const float* __restrict__ anchor) {
   griddep_launch_dependents();
   griddep_wait();
-  const SgdHyper h = load_sgd_hyper(hyper);
+  const SgdHyper h = PROX ? load_sgd_hyper_prox(hyper) : load_sgd_hyper(hyper);
   const long long nv = n >> 2;
   uint8_t* wire = nullptr;
   float pscale = 1.f;
@@ -49,11 +51,21 @@ fused_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict
     wire = reinterpret_cast<uint8_t*>(*pk.wire_slot);
     if (pk.scale != nullptr) pscale = *pk.scale;
   }
+  // delta upload of a FedProx step: the anchor IS the global copy the wire value is taken against -- read it once
+  const bool anchor_is_global = PROX && anchor == pk.global_w;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < nv;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     float4 mv = mom != nullptr ? reinterpret_cast<float4*>(mom)[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-    const float4 wv = sgd_update4(h, reinterpret_cast<float4*>(w)[i], reinterpret_cast<float4*>(g)[i], mv,
-                                  mom != nullptr, nesterov);
+    float4 av = make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 wv;
+    if constexpr (PROX) {
+      av = reinterpret_cast<const float4*>(anchor)[i];
+      wv = sgd_update4_prox(h, reinterpret_cast<float4*>(w)[i], reinterpret_cast<float4*>(g)[i], av, mv,
+                            mom != nullptr, nesterov);
+    } else {
+      wv = sgd_update4(h, reinterpret_cast<float4*>(w)[i], reinterpret_cast<float4*>(g)[i], mv, mom != nullptr,
+                       nesterov);
+    }
     if (mom != nullptr) reinterpret_cast<float4*>(mom)[i] = mv;
     reinterpret_cast<float4*>(w)[i] = wv;
     if (zero_grad) reinterpret_cast<float4*>(g)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -61,7 +73,7 @@ fused_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict
     if (wire != nullptr) {
       float4 d = wv;
       if (pk.global_w != nullptr) {
-        const float4 gl = reinterpret_cast<const float4*>(pk.global_w)[i];
+        const float4 gl = anchor_is_global ? av : reinterpret_cast<const float4*>(pk.global_w)[i];
         d.x -= gl.x; d.y -= gl.y; d.z -= gl.z; d.w -= gl.w;
       }
       d.x *= pscale; d.y *= pscale; d.z *= pscale; d.w *= pscale;
@@ -87,7 +99,8 @@ fused_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict
   if (blockIdx.x == 0) {
     for (long long i = (nv << 2) + threadIdx.x; i < n; i += blockDim.x) {
       float mv = mom != nullptr ? mom[i] : 0.f;
-      const float wv = sgd_update(h, w[i], g[i], mv, mom != nullptr, nesterov);
+      const float wv = PROX ? sgd_update_prox(h, w[i], g[i], anchor[i], mv, mom != nullptr, nesterov)
+                            : sgd_update(h, w[i], g[i], mv, mom != nullptr, nesterov);
       if (mom != nullptr) mom[i] = mv;
       w[i] = wv;
       if (zero_grad) g[i] = 0.f;
@@ -96,27 +109,36 @@ fused_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict
   }
 }
 
+__device__ __forceinline__ bool same_bits4(float4 a, float4 b) {
+  return __float_as_uint(a.x) == __float_as_uint(b.x) && __float_as_uint(a.y) == __float_as_uint(b.y) &&
+         __float_as_uint(a.z) == __float_as_uint(b.z) && __float_as_uint(a.w) == __float_as_uint(b.w);
+}
+
 // ------------------------------------------------------------------ leftover SGD of a step with an optimizer epilogue
 // When the weight-gradient GEMMs of a step applied SGD in their epilogue (gemm_wgmma.cu), what is left is a set of
 // arena ranges, given as a device table of chunks {offset, length, kind} -- one chunk per CTA iteration.
 //   kind 0: parameters with a gradient -- the update of fused_sgd_kernel, gradient zeroed afterwards;
 //   kind 1: parameters whose gradient is identically zero (the off-centre taps of a k x k convolution on a 1x1 map) --
-//           the update with g = 0, gradient never read.  With weight decay 0 and no momentum buffer that update is the
-//           identity, and the chunk is skipped; this is decided here from `hyper`, so a captured graph stays exact when
-//           it is replayed with new hyper-parameters.
+//           the update with g = 0, gradient never read.  With weight decay 0, no momentum buffer and no proximal term
+//           that update is the identity, and the chunk is skipped; this is decided here from `hyper`, so a captured
+//           graph stays exact when it is replayed with new hyper-parameters.
+// With an anchor (FedProx) a kind-1 element moves only by prox*(w - a) [+ wd*w]: without a momentum buffer it is stored
+// only where its bits change.  In engine rounds these taps equal the global model all round, so nothing is written.
+template <bool PROX>
 __global__ void __launch_bounds__(EW_THREADS)
 fused_sgd_segments_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict__ mom,
                           __nv_bfloat16* __restrict__ wb, const long long* __restrict__ seg, int n_seg,
-                          const float* __restrict__ hyper, int nesterov) {
+                          const float* __restrict__ hyper, int nesterov, const float* __restrict__ anchor) {
   griddep_launch_dependents();
   griddep_wait();
-  const SgdHyper h = load_sgd_hyper(hyper);
+  const SgdHyper h = PROX ? load_sgd_hyper_prox(hyper) : load_sgd_hyper(hyper);
   const bool has_mom = mom != nullptr;
-  const bool nograd_is_identity = h.wd == 0.f && !has_mom;
+  const bool nograd_is_identity = h.prox == 0.f && h.wd == 0.f && !has_mom;
   for (int s = blockIdx.x; s < n_seg; s += gridDim.x) {
     const long long off = seg[3 * s], len = seg[3 * s + 1];
     const bool has_grad = seg[3 * s + 2] == 0;
     if (!has_grad && nograd_is_identity) continue;      // block-uniform
+    const bool sparse_store = PROX && !has_grad && !has_mom;
     long long done = 0;
     if ((off & 3) == 0) {
       const long long nv = len >> 2;
@@ -124,8 +146,12 @@ fused_sgd_segments_kernel(float* __restrict__ w, float* __restrict__ g, float* _
         const long long e = off + (i << 2);
         float4 mv = has_mom ? *reinterpret_cast<float4*>(mom + e) : make_float4(0.f, 0.f, 0.f, 0.f);
         const float4 gv = has_grad ? *reinterpret_cast<float4*>(g + e) : make_float4(0.f, 0.f, 0.f, 0.f);
-        const float4 wv = sgd_update4(h, *reinterpret_cast<float4*>(w + e), gv, mv, has_mom, nesterov);
+        const float4 w0 = *reinterpret_cast<float4*>(w + e);
+        const float4 wv = PROX ? sgd_update4_prox(h, w0, gv, *reinterpret_cast<const float4*>(anchor + e), mv, has_mom,
+                                                  nesterov)
+                               : sgd_update4(h, w0, gv, mv, has_mom, nesterov);
         if (has_mom) *reinterpret_cast<float4*>(mom + e) = mv;
+        if (sparse_store && same_bits4(w0, wv)) continue;
         *reinterpret_cast<float4*>(w + e) = wv;
         if (has_grad) *reinterpret_cast<float4*>(g + e) = make_float4(0.f, 0.f, 0.f, 0.f);
         if (wb != nullptr) *reinterpret_cast<uint2*>(wb + e) = make_uint2(pack_bf16x2(wv.x, wv.y), pack_bf16x2(wv.z, wv.w));
@@ -135,8 +161,12 @@ fused_sgd_segments_kernel(float* __restrict__ w, float* __restrict__ g, float* _
     for (long long i = done + threadIdx.x; i < len; i += blockDim.x) {
       const long long e = off + i;
       float mv = has_mom ? mom[e] : 0.f;
-      const float wv = sgd_update(h, w[e], has_grad ? g[e] : 0.f, mv, has_mom, nesterov);
+      const float gv = has_grad ? g[e] : 0.f;
+      const float w0 = w[e];
+      const float wv = PROX ? sgd_update_prox(h, w0, gv, anchor[e], mv, has_mom, nesterov)
+                            : sgd_update(h, w0, gv, mv, has_mom, nesterov);
       if (has_mom) mom[e] = mv;
+      if (sparse_store && __float_as_uint(w0) == __float_as_uint(wv)) continue;
       w[e] = wv;
       if (has_grad) g[e] = 0.f;
       if (wb != nullptr) wb[e] = __float2bfloat16_rn(wv);
@@ -511,24 +541,27 @@ using namespace b200;
 extern "C" int b200_fused_sgd(float* w, float* g, float* mom, void* w_bf16, long long n, const float* hyper,
                               int zero_grad, int nesterov, const unsigned long long* wire_slot,
                               const float* pack_global, const float* pack_scale, long long n_pack, int wire_fp32,
-                              cudaStream_t stream) {
+                              const float* prox_anchor, cudaStream_t stream) {
   if (n <= 0) return 0;
   SgdPack pk;
   pk.wire_slot = wire_slot; pk.global_w = pack_global; pk.scale = pack_scale;
   pk.n_pack = n_pack > n ? n_pack : n; pk.wire_fp32 = wire_fp32;
   if (wire_slot != nullptr && ((n & 7) || (pk.n_pack & 7))) return -2;
-  launch_pdl(fused_sgd_kernel, ew_grid(n >> 2), EW_THREADS, 0, stream, w, g, mom, reinterpret_cast<__nv_bfloat16*>(w_bf16),
-             n, hyper, zero_grad, nesterov, pk);
+  if (reinterpret_cast<uintptr_t>(prox_anchor) & 15) return -2;      // read as float4 at the offsets of w
+  launch_pdl(prox_anchor != nullptr ? fused_sgd_kernel<true> : fused_sgd_kernel<false>, ew_grid(n >> 2), EW_THREADS, 0,
+             stream, w, g, mom, reinterpret_cast<__nv_bfloat16*>(w_bf16), n, hyper, zero_grad, nesterov, pk, prox_anchor);
   RET_LAST();
 }
 extern "C" int b200_fused_sgd_segments(float* w, float* g, float* mom, void* w_bf16, const long long* segments, int n_seg,
-                                       const float* hyper, int nesterov, cudaStream_t stream) {
+                                       const float* hyper, int nesterov, const float* prox_anchor, cudaStream_t stream) {
   if (n_seg <= 0) return 0;
-  if ((reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(mom)) & 15 ||
+  if ((reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(mom) |
+       reinterpret_cast<uintptr_t>(prox_anchor)) & 15 ||
       reinterpret_cast<uintptr_t>(w_bf16) & 7)
     return -2;
-  launch_pdl(fused_sgd_segments_kernel, ew_grid(n_seg * static_cast<long long>(EW_THREADS)), EW_THREADS, 0, stream, w, g,
-             mom, reinterpret_cast<__nv_bfloat16*>(w_bf16), segments, n_seg, hyper, nesterov);
+  launch_pdl(prox_anchor != nullptr ? fused_sgd_segments_kernel<true> : fused_sgd_segments_kernel<false>,
+             ew_grid(n_seg * static_cast<long long>(EW_THREADS)), EW_THREADS, 0, stream, w, g, mom,
+             reinterpret_cast<__nv_bfloat16*>(w_bf16), segments, n_seg, hyper, nesterov, prox_anchor);
   RET_LAST();
 }
 extern "C" int b200_fold_client(float* acc, float* theta, const float* global_w, void* w_bf16, float* mom, long long n_mom,

@@ -93,6 +93,8 @@ struct GemmParams {
   const float* bn_shift = nullptr;
   const __nv_bfloat16* residual = nullptr;   // optional, [M, ldr]
   long long ldr = 0;
+  // FedProx anchor of the optimizer epilogue, indexed like sgd_theta; nullptr: no proximal term (sgd_hyper has 4 floats)
+  const float* sgd_anchor = nullptr;
 };
 
 // Wait until every arrival flag covering arena elements [e0, e1] has reached `need` (published by the FedAvg kernel with
@@ -330,9 +332,12 @@ __device__ __forceinline__ void store_row_chunk(const GemmParams& p, int row, in
 // The tile holds the complete gradient of these weights (single K pass), so the SGD step runs here and the gradient
 // buffer is never touched.  0 + v is the value a red.add into the zeroed gradient would have left (-0 becomes +0), and
 // sgd_update is the arena optimizer's arithmetic: the result matches accumulate-then-fused_sgd bit for bit.
+// PROX: FedProx step, the anchor (sgd_anchor) is read beside theta.
+template <bool PROX>
 __device__ __forceinline__ void sgd_epilogue_chunk(const GemmParams& p, size_t e, int col0, const float (&v)[32],
                                                    bool vec) {
-  const SgdHyper h = load_sgd_hyper(p.sgd_hyper);
+  const float* a = PROX ? p.sgd_anchor + e : nullptr;
+  const SgdHyper h = PROX ? load_sgd_hyper_prox(p.sgd_hyper) : load_sgd_hyper(p.sgd_hyper);
   float* w = p.sgd_theta + e;
   float* m = p.sgd_mom != nullptr ? p.sgd_mom + e : nullptr;
   __nv_bfloat16* wb = p.sgd_wb != nullptr ? p.sgd_wb + e : nullptr;
@@ -343,7 +348,10 @@ __device__ __forceinline__ void sgd_epilogue_chunk(const GemmParams& p, size_t e
       float4 mv = m != nullptr ? *reinterpret_cast<const float4*>(m + j) : make_float4(0.f, 0.f, 0.f, 0.f);
       const float4 gv = make_float4(__fadd_rn(0.f, v[j]), __fadd_rn(0.f, v[j + 1]), __fadd_rn(0.f, v[j + 2]),
                                     __fadd_rn(0.f, v[j + 3]));
-      const float4 wv = sgd_update4(h, *reinterpret_cast<const float4*>(w + j), gv, mv, m != nullptr, nest);
+      const float4 w0 = *reinterpret_cast<const float4*>(w + j);
+      const float4 wv = PROX ? sgd_update4_prox(h, w0, gv, *reinterpret_cast<const float4*>(a + j), mv, m != nullptr,
+                                                nest)
+                             : sgd_update4(h, w0, gv, mv, m != nullptr, nest);
       *reinterpret_cast<float4*>(w + j) = wv;
       if (m != nullptr) *reinterpret_cast<float4*>(m + j) = mv;
       if (wb != nullptr) *reinterpret_cast<uint2*>(wb + j) = make_uint2(pack_bf16x2(wv.x, wv.y), pack_bf16x2(wv.z, wv.w));
@@ -353,7 +361,9 @@ __device__ __forceinline__ void sgd_epilogue_chunk(const GemmParams& p, size_t e
     for (int j = 0; j < 32; ++j) {
       if (col0 + j < p.N) {
         float mv = m != nullptr ? m[j] : 0.f;
-        const float wv = sgd_update(h, w[j], __fadd_rn(0.f, v[j]), mv, m != nullptr, nest);
+        const float gj = __fadd_rn(0.f, v[j]);
+        const float wv = PROX ? sgd_update_prox(h, w[j], gj, a[j], mv, m != nullptr, nest)
+                              : sgd_update(h, w[j], gj, mv, m != nullptr, nest);
         w[j] = wv;
         if (m != nullptr) m[j] = mv;
         if (wb != nullptr) wb[j] = __float2bfloat16_rn(wv);
@@ -457,8 +467,9 @@ __device__ __forceinline__ void s2_load_ktile(const CUtensorMap* tmA, const CUte
 // no col2im); 4 = implicit dgrad of a stride-2 convolution, one parity class of dx pixels per group of M tiles (see
 // s2_class).  See csrc/im2col_tma.cu for the tensor maps.
 // SGD: optimizer epilogue instantiation (weight gradients only) -- every other GEMM keeps the plain epilogue.
+// PROX (with SGD): the FedProx form of that epilogue.
 // AFFINE: eval-mode BatchNorm epilogue instantiation (affine_chunk, forward convolutions in evaluation).
-template <int BN, int STAGES, int CONV = 0, bool SGD = false, bool AFFINE = false>
+template <int BN, int STAGES, int CONV = 0, bool SGD = false, bool AFFINE = false, bool PROX = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                          const GemmParams p) {
@@ -618,7 +629,8 @@ gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
                      static_cast<size_t>(bz_inner) * p.d_inner) * elt;
     const bool vec_ok = ((reinterpret_cast<uintptr_t>(p.D) & 15) == 0) && ((p.ldd * elt) % 16 == 0);
     const bool sgd_vec = SGD && (p.ldd % 4 == 0) &&
-                         ((reinterpret_cast<uintptr_t>(p.sgd_theta) | reinterpret_cast<uintptr_t>(p.sgd_mom)) & 15) == 0 &&
+                         ((reinterpret_cast<uintptr_t>(p.sgd_theta) | reinterpret_cast<uintptr_t>(p.sgd_mom) |
+                           (PROX ? reinterpret_cast<uintptr_t>(p.sgd_anchor) : 0)) & 15) == 0 &&
                          (reinterpret_cast<uintptr_t>(p.sgd_wb) & 7) == 0;
     // fused BatchNorm statistics: per row quarter column sums, [4 quarters][2 * BN] floats
     float* sstat = cstat + q * 2 * BN;
@@ -645,7 +657,7 @@ gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       }
       const bool full = (col0 + 32 <= p.N);
       if constexpr (SGD) {
-        sgd_epilogue_chunk(p, static_cast<size_t>(row) * p.ldd + col0, col0, v, sgd_vec);
+        sgd_epilogue_chunk<PROX>(p, static_cast<size_t>(row) * p.ldd + col0, col0, v, sgd_vec);
         continue;
       }
       if (p.atomic_out) {
@@ -1144,7 +1156,7 @@ static int clamp_bn(int bn) { return bn > 128 ? 128 : bn; }
 
 static void set_sgd_epilogue(GemmParams& p, const B200SgdEpilogue& s) {
   p.sgd_hyper = s.hyper; p.sgd_theta = s.theta; p.sgd_wb = reinterpret_cast<__nv_bfloat16*>(s.theta_bf16);
-  p.sgd_mom = s.mom; p.sgd_nesterov = s.nesterov;
+  p.sgd_mom = s.mom; p.sgd_nesterov = s.nesterov; p.sgd_anchor = s.anchor;
 }
 
 static void set_affine_epilogue(GemmParams& p, const B200AffineEpilogue& a) {
@@ -1160,21 +1172,29 @@ static bool affine_ok(const B200AffineEpilogue& a, int N) {
          (a.residual == nullptr || (a.ldr % 8 == 0 && a.ldr >= N));
 }
 
-template <int BN, int STAGES, int CONV = 0, bool SGD = false, bool AFFINE = false>
+template <int BN, int STAGES, int CONV = 0, bool SGD = false, bool AFFINE = false, bool PROX = false>
 static int launch_fixed(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, dim3 grid,
                       cudaStream_t stream) {
   constexpr int smem = STAGES * SmemLayout<BN>::STAGE_BYTES + 2 * STAGES * 8 + 8 * BN * 4 + 1024;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD, AFFINE>,
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD, AFFINE, PROX>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return static_cast<int>(e);
     configured = true;
   }
-  cudaError_t le = launch_pdl(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD, AFFINE>, grid, GEMM_THREADS, smem, stream,
+  cudaError_t le = launch_pdl(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD, AFFINE, PROX>, grid, GEMM_THREADS, smem, stream,
                               ta, tb, p);
   if (le != cudaSuccess) return static_cast<int>(le);
   return static_cast<int>(cudaGetLastError());
+}
+
+// the optimizer-epilogue instantiation, in its FedProx form when the step has an anchor
+template <int BN, int STAGES, int CONV>
+static int launch_fixed_sgd(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, dim3 grid,
+                            cudaStream_t stream) {
+  return p.sgd_anchor != nullptr ? launch_fixed<BN, STAGES, CONV, true, false, true>(ta, tb, p, grid, stream)
+                                 : launch_fixed<BN, STAGES, CONV, true>(ta, tb, p, grid, stream);
 }
 
 template <int BN, int STAGES>
@@ -1361,8 +1381,8 @@ extern "C" int b200_gemm_bf16(const void* a, const void* b, void* d, const float
   // little shared memory
   if (sgd != nullptr) {
     if (bn == 128)
-      return shallow ? launch_fixed<128, 3, 0, true>(ta, tb, p, grid, stream) : launch_fixed<128, 6, 0, true>(ta, tb, p, grid, stream);
-    return shallow ? launch_fixed<64, 4, 0, true>(ta, tb, p, grid, stream) : launch_fixed<64, 8, 0, true>(ta, tb, p, grid, stream);
+      return shallow ? launch_fixed_sgd<128, 3, 0>(ta, tb, p, grid, stream) : launch_fixed_sgd<128, 6, 0>(ta, tb, p, grid, stream);
+    return shallow ? launch_fixed_sgd<64, 4, 0>(ta, tb, p, grid, stream) : launch_fixed_sgd<64, 8, 0>(ta, tb, p, grid, stream);
   }
   if (bn == 128) return shallow ? launch_fixed<128, 3>(ta, tb, p, grid, stream) : launch_fixed<128, 6>(ta, tb, p, grid, stream);
   return shallow ? launch_fixed<64, 4>(ta, tb, p, grid, stream) : launch_fixed<64, 8>(ta, tb, p, grid, stream);
@@ -1612,8 +1632,8 @@ extern "C" int b200_conv_igemm_wgrad(const void* dy, const void* x, float* dw, i
   p.conv_taps = KH * KW; p.conv_ncol = Cin;
   dim3 grid((Kc + bn - 1) / bn, (Cout + BM - 1) / BM, split_k);
   if (sgd != nullptr) {
-    if (bn == 128) return launch_fixed<128, 6, 2, true>(ta, tb, p, grid, stream);
-    return launch_fixed<64, 8, 2, true>(ta, tb, p, grid, stream);
+    if (bn == 128) return launch_fixed_sgd<128, 6, 2>(ta, tb, p, grid, stream);
+    return launch_fixed_sgd<64, 8, 2>(ta, tb, p, grid, stream);
   }
   if (bn == 128) return launch_fixed<128, 6, 2>(ta, tb, p, grid, stream);
   return launch_fixed<64, 8, 2>(ta, tb, p, grid, stream);

@@ -11,14 +11,15 @@ extern "C" {
 
 // Optimizer epilogue of a weight-gradient GEMM: instead of accumulating the gradient into D, apply the SGD step to the
 // parameters in place.  theta / theta_bf16 / mom point at the element that D[0, 0] would address and are indexed like
-// D (same ldd).  hyper = device float[4] as for b200_fused_sgd.  A launcher that cannot apply it returns
-// B200_SGD_EPILOGUE_DECLINED and touches nothing; the caller then accumulates the gradient as usual.
+// D (same ldd).  hyper = device float[4] as for b200_fused_sgd (float[5] with an anchor).  A launcher that cannot apply
+// it returns B200_SGD_EPILOGUE_DECLINED and touches nothing; the caller then accumulates the gradient as usual.
 struct B200SgdEpilogue {
   float* theta;
   void* theta_bf16;                 // or nullptr
   float* mom;                       // or nullptr (no momentum buffer)
   const float* hyper;
   int nesterov;
+  const float* anchor;              // FedProx anchor (global model), indexed like theta, or nullptr (no proximal term)
 };
 #define B200_SGD_EPILOGUE_DECLINED (-6)
 
@@ -79,15 +80,17 @@ int b200_gemm_simt(const void* a, const void* b, void* d, const float* bias, int
                    float alpha, cudaStream_t stream);
 
 // ---- elementwise.cu
-// hyper = device float[4] {lr, momentum, weight_decay, dampening}
+// hyper = device float[4] {lr, momentum, weight_decay, dampening}; with prox_anchor != nullptr float[5], the fifth being
+// the FedProx coefficient mu of the term mu * (w - prox_anchor) added to the gradient (prox_anchor indexed like w)
 // wire_slot != nullptr: also emit the client's wire copy for the round-end collective (see SgdPack in elementwise.cu)
 int b200_fused_sgd(float* w, float* g, float* mom, void* w_bf16, long long n, const float* hyper, int zero_grad,
                    int nesterov, const unsigned long long* wire_slot, const float* pack_global,
-                   const float* pack_scale, long long n_pack, int wire_fp32, cudaStream_t stream);
+                   const float* pack_scale, long long n_pack, int wire_fp32, const float* prox_anchor,
+                   cudaStream_t stream);
 // the same step over a device table of n_seg arena chunks {offset, length, kind} (int64 [n_seg][3]); kind 0: with a
 // gradient (zeroed afterwards), kind 1: gradient identically zero (never read)
 int b200_fused_sgd_segments(float* w, float* g, float* mom, void* w_bf16, const long long* segments, int n_seg,
-                            const float* hyper, int nesterov, cudaStream_t stream);
+                            const float* hyper, int nesterov, const float* prox_anchor, cudaStream_t stream);
 // logical-client fold: acc (+)= nk * (theta - global) [+ reset of the replica]; mode 2: theta = global + acc * nk
 int b200_fold_client(float* acc, float* theta, const float* global_w, void* w_bf16, float* mom, long long n_mom, long long n,
                      float nk, int mode, int reset, cudaStream_t stream);

@@ -77,7 +77,7 @@ def make_gpu_worker(app, model, host: str, port: int, cfg: FederationConfig):
     return GpuExperimentWorker(app, model, host, device=dev, shard_fn=lambda: (X, y), backend=cfg.backend,
                                wire_dtype=cfg.wire_dtype, momentum=cfg.momentum, port=port,
                                heartbeat_time=cfg.heartbeat_time,
-                               train_kwargs={"lr": cfg.lr, "batch_size": cfg.batch_size})
+                               train_kwargs={"lr": cfg.lr, "batch_size": cfg.batch_size, "prox_mu": cfg.prox_mu})
 
 
 def make_app(role: str, host: str, port: int, cfg: Optional[FederationConfig] = None) -> web.Application:
@@ -96,7 +96,7 @@ def make_app(role: str, host: str, port: int, cfg: Optional[FederationConfig] = 
     elif role == "worker":
         worker = LinearTestWorker(
             app, model, host, port=port, heartbeat_time=cfg.heartbeat_time,
-            train_kwargs={"lr": cfg.lr, "batch_size": cfg.batch_size},
+            train_kwargs={"lr": cfg.lr, "batch_size": cfg.batch_size, "prox_mu": cfg.prox_mu},
             seed=(cfg.seed * 1000 + port) if cfg.seed else None)
         app["worker"] = worker
     else:
@@ -115,7 +115,10 @@ def main(argv=None) -> None:
     ns = parser.parse_args(argv)
     logging.basicConfig(level=logging.INFO if ns.verbose else logging.WARNING,
                         format="%(asctime)s %(name)s %(message)s")
-    cfg = FederationConfig.from_args(ns)
+    try:
+        cfg = FederationConfig.from_args(ns)
+    except ValueError as exc:
+        parser.error(str(exc))
     app = make_app(ns.role, ns.host, ns.port, cfg)
     web.run_app(app, host=ns.bind, port=ns.port, print=print if ns.verbose else None)
 

@@ -30,6 +30,7 @@ class FederatedModule(nn.Module):
     default_batch_size = 32
     default_momentum = 0.0
     default_weight_decay = 0.0
+    default_prox_mu = 0.0          # FedProx coefficient (0: plain SGD)
 
     def signature(self):
         return tuple((k, *v.shape) for k, v in self.state_dict().items())
@@ -47,6 +48,7 @@ class FederatedModule(nn.Module):
         batch_size = self.default_batch_size if batch_size is None else batch_size
         kw.setdefault("momentum", self.default_momentum)
         kw.setdefault("weight_decay", self.default_weight_decay)
+        kw.setdefault("prox_mu", self.default_prox_mu)
         trainer = getattr(self, "_graphed_trainer", None)
         if X.is_cuda and trainer is not None:
             return trainer.run(X, y, n_epoch=n_epoch, lr=lr, batch_size=batch_size, **kw)

@@ -26,7 +26,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from ..metrics import phase
-from ..train import GraphedLocalSGD, PortableLocalSGD
+from ..train import GraphedLocalSGD, PortableLocalSGD, check_prox_mu
 from .arena import ParamArena
 from .fedavg import FedAvgSession, NcclSession
 
@@ -62,7 +62,10 @@ class FederatedEngine:
                  lr: float = 0.05, batch_size: int = 128, momentum: float = 0.0, weight_decay: float = 0.0,
                  wire_dtype: str = "bf16", mode: str = "delta", n_ctas: Optional[int] = None, use_graph: bool = True,
                  logical_clients: int = 0, sample_k: Optional[int] = None, seed: int = 0, name: str = "exp",
-                 nvls: "bool | str" = "auto", tile_flags: bool = False):
+                 nvls: "bool | str" = "auto", tile_flags: bool = False, prox_mu: float = 0.0):
+        """``prox_mu > 0``: FedProx local training -- every step adds ``prox_mu * (theta - global_w)`` to the gradient,
+        ``global_w`` being the global model the round started from (for logical clients too: each starts from it)."""
+        prox_mu = check_prox_mu(prox_mu)
         self.device = torch.device(device)
         self.model = model
         self.name = name
@@ -101,7 +104,7 @@ class FederatedEngine:
         if self.k3:
             self.session.gate_first_conv(model.conv1)
             self.trainer.k3_join = self.sync
-        self.hp = dict(lr=lr, batch_size=batch_size, momentum=momentum, weight_decay=weight_decay)
+        self.hp = dict(lr=lr, batch_size=batch_size, momentum=momentum, weight_decay=weight_decay, prox_mu=prox_mu)
         self.n_rounds = 0
         self.logical_clients = logical_clients if logical_clients and logical_clients > self.world else 0
         self.sample_k = sample_k

@@ -16,6 +16,10 @@ Two executions of the same contract:
   the flat arena, so the optimizer takes at most one launch per step beyond the
   weight-gradient GEMM epilogues instead of one launch per tensor.  No host
   synchronisation inside an epoch.
+
+Every trainer takes ``prox_mu`` (FedProx, Li et al. 2020): the step adds
+``prox_mu * (w - w_global)`` to the gradient, ``w_global`` being the global model
+the round started from.  ``prox_mu = 0`` is plain SGD.
 """
 from __future__ import annotations
 
@@ -38,16 +42,36 @@ def _loss_fn(kind):
     raise ValueError("unknown loss {!r}".format(kind))
 
 
+def check_prox_mu(prox_mu: float) -> float:
+    """The FedProx coefficient as a float; ``ValueError`` unless it is a finite number >= 0."""
+    mu = float(prox_mu)
+    if not (0.0 <= mu < float("inf")):
+        raise ValueError("prox_mu must be a finite number >= 0, got {!r}".format(prox_mu))
+    return mu
+
+
+def _add_prox_term(params, anchors, prox_mu: float) -> None:
+    """FedProx: ``grad += prox_mu * (w - anchor)`` before the optimizer step (what the reference implementation does)."""
+    with torch.no_grad():
+        for p, a in zip(params, anchors):
+            if p.grad is not None:
+                p.grad.add_(p.detach() - a, alpha=prox_mu)
+
+
 def run_local_sgd(model: nn.Module, X: torch.Tensor, y: torch.Tensor, *, n_epoch: int = 32,
                   lr: float = 0.001, batch_size: int = 32, momentum: float = 0.0,
                   weight_decay: float = 0.0, loss: "str | Callable" = "mse",
                   verbose: bool = False, reshuffle_each_epoch: bool = False,
-                  generator: Optional[torch.Generator] = None) -> List[float]:
-    """Portable local SGD; returns the per-epoch mean loss."""
+                  generator: Optional[torch.Generator] = None, prox_mu: float = 0.0) -> List[float]:
+    """Portable local SGD; returns the per-epoch mean loss.  ``prox_mu > 0``: FedProx, anchored on the parameters as
+    they are on entry -- the global model the worker has just loaded."""
     criterion = _loss_fn(loss)
+    prox_mu = check_prox_mu(prox_mu)
     n = X.shape[0]
     nn.Module.train(model, True)
-    optimizer = torch.optim.SGD(model.parameters(), lr=lr, momentum=momentum,
+    params = list(model.parameters())
+    anchors = [p.detach().clone() for p in params] if prox_mu > 0 else None
+    optimizer = torch.optim.SGD(params, lr=lr, momentum=momentum,
                                 weight_decay=weight_decay)
     idxs = torch.randperm(n, generator=generator).to(X.device)
     loss_history: List[float] = []
@@ -64,6 +88,8 @@ def run_local_sgd(model: nn.Module, X: torch.Tensor, y: torch.Tensor, *, n_epoch
             loss_batch = criterion(output, target)
             batch_iter.update_loss(loss_batch)
             loss_batch.backward()
+            if anchors is not None:
+                _add_prox_term(params, anchors, prox_mu)
             optimizer.step()
         loss_history.append(batch_iter.loss)
     return loss_history
@@ -117,7 +143,8 @@ class GraphedLocalSGD:
 
     A model that offers ``explicit_step`` trains with it whenever it runs in bf16
     with the cross-entropy loss; MXFP8, MSE and models without one go through
-    autograd.  SGD runs in one of two places.  In a hand-scheduled step the
+    autograd.  ``run(prox_mu > 0)`` adds FedProx's pull toward ``arena.global_w`` in every
+    SGD kernel.  SGD runs in one of two places.  In a hand-scheduled step the
     split-K = 1 convolution weight-gradient GEMMs apply it in their epilogue and
     ``fused_sgd_segments`` updates the rest of the arena.  The epoch's last step
     (it also writes the upload copy), ragged eager steps and autograd steps run
@@ -148,7 +175,8 @@ class GraphedLocalSGD:
         self.graph_emits_wire = False
         dev = arena.device
         self.device = dev
-        self.hyper = torch.zeros(4, dtype=torch.float32, device=dev)
+        self.hyper = torch.zeros(5, dtype=torch.float32, device=dev)   # [lr, momentum, wd, dampening, prox_mu]
+        self.prox = False             # FedProx: every SGD kernel of the step reads the anchor arena.global_w
         self.loss_acc = torch.zeros(2, dtype=torch.float32, device=dev)
         self._graphs = {}           # (n, batch, x_shape, y_shape) -> captured epoch
         self._hyper_host = None
@@ -187,15 +215,16 @@ class GraphedLocalSGD:
             explicit = None            # the hand-scheduled step drives the bf16 conv kernels; MXFP8 convs go through autograd
         a = self.arena
         bf = a.theta_bf16
+        anchor = a.global_w if self.prox else None
         if explicit is not None and self.loss_kind in ("ce", "cross_entropy"):
             # hand-scheduled forward + loss + backward (no autograd engine): two-piece block gradients, parallel shortcut
             # branch; the loss kernel accumulates straight into the epoch's running sums
             if fuse_sgd and not emit_wire:
                 # the split-K = 1 convolution weight gradients apply SGD in their GEMM epilogue; one launch covers the rest
-                with self.bnn.SGD_EPI.open(a, self.hyper, self.nesterov) as epi:
+                with self.bnn.SGD_EPI.open(a, self.hyper, self.nesterov, prox=self.prox) as epi:
                     explicit(xb, yb, loss_acc=self.loss_acc, after_first_gemm=self._first_gemm_hook)
                 F.fused_sgd_segments(a.theta, a.grad, self.hyper, self._segment_table(epi.fused, epi.nograd),
-                                     a.momentum, bf, nesterov=self.nesterov)
+                                     a.momentum, bf, nesterov=self.nesterov, prox_anchor=anchor)
                 self.emitted_wire = False
                 return
             explicit(xb, yb, loss_acc=self.loss_acc, after_first_gemm=self._first_gemm_hook)
@@ -208,7 +237,8 @@ class GraphedLocalSGD:
         # one optimizer pass over the whole arena; the epoch's last step also emits the upload copy
         pack = self.pack if emit_wire else None
         F.fused_sgd(a.theta[: a.n_param], a.grad, self.hyper, a.momentum,
-                    bf[: a.n_param] if bf is not None else None, zero_grad=True, nesterov=self.nesterov, pack=pack)
+                    bf[: a.n_param] if bf is not None else None, zero_grad=True, nesterov=self.nesterov, pack=pack,
+                    prox_anchor=anchor[: a.n_param] if anchor is not None else None)
         self.emitted_wire = pack is not None
         if stats is not None:
             self.loss_acc.add_(stats)
@@ -223,8 +253,8 @@ class GraphedLocalSGD:
             table = self._seg_tables[key] = torch.tensor(segs, dtype=torch.int64).view(-1, 3).to(self.device)
         return table
 
-    def _set_hyper(self, lr, momentum, weight_decay, dampening=0.0):
-        vals = (float(lr), float(momentum), float(weight_decay), float(dampening))
+    def _set_hyper(self, lr, momentum, weight_decay, dampening=0.0, prox_mu=0.0):
+        vals = (float(lr), float(momentum), float(weight_decay), float(dampening), float(prox_mu))
         if vals != self._hyper_host:
             self.hyper.copy_(torch.tensor(vals, dtype=torch.float32))
             self._hyper_host = vals
@@ -391,17 +421,24 @@ class GraphedLocalSGD:
 
     def run(self, X, y, n_epoch: int = 1, lr: float = 0.001, batch_size: int = 32, momentum: float = 0.0,
             weight_decay: float = 0.0, reshuffle_each_epoch: bool = False, return_device: bool = False,
-            **_ignored):
+            prox_mu: float = 0.0, **_ignored):
+        """``prox_mu > 0``: FedProx toward ``arena.global_w``, the global model the round started from."""
         assert X.is_cuda, "GraphedLocalSGD needs a device-resident shard"
+        prox_mu = check_prox_mu(prox_mu)
+        if prox_mu > 0 and self.arena.global_w is None:
+            raise ValueError("prox_mu > 0 needs the arena's global copy (ParamArena(keep_global=True))")
         nn.Module.train(self.model, True)
         n = X.shape[0]
         batch_size = min(batch_size, n)
         n_steps = n // batch_size
         tail = n - n_steps * batch_size
-        self._set_hyper(lr, momentum, weight_decay)
+        self._set_hyper(lr, momentum, weight_decay, prox_mu=prox_mu)
+        self.prox = prox_mu > 0
         if momentum and self.arena.momentum is None:
             self.arena.momentum = torch.zeros_like(self.arena.grad)
-        key = (n, batch_size, tuple(X.shape[1:]), tuple(y.shape[1:]), X.data_ptr(), y.data_ptr(), bool(momentum))
+        # the anchor pointer is baked into the captured launches; the coefficient is read from `hyper` at replay
+        key = (n, batch_size, tuple(X.shape[1:]), tuple(y.shape[1:]), X.data_ptr(), y.data_ptr(), bool(momentum),
+               self.prox)
         epoch_losses = torch.zeros(n_epoch, 2, dtype=torch.float32, device=self.device)
         if self.use_graph:
             ent = self._graphs.get(key)
@@ -458,12 +495,22 @@ class PortableLocalSGD:
         self.last_stats = {}
 
     def run(self, X, y, n_epoch: int = 1, lr: float = 0.001, batch_size: int = 32, momentum: float = 0.0,
-            weight_decay: float = 0.0, reshuffle_each_epoch: bool = False, return_device: bool = False, **_ignored):
+            weight_decay: float = 0.0, reshuffle_each_epoch: bool = False, return_device: bool = False,
+            prox_mu: float = 0.0, **_ignored):
+        """``prox_mu > 0``: FedProx toward ``arena.global_w``, the global model the round started from."""
         criterion = _loss_fn(self.loss_kind)
+        prox_mu = check_prox_mu(prox_mu)
         n = X.shape[0]
         batch_size = min(batch_size, n)
         nn.Module.train(self.model, True)
-        opt = torch.optim.SGD(self.model.parameters(), lr=lr, momentum=momentum, weight_decay=weight_decay)
+        a = self.arena
+        if prox_mu > 0 and a.global_w is None:
+            raise ValueError("prox_mu > 0 needs the arena's global copy (ParamArena(keep_global=True))")
+        params, anchors = [], []
+        for name, p in self.model.named_parameters():
+            params.append(p)
+            anchors.append(a._view(a.global_w, a.slots[name]) if prox_mu > 0 else None)
+        opt = torch.optim.SGD(params, lr=lr, momentum=momentum, weight_decay=weight_decay)
         perm = torch.randperm(n)
         out = torch.zeros(n_epoch, 2, dtype=torch.float32)
         steps = 1
@@ -480,6 +527,8 @@ class PortableLocalSGD:
                     tgt = tgt.reshape(pred.shape)
                 loss = criterion(pred.float() if tgt.dtype.is_floating_point else pred, tgt)
                 loss.backward()
+                if prox_mu > 0:
+                    _add_prox_term(params, anchors, prox_mu)
                 opt.step()
                 out[e, 0] += float(loss.detach())
                 if not tgt.dtype.is_floating_point:
