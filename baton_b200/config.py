@@ -28,6 +28,10 @@ class FederationConfig:
     momentum: float = 0.0
     weight_decay: float = 0.0
     prox_mu: float = 0.0               # FedProx proximal coefficient (0: FedAvg's plain local SGD)
+    dp_clip: float = 0.0               # DP-FedAvg: L2 clip norm of a client's update (0: DP off)
+    dp_noise_multiplier: float = 0.0   # DP-FedAvg: noise std on the sum of clipped updates, in units of dp_clip
+    dp_delta: float = 1e-5             # DP-FedAvg: delta of the (epsilon, delta) the manager reports
+    dp_seed: Optional[int] = None      # DP-FedAvg noise key (None: secret random; an explicit key is for tests only)
     partition: str = "iid"             # iid | label_skew | dirichlet
     alpha: float = 0.1                 # Dirichlet concentration
     samples_per_client: int = 4096
@@ -42,6 +46,17 @@ class FederationConfig:
     def __post_init__(self):
         if not (0.0 <= float(self.prox_mu) < float("inf")):
             raise ValueError("prox_mu must be a finite number >= 0, got {!r}".format(self.prox_mu))
+        from .parallel.dp import check_dp
+        check_dp(self.dp_clip, self.dp_noise_multiplier)
+        if not (0.0 < float(self.dp_delta) < 1.0):
+            raise ValueError("dp_delta must lie in (0, 1), got {!r}".format(self.dp_delta))
+
+    def dp_config(self):
+        """The :class:`~baton_b200.parallel.dp.DPConfig` of these fields, or None when DP is off (``dp_clip == 0``)."""
+        if self.dp_clip <= 0.0:
+            return None
+        from .parallel.dp import DPConfig
+        return DPConfig(self.dp_clip, self.dp_noise_multiplier, seed=self.dp_seed)
 
     def to_json(self) -> str:
         return json.dumps(asdict(self), sort_keys=True)
@@ -61,7 +76,7 @@ class FederationConfig:
             flag = "--" + f.name.replace("_", "-")
             default = f.default
             typ = type(default) if default is not None else None
-            if f.name in ("sample_k",):
+            if f.name in ("sample_k", "dp_seed"):
                 typ = int
             if f.name in ("round_timeout",):
                 typ = float

@@ -38,6 +38,7 @@ from ..metrics import RoundMetrics
 from ..parallel import wire
 from ..parallel.aggregate import fedavg_loss_history
 from ..parallel.dataplane import ManagerPlane, make_manager_plane
+from ..parallel.dp import RDPAccountant
 from ..utils.misc import SYSTEM_CLOCK, Clock, json_clean
 from .client_manager import ClientManager
 from .update_manager import UpdateException, UpdateManager
@@ -80,14 +81,23 @@ class Experiment:
                  sample_fraction: Optional[float] = None, seed: Optional[int] = None,
                  round_timeout: Optional[float] = None, checkpoint_dir: Optional[str] = None,
                  checkpoint_every: int = 1, resume: bool = False, clock: Clock = SYSTEM_CLOCK,
-                 trusted_peers: bool = False):
+                 trusted_peers: bool = False, dp=None, dp_delta: float = 1e-5):
+        """``dp`` (a :class:`~baton_b200.parallel.dp.DPConfig`): aggregate with DP-FedAvg -- on the manager for the
+        ``http`` plane, on the seats for the seated planes (the plan carries the clip norm, noise and key) -- and
+        account every aggregated round at ``q`` = participants / registered clients; ``/metrics`` reports the
+        ``(epsilon, dp_delta)`` spent."""
         self.name = name
         self.model = model
         self.app = app
         self.clock = clock
         self.client_manager = ClientManager(name, app, client_ttl, clock=clock, seed=seed)
         self.update_manager = UpdateManager(name)
-        self.plane: ManagerPlane = make_manager_plane(dataplane)
+        self.plane: ManagerPlane = make_manager_plane(dataplane, dp=dp)
+        self.dp = dp
+        self.dp_delta = float(dp_delta)
+        self.dp_accountant = RDPAccountant(dp.noise_multiplier) if dp is not None else None
+        self._dp_q = 1.0
+        self._dp_clipped = [0, 0]            # client updates with s < 1, client updates with a known factor
         self.sample_k = sample_k
         self.sample_fraction = sample_fraction
         self.round_timeout = round_timeout
@@ -134,7 +144,19 @@ class Experiment:
         return web.json_response(json_clean(self.update_manager.state()))
 
     async def get_metrics(self, request: web.Request) -> web.Response:
-        return web.json_response(json_clean(self.metrics.summary()))
+        out = self.metrics.summary()
+        if self.dp is not None:
+            out["dp"] = self.dp_summary()
+        return web.json_response(json_clean(out))
+
+    def dp_summary(self) -> dict:
+        """Privacy spent so far: ``epsilon`` at ``delta`` over ``rounds`` aggregated DP rounds; ``clipped_fraction`` is
+        the share of client updates with ``s < 1`` where the manager saw the factors (``http`` plane), else None."""
+        eps, _ = self.dp_accountant.get_privacy_spent(self.dp_delta)
+        known = self._dp_clipped[1]
+        return {"clip": self.dp.clip, "noise_multiplier": self.dp.noise_multiplier,
+                "rounds": self.dp_accountant.rounds, "epsilon": eps, "delta": self.dp_delta,
+                "clipped_fraction": (self._dp_clipped[0] / known) if known else None}
 
     async def get_state_dict(self, request: web.Request) -> web.Response:
         """Pickled global ``state_dict`` (the checkpoint layout), refreshed from
@@ -223,6 +245,7 @@ class Experiment:
         k = self.sample_k if sample_k is None else sample_k
         chosen = self.client_manager.sample(k, self.sample_fraction)
         self.update_manager.update_meta["sampled"] = list(chosen)
+        self._dp_q = len(chosen) / float(len(self.client_manager))     # DP accounting: sampling rate of this round
         if self.plane.carries_tensors:
             await self.pull_global()
         body = self.plane.round_start_message(self.model, update_name, n_epoch, extra)
@@ -359,6 +382,12 @@ class Experiment:
                 aggregated = False
             finally:
                 self.update_manager.end_update()
+            if aggregated and self.dp_accountant is not None:
+                self.dp_accountant.step(self._dp_q)
+                factors = getattr(self.plane, "last_clip_factors", None)
+                if factors:
+                    self._dp_clipped[0] += sum(1 for s in factors if s < 1.0)
+                    self._dp_clipped[1] += len(factors)
             if not N:
                 log.info("no responses for %s", update_name)
                 self.metrics.add(update_name=update_name, n_clients=0, n_samples=0,

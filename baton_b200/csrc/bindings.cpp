@@ -447,13 +447,14 @@ void fedavg_allreduce(const std::vector<int64_t>& wire_ptrs, const std::vector<i
                       bool counts_from_flags, int64_t alive_mask, int64_t rank, int64_t world, int64_t wire_kind,
                       bool delta, bool use_nvls, int64_t epoch, const std::optional<at::Tensor>& tile_flags,
                       int64_t flag_value, int64_t tile_elems, int64_t n_ctas, int64_t timeout_log2,
-                      const std::optional<at::Tensor>& status, const std::optional<at::Tensor>& phase_ns, bool prepacked) {
+                      const std::optional<at::Tensor>& status, const std::optional<at::Tensor>& phase_ns, bool prepacked,
+                      const std::vector<int64_t>& clip_page_ptrs, double dp_noise_std, int64_t dp_seed, int64_t dp_round) {
   CHECK_CUDA(theta);
   TORCH_CHECK(world <= B200_MAX_RANKS && static_cast<int64_t>(wire_ptrs.size()) == world &&
               static_cast<int64_t>(pad_ptrs.size()) == world && static_cast<int64_t>(n_samples.size()) == world);
   TORCH_CHECK(theta.scalar_type() == at::kFloat && theta.is_contiguous());
   const c10::cuda::CUDAGuard guard(theta.device());
-  FedAvgArgs a = {};
+  FedAvgDPArgs a = {};
   for (int64_t k = 0; k < world; ++k) {
     a.wire[k] = reinterpret_cast<void*>(wire_ptrs[k]);
     a.pads[k] = reinterpret_cast<unsigned long long*>(pad_ptrs[k]);
@@ -493,9 +494,51 @@ void fedavg_allreduce(const std::vector<int64_t>& wire_ptrs, const std::vector<i
     TORCH_CHECK(phase_ns->scalar_type() == at::kLong && phase_ns->numel() >= 16, "phase_ns: int64[16]");
     a.phase_ns = reinterpret_cast<unsigned long long*>(phase_ns->data_ptr<int64_t>());
   }
+  // DP-FedAvg: one clip page per rank (empty = off); the seed is the 64-bit Philox key, passed as its int64 bit pattern
+  const bool dp = !clip_page_ptrs.empty();
+  if (dp) {
+    TORCH_CHECK(static_cast<int64_t>(clip_page_ptrs.size()) == world, "DP: one clip page per rank");
+    for (int64_t k = 0; k < world; ++k) a.clip_page[k] = reinterpret_cast<const float*>(clip_page_ptrs[k]);
+    a.noise_std = static_cast<float>(dp_noise_std);
+    a.seed = static_cast<unsigned long long>(dp_seed);
+    a.round = static_cast<uint32_t>(dp_round);
+    TORCH_CHECK(delta && !use_nvls, "DP needs delta mode on peer loads");
+  }
   TORCH_CHECK(!delta || a.global_w != nullptr, "delta mode needs the global copy");
   TORCH_CHECK(!use_nvls || a.wire_mc != nullptr, "NVLS mode needs the multicast address");
-  check(b200_fedavg_allreduce(&a, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce");
+  check(dp ? b200_fedavg_allreduce_dp(&a, static_cast<int>(n_ctas), cur_stream())
+           : b200_fedavg_allreduce(&a, static_cast<int>(n_ctas), cur_stream()),
+        "fedavg_allreduce");
+}
+
+// DP clip factor of theta against global_w over theta's n elements; work: int64 [DP_WORK_WORDS], zeroed once
+void dp_clip_factor(const at::Tensor& theta, const at::Tensor& global_w, double clip, at::Tensor work, at::Tensor s_out,
+                    at::Tensor norm_out, int64_t s_copy, const std::optional<at::Tensor>& nonfinite) {
+  CHECK_CUDA(theta); CHECK_CUDA(global_w); CHECK_CUDA(work); CHECK_CUDA(s_out); CHECK_CUDA(norm_out);
+  TORCH_CHECK(theta.scalar_type() == at::kFloat && global_w.scalar_type() == at::kFloat && theta.is_contiguous() &&
+              global_w.is_contiguous() && global_w.numel() >= theta.numel(), "dp_clip_factor: fp32 theta / global_w");
+  TORCH_CHECK(work.scalar_type() == at::kLong && work.numel() >= B200_DP_WORK_WORDS, "dp_clip_factor: int64 work");
+  TORCH_CHECK(s_out.scalar_type() == at::kFloat && norm_out.scalar_type() == at::kFloat && s_out.numel() >= 1 &&
+              norm_out.numel() >= 1, "dp_clip_factor: fp32 outputs");
+  TORCH_CHECK(!nonfinite.has_value() || nonfinite->scalar_type() == at::kInt, "dp_clip_factor: int32 counter");
+  const c10::cuda::CUDAGuard guard(theta.device());
+  check(b200_dp_clip_factor(theta.data_ptr<float>(), global_w.data_ptr<float>(), theta.numel(), static_cast<float>(clip),
+                            work.data_ptr(), s_out.data_ptr<float>(), norm_out.data_ptr<float>(),
+                            reinterpret_cast<float*>(s_copy), opt_ptr<int>(nonfinite), cur_stream()),
+        "dp_clip_factor");
+}
+
+void fold_client_scaled(at::Tensor acc, at::Tensor theta, const at::Tensor& global_w, const std::optional<at::Tensor>& wb,
+                        const std::optional<at::Tensor>& mom, const at::Tensor& s, bool first, bool reset) {
+  CHECK_CUDA(acc); CHECK_CUDA(s);
+  TORCH_CHECK(acc.scalar_type() == at::kFloat && theta.scalar_type() == at::kFloat && global_w.scalar_type() == at::kFloat &&
+              s.scalar_type() == at::kFloat && s.numel() >= 1);
+  TORCH_CHECK(acc.numel() == theta.numel() && theta.numel() == global_w.numel());
+  const c10::cuda::CUDAGuard guard(acc.device());
+  check(b200_fold_client_scaled(acc.data_ptr<float>(), theta.data_ptr<float>(), global_w.data_ptr<float>(),
+                                opt_ptr<void>(wb), opt_ptr<float>(mom), mom.has_value() && mom->defined() ? mom->numel() : 0,
+                                theta.numel(), s.data_ptr<float>(), first, reset, cur_stream()),
+        "fold_client_scaled");
 }
 
 void flag_barrier(const std::vector<int64_t>& pad_ptrs, int64_t rank, int64_t world, int64_t alive_mask, int64_t epoch,
@@ -784,6 +827,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("embedding_bwd", &embedding_bwd);
   m.def("fedavg_allreduce", &fedavg_allreduce);
   m.def("flag_barrier", &flag_barrier);
+  m.attr("DP_WORK_WORDS") = B200_DP_WORK_WORDS;
+  m.def("dp_clip_factor", &dp_clip_factor);
+  m.def("fold_client_scaled", &fold_client_scaled);
   m.def("im2col", &im2col);
   m.def("col2im", &col2im);
   m.def("maxpool", &maxpool);

@@ -38,6 +38,7 @@
 #include "ptx.cuh"
 #include "launch.h"
 #include "mx.cuh"
+#include "dp.cuh"
 
 namespace b200 {
 
@@ -191,12 +192,11 @@ __device__ __forceinline__ void phase_stamp(const FedAvgArgs& a, int slot) {
 #endif
 }
 
-template <int WIRE>
-// One 512-thread CTA per SM, capped at 96 registers per thread (48 K of the SM's 64 K): the rest of the register file
-// stays available to small kernels of the NEXT round (batch gather, im2col, the flag-gated weight staging of
-// bcast_gemm) that are launched on the compute stream while this kernel is still running on its side stream -- and
-// a flag-gated consumer that became resident first can never keep this (cooperatively launched) grid from fitting.
-__global__ void __maxnreg__(96) fedavg_allreduce_kernel(const __grid_constant__ FedAvgArgs a) {
+// DP: DP-FedAvg (see launch.h / DESIGN.md): w_k = n_k s_k / N with s_k from rank k's clip page, and the owner of a tile
+// adds sigma C / N * z[i] to its fp32 sum before the cast.  The loss and the integer side arena keep the weights n_k / N.
+// The whole round; Args is FedAvgDPArgs when DP.
+template <int WIRE, bool DP, typename Args>
+__device__ __forceinline__ void fedavg_round(const Args& a) {
   using W = Wire<WIRE>;
   constexpr int VEC = W::VEC;
   constexpr bool SCALED = W::SCALED;
@@ -208,6 +208,7 @@ __global__ void __maxnreg__(96) fedavg_allreduce_kernel(const __grid_constant__ 
   __shared__ float s_w[B200_MAX_RANKS];
   __shared__ uint32_t s_payload[B200_MAX_RANKS];  // indexed by rank
   __shared__ float s_inv_total;
+  __shared__ float s_part[DP ? B200_MAX_RANKS : 1];   // DP: participation weights n_k / N (loss, integer arena)
   int A = 0, my_pos = -1;
   for (int k = 0; k < a.world; ++k)
     if ((a.alive_mask >> k) & 1u) {
@@ -311,6 +312,13 @@ __global__ void __maxnreg__(96) fedavg_allreduce_kernel(const __grid_constant__ 
       total += nk;
     }
     const float inv = total > 0.f ? 1.f / total : 0.f;
+    if constexpr (DP) {
+      for (int k = 0; k < A; ++k) {
+        s_part[k] = s_w[k] * inv;
+        // a non-participant's page may hold an older round's factor: only read it for n_k != 0
+        s_w[k] = s_w[k] != 0.f ? s_w[k] * *reinterpret_cast<const volatile float*>(a.clip_page[s_rank[k]]) : 0.f;
+      }
+    }
     for (int k = 0; k < A; ++k) s_w[k] *= inv;
     s_inv_total = inv;
   }
@@ -393,6 +401,17 @@ __global__ void __maxnreg__(96) fedavg_allreduce_kernel(const __grid_constant__ 
         for (int u = 0; u < U; ++u) {
           const int i = i0 + u * STEP;
           const bool valid = i < len;
+          if constexpr (DP) {
+            if (valid) {
+              const float ns = a.noise_std * s_inv_total;
+#pragma unroll
+              for (int j = 0; j < VEC; j += 4) {
+                const float4 z = dp_normal4(a.seed, a.round, static_cast<unsigned long long>(base + i + j) >> 2);
+                acc[u][j] = fmaf(ns, z.x, acc[u][j]); acc[u][j + 1] = fmaf(ns, z.y, acc[u][j + 1]);
+                acc[u][j + 2] = fmaf(ns, z.z, acc[u][j + 2]); acc[u][j + 3] = fmaf(ns, z.w, acc[u][j + 3]);
+              }
+            }
+          }
           float inv = 1.f;
           int e = 0;
           if constexpr (SCALED) {
@@ -425,7 +444,11 @@ __global__ void __maxnreg__(96) fedavg_allreduce_kernel(const __grid_constant__ 
     for (int e = threadIdx.x; e < a.n_loss; e += FEDAVG_THREADS) {
       float acc = 0.f;
       for (int k = 0; k < A; ++k)
-        if (s_w[k] != 0.f) acc = fmaf(s_w[k], *reinterpret_cast<volatile float*>(s_loss[k] + e), acc);
+        if constexpr (DP) {
+          if (s_part[k] != 0.f) acc = fmaf(s_part[k], *reinterpret_cast<volatile float*>(s_loss[k] + e), acc);
+        } else if (s_w[k] != 0.f) {
+          acc = fmaf(s_w[k], *reinterpret_cast<volatile float*>(s_loss[k] + e), acc);
+        }
       a.loss_out[e] = acc;
     }
   }
@@ -505,7 +528,7 @@ __global__ void __maxnreg__(96) fedavg_allreduce_kernel(const __grid_constant__ 
     for (int i = threadIdx.x; i < a.n_int; i += FEDAVG_THREADS) {
       long long m = a.int_local[i];
       for (int k = 0; k < A; ++k)
-        if (s_w[k] != 0.f) {
+        if ((DP ? s_part[k] : s_w[k]) != 0.f) {
           const long long v = *reinterpret_cast<volatile long long*>(s_int[k] + i);
           m = v > m ? v : m;
         }
@@ -521,6 +544,19 @@ __global__ void __maxnreg__(96) fedavg_allreduce_kernel(const __grid_constant__ 
   phase_stamp(a, 6);
 }
 
+// One 512-thread CTA per SM, capped at 96 registers per thread (48 K of the SM's 64 K): the rest of the register file
+// stays available to small kernels of the NEXT round (batch gather, im2col, the flag-gated weight staging of
+// bcast_gemm) that are launched on the compute stream while this kernel is still running on its side stream -- and
+// a flag-gated consumer that became resident first can never keep this (cooperatively launched) grid from fitting.
+template <int WIRE>
+__global__ void __maxnreg__(96) fedavg_allreduce_kernel(const __grid_constant__ FedAvgArgs a) {
+  fedavg_round<WIRE, false>(a);
+}
+template <int WIRE>
+__global__ void __maxnreg__(96) fedavg_allreduce_dp_kernel(const __grid_constant__ FedAvgDPArgs a) {
+  fedavg_round<WIRE, true>(a);
+}
+
 // stand-alone cross-GPU barrier on the pads (one CTA): fences host-side phases
 __global__ void flag_barrier_kernel(FedAvgArgs a, int slot) {
   const int t = threadIdx.x;
@@ -534,6 +570,84 @@ __global__ void flag_barrier_kernel(FedAvgArgs a, int slot) {
   }
 }
 
+// ---------------------------------------------------------------- DP clip factor and clipped logical-client fold
+// ||theta - global||^2 over [0, n): a FIXED grid of B200_DP_NORM_BLOCKS CTAs (independent of the SM count), fp64
+// throughout (differences and squares too, so no finite update overflows to a non-finite norm), one slot of `work` per
+// CTA, and the last CTA to finish sums the slots in index order -- two launches on the same data give the same bits.  work[B200_DP_NORM_BLOCKS] is the arrival counter (reset by the last CTA).
+constexpr int DP_NORM_THREADS = 256;
+__global__ void __launch_bounds__(DP_NORM_THREADS)
+dp_clip_factor_kernel(const float* __restrict__ theta, const float* __restrict__ global_w, long long n, float clip,
+                      unsigned long long* __restrict__ work, float* s_out, float* norm_out, float* s_copy, int* nonfinite) {
+  __shared__ double red[DP_NORM_THREADS / 32];
+  __shared__ bool last;
+  const long long nv = n >> 2;
+  double d = 0.0;
+  for (long long i = blockIdx.x * static_cast<long long>(DP_NORM_THREADS) + threadIdx.x; i < nv;
+       i += static_cast<long long>(B200_DP_NORM_BLOCKS) * DP_NORM_THREADS) {
+    const float4 t = __ldcs(reinterpret_cast<const float4*>(theta) + i);
+    const float4 g = __ldcs(reinterpret_cast<const float4*>(global_w) + i);
+    const double dx = static_cast<double>(t.x) - g.x, dy = static_cast<double>(t.y) - g.y;
+    const double dz = static_cast<double>(t.z) - g.z, dw = static_cast<double>(t.w) - g.w;
+    d = fma(dx, dx, d); d = fma(dy, dy, d); d = fma(dz, dz, d); d = fma(dw, dw, d);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = d;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double b = 0.0;
+    for (int w = 0; w < DP_NORM_THREADS / 32; ++w) b += red[w];
+    reinterpret_cast<double*>(work)[blockIdx.x] = b;
+    __threadfence();
+    last = atomicAdd(work + B200_DP_NORM_BLOCKS, 1ull) == B200_DP_NORM_BLOCKS - 1;
+  }
+  __syncthreads();
+  if (!last || threadIdx.x != 0) return;
+  __threadfence();
+  double sq = 0.0;
+  for (int b = 0; b < B200_DP_NORM_BLOCKS; ++b) sq += reinterpret_cast<const volatile double*>(work)[b];
+  work[B200_DP_NORM_BLOCKS] = 0ull;
+  const double norm = sqrt(sq);
+  float s;
+  if (!isfinite(norm)) {
+    s = 0.f;
+    if (nonfinite != nullptr) atomicAdd(nonfinite, 1);
+  } else {
+    s = norm > static_cast<double>(clip) ? static_cast<float>(static_cast<double>(clip) / norm) : 1.f;
+  }
+  s_out[0] = s;
+  if (s_copy != nullptr) s_copy[0] = s;
+  norm_out[0] = static_cast<float>(norm);
+}
+
+// acc (+)= s * (theta - global) with s = *s_dev (written by dp_clip_factor_kernel just before), and the replica reset of
+// fold_client_kernel (elementwise.cu), which this mirrors; kept separate so that kernel's instruction stream is unchanged.
+// Unlike it, this one is launched without programmatic dependent launch: it follows the norm kernel, a plain launch.
+// s == 0 (non-finite update): the client adds nothing, and its NaNs never reach acc.
+__global__ void __launch_bounds__(DP_NORM_THREADS)
+fold_client_scaled_kernel(float* __restrict__ acc, float* __restrict__ theta, const float* __restrict__ global_w,
+                          __nv_bfloat16* __restrict__ wb, float* __restrict__ mom, long long n_mom, long long n,
+                          const float* __restrict__ s_dev, int first, int reset) {
+  const float s = *s_dev;
+  const long long nv = n >> 2;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < nv;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float4 g = reinterpret_cast<const float4*>(global_w)[i];
+    const float4 t = reinterpret_cast<const float4*>(theta)[i];
+    float4 a = first ? make_float4(0.f, 0.f, 0.f, 0.f) : reinterpret_cast<const float4*>(acc)[i];
+    if (s != 0.f) {
+      a.x = fmaf(s, t.x - g.x, a.x); a.y = fmaf(s, t.y - g.y, a.y);
+      a.z = fmaf(s, t.z - g.z, a.z); a.w = fmaf(s, t.w - g.w, a.w);
+    }
+    reinterpret_cast<float4*>(acc)[i] = a;
+    if (reset) {
+      reinterpret_cast<float4*>(theta)[i] = g;
+      if (wb != nullptr) reinterpret_cast<uint2*>(wb)[i] = make_uint2(pack_bf16x2(g.x, g.y), pack_bf16x2(g.z, g.w));
+      if (mom != nullptr && (i << 2) < n_mom) reinterpret_cast<float4*>(mom)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  }
+}
+
 }  // namespace b200
 
 // The kernel spins on cross-GPU flags per CTA, so every CTA of the grid must be resident at the same time or the ranks
@@ -541,27 +655,29 @@ __global__ void flag_barrier_kernel(FedAvgArgs a, int slot) {
 // (cudaErrorCooperativeLaunchTooLarge) and schedules all CTAs together, also next to work on other streams -- instead
 // of the plain <<<>>> of round 1, which was only safe on an otherwise idle GPU.  The grid is clamped to what
 // cudaOccupancyMaxActiveBlocksPerMultiprocessor allows on this device.
-template <int WIRE>
-static int launch_fedavg(const FedAvgArgs* args, int n_ctas, cudaStream_t stream) {
+template <int WIRE, bool DP, typename Args>
+static int launch_fedavg(const Args* args, int n_ctas, cudaStream_t stream) {
   using namespace b200;
   static int max_ctas = -1;
+  const void* kernel = DP ? reinterpret_cast<const void*>(fedavg_allreduce_dp_kernel<WIRE>)
+                          : reinterpret_cast<const void*>(fedavg_allreduce_kernel<WIRE>);
   if (max_ctas < 0) {
     int dev = 0, sms = 0, per_sm = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fedavg_allreduce_kernel<WIRE>, FEDAVG_THREADS, 0);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, FEDAVG_THREADS, 0);
     max_ctas = sms * per_sm;
     if (max_ctas < 1) max_ctas = 1;
   }
   if (n_ctas > max_ctas) n_ctas = max_ctas;
-  void* kargs[] = {const_cast<FedAvgArgs*>(args)};
-  cudaError_t e = cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(fedavg_allreduce_kernel<WIRE>), dim3(n_ctas),
-                                              dim3(FEDAVG_THREADS), kargs, 0, stream);
+  void* kargs[] = {const_cast<Args*>(args)};
+  cudaError_t e = cudaLaunchCooperativeKernel(kernel, dim3(n_ctas), dim3(FEDAVG_THREADS), kargs, 0, stream);
   if (e != cudaSuccess) return static_cast<int>(e);
   return static_cast<int>(cudaGetLastError());
 }
 
-extern "C" int b200_fedavg_allreduce(const FedAvgArgs* args, int n_ctas, cudaStream_t stream) {
+template <bool DP, typename Args>
+static int fedavg_dispatch(const Args* args, int n_ctas, cudaStream_t stream) {
   using namespace b200;
   if (args->world > B200_MAX_RANKS || args->n % 8 != 0 || args->tile_elems % 8 != 0) return -2;
   if (args->tile_flags != nullptr && args->tile_elems % FLAG_GRANULE != 0) return -2;
@@ -569,10 +685,22 @@ extern "C" int b200_fedavg_allreduce(const FedAvgArgs* args, int n_ctas, cudaStr
   if (args->wire_kind == 2) {
     // block-scaled fp8 wire: 32-element blocks must not straddle tiles, and the switch cannot rescale
     if (args->tile_elems % 32 != 0 || args->use_nvls) return -2;
-    return launch_fedavg<2>(args, n_ctas, stream);
+    return launch_fedavg<2, DP>(args, n_ctas, stream);
   }
-  if (args->wire_kind == 1) return launch_fedavg<1>(args, n_ctas, stream);
-  return launch_fedavg<0>(args, n_ctas, stream);
+  if (args->wire_kind == 1) return launch_fedavg<1, DP>(args, n_ctas, stream);
+  return launch_fedavg<0, DP>(args, n_ctas, stream);
+}
+
+extern "C" int b200_fedavg_allreduce(const FedAvgArgs* args, int n_ctas, cudaStream_t stream) {
+  return fedavg_dispatch<false>(args, n_ctas, stream);
+}
+
+extern "C" int b200_fedavg_allreduce_dp(const FedAvgDPArgs* args, int n_ctas, cudaStream_t stream) {
+  // the switch adds the raw wire values, but the clip factors are applied on the reader side: DP runs on peer loads
+  if (args->use_nvls || !args->delta || args->world > B200_MAX_RANKS) return -2;
+  for (int k = 0; k < args->world; ++k)
+    if (((args->alive_mask >> k) & 1u) && args->clip_page[k] == nullptr) return -2;
+  return fedavg_dispatch<true>(args, n_ctas, stream);
 }
 
 extern "C" int b200_flag_barrier(unsigned long long* const* pads, int rank, int world, uint32_t alive_mask,
@@ -583,6 +711,30 @@ extern "C" int b200_flag_barrier(unsigned long long* const* pads, int rank, int 
   for (int k = 0; k < world; ++k) a.pads[k] = pads[k];
   a.rank = rank; a.world = world; a.alive_mask = alive_mask; a.epoch = epoch;
   flag_barrier_kernel<<<1, 32, 0, stream>>>(a, slot);
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int b200_dp_clip_factor(const float* theta, const float* global_w, long long n, float clip, void* work,
+                                   float* s_out, float* norm_out, float* s_copy, int* nonfinite, cudaStream_t stream) {
+  using namespace b200;
+  if (n % 4 != 0 || !(clip >= 0.f) || work == nullptr || s_out == nullptr || norm_out == nullptr) return -2;
+  if ((reinterpret_cast<uintptr_t>(theta) | reinterpret_cast<uintptr_t>(global_w)) & 15) return -2;
+  dp_clip_factor_kernel<<<B200_DP_NORM_BLOCKS, DP_NORM_THREADS, 0, stream>>>(
+      theta, global_w, n, clip, static_cast<unsigned long long*>(work), s_out, norm_out, s_copy, nonfinite);
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int b200_fold_client_scaled(float* acc, float* theta, const float* global_w, void* w_bf16, float* mom,
+                                       long long n_mom, long long n, const float* s, int first, int reset,
+                                       cudaStream_t stream) {
+  using namespace b200;
+  if (n <= 0) return 0;
+  if (n & 3) return -2;
+  long long g = (n / 4 + DP_NORM_THREADS - 1) / DP_NORM_THREADS;
+  const long long cap = 8ll * device_sm_count();
+  if (g > cap) g = cap;
+  fold_client_scaled_kernel<<<static_cast<unsigned>(g), DP_NORM_THREADS, 0, stream>>>(
+      acc, theta, global_w, reinterpret_cast<__nv_bfloat16*>(w_bf16), mom, n_mom, n, s, first, reset);
   return static_cast<int>(cudaGetLastError());
 }
 

@@ -149,7 +149,27 @@ struct FedAvgArgs {
   int* status;                      // device int: set non-zero on barrier timeout
   unsigned long long* phase_ns;     // optional [16]: %globaltimer at the phase boundaries (first / last CTA), or nullptr
 };
+// DP-FedAvg round (fedavg_allreduce_kernel<WIRE, true>): clipped weights w_k = n_k s_k / N and Gaussian noise on the
+// reduced sum.  A separate type derived from FedAvgArgs, so the plain kernels and flag_barrier_kernel keep their
+// parameter layout.
+struct FedAvgDPArgs : FedAvgArgs {
+  const float* clip_page[B200_MAX_RANKS];   // peer-mapped: clip_page[k][0] = s_k of rank k for this round
+  float noise_std;                  // sigma * C (noise on the sum; the kernel divides by N with the weights)
+  unsigned long long seed;          // Philox key
+  uint32_t round;                   // Philox counter word 2: the collective's round index
+};
 int b200_fedavg_allreduce(const FedAvgArgs* args, int n_ctas, cudaStream_t stream);
+int b200_fedavg_allreduce_dp(const FedAvgDPArgs* args, int n_ctas, cudaStream_t stream);   // delta mode, peer loads only
+// DP clip factor: s = min(1, clip / ||theta - global_w||_2) over [0, n), norm in fp64 (s = 0 when it is not finite), written to
+// s_out[0] (and s_copy[0] when given), the norm to norm_out[0]; a non-finite norm adds 1 to *nonfinite (optional).
+// Deterministic: fixed grid, per-block partials in work (int64 [B200_DP_WORK_WORDS], zero on first use), last-block finish.
+#define B200_DP_NORM_BLOCKS 264
+#define B200_DP_WORK_WORDS (B200_DP_NORM_BLOCKS + 1)
+int b200_dp_clip_factor(const float* theta, const float* global_w, long long n, float clip, void* work, float* s_out,
+                        float* norm_out, float* s_copy, int* nonfinite, cudaStream_t stream);
+// clipped logical-client fold: acc (+)= s[0] * (theta - global) with s read from device memory, reset as b200_fold_client
+int b200_fold_client_scaled(float* acc, float* theta, const float* global_w, void* w_bf16, float* mom, long long n_mom,
+                            long long n, const float* s, int first, int reset, cudaStream_t stream);
 int b200_flag_barrier(unsigned long long* const* pads, int rank, int world, uint32_t alive_mask, uint32_t epoch,
                       int slot, cudaStream_t stream);
 

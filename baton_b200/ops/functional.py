@@ -266,6 +266,23 @@ def fold_finish(acc: torch.Tensor, theta: torch.Tensor, global_w: torch.Tensor, 
     load().fold_client(acc, theta, global_w, None, None, 1.0 / float(total), 2, False)
 
 
+def dp_clip_factor(theta: torch.Tensor, global_w: torch.Tensor, clip: float, work: torch.Tensor, s_out: torch.Tensor,
+                   norm_out: torch.Tensor, *, s_copy_ptr: int = 0, nonfinite: Optional[torch.Tensor] = None) -> None:
+    """DP-FedAvg clip factor: ``s_out[0] = min(1, clip / ||theta - global_w||)`` (0 for a non-finite norm, which also
+    adds 1 to ``nonfinite``), ``norm_out[0]`` = the norm.  Deterministic (fixed grid and summation order).  ``work``:
+    int64 ``[DP_WORK_WORDS]`` of zeros, reusable by launches on the same stream.  ``s_copy_ptr``: device address that
+    receives a second copy of ``s`` (the collective's clip page)."""
+    load().dp_clip_factor(theta, global_w, float(clip), work, s_out, norm_out, int(s_copy_ptr), nonfinite)
+
+
+def fold_client_scaled(acc: torch.Tensor, theta: torch.Tensor, global_w: torch.Tensor, s: torch.Tensor, *,
+                       first: bool = False, reset: bool = False, w_bf16: Optional[torch.Tensor] = None,
+                       momentum: Optional[torch.Tensor] = None) -> None:
+    """:func:`fold_client` with the weight read from the device scalar ``s[0]`` (a DP clip factor): ``acc (+)= s *
+    (theta - global)``; ``s == 0`` adds nothing, even where theta is not finite."""
+    load().fold_client_scaled(acc, theta, global_w, w_bf16, momentum, s, first, reset)
+
+
 def cast(src: torch.Tensor, dtype: torch.dtype, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     if out is None:
         out = torch.empty(src.shape, dtype=dtype, device=src.device)

@@ -93,6 +93,54 @@ def fedavg_into(global_state: Mapping[str, torch.Tensor],
     return True
 
 
+@torch.no_grad()
+def dp_fedavg_into(global_state: Mapping[str, torch.Tensor], client_states: Sequence[Mapping[str, torch.Tensor]], *,
+                   clip: float, noise_multiplier: float, seed: int, round_index: int,
+                   int_policy: str = "max") -> List[float]:
+    """DP-FedAvg (``parallel/dp.py``) written in place into ``global_state``: every client's update ``Delta_k`` is its
+    float entries minus the global ones, taken as ONE vector in ``global_state`` order; ``s_k = min(1, clip /
+    ||Delta_k||)`` (0 when not finite -- the client still counts in m); ``global += (sum_k s_k Delta_k + sigma C z) / m``
+    with uniform weights and ``z`` the Philox stream ``(seed, round_index)`` over the same element order.  Integer
+    entries follow ``int_policy`` over all clients.  Computed in float64, cast once.  Returns the clip factors."""
+    from .dp import check_dp, norm_to_factor, normals
+    import math
+    clip, sigma = check_dp(clip, noise_multiplier)
+    m = len(client_states)
+    if m == 0:
+        return []
+    fkeys = [k for k, v in global_state.items() if v.is_floating_point()]
+    for sd in client_states:
+        missing = [k for k in global_state if k not in sd]
+        if missing:
+            raise KeyError("client state_dict is missing {!r}".format(missing[0]))
+    deltas = []
+    for sd in client_states:
+        deltas.append([sd[k].detach().to(device="cpu", dtype=torch.float64).reshape(-1)
+                       - global_state[k].detach().to(device="cpu", dtype=torch.float64).reshape(-1) for k in fkeys])
+    factors = []
+    for d in deltas:
+        sq = sum(float(t.pow(2).sum()) for t in d)
+        factors.append(norm_to_factor(math.sqrt(sq) if math.isfinite(sq) else float("nan"), clip))
+    n_total = sum(global_state[k].numel() for k in fkeys)
+    z = torch.from_numpy(normals(seed, round_index, n_total)) if sigma > 0.0 else None
+    off = 0
+    for i, k in enumerate(fkeys):
+        g = global_state[k]
+        acc = torch.zeros(g.numel(), dtype=torch.float64)
+        for d, sk in zip(deltas, factors):
+            if sk != 0.0:
+                acc.add_(d[i], alpha=sk)
+        if z is not None:
+            acc.add_(z[off: off + g.numel()], alpha=sigma * clip)
+        off += g.numel()
+        new = g.detach().to(device="cpu", dtype=torch.float64).reshape(-1) + acc / m
+        g.copy_(new.reshape(g.shape).to(device=g.device, dtype=g.dtype))
+    for k, v in global_state.items():
+        if not v.is_floating_point():
+            _reduce_int(v, [sd[k] for sd in client_states], [1.0 / m] * m, int_policy)
+    return factors
+
+
 def fedavg_loss_history(loss_histories: Sequence[Sequence[float]], n_samples: Sequence[float],
                         n_epoch: Optional[int] = None) -> List[float]:
     """Per-epoch sample-weighted loss (manager.py:127-130).  A client that

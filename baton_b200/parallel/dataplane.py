@@ -27,7 +27,7 @@ from typing import Any, Dict, List, Mapping, Optional
 import torch
 
 from . import wire
-from .aggregate import fedavg_into
+from .aggregate import dp_fedavg_into, fedavg_into
 
 log = logging.getLogger("baton_b200.dataplane")
 
@@ -52,13 +52,20 @@ class ManagerPlane:
 
 
 class HttpManagerPlane(ManagerPlane):
-    """Reference wire format: full weights in both directions."""
+    """Reference wire format: full weights in both directions.  ``dp`` (a :class:`~baton_b200.parallel.dp.DPConfig`):
+    the manager aggregates with DP-FedAvg (:func:`~baton_b200.parallel.aggregate.dp_fedavg_into`) instead of the
+    sample-weighted mean.  As in the plain mean, an upload with ``n_samples == 0`` (a client that trained nothing) is
+    not a participant; a round without participants aggregates nothing and does not advance the noise stream.
+    ``last_clip_factors`` holds the factors of the last aggregated round."""
 
     name = "http"
     carries_tensors = True
 
-    def __init__(self, int_policy: str = "max"):
+    def __init__(self, int_policy: str = "max", dp=None):
         self.int_policy = int_policy
+        self.dp = dp
+        self.dp_rounds = 0
+        self.last_clip_factors: List[float] = []
 
     def round_start_message(self, model, update_name, n_epoch, extra=None) -> bytes:
         sd = model.state_dict()
@@ -78,8 +85,18 @@ class HttpManagerPlane(ManagerPlane):
         # the reduce raise half-way must not leave the global model half-written
         live = experiment.model.state_dict()
         scratch = type(live)((k, v.detach().clone()) for k, v in live.items())
-        ok = fedavg_into(scratch, [d["state_dict"] for d in datas], [d["n_samples"] for d in datas],
-                         int_policy=self.int_policy)
+        if self.dp is not None:
+            datas = [d for d in datas if float(d.get("n_samples", 0)) > 0]
+            if not datas:
+                return False
+            self.last_clip_factors = dp_fedavg_into(scratch, [d["state_dict"] for d in datas], clip=self.dp.clip,
+                                                    noise_multiplier=self.dp.noise_multiplier, seed=self.dp.seed,
+                                                    round_index=self.dp_rounds, int_policy=self.int_policy)
+            self.dp_rounds += 1
+            ok = True
+        else:
+            ok = fedavg_into(scratch, [d["state_dict"] for d in datas], [d["n_samples"] for d in datas],
+                             int_policy=self.int_policy)
         if ok:
             with torch.no_grad():
                 for k, v in live.items():
@@ -104,11 +121,15 @@ class SeatedManagerPlane(ManagerPlane):
 
     carries_tensors = False
 
-    def __init__(self, name: str = "fused", world_size: Optional[int] = None, distribute_initial: bool = True):
+    def __init__(self, name: str = "fused", world_size: Optional[int] = None, distribute_initial: bool = True,
+                 dp=None):
         self.name = name
         self.world_size = world_size
         self.distribute_initial = distribute_initial
         self.n_aggregates = 0
+        # DP-FedAvg (a DPConfig): the plan weights count CLIENTS per rank and carries {"dp": {clip, noise_multiplier,
+        # seed}}, so every seat runs the same estimator with the manager's noise key
+        self.dp = dp
 
     def round_start_message(self, model, update_name, n_epoch, extra=None) -> bytes:
         msg = {"update_name": update_name, "n_epoch": n_epoch, "dataplane": self.name}
@@ -143,10 +164,16 @@ class SeatedManagerPlane(ManagerPlane):
             rank = d.get("rank", rec.get("rank") if rec else None)
             if rank is None:
                 continue
-            seats[int(rank)] = seats.get(int(rank), 0.0) + float(d["n_samples"])
+            n = float(d["n_samples"])
+            if self.dp is not None:
+                n = 1.0 if n > 0 else 0.0          # DP: uniform over the clients that trained
+            seats[int(rank)] = seats.get(int(rank), 0.0) + n
         world = self.world_size or (max(alive + list(seats)) + 1 if (alive or seats) else 0)
         n_by_rank = [seats.get(r, 0.0) for r in range(world)]
-        return {"n_samples_by_rank": n_by_rank, "alive_ranks": sorted(set(alive) | set(seats))}
+        plan = {"n_samples_by_rank": n_by_rank, "alive_ranks": sorted(set(alive) | set(seats))}
+        if self.dp is not None:
+            plan["dp"] = {"clip": self.dp.clip, "noise_multiplier": self.dp.noise_multiplier, "seed": self.dp.seed}
+        return plan
 
     async def aggregate(self, experiment, responses) -> bool:
         plan = self.rank_weights(experiment, responses)
@@ -239,21 +266,28 @@ class SeatedWorkerPlane(WorkerPlane):
 
     def aggregate(self, worker, plan) -> None:
         kw = {}
-        if plan.get("round") is not None and hasattr(self.session, "base_epoch"):
+        # the round index sets the barrier epoch of the fused session and, under DP, the noise stream's round
+        if plan.get("round") is not None and (hasattr(self.session, "base_epoch") or plan.get("dp")):
             kw["round_index"] = int(plan["round"])
+        if plan.get("dp"):
+            from .dp import DPConfig
+            d = plan["dp"]
+            kw["dp"] = DPConfig(float(d["clip"]), float(d["noise_multiplier"]), seed=int(d["seed"]))
         self.session.aggregate(plan["n_samples_by_rank"], plan.get("alive_ranks"), **kw)
         check = getattr(self.session, "check", None)
         if check is not None:
             check()             # a peer that died mid-collective surfaces here as an error, not as a hang
 
 
-def make_manager_plane(spec) -> ManagerPlane:
+def make_manager_plane(spec, dp=None) -> ManagerPlane:
     if isinstance(spec, ManagerPlane):
+        if dp is not None and getattr(spec, "dp", None) is None:
+            raise ValueError("a DP experiment needs a data plane built with the same dp=")
         return spec
     if spec in (None, "http", "http_pickle"):
-        return HttpManagerPlane()
+        return HttpManagerPlane(dp=dp)
     if spec in ("fused", "nccl"):
-        return SeatedManagerPlane(spec)
+        return SeatedManagerPlane(spec, dp=dp)
     raise ValueError("unknown data plane {!r}".format(spec))
 
 

@@ -28,6 +28,7 @@ import torch
 from ..metrics import phase
 from ..train import GraphedLocalSGD, PortableLocalSGD, check_prox_mu
 from .arena import ParamArena
+from .dp import DPConfig, RDPAccountant, check_dp, clip_factor
 from .fedavg import FedAvgSession, NcclSession
 
 
@@ -62,10 +63,20 @@ class FederatedEngine:
                  lr: float = 0.05, batch_size: int = 128, momentum: float = 0.0, weight_decay: float = 0.0,
                  wire_dtype: str = "bf16", mode: str = "delta", n_ctas: Optional[int] = None, use_graph: bool = True,
                  logical_clients: int = 0, sample_k: Optional[int] = None, seed: int = 0, name: str = "exp",
-                 nvls: "bool | str" = "auto", tile_flags: bool = False, prox_mu: float = 0.0):
+                 nvls: "bool | str" = "auto", tile_flags: bool = False, prox_mu: float = 0.0,
+                 dp_clip: float = 0.0, dp_noise_multiplier: float = 0.0, dp_seed: Optional[int] = None):
         """``prox_mu > 0``: FedProx local training -- every step adds ``prox_mu * (theta - global_w)`` to the gradient,
-        ``global_w`` being the global model the round started from (for logical clients too: each starts from it)."""
+        ``global_w`` being the global model the round started from (for logical clients too: each starts from it).
+
+        ``dp_clip > 0``: DP-FedAvg (``parallel/dp.py``) -- every participating client's update is clipped to L2 norm
+        ``dp_clip``, the participants are averaged uniformly and Gaussian noise of std ``dp_noise_multiplier * dp_clip``
+        is added to the sum.  ``dp_seed``: Philox key of the noise (``None``: a secret random key; an explicit seed makes
+        the noise predictable -- tests and reproductions only).  ``dp_clip = 0`` runs exactly the plain engine."""
         prox_mu = check_prox_mu(prox_mu)
+        dp_clip, dp_noise_multiplier = check_dp(dp_clip, dp_noise_multiplier)
+        self.dp = DPConfig(dp_clip, dp_noise_multiplier, dp_seed) if dp_clip > 0.0 else None
+        if self.dp is not None and mode != "delta":
+            raise ValueError("DP-FedAvg needs mode='delta'")
         self.device = torch.device(device)
         self.model = model
         self.name = name
@@ -84,7 +95,9 @@ class FederatedEngine:
             self.trainer = PortableLocalSGD(model, self.arena, loss=loss)
         Session = {"fused": FedAvgSession, "nccl": NcclSession}[backend]
         self.session = Session(self.arena, group, wire_dtype=wire_dtype, mode=mode, n_ctas=n_ctas, nvls=nvls,
-                               tile_flags=tile_flags)
+                               tile_flags=tile_flags, dp=self.dp)
+        self.dp = self.session.dp                  # rank 0's noise key
+        self.accountant = RDPAccountant(self.dp.noise_multiplier) if self.dp is not None else None
         self.backend = backend
         self.rank, self.world = self.session.rank, self.session.world
         # K4: the last SGD step of the captured epoch writes the upload copy itself (no pack phase in the collective);
@@ -112,6 +125,10 @@ class FederatedEngine:
         self._stage: Dict[Tuple, Tuple[torch.Tensor, torch.Tensor]] = {}
         self._eval_stage: Dict[Tuple, Tuple[torch.Tensor, torch.Tensor]] = {}
         self._acc = None
+        self._dp_rec = None              # DP with logical clients: [clip factor, norm] per hosted client of the round
+        self._dp_n = 0
+        self._dp_work = None             # ... the norm kernel's partials (CUDA)
+        self._dp_bad = 0                 # ... non-finite client updates so far (device counter on CUDA)
         self.last_losses_dev = None
         self.samples_trained = 0          # samples this rank pushed through local SGD (per epoch)
         self.phase_s: Dict[str, float] = {}   # host seconds per NVTX phase (launch cost; device time is in bench.py)
@@ -175,11 +192,15 @@ class FederatedEngine:
                 total_n = X.shape[0]
         else:
             # time-sliced logical clients: fold n_k * (theta_k - global) locally, then upload the mean
+            # (DP: s_k * (theta_k - global) for every hosted client, even a single one, and the mean over clients)
             self.sync()
-            if len(mine) > 1 and self._acc is None:
+            fold = len(mine) > 1 or (self.dp is not None and mine)
+            if fold and self._acc is None:
                 self._acc = torch.zeros_like(a.theta)
-            if len(mine) > 1 and not a.theta.is_cuda:
+            if fold and not a.theta.is_cuda:
                 self._acc.zero_()
+            if self.dp is not None:
+                self._dp_begin(len(mine))
             for j, cid in enumerate(mine):
                 X, y = shards(cid)
                 if not X.is_cuda:
@@ -188,7 +209,9 @@ class FederatedEngine:
                 nk = X.shape[0]
                 losses_dev = ld * nk if losses_dev is None else losses_dev + ld * nk
                 total_n += nk
-                if len(mine) > 1:
+                if self.dp is not None:
+                    self._dp_fold(j, more=j + 1 < len(mine))
+                elif len(mine) > 1:
                     more = j + 1 < len(mine)           # the next co-resident client starts from the global model
                     if a.theta.is_cuda:
                         from ..ops import functional as F     # ONE kernel: fold the delta + reset the replica
@@ -201,12 +224,13 @@ class FederatedEngine:
                             a.sync_shadow()
                             if a.momentum is not None:
                                 a.momentum.zero_()
-            if len(mine) > 1:
+            if fold:
+                m_r = len(mine) if self.dp is not None else total_n
                 if a.theta.is_cuda:
                     from ..ops import functional as F
-                    F.fold_finish(self._acc, a.theta, a.global_w, total_n)
+                    F.fold_finish(self._acc, a.theta, a.global_w, m_r)
                 else:
-                    torch.add(a.global_w, self._acc, alpha=1.0 / total_n, out=a.theta)
+                    torch.add(a.global_w, self._acc, alpha=1.0 / m_r, out=a.theta)
             if losses_dev is not None and total_n:
                 losses_dev = losses_dev / total_n
         self.last_losses_dev = losses_dev
@@ -215,8 +239,12 @@ class FederatedEngine:
         if losses_dev is not None:
             steps = max(1, self.trainer.last_steps)
             loss_for_wire = losses_dev[:, 0] / steps
+        # DP: the weights count clients (1 per seat, m_r with logical clients), not samples
+        my_n = float(total_n) if self.dp is None else float(len(mine) if self.logical_clients else (1 if mine else 0))
         with phase("baton.aggregate_broadcast", self.phase_s):
-            self._aggregate(float(total_n), loss_for_wire)
+            self._aggregate(my_n, loss_for_wire, clipped=bool(self.dp is not None and self.logical_clients))
+        if self.accountant is not None:
+            self.accountant.step(len(participants) / float(self.logical_clients or self.world))
         self.n_rounds += 1
         hist: List[float] = []
         if read_loss and losses_dev is not None:
@@ -230,8 +258,86 @@ class FederatedEngine:
         if join is not None:
             join()
 
-    def _aggregate(self, my_n: float, loss_dev) -> None:
+    # ------------------------------------------------------------------ differential privacy
+    def _dp_begin(self, n_mine: int) -> None:
+        dev = self.arena.theta.device
+        if self._dp_rec is None or self._dp_rec.shape[0] < max(n_mine, 1):
+            self._dp_rec = torch.zeros(max(n_mine, 1), 2, dtype=torch.float32, device=dev)
+        if self._dp_work is None and dev.type == "cuda":
+            from ..ops._ext import load
+            self._dp_work = torch.zeros(load().DP_WORK_WORDS, dtype=torch.int64, device=dev)
+            self._dp_bad = torch.zeros(1, dtype=torch.int32, device=dev)
+        self._dp_n = n_mine
+
+    def _dp_fold(self, j: int, more: bool) -> None:
+        """Clip hosted client ``j``'s update into the accumulator and (``more``) reset the replica for the next one.
+        On CUDA the factor stays on the device: norm kernel -> device scalar -> scaled fold, no host synchronisation."""
+        a = self.arena
+        if a.theta.is_cuda:
+            from ..ops import functional as F
+            rec = self._dp_rec[j]
+            F.dp_clip_factor(a.theta, a.global_w, self.dp.clip, self._dp_work, rec[0:1], rec[1:2], nonfinite=self._dp_bad)
+            F.fold_client_scaled(self._acc, a.theta, a.global_w, rec[0:1], first=(j == 0), reset=more,
+                                 w_bf16=a.theta_bf16, momentum=a.momentum)
+            return
+        sj, norm = clip_factor(a.theta - a.global_w, self.dp.clip)
+        self._dp_rec[j, 0], self._dp_rec[j, 1] = sj, norm
+        if sj == 0.0:
+            self._dp_bad += 1
+        else:
+            self._acc.add_(a.theta - a.global_w, alpha=sj)
+        if more:
+            a.theta.copy_(a.global_w)
+            a.sync_shadow()
+            if a.momentum is not None:
+                a.momentum.zero_()
+
+    def last_clip_factors(self) -> List[float]:
+        """Clip factors ``s`` of the clients this rank trained in the last round (a host read)."""
+        if self.dp is None:
+            return []
+        self.sync()
+        if self.logical_clients:
+            return self._dp_rec[: self._dp_n, 0].tolist() if self._dp_rec is not None else []
+        return self.session.last_clip_factors()
+
+    def last_update_norms(self) -> List[float]:
+        """L2 norms of the updates of the clients this rank hosted in the last logical-client DP round (a host read)."""
+        if self.dp is None or not self.logical_clients or self._dp_rec is None:
+            return []
+        self.sync()
+        return self._dp_rec[: self._dp_n, 1].tolist()
+
+    def nonfinite_updates(self) -> int:
+        """Client updates of this rank so far whose norm was not finite (clipped to nothing, still counted in m)."""
+        if self.dp is None:
+            return 0
+        self.sync()
+        return int(self._dp_bad) + self.session.nonfinite_updates()
+
+    def privacy_spent(self, delta: float = 1e-5):
+        """``(epsilon, order)`` of the DP rounds run so far at ``delta`` (RDP accountant of the sampled Gaussian
+        mechanism; a fixed-size participant sample is accounted as Poisson sampling at rate k / K)."""
+        if self.accountant is None:
+            raise RuntimeError("differential privacy is off (dp_clip = 0)")
+        return self.accountant.get_privacy_spent(delta)
+
+    def _aggregate(self, my_n: float, loss_dev, clipped: bool = False) -> None:
         s = self.session
+        if self.dp is not None:
+            kw = {"clipped": clipped}
+            if isinstance(s, FedAvgSession):
+                kw["on_side_stream"] = bool(self.overlap_collective)
+                kw["prepacked"] = bool(self.prepack and getattr(self.trainer, "emitted_wire", False) and my_n > 0
+                                       and not getattr(self.trainer, "last_had_tail_step", False))
+            if loss_dev is not None and hasattr(s, "loss_local"):
+                k = min(loss_dev.numel(), s.loss_local.numel())
+                s.loss_local.zero_()
+                s.loss_local[:k].copy_(loss_dev[:k])
+                s.aggregate(my_n=my_n, **kw)
+            else:
+                s.aggregate(my_n=my_n, loss_history=loss_dev.tolist() if loss_dev is not None else None, **kw)
+            return
         side = bool(self.overlap_collective and isinstance(s, FedAvgSession))
         if loss_dev is not None and hasattr(s, "loss_local"):
             k = min(loss_dev.numel(), s.loss_local.numel())

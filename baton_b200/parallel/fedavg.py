@@ -12,6 +12,12 @@ and ``load_state_dict`` (worker.py:98).  ``NcclSession`` implements the same
 interface with ``torch.distributed`` collectives: it is the BASELINE the fused
 kernel is measured against and the oracle the tests compare with -- not the
 product path.
+
+Both take ``dp=DPConfig(...)`` (``parallel/dp.py``): DP-FedAvg, the clipped uniform mean of the participants' updates
+plus Gaussian noise on the sum.  The fused session clips with one deterministic norm kernel per round on the
+collective's stream, publishes the factor in a small per-rank CLIP PAGE of the symmetric buffer, and the collective
+applies it on the reader side and adds the noise in the tile owner's fp32 accumulator; DP rounds always run on peer
+loads (the switch of NVLS adds raw wire values, before the factors are known).
 """
 from __future__ import annotations
 
@@ -20,6 +26,7 @@ from typing import List, Optional, Sequence
 import torch
 
 from .arena import ParamArena
+from .dp import DPConfig, clip_factor, normals
 from .symm import SymmetricBuffer
 
 MAX_LOSS = 64       # per-epoch loss slots carried through the collective
@@ -30,13 +37,31 @@ def _align(x: int, a: int) -> int:
     return (x + a - 1) // a * a
 
 
+def _check_dp_mode(dp: Optional[DPConfig], delta: bool) -> None:
+    if dp is not None and not delta:
+        raise ValueError("DP-FedAvg clips and noises the update theta - global: it needs mode='delta'")
+
+
+def _agree_seed(dp: Optional[DPConfig], group) -> Optional[DPConfig]:
+    """Every rank must draw the same noise: take rank 0's Philox key (a DPConfig built with seed=None differs per
+    process)."""
+    import torch.distributed as dist
+    if dp is None or not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
+        return dp
+    box = [dp.seed]
+    src = dist.get_global_rank(group, 0) if group is not None else 0
+    dist.broadcast_object_list(box, src=src, group=group)
+    return DPConfig(dp.clip, dp.noise_multiplier, seed=int(box[0]))
+
+
 class FedAvgSession:
     def __init__(self, arena: ParamArena, group=None, *, wire_dtype: str = "bf16", mode: str = "delta",
                  nvls: "bool | str" = "auto", n_ctas: Optional[int] = None, tile_elems: int = 0, timeout_log2: int = 24,
-                 reset_momentum: bool = True, tile_flags: bool = False):
+                 reset_momentum: bool = True, tile_flags: bool = False, dp: Optional[DPConfig] = None):
         from ..ops._ext import load
         self._C = load()
         assert wire_dtype in ("bf16", "fp32", "fp8") and mode in ("delta", "weights")
+        _check_dp_mode(dp, mode == "delta")
         self.arena = arena
         self.device = arena.device
         self.group = group
@@ -59,10 +84,12 @@ class FedAvgSession:
         self.half_wire = _align(self.wire_bytes(), 2 << 20)          # multicast-friendly granularity
         self.half_int = _align(max(arena.n_int, 1) * 8, 256)
         self.half_loss = _align(MAX_LOSS * 4, 256)
+        self.half_clip = 256                                          # DP: this rank's clip factor s_r
         self.off_wire = 0
         self.off_int = 2 * self.half_wire
         self.off_loss = self.off_int + 2 * self.half_int
-        self.off_pads = _align(self.off_loss + 2 * self.half_loss, 256)
+        self.off_clip = self.off_loss + 2 * self.half_loss
+        self.off_pads = _align(self.off_clip + 2 * self.half_clip, 256)
         total = _align(self.off_pads + (MAX_CTAS + 8) * self._C.MAX_RANKS * 8, 2 << 20)
         self.symm = SymmetricBuffer(total, self.device, group)
         self.rank, self.world = self.symm.rank, self.symm.world
@@ -70,6 +97,14 @@ class FedAvgSession:
         self.use_nvls = self.symm.has_multicast if nvls == "auto" else (bool(nvls) and self.symm.has_multicast)
         if self.wire_kind == 2:
             self.use_nvls = False      # the switch adds raw elements; block scales need the P2P path
+        self.dp = _agree_seed(dp, group)
+        if self.dp is not None:
+            self.use_nvls = False      # the clip factors are applied by the readers: DP rounds run on peer loads
+        # DP bookkeeping: norm-kernel partials, the last clip factor / norm of this rank, non-finite updates so far
+        self.dp_work = torch.zeros(self._C.DP_WORK_WORDS, dtype=torch.int64, device=self.device)
+        self.dp_s = torch.ones(1, dtype=torch.float32, device=self.device)
+        self.dp_norm = torch.zeros(1, dtype=torch.float32, device=self.device)
+        self.dp_nonfinite = torch.zeros(1, dtype=torch.int32, device=self.device)
         self.epoch = 0
         self.rounds = 0
         self.stale = False          # True after a round this seat sat out: its weights are no longer the global model
@@ -175,7 +210,8 @@ class FedAvgSession:
     def aggregate(self, n_samples_by_rank: Optional[Sequence[float]] = None,
                   alive_ranks: Optional[Sequence[int]] = None, my_n: Optional[float] = None,
                   loss_history: Optional[Sequence[float]] = None, on_side_stream: bool = False,
-                  round_index: Optional[int] = None, prepacked: bool = False) -> None:
+                  round_index: Optional[int] = None, prepacked: bool = False, dp: Optional[DPConfig] = None,
+                  clipped: bool = False) -> None:
         """Launch the fused reduce+broadcast+apply.  Either the full per-rank sample
         counts are given (manager-driven rounds: the plan comes over HTTP) or only this
         rank's own count ``my_n`` (SPMD engine: peers' counts ride on the barrier flags).
@@ -183,8 +219,15 @@ class FedAvgSession:
         ``round_index``: number of aggregations the MANAGER has dispatched before this one.  The manager is the single
         authority for it: the barrier epoch becomes ``base_epoch + 3 * round_index`` on every seat, so a seat that sat
         out rounds (evicted, re-registered) re-enters in step with its peers instead of racing them with a lagging
-        counter (epochs must never run backwards: the pads keep the highest epoch ever seen)."""
+        counter (epochs must never run backwards: the pads keep the highest epoch ever seen).
+
+        ``dp`` (default: the session's): a DP-FedAvg round.  The counts must then be CLIENTS per rank (1 for a plain
+        seat), not samples, and every rank must pass the same ``dp`` (the manager's plan carries it; a session built
+        with ``dp=`` agreed on rank 0's key at construction).  ``clipped=True``: this rank's upload is already a sum of clipped updates divided by its
+        count (logical clients folded with :func:`ops.functional.fold_client_scaled`), so its clip factor is 1."""
         world = self.world
+        dp = dp if dp is not None else self.dp
+        _check_dp_mode(dp, self.delta)
         if round_index is not None:
             self.epoch = (self.base_epoch + 3 * int(round_index)) & 0xFFFFFFFF
         if n_samples_by_rank is not None:
@@ -214,7 +257,7 @@ class FedAvgSession:
         a = self.arena
         # the optimizer's wire copy is only valid for the round / scale it was armed for and when the collective runs
         # the way arm_prepack assumed (NVLS needs every rank alive); otherwise the kernel packs itself (always correct)
-        nvls_now = bool(self.use_nvls and len(alive) == world)
+        nvls_now = bool(self.use_nvls and len(alive) == world and dp is None)
         want_scale = (counts[self.rank] if not from_flags else float(my_n)) if (self.use_nvls and world > 1) else 1.0
         prepacked = bool(prepacked and self.wire_kind != 2 and self._armed_for == (self.epoch, float(want_scale))
                          and (nvls_now == bool(self.use_nvls and world > 1)))
@@ -228,9 +271,10 @@ class FedAvgSession:
             tile = (tile + self.FLAG_GRANULE - 1) // self.FLAG_GRANULE * self.FLAG_GRANULE
         self.last_tile_elems = tile
         flag_value = self.rounds + 1
-        par = (self.epoch // 3) & 1            # round parity: which half of the wire / int / loss pages this round uses
+        par = (self.epoch // 3) & 1            # round parity: which half of the wire / int / loss / clip pages this round uses
         o_wire, o_int, o_loss = (self.off_wire + par * self.half_wire, self.off_int + par * self.half_int,
                                  self.off_loss + par * self.half_loss)
+        o_clip = self.off_clip + par * self.half_clip
         cur = torch.cuda.current_stream(self.device)
         stream = self.stream if on_side_stream else cur
         if self.tile_flags is not None:
@@ -238,21 +282,46 @@ class FedAvgSession:
         if on_side_stream:
             stream.wait_stream(cur)
         with torch.cuda.stream(stream):
+            dp_args = ([], 0.0, 0, 0)
+            if dp is not None:
+                from ..ops import functional as F
+                page = self.symm.view(o_clip, 1, torch.float32)
+                if clipped:
+                    page.fill_(1.0)
+                    self.dp_s.fill_(1.0)
+                else:     # theta is final here: the norm pass runs right before the collective, on its stream
+                    F.dp_clip_factor(a.theta, a.global_w, dp.clip, self.dp_work, self.dp_s, self.dp_norm,
+                                     s_copy_ptr=page.data_ptr(), nonfinite=self.dp_nonfinite)
+                seed = dp.seed - (1 << 64) if dp.seed >= (1 << 63) else dp.seed      # int64 bit pattern of the key
+                dp_args = (self.symm.peer_ptrs(o_clip), dp.noise_std, seed, self.dp_round())
             self._C.fedavg_allreduce(
                 self.symm.peer_ptrs(o_wire), self.symm.peer_ptrs(self.off_pads),
-                self.symm.mc(o_wire) if self.use_nvls else 0,
+                self.symm.mc(o_wire) if nvls_now else 0,
                 a.theta, a.global_w, a.theta_bf16,
                 a.momentum if self.reset_momentum else None,
                 a.int_arena if a.n_int > 0 else None,
                 self.symm.peer_ptrs(o_int) if a.n_int > 0 else [],
                 self.loss_local, self.symm.peer_ptrs(o_loss), self.loss_out,
                 counts, from_flags, mask, self.rank, world, self.wire_kind, self.delta,
-                bool(self.use_nvls and len(alive) == world), self.epoch,
+                nvls_now, self.epoch,
                 self.tile_flags, flag_value, tile, self.n_ctas, self.timeout_log2, self.status, self.phase_ns,
-                prepacked)
+                prepacked, *dp_args)
         self.epoch = (self.epoch + 3) & 0xFFFFFFFF     # uint32 wrap: the kernel compares signed differences
         self.rounds += 1
         self._side_pending = on_side_stream
+
+    def dp_round(self) -> int:
+        """Round index of the noise stream: ``(epoch - base_epoch) / 3``, identical on every rank (the plan's
+        ``round`` in manager-driven rounds)."""
+        return ((self.epoch - self.base_epoch) & 0xFFFFFFFF) // 3
+
+    def last_clip_factors(self) -> List[float]:
+        """This rank's clip factor of the last DP round (host read)."""
+        return self.dp_s.tolist()
+
+    def nonfinite_updates(self) -> int:
+        """DP rounds so far in which this rank's update had a non-finite norm (and was given s = 0)."""
+        return int(self.dp_nonfinite.item())
 
     def join(self) -> None:
         """Make the compute stream wait for a side-stream collective."""
@@ -325,10 +394,14 @@ class NcclSession:
     """Same contract through ``torch.distributed`` collectives (baseline / oracle)."""
 
     def __init__(self, arena: ParamArena, group=None, *, wire_dtype: str = "bf16", mode: str = "delta",
-                 reset_momentum: bool = True, **_unused):
+                 reset_momentum: bool = True, dp: Optional[DPConfig] = None, **_unused):
         import torch.distributed as dist
+        _check_dp_mode(dp, mode == "delta")
         self.dist = dist
         self.arena, self.group, self.device = arena, group, arena.device
+        self.dp = _agree_seed(dp, group)
+        self.dp_s = [1.0]
+        self.dp_nonfinite = 0
         self.wire_dtype = torch.bfloat16 if wire_dtype == "bf16" else torch.float32
         self.delta = mode == "delta"
         self.reset_momentum = reset_momentum
@@ -342,8 +415,17 @@ class NcclSession:
         self.rounds = 0
 
     @torch.no_grad()
-    def aggregate(self, n_samples_by_rank=None, alive_ranks=None, my_n=None, loss_history=None, **_unused) -> None:
+    def aggregate(self, n_samples_by_rank=None, alive_ranks=None, my_n=None, loss_history=None,
+                  dp: Optional[DPConfig] = None, clipped: bool = False, round_index: Optional[int] = None,
+                  **_unused) -> None:
+        """DP-FedAvg (``dp``, default the session's): the same estimator as the fused kernel -- clip locally, all-reduce,
+        then add the host-generated noise ``sigma C z(seed, round) / m`` after the reduce.  ``round_index`` (the
+        manager's plan) sets the round counter, as it sets the fused session's barrier epoch."""
+        if round_index is not None:
+            self.rounds = int(round_index)
         a, dist = self.arena, self.dist
+        dp = dp if dp is not None else self.dp
+        _check_dp_mode(dp, self.delta)
         if n_samples_by_rank is not None:
             counts = torch.tensor([float(x) for x in n_samples_by_rank][: self.world], device=self.device)
         else:
@@ -355,7 +437,18 @@ class NcclSession:
         total = counts.sum()
         w = counts[self.rank] / total
         src = (a.theta - a.global_w) if self.delta else a.theta
-        self.wire.copy_((src * w).to(self.wire_dtype))
+        if dp is not None:
+            s = 1.0
+            if not clipped and float(counts[self.rank]) != 0.0:
+                s, _ = clip_factor(src, dp.clip)
+                self.dp_nonfinite += int(s == 0.0)
+            self.dp_s = [s]
+            wd = w * s
+            if s == 0.0 or float(counts[self.rank]) == 0.0:
+                src, wd = torch.zeros_like(src), 0.0          # a non-finite update contributes nothing (0 * nan = nan)
+            self.wire.copy_((src * wd).to(self.wire_dtype))
+        else:
+            self.wire.copy_((src * w).to(self.wire_dtype))
         if self.world > 1:
             dist.all_reduce(self.wire, group=self.group)
         # every rank joins the loss reduce every round -- a rank that hosts no sampled client this round
@@ -367,7 +460,11 @@ class NcclSession:
         if self.world > 1:
             dist.all_reduce(self.loss_buf, group=self.group)
         self.loss_out.copy_(self.loss_buf)
-        if self.delta:
+        if dp is not None and dp.noise_std > 0.0 and float(total) > 0.0:
+            z = torch.from_numpy(normals(dp.seed, self.rounds & 0xFFFFFFFF, a.n)).to(device=self.device,
+                                                                                      dtype=torch.float32)
+            a.global_w.add_(self.wire.float() + z * (dp.noise_std / float(total)))
+        elif self.delta:
             a.global_w.add_(self.wire.float())
         else:
             a.global_w.copy_(self.wire.float())
@@ -379,6 +476,15 @@ class NcclSession:
         if self.reset_momentum and a.momentum is not None:
             a.momentum.zero_()
         self.rounds += 1
+
+    def dp_round(self) -> int:
+        return self.rounds & 0xFFFFFFFF
+
+    def last_clip_factors(self) -> List[float]:
+        return list(self.dp_s)
+
+    def nonfinite_updates(self) -> int:
+        return self.dp_nonfinite
 
     def join(self) -> None:
         pass
