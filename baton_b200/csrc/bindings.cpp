@@ -75,7 +75,7 @@ inline std::optional<B200AffineEpilogue> affine_epilogue(const std::optional<at:
 // ---- in-graph kernel timeline (pdl.cuh): every translation unit owns a copy of the trace pointer
 extern "C" {
 #define B200_TRACE_TUS(X) X(gemm_wgmma) X(gemm_fp8) X(quant) X(attention) X(im2col_tma) X(gemm_simt) X(fedavg) \
-  X(elementwise) X(conv) X(norm) X(loss)
+  X(elementwise) X(conv) X(norm) X(loss) X(conv_halo)
 #define B200_DECL(tu) int b200_trace_set_##tu(unsigned long long* p);
 B200_TRACE_TUS(B200_DECL)
 #undef B200_DECL
@@ -229,6 +229,28 @@ bool conv_igemm_dgrad(const at::Tensor& dy, const at::Tensor& w, at::Tensor dx, 
                                        static_cast<int>(cluster_k), static_cast<int>(force_bn), cur_stream());
   if (rc == -2) return false;
   check(rc, "conv_igemm_dgrad");
+  return true;
+}
+// halo-tiled 3x3 stride-1 convolution: src [N, H, W, 64] (x forward, dy dgrad), w [Cout, 9*Cin], out [N*H*W, Nout]
+// (Nout = Cout forward, Cin dgrad); false = shape not supported by the kernel
+bool conv_halo(const at::Tensor& src, const at::Tensor& w, at::Tensor out, bool dgrad, int64_t mc,
+               const std::optional<at::Tensor>& col_stats) {
+  CHECK_CUDA(src); CHECK_CUDA(w); CHECK_CUDA(out);
+  TORCH_CHECK(src.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16 && out.scalar_type() == at::kBFloat16 &&
+              src.dim() == 4 && src.size(3) == 64 && src.is_contiguous() && w.is_contiguous() && out.is_contiguous());
+  const int64_t rows = src.size(0) * src.size(1) * src.size(2);
+  TORCH_CHECK(rows > 0 && out.numel() % rows == 0, "conv_halo: out must hold [N*H*W, Nout] elements");
+  const int64_t nout = out.numel() / rows;
+  TORCH_CHECK(w.numel() == (dgrad ? 64 * 9 * nout : nout * 9 * 64), "conv_halo: w must be [Cout, 9*Cin]");
+  TORCH_CHECK(dgrad ? !col_stats.has_value()
+                    : (!col_stats.has_value() || (col_stats->scalar_type() == at::kFloat && col_stats->numel() >= 2 * nout)),
+              "conv_halo: col_stats is a [2 Cout] fp32 buffer of the forward");
+  const c10::cuda::CUDAGuard guard(src.device());
+  const int rc = b200_conv_halo(cptr(src), cptr(w), ptr(out), static_cast<int>(src.size(0)), static_cast<int>(src.size(1)),
+                                static_cast<int>(src.size(2)), static_cast<int>(nout), dgrad ? 1 : 0,
+                                static_cast<int>(mc), opt_ptr<float>(col_stats), cur_stream());
+  if (rc == -2) return false;
+  check(rc, "conv_halo");
   return true;
 }
 // stride 2: `ntaps` (4) taps per parity class, `taps` (4 x 4) packed tap words (ops/functional.py conv_s2_dgrad_taps)
@@ -807,6 +829,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("conv_igemm_wgrad", &conv_igemm_wgrad);
   m.def("conv_igemm_dgrad", &conv_igemm_dgrad);
   m.def("conv_igemm_dgrad_s2", &conv_igemm_dgrad_s2);
+  m.def("conv_halo", &conv_halo);
   m.def("gemm_batched", &gemm_batched);
   m.def("gemm_fp8", &gemm_fp8);
   m.def("quant_mx_rows", &quant_mx_rows);

@@ -27,6 +27,7 @@
 // the rest of the model is still landing over NVLink.
 #define B200_TU_TAG 1
 #include "ptx.cuh"
+#include "epilogue.cuh"
 #include "launch.h"
 #include "pdl.cuh"
 #include "sgd.cuh"
@@ -128,15 +129,6 @@ __device__ __forceinline__ float apply_act(float v, int act) {
   return v;
 }
 
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 __device__ __forceinline__ float4 ld_dsmem_f4(uint32_t local_smem_addr, uint32_t cta_rank) {
   uint32_t remote;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local_smem_addr), "r"(cta_rank));
@@ -148,25 +140,6 @@ __device__ __forceinline__ float4 ld_dsmem_f4(uint32_t local_smem_addr, uint32_t
   return v;
 }
 
-// bias + activation + cast + store of `NV` consecutive output columns of one row
-// Column sums of a 32 x 32 register block held one ROW per lane.  Butterfly: at every step a lane keeps one
-// half of its remaining columns and trades the other half with its partner, so after 5 steps (31 shuffles)
-// lane j owns the complete sum of column j.
-#define COLSUM_STEP(OFF, HALF)                                                  \
-  {                                                                             \
-    const bool upper = (lane & (OFF)) != 0;                                     \
-    _Pragma("unroll") for (int i = 0; i < (HALF); ++i) {                        \
-      const float keep = upper ? t[i + (HALF)] : t[i];                          \
-      const float send = upper ? t[i] : t[i + (HALF)];                          \
-      t[i] = keep + __shfl_xor_sync(0xffffffffu, send, (OFF));                  \
-    }                                                                           \
-  }
-__device__ __forceinline__ float warp_colsum32(float (&t)[32]) {
-  const uint32_t lane = lane_id();
-  COLSUM_STEP(16, 16) COLSUM_STEP(8, 8) COLSUM_STEP(4, 4) COLSUM_STEP(2, 2) COLSUM_STEP(1, 1)
-  return t[0];
-}
-#undef COLSUM_STEP
 // BatchNorm batch statistics fused into the producing GEMM: every lane of the warp must call this.  Rows
 // beyond M hold exact zeros (TMA zero-fills out-of-range operand rows; no bias / activation in this mode).
 __device__ __forceinline__ void accumulate_col_stats(const GemmParams& p, int col0, const float (&v)[32]) {
@@ -183,23 +156,6 @@ __device__ __forceinline__ void accumulate_col_stats(const GemmParams& p, int co
     atomicAdd(p.col_stats + col, cs);
     atomicAdd(p.col_stats + p.N + col, cq);
   }
-}
-
-// Same butterflies, but the warp's column sums go to shared memory (`sbuf[0:BN]` sums, `sbuf[BN:2BN]` sums of squares of
-// ONE warp): the four epilogue warps of a CTA are combined there and the CTA issues ONE global atomic per statistic
-// instead of four -- with 256 CTAs (ResNet stem) the atomics of a launch pile up on 2 N addresses and serialise in L2.
-__device__ __forceinline__ void stage_col_stats(float* sbuf, int BNv, int c, const float (&v)[32]) {
-  float s[32], q[32];
-#pragma unroll
-  for (int j = 0; j < 32; ++j) {
-    const float r = __bfloat162float(__float2bfloat16_rn(v[j]));
-    s[j] = r;
-    q[j] = r * r;
-  }
-  const float cs = warp_colsum32(s), cq = warp_colsum32(q);
-  const int lane = static_cast<int>(lane_id());
-  sbuf[c + lane] = cs;
-  sbuf[BNv + c + lane] = cq;
 }
 
 // alpha / bias / activation of one row chunk.  The (activation, bias) combination is resolved ONCE per chunk
@@ -1287,6 +1243,24 @@ extern "C" int b200_encode_map4_bf16(void* map, const void* base, long long rows
                                      int box_cols, int box_rows) {
   return b200::make_map4(reinterpret_cast<CUtensorMap*>(map), base, rows, cols, ld, inner, s_inner, outer, s_outer,
                          box_cols, box_rows);
+}
+// 4-D bf16 tensor map with an arbitrary box (conv_halo.cu: one halo box of whole images); dims innermost first,
+// `stride_bytes` of dims 1..3, 128B swizzle, out-of-bounds elements read as zero
+extern "C" int b200_encode_map4_box_bf16(void* map, const void* base, const long long* dims, const long long* stride_bytes,
+                                         const int* box) {
+  b200::EncodeTiledFn fn = b200::get_encode_fn();
+  if (fn == nullptr) return -1;
+  cuuint64_t gdim[4], gstr[3];
+  cuuint32_t bx[4], estr[4] = {1, 1, 1, 1};
+  for (int i = 0; i < 4; ++i) {
+    gdim[i] = static_cast<cuuint64_t>(dims[i]);
+    bx[i] = static_cast<cuuint32_t>(box[i]);
+    if (i < 3) gstr[i] = static_cast<cuuint64_t>(stride_bytes[i]);
+  }
+  CUresult r = fn(reinterpret_cast<CUtensorMap*>(map), CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), gdim,
+                  gstr, bx, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : static_cast<int>(r);
 }
 
 extern "C" int b200_gemm_bf16(const void* a, const void* b, void* d, const float* bias, int M, int N, int K,

@@ -358,20 +358,65 @@ def im2col(x: torch.Tensor, kh: int, kw: int, stride: int, pad: int) -> Tuple[to
     return col, ho, wo, kp
 
 
+HALO_BM = 64                      # output pixels of one halo-kernel tile (conv_halo.cu)
+_HALO_MAX_SMEM = 227 * 1024       # shared memory one H100 block may use
+
+
+def halo_smem_bytes(h: int, w: int) -> int:
+    """Shared memory of the halo kernel: the halo of ``64 / (h w)`` images (rounded up to 1 KB), nine 8 KB weight
+    slots, barriers, column statistics and the 1 KB realignment (conv_halo.cu halo_fixed_bytes)."""
+    halo = round_up((HALO_BM // (h * w)) * (h + 2) * (w + 2) * 128, 1024)
+    return halo + 9 * 8192 + 16 * 8 + 4 * 64 * 4 + 1024
+
+
+def halo_eligible(kh: int, kw: int, stride: int, pad: int, c: int, h: int, w: int, affine: Optional[dict] = None) -> bool:
+    """Whether the halo-tiled kernel takes a convolution: 3x3, stride 1, pad 1, the gathered tensor (``x`` forward,
+    ``dy`` dgrad) is one 64-channel block, a 64-row tile holds whole ``h x w`` images, the halo and the nine weight
+    slots fit in shared memory, and no eval-mode ``affine`` epilogue is asked for."""
+    return (kh == 3 and kw == 3 and stride == 1 and pad == 1 and c == 64 and h * w <= HALO_BM and
+            HALO_BM % (h * w) == 0 and affine is None and halo_smem_bytes(h, w) <= _HALO_MAX_SMEM)
+
+
+def halo_cluster(m_rows: int) -> int:
+    """CTAs of a halo-kernel cluster along M sharing the weight tiles: 4, or 2 / 1 when the tile count does not divide."""
+    tiles = (m_rows + HALO_BM - 1) // HALO_BM
+    return 4 if tiles % 4 == 0 else 2 if tiles % 2 == 0 else 1
+
+
+def _conv_path(path: Optional[str], eligible: bool) -> str:
+    if path is None:
+        return "halo" if eligible else "im2col"
+    if path not in ("halo", "im2col"):
+        raise ValueError("path must be None, 'halo' or 'im2col', not {!r}".format(path))
+    if path == "halo" and not eligible:
+        raise ValueError("the halo kernel does not take this convolution (see halo_eligible)")
+    return path
+
+
 def conv_igemm_fwd(x: torch.Tensor, w2d: torch.Tensor, kh: int, kw: int, stride: int, pad: int,
                    col_stats: Optional[torch.Tensor] = None, affine: Optional[dict] = None,
                    cluster_k: Optional[int] = None, force_bn: int = 0,
-                   out: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
+                   out: Optional[torch.Tensor] = None, path: Optional[str] = None,
+                   mc: Optional[int] = None) -> Optional[torch.Tensor]:
     """Implicit-GEMM convolution forward: ``y[N*Ho*Wo, Cout]`` straight from NHWC ``x`` through TMA
     im2col loads (no ``col`` buffer).  ``w2d``: ``[Cout, kh*kw*Cin]`` channels_last weights.  ``affine``: eval-mode
     BatchNorm epilogue as in :func:`gemm`.  ``out``: contiguous bf16 ``[N*Ho*Wo, Cout]`` to write.  Returns ``None``
-    when the shape (or the epilogue) is not supported (Cin % 64 != 0)."""
+    when the shape (or the epilogue) is not supported (Cin % 64 != 0).
+
+    ``path``: ``None`` takes the halo-tiled kernel whenever :func:`halo_eligible` holds and the im2col-mode kernel
+    otherwise; ``"halo"`` / ``"im2col"`` force one (``"halo"`` on a shape it does not take raises).  ``mc``: cluster
+    size of the halo kernel (default :func:`halo_cluster`); ``cluster_k`` / ``force_bn`` apply to the im2col path."""
     n, h, w, c = x.shape
     cout = w2d.shape[0]
     if c % 64 or w2d.shape[1] != kh * kw * c or not x.is_contiguous() or not w2d.is_contiguous():
         return None
     ho, wo = conv_out_size(h, kh, stride, pad), conv_out_size(w, kw, stride, pad)
     M, K = n * ho * wo, kh * kw * c
+    if _conv_path(path, halo_eligible(kh, kw, stride, pad, c, h, w, affine) and cout % 8 == 0) == "halo":
+        y = out if out is not None else torch.empty((M, cout), dtype=BF16, device=x.device)
+        if not load().conv_halo(x, w2d, y, False, mc or halo_cluster(M), col_stats):
+            raise RuntimeError("conv_halo declined a convolution halo_eligible admits")
+        return y
     bn = force_bn or pick_bn(M, cout)
     if cluster_k is None:
         cluster_k = pick_cluster_k(M, cout, K, bn)
@@ -415,17 +460,24 @@ def conv_s2_dgrad_taps(kh: int, kw: int, pad: int, ho: int, wo: int) -> Optional
 
 
 def conv_igemm_dgrad(dy: torch.Tensor, w2d: torch.Tensor, in_shape, kh: int, kw: int, pad: int, stride: int = 1,
-                     out: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
+                     out: Optional[torch.Tensor] = None, path: Optional[str] = None,
+                     mc: Optional[int] = None) -> Optional[torch.Tensor]:
     """Implicit-GEMM input gradient of a stride-1 or stride-2 convolution: ``dx[N, H, W, Cin]`` from NHWC ``dy`` and
     the channels_last weights ``w2d [Cout, kh*kw*Cin]``, gathered by TMA im2col, with the weight slab of each tap
     loaded MN-major in place (no ``dcol`` buffer, no col2im, no weight transpose).  Stride 1: the flipped-filter
     convolution of ``dy``.  Stride 2: one launch over the four parity classes of :func:`conv_s2_dgrad_taps`.
     ``out``: contiguous bf16 ``[N, H, W, Cin]`` to write (every element is written).  Returns ``None`` when the shape
-    is not supported (channels not multiples of 64, other strides)."""
+    is not supported (channels not multiples of 64, other strides).  ``path`` / ``mc``: as in :func:`conv_igemm_fwd`
+    (the halo kernel gathers ``dy``, so ``Cout`` must be 64)."""
     n, h, w, c = in_shape
     cout = dy.shape[-1]
     if c % 64 or cout % 64 or w2d.shape[1] != kh * kw * c or not dy.is_contiguous() or not w2d.is_contiguous():
         return None
+    if _conv_path(path, halo_eligible(kh, kw, stride, pad, cout, h, w)) == "halo":
+        dx = out if out is not None else torch.empty((n, h, w, c), dtype=BF16, device=dy.device)
+        if not load().conv_halo(dy, w2d, dx, True, mc or halo_cluster(n * h * w), None):
+            raise RuntimeError("conv_halo declined a convolution halo_eligible admits")
+        return dx
     if stride == 1:
         M, K = n * h * w, kh * kw * cout
         bn = pick_bn(M, c)

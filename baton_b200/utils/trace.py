@@ -18,12 +18,12 @@ from __future__ import annotations
 import collections
 import os
 import re
-from typing import Dict, List, Tuple
+from typing import Callable, Dict, List, Tuple
 
 import torch
 
 _TUS = ["?", "gemm_wgmma", "gemm_fp8", "quant", "attention", "im2col_tma", "gemm_simt", "fedavg", "elementwise",
-        "conv", "norm", "loss"]
+        "conv", "norm", "loss", "conv_halo"]
 _CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "csrc")
 _NAME_CACHE: Dict[int, str] = {}
 
@@ -71,6 +71,28 @@ def kernel_name(tag: int) -> str:
     return name
 
 
+def timeline_rows(records: List[Tuple[int, int]], name: Callable[[int], str] = kernel_name) -> List[dict]:
+    """Rows of :meth:`KernelTrace.timeline` from time-sorted ``(t_ns, tag)`` records.  The "resident" stamp
+    (griddep_launch_dependents) and the "dependencies done" stamp (griddep_wait) of one launch sit on different source
+    lines, so their tags differ: they are paired per kernel NAME, first resident stamp to first dependencies-done stamp."""
+    resident = collections.defaultdict(collections.deque)
+    rows = []
+    for t, tag in records:
+        if abs(tag) >= POINT_BASE:
+            continue
+        k = name(tag)
+        if tag < 0:
+            resident[k].append(t)
+        else:
+            pre = resident[k].popleft() if resident[k] else t
+            rows.append({"t_ns": t, "tag": tag, "name": k, "early_ns": t - pre})
+    for a, b in zip(rows, rows[1:]):
+        a["slot_ns"] = b["t_ns"] - a["t_ns"]
+    if rows:
+        rows[-1]["slot_ns"] = 0
+    return rows
+
+
 class KernelTrace:
     def __init__(self, capacity: int = 1 << 16, device=None):
         from ..ops._ext import load
@@ -102,20 +124,7 @@ class KernelTrace:
     def timeline(self) -> List[dict]:
         """One row per kernel: start of its critical-path slot (dependencies done), the slot length (until the next
         kernel's dependencies are done) and how long before that its first CTA was already resident (PDL overlap)."""
-        rec = [r for r in self.records() if abs(r[1]) < POINT_BASE]
-        resident = collections.defaultdict(list)
-        rows = []
-        for t, tag in rec:
-            if tag < 0:
-                resident[-tag].append(t)
-            else:
-                pre = resident[tag].pop(0) if resident[tag] else t
-                rows.append({"t_ns": t, "tag": tag, "name": kernel_name(tag), "early_ns": t - pre})
-        for a, b in zip(rows, rows[1:]):
-            a["slot_ns"] = b["t_ns"] - a["t_ns"]
-        if rows:
-            rows[-1]["slot_ns"] = 0
-        return rows
+        return timeline_rows(self.records())
 
     def points(self) -> List[Tuple[int, str]]:
         """``[(t_ns, label)]`` of everything in time order: kernel starts (``> name``) and intra-kernel TRACE_POINTs."""
