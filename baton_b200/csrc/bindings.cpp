@@ -34,19 +34,34 @@ inline const float* prox_anchor(const std::optional<at::Tensor>& anchor, int64_t
   return anchor->data_ptr<float>();
 }
 
-// optimizer epilogue of a weight-gradient GEMM: theta / theta_bf16 / momentum / anchor start at the element of D[0, 0]
+// SCAFFOLD correction of an SGD step: fp32, contiguous, at least as long as the parameters it corrects; no anchor
+inline const float* scaf_corr(const std::optional<at::Tensor>& corr, int64_t numel, const float* anchor) {
+  if (!corr.has_value() || !corr->defined()) return nullptr;
+  CHECK_CUDA(*corr);
+  TORCH_CHECK(corr->scalar_type() == at::kFloat && corr->is_contiguous() && corr->numel() >= numel,
+              "scaffold correction: contiguous fp32 covering the parameters");
+  TORCH_CHECK(anchor == nullptr, "an SGD step takes a FedProx anchor or a SCAFFOLD correction, not both");
+  return corr->data_ptr<float>();
+}
+
+// optimizer epilogue of a weight-gradient GEMM: theta / theta_bf16 / momentum / anchor / correction start at the element
+// of D[0, 0]
 inline std::optional<B200SgdEpilogue> sgd_epilogue(const std::optional<at::Tensor>& theta,
                                                    const std::optional<at::Tensor>& theta_bf16,
                                                    const std::optional<at::Tensor>& mom,
                                                    const std::optional<at::Tensor>& hyper, bool nesterov,
-                                                   const std::optional<at::Tensor>& anchor) {
+                                                   const std::optional<at::Tensor>& anchor,
+                                                   const std::optional<at::Tensor>& corr) {
   if (!hyper.has_value() || !hyper->defined()) return std::nullopt;
   TORCH_CHECK(theta.has_value() && theta->scalar_type() == at::kFloat && hyper->scalar_type() == at::kFloat &&
                   (!theta_bf16.has_value() || theta_bf16->scalar_type() == at::kBFloat16) &&
                   (!mom.has_value() || mom->scalar_type() == at::kFloat),
               "sgd epilogue: fp32 theta / momentum / hyper, bf16 shadow");
+  const float* a = prox_anchor(anchor, theta->numel(), *hyper);
+  // theta runs to the end of the arena, the correction to the end of the parameters: the GEMM only addresses its
+  // output's elements, which are parameters
   return B200SgdEpilogue{theta->data_ptr<float>(), opt_ptr<void>(theta_bf16), opt_ptr<float>(mom),
-                         hyper->data_ptr<float>(), nesterov ? 1 : 0, prox_anchor(anchor, theta->numel(), *hyper)};
+                         hyper->data_ptr<float>(), nesterov ? 1 : 0, a, scaf_corr(corr, 0, a)};
 }
 
 // eval-mode BatchNorm epilogue of a forward GEMM: fp32 [N] scale and shift, optional bf16 residual rows
@@ -104,7 +119,8 @@ bool gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor d, const std::opt
           const std::optional<at::Tensor>& col_stats, const std::optional<at::Tensor>& flag_epoch_word,
           const std::optional<at::Tensor>& sgd_theta, const std::optional<at::Tensor>& sgd_theta_bf16,
           const std::optional<at::Tensor>& sgd_mom, const std::optional<at::Tensor>& sgd_hyper, bool sgd_nesterov,
-          const std::optional<at::Tensor>& sgd_anchor, const std::optional<at::Tensor>& bn_scale, const std::optional<at::Tensor>& bn_shift,
+          const std::optional<at::Tensor>& sgd_anchor, const std::optional<at::Tensor>& sgd_corr,
+          const std::optional<at::Tensor>& bn_scale, const std::optional<at::Tensor>& bn_shift,
           const std::optional<at::Tensor>& residual, bool bn_relu) {
   CHECK_CUDA(a); CHECK_CUDA(b); CHECK_CUDA(d);
   TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16, "gemm operands must be bf16");
@@ -123,7 +139,7 @@ bool gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor d, const std::opt
     return true;
   }
   const std::optional<B200SgdEpilogue> sgd =
-      sgd_epilogue(sgd_theta, sgd_theta_bf16, sgd_mom, sgd_hyper, sgd_nesterov, sgd_anchor);
+      sgd_epilogue(sgd_theta, sgd_theta_bf16, sgd_mom, sgd_hyper, sgd_nesterov, sgd_anchor, sgd_corr);
   const std::optional<B200AffineEpilogue> affine = affine_epilogue(bn_scale, bn_shift, residual, bn_relu, M, N);
   const int rc = b200_gemm_bf16(cptr(a), cptr(b), ptr(d), bp, M, N, K, lda, ldb, ldd, a_mn, b_mn, out_fp32, act, split_k,
                                 accumulate, static_cast<float>(alpha), opt_ptr<const uint32_t>(flags),
@@ -277,13 +293,14 @@ bool conv_igemm_wgrad(const at::Tensor& dy, const at::Tensor& x, at::Tensor dw, 
                       int64_t stride, int64_t pad, int64_t ho, int64_t wo, int64_t split_k, int64_t force_bn,
                       const std::optional<at::Tensor>& sgd_theta, const std::optional<at::Tensor>& sgd_theta_bf16,
                       const std::optional<at::Tensor>& sgd_mom, const std::optional<at::Tensor>& sgd_hyper,
-                      bool sgd_nesterov, const std::optional<at::Tensor>& sgd_anchor) {
+                      bool sgd_nesterov, const std::optional<at::Tensor>& sgd_anchor,
+                      const std::optional<at::Tensor>& sgd_corr) {
   CHECK_CUDA(dy); CHECK_CUDA(x); CHECK_CUDA(dw);
   TORCH_CHECK(x.scalar_type() == at::kBFloat16 && dy.scalar_type() == at::kBFloat16 && dw.scalar_type() == at::kFloat &&
               x.dim() == 4 && x.is_contiguous() && dy.is_contiguous());
   const c10::cuda::CUDAGuard guard(x.device());
   const std::optional<B200SgdEpilogue> sgd =
-      sgd_epilogue(sgd_theta, sgd_theta_bf16, sgd_mom, sgd_hyper, sgd_nesterov, sgd_anchor);
+      sgd_epilogue(sgd_theta, sgd_theta_bf16, sgd_mom, sgd_hyper, sgd_nesterov, sgd_anchor, sgd_corr);
   const int rc = b200_conv_igemm_wgrad(cptr(dy), cptr(x), dw.data_ptr<float>(), static_cast<int>(x.size(0)),
                                        static_cast<int>(x.size(1)), static_cast<int>(x.size(2)), static_cast<int>(x.size(3)),
                                        static_cast<int>(cout), static_cast<int>(kh), static_cast<int>(kw),
@@ -325,33 +342,59 @@ void dequant_mx(const at::Tensor& q, const at::Tensor& sf, at::Tensor out, int64
 void fused_sgd(at::Tensor w, at::Tensor g, const std::optional<at::Tensor>& mom, const std::optional<at::Tensor>& wb,
                const at::Tensor& hyper, bool zero_grad, bool nesterov, const std::optional<at::Tensor>& wire_slot,
                const std::optional<at::Tensor>& pack_global, const std::optional<at::Tensor>& pack_scale, int64_t n_pack,
-               bool wire_fp32, const std::optional<at::Tensor>& prox_anchor_) {
+               bool wire_fp32, const std::optional<at::Tensor>& prox_anchor_, const std::optional<at::Tensor>& corr) {
   CHECK_CUDA(w);
   TORCH_CHECK(w.scalar_type() == at::kFloat && g.scalar_type() == at::kFloat && hyper.scalar_type() == at::kFloat);
   TORCH_CHECK(w.is_contiguous() && g.is_contiguous() && w.numel() == g.numel());
   const c10::cuda::CUDAGuard guard(w.device());
+  const float* anchor = prox_anchor(prox_anchor_, w.numel(), hyper);
   check(b200_fused_sgd(w.data_ptr<float>(), g.data_ptr<float>(), opt_ptr<float>(mom), opt_ptr<void>(wb), w.numel(),
                        hyper.data_ptr<float>(), zero_grad, nesterov,
                        reinterpret_cast<const unsigned long long*>(opt_ptr<const int64_t>(wire_slot)),
-                       opt_ptr<const float>(pack_global), opt_ptr<const float>(pack_scale), n_pack, wire_fp32,
-                       prox_anchor(prox_anchor_, w.numel(), hyper), cur_stream()),
+                       opt_ptr<const float>(pack_global), opt_ptr<const float>(pack_scale), n_pack, wire_fp32, anchor,
+                       scaf_corr(corr, w.numel(), anchor), cur_stream()),
         "fused_sgd");
 }
 
 // segments: int64 [n][3] device table {offset, length, kind} over the arena (see fused_sgd_segments_kernel)
 void fused_sgd_segments(at::Tensor w, at::Tensor g, const std::optional<at::Tensor>& mom,
                         const std::optional<at::Tensor>& wb, const at::Tensor& segments, const at::Tensor& hyper,
-                        bool nesterov, const std::optional<at::Tensor>& prox_anchor_) {
+                        bool nesterov, const std::optional<at::Tensor>& prox_anchor_,
+                        const std::optional<at::Tensor>& corr) {
   CHECK_CUDA(w); CHECK_CUDA(segments);
   TORCH_CHECK(w.scalar_type() == at::kFloat && g.scalar_type() == at::kFloat && hyper.scalar_type() == at::kFloat);
   TORCH_CHECK(segments.scalar_type() == at::kLong && segments.dim() == 2 && segments.size(1) == 3 &&
               segments.is_contiguous(), "segments: contiguous int64 [n, 3]");
   const c10::cuda::CUDAGuard guard(w.device());
+  const float* anchor = prox_anchor(prox_anchor_, w.numel(), hyper);
   check(b200_fused_sgd_segments(w.data_ptr<float>(), g.data_ptr<float>(), opt_ptr<float>(mom), opt_ptr<void>(wb),
                                 reinterpret_cast<const long long*>(segments.data_ptr<int64_t>()),
-                                static_cast<int>(segments.size(0)), hyper.data_ptr<float>(), nesterov,
-                                prox_anchor(prox_anchor_, w.numel(), hyper), cur_stream()),
+                                static_cast<int>(segments.size(0)), hyper.data_ptr<float>(), nesterov, anchor,
+                                scaf_corr(corr, g.numel(), anchor), cur_stream()),
         "fused_sgd_segments");
+}
+
+// SCAFFOLD control variates over the parameters: every buffer fp32, contiguous, at least n elements
+inline void check_cv(const at::Tensor& t, int64_t n) {
+  CHECK_CUDA(t);
+  TORCH_CHECK(t.scalar_type() == at::kFloat && t.is_contiguous() && t.numel() >= n,
+              "scaffold: contiguous fp32 buffers covering the parameters");
+}
+void scaffold_corr(at::Tensor corr, const at::Tensor& c, const at::Tensor& ci) {
+  const int64_t n = corr.numel();
+  check_cv(corr, n); check_cv(c, n); check_cv(ci, n);
+  const c10::cuda::CUDAGuard guard(corr.device());
+  check(b200_scaffold_corr(corr.data_ptr<float>(), c.data_ptr<float>(), ci.data_ptr<float>(), n, cur_stream()),
+        "scaffold_corr");
+}
+void scaffold_dc(at::Tensor up, at::Tensor ci, const at::Tensor& c, const at::Tensor& global_w, const at::Tensor& theta,
+                 double inv_k_eta, bool first) {
+  const int64_t n = up.numel();
+  check_cv(up, n); check_cv(ci, n); check_cv(c, n); check_cv(global_w, n); check_cv(theta, n);
+  const c10::cuda::CUDAGuard guard(up.device());
+  check(b200_scaffold_dc(up.data_ptr<float>(), ci.data_ptr<float>(), c.data_ptr<float>(), global_w.data_ptr<float>(),
+                         theta.data_ptr<float>(), n, static_cast<float>(inv_k_eta), first ? 1 : 0, cur_stream()),
+        "scaffold_dc");
 }
 
 void fold_client(at::Tensor acc, at::Tensor theta, const at::Tensor& global_w, const std::optional<at::Tensor>& wb,
@@ -470,7 +513,9 @@ void fedavg_allreduce(const std::vector<int64_t>& wire_ptrs, const std::vector<i
                       bool delta, bool use_nvls, int64_t epoch, const std::optional<at::Tensor>& tile_flags,
                       int64_t flag_value, int64_t tile_elems, int64_t n_ctas, int64_t timeout_log2,
                       const std::optional<at::Tensor>& status, const std::optional<at::Tensor>& phase_ns, bool prepacked,
-                      const std::vector<int64_t>& clip_page_ptrs, double dp_noise_std, int64_t dp_seed, int64_t dp_round) {
+                      const std::vector<int64_t>& clip_page_ptrs, double dp_noise_std, int64_t dp_seed, int64_t dp_round,
+                      const std::optional<at::Tensor>& scaf_dc, const std::optional<at::Tensor>& scaf_c,
+                      int64_t scaf_seg1_off, double scaf_inv_clients) {
   CHECK_CUDA(theta);
   TORCH_CHECK(world <= B200_MAX_RANKS && static_cast<int64_t>(wire_ptrs.size()) == world &&
               static_cast<int64_t>(pad_ptrs.size()) == world && static_cast<int64_t>(n_samples.size()) == world);
@@ -528,6 +573,22 @@ void fedavg_allreduce(const std::vector<int64_t>& wire_ptrs, const std::vector<i
   }
   TORCH_CHECK(!delta || a.global_w != nullptr, "delta mode needs the global copy");
   TORCH_CHECK(!use_nvls || a.wire_mc != nullptr, "NVLS mode needs the multicast address");
+  // SCAFFOLD: the control-variate segment (dc in, c updated) rides in the same launch
+  if (scaf_c.has_value() && scaf_c->defined()) {
+    TORCH_CHECK(!dp && delta && !use_nvls, "SCAFFOLD rounds need delta mode on peer loads, without DP");
+    TORCH_CHECK(scaf_dc.has_value() && scaf_dc->defined(), "SCAFFOLD: dc and c go together");
+    check_cv(*scaf_c, scaf_c->numel());
+    check_cv(*scaf_dc, scaf_c->numel());
+    FedAvgScaffoldArgs sa = {};
+    static_cast<FedAvgArgs&>(sa) = static_cast<const FedAvgArgs&>(a);
+    sa.dc = scaf_dc->data_ptr<float>();
+    sa.c = scaf_c->data_ptr<float>();
+    sa.n_c = scaf_c->numel();
+    sa.seg1_off = scaf_seg1_off;
+    sa.inv_clients = static_cast<float>(scaf_inv_clients);
+    check(b200_fedavg_allreduce_scaffold(&sa, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce");
+    return;
+  }
   check(dp ? b200_fedavg_allreduce_dp(&a, static_cast<int>(n_ctas), cur_stream())
            : b200_fedavg_allreduce(&a, static_cast<int>(n_ctas), cur_stream()),
         "fedavg_allreduce");
@@ -839,6 +900,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fused_sgd_segments", &fused_sgd_segments);
   m.def("weighted_sum", &weighted_sum);
   m.def("fold_client", &fold_client);
+  m.def("scaffold_corr", &scaffold_corr);
+  m.def("scaffold_dc", &scaffold_dc);
   m.def("cast", &cast);
   m.def("gather_rows", &gather_rows);
   m.def("colsum", &colsum);

@@ -35,12 +35,15 @@ struct SgdPack {
   int wire_fp32;                         // 0: bf16 wire, 1: fp32 wire
 };
 
-// PROX: FedProx step toward `anchor` (indexed like w); otherwise `anchor` is not read.
-template <bool PROX>
+// PROX: FedProx step toward the anchor `aux` (indexed like w).  SCAF: SCAFFOLD step, `aux` is the correction c - c_i
+// (indexed like w).  The two are exclusive; with neither, `aux` is not read.  One pointer serves both so the plain and
+// FedProx instantiations keep their parameter list.
+template <bool PROX, bool SCAF = false>
 __global__ void __launch_bounds__(EW_THREADS)
 fused_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict__ mom,
                  __nv_bfloat16* __restrict__ wb, long long n, const float* __restrict__ hyper, int zero_grad,
-                 int nesterov, const SgdPack pk, const float* __restrict__ anchor) {
+                 int nesterov, const SgdPack pk, const float* __restrict__ aux) {
+  static_assert(!(PROX && SCAF), "FedProx and SCAFFOLD are exclusive");
   griddep_launch_dependents();
   griddep_wait();
   const SgdHyper h = PROX ? load_sgd_hyper_prox(hyper) : load_sgd_hyper(hyper);
@@ -52,16 +55,19 @@ fused_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict
     if (pk.scale != nullptr) pscale = *pk.scale;
   }
   // delta upload of a FedProx step: the anchor IS the global copy the wire value is taken against -- read it once
-  const bool anchor_is_global = PROX && anchor == pk.global_w;
+  const bool anchor_is_global = PROX && aux == pk.global_w;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < nv;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     float4 mv = mom != nullptr ? reinterpret_cast<float4*>(mom)[i] : make_float4(0.f, 0.f, 0.f, 0.f);
     float4 av = make_float4(0.f, 0.f, 0.f, 0.f);
     float4 wv;
     if constexpr (PROX) {
-      av = reinterpret_cast<const float4*>(anchor)[i];
+      av = reinterpret_cast<const float4*>(aux)[i];
       wv = sgd_update4_prox(h, reinterpret_cast<float4*>(w)[i], reinterpret_cast<float4*>(g)[i], av, mv,
                             mom != nullptr, nesterov);
+    } else if constexpr (SCAF) {
+      wv = sgd_update4_scaf(h, reinterpret_cast<float4*>(w)[i], reinterpret_cast<float4*>(g)[i],
+                            reinterpret_cast<const float4*>(aux)[i], mv, mom != nullptr, nesterov);
     } else {
       wv = sgd_update4(h, reinterpret_cast<float4*>(w)[i], reinterpret_cast<float4*>(g)[i], mv, mom != nullptr,
                        nesterov);
@@ -99,8 +105,9 @@ fused_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict
   if (blockIdx.x == 0) {
     for (long long i = (nv << 2) + threadIdx.x; i < n; i += blockDim.x) {
       float mv = mom != nullptr ? mom[i] : 0.f;
-      const float wv = PROX ? sgd_update_prox(h, w[i], g[i], anchor[i], mv, mom != nullptr, nesterov)
-                            : sgd_update(h, w[i], g[i], mv, mom != nullptr, nesterov);
+      const float wv = PROX ? sgd_update_prox(h, w[i], g[i], aux[i], mv, mom != nullptr, nesterov)
+                       : SCAF ? sgd_update_scaf(h, w[i], g[i], aux[i], mv, mom != nullptr, nesterov)
+                              : sgd_update(h, w[i], g[i], mv, mom != nullptr, nesterov);
       if (mom != nullptr) mom[i] = mv;
       w[i] = wv;
       if (zero_grad) g[i] = 0.f;
@@ -124,21 +131,24 @@ __device__ __forceinline__ bool same_bits4(float4 a, float4 b) {
 //           graph stays exact when it is replayed with new hyper-parameters.
 // With an anchor (FedProx) a kind-1 element moves only by prox*(w - a) [+ wd*w]: without a momentum buffer it is stored
 // only where its bits change.  In engine rounds these taps equal the global model all round, so nothing is written.
-template <bool PROX>
+// SCAF (`aux` = the correction c - c_i, as in fused_sgd_kernel): a kind-1 element moves by -lr * (corr [+ wd*w]), so
+// kind-1 chunks are never skipped; they use the same sparse store (a zero correction writes nothing).
+template <bool PROX, bool SCAF = false>
 __global__ void __launch_bounds__(EW_THREADS)
 fused_sgd_segments_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict__ mom,
                           __nv_bfloat16* __restrict__ wb, const long long* __restrict__ seg, int n_seg,
-                          const float* __restrict__ hyper, int nesterov, const float* __restrict__ anchor) {
+                          const float* __restrict__ hyper, int nesterov, const float* __restrict__ aux) {
+  static_assert(!(PROX && SCAF), "FedProx and SCAFFOLD are exclusive");
   griddep_launch_dependents();
   griddep_wait();
   const SgdHyper h = PROX ? load_sgd_hyper_prox(hyper) : load_sgd_hyper(hyper);
   const bool has_mom = mom != nullptr;
-  const bool nograd_is_identity = h.prox == 0.f && h.wd == 0.f && !has_mom;
+  const bool nograd_is_identity = !SCAF && h.prox == 0.f && h.wd == 0.f && !has_mom;
   for (int s = blockIdx.x; s < n_seg; s += gridDim.x) {
     const long long off = seg[3 * s], len = seg[3 * s + 1];
     const bool has_grad = seg[3 * s + 2] == 0;
     if (!has_grad && nograd_is_identity) continue;      // block-uniform
-    const bool sparse_store = PROX && !has_grad && !has_mom;
+    const bool sparse_store = (PROX || SCAF) && !has_grad && !has_mom;
     long long done = 0;
     if ((off & 3) == 0) {
       const long long nv = len >> 2;
@@ -147,9 +157,11 @@ fused_sgd_segments_kernel(float* __restrict__ w, float* __restrict__ g, float* _
         float4 mv = has_mom ? *reinterpret_cast<float4*>(mom + e) : make_float4(0.f, 0.f, 0.f, 0.f);
         const float4 gv = has_grad ? *reinterpret_cast<float4*>(g + e) : make_float4(0.f, 0.f, 0.f, 0.f);
         const float4 w0 = *reinterpret_cast<float4*>(w + e);
-        const float4 wv = PROX ? sgd_update4_prox(h, w0, gv, *reinterpret_cast<const float4*>(anchor + e), mv, has_mom,
+        const float4 wv = PROX ? sgd_update4_prox(h, w0, gv, *reinterpret_cast<const float4*>(aux + e), mv, has_mom,
                                                   nesterov)
-                               : sgd_update4(h, w0, gv, mv, has_mom, nesterov);
+                          : SCAF ? sgd_update4_scaf(h, w0, gv, *reinterpret_cast<const float4*>(aux + e), mv, has_mom,
+                                                    nesterov)
+                                 : sgd_update4(h, w0, gv, mv, has_mom, nesterov);
         if (has_mom) *reinterpret_cast<float4*>(mom + e) = mv;
         if (sparse_store && same_bits4(w0, wv)) continue;
         *reinterpret_cast<float4*>(w + e) = wv;
@@ -163,8 +175,9 @@ fused_sgd_segments_kernel(float* __restrict__ w, float* __restrict__ g, float* _
       float mv = has_mom ? mom[e] : 0.f;
       const float gv = has_grad ? g[e] : 0.f;
       const float w0 = w[e];
-      const float wv = PROX ? sgd_update_prox(h, w0, gv, anchor[e], mv, has_mom, nesterov)
-                            : sgd_update(h, w0, gv, mv, has_mom, nesterov);
+      const float wv = PROX ? sgd_update_prox(h, w0, gv, aux[e], mv, has_mom, nesterov)
+                       : SCAF ? sgd_update_scaf(h, w0, gv, aux[e], mv, has_mom, nesterov)
+                              : sgd_update(h, w0, gv, mv, has_mom, nesterov);
       if (has_mom) mom[e] = mv;
       if (sparse_store && __float_as_uint(w0) == __float_as_uint(wv)) continue;
       w[e] = wv;
@@ -204,6 +217,48 @@ fold_client_kernel(float* __restrict__ acc, float* __restrict__ theta, const flo
       if (wb != nullptr) reinterpret_cast<uint2*>(wb)[i] = make_uint2(pack_bf16x2(g.x, g.y), pack_bf16x2(g.z, g.w));
       if (mom != nullptr && (i << 2) < n_mom) reinterpret_cast<float4*>(mom)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
+  }
+}
+
+// ------------------------------------------------------------------ SCAFFOLD control variates (n = the parameters)
+// Before client i trains: corr = c - c_i (the correction its SGD steps add to the gradient).
+__global__ void __launch_bounds__(EW_THREADS)
+scaffold_corr_kernel(float* __restrict__ corr, const float* __restrict__ c, const float* __restrict__ ci, long long n) {
+  griddep_launch_dependents();
+  griddep_wait();
+  const long long nv = n >> 2;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < nv;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float4 a = reinterpret_cast<const float4*>(c)[i], b = reinterpret_cast<const float4*>(ci)[i];
+    reinterpret_cast<float4*>(corr)[i] = make_float4(a.x - b.x, a.y - b.y, a.z - b.z, a.w - b.w);
+  }
+}
+
+// After client i trained K steps at lr eta (option II of the paper): dc = (global - theta) * inv_k_eta - c with
+// inv_k_eta = 1 / (K eta); c_i += dc; and the rank's upload of the control-variate segment up = dc (first hosted
+// client of the round) or up += dc (later ones).  Runs before the logical-client fold resets theta.
+__global__ void __launch_bounds__(EW_THREADS)
+scaffold_dc_kernel(float* __restrict__ up, float* __restrict__ ci, const float* __restrict__ c,
+                   const float* __restrict__ global_w, const float* __restrict__ theta, long long n, float inv_k_eta,
+                   int first) {
+  griddep_launch_dependents();
+  griddep_wait();
+  const long long nv = n >> 2;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < nv;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float4 g = reinterpret_cast<const float4*>(global_w)[i], t = reinterpret_cast<const float4*>(theta)[i];
+    const float4 cv = reinterpret_cast<const float4*>(c)[i];
+    const float4 d = make_float4(fmaf(g.x - t.x, inv_k_eta, -cv.x), fmaf(g.y - t.y, inv_k_eta, -cv.y),
+                                 fmaf(g.z - t.z, inv_k_eta, -cv.z), fmaf(g.w - t.w, inv_k_eta, -cv.w));
+    float4 a = reinterpret_cast<const float4*>(ci)[i];
+    a.x += d.x; a.y += d.y; a.z += d.z; a.w += d.w;
+    reinterpret_cast<float4*>(ci)[i] = a;
+    float4 u = d;
+    if (!first) {
+      const float4 p = reinterpret_cast<const float4*>(up)[i];
+      u.x += p.x; u.y += p.y; u.z += p.z; u.w += p.w;
+    }
+    reinterpret_cast<float4*>(up)[i] = u;
   }
 }
 
@@ -541,27 +596,54 @@ using namespace b200;
 extern "C" int b200_fused_sgd(float* w, float* g, float* mom, void* w_bf16, long long n, const float* hyper,
                               int zero_grad, int nesterov, const unsigned long long* wire_slot,
                               const float* pack_global, const float* pack_scale, long long n_pack, int wire_fp32,
-                              const float* prox_anchor, cudaStream_t stream) {
+                              const float* prox_anchor, const float* corr, cudaStream_t stream) {
   if (n <= 0) return 0;
   SgdPack pk;
   pk.wire_slot = wire_slot; pk.global_w = pack_global; pk.scale = pack_scale;
   pk.n_pack = n_pack > n ? n_pack : n; pk.wire_fp32 = wire_fp32;
   if (wire_slot != nullptr && ((n & 7) || (pk.n_pack & 7))) return -2;
-  if (reinterpret_cast<uintptr_t>(prox_anchor) & 15) return -2;      // read as float4 at the offsets of w
-  launch_pdl(prox_anchor != nullptr ? fused_sgd_kernel<true> : fused_sgd_kernel<false>, ew_grid(n >> 2), EW_THREADS, 0,
-             stream, w, g, mom, reinterpret_cast<__nv_bfloat16*>(w_bf16), n, hyper, zero_grad, nesterov, pk, prox_anchor);
+  if (prox_anchor != nullptr && corr != nullptr) return -2;
+  // read as float4 at the offsets of w
+  if ((reinterpret_cast<uintptr_t>(prox_anchor) | reinterpret_cast<uintptr_t>(corr)) & 15) return -2;
+  auto kernel = prox_anchor != nullptr ? fused_sgd_kernel<true>
+                : corr != nullptr      ? fused_sgd_kernel<false, true>
+                                       : fused_sgd_kernel<false>;
+  launch_pdl(kernel, ew_grid(n >> 2), EW_THREADS, 0, stream, w, g, mom, reinterpret_cast<__nv_bfloat16*>(w_bf16), n,
+             hyper, zero_grad, nesterov, pk, prox_anchor != nullptr ? prox_anchor : corr);
   RET_LAST();
 }
 extern "C" int b200_fused_sgd_segments(float* w, float* g, float* mom, void* w_bf16, const long long* segments, int n_seg,
-                                       const float* hyper, int nesterov, const float* prox_anchor, cudaStream_t stream) {
+                                       const float* hyper, int nesterov, const float* prox_anchor, const float* corr,
+                                       cudaStream_t stream) {
   if (n_seg <= 0) return 0;
   if ((reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(mom) |
-       reinterpret_cast<uintptr_t>(prox_anchor)) & 15 ||
+       reinterpret_cast<uintptr_t>(prox_anchor) | reinterpret_cast<uintptr_t>(corr)) & 15 ||
       reinterpret_cast<uintptr_t>(w_bf16) & 7)
     return -2;
-  launch_pdl(prox_anchor != nullptr ? fused_sgd_segments_kernel<true> : fused_sgd_segments_kernel<false>,
-             ew_grid(n_seg * static_cast<long long>(EW_THREADS)), EW_THREADS, 0, stream, w, g, mom,
-             reinterpret_cast<__nv_bfloat16*>(w_bf16), segments, n_seg, hyper, nesterov, prox_anchor);
+  if (prox_anchor != nullptr && corr != nullptr) return -2;
+  auto kernel = prox_anchor != nullptr ? fused_sgd_segments_kernel<true>
+                : corr != nullptr      ? fused_sgd_segments_kernel<false, true>
+                                       : fused_sgd_segments_kernel<false>;
+  launch_pdl(kernel, ew_grid(n_seg * static_cast<long long>(EW_THREADS)), EW_THREADS, 0, stream, w, g, mom,
+             reinterpret_cast<__nv_bfloat16*>(w_bf16), segments, n_seg, hyper, nesterov,
+             prox_anchor != nullptr ? prox_anchor : corr);
+  RET_LAST();
+}
+extern "C" int b200_scaffold_corr(float* corr, const float* c, const float* ci, long long n, cudaStream_t stream) {
+  if (n <= 0) return 0;
+  if ((n & 3) || ((reinterpret_cast<uintptr_t>(corr) | reinterpret_cast<uintptr_t>(c) |
+                   reinterpret_cast<uintptr_t>(ci)) & 15))
+    return -2;
+  launch_pdl(scaffold_corr_kernel, ew_grid(n >> 2), EW_THREADS, 0, stream, corr, c, ci, n);
+  RET_LAST();
+}
+extern "C" int b200_scaffold_dc(float* up, float* ci, const float* c, const float* global_w, const float* theta,
+                                long long n, float inv_k_eta, int first, cudaStream_t stream) {
+  if (n <= 0) return 0;
+  if ((n & 3) || ((reinterpret_cast<uintptr_t>(up) | reinterpret_cast<uintptr_t>(ci) | reinterpret_cast<uintptr_t>(c) |
+                   reinterpret_cast<uintptr_t>(global_w) | reinterpret_cast<uintptr_t>(theta)) & 15))
+    return -2;
+  launch_pdl(scaffold_dc_kernel, ew_grid(n >> 2), EW_THREADS, 0, stream, up, ci, c, global_w, theta, n, inv_k_eta, first);
   RET_LAST();
 }
 extern "C" int b200_fold_client(float* acc, float* theta, const float* global_w, void* w_bf16, float* mom, long long n_mom,

@@ -192,11 +192,150 @@ __device__ __forceinline__ void phase_stamp(const FedAvgArgs& a, int slot) {
 #endif
 }
 
+// ---------------------------------------------------------------- SCAFFOLD: the control-variate segment
+// Segment 1 of a SCAFFOLD round is a second wire of n elements at byte offset `off` of every rank's wire half (fp8:
+// its scale bytes behind its n payload bytes).  Its tiles are mapped to owners and CTAs exactly like segment 0's
+// (owner = (t mod A)-th live rank, CTA = (t div A) mod G), so the per-CTA barriers of the round cover it too.  The three
+// phases below are kept apart from fedavg_round's own loops so the plain and DP kernels keep their instruction streams.
+
+// phase 0: wire = cast(src) over the tiles this CTA packs
+template <int WIRE>
+__device__ __forceinline__ void seg_pack(uint8_t* wire, const float* __restrict__ src, long long n, int T, int A, int G) {
+  using W = Wire<WIRE>;
+  constexpr int VEC = W::VEC;
+  constexpr size_t esz = W::VBYTES / VEC;
+  const long long n_tiles = (n + T - 1) / T;
+  const int lane_elems = static_cast<int>(threadIdx.x & 31) * VEC;
+  for (long long q = blockIdx.x; q * A < n_tiles; q += G) {
+    for (int r = 0; r < A; ++r) {
+      const long long t = q * A + r;
+      if (t >= n_tiles) break;
+      const long long base = t * T;
+      const int len = static_cast<int>((n - base) < T ? (n - base) : T);
+      for (int i = threadIdx.x * VEC; i - lane_elems < len; i += FEDAVG_THREADS * VEC) {   // warp-uniform bound
+        const bool valid = i < len;
+        float f[VEC];
+#pragma unroll
+        for (int j = 0; j < VEC; ++j) f[j] = 0.f;
+        if (valid) {
+#pragma unroll
+          for (int j = 0; j < VEC; j += 4) {
+            const float4 v = __ldcs(reinterpret_cast<const float4*>(src + base + i + j));
+            f[j] = v.x; f[j + 1] = v.y; f[j + 2] = v.z; f[j + 3] = v.w;
+          }
+        }
+        float inv = 1.f;
+        if constexpr (W::SCALED) {
+          const int e = quad_block_exponent<VEC>(f);
+          inv = exp2_int(-e);
+          if (valid && (threadIdx.x & 3) == 0) wire[n + ((base + i) >> 5)] = static_cast<uint8_t>(e + 127);
+        }
+        if (valid) W::st(wire + (base + i) * esz, W::pack(f, inv));
+      }
+    }
+  }
+}
+
+// phase 1: the owner of a tile sums weight * wire_k over the participants (part[k] != 0, fixed rank order) and stores
+// the cast result into that tile of every live rank's segment
+template <int WIRE>
+__device__ __forceinline__ void seg_reduce(uint8_t* const* s_wire, const float* part, size_t off, float weight,
+                                           long long n, int T, int A, int G, int my_pos) {
+  using W = Wire<WIRE>;
+  constexpr int VEC = W::VEC;
+  constexpr int KG = 4;                          // peers whose loads are issued together
+  constexpr size_t esz = W::VBYTES / VEC;
+  const long long n_tiles = (n + T - 1) / T;
+  const int lane_elems = static_cast<int>(threadIdx.x & 31) * VEC;
+  for (long long t = my_pos + static_cast<long long>(blockIdx.x) * A; t < n_tiles; t += static_cast<long long>(G) * A) {
+    const long long base = t * T;
+    const int len = static_cast<int>((n - base) < T ? (n - base) : T);
+    for (int i = threadIdx.x * VEC; i - lane_elems < len; i += FEDAVG_THREADS * VEC) {
+      const bool valid = i < len;
+      const size_t eo = off + (base + i) * esz, so = off + n + ((base + i) >> 5);
+      float acc[VEC];
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) acc[j] = 0.f;
+#pragma unroll 1
+      for (int k0 = 0; k0 < A; k0 += KG) {
+        uint4 v[KG];
+        uint32_t sc[KG];
+        if (valid) {
+#pragma unroll
+          for (int k = 0; k < KG; ++k)
+            if (k0 + k < A && part[k0 + k] != 0.f) {
+              v[k] = W::ld(s_wire[k0 + k] + eo);
+              if constexpr (W::SCALED) sc[k] = ld_volatile_u8(s_wire[k0 + k] + so);
+            }
+#pragma unroll
+          for (int k = 0; k < KG; ++k)
+            if (k0 + k < A && part[k0 + k] != 0.f) {
+              float f[VEC];
+              float scale = 1.f;
+              if constexpr (W::SCALED) scale = exp2_int(static_cast<int>(sc[k]) - 127);
+              W::unpack(v[k], f, scale);
+#pragma unroll
+              for (int j = 0; j < VEC; ++j) acc[j] = fmaf(weight, f[j], acc[j]);
+            }
+        }
+      }
+      float inv = 1.f;
+      int e = 0;
+      if constexpr (W::SCALED) {
+        e = quad_block_exponent<VEC>(acc);
+        inv = exp2_int(-e);
+      }
+      if (valid) {
+        const uint4 out = W::pack(acc, inv);
+        for (int k = 0; k < A; ++k) {
+          W::st_na(s_wire[k] + eo, out);
+          if constexpr (W::SCALED)
+            if ((threadIdx.x & 3) == 0) st_volatile_u8(s_wire[k] + so, static_cast<uint32_t>(e + 127));
+        }
+      }
+    }
+  }
+}
+
+// phase 2: dst += the reduced segment, over the tiles this CTA applies (the ones it packed)
+template <int WIRE>
+__device__ __forceinline__ void seg_apply_add(const uint8_t* wire, float* __restrict__ dst, long long n, int T, int A,
+                                              int G) {
+  using W = Wire<WIRE>;
+  constexpr int VEC = W::VEC;
+  constexpr size_t esz = W::VBYTES / VEC;
+  const long long n_tiles = (n + T - 1) / T;
+  for (long long q = blockIdx.x; q * A < n_tiles; q += G) {
+    for (int r = 0; r < A; ++r) {
+      const long long t = q * A + r;
+      if (t >= n_tiles) break;
+      const long long base = t * T;
+      const int len = static_cast<int>((n - base) < T ? (n - base) : T);
+      for (int i = threadIdx.x * VEC; i < len; i += FEDAVG_THREADS * VEC) {
+        const uint4 wv = W::ld(wire + (base + i) * esz);
+        float scale = 1.f;
+        if constexpr (W::SCALED) scale = exp2_int(static_cast<int>(ld_volatile_u8(wire + n + ((base + i) >> 5))) - 127);
+        float f[VEC];
+        W::unpack(wv, f, scale);
+#pragma unroll
+        for (int j = 0; j < VEC; j += 4) {
+          float4 c = *reinterpret_cast<const float4*>(dst + base + i + j);
+          c.x += f[j]; c.y += f[j + 1]; c.z += f[j + 2]; c.w += f[j + 3];
+          *reinterpret_cast<float4*>(dst + base + i + j) = c;
+        }
+      }
+    }
+  }
+}
+
 // DP: DP-FedAvg (see launch.h / DESIGN.md): w_k = n_k s_k / N with s_k from rank k's clip page, and the owner of a tile
 // adds sigma C / N * z[i] to its fp32 sum before the cast.  The loss and the integer side arena keep the weights n_k / N.
-// The whole round; Args is FedAvgDPArgs when DP.
-template <int WIRE, bool DP, typename Args>
+// SCAF: a SCAFFOLD round -- segment 1 (the control variates, see seg_pack) rides between the same barriers; every
+// participant weighs 1 / N there.
+// The whole round; Args is FedAvgDPArgs when DP, FedAvgScaffoldArgs when SCAF.
+template <int WIRE, bool DP, bool SCAF = false, typename Args>
 __device__ __forceinline__ void fedavg_round(const Args& a) {
+  static_assert(!(DP && SCAF), "DP-FedAvg and SCAFFOLD are exclusive");
   using W = Wire<WIRE>;
   constexpr int VEC = W::VEC;
   constexpr bool SCALED = W::SCALED;
@@ -293,6 +432,9 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
         }
       }
     }
+  }
+  if constexpr (SCAF) {
+    if (my_n != 0.f) seg_pack<WIRE>(my_wire + a.seg1_off, a.dc, a.n_c, T, A, G);
   }
   if (blockIdx.x == 0) {
     // integer side arena (num_batches_tracked ...) and the local per-epoch losses
@@ -436,9 +578,15 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
       }
     }
   };
-  if (A <= 2) reduce_tiles(std::integral_constant<int, 4>{});
-  else if (A <= 4) reduce_tiles(std::integral_constant<int, 2>{});
-  else reduce_tiles(std::integral_constant<int, 1>{});
+  if constexpr (SCAF) {
+    // one wire vector per trip: the same sums in the same rank order as the wider trips, in fewer registers
+    reduce_tiles(std::integral_constant<int, 1>{});
+  } else {
+    if (A <= 2) reduce_tiles(std::integral_constant<int, 4>{});
+    else if (A <= 4) reduce_tiles(std::integral_constant<int, 2>{});
+    else reduce_tiles(std::integral_constant<int, 1>{});
+  }
+  if constexpr (SCAF) seg_reduce<WIRE>(s_wire, s_w, static_cast<size_t>(a.seg1_off), a.inv_clients, a.n_c, T, A, G, my_pos);
   // weighted per-epoch loss (manager.py:127-130); every rank computes the same tiny vector
   if (blockIdx.x == 0 && a.loss_out != nullptr) {
     for (int e = threadIdx.x; e < a.n_loss; e += FEDAVG_THREADS) {
@@ -523,6 +671,7 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
       }
     }
   }
+  if constexpr (SCAF) seg_apply_add<WIRE>(my_wire + a.seg1_off, a.c, a.n_c, T, A, G);
   // integer side arena: max over participants (BatchNorm step counters only ever grow)
   if (a.n_int > 0 && blockIdx.x == 0) {
     for (int i = threadIdx.x; i < a.n_int; i += FEDAVG_THREADS) {
@@ -555,6 +704,10 @@ __global__ void __maxnreg__(96) fedavg_allreduce_kernel(const __grid_constant__ 
 template <int WIRE>
 __global__ void __maxnreg__(96) fedavg_allreduce_dp_kernel(const __grid_constant__ FedAvgDPArgs a) {
   fedavg_round<WIRE, true>(a);
+}
+template <int WIRE>
+__global__ void __maxnreg__(96) fedavg_allreduce_scaffold_kernel(const __grid_constant__ FedAvgScaffoldArgs a) {
+  fedavg_round<WIRE, false, true>(a);
 }
 
 // stand-alone cross-GPU barrier on the pads (one CTA): fences host-side phases
@@ -655,12 +808,13 @@ fold_client_scaled_kernel(float* __restrict__ acc, float* __restrict__ theta, co
 // (cudaErrorCooperativeLaunchTooLarge) and schedules all CTAs together, also next to work on other streams -- instead
 // of the plain <<<>>> of round 1, which was only safe on an otherwise idle GPU.  The grid is clamped to what
 // cudaOccupancyMaxActiveBlocksPerMultiprocessor allows on this device.
-template <int WIRE, bool DP, typename Args>
+template <int WIRE, bool DP, bool SCAF, typename Args>
 static int launch_fedavg(const Args* args, int n_ctas, cudaStream_t stream) {
   using namespace b200;
   static int max_ctas = -1;
-  const void* kernel = DP ? reinterpret_cast<const void*>(fedavg_allreduce_dp_kernel<WIRE>)
-                          : reinterpret_cast<const void*>(fedavg_allreduce_kernel<WIRE>);
+  const void* kernel = SCAF ? reinterpret_cast<const void*>(fedavg_allreduce_scaffold_kernel<WIRE>)
+                       : DP ? reinterpret_cast<const void*>(fedavg_allreduce_dp_kernel<WIRE>)
+                            : reinterpret_cast<const void*>(fedavg_allreduce_kernel<WIRE>);
   if (max_ctas < 0) {
     int dev = 0, sms = 0, per_sm = 0;
     cudaGetDevice(&dev);
@@ -676,7 +830,7 @@ static int launch_fedavg(const Args* args, int n_ctas, cudaStream_t stream) {
   return static_cast<int>(cudaGetLastError());
 }
 
-template <bool DP, typename Args>
+template <bool DP, bool SCAF, typename Args>
 static int fedavg_dispatch(const Args* args, int n_ctas, cudaStream_t stream) {
   using namespace b200;
   if (args->world > B200_MAX_RANKS || args->n % 8 != 0 || args->tile_elems % 8 != 0) return -2;
@@ -685,14 +839,14 @@ static int fedavg_dispatch(const Args* args, int n_ctas, cudaStream_t stream) {
   if (args->wire_kind == 2) {
     // block-scaled fp8 wire: 32-element blocks must not straddle tiles, and the switch cannot rescale
     if (args->tile_elems % 32 != 0 || args->use_nvls) return -2;
-    return launch_fedavg<2, DP>(args, n_ctas, stream);
+    return launch_fedavg<2, DP, SCAF>(args, n_ctas, stream);
   }
-  if (args->wire_kind == 1) return launch_fedavg<1, DP>(args, n_ctas, stream);
-  return launch_fedavg<0, DP>(args, n_ctas, stream);
+  if (args->wire_kind == 1) return launch_fedavg<1, DP, SCAF>(args, n_ctas, stream);
+  return launch_fedavg<0, DP, SCAF>(args, n_ctas, stream);
 }
 
 extern "C" int b200_fedavg_allreduce(const FedAvgArgs* args, int n_ctas, cudaStream_t stream) {
-  return fedavg_dispatch<false>(args, n_ctas, stream);
+  return fedavg_dispatch<false, false>(args, n_ctas, stream);
 }
 
 extern "C" int b200_fedavg_allreduce_dp(const FedAvgDPArgs* args, int n_ctas, cudaStream_t stream) {
@@ -700,7 +854,15 @@ extern "C" int b200_fedavg_allreduce_dp(const FedAvgDPArgs* args, int n_ctas, cu
   if (args->use_nvls || !args->delta || args->world > B200_MAX_RANKS) return -2;
   for (int k = 0; k < args->world; ++k)
     if (((args->alive_mask >> k) & 1u) && args->clip_page[k] == nullptr) return -2;
-  return fedavg_dispatch<true>(args, n_ctas, stream);
+  return fedavg_dispatch<true, false>(args, n_ctas, stream);
+}
+
+extern "C" int b200_fedavg_allreduce_scaffold(const FedAvgScaffoldArgs* args, int n_ctas, cudaStream_t stream) {
+  // 1 / N weighs every participant's raw wire value on the reader side: SCAFFOLD runs on peer loads
+  if (args->use_nvls || !args->delta || args->dc == nullptr || args->c == nullptr || args->n_c <= 0 ||
+      args->n_c % 8 != 0 || args->seg1_off % 16 != 0)
+    return -2;
+  return fedavg_dispatch<false, true>(args, n_ctas, stream);
 }
 
 extern "C" int b200_flag_barrier(unsigned long long* const* pads, int rank, int world, uint32_t alive_mask,

@@ -96,6 +96,8 @@ struct GemmParams {
   long long ldr = 0;
   // FedProx anchor of the optimizer epilogue, indexed like sgd_theta; nullptr: no proximal term (sgd_hyper has 4 floats)
   const float* sgd_anchor = nullptr;
+  // SCAFFOLD correction c - c_i of the optimizer epilogue, indexed like sgd_theta; nullptr: no correction term
+  const float* sgd_corr = nullptr;
 };
 
 // Wait until every arrival flag covering arena elements [e0, e1] has reached `need` (published by the FedAvg kernel with
@@ -288,11 +290,12 @@ __device__ __forceinline__ void store_row_chunk(const GemmParams& p, int row, in
 // The tile holds the complete gradient of these weights (single K pass), so the SGD step runs here and the gradient
 // buffer is never touched.  0 + v is the value a red.add into the zeroed gradient would have left (-0 becomes +0), and
 // sgd_update is the arena optimizer's arithmetic: the result matches accumulate-then-fused_sgd bit for bit.
-// PROX: FedProx step, the anchor (sgd_anchor) is read beside theta.
-template <bool PROX>
+// PROX: FedProx step, the anchor (sgd_anchor) is read beside theta.  SCAF: SCAFFOLD step, the correction (sgd_corr)
+// is read beside theta instead.
+template <bool PROX, bool SCAF = false>
 __device__ __forceinline__ void sgd_epilogue_chunk(const GemmParams& p, size_t e, int col0, const float (&v)[32],
                                                    bool vec) {
-  const float* a = PROX ? p.sgd_anchor + e : nullptr;
+  const float* a = PROX ? p.sgd_anchor + e : SCAF ? p.sgd_corr + e : nullptr;
   const SgdHyper h = PROX ? load_sgd_hyper_prox(p.sgd_hyper) : load_sgd_hyper(p.sgd_hyper);
   float* w = p.sgd_theta + e;
   float* m = p.sgd_mom != nullptr ? p.sgd_mom + e : nullptr;
@@ -307,7 +310,9 @@ __device__ __forceinline__ void sgd_epilogue_chunk(const GemmParams& p, size_t e
       const float4 w0 = *reinterpret_cast<const float4*>(w + j);
       const float4 wv = PROX ? sgd_update4_prox(h, w0, gv, *reinterpret_cast<const float4*>(a + j), mv, m != nullptr,
                                                 nest)
-                             : sgd_update4(h, w0, gv, mv, m != nullptr, nest);
+                        : SCAF ? sgd_update4_scaf(h, w0, gv, *reinterpret_cast<const float4*>(a + j), mv, m != nullptr,
+                                                  nest)
+                               : sgd_update4(h, w0, gv, mv, m != nullptr, nest);
       *reinterpret_cast<float4*>(w + j) = wv;
       if (m != nullptr) *reinterpret_cast<float4*>(m + j) = mv;
       if (wb != nullptr) *reinterpret_cast<uint2*>(wb + j) = make_uint2(pack_bf16x2(wv.x, wv.y), pack_bf16x2(wv.z, wv.w));
@@ -319,7 +324,8 @@ __device__ __forceinline__ void sgd_epilogue_chunk(const GemmParams& p, size_t e
         float mv = m != nullptr ? m[j] : 0.f;
         const float gj = __fadd_rn(0.f, v[j]);
         const float wv = PROX ? sgd_update_prox(h, w[j], gj, a[j], mv, m != nullptr, nest)
-                              : sgd_update(h, w[j], gj, mv, m != nullptr, nest);
+                         : SCAF ? sgd_update_scaf(h, w[j], gj, a[j], mv, m != nullptr, nest)
+                                : sgd_update(h, w[j], gj, mv, m != nullptr, nest);
         w[j] = wv;
         if (m != nullptr) m[j] = mv;
         if (wb != nullptr) wb[j] = __float2bfloat16_rn(wv);
@@ -423,9 +429,9 @@ __device__ __forceinline__ void s2_load_ktile(const CUtensorMap* tmA, const CUte
 // no col2im); 4 = implicit dgrad of a stride-2 convolution, one parity class of dx pixels per group of M tiles (see
 // s2_class).  See csrc/im2col_tma.cu for the tensor maps.
 // SGD: optimizer epilogue instantiation (weight gradients only) -- every other GEMM keeps the plain epilogue.
-// PROX (with SGD): the FedProx form of that epilogue.
+// PROX (with SGD): the FedProx form of that epilogue.  SCAF (with SGD): its SCAFFOLD form.
 // AFFINE: eval-mode BatchNorm epilogue instantiation (affine_chunk, forward convolutions in evaluation).
-template <int BN, int STAGES, int CONV = 0, bool SGD = false, bool AFFINE = false, bool PROX = false>
+template <int BN, int STAGES, int CONV = 0, bool SGD = false, bool AFFINE = false, bool PROX = false, bool SCAF = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                          const GemmParams p) {
@@ -586,7 +592,8 @@ gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     const bool vec_ok = ((reinterpret_cast<uintptr_t>(p.D) & 15) == 0) && ((p.ldd * elt) % 16 == 0);
     const bool sgd_vec = SGD && (p.ldd % 4 == 0) &&
                          ((reinterpret_cast<uintptr_t>(p.sgd_theta) | reinterpret_cast<uintptr_t>(p.sgd_mom) |
-                           (PROX ? reinterpret_cast<uintptr_t>(p.sgd_anchor) : 0)) & 15) == 0 &&
+                           (PROX ? reinterpret_cast<uintptr_t>(p.sgd_anchor) : 0) |
+                           (SCAF ? reinterpret_cast<uintptr_t>(p.sgd_corr) : 0)) & 15) == 0 &&
                          (reinterpret_cast<uintptr_t>(p.sgd_wb) & 7) == 0;
     // fused BatchNorm statistics: per row quarter column sums, [4 quarters][2 * BN] floats
     float* sstat = cstat + q * 2 * BN;
@@ -613,7 +620,7 @@ gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       }
       const bool full = (col0 + 32 <= p.N);
       if constexpr (SGD) {
-        sgd_epilogue_chunk<PROX>(p, static_cast<size_t>(row) * p.ldd + col0, col0, v, sgd_vec);
+        sgd_epilogue_chunk<PROX, SCAF>(p, static_cast<size_t>(row) * p.ldd + col0, col0, v, sgd_vec);
         continue;
       }
       if (p.atomic_out) {
@@ -1112,7 +1119,7 @@ static int clamp_bn(int bn) { return bn > 128 ? 128 : bn; }
 
 static void set_sgd_epilogue(GemmParams& p, const B200SgdEpilogue& s) {
   p.sgd_hyper = s.hyper; p.sgd_theta = s.theta; p.sgd_wb = reinterpret_cast<__nv_bfloat16*>(s.theta_bf16);
-  p.sgd_mom = s.mom; p.sgd_nesterov = s.nesterov; p.sgd_anchor = s.anchor;
+  p.sgd_mom = s.mom; p.sgd_nesterov = s.nesterov; p.sgd_anchor = s.anchor; p.sgd_corr = s.corr;
 }
 
 static void set_affine_epilogue(GemmParams& p, const B200AffineEpilogue& a) {
@@ -1128,27 +1135,30 @@ static bool affine_ok(const B200AffineEpilogue& a, int N) {
          (a.residual == nullptr || (a.ldr % 8 == 0 && a.ldr >= N));
 }
 
-template <int BN, int STAGES, int CONV = 0, bool SGD = false, bool AFFINE = false, bool PROX = false>
+template <int BN, int STAGES, int CONV = 0, bool SGD = false, bool AFFINE = false, bool PROX = false, bool SCAF = false>
 static int launch_fixed(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, dim3 grid,
                       cudaStream_t stream) {
   constexpr int smem = STAGES * SmemLayout<BN>::STAGE_BYTES + 2 * STAGES * 8 + 8 * BN * 4 + 1024;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD, AFFINE, PROX>,
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD, AFFINE, PROX, SCAF>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return static_cast<int>(e);
     configured = true;
   }
-  cudaError_t le = launch_pdl(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD, AFFINE, PROX>, grid, GEMM_THREADS, smem, stream,
+  cudaError_t le = launch_pdl(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD, AFFINE, PROX, SCAF>, grid, GEMM_THREADS, smem, stream,
                               ta, tb, p);
   if (le != cudaSuccess) return static_cast<int>(le);
   return static_cast<int>(cudaGetLastError());
 }
 
-// the optimizer-epilogue instantiation, in its FedProx form when the step has an anchor
+// the optimizer-epilogue instantiation, in its FedProx form when the step has an anchor, in its SCAFFOLD form when it
+// has a correction
 template <int BN, int STAGES, int CONV>
 static int launch_fixed_sgd(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, dim3 grid,
                             cudaStream_t stream) {
+  if (p.sgd_anchor != nullptr && p.sgd_corr != nullptr) return -2;
+  if (p.sgd_corr != nullptr) return launch_fixed<BN, STAGES, CONV, true, false, false, true>(ta, tb, p, grid, stream);
   return p.sgd_anchor != nullptr ? launch_fixed<BN, STAGES, CONV, true, false, true>(ta, tb, p, grid, stream)
                                  : launch_fixed<BN, STAGES, CONV, true>(ta, tb, p, grid, stream);
 }

@@ -20,6 +20,7 @@ struct B200SgdEpilogue {
   const float* hyper;
   int nesterov;
   const float* anchor;              // FedProx anchor (global model), indexed like theta, or nullptr (no proximal term)
+  const float* corr;                // SCAFFOLD correction c - c_i, indexed like theta, or nullptr (exclusive with anchor)
 };
 #define B200_SGD_EPILOGUE_DECLINED (-6)
 
@@ -85,15 +86,22 @@ int b200_gemm_simt(const void* a, const void* b, void* d, const float* bias, int
 // ---- elementwise.cu
 // hyper = device float[4] {lr, momentum, weight_decay, dampening}; with prox_anchor != nullptr float[5], the fifth being
 // the FedProx coefficient mu of the term mu * (w - prox_anchor) added to the gradient (prox_anchor indexed like w)
+// corr != nullptr (SCAFFOLD, exclusive with prox_anchor): the correction c - c_i, indexed like w, added to the gradient
 // wire_slot != nullptr: also emit the client's wire copy for the round-end collective (see SgdPack in elementwise.cu)
 int b200_fused_sgd(float* w, float* g, float* mom, void* w_bf16, long long n, const float* hyper, int zero_grad,
                    int nesterov, const unsigned long long* wire_slot, const float* pack_global,
                    const float* pack_scale, long long n_pack, int wire_fp32, const float* prox_anchor,
-                   cudaStream_t stream);
+                   const float* corr, cudaStream_t stream);
 // the same step over a device table of n_seg arena chunks {offset, length, kind} (int64 [n_seg][3]); kind 0: with a
 // gradient (zeroed afterwards), kind 1: gradient identically zero (never read)
 int b200_fused_sgd_segments(float* w, float* g, float* mom, void* w_bf16, const long long* segments, int n_seg,
-                            const float* hyper, int nesterov, const float* prox_anchor, cudaStream_t stream);
+                            const float* hyper, int nesterov, const float* prox_anchor, const float* corr,
+                            cudaStream_t stream);
+// SCAFFOLD control variates over n parameters (n % 4 == 0, 16-byte aligned): corr = c - c_i before a client trains;
+// after it trained, dc = (global_w - theta) * inv_k_eta - c, c_i += dc, up = dc (first != 0) or up += dc
+int b200_scaffold_corr(float* corr, const float* c, const float* ci, long long n, cudaStream_t stream);
+int b200_scaffold_dc(float* up, float* ci, const float* c, const float* global_w, const float* theta, long long n,
+                     float inv_k_eta, int first, cudaStream_t stream);
 // logical-client fold: acc (+)= nk * (theta - global) [+ reset of the replica]; mode 2: theta = global + acc * nk
 int b200_fold_client(float* acc, float* theta, const float* global_w, void* w_bf16, float* mom, long long n_mom, long long n,
                      float nk, int mode, int reset, cudaStream_t stream);
@@ -161,8 +169,19 @@ struct FedAvgDPArgs : FedAvgArgs {
   unsigned long long seed;          // Philox key
   uint32_t round;                   // Philox counter word 2: the collective's round index
 };
+// SCAFFOLD round (fedavg_allreduce_scaffold_kernel<WIRE>): the plain round over segment 0 plus, between the same two
+// barriers, a second segment of n_c elements at byte offset seg1_off of every wire half: each participant (n_k != 0)
+// packs cast(dc), the tile owner reduces with weight inv_clients = 1 / N, and every live rank applies c += result.
+struct FedAvgScaffoldArgs : FedAvgArgs {
+  const float* dc;                  // local: this rank's summed control-variate updates [n_c]
+  float* c;                         // local: the server control variate [n_c]
+  long long n_c;                    // elements of segment 1 (the parameters; multiple of 8)
+  long long seg1_off;               // byte offset of segment 1 inside each wire half (multiple of 16)
+  float inv_clients;                // 1 / N, N = the client population
+};
 int b200_fedavg_allreduce(const FedAvgArgs* args, int n_ctas, cudaStream_t stream);
 int b200_fedavg_allreduce_dp(const FedAvgDPArgs* args, int n_ctas, cudaStream_t stream);   // delta mode, peer loads only
+int b200_fedavg_allreduce_scaffold(const FedAvgScaffoldArgs* args, int n_ctas, cudaStream_t stream);   // delta, peer loads
 // DP clip factor: s = min(1, clip / ||theta - global_w||_2) over [0, n), norm in fp64 (s = 0 when it is not finite), written to
 // s_out[0] (and s_copy[0] when given), the norm to norm_out[0]; a non-finite norm adds 1 to *nonfinite (optional).
 // Deterministic: fixed grid, per-block partials in work (int64 [B200_DP_WORK_WORDS], zero on first use), last-block finish.

@@ -3,7 +3,8 @@
 // lives here once:
 //     g' = g + wd*w [+ prox*(w - a)] ;  m = mu*m + (1-damp)*g' ;  step = nesterov ? g' + mu*m : m ;  w -= lr*step
 // (without a momentum buffer: step = g').  The bracketed term is FedProx's proximal pull toward the anchor `a`, the
-// global model the round started from; only the *_prox forms add it.  Hyper-parameters come from device memory so a
+// global model the round started from; only the *_prox forms add it.  The *_scaf forms instead add SCAFFOLD's
+// correction c - c_i:  g' = (g + wd*w) + corr.  Hyper-parameters come from device memory so a
 // captured CUDA graph can be replayed with a new lr or prox coefficient.
 #pragma once
 
@@ -42,6 +43,12 @@ __device__ __forceinline__ float sgd_update_prox(const SgdHyper& h, float w, flo
   return sgd_apply(h, w, fmaf(h.prox, w - a, fmaf(h.wd, w, g)), m, has_mom, nesterov);
 }
 
+// the same with SCAFFOLD's control-variate correction `corr` = c - c_i added to the gradient (after weight decay)
+__device__ __forceinline__ float sgd_update_scaf(const SgdHyper& h, float w, float g, float corr, float& m, bool has_mom,
+                                                 bool nesterov) {
+  return sgd_apply(h, w, fmaf(h.wd, w, g) + corr, m, has_mom, nesterov);
+}
+
 __device__ __forceinline__ float4 sgd_update4(const SgdHyper& h, float4 w, float4 g, float4& m, bool has_mom,
                                               bool nesterov) {
   w.x = sgd_update(h, w.x, g.x, m.x, has_mom, nesterov);
@@ -57,6 +64,15 @@ __device__ __forceinline__ float4 sgd_update4_prox(const SgdHyper& h, float4 w, 
   w.y = sgd_update_prox(h, w.y, g.y, a.y, m.y, has_mom, nesterov);
   w.z = sgd_update_prox(h, w.z, g.z, a.z, m.z, has_mom, nesterov);
   w.w = sgd_update_prox(h, w.w, g.w, a.w, m.w, has_mom, nesterov);
+  return w;
+}
+
+__device__ __forceinline__ float4 sgd_update4_scaf(const SgdHyper& h, float4 w, float4 g, float4 c, float4& m,
+                                                   bool has_mom, bool nesterov) {
+  w.x = sgd_update_scaf(h, w.x, g.x, c.x, m.x, has_mom, nesterov);
+  w.y = sgd_update_scaf(h, w.y, g.y, c.y, m.y, has_mom, nesterov);
+  w.z = sgd_update_scaf(h, w.z, g.z, c.z, m.z, has_mom, nesterov);
+  w.w = sgd_update_scaf(h, w.w, g.w, c.w, m.w, has_mom, nesterov);
   return w;
 }
 

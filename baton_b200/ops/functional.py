@@ -113,7 +113,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
     if use_simt:
         assert col_stats is None, "fused column statistics need the tensor-core path"
         C.gemm(a, b, out, bias, M, N, K, lda, ldb, ldd, a_mn, b_mn, act, 1, accumulate, alpha, None, 0, 0, 0, -1, 0,
-               True, None, None, None, None, None, None, False, None, None, None, None, False)
+               True, None, None, None, None, None, None, False, None, None, None, None, None, False)
         return out
     bn = force_bn or pick_bn(M, N)
     if col_stats is not None:
@@ -135,7 +135,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
     if not C.gemm(a, b, out, bias, M, N, K, lda, ldb, ldd, a_mn, b_mn, act, split_k, accumulate, alpha, flags, flag_epoch,
                   flag_elem_off, flag_tile_elems, flag_bias_off, bn, False, col_stats, flag_epoch_word, sg.get("theta"),
                   sg.get("theta_bf16"), sg.get("momentum"), sg.get("hyper"), bool(sg.get("nesterov", False)),
-                  sg.get("anchor"), af.get("scale"), af.get("shift"), af.get("residual"), bool(af.get("relu", False))):
+                  sg.get("anchor"), sg.get("corr"), af.get("scale"), af.get("shift"), af.get("residual"), bool(af.get("relu", False))):
         return None
     return out
 
@@ -168,12 +168,16 @@ def gemm_stats_fusable(M: int, N: int, K: int) -> bool:
 # ---------------------------------------------------------------------------- elementwise / optimizer
 def fused_sgd(w: torch.Tensor, g: torch.Tensor, hyper: torch.Tensor, momentum_buf: Optional[torch.Tensor] = None,
               w_bf16: Optional[torch.Tensor] = None, zero_grad: bool = True, nesterov: bool = False,
-              pack: Optional[dict] = None, prox_anchor: Optional[torch.Tensor] = None) -> None:
+              pack: Optional[dict] = None, prox_anchor: Optional[torch.Tensor] = None,
+              corr: Optional[torch.Tensor] = None) -> None:
     """One kernel over the whole flat arena (reference: ``optimizer.step()``, demo.py:47).
 
     ``prox_anchor`` (FedProx): fp32 buffer indexed like ``w`` (the global model the round started from); the step adds
     ``hyper[4] * (w - prox_anchor)`` to the gradient, so ``hyper`` then holds 5 floats
     ``[lr, momentum, weight_decay, dampening, prox_mu]``.  ``None``: no proximal term, ``hyper[4]`` is never read.
+
+    ``corr`` (SCAFFOLD, exclusive with ``prox_anchor``): fp32 buffer indexed like ``w`` holding ``c - c_i``; the step
+    adds it to the gradient after weight decay.
 
     ``pack`` (SURVEY K4, "emits the upload copy"): ``{"wire_slot": int64[1] device word holding the wire address,
     "global_w": fp32 global copy or None, "scale": fp32[1] device scalar or None, "n_pack": elements to pack
@@ -182,20 +186,22 @@ def fused_sgd(w: torch.Tensor, g: torch.Tensor, hyper: torch.Tensor, momentum_bu
     pk = pack or {}
     load().fused_sgd(w, g, momentum_buf, w_bf16, hyper, zero_grad, nesterov, pk.get("wire_slot"),
                      pk.get("global_w"), pk.get("scale"), int(pk.get("n_pack", 0)), bool(pk.get("wire_fp32", False)),
-                     prox_anchor)
+                     prox_anchor, corr)
 
 
 def sgd_epilogue_args(theta: torch.Tensor, grad: torch.Tensor, grad_view: torch.Tensor, hyper: torch.Tensor,
                       momentum: Optional[torch.Tensor] = None, theta_bf16: Optional[torch.Tensor] = None,
-                      nesterov: bool = False, anchor: Optional[torch.Tensor] = None) -> dict:
+                      nesterov: bool = False, anchor: Optional[torch.Tensor] = None,
+                      corr: Optional[torch.Tensor] = None) -> dict:
     """``sgd=`` argument of a weight-gradient GEMM whose output ``grad_view`` is a view of the flat gradient ``grad``:
-    the parameter, bf16 shadow, momentum and FedProx anchor buffers (same offsets as ``grad``) from the element
-    ``grad_view[0, 0]`` on.  With an ``anchor`` the step is the one of :func:`fused_sgd` with ``prox_anchor``."""
+    the parameter, bf16 shadow, momentum, FedProx anchor and SCAFFOLD correction buffers (same offsets as ``grad``)
+    from the element ``grad_view[0, 0]`` on.  With an ``anchor`` the step is the one of :func:`fused_sgd` with
+    ``prox_anchor``, with a ``corr`` the one with ``corr``."""
     off = (grad_view.data_ptr() - grad.data_ptr()) // grad.element_size()
     assert 0 <= off < grad.numel(), "the GEMM output is not a view of the gradient arena"
     return {"theta": theta[off:], "theta_bf16": theta_bf16[off:] if theta_bf16 is not None else None,
             "momentum": momentum[off:] if momentum is not None else None, "hyper": hyper, "nesterov": nesterov,
-            "anchor": anchor[off:] if anchor is not None else None}
+            "anchor": anchor[off:] if anchor is not None else None, "corr": corr[off:] if corr is not None else None}
 
 
 SGD_CHUNK = 8192       # arena elements per chunk of the leftover optimizer pass (one CTA iteration each)
@@ -232,11 +238,25 @@ def sgd_segments(n: int, fused: Sequence[Tuple[int, int, int, int]], nograd: Seq
 
 def fused_sgd_segments(w: torch.Tensor, g: torch.Tensor, hyper: torch.Tensor, segments: torch.Tensor,
                        momentum_buf: Optional[torch.Tensor] = None, w_bf16: Optional[torch.Tensor] = None,
-                       nesterov: bool = False, prox_anchor: Optional[torch.Tensor] = None) -> None:
+                       nesterov: bool = False, prox_anchor: Optional[torch.Tensor] = None,
+                       corr: Optional[torch.Tensor] = None) -> None:
     """The step of :func:`fused_sgd` over the arena chunks of ``segments`` (device int64 ``[S, 3]`` from
-    :func:`sgd_segments`); chunks of kind 1 never read the gradient.  ``prox_anchor`` as in :func:`fused_sgd`; a
-    kind-1 element without a momentum buffer is then written only where the step changes it."""
-    load().fused_sgd_segments(w, g, momentum_buf, w_bf16, segments, hyper, nesterov, prox_anchor)
+    :func:`sgd_segments`); chunks of kind 1 never read the gradient.  ``prox_anchor`` and ``corr`` as in
+    :func:`fused_sgd`; a kind-1 element without a momentum buffer is then written only where the step changes it."""
+    load().fused_sgd_segments(w, g, momentum_buf, w_bf16, segments, hyper, nesterov, prox_anchor, corr)
+
+
+def scaffold_corr(corr: torch.Tensor, c: torch.Tensor, c_i: torch.Tensor) -> None:
+    """SCAFFOLD: ``corr = c - c_i`` over ``corr.numel()`` parameters, the correction client ``i`` trains with."""
+    load().scaffold_corr(corr, c, c_i)
+
+
+def scaffold_dc(up: torch.Tensor, c_i: torch.Tensor, c: torch.Tensor, global_w: torch.Tensor, theta: torch.Tensor,
+                inv_k_eta: float, *, first: bool) -> None:
+    """SCAFFOLD after client ``i`` trained ``K`` steps at learning rate ``eta`` (option II): ``dc = (global_w - theta)
+    * inv_k_eta - c`` with ``inv_k_eta = 1 / (K eta)``; ``c_i += dc``; ``up = dc`` (``first``) or ``up += dc``.  Over
+    ``up.numel()`` parameters."""
+    load().scaffold_dc(up, c_i, c, global_w, theta, float(inv_k_eta), bool(first))
 
 
 def weighted_sum_(dst: torch.Tensor, srcs: Sequence[torch.Tensor], weights: Sequence[float]) -> torch.Tensor:
@@ -515,7 +535,7 @@ def conv_igemm_wgrad_(dy2d: torch.Tensor, x: torch.Tensor, dw2d: torch.Tensor, k
     sg = sgd or {}
     return bool(load().conv_igemm_wgrad(dy2d, x, dw2d, cout, kh, kw, stride, pad, ho, wo, split_k, bn,
                                         sg.get("theta"), sg.get("theta_bf16"), sg.get("momentum"), sg.get("hyper"),
-                                        bool(sg.get("nesterov", False)), sg.get("anchor")))
+                                        bool(sg.get("nesterov", False)), sg.get("anchor"), sg.get("corr")))
 
 
 def col2im(col: torch.Tensor, shape: Tuple[int, int, int, int], kh: int, kw: int, stride: int, pad: int,

@@ -180,15 +180,17 @@ class _SgdEpilogue:
     ``(offset, rows, cols, ld)`` and, for centre-tap convolutions, the ``nograd`` range ``(offset, length)`` of the whole
     weight (its other taps never receive a gradient).  The trainer's leftover optimizer pass covers the rest of the
     arena (``F.sgd_segments``).  The gradient of a fused block is never written, so it stays zero for unfused steps.
-    ``prox``: FedProx step anchored on ``arena.global_w`` (``hyper`` then holds the coefficient as its fifth float)."""
+    ``prox``: FedProx step anchored on ``arena.global_w`` (``hyper`` then holds the coefficient as its fifth float).
+    ``corr``: SCAFFOLD step with the correction ``c - c_i`` (fp32, indexed like the parameters)."""
 
     def __init__(self):
         self.arena = None
 
     @contextlib.contextmanager
-    def open(self, arena, hyper, nesterov, prox=False):
+    def open(self, arena, hyper, nesterov, prox=False, corr=None):
         self.arena, self.hyper, self.nesterov = arena, hyper, nesterov
         self.anchor = arena.global_w if prox else None
+        self.corr = corr
         self.fused, self.nograd = [], []
         try:
             yield self
@@ -205,7 +207,7 @@ class _SgdEpilogue:
         if a is None:
             return None
         return F.sgd_epilogue_args(a.theta, a.grad, out2d, self.hyper, a.momentum, a.theta_bf16, self.nesterov,
-                                   self.anchor)
+                                   self.anchor, self.corr)
 
     def record(self, out2d, nograd_of=None):
         off = (out2d.data_ptr() - self.arena.grad.data_ptr()) // 4

@@ -30,6 +30,7 @@ from ..train import GraphedLocalSGD, PortableLocalSGD, check_prox_mu
 from .arena import ParamArena
 from .dp import DPConfig, RDPAccountant, check_dp, clip_factor
 from .fedavg import FedAvgSession, NcclSession
+from .scaffold import ScaffoldState
 
 
 @dataclass
@@ -64,16 +65,32 @@ class FederatedEngine:
                  wire_dtype: str = "bf16", mode: str = "delta", n_ctas: Optional[int] = None, use_graph: bool = True,
                  logical_clients: int = 0, sample_k: Optional[int] = None, seed: int = 0, name: str = "exp",
                  nvls: "bool | str" = "auto", tile_flags: bool = False, prox_mu: float = 0.0,
-                 dp_clip: float = 0.0, dp_noise_multiplier: float = 0.0, dp_seed: Optional[int] = None):
+                 dp_clip: float = 0.0, dp_noise_multiplier: float = 0.0, dp_seed: Optional[int] = None,
+                 scaffold: bool = False):
         """``prox_mu > 0``: FedProx local training -- every step adds ``prox_mu * (theta - global_w)`` to the gradient,
         ``global_w`` being the global model the round started from (for logical clients too: each starts from it).
 
         ``dp_clip > 0``: DP-FedAvg (``parallel/dp.py``) -- every participating client's update is clipped to L2 norm
         ``dp_clip``, the participants are averaged uniformly and Gaussian noise of std ``dp_noise_multiplier * dp_clip``
         is added to the sum.  ``dp_seed``: Philox key of the noise (``None``: a secret random key; an explicit seed makes
-        the noise predictable -- tests and reproductions only).  ``dp_clip = 0`` runs exactly the plain engine."""
+        the noise predictable -- tests and reproductions only).  ``dp_clip = 0`` runs exactly the plain engine.
+
+        ``scaffold=True``: SCAFFOLD (``parallel/scaffold.py``) -- every local step adds the correction ``c - c_i`` to
+        the gradient, and each round also updates the control variates (option II), the server's one through the
+        round's collective.  The model update stays the sample-weighted FedAvg mean.  :meth:`control_variates` reads
+        them.  It cannot be combined with DP, FedProx, ``mode='weights'`` or ``tile_flags``."""
         prox_mu = check_prox_mu(prox_mu)
         dp_clip, dp_noise_multiplier = check_dp(dp_clip, dp_noise_multiplier)
+        if scaffold:
+            if dp_clip > 0.0:
+                raise ValueError("SCAFFOLD with DP-FedAvg is not supported: DP would also have to clip and noise dc")
+            if prox_mu > 0.0:
+                raise ValueError("SCAFFOLD and FedProx (prox_mu > 0) are exclusive")
+            if mode != "delta":
+                raise ValueError("SCAFFOLD needs mode='delta'")
+            if tile_flags:
+                raise ValueError("SCAFFOLD with tile_flags is not supported: the correction c - c_i reads c, which "
+                                 "the previous round's collective writes, so it cannot run ahead of the join")
         self.dp = DPConfig(dp_clip, dp_noise_multiplier, dp_seed) if dp_clip > 0.0 else None
         if self.dp is not None and mode != "delta":
             raise ValueError("DP-FedAvg needs mode='delta'")
@@ -95,7 +112,7 @@ class FederatedEngine:
             self.trainer = PortableLocalSGD(model, self.arena, loss=loss)
         Session = {"fused": FedAvgSession, "nccl": NcclSession}[backend]
         self.session = Session(self.arena, group, wire_dtype=wire_dtype, mode=mode, n_ctas=n_ctas, nvls=nvls,
-                               tile_flags=tile_flags, dp=self.dp)
+                               tile_flags=tile_flags, dp=self.dp, scaffold=scaffold)
         self.dp = self.session.dp                  # rank 0's noise key
         self.accountant = RDPAccountant(self.dp.noise_multiplier) if self.dp is not None else None
         self.backend = backend
@@ -121,6 +138,7 @@ class FederatedEngine:
         self.n_rounds = 0
         self.logical_clients = logical_clients if logical_clients and logical_clients > self.world else 0
         self.sample_k = sample_k
+        self.scaf = ScaffoldState(self.arena.n_param, self.device) if scaffold else None
         self._rng = random.Random(seed)            # identical stream on every rank
         self._stage: Dict[Tuple, Tuple[torch.Tensor, torch.Tensor]] = {}
         self._eval_stage: Dict[Tuple, Tuple[torch.Tensor, torch.Tensor]] = {}
@@ -188,7 +206,7 @@ class FederatedEngine:
                 if self.prepack and self.trainer.pack is not None:
                     self.session.arm_prepack(float(X.shape[0]))
                 with phase("baton.local_train", self.phase_s):
-                    losses_dev = self.trainer.run(X, y, n_epoch=n_epoch, return_device=True, **self.hp)
+                    losses_dev = self._train_client(self.rank, X, y, n_epoch, first=True)
                 total_n = X.shape[0]
         else:
             # time-sliced logical clients: fold n_k * (theta_k - global) locally, then upload the mean
@@ -205,7 +223,7 @@ class FederatedEngine:
                 X, y = shards(cid)
                 if not X.is_cuda:
                     X, y = self.stage(X, y, slot=j)
-                ld = self.trainer.run(X, y, n_epoch=n_epoch, return_device=True, **self.hp)
+                ld = self._train_client(cid, X, y, n_epoch, first=(j == 0))
                 nk = X.shape[0]
                 losses_dev = ld * nk if losses_dev is None else losses_dev + ld * nk
                 total_n += nk
@@ -250,6 +268,24 @@ class FederatedEngine:
         if read_loss and losses_dev is not None:
             hist = loss_for_wire.tolist()       # device -> host read of the round's result
         return RoundResult(update_name, int(total_n), hist, participants)
+
+    def _train_client(self, cid: int, X, y, n_epoch: int, first: bool):
+        """Local training of client ``cid`` on the replica; with SCAFFOLD, its correction before and its control-variate
+        update after (before any fold resets the replica)."""
+        if self.scaf is None:
+            return self.trainer.run(X, y, n_epoch=n_epoch, return_device=True, **self.hp)
+        self.scaf.begin_client(cid)
+        ld = self.trainer.run(X, y, n_epoch=n_epoch, return_device=True, corr=self.scaf.corr, **self.hp)
+        self.scaf.end_client(cid, self.arena, n_epoch * self.trainer.last_steps, self.hp["lr"], first=first)
+        return ld
+
+    def control_variates(self):
+        """SCAFFOLD's ``(c, {client_id: c_i})``: the server control variate and those of the clients this rank hosts
+        that have taken part so far (fp32 tensors over the parameters, on the engine's device; live, not copies)."""
+        if self.scaf is None:
+            raise RuntimeError("SCAFFOLD is off (scaffold=False)")
+        self.sync()
+        return self.scaf.c, dict(self.scaf.c_i)
 
     def sync(self) -> None:
         """Make the compute stream wait for a collective that is still running on the side stream (call before
@@ -324,6 +360,10 @@ class FederatedEngine:
 
     def _aggregate(self, my_n: float, loss_dev, clipped: bool = False) -> None:
         s = self.session
+        if self.scaf is not None:      # SCAFFOLD: c += (sum of the ranks' dc) / N in the same collective
+            s.aggregate(my_n=my_n, control=(self.scaf.c, self.scaf.up, self.logical_clients or self.world),
+                        **self._aggregate_kwargs(s, my_n, loss_dev))
+            return
         if self.dp is not None:
             kw = {"clipped": clipped}
             if isinstance(s, FedAvgSession):
@@ -350,6 +390,21 @@ class FederatedEngine:
             s.aggregate(my_n=my_n, loss_history=loss_dev.tolist())
         else:
             s.aggregate(my_n=my_n)
+
+    def _aggregate_kwargs(self, s, my_n: float, loss_dev) -> dict:
+        """Loss, upload and stream arguments of a round's ``aggregate`` (the plain round's choices)."""
+        kw = {}
+        if isinstance(s, FedAvgSession):
+            kw["on_side_stream"] = bool(self.overlap_collective)
+            kw["prepacked"] = bool(self.prepack and getattr(self.trainer, "emitted_wire", False) and my_n > 0
+                                   and not getattr(self.trainer, "last_had_tail_step", False))
+        if loss_dev is not None and hasattr(s, "loss_local"):
+            k = min(loss_dev.numel(), s.loss_local.numel())
+            s.loss_local.zero_()
+            s.loss_local[:k].copy_(loss_dev[:k])
+        elif loss_dev is not None:
+            kw["loss_history"] = loss_dev.tolist()
+        return kw
 
     def global_loss(self, n_epoch: int) -> List[float]:
         return self.session.reduced_loss(n_epoch)

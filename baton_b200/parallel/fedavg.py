@@ -18,6 +18,11 @@ plus Gaussian noise on the sum.  The fused session clips with one deterministic 
 collective's stream, publishes the factor in a small per-rank CLIP PAGE of the symmetric buffer, and the collective
 applies it on the reader side and adds the noise in the tile owner's fp32 accumulator; DP rounds always run on peer
 loads (the switch of NVLS adds raw wire values, before the factors are known).
+
+Both take ``scaffold=True`` (SCAFFOLD, ``parallel/scaffold.py``): every round then also carries the control-variate
+update, ``aggregate(control=(c, dc, N))`` -- ``c += (sum over ranks of dc) / N``.  The fused session lays out each
+parity half of its wire as ``[segment 0 | pad | segment 1]`` (segment 1: ``dc`` over the parameters, in the session's
+wire format) and the collective reduces both segments in one launch, on peer loads.
 """
 from __future__ import annotations
 
@@ -42,6 +47,20 @@ def _check_dp_mode(dp: Optional[DPConfig], delta: bool) -> None:
         raise ValueError("DP-FedAvg clips and noises the update theta - global: it needs mode='delta'")
 
 
+def _check_scaffold(scaffold: bool, dp: Optional[DPConfig], delta: bool) -> None:
+    if scaffold and not delta:
+        raise ValueError("SCAFFOLD needs mode='delta'")
+    if scaffold and dp is not None:
+        raise ValueError("SCAFFOLD and DP-FedAvg are exclusive: DP would have to clip and noise dc too")
+
+
+def _check_control(scaffold: bool, control) -> None:
+    if scaffold and control is None:
+        raise ValueError("a SCAFFOLD session needs control=(c, dc, n_clients) every round")
+    if not scaffold and control is not None:
+        raise ValueError("control= needs a session built with scaffold=True")
+
+
 def _agree_seed(dp: Optional[DPConfig], group) -> Optional[DPConfig]:
     """Every rank must draw the same noise: take rank 0's Philox key (a DPConfig built with seed=None differs per
     process)."""
@@ -57,11 +76,14 @@ def _agree_seed(dp: Optional[DPConfig], group) -> Optional[DPConfig]:
 class FedAvgSession:
     def __init__(self, arena: ParamArena, group=None, *, wire_dtype: str = "bf16", mode: str = "delta",
                  nvls: "bool | str" = "auto", n_ctas: Optional[int] = None, tile_elems: int = 0, timeout_log2: int = 24,
-                 reset_momentum: bool = True, tile_flags: bool = False, dp: Optional[DPConfig] = None):
+                 reset_momentum: bool = True, tile_flags: bool = False, dp: Optional[DPConfig] = None,
+                 scaffold: bool = False):
         from ..ops._ext import load
         self._C = load()
         assert wire_dtype in ("bf16", "fp32", "fp8") and mode in ("delta", "weights")
         _check_dp_mode(dp, mode == "delta")
+        _check_scaffold(scaffold, dp, mode == "delta")
+        self.scaffold = bool(scaffold)
         self.arena = arena
         self.device = arena.device
         self.group = group
@@ -81,6 +103,8 @@ class FedAvgSession:
         self.reset_momentum = reset_momentum
         # wire / int / loss pages exist TWICE (round parity): the kernel has no closing barrier, a rank that races ahead
         # packs the next round into the other half while a slow peer still applies this one (csrc/fedavg.cu)
+        # SCAFFOLD: segment 1 (dc over the parameters) starts at seg1_off of each half
+        self.seg1_off = _align(self._seg_bytes(arena.n), 256) if self.scaffold else 0
         self.half_wire = _align(self.wire_bytes(), 2 << 20)          # multicast-friendly granularity
         self.half_int = _align(max(arena.n_int, 1) * 8, 256)
         self.half_loss = _align(MAX_LOSS * 4, 256)
@@ -98,8 +122,9 @@ class FedAvgSession:
         if self.wire_kind == 2:
             self.use_nvls = False      # the switch adds raw elements; block scales need the P2P path
         self.dp = _agree_seed(dp, group)
-        if self.dp is not None:
-            self.use_nvls = False      # the clip factors are applied by the readers: DP rounds run on peer loads
+        if self.dp is not None or self.scaffold:
+            # the clip factors / the 1 / N of the control variates are applied by the readers: peer loads only
+            self.use_nvls = False
         # DP bookkeeping: norm-kernel partials, the last clip factor / norm of this rank, non-finite updates so far
         self.dp_work = torch.zeros(self._C.DP_WORK_WORDS, dtype=torch.int64, device=self.device)
         self.dp_s = torch.ones(1, dtype=torch.float32, device=self.device)
@@ -211,7 +236,7 @@ class FedAvgSession:
                   alive_ranks: Optional[Sequence[int]] = None, my_n: Optional[float] = None,
                   loss_history: Optional[Sequence[float]] = None, on_side_stream: bool = False,
                   round_index: Optional[int] = None, prepacked: bool = False, dp: Optional[DPConfig] = None,
-                  clipped: bool = False) -> None:
+                  clipped: bool = False, control=None) -> None:
         """Launch the fused reduce+broadcast+apply.  Either the full per-rank sample
         counts are given (manager-driven rounds: the plan comes over HTTP) or only this
         rank's own count ``my_n`` (SPMD engine: peers' counts ride on the barrier flags).
@@ -224,10 +249,19 @@ class FedAvgSession:
         ``dp`` (default: the session's): a DP-FedAvg round.  The counts must then be CLIENTS per rank (1 for a plain
         seat), not samples, and every rank must pass the same ``dp`` (the manager's plan carries it; a session built
         with ``dp=`` agreed on rank 0's key at construction).  ``clipped=True``: this rank's upload is already a sum of clipped updates divided by its
-        count (logical clients folded with :func:`ops.functional.fold_client_scaled`), so its clip factor is 1."""
+        count (logical clients folded with :func:`ops.functional.fold_client_scaled`), so its clip factor is 1.
+
+        ``control = (c, dc, n_clients)`` (every round of a ``scaffold=True`` session, and only there): SCAFFOLD's
+        server control-variate update in the same launch -- ``c += (sum over participating ranks of dc) / n_clients``
+        on every live rank.  ``c`` and ``dc`` are fp32 over the arena's parameters; ``dc`` is this rank's summed client
+        updates (read only when this rank participates).  The optimizer-emitted upload (``prepacked``) covers the
+        model segment only."""
         world = self.world
         dp = dp if dp is not None else self.dp
         _check_dp_mode(dp, self.delta)
+        _check_control(self.scaffold, control)
+        if control is not None and dp is not None:
+            raise ValueError("SCAFFOLD and DP-FedAvg are exclusive")
         if round_index is not None:
             self.epoch = (self.base_epoch + 3 * int(round_index)) & 0xFFFFFFFF
         if n_samples_by_rank is not None:
@@ -294,6 +328,11 @@ class FedAvgSession:
                                      s_copy_ptr=page.data_ptr(), nonfinite=self.dp_nonfinite)
                 seed = dp.seed - (1 << 64) if dp.seed >= (1 << 63) else dp.seed      # int64 bit pattern of the key
                 dp_args = (self.symm.peer_ptrs(o_clip), dp.noise_std, seed, self.dp_round())
+            scaf_args = (None, None, 0, 0.0)
+            if control is not None:
+                c, dc, n_clients = control
+                n_p = self.arena.n_param
+                scaf_args = (dc[:n_p], c[:n_p], self.seg1_off, 1.0 / float(n_clients))
             self._C.fedavg_allreduce(
                 self.symm.peer_ptrs(o_wire), self.symm.peer_ptrs(self.off_pads),
                 self.symm.mc(o_wire) if nvls_now else 0,
@@ -305,7 +344,7 @@ class FedAvgSession:
                 counts, from_flags, mask, self.rank, world, self.wire_kind, self.delta,
                 nvls_now, self.epoch,
                 self.tile_flags, flag_value, tile, self.n_ctas, self.timeout_log2, self.status, self.phase_ns,
-                prepacked, *dp_args)
+                prepacked, *dp_args, *scaf_args)
         self.epoch = (self.epoch + 3) & 0xFFFFFFFF     # uint32 wrap: the kernel compares signed differences
         self.rounds += 1
         self._side_pending = on_side_stream
@@ -382,21 +421,28 @@ class FedAvgSession:
             self.status.zero_()
             raise RuntimeError("FedAvg collective timed out waiting for rank {}".format(code - 1))
 
-    def wire_bytes(self) -> int:
-        """Bytes one client uploads per round (fp8: e4m3 payload + one UE8M0 scale byte per 32 elements)."""
-        n = self.arena.n
+    def _seg_bytes(self, n: int) -> int:
         if self.wire_kind == 2:
             return n + (n + 31) // 32
         return n * (2 if self.wire_kind == 1 else 4)
+
+    def wire_bytes(self) -> int:
+        """Bytes one client uploads per round (fp8: e4m3 payload + one UE8M0 scale byte per 32 elements); with
+        SCAFFOLD, the model segment, its padding and the control-variate segment."""
+        if self.scaffold:
+            return self.seg1_off + self._seg_bytes(self.arena.n_param)
+        return self._seg_bytes(self.arena.n)
 
 
 class NcclSession:
     """Same contract through ``torch.distributed`` collectives (baseline / oracle)."""
 
     def __init__(self, arena: ParamArena, group=None, *, wire_dtype: str = "bf16", mode: str = "delta",
-                 reset_momentum: bool = True, dp: Optional[DPConfig] = None, **_unused):
+                 reset_momentum: bool = True, dp: Optional[DPConfig] = None, scaffold: bool = False, **_unused):
         import torch.distributed as dist
         _check_dp_mode(dp, mode == "delta")
+        _check_scaffold(scaffold, dp, mode == "delta")
+        self.scaffold = bool(scaffold)
         self.dist = dist
         self.arena, self.group, self.device = arena, group, arena.device
         self.dp = _agree_seed(dp, group)
@@ -417,10 +463,13 @@ class NcclSession:
     @torch.no_grad()
     def aggregate(self, n_samples_by_rank=None, alive_ranks=None, my_n=None, loss_history=None,
                   dp: Optional[DPConfig] = None, clipped: bool = False, round_index: Optional[int] = None,
-                  **_unused) -> None:
+                  control=None, **_unused) -> None:
         """DP-FedAvg (``dp``, default the session's): the same estimator as the fused kernel -- clip locally, all-reduce,
         then add the host-generated noise ``sigma C z(seed, round) / m`` after the reduce.  ``round_index`` (the
-        manager's plan) sets the round counter, as it sets the fused session's barrier epoch."""
+        manager's plan) sets the round counter, as it sets the fused session's barrier epoch.  ``control = (c, dc,
+        n_clients)``: SCAFFOLD, as in :meth:`FedAvgSession.aggregate` -- all-reduce ``dc`` as a sum (a rank without
+        participants contributes zeros), then ``c += sum / n_clients``."""
+        _check_control(self.scaffold, control)
         if round_index is not None:
             self.rounds = int(round_index)
         a, dist = self.arena, self.dist
@@ -475,6 +524,13 @@ class NcclSession:
             dist.all_reduce(a.int_arena, op=dist.ReduceOp.MAX, group=self.group)
         if self.reset_momentum and a.momentum is not None:
             a.momentum.zero_()
+        if control is not None:
+            c, dc, n_clients = control
+            n_p = a.n_param
+            tot = dc[:n_p].clone() if float(counts[self.rank]) != 0.0 else torch.zeros_like(c[:n_p])
+            if self.world > 1:
+                dist.all_reduce(tot, group=self.group)
+            c[:n_p].add_(tot / float(n_clients))
         self.rounds += 1
 
     def dp_round(self) -> int:
@@ -496,4 +552,5 @@ class NcclSession:
         pass
 
     def wire_bytes(self) -> int:
-        return self.arena.n * (2 if self.wire_dtype == torch.bfloat16 else 4)
+        n = self.arena.n + (self.arena.n_param if self.scaffold else 0)
+        return n * (2 if self.wire_dtype == torch.bfloat16 else 4)

@@ -19,7 +19,9 @@ Two executions of the same contract:
 
 Every trainer takes ``prox_mu`` (FedProx, Li et al. 2020): the step adds
 ``prox_mu * (w - w_global)`` to the gradient, ``w_global`` being the global model
-the round started from.  ``prox_mu = 0`` is plain SGD.
+the round started from.  ``prox_mu = 0`` is plain SGD.  The arena trainers also
+take ``corr`` (SCAFFOLD, Karimireddy et al. 2020): an fp32 buffer indexed like
+the parameters, holding ``c - c_i``, that every step adds to the gradient.
 """
 from __future__ import annotations
 
@@ -56,6 +58,15 @@ def _add_prox_term(params, anchors, prox_mu: float) -> None:
         for p, a in zip(params, anchors):
             if p.grad is not None:
                 p.grad.add_(p.detach() - a, alpha=prox_mu)
+
+
+def _check_corr(corr, prox_mu: float, arena) -> None:
+    if corr is None:
+        return
+    if prox_mu > 0:
+        raise ValueError("SCAFFOLD's correction and FedProx's proximal term are exclusive")
+    if corr.dtype != torch.float32 or not corr.is_contiguous() or corr.numel() < arena.n_param:
+        raise ValueError("corr must be a contiguous fp32 buffer covering the arena's parameters")
 
 
 def run_local_sgd(model: nn.Module, X: torch.Tensor, y: torch.Tensor, *, n_epoch: int = 32,
@@ -177,6 +188,7 @@ class GraphedLocalSGD:
         self.device = dev
         self.hyper = torch.zeros(5, dtype=torch.float32, device=dev)   # [lr, momentum, wd, dampening, prox_mu]
         self.prox = False             # FedProx: every SGD kernel of the step reads the anchor arena.global_w
+        self.corr = None              # SCAFFOLD: every SGD kernel of the step reads this correction c - c_i
         self.loss_acc = torch.zeros(2, dtype=torch.float32, device=dev)
         self._graphs = {}           # (n, batch, x_shape, y_shape) -> captured epoch
         self._hyper_host = None
@@ -221,10 +233,10 @@ class GraphedLocalSGD:
             # branch; the loss kernel accumulates straight into the epoch's running sums
             if fuse_sgd and not emit_wire:
                 # the split-K = 1 convolution weight gradients apply SGD in their GEMM epilogue; one launch covers the rest
-                with self.bnn.SGD_EPI.open(a, self.hyper, self.nesterov, prox=self.prox) as epi:
+                with self.bnn.SGD_EPI.open(a, self.hyper, self.nesterov, prox=self.prox, corr=self.corr) as epi:
                     explicit(xb, yb, loss_acc=self.loss_acc, after_first_gemm=self._first_gemm_hook)
                 F.fused_sgd_segments(a.theta, a.grad, self.hyper, self._segment_table(epi.fused, epi.nograd),
-                                     a.momentum, bf, nesterov=self.nesterov, prox_anchor=anchor)
+                                     a.momentum, bf, nesterov=self.nesterov, prox_anchor=anchor, corr=self.corr)
                 self.emitted_wire = False
                 return
             explicit(xb, yb, loss_acc=self.loss_acc, after_first_gemm=self._first_gemm_hook)
@@ -238,7 +250,8 @@ class GraphedLocalSGD:
         pack = self.pack if emit_wire else None
         F.fused_sgd(a.theta[: a.n_param], a.grad, self.hyper, a.momentum,
                     bf[: a.n_param] if bf is not None else None, zero_grad=True, nesterov=self.nesterov, pack=pack,
-                    prox_anchor=anchor[: a.n_param] if anchor is not None else None)
+                    prox_anchor=anchor[: a.n_param] if anchor is not None else None,
+                    corr=self.corr[: a.n_param] if self.corr is not None else None)
         self.emitted_wire = pack is not None
         if stats is not None:
             self.loss_acc.add_(stats)
@@ -421,12 +434,15 @@ class GraphedLocalSGD:
 
     def run(self, X, y, n_epoch: int = 1, lr: float = 0.001, batch_size: int = 32, momentum: float = 0.0,
             weight_decay: float = 0.0, reshuffle_each_epoch: bool = False, return_device: bool = False,
-            prox_mu: float = 0.0, **_ignored):
-        """``prox_mu > 0``: FedProx toward ``arena.global_w``, the global model the round started from."""
+            prox_mu: float = 0.0, corr: Optional[torch.Tensor] = None, **_ignored):
+        """``prox_mu > 0``: FedProx toward ``arena.global_w``, the global model the round started from.  ``corr``:
+        SCAFFOLD's correction ``c - c_i`` (fp32 device buffer of ``arena.n_param`` elements), added to every step's
+        gradient; it is read at replay, so the caller may rewrite it between runs."""
         assert X.is_cuda, "GraphedLocalSGD needs a device-resident shard"
         prox_mu = check_prox_mu(prox_mu)
         if prox_mu > 0 and self.arena.global_w is None:
             raise ValueError("prox_mu > 0 needs the arena's global copy (ParamArena(keep_global=True))")
+        _check_corr(corr, prox_mu, self.arena)
         nn.Module.train(self.model, True)
         n = X.shape[0]
         batch_size = min(batch_size, n)
@@ -434,11 +450,13 @@ class GraphedLocalSGD:
         tail = n - n_steps * batch_size
         self._set_hyper(lr, momentum, weight_decay, prox_mu=prox_mu)
         self.prox = prox_mu > 0
+        self.corr = corr
         if momentum and self.arena.momentum is None:
             self.arena.momentum = torch.zeros_like(self.arena.grad)
-        # the anchor pointer is baked into the captured launches; the coefficient is read from `hyper` at replay
+        # the anchor and correction pointers are baked into the captured launches; the coefficient is read from `hyper`
+        # at replay
         key = (n, batch_size, tuple(X.shape[1:]), tuple(y.shape[1:]), X.data_ptr(), y.data_ptr(), bool(momentum),
-               self.prox)
+               self.prox, corr.data_ptr() if corr is not None else None)
         epoch_losses = torch.zeros(n_epoch, 2, dtype=torch.float32, device=self.device)
         if self.use_graph:
             ent = self._graphs.get(key)
@@ -496,20 +514,23 @@ class PortableLocalSGD:
 
     def run(self, X, y, n_epoch: int = 1, lr: float = 0.001, batch_size: int = 32, momentum: float = 0.0,
             weight_decay: float = 0.0, reshuffle_each_epoch: bool = False, return_device: bool = False,
-            prox_mu: float = 0.0, **_ignored):
-        """``prox_mu > 0``: FedProx toward ``arena.global_w``, the global model the round started from."""
+            prox_mu: float = 0.0, corr: Optional[torch.Tensor] = None, **_ignored):
+        """``prox_mu > 0``: FedProx toward ``arena.global_w``, the global model the round started from.  ``corr``:
+        SCAFFOLD's correction ``c - c_i`` (fp32, indexed like the arena's parameters), added to every gradient."""
         criterion = _loss_fn(self.loss_kind)
         prox_mu = check_prox_mu(prox_mu)
+        _check_corr(corr, prox_mu, self.arena)
         n = X.shape[0]
         batch_size = min(batch_size, n)
         nn.Module.train(self.model, True)
         a = self.arena
         if prox_mu > 0 and a.global_w is None:
             raise ValueError("prox_mu > 0 needs the arena's global copy (ParamArena(keep_global=True))")
-        params, anchors = [], []
+        params, anchors, corrs = [], [], []
         for name, p in self.model.named_parameters():
             params.append(p)
             anchors.append(a._view(a.global_w, a.slots[name]) if prox_mu > 0 else None)
+            corrs.append(a._view(corr, a.slots[name]) if corr is not None else None)
         opt = torch.optim.SGD(params, lr=lr, momentum=momentum, weight_decay=weight_decay)
         perm = torch.randperm(n)
         out = torch.zeros(n_epoch, 2, dtype=torch.float32)
@@ -529,6 +550,10 @@ class PortableLocalSGD:
                 loss.backward()
                 if prox_mu > 0:
                     _add_prox_term(params, anchors, prox_mu)
+                if corr is not None:
+                    with torch.no_grad():
+                        for p, cv in zip(params, corrs):     # a parameter without a gradient still moves by corr
+                            p.grad = cv.clone() if p.grad is None else p.grad.add_(cv)
                 opt.step()
                 out[e, 0] += float(loss.detach())
                 if not tgt.dtype.is_floating_point:
