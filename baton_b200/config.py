@@ -28,6 +28,10 @@ class FederationConfig:
     momentum: float = 0.0
     weight_decay: float = 0.0
     prox_mu: float = 0.0               # FedProx proximal coefficient (0: FedAvg's plain local SGD)
+    optimizer: str = "sgd"             # local optimizer: sgd | adamw (a fresh torch.optim.AdamW per client and round)
+    adam_beta1: float = 0.9            # AdamW betas and eps (read only with optimizer='adamw')
+    adam_beta2: float = 0.999
+    adam_eps: float = 1e-8
     dp_clip: float = 0.0               # DP-FedAvg: L2 clip norm of a client's update (0: DP off)
     dp_noise_multiplier: float = 0.0   # DP-FedAvg: noise std on the sum of clipped updates, in units of dp_clip
     dp_delta: float = 1e-5             # DP-FedAvg: delta of the (epsilon, delta) the manager reports
@@ -46,10 +50,20 @@ class FederationConfig:
     def __post_init__(self):
         if not (0.0 <= float(self.prox_mu) < float("inf")):
             raise ValueError("prox_mu must be a finite number >= 0, got {!r}".format(self.prox_mu))
+        from .train import check_adamw, check_optimizer
+        check_optimizer(self.optimizer, self.momentum, prox_mu=float(self.prox_mu))
+        check_adamw((self.adam_beta1, self.adam_beta2), self.adam_eps)
         from .parallel.dp import check_dp
         check_dp(self.dp_clip, self.dp_noise_multiplier)
         if not (0.0 < float(self.dp_delta) < 1.0):
             raise ValueError("dp_delta must lie in (0, 1), got {!r}".format(self.dp_delta))
+
+    def train_kwargs(self) -> dict:
+        """Local-training keyword arguments of a worker (``FederatedModule.local_train``)."""
+        kw = {"lr": self.lr, "batch_size": self.batch_size, "prox_mu": self.prox_mu}
+        if self.optimizer != "sgd":
+            kw.update(optimizer=self.optimizer, betas=(self.adam_beta1, self.adam_beta2), eps=self.adam_eps)
+        return kw
 
     def dp_config(self):
         """The :class:`~baton_b200.parallel.dp.DPConfig` of these fields, or None when DP is off (``dp_clip == 0``)."""

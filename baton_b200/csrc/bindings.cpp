@@ -44,14 +44,29 @@ inline const float* scaf_corr(const std::optional<at::Tensor>& corr, int64_t num
   return corr->data_ptr<float>();
 }
 
-// optimizer epilogue of a weight-gradient GEMM: theta / theta_bf16 / momentum / anchor / correction start at the element
-// of D[0, 0]
+// AdamW second moment of an optimizer step: fp32, contiguous, at least as long as the parameters; it needs the first
+// moment (the momentum buffer), the step's AdamW row as `hyper` (ADAMW_ROW = 12 floats) and no FedProx / SCAFFOLD term
+inline float* adam_v_ptr(const std::optional<at::Tensor>& v, int64_t numel, const float* mom, const at::Tensor& hyper,
+                         const float* anchor, const float* corr) {
+  if (!v.has_value() || !v->defined()) return nullptr;
+  CHECK_CUDA(*v);
+  TORCH_CHECK(v->scalar_type() == at::kFloat && v->is_contiguous() && v->numel() >= numel,
+              "adamw second moment: contiguous fp32 covering the parameters");
+  TORCH_CHECK(mom != nullptr, "an AdamW step needs the first-moment (momentum) buffer");
+  TORCH_CHECK(hyper.numel() >= 12, "an AdamW step takes its step row (12 floats) as hyper");
+  TORCH_CHECK(anchor == nullptr && corr == nullptr, "an AdamW step takes no FedProx anchor or SCAFFOLD correction");
+  return v->data_ptr<float>();
+}
+
+// optimizer epilogue of a weight-gradient GEMM: theta / theta_bf16 / momentum / anchor / correction / second moment
+// start at the element of D[0, 0]
 inline std::optional<B200SgdEpilogue> sgd_epilogue(const std::optional<at::Tensor>& theta,
                                                    const std::optional<at::Tensor>& theta_bf16,
                                                    const std::optional<at::Tensor>& mom,
                                                    const std::optional<at::Tensor>& hyper, bool nesterov,
                                                    const std::optional<at::Tensor>& anchor,
-                                                   const std::optional<at::Tensor>& corr) {
+                                                   const std::optional<at::Tensor>& corr,
+                                                   const std::optional<at::Tensor>& adam_v) {
   if (!hyper.has_value() || !hyper->defined()) return std::nullopt;
   TORCH_CHECK(theta.has_value() && theta->scalar_type() == at::kFloat && hyper->scalar_type() == at::kFloat &&
                   (!theta_bf16.has_value() || theta_bf16->scalar_type() == at::kBFloat16) &&
@@ -60,8 +75,10 @@ inline std::optional<B200SgdEpilogue> sgd_epilogue(const std::optional<at::Tenso
   const float* a = prox_anchor(anchor, theta->numel(), *hyper);
   // theta runs to the end of the arena, the correction to the end of the parameters: the GEMM only addresses its
   // output's elements, which are parameters
+  const float* c = scaf_corr(corr, 0, a);
   return B200SgdEpilogue{theta->data_ptr<float>(), opt_ptr<void>(theta_bf16), opt_ptr<float>(mom),
-                         hyper->data_ptr<float>(), nesterov ? 1 : 0, a, scaf_corr(corr, 0, a)};
+                         hyper->data_ptr<float>(), nesterov ? 1 : 0, a, c,
+                         adam_v_ptr(adam_v, 0, opt_ptr<float>(mom), *hyper, a, c)};
 }
 
 // eval-mode BatchNorm epilogue of a forward GEMM: fp32 [N] scale and shift, optional bf16 residual rows
@@ -120,7 +137,7 @@ bool gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor d, const std::opt
           const std::optional<at::Tensor>& sgd_theta, const std::optional<at::Tensor>& sgd_theta_bf16,
           const std::optional<at::Tensor>& sgd_mom, const std::optional<at::Tensor>& sgd_hyper, bool sgd_nesterov,
           const std::optional<at::Tensor>& sgd_anchor, const std::optional<at::Tensor>& sgd_corr,
-          const std::optional<at::Tensor>& bn_scale, const std::optional<at::Tensor>& bn_shift,
+          const std::optional<at::Tensor>& sgd_v, const std::optional<at::Tensor>& bn_scale, const std::optional<at::Tensor>& bn_shift,
           const std::optional<at::Tensor>& residual, bool bn_relu) {
   CHECK_CUDA(a); CHECK_CUDA(b); CHECK_CUDA(d);
   TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16, "gemm operands must be bf16");
@@ -139,7 +156,7 @@ bool gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor d, const std::opt
     return true;
   }
   const std::optional<B200SgdEpilogue> sgd =
-      sgd_epilogue(sgd_theta, sgd_theta_bf16, sgd_mom, sgd_hyper, sgd_nesterov, sgd_anchor, sgd_corr);
+      sgd_epilogue(sgd_theta, sgd_theta_bf16, sgd_mom, sgd_hyper, sgd_nesterov, sgd_anchor, sgd_corr, sgd_v);
   const std::optional<B200AffineEpilogue> affine = affine_epilogue(bn_scale, bn_shift, residual, bn_relu, M, N);
   const int rc = b200_gemm_bf16(cptr(a), cptr(b), ptr(d), bp, M, N, K, lda, ldb, ldd, a_mn, b_mn, out_fp32, act, split_k,
                                 accumulate, static_cast<float>(alpha), opt_ptr<const uint32_t>(flags),
@@ -294,13 +311,13 @@ bool conv_igemm_wgrad(const at::Tensor& dy, const at::Tensor& x, at::Tensor dw, 
                       const std::optional<at::Tensor>& sgd_theta, const std::optional<at::Tensor>& sgd_theta_bf16,
                       const std::optional<at::Tensor>& sgd_mom, const std::optional<at::Tensor>& sgd_hyper,
                       bool sgd_nesterov, const std::optional<at::Tensor>& sgd_anchor,
-                      const std::optional<at::Tensor>& sgd_corr) {
+                      const std::optional<at::Tensor>& sgd_corr, const std::optional<at::Tensor>& sgd_v) {
   CHECK_CUDA(dy); CHECK_CUDA(x); CHECK_CUDA(dw);
   TORCH_CHECK(x.scalar_type() == at::kBFloat16 && dy.scalar_type() == at::kBFloat16 && dw.scalar_type() == at::kFloat &&
               x.dim() == 4 && x.is_contiguous() && dy.is_contiguous());
   const c10::cuda::CUDAGuard guard(x.device());
   const std::optional<B200SgdEpilogue> sgd =
-      sgd_epilogue(sgd_theta, sgd_theta_bf16, sgd_mom, sgd_hyper, sgd_nesterov, sgd_anchor, sgd_corr);
+      sgd_epilogue(sgd_theta, sgd_theta_bf16, sgd_mom, sgd_hyper, sgd_nesterov, sgd_anchor, sgd_corr, sgd_v);
   const int rc = b200_conv_igemm_wgrad(cptr(dy), cptr(x), dw.data_ptr<float>(), static_cast<int>(x.size(0)),
                                        static_cast<int>(x.size(1)), static_cast<int>(x.size(2)), static_cast<int>(x.size(3)),
                                        static_cast<int>(cout), static_cast<int>(kh), static_cast<int>(kw),
@@ -342,17 +359,19 @@ void dequant_mx(const at::Tensor& q, const at::Tensor& sf, at::Tensor out, int64
 void fused_sgd(at::Tensor w, at::Tensor g, const std::optional<at::Tensor>& mom, const std::optional<at::Tensor>& wb,
                const at::Tensor& hyper, bool zero_grad, bool nesterov, const std::optional<at::Tensor>& wire_slot,
                const std::optional<at::Tensor>& pack_global, const std::optional<at::Tensor>& pack_scale, int64_t n_pack,
-               bool wire_fp32, const std::optional<at::Tensor>& prox_anchor_, const std::optional<at::Tensor>& corr) {
+               bool wire_fp32, const std::optional<at::Tensor>& prox_anchor_, const std::optional<at::Tensor>& corr,
+               const std::optional<at::Tensor>& adam_v) {
   CHECK_CUDA(w);
   TORCH_CHECK(w.scalar_type() == at::kFloat && g.scalar_type() == at::kFloat && hyper.scalar_type() == at::kFloat);
   TORCH_CHECK(w.is_contiguous() && g.is_contiguous() && w.numel() == g.numel());
   const c10::cuda::CUDAGuard guard(w.device());
   const float* anchor = prox_anchor(prox_anchor_, w.numel(), hyper);
+  const float* c = scaf_corr(corr, w.numel(), anchor);
   check(b200_fused_sgd(w.data_ptr<float>(), g.data_ptr<float>(), opt_ptr<float>(mom), opt_ptr<void>(wb), w.numel(),
                        hyper.data_ptr<float>(), zero_grad, nesterov,
                        reinterpret_cast<const unsigned long long*>(opt_ptr<const int64_t>(wire_slot)),
                        opt_ptr<const float>(pack_global), opt_ptr<const float>(pack_scale), n_pack, wire_fp32, anchor,
-                       scaf_corr(corr, w.numel(), anchor), cur_stream()),
+                       c, adam_v_ptr(adam_v, w.numel(), opt_ptr<float>(mom), hyper, anchor, c), cur_stream()),
         "fused_sgd");
 }
 
@@ -360,17 +379,18 @@ void fused_sgd(at::Tensor w, at::Tensor g, const std::optional<at::Tensor>& mom,
 void fused_sgd_segments(at::Tensor w, at::Tensor g, const std::optional<at::Tensor>& mom,
                         const std::optional<at::Tensor>& wb, const at::Tensor& segments, const at::Tensor& hyper,
                         bool nesterov, const std::optional<at::Tensor>& prox_anchor_,
-                        const std::optional<at::Tensor>& corr) {
+                        const std::optional<at::Tensor>& corr, const std::optional<at::Tensor>& adam_v) {
   CHECK_CUDA(w); CHECK_CUDA(segments);
   TORCH_CHECK(w.scalar_type() == at::kFloat && g.scalar_type() == at::kFloat && hyper.scalar_type() == at::kFloat);
   TORCH_CHECK(segments.scalar_type() == at::kLong && segments.dim() == 2 && segments.size(1) == 3 &&
               segments.is_contiguous(), "segments: contiguous int64 [n, 3]");
   const c10::cuda::CUDAGuard guard(w.device());
   const float* anchor = prox_anchor(prox_anchor_, w.numel(), hyper);
+  const float* c = scaf_corr(corr, g.numel(), anchor);
   check(b200_fused_sgd_segments(w.data_ptr<float>(), g.data_ptr<float>(), opt_ptr<float>(mom), opt_ptr<void>(wb),
                                 reinterpret_cast<const long long*>(segments.data_ptr<int64_t>()),
-                                static_cast<int>(segments.size(0)), hyper.data_ptr<float>(), nesterov, anchor,
-                                scaf_corr(corr, g.numel(), anchor), cur_stream()),
+                                static_cast<int>(segments.size(0)), hyper.data_ptr<float>(), nesterov, anchor, c,
+                                adam_v_ptr(adam_v, g.numel(), opt_ptr<float>(mom), hyper, anchor, c), cur_stream()),
         "fused_sgd_segments");
 }
 

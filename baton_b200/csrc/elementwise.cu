@@ -35,17 +35,75 @@ struct SgdPack {
   int wire_fp32;                         // 0: bf16 wire, 1: fp32 wire
 };
 
+// The upload copy of one 4-element group of new weights (SgdPack; `i` indexes float4 groups)
+__device__ __forceinline__ void sgd_pack4(const SgdPack& pk, uint8_t* wire, float pscale, long long i, float4 d) {
+  if (pk.global_w != nullptr) {
+    const float4 gl = reinterpret_cast<const float4*>(pk.global_w)[i];
+    d.x -= gl.x; d.y -= gl.y; d.z -= gl.z; d.w -= gl.w;
+  }
+  d.x *= pscale; d.y *= pscale; d.z *= pscale; d.w *= pscale;
+  if (pk.wire_fp32) reinterpret_cast<float4*>(wire)[i] = d;
+  else reinterpret_cast<uint2*>(wire)[i] = make_uint2(pack_bf16x2(d.x, d.y), pack_bf16x2(d.z, d.w));
+}
+
+// Body of the AdamW form of fused_sgd_kernel: the same passes (update + gradient zeroing + bf16 shadow + upload copy,
+// then the pack-only float buffers, then the scalar tail) with adamw_update in place of the SGD step.
+__device__ __forceinline__ void adamw_arena(float* __restrict__ w, float* __restrict__ g, float* __restrict__ m,
+                                            float* __restrict__ v, __nv_bfloat16* __restrict__ wb, long long n,
+                                            const AdamHyper h, int zero_grad, const SgdPack& pk) {
+  const long long nv = n >> 2;
+  uint8_t* wire = nullptr;
+  float pscale = 1.f;
+  if (pk.wire_slot != nullptr) {
+    wire = reinterpret_cast<uint8_t*>(*pk.wire_slot);
+    if (pk.scale != nullptr) pscale = *pk.scale;
+  }
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < nv; i += stride) {
+    float4 mv = reinterpret_cast<const float4*>(m)[i], vv = reinterpret_cast<const float4*>(v)[i];
+    const float4 wv = adamw_update4(h, reinterpret_cast<const float4*>(w)[i], reinterpret_cast<const float4*>(g)[i],
+                                    mv, vv);
+    reinterpret_cast<float4*>(m)[i] = mv;
+    reinterpret_cast<float4*>(v)[i] = vv;
+    reinterpret_cast<float4*>(w)[i] = wv;
+    if (zero_grad) reinterpret_cast<float4*>(g)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (wb != nullptr) reinterpret_cast<uint2*>(wb)[i] = make_uint2(pack_bf16x2(wv.x, wv.y), pack_bf16x2(wv.z, wv.w));
+    if (wire != nullptr) sgd_pack4(pk, wire, pscale, i, wv);
+  }
+  if (wire != nullptr) {      // float buffers behind the parameters: pack only (n and n_pack are multiples of 8)
+    for (long long i = nv + blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < (pk.n_pack >> 2);
+         i += stride)
+      sgd_pack4(pk, wire, pscale, i, reinterpret_cast<const float4*>(w)[i]);
+  }
+  if (blockIdx.x == 0) {
+    for (long long i = (nv << 2) + threadIdx.x; i < n; i += blockDim.x) {
+      const float wv = adamw_update(h, w[i], g[i], m[i], v[i]);
+      w[i] = wv;
+      if (zero_grad) g[i] = 0.f;
+      if (wb != nullptr) wb[i] = __float2bfloat16_rn(wv);
+    }
+  }
+}
+
 // PROX: FedProx step toward the anchor `aux` (indexed like w).  SCAF: SCAFFOLD step, `aux` is the correction c - c_i
 // (indexed like w).  The two are exclusive; with neither, `aux` is not read.  One pointer serves both so the plain and
 // FedProx instantiations keep their parameter list.
-template <bool PROX, bool SCAF = false>
+// ADAM: the AdamW step of sgd.cuh instead of SGD.  `hyper` is then the step's AdamW row (ADAMW_ROW floats), `mom` the
+// first moment m and `aux` the second moment v, which this form also writes (each element is read once, by the thread
+// that writes it); `nesterov` is not read.
+template <bool PROX, bool SCAF = false, bool ADAM = false>
 __global__ void __launch_bounds__(EW_THREADS)
 fused_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict__ mom,
                  __nv_bfloat16* __restrict__ wb, long long n, const float* __restrict__ hyper, int zero_grad,
                  int nesterov, const SgdPack pk, const float* __restrict__ aux) {
   static_assert(!(PROX && SCAF), "FedProx and SCAFFOLD are exclusive");
+  static_assert(!(ADAM && (PROX || SCAF)), "AdamW takes neither the FedProx nor the SCAFFOLD term");
   griddep_launch_dependents();
   griddep_wait();
+  if constexpr (ADAM) {
+    adamw_arena(w, g, mom, const_cast<float*>(aux), wb, n, load_adam_hyper(hyper), zero_grad, pk);
+    return;
+  }
   const SgdHyper h = PROX ? load_sgd_hyper_prox(hyper) : load_sgd_hyper(hyper);
   const long long nv = n >> 2;
   uint8_t* wire = nullptr;
@@ -121,6 +179,50 @@ __device__ __forceinline__ bool same_bits4(float4 a, float4 b) {
          __float_as_uint(a.z) == __float_as_uint(b.z) && __float_as_uint(a.w) == __float_as_uint(b.w);
 }
 
+// Body of the AdamW form of fused_sgd_segments_kernel.  A kind-1 element has g = 0 at every step, so its m and v are
+// 0 from the first step of a run on (the first step ignores what is stored), and its step is w *= (1 - lr*wd): the
+// identity exactly when that factor rounds to 1, i.e. with weight decay 0.  Kind-1 chunks are then skipped -- except
+// at the first step, where they are processed once so that their stored m and v really are 0 for the whole-arena
+// steps of the run (the momentum buffer may hold an earlier SGD run's momentum).  The skip is decided from the step
+// row in device memory, so a captured epoch stays exact.  Kind-1 weights are stored only where their bits change.
+__device__ __forceinline__ void adamw_segments(float* __restrict__ w, float* __restrict__ g, float* __restrict__ m,
+                                               float* __restrict__ v, __nv_bfloat16* __restrict__ wb,
+                                               const long long* __restrict__ seg, int n_seg, const AdamHyper h) {
+  const bool nograd_is_identity = h.decay == 1.f && !h.first;
+  for (int s = blockIdx.x; s < n_seg; s += gridDim.x) {
+    const long long off = seg[3 * s], len = seg[3 * s + 1];
+    const bool has_grad = seg[3 * s + 2] == 0;
+    if (!has_grad && nograd_is_identity) continue;      // block-uniform
+    long long done = 0;
+    if ((off & 3) == 0) {
+      const long long nv = len >> 2;
+      for (long long i = threadIdx.x; i < nv; i += blockDim.x) {
+        const long long e = off + (i << 2);
+        float4 mv = *reinterpret_cast<const float4*>(m + e), vv = *reinterpret_cast<const float4*>(v + e);
+        const float4 gv = has_grad ? *reinterpret_cast<const float4*>(g + e) : make_float4(0.f, 0.f, 0.f, 0.f);
+        const float4 w0 = *reinterpret_cast<const float4*>(w + e);
+        const float4 wv = adamw_update4(h, w0, gv, mv, vv);
+        *reinterpret_cast<float4*>(m + e) = mv;
+        *reinterpret_cast<float4*>(v + e) = vv;
+        if (!has_grad && same_bits4(w0, wv)) continue;
+        *reinterpret_cast<float4*>(w + e) = wv;
+        if (has_grad) *reinterpret_cast<float4*>(g + e) = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (wb != nullptr) *reinterpret_cast<uint2*>(wb + e) = make_uint2(pack_bf16x2(wv.x, wv.y), pack_bf16x2(wv.z, wv.w));
+      }
+      done = nv << 2;
+    }
+    for (long long i = done + threadIdx.x; i < len; i += blockDim.x) {
+      const long long e = off + i;
+      const float w0 = w[e];
+      const float wv = adamw_update(h, w0, has_grad ? g[e] : 0.f, m[e], v[e]);
+      if (!has_grad && __float_as_uint(w0) == __float_as_uint(wv)) continue;
+      w[e] = wv;
+      if (has_grad) g[e] = 0.f;
+      if (wb != nullptr) wb[e] = __float2bfloat16_rn(wv);
+    }
+  }
+}
+
 // ------------------------------------------------------------------ leftover SGD of a step with an optimizer epilogue
 // When the weight-gradient GEMMs of a step applied SGD in their epilogue (gemm_wgmma.cu), what is left is a set of
 // arena ranges, given as a device table of chunks {offset, length, kind} -- one chunk per CTA iteration.
@@ -133,14 +235,20 @@ __device__ __forceinline__ bool same_bits4(float4 a, float4 b) {
 // only where its bits change.  In engine rounds these taps equal the global model all round, so nothing is written.
 // SCAF (`aux` = the correction c - c_i, as in fused_sgd_kernel): a kind-1 element moves by -lr * (corr [+ wd*w]), so
 // kind-1 chunks are never skipped; they use the same sparse store (a zero correction writes nothing).
-template <bool PROX, bool SCAF = false>
+// ADAM (`hyper` = the AdamW step row, `mom` = m, `aux` = v, as in fused_sgd_kernel): see adamw_segments.
+template <bool PROX, bool SCAF = false, bool ADAM = false>
 __global__ void __launch_bounds__(EW_THREADS)
 fused_sgd_segments_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict__ mom,
                           __nv_bfloat16* __restrict__ wb, const long long* __restrict__ seg, int n_seg,
                           const float* __restrict__ hyper, int nesterov, const float* __restrict__ aux) {
   static_assert(!(PROX && SCAF), "FedProx and SCAFFOLD are exclusive");
+  static_assert(!(ADAM && (PROX || SCAF)), "AdamW takes neither the FedProx nor the SCAFFOLD term");
   griddep_launch_dependents();
   griddep_wait();
+  if constexpr (ADAM) {
+    adamw_segments(w, g, mom, const_cast<float*>(aux), wb, seg, n_seg, load_adam_hyper(hyper));
+    return;
+  }
   const SgdHyper h = PROX ? load_sgd_hyper_prox(hyper) : load_sgd_hyper(hyper);
   const bool has_mom = mom != nullptr;
   const bool nograd_is_identity = !SCAF && h.prox == 0.f && h.wd == 0.f && !has_mom;
@@ -596,37 +704,45 @@ using namespace b200;
 extern "C" int b200_fused_sgd(float* w, float* g, float* mom, void* w_bf16, long long n, const float* hyper,
                               int zero_grad, int nesterov, const unsigned long long* wire_slot,
                               const float* pack_global, const float* pack_scale, long long n_pack, int wire_fp32,
-                              const float* prox_anchor, const float* corr, cudaStream_t stream) {
+                              const float* prox_anchor, const float* corr, float* adam_v, cudaStream_t stream) {
   if (n <= 0) return 0;
   SgdPack pk;
   pk.wire_slot = wire_slot; pk.global_w = pack_global; pk.scale = pack_scale;
   pk.n_pack = n_pack > n ? n_pack : n; pk.wire_fp32 = wire_fp32;
   if (wire_slot != nullptr && ((n & 7) || (pk.n_pack & 7))) return -2;
   if (prox_anchor != nullptr && corr != nullptr) return -2;
+  if (adam_v != nullptr && (prox_anchor != nullptr || corr != nullptr || mom == nullptr)) return -2;
   // read as float4 at the offsets of w
-  if ((reinterpret_cast<uintptr_t>(prox_anchor) | reinterpret_cast<uintptr_t>(corr)) & 15) return -2;
-  auto kernel = prox_anchor != nullptr ? fused_sgd_kernel<true>
+  if ((reinterpret_cast<uintptr_t>(prox_anchor) | reinterpret_cast<uintptr_t>(corr) |
+       reinterpret_cast<uintptr_t>(adam_v)) & 15)
+    return -2;
+  auto kernel = adam_v != nullptr      ? fused_sgd_kernel<false, false, true>
+                : prox_anchor != nullptr ? fused_sgd_kernel<true>
                 : corr != nullptr      ? fused_sgd_kernel<false, true>
                                        : fused_sgd_kernel<false>;
   launch_pdl(kernel, ew_grid(n >> 2), EW_THREADS, 0, stream, w, g, mom, reinterpret_cast<__nv_bfloat16*>(w_bf16), n,
-             hyper, zero_grad, nesterov, pk, prox_anchor != nullptr ? prox_anchor : corr);
+             hyper, zero_grad, nesterov, pk,
+             adam_v != nullptr ? adam_v : prox_anchor != nullptr ? prox_anchor : corr);
   RET_LAST();
 }
 extern "C" int b200_fused_sgd_segments(float* w, float* g, float* mom, void* w_bf16, const long long* segments, int n_seg,
                                        const float* hyper, int nesterov, const float* prox_anchor, const float* corr,
-                                       cudaStream_t stream) {
+                                       float* adam_v, cudaStream_t stream) {
   if (n_seg <= 0) return 0;
   if ((reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(mom) |
-       reinterpret_cast<uintptr_t>(prox_anchor) | reinterpret_cast<uintptr_t>(corr)) & 15 ||
+       reinterpret_cast<uintptr_t>(prox_anchor) | reinterpret_cast<uintptr_t>(corr) |
+       reinterpret_cast<uintptr_t>(adam_v)) & 15 ||
       reinterpret_cast<uintptr_t>(w_bf16) & 7)
     return -2;
   if (prox_anchor != nullptr && corr != nullptr) return -2;
-  auto kernel = prox_anchor != nullptr ? fused_sgd_segments_kernel<true>
+  if (adam_v != nullptr && (prox_anchor != nullptr || corr != nullptr || mom == nullptr)) return -2;
+  auto kernel = adam_v != nullptr        ? fused_sgd_segments_kernel<false, false, true>
+                : prox_anchor != nullptr ? fused_sgd_segments_kernel<true>
                 : corr != nullptr      ? fused_sgd_segments_kernel<false, true>
                                        : fused_sgd_segments_kernel<false>;
   launch_pdl(kernel, ew_grid(n_seg * static_cast<long long>(EW_THREADS)), EW_THREADS, 0, stream, w, g, mom,
              reinterpret_cast<__nv_bfloat16*>(w_bf16), segments, n_seg, hyper, nesterov,
-             prox_anchor != nullptr ? prox_anchor : corr);
+             adam_v != nullptr ? adam_v : prox_anchor != nullptr ? prox_anchor : corr);
   RET_LAST();
 }
 extern "C" int b200_scaffold_corr(float* corr, const float* c, const float* ci, long long n, cudaStream_t stream) {

@@ -98,6 +98,9 @@ struct GemmParams {
   const float* sgd_anchor = nullptr;
   // SCAFFOLD correction c - c_i of the optimizer epilogue, indexed like sgd_theta; nullptr: no correction term
   const float* sgd_corr = nullptr;
+  // AdamW second moment of the optimizer epilogue, indexed like sgd_theta (sgd_mom is then the first moment and
+  // sgd_hyper the step's AdamW row); nullptr: SGD
+  float* sgd_v = nullptr;
 };
 
 // Wait until every arrival flag covering arena elements [e0, e1] has reached `need` (published by the FedAvg kernel with
@@ -294,6 +297,43 @@ __device__ __forceinline__ void store_row_chunk(const GemmParams& p, int row, in
 // is read beside theta instead.
 template <bool PROX, bool SCAF = false>
 __device__ __forceinline__ void sgd_epilogue_chunk(const GemmParams& p, size_t e, int col0, const float (&v)[32],
+                                                   bool vec);
+
+// The AdamW form (adamw_update of sgd.cuh, the arithmetic of the arena kernels' AdamW instantiations): m is sgd_mom,
+// v is sgd_v, the coefficients are the step row at sgd_hyper.
+__device__ __forceinline__ void adamw_epilogue_chunk(const GemmParams& p, size_t e, int col0, const float (&v)[32],
+                                                     bool vec) {
+  const AdamHyper h = load_adam_hyper(p.sgd_hyper);
+  float* w = p.sgd_theta + e;
+  float* m = p.sgd_mom + e;
+  float* sq = p.sgd_v + e;
+  __nv_bfloat16* wb = p.sgd_wb != nullptr ? p.sgd_wb + e : nullptr;
+  if (vec && col0 + 32 <= p.N) {
+#pragma unroll
+    for (int j = 0; j < 32; j += 4) {
+      float4 mv = *reinterpret_cast<const float4*>(m + j), vv = *reinterpret_cast<const float4*>(sq + j);
+      const float4 gv = make_float4(__fadd_rn(0.f, v[j]), __fadd_rn(0.f, v[j + 1]), __fadd_rn(0.f, v[j + 2]),
+                                    __fadd_rn(0.f, v[j + 3]));
+      const float4 wv = adamw_update4(h, *reinterpret_cast<const float4*>(w + j), gv, mv, vv);
+      *reinterpret_cast<float4*>(w + j) = wv;
+      *reinterpret_cast<float4*>(m + j) = mv;
+      *reinterpret_cast<float4*>(sq + j) = vv;
+      if (wb != nullptr) *reinterpret_cast<uint2*>(wb + j) = make_uint2(pack_bf16x2(wv.x, wv.y), pack_bf16x2(wv.z, wv.w));
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      if (col0 + j < p.N) {
+        const float wv = adamw_update(h, w[j], __fadd_rn(0.f, v[j]), m[j], sq[j]);
+        w[j] = wv;
+        if (wb != nullptr) wb[j] = __float2bfloat16_rn(wv);
+      }
+    }
+  }
+}
+
+template <bool PROX, bool SCAF>
+__device__ __forceinline__ void sgd_epilogue_chunk(const GemmParams& p, size_t e, int col0, const float (&v)[32],
                                                    bool vec) {
   const float* a = PROX ? p.sgd_anchor + e : SCAF ? p.sgd_corr + e : nullptr;
   const SgdHyper h = PROX ? load_sgd_hyper_prox(p.sgd_hyper) : load_sgd_hyper(p.sgd_hyper);
@@ -429,9 +469,11 @@ __device__ __forceinline__ void s2_load_ktile(const CUtensorMap* tmA, const CUte
 // no col2im); 4 = implicit dgrad of a stride-2 convolution, one parity class of dx pixels per group of M tiles (see
 // s2_class).  See csrc/im2col_tma.cu for the tensor maps.
 // SGD: optimizer epilogue instantiation (weight gradients only) -- every other GEMM keeps the plain epilogue.
-// PROX (with SGD): the FedProx form of that epilogue.  SCAF (with SGD): its SCAFFOLD form.
+// PROX (with SGD): the FedProx form of that epilogue.  SCAF (with SGD): its SCAFFOLD form.  ADAM (with SGD): its
+// AdamW form (adamw_epilogue_chunk).
 // AFFINE: eval-mode BatchNorm epilogue instantiation (affine_chunk, forward convolutions in evaluation).
-template <int BN, int STAGES, int CONV = 0, bool SGD = false, bool AFFINE = false, bool PROX = false, bool SCAF = false>
+template <int BN, int STAGES, int CONV = 0, bool SGD = false, bool AFFINE = false, bool PROX = false, bool SCAF = false,
+          bool ADAM = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                          const GemmParams p) {
@@ -593,7 +635,8 @@ gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     const bool sgd_vec = SGD && (p.ldd % 4 == 0) &&
                          ((reinterpret_cast<uintptr_t>(p.sgd_theta) | reinterpret_cast<uintptr_t>(p.sgd_mom) |
                            (PROX ? reinterpret_cast<uintptr_t>(p.sgd_anchor) : 0) |
-                           (SCAF ? reinterpret_cast<uintptr_t>(p.sgd_corr) : 0)) & 15) == 0 &&
+                           (SCAF ? reinterpret_cast<uintptr_t>(p.sgd_corr) : 0) |
+                           (ADAM ? reinterpret_cast<uintptr_t>(p.sgd_v) : 0)) & 15) == 0 &&
                          (reinterpret_cast<uintptr_t>(p.sgd_wb) & 7) == 0;
     // fused BatchNorm statistics: per row quarter column sums, [4 quarters][2 * BN] floats
     float* sstat = cstat + q * 2 * BN;
@@ -620,7 +663,8 @@ gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       }
       const bool full = (col0 + 32 <= p.N);
       if constexpr (SGD) {
-        sgd_epilogue_chunk<PROX, SCAF>(p, static_cast<size_t>(row) * p.ldd + col0, col0, v, sgd_vec);
+        if constexpr (ADAM) adamw_epilogue_chunk(p, static_cast<size_t>(row) * p.ldd + col0, col0, v, sgd_vec);
+        else sgd_epilogue_chunk<PROX, SCAF>(p, static_cast<size_t>(row) * p.ldd + col0, col0, v, sgd_vec);
         continue;
       }
       if (p.atomic_out) {
@@ -1119,7 +1163,7 @@ static int clamp_bn(int bn) { return bn > 128 ? 128 : bn; }
 
 static void set_sgd_epilogue(GemmParams& p, const B200SgdEpilogue& s) {
   p.sgd_hyper = s.hyper; p.sgd_theta = s.theta; p.sgd_wb = reinterpret_cast<__nv_bfloat16*>(s.theta_bf16);
-  p.sgd_mom = s.mom; p.sgd_nesterov = s.nesterov; p.sgd_anchor = s.anchor; p.sgd_corr = s.corr;
+  p.sgd_mom = s.mom; p.sgd_nesterov = s.nesterov; p.sgd_anchor = s.anchor; p.sgd_corr = s.corr; p.sgd_v = s.v;
 }
 
 static void set_affine_epilogue(GemmParams& p, const B200AffineEpilogue& a) {
@@ -1135,29 +1179,34 @@ static bool affine_ok(const B200AffineEpilogue& a, int N) {
          (a.residual == nullptr || (a.ldr % 8 == 0 && a.ldr >= N));
 }
 
-template <int BN, int STAGES, int CONV = 0, bool SGD = false, bool AFFINE = false, bool PROX = false, bool SCAF = false>
+template <int BN, int STAGES, int CONV = 0, bool SGD = false, bool AFFINE = false, bool PROX = false, bool SCAF = false,
+          bool ADAM = false>
 static int launch_fixed(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, dim3 grid,
                       cudaStream_t stream) {
   constexpr int smem = STAGES * SmemLayout<BN>::STAGE_BYTES + 2 * STAGES * 8 + 8 * BN * 4 + 1024;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD, AFFINE, PROX, SCAF>,
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD, AFFINE, PROX, SCAF, ADAM>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return static_cast<int>(e);
     configured = true;
   }
-  cudaError_t le = launch_pdl(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD, AFFINE, PROX, SCAF>, grid, GEMM_THREADS, smem, stream,
+  cudaError_t le = launch_pdl(gemm_bf16_fixed_kernel<BN, STAGES, CONV, SGD, AFFINE, PROX, SCAF, ADAM>, grid, GEMM_THREADS, smem, stream,
                               ta, tb, p);
   if (le != cudaSuccess) return static_cast<int>(le);
   return static_cast<int>(cudaGetLastError());
 }
 
 // the optimizer-epilogue instantiation, in its FedProx form when the step has an anchor, in its SCAFFOLD form when it
-// has a correction
+// has a correction, in its AdamW form when it has a second moment
 template <int BN, int STAGES, int CONV>
 static int launch_fixed_sgd(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, dim3 grid,
                             cudaStream_t stream) {
   if (p.sgd_anchor != nullptr && p.sgd_corr != nullptr) return -2;
+  if (p.sgd_v != nullptr) {
+    if (p.sgd_anchor != nullptr || p.sgd_corr != nullptr || p.sgd_mom == nullptr) return -2;
+    return launch_fixed<BN, STAGES, CONV, true, false, false, false, true>(ta, tb, p, grid, stream);
+  }
   if (p.sgd_corr != nullptr) return launch_fixed<BN, STAGES, CONV, true, false, false, true>(ta, tb, p, grid, stream);
   return p.sgd_anchor != nullptr ? launch_fixed<BN, STAGES, CONV, true, false, true>(ta, tb, p, grid, stream)
                                  : launch_fixed<BN, STAGES, CONV, true>(ta, tb, p, grid, stream);

@@ -21,6 +21,8 @@ struct B200SgdEpilogue {
   int nesterov;
   const float* anchor;              // FedProx anchor (global model), indexed like theta, or nullptr (no proximal term)
   const float* corr;                // SCAFFOLD correction c - c_i, indexed like theta, or nullptr (exclusive with anchor)
+  float* v;                         // AdamW second moment, indexed like theta, or nullptr (SGD).  With it, mom is the
+                                    // first moment and hyper the step's AdamW row (ADAMW_ROW floats, csrc/sgd.cuh)
 };
 #define B200_SGD_EPILOGUE_DECLINED (-6)
 
@@ -88,15 +90,17 @@ int b200_gemm_simt(const void* a, const void* b, void* d, const float* bias, int
 // the FedProx coefficient mu of the term mu * (w - prox_anchor) added to the gradient (prox_anchor indexed like w)
 // corr != nullptr (SCAFFOLD, exclusive with prox_anchor): the correction c - c_i, indexed like w, added to the gradient
 // wire_slot != nullptr: also emit the client's wire copy for the round-end collective (see SgdPack in elementwise.cu)
+// adam_v != nullptr: the AdamW step instead of SGD (no anchor, no correction): mom is the first moment, adam_v the
+// second, hyper the step's AdamW row of ADAMW_ROW floats (csrc/sgd.cuh); nesterov is not read
 int b200_fused_sgd(float* w, float* g, float* mom, void* w_bf16, long long n, const float* hyper, int zero_grad,
                    int nesterov, const unsigned long long* wire_slot, const float* pack_global,
                    const float* pack_scale, long long n_pack, int wire_fp32, const float* prox_anchor,
-                   const float* corr, cudaStream_t stream);
+                   const float* corr, float* adam_v, cudaStream_t stream);
 // the same step over a device table of n_seg arena chunks {offset, length, kind} (int64 [n_seg][3]); kind 0: with a
 // gradient (zeroed afterwards), kind 1: gradient identically zero (never read)
 int b200_fused_sgd_segments(float* w, float* g, float* mom, void* w_bf16, const long long* segments, int n_seg,
                             const float* hyper, int nesterov, const float* prox_anchor, const float* corr,
-                            cudaStream_t stream);
+                            float* adam_v, cudaStream_t stream);
 // SCAFFOLD control variates over n parameters (n % 4 == 0, 16-byte aligned): corr = c - c_i before a client trains;
 // after it trained, dc = (global_w - theta) * inv_k_eta - c, c_i += dc, up = dc (first != 0) or up += dc
 int b200_scaffold_corr(float* corr, const float* c, const float* ci, long long n, cudaStream_t stream);

@@ -76,4 +76,46 @@ __device__ __forceinline__ float4 sgd_update4_scaf(const SgdHyper& h, float4 w, 
   return w;
 }
 
+// ------------------------------------------------------------------ AdamW (torch.optim.AdamW, one parameter group)
+//     w = w * (1 - lr*wd) ;  m = b1*m + (1-b1)*g ;  v = b2*v + (1-b2)*g^2 ;
+//     w -= (lr / (1-b1^t)) * m / (sqrt(v) / sqrt(1-b2^t) + eps)
+// The coefficients of local step t come as ONE row of device floats (ADAMW_ROW), written by the host in fp64 and rounded
+// once: every kernel of a step reads the same row, so all three optimizer sites see the same fp32 coefficients, and a
+// captured epoch reads its step's row at replay (the host refreshes the rows between replays).  At t == 1 (`first`) the
+// stored m and v are ignored -- the state of a fresh optimizer -- so a new round, the next logical client and the
+// captured warm-up steps need no reset pass.  The operations are the IEEE-rounded intrinsics so that fast-math builds
+// cannot contract them differently at the three sites.
+constexpr int ADAMW_ROW = 12;   // floats per step row (48 B): the fields of AdamHyper, then padding
+
+struct AdamHyper {
+  float decay;          // 1 - lr*wd
+  float b1, omb1;       // beta1, 1 - beta1
+  float b2, omb2;       // beta2, 1 - beta2
+  float eps;
+  float step;           // lr / (1 - beta1^t)
+  float inv_bc2;        // 1 / sqrt(1 - beta2^t)
+  bool first;           // t == 1
+};
+
+__device__ __forceinline__ AdamHyper load_adam_hyper(const float* r) {
+  return AdamHyper{r[0], r[1], r[2], r[3], r[4], r[5], r[6], r[7], r[8] != 0.f};
+}
+
+// returns the new w; m and v are read (unless h.first) and updated
+__device__ __forceinline__ float adamw_update(const AdamHyper& h, float w, float g, float& m, float& v) {
+  const float m0 = h.first ? 0.f : m, v0 = h.first ? 0.f : v;
+  m = fmaf(h.b1, m0, __fmul_rn(h.omb1, g));
+  v = fmaf(h.b2, v0, __fmul_rn(__fmul_rn(h.omb2, g), g));
+  const float denom = fmaf(__fsqrt_rn(v), h.inv_bc2, h.eps);
+  return fmaf(-h.step, __fdiv_rn(m, denom), __fmul_rn(w, h.decay));
+}
+
+__device__ __forceinline__ float4 adamw_update4(const AdamHyper& h, float4 w, float4 g, float4& m, float4& v) {
+  w.x = adamw_update(h, w.x, g.x, m.x, v.x);
+  w.y = adamw_update(h, w.y, g.y, m.y, v.y);
+  w.z = adamw_update(h, w.z, g.z, m.z, v.z);
+  w.w = adamw_update(h, w.w, g.w, m.w, v.w);
+  return w;
+}
+
 }  // namespace b200

@@ -77,7 +77,7 @@ def make_gpu_worker(app, model, host: str, port: int, cfg: FederationConfig):
     return GpuExperimentWorker(app, model, host, device=dev, shard_fn=lambda: (X, y), backend=cfg.backend,
                                wire_dtype=cfg.wire_dtype, momentum=cfg.momentum, port=port,
                                heartbeat_time=cfg.heartbeat_time,
-                               train_kwargs={"lr": cfg.lr, "batch_size": cfg.batch_size, "prox_mu": cfg.prox_mu})
+                               train_kwargs=cfg.train_kwargs())
 
 
 def make_app(role: str, host: str, port: int, cfg: Optional[FederationConfig] = None) -> web.Application:
@@ -96,7 +96,7 @@ def make_app(role: str, host: str, port: int, cfg: Optional[FederationConfig] = 
     elif role == "worker":
         worker = LinearTestWorker(
             app, model, host, port=port, heartbeat_time=cfg.heartbeat_time,
-            train_kwargs={"lr": cfg.lr, "batch_size": cfg.batch_size, "prox_mu": cfg.prox_mu},
+            train_kwargs=cfg.train_kwargs(),
             seed=(cfg.seed * 1000 + port) if cfg.seed else None)
         app["worker"] = worker
     else:

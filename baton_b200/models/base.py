@@ -31,6 +31,7 @@ class FederatedModule(nn.Module):
     default_momentum = 0.0
     default_weight_decay = 0.0
     default_prox_mu = 0.0          # FedProx coefficient (0: plain SGD)
+    default_optimizer = "sgd"      # local optimizer: "sgd" or "adamw" (betas / eps: local_train keywords)
 
     def signature(self):
         return tuple((k, *v.shape) for k, v in self.state_dict().items())
@@ -49,6 +50,7 @@ class FederatedModule(nn.Module):
         kw.setdefault("momentum", self.default_momentum)
         kw.setdefault("weight_decay", self.default_weight_decay)
         kw.setdefault("prox_mu", self.default_prox_mu)
+        kw.setdefault("optimizer", self.default_optimizer)
         trainer = getattr(self, "_graphed_trainer", None)
         if X.is_cuda and trainer is not None:
             return trainer.run(X, y, n_epoch=n_epoch, lr=lr, batch_size=batch_size, **kw)

@@ -113,7 +113,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
     if use_simt:
         assert col_stats is None, "fused column statistics need the tensor-core path"
         C.gemm(a, b, out, bias, M, N, K, lda, ldb, ldd, a_mn, b_mn, act, 1, accumulate, alpha, None, 0, 0, 0, -1, 0,
-               True, None, None, None, None, None, None, False, None, None, None, None, None, False)
+               True, None, None, None, None, None, None, False, None, None, None, None, None, None, False)
         return out
     bn = force_bn or pick_bn(M, N)
     if col_stats is not None:
@@ -135,7 +135,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
     if not C.gemm(a, b, out, bias, M, N, K, lda, ldb, ldd, a_mn, b_mn, act, split_k, accumulate, alpha, flags, flag_epoch,
                   flag_elem_off, flag_tile_elems, flag_bias_off, bn, False, col_stats, flag_epoch_word, sg.get("theta"),
                   sg.get("theta_bf16"), sg.get("momentum"), sg.get("hyper"), bool(sg.get("nesterov", False)),
-                  sg.get("anchor"), sg.get("corr"), af.get("scale"), af.get("shift"), af.get("residual"), bool(af.get("relu", False))):
+                  sg.get("anchor"), sg.get("corr"), sg.get("adam_v"), af.get("scale"), af.get("shift"), af.get("residual"), bool(af.get("relu", False))):
         return None
     return out
 
@@ -169,8 +169,11 @@ def gemm_stats_fusable(M: int, N: int, K: int) -> bool:
 def fused_sgd(w: torch.Tensor, g: torch.Tensor, hyper: torch.Tensor, momentum_buf: Optional[torch.Tensor] = None,
               w_bf16: Optional[torch.Tensor] = None, zero_grad: bool = True, nesterov: bool = False,
               pack: Optional[dict] = None, prox_anchor: Optional[torch.Tensor] = None,
-              corr: Optional[torch.Tensor] = None) -> None:
+              corr: Optional[torch.Tensor] = None, adam_v: Optional[torch.Tensor] = None) -> None:
     """One kernel over the whole flat arena (reference: ``optimizer.step()``, demo.py:47).
+
+    ``adam_v`` (AdamW, exclusive with ``prox_anchor`` and ``corr``): fp32 second moment indexed like ``w``; the step is
+    then AdamW's, ``momentum_buf`` (required) is the first moment and ``hyper`` the step's row of :func:`adamw_rows`.
 
     ``prox_anchor`` (FedProx): fp32 buffer indexed like ``w`` (the global model the round started from); the step adds
     ``hyper[4] * (w - prox_anchor)`` to the gradient, so ``hyper`` then holds 5 floats
@@ -186,22 +189,44 @@ def fused_sgd(w: torch.Tensor, g: torch.Tensor, hyper: torch.Tensor, momentum_bu
     pk = pack or {}
     load().fused_sgd(w, g, momentum_buf, w_bf16, hyper, zero_grad, nesterov, pk.get("wire_slot"),
                      pk.get("global_w"), pk.get("scale"), int(pk.get("n_pack", 0)), bool(pk.get("wire_fp32", False)),
-                     prox_anchor, corr)
+                     prox_anchor, corr, adam_v)
+
+
+ADAMW_ROW = 12         # floats per AdamW step row (csrc/sgd.cuh: ADAMW_ROW / AdamHyper)
+
+
+def adamw_rows(lr: float, betas: Tuple[float, float], eps: float, weight_decay: float, t0: int, count: int,
+               first: bool = True) -> torch.Tensor:
+    """fp32 ``[count, ADAMW_ROW]`` AdamW coefficients of local steps ``t0 .. t0 + count - 1`` (``t`` counts from 1),
+    computed in fp64 and rounded once: ``{1 - lr*wd, b1, 1 - b1, b2, 1 - b2, eps, lr / (1 - b1^t),
+    1 / sqrt(1 - b2^t), t == 1}`` -- the bias corrections of ``torch.optim.AdamW``.  ``first=False`` never marks a
+    row as the first step."""
+    b1, b2 = float(betas[0]), float(betas[1])
+    lr, eps, wd = float(lr), float(eps), float(weight_decay)
+    rows = torch.zeros(count, ADAMW_ROW, dtype=torch.float64)
+    t = torch.arange(t0, t0 + count, dtype=torch.float64)
+    rows[:, 0] = 1.0 - lr * wd
+    rows[:, 1], rows[:, 2], rows[:, 3], rows[:, 4], rows[:, 5] = b1, 1.0 - b1, b2, 1.0 - b2, eps
+    rows[:, 6] = lr / (1.0 - torch.pow(torch.tensor(b1, dtype=torch.float64), t))
+    rows[:, 7] = 1.0 / torch.sqrt(1.0 - torch.pow(torch.tensor(b2, dtype=torch.float64), t))
+    rows[:, 8] = ((t == 1) & first).to(torch.float64)
+    return rows.to(torch.float32)
 
 
 def sgd_epilogue_args(theta: torch.Tensor, grad: torch.Tensor, grad_view: torch.Tensor, hyper: torch.Tensor,
                       momentum: Optional[torch.Tensor] = None, theta_bf16: Optional[torch.Tensor] = None,
                       nesterov: bool = False, anchor: Optional[torch.Tensor] = None,
-                      corr: Optional[torch.Tensor] = None) -> dict:
+                      corr: Optional[torch.Tensor] = None, adam_v: Optional[torch.Tensor] = None) -> dict:
     """``sgd=`` argument of a weight-gradient GEMM whose output ``grad_view`` is a view of the flat gradient ``grad``:
-    the parameter, bf16 shadow, momentum, FedProx anchor and SCAFFOLD correction buffers (same offsets as ``grad``)
-    from the element ``grad_view[0, 0]`` on.  With an ``anchor`` the step is the one of :func:`fused_sgd` with
-    ``prox_anchor``, with a ``corr`` the one with ``corr``."""
+    the parameter, bf16 shadow, momentum, FedProx anchor, SCAFFOLD correction and AdamW second-moment buffers (same
+    offsets as ``grad``) from the element ``grad_view[0, 0]`` on.  With an ``anchor`` the step is the one of
+    :func:`fused_sgd` with ``prox_anchor``, with a ``corr`` the one with ``corr``, with an ``adam_v`` AdamW's."""
     off = (grad_view.data_ptr() - grad.data_ptr()) // grad.element_size()
     assert 0 <= off < grad.numel(), "the GEMM output is not a view of the gradient arena"
     return {"theta": theta[off:], "theta_bf16": theta_bf16[off:] if theta_bf16 is not None else None,
             "momentum": momentum[off:] if momentum is not None else None, "hyper": hyper, "nesterov": nesterov,
-            "anchor": anchor[off:] if anchor is not None else None, "corr": corr[off:] if corr is not None else None}
+            "anchor": anchor[off:] if anchor is not None else None, "corr": corr[off:] if corr is not None else None,
+            "adam_v": adam_v[off:] if adam_v is not None else None}
 
 
 SGD_CHUNK = 8192       # arena elements per chunk of the leftover optimizer pass (one CTA iteration each)
@@ -239,11 +264,12 @@ def sgd_segments(n: int, fused: Sequence[Tuple[int, int, int, int]], nograd: Seq
 def fused_sgd_segments(w: torch.Tensor, g: torch.Tensor, hyper: torch.Tensor, segments: torch.Tensor,
                        momentum_buf: Optional[torch.Tensor] = None, w_bf16: Optional[torch.Tensor] = None,
                        nesterov: bool = False, prox_anchor: Optional[torch.Tensor] = None,
-                       corr: Optional[torch.Tensor] = None) -> None:
+                       corr: Optional[torch.Tensor] = None, adam_v: Optional[torch.Tensor] = None) -> None:
     """The step of :func:`fused_sgd` over the arena chunks of ``segments`` (device int64 ``[S, 3]`` from
-    :func:`sgd_segments`); chunks of kind 1 never read the gradient.  ``prox_anchor`` and ``corr`` as in
-    :func:`fused_sgd`; a kind-1 element without a momentum buffer is then written only where the step changes it."""
-    load().fused_sgd_segments(w, g, momentum_buf, w_bf16, segments, hyper, nesterov, prox_anchor, corr)
+    :func:`sgd_segments`); chunks of kind 1 never read the gradient.  ``prox_anchor``, ``corr`` and ``adam_v`` as in
+    :func:`fused_sgd`; a kind-1 element without a momentum buffer (or with AdamW) is then written only where the step
+    changes it."""
+    load().fused_sgd_segments(w, g, momentum_buf, w_bf16, segments, hyper, nesterov, prox_anchor, corr, adam_v)
 
 
 def scaffold_corr(corr: torch.Tensor, c: torch.Tensor, c_i: torch.Tensor) -> None:
@@ -535,7 +561,8 @@ def conv_igemm_wgrad_(dy2d: torch.Tensor, x: torch.Tensor, dw2d: torch.Tensor, k
     sg = sgd or {}
     return bool(load().conv_igemm_wgrad(dy2d, x, dw2d, cout, kh, kw, stride, pad, ho, wo, split_k, bn,
                                         sg.get("theta"), sg.get("theta_bf16"), sg.get("momentum"), sg.get("hyper"),
-                                        bool(sg.get("nesterov", False)), sg.get("anchor"), sg.get("corr")))
+                                        bool(sg.get("nesterov", False)), sg.get("anchor"), sg.get("corr"),
+                                        sg.get("adam_v")))
 
 
 def col2im(col: torch.Tensor, shape: Tuple[int, int, int, int], kh: int, kw: int, stride: int, pad: int,

@@ -181,16 +181,18 @@ class _SgdEpilogue:
     weight (its other taps never receive a gradient).  The trainer's leftover optimizer pass covers the rest of the
     arena (``F.sgd_segments``).  The gradient of a fused block is never written, so it stays zero for unfused steps.
     ``prox``: FedProx step anchored on ``arena.global_w`` (``hyper`` then holds the coefficient as its fifth float).
-    ``corr``: SCAFFOLD step with the correction ``c - c_i`` (fp32, indexed like the parameters)."""
+    ``corr``: SCAFFOLD step with the correction ``c - c_i`` (fp32, indexed like the parameters).
+    ``adam_v``: AdamW step with this second moment (``arena.momentum`` is the first, ``hyper`` the step's AdamW row)."""
 
     def __init__(self):
         self.arena = None
 
     @contextlib.contextmanager
-    def open(self, arena, hyper, nesterov, prox=False, corr=None):
+    def open(self, arena, hyper, nesterov, prox=False, corr=None, adam_v=None):
         self.arena, self.hyper, self.nesterov = arena, hyper, nesterov
         self.anchor = arena.global_w if prox else None
         self.corr = corr
+        self.adam_v = adam_v
         self.fused, self.nograd = [], []
         try:
             yield self
@@ -207,7 +209,7 @@ class _SgdEpilogue:
         if a is None:
             return None
         return F.sgd_epilogue_args(a.theta, a.grad, out2d, self.hyper, a.momentum, a.theta_bf16, self.nesterov,
-                                   self.anchor, self.corr)
+                                   self.anchor, self.corr, self.adam_v)
 
     def record(self, out2d, nograd_of=None):
         off = (out2d.data_ptr() - self.arena.grad.data_ptr()) // 4

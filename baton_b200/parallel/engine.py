@@ -26,7 +26,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from ..metrics import phase
-from ..train import GraphedLocalSGD, PortableLocalSGD, check_prox_mu
+from ..train import GraphedLocalSGD, PortableLocalSGD, check_adamw, check_optimizer, check_prox_mu
 from .arena import ParamArena
 from .dp import DPConfig, RDPAccountant, check_dp, clip_factor
 from .fedavg import FedAvgSession, NcclSession
@@ -66,7 +66,8 @@ class FederatedEngine:
                  logical_clients: int = 0, sample_k: Optional[int] = None, seed: int = 0, name: str = "exp",
                  nvls: "bool | str" = "auto", tile_flags: bool = False, prox_mu: float = 0.0,
                  dp_clip: float = 0.0, dp_noise_multiplier: float = 0.0, dp_seed: Optional[int] = None,
-                 scaffold: bool = False):
+                 scaffold: bool = False, optimizer: str = "sgd", betas: Tuple[float, float] = (0.9, 0.999),
+                 eps: float = 1e-8):
         """``prox_mu > 0``: FedProx local training -- every step adds ``prox_mu * (theta - global_w)`` to the gradient,
         ``global_w`` being the global model the round started from (for logical clients too: each starts from it).
 
@@ -78,8 +79,19 @@ class FederatedEngine:
         ``scaffold=True``: SCAFFOLD (``parallel/scaffold.py``) -- every local step adds the correction ``c - c_i`` to
         the gradient, and each round also updates the control variates (option II), the server's one through the
         round's collective.  The model update stays the sample-weighted FedAvg mean.  :meth:`control_variates` reads
-        them.  It cannot be combined with DP, FedProx, ``mode='weights'`` or ``tile_flags``."""
+        them.  It cannot be combined with DP, FedProx, ``mode='weights'`` or ``tile_flags``.
+
+        ``optimizer="adamw"``: every client's local steps are those of a fresh ``torch.optim.AdamW(lr, betas, eps,
+        weight_decay)`` (one parameter group, weight decay on every parameter), created anew for each client and
+        round; the server update stays the FedAvg mean.  It cannot be combined with ``momentum``, SCAFFOLD or FedProx.
+        The second moment costs one more fp32 buffer over the parameters."""
         prox_mu = check_prox_mu(prox_mu)
+        adam = check_optimizer(optimizer, momentum, prox_mu=prox_mu)
+        if adam:
+            if scaffold:
+                raise ValueError("AdamW with SCAFFOLD is not supported: option II's dc = (x - theta) / (K lr) - c "
+                                 "assumes SGD steps")
+            betas, eps = check_adamw(betas, eps)
         dp_clip, dp_noise_multiplier = check_dp(dp_clip, dp_noise_multiplier)
         if scaffold:
             if dp_clip > 0.0:
@@ -135,6 +147,8 @@ class FederatedEngine:
             self.session.gate_first_conv(model.conv1)
             self.trainer.k3_join = self.sync
         self.hp = dict(lr=lr, batch_size=batch_size, momentum=momentum, weight_decay=weight_decay, prox_mu=prox_mu)
+        if adam:
+            self.hp.update(optimizer=optimizer, betas=betas, eps=eps)
         self.n_rounds = 0
         self.logical_clients = logical_clients if logical_clients and logical_clients > self.world else 0
         self.sample_k = sample_k

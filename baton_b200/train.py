@@ -22,11 +22,17 @@ Every trainer takes ``prox_mu`` (FedProx, Li et al. 2020): the step adds
 the round started from.  ``prox_mu = 0`` is plain SGD.  The arena trainers also
 take ``corr`` (SCAFFOLD, Karimireddy et al. 2020): an fp32 buffer indexed like
 the parameters, holding ``c - c_i``, that every step adds to the gradient.
+
+Every trainer also takes ``optimizer="adamw"`` (with ``betas`` and ``eps``): the local
+steps are those of ``torch.optim.AdamW`` with one parameter group, created fresh for
+each run -- the reference builds its optimizer inside every ``train()`` call.  The
+step count ``t`` runs across the epochs of one run.  AdamW takes no momentum,
+Nesterov, FedProx or SCAFFOLD term.
 """
 from __future__ import annotations
 
 from collections import OrderedDict
-from typing import Callable, List, Optional
+from typing import Callable, List, Optional, Tuple
 
 import torch
 from torch import nn
@@ -52,6 +58,41 @@ def check_prox_mu(prox_mu: float) -> float:
     return mu
 
 
+OPTIMIZERS = ("sgd", "adamw")
+
+
+def check_adamw(betas, eps) -> Tuple[Tuple[float, float], float]:
+    """AdamW's ``(betas, eps)`` as floats; ``ValueError`` unless both betas are in [0, 1) and ``eps > 0`` (finite)."""
+    try:
+        b1, b2 = (float(b) for b in betas)
+    except (TypeError, ValueError):
+        raise ValueError("betas must be a pair of numbers, got {!r}".format(betas)) from None
+    for name, b in (("beta1", b1), ("beta2", b2)):
+        if not 0.0 <= b < 1.0:
+            raise ValueError("AdamW {} must be in [0, 1), got {!r}".format(name, b))
+    eps = float(eps)
+    if not 0.0 < eps < float("inf"):
+        raise ValueError("AdamW eps must be a finite number > 0, got {!r}".format(eps))
+    return (b1, b2), eps
+
+
+def check_optimizer(optimizer: str, momentum: float = 0.0, nesterov: bool = False, prox_mu: float = 0.0,
+                    corr=None) -> bool:
+    """True for ``"adamw"``, False for ``"sgd"``; ``ValueError`` for another name, or for AdamW together with
+    momentum, Nesterov, FedProx or SCAFFOLD (terms of the SGD step)."""
+    if optimizer not in OPTIMIZERS:
+        raise ValueError("optimizer must be one of {}, got {!r}".format(OPTIMIZERS, optimizer))
+    if optimizer != "adamw":
+        return False
+    if momentum or nesterov:
+        raise ValueError("momentum / nesterov are SGD options; AdamW keeps its own moments (betas)")
+    if prox_mu > 0:
+        raise ValueError("AdamW with FedProx (prox_mu > 0) is not supported")
+    if corr is not None:
+        raise ValueError("AdamW with SCAFFOLD is not supported: its control-variate update assumes SGD steps")
+    return True
+
+
 def _add_prox_term(params, anchors, prox_mu: float) -> None:
     """FedProx: ``grad += prox_mu * (w - anchor)`` before the optimizer step (what the reference implementation does)."""
     with torch.no_grad():
@@ -73,17 +114,24 @@ def run_local_sgd(model: nn.Module, X: torch.Tensor, y: torch.Tensor, *, n_epoch
                   lr: float = 0.001, batch_size: int = 32, momentum: float = 0.0,
                   weight_decay: float = 0.0, loss: "str | Callable" = "mse",
                   verbose: bool = False, reshuffle_each_epoch: bool = False,
-                  generator: Optional[torch.Generator] = None, prox_mu: float = 0.0) -> List[float]:
+                  generator: Optional[torch.Generator] = None, prox_mu: float = 0.0, optimizer: str = "sgd",
+                  betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8) -> List[float]:
     """Portable local SGD; returns the per-epoch mean loss.  ``prox_mu > 0``: FedProx, anchored on the parameters as
-    they are on entry -- the global model the worker has just loaded."""
+    they are on entry -- the global model the worker has just loaded.  ``optimizer="adamw"``: a fresh
+    ``torch.optim.AdamW(lr, betas, eps, weight_decay)`` instead of SGD."""
     criterion = _loss_fn(loss)
     prox_mu = check_prox_mu(prox_mu)
+    adam = check_optimizer(optimizer, momentum, prox_mu=prox_mu)
     n = X.shape[0]
     nn.Module.train(model, True)
     params = list(model.parameters())
     anchors = [p.detach().clone() for p in params] if prox_mu > 0 else None
-    optimizer = torch.optim.SGD(params, lr=lr, momentum=momentum,
-                                weight_decay=weight_decay)
+    if adam:
+        betas, eps = check_adamw(betas, eps)
+        optimizer = torch.optim.AdamW(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay)
+    else:
+        optimizer = torch.optim.SGD(params, lr=lr, momentum=momentum,
+                                    weight_decay=weight_decay)
     idxs = torch.randperm(n, generator=generator).to(X.device)
     loss_history: List[float] = []
     for epoch in range(n_epoch):
@@ -161,6 +209,13 @@ class GraphedLocalSGD:
     (it also writes the upload copy), ragged eager steps and autograd steps run
     ONE ``fused_sgd`` kernel over the whole arena instead.
 
+    ``run(optimizer="adamw")`` runs AdamW in the same three places.  Its first moment is
+    ``arena.momentum`` and its second ``arena.adam_v``.  The per-step bias corrections
+    come from a table of rows (``F.adamw_rows``), one row per local step of the run.  It
+    is built on the host when the run starts and copied to the device once.  Before each
+    epoch's replay, that epoch's rows are copied into the epoch graph's row buffer, and
+    captured step ``s`` reads row ``s``.  The ragged eager step uses the buffer's last row.
+
     ``model`` must already be adopted by a :class:`~baton_b200.parallel.arena.ParamArena`
     (``arena``); the engine is what ``FederatedModule.local_train`` dispatches to
     for CUDA shards (``model._graphed_trainer``).
@@ -189,6 +244,8 @@ class GraphedLocalSGD:
         self.hyper = torch.zeros(5, dtype=torch.float32, device=dev)   # [lr, momentum, wd, dampening, prox_mu]
         self.prox = False             # FedProx: every SGD kernel of the step reads the anchor arena.global_w
         self.corr = None              # SCAFFOLD: every SGD kernel of the step reads this correction c - c_i
+        self.adam = False             # AdamW: every optimizer kernel of the step reads its step row and arena.adam_v
+        self._adam_table = (None, None)   # (host key, device [n_epoch * steps, ADAMW_ROW] rows of the run)
         self.loss_acc = torch.zeros(2, dtype=torch.float32, device=dev)
         self._graphs = {}           # (n, batch, x_shape, y_shape) -> captured epoch
         self._hyper_host = None
@@ -213,10 +270,11 @@ class GraphedLocalSGD:
         yb = F.gather_rows(y, idx) if y.dtype == torch.int64 and y.dim() == 1 else y.index_select(0, idx)
         return xb, yb
 
-    def _step(self, X, y, idx, batch=None, emit_wire=False, fuse_sgd=True):
+    def _step(self, X, y, idx, batch=None, emit_wire=False, fuse_sgd=True, row=None):
         """One SGD step on ``X[idx], y[idx]`` (or on the already gathered ``batch``).  ``emit_wire``: last step of
         an epoch -- the optimizer kernel also writes the upload copy for the round-end collective (``self.pack``).
-        ``fuse_sgd=False``: no optimizer epilogue in the weight-gradient GEMMs (one optimizer pass over the arena)."""
+        ``fuse_sgd=False``: no optimizer epilogue in the weight-gradient GEMMs (one optimizer pass over the arena).
+        ``row``: with AdamW, the device row of this step's coefficients (``F.adamw_rows``)."""
         F = self.F
         xb, yb = batch if batch is not None else self._gather(X, y, idx)
         ws = getattr(self.model, "stats_workspace", None)
@@ -228,15 +286,19 @@ class GraphedLocalSGD:
         a = self.arena
         bf = a.theta_bf16
         anchor = a.global_w if self.prox else None
+        hyper = row if self.adam else self.hyper
+        adam_v = a.adam_v if self.adam else None
         if explicit is not None and self.loss_kind in ("ce", "cross_entropy"):
             # hand-scheduled forward + loss + backward (no autograd engine): two-piece block gradients, parallel shortcut
             # branch; the loss kernel accumulates straight into the epoch's running sums
             if fuse_sgd and not emit_wire:
                 # the split-K = 1 convolution weight gradients apply SGD in their GEMM epilogue; one launch covers the rest
-                with self.bnn.SGD_EPI.open(a, self.hyper, self.nesterov, prox=self.prox, corr=self.corr) as epi:
+                with self.bnn.SGD_EPI.open(a, hyper, self.nesterov, prox=self.prox, corr=self.corr,
+                                           adam_v=adam_v) as epi:
                     explicit(xb, yb, loss_acc=self.loss_acc, after_first_gemm=self._first_gemm_hook)
-                F.fused_sgd_segments(a.theta, a.grad, self.hyper, self._segment_table(epi.fused, epi.nograd),
-                                     a.momentum, bf, nesterov=self.nesterov, prox_anchor=anchor, corr=self.corr)
+                F.fused_sgd_segments(a.theta, a.grad, hyper, self._segment_table(epi.fused, epi.nograd),
+                                     a.momentum, bf, nesterov=self.nesterov, prox_anchor=anchor, corr=self.corr,
+                                     adam_v=adam_v)
                 self.emitted_wire = False
                 return
             explicit(xb, yb, loss_acc=self.loss_acc, after_first_gemm=self._first_gemm_hook)
@@ -248,10 +310,10 @@ class GraphedLocalSGD:
             self.bnn.WGRAD.join()      # weight-gradient GEMMs run on a side stream; they must land before the step
         # one optimizer pass over the whole arena; the epoch's last step also emits the upload copy
         pack = self.pack if emit_wire else None
-        F.fused_sgd(a.theta[: a.n_param], a.grad, self.hyper, a.momentum,
+        F.fused_sgd(a.theta[: a.n_param], a.grad, hyper, a.momentum,
                     bf[: a.n_param] if bf is not None else None, zero_grad=True, nesterov=self.nesterov, pack=pack,
                     prox_anchor=anchor[: a.n_param] if anchor is not None else None,
-                    corr=self.corr[: a.n_param] if self.corr is not None else None)
+                    corr=self.corr[: a.n_param] if self.corr is not None else None, adam_v=adam_v)
         self.emitted_wire = pack is not None
         if stats is not None:
             self.loss_acc.add_(stats)
@@ -272,8 +334,19 @@ class GraphedLocalSGD:
             self.hyper.copy_(torch.tensor(vals, dtype=torch.float32))
             self._hyper_host = vals
 
+    def _adam_rows(self, lr, betas, eps, weight_decay, n_epoch, steps):
+        """Device ``[n_epoch * steps, ADAMW_ROW]`` AdamW coefficients of every local step of a run (step ``t`` counts
+        across epochs); copied to the device only when they change."""
+        key = (float(lr), tuple(betas), float(eps), float(weight_decay), n_epoch, steps)
+        if self._adam_table[0] != key:
+            rows = self.F.adamw_rows(lr, betas, eps, weight_decay, 1, n_epoch * steps)
+            self._adam_table = (key, rows.to(self.device))
+        return self._adam_table[1]
+
     # -------------------------------------------------------------- epoch graph
-    def _capture(self, X, y, n_steps, batch_size):
+    def _capture(self, X, y, n_steps, batch_size, rows=None):
+        """``rows``: with AdamW, the device row buffer captured step ``s`` reads row ``s`` of (holding the first
+        epoch's rows, which the warm-up steps use too); kept in the returned entry."""
         perm = torch.zeros(n_steps * batch_size, dtype=torch.int64, device=self.device)
         perm.copy_(torch.arange(n_steps * batch_size, device=self.device) % X.shape[0])
         side = torch.cuda.Stream(device=self.device)
@@ -284,7 +357,7 @@ class GraphedLocalSGD:
             snap_i = self.arena.int_arena.clone()
             snap_m = self.arena.momentum.clone() if self.arena.momentum is not None else None
             for _ in range(2):
-                self._step(X, y, perm[:batch_size])
+                self._step(X, y, perm[:batch_size], row=rows[0] if rows is not None else None)
         torch.cuda.current_stream(self.device).wait_stream(side)
         torch.cuda.synchronize(self.device)
         from .ops._ext import total_launches
@@ -299,7 +372,8 @@ class GraphedLocalSGD:
             for s in range(n_steps):
                 self._step(X, y, None, batch=(Xp[s * batch_size:(s + 1) * batch_size],
                                               yp[s * batch_size:(s + 1) * batch_size]),
-                           emit_wire=(s == n_steps - 1 and self.pack is not None))
+                           emit_wire=(s == n_steps - 1 and self.pack is not None),
+                           row=rows[s] if rows is not None else None)
             self.graph_emits_wire = self.pack is not None
 
         if (self.k3_join is not None and hasattr(self.model, "explicit_step")
@@ -345,7 +419,7 @@ class GraphedLocalSGD:
         self.arena.grad.zero_()
         self.arena.sync_shadow()
         self.loss_acc.zero_()
-        return {"graph": graph, "graph2": graph2, "perm": perm, "X": X, "y": y}
+        return {"graph": graph, "graph2": graph2, "perm": perm, "X": X, "y": y, "rows": rows}
 
     # -------------------------------------------------------------- evaluation
     def _eval_pass(self, X, y, batch_size, explicit):
@@ -434,39 +508,52 @@ class GraphedLocalSGD:
 
     def run(self, X, y, n_epoch: int = 1, lr: float = 0.001, batch_size: int = 32, momentum: float = 0.0,
             weight_decay: float = 0.0, reshuffle_each_epoch: bool = False, return_device: bool = False,
-            prox_mu: float = 0.0, corr: Optional[torch.Tensor] = None, **_ignored):
+            prox_mu: float = 0.0, corr: Optional[torch.Tensor] = None, optimizer: str = "sgd",
+            betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8, **_ignored):
         """``prox_mu > 0``: FedProx toward ``arena.global_w``, the global model the round started from.  ``corr``:
         SCAFFOLD's correction ``c - c_i`` (fp32 device buffer of ``arena.n_param`` elements), added to every step's
-        gradient; it is read at replay, so the caller may rewrite it between runs."""
+        gradient; it is read at replay, so the caller may rewrite it between runs.  ``optimizer="adamw"``: the steps of
+        a fresh ``torch.optim.AdamW(lr, betas, eps, weight_decay)`` instead of SGD."""
         assert X.is_cuda, "GraphedLocalSGD needs a device-resident shard"
         prox_mu = check_prox_mu(prox_mu)
         if prox_mu > 0 and self.arena.global_w is None:
             raise ValueError("prox_mu > 0 needs the arena's global copy (ParamArena(keep_global=True))")
         _check_corr(corr, prox_mu, self.arena)
+        self.adam = check_optimizer(optimizer, momentum, self.nesterov, prox_mu, corr)
+        if self.adam:
+            betas, eps = check_adamw(betas, eps)
         nn.Module.train(self.model, True)
         n = X.shape[0]
         batch_size = min(batch_size, n)
         n_steps = n // batch_size
         tail = n - n_steps * batch_size
+        steps = n_steps + (1 if tail else 0)
         self._set_hyper(lr, momentum, weight_decay, prox_mu=prox_mu)
         self.prox = prox_mu > 0
         self.corr = corr
-        if momentum and self.arena.momentum is None:
+        if (momentum or self.adam) and self.arena.momentum is None:
             self.arena.momentum = torch.zeros_like(self.arena.grad)
+        if self.adam and self.arena.adam_v is None:
+            self.arena.adam_v = torch.zeros_like(self.arena.grad)
+        # every step of the run, t = 1 .. n_epoch * steps; the first ignores the stored moments (a fresh optimizer)
+        table = self._adam_rows(lr, betas, eps, weight_decay, n_epoch, steps) if self.adam else None
         # the anchor and correction pointers are baked into the captured launches; the coefficient is read from `hyper`
         # at replay
         key = (n, batch_size, tuple(X.shape[1:]), tuple(y.shape[1:]), X.data_ptr(), y.data_ptr(), bool(momentum),
-               self.prox, corr.data_ptr() if corr is not None else None)
+               self.prox, corr.data_ptr() if corr is not None else None, self.adam)
         epoch_losses = torch.zeros(n_epoch, 2, dtype=torch.float32, device=self.device)
         if self.use_graph:
             ent = self._graphs.get(key)
             if ent is None:
-                ent = self._graphs[key] = self._capture(X, y, n_steps, batch_size)
+                rows = table[:steps].clone() if self.adam else None
+                ent = self._graphs[key] = self._capture(X, y, n_steps, batch_size, rows)
             perm_full = torch.randperm(n, device=self.device)
             for e in range(n_epoch):
                 if reshuffle_each_epoch and e > 0:
                     perm_full = torch.randperm(n, device=self.device)
                 ent["perm"].copy_(perm_full[: n_steps * batch_size])
+                if self.adam:
+                    ent["rows"].copy_(table[e * steps:(e + 1) * steps])
                 self.loss_acc.zero_()
                 ent["graph"].replay()
                 if ent.get("graph2") is not None:
@@ -474,7 +561,8 @@ class GraphedLocalSGD:
                     ent["graph2"].replay()
                 if tail:
                     with torch.enable_grad():
-                        self._step(X, y, perm_full[n_steps * batch_size:], fuse_sgd=False)
+                        self._step(X, y, perm_full[n_steps * batch_size:], fuse_sgd=False,
+                                   row=ent["rows"][n_steps] if self.adam else None)
                 epoch_losses[e].copy_(self.loss_acc)
         else:
             perm_full = torch.randperm(n, device=self.device)
@@ -482,11 +570,10 @@ class GraphedLocalSGD:
                 if reshuffle_each_epoch and e > 0:
                     perm_full = torch.randperm(n, device=self.device)
                 self.loss_acc.zero_()
-                for idx in torch.split(perm_full, batch_size):
+                for s, idx in enumerate(torch.split(perm_full, batch_size)):
                     with torch.enable_grad():
-                        self._step(X, y, idx)
+                        self._step(X, y, idx, row=table[e * steps + s] if self.adam else None)
                 epoch_losses[e].copy_(self.loss_acc)
-        steps = n_steps + (1 if tail else 0)
         self.last_steps = steps
         self.last_had_tail_step = bool(tail)        # a ragged eager step ran after the graph: its SGD did not emit the wire
         if self.use_graph:
@@ -514,12 +601,15 @@ class PortableLocalSGD:
 
     def run(self, X, y, n_epoch: int = 1, lr: float = 0.001, batch_size: int = 32, momentum: float = 0.0,
             weight_decay: float = 0.0, reshuffle_each_epoch: bool = False, return_device: bool = False,
-            prox_mu: float = 0.0, corr: Optional[torch.Tensor] = None, **_ignored):
+            prox_mu: float = 0.0, corr: Optional[torch.Tensor] = None, optimizer: str = "sgd",
+            betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8, **_ignored):
         """``prox_mu > 0``: FedProx toward ``arena.global_w``, the global model the round started from.  ``corr``:
-        SCAFFOLD's correction ``c - c_i`` (fp32, indexed like the arena's parameters), added to every gradient."""
+        SCAFFOLD's correction ``c - c_i`` (fp32, indexed like the arena's parameters), added to every gradient.
+        ``optimizer="adamw"``: a fresh ``torch.optim.AdamW(lr, betas, eps, weight_decay)`` instead of SGD."""
         criterion = _loss_fn(self.loss_kind)
         prox_mu = check_prox_mu(prox_mu)
         _check_corr(corr, prox_mu, self.arena)
+        adam = check_optimizer(optimizer, momentum, prox_mu=prox_mu, corr=corr)
         n = X.shape[0]
         batch_size = min(batch_size, n)
         nn.Module.train(self.model, True)
@@ -531,7 +621,11 @@ class PortableLocalSGD:
             params.append(p)
             anchors.append(a._view(a.global_w, a.slots[name]) if prox_mu > 0 else None)
             corrs.append(a._view(corr, a.slots[name]) if corr is not None else None)
-        opt = torch.optim.SGD(params, lr=lr, momentum=momentum, weight_decay=weight_decay)
+        if adam:
+            betas, eps = check_adamw(betas, eps)
+            opt = torch.optim.AdamW(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay)
+        else:
+            opt = torch.optim.SGD(params, lr=lr, momentum=momentum, weight_decay=weight_decay)
         perm = torch.randperm(n)
         out = torch.zeros(n_epoch, 2, dtype=torch.float32)
         steps = 1
