@@ -36,6 +36,8 @@ class FederationConfig:
     dp_noise_multiplier: float = 0.0   # DP-FedAvg: noise std on the sum of clipped updates, in units of dp_clip
     dp_delta: float = 1e-5             # DP-FedAvg: delta of the (epsilon, delta) the manager reports
     dp_seed: Optional[int] = None      # DP-FedAvg noise key (None: secret random; an explicit key is for tests only)
+    aggregator: str = "mean"           # mean | median | trimmed_mean (coordinate-wise, unweighted over clients)
+    trim_ratio: float = 0.1            # trimmed_mean: fraction trimmed at each end, 0 <= beta < 0.5
     partition: str = "iid"             # iid | label_skew | dirichlet
     alpha: float = 0.1                 # Dirichlet concentration
     samples_per_client: int = 4096
@@ -57,6 +59,10 @@ class FederationConfig:
         check_dp(self.dp_clip, self.dp_noise_multiplier)
         if not (0.0 < float(self.dp_delta) < 1.0):
             raise ValueError("dp_delta must lie in (0, 1), got {!r}".format(self.dp_delta))
+        from .parallel.robust import check_aggregator
+        self.trim_ratio = check_aggregator(self.aggregator, self.trim_ratio)
+        if self.aggregator != "mean" and float(self.dp_clip) > 0.0:
+            raise ValueError("a robust aggregator with DP-FedAvg is not supported")
 
     def train_kwargs(self) -> dict:
         """Local-training keyword arguments of a worker (``FederatedModule.local_train``)."""
@@ -71,6 +77,13 @@ class FederationConfig:
             return None
         from .parallel.dp import DPConfig
         return DPConfig(self.dp_clip, self.dp_noise_multiplier, seed=self.dp_seed)
+
+    def robust_config(self):
+        """The :class:`~baton_b200.parallel.robust.RobustConfig` of these fields, or None for the mean."""
+        if self.aggregator == "mean":
+            return None
+        from .parallel.robust import RobustConfig
+        return RobustConfig(self.aggregator, self.trim_ratio)
 
     def to_json(self) -> str:
         return json.dumps(asdict(self), sort_keys=True)

@@ -81,18 +81,25 @@ class Experiment:
                  sample_fraction: Optional[float] = None, seed: Optional[int] = None,
                  round_timeout: Optional[float] = None, checkpoint_dir: Optional[str] = None,
                  checkpoint_every: int = 1, resume: bool = False, clock: Clock = SYSTEM_CLOCK,
-                 trusted_peers: bool = False, dp=None, dp_delta: float = 1e-5):
+                 trusted_peers: bool = False, dp=None, dp_delta: float = 1e-5, robust=None):
         """``dp`` (a :class:`~baton_b200.parallel.dp.DPConfig`): aggregate with DP-FedAvg -- on the manager for the
         ``http`` plane, on the seats for the seated planes (the plan carries the clip norm, noise and key) -- and
         account every aggregated round at ``q`` = participants / registered clients; ``/metrics`` reports the
-        ``(epsilon, dp_delta)`` spent."""
+        ``(epsilon, dp_delta)`` spent.
+
+        ``robust`` (a :class:`~baton_b200.parallel.robust.RobustConfig`): aggregate with the coordinate-wise median or
+        trimmed mean of the participants' updates -- on the manager for the ``http`` plane, on the seats for the seated
+        planes (the plan carries it); ``/metrics`` reports the aggregator."""
         self.name = name
         self.model = model
         self.app = app
         self.clock = clock
         self.client_manager = ClientManager(name, app, client_ttl, clock=clock, seed=seed)
         self.update_manager = UpdateManager(name)
-        self.plane: ManagerPlane = make_manager_plane(dataplane, dp=dp)
+        if robust is not None and dp is not None:
+            raise ValueError("robust aggregation with DP-FedAvg is not supported")
+        self.plane: ManagerPlane = make_manager_plane(dataplane, dp=dp, robust=robust)
+        self.robust = robust
         self.dp = dp
         self.dp_delta = float(dp_delta)
         self.dp_accountant = RDPAccountant(dp.noise_multiplier) if dp is not None else None
@@ -147,6 +154,7 @@ class Experiment:
         out = self.metrics.summary()
         if self.dp is not None:
             out["dp"] = self.dp_summary()
+        out["aggregator"] = self.robust.to_dict() if self.robust is not None else {"kind": "mean"}
         return web.json_response(json_clean(out))
 
     def dp_summary(self) -> dict:

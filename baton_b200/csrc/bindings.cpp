@@ -523,25 +523,22 @@ void pad_rows(const at::Tensor& s, at::Tensor d, int64_t rows, int64_t k, int64_
 }
 
 // ---- fused FedAvg collective -------------------------------------------------------------------
-void fedavg_allreduce(const std::vector<int64_t>& wire_ptrs, const std::vector<int64_t>& pad_ptrs, int64_t wire_mc,
-                      at::Tensor theta, const std::optional<at::Tensor>& global_w,
-                      const std::optional<at::Tensor>& theta_bf16, const std::optional<at::Tensor>& momentum,
-                      const std::optional<at::Tensor>& int_local, const std::vector<int64_t>& int_wire_ptrs,
-                      const std::optional<at::Tensor>& loss_local, const std::vector<int64_t>& loss_wire_ptrs,
-                      const std::optional<at::Tensor>& loss_out, const std::vector<double>& n_samples,
-                      bool counts_from_flags, int64_t alive_mask, int64_t rank, int64_t world, int64_t wire_kind,
-                      bool delta, bool use_nvls, int64_t epoch, const std::optional<at::Tensor>& tile_flags,
-                      int64_t flag_value, int64_t tile_elems, int64_t n_ctas, int64_t timeout_log2,
-                      const std::optional<at::Tensor>& status, const std::optional<at::Tensor>& phase_ns, bool prepacked,
-                      const std::vector<int64_t>& clip_page_ptrs, double dp_noise_std, int64_t dp_seed, int64_t dp_round,
-                      const std::optional<at::Tensor>& scaf_dc, const std::optional<at::Tensor>& scaf_c,
-                      int64_t scaf_seg1_off, double scaf_inv_clients) {
+// the arguments every variant of the collective shares
+static void fill_fedavg_args(FedAvgArgs& a, const std::vector<int64_t>& wire_ptrs, const std::vector<int64_t>& pad_ptrs,
+                             int64_t wire_mc, at::Tensor& theta, const std::optional<at::Tensor>& global_w,
+                             const std::optional<at::Tensor>& theta_bf16, const std::optional<at::Tensor>& momentum,
+                             const std::optional<at::Tensor>& int_local, const std::vector<int64_t>& int_wire_ptrs,
+                             const std::optional<at::Tensor>& loss_local, const std::vector<int64_t>& loss_wire_ptrs,
+                             const std::optional<at::Tensor>& loss_out, const std::vector<double>& n_samples,
+                             bool counts_from_flags, int64_t alive_mask, int64_t rank, int64_t world, int64_t wire_kind,
+                             bool delta, bool use_nvls, int64_t epoch, const std::optional<at::Tensor>& tile_flags,
+                             int64_t flag_value, int64_t tile_elems, int64_t timeout_log2,
+                             const std::optional<at::Tensor>& status, const std::optional<at::Tensor>& phase_ns,
+                             bool prepacked) {
   CHECK_CUDA(theta);
   TORCH_CHECK(world <= B200_MAX_RANKS && static_cast<int64_t>(wire_ptrs.size()) == world &&
               static_cast<int64_t>(pad_ptrs.size()) == world && static_cast<int64_t>(n_samples.size()) == world);
   TORCH_CHECK(theta.scalar_type() == at::kFloat && theta.is_contiguous());
-  const c10::cuda::CUDAGuard guard(theta.device());
-  FedAvgDPArgs a = {};
   for (int64_t k = 0; k < world; ++k) {
     a.wire[k] = reinterpret_cast<void*>(wire_ptrs[k]);
     a.pads[k] = reinterpret_cast<unsigned long long*>(pad_ptrs[k]);
@@ -581,6 +578,26 @@ void fedavg_allreduce(const std::vector<int64_t>& wire_ptrs, const std::vector<i
     TORCH_CHECK(phase_ns->scalar_type() == at::kLong && phase_ns->numel() >= 16, "phase_ns: int64[16]");
     a.phase_ns = reinterpret_cast<unsigned long long*>(phase_ns->data_ptr<int64_t>());
   }
+}
+
+void fedavg_allreduce(const std::vector<int64_t>& wire_ptrs, const std::vector<int64_t>& pad_ptrs, int64_t wire_mc,
+                      at::Tensor theta, const std::optional<at::Tensor>& global_w,
+                      const std::optional<at::Tensor>& theta_bf16, const std::optional<at::Tensor>& momentum,
+                      const std::optional<at::Tensor>& int_local, const std::vector<int64_t>& int_wire_ptrs,
+                      const std::optional<at::Tensor>& loss_local, const std::vector<int64_t>& loss_wire_ptrs,
+                      const std::optional<at::Tensor>& loss_out, const std::vector<double>& n_samples,
+                      bool counts_from_flags, int64_t alive_mask, int64_t rank, int64_t world, int64_t wire_kind,
+                      bool delta, bool use_nvls, int64_t epoch, const std::optional<at::Tensor>& tile_flags,
+                      int64_t flag_value, int64_t tile_elems, int64_t n_ctas, int64_t timeout_log2,
+                      const std::optional<at::Tensor>& status, const std::optional<at::Tensor>& phase_ns, bool prepacked,
+                      const std::vector<int64_t>& clip_page_ptrs, double dp_noise_std, int64_t dp_seed, int64_t dp_round,
+                      const std::optional<at::Tensor>& scaf_dc, const std::optional<at::Tensor>& scaf_c,
+                      int64_t scaf_seg1_off, double scaf_inv_clients) {
+  FedAvgDPArgs a = {};
+  fill_fedavg_args(a, wire_ptrs, pad_ptrs, wire_mc, theta, global_w, theta_bf16, momentum, int_local, int_wire_ptrs,
+                   loss_local, loss_wire_ptrs, loss_out, n_samples, counts_from_flags, alive_mask, rank, world, wire_kind,
+                   delta, use_nvls, epoch, tile_flags, flag_value, tile_elems, timeout_log2, status, phase_ns, prepacked);
+  const c10::cuda::CUDAGuard guard(theta.device());
   // DP-FedAvg: one clip page per rank (empty = off); the seed is the 64-bit Philox key, passed as its int64 bit pattern
   const bool dp = !clip_page_ptrs.empty();
   if (dp) {
@@ -612,6 +629,50 @@ void fedavg_allreduce(const std::vector<int64_t>& wire_ptrs, const std::vector<i
   check(dp ? b200_fedavg_allreduce_dp(&a, static_cast<int>(n_ctas), cur_stream())
            : b200_fedavg_allreduce(&a, static_cast<int>(n_ctas), cur_stream()),
         "fedavg_allreduce");
+}
+
+// robust round: seg_page_ptrs = every rank's count page, trim_b = floor(beta * P) for P = 0 .. 32 (trimmed mean)
+void fedavg_allreduce_robust(const std::vector<int64_t>& wire_ptrs, const std::vector<int64_t>& pad_ptrs,
+                             at::Tensor theta, const at::Tensor& global_w, const std::optional<at::Tensor>& theta_bf16,
+                             const std::optional<at::Tensor>& momentum, const std::optional<at::Tensor>& int_local,
+                             const std::vector<int64_t>& int_wire_ptrs, const std::optional<at::Tensor>& loss_local,
+                             const std::vector<int64_t>& loss_wire_ptrs, const std::optional<at::Tensor>& loss_out,
+                             const std::vector<double>& n_samples, bool counts_from_flags, int64_t alive_mask, int64_t rank,
+                             int64_t world, int64_t wire_kind, int64_t epoch, int64_t tile_elems, int64_t n_ctas,
+                             int64_t timeout_log2, const std::optional<at::Tensor>& status,
+                             const std::optional<at::Tensor>& phase_ns, bool prepacked,
+                             const std::vector<int64_t>& seg_page_ptrs, int64_t my_segs, int64_t seg_stride, int64_t kind,
+                             const std::vector<int64_t>& trim_b) {
+  FedAvgRobustArgs a = {};
+  fill_fedavg_args(a, wire_ptrs, pad_ptrs, 0, theta, global_w, theta_bf16, momentum, int_local, int_wire_ptrs, loss_local,
+                   loss_wire_ptrs, loss_out, n_samples, counts_from_flags, alive_mask, rank, world, wire_kind, true, false,
+                   epoch, std::nullopt, 0, tile_elems, timeout_log2, status, phase_ns, prepacked);
+  TORCH_CHECK(static_cast<int64_t>(seg_page_ptrs.size()) == world, "robust: one count page per rank");
+  TORCH_CHECK(static_cast<int64_t>(trim_b.size()) == B200_MAX_ROBUST_CLIENTS + 1, "robust: trim_b for P = 0 .. 32");
+  TORCH_CHECK(my_segs >= 0 && my_segs <= B200_MAX_ROBUST_CLIENTS, "robust: at most 32 segments per rank");
+  for (int64_t k = 0; k < world; ++k) a.seg_page[k] = reinterpret_cast<uint32_t*>(seg_page_ptrs[k]);
+  for (int p = 0; p <= B200_MAX_ROBUST_CLIENTS; ++p) {
+    TORCH_CHECK(trim_b[p] >= 0 && 2 * trim_b[p] < (p > 0 ? p : 1), "robust: need P - 2b >= 1");
+    a.trim_b[p] = static_cast<uint8_t>(trim_b[p]);
+  }
+  a.my_segs = static_cast<uint32_t>(my_segs);
+  a.seg_stride = seg_stride;
+  a.kind = static_cast<int>(kind);
+  const c10::cuda::CUDAGuard guard(theta.device());
+  check(b200_fedavg_allreduce_robust(&a, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_robust");
+}
+
+// one logical client's wire segment at address seg (see b200_pack_client)
+void pack_client(int64_t seg, at::Tensor theta, const at::Tensor& global_w, const std::optional<at::Tensor>& wb,
+                 const std::optional<at::Tensor>& mom, int64_t wire_kind, bool reset) {
+  CHECK_CUDA(theta);
+  TORCH_CHECK(theta.scalar_type() == at::kFloat && global_w.scalar_type() == at::kFloat && theta.is_contiguous() &&
+              global_w.is_contiguous() && global_w.numel() == theta.numel(), "pack_client: fp32 theta / global_w");
+  const c10::cuda::CUDAGuard guard(theta.device());
+  check(b200_pack_client(reinterpret_cast<void*>(seg), theta.data_ptr<float>(), global_w.data_ptr<float>(),
+                         opt_ptr<void>(wb), opt_ptr<float>(mom), mom.has_value() && mom->defined() ? mom->numel() : 0,
+                         theta.numel(), static_cast<int>(wire_kind), reset ? 1 : 0, cur_stream()),
+        "pack_client");
 }
 
 // DP clip factor of theta against global_w over theta's n elements; work: int64 [DP_WORK_WORDS], zeroed once
@@ -932,6 +993,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("pad_rows", &pad_rows);
   m.def("embedding_bwd", &embedding_bwd);
   m.def("fedavg_allreduce", &fedavg_allreduce);
+  m.def("fedavg_allreduce_robust", &fedavg_allreduce_robust);
+  m.def("pack_client", &pack_client);
+  m.attr("MAX_ROBUST_CLIENTS") = B200_MAX_ROBUST_CLIENTS;
   m.def("flag_barrier", &flag_barrier);
   m.attr("DP_WORK_WORDS") = B200_DP_WORK_WORDS;
   m.def("dp_clip_factor", &dp_clip_factor);

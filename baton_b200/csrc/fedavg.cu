@@ -328,14 +328,232 @@ __device__ __forceinline__ void seg_apply_add(const uint8_t* wire, float* __rest
   }
 }
 
+// ---------------------------------------------------------------- robust rounds: coordinate-wise median / trimmed mean
+// Phase 1 of a robust round replaces the weighted sum with a selection across the P participating client segments.  The
+// owner of a tile walks it in chunks of CH = ROBUST_STAGE / NP elements (NP = P rounded up to 8, 16 or 32):
+//   load    all threads pull the chunk of every segment with 16-byte (fp8: 8-byte) loads, 32 / VEC per thread issued
+//           before the first use, decode to fp32 and store order-preserving uint32 keys into shared memory [NP][CH];
+//   select  thread c takes column c into registers (padding rows: key 0xFFFFFFFF, above every value), sorts it with a
+//           bitonic network (NP = 32: two runs of 16 and a bitonic merge through shared memory), writes it back and
+//           puts the selected value into row 0 of its own column;
+//   store   the threads cast row 0 to the wire format (fp8: the quad's block exponent) and store it into seg 0 of every
+//           live replica, where the plain apply phase finds it.
+// The result of an element depends only on the multiset of its P values, never on the tile size, the CTA count, the
+// owner or the order of the segments.  IEEE-rounded intrinsics keep --use_fast_math from reassociating or approximating.
+constexpr int ROBUST_STAGE = 16384;   // uint32 keys staged per chunk (64 KB of dynamic shared memory)
+constexpr int ROBUST_SMEM = ROBUST_STAGE * 4 + B200_MAX_ROBUST_CLIENTS * 8 + 16;
+
+// total order on floats as uint32 keys: -inf < ... < -0 < +0 < ... < +inf < NaN (every NaN canonicalised to 0x7FC00000)
+__device__ __forceinline__ uint32_t robust_key(float x) {
+  uint32_t u = __float_as_uint(x);
+  if ((u & 0x7FFFFFFFu) > 0x7F800000u) u = 0x7FC00000u;
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float robust_unkey(uint32_t k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k);
+}
+
+template <int NP>
+__device__ __forceinline__ void bitonic_sort(uint32_t (&k)[NP]) {
+#pragma unroll
+  for (int size = 2; size <= NP; size <<= 1)
+#pragma unroll
+    for (int stride = size >> 1; stride > 0; stride >>= 1)
+#pragma unroll
+      for (int i = 0; i < NP; ++i) {
+        const int j = i ^ stride;
+        if (j > i) {
+          const uint32_t lo = min(k[i], k[j]), hi = max(k[i], k[j]);
+          const bool up = (i & size) == 0;
+          k[i] = up ? lo : hi;
+          k[j] = up ? hi : lo;
+        }
+      }
+}
+
+// ascending bitonic merge: sorts a bitonic sequence of N keys
+template <int N>
+__device__ __forceinline__ void bitonic_merge(uint32_t (&k)[N]) {
+#pragma unroll
+  for (int stride = N >> 1; stride > 0; stride >>= 1)
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+      const int j = i ^ stride;
+      if (j > i) {
+        const uint32_t lo = min(k[i], k[j]), hi = max(k[i], k[j]);
+        k[i] = lo;
+        k[j] = hi;
+      }
+    }
+}
+
+// median: x[P/2] for odd P, 0.5 * (x[(P-1)/2] + x[P/2]) for even P; trimmed mean: (x[b] + ... + x[P-b-1]) / (P - 2b),
+// added in ascending order from 0; P == 0: 0 (the round changes nothing).  x = the sorted column col of the stage.
+__device__ __forceinline__ float robust_select(const uint32_t* col, int stride, int P, int kind, int b) {
+  if (P == 0) return 0.f;
+  if (kind == 0) {
+    const int i0 = (P - 1) >> 1, i1 = P >> 1;
+    const float x1 = robust_unkey(col[i1 * stride]);
+    return i0 == i1 ? x1 : __fmul_rn(0.5f, __fadd_rn(robust_unkey(col[i0 * stride]), x1));
+  }
+  float acc = 0.f;
+  for (int j = b; j < P - b; ++j) acc = __fadd_rn(acc, robust_unkey(col[j * stride]));
+  return __fdiv_rn(acc, static_cast<float>(P - 2 * b));
+}
+
+template <int WIRE, int NP>
+__device__ __forceinline__ void robust_tiles(const FedAvgRobustArgs& a, uint8_t* const* s_wire, const uint8_t* const* src,
+                                             uint32_t* stage, int P, int A, int my_pos) {
+  using W = Wire<WIRE>;
+  constexpr int VEC = W::VEC;
+  constexpr size_t esz = W::VBYTES / VEC;
+  constexpr int CH = ROBUST_STAGE / NP;          // elements per chunk
+  constexpr int VPR = CH / VEC;                  // wire vectors per segment row of a chunk
+  constexpr int R = NP * VPR / FEDAVG_THREADS;   // loads per thread per chunk
+  constexpr int RG = 4;                          // ... in groups of RG in flight
+  static_assert(R * FEDAVG_THREADS == NP * VPR && R % RG == 0, "the stage must split evenly over the threads");
+  const int G = gridDim.x;
+  const long long n = a.n;
+  const int T = a.tile_elems;
+  const long long n_tiles = (n + T - 1) / T;
+  const int b = a.trim_b[P];
+  const int lane_elems = static_cast<int>(threadIdx.x & 31) * VEC;
+  for (long long t = my_pos + static_cast<long long>(blockIdx.x) * A; t < n_tiles; t += static_cast<long long>(G) * A) {
+    const long long base = t * T;
+    const int len = static_cast<int>((n - base) < T ? (n - base) : T);
+    for (int c0 = 0; c0 < len; c0 += CH) {
+      const int clen = len - c0 < CH ? len - c0 : CH;
+      const long long e0 = base + c0;
+      // ---- load: RG loads per thread issued before the first decode
+#pragma unroll 1
+      for (int r0 = 0; r0 < R; r0 += RG) {
+        uint4 v[RG];
+        uint32_t sc[RG];
+#pragma unroll
+        for (int r = 0; r < RG; ++r) {
+          const int w = threadIdx.x + (r0 + r) * FEDAVG_THREADS, p = w / VPR, q = (w % VPR) * VEC;
+          if (p < P && q < clen) {
+            v[r] = W::ld(src[p] + (e0 + q) * esz);
+            if constexpr (W::SCALED) sc[r] = ld_volatile_u8(src[p] + n + ((e0 + q) >> 5));
+          }
+        }
+#pragma unroll
+        for (int r = 0; r < RG; ++r) {
+          const int w = threadIdx.x + (r0 + r) * FEDAVG_THREADS, p = w / VPR, q = (w % VPR) * VEC;
+          if (p < P && q < clen) {
+            float f[VEC];
+            float scale = 1.f;
+            if constexpr (W::SCALED) scale = exp2_int(static_cast<int>(sc[r]) - 127);
+            W::unpack(v[r], f, scale);
+#pragma unroll
+            for (int j = 0; j < VEC; j += 4)
+              *reinterpret_cast<uint4*>(stage + p * CH + q + j) =
+                  make_uint4(robust_key(f[j]), robust_key(f[j + 1]), robust_key(f[j + 2]), robust_key(f[j + 3]));
+          }
+        }
+      }
+      __syncthreads();
+      // ---- select: one column per thread
+#pragma unroll 1
+      for (int c = threadIdx.x; c < clen; c += FEDAVG_THREADS) {
+        // sorted back into the column (only this thread reads it), then selected from there.  32 rows do not fit in
+        // registers as one network: they are sorted as two runs of 16, a half-cleaner (row i against row 31 - i) puts
+        // the 16 smallest keys into rows 0..15 and the 16 largest into rows 16..31, each half bitonic, and a 16-wide
+        // bitonic merge sorts each half
+        constexpr int NR = NP < 16 ? NP : 16;
+        uint32_t* col = stage + c;
+#pragma unroll
+        for (int h = 0; h < NP; h += NR) {
+          uint32_t k[NR];
+#pragma unroll
+          for (int j = 0; j < NR; ++j) k[j] = h + j < P ? col[(h + j) * CH] : 0xFFFFFFFFu;
+          bitonic_sort<NR>(k);
+#pragma unroll
+          for (int j = 0; j < NR; ++j)
+            if (NP > 16 || j < P) col[(h + j) * CH] = k[j];
+        }
+        if constexpr (NP > 16) {
+#pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            const uint32_t x = col[i * CH], y = col[(31 - i) * CH];
+            col[i * CH] = min(x, y);
+            col[(31 - i) * CH] = max(x, y);
+          }
+#pragma unroll
+          for (int h = 0; h < 32; h += 16) {
+            uint32_t k[16];
+#pragma unroll
+            for (int j = 0; j < 16; ++j) k[j] = col[(h + j) * CH];
+            bitonic_merge<16>(k);
+#pragma unroll
+            for (int j = 0; j < 16; ++j) col[(h + j) * CH] = k[j];
+          }
+        }
+        stage[c] = __float_as_uint(robust_select(col, CH, P, a.kind, b));
+      }
+      __syncthreads();
+      // ---- cast + store into seg 0 of every live replica (warp-uniform bound: the fp8 quads shuffle)
+      for (int i = threadIdx.x * VEC; i - lane_elems < clen; i += FEDAVG_THREADS * VEC) {
+        const bool valid = i < clen;
+        float f[VEC];
+#pragma unroll
+        for (int j = 0; j < VEC; ++j) f[j] = valid ? __uint_as_float(stage[i + j]) : 0.f;
+        float inv = 1.f;
+        int e = 0;
+        if constexpr (W::SCALED) {
+          e = quad_block_exponent<VEC>(f);
+          inv = exp2_int(-e);
+        }
+        if (valid) {
+          const size_t off = (e0 + i) * esz;
+          const uint4 out = W::pack(f, inv);
+#pragma unroll 1
+          for (int k = 0; k < A; ++k) {
+            W::st_na(s_wire[k] + off, out);
+            if constexpr (W::SCALED)
+              if ((threadIdx.x & 3) == 0) st_volatile_u8(s_wire[k] + n + ((e0 + i) >> 5), static_cast<uint32_t>(e + 127));
+          }
+        }
+      }
+      __syncthreads();   // the next chunk reuses the stage
+    }
+  }
+}
+
+// phase 1 of a robust round: gather the P client segments of the live ranks (counts from their pages), then select
+template <int WIRE>
+__device__ __forceinline__ void robust_reduce(const FedAvgRobustArgs& a, uint8_t* const* s_wire, const int* s_rank, int A,
+                                              int my_pos) {
+  extern __shared__ __align__(16) uint8_t robust_smem[];
+  uint32_t* stage = reinterpret_cast<uint32_t*>(robust_smem);
+  const uint8_t** src = reinterpret_cast<const uint8_t**>(robust_smem + ROBUST_STAGE * 4);
+  int* s_P = reinterpret_cast<int*>(robust_smem + ROBUST_STAGE * 4 + B200_MAX_ROBUST_CLIENTS * 8);
+  if (threadIdx.x == 0) {
+    int P = 0;
+    for (int k = 0; k < A; ++k) {
+      const uint32_t m = *reinterpret_cast<const volatile uint32_t*>(a.seg_page[s_rank[k]]);
+      for (uint32_t j = 0; j < m && P < B200_MAX_ROBUST_CLIENTS; ++j)   // the host keeps P <= 32
+        src[P++] = s_wire[k] + static_cast<size_t>(j) * static_cast<size_t>(a.seg_stride);
+    }
+    *s_P = P;
+  }
+  __syncthreads();
+  const int P = *s_P;
+  if (P <= 8) robust_tiles<WIRE, 8>(a, s_wire, src, stage, P, A, my_pos);
+  else if (P <= 16) robust_tiles<WIRE, 16>(a, s_wire, src, stage, P, A, my_pos);
+  else robust_tiles<WIRE, 32>(a, s_wire, src, stage, P, A, my_pos);
+}
+
 // DP: DP-FedAvg (see launch.h / DESIGN.md): w_k = n_k s_k / N with s_k from rank k's clip page, and the owner of a tile
 // adds sigma C / N * z[i] to its fp32 sum before the cast.  The loss and the integer side arena keep the weights n_k / N.
 // SCAF: a SCAFFOLD round -- segment 1 (the control variates, see seg_pack) rides between the same barriers; every
 // participant weighs 1 / N there.
-// The whole round; Args is FedAvgDPArgs when DP, FedAvgScaffoldArgs when SCAF.
-template <int WIRE, bool DP, bool SCAF = false, typename Args>
+// ROBUST: a robust round (robust_reduce above); every rank publishes its segment count before barrier 1.
+// The whole round; Args is FedAvgDPArgs when DP, FedAvgScaffoldArgs when SCAF, FedAvgRobustArgs when ROBUST.
+template <int WIRE, bool DP, bool SCAF = false, bool ROBUST = false, typename Args>
 __device__ __forceinline__ void fedavg_round(const Args& a) {
   static_assert(!(DP && SCAF), "DP-FedAvg and SCAFFOLD are exclusive");
+  static_assert(!(ROBUST && (DP || SCAF)), "robust rounds exclude DP-FedAvg and SCAFFOLD");
   using W = Wire<WIRE>;
   constexpr int VEC = W::VEC;
   constexpr bool SCALED = W::SCALED;
@@ -440,6 +658,10 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
     // integer side arena (num_batches_tracked ...) and the local per-epoch losses
     for (int i = threadIdx.x; i < a.n_int; i += FEDAVG_THREADS) a.int_wire[a.rank][i] = a.int_local[i];
     for (int i = threadIdx.x; i < a.n_loss; i += FEDAVG_THREADS) a.loss_wire[a.rank][i] = a.loss_local[i];
+  }
+  if constexpr (ROBUST) {
+    // every CTA publishes the count (same value): CTA b's barrier then covers it for CTA b of every peer
+    if (threadIdx.x == 0) *reinterpret_cast<volatile uint32_t*>(a.seg_page[a.rank]) = a.my_segs;
   }
   phase_stamp(a, 1);                                   // pack done
   if (!cta_barrier_all_ranks(a, a.epoch + 1, __float_as_uint(my_n), s_payload)) return;
@@ -578,7 +800,9 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
       }
     }
   };
-  if constexpr (SCAF) {
+  if constexpr (ROBUST) {
+    robust_reduce<WIRE>(a, s_wire, s_rank, A, my_pos);
+  } else if constexpr (SCAF) {
     // one wire vector per trip: the same sums in the same rank order as the wider trips, in fewer registers
     reduce_tiles(std::integral_constant<int, 1>{});
   } else {
@@ -709,6 +933,62 @@ template <int WIRE>
 __global__ void __maxnreg__(96) fedavg_allreduce_scaffold_kernel(const __grid_constant__ FedAvgScaffoldArgs a) {
   fedavg_round<WIRE, false, true>(a);
 }
+// robust round: ROBUST_SMEM bytes of dynamic shared memory (the selection stage), the same 96-register cap
+template <int WIRE>
+__global__ void __maxnreg__(96) fedavg_allreduce_robust_kernel(const __grid_constant__ FedAvgRobustArgs a) {
+  fedavg_round<WIRE, false, false, true>(a);
+}
+
+// one logical client's upload into its wire segment: the phase-0 pack of fedavg_round (delta mode, scale 1) over the
+// whole arena, plus fold_client_kernel's replica reset.  Loop bounds are warp-uniform so the fp8 quads can shuffle.
+template <int WIRE>
+__global__ void __launch_bounds__(256)
+pack_client_kernel(uint8_t* __restrict__ seg, float* __restrict__ theta, const float* __restrict__ global_w,
+                   __nv_bfloat16* __restrict__ wb, float* __restrict__ mom, long long n_mom, long long n, int reset) {
+  using W = Wire<WIRE>;
+  constexpr int VEC = W::VEC;
+  constexpr size_t esz = W::VBYTES / VEC;
+  const long long nvec = n / VEC;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  const int lane = threadIdx.x & 31;
+  for (long long v0 = static_cast<long long>(blockIdx.x) * blockDim.x + (threadIdx.x & ~31); v0 < nvec; v0 += stride) {
+    const long long v = v0 + lane;
+    const bool valid = v < nvec;
+    float f[VEC];
+    float4 g[VEC / 4];
+#pragma unroll
+    for (int j = 0; j < VEC; ++j) f[j] = 0.f;
+    if (valid) {
+#pragma unroll
+      for (int j = 0; j < VEC; j += 4) {
+        const float4 t = *reinterpret_cast<const float4*>(theta + v * VEC + j);
+        g[j >> 2] = *reinterpret_cast<const float4*>(global_w + v * VEC + j);
+        f[j] = t.x - g[j >> 2].x; f[j + 1] = t.y - g[j >> 2].y;
+        f[j + 2] = t.z - g[j >> 2].z; f[j + 3] = t.w - g[j >> 2].w;
+      }
+    }
+    float inv = 1.f;
+    if constexpr (W::SCALED) {
+      const int e = quad_block_exponent<VEC>(f);
+      inv = exp2_int(-e);
+      if (valid && (lane & 3) == 0) seg[n + ((v * VEC) >> 5)] = static_cast<uint8_t>(e + 127);
+    }
+    if (valid) {
+      W::st(seg + v * VEC * esz, W::pack(f, inv));
+      if (reset) {
+#pragma unroll
+        for (int j = 0; j < VEC; j += 4) {
+          const long long i = v * VEC + j;
+          *reinterpret_cast<float4*>(theta + i) = g[j >> 2];
+          if (wb != nullptr)
+            *reinterpret_cast<uint2*>(wb + i) = make_uint2(pack_bf16x2(g[j >> 2].x, g[j >> 2].y),
+                                                           pack_bf16x2(g[j >> 2].z, g[j >> 2].w));
+          if (mom != nullptr && i < n_mom) *reinterpret_cast<float4*>(mom + i) = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+      }
+    }
+  }
+}
 
 // stand-alone cross-GPU barrier on the pads (one CTA): fences host-side phases
 __global__ void flag_barrier_kernel(FedAvgArgs a, int slot) {
@@ -808,29 +1088,35 @@ fold_client_scaled_kernel(float* __restrict__ acc, float* __restrict__ theta, co
 // (cudaErrorCooperativeLaunchTooLarge) and schedules all CTAs together, also next to work on other streams -- instead
 // of the plain <<<>>> of round 1, which was only safe on an otherwise idle GPU.  The grid is clamped to what
 // cudaOccupancyMaxActiveBlocksPerMultiprocessor allows on this device.
-template <int WIRE, bool DP, bool SCAF, typename Args>
+template <int WIRE, bool DP, bool SCAF, typename Args, bool ROBUST = false>
 static int launch_fedavg(const Args* args, int n_ctas, cudaStream_t stream) {
   using namespace b200;
   static int max_ctas = -1;
-  const void* kernel = SCAF ? reinterpret_cast<const void*>(fedavg_allreduce_scaffold_kernel<WIRE>)
+  const void* kernel = ROBUST ? reinterpret_cast<const void*>(fedavg_allreduce_robust_kernel<WIRE>)
+                       : SCAF ? reinterpret_cast<const void*>(fedavg_allreduce_scaffold_kernel<WIRE>)
                        : DP ? reinterpret_cast<const void*>(fedavg_allreduce_dp_kernel<WIRE>)
                             : reinterpret_cast<const void*>(fedavg_allreduce_kernel<WIRE>);
+  const int smem = ROBUST ? ROBUST_SMEM : 0;
   if (max_ctas < 0) {
     int dev = 0, sms = 0, per_sm = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, FEDAVG_THREADS, 0);
+    if (ROBUST) {
+      cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+      if (e != cudaSuccess) return static_cast<int>(e);
+    }
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, FEDAVG_THREADS, smem);
     max_ctas = sms * per_sm;
     if (max_ctas < 1) max_ctas = 1;
   }
   if (n_ctas > max_ctas) n_ctas = max_ctas;
   void* kargs[] = {const_cast<Args*>(args)};
-  cudaError_t e = cudaLaunchCooperativeKernel(kernel, dim3(n_ctas), dim3(FEDAVG_THREADS), kargs, 0, stream);
+  cudaError_t e = cudaLaunchCooperativeKernel(kernel, dim3(n_ctas), dim3(FEDAVG_THREADS), kargs, smem, stream);
   if (e != cudaSuccess) return static_cast<int>(e);
   return static_cast<int>(cudaGetLastError());
 }
 
-template <bool DP, bool SCAF, typename Args>
+template <bool DP, bool SCAF, typename Args, bool ROBUST = false>
 static int fedavg_dispatch(const Args* args, int n_ctas, cudaStream_t stream) {
   using namespace b200;
   if (args->world > B200_MAX_RANKS || args->n % 8 != 0 || args->tile_elems % 8 != 0) return -2;
@@ -839,10 +1125,42 @@ static int fedavg_dispatch(const Args* args, int n_ctas, cudaStream_t stream) {
   if (args->wire_kind == 2) {
     // block-scaled fp8 wire: 32-element blocks must not straddle tiles, and the switch cannot rescale
     if (args->tile_elems % 32 != 0 || args->use_nvls) return -2;
-    return launch_fedavg<2, DP, SCAF>(args, n_ctas, stream);
+    return launch_fedavg<2, DP, SCAF, Args, ROBUST>(args, n_ctas, stream);
   }
-  if (args->wire_kind == 1) return launch_fedavg<1, DP, SCAF>(args, n_ctas, stream);
-  return launch_fedavg<0, DP, SCAF>(args, n_ctas, stream);
+  if (args->wire_kind == 1) return launch_fedavg<1, DP, SCAF, Args, ROBUST>(args, n_ctas, stream);
+  return launch_fedavg<0, DP, SCAF, Args, ROBUST>(args, n_ctas, stream);
+}
+
+extern "C" int b200_fedavg_allreduce_robust(const FedAvgRobustArgs* args, int n_ctas, cudaStream_t stream) {
+  // a selection is not a sum: robust rounds run on peer loads, never on the switch
+  if (args->use_nvls || !args->delta || args->my_segs > B200_MAX_ROBUST_CLIENTS || args->seg_stride % 256 != 0 ||
+      (args->kind != 0 && args->kind != 1) || args->world > B200_MAX_RANKS)
+    return -2;
+  for (int k = 0; k < args->world; ++k)
+    if (((args->alive_mask >> k) & 1u) && args->seg_page[k] == nullptr) return -2;
+  return fedavg_dispatch<false, false, FedAvgRobustArgs, true>(args, n_ctas, stream);
+}
+
+extern "C" int b200_pack_client(void* seg, float* theta, const float* global_w, void* w_bf16, float* mom, long long n_mom,
+                                long long n, int wire_kind, int reset, cudaStream_t stream) {
+  using namespace b200;
+  if (n <= 0) return 0;
+  if (n % 8 != 0 || wire_kind < 0 || wire_kind > 2) return -2;
+  if ((reinterpret_cast<uintptr_t>(theta) | reinterpret_cast<uintptr_t>(global_w) | reinterpret_cast<uintptr_t>(seg)) & 15)
+    return -2;
+  const int vec = wire_kind == 0 ? 4 : 8;
+  long long g = (n / vec + 255) / 256;
+  const long long cap = 8ll * device_sm_count();
+  if (g > cap) g = cap;
+  auto* wb = reinterpret_cast<__nv_bfloat16*>(w_bf16);
+  auto* s = static_cast<uint8_t*>(seg);
+  if (wire_kind == 2)
+    pack_client_kernel<2><<<static_cast<unsigned>(g), 256, 0, stream>>>(s, theta, global_w, wb, mom, n_mom, n, reset);
+  else if (wire_kind == 1)
+    pack_client_kernel<1><<<static_cast<unsigned>(g), 256, 0, stream>>>(s, theta, global_w, wb, mom, n_mom, n, reset);
+  else
+    pack_client_kernel<0><<<static_cast<unsigned>(g), 256, 0, stream>>>(s, theta, global_w, wb, mom, n_mom, n, reset);
+  return static_cast<int>(cudaGetLastError());
 }
 
 extern "C" int b200_fedavg_allreduce(const FedAvgArgs* args, int n_ctas, cudaStream_t stream) {

@@ -183,7 +183,27 @@ struct FedAvgScaffoldArgs : FedAvgArgs {
   long long seg1_off;               // byte offset of segment 1 inside each wire half (multiple of 16)
   float inv_clients;                // 1 / N, N = the client population
 };
+// Robust round (fedavg_allreduce_robust_kernel<WIRE>): coordinate-wise median or trimmed mean over the participating
+// CLIENTS instead of the weighted mean.  Each wire half holds up to S client segments of seg_stride bytes
+// ([seg 0 | pad | seg 1 | ...], seg 0 at the half's start = the plain layout); rank k publishes its segment count m_k in
+// its page seg_page[k][0] (written by the kernel from my_segs), P = sum of m_k over the live ranks <= 32.  The owner of a
+// tile sorts the P decoded values of every element (total order, NaN above +inf), selects, and stores cast(result) into
+// seg 0 of every live replica; the apply phase is the plain one.  Loss and integer arena: as in the plain round.
+#define B200_MAX_ROBUST_CLIENTS 32
+struct FedAvgRobustArgs : FedAvgArgs {
+  uint32_t* seg_page[B200_MAX_RANKS];   // peer-mapped: seg_page[k][0] = m_k of rank k for this round
+  uint32_t my_segs;                 // m_r of this rank (0: not a participant)
+  long long seg_stride;             // bytes from one client segment to the next (multiple of 256)
+  int kind;                         // 0: median, 1: trimmed mean
+  uint8_t trim_b[B200_MAX_ROBUST_CLIENTS + 1];   // trimmed mean: b = floor(beta * P) for P = 0 .. 32 (host-computed)
+};
 int b200_fedavg_allreduce(const FedAvgArgs* args, int n_ctas, cudaStream_t stream);
+int b200_fedavg_allreduce_robust(const FedAvgRobustArgs* args, int n_ctas, cudaStream_t stream);   // delta, peer loads
+// one logical client's upload: seg = cast(theta - global_w) in wire format wire_kind (fp8: scales behind the n payload
+// bytes), exactly the collective's own pack; reset != 0 also returns the replica to the global model (theta, bf16
+// shadow, momentum [0, n_mom)) as b200_fold_client does.  n % 8 == 0, 16-byte aligned fp32 arrays.
+int b200_pack_client(void* seg, float* theta, const float* global_w, void* w_bf16, float* mom, long long n_mom,
+                     long long n, int wire_kind, int reset, cudaStream_t stream);
 int b200_fedavg_allreduce_dp(const FedAvgDPArgs* args, int n_ctas, cudaStream_t stream);   // delta mode, peer loads only
 int b200_fedavg_allreduce_scaffold(const FedAvgScaffoldArgs* args, int n_ctas, cudaStream_t stream);   // delta, peer loads
 // DP clip factor: s = min(1, clip / ||theta - global_w||_2) over [0, n), norm in fp64 (s = 0 when it is not finite), written to

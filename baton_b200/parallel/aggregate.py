@@ -159,3 +159,33 @@ def fedavg_loss_history(loss_histories: Sequence[Sequence[float]], n_samples: Se
         if den > 0:
             out.append(num / den)
     return out
+
+
+@torch.no_grad()
+def robust_into(global_state: Mapping[str, torch.Tensor], client_states: Sequence[Mapping[str, torch.Tensor]], cfg,
+                int_policy: str = "max") -> bool:
+    """Coordinate-wise median / trimmed mean (``parallel/robust.py``, ``cfg`` a ``RobustConfig``) written in place into
+    ``global_state``: every client's delta is its float entries minus the global ones in fp32, taken in
+    ``global_state`` order; ``global += robust_combine(deltas)``, unweighted over clients.  Integer entries follow
+    ``int_policy`` over all clients.  Returns False (and touches nothing) without clients."""
+    from .robust import check_participants, robust_combine
+    m = len(client_states)
+    if m == 0:
+        return False
+    check_participants(m)
+    for sd in client_states:
+        missing = [k for k in global_state if k not in sd]
+        if missing:
+            raise KeyError("client state_dict is missing {!r}".format(missing[0]))
+    for k, g in global_state.items():
+        if not g.is_floating_point():
+            continue
+        g32 = g.detach().to(device="cpu", dtype=torch.float32).reshape(-1)
+        stack = torch.stack([sd[k].detach().to(device="cpu", dtype=torch.float32).reshape(-1) - g32
+                             for sd in client_states])
+        new = g32 + robust_combine(stack, cfg)
+        g.copy_(new.reshape(g.shape).to(device=g.device, dtype=g.dtype))
+    for k, v in global_state.items():
+        if not v.is_floating_point():
+            _reduce_int(v, [sd[k] for sd in client_states], [1.0 / m] * m, int_policy)
+    return True

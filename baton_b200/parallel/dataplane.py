@@ -27,7 +27,7 @@ from typing import Any, Dict, List, Mapping, Optional
 import torch
 
 from . import wire
-from .aggregate import dp_fedavg_into, fedavg_into
+from .aggregate import dp_fedavg_into, fedavg_into, robust_into
 
 log = logging.getLogger("baton_b200.dataplane")
 
@@ -56,14 +56,20 @@ class HttpManagerPlane(ManagerPlane):
     the manager aggregates with DP-FedAvg (:func:`~baton_b200.parallel.aggregate.dp_fedavg_into`) instead of the
     sample-weighted mean.  As in the plain mean, an upload with ``n_samples == 0`` (a client that trained nothing) is
     not a participant; a round without participants aggregates nothing and does not advance the noise stream.
-    ``last_clip_factors`` holds the factors of the last aggregated round."""
+    ``last_clip_factors`` holds the factors of the last aggregated round.  ``robust`` (a
+    :class:`~baton_b200.parallel.robust.RobustConfig`, exclusive with ``dp``): the coordinate-wise median / trimmed mean
+    of the participants' updates (:func:`~baton_b200.parallel.aggregate.robust_into`), uploads with ``n_samples == 0``
+    excluded as under DP."""
 
     name = "http"
     carries_tensors = True
 
-    def __init__(self, int_policy: str = "max", dp=None):
+    def __init__(self, int_policy: str = "max", dp=None, robust=None):
+        if dp is not None and robust is not None:
+            raise ValueError("robust aggregation with DP-FedAvg is not supported")
         self.int_policy = int_policy
         self.dp = dp
+        self.robust = robust
         self.dp_rounds = 0
         self.last_clip_factors: List[float] = []
 
@@ -85,7 +91,10 @@ class HttpManagerPlane(ManagerPlane):
         # the reduce raise half-way must not leave the global model half-written
         live = experiment.model.state_dict()
         scratch = type(live)((k, v.detach().clone()) for k, v in live.items())
-        if self.dp is not None:
+        if self.robust is not None:
+            datas = [d for d in datas if float(d.get("n_samples", 0)) > 0]
+            ok = robust_into(scratch, [d["state_dict"] for d in datas], self.robust, int_policy=self.int_policy)
+        elif self.dp is not None:
             datas = [d for d in datas if float(d.get("n_samples", 0)) > 0]
             if not datas:
                 return False
@@ -122,7 +131,11 @@ class SeatedManagerPlane(ManagerPlane):
     carries_tensors = False
 
     def __init__(self, name: str = "fused", world_size: Optional[int] = None, distribute_initial: bool = True,
-                 dp=None):
+                 dp=None, robust=None):
+        if dp is not None and robust is not None:
+            raise ValueError("robust aggregation with DP-FedAvg is not supported")
+        # robust (a RobustConfig): the plan carries {"robust": {kind, trim_ratio}}; every seat uploads one segment
+        self.robust = robust
         self.name = name
         self.world_size = world_size
         self.distribute_initial = distribute_initial
@@ -173,6 +186,8 @@ class SeatedManagerPlane(ManagerPlane):
         plan = {"n_samples_by_rank": n_by_rank, "alive_ranks": sorted(set(alive) | set(seats))}
         if self.dp is not None:
             plan["dp"] = {"clip": self.dp.clip, "noise_multiplier": self.dp.noise_multiplier, "seed": self.dp.seed}
+        if self.robust is not None:
+            plan["robust"] = self.robust.to_dict()
         return plan
 
     async def aggregate(self, experiment, responses) -> bool:
@@ -273,21 +288,27 @@ class SeatedWorkerPlane(WorkerPlane):
             from .dp import DPConfig
             d = plan["dp"]
             kw["dp"] = DPConfig(float(d["clip"]), float(d["noise_multiplier"]), seed=int(d["seed"]))
+        if plan.get("robust"):
+            from .robust import RobustConfig
+            r = plan["robust"]
+            kw["robust"] = RobustConfig(str(r["kind"]), float(r["trim_ratio"]))
         self.session.aggregate(plan["n_samples_by_rank"], plan.get("alive_ranks"), **kw)
         check = getattr(self.session, "check", None)
         if check is not None:
             check()             # a peer that died mid-collective surfaces here as an error, not as a hang
 
 
-def make_manager_plane(spec, dp=None) -> ManagerPlane:
+def make_manager_plane(spec, dp=None, robust=None) -> ManagerPlane:
     if isinstance(spec, ManagerPlane):
         if dp is not None and getattr(spec, "dp", None) is None:
             raise ValueError("a DP experiment needs a data plane built with the same dp=")
+        if robust is not None and getattr(spec, "robust", None) is None:
+            raise ValueError("a robust experiment needs a data plane built with the same robust=")
         return spec
     if spec in (None, "http", "http_pickle"):
-        return HttpManagerPlane(dp=dp)
+        return HttpManagerPlane(dp=dp, robust=robust)
     if spec in ("fused", "nccl"):
-        return SeatedManagerPlane(spec, dp=dp)
+        return SeatedManagerPlane(spec, dp=dp, robust=robust)
     raise ValueError("unknown data plane {!r}".format(spec))
 
 

@@ -23,6 +23,13 @@ Both take ``scaffold=True`` (SCAFFOLD, ``parallel/scaffold.py``): every round th
 update, ``aggregate(control=(c, dc, N))`` -- ``c += (sum over ranks of dc) / N``.  The fused session lays out each
 parity half of its wire as ``[segment 0 | pad | segment 1]`` (segment 1: ``dc`` over the parameters, in the session's
 wire format) and the collective reduces both segments in one launch, on peer loads.
+
+Both take ``robust=RobustConfig(...)`` (``parallel/robust.py``): the round's update is the coordinate-wise median or
+trimmed mean of the participating CLIENTS' deltas instead of the weighted mean.  A median of per-rank sums is not a
+median of clients, so every hosted client uploads its own segment: ``max_clients=S`` lays out each parity half of the
+fused session's wire as ``[seg 0 | pad | seg 1 | ... | seg S-1]`` (``S = 1`` is the plain layout), ``pack_client(j)``
+fills segment ``j`` and ``aggregate(..., n_clients=m)`` runs the robust kernel over the ``m`` segments of every rank
+(their counts travel in a per-rank page), always on peer loads.
 """
 from __future__ import annotations
 
@@ -32,6 +39,7 @@ import torch
 
 from .arena import ParamArena
 from .dp import DPConfig, clip_factor, normals
+from .robust import MAX_ROBUST_CLIENTS, RobustConfig, robust_combine
 from .symm import SymmetricBuffer
 
 MAX_LOSS = 64       # per-epoch loss slots carried through the collective
@@ -52,6 +60,28 @@ def _check_scaffold(scaffold: bool, dp: Optional[DPConfig], delta: bool) -> None
         raise ValueError("SCAFFOLD needs mode='delta'")
     if scaffold and dp is not None:
         raise ValueError("SCAFFOLD and DP-FedAvg are exclusive: DP would have to clip and noise dc too")
+
+
+def _check_robust(robust: Optional[RobustConfig], dp: Optional[DPConfig], scaffold: bool, delta: bool,
+                  tile_flags: bool, max_clients: int) -> int:
+    if robust is None:
+        if int(max_clients) != 1:
+            raise ValueError("max_clients > 1 needs a robust aggregator: plain rounds fold their clients into one upload")
+        return 1
+    if not isinstance(robust, RobustConfig):
+        raise TypeError("robust= takes a RobustConfig")
+    if not delta:
+        raise ValueError("robust aggregation combines the updates theta - global: it needs mode='delta'")
+    if dp is not None:
+        raise ValueError("robust aggregation with DP-FedAvg is not supported: DP's sensitivity bound assumes the clipped "
+                         "mean")
+    if scaffold:
+        raise ValueError("robust aggregation with SCAFFOLD is not supported: its control-variate update is a mean")
+    if tile_flags:
+        raise ValueError("robust aggregation with tile_flags is not supported")
+    if not (1 <= int(max_clients) <= MAX_ROBUST_CLIENTS):
+        raise ValueError("max_clients must be in 1..{}, got {!r}".format(MAX_ROBUST_CLIENTS, max_clients))
+    return int(max_clients)
 
 
 def _check_control(scaffold: bool, control) -> None:
@@ -77,12 +107,14 @@ class FedAvgSession:
     def __init__(self, arena: ParamArena, group=None, *, wire_dtype: str = "bf16", mode: str = "delta",
                  nvls: "bool | str" = "auto", n_ctas: Optional[int] = None, tile_elems: int = 0, timeout_log2: int = 24,
                  reset_momentum: bool = True, tile_flags: bool = False, dp: Optional[DPConfig] = None,
-                 scaffold: bool = False):
+                 scaffold: bool = False, robust: Optional[RobustConfig] = None, max_clients: int = 1):
         from ..ops._ext import load
         self._C = load()
         assert wire_dtype in ("bf16", "fp32", "fp8") and mode in ("delta", "weights")
         _check_dp_mode(dp, mode == "delta")
         _check_scaffold(scaffold, dp, mode == "delta")
+        self.max_clients = _check_robust(robust, dp, scaffold, mode == "delta", tile_flags, max_clients)
+        self.robust = robust
         self.scaffold = bool(scaffold)
         self.arena = arena
         self.device = arena.device
@@ -105,10 +137,13 @@ class FedAvgSession:
         # packs the next round into the other half while a slow peer still applies this one (csrc/fedavg.cu)
         # SCAFFOLD: segment 1 (dc over the parameters) starts at seg1_off of each half
         self.seg1_off = _align(self._seg_bytes(arena.n), 256) if self.scaffold else 0
-        self.half_wire = _align(self.wire_bytes(), 2 << 20)          # multicast-friendly granularity
+        # robust: S client segments per half, seg_stride bytes apart (2 * S * seg_stride bytes of symmetric memory)
+        self.seg_stride = _align(self._seg_bytes(arena.n), 256)
+        half = self.max_clients * self.seg_stride if robust is not None else self.wire_bytes()
+        self.half_wire = _align(half, 2 << 20)                        # multicast-friendly granularity
         self.half_int = _align(max(arena.n_int, 1) * 8, 256)
         self.half_loss = _align(MAX_LOSS * 4, 256)
-        self.half_clip = 256                                          # DP: this rank's clip factor s_r
+        self.half_clip = 256                                          # DP: this rank's clip factor s_r; robust: m_r
         self.off_wire = 0
         self.off_int = 2 * self.half_wire
         self.off_loss = self.off_int + 2 * self.half_int
@@ -122,9 +157,11 @@ class FedAvgSession:
         if self.wire_kind == 2:
             self.use_nvls = False      # the switch adds raw elements; block scales need the P2P path
         self.dp = _agree_seed(dp, group)
-        if self.dp is not None or self.scaffold:
-            # the clip factors / the 1 / N of the control variates are applied by the readers: peer loads only
+        if self.dp is not None or self.scaffold or self.robust is not None:
+            # the clip factors / the 1 / N of the control variates are applied by the readers, and a selection is not
+            # a sum: peer loads only
             self.use_nvls = False
+        self._packed_epoch = None   # robust: barrier epoch whose wire half pack_client filled
         # DP bookkeeping: norm-kernel partials, the last clip factor / norm of this rank, non-finite updates so far
         self.dp_work = torch.zeros(self._C.DP_WORK_WORDS, dtype=torch.int64, device=self.device)
         self.dp_s = torch.ones(1, dtype=torch.float32, device=self.device)
@@ -231,12 +268,32 @@ class FedAvgSession:
             self.pack_scale.fill_(scale)
             self._armed_for = key
 
+    # ------------------------------------------------------------------ robust rounds: one segment per client
+    def segment_ptr(self, j: int) -> int:
+        """Device address of client segment ``j`` of this rank's wire half for the upcoming round."""
+        par = (self.epoch // 3) & 1
+        return self.symm.peer_ptrs(self.off_wire + par * self.half_wire)[self.rank] + int(j) * self.seg_stride
+
+    def pack_client(self, j: int, reset: bool = False) -> None:
+        """Upload the replica's client into segment ``j`` of the upcoming round: ``seg_j = cast(theta - global)`` in
+        the wire format (the collective's own pack, fp8 block scales included).  ``reset``: also return the replica
+        to the global model (theta, bf16 shadow, momentum) for the next hosted client.  Runs on the current stream."""
+        if self.robust is None:
+            raise RuntimeError("pack_client needs a session built with robust=")
+        if not (0 <= int(j) < self.max_clients):
+            raise ValueError("segment {} out of range (max_clients={})".format(j, self.max_clients))
+        a = self.arena
+        self._C.pack_client(self.segment_ptr(j), a.theta, a.global_w, a.theta_bf16,
+                            a.momentum if reset else None, self.wire_kind, bool(reset))
+        self._packed_epoch = self.epoch
+
     # ------------------------------------------------------------------ the collective
     def aggregate(self, n_samples_by_rank: Optional[Sequence[float]] = None,
                   alive_ranks: Optional[Sequence[int]] = None, my_n: Optional[float] = None,
                   loss_history: Optional[Sequence[float]] = None, on_side_stream: bool = False,
                   round_index: Optional[int] = None, prepacked: bool = False, dp: Optional[DPConfig] = None,
-                  clipped: bool = False, control=None) -> None:
+                  clipped: bool = False, control=None, n_clients: Optional[int] = None,
+                  robust: Optional[RobustConfig] = None) -> None:
         """Launch the fused reduce+broadcast+apply.  Either the full per-rank sample
         counts are given (manager-driven rounds: the plan comes over HTTP) or only this
         rank's own count ``my_n`` (SPMD engine: peers' counts ride on the barrier flags).
@@ -255,13 +312,24 @@ class FedAvgSession:
         server control-variate update in the same launch -- ``c += (sum over participating ranks of dc) / n_clients``
         on every live rank.  ``c`` and ``dc`` are fp32 over the arena's parameters; ``dc`` is this rank's summed client
         updates (read only when this rank participates).  The optimizer-emitted upload (``prepacked``) covers the
-        model segment only."""
+        model segment only.
+
+        ``n_clients`` (sessions built with ``robust=``): the number of client segments this rank contributes, filled by
+        :meth:`pack_client` for this round (default: 1 when this rank's count is non-zero, packed by the kernel or by
+        the optimizer).  The robust kernel then combines the segments of every live rank.  ``robust`` (default: the
+        session's): a robust round on any delta-mode session without arrival flags, one segment per rank (the seated
+        planes' plan carries it)."""
         world = self.world
         dp = dp if dp is not None else self.dp
         _check_dp_mode(dp, self.delta)
         _check_control(self.scaffold, control)
         if control is not None and dp is not None:
             raise ValueError("SCAFFOLD and DP-FedAvg are exclusive")
+        robust = robust if robust is not None else self.robust
+        if robust is not None and robust is not self.robust:
+            _check_robust(robust, dp, self.scaffold, self.delta, self.tile_flags is not None, 1)
+        if robust is None and n_clients is not None:
+            raise ValueError("n_clients= needs a robust session or robust=")
         if round_index is not None:
             self.epoch = (self.base_epoch + 3 * int(round_index)) & 0xFFFFFFFF
         if n_samples_by_rank is not None:
@@ -291,10 +359,20 @@ class FedAvgSession:
         a = self.arena
         # the optimizer's wire copy is only valid for the round / scale it was armed for and when the collective runs
         # the way arm_prepack assumed (NVLS needs every rank alive); otherwise the kernel packs itself (always correct)
-        nvls_now = bool(self.use_nvls and len(alive) == world and dp is None)
+        nvls_now = bool(self.use_nvls and len(alive) == world and dp is None and robust is None)
         want_scale = (counts[self.rank] if not from_flags else float(my_n)) if (self.use_nvls and world > 1) else 1.0
         prepacked = bool(prepacked and self.wire_kind != 2 and self._armed_for == (self.epoch, float(want_scale))
                          and (nvls_now == bool(self.use_nvls and world > 1)))
+        if robust is not None:
+            m = (1 if counts[self.rank] != 0.0 else 0) if n_clients is None else int(n_clients)
+            if not (0 <= m <= self.max_clients):
+                raise ValueError("n_clients={} outside 0..max_clients={}".format(m, self.max_clients))
+            if n_clients is not None and m > 0:
+                if self._packed_epoch != self.epoch:
+                    raise RuntimeError("the client segments were not packed for this round (pack_client before "
+                                       "aggregate, with the same round index)")
+                prepacked = True
+            self._packed_epoch = None
         self.last_prepacked = prepacked
         if self.tile_elems:
             tile = self.tile_elems
@@ -315,6 +393,20 @@ class FedAvgSession:
             self.epoch_word.fill_(flag_value)       # compute stream: whatever is enqueued after this call waits for THIS round
         if on_side_stream:
             stream.wait_stream(cur)
+        if robust is not None:
+            with torch.cuda.stream(stream):
+                self._C.fedavg_allreduce_robust(
+                    self.symm.peer_ptrs(o_wire), self.symm.peer_ptrs(self.off_pads),
+                    a.theta, a.global_w, a.theta_bf16, a.momentum if self.reset_momentum else None,
+                    a.int_arena if a.n_int > 0 else None, self.symm.peer_ptrs(o_int) if a.n_int > 0 else [],
+                    self.loss_local, self.symm.peer_ptrs(o_loss), self.loss_out,
+                    counts, from_flags, mask, self.rank, world, self.wire_kind, self.epoch, tile, self.n_ctas,
+                    self.timeout_log2, self.status, self.phase_ns, prepacked,
+                    self.symm.peer_ptrs(o_clip), m, self.seg_stride, robust.kind_id, robust.trim_table())
+            self.epoch = (self.epoch + 3) & 0xFFFFFFFF
+            self.rounds += 1
+            self._side_pending = on_side_stream
+            return
         with torch.cuda.stream(stream):
             dp_args = ([], 0.0, 0, 0)
             if dp is not None:
@@ -438,10 +530,13 @@ class NcclSession:
     """Same contract through ``torch.distributed`` collectives (baseline / oracle)."""
 
     def __init__(self, arena: ParamArena, group=None, *, wire_dtype: str = "bf16", mode: str = "delta",
-                 reset_momentum: bool = True, dp: Optional[DPConfig] = None, scaffold: bool = False, **_unused):
+                 reset_momentum: bool = True, dp: Optional[DPConfig] = None, scaffold: bool = False,
+                 robust: Optional[RobustConfig] = None, max_clients: int = 1, tile_flags: bool = False, **_unused):
         import torch.distributed as dist
         _check_dp_mode(dp, mode == "delta")
         _check_scaffold(scaffold, dp, mode == "delta")
+        self.max_clients = _check_robust(robust, dp, scaffold, mode == "delta", tile_flags, max_clients)
+        self.robust = robust
         self.scaffold = bool(scaffold)
         self.dist = dist
         self.arena, self.group, self.device = arena, group, arena.device
@@ -455,15 +550,59 @@ class NcclSession:
         self.world = dist.get_world_size(group) if inited else 1
         self.rank = dist.get_rank(group) if inited else 0
         self.wire = torch.zeros(arena.n, dtype=self.wire_dtype, device=self.device)
+        # robust: this rank's client segments (wire format) and how many of them pack_client filled this round
+        self.segs = (torch.zeros(self.max_clients, arena.n, dtype=self.wire_dtype, device=self.device)
+                     if robust is not None else None)
         self.counts = torch.zeros(self.world, dtype=torch.float32, device=self.device)
         self.loss_buf = torch.zeros(MAX_LOSS, dtype=torch.float32, device=self.device)
         self.loss_out = torch.zeros(MAX_LOSS, dtype=torch.float32, device=self.device)
         self.rounds = 0
 
     @torch.no_grad()
+    def pack_client(self, j: int, reset: bool = False) -> None:
+        """Segment ``j`` = the wire-format delta of the replica's client; ``reset`` returns the replica to the global
+        model (as :meth:`FedAvgSession.pack_client`)."""
+        if self.robust is None:
+            raise RuntimeError("pack_client needs a session built with robust=")
+        if not (0 <= int(j) < self.max_clients):
+            raise ValueError("segment {} out of range (max_clients={})".format(j, self.max_clients))
+        a = self.arena
+        self.segs[int(j)].copy_((a.theta - a.global_w).to(self.wire_dtype))
+        if reset:
+            a.theta.copy_(a.global_w)
+            a.sync_shadow()
+            if a.momentum is not None:
+                a.momentum.zero_()
+
+    def _robust_update(self, counts, n_clients, robust: RobustConfig) -> torch.Tensor:
+        """All-gather every rank's segments (padded to ``max_clients``) and their counts; ``robust_combine`` over the
+        participants, rounded to the wire format as the fused kernel stores it."""
+        a, dist = self.arena, self.dist
+        if self.segs is None:       # a plain session asked for a robust round (seated plan): one segment
+            self.segs = torch.zeros(1, a.n, dtype=self.wire_dtype, device=self.device)
+        m = (1 if float(counts[self.rank]) != 0.0 else 0) if n_clients is None else int(n_clients)
+        if not (0 <= m <= self.segs.shape[0]):
+            raise ValueError("n_clients={} outside 0..max_clients={}".format(m, self.max_clients))
+        if n_clients is None and m:
+            self.segs[0].copy_((a.theta - a.global_w).to(self.wire_dtype))
+        mine = self.segs.float()
+        ms = torch.tensor([m], dtype=torch.int64, device=self.device)
+        if self.world > 1:
+            all_m = [torch.zeros_like(ms) for _ in range(self.world)]
+            dist.all_gather(all_m, ms, group=self.group)
+            all_s = [torch.zeros_like(mine) for _ in range(self.world)]
+            dist.all_gather(all_s, mine, group=self.group)
+        else:
+            all_m, all_s = [ms], [mine]
+        rows = [sg[: int(mk)] for sg, mk in zip(all_s, all_m)]
+        stacked = torch.cat(rows, 0) if rows else mine[:0]
+        return robust_combine(stacked, robust).to(self.wire_dtype).float()
+
+    @torch.no_grad()
     def aggregate(self, n_samples_by_rank=None, alive_ranks=None, my_n=None, loss_history=None,
                   dp: Optional[DPConfig] = None, clipped: bool = False, round_index: Optional[int] = None,
-                  control=None, **_unused) -> None:
+                  control=None, n_clients: Optional[int] = None, robust: Optional[RobustConfig] = None,
+                  **_unused) -> None:
         """DP-FedAvg (``dp``, default the session's): the same estimator as the fused kernel -- clip locally, all-reduce,
         then add the host-generated noise ``sigma C z(seed, round) / m`` after the reduce.  ``round_index`` (the
         manager's plan) sets the round counter, as it sets the fused session's barrier epoch.  ``control = (c, dc,
@@ -486,7 +625,13 @@ class NcclSession:
         total = counts.sum()
         w = counts[self.rank] / total
         src = (a.theta - a.global_w) if self.delta else a.theta
-        if dp is not None:
+        robust = robust if robust is not None else self.robust
+        if robust is not None:
+            upd = self._robust_update(counts, n_clients, robust)
+            w = w if float(total) > 0.0 else torch.zeros_like(w)
+        elif n_clients is not None:
+            raise ValueError("n_clients= needs a session built with robust=")
+        elif dp is not None:
             s = 1.0
             if not clipped and float(counts[self.rank]) != 0.0:
                 s, _ = clip_factor(src, dp.clip)
@@ -498,7 +643,7 @@ class NcclSession:
             self.wire.copy_((src * wd).to(self.wire_dtype))
         else:
             self.wire.copy_((src * w).to(self.wire_dtype))
-        if self.world > 1:
+        if self.world > 1 and robust is None:
             dist.all_reduce(self.wire, group=self.group)
         # every rank joins the loss reduce every round -- a rank that hosts no sampled client this round
         # contributes zeros (weight 0); skipping the call there would desynchronise the collectives
@@ -509,7 +654,9 @@ class NcclSession:
         if self.world > 1:
             dist.all_reduce(self.loss_buf, group=self.group)
         self.loss_out.copy_(self.loss_buf)
-        if dp is not None and dp.noise_std > 0.0 and float(total) > 0.0:
+        if robust is not None:
+            a.global_w.add_(upd)
+        elif dp is not None and dp.noise_std > 0.0 and float(total) > 0.0:
             z = torch.from_numpy(normals(dp.seed, self.rounds & 0xFFFFFFFF, a.n)).to(device=self.device,
                                                                                       dtype=torch.float32)
             a.global_w.add_(self.wire.float() + z * (dp.noise_std / float(total)))

@@ -31,6 +31,8 @@ Nesterov, FedProx or SCAFFOLD term.
 """
 from __future__ import annotations
 
+import contextlib
+import gc
 from collections import OrderedDict
 from typing import Callable, List, Optional, Tuple
 
@@ -189,6 +191,21 @@ def _eval_batch_generic(model, xb, yb, acc, loss_kind, F):
         # per-sample mean squared error, summed over the batch: the mean over samples is mse_loss of the whole shard
         per_row = max(1, out.numel() // max(1, out.shape[0]))
         F.load().mse(out.contiguous(), yb.reshape(out.shape).contiguous().float(), None, acc, 1.0 / per_row)
+
+
+@contextlib.contextmanager
+def _no_gc_during_capture():
+    """Keep the cyclic garbage collector from running while a CUDA graph is captured.  A model and its graphed trainer
+    reference each other, so a dropped engine's graphs are freed only by the collector, which can run at any allocation.
+    Destroying a graph is not permitted while a stream is capturing, and the attempt invalidates the capture in progress;
+    deferred until after the capture, it is harmless."""
+    enabled = gc.isenabled()
+    gc.disable()
+    try:
+        yield
+    finally:
+        if enabled:
+            gc.enable()
 
 
 class GraphedLocalSGD:
@@ -395,7 +412,7 @@ class GraphedLocalSGD:
                     graph.capture_end()
                     graph2.capture_begin(pool=pool)
             self._first_gemm_hook = cut
-            with torch.cuda.stream(cap):
+            with torch.cuda.stream(cap), _no_gc_during_capture():
                 graph.capture_begin(pool=pool)
                 try:
                     body()
@@ -406,7 +423,7 @@ class GraphedLocalSGD:
             if not state["cut"]:
                 graph2 = None
         else:
-            with torch.cuda.graph(graph):
+            with _no_gc_during_capture(), torch.cuda.graph(graph):
                 body()
         self.kernels_per_epoch = total_launches() - c0      # our kernels inside one epoch graph
         self.n_kernels_per_step = self.kernels_per_epoch // max(1, n_steps)
@@ -495,7 +512,7 @@ class GraphedLocalSGD:
         torch.cuda.synchronize(self.device)
         graph = torch.cuda.CUDAGraph()
         c0 = launch_counts()
-        with torch.cuda.graph(graph):
+        with _no_gc_during_capture(), torch.cuda.graph(graph):
             self._eval_pass(X, y, batch_size, explicit)
         self.eval_launches = launch_counts() - c0
         self.eval_captures = getattr(self, "eval_captures", 0) + 1
