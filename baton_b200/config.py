@@ -36,8 +36,10 @@ class FederationConfig:
     dp_noise_multiplier: float = 0.0   # DP-FedAvg: noise std on the sum of clipped updates, in units of dp_clip
     dp_delta: float = 1e-5             # DP-FedAvg: delta of the (epsilon, delta) the manager reports
     dp_seed: Optional[int] = None      # DP-FedAvg noise key (None: secret random; an explicit key is for tests only)
-    aggregator: str = "mean"           # mean | median | trimmed_mean (coordinate-wise, unweighted over clients)
+    aggregator: str = "mean"           # mean | median | trimmed_mean (coordinate-wise) | krum (Multi-Krum); unweighted
     trim_ratio: float = 0.1            # trimmed_mean: fraction trimmed at each end, 0 <= beta < 0.5
+    krum_f: int = 0                    # krum: Byzantine clients assumed (needs >= 2f + 3 participants per round)
+    krum_m: Optional[int] = None       # krum: clients kept (None: participants - f; 1: classic Krum)
     partition: str = "iid"             # iid | label_skew | dirichlet
     alpha: float = 0.1                 # Dirichlet concentration
     samples_per_client: int = 4096
@@ -63,6 +65,11 @@ class FederationConfig:
         self.trim_ratio = check_aggregator(self.aggregator, self.trim_ratio)
         if self.aggregator != "mean" and float(self.dp_clip) > 0.0:
             raise ValueError("a robust aggregator with DP-FedAvg is not supported")
+        if self.aggregator == "krum":
+            from .parallel.robust import check_krum, check_krum_participants
+            check_krum(self.krum_f, self.krum_m)
+            population = self.logical_clients if self.logical_clients > self.clients else self.clients
+            check_krum_participants(min(self.sample_k, population) if self.sample_k else population, self.krum_f)
 
     def train_kwargs(self) -> dict:
         """Local-training keyword arguments of a worker (``FederatedModule.local_train``)."""
@@ -83,7 +90,7 @@ class FederationConfig:
         if self.aggregator == "mean":
             return None
         from .parallel.robust import RobustConfig
-        return RobustConfig(self.aggregator, self.trim_ratio)
+        return RobustConfig(self.aggregator, self.trim_ratio, self.krum_f, self.krum_m)
 
     def to_json(self) -> str:
         return json.dumps(asdict(self), sort_keys=True)
@@ -103,7 +110,7 @@ class FederationConfig:
             flag = "--" + f.name.replace("_", "-")
             default = f.default
             typ = type(default) if default is not None else None
-            if f.name in ("sample_k", "dp_seed"):
+            if f.name in ("sample_k", "dp_seed", "krum_m"):
                 typ = int
             if f.name in ("round_timeout",):
                 typ = float

@@ -53,8 +53,10 @@ class GpuExperimentWorker(EvaluatingSeat, ExperimentWorker):
                  backend: str = "fused", group=None, loss: str = "ce", wire_dtype: str = "bf16",
                  momentum: float = 0.0, use_graph: bool = True, n_ctas: int = 64,
                  eval_shard_fn: Optional[Callable[[], Tuple[torch.Tensor, torch.Tensor]]] = None,
-                 eval_batch_size: int = 512, **kwargs):
-        """``eval_shard_fn`` (optional): ``() -> (X, y)``, this seat's held-out shard for ``POST /{name}/evaluate``."""
+                 eval_batch_size: int = 512, robust=None, **kwargs):
+        """``eval_shard_fn`` (optional): ``() -> (X, y)``, this seat's held-out shard for ``POST /{name}/evaluate``.
+        ``robust`` (optional :class:`~baton_b200.parallel.robust.RobustConfig`): the session's aggregator.  A seat of a
+        Krum experiment needs it, because a fused Krum session allocates its distance page at construction."""
         self.device = torch.device(device)
         self.eval_shard_fn, self.eval_batch_size = eval_shard_fn, eval_batch_size
         self._eval_stage = None
@@ -65,7 +67,7 @@ class GpuExperimentWorker(EvaluatingSeat, ExperimentWorker):
         self.trainer = GraphedLocalSGD(model, self.arena, loss=loss, use_graph=use_graph)
         model._graphed_trainer = self.trainer
         Session = {"fused": FedAvgSession, "nccl": NcclSession}[backend]
-        self.fed_session = Session(self.arena, group, wire_dtype=wire_dtype, n_ctas=n_ctas)
+        self.fed_session = Session(self.arena, group, wire_dtype=wire_dtype, n_ctas=n_ctas, robust=robust)
         self.shard_fn = shard_fn
         self._stage = None
         train_kwargs = dict(kwargs.pop("train_kwargs", None) or {})

@@ -662,6 +662,64 @@ void fedavg_allreduce_robust(const std::vector<int64_t>& wire_ptrs, const std::v
   check(b200_fedavg_allreduce_robust(&a, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_robust");
 }
 
+// Multi-Krum round: the robust round's arguments plus every rank's distance page, the local work / sync / report
+// buffers and the per-P tables k and m (the kept mean runs as the trimmed mean with b = 0)
+void fedavg_allreduce_krum(const std::vector<int64_t>& wire_ptrs, const std::vector<int64_t>& pad_ptrs, at::Tensor theta,
+                           const at::Tensor& global_w, const std::optional<at::Tensor>& theta_bf16,
+                           const std::optional<at::Tensor>& momentum, const std::optional<at::Tensor>& int_local,
+                           const std::vector<int64_t>& int_wire_ptrs, const std::optional<at::Tensor>& loss_local,
+                           const std::vector<int64_t>& loss_wire_ptrs, const std::optional<at::Tensor>& loss_out,
+                           const std::vector<double>& n_samples, bool counts_from_flags, int64_t alive_mask, int64_t rank,
+                           int64_t world, int64_t wire_kind, int64_t epoch, int64_t tile_elems, int64_t n_ctas,
+                           int64_t timeout_log2, const std::optional<at::Tensor>& status,
+                           const std::optional<at::Tensor>& phase_ns, bool prepacked,
+                           const std::vector<int64_t>& seg_page_ptrs, int64_t my_segs, int64_t seg_stride,
+                           const std::vector<int64_t>& dist_page_ptrs, at::Tensor work, at::Tensor sync,
+                           const std::optional<at::Tensor>& report, const std::vector<int64_t>& krum_k,
+                           const std::vector<int64_t>& krum_m) {
+  FedAvgKrumArgs a = {};
+  fill_fedavg_args(a, wire_ptrs, pad_ptrs, 0, theta, global_w, theta_bf16, momentum, int_local, int_wire_ptrs, loss_local,
+                   loss_wire_ptrs, loss_out, n_samples, counts_from_flags, alive_mask, rank, world, wire_kind, true, false,
+                   epoch, std::nullopt, 0, tile_elems, timeout_log2, status, phase_ns, prepacked);
+  TORCH_CHECK(static_cast<int64_t>(seg_page_ptrs.size()) == world, "krum: one count page per rank");
+  TORCH_CHECK(static_cast<int64_t>(dist_page_ptrs.size()) == world, "krum: one distance page per rank");
+  TORCH_CHECK(static_cast<int64_t>(krum_k.size()) == B200_MAX_ROBUST_CLIENTS + 1 &&
+                  static_cast<int64_t>(krum_m.size()) == B200_MAX_ROBUST_CLIENTS + 1,
+              "krum: k and m for P = 0 .. 32");
+  TORCH_CHECK(my_segs >= 0 && my_segs <= B200_MAX_ROBUST_CLIENTS, "krum: at most 32 segments per rank");
+  CHECK_CUDA(work);
+  CHECK_CUDA(sync);
+  TORCH_CHECK(work.scalar_type() == at::kDouble && work.is_contiguous() &&
+                  work.numel() >= static_cast<int64_t>(B200_KRUM_MAX_CTAS) * B200_KRUM_PAIRS,
+              "krum: work = float64[B200_KRUM_MAX_CTAS * B200_KRUM_PAIRS]");
+  TORCH_CHECK(sync.scalar_type() == at::kInt && sync.numel() >= 2, "krum: sync = int32[2]");
+  for (int64_t k = 0; k < world; ++k) {
+    a.seg_page[k] = reinterpret_cast<uint32_t*>(seg_page_ptrs[k]);
+    a.dist_page[k] = reinterpret_cast<double*>(dist_page_ptrs[k]);
+  }
+  for (int p = 0; p <= B200_MAX_ROBUST_CLIENTS; ++p) {
+    TORCH_CHECK(krum_k[p] >= 0 && krum_k[p] < (p > 0 ? p : 1), "krum: need 0 <= k < P");
+    TORCH_CHECK(krum_m[p] >= (p > 0 ? 1 : 0) && krum_m[p] <= p, "krum: need 1 <= m <= P");
+    a.krum_k[p] = static_cast<uint8_t>(krum_k[p]);
+    a.krum_m[p] = static_cast<uint8_t>(krum_m[p]);
+    a.trim_b[p] = 0;
+  }
+  a.my_segs = static_cast<uint32_t>(my_segs);
+  a.seg_stride = seg_stride;
+  a.kind = 1;
+  a.work = work.data_ptr<double>();
+  a.sync = reinterpret_cast<unsigned int*>(sync.data_ptr<int>());
+  a.report = nullptr;
+  if (report.has_value() && report->defined()) {
+    CHECK_CUDA(*report);
+    TORCH_CHECK(report->scalar_type() == at::kDouble && report->is_contiguous() && report->numel() >= B200_KRUM_REPORT,
+                "krum: report = float64[B200_KRUM_REPORT]");
+    a.report = report->data_ptr<double>();
+  }
+  const c10::cuda::CUDAGuard guard(theta.device());
+  check(b200_fedavg_allreduce_krum(&a, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_krum");
+}
+
 // one logical client's wire segment at address seg (see b200_pack_client)
 void pack_client(int64_t seg, at::Tensor theta, const at::Tensor& global_w, const std::optional<at::Tensor>& wb,
                  const std::optional<at::Tensor>& mom, int64_t wire_kind, bool reset) {
@@ -994,6 +1052,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("embedding_bwd", &embedding_bwd);
   m.def("fedavg_allreduce", &fedavg_allreduce);
   m.def("fedavg_allreduce_robust", &fedavg_allreduce_robust);
+  m.def("fedavg_allreduce_krum", &fedavg_allreduce_krum);
+  m.attr("KRUM_MAX_CTAS") = B200_KRUM_MAX_CTAS;
+  m.attr("KRUM_PAIRS") = B200_KRUM_PAIRS;
+  m.attr("KRUM_REPORT") = B200_KRUM_REPORT;
   m.def("pack_client", &pack_client);
   m.attr("MAX_ROBUST_CLIENTS") = B200_MAX_ROBUST_CLIENTS;
   m.def("flag_barrier", &flag_barrier);

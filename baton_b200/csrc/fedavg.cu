@@ -401,9 +401,11 @@ __device__ __forceinline__ float robust_select(const uint32_t* col, int stride, 
   return __fdiv_rn(acc, static_cast<float>(P - 2 * b));
 }
 
+// load: elements [e0, e0 + clen) of the P segments src[0 .. P) into the stage [NP][CH] as order-preserving keys, RG
+// wire vectors per thread issued before the first decode (shared by the selection and Krum's distance pass)
 template <int WIRE, int NP>
-__device__ __forceinline__ void robust_tiles(const FedAvgRobustArgs& a, uint8_t* const* s_wire, const uint8_t* const* src,
-                                             uint32_t* stage, int P, int A, int my_pos) {
+__device__ __forceinline__ void robust_stage(const uint8_t* const* src, uint32_t* stage, int P, long long n, long long e0,
+                                             int clen) {
   using W = Wire<WIRE>;
   constexpr int VEC = W::VEC;
   constexpr size_t esz = W::VBYTES / VEC;
@@ -412,6 +414,42 @@ __device__ __forceinline__ void robust_tiles(const FedAvgRobustArgs& a, uint8_t*
   constexpr int R = NP * VPR / FEDAVG_THREADS;   // loads per thread per chunk
   constexpr int RG = 4;                          // ... in groups of RG in flight
   static_assert(R * FEDAVG_THREADS == NP * VPR && R % RG == 0, "the stage must split evenly over the threads");
+#pragma unroll 1
+  for (int r0 = 0; r0 < R; r0 += RG) {
+    uint4 v[RG];
+    uint32_t sc[RG];
+#pragma unroll
+    for (int r = 0; r < RG; ++r) {
+      const int w = threadIdx.x + (r0 + r) * FEDAVG_THREADS, p = w / VPR, q = (w % VPR) * VEC;
+      if (p < P && q < clen) {
+        v[r] = W::ld(src[p] + (e0 + q) * esz);
+        if constexpr (W::SCALED) sc[r] = ld_volatile_u8(src[p] + n + ((e0 + q) >> 5));
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < RG; ++r) {
+      const int w = threadIdx.x + (r0 + r) * FEDAVG_THREADS, p = w / VPR, q = (w % VPR) * VEC;
+      if (p < P && q < clen) {
+        float f[VEC];
+        float scale = 1.f;
+        if constexpr (W::SCALED) scale = exp2_int(static_cast<int>(sc[r]) - 127);
+        W::unpack(v[r], f, scale);
+#pragma unroll
+        for (int j = 0; j < VEC; j += 4)
+          *reinterpret_cast<uint4*>(stage + p * CH + q + j) =
+              make_uint4(robust_key(f[j]), robust_key(f[j + 1]), robust_key(f[j + 2]), robust_key(f[j + 3]));
+      }
+    }
+  }
+}
+
+template <int WIRE, int NP>
+__device__ __forceinline__ void robust_tiles(const FedAvgRobustArgs& a, uint8_t* const* s_wire, const uint8_t* const* src,
+                                             uint32_t* stage, int P, int A, int my_pos) {
+  using W = Wire<WIRE>;
+  constexpr int VEC = W::VEC;
+  constexpr size_t esz = W::VBYTES / VEC;
+  constexpr int CH = ROBUST_STAGE / NP;          // elements per chunk
   const int G = gridDim.x;
   const long long n = a.n;
   const int T = a.tile_elems;
@@ -424,34 +462,7 @@ __device__ __forceinline__ void robust_tiles(const FedAvgRobustArgs& a, uint8_t*
     for (int c0 = 0; c0 < len; c0 += CH) {
       const int clen = len - c0 < CH ? len - c0 : CH;
       const long long e0 = base + c0;
-      // ---- load: RG loads per thread issued before the first decode
-#pragma unroll 1
-      for (int r0 = 0; r0 < R; r0 += RG) {
-        uint4 v[RG];
-        uint32_t sc[RG];
-#pragma unroll
-        for (int r = 0; r < RG; ++r) {
-          const int w = threadIdx.x + (r0 + r) * FEDAVG_THREADS, p = w / VPR, q = (w % VPR) * VEC;
-          if (p < P && q < clen) {
-            v[r] = W::ld(src[p] + (e0 + q) * esz);
-            if constexpr (W::SCALED) sc[r] = ld_volatile_u8(src[p] + n + ((e0 + q) >> 5));
-          }
-        }
-#pragma unroll
-        for (int r = 0; r < RG; ++r) {
-          const int w = threadIdx.x + (r0 + r) * FEDAVG_THREADS, p = w / VPR, q = (w % VPR) * VEC;
-          if (p < P && q < clen) {
-            float f[VEC];
-            float scale = 1.f;
-            if constexpr (W::SCALED) scale = exp2_int(static_cast<int>(sc[r]) - 127);
-            W::unpack(v[r], f, scale);
-#pragma unroll
-            for (int j = 0; j < VEC; j += 4)
-              *reinterpret_cast<uint4*>(stage + p * CH + q + j) =
-                  make_uint4(robust_key(f[j]), robust_key(f[j + 1]), robust_key(f[j + 2]), robust_key(f[j + 3]));
-          }
-        }
-      }
+      robust_stage<WIRE, NP>(src, stage, P, n, e0, clen);
       __syncthreads();
       // ---- select: one column per thread
 #pragma unroll 1
@@ -521,13 +532,9 @@ __device__ __forceinline__ void robust_tiles(const FedAvgRobustArgs& a, uint8_t*
 }
 
 // phase 1 of a robust round: gather the P client segments of the live ranks (counts from their pages), then select
-template <int WIRE>
-__device__ __forceinline__ void robust_reduce(const FedAvgRobustArgs& a, uint8_t* const* s_wire, const int* s_rank, int A,
-                                              int my_pos) {
-  extern __shared__ __align__(16) uint8_t robust_smem[];
-  uint32_t* stage = reinterpret_cast<uint32_t*>(robust_smem);
-  const uint8_t** src = reinterpret_cast<const uint8_t**>(robust_smem + ROBUST_STAGE * 4);
-  int* s_P = reinterpret_cast<int*>(robust_smem + ROBUST_STAGE * 4 + B200_MAX_ROBUST_CLIENTS * 8);
+// the P client segments of the live ranks in segment order (rank position, then the rank's segment order) into src
+__device__ __forceinline__ int robust_gather(const FedAvgRobustArgs& a, uint8_t* const* s_wire, const int* s_rank, int A,
+                                             const uint8_t** src, int* s_P) {
   if (threadIdx.x == 0) {
     int P = 0;
     for (int k = 0; k < A; ++k) {
@@ -538,10 +545,273 @@ __device__ __forceinline__ void robust_reduce(const FedAvgRobustArgs& a, uint8_t
     *s_P = P;
   }
   __syncthreads();
-  const int P = *s_P;
+  return *s_P;
+}
+
+template <int WIRE>
+__device__ __forceinline__ void robust_reduce(const FedAvgRobustArgs& a, uint8_t* const* s_wire, const int* s_rank, int A,
+                                              int my_pos) {
+  extern __shared__ __align__(16) uint8_t robust_smem[];
+  uint32_t* stage = reinterpret_cast<uint32_t*>(robust_smem);
+  const uint8_t** src = reinterpret_cast<const uint8_t**>(robust_smem + ROBUST_STAGE * 4);
+  int* s_P = reinterpret_cast<int*>(robust_smem + ROBUST_STAGE * 4 + B200_MAX_ROBUST_CLIENTS * 8);
+  const int P = robust_gather(a, s_wire, s_rank, A, src, s_P);
   if (P <= 8) robust_tiles<WIRE, 8>(a, s_wire, src, stage, P, A, my_pos);
   else if (P <= 16) robust_tiles<WIRE, 16>(a, s_wire, src, stage, P, A, my_pos);
   else robust_tiles<WIRE, 32>(a, s_wire, src, stage, P, A, my_pos);
+}
+
+// ---------------------------------------------------------------- Multi-Krum rounds (see launch.h / parallel/robust.py)
+// Phase 1 of a Krum round, between barrier 1 (epoch + 1) and barrier 2 (epoch + 3):
+//   distances  the owner of a tile stages the P segments chunk by chunk (robust_stage) and adds the upper-triangle
+//              pair sums (x_i - x_j)^2 from shared memory: 4 x 4 register blocks of rows, 4 columns per lane, 16 fp32
+//              sums per lane reduced over the warp by a transpose-reduce (16 shuffles), the 128-column slices of a
+//              chunk added in slice order in fp32, and the chunk's sum added to one fp64 accumulator per pair;
+//   rank       every CTA writes its P(P-1)/2 fp64 partials into its slot of a local work buffer; the last CTA to
+//              arrive (a device counter the launcher zeroes) adds the slots in CTA order into this rank's distance page;
+//              the other CTAs wait for it with a bounded spin (not a grid sync: a CTA whose cross-GPU barrier timed
+//              out has returned, and an unbounded grid-wide wait would hang the rest of the grid);
+//   exchange   a per-CTA cross-rank barrier at epoch + 2: once CTA b passes it, CTA b of every live rank has passed
+//              the rank step, so every page is complete.  Every CTA adds the A pages in rank order: every CTA of every
+//              rank holds the same D bits and computes the same scores and kept set;
+//   kept mean  robust_tiles over the m kept segments with the trimmed mean and b = 0 (the host sets kind and trim_b).
+// P <= 2 skips the distances and the exchange on every rank alike (P is known identically after barrier 1): all
+// scores tie and the first m segments are kept.
+constexpr int KRUM_PAIRS = B200_KRUM_PAIRS;
+constexpr int KRUM_ITEMS = 144;                 // (block pair, 128-column slice) items per chunk at NP = 32 (the most)
+constexpr int KRUM_PART_OFF = ROBUST_SMEM;      // float [KRUM_ITEMS][16]: per-item pair sums of a chunk
+constexpr int KRUM_D_OFF = KRUM_PART_OFF + KRUM_ITEMS * 16 * 4;              // double [32][32]
+constexpr int KRUM_SCORE_OFF = KRUM_D_OFF + B200_MAX_ROBUST_CLIENTS * B200_MAX_ROBUST_CLIENTS * 8;   // double [32]
+constexpr int KRUM_KEPT_OFF = KRUM_SCORE_OFF + B200_MAX_ROBUST_CLIENTS * 8;  // int [32] + the "last CTA" word
+constexpr int KRUM_SMEM = KRUM_KEPT_OFF + (B200_MAX_ROBUST_CLIENTS + 4) * 4;
+
+__device__ __forceinline__ uint32_t ld_acquire_gpu_u32(const uint32_t* p) {
+  uint32_t v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+
+// pair p of the upper triangle of P rows (row-major: (0,1), (0,2), ..., (1,2), ...)
+__device__ __forceinline__ void krum_pair(int p, int P, int& i, int& j) {
+  i = 0;
+  while (p >= P - 1 - i) {
+    p -= P - 1 - i;
+    ++i;
+  }
+  j = i + 1 + p;
+}
+
+// one step of the warp transpose-reduce of 16 values: lanes with bit 2H set keep values H .. 2H-1, the others 0 .. H-1,
+// each added to its partner's copy
+template <int H>
+__device__ __forceinline__ void krum_reduce_step(float (&v)[16], int lane) {
+  const bool upper = (lane & (2 * H)) != 0;
+#pragma unroll
+  for (int q = 0; q < H; ++q) {
+    const float send = upper ? v[q] : v[q + H];
+    const float keep = upper ? v[q + H] : v[q];
+    v[q] = __fadd_rn(keep, __shfl_xor_sync(0xffffffffu, send, 2 * H));
+  }
+}
+
+// this CTA's fp64 sums of (x_i - x_j)^2 over its tiles, for the pair (pi, pj) of this thread (pi < 0: none)
+template <int WIRE, int NP>
+__device__ __forceinline__ double krum_distances(const FedAvgKrumArgs& a, const uint8_t* const* src, uint32_t* stage,
+                                                 float* part, int P, int A, int my_pos, int pi, int pj) {
+  constexpr int CH = ROBUST_STAGE / NP;
+  constexpr int NB = NP / 4;                      // 4-row blocks
+  constexpr int NBLK = NB * (NB + 1) / 2;         // block pairs bi <= bj
+  constexpr int SLICES = CH / 128;                // 128-column slices: 4 columns per lane
+  constexpr int ITEMS = NBLK * SLICES;
+  static_assert(ITEMS % (FEDAVG_THREADS / 32) == 0 && ITEMS <= KRUM_ITEMS, "items must split evenly over the warps");
+  const int G = gridDim.x;
+  const long long n = a.n;
+  const int T = a.tile_elems;
+  const long long n_tiles = (n + T - 1) / T;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  int my_item = -1, my_idx = 0;
+  if (pi >= 0) {
+    const int bi = pi >> 2, bj = pj >> 2;
+    my_item = (bi * NB - bi * (bi - 1) / 2 + bj - bi) * SLICES;
+    my_idx = (pi & 3) * 4 + (pj & 3);
+  }
+  double acc = 0.0;
+  for (long long t = my_pos + static_cast<long long>(blockIdx.x) * A; t < n_tiles; t += static_cast<long long>(G) * A) {
+    const long long base = t * T;
+    const int len = static_cast<int>((n - base) < T ? (n - base) : T);
+    for (int c0 = 0; c0 < len; c0 += CH) {
+      const int clen = len - c0 < CH ? len - c0 : CH;
+      robust_stage<WIRE, NP>(src, stage, P, n, base + c0, clen);
+      __syncthreads();
+#pragma unroll 1
+      for (int it = warp; it < ITEMS; it += FEDAVG_THREADS / 32) {
+        int bi = 0, r = it / SLICES;
+        while (r >= NB - bi) {
+          r -= NB - bi;
+          ++bi;
+        }
+        const int bj = bi + r, c1 = (it % SLICES) * 128 + lane;
+        float v[16];
+#pragma unroll
+        for (int q = 0; q < 16; ++q) v[q] = 0.f;
+#pragma unroll 1
+        for (int u = 0; u < 4; ++u) {
+          const int c = c1 + 32 * u;
+          if (c < clen) {
+            float xi[4], xj[4];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              xi[q] = robust_unkey(stage[(4 * bi + q) * CH + c]);
+              xj[q] = robust_unkey(stage[(4 * bj + q) * CH + c]);
+            }
+#pragma unroll
+            for (int q = 0; q < 4; ++q)
+#pragma unroll
+              for (int w = 0; w < 4; ++w) {
+                const float d = __fsub_rn(xi[q], xj[w]);
+                v[q * 4 + w] = __fmaf_rn(d, d, v[q * 4 + w]);
+              }
+          }
+        }
+        // transpose-reduce: after the step over lane bit o, a lane keeps the half of its values selected by that bit;
+        // lane l ends with the warp sum of value ((l >> 1) & 15) (the last step adds the two lanes that share it)
+        krum_reduce_step<8>(v, lane);
+        krum_reduce_step<4>(v, lane);
+        krum_reduce_step<2>(v, lane);
+        krum_reduce_step<1>(v, lane);
+        v[0] = __fadd_rn(v[0], __shfl_xor_sync(0xffffffffu, v[0], 1));
+        if ((lane & 1) == 0) part[it * 16 + (lane >> 1)] = v[0];
+      }
+      __syncthreads();
+      if (my_item >= 0) {
+        float sum = 0.f;
+#pragma unroll 1
+        for (int sl = 0; sl < SLICES; ++sl) sum = __fadd_rn(sum, part[(my_item + sl) * 16 + my_idx]);
+        acc += static_cast<double>(sum);
+      }
+      // the next chunk's stage load may start: the stage was last read before the barrier above, and part is rewritten
+      // only after the barrier that follows that load
+    }
+  }
+  return acc;
+}
+
+// CTA partials -> this rank's distance page (last CTA to arrive, CTA order); false on timeout (status written)
+__device__ __forceinline__ bool krum_rank_reduce(const FedAvgKrumArgs& a, double acc, int npairs, int* s_last) {
+  const int G = gridDim.x;
+  if (static_cast<int>(threadIdx.x) < npairs) a.work[static_cast<size_t>(blockIdx.x) * KRUM_PAIRS + threadIdx.x] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    *s_last = atomicAdd(a.sync, 1u) == static_cast<unsigned>(G - 1);
+  }
+  __syncthreads();
+  bool ok = true;
+  if (*s_last) {
+    __threadfence();
+    if (static_cast<int>(threadIdx.x) < npairs) {
+      double d = 0.0;
+      for (int b = 0; b < G; ++b)
+        d += *reinterpret_cast<const volatile double*>(a.work + static_cast<size_t>(b) * KRUM_PAIRS + threadIdx.x);
+      a.dist_page[a.rank][threadIdx.x] = d;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      __threadfence_system();
+      atomicExch(a.sync + 1, 1u);
+    }
+  } else if (threadIdx.x == 0) {
+    unsigned long long spins = 0;
+    const unsigned long long limit = a.timeout_log2 > 0 ? (1ull << a.timeout_log2) : ~0ull;
+    while (ld_acquire_gpu_u32(a.sync + 1) == 0u) {
+      if (++spins > limit) {
+        ok = false;
+        if (a.status != nullptr) atomicExch(a.status, 1 + a.rank);
+        break;
+      }
+    }
+  }
+  return __syncthreads_and(ok ? 1 : 0) != 0;
+}
+
+template <int WIRE>
+__device__ __forceinline__ bool krum_reduce(const FedAvgKrumArgs& a, uint8_t* const* s_wire, const int* s_rank, int A,
+                                            int my_pos) {
+  extern __shared__ __align__(16) uint8_t robust_smem[];
+  uint32_t* stage = reinterpret_cast<uint32_t*>(robust_smem);
+  const uint8_t** src = reinterpret_cast<const uint8_t**>(robust_smem + ROBUST_STAGE * 4);
+  int* s_P = reinterpret_cast<int*>(robust_smem + ROBUST_STAGE * 4 + B200_MAX_ROBUST_CLIENTS * 8);
+  float* part = reinterpret_cast<float*>(robust_smem + KRUM_PART_OFF);
+  double* Dm = reinterpret_cast<double*>(robust_smem + KRUM_D_OFF);
+  double* score = reinterpret_cast<double*>(robust_smem + KRUM_SCORE_OFF);
+  int* kept = reinterpret_cast<int*>(robust_smem + KRUM_KEPT_OFF);
+  const int P = robust_gather(a, s_wire, s_rank, A, src, s_P);
+  constexpr int MC = B200_MAX_ROBUST_CLIENTS;
+  for (int i = threadIdx.x; i < MC * MC; i += FEDAVG_THREADS) Dm[i] = 0.0;
+  if (P > 2) {
+    const int npairs = P * (P - 1) / 2;
+    int pi = -1, pj = -1;
+    if (static_cast<int>(threadIdx.x) < npairs) krum_pair(threadIdx.x, P, pi, pj);
+    double acc;
+    if (P <= 8) acc = krum_distances<WIRE, 8>(a, src, stage, part, P, A, my_pos, pi, pj);
+    else if (P <= 16) acc = krum_distances<WIRE, 16>(a, src, stage, part, P, A, my_pos, pi, pj);
+    else acc = krum_distances<WIRE, 32>(a, src, stage, part, P, A, my_pos, pi, pj);
+    if (!krum_rank_reduce(a, acc, npairs, kept + MC)) return false;
+    if (!cta_barrier_all_ranks(a, a.epoch + 2, 0u, nullptr)) return false;
+    if (pi >= 0) {
+      double d = 0.0;
+      for (int k = 0; k < A; ++k) d += *reinterpret_cast<const volatile double*>(a.dist_page[s_rank[k]] + threadIdx.x);
+      if ((__double_as_longlong(d) & 0x7FF0000000000000ll) == 0x7FF0000000000000ll) d = __longlong_as_double(0x7FF0000000000000ll);
+      Dm[pi * MC + pj] = d;
+      Dm[pj * MC + pi] = d;
+    }
+  }
+  __syncthreads();
+  // score_i: the k smallest D[i][j], j != i, added in ascending order in fp64
+  const int kk = a.krum_k[P], m = a.krum_m[P];
+  if (static_cast<int>(threadIdx.x) < P) {
+    const int i = threadIdx.x;
+    uint32_t taken = 1u << i;
+    double acc = 0.0;
+    for (int t = 0; t < kk; ++t) {
+      int bj = -1;
+      double best = 0.0;
+      for (int j = 0; j < P; ++j)
+        if (!((taken >> j) & 1u) && (bj < 0 || Dm[i * MC + j] < best)) {
+          bj = j;
+          best = Dm[i * MC + j];
+        }
+      taken |= 1u << bj;
+      acc += best;
+    }
+    score[i] = acc;
+  }
+  __syncthreads();
+  if (static_cast<int>(threadIdx.x) < P) {
+    const int i = threadIdx.x;
+    int r = 0;
+    for (int j = 0; j < P; ++j) r += (score[j] < score[i] || (score[j] == score[i] && j < i)) ? 1 : 0;
+    kept[i] = r < m ? 1 : 0;
+  }
+  __syncthreads();
+  if (blockIdx.x == 0 && a.report != nullptr) {
+    for (int i = threadIdx.x; i < MC * MC; i += FEDAVG_THREADS) a.report[1 + i] = Dm[i];
+    if (static_cast<int>(threadIdx.x) < MC) {
+      a.report[1 + MC * MC + threadIdx.x] = static_cast<int>(threadIdx.x) < P ? score[threadIdx.x] : 0.0;
+      a.report[1 + MC * MC + MC + threadIdx.x] = static_cast<int>(threadIdx.x) < P ? kept[threadIdx.x] : 0;
+    }
+    if (threadIdx.x == 0) a.report[0] = P;
+  }
+  if (threadIdx.x == 0) {     // the kept segments, in segment order
+    int w = 0;
+    for (int i = 0; i < P; ++i)
+      if (kept[i]) src[w++] = src[i];
+  }
+  __syncthreads();
+  if (m <= 8) robust_tiles<WIRE, 8>(a, s_wire, src, stage, m, A, my_pos);
+  else if (m <= 16) robust_tiles<WIRE, 16>(a, s_wire, src, stage, m, A, my_pos);
+  else robust_tiles<WIRE, 32>(a, s_wire, src, stage, m, A, my_pos);
+  return true;
 }
 
 // DP: DP-FedAvg (see launch.h / DESIGN.md): w_k = n_k s_k / N with s_k from rank k's clip page, and the owner of a tile
@@ -549,8 +819,10 @@ __device__ __forceinline__ void robust_reduce(const FedAvgRobustArgs& a, uint8_t
 // SCAF: a SCAFFOLD round -- segment 1 (the control variates, see seg_pack) rides between the same barriers; every
 // participant weighs 1 / N there.
 // ROBUST: a robust round (robust_reduce above); every rank publishes its segment count before barrier 1.
-// The whole round; Args is FedAvgDPArgs when DP, FedAvgScaffoldArgs when SCAF, FedAvgRobustArgs when ROBUST.
-template <int WIRE, bool DP, bool SCAF = false, bool ROBUST = false, typename Args>
+// KRUM (with ROBUST): a Multi-Krum round (krum_reduce above): the exchange barrier takes epoch + 2, barrier 2 epoch + 3.
+// The whole round; Args is FedAvgDPArgs when DP, FedAvgScaffoldArgs when SCAF, FedAvgRobustArgs when ROBUST,
+// FedAvgKrumArgs when KRUM.
+template <int WIRE, bool DP, bool SCAF = false, bool ROBUST = false, bool KRUM = false, typename Args>
 __device__ __forceinline__ void fedavg_round(const Args& a) {
   static_assert(!(DP && SCAF), "DP-FedAvg and SCAFFOLD are exclusive");
   static_assert(!(ROBUST && (DP || SCAF)), "robust rounds exclude DP-FedAvg and SCAFFOLD");
@@ -800,7 +1072,9 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
       }
     }
   };
-  if constexpr (ROBUST) {
+  if constexpr (KRUM) {
+    if (!krum_reduce<WIRE>(a, s_wire, s_rank, A, my_pos)) return;
+  } else if constexpr (ROBUST) {
     robust_reduce<WIRE>(a, s_wire, s_rank, A, my_pos);
   } else if constexpr (SCAF) {
     // one wire vector per trip: the same sums in the same rank order as the wider trips, in fewer registers
@@ -825,7 +1099,7 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
     }
   }
   phase_stamp(a, 3);                                   // reduce + broadcast done
-  if (!cta_barrier_all_ranks(a, a.epoch + 2, 0u, nullptr)) return;
+  if (!cta_barrier_all_ranks(a, a.epoch + (KRUM ? 3 : 2), 0u, nullptr)) return;
   phase_stamp(a, 4);                                   // barrier 2 passed
 
   // ---------------------------------------------------------------- phase 2: running-mean apply
@@ -937,6 +1211,11 @@ __global__ void __maxnreg__(96) fedavg_allreduce_scaffold_kernel(const __grid_co
 template <int WIRE>
 __global__ void __maxnreg__(96) fedavg_allreduce_robust_kernel(const __grid_constant__ FedAvgRobustArgs a) {
   fedavg_round<WIRE, false, false, true>(a);
+}
+// Multi-Krum round: KRUM_SMEM bytes of dynamic shared memory, the same 96-register cap
+template <int WIRE>
+__global__ void __maxnreg__(96) fedavg_allreduce_krum_kernel(const __grid_constant__ FedAvgKrumArgs a) {
+  fedavg_round<WIRE, false, false, true, true>(a);
 }
 
 // one logical client's upload into its wire segment: the phase-0 pack of fedavg_round (delta mode, scale 1) over the
@@ -1088,15 +1367,16 @@ fold_client_scaled_kernel(float* __restrict__ acc, float* __restrict__ theta, co
 // (cudaErrorCooperativeLaunchTooLarge) and schedules all CTAs together, also next to work on other streams -- instead
 // of the plain <<<>>> of round 1, which was only safe on an otherwise idle GPU.  The grid is clamped to what
 // cudaOccupancyMaxActiveBlocksPerMultiprocessor allows on this device.
-template <int WIRE, bool DP, bool SCAF, typename Args, bool ROBUST = false>
+template <int WIRE, bool DP, bool SCAF, typename Args, bool ROBUST = false, bool KRUM = false>
 static int launch_fedavg(const Args* args, int n_ctas, cudaStream_t stream) {
   using namespace b200;
   static int max_ctas = -1;
-  const void* kernel = ROBUST ? reinterpret_cast<const void*>(fedavg_allreduce_robust_kernel<WIRE>)
+  const void* kernel = KRUM ? reinterpret_cast<const void*>(fedavg_allreduce_krum_kernel<WIRE>)
+                       : ROBUST ? reinterpret_cast<const void*>(fedavg_allreduce_robust_kernel<WIRE>)
                        : SCAF ? reinterpret_cast<const void*>(fedavg_allreduce_scaffold_kernel<WIRE>)
                        : DP ? reinterpret_cast<const void*>(fedavg_allreduce_dp_kernel<WIRE>)
                             : reinterpret_cast<const void*>(fedavg_allreduce_kernel<WIRE>);
-  const int smem = ROBUST ? ROBUST_SMEM : 0;
+  const int smem = KRUM ? KRUM_SMEM : ROBUST ? ROBUST_SMEM : 0;
   if (max_ctas < 0) {
     int dev = 0, sms = 0, per_sm = 0;
     cudaGetDevice(&dev);
@@ -1110,13 +1390,18 @@ static int launch_fedavg(const Args* args, int n_ctas, cudaStream_t stream) {
     if (max_ctas < 1) max_ctas = 1;
   }
   if (n_ctas > max_ctas) n_ctas = max_ctas;
+  if constexpr (KRUM) {
+    // the rank step's arrival counter and done flag start at zero every launch (also after a timed-out one)
+    cudaError_t e = cudaMemsetAsync(args->sync, 0, 2 * sizeof(unsigned int), stream);
+    if (e != cudaSuccess) return static_cast<int>(e);
+  }
   void* kargs[] = {const_cast<Args*>(args)};
   cudaError_t e = cudaLaunchCooperativeKernel(kernel, dim3(n_ctas), dim3(FEDAVG_THREADS), kargs, smem, stream);
   if (e != cudaSuccess) return static_cast<int>(e);
   return static_cast<int>(cudaGetLastError());
 }
 
-template <bool DP, bool SCAF, typename Args, bool ROBUST = false>
+template <bool DP, bool SCAF, typename Args, bool ROBUST = false, bool KRUM = false>
 static int fedavg_dispatch(const Args* args, int n_ctas, cudaStream_t stream) {
   using namespace b200;
   if (args->world > B200_MAX_RANKS || args->n % 8 != 0 || args->tile_elems % 8 != 0) return -2;
@@ -1125,10 +1410,10 @@ static int fedavg_dispatch(const Args* args, int n_ctas, cudaStream_t stream) {
   if (args->wire_kind == 2) {
     // block-scaled fp8 wire: 32-element blocks must not straddle tiles, and the switch cannot rescale
     if (args->tile_elems % 32 != 0 || args->use_nvls) return -2;
-    return launch_fedavg<2, DP, SCAF, Args, ROBUST>(args, n_ctas, stream);
+    return launch_fedavg<2, DP, SCAF, Args, ROBUST, KRUM>(args, n_ctas, stream);
   }
-  if (args->wire_kind == 1) return launch_fedavg<1, DP, SCAF, Args, ROBUST>(args, n_ctas, stream);
-  return launch_fedavg<0, DP, SCAF, Args, ROBUST>(args, n_ctas, stream);
+  if (args->wire_kind == 1) return launch_fedavg<1, DP, SCAF, Args, ROBUST, KRUM>(args, n_ctas, stream);
+  return launch_fedavg<0, DP, SCAF, Args, ROBUST, KRUM>(args, n_ctas, stream);
 }
 
 extern "C" int b200_fedavg_allreduce_robust(const FedAvgRobustArgs* args, int n_ctas, cudaStream_t stream) {
@@ -1139,6 +1424,20 @@ extern "C" int b200_fedavg_allreduce_robust(const FedAvgRobustArgs* args, int n_
   for (int k = 0; k < args->world; ++k)
     if (((args->alive_mask >> k) & 1u) && args->seg_page[k] == nullptr) return -2;
   return fedavg_dispatch<false, false, FedAvgRobustArgs, true>(args, n_ctas, stream);
+}
+
+extern "C" int b200_fedavg_allreduce_krum(const FedAvgKrumArgs* args, int n_ctas, cudaStream_t stream) {
+  // the kept mean is the trimmed mean with b = 0: the host passes kind 1 and a zero trim table
+  if (args->use_nvls || !args->delta || args->my_segs > B200_MAX_ROBUST_CLIENTS || args->seg_stride % 256 != 0 ||
+      args->kind != 1 || args->world > B200_MAX_RANKS || args->work == nullptr || args->sync == nullptr)
+    return -2;
+  for (int p = 0; p <= B200_MAX_ROBUST_CLIENTS; ++p)
+    if (args->trim_b[p] != 0 || args->krum_m[p] > p || (p > 0 && args->krum_m[p] < 1) || args->krum_k[p] >= (p > 0 ? p : 1))
+      return -2;
+  if (n_ctas > B200_KRUM_MAX_CTAS) n_ctas = B200_KRUM_MAX_CTAS;
+  for (int k = 0; k < args->world; ++k)
+    if (((args->alive_mask >> k) & 1u) && (args->seg_page[k] == nullptr || args->dist_page[k] == nullptr)) return -2;
+  return fedavg_dispatch<false, false, FedAvgKrumArgs, true, true>(args, n_ctas, stream);
 }
 
 extern "C" int b200_pack_client(void* seg, float* theta, const float* global_w, void* w_bf16, float* mom, long long n_mom,

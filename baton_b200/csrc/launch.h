@@ -197,8 +197,28 @@ struct FedAvgRobustArgs : FedAvgArgs {
   int kind;                         // 0: median, 1: trimmed mean
   uint8_t trim_b[B200_MAX_ROBUST_CLIENTS + 1];   // trimmed mean: b = floor(beta * P) for P = 0 .. 32 (host-computed)
 };
+// Multi-Krum round (fedavg_allreduce_krum_kernel<WIRE>): the robust round's segments and apply, with a selection of
+// whole clients in phase 1.  Every CTA adds the pair sums (x_i - x_j)^2 of its tiles into work[cta][pair]; the last CTA
+// of the rank (counter sync[0], zeroed by the launcher) adds them in CTA order into this rank's page dist_page[rank]
+// and raises sync[1]; after a per-CTA barrier at epoch + 2 every CTA adds the live ranks' pages in rank order, scores
+// every client by the krum_k[P] smallest distances (fp64, ascending), keeps the krum_m[P] lowest (score, position)
+// and runs the robust selection over the kept segments with kind = 1 (trimmed mean) and trim_b = 0.  Barrier 2 takes
+// epoch + 3, so a launch owns epoch+1 .. epoch+3 as every round does.  CTA 0 writes report: [0] = P, [1 + 32 i + j] =
+// D[i][j], [1 + 1024 + i] = score_i, [1 + 1024 + 32 + i] = 1 if client i is kept.
+#define B200_KRUM_PAIRS 496         // 32 * 31 / 2: one page / work slot of fp64 pair sums
+#define B200_KRUM_MAX_CTAS 296      // work slots; the launcher clamps the grid to it
+#define B200_KRUM_REPORT (1 + B200_MAX_ROBUST_CLIENTS * B200_MAX_ROBUST_CLIENTS + 2 * B200_MAX_ROBUST_CLIENTS)
+struct FedAvgKrumArgs : FedAvgRobustArgs {
+  double* dist_page[B200_MAX_RANKS];   // peer-mapped: this round's half of rank k's distance page (>= 496 doubles)
+  double* work;                     // local: [B200_KRUM_MAX_CTAS][B200_KRUM_PAIRS] per-CTA partial sums
+  unsigned int* sync;               // local: [2] arrival counter, done flag
+  double* report;                   // local: [B200_KRUM_REPORT] or nullptr
+  uint8_t krum_k[B200_MAX_ROBUST_CLIENTS + 1];   // neighbours per score for P = 0 .. 32 (host-computed)
+  uint8_t krum_m[B200_MAX_ROBUST_CLIENTS + 1];   // clients kept for P = 0 .. 32
+};
 int b200_fedavg_allreduce(const FedAvgArgs* args, int n_ctas, cudaStream_t stream);
 int b200_fedavg_allreduce_robust(const FedAvgRobustArgs* args, int n_ctas, cudaStream_t stream);   // delta, peer loads
+int b200_fedavg_allreduce_krum(const FedAvgKrumArgs* args, int n_ctas, cudaStream_t stream);       // delta, peer loads
 // one logical client's upload: seg = cast(theta - global_w) in wire format wire_kind (fp8: scales behind the n payload
 // bytes), exactly the collective's own pack; reset != 0 also returns the replica to the global model (theta, bf16
 // shadow, momentum [0, n_mom)) as b200_fold_client does.  n % 8 == 0, 16-byte aligned fp32 arrays.

@@ -74,10 +74,12 @@ def make_gpu_worker(app, model, host: str, port: int, cfg: FederationConfig):
     specs = (dirichlet_label_shards(world, cfg.num_classes, cfg.samples_per_client, cfg.alpha, cfg.seed)
              if cfg.partition == "dirichlet" else iid_label_shards(world, cfg.num_classes, cfg.samples_per_client))
     X, y = image_shard(specs[rank], seed=cfg.seed, dtype=torch.bfloat16, pin=True)
+    robust = cfg.robust_config()
     return GpuExperimentWorker(app, model, host, device=dev, shard_fn=lambda: (X, y), backend=cfg.backend,
                                wire_dtype=cfg.wire_dtype, momentum=cfg.momentum, port=port,
                                heartbeat_time=cfg.heartbeat_time,
-                               train_kwargs=cfg.train_kwargs())
+                               train_kwargs=cfg.train_kwargs(),
+                               robust=robust if robust is not None and robust.kind == "krum" else None)
 
 
 def make_app(role: str, host: str, port: int, cfg: Optional[FederationConfig] = None) -> web.Application:

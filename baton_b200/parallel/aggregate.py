@@ -164,11 +164,13 @@ def fedavg_loss_history(loss_histories: Sequence[Sequence[float]], n_samples: Se
 @torch.no_grad()
 def robust_into(global_state: Mapping[str, torch.Tensor], client_states: Sequence[Mapping[str, torch.Tensor]], cfg,
                 int_policy: str = "max") -> bool:
-    """Coordinate-wise median / trimmed mean (``parallel/robust.py``, ``cfg`` a ``RobustConfig``) written in place into
-    ``global_state``: every client's delta is its float entries minus the global ones in fp32, taken in
-    ``global_state`` order; ``global += robust_combine(deltas)``, unweighted over clients.  Integer entries follow
-    ``int_policy`` over all clients.  Returns False (and touches nothing) without clients."""
-    from .robust import check_participants, robust_combine
+    """Coordinate-wise median / trimmed mean or Multi-Krum (``parallel/robust.py``, ``cfg`` a ``RobustConfig``) written
+    in place into ``global_state``: every client's delta is its float entries minus the global ones in fp32, taken in
+    ``global_state`` order; ``global += robust_combine(deltas)``, unweighted over clients.  Krum's distances span every
+    float entry, so it takes two passes: the first selects the kept clients over the concatenated deltas, the second
+    applies their plain mean key by key.  Integer entries follow ``int_policy`` over all clients.  Returns False (and
+    touches nothing) without clients."""
+    from .robust import RobustConfig, check_participants, krum_select, robust_combine
     m = len(client_states)
     if m == 0:
         return False
@@ -177,12 +179,22 @@ def robust_into(global_state: Mapping[str, torch.Tensor], client_states: Sequenc
         missing = [k for k in global_state if k not in sd]
         if missing:
             raise KeyError("client state_dict is missing {!r}".format(missing[0]))
+    if cfg.kind == "krum":
+        floats = [k for k, g in global_state.items() if g.is_floating_point()]
+        flat = torch.cat([torch.stack([sd[k].detach().to(device="cpu", dtype=torch.float32).reshape(-1)
+                                       - global_state[k].detach().to(device="cpu", dtype=torch.float32).reshape(-1)
+                                       for sd in client_states]) for k in floats], 1)
+        kept = krum_select(flat, cfg)[2].tolist()
+        rows = [sd for sd, keep in zip(client_states, kept) if keep]
+        cfg = RobustConfig("trimmed_mean", 0.0)
+    else:
+        rows = client_states
     for k, g in global_state.items():
         if not g.is_floating_point():
             continue
         g32 = g.detach().to(device="cpu", dtype=torch.float32).reshape(-1)
         stack = torch.stack([sd[k].detach().to(device="cpu", dtype=torch.float32).reshape(-1) - g32
-                             for sd in client_states])
+                             for sd in rows])
         new = g32 + robust_combine(stack, cfg)
         g.copy_(new.reshape(g.shape).to(device=g.device, dtype=g.dtype))
     for k, v in global_state.items():

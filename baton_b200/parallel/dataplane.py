@@ -58,8 +58,8 @@ class HttpManagerPlane(ManagerPlane):
     not a participant; a round without participants aggregates nothing and does not advance the noise stream.
     ``last_clip_factors`` holds the factors of the last aggregated round.  ``robust`` (a
     :class:`~baton_b200.parallel.robust.RobustConfig`, exclusive with ``dp``): the coordinate-wise median / trimmed mean
-    of the participants' updates (:func:`~baton_b200.parallel.aggregate.robust_into`), uploads with ``n_samples == 0``
-    excluded as under DP."""
+    or the Multi-Krum mean of the participants' updates (:func:`~baton_b200.parallel.aggregate.robust_into`), uploads
+    with ``n_samples == 0`` excluded as under DP."""
 
     name = "http"
     carries_tensors = True
@@ -134,7 +134,7 @@ class SeatedManagerPlane(ManagerPlane):
                  dp=None, robust=None):
         if dp is not None and robust is not None:
             raise ValueError("robust aggregation with DP-FedAvg is not supported")
-        # robust (a RobustConfig): the plan carries {"robust": {kind, trim_ratio}}; every seat uploads one segment
+        # robust (a RobustConfig): the plan carries {"robust": RobustConfig.to_dict()}; every seat uploads one segment
         self.robust = robust
         self.name = name
         self.world_size = world_size
@@ -290,8 +290,7 @@ class SeatedWorkerPlane(WorkerPlane):
             kw["dp"] = DPConfig(float(d["clip"]), float(d["noise_multiplier"]), seed=int(d["seed"]))
         if plan.get("robust"):
             from .robust import RobustConfig
-            r = plan["robust"]
-            kw["robust"] = RobustConfig(str(r["kind"]), float(r["trim_ratio"]))
+            kw["robust"] = RobustConfig.from_dict(plan["robust"])
         self.session.aggregate(plan["n_samples_by_rank"], plan.get("alive_ranks"), **kw)
         check = getattr(self.session, "check", None)
         if check is not None:

@@ -30,7 +30,7 @@ from ..train import GraphedLocalSGD, PortableLocalSGD, check_adamw, check_optimi
 from .arena import ParamArena
 from .dp import DPConfig, RDPAccountant, check_dp, clip_factor
 from .fedavg import FedAvgSession, NcclSession
-from .robust import RobustConfig, check_aggregator, check_participants
+from .robust import RobustConfig, check_aggregator, check_krum_participants, check_participants
 from .scaffold import ScaffoldState
 
 
@@ -68,7 +68,8 @@ class FederatedEngine:
                  nvls: "bool | str" = "auto", tile_flags: bool = False, prox_mu: float = 0.0,
                  dp_clip: float = 0.0, dp_noise_multiplier: float = 0.0, dp_seed: Optional[int] = None,
                  scaffold: bool = False, optimizer: str = "sgd", betas: Tuple[float, float] = (0.9, 0.999),
-                 eps: float = 1e-8, aggregator: str = "mean", trim_ratio: float = 0.1):
+                 eps: float = 1e-8, aggregator: str = "mean", trim_ratio: float = 0.1, krum_f: int = 0,
+                 krum_m: Optional[int] = None):
         """``prox_mu > 0``: FedProx local training -- every step adds ``prox_mu * (theta - global_w)`` to the gradient,
         ``global_w`` being the global model the round started from (for logical clients too: each starts from it).
 
@@ -93,7 +94,13 @@ class FederatedEngine:
         round.  Every hosted participant uploads its own wire segment instead of being folded: ``S = min(ceil(L /
         world), sample_k or L)`` segments for ``L`` logical clients, which costs ``2 * S * wire bytes`` of symmetric
         memory per GPU (16 segments of a bf16 ResNet-18 are about 0.7 GB).  It cannot be combined with DP, SCAFFOLD,
-        ``mode='weights'`` or ``tile_flags``; FedProx, AdamW, momentum and the fp8 wire combine freely."""
+        ``mode='weights'`` or ``tile_flags``; FedProx, AdamW, momentum and the fp8 wire combine freely.
+
+        ``aggregator="krum"``: Multi-Krum -- each participant is scored by its summed squared distances to its nearest
+        ``P - krum_f - 2`` fellow participants, and the plain mean of the ``krum_m`` best-scoring updates (default ``P -
+        krum_f``; 1 is classic Krum) is applied.  The planned participants per round must number at least ``2 krum_f +
+        3``; a round with fewer still runs, with ``k`` and ``m`` clamped (``parallel/robust.py``).  The other robust
+        aggregators' rules and costs apply.  :meth:`last_krum` reports the last round's scores by client id."""
         prox_mu = check_prox_mu(prox_mu)
         adam = check_optimizer(optimizer, momentum, prox_mu=prox_mu)
         if adam:
@@ -113,7 +120,7 @@ class FederatedEngine:
                 raise ValueError("SCAFFOLD with tile_flags is not supported: the correction c - c_i reads c, which "
                                  "the previous round's collective writes, so it cannot run ahead of the join")
         trim_ratio = check_aggregator(aggregator, trim_ratio)
-        self.robust = RobustConfig(aggregator, trim_ratio) if aggregator != "mean" else None
+        self.robust = RobustConfig(aggregator, trim_ratio, krum_f, krum_m) if aggregator != "mean" else None
         if self.robust is not None:
             if dp_clip > 0.0:
                 raise ValueError("a robust aggregator with DP-FedAvg is not supported: DP's noise is calibrated to the "
@@ -149,7 +156,10 @@ class FederatedEngine:
         if self.robust is not None:
             world = self._group_size(group)
             population = logical_clients if logical_clients and logical_clients > world else world
-            check_participants(min(sample_k, population) if sample_k else population)
+            planned = min(sample_k, population) if sample_k else population
+            check_participants(planned)
+            if self.robust.kind == "krum":
+                check_krum_participants(planned, self.robust.krum_f)
             per_rank = -(-population // world) if population > world else 1
             robust_kw = {"robust": self.robust, "max_clients": min(per_rank, sample_k or population)}
         self.session = Session(self.arena, group, wire_dtype=wire_dtype, mode=mode, n_ctas=n_ctas, nvls=nvls,
@@ -179,6 +189,7 @@ class FederatedEngine:
         if adam:
             self.hp.update(optimizer=optimizer, betas=betas, eps=eps)
         self.n_rounds = 0
+        self._last_participants: Optional[List[int]] = None
         self.logical_clients = logical_clients if logical_clients and logical_clients > self.world else 0
         self.sample_k = sample_k
         self.scaf = ScaffoldState(self.arena.n_param, self.device) if scaffold else None
@@ -239,6 +250,7 @@ class FederatedEngine:
         that are staged first); with logical clients a callable ``client_id -> (X, y)``."""
         update_name = "update_{}_{:05d}".format(self.name, self.n_rounds)
         participants = self.draw_participants()
+        self._last_participants = participants
         mine = [c for c in participants if self.hosted(c)]
         a = self.arena
         total_n = 0
@@ -332,6 +344,20 @@ class FederatedEngine:
         if read_loss and losses_dev is not None:
             hist = loss_for_wire.tolist()       # device -> host read of the round's result
         return RoundResult(update_name, int(total_n), hist, participants)
+
+    def last_krum(self) -> Dict[int, Tuple[float, bool]]:
+        """``{client_id: (score, kept)}`` of the last Krum round's participants (a host read).  The session reports in
+        segment order -- live ranks in order, then each rank's hosted participants in draw order -- and every rank
+        knows the draw and who hosts whom, so every rank returns the same mapping."""
+        if self.robust is None or self.robust.kind != "krum":
+            raise RuntimeError("last_krum needs aggregator='krum'")
+        if self._last_participants is None:
+            raise RuntimeError("no round has run yet")
+        _, scores, kept = self.session.last_krum()
+        order = [c for r in range(self.world) for c in self._last_participants if c % self.world == r]
+        if len(order) != len(scores):
+            raise RuntimeError("the session reports {} clients, the round had {}".format(len(scores), len(order)))
+        return {c: (float(scores[i]), bool(kept[i])) for i, c in enumerate(order)}
 
     def _train_client(self, cid: int, X, y, n_epoch: int, first: bool):
         """Local training of client ``cid`` on the replica; with SCAFFOLD, its correction before and its control-variate

@@ -30,6 +30,10 @@ median of clients, so every hosted client uploads its own segment: ``max_clients
 fused session's wire as ``[seg 0 | pad | seg 1 | ... | seg S-1]`` (``S = 1`` is the plain layout), ``pack_client(j)``
 fills segment ``j`` and ``aggregate(..., n_clients=m)`` runs the robust kernel over the ``m`` segments of every rank
 (their counts travel in a per-rank page), always on peer loads.
+
+``robust=RobustConfig("krum", krum_f=f, krum_m=m)`` selects Multi-Krum: the fused session then also allocates a
+per-rank DISTANCE PAGE (4 KB per round parity) through which the ranks exchange their partial pair distances inside the
+collective, and :meth:`last_krum` returns the last round's distances, scores and kept clients in segment order.
 """
 from __future__ import annotations
 
@@ -39,7 +43,7 @@ import torch
 
 from .arena import ParamArena
 from .dp import DPConfig, clip_factor, normals
-from .robust import MAX_ROBUST_CLIENTS, RobustConfig, robust_combine
+from .robust import MAX_ROBUST_CLIENTS, RobustConfig, krum_select, robust_combine
 from .symm import SymmetricBuffer
 
 MAX_LOSS = 64       # per-epoch loss slots carried through the collective
@@ -115,6 +119,7 @@ class FedAvgSession:
         _check_scaffold(scaffold, dp, mode == "delta")
         self.max_clients = _check_robust(robust, dp, scaffold, mode == "delta", tile_flags, max_clients)
         self.robust = robust
+        self.krum = robust is not None and robust.kind == "krum"
         self.scaffold = bool(scaffold)
         self.arena = arena
         self.device = arena.device
@@ -144,11 +149,14 @@ class FedAvgSession:
         self.half_int = _align(max(arena.n_int, 1) * 8, 256)
         self.half_loss = _align(MAX_LOSS * 4, 256)
         self.half_clip = 256                                          # DP: this rank's clip factor s_r; robust: m_r
+        # Krum: this rank's fp64 pair distances of the round (496 at P = 32); only Krum sessions have the page
+        self.half_dist = _align(self._C.KRUM_PAIRS * 8, 4096) if self.krum else 0
         self.off_wire = 0
         self.off_int = 2 * self.half_wire
         self.off_loss = self.off_int + 2 * self.half_int
         self.off_clip = self.off_loss + 2 * self.half_loss
-        self.off_pads = _align(self.off_clip + 2 * self.half_clip, 256)
+        self.off_dist = self.off_clip + 2 * self.half_clip
+        self.off_pads = _align(self.off_dist + 2 * self.half_dist, 256)
         total = _align(self.off_pads + (MAX_CTAS + 8) * self._C.MAX_RANKS * 8, 2 << 20)
         self.symm = SymmetricBuffer(total, self.device, group)
         self.rank, self.world = self.symm.rank, self.symm.world
@@ -162,6 +170,11 @@ class FedAvgSession:
             # a sum: peer loads only
             self.use_nvls = False
         self._packed_epoch = None   # robust: barrier epoch whose wire half pack_client filled
+        if self.krum:   # the rank step's per-CTA partials and counters, and the host report (csrc/launch.h)
+            self.krum_work = torch.zeros(self._C.KRUM_MAX_CTAS * self._C.KRUM_PAIRS, dtype=torch.float64,
+                                         device=self.device)
+            self.krum_sync = torch.zeros(2, dtype=torch.int32, device=self.device)
+            self.krum_report = torch.zeros(self._C.KRUM_REPORT, dtype=torch.float64, device=self.device)
         # DP bookkeeping: norm-kernel partials, the last clip factor / norm of this rank, non-finite updates so far
         self.dp_work = torch.zeros(self._C.DP_WORK_WORDS, dtype=torch.int64, device=self.device)
         self.dp_s = torch.ones(1, dtype=torch.float32, device=self.device)
@@ -330,6 +343,9 @@ class FedAvgSession:
             _check_robust(robust, dp, self.scaffold, self.delta, self.tile_flags is not None, 1)
         if robust is None and n_clients is not None:
             raise ValueError("n_clients= needs a robust session or robust=")
+        if robust is not None and robust.kind == "krum" and not self.krum:
+            raise ValueError("a Krum round needs a session built with robust=RobustConfig('krum', ...): the ranks "
+                             "exchange their distances through a page only Krum sessions allocate")
         if round_index is not None:
             self.epoch = (self.base_epoch + 3 * int(round_index)) & 0xFFFFFFFF
         if n_samples_by_rank is not None:
@@ -393,6 +409,23 @@ class FedAvgSession:
             self.epoch_word.fill_(flag_value)       # compute stream: whatever is enqueued after this call waits for THIS round
         if on_side_stream:
             stream.wait_stream(cur)
+        if robust is not None and robust.kind == "krum":
+            o_dist = self.off_dist + par * self.half_dist
+            k_tab, m_tab = robust.krum_tables()
+            with torch.cuda.stream(stream):
+                self._C.fedavg_allreduce_krum(
+                    self.symm.peer_ptrs(o_wire), self.symm.peer_ptrs(self.off_pads),
+                    a.theta, a.global_w, a.theta_bf16, a.momentum if self.reset_momentum else None,
+                    a.int_arena if a.n_int > 0 else None, self.symm.peer_ptrs(o_int) if a.n_int > 0 else [],
+                    self.loss_local, self.symm.peer_ptrs(o_loss), self.loss_out,
+                    counts, from_flags, mask, self.rank, world, self.wire_kind, self.epoch, tile, self.n_ctas,
+                    self.timeout_log2, self.status, self.phase_ns, prepacked,
+                    self.symm.peer_ptrs(o_clip), m, self.seg_stride, self.symm.peer_ptrs(o_dist),
+                    self.krum_work, self.krum_sync, self.krum_report, k_tab, m_tab)
+            self.epoch = (self.epoch + 3) & 0xFFFFFFFF
+            self.rounds += 1
+            self._side_pending = on_side_stream
+            return
         if robust is not None:
             with torch.cuda.stream(stream):
                 self._C.fedavg_allreduce_robust(
@@ -440,6 +473,19 @@ class FedAvgSession:
         self.epoch = (self.epoch + 3) & 0xFFFFFFFF     # uint32 wrap: the kernel compares signed differences
         self.rounds += 1
         self._side_pending = on_side_stream
+
+    def last_krum(self):
+        """``(D, scores, kept)`` of the last Krum round, in segment order (a host read): the fp64 ``[P, P]`` squared
+        distances the collective computed (non-finite: +inf), the fp64 ``[P]`` scores and the bool ``[P]`` kept mask.
+        With ``P <= 2`` the collective skips the distances: ``D`` and the scores read 0 and the first ``m`` are kept."""
+        if not self.krum:
+            raise RuntimeError("last_krum needs a session built with robust=RobustConfig('krum', ...)")
+        self.join()
+        r = self.krum_report.cpu()
+        mc = MAX_ROBUST_CLIENTS
+        p = int(r[0])
+        D = r[1: 1 + mc * mc].view(mc, mc)[:p, :p].clone()
+        return D, r[1 + mc * mc: 1 + mc * mc + p].clone(), r[1 + mc * mc + mc: 1 + mc * mc + mc + p] != 0
 
     def dp_round(self) -> int:
         """Round index of the noise stream: ``(epoch - base_epoch) / 3``, identical on every rank (the plan's
@@ -537,6 +583,7 @@ class NcclSession:
         _check_scaffold(scaffold, dp, mode == "delta")
         self.max_clients = _check_robust(robust, dp, scaffold, mode == "delta", tile_flags, max_clients)
         self.robust = robust
+        self._last_krum = None
         self.scaffold = bool(scaffold)
         self.dist = dist
         self.arena, self.group, self.device = arena, group, arena.device
@@ -596,7 +643,18 @@ class NcclSession:
             all_m, all_s = [ms], [mine]
         rows = [sg[: int(mk)] for sg, mk in zip(all_s, all_m)]
         stacked = torch.cat(rows, 0) if rows else mine[:0]
+        if robust.kind == "krum":      # the same oracle, with the selection kept for last_krum()
+            self._last_krum = krum_select(stacked, robust)
+            stacked = stacked[self._last_krum[2].to(stacked.device)]
+            robust = RobustConfig("trimmed_mean", 0.0)
         return robust_combine(stacked, robust).to(self.wire_dtype).float()
+
+    def last_krum(self):
+        """``(D, scores, kept)`` of the last Krum round in segment order, as :meth:`FedAvgSession.last_krum` (here the
+        host oracle's fp64 values)."""
+        if self._last_krum is None:
+            raise RuntimeError("no Krum round has run on this session")
+        return self._last_krum
 
     @torch.no_grad()
     def aggregate(self, n_samples_by_rank=None, alive_ranks=None, my_n=None, loss_history=None,

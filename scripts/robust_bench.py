@@ -1,13 +1,17 @@
-"""Robust aggregation (coordinate-wise median / trimmed mean) on the flagship configuration: what it costs per round and
-what it does to accuracy under label-flipping clients.
+"""Robust aggregation (coordinate-wise median / trimmed mean, Multi-Krum) on the flagship configuration: what it costs
+per round and what it does to accuracy under label-flipping and model-poisoning clients.
 
 * round: ResNet-18, 1 GPU, one client, 4096 samples, batch 128, bf16 wire, 256 MiB L2 flush between rounds.  Engines with
   ``aggregator`` mean / median / trimmed_mean; blocks of device-timed rounds alternate between them (median + range).
 * logical: 16 logical clients of 512 samples on one GPU, 8 sampled per round (the tile owner selects over 8 segments),
-  mean against median.
-* collective: the robust kernel alone on ResNet-18's arena with P = 8, 16, 32 packed segments, against the plain one.
-* utility: 16 Dirichlet(0.1) clients, 8 per round, 15 rounds, 0 or 4 label-flipping attackers (their shards carry
-  permuted labels); held-out accuracy for mean / median / trimmed_mean (beta = 0.25).
+  mean against median and Multi-Krum (f = 2).
+* collective: the robust and Krum kernels alone on ResNet-18's arena with P = 8, 16, 32 packed segments, against the
+  plain one.
+* utility: 16 Dirichlet(0.1) clients, 8 per round, 15 rounds, held-out accuracy for mean / median / trimmed_mean
+  (beta = 0.25) / Multi-Krum (f = 2) with 0 attackers, 4 label-flipping attackers (their shards carry permuted labels)
+  and 4 model-poisoning attackers (they upload -POISON_SCALE times their honest delta).  The poisoned rounds are driven
+  here (train, rewrite theta, pack_client, aggregate) with every aggregator on a robust session; "mean" there is the
+  trimmed mean with beta = 0, the unweighted mean, equal to the weighted one because every client holds as many samples.
 
     python scripts/robust_bench.py [--reps 5] [--rounds-per-rep 5] [--parts round,logical,collective] [--skip-utility]
 
@@ -25,6 +29,8 @@ from fedprox_bench import card  # noqa: E402
 
 AGGS = (("mean", {}), ("median", {"aggregator": "median"}),
         ("trimmed_mean", {"aggregator": "trimmed_mean", "trim_ratio": 0.25}))
+KRUM = ("multi_krum", {"aggregator": "krum", "krum_f": 2})
+POISON_SCALE = 4.0
 
 
 def _alternate(torch, engines, run, reps, per_rep):
@@ -81,7 +87,7 @@ def logical_cost(args, torch, dev):
     specs = dirichlet_label_shards(16, 10, 512, alpha=0.5, seed=11)
     shards = {c: tuple(t.to(dev) for t in image_shard(specs[c], seed=3, dtype=torch.bfloat16)) for c in range(16)}
     engines = {}
-    for name, kw in AGGS[:2]:
+    for name, kw in AGGS[:2] + (KRUM,):
         torch.manual_seed(0)
         engines[name] = FederatedEngine(resnet18(10), dev, backend="fused", lr=0.05, batch_size=128, n_ctas=132,
                                         seed=5, logical_clients=16, sample_k=8, **kw)
@@ -105,7 +111,8 @@ def collective_cost(args, torch, dev):
     torch.manual_seed(0)
     arena = ParamArena(resnet18(10), dev, momentum=False)
     for label, cfg, P in [("mean", None, 1)] + [("median_P{}".format(p), RobustConfig("median"), p) for p in (8, 16, 32)] \
-            + [("trimmed_P{}".format(p), RobustConfig("trimmed_mean", 0.25), p) for p in (8, 32)]:
+            + [("trimmed_P{}".format(p), RobustConfig("trimmed_mean", 0.25), p) for p in (8, 32)] \
+            + [("krum_P{}".format(p), RobustConfig("krum", krum_f=2), p) for p in (8, 16, 32)]:
         sess = FedAvgSession(arena, wire_dtype="bf16", mode="delta", n_ctas=132, nvls=False, robust=cfg,
                              max_clients=P)
         ts = []
@@ -140,21 +147,44 @@ def utility(args, torch, dev):
     held = (Xe.to(dev), ye.to(dev))
     perm = torch.tensor([3, 7, 0, 9, 5, 1, 8, 2, 6, 4], device=dev)       # the attackers' label map
     table = {}
-    for n_bad in (0, 4):
-        shards = {c: (clean[c][0], perm[clean[c][1]] if c < n_bad else clean[c][1]) for c in range(n_clients)}
-        for name, kw in AGGS:
+
+    def poisoned_round(eng, n_bad):
+        """One round with every participant packed by hand; attackers upload -POISON_SCALE x their honest delta."""
+        a, sess = eng.arena, eng.session
+        parts = eng.draw_participants()
+        eng.sync()
+        for j, cid in enumerate(parts):
+            X, y = clean[cid]
+            eng.trainer.run(X, y, n_epoch=1, return_device=True, **eng.hp)
+            if cid < n_bad:
+                a.theta.copy_(a.global_w - POISON_SCALE * (a.theta - a.global_w))
+            sess.pack_client(j, reset=j + 1 < len(parts))
+        sess.aggregate(my_n=float(len(parts)), n_clients=len(parts))
+
+    for attack, n_bad in (("none", 0), ("label_flip", 4), ("model_poison", 4)):
+        shards = {c: (clean[c][0], perm[clean[c][1]] if c < n_bad and attack == "label_flip" else clean[c][1])
+                  for c in range(n_clients)}
+        for name, kw in AGGS + (KRUM,):
+            if attack == "model_poison" and name == "mean":
+                kw = {"aggregator": "trimmed_mean", "trim_ratio": 0.0}
             torch.manual_seed(0)
             eng = FederatedEngine(resnet18(10), dev, backend="fused", lr=0.05, batch_size=128,
                                   logical_clients=n_clients, sample_k=k, seed=5, **kw)
             for _ in range(args.utility_rounds):
-                eng.run_round(lambda c: shards[c], n_epoch=1, read_loss=False)
+                if attack == "model_poison":
+                    poisoned_round(eng, n_bad)
+                else:
+                    eng.run_round(lambda c: shards[c], n_epoch=1, read_loss=False)
+            eng.session.check()
             res = eng.evaluate(lambda c: held if c == 0 else None, batch_size=512)
-            table["attackers{}_{}".format(n_bad, name)] = round(res.accuracy, 4)
-            print("utility attackers={} {:<12} accuracy {:.4f}".format(n_bad, name, res.accuracy), flush=True)
+            table["{}{}_{}".format(attack, n_bad, name)] = round(res.accuracy, 4)
+            print("utility attack={} attackers={} {:<12} accuracy {:.4f}".format(attack, n_bad, name, res.accuracy),
+                  flush=True)
             del eng
             torch.cuda.empty_cache()
     return {"clients": n_clients, "sampled": k, "client_samples": args.client_samples, "alpha": 0.1,
-            "rounds": args.utility_rounds, "trim_ratio": 0.25, "heldout_accuracy": table}
+            "rounds": args.utility_rounds, "trim_ratio": 0.25, "krum_f": 2, "poison_scale": POISON_SCALE,
+            "heldout_accuracy": table}
 
 
 def main():
