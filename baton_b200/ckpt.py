@@ -6,7 +6,8 @@ The reference keeps the global model and ``loss_history`` only in manager RAM
 
     {"state_dict", "n_updates", "loss_history", "update_name", "name", "format"}
 
-with ``torch.save``.  ``state_dict`` is the plain PyTorch layout (name -> tensor
+with ``torch.save``, plus ``"server_opt": {"config", "m", "v"}`` when the experiment runs a server optimizer.
+``state_dict`` is the plain PyTorch layout (name -> tensor
 in module order), so ``torch.load(path)["state_dict"]`` drops straight into a
 stock ``nn.Module.load_state_dict`` -- the same layout the reference ships on
 the wire (manager.py:78).  Writes are atomic (tmp + rename) and the last
@@ -31,7 +32,8 @@ def _cpu_state_dict(model_or_sd) -> "OrderedDict[str, torch.Tensor]":
     return OrderedDict((k, v.detach().to("cpu").clone()) for k, v in sd.items())
 
 
-def save_checkpoint(directory: str, name: str, model, update_manager, *, keep: int = 3) -> str:
+def save_checkpoint(directory: str, name: str, model, update_manager, *, keep: int = 3,
+                    server_opt: Optional[dict] = None) -> str:
     os.makedirs(directory, exist_ok=True)
     snap = update_manager.snapshot()
     payload = {
@@ -42,6 +44,8 @@ def save_checkpoint(directory: str, name: str, model, update_manager, *, keep: i
         "loss_history": snap["loss_history"],
         "update_name": snap["update_name"],
     }
+    if server_opt is not None:
+        payload["server_opt"] = server_opt
     final = os.path.join(directory, "{}_{:05d}.pt".format(name, snap["n_updates"]))
     fd, tmp = tempfile.mkstemp(dir=directory, suffix=".tmp")
     os.close(fd)

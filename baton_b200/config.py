@@ -40,6 +40,11 @@ class FederationConfig:
     trim_ratio: float = 0.1            # trimmed_mean: fraction trimmed at each end, 0 <= beta < 0.5
     krum_f: int = 0                    # krum: Byzantine clients assumed (needs >= 2f + 3 participants per round)
     krum_m: Optional[int] = None       # krum: clients kept (None: participants - f; 1: classic Krum)
+    server_opt: str = "none"           # server optimizer on the aggregate: none | avgm | adagrad | yogi | adam
+    server_lr: Optional[float] = None  # server learning rate (required with a server optimizer; no default)
+    server_beta1: float = 0.9          # server optimizer decays and adaptivity floor (Reddi et al.'s defaults)
+    server_beta2: float = 0.99
+    server_tau: float = 1e-3
     partition: str = "iid"             # iid | label_skew | dirichlet
     alpha: float = 0.1                 # Dirichlet concentration
     samples_per_client: int = 4096
@@ -71,6 +76,12 @@ class FederationConfig:
             population = self.logical_clients if self.logical_clients > self.clients else self.clients
             check_krum_participants(min(self.sample_k, population) if self.sample_k else population, self.krum_f)
 
+        if self.server_opt != "none":
+            self.server_opt_config()          # validates kind, lr, betas and tau
+            if self.backend in ("fused", "nccl"):
+                from .parallel.dataplane import SEATED_SERVER_OPT
+                raise ValueError(SEATED_SERVER_OPT)
+
     def train_kwargs(self) -> dict:
         """Local-training keyword arguments of a worker (``FederatedModule.local_train``)."""
         kw = {"lr": self.lr, "batch_size": self.batch_size, "prox_mu": self.prox_mu}
@@ -92,6 +103,13 @@ class FederationConfig:
         from .parallel.robust import RobustConfig
         return RobustConfig(self.aggregator, self.trim_ratio, self.krum_f, self.krum_m)
 
+    def server_opt_config(self):
+        """The :class:`~baton_b200.parallel.server_opt.ServerOptConfig` of these fields, or None (``"none"``)."""
+        if self.server_opt == "none":
+            return None
+        from .parallel.server_opt import ServerOptConfig
+        return ServerOptConfig(self.server_opt, self.server_lr, self.server_beta1, self.server_beta2, self.server_tau)
+
     def to_json(self) -> str:
         return json.dumps(asdict(self), sort_keys=True)
 
@@ -112,7 +130,7 @@ class FederationConfig:
             typ = type(default) if default is not None else None
             if f.name in ("sample_k", "dp_seed", "krum_m"):
                 typ = int
-            if f.name in ("round_timeout",):
+            if f.name in ("round_timeout", "server_lr"):
                 typ = float
             if f.name in ("checkpoint_dir",):
                 typ = str

@@ -37,7 +37,7 @@ from .. import ckpt
 from ..metrics import RoundMetrics
 from ..parallel import wire
 from ..parallel.aggregate import fedavg_loss_history
-from ..parallel.dataplane import ManagerPlane, make_manager_plane
+from ..parallel.dataplane import HttpManagerPlane, ManagerPlane, make_manager_plane
 from ..parallel.dp import RDPAccountant
 from ..utils.misc import SYSTEM_CLOCK, Clock, json_clean
 from .client_manager import ClientManager
@@ -81,7 +81,7 @@ class Experiment:
                  sample_fraction: Optional[float] = None, seed: Optional[int] = None,
                  round_timeout: Optional[float] = None, checkpoint_dir: Optional[str] = None,
                  checkpoint_every: int = 1, resume: bool = False, clock: Clock = SYSTEM_CLOCK,
-                 trusted_peers: bool = False, dp=None, dp_delta: float = 1e-5, robust=None):
+                 trusted_peers: bool = False, dp=None, dp_delta: float = 1e-5, robust=None, server_opt=None):
         """``dp`` (a :class:`~baton_b200.parallel.dp.DPConfig`): aggregate with DP-FedAvg -- on the manager for the
         ``http`` plane, on the seats for the seated planes (the plan carries the clip norm, noise and key) -- and
         account every aggregated round at ``q`` = participants / registered clients; ``/metrics`` reports the
@@ -89,7 +89,12 @@ class Experiment:
 
         ``robust`` (a :class:`~baton_b200.parallel.robust.RobustConfig`): aggregate with the coordinate-wise median or
         trimmed mean of the participants' updates -- on the manager for the ``http`` plane, on the seats for the seated
-        planes (the plan carries it); ``/metrics`` reports the aggregator."""
+        planes (the plan carries it); ``/metrics`` reports the aggregator.
+
+        ``server_opt`` (a :class:`~baton_b200.parallel.server_opt.ServerOptConfig`, ``http`` plane only): the manager
+        steps the global parameters with FedAvgM / FedAdagrad / FedYogi / FedAdam on the round's aggregate; checkpoints
+        carry the optimizer state (``"server_opt"``; a file without it restores the initial state) and ``/metrics``
+        reports the optimizer.  The seated planes reject it."""
         self.name = name
         self.model = model
         self.app = app
@@ -98,8 +103,9 @@ class Experiment:
         self.update_manager = UpdateManager(name)
         if robust is not None and dp is not None:
             raise ValueError("robust aggregation with DP-FedAvg is not supported")
-        self.plane: ManagerPlane = make_manager_plane(dataplane, dp=dp, robust=robust)
+        self.plane: ManagerPlane = make_manager_plane(dataplane, dp=dp, robust=robust, server_opt=server_opt)
         self.robust = robust
+        self.server_opt = server_opt
         self.dp = dp
         self.dp_delta = float(dp_delta)
         self.dp_accountant = RDPAccountant(dp.noise_multiplier) if dp is not None else None
@@ -123,7 +129,10 @@ class Experiment:
         if resume and checkpoint_dir:
             path = ckpt.latest_checkpoint(checkpoint_dir, name)
             if path:
-                ckpt.load_checkpoint(path, self.model, self.update_manager)
+                payload = ckpt.load_checkpoint(path, self.model, self.update_manager)
+                if server_opt is not None:
+                    dev = next(self.model.parameters()).device
+                    self.plane.load_server_state(payload.get("server_opt"), device=dev)
                 self.last_checkpoint = path
                 log.info("resumed %s from %s (n_updates=%d)", name, path, self.update_manager.n_updates)
         app.on_cleanup.append(self._on_cleanup)
@@ -155,6 +164,7 @@ class Experiment:
         if self.dp is not None:
             out["dp"] = self.dp_summary()
         out["aggregator"] = self.robust.to_dict() if self.robust is not None else {"kind": "mean"}
+        out["server_opt"] = self.server_opt.to_dict() if self.server_opt is not None else {"kind": "none"}
         return web.json_response(json_clean(out))
 
     def dp_summary(self) -> dict:
@@ -452,10 +462,11 @@ class Experiment:
         if not self.checkpoint_dir:
             return None
         await self.pull_global()
+        sopt = self.plane.server_state() if isinstance(self.plane, HttpManagerPlane) else None   # this round's state
         loop = asyncio.get_running_loop()
         path = await loop.run_in_executor(
-            None, lambda: ckpt.save_checkpoint(self.checkpoint_dir, self.name, self.model,
-                                               self.update_manager))
+            None, lambda: ckpt.save_checkpoint(self.checkpoint_dir, self.name, self.model, self.update_manager,
+                                               server_opt=sopt))
         self.last_checkpoint = path
         return path
 

@@ -580,6 +580,37 @@ static void fill_fedavg_args(FedAvgArgs& a, const std::vector<int64_t>& wire_ptr
   }
 }
 
+// server optimizer (parallel/server_opt.py): m given -> the *_sopt kernel of the round, with the state over the first
+// n_param elements and the six fp32 coefficients
+static bool want_sopt(const std::optional<at::Tensor>& m) { return m.has_value() && m->defined(); }
+
+template <class Base>
+static ServerOptArgs<Base> sopt_args(const Base& a, const std::optional<at::Tensor>& m, const std::optional<at::Tensor>& v,
+                                     int64_t n_param, int64_t kind, const std::vector<double>& coef) {
+  TORCH_CHECK(kind >= 0 && kind <= 3, "server optimizer: kind in 0..3");
+  TORCH_CHECK(coef.size() == 6, "server optimizer: six coefficients");
+  TORCH_CHECK(n_param >= 0 && n_param % 8 == 0 && n_param <= a.n, "server optimizer: n_param % 8 == 0, <= n");
+  auto state_ok = [&](const at::Tensor& t) {
+    CHECK_CUDA(t);
+    TORCH_CHECK(t.scalar_type() == at::kFloat && t.is_contiguous() && t.numel() >= n_param,
+                "server optimizer: contiguous fp32 state covering the parameters");
+  };
+  state_ok(*m);
+  ServerOptArgs<Base> s = {};
+  static_cast<Base&>(s) = a;
+  s.m = m->data_ptr<float>();
+  s.v = nullptr;
+  if (kind != 0) {
+    TORCH_CHECK(v.has_value() && v->defined(), "server optimizer: this kind needs v");
+    state_ok(*v);
+    s.v = v->data_ptr<float>();
+  }
+  s.n_param = n_param;
+  s.kind = static_cast<int>(kind);
+  for (int i = 0; i < 6; ++i) s.coef[i] = static_cast<float>(coef[i]);
+  return s;
+}
+
 void fedavg_allreduce(const std::vector<int64_t>& wire_ptrs, const std::vector<int64_t>& pad_ptrs, int64_t wire_mc,
                       at::Tensor theta, const std::optional<at::Tensor>& global_w,
                       const std::optional<at::Tensor>& theta_bf16, const std::optional<at::Tensor>& momentum,
@@ -592,7 +623,9 @@ void fedavg_allreduce(const std::vector<int64_t>& wire_ptrs, const std::vector<i
                       const std::optional<at::Tensor>& status, const std::optional<at::Tensor>& phase_ns, bool prepacked,
                       const std::vector<int64_t>& clip_page_ptrs, double dp_noise_std, int64_t dp_seed, int64_t dp_round,
                       const std::optional<at::Tensor>& scaf_dc, const std::optional<at::Tensor>& scaf_c,
-                      int64_t scaf_seg1_off, double scaf_inv_clients) {
+                      int64_t scaf_seg1_off, double scaf_inv_clients,
+                      const std::optional<at::Tensor>& sopt_m, const std::optional<at::Tensor>& sopt_v,
+                      int64_t sopt_n_param, int64_t sopt_kind, const std::vector<double>& sopt_coef) {
   FedAvgDPArgs a = {};
   fill_fedavg_args(a, wire_ptrs, pad_ptrs, wire_mc, theta, global_w, theta_bf16, momentum, int_local, int_wire_ptrs,
                    loss_local, loss_wire_ptrs, loss_out, n_samples, counts_from_flags, alive_mask, rank, world, wire_kind,
@@ -623,7 +656,22 @@ void fedavg_allreduce(const std::vector<int64_t>& wire_ptrs, const std::vector<i
     sa.n_c = scaf_c->numel();
     sa.seg1_off = scaf_seg1_off;
     sa.inv_clients = static_cast<float>(scaf_inv_clients);
+    if (want_sopt(sopt_m)) {
+      const auto so = sopt_args(sa, sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
+      check(b200_fedavg_allreduce_scaffold_sopt(&so, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce");
+      return;
+    }
     check(b200_fedavg_allreduce_scaffold(&sa, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce");
+    return;
+  }
+  if (want_sopt(sopt_m)) {
+    if (dp) {
+      const auto so = sopt_args(a, sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
+      check(b200_fedavg_allreduce_dp_sopt(&so, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce");
+    } else {
+      const auto so = sopt_args(static_cast<const FedAvgArgs&>(a), sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
+      check(b200_fedavg_allreduce_sopt(&so, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce");
+    }
     return;
   }
   check(dp ? b200_fedavg_allreduce_dp(&a, static_cast<int>(n_ctas), cur_stream())
@@ -642,7 +690,9 @@ void fedavg_allreduce_robust(const std::vector<int64_t>& wire_ptrs, const std::v
                              int64_t timeout_log2, const std::optional<at::Tensor>& status,
                              const std::optional<at::Tensor>& phase_ns, bool prepacked,
                              const std::vector<int64_t>& seg_page_ptrs, int64_t my_segs, int64_t seg_stride, int64_t kind,
-                             const std::vector<int64_t>& trim_b) {
+                             const std::vector<int64_t>& trim_b,
+                             const std::optional<at::Tensor>& sopt_m, const std::optional<at::Tensor>& sopt_v,
+                             int64_t sopt_n_param, int64_t sopt_kind, const std::vector<double>& sopt_coef) {
   FedAvgRobustArgs a = {};
   fill_fedavg_args(a, wire_ptrs, pad_ptrs, 0, theta, global_w, theta_bf16, momentum, int_local, int_wire_ptrs, loss_local,
                    loss_wire_ptrs, loss_out, n_samples, counts_from_flags, alive_mask, rank, world, wire_kind, true, false,
@@ -659,6 +709,11 @@ void fedavg_allreduce_robust(const std::vector<int64_t>& wire_ptrs, const std::v
   a.seg_stride = seg_stride;
   a.kind = static_cast<int>(kind);
   const c10::cuda::CUDAGuard guard(theta.device());
+  if (want_sopt(sopt_m)) {
+    const auto so = sopt_args(a, sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
+    check(b200_fedavg_allreduce_robust_sopt(&so, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_robust");
+    return;
+  }
   check(b200_fedavg_allreduce_robust(&a, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_robust");
 }
 
@@ -676,7 +731,9 @@ void fedavg_allreduce_krum(const std::vector<int64_t>& wire_ptrs, const std::vec
                            const std::vector<int64_t>& seg_page_ptrs, int64_t my_segs, int64_t seg_stride,
                            const std::vector<int64_t>& dist_page_ptrs, at::Tensor work, at::Tensor sync,
                            const std::optional<at::Tensor>& report, const std::vector<int64_t>& krum_k,
-                           const std::vector<int64_t>& krum_m) {
+                           const std::vector<int64_t>& krum_m,
+                           const std::optional<at::Tensor>& sopt_m, const std::optional<at::Tensor>& sopt_v,
+                           int64_t sopt_n_param, int64_t sopt_kind, const std::vector<double>& sopt_coef) {
   FedAvgKrumArgs a = {};
   fill_fedavg_args(a, wire_ptrs, pad_ptrs, 0, theta, global_w, theta_bf16, momentum, int_local, int_wire_ptrs, loss_local,
                    loss_wire_ptrs, loss_out, n_samples, counts_from_flags, alive_mask, rank, world, wire_kind, true, false,
@@ -717,6 +774,11 @@ void fedavg_allreduce_krum(const std::vector<int64_t>& wire_ptrs, const std::vec
     a.report = report->data_ptr<double>();
   }
   const c10::cuda::CUDAGuard guard(theta.device());
+  if (want_sopt(sopt_m)) {
+    const auto so = sopt_args(a, sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
+    check(b200_fedavg_allreduce_krum_sopt(&so, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_krum");
+    return;
+  }
   check(b200_fedavg_allreduce_krum(&a, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_krum");
 }
 

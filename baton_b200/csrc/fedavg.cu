@@ -814,15 +814,88 @@ __device__ __forceinline__ bool krum_reduce(const FedAvgKrumArgs& a, uint8_t* co
   return true;
 }
 
+// ---------------------------------------------------------------- server optimizer (see launch.h / parallel/server_opt.py)
+// one element: the state update, then the model update, each operation rounded separately (no FMA contraction)
+__device__ __forceinline__ float sopt_step(float x, float d, float& m, float& v, int kind, const float* c) {
+  if (kind == 0) {
+    m = __fadd_rn(__fmul_rn(c[0], m), d);
+    return __fadd_rn(x, __fmul_rn(c[4], m));
+  }
+  m = __fadd_rn(__fmul_rn(c[0], m), __fmul_rn(c[1], d));
+  const float dd = __fmul_rn(d, d);
+  if (kind == 1) {
+    v = __fadd_rn(v, dd);
+  } else if (kind == 2) {
+    const float s = __fsub_rn(v, dd);
+    v = __fsub_rn(v, __fmul_rn(__fmul_rn(c[3], dd), s > 0.f ? 1.f : (s < 0.f ? -1.f : 0.f)));
+  } else {
+    v = __fadd_rn(__fmul_rn(c[2], v), __fmul_rn(c[3], dd));
+  }
+  return __fadd_rn(x, __fdiv_rn(__fmul_rn(c[4], m), __fadd_rn(__fsqrt_rn(v), c[5])));
+}
+
+// the apply phase of one tile in a server-optimizer round: ONE wire vector per trip (the plain loop's two, plus m and v,
+// would not fit under the 96-register cap).  Parameter vectors (n_param % 8 == 0: a vector never straddles it) take
+// the step, or keep the global model when the round had no weight (step == false); buffers take global += d as in the
+// plain loop.  Then theta, the bf16 shadow and the momentum reset, as there.
+template <int WIRE, typename Args>
+__device__ __forceinline__ void sopt_apply_tile(const Args& a, const uint8_t* my_wire, long long base, int len,
+                                                float apply_scale, bool step) {
+  using W = Wire<WIRE>;
+  constexpr int VEC = W::VEC;
+  constexpr size_t esz = W::VBYTES / VEC;
+  const size_t sc_off = static_cast<size_t>(a.n);
+  for (int i = threadIdx.x * VEC; i < len; i += FEDAVG_THREADS * VEC) {
+    const long long e = base + i;
+    const uint4 wv = W::ld(my_wire + e * esz);
+    float scale = 1.f;
+    if constexpr (W::SCALED) scale = exp2_int(static_cast<int>(ld_volatile_u8(my_wire + sc_off + (e >> 5))) - 127);
+    float f[VEC];
+    W::unpack(wv, f, scale);
+    const bool opt = e < a.n_param;
+#pragma unroll
+    for (int j = 0; j < VEC; j += 4) {
+      const float4 g = *reinterpret_cast<const float4*>(a.global_w + e + j);
+      float4 nw = g;
+      if (opt) {
+        if (step) {
+          float4 m4 = *reinterpret_cast<const float4*>(a.m + e + j);
+          float4 v4 = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (a.kind != 0) v4 = *reinterpret_cast<const float4*>(a.v + e + j);
+          nw.x = sopt_step(g.x, __fmul_rn(f[j], apply_scale), m4.x, v4.x, a.kind, a.coef);
+          nw.y = sopt_step(g.y, __fmul_rn(f[j + 1], apply_scale), m4.y, v4.y, a.kind, a.coef);
+          nw.z = sopt_step(g.z, __fmul_rn(f[j + 2], apply_scale), m4.z, v4.z, a.kind, a.coef);
+          nw.w = sopt_step(g.w, __fmul_rn(f[j + 3], apply_scale), m4.w, v4.w, a.kind, a.coef);
+          *reinterpret_cast<float4*>(a.m + e + j) = m4;
+          if (a.kind != 0) *reinterpret_cast<float4*>(a.v + e + j) = v4;
+        }
+      } else {
+        nw = make_float4(f[j] * apply_scale + g.x, f[j + 1] * apply_scale + g.y, f[j + 2] * apply_scale + g.z,
+                         f[j + 3] * apply_scale + g.w);
+      }
+      *reinterpret_cast<float4*>(a.global_w + e + j) = nw;
+      *reinterpret_cast<float4*>(a.theta + e + j) = nw;
+      if (a.momentum != nullptr && e + j < a.n_momentum)
+        *reinterpret_cast<float4*>(a.momentum + e + j) = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (a.theta_bf16 != nullptr) {
+        const uint2 o = make_uint2(pack_bf16x2(nw.x, nw.y), pack_bf16x2(nw.z, nw.w));
+        *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(a.theta_bf16) + (e + j) * 2) = o;
+      }
+    }
+  }
+}
+
 // DP: DP-FedAvg (see launch.h / DESIGN.md): w_k = n_k s_k / N with s_k from rank k's clip page, and the owner of a tile
 // adds sigma C / N * z[i] to its fp32 sum before the cast.  The loss and the integer side arena keep the weights n_k / N.
 // SCAF: a SCAFFOLD round -- segment 1 (the control variates, see seg_pack) rides between the same barriers; every
 // participant weighs 1 / N there.
 // ROBUST: a robust round (robust_reduce above); every rank publishes its segment count before barrier 1.
 // KRUM (with ROBUST): a Multi-Krum round (krum_reduce above): the exchange barrier takes epoch + 2, barrier 2 epoch + 3.
+// SOPT (with any of the above): a server-optimizer round -- the apply phase runs sopt_apply_tile.
 // The whole round; Args is FedAvgDPArgs when DP, FedAvgScaffoldArgs when SCAF, FedAvgRobustArgs when ROBUST,
-// FedAvgKrumArgs when KRUM.
-template <int WIRE, bool DP, bool SCAF = false, bool ROBUST = false, bool KRUM = false, typename Args>
+// FedAvgKrumArgs when KRUM, and ServerOptArgs<that> when SOPT.
+template <int WIRE, bool DP, bool SCAF = false, bool ROBUST = false, bool KRUM = false, bool SOPT = false,
+          typename Args>
 __device__ __forceinline__ void fedavg_round(const Args& a) {
   static_assert(!(DP && SCAF), "DP-FedAvg and SCAFFOLD are exclusive");
   static_assert(!(ROBUST && (DP || SCAF)), "robust rounds exclude DP-FedAvg and SCAFFOLD");
@@ -1079,6 +1152,11 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
   } else if constexpr (SCAF) {
     // one wire vector per trip: the same sums in the same rank order as the wider trips, in fewer registers
     reduce_tiles(std::integral_constant<int, 1>{});
+  } else if constexpr (SOPT) {
+    // at most two vectors per trip (one with DP's noise): with more, the server-optimizer kernels spill (the same sums
+    // in the same order)
+    if (!DP && A <= 4) reduce_tiles(std::integral_constant<int, 2>{});
+    else reduce_tiles(std::integral_constant<int, 1>{});
   } else {
     if (A <= 2) reduce_tiles(std::integral_constant<int, 4>{});
     else if (A <= 4) reduce_tiles(std::integral_constant<int, 2>{});
@@ -1112,7 +1190,8 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
       const long long base = t * T;
       const int len = static_cast<int>((n - base) < T ? (n - base) : T);
       constexpr int STEP = FEDAVG_THREADS * VEC;
-      for (int i0 = threadIdx.x * VEC; i0 < len; i0 += 2 * STEP) {
+      if constexpr (SOPT) sopt_apply_tile<WIRE>(a, my_wire, base, len, apply_scale, s_inv_total != 0.f);
+      else for (int i0 = threadIdx.x * VEC; i0 < len; i0 += 2 * STEP) {
         uint4 wv[2];
         uint32_t sc[2];
         float4 gg[2][VEC / 4];
@@ -1216,6 +1295,29 @@ __global__ void __maxnreg__(96) fedavg_allreduce_robust_kernel(const __grid_cons
 template <int WIRE>
 __global__ void __maxnreg__(96) fedavg_allreduce_krum_kernel(const __grid_constant__ FedAvgKrumArgs a) {
   fedavg_round<WIRE, false, false, true, true>(a);
+}
+// the same five rounds with the server optimizer in the apply phase (kind chosen at run time: one branch per launch)
+template <int WIRE>
+__global__ void __maxnreg__(96) fedavg_allreduce_sopt_kernel(const __grid_constant__ ServerOptArgs<FedAvgArgs> a) {
+  fedavg_round<WIRE, false, false, false, false, true>(a);
+}
+template <int WIRE>
+__global__ void __maxnreg__(96) fedavg_allreduce_dp_sopt_kernel(const __grid_constant__ ServerOptArgs<FedAvgDPArgs> a) {
+  fedavg_round<WIRE, true, false, false, false, true>(a);
+}
+template <int WIRE>
+__global__ void __maxnreg__(96)
+fedavg_allreduce_scaffold_sopt_kernel(const __grid_constant__ ServerOptArgs<FedAvgScaffoldArgs> a) {
+  fedavg_round<WIRE, false, true, false, false, true>(a);
+}
+template <int WIRE>
+__global__ void __maxnreg__(96)
+fedavg_allreduce_robust_sopt_kernel(const __grid_constant__ ServerOptArgs<FedAvgRobustArgs> a) {
+  fedavg_round<WIRE, false, false, true, false, true>(a);
+}
+template <int WIRE>
+__global__ void __maxnreg__(96) fedavg_allreduce_krum_sopt_kernel(const __grid_constant__ ServerOptArgs<FedAvgKrumArgs> a) {
+  fedavg_round<WIRE, false, false, true, true, true>(a);
 }
 
 // one logical client's upload into its wire segment: the phase-0 pack of fedavg_round (delta mode, scale 1) over the
@@ -1367,15 +1469,29 @@ fold_client_scaled_kernel(float* __restrict__ acc, float* __restrict__ theta, co
 // (cudaErrorCooperativeLaunchTooLarge) and schedules all CTAs together, also next to work on other streams -- instead
 // of the plain <<<>>> of round 1, which was only safe on an otherwise idle GPU.  The grid is clamped to what
 // cudaOccupancyMaxActiveBlocksPerMultiprocessor allows on this device.
-template <int WIRE, bool DP, bool SCAF, typename Args, bool ROBUST = false, bool KRUM = false>
+template <int WIRE, bool DP, bool SCAF, bool ROBUST, bool KRUM, bool SOPT>
+static const void* fedavg_kernel() {
+  using namespace b200;
+  if constexpr (SOPT) {
+    if constexpr (KRUM) return reinterpret_cast<const void*>(fedavg_allreduce_krum_sopt_kernel<WIRE>);
+    else if constexpr (ROBUST) return reinterpret_cast<const void*>(fedavg_allreduce_robust_sopt_kernel<WIRE>);
+    else if constexpr (SCAF) return reinterpret_cast<const void*>(fedavg_allreduce_scaffold_sopt_kernel<WIRE>);
+    else if constexpr (DP) return reinterpret_cast<const void*>(fedavg_allreduce_dp_sopt_kernel<WIRE>);
+    else return reinterpret_cast<const void*>(fedavg_allreduce_sopt_kernel<WIRE>);
+  } else {
+    return KRUM ? reinterpret_cast<const void*>(fedavg_allreduce_krum_kernel<WIRE>)
+           : ROBUST ? reinterpret_cast<const void*>(fedavg_allreduce_robust_kernel<WIRE>)
+           : SCAF ? reinterpret_cast<const void*>(fedavg_allreduce_scaffold_kernel<WIRE>)
+           : DP ? reinterpret_cast<const void*>(fedavg_allreduce_dp_kernel<WIRE>)
+                : reinterpret_cast<const void*>(fedavg_allreduce_kernel<WIRE>);
+  }
+}
+
+template <int WIRE, bool DP, bool SCAF, typename Args, bool ROBUST = false, bool KRUM = false, bool SOPT = false>
 static int launch_fedavg(const Args* args, int n_ctas, cudaStream_t stream) {
   using namespace b200;
   static int max_ctas = -1;
-  const void* kernel = KRUM ? reinterpret_cast<const void*>(fedavg_allreduce_krum_kernel<WIRE>)
-                       : ROBUST ? reinterpret_cast<const void*>(fedavg_allreduce_robust_kernel<WIRE>)
-                       : SCAF ? reinterpret_cast<const void*>(fedavg_allreduce_scaffold_kernel<WIRE>)
-                       : DP ? reinterpret_cast<const void*>(fedavg_allreduce_dp_kernel<WIRE>)
-                            : reinterpret_cast<const void*>(fedavg_allreduce_kernel<WIRE>);
+  const void* kernel = fedavg_kernel<WIRE, DP, SCAF, ROBUST, KRUM, SOPT>();
   const int smem = KRUM ? KRUM_SMEM : ROBUST ? ROBUST_SMEM : 0;
   if (max_ctas < 0) {
     int dev = 0, sms = 0, per_sm = 0;
@@ -1401,7 +1517,7 @@ static int launch_fedavg(const Args* args, int n_ctas, cudaStream_t stream) {
   return static_cast<int>(cudaGetLastError());
 }
 
-template <bool DP, bool SCAF, typename Args, bool ROBUST = false, bool KRUM = false>
+template <bool DP, bool SCAF, typename Args, bool ROBUST = false, bool KRUM = false, bool SOPT = false>
 static int fedavg_dispatch(const Args* args, int n_ctas, cudaStream_t stream) {
   using namespace b200;
   if (args->world > B200_MAX_RANKS || args->n % 8 != 0 || args->tile_elems % 8 != 0) return -2;
@@ -1410,34 +1526,95 @@ static int fedavg_dispatch(const Args* args, int n_ctas, cudaStream_t stream) {
   if (args->wire_kind == 2) {
     // block-scaled fp8 wire: 32-element blocks must not straddle tiles, and the switch cannot rescale
     if (args->tile_elems % 32 != 0 || args->use_nvls) return -2;
-    return launch_fedavg<2, DP, SCAF, Args, ROBUST, KRUM>(args, n_ctas, stream);
+    return launch_fedavg<2, DP, SCAF, Args, ROBUST, KRUM, SOPT>(args, n_ctas, stream);
   }
-  if (args->wire_kind == 1) return launch_fedavg<1, DP, SCAF, Args, ROBUST, KRUM>(args, n_ctas, stream);
-  return launch_fedavg<0, DP, SCAF, Args, ROBUST, KRUM>(args, n_ctas, stream);
+  if (args->wire_kind == 1) return launch_fedavg<1, DP, SCAF, Args, ROBUST, KRUM, SOPT>(args, n_ctas, stream);
+  return launch_fedavg<0, DP, SCAF, Args, ROBUST, KRUM, SOPT>(args, n_ctas, stream);
 }
 
-extern "C" int b200_fedavg_allreduce_robust(const FedAvgRobustArgs* args, int n_ctas, cudaStream_t stream) {
+static bool robust_args_ok(const FedAvgRobustArgs* args) {
   // a selection is not a sum: robust rounds run on peer loads, never on the switch
   if (args->use_nvls || !args->delta || args->my_segs > B200_MAX_ROBUST_CLIENTS || args->seg_stride % 256 != 0 ||
       (args->kind != 0 && args->kind != 1) || args->world > B200_MAX_RANKS)
-    return -2;
+    return false;
   for (int k = 0; k < args->world; ++k)
-    if (((args->alive_mask >> k) & 1u) && args->seg_page[k] == nullptr) return -2;
+    if (((args->alive_mask >> k) & 1u) && args->seg_page[k] == nullptr) return false;
+  return true;
+}
+
+static bool krum_args_ok(const FedAvgKrumArgs* args) {
+  // the kept mean is the trimmed mean with b = 0: the host passes kind 1 and a zero trim table
+  if (args->use_nvls || !args->delta || args->my_segs > B200_MAX_ROBUST_CLIENTS || args->seg_stride % 256 != 0 ||
+      args->kind != 1 || args->world > B200_MAX_RANKS || args->work == nullptr || args->sync == nullptr)
+    return false;
+  for (int p = 0; p <= B200_MAX_ROBUST_CLIENTS; ++p)
+    if (args->trim_b[p] != 0 || args->krum_m[p] > p || (p > 0 && args->krum_m[p] < 1) || args->krum_k[p] >= (p > 0 ? p : 1))
+      return false;
+  for (int k = 0; k < args->world; ++k)
+    if (((args->alive_mask >> k) & 1u) && (args->seg_page[k] == nullptr || args->dist_page[k] == nullptr)) return false;
+  return true;
+}
+
+static bool dp_args_ok(const FedAvgDPArgs* args) {
+  // the switch adds the raw wire values, but the clip factors are applied on the reader side: DP runs on peer loads
+  if (args->use_nvls || !args->delta || args->world > B200_MAX_RANKS) return false;
+  for (int k = 0; k < args->world; ++k)
+    if (((args->alive_mask >> k) & 1u) && args->clip_page[k] == nullptr) return false;
+  return true;
+}
+
+static bool scaffold_args_ok(const FedAvgScaffoldArgs* args) {
+  // 1 / N weighs every participant's raw wire value on the reader side: SCAFFOLD runs on peer loads
+  return !(args->use_nvls || !args->delta || args->dc == nullptr || args->c == nullptr || args->n_c <= 0 ||
+           args->n_c % 8 != 0 || args->seg1_off % 16 != 0);
+}
+
+// the server step needs the pseudo-gradient (delta mode), the global copy and the state over [0, n_param)
+template <class Base>
+static bool sopt_args_ok(const ServerOptArgs<Base>* args) {
+  return args->delta && args->global_w != nullptr && args->m != nullptr && args->kind >= 0 && args->kind <= 3 &&
+         (args->kind == 0 || args->v != nullptr) && args->n_param >= 0 && args->n_param % 8 == 0 &&
+         args->n_param <= args->n;
+}
+
+extern "C" int b200_fedavg_allreduce_robust(const FedAvgRobustArgs* args, int n_ctas, cudaStream_t stream) {
+  if (!robust_args_ok(args)) return -2;
   return fedavg_dispatch<false, false, FedAvgRobustArgs, true>(args, n_ctas, stream);
 }
 
 extern "C" int b200_fedavg_allreduce_krum(const FedAvgKrumArgs* args, int n_ctas, cudaStream_t stream) {
-  // the kept mean is the trimmed mean with b = 0: the host passes kind 1 and a zero trim table
-  if (args->use_nvls || !args->delta || args->my_segs > B200_MAX_ROBUST_CLIENTS || args->seg_stride % 256 != 0 ||
-      args->kind != 1 || args->world > B200_MAX_RANKS || args->work == nullptr || args->sync == nullptr)
-    return -2;
-  for (int p = 0; p <= B200_MAX_ROBUST_CLIENTS; ++p)
-    if (args->trim_b[p] != 0 || args->krum_m[p] > p || (p > 0 && args->krum_m[p] < 1) || args->krum_k[p] >= (p > 0 ? p : 1))
-      return -2;
+  if (!krum_args_ok(args)) return -2;
   if (n_ctas > B200_KRUM_MAX_CTAS) n_ctas = B200_KRUM_MAX_CTAS;
-  for (int k = 0; k < args->world; ++k)
-    if (((args->alive_mask >> k) & 1u) && (args->seg_page[k] == nullptr || args->dist_page[k] == nullptr)) return -2;
   return fedavg_dispatch<false, false, FedAvgKrumArgs, true, true>(args, n_ctas, stream);
+}
+
+extern "C" int b200_fedavg_allreduce_sopt(const ServerOptArgs<FedAvgArgs>* args, int n_ctas, cudaStream_t stream) {
+  if (!sopt_args_ok(args)) return -2;
+  return fedavg_dispatch<false, false, ServerOptArgs<FedAvgArgs>, false, false, true>(args, n_ctas, stream);
+}
+
+extern "C" int b200_fedavg_allreduce_dp_sopt(const ServerOptArgs<FedAvgDPArgs>* args, int n_ctas, cudaStream_t stream) {
+  if (!sopt_args_ok(args) || !dp_args_ok(args)) return -2;
+  return fedavg_dispatch<true, false, ServerOptArgs<FedAvgDPArgs>, false, false, true>(args, n_ctas, stream);
+}
+
+extern "C" int b200_fedavg_allreduce_scaffold_sopt(const ServerOptArgs<FedAvgScaffoldArgs>* args, int n_ctas,
+                                                   cudaStream_t stream) {
+  if (!sopt_args_ok(args) || !scaffold_args_ok(args)) return -2;
+  return fedavg_dispatch<false, true, ServerOptArgs<FedAvgScaffoldArgs>, false, false, true>(args, n_ctas, stream);
+}
+
+extern "C" int b200_fedavg_allreduce_robust_sopt(const ServerOptArgs<FedAvgRobustArgs>* args, int n_ctas,
+                                                 cudaStream_t stream) {
+  if (!sopt_args_ok(args) || !robust_args_ok(args)) return -2;
+  return fedavg_dispatch<false, false, ServerOptArgs<FedAvgRobustArgs>, true, false, true>(args, n_ctas, stream);
+}
+
+extern "C" int b200_fedavg_allreduce_krum_sopt(const ServerOptArgs<FedAvgKrumArgs>* args, int n_ctas,
+                                               cudaStream_t stream) {
+  if (!sopt_args_ok(args) || !krum_args_ok(args)) return -2;
+  if (n_ctas > B200_KRUM_MAX_CTAS) n_ctas = B200_KRUM_MAX_CTAS;
+  return fedavg_dispatch<false, false, ServerOptArgs<FedAvgKrumArgs>, true, true, true>(args, n_ctas, stream);
 }
 
 extern "C" int b200_pack_client(void* seg, float* theta, const float* global_w, void* w_bf16, float* mom, long long n_mom,
@@ -1467,18 +1644,12 @@ extern "C" int b200_fedavg_allreduce(const FedAvgArgs* args, int n_ctas, cudaStr
 }
 
 extern "C" int b200_fedavg_allreduce_dp(const FedAvgDPArgs* args, int n_ctas, cudaStream_t stream) {
-  // the switch adds the raw wire values, but the clip factors are applied on the reader side: DP runs on peer loads
-  if (args->use_nvls || !args->delta || args->world > B200_MAX_RANKS) return -2;
-  for (int k = 0; k < args->world; ++k)
-    if (((args->alive_mask >> k) & 1u) && args->clip_page[k] == nullptr) return -2;
+  if (!dp_args_ok(args)) return -2;
   return fedavg_dispatch<true, false>(args, n_ctas, stream);
 }
 
 extern "C" int b200_fedavg_allreduce_scaffold(const FedAvgScaffoldArgs* args, int n_ctas, cudaStream_t stream) {
-  // 1 / N weighs every participant's raw wire value on the reader side: SCAFFOLD runs on peer loads
-  if (args->use_nvls || !args->delta || args->dc == nullptr || args->c == nullptr || args->n_c <= 0 ||
-      args->n_c % 8 != 0 || args->seg1_off % 16 != 0)
-    return -2;
+  if (!scaffold_args_ok(args)) return -2;
   return fedavg_dispatch<false, true>(args, n_ctas, stream);
 }
 

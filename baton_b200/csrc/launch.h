@@ -216,6 +216,27 @@ struct FedAvgKrumArgs : FedAvgRobustArgs {
   uint8_t krum_k[B200_MAX_ROBUST_CLIENTS + 1];   // neighbours per score for P = 0 .. 32 (host-computed)
   uint8_t krum_m[B200_MAX_ROBUST_CLIENTS + 1];   // clients kept for P = 0 .. 32
 };
+// Server-optimizer round (the *_sopt kernels, any of the kinds above): the apply phase runs FedAvgM / FedAdagrad /
+// FedYogi / FedAdam (parallel/server_opt.py) on the parameter elements [0, n_param) instead of global += d, with
+// d = decode(wire) * apply_scale:  m = c0*m + d, x += c4*m (kind 0, avgm), or m = c0*m + c1*d, v by kind (1 adagrad:
+// v + d*d, 2 yogi: v - c3*(d*d)*sign(v - d*d), 3 adam: c2*v + c3*(d*d)), x += c4*m / (sqrt(v) + c5); every operation
+// rounded separately.  c = coef = {b1, 1-b1, b2, 1-b2, lr, tau} in fp32 (host-computed).  Float buffers [n_param, n) keep
+// global += d; a round with total weight 0 leaves x, m and v unchanged.  Delta mode only; n_param % 8 == 0.
+extern "C++" {
+template <class Base>
+struct ServerOptArgs : Base {
+  float* m;                         // local: first moment over the parameters [n_param]
+  float* v;                         // local: second moment [n_param] (nullptr for kind 0)
+  long long n_param;                // parameter elements at the start of the arena (multiple of 8)
+  int kind;                         // 0 avgm, 1 adagrad, 2 yogi, 3 adam
+  float coef[6];                    // b1, 1 - b1, b2, 1 - b2, lr, tau
+};
+}
+int b200_fedavg_allreduce_sopt(const ServerOptArgs<FedAvgArgs>* args, int n_ctas, cudaStream_t stream);
+int b200_fedavg_allreduce_dp_sopt(const ServerOptArgs<FedAvgDPArgs>* args, int n_ctas, cudaStream_t stream);
+int b200_fedavg_allreduce_scaffold_sopt(const ServerOptArgs<FedAvgScaffoldArgs>* args, int n_ctas, cudaStream_t stream);
+int b200_fedavg_allreduce_robust_sopt(const ServerOptArgs<FedAvgRobustArgs>* args, int n_ctas, cudaStream_t stream);
+int b200_fedavg_allreduce_krum_sopt(const ServerOptArgs<FedAvgKrumArgs>* args, int n_ctas, cudaStream_t stream);
 int b200_fedavg_allreduce(const FedAvgArgs* args, int n_ctas, cudaStream_t stream);
 int b200_fedavg_allreduce_robust(const FedAvgRobustArgs* args, int n_ctas, cudaStream_t stream);   // delta, peer loads
 int b200_fedavg_allreduce_krum(const FedAvgKrumArgs* args, int n_ctas, cudaStream_t stream);       // delta, peer loads

@@ -91,7 +91,8 @@ def make_app(role: str, host: str, port: int, cfg: Optional[FederationConfig] = 
         manager.register_experiment(
             model, client_ttl=cfg.client_ttl, sample_k=cfg.sample_k, seed=cfg.seed, dataplane=cfg.backend,
             round_timeout=cfg.round_timeout, checkpoint_dir=cfg.checkpoint_dir,
-            resume=bool(cfg.checkpoint_dir), dp=cfg.dp_config(), dp_delta=cfg.dp_delta, robust=cfg.robust_config())
+            resume=bool(cfg.checkpoint_dir), dp=cfg.dp_config(), dp_delta=cfg.dp_delta, robust=cfg.robust_config(),
+            server_opt=cfg.server_opt_config())
         app["manager"] = manager
     elif role == "worker" and cfg.backend in ("fused", "nccl"):
         app["worker"] = make_gpu_worker(app, model, host, port, cfg)

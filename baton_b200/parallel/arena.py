@@ -86,6 +86,10 @@ class ParamArena:
         self.grad = torch.zeros(self.n_param, dtype=torch.float32, device=device)
         self.momentum = torch.zeros(self.n_param, dtype=torch.float32, device=device) if momentum else None
         self.adam_v = None            # AdamW second moment over the parameters, allocated by the first AdamW run
+        # server optimizer state over the parameters (parallel/server_opt.py), allocated by a session built with
+        # server_opt=; server_v stays None for FedAvgM
+        self.server_m = None
+        self.server_v = None
         self.theta_bf16 = torch.zeros(self.n, dtype=torch.bfloat16, device=device) if bf16_shadow else None
         self.global_w = torch.zeros(self.n, dtype=torch.float32, device=device) if keep_global else None
         self.int_arena = torch.zeros(max(self.n_int, 1), dtype=torch.int64, device=device)
@@ -172,6 +176,10 @@ class ParamArena:
             out["momentum"] = self.momentum.numel() * 4
         if self.adam_v is not None:
             out["adam_v"] = self.adam_v.numel() * 4
+        if self.server_m is not None:
+            out["server_m"] = self.server_m.numel() * 4
+        if self.server_v is not None:
+            out["server_v"] = self.server_v.numel() * 4
         if self.theta_bf16 is not None:
             out["theta_bf16"] = self.theta_bf16.numel() * 2
         if self.global_w is not None:

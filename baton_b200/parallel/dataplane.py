@@ -28,6 +28,7 @@ import torch
 
 from . import wire
 from .aggregate import dp_fedavg_into, fedavg_into, robust_into
+from .server_opt import ServerOptConfig, server_step_
 
 log = logging.getLogger("baton_b200.dataplane")
 
@@ -59,17 +60,26 @@ class HttpManagerPlane(ManagerPlane):
     ``last_clip_factors`` holds the factors of the last aggregated round.  ``robust`` (a
     :class:`~baton_b200.parallel.robust.RobustConfig`, exclusive with ``dp``): the coordinate-wise median / trimmed mean
     or the Multi-Krum mean of the participants' updates (:func:`~baton_b200.parallel.aggregate.robust_into`), uploads
-    with ``n_samples == 0`` excluded as under DP."""
+    with ``n_samples == 0`` excluded as under DP.  ``server_opt`` (a
+    :class:`~baton_b200.parallel.server_opt.ServerOptConfig`): the round's aggregate is computed as above into a scratch
+    copy, then ``d = scratch - live`` over the model's parameters (``named_parameters`` order, one fp32 vector) drives
+    :func:`~baton_b200.parallel.server_opt.server_step_`; buffers take the aggregate as before.  The state ``(m, v)``
+    lives here (:meth:`server_state`, :meth:`load_server_state`)."""
 
     name = "http"
     carries_tensors = True
 
-    def __init__(self, int_policy: str = "max", dp=None, robust=None):
+    def __init__(self, int_policy: str = "max", dp=None, robust=None, server_opt=None):
         if dp is not None and robust is not None:
             raise ValueError("robust aggregation with DP-FedAvg is not supported")
+        if server_opt is not None and not isinstance(server_opt, ServerOptConfig):
+            raise TypeError("server_opt= takes a ServerOptConfig")
         self.int_policy = int_policy
         self.dp = dp
         self.robust = robust
+        self.server_opt = server_opt
+        self.server_m: Optional[torch.Tensor] = None     # allocated by the first server step (m = 0, v = tau^2)
+        self.server_v: Optional[torch.Tensor] = None
         self.dp_rounds = 0
         self.last_clip_factors: List[float] = []
 
@@ -106,11 +116,50 @@ class HttpManagerPlane(ManagerPlane):
         else:
             ok = fedavg_into(scratch, [d["state_dict"] for d in datas], [d["n_samples"] for d in datas],
                              int_policy=self.int_policy)
+        if ok and self.server_opt is not None:
+            self._server_step(experiment.model, live, scratch)
         if ok:
             with torch.no_grad():
                 for k, v in live.items():
                     v.copy_(scratch[k])
         return ok
+
+    @torch.no_grad()
+    def _server_step(self, model, live, scratch) -> None:
+        """Replace the parameters' aggregate in ``scratch`` by the server optimizer's step from ``live``."""
+        names = [n for n, _ in model.named_parameters()]
+        x = torch.cat([live[n].detach().reshape(-1).float() for n in names])
+        d = torch.cat([scratch[n].reshape(-1).float() for n in names]) - x
+        if self.server_m is None or self.server_m.numel() != x.numel():
+            self.server_m, self.server_v = self.server_opt.init_state(x.numel(), x.device)
+        server_step_(x, d, self.server_m, self.server_v, self.server_opt)
+        off = 0
+        for n in names:
+            t = scratch[n]
+            t.copy_(x[off: off + t.numel()].view(t.shape).to(t.dtype))
+            off += t.numel()
+
+    def server_state(self) -> Optional[dict]:
+        """The checkpoint entry of the server optimizer: ``{"config", "m", "v"}`` on the CPU (``m`` / ``v`` None before
+        the first step, ``v`` None for FedAvgM), or None without one."""
+        if self.server_opt is None:
+            return None
+        cpu = (lambda t: t.detach().to("cpu").clone() if t is not None else None)
+        return {"config": self.server_opt.to_dict(), "m": cpu(self.server_m), "v": cpu(self.server_v)}
+
+    def load_server_state(self, entry: Optional[dict], device=None) -> None:
+        """Restore :meth:`server_state`; ``None`` (a checkpoint without the entry) restores the initial state."""
+        if self.server_opt is None:
+            return
+        if entry is None or entry.get("m") is None:
+            self.server_m = self.server_v = None
+            return
+        saved = ServerOptConfig.from_dict(entry["config"])
+        if saved != self.server_opt:
+            raise ValueError("the checkpoint's server optimizer {} differs from this experiment's {}".format(
+                saved.to_dict(), self.server_opt.to_dict()))
+        self.server_m = entry["m"].to(device=device, dtype=torch.float32)
+        self.server_v = entry["v"].to(device=device, dtype=torch.float32) if entry.get("v") is not None else None
 
 
 class SeatedManagerPlane(ManagerPlane):
@@ -297,15 +346,24 @@ class SeatedWorkerPlane(WorkerPlane):
             check()             # a peer that died mid-collective surfaces here as an error, not as a hang
 
 
-def make_manager_plane(spec, dp=None, robust=None) -> ManagerPlane:
+SEATED_SERVER_OPT = ("a server optimizer needs the http plane: on the seated planes its state would be replicated on "
+                     "the seats, an evicted seat would return with stale m and v, and the manager holds no copy to "
+                     "resend")
+
+
+def make_manager_plane(spec, dp=None, robust=None, server_opt=None) -> ManagerPlane:
+    if server_opt is not None and not (spec in (None, "http", "http_pickle") or isinstance(spec, HttpManagerPlane)):
+        raise ValueError(SEATED_SERVER_OPT)
     if isinstance(spec, ManagerPlane):
+        if server_opt is not None and getattr(spec, "server_opt", None) != server_opt:
+            raise ValueError("a server-optimizer experiment needs a data plane built with the same server_opt=")
         if dp is not None and getattr(spec, "dp", None) is None:
             raise ValueError("a DP experiment needs a data plane built with the same dp=")
         if robust is not None and getattr(spec, "robust", None) is None:
             raise ValueError("a robust experiment needs a data plane built with the same robust=")
         return spec
     if spec in (None, "http", "http_pickle"):
-        return HttpManagerPlane(dp=dp, robust=robust)
+        return HttpManagerPlane(dp=dp, robust=robust, server_opt=server_opt)
     if spec in ("fused", "nccl"):
         return SeatedManagerPlane(spec, dp=dp, robust=robust)
     raise ValueError("unknown data plane {!r}".format(spec))

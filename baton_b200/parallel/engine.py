@@ -31,6 +31,7 @@ from .arena import ParamArena
 from .dp import DPConfig, RDPAccountant, check_dp, clip_factor
 from .fedavg import FedAvgSession, NcclSession
 from .robust import RobustConfig, check_aggregator, check_krum_participants, check_participants
+from .server_opt import ServerOptConfig
 from .scaffold import ScaffoldState
 
 
@@ -69,7 +70,8 @@ class FederatedEngine:
                  dp_clip: float = 0.0, dp_noise_multiplier: float = 0.0, dp_seed: Optional[int] = None,
                  scaffold: bool = False, optimizer: str = "sgd", betas: Tuple[float, float] = (0.9, 0.999),
                  eps: float = 1e-8, aggregator: str = "mean", trim_ratio: float = 0.1, krum_f: int = 0,
-                 krum_m: Optional[int] = None):
+                 krum_m: Optional[int] = None, server_opt: Optional[str] = None, server_lr: Optional[float] = None,
+                 server_betas: Tuple[float, float] = (0.9, 0.99), server_tau: float = 1e-3):
         """``prox_mu > 0``: FedProx local training -- every step adds ``prox_mu * (theta - global_w)`` to the gradient,
         ``global_w`` being the global model the round started from (for logical clients too: each starts from it).
 
@@ -100,7 +102,20 @@ class FederatedEngine:
         ``P - krum_f - 2`` fellow participants, and the plain mean of the ``krum_m`` best-scoring updates (default ``P -
         krum_f``; 1 is classic Krum) is applied.  The planned participants per round must number at least ``2 krum_f +
         3``; a round with fewer still runs, with ``k`` and ``m`` clamped (``parallel/robust.py``).  The other robust
-        aggregators' rules and costs apply.  :meth:`last_krum` reports the last round's scores by client id."""
+        aggregators' rules and costs apply.  :meth:`last_krum` reports the last round's scores by client id.
+
+        ``server_opt="avgm"`` / ``"adagrad"`` / ``"yogi"`` / ``"adam"`` (``parallel/server_opt.py``): FedAvgM, FedAdagrad,
+        FedYogi or FedAdam on the server -- the round's aggregate, whichever aggregator computed it, drives a stateful
+        step of size ``server_lr`` (required) with ``server_betas`` and ``server_tau`` on the parameters; buffers keep
+        ``global += aggregate``.  The state costs one (FedAvgM) or two fp32 buffers over the parameters on every rank;
+        :meth:`server_state` reads it.  It needs ``mode='delta'``.  ``None`` (the default) runs exactly the plain
+        engine."""
+        sopt = None
+        if server_opt is not None:
+            if mode != "delta":
+                raise ValueError("a server optimizer needs mode='delta': mode='weights' has no pseudo-gradient")
+            b1, b2 = server_betas
+            sopt = ServerOptConfig(server_opt, server_lr, b1, b2, server_tau)
         prox_mu = check_prox_mu(prox_mu)
         adam = check_optimizer(optimizer, momentum, prox_mu=prox_mu)
         if adam:
@@ -163,7 +178,7 @@ class FederatedEngine:
             per_rank = -(-population // world) if population > world else 1
             robust_kw = {"robust": self.robust, "max_clients": min(per_rank, sample_k or population)}
         self.session = Session(self.arena, group, wire_dtype=wire_dtype, mode=mode, n_ctas=n_ctas, nvls=nvls,
-                               tile_flags=tile_flags, dp=self.dp, scaffold=scaffold, **robust_kw)
+                               tile_flags=tile_flags, dp=self.dp, scaffold=scaffold, server_opt=sopt, **robust_kw)
         self.dp = self.session.dp                  # rank 0's noise key
         self.accountant = RDPAccountant(self.dp.noise_multiplier) if self.dp is not None else None
         self.backend = backend
@@ -358,6 +373,12 @@ class FederatedEngine:
         if len(order) != len(scores):
             raise RuntimeError("the session reports {} clients, the round had {}".format(len(scores), len(order)))
         return {c: (float(scores[i]), bool(kept[i])) for i, c in enumerate(order)}
+
+    def server_state(self):
+        """``(m, v)``: the server optimizer's state over the parameters (live fp32 tensors on the engine's device, equal
+        on every rank; ``v`` is None for FedAvgM)."""
+        self.sync()
+        return self.session.server_state()
 
     def _train_client(self, cid: int, X, y, n_epoch: int, first: bool):
         """Local training of client ``cid`` on the replica; with SCAFFOLD, its correction before and its control-variate

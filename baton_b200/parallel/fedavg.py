@@ -34,6 +34,12 @@ fills segment ``j`` and ``aggregate(..., n_clients=m)`` runs the robust kernel o
 ``robust=RobustConfig("krum", krum_f=f, krum_m=m)`` selects Multi-Krum: the fused session then also allocates a
 per-rank DISTANCE PAGE (4 KB per round parity) through which the ranks exchange their partial pair distances inside the
 collective, and :meth:`last_krum` returns the last round's distances, scores and kept clients in segment order.
+
+Both take ``server_opt=ServerOptConfig(...)`` (``parallel/server_opt.py``): FedAvgM, FedAdagrad, FedYogi or FedAdam
+applied to the round's aggregate, whatever computed it (mean, DP, SCAFFOLD, median, trimmed mean, Krum).  The session
+allocates the state ``arena.server_m`` / ``arena.server_v`` over the parameters, replicated on every rank; the fused
+session runs the ``*_sopt`` instantiation of the round's kernel, whose apply phase takes the step, and
+:class:`NcclSession` calls :func:`server_step_` where it would add the aggregate.  :meth:`server_state` reads the state.
 """
 from __future__ import annotations
 
@@ -44,6 +50,7 @@ import torch
 from .arena import ParamArena
 from .dp import DPConfig, clip_factor, normals
 from .robust import MAX_ROBUST_CLIENTS, RobustConfig, krum_select, robust_combine
+from .server_opt import ServerOptConfig, apply_update_
 from .symm import SymmetricBuffer
 
 MAX_LOSS = 64       # per-epoch loss slots carried through the collective
@@ -88,6 +95,19 @@ def _check_robust(robust: Optional[RobustConfig], dp: Optional[DPConfig], scaffo
     return int(max_clients)
 
 
+def _init_server_opt(arena: ParamArena, server_opt: Optional[ServerOptConfig], delta: bool) -> Optional[ServerOptConfig]:
+    """Validate a session's ``server_opt`` and allocate its fresh state in the arena (``m = 0``, ``v = tau^2``)."""
+    if server_opt is None:
+        return None
+    if not isinstance(server_opt, ServerOptConfig):
+        raise TypeError("server_opt= takes a ServerOptConfig")
+    if not delta:
+        raise ValueError("a server optimizer steps on the pseudo-gradient global - aggregate: it needs mode='delta' "
+                         "(mode='weights' has none)")
+    arena.server_m, arena.server_v = server_opt.init_state(arena.n_param, arena.device)
+    return server_opt
+
+
 def _check_control(scaffold: bool, control) -> None:
     if scaffold and control is None:
         raise ValueError("a SCAFFOLD session needs control=(c, dc, n_clients) every round")
@@ -111,10 +131,13 @@ class FedAvgSession:
     def __init__(self, arena: ParamArena, group=None, *, wire_dtype: str = "bf16", mode: str = "delta",
                  nvls: "bool | str" = "auto", n_ctas: Optional[int] = None, tile_elems: int = 0, timeout_log2: int = 24,
                  reset_momentum: bool = True, tile_flags: bool = False, dp: Optional[DPConfig] = None,
-                 scaffold: bool = False, robust: Optional[RobustConfig] = None, max_clients: int = 1):
+                 scaffold: bool = False, robust: Optional[RobustConfig] = None, max_clients: int = 1,
+                 server_opt: Optional[ServerOptConfig] = None):
         from ..ops._ext import load
         self._C = load()
         assert wire_dtype in ("bf16", "fp32", "fp8") and mode in ("delta", "weights")
+        self.server_opt = _init_server_opt(arena, server_opt, mode == "delta")
+        self._sopt_coef = list(server_opt.coefficients()) if server_opt is not None else []
         _check_dp_mode(dp, mode == "delta")
         _check_scaffold(scaffold, dp, mode == "delta")
         self.max_clients = _check_robust(robust, dp, scaffold, mode == "delta", tile_flags, max_clients)
@@ -240,6 +263,20 @@ class FedAvgSession:
         if not torch.equal(self.arena.theta[: self.arena.n_param], self.arena.global_w[: self.arena.n_param]):
             return                                   # replicas already drifted: keep the default
         best = {}
+        sopt, self.server_opt = self.server_opt, None    # zero deltas must not step the server optimizer's state
+        try:
+            best = self._time_nvls_modes(iters)
+        finally:
+            self.server_opt = sopt
+        t = torch.tensor([best[False], best[True]], device=self.device, dtype=torch.float64)
+        dist.all_reduce(t, op=dist.ReduceOp.MAX, group=self.group)
+        self.use_nvls = bool(t[1] < t[0])
+        self.nvls_choice = "autotuned p2p {:.0f} us vs nvls {:.0f} us".format(float(t[0]) * 1e3, float(t[1]) * 1e3)
+        self.check()
+        self.symm.barrier()
+
+    def _time_nvls_modes(self, iters: int) -> dict:
+        best = {}
         for mode in (False, True):
             self.use_nvls = mode
             ts = []
@@ -252,12 +289,7 @@ class FedAvgSession:
                 if it:
                     ts.append(e0.elapsed_time(e1))
             best[mode] = min(ts)
-        t = torch.tensor([best[False], best[True]], device=self.device, dtype=torch.float64)
-        dist.all_reduce(t, op=dist.ReduceOp.MAX, group=self.group)
-        self.use_nvls = bool(t[1] < t[0])
-        self.nvls_choice = "autotuned p2p {:.0f} us vs nvls {:.0f} us".format(float(t[0]) * 1e3, float(t[1]) * 1e3)
-        self.check()
-        self.symm.barrier()
+        return best
 
     # ------------------------------------------------------------------ K4: upload copy emitted by the optimizer
     def pack_spec(self) -> Optional[dict]:
@@ -421,7 +453,7 @@ class FedAvgSession:
                     counts, from_flags, mask, self.rank, world, self.wire_kind, self.epoch, tile, self.n_ctas,
                     self.timeout_log2, self.status, self.phase_ns, prepacked,
                     self.symm.peer_ptrs(o_clip), m, self.seg_stride, self.symm.peer_ptrs(o_dist),
-                    self.krum_work, self.krum_sync, self.krum_report, k_tab, m_tab)
+                    self.krum_work, self.krum_sync, self.krum_report, k_tab, m_tab, *self._sopt_args())
             self.epoch = (self.epoch + 3) & 0xFFFFFFFF
             self.rounds += 1
             self._side_pending = on_side_stream
@@ -435,7 +467,8 @@ class FedAvgSession:
                     self.loss_local, self.symm.peer_ptrs(o_loss), self.loss_out,
                     counts, from_flags, mask, self.rank, world, self.wire_kind, self.epoch, tile, self.n_ctas,
                     self.timeout_log2, self.status, self.phase_ns, prepacked,
-                    self.symm.peer_ptrs(o_clip), m, self.seg_stride, robust.kind_id, robust.trim_table())
+                    self.symm.peer_ptrs(o_clip), m, self.seg_stride, robust.kind_id, robust.trim_table(),
+                    *self._sopt_args())
             self.epoch = (self.epoch + 3) & 0xFFFFFFFF
             self.rounds += 1
             self._side_pending = on_side_stream
@@ -469,10 +502,24 @@ class FedAvgSession:
                 counts, from_flags, mask, self.rank, world, self.wire_kind, self.delta,
                 nvls_now, self.epoch,
                 self.tile_flags, flag_value, tile, self.n_ctas, self.timeout_log2, self.status, self.phase_ns,
-                prepacked, *dp_args, *scaf_args)
+                prepacked, *dp_args, *scaf_args, *self._sopt_args())
         self.epoch = (self.epoch + 3) & 0xFFFFFFFF     # uint32 wrap: the kernel compares signed differences
         self.rounds += 1
         self._side_pending = on_side_stream
+
+    def _sopt_args(self) -> tuple:
+        """The collective's server-optimizer arguments ``(m, v, n_param, kind, coefficients)`` (``m`` None: off)."""
+        if self.server_opt is None:
+            return (None, None, 0, 0, [])
+        a = self.arena
+        return (a.server_m, a.server_v, a.n_param, self.server_opt.kind_id, self._sopt_coef)
+
+    def server_state(self):
+        """``(m, v)``: the server optimizer's state over the parameters (live tensors; ``v`` is None for FedAvgM)."""
+        if self.server_opt is None:
+            raise RuntimeError("server_state needs a session built with server_opt=")
+        self.join()
+        return self.arena.server_m, self.arena.server_v
 
     def last_krum(self):
         """``(D, scores, kept)`` of the last Krum round, in segment order (a host read): the fp64 ``[P, P]`` squared
@@ -577,8 +624,10 @@ class NcclSession:
 
     def __init__(self, arena: ParamArena, group=None, *, wire_dtype: str = "bf16", mode: str = "delta",
                  reset_momentum: bool = True, dp: Optional[DPConfig] = None, scaffold: bool = False,
-                 robust: Optional[RobustConfig] = None, max_clients: int = 1, tile_flags: bool = False, **_unused):
+                 robust: Optional[RobustConfig] = None, max_clients: int = 1, tile_flags: bool = False,
+                 server_opt: Optional[ServerOptConfig] = None, **_unused):
         import torch.distributed as dist
+        self.server_opt = _init_server_opt(arena, server_opt, mode == "delta")
         _check_dp_mode(dp, mode == "delta")
         _check_scaffold(scaffold, dp, mode == "delta")
         self.max_clients = _check_robust(robust, dp, scaffold, mode == "delta", tile_flags, max_clients)
@@ -712,16 +761,22 @@ class NcclSession:
         if self.world > 1:
             dist.all_reduce(self.loss_buf, group=self.group)
         self.loss_out.copy_(self.loss_buf)
+        d = None                        # the round's aggregate (delta mode)
         if robust is not None:
-            a.global_w.add_(upd)
+            d = upd
         elif dp is not None and dp.noise_std > 0.0 and float(total) > 0.0:
             z = torch.from_numpy(normals(dp.seed, self.rounds & 0xFFFFFFFF, a.n)).to(device=self.device,
                                                                                       dtype=torch.float32)
-            a.global_w.add_(self.wire.float() + z * (dp.noise_std / float(total)))
+            d = self.wire.float() + z * (dp.noise_std / float(total))
         elif self.delta:
-            a.global_w.add_(self.wire.float())
-        else:
+            d = self.wire.float()
+        if d is None:
             a.global_w.copy_(self.wire.float())
+        elif self.server_opt is not None:
+            if float(total) > 0.0:      # a round without weight leaves the model and the state unchanged
+                apply_update_(a.global_w, d, a.n_param, a.server_m, a.server_v, self.server_opt)
+        else:
+            a.global_w.add_(d)
         a.theta.copy_(a.global_w)
         if a.theta_bf16 is not None:
             a.theta_bf16.copy_(a.theta.to(torch.bfloat16))
@@ -740,6 +795,12 @@ class NcclSession:
 
     def dp_round(self) -> int:
         return self.rounds & 0xFFFFFFFF
+
+    def server_state(self):
+        """``(m, v)`` as :meth:`FedAvgSession.server_state`."""
+        if self.server_opt is None:
+            raise RuntimeError("server_state needs a session built with server_opt=")
+        return self.arena.server_m, self.arena.server_v
 
     def last_clip_factors(self) -> List[float]:
         return list(self.dp_s)
