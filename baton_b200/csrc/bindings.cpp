@@ -782,6 +782,84 @@ void fedavg_allreduce_krum(const std::vector<int64_t>& wire_ptrs, const std::vec
   check(b200_fedavg_allreduce_krum(&a, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_krum");
 }
 
+// top-k round: the sparse lists sit at byte offsets rowptr_off / off_off / val_off of every rank's wire half
+void fedavg_allreduce_topk(const std::vector<int64_t>& wire_ptrs, const std::vector<int64_t>& pad_ptrs, at::Tensor theta,
+                           const at::Tensor& global_w, const std::optional<at::Tensor>& theta_bf16,
+                           const std::optional<at::Tensor>& momentum, const std::optional<at::Tensor>& int_local,
+                           const std::vector<int64_t>& int_wire_ptrs, const std::optional<at::Tensor>& loss_local,
+                           const std::vector<int64_t>& loss_wire_ptrs, const std::optional<at::Tensor>& loss_out,
+                           const std::vector<double>& n_samples, bool counts_from_flags, int64_t alive_mask, int64_t rank,
+                           int64_t world, int64_t wire_kind, int64_t epoch, int64_t tile_elems, int64_t n_ctas,
+                           int64_t timeout_log2, const std::optional<at::Tensor>& status,
+                           const std::optional<at::Tensor>& phase_ns, int64_t rowptr_off, int64_t off_off, int64_t val_off,
+                           const std::optional<at::Tensor>& sopt_m, const std::optional<at::Tensor>& sopt_v,
+                           int64_t sopt_n_param, int64_t sopt_kind, const std::vector<double>& sopt_coef) {
+  FedAvgTopkArgs a = {};
+  fill_fedavg_args(a, wire_ptrs, pad_ptrs, 0, theta, global_w, theta_bf16, momentum, int_local, int_wire_ptrs, loss_local,
+                   loss_wire_ptrs, loss_out, n_samples, counts_from_flags, alive_mask, rank, world, wire_kind, true, false,
+                   epoch, std::nullopt, 0, tile_elems, timeout_log2, status, phase_ns, true);
+  a.rowptr_off = rowptr_off;
+  a.off_off = off_off;
+  a.val_off = val_off;
+  const c10::cuda::CUDAGuard guard(theta.device());
+  if (want_sopt(sopt_m)) {
+    const auto so = sopt_args(a, sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
+    check(b200_fedavg_allreduce_topk_sopt(&so, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_topk");
+    return;
+  }
+  check(b200_fedavg_allreduce_topk(&a, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_topk");
+}
+
+static void check_topk_io(const at::Tensor& theta, const at::Tensor& global_w, const at::Tensor& work) {
+  CHECK_CUDA(theta); CHECK_CUDA(global_w); CHECK_CUDA(work);
+  TORCH_CHECK(theta.scalar_type() == at::kFloat && global_w.scalar_type() == at::kFloat && theta.is_contiguous() &&
+                  global_w.is_contiguous() && global_w.numel() == theta.numel(),
+              "top-k: fp32 theta / global_w of one size");
+  TORCH_CHECK(work.scalar_type() == at::kInt && work.is_contiguous() && work.numel() >= B200_TOPK_WORK_WORDS(theta.numel()),
+              "top-k: int32 work of B200_TOPK_WORK_WORDS(n) words");
+}
+static float* topk_u(const at::Tensor& theta, at::Tensor& u) {
+  CHECK_CUDA(u);
+  TORCH_CHECK(u.scalar_type() == at::kFloat && u.is_contiguous() && u.numel() == theta.numel(), "top-k: fp32 u over theta");
+  return u.data_ptr<float>();
+}
+
+// one client's selection into the sparse lists at rowptr / off / val (device addresses, e.g. in the wire)
+void topk_pack(const at::Tensor& theta, const at::Tensor& global_w, at::Tensor u, bool ef, int64_t k, at::Tensor work,
+               int64_t rowptr, int64_t off, int64_t val, int64_t wire_kind, int64_t cap) {
+  check_topk_io(theta, global_w, work);
+  const c10::cuda::CUDAGuard guard(theta.device());
+  check(b200_topk_pack(theta.data_ptr<float>(), global_w.data_ptr<float>(), topk_u(theta, u), ef ? 1 : 0, theta.numel(),
+                       k, work.data_ptr<int>(), reinterpret_cast<uint32_t*>(rowptr), reinterpret_cast<uint16_t*>(off),
+                       reinterpret_cast<void*>(val), static_cast<int>(wire_kind), cap, cur_stream()),
+        "topk_pack");
+}
+
+void topk_fold(at::Tensor theta, const at::Tensor& global_w, at::Tensor u, bool ef, int64_t k, at::Tensor work,
+               at::Tensor acc, double nk, bool first, const std::optional<at::Tensor>& wb,
+               const std::optional<at::Tensor>& mom, bool reset) {
+  check_topk_io(theta, global_w, work);
+  CHECK_CUDA(acc);
+  TORCH_CHECK(acc.scalar_type() == at::kFloat && acc.is_contiguous() && acc.numel() == theta.numel(),
+              "topk_fold: fp32 acc over theta");
+  const c10::cuda::CUDAGuard guard(theta.device());
+  check(b200_topk_fold(theta.data_ptr<float>(), global_w.data_ptr<float>(), topk_u(theta, u), ef ? 1 : 0, theta.numel(),
+                       k, work.data_ptr<int>(), acc.data_ptr<float>(), static_cast<float>(nk), first ? 1 : 0,
+                       opt_ptr<void>(wb), opt_ptr<float>(mom), mom.has_value() && mom->defined() ? mom->numel() : 0,
+                       reset ? 1 : 0, cur_stream()),
+        "topk_fold");
+}
+
+void nonzero_pack(const at::Tensor& theta, const at::Tensor& global_w, at::Tensor work, int64_t rowptr, int64_t off,
+                  int64_t val, int64_t wire_kind, int64_t cap) {
+  check_topk_io(theta, global_w, work);
+  const c10::cuda::CUDAGuard guard(theta.device());
+  check(b200_nonzero_pack(theta.data_ptr<float>(), global_w.data_ptr<float>(), theta.numel(), work.data_ptr<int>(),
+                          reinterpret_cast<uint32_t*>(rowptr), reinterpret_cast<uint16_t*>(off),
+                          reinterpret_cast<void*>(val), static_cast<int>(wire_kind), cap, cur_stream()),
+        "nonzero_pack");
+}
+
 // one logical client's wire segment at address seg (see b200_pack_client)
 void pack_client(int64_t seg, at::Tensor theta, const at::Tensor& global_w, const std::optional<at::Tensor>& wb,
                  const std::optional<at::Tensor>& mom, int64_t wire_kind, bool reset) {
@@ -1118,6 +1196,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.attr("KRUM_MAX_CTAS") = B200_KRUM_MAX_CTAS;
   m.attr("KRUM_PAIRS") = B200_KRUM_PAIRS;
   m.attr("KRUM_REPORT") = B200_KRUM_REPORT;
+  m.def("fedavg_allreduce_topk", &fedavg_allreduce_topk);
+  m.def("topk_pack", &topk_pack);
+  m.def("topk_fold", &topk_fold);
+  m.def("nonzero_pack", &nonzero_pack);
+  m.def("topk_work_words", [](int64_t n) { return static_cast<int64_t>(B200_TOPK_WORK_WORDS(n)); });
   m.def("pack_client", &pack_client);
   m.attr("MAX_ROBUST_CLIENTS") = B200_MAX_ROBUST_CLIENTS;
   m.def("flag_barrier", &flag_barrier);

@@ -814,6 +814,104 @@ __device__ __forceinline__ bool krum_reduce(const FedAvgKrumArgs& a, uint8_t* co
   return true;
 }
 
+// ---------------------------------------------------------------- top-k rounds (see launch.h / parallel/compress.py)
+// Phase 1 of a top-k round: the owner of a tile walks it in chunks of TOPK_CHUNK_G granules (1024 elements each).
+//   stage   the chunk's TOPK_CHUNK_G + 1 row pointers of every live participant, one remote load per (rank, word), into
+//           shared memory, and the fp32 accumulator tile of the chunk is zeroed;
+//   add     warp w owns granule w of the chunk: for every live participant in rank order it adds w_k * value at the
+//           entries' offsets, four entries per lane in flight.  Offsets inside one rank's granule are distinct, so the
+//           lanes never collide; the __syncwarp between ranks orders the adds of one element by rank, and the sum of
+//           every element is fmaf(w_k, x, acc) from 0 over the ranks that sent it, as the dense reduce computes it
+//           (a rank that did not send an element would add w_k * 0, which changes nothing);
+//   store   the tile is cast to the wire format and stored into seg 0 of every live replica, where the apply finds it.
+constexpr int TOPK_CHUNK_G = FEDAVG_THREADS / 32;                  // one granule per warp
+constexpr int TOPK_SMEM = TOPK_CHUNK_G * FLAG_GRANULE * 4 + B200_MAX_RANKS * (TOPK_CHUNK_G + 1) * 4;
+
+__device__ __forceinline__ uint32_t ld_volatile_u32(const void* p) {
+  uint32_t r;
+  asm volatile("ld.volatile.global.u32 %0, [%1];" : "=r"(r) : "l"(p) : "memory");
+  return r;
+}
+__device__ __forceinline__ uint32_t ld_volatile_u16(const void* p) {
+  uint16_t r;
+  asm volatile("ld.volatile.global.u16 %0, [%1];" : "=h"(r) : "l"(p) : "memory");
+  return r;
+}
+
+template <int WIRE>
+__device__ __forceinline__ void topk_reduce(const FedAvgTopkArgs& a, uint8_t* const* s_wire, const float* s_w, int A,
+                                            int my_pos) {
+  static_assert(WIRE == 0 || WIRE == 1, "top-k rounds carry fp32 or bf16 values");
+  using W = Wire<WIRE>;
+  constexpr int VEC = W::VEC;
+  constexpr size_t esz = W::VBYTES / VEC;
+  constexpr int U = 4;                               // entries per lane in flight
+  extern __shared__ __align__(16) uint8_t topk_smem[];
+  float* acc = reinterpret_cast<float*>(topk_smem);
+  uint32_t* rp = reinterpret_cast<uint32_t*>(topk_smem + TOPK_CHUNK_G * FLAG_GRANULE * 4);   // [rank pos][CHUNK_G + 1]
+  const int G = gridDim.x;
+  const long long n = a.n;
+  const int T = a.tile_elems;
+  const long long n_tiles = (n + T - 1) / T;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (long long t = my_pos + static_cast<long long>(blockIdx.x) * A; t < n_tiles; t += static_cast<long long>(G) * A) {
+    const long long base = t * T;
+    const int ng = static_cast<int>(((n - base) < T ? (n - base) : T) / FLAG_GRANULE);
+    for (int c0 = 0; c0 < ng; c0 += TOPK_CHUNK_G) {
+      const int cg = ng - c0 < TOPK_CHUNK_G ? ng - c0 : TOPK_CHUNK_G;
+      const long long g0 = base / FLAG_GRANULE + c0;
+      for (int i = threadIdx.x; i < A * (TOPK_CHUNK_G + 1); i += FEDAVG_THREADS) {
+        const int k = i / (TOPK_CHUNK_G + 1), j = i % (TOPK_CHUNK_G + 1);
+        if (j <= cg && s_w[k] != 0.f) rp[i] = ld_volatile_u32(s_wire[k] + a.rowptr_off + (g0 + j) * 4);
+      }
+      for (int i = threadIdx.x * 4; i < cg * FLAG_GRANULE; i += FEDAVG_THREADS * 4)
+        *reinterpret_cast<float4*>(acc + i) = make_float4(0.f, 0.f, 0.f, 0.f);
+      __syncthreads();
+      if (warp < cg) {
+        float* ag = acc + warp * FLAG_GRANULE;
+#pragma unroll 1
+        for (int k = 0; k < A; ++k) {
+          const float w = s_w[k];
+          if (w == 0.f) continue;
+          const uint8_t* src = s_wire[k];
+          const uint32_t e1 = rp[k * (TOPK_CHUNK_G + 1) + warp + 1];
+#pragma unroll 1
+          for (uint32_t e = rp[k * (TOPK_CHUNK_G + 1) + warp] + lane; e < e1; e += 32 * U) {
+            uint32_t o[U], v[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+              const uint32_t j = e + 32 * u;
+              if (j < e1) {
+                o[u] = ld_volatile_u16(src + a.off_off + static_cast<size_t>(j) * 2);
+                v[u] = WIRE == 0 ? ld_volatile_u32(src + a.val_off + static_cast<size_t>(j) * 4)
+                                 : ld_volatile_u16(src + a.val_off + static_cast<size_t>(j) * 2);
+              }
+            }
+#pragma unroll
+            for (int u = 0; u < U; ++u)
+              if (e + 32 * u < e1) {
+                const float x = WIRE == 0 ? __uint_as_float(v[u]) : __uint_as_float(v[u] << 16);
+                ag[o[u]] = fmaf(w, x, ag[o[u]]);
+              }
+          }
+          __syncwarp();
+        }
+      }
+      __syncthreads();
+      for (int i = threadIdx.x * VEC; i < cg * FLAG_GRANULE; i += FEDAVG_THREADS * VEC) {
+        float f[VEC];
+#pragma unroll
+        for (int j = 0; j < VEC; ++j) f[j] = acc[i + j];
+        const uint4 out = W::pack(f, 1.f);
+        const size_t off = (base + static_cast<long long>(c0) * FLAG_GRANULE + i) * esz;
+#pragma unroll 1
+        for (int k = 0; k < A; ++k) W::st_na(s_wire[k] + off, out);
+      }
+      __syncthreads();   // the next chunk reuses the tile and the row pointers
+    }
+  }
+}
+
 // ---------------------------------------------------------------- server optimizer (see launch.h / parallel/server_opt.py)
 // one element: the state update, then the model update, each operation rounded separately (no FMA contraction)
 __device__ __forceinline__ float sopt_step(float x, float d, float& m, float& v, int kind, const float* c) {
@@ -892,13 +990,15 @@ __device__ __forceinline__ void sopt_apply_tile(const Args& a, const uint8_t* my
 // ROBUST: a robust round (robust_reduce above); every rank publishes its segment count before barrier 1.
 // KRUM (with ROBUST): a Multi-Krum round (krum_reduce above): the exchange barrier takes epoch + 2, barrier 2 epoch + 3.
 // SOPT (with any of the above): a server-optimizer round -- the apply phase runs sopt_apply_tile.
+// TOPK: a top-k round (topk_reduce above): no pack phase, the uploads are sparse lists written before the launch.
 // The whole round; Args is FedAvgDPArgs when DP, FedAvgScaffoldArgs when SCAF, FedAvgRobustArgs when ROBUST,
-// FedAvgKrumArgs when KRUM, and ServerOptArgs<that> when SOPT.
+// FedAvgKrumArgs when KRUM, FedAvgTopkArgs when TOPK, and ServerOptArgs<that> when SOPT.
 template <int WIRE, bool DP, bool SCAF = false, bool ROBUST = false, bool KRUM = false, bool SOPT = false,
-          typename Args>
+          bool TOPK = false, typename Args>
 __device__ __forceinline__ void fedavg_round(const Args& a) {
   static_assert(!(DP && SCAF), "DP-FedAvg and SCAFFOLD are exclusive");
   static_assert(!(ROBUST && (DP || SCAF)), "robust rounds exclude DP-FedAvg and SCAFFOLD");
+  static_assert(!(TOPK && (DP || SCAF || ROBUST)), "top-k rounds exclude DP-FedAvg, SCAFFOLD and robust aggregation");
   using W = Wire<WIRE>;
   constexpr int VEC = W::VEC;
   constexpr bool SCALED = W::SCALED;
@@ -941,7 +1041,7 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
   // Loop bounds are warp-uniform (first lane's element) so the block-scale shuffles are legal.
   const float pack_scale = a.use_nvls ? my_n * a.nvls_prescale : 1.0f;
   phase_stamp(a, 0);                                   // start
-  if ((my_n != 0.f || a.use_nvls) && !a.prepacked) {
+  if (!TOPK && (my_n != 0.f || a.use_nvls) && !a.prepacked) {
     for (long long q = blockIdx.x; q * A < n_tiles; q += G) {
       for (int r = 0; r < A; ++r) {
         const long long t = q * A + r;
@@ -1147,6 +1247,8 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
   };
   if constexpr (KRUM) {
     if (!krum_reduce<WIRE>(a, s_wire, s_rank, A, my_pos)) return;
+  } else if constexpr (TOPK) {
+    topk_reduce<WIRE>(a, s_wire, s_w, A, my_pos);
   } else if constexpr (ROBUST) {
     robust_reduce<WIRE>(a, s_wire, s_rank, A, my_pos);
   } else if constexpr (SCAF) {
@@ -1320,6 +1422,16 @@ __global__ void __maxnreg__(96) fedavg_allreduce_krum_sopt_kernel(const __grid_c
   fedavg_round<WIRE, false, false, true, true, true>(a);
 }
 
+// top-k round: TOPK_SMEM bytes of dynamic shared memory (the accumulator tile), the same 96-register cap
+template <int WIRE>
+__global__ void __maxnreg__(96) fedavg_allreduce_topk_kernel(const __grid_constant__ FedAvgTopkArgs a) {
+  fedavg_round<WIRE, false, false, false, false, false, true>(a);
+}
+template <int WIRE>
+__global__ void __maxnreg__(96) fedavg_allreduce_topk_sopt_kernel(const __grid_constant__ ServerOptArgs<FedAvgTopkArgs> a) {
+  fedavg_round<WIRE, false, false, false, false, true, true>(a);
+}
+
 // one logical client's upload into its wire segment: the phase-0 pack of fedavg_round (delta mode, scale 1) over the
 // whole arena, plus fold_client_kernel's replica reset.  Loop bounds are warp-uniform so the fp8 quads can shuffle.
 template <int WIRE>
@@ -1469,10 +1581,13 @@ fold_client_scaled_kernel(float* __restrict__ acc, float* __restrict__ theta, co
 // (cudaErrorCooperativeLaunchTooLarge) and schedules all CTAs together, also next to work on other streams -- instead
 // of the plain <<<>>> of round 1, which was only safe on an otherwise idle GPU.  The grid is clamped to what
 // cudaOccupancyMaxActiveBlocksPerMultiprocessor allows on this device.
-template <int WIRE, bool DP, bool SCAF, bool ROBUST, bool KRUM, bool SOPT>
+template <int WIRE, bool DP, bool SCAF, bool ROBUST, bool KRUM, bool SOPT, bool TOPK = false>
 static const void* fedavg_kernel() {
   using namespace b200;
-  if constexpr (SOPT) {
+  if constexpr (TOPK) {
+    return SOPT ? reinterpret_cast<const void*>(fedavg_allreduce_topk_sopt_kernel<WIRE>)
+                : reinterpret_cast<const void*>(fedavg_allreduce_topk_kernel<WIRE>);
+  } else if constexpr (SOPT) {
     if constexpr (KRUM) return reinterpret_cast<const void*>(fedavg_allreduce_krum_sopt_kernel<WIRE>);
     else if constexpr (ROBUST) return reinterpret_cast<const void*>(fedavg_allreduce_robust_sopt_kernel<WIRE>);
     else if constexpr (SCAF) return reinterpret_cast<const void*>(fedavg_allreduce_scaffold_sopt_kernel<WIRE>);
@@ -1487,17 +1602,18 @@ static const void* fedavg_kernel() {
   }
 }
 
-template <int WIRE, bool DP, bool SCAF, typename Args, bool ROBUST = false, bool KRUM = false, bool SOPT = false>
+template <int WIRE, bool DP, bool SCAF, typename Args, bool ROBUST = false, bool KRUM = false, bool SOPT = false,
+          bool TOPK = false>
 static int launch_fedavg(const Args* args, int n_ctas, cudaStream_t stream) {
   using namespace b200;
   static int max_ctas = -1;
-  const void* kernel = fedavg_kernel<WIRE, DP, SCAF, ROBUST, KRUM, SOPT>();
-  const int smem = KRUM ? KRUM_SMEM : ROBUST ? ROBUST_SMEM : 0;
+  const void* kernel = fedavg_kernel<WIRE, DP, SCAF, ROBUST, KRUM, SOPT, TOPK>();
+  const int smem = KRUM ? KRUM_SMEM : ROBUST ? ROBUST_SMEM : TOPK ? TOPK_SMEM : 0;
   if (max_ctas < 0) {
     int dev = 0, sms = 0, per_sm = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (ROBUST) {
+    if (ROBUST || TOPK) {
       cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
       if (e != cudaSuccess) return static_cast<int>(e);
     }
@@ -1615,6 +1731,30 @@ extern "C" int b200_fedavg_allreduce_krum_sopt(const ServerOptArgs<FedAvgKrumArg
   if (!sopt_args_ok(args) || !krum_args_ok(args)) return -2;
   if (n_ctas > B200_KRUM_MAX_CTAS) n_ctas = B200_KRUM_MAX_CTAS;
   return fedavg_dispatch<false, false, ServerOptArgs<FedAvgKrumArgs>, true, true, true>(args, n_ctas, stream);
+}
+
+// a sum of sparse lists needs the peer loads (the switch adds dense vectors), the delta, whole granules per tile and
+// aligned list offsets; fp8's block scales have no meaning on a list
+template <bool SOPT, class Args>
+static int topk_dispatch(const Args* args, int n_ctas, cudaStream_t stream) {
+  using namespace b200;
+  if (args->use_nvls || !args->delta || args->tile_flags != nullptr || args->world > B200_MAX_RANKS ||
+      args->n % FLAG_GRANULE != 0 || args->tile_elems <= 0 || args->tile_elems % FLAG_GRANULE != 0 ||
+      args->rowptr_off % 4 != 0 || args->off_off % 2 != 0 || args->val_off % 4 != 0 ||
+      (args->wire_kind != 0 && args->wire_kind != 1))
+    return -2;
+  if (n_ctas < 1) n_ctas = 1;
+  if (args->wire_kind == 1) return launch_fedavg<1, false, false, Args, false, false, SOPT, true>(args, n_ctas, stream);
+  return launch_fedavg<0, false, false, Args, false, false, SOPT, true>(args, n_ctas, stream);
+}
+
+extern "C" int b200_fedavg_allreduce_topk(const FedAvgTopkArgs* args, int n_ctas, cudaStream_t stream) {
+  return topk_dispatch<false>(args, n_ctas, stream);
+}
+
+extern "C" int b200_fedavg_allreduce_topk_sopt(const ServerOptArgs<FedAvgTopkArgs>* args, int n_ctas, cudaStream_t stream) {
+  if (!sopt_args_ok(args)) return -2;
+  return topk_dispatch<true>(args, n_ctas, stream);
 }
 
 extern "C" int b200_pack_client(void* seg, float* theta, const float* global_w, void* w_bf16, float* mom, long long n_mom,

@@ -259,6 +259,35 @@ int b200_fold_client_scaled(float* acc, float* theta, const float* global_w, voi
                             long long n, const float* s, int first, int reset, cudaStream_t stream);
 int b200_flag_barrier(unsigned long long* const* pads, int rank, int world, uint32_t alive_mask, uint32_t epoch,
                       int slot, cudaStream_t stream);
+// Top-k round (fedavg_allreduce_topk_kernel<WIRE>, fp32 / bf16 wire, delta mode, peer loads, no arrival flags): every
+// participant's upload is a sparse list in its wire half, written before the launch by b200_topk_pack /
+// b200_nonzero_pack (compress.cu): uint32 rowptr[n / 1024 + 1] at rowptr_off, uint16 off[cap] at off_off (the offset of
+// an entry inside its 1024-element granule), values[cap] in the wire dtype at val_off, entries in index order.  The
+// owner of a tile adds w_k * value into an fp32 shared-memory tile, live ranks in order (fmaf from 0, skipping w_k == 0,
+// as the dense reduce), and stores the cast dense result into seg 0 of every live replica; pack phase: none; barriers,
+// apply, loss and integer arena: the plain round's.  n and tile_elems are multiples of 1024.
+struct FedAvgTopkArgs : FedAvgArgs {
+  long long rowptr_off;             // byte offsets inside every rank's wire half
+  long long off_off;
+  long long val_off;
+};
+int b200_fedavg_allreduce_topk(const FedAvgTopkArgs* args, int n_ctas, cudaStream_t stream);
+int b200_fedavg_allreduce_topk_sopt(const ServerOptArgs<FedAvgTopkArgs>* args, int n_ctas, cudaStream_t stream);
+
+// ---- compress.cu: top-k selection with error feedback (parallel/compress.py)
+// work: int32 [B200_TOPK_WORK_WORDS(n)] scratch; n % 1024 == 0, 1 <= k <= n, 16-byte aligned fp32 arrays.
+#define B200_TOPK_WORK_WORDS(n) (4624 + 4 * ((n) / 1024) + 1)
+// u = (theta - global_w) [+ u when ef] (each operation rounded), the k largest |u| (ties: lower index) compacted into
+// rowptr / off / val (wire_kind 0 fp32, 1 bf16; cap >= k entries); ef: u = 0 on the kept entries (u is the residual)
+int b200_topk_pack(const float* theta, const float* global_w, float* u, int ef, long long n, long long k, int* work,
+                   uint32_t* rowptr, uint16_t* off, void* val, int wire_kind, long long cap, cudaStream_t stream);
+// the same selection folded into acc: acc (+)= nk * topk(u) (first: from 0), residual as above; reset: theta = global,
+// bf16 shadow, momentum [0, n_mom) = 0 (the next co-resident client starts from the global model)
+int b200_topk_fold(float* theta, const float* global_w, float* u, int ef, long long n, long long k, int* work, float* acc,
+                   float nk, int first, void* w_bf16, float* mom, long long n_mom, int reset, cudaStream_t stream);
+// the entries where theta != global_w, value cast(theta - global_w), in the same format (at most cap; the rest dropped)
+int b200_nonzero_pack(const float* theta, const float* global_w, long long n, int* work, uint32_t* rowptr, uint16_t* off,
+                      void* val, int wire_kind, long long cap, cudaStream_t stream);
 
 // ---- conv.cu
 int b200_im2col_nhwc(const void* x, void* col, int N, int H, int W, int C, int KH, int KW, int stride, int pad,

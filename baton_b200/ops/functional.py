@@ -312,6 +312,36 @@ def fold_finish(acc: torch.Tensor, theta: torch.Tensor, global_w: torch.Tensor, 
     load().fold_client(acc, theta, global_w, None, None, 1.0 / float(total), 2, False)
 
 
+def topk_work(n: int, device) -> torch.Tensor:
+    """Scratch of the top-k kernels for an ``n``-element arena (int32; reusable by launches on the same stream)."""
+    return torch.zeros(int(load().topk_work_words(int(n))), dtype=torch.int32, device=device)
+
+
+def topk_pack(theta: torch.Tensor, global_w: torch.Tensor, u: torch.Tensor, k: int, work: torch.Tensor, rowptr: int,
+              off: int, val: int, *, ef: bool, wire_fp32: bool, cap: int) -> None:
+    """One client's top-k upload (``parallel/compress.py``): ``u = (theta - global) [+ u]`` (``ef``: ``u`` holds the
+    residual), the ``k`` largest ``|u|`` (ties: lower index) written as a sparse list at the device addresses ``rowptr``
+    (uint32 ``[n / 1024 + 1]``), ``off`` (uint16 ``[cap]``) and ``val`` (``[cap]`` fp32 or bf16); with ``ef`` the
+    residual ``u`` becomes 0 on the kept entries."""
+    load().topk_pack(theta, global_w, u, bool(ef), int(k), work, int(rowptr), int(off), int(val),
+                     0 if wire_fp32 else 1, int(cap))
+
+
+def topk_fold(theta: torch.Tensor, global_w: torch.Tensor, u: torch.Tensor, k: int, work: torch.Tensor,
+              acc: torch.Tensor, nk: float, *, ef: bool, first: bool = False, reset: bool = False,
+              w_bf16: Optional[torch.Tensor] = None, momentum: Optional[torch.Tensor] = None) -> None:
+    """:func:`fold_client` for a top-k client: the selection of :func:`topk_pack`, then ``acc (+)= nk * topk(u)``, the
+    residual update and (``reset``) the replica reset."""
+    load().topk_fold(theta, global_w, u, bool(ef), int(k), work, acc, float(nk), bool(first), w_bf16, momentum,
+                     bool(reset))
+
+
+def nonzero_pack(theta: torch.Tensor, global_w: torch.Tensor, work: torch.Tensor, rowptr: int, off: int, val: int, *,
+                 wire_fp32: bool, cap: int) -> None:
+    """The sparse list of the entries where ``theta != global``, value ``cast(theta - global)`` (at most ``cap``)."""
+    load().nonzero_pack(theta, global_w, work, int(rowptr), int(off), int(val), 0 if wire_fp32 else 1, int(cap))
+
+
 def dp_clip_factor(theta: torch.Tensor, global_w: torch.Tensor, clip: float, work: torch.Tensor, s_out: torch.Tensor,
                    norm_out: torch.Tensor, *, s_copy_ptr: int = 0, nonfinite: Optional[torch.Tensor] = None) -> None:
     """DP-FedAvg clip factor: ``s_out[0] = min(1, clip / ||theta - global_w||)`` (0 for a non-finite norm, which also

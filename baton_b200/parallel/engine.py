@@ -28,6 +28,7 @@ import torch
 from ..metrics import phase
 from ..train import GraphedLocalSGD, PortableLocalSGD, check_adamw, check_optimizer, check_prox_mu
 from .arena import ParamArena
+from .compress import TopKConfig, TopKState, check_topk_exclusions
 from .dp import DPConfig, RDPAccountant, check_dp, clip_factor
 from .fedavg import FedAvgSession, NcclSession
 from .robust import RobustConfig, check_aggregator, check_krum_participants, check_participants
@@ -71,7 +72,8 @@ class FederatedEngine:
                  scaffold: bool = False, optimizer: str = "sgd", betas: Tuple[float, float] = (0.9, 0.999),
                  eps: float = 1e-8, aggregator: str = "mean", trim_ratio: float = 0.1, krum_f: int = 0,
                  krum_m: Optional[int] = None, server_opt: Optional[str] = None, server_lr: Optional[float] = None,
-                 server_betas: Tuple[float, float] = (0.9, 0.99), server_tau: float = 1e-3):
+                 server_betas: Tuple[float, float] = (0.9, 0.99), server_tau: float = 1e-3,
+                 compress: Optional[str] = None, topk_ratio: float = 0.01, error_feedback: bool = True):
         """``prox_mu > 0``: FedProx local training -- every step adds ``prox_mu * (theta - global_w)`` to the gradient,
         ``global_w`` being the global model the round started from (for logical clients too: each starts from it).
 
@@ -109,7 +111,23 @@ class FederatedEngine:
         step of size ``server_lr`` (required) with ``server_betas`` and ``server_tau`` on the parameters; buffers keep
         ``global += aggregate``.  The state costs one (FedAvgM) or two fp32 buffers over the parameters on every rank;
         :meth:`server_state` reads it.  It needs ``mode='delta'``.  ``None`` (the default) runs exactly the plain
-        engine."""
+        engine.
+
+        ``compress="topk"`` (``parallel/compress.py``): every participating client uploads only its ``k = max(1,
+        ceil(topk_ratio * n_float))`` largest-magnitude update entries (``n_float``: the float ``state_dict`` elements);
+        with ``error_feedback`` the rest is carried in a per-client fp32 residual over the arena, kept on the rank that
+        hosts the client (:meth:`topk_residuals`), and added to its next update.  The round's update is the
+        sample-weighted mean of the sparse uploads; the downlink stays dense.  It cannot be combined with the fp8 wire,
+        DP, a robust aggregator, SCAFFOLD, ``mode='weights'`` or ``tile_flags``; FedProx, AdamW, momentum, logical
+        clients and every server optimizer combine freely.  :meth:`last_upload_bytes` reports the upload.  ``None``
+        (the default) runs exactly the plain engine."""
+        if compress not in (None, "topk"):
+            raise ValueError("compress must be None or 'topk', got {!r}".format(compress))
+        self.topk = TopKConfig(topk_ratio, error_feedback) if compress == "topk" else None
+        if self.topk is not None:
+            check_topk_exclusions(wire_dtype=wire_dtype, dp=dp_clip if dp_clip else None,
+                                  robust=aggregator if aggregator != "mean" else None, scaffold=scaffold,
+                                  delta=mode == "delta", tile_flags=tile_flags)
         sopt = None
         if server_opt is not None:
             if mode != "delta":
@@ -168,6 +186,11 @@ class FederatedEngine:
             self.trainer = PortableLocalSGD(model, self.arena, loss=loss)
         Session = {"fused": FedAvgSession, "nccl": NcclSession}[backend]
         robust_kw = {}
+        if self.topk is not None:     # with logical clients the folded upload is the union of S clients' supports
+            world = self._group_size(group)
+            population = logical_clients if logical_clients and logical_clients > world else world
+            per_rank = -(-population // world) if population > world else 1
+            robust_kw = {"topk": self.topk, "max_clients": min(per_rank, sample_k or population)}
         if self.robust is not None:
             world = self._group_size(group)
             population = logical_clients if logical_clients and logical_clients > world else world
@@ -185,7 +208,7 @@ class FederatedEngine:
         self.rank, self.world = self.session.rank, self.session.world
         # K4: the last SGD step of the captured epoch writes the upload copy itself (no pack phase in the collective);
         # only for the plain one-client-per-GPU rounds -- logical clients fold their deltas after training
-        self.prepack = (backend == "fused" and self.device.type == "cuda"
+        self.prepack = (backend == "fused" and self.device.type == "cuda" and self.topk is None
                         and not (logical_clients and logical_clients > self.world))
         if self.prepack and hasattr(self.session, "pack_spec"):
             self.trainer.pack = self.session.pack_spec()
@@ -208,6 +231,8 @@ class FederatedEngine:
         self.logical_clients = logical_clients if logical_clients and logical_clients > self.world else 0
         self.sample_k = sample_k
         self.scaf = ScaffoldState(self.arena.n_param, self.device) if scaffold else None
+        self.topk_state = (TopKState(self.arena.n, self.device)
+                           if self.topk is not None and self.topk.error_feedback else None)
         self._rng = random.Random(seed)            # identical stream on every rank
         self._stage: Dict[Tuple, Tuple[torch.Tensor, torch.Tensor]] = {}
         self._eval_stage: Dict[Tuple, Tuple[torch.Tensor, torch.Tensor]] = {}
@@ -283,6 +308,8 @@ class FederatedEngine:
                 with phase("baton.local_train", self.phase_s):
                     losses_dev = self._train_client(self.rank, X, y, n_epoch, first=True)
                 total_n = X.shape[0]
+                if self.topk is not None:
+                    self.session.pack_topk(self._residual(self.rank))
         elif self.robust is not None:
             # robust: every hosted participant uploads its own segment (a median of per-rank sums is not a median of
             # clients); the next co-resident client starts from the global model
@@ -319,6 +346,14 @@ class FederatedEngine:
                 total_n += nk
                 if self.dp is not None:
                     self._dp_fold(j, more=j + 1 < len(mine))
+                elif self.topk is not None:
+                    # top-k: one hosted client uploads its own list; several fold n_k * topk(u_k), then upload the
+                    # folded mean's non-zero entries
+                    if len(mine) == 1:
+                        self.session.pack_topk(self._residual(cid))
+                    else:
+                        self.session.fold_topk(self._acc, self._residual(cid), nk, first=(j == 0),
+                                               reset=j + 1 < len(mine))
                 elif len(mine) > 1:
                     more = j + 1 < len(mine)           # the next co-resident client starts from the global model
                     if a.theta.is_cuda:
@@ -339,6 +374,8 @@ class FederatedEngine:
                     F.fold_finish(self._acc, a.theta, a.global_w, m_r)
                 else:
                     torch.add(a.global_w, self._acc, alpha=1.0 / m_r, out=a.theta)
+                if self.topk is not None:
+                    self.session.pack_nonzero()
             if losses_dev is not None and total_n:
                 losses_dev = losses_dev / total_n
         self.last_losses_dev = losses_dev
@@ -359,6 +396,23 @@ class FederatedEngine:
         if read_loss and losses_dev is not None:
             hist = loss_for_wire.tolist()       # device -> host read of the round's result
         return RoundResult(update_name, int(total_n), hist, participants)
+
+    def _residual(self, cid: int) -> Optional[torch.Tensor]:
+        return self.topk_state.residual(cid) if self.topk_state is not None else None
+
+    def topk_residuals(self) -> Dict[int, torch.Tensor]:
+        """``{client_id: e}``: the error-feedback residuals of the clients this rank hosts that have taken part so far
+        (fp32 over the arena, on the engine's device; live, not copies).  Empty without error feedback."""
+        if self.topk is None:
+            raise RuntimeError("top-k uploads are off (compress=None)")
+        self.sync()
+        return dict(self.topk_state.e) if self.topk_state is not None else {}
+
+    def last_upload_bytes(self) -> int:
+        """Bytes this rank uploaded in the last round (a host read): the sparse list with ``compress='topk'`` (0 when it
+        hosted no participant), else the dense wire."""
+        self.sync()
+        return self.session.last_upload_bytes() if self.topk is not None else self.session.wire_bytes()
 
     def last_krum(self) -> Dict[int, Tuple[float, bool]]:
         """``{client_id: (score, kept)}`` of the last Krum round's participants (a host read).  The session reports in

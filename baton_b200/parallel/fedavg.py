@@ -35,6 +35,15 @@ fills segment ``j`` and ``aggregate(..., n_clients=m)`` runs the robust kernel o
 per-rank DISTANCE PAGE (4 KB per round parity) through which the ranks exchange their partial pair distances inside the
 collective, and :meth:`last_krum` returns the last round's distances, scores and kept clients in segment order.
 
+Both take ``topk=TopKConfig(ratio, error_feedback)`` (``parallel/compress.py``): every participating client uploads only
+its ``k`` largest-magnitude update entries (the rest carried in its residual).  Each parity half of the fused session's
+wire is then ``[seg 0: the dense result | pad | sparse segment]``, the sparse segment being ``uint32 rowptr[n / 1024 +
+1] | pad | uint16 off[cap] | pad | values[cap]`` in the wire dtype (fp32 or bf16).  :meth:`pack_topk` selects and
+compacts one client into it, :meth:`fold_topk` folds a co-resident logical client's selection into an accumulator and
+:meth:`pack_nonzero` compacts the folded mean; the collective's owners add the lists into a shared-memory tile on peer
+loads (the switch cannot add sparse lists).  ``cap = k``, or ``min(n, max_clients * k)`` for ``max_clients`` folded
+clients.  The optimizer-emitted upload is off: the selection needs all of ``u``.
+
 Both take ``server_opt=ServerOptConfig(...)`` (``parallel/server_opt.py``): FedAvgM, FedAdagrad, FedYogi or FedAdam
 applied to the round's aggregate, whatever computed it (mean, DP, SCAFFOLD, median, trimmed mean, Krum).  The session
 allocates the state ``arena.server_m`` / ``arena.server_v`` over the parameters, replicated on every rank; the fused
@@ -48,6 +57,7 @@ from typing import List, Optional, Sequence
 import torch
 
 from .arena import ParamArena
+from .compress import TopKConfig, check_topk_exclusions, n_float, sparse_upload_bytes, topk_ef_
 from .dp import DPConfig, clip_factor, normals
 from .robust import MAX_ROBUST_CLIENTS, RobustConfig, krum_select, robust_combine
 from .server_opt import ServerOptConfig, apply_update_
@@ -74,8 +84,12 @@ def _check_scaffold(scaffold: bool, dp: Optional[DPConfig], delta: bool) -> None
 
 
 def _check_robust(robust: Optional[RobustConfig], dp: Optional[DPConfig], scaffold: bool, delta: bool,
-                  tile_flags: bool, max_clients: int) -> int:
+                  tile_flags: bool, max_clients: int, topk: Optional[TopKConfig] = None) -> int:
     if robust is None:
+        if topk is not None:      # the folded clients' union of supports sizes the sparse segment
+            if int(max_clients) < 1:
+                raise ValueError("max_clients must be >= 1, got {!r}".format(max_clients))
+            return int(max_clients)
         if int(max_clients) != 1:
             raise ValueError("max_clients > 1 needs a robust aggregator: plain rounds fold their clients into one upload")
         return 1
@@ -93,6 +107,17 @@ def _check_robust(robust: Optional[RobustConfig], dp: Optional[DPConfig], scaffo
     if not (1 <= int(max_clients) <= MAX_ROBUST_CLIENTS):
         raise ValueError("max_clients must be in 1..{}, got {!r}".format(MAX_ROBUST_CLIENTS, max_clients))
     return int(max_clients)
+
+
+def _check_topk(topk: Optional[TopKConfig], wire_dtype: str, dp, robust, scaffold: bool, delta: bool,
+                tile_flags: bool) -> Optional[TopKConfig]:
+    if topk is None:
+        return None
+    if not isinstance(topk, TopKConfig):
+        raise TypeError("topk= takes a TopKConfig")
+    check_topk_exclusions(wire_dtype=wire_dtype, dp=dp, robust=robust, scaffold=scaffold, delta=delta,
+                          tile_flags=tile_flags)
+    return topk
 
 
 def _init_server_opt(arena: ParamArena, server_opt: Optional[ServerOptConfig], delta: bool) -> Optional[ServerOptConfig]:
@@ -132,15 +157,16 @@ class FedAvgSession:
                  nvls: "bool | str" = "auto", n_ctas: Optional[int] = None, tile_elems: int = 0, timeout_log2: int = 24,
                  reset_momentum: bool = True, tile_flags: bool = False, dp: Optional[DPConfig] = None,
                  scaffold: bool = False, robust: Optional[RobustConfig] = None, max_clients: int = 1,
-                 server_opt: Optional[ServerOptConfig] = None):
+                 server_opt: Optional[ServerOptConfig] = None, topk: Optional[TopKConfig] = None):
         from ..ops._ext import load
         self._C = load()
         assert wire_dtype in ("bf16", "fp32", "fp8") and mode in ("delta", "weights")
+        self.topk = _check_topk(topk, wire_dtype, dp, robust, scaffold, mode == "delta", tile_flags)
         self.server_opt = _init_server_opt(arena, server_opt, mode == "delta")
         self._sopt_coef = list(server_opt.coefficients()) if server_opt is not None else []
         _check_dp_mode(dp, mode == "delta")
         _check_scaffold(scaffold, dp, mode == "delta")
-        self.max_clients = _check_robust(robust, dp, scaffold, mode == "delta", tile_flags, max_clients)
+        self.max_clients = _check_robust(robust, dp, scaffold, mode == "delta", tile_flags, max_clients, self.topk)
         self.robust = robust
         self.krum = robust is not None and robust.kind == "krum"
         self.scaffold = bool(scaffold)
@@ -168,6 +194,15 @@ class FedAvgSession:
         # robust: S client segments per half, seg_stride bytes apart (2 * S * seg_stride bytes of symmetric memory)
         self.seg_stride = _align(self._seg_bytes(arena.n), 256)
         half = self.max_clients * self.seg_stride if robust is not None else self.wire_bytes()
+        if self.topk is not None:
+            if arena.n % self.FLAG_GRANULE:
+                raise ValueError("top-k uploads need an arena of whole 1024-element granules")
+            self.topk_k = self.topk.k(n_float(arena))
+            self.topk_cap = min(arena.n, self.max_clients * self.topk_k)
+            self.topk_rowptr_off = _align(self._seg_bytes(arena.n), 256)
+            self.topk_off_off = self.topk_rowptr_off + _align(4 * (arena.n // self.FLAG_GRANULE + 1), 256)
+            self.topk_val_off = self.topk_off_off + _align(2 * self.topk_cap, 256)
+            half = self.topk_val_off + self.topk_cap * (4 if wire_dtype == "fp32" else 2)
         self.half_wire = _align(half, 2 << 20)                        # multicast-friendly granularity
         self.half_int = _align(max(arena.n_int, 1) * 8, 256)
         self.half_loss = _align(MAX_LOSS * 4, 256)
@@ -188,10 +223,14 @@ class FedAvgSession:
         if self.wire_kind == 2:
             self.use_nvls = False      # the switch adds raw elements; block scales need the P2P path
         self.dp = _agree_seed(dp, group)
-        if self.dp is not None or self.scaffold or self.robust is not None:
-            # the clip factors / the 1 / N of the control variates are applied by the readers, and a selection is not
-            # a sum: peer loads only
+        if self.dp is not None or self.scaffold or self.robust is not None or self.topk is not None:
+            # the clip factors / the 1 / N of the control variates are applied by the readers, a selection is not
+            # a sum, and the switch cannot add sparse lists: peer loads only
             self.use_nvls = False
+        self._topk_work = None          # top-k: the selection's scratch, the residual-less u, the last upload's row end
+        self._topk_u = None
+        self._topk_end = None
+        self._topk_sent = None
         self._packed_epoch = None   # robust: barrier epoch whose wire half pack_client filled
         if self.krum:   # the rank step's per-CTA partials and counters, and the host report (csrc/launch.h)
             self.krum_work = torch.zeros(self._C.KRUM_MAX_CTAS * self._C.KRUM_PAIRS, dtype=torch.float64,
@@ -295,7 +334,7 @@ class FedAvgSession:
     def pack_spec(self) -> Optional[dict]:
         """Arguments for ``ops.fused_sgd(pack=...)`` (stable device tensors: safe to capture), or None when the wire
         format needs the in-kernel pack (block-scaled fp8)."""
-        if self.wire_kind == 2 or self.device.type != "cuda":
+        if self.wire_kind == 2 or self.device.type != "cuda" or self.topk is not None:
             return None
         a = self.arena
         return {"wire_slot": self.wire_slot, "global_w": a.global_w if self.delta else None, "scale": self.pack_scale,
@@ -331,6 +370,78 @@ class FedAvgSession:
         self._C.pack_client(self.segment_ptr(j), a.theta, a.global_w, a.theta_bf16,
                             a.momentum if reset else None, self.wire_kind, bool(reset))
         self._packed_epoch = self.epoch
+
+    # ------------------------------------------------------------------ top-k rounds: sparse uploads
+    def _topk_lists(self):
+        if self.topk is None:
+            raise RuntimeError("top-k uploads need a session built with topk=")
+        if self._topk_work is None:
+            from ..ops import functional as F
+            self._topk_work = F.topk_work(self.arena.n, self.device)
+        base = self.segment_ptr(0)
+        par = (self.epoch // 3) & 1
+        self._topk_end = (self.epoch, self.off_wire + par * self.half_wire + self.topk_rowptr_off
+                          + 4 * (self.arena.n // self.FLAG_GRANULE))
+        return base + self.topk_rowptr_off, base + self.topk_off_off, base + self.topk_val_off
+
+    def _topk_residual(self, e: Optional[torch.Tensor]) -> torch.Tensor:
+        if self.topk.error_feedback:
+            if e is None or e.dtype != torch.float32 or e.numel() != self.arena.n:
+                raise ValueError("error feedback needs the client's fp32 residual over the arena")
+            return e
+        if self._topk_u is None:
+            self._topk_u = torch.empty_like(self.arena.theta)
+        return self._topk_u
+
+    def pack_topk(self, e: Optional[torch.Tensor] = None) -> None:
+        """Upload the replica's client as its top-k list for the upcoming round: ``u = (theta - global) + e``, the ``k``
+        largest ``|u|`` into the sparse segment, ``e`` = the rest (``e``: the client's residual, required with error
+        feedback and ignored without).  Runs on the current stream."""
+        from ..ops import functional as F
+        a = self.arena
+        u = self._topk_residual(e)
+        rowptr, off, val = self._topk_lists()
+        F.topk_pack(a.theta, a.global_w, u, self.topk_k, self._topk_work, rowptr, off, val,
+                    ef=self.topk.error_feedback, wire_fp32=self.wire_kind == 0, cap=self.topk_cap)
+        self._packed_epoch = self.epoch
+
+    def fold_topk(self, acc: torch.Tensor, e: Optional[torch.Tensor], nk: float, first: bool, reset: bool) -> None:
+        """A co-resident logical client: ``acc (+)= nk * topk(u)`` (``first``: from 0), its residual updated, and
+        (``reset``) the replica returned to the global model for the next one.  :meth:`pack_nonzero` uploads the fold."""
+        from ..ops import functional as F
+        a = self.arena
+        u = self._topk_residual(e)
+        if self._topk_work is None:
+            self._topk_work = F.topk_work(a.n, self.device)
+        F.topk_fold(a.theta, a.global_w, u, self.topk_k, self._topk_work, acc, nk, ef=self.topk.error_feedback,
+                    first=first, reset=reset, w_bf16=a.theta_bf16, momentum=a.momentum)
+
+    def pack_nonzero(self) -> None:
+        """Upload ``theta - global`` where it is non-zero (the folded mean of the hosted clients: at most ``cap``
+        entries, the union of their supports)."""
+        from ..ops import functional as F
+        a = self.arena
+        rowptr, off, val = self._topk_lists()
+        F.nonzero_pack(a.theta, a.global_w, self._topk_work, rowptr, off, val, wire_fp32=self.wire_kind == 0,
+                       cap=self.topk_cap)
+        self._packed_epoch = self.epoch
+
+    def last_upload_entries(self) -> int:
+        """Entries of this rank's upload in the last top-k round (a host read; 0 when it sent none)."""
+        if self.topk is None:
+            raise RuntimeError("last_upload_entries needs a session built with topk=")
+        if self._topk_sent is None:
+            return 0
+        self.join()
+        return int(self.symm.view(self._topk_sent, 1, torch.int32).item())
+
+    def last_upload_bytes(self) -> int:
+        """Bytes of this rank's upload in the last round: the sparse list of a top-k round, else :meth:`wire_bytes`."""
+        if self.topk is None:
+            return self.wire_bytes()
+        if self._topk_sent is None:
+            return 0
+        return sparse_upload_bytes(self.arena.n, self.last_upload_entries(), self.wire_dtype)
 
     # ------------------------------------------------------------------ the collective
     def aggregate(self, n_samples_by_rank: Optional[Sequence[float]] = None,
@@ -371,6 +482,8 @@ class FedAvgSession:
         if control is not None and dp is not None:
             raise ValueError("SCAFFOLD and DP-FedAvg are exclusive")
         robust = robust if robust is not None else self.robust
+        if self.topk is not None and (dp is not None or robust is not None):
+            raise ValueError("a top-k session runs top-k rounds only (no DP-FedAvg or robust rounds)")
         if robust is not None and robust is not self.robust:
             _check_robust(robust, dp, self.scaffold, self.delta, self.tile_flags is not None, 1)
         if robust is None and n_clients is not None:
@@ -427,7 +540,8 @@ class FedAvgSession:
         else:   # one tile per (live rank, CTA): n / (A * G), rounded up to a multiple of 8 elements
             per = -(-a.n // (len(alive) * self.n_ctas))
             tile = max(self.min_tile, (per + 31) // 32 * 32)
-        if self.tile_flags is not None:      # arrival flags cover fixed 1024-element granules: tiles must not split one
+        if self.tile_flags is not None or self.topk is not None:
+            # arrival flags and sparse rows cover fixed 1024-element granules: tiles must not split one
             tile = (tile + self.FLAG_GRANULE - 1) // self.FLAG_GRANULE * self.FLAG_GRANULE
         self.last_tile_elems = tile
         flag_value = self.rounds + 1
@@ -441,6 +555,25 @@ class FedAvgSession:
             self.epoch_word.fill_(flag_value)       # compute stream: whatever is enqueued after this call waits for THIS round
         if on_side_stream:
             stream.wait_stream(cur)
+        if self.topk is not None:
+            if counts[self.rank] != 0.0 and self._packed_epoch != self.epoch:
+                raise RuntimeError("a top-k round needs this rank's upload packed for it (pack_topk or pack_nonzero "
+                                   "before aggregate, with the same round index)")
+            self._topk_sent = self._topk_end[1] if counts[self.rank] != 0.0 else None
+            self._packed_epoch = None
+            with torch.cuda.stream(stream):
+                self._C.fedavg_allreduce_topk(
+                    self.symm.peer_ptrs(o_wire), self.symm.peer_ptrs(self.off_pads),
+                    a.theta, a.global_w, a.theta_bf16, a.momentum if self.reset_momentum else None,
+                    a.int_arena if a.n_int > 0 else None, self.symm.peer_ptrs(o_int) if a.n_int > 0 else [],
+                    self.loss_local, self.symm.peer_ptrs(o_loss), self.loss_out,
+                    counts, from_flags, mask, self.rank, world, self.wire_kind, self.epoch, tile, self.n_ctas,
+                    self.timeout_log2, self.status, self.phase_ns, self.topk_rowptr_off, self.topk_off_off,
+                    self.topk_val_off, *self._sopt_args())
+            self.epoch = (self.epoch + 3) & 0xFFFFFFFF
+            self.rounds += 1
+            self._side_pending = on_side_stream
+            return
         if robust is not None and robust.kind == "krum":
             o_dist = self.off_dist + par * self.half_dist
             k_tab, m_tab = robust.krum_tables()
@@ -625,12 +758,18 @@ class NcclSession:
     def __init__(self, arena: ParamArena, group=None, *, wire_dtype: str = "bf16", mode: str = "delta",
                  reset_momentum: bool = True, dp: Optional[DPConfig] = None, scaffold: bool = False,
                  robust: Optional[RobustConfig] = None, max_clients: int = 1, tile_flags: bool = False,
-                 server_opt: Optional[ServerOptConfig] = None, **_unused):
+                 server_opt: Optional[ServerOptConfig] = None, topk: Optional[TopKConfig] = None, **_unused):
         import torch.distributed as dist
+        self.topk = _check_topk(topk, wire_dtype, dp, robust, scaffold, mode == "delta", tile_flags)
         self.server_opt = _init_server_opt(arena, server_opt, mode == "delta")
         _check_dp_mode(dp, mode == "delta")
         _check_scaffold(scaffold, dp, mode == "delta")
-        self.max_clients = _check_robust(robust, dp, scaffold, mode == "delta", tile_flags, max_clients)
+        self.max_clients = _check_robust(robust, dp, scaffold, mode == "delta", tile_flags, max_clients, self.topk)
+        # top-k: k, this rank's upload of the round as a dense fp32 vector (zeros off its support) and its entry count
+        self.topk_k = self.topk.k(n_float(arena)) if self.topk is not None else 0
+        self._topk_up = None
+        self._topk_entries = None
+        self._topk_sent = None
         self.robust = robust
         self._last_krum = None
         self.scaffold = bool(scaffold)
@@ -669,6 +808,59 @@ class NcclSession:
             a.sync_shadow()
             if a.momentum is not None:
                 a.momentum.zero_()
+
+    def _topk_residual(self, e: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+        if self.topk is None:
+            raise RuntimeError("top-k uploads need a session built with topk=")
+        if not self.topk.error_feedback:
+            return None
+        if e is None or e.dtype != torch.float32 or e.numel() != self.arena.n:
+            raise ValueError("error feedback needs the client's fp32 residual over the arena")
+        return e
+
+    @torch.no_grad()
+    def pack_topk(self, e: Optional[torch.Tensor] = None) -> None:
+        """This rank's upload = ``topk(u)`` of the replica's client, ``e`` updated (as :meth:`FedAvgSession.pack_topk`,
+        through the host rule :func:`topk_ef_`)."""
+        a = self.arena
+        idx, vals = topk_ef_(a.theta, a.global_w, self._topk_residual(e), self.topk_k)
+        self._topk_up = torch.zeros_like(a.theta)
+        self._topk_up[idx] = vals
+        self._topk_entries = int(idx.numel())
+
+    @torch.no_grad()
+    def fold_topk(self, acc: torch.Tensor, e: Optional[torch.Tensor], nk: float, first: bool, reset: bool) -> None:
+        """``acc (+)= nk * topk(u)`` of the replica's client, ``e`` updated, and (``reset``) the replica reset."""
+        a = self.arena
+        idx, vals = topk_ef_(a.theta, a.global_w, self._topk_residual(e), self.topk_k)
+        if first:
+            acc.zero_()
+        acc[idx] += vals * float(nk)
+        if reset:
+            a.theta.copy_(a.global_w)
+            a.sync_shadow()
+            if a.momentum is not None:
+                a.momentum.zero_()
+
+    @torch.no_grad()
+    def pack_nonzero(self) -> None:
+        """This rank's upload = ``theta - global`` (the folded mean of its clients), entries where they differ."""
+        a = self.arena
+        self._topk_up = a.theta - a.global_w
+        self._topk_entries = int((a.theta != a.global_w).sum())
+
+    def last_upload_entries(self) -> int:
+        if self.topk is None:
+            raise RuntimeError("last_upload_entries needs a session built with topk=")
+        return self._topk_sent or 0
+
+    def last_upload_bytes(self) -> int:
+        if self.topk is None:
+            return self.wire_bytes()
+        if self._topk_sent is None:
+            return 0
+        return sparse_upload_bytes(self.arena.n, self._topk_sent,
+                                   "bf16" if self.wire_dtype == torch.bfloat16 else "fp32")
 
     def _robust_update(self, counts, n_clients, robust: RobustConfig) -> torch.Tensor:
         """All-gather every rank's segments (padded to ``max_clients``) and their counts; ``robust_combine`` over the
@@ -733,6 +925,15 @@ class NcclSession:
         w = counts[self.rank] / total
         src = (a.theta - a.global_w) if self.delta else a.theta
         robust = robust if robust is not None else self.robust
+        if self.topk is not None:
+            if dp is not None or robust is not None:
+                raise ValueError("a top-k session runs top-k rounds only (no DP-FedAvg or robust rounds)")
+            mine = float(counts[self.rank]) != 0.0
+            if mine and self._topk_up is None:
+                raise RuntimeError("a top-k round needs this rank's upload packed for it (pack_topk or pack_nonzero)")
+            src = self._topk_up if mine else torch.zeros_like(a.theta)
+            self._topk_sent = self._topk_entries if mine else None
+            self._topk_up = None
         if robust is not None:
             upd = self._robust_update(counts, n_clients, robust)
             w = w if float(total) > 0.0 else torch.zeros_like(w)
