@@ -578,12 +578,12 @@ static void fill_fedavg_args(FedAvgArgs& a, const std::vector<int64_t>& wire_ptr
     TORCH_CHECK(phase_ns->scalar_type() == at::kLong && phase_ns->numel() >= 16, "phase_ns: int64[16]");
     a.phase_ns = reinterpret_cast<unsigned long long*>(phase_ns->data_ptr<int64_t>());
   }
+  TORCH_CHECK(!delta || a.global_w != nullptr, "delta mode needs the global copy");
+  TORCH_CHECK(!use_nvls || a.wire_mc != nullptr, "NVLS mode needs the multicast address");
 }
 
-// server optimizer (parallel/server_opt.py): m given -> the *_sopt kernel of the round, with the state over the first
-// n_param elements and the six fp32 coefficients
-static bool want_sopt(const std::optional<at::Tensor>& m) { return m.has_value() && m->defined(); }
-
+// server optimizer (parallel/server_opt.py): the round's args with the state over the first n_param elements and the six
+// fp32 coefficients
 template <class Base>
 static ServerOptArgs<Base> sopt_args(const Base& a, const std::optional<at::Tensor>& m, const std::optional<at::Tensor>& v,
                                      int64_t n_param, int64_t kind, const std::vector<double>& coef) {
@@ -611,6 +611,22 @@ static ServerOptArgs<Base> sopt_args(const Base& a, const std::optional<at::Tens
   return s;
 }
 
+// One round of a's kind (b200_fedavg_round); sopt_m given: with the server optimizer in the apply phase
+template <class Base>
+static void launch_round(const at::Tensor& theta, const Base& a, int64_t n_ctas, const char* name,
+                         const std::optional<at::Tensor>& sopt_m, const std::optional<at::Tensor>& sopt_v,
+                         int64_t sopt_n_param, int64_t sopt_kind, const std::vector<double>& sopt_coef) {
+  const c10::cuda::CUDAGuard guard(theta.device());
+  if (sopt_m.has_value() && sopt_m->defined()) {
+    const auto so = sopt_args(a, sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
+    check(b200_fedavg_round(&so, static_cast<int>(n_ctas), cur_stream()), name);
+  } else {
+    check(b200_fedavg_round(&a, static_cast<int>(n_ctas), cur_stream()), name);
+  }
+}
+
+// Every binding of the collective takes the same leading arguments, wire_ptrs .. prepacked (fill_fedavg_args plus
+// n_ctas), then its own, then the server optimizer's (m, v, n_param, kind, coefficients; m None: off).
 void fedavg_allreduce(const std::vector<int64_t>& wire_ptrs, const std::vector<int64_t>& pad_ptrs, int64_t wire_mc,
                       at::Tensor theta, const std::optional<at::Tensor>& global_w,
                       const std::optional<at::Tensor>& theta_bf16, const std::optional<at::Tensor>& momentum,
@@ -630,7 +646,6 @@ void fedavg_allreduce(const std::vector<int64_t>& wire_ptrs, const std::vector<i
   fill_fedavg_args(a, wire_ptrs, pad_ptrs, wire_mc, theta, global_w, theta_bf16, momentum, int_local, int_wire_ptrs,
                    loss_local, loss_wire_ptrs, loss_out, n_samples, counts_from_flags, alive_mask, rank, world, wire_kind,
                    delta, use_nvls, epoch, tile_flags, flag_value, tile_elems, timeout_log2, status, phase_ns, prepacked);
-  const c10::cuda::CUDAGuard guard(theta.device());
   // DP-FedAvg: one clip page per rank (empty = off); the seed is the 64-bit Philox key, passed as its int64 bit pattern
   const bool dp = !clip_page_ptrs.empty();
   if (dp) {
@@ -641,8 +656,6 @@ void fedavg_allreduce(const std::vector<int64_t>& wire_ptrs, const std::vector<i
     a.round = static_cast<uint32_t>(dp_round);
     TORCH_CHECK(delta && !use_nvls, "DP needs delta mode on peer loads");
   }
-  TORCH_CHECK(!delta || a.global_w != nullptr, "delta mode needs the global copy");
-  TORCH_CHECK(!use_nvls || a.wire_mc != nullptr, "NVLS mode needs the multicast address");
   // SCAFFOLD: the control-variate segment (dc in, c updated) rides in the same launch
   if (scaf_c.has_value() && scaf_c->defined()) {
     TORCH_CHECK(!dp && delta && !use_nvls, "SCAFFOLD rounds need delta mode on peer loads, without DP");
@@ -656,47 +669,34 @@ void fedavg_allreduce(const std::vector<int64_t>& wire_ptrs, const std::vector<i
     sa.n_c = scaf_c->numel();
     sa.seg1_off = scaf_seg1_off;
     sa.inv_clients = static_cast<float>(scaf_inv_clients);
-    if (want_sopt(sopt_m)) {
-      const auto so = sopt_args(sa, sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
-      check(b200_fedavg_allreduce_scaffold_sopt(&so, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce");
-      return;
-    }
-    check(b200_fedavg_allreduce_scaffold(&sa, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce");
-    return;
+    launch_round(theta, sa, n_ctas, "fedavg_allreduce", sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
+  } else if (dp) {
+    launch_round(theta, a, n_ctas, "fedavg_allreduce", sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
+  } else {
+    launch_round(theta, static_cast<const FedAvgArgs&>(a), n_ctas, "fedavg_allreduce", sopt_m, sopt_v, sopt_n_param,
+                 sopt_kind, sopt_coef);
   }
-  if (want_sopt(sopt_m)) {
-    if (dp) {
-      const auto so = sopt_args(a, sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
-      check(b200_fedavg_allreduce_dp_sopt(&so, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce");
-    } else {
-      const auto so = sopt_args(static_cast<const FedAvgArgs&>(a), sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
-      check(b200_fedavg_allreduce_sopt(&so, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce");
-    }
-    return;
-  }
-  check(dp ? b200_fedavg_allreduce_dp(&a, static_cast<int>(n_ctas), cur_stream())
-           : b200_fedavg_allreduce(&a, static_cast<int>(n_ctas), cur_stream()),
-        "fedavg_allreduce");
 }
 
 // robust round: seg_page_ptrs = every rank's count page, trim_b = floor(beta * P) for P = 0 .. 32 (trimmed mean)
 void fedavg_allreduce_robust(const std::vector<int64_t>& wire_ptrs, const std::vector<int64_t>& pad_ptrs,
-                             at::Tensor theta, const at::Tensor& global_w, const std::optional<at::Tensor>& theta_bf16,
-                             const std::optional<at::Tensor>& momentum, const std::optional<at::Tensor>& int_local,
-                             const std::vector<int64_t>& int_wire_ptrs, const std::optional<at::Tensor>& loss_local,
-                             const std::vector<int64_t>& loss_wire_ptrs, const std::optional<at::Tensor>& loss_out,
-                             const std::vector<double>& n_samples, bool counts_from_flags, int64_t alive_mask, int64_t rank,
-                             int64_t world, int64_t wire_kind, int64_t epoch, int64_t tile_elems, int64_t n_ctas,
-                             int64_t timeout_log2, const std::optional<at::Tensor>& status,
-                             const std::optional<at::Tensor>& phase_ns, bool prepacked,
-                             const std::vector<int64_t>& seg_page_ptrs, int64_t my_segs, int64_t seg_stride, int64_t kind,
-                             const std::vector<int64_t>& trim_b,
+                             int64_t wire_mc, at::Tensor theta, const std::optional<at::Tensor>& global_w,
+                             const std::optional<at::Tensor>& theta_bf16, const std::optional<at::Tensor>& momentum,
+                             const std::optional<at::Tensor>& int_local, const std::vector<int64_t>& int_wire_ptrs,
+                             const std::optional<at::Tensor>& loss_local, const std::vector<int64_t>& loss_wire_ptrs,
+                             const std::optional<at::Tensor>& loss_out, const std::vector<double>& n_samples,
+                             bool counts_from_flags, int64_t alive_mask, int64_t rank, int64_t world, int64_t wire_kind,
+                             bool delta, bool use_nvls, int64_t epoch, const std::optional<at::Tensor>& tile_flags,
+                             int64_t flag_value, int64_t tile_elems, int64_t n_ctas, int64_t timeout_log2,
+                             const std::optional<at::Tensor>& status, const std::optional<at::Tensor>& phase_ns,
+                             bool prepacked, const std::vector<int64_t>& seg_page_ptrs, int64_t my_segs,
+                             int64_t seg_stride, int64_t kind, const std::vector<int64_t>& trim_b,
                              const std::optional<at::Tensor>& sopt_m, const std::optional<at::Tensor>& sopt_v,
                              int64_t sopt_n_param, int64_t sopt_kind, const std::vector<double>& sopt_coef) {
   FedAvgRobustArgs a = {};
-  fill_fedavg_args(a, wire_ptrs, pad_ptrs, 0, theta, global_w, theta_bf16, momentum, int_local, int_wire_ptrs, loss_local,
-                   loss_wire_ptrs, loss_out, n_samples, counts_from_flags, alive_mask, rank, world, wire_kind, true, false,
-                   epoch, std::nullopt, 0, tile_elems, timeout_log2, status, phase_ns, prepacked);
+  fill_fedavg_args(a, wire_ptrs, pad_ptrs, wire_mc, theta, global_w, theta_bf16, momentum, int_local, int_wire_ptrs,
+                   loss_local, loss_wire_ptrs, loss_out, n_samples, counts_from_flags, alive_mask, rank, world, wire_kind,
+                   delta, use_nvls, epoch, tile_flags, flag_value, tile_elems, timeout_log2, status, phase_ns, prepacked);
   TORCH_CHECK(static_cast<int64_t>(seg_page_ptrs.size()) == world, "robust: one count page per rank");
   TORCH_CHECK(static_cast<int64_t>(trim_b.size()) == B200_MAX_ROBUST_CLIENTS + 1, "robust: trim_b for P = 0 .. 32");
   TORCH_CHECK(my_segs >= 0 && my_segs <= B200_MAX_ROBUST_CLIENTS, "robust: at most 32 segments per rank");
@@ -708,36 +708,31 @@ void fedavg_allreduce_robust(const std::vector<int64_t>& wire_ptrs, const std::v
   a.my_segs = static_cast<uint32_t>(my_segs);
   a.seg_stride = seg_stride;
   a.kind = static_cast<int>(kind);
-  const c10::cuda::CUDAGuard guard(theta.device());
-  if (want_sopt(sopt_m)) {
-    const auto so = sopt_args(a, sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
-    check(b200_fedavg_allreduce_robust_sopt(&so, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_robust");
-    return;
-  }
-  check(b200_fedavg_allreduce_robust(&a, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_robust");
+  launch_round(theta, a, n_ctas, "fedavg_allreduce_robust", sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
 }
 
-// Multi-Krum round: the robust round's arguments plus every rank's distance page, the local work / sync / report
+// Multi-Krum round: the robust round's count pages plus every rank's distance page, the local work / sync / report
 // buffers and the per-P tables k and m (the kept mean runs as the trimmed mean with b = 0)
-void fedavg_allreduce_krum(const std::vector<int64_t>& wire_ptrs, const std::vector<int64_t>& pad_ptrs, at::Tensor theta,
-                           const at::Tensor& global_w, const std::optional<at::Tensor>& theta_bf16,
-                           const std::optional<at::Tensor>& momentum, const std::optional<at::Tensor>& int_local,
-                           const std::vector<int64_t>& int_wire_ptrs, const std::optional<at::Tensor>& loss_local,
-                           const std::vector<int64_t>& loss_wire_ptrs, const std::optional<at::Tensor>& loss_out,
-                           const std::vector<double>& n_samples, bool counts_from_flags, int64_t alive_mask, int64_t rank,
-                           int64_t world, int64_t wire_kind, int64_t epoch, int64_t tile_elems, int64_t n_ctas,
-                           int64_t timeout_log2, const std::optional<at::Tensor>& status,
-                           const std::optional<at::Tensor>& phase_ns, bool prepacked,
-                           const std::vector<int64_t>& seg_page_ptrs, int64_t my_segs, int64_t seg_stride,
+void fedavg_allreduce_krum(const std::vector<int64_t>& wire_ptrs, const std::vector<int64_t>& pad_ptrs, int64_t wire_mc,
+                           at::Tensor theta, const std::optional<at::Tensor>& global_w,
+                           const std::optional<at::Tensor>& theta_bf16, const std::optional<at::Tensor>& momentum,
+                           const std::optional<at::Tensor>& int_local, const std::vector<int64_t>& int_wire_ptrs,
+                           const std::optional<at::Tensor>& loss_local, const std::vector<int64_t>& loss_wire_ptrs,
+                           const std::optional<at::Tensor>& loss_out, const std::vector<double>& n_samples,
+                           bool counts_from_flags, int64_t alive_mask, int64_t rank, int64_t world, int64_t wire_kind,
+                           bool delta, bool use_nvls, int64_t epoch, const std::optional<at::Tensor>& tile_flags,
+                           int64_t flag_value, int64_t tile_elems, int64_t n_ctas, int64_t timeout_log2,
+                           const std::optional<at::Tensor>& status, const std::optional<at::Tensor>& phase_ns,
+                           bool prepacked, const std::vector<int64_t>& seg_page_ptrs, int64_t my_segs, int64_t seg_stride,
                            const std::vector<int64_t>& dist_page_ptrs, at::Tensor work, at::Tensor sync,
                            const std::optional<at::Tensor>& report, const std::vector<int64_t>& krum_k,
                            const std::vector<int64_t>& krum_m,
                            const std::optional<at::Tensor>& sopt_m, const std::optional<at::Tensor>& sopt_v,
                            int64_t sopt_n_param, int64_t sopt_kind, const std::vector<double>& sopt_coef) {
   FedAvgKrumArgs a = {};
-  fill_fedavg_args(a, wire_ptrs, pad_ptrs, 0, theta, global_w, theta_bf16, momentum, int_local, int_wire_ptrs, loss_local,
-                   loss_wire_ptrs, loss_out, n_samples, counts_from_flags, alive_mask, rank, world, wire_kind, true, false,
-                   epoch, std::nullopt, 0, tile_elems, timeout_log2, status, phase_ns, prepacked);
+  fill_fedavg_args(a, wire_ptrs, pad_ptrs, wire_mc, theta, global_w, theta_bf16, momentum, int_local, int_wire_ptrs,
+                   loss_local, loss_wire_ptrs, loss_out, n_samples, counts_from_flags, alive_mask, rank, world, wire_kind,
+                   delta, use_nvls, epoch, tile_flags, flag_value, tile_elems, timeout_log2, status, phase_ns, prepacked);
   TORCH_CHECK(static_cast<int64_t>(seg_page_ptrs.size()) == world, "krum: one count page per rank");
   TORCH_CHECK(static_cast<int64_t>(dist_page_ptrs.size()) == world, "krum: one distance page per rank");
   TORCH_CHECK(static_cast<int64_t>(krum_k.size()) == B200_MAX_ROBUST_CLIENTS + 1 &&
@@ -773,41 +768,31 @@ void fedavg_allreduce_krum(const std::vector<int64_t>& wire_ptrs, const std::vec
                 "krum: report = float64[B200_KRUM_REPORT]");
     a.report = report->data_ptr<double>();
   }
-  const c10::cuda::CUDAGuard guard(theta.device());
-  if (want_sopt(sopt_m)) {
-    const auto so = sopt_args(a, sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
-    check(b200_fedavg_allreduce_krum_sopt(&so, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_krum");
-    return;
-  }
-  check(b200_fedavg_allreduce_krum(&a, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_krum");
+  launch_round(theta, a, n_ctas, "fedavg_allreduce_krum", sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
 }
 
 // top-k round: the sparse lists sit at byte offsets rowptr_off / off_off / val_off of every rank's wire half
-void fedavg_allreduce_topk(const std::vector<int64_t>& wire_ptrs, const std::vector<int64_t>& pad_ptrs, at::Tensor theta,
-                           const at::Tensor& global_w, const std::optional<at::Tensor>& theta_bf16,
-                           const std::optional<at::Tensor>& momentum, const std::optional<at::Tensor>& int_local,
-                           const std::vector<int64_t>& int_wire_ptrs, const std::optional<at::Tensor>& loss_local,
-                           const std::vector<int64_t>& loss_wire_ptrs, const std::optional<at::Tensor>& loss_out,
-                           const std::vector<double>& n_samples, bool counts_from_flags, int64_t alive_mask, int64_t rank,
-                           int64_t world, int64_t wire_kind, int64_t epoch, int64_t tile_elems, int64_t n_ctas,
-                           int64_t timeout_log2, const std::optional<at::Tensor>& status,
-                           const std::optional<at::Tensor>& phase_ns, int64_t rowptr_off, int64_t off_off, int64_t val_off,
+void fedavg_allreduce_topk(const std::vector<int64_t>& wire_ptrs, const std::vector<int64_t>& pad_ptrs, int64_t wire_mc,
+                           at::Tensor theta, const std::optional<at::Tensor>& global_w,
+                           const std::optional<at::Tensor>& theta_bf16, const std::optional<at::Tensor>& momentum,
+                           const std::optional<at::Tensor>& int_local, const std::vector<int64_t>& int_wire_ptrs,
+                           const std::optional<at::Tensor>& loss_local, const std::vector<int64_t>& loss_wire_ptrs,
+                           const std::optional<at::Tensor>& loss_out, const std::vector<double>& n_samples,
+                           bool counts_from_flags, int64_t alive_mask, int64_t rank, int64_t world, int64_t wire_kind,
+                           bool delta, bool use_nvls, int64_t epoch, const std::optional<at::Tensor>& tile_flags,
+                           int64_t flag_value, int64_t tile_elems, int64_t n_ctas, int64_t timeout_log2,
+                           const std::optional<at::Tensor>& status, const std::optional<at::Tensor>& phase_ns,
+                           bool prepacked, int64_t rowptr_off, int64_t off_off, int64_t val_off,
                            const std::optional<at::Tensor>& sopt_m, const std::optional<at::Tensor>& sopt_v,
                            int64_t sopt_n_param, int64_t sopt_kind, const std::vector<double>& sopt_coef) {
   FedAvgTopkArgs a = {};
-  fill_fedavg_args(a, wire_ptrs, pad_ptrs, 0, theta, global_w, theta_bf16, momentum, int_local, int_wire_ptrs, loss_local,
-                   loss_wire_ptrs, loss_out, n_samples, counts_from_flags, alive_mask, rank, world, wire_kind, true, false,
-                   epoch, std::nullopt, 0, tile_elems, timeout_log2, status, phase_ns, true);
+  fill_fedavg_args(a, wire_ptrs, pad_ptrs, wire_mc, theta, global_w, theta_bf16, momentum, int_local, int_wire_ptrs,
+                   loss_local, loss_wire_ptrs, loss_out, n_samples, counts_from_flags, alive_mask, rank, world, wire_kind,
+                   delta, use_nvls, epoch, tile_flags, flag_value, tile_elems, timeout_log2, status, phase_ns, prepacked);
   a.rowptr_off = rowptr_off;
   a.off_off = off_off;
   a.val_off = val_off;
-  const c10::cuda::CUDAGuard guard(theta.device());
-  if (want_sopt(sopt_m)) {
-    const auto so = sopt_args(a, sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
-    check(b200_fedavg_allreduce_topk_sopt(&so, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_topk");
-    return;
-  }
-  check(b200_fedavg_allreduce_topk(&a, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_topk");
+  launch_round(theta, a, n_ctas, "fedavg_allreduce_topk", sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
 }
 
 static void check_topk_io(const at::Tensor& theta, const at::Tensor& global_w, const at::Tensor& work) {
@@ -901,15 +886,6 @@ void fold_client_scaled(at::Tensor acc, at::Tensor theta, const at::Tensor& glob
                                 opt_ptr<void>(wb), opt_ptr<float>(mom), mom.has_value() && mom->defined() ? mom->numel() : 0,
                                 theta.numel(), s.data_ptr<float>(), first, reset, cur_stream()),
         "fold_client_scaled");
-}
-
-void flag_barrier(const std::vector<int64_t>& pad_ptrs, int64_t rank, int64_t world, int64_t alive_mask, int64_t epoch,
-                  int64_t slot) {
-  std::vector<unsigned long long*> pads;
-  for (auto p : pad_ptrs) pads.push_back(reinterpret_cast<unsigned long long*>(p));
-  check(b200_flag_barrier(pads.data(), rank, world, static_cast<uint32_t>(alive_mask), static_cast<uint32_t>(epoch), slot,
-                          cur_stream()),
-        "flag_barrier");
 }
 
 // ---- conv plumbing -------------------------------------------------------------------------------
@@ -1203,7 +1179,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("topk_work_words", [](int64_t n) { return static_cast<int64_t>(B200_TOPK_WORK_WORDS(n)); });
   m.def("pack_client", &pack_client);
   m.attr("MAX_ROBUST_CLIENTS") = B200_MAX_ROBUST_CLIENTS;
-  m.def("flag_barrier", &flag_barrier);
   m.attr("DP_WORK_WORDS") = B200_DP_WORK_WORDS;
   m.def("dp_clip_factor", &dp_clip_factor);
   m.def("fold_client_scaled", &fold_client_scaled);

@@ -983,22 +983,38 @@ __device__ __forceinline__ void sopt_apply_tile(const Args& a, const uint8_t* my
   }
 }
 
-// DP: DP-FedAvg (see launch.h / DESIGN.md): w_k = n_k s_k / N with s_k from rank k's clip page, and the owner of a tile
-// adds sigma C / N * z[i] to its fp32 sum before the cast.  The loss and the integer side arena keep the weights n_k / N.
-// SCAF: a SCAFFOLD round -- segment 1 (the control variates, see seg_pack) rides between the same barriers; every
-// participant weighs 1 / N there.
-// ROBUST: a robust round (robust_reduce above); every rank publishes its segment count before barrier 1.
-// KRUM (with ROBUST): a Multi-Krum round (krum_reduce above): the exchange barrier takes epoch + 2, barrier 2 epoch + 3.
-// SOPT (with any of the above): a server-optimizer round -- the apply phase runs sopt_apply_tile.
-// TOPK: a top-k round (topk_reduce above): no pack phase, the uploads are sparse lists written before the launch.
-// The whole round; Args is FedAvgDPArgs when DP, FedAvgScaffoldArgs when SCAF, FedAvgRobustArgs when ROBUST,
-// FedAvgKrumArgs when KRUM, FedAvgTopkArgs when TOPK, and ServerOptArgs<that> when SOPT.
-template <int WIRE, bool DP, bool SCAF = false, bool ROBUST = false, bool KRUM = false, bool SOPT = false,
-          bool TOPK = false, typename Args>
+// The kind of aggregation a round runs.  Every kind is one args struct of launch.h, and RoundOf maps the struct to its
+// kind (and whether the apply phase runs the server optimizer): fedavg_round_kernel<WIRE, Args> is the round's kernel.
+enum class Agg { mean, dp, scaffold, robust, krum, topk };
+template <class Args> struct RoundOf;
+template <Agg K> struct RoundKind { static constexpr Agg kind = K; static constexpr bool sopt = false; };
+template <> struct RoundOf<FedAvgArgs> : RoundKind<Agg::mean> {};
+template <> struct RoundOf<FedAvgDPArgs> : RoundKind<Agg::dp> {};
+template <> struct RoundOf<FedAvgScaffoldArgs> : RoundKind<Agg::scaffold> {};
+template <> struct RoundOf<FedAvgRobustArgs> : RoundKind<Agg::robust> {};
+template <> struct RoundOf<FedAvgKrumArgs> : RoundKind<Agg::krum> {};
+template <> struct RoundOf<FedAvgTopkArgs> : RoundKind<Agg::topk> {};
+template <class Base> struct RoundOf<ServerOptArgs<Base>> {
+  static constexpr Agg kind = RoundOf<Base>::kind;
+  static constexpr bool sopt = true;
+};
+
+// K == Agg::mean: the weighted mean w_k = n_k / N.
+// Agg::dp: DP-FedAvg (see launch.h / DESIGN.md): w_k = n_k s_k / N with s_k from rank k's clip page, and the owner of a
+// tile adds sigma C / N * z[i] to its fp32 sum before the cast.  The loss and the integer side arena keep the weights
+// n_k / N.
+// Agg::scaffold: a SCAFFOLD round -- segment 1 (the control variates, see seg_pack) rides between the same barriers;
+// every participant weighs 1 / N there.
+// Agg::robust: a robust round (robust_reduce above); every rank publishes its segment count before barrier 1.
+// Agg::krum: a Multi-Krum round (krum_reduce above), a robust round whose exchange barrier takes epoch + 2 and barrier 2
+// epoch + 3.
+// Agg::topk: a top-k round (topk_reduce above): no pack phase, the uploads are sparse lists written before the launch.
+// SOPT (with any kind): a server-optimizer round -- the apply phase runs sopt_apply_tile.
+// The whole round; Args is the kind's args struct (ServerOptArgs<that> when SOPT), see RoundOf.
+template <int WIRE, Agg K, bool SOPT, typename Args>
 __device__ __forceinline__ void fedavg_round(const Args& a) {
-  static_assert(!(DP && SCAF), "DP-FedAvg and SCAFFOLD are exclusive");
-  static_assert(!(ROBUST && (DP || SCAF)), "robust rounds exclude DP-FedAvg and SCAFFOLD");
-  static_assert(!(TOPK && (DP || SCAF || ROBUST)), "top-k rounds exclude DP-FedAvg, SCAFFOLD and robust aggregation");
+  constexpr bool DP = K == Agg::dp, SCAF = K == Agg::scaffold, KRUM = K == Agg::krum, TOPK = K == Agg::topk;
+  constexpr bool ROBUST = K == Agg::robust || KRUM;
   using W = Wire<WIRE>;
   constexpr int VEC = W::VEC;
   constexpr bool SCALED = W::SCALED;
@@ -1376,60 +1392,10 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
 // stays available to small kernels of the NEXT round (batch gather, im2col, the flag-gated weight staging of
 // bcast_gemm) that are launched on the compute stream while this kernel is still running on its side stream -- and
 // a flag-gated consumer that became resident first can never keep this (cooperatively launched) grid from fitting.
-template <int WIRE>
-__global__ void __maxnreg__(96) fedavg_allreduce_kernel(const __grid_constant__ FedAvgArgs a) {
-  fedavg_round<WIRE, false>(a);
-}
-template <int WIRE>
-__global__ void __maxnreg__(96) fedavg_allreduce_dp_kernel(const __grid_constant__ FedAvgDPArgs a) {
-  fedavg_round<WIRE, true>(a);
-}
-template <int WIRE>
-__global__ void __maxnreg__(96) fedavg_allreduce_scaffold_kernel(const __grid_constant__ FedAvgScaffoldArgs a) {
-  fedavg_round<WIRE, false, true>(a);
-}
-// robust round: ROBUST_SMEM bytes of dynamic shared memory (the selection stage), the same 96-register cap
-template <int WIRE>
-__global__ void __maxnreg__(96) fedavg_allreduce_robust_kernel(const __grid_constant__ FedAvgRobustArgs a) {
-  fedavg_round<WIRE, false, false, true>(a);
-}
-// Multi-Krum round: KRUM_SMEM bytes of dynamic shared memory, the same 96-register cap
-template <int WIRE>
-__global__ void __maxnreg__(96) fedavg_allreduce_krum_kernel(const __grid_constant__ FedAvgKrumArgs a) {
-  fedavg_round<WIRE, false, false, true, true>(a);
-}
-// the same five rounds with the server optimizer in the apply phase (kind chosen at run time: one branch per launch)
-template <int WIRE>
-__global__ void __maxnreg__(96) fedavg_allreduce_sopt_kernel(const __grid_constant__ ServerOptArgs<FedAvgArgs> a) {
-  fedavg_round<WIRE, false, false, false, false, true>(a);
-}
-template <int WIRE>
-__global__ void __maxnreg__(96) fedavg_allreduce_dp_sopt_kernel(const __grid_constant__ ServerOptArgs<FedAvgDPArgs> a) {
-  fedavg_round<WIRE, true, false, false, false, true>(a);
-}
-template <int WIRE>
-__global__ void __maxnreg__(96)
-fedavg_allreduce_scaffold_sopt_kernel(const __grid_constant__ ServerOptArgs<FedAvgScaffoldArgs> a) {
-  fedavg_round<WIRE, false, true, false, false, true>(a);
-}
-template <int WIRE>
-__global__ void __maxnreg__(96)
-fedavg_allreduce_robust_sopt_kernel(const __grid_constant__ ServerOptArgs<FedAvgRobustArgs> a) {
-  fedavg_round<WIRE, false, false, true, false, true>(a);
-}
-template <int WIRE>
-__global__ void __maxnreg__(96) fedavg_allreduce_krum_sopt_kernel(const __grid_constant__ ServerOptArgs<FedAvgKrumArgs> a) {
-  fedavg_round<WIRE, false, false, true, true, true>(a);
-}
-
-// top-k round: TOPK_SMEM bytes of dynamic shared memory (the accumulator tile), the same 96-register cap
-template <int WIRE>
-__global__ void __maxnreg__(96) fedavg_allreduce_topk_kernel(const __grid_constant__ FedAvgTopkArgs a) {
-  fedavg_round<WIRE, false, false, false, false, false, true>(a);
-}
-template <int WIRE>
-__global__ void __maxnreg__(96) fedavg_allreduce_topk_sopt_kernel(const __grid_constant__ ServerOptArgs<FedAvgTopkArgs> a) {
-  fedavg_round<WIRE, false, false, false, false, true, true>(a);
+// Robust, Krum and top-k rounds also take dynamic shared memory (ROBUST_SMEM, KRUM_SMEM, TOPK_SMEM: see round_smem).
+template <int WIRE, typename Args>
+__global__ void __maxnreg__(96) fedavg_round_kernel(const __grid_constant__ Args a) {
+  fedavg_round<WIRE, RoundOf<Args>::kind, RoundOf<Args>::sopt>(a);
 }
 
 // one logical client's upload into its wire segment: the phase-0 pack of fedavg_round (delta mode, scale 1) over the
@@ -1479,19 +1445,6 @@ pack_client_kernel(uint8_t* __restrict__ seg, float* __restrict__ theta, const f
           if (mom != nullptr && i < n_mom) *reinterpret_cast<float4*>(mom + i) = make_float4(0.f, 0.f, 0.f, 0.f);
         }
       }
-    }
-  }
-}
-
-// stand-alone cross-GPU barrier on the pads (one CTA): fences host-side phases
-__global__ void flag_barrier_kernel(FedAvgArgs a, int slot) {
-  const int t = threadIdx.x;
-  if (t < a.world && ((a.alive_mask >> t) & 1u)) {
-    fence_sys();
-    st_release_sys_u64(a.pads[t] + (static_cast<size_t>(slot) * B200_MAX_RANKS + a.rank),
-                       static_cast<unsigned long long>(a.epoch) << 32);
-    const unsigned long long* mine = a.pads[a.rank] + (static_cast<size_t>(slot) * B200_MAX_RANKS + t);
-    while (static_cast<int32_t>(static_cast<uint32_t>(ld_acquire_sys_u64(mine) >> 32) - a.epoch) < 0) {
     }
   }
 }
@@ -1580,40 +1533,20 @@ fold_client_scaled_kernel(float* __restrict__ acc, float* __restrict__ theta, co
 // deadlock each other.  It is therefore launched COOPERATIVELY: the runtime refuses a grid that cannot be co-resident
 // (cudaErrorCooperativeLaunchTooLarge) and schedules all CTAs together, also next to work on other streams -- instead
 // of the plain <<<>>> of round 1, which was only safe on an otherwise idle GPU.  The grid is clamped to what
-// cudaOccupancyMaxActiveBlocksPerMultiprocessor allows on this device.
-template <int WIRE, bool DP, bool SCAF, bool ROBUST, bool KRUM, bool SOPT, bool TOPK = false>
-static const void* fedavg_kernel() {
+// cudaOccupancyMaxActiveBlocksPerMultiprocessor allows on this device, cached per kernel (each kind takes its own
+// dynamic shared memory).
+template <int WIRE, class Args>
+static int launch_round_kernel(const Args* args, int n_ctas, cudaStream_t stream) {
   using namespace b200;
-  if constexpr (TOPK) {
-    return SOPT ? reinterpret_cast<const void*>(fedavg_allreduce_topk_sopt_kernel<WIRE>)
-                : reinterpret_cast<const void*>(fedavg_allreduce_topk_kernel<WIRE>);
-  } else if constexpr (SOPT) {
-    if constexpr (KRUM) return reinterpret_cast<const void*>(fedavg_allreduce_krum_sopt_kernel<WIRE>);
-    else if constexpr (ROBUST) return reinterpret_cast<const void*>(fedavg_allreduce_robust_sopt_kernel<WIRE>);
-    else if constexpr (SCAF) return reinterpret_cast<const void*>(fedavg_allreduce_scaffold_sopt_kernel<WIRE>);
-    else if constexpr (DP) return reinterpret_cast<const void*>(fedavg_allreduce_dp_sopt_kernel<WIRE>);
-    else return reinterpret_cast<const void*>(fedavg_allreduce_sopt_kernel<WIRE>);
-  } else {
-    return KRUM ? reinterpret_cast<const void*>(fedavg_allreduce_krum_kernel<WIRE>)
-           : ROBUST ? reinterpret_cast<const void*>(fedavg_allreduce_robust_kernel<WIRE>)
-           : SCAF ? reinterpret_cast<const void*>(fedavg_allreduce_scaffold_kernel<WIRE>)
-           : DP ? reinterpret_cast<const void*>(fedavg_allreduce_dp_kernel<WIRE>)
-                : reinterpret_cast<const void*>(fedavg_allreduce_kernel<WIRE>);
-  }
-}
-
-template <int WIRE, bool DP, bool SCAF, typename Args, bool ROBUST = false, bool KRUM = false, bool SOPT = false,
-          bool TOPK = false>
-static int launch_fedavg(const Args* args, int n_ctas, cudaStream_t stream) {
-  using namespace b200;
+  constexpr Agg K = RoundOf<Args>::kind;
+  constexpr int smem = K == Agg::krum ? KRUM_SMEM : K == Agg::robust ? ROBUST_SMEM : K == Agg::topk ? TOPK_SMEM : 0;
+  const void* kernel = reinterpret_cast<const void*>(fedavg_round_kernel<WIRE, Args>);
   static int max_ctas = -1;
-  const void* kernel = fedavg_kernel<WIRE, DP, SCAF, ROBUST, KRUM, SOPT, TOPK>();
-  const int smem = KRUM ? KRUM_SMEM : ROBUST ? ROBUST_SMEM : TOPK ? TOPK_SMEM : 0;
   if (max_ctas < 0) {
     int dev = 0, sms = 0, per_sm = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (ROBUST || TOPK) {
+    if (smem != 0) {
       cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
       if (e != cudaSuccess) return static_cast<int>(e);
     }
@@ -1622,7 +1555,7 @@ static int launch_fedavg(const Args* args, int n_ctas, cudaStream_t stream) {
     if (max_ctas < 1) max_ctas = 1;
   }
   if (n_ctas > max_ctas) n_ctas = max_ctas;
-  if constexpr (KRUM) {
+  if constexpr (K == Agg::krum) {
     // the rank step's arrival counter and done flag start at zero every launch (also after a timed-out one)
     cudaError_t e = cudaMemsetAsync(args->sync, 0, 2 * sizeof(unsigned int), stream);
     if (e != cudaSuccess) return static_cast<int>(e);
@@ -1633,25 +1566,10 @@ static int launch_fedavg(const Args* args, int n_ctas, cudaStream_t stream) {
   return static_cast<int>(cudaGetLastError());
 }
 
-template <bool DP, bool SCAF, typename Args, bool ROBUST = false, bool KRUM = false, bool SOPT = false>
-static int fedavg_dispatch(const Args* args, int n_ctas, cudaStream_t stream) {
-  using namespace b200;
-  if (args->world > B200_MAX_RANKS || args->n % 8 != 0 || args->tile_elems % 8 != 0) return -2;
-  if (args->tile_flags != nullptr && args->tile_elems % FLAG_GRANULE != 0) return -2;
-  if (n_ctas < 1) n_ctas = 1;
-  if (args->wire_kind == 2) {
-    // block-scaled fp8 wire: 32-element blocks must not straddle tiles, and the switch cannot rescale
-    if (args->tile_elems % 32 != 0 || args->use_nvls) return -2;
-    return launch_fedavg<2, DP, SCAF, Args, ROBUST, KRUM, SOPT>(args, n_ctas, stream);
-  }
-  if (args->wire_kind == 1) return launch_fedavg<1, DP, SCAF, Args, ROBUST, KRUM, SOPT>(args, n_ctas, stream);
-  return launch_fedavg<0, DP, SCAF, Args, ROBUST, KRUM, SOPT>(args, n_ctas, stream);
-}
-
 static bool robust_args_ok(const FedAvgRobustArgs* args) {
   // a selection is not a sum: robust rounds run on peer loads, never on the switch
-  if (args->use_nvls || !args->delta || args->my_segs > B200_MAX_ROBUST_CLIENTS || args->seg_stride % 256 != 0 ||
-      (args->kind != 0 && args->kind != 1) || args->world > B200_MAX_RANKS)
+  if (args->use_nvls || !args->delta || args->tile_flags != nullptr || args->my_segs > B200_MAX_ROBUST_CLIENTS ||
+      args->seg_stride % 256 != 0 || (args->kind != 0 && args->kind != 1) || args->world > B200_MAX_RANKS)
     return false;
   for (int k = 0; k < args->world; ++k)
     if (((args->alive_mask >> k) & 1u) && args->seg_page[k] == nullptr) return false;
@@ -1660,8 +1578,9 @@ static bool robust_args_ok(const FedAvgRobustArgs* args) {
 
 static bool krum_args_ok(const FedAvgKrumArgs* args) {
   // the kept mean is the trimmed mean with b = 0: the host passes kind 1 and a zero trim table
-  if (args->use_nvls || !args->delta || args->my_segs > B200_MAX_ROBUST_CLIENTS || args->seg_stride % 256 != 0 ||
-      args->kind != 1 || args->world > B200_MAX_RANKS || args->work == nullptr || args->sync == nullptr)
+  if (args->use_nvls || !args->delta || args->tile_flags != nullptr || args->my_segs > B200_MAX_ROBUST_CLIENTS ||
+      args->seg_stride % 256 != 0 || args->kind != 1 || args->world > B200_MAX_RANKS || args->work == nullptr ||
+      args->sync == nullptr)
     return false;
   for (int p = 0; p <= B200_MAX_ROBUST_CLIENTS; ++p)
     if (args->trim_b[p] != 0 || args->krum_m[p] > p || (p > 0 && args->krum_m[p] < 1) || args->krum_k[p] >= (p > 0 ? p : 1))
@@ -1685,6 +1604,16 @@ static bool scaffold_args_ok(const FedAvgScaffoldArgs* args) {
            args->n_c % 8 != 0 || args->seg1_off % 16 != 0);
 }
 
+// a sum of sparse lists needs the peer loads (the switch adds dense vectors), the delta, the lists written before the
+// launch, whole granules per tile and aligned list offsets; fp8's block scales have no meaning on a list
+static bool topk_args_ok(const FedAvgTopkArgs* args) {
+  using b200::FLAG_GRANULE;
+  return !(args->use_nvls || !args->delta || !args->prepacked || args->tile_flags != nullptr ||
+           args->world > B200_MAX_RANKS || args->n % FLAG_GRANULE != 0 || args->tile_elems <= 0 ||
+           args->tile_elems % FLAG_GRANULE != 0 || args->rowptr_off % 4 != 0 || args->off_off % 2 != 0 ||
+           args->val_off % 4 != 0 || (args->wire_kind != 0 && args->wire_kind != 1));
+}
+
 // the server step needs the pseudo-gradient (delta mode), the global copy and the state over [0, n_param)
 template <class Base>
 static bool sopt_args_ok(const ServerOptArgs<Base>* args) {
@@ -1693,69 +1622,49 @@ static bool sopt_args_ok(const ServerOptArgs<Base>* args) {
          args->n_param <= args->n;
 }
 
-extern "C" int b200_fedavg_allreduce_robust(const FedAvgRobustArgs* args, int n_ctas, cudaStream_t stream) {
-  if (!robust_args_ok(args)) return -2;
-  return fedavg_dispatch<false, false, FedAvgRobustArgs, true>(args, n_ctas, stream);
-}
-
-extern "C" int b200_fedavg_allreduce_krum(const FedAvgKrumArgs* args, int n_ctas, cudaStream_t stream) {
-  if (!krum_args_ok(args)) return -2;
-  if (n_ctas > B200_KRUM_MAX_CTAS) n_ctas = B200_KRUM_MAX_CTAS;
-  return fedavg_dispatch<false, false, FedAvgKrumArgs, true, true>(args, n_ctas, stream);
-}
-
-extern "C" int b200_fedavg_allreduce_sopt(const ServerOptArgs<FedAvgArgs>* args, int n_ctas, cudaStream_t stream) {
-  if (!sopt_args_ok(args)) return -2;
-  return fedavg_dispatch<false, false, ServerOptArgs<FedAvgArgs>, false, false, true>(args, n_ctas, stream);
-}
-
-extern "C" int b200_fedavg_allreduce_dp_sopt(const ServerOptArgs<FedAvgDPArgs>* args, int n_ctas, cudaStream_t stream) {
-  if (!sopt_args_ok(args) || !dp_args_ok(args)) return -2;
-  return fedavg_dispatch<true, false, ServerOptArgs<FedAvgDPArgs>, false, false, true>(args, n_ctas, stream);
-}
-
-extern "C" int b200_fedavg_allreduce_scaffold_sopt(const ServerOptArgs<FedAvgScaffoldArgs>* args, int n_ctas,
-                                                   cudaStream_t stream) {
-  if (!sopt_args_ok(args) || !scaffold_args_ok(args)) return -2;
-  return fedavg_dispatch<false, true, ServerOptArgs<FedAvgScaffoldArgs>, false, false, true>(args, n_ctas, stream);
-}
-
-extern "C" int b200_fedavg_allreduce_robust_sopt(const ServerOptArgs<FedAvgRobustArgs>* args, int n_ctas,
-                                                 cudaStream_t stream) {
-  if (!sopt_args_ok(args) || !robust_args_ok(args)) return -2;
-  return fedavg_dispatch<false, false, ServerOptArgs<FedAvgRobustArgs>, true, false, true>(args, n_ctas, stream);
-}
-
-extern "C" int b200_fedavg_allreduce_krum_sopt(const ServerOptArgs<FedAvgKrumArgs>* args, int n_ctas,
-                                               cudaStream_t stream) {
-  if (!sopt_args_ok(args) || !krum_args_ok(args)) return -2;
-  if (n_ctas > B200_KRUM_MAX_CTAS) n_ctas = B200_KRUM_MAX_CTAS;
-  return fedavg_dispatch<false, false, ServerOptArgs<FedAvgKrumArgs>, true, true, true>(args, n_ctas, stream);
-}
-
-// a sum of sparse lists needs the peer loads (the switch adds dense vectors), the delta, whole granules per tile and
-// aligned list offsets; fp8's block scales have no meaning on a list
-template <bool SOPT, class Args>
-static int topk_dispatch(const Args* args, int n_ctas, cudaStream_t stream) {
+template <class Args>
+int b200_fedavg_round(const Args* args, int n_ctas, cudaStream_t stream) {
   using namespace b200;
-  if (args->use_nvls || !args->delta || args->tile_flags != nullptr || args->world > B200_MAX_RANKS ||
-      args->n % FLAG_GRANULE != 0 || args->tile_elems <= 0 || args->tile_elems % FLAG_GRANULE != 0 ||
-      args->rowptr_off % 4 != 0 || args->off_off % 2 != 0 || args->val_off % 4 != 0 ||
-      (args->wire_kind != 0 && args->wire_kind != 1))
-    return -2;
+  constexpr Agg K = RoundOf<Args>::kind;
+  if (args->world > B200_MAX_RANKS || args->n % 8 != 0 || args->tile_elems % 8 != 0) return -2;
+  if (args->tile_flags != nullptr && args->tile_elems % FLAG_GRANULE != 0) return -2;
+  // block-scaled fp8 wire: 32-element blocks must not straddle tiles, and the switch cannot rescale
+  if (args->wire_kind == 2 && (args->tile_elems % 32 != 0 || args->use_nvls)) return -2;
+  if constexpr (RoundOf<Args>::sopt) {
+    if (!sopt_args_ok(args)) return -2;
+  }
+  if constexpr (K == Agg::dp) {
+    if (!dp_args_ok(args)) return -2;
+  } else if constexpr (K == Agg::scaffold) {
+    if (!scaffold_args_ok(args)) return -2;
+  } else if constexpr (K == Agg::robust) {
+    if (!robust_args_ok(args)) return -2;
+  } else if constexpr (K == Agg::krum) {
+    if (!krum_args_ok(args)) return -2;
+    if (n_ctas > B200_KRUM_MAX_CTAS) n_ctas = B200_KRUM_MAX_CTAS;
+  } else if constexpr (K == Agg::topk) {
+    if (!topk_args_ok(args)) return -2;
+  }
   if (n_ctas < 1) n_ctas = 1;
-  if (args->wire_kind == 1) return launch_fedavg<1, false, false, Args, false, false, SOPT, true>(args, n_ctas, stream);
-  return launch_fedavg<0, false, false, Args, false, false, SOPT, true>(args, n_ctas, stream);
+  if constexpr (K != Agg::topk) {   // top-k rounds carry fp32 or bf16 values only
+    if (args->wire_kind == 2) return launch_round_kernel<2>(args, n_ctas, stream);
+  }
+  if (args->wire_kind == 1) return launch_round_kernel<1>(args, n_ctas, stream);
+  return launch_round_kernel<0>(args, n_ctas, stream);
 }
 
-extern "C" int b200_fedavg_allreduce_topk(const FedAvgTopkArgs* args, int n_ctas, cudaStream_t stream) {
-  return topk_dispatch<false>(args, n_ctas, stream);
-}
-
-extern "C" int b200_fedavg_allreduce_topk_sopt(const ServerOptArgs<FedAvgTopkArgs>* args, int n_ctas, cudaStream_t stream) {
-  if (!sopt_args_ok(args)) return -2;
-  return topk_dispatch<true>(args, n_ctas, stream);
-}
+template int b200_fedavg_round(const FedAvgArgs*, int, cudaStream_t);
+template int b200_fedavg_round(const FedAvgDPArgs*, int, cudaStream_t);
+template int b200_fedavg_round(const FedAvgScaffoldArgs*, int, cudaStream_t);
+template int b200_fedavg_round(const FedAvgRobustArgs*, int, cudaStream_t);
+template int b200_fedavg_round(const FedAvgKrumArgs*, int, cudaStream_t);
+template int b200_fedavg_round(const FedAvgTopkArgs*, int, cudaStream_t);
+template int b200_fedavg_round(const ServerOptArgs<FedAvgArgs>*, int, cudaStream_t);
+template int b200_fedavg_round(const ServerOptArgs<FedAvgDPArgs>*, int, cudaStream_t);
+template int b200_fedavg_round(const ServerOptArgs<FedAvgScaffoldArgs>*, int, cudaStream_t);
+template int b200_fedavg_round(const ServerOptArgs<FedAvgRobustArgs>*, int, cudaStream_t);
+template int b200_fedavg_round(const ServerOptArgs<FedAvgKrumArgs>*, int, cudaStream_t);
+template int b200_fedavg_round(const ServerOptArgs<FedAvgTopkArgs>*, int, cudaStream_t);
 
 extern "C" int b200_pack_client(void* seg, float* theta, const float* global_w, void* w_bf16, float* mom, long long n_mom,
                                 long long n, int wire_kind, int reset, cudaStream_t stream) {
@@ -1776,31 +1685,6 @@ extern "C" int b200_pack_client(void* seg, float* theta, const float* global_w, 
     pack_client_kernel<1><<<static_cast<unsigned>(g), 256, 0, stream>>>(s, theta, global_w, wb, mom, n_mom, n, reset);
   else
     pack_client_kernel<0><<<static_cast<unsigned>(g), 256, 0, stream>>>(s, theta, global_w, wb, mom, n_mom, n, reset);
-  return static_cast<int>(cudaGetLastError());
-}
-
-extern "C" int b200_fedavg_allreduce(const FedAvgArgs* args, int n_ctas, cudaStream_t stream) {
-  return fedavg_dispatch<false, false>(args, n_ctas, stream);
-}
-
-extern "C" int b200_fedavg_allreduce_dp(const FedAvgDPArgs* args, int n_ctas, cudaStream_t stream) {
-  if (!dp_args_ok(args)) return -2;
-  return fedavg_dispatch<true, false>(args, n_ctas, stream);
-}
-
-extern "C" int b200_fedavg_allreduce_scaffold(const FedAvgScaffoldArgs* args, int n_ctas, cudaStream_t stream) {
-  if (!scaffold_args_ok(args)) return -2;
-  return fedavg_dispatch<false, true>(args, n_ctas, stream);
-}
-
-extern "C" int b200_flag_barrier(unsigned long long* const* pads, int rank, int world, uint32_t alive_mask,
-                                 uint32_t epoch, int slot, cudaStream_t stream) {
-  using namespace b200;
-  if (world > B200_MAX_RANKS) return -2;
-  FedAvgArgs a = {};
-  for (int k = 0; k < world; ++k) a.pads[k] = pads[k];
-  a.rank = rank; a.world = world; a.alive_mask = alive_mask; a.epoch = epoch;
-  flag_barrier_kernel<<<1, 32, 0, stream>>>(a, slot);
   return static_cast<int>(cudaGetLastError());
 }
 

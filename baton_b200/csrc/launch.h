@@ -164,18 +164,18 @@ struct FedAvgArgs {
   int* status;                      // device int: set non-zero on barrier timeout
   unsigned long long* phase_ns;     // optional [16]: %globaltimer at the phase boundaries (first / last CTA), or nullptr
 };
-// DP-FedAvg round (fedavg_allreduce_kernel<WIRE, true>): clipped weights w_k = n_k s_k / N and Gaussian noise on the
-// reduced sum.  A separate type derived from FedAvgArgs, so the plain kernels and flag_barrier_kernel keep their
-// parameter layout.
+// Every other kind of round has its own args struct derived from FedAvgArgs (FedAvgArgs itself: the plain weighted mean).
+// The struct is the kernel's parameter layout and selects the kernel: see b200_fedavg_round below.
+// DP-FedAvg round (delta mode, peer loads): clipped weights w_k = n_k s_k / N and Gaussian noise on the reduced sum.
 struct FedAvgDPArgs : FedAvgArgs {
   const float* clip_page[B200_MAX_RANKS];   // peer-mapped: clip_page[k][0] = s_k of rank k for this round
   float noise_std;                  // sigma * C (noise on the sum; the kernel divides by N with the weights)
   unsigned long long seed;          // Philox key
   uint32_t round;                   // Philox counter word 2: the collective's round index
 };
-// SCAFFOLD round (fedavg_allreduce_scaffold_kernel<WIRE>): the plain round over segment 0 plus, between the same two
-// barriers, a second segment of n_c elements at byte offset seg1_off of every wire half: each participant (n_k != 0)
-// packs cast(dc), the tile owner reduces with weight inv_clients = 1 / N, and every live rank applies c += result.
+// SCAFFOLD round (delta mode, peer loads): the plain round over segment 0 plus, between the same two barriers, a second
+// segment of n_c elements at byte offset seg1_off of every wire half: each participant (n_k != 0) packs cast(dc), the
+// tile owner reduces with weight inv_clients = 1 / N, and every live rank applies c += result.
 struct FedAvgScaffoldArgs : FedAvgArgs {
   const float* dc;                  // local: this rank's summed control-variate updates [n_c]
   float* c;                         // local: the server control variate [n_c]
@@ -183,7 +183,7 @@ struct FedAvgScaffoldArgs : FedAvgArgs {
   long long seg1_off;               // byte offset of segment 1 inside each wire half (multiple of 16)
   float inv_clients;                // 1 / N, N = the client population
 };
-// Robust round (fedavg_allreduce_robust_kernel<WIRE>): coordinate-wise median or trimmed mean over the participating
+// Robust round (delta mode, peer loads, no arrival flags): coordinate-wise median or trimmed mean over the participating
 // CLIENTS instead of the weighted mean.  Each wire half holds up to S client segments of seg_stride bytes
 // ([seg 0 | pad | seg 1 | ...], seg 0 at the half's start = the plain layout); rank k publishes its segment count m_k in
 // its page seg_page[k][0] (written by the kernel from my_segs), P = sum of m_k over the live ranks <= 32.  The owner of a
@@ -197,8 +197,8 @@ struct FedAvgRobustArgs : FedAvgArgs {
   int kind;                         // 0: median, 1: trimmed mean
   uint8_t trim_b[B200_MAX_ROBUST_CLIENTS + 1];   // trimmed mean: b = floor(beta * P) for P = 0 .. 32 (host-computed)
 };
-// Multi-Krum round (fedavg_allreduce_krum_kernel<WIRE>): the robust round's segments and apply, with a selection of
-// whole clients in phase 1.  Every CTA adds the pair sums (x_i - x_j)^2 of its tiles into work[cta][pair]; the last CTA
+// Multi-Krum round (as the robust round: delta mode, peer loads, no arrival flags): the robust round's segments and
+// apply, with a selection of whole clients in phase 1.  Every CTA adds the pair sums (x_i - x_j)^2 of its tiles into work[cta][pair]; the last CTA
 // of the rank (counter sync[0], zeroed by the launcher) adds them in CTA order into this rank's page dist_page[rank]
 // and raises sync[1]; after a per-CTA barrier at epoch + 2 every CTA adds the live ranks' pages in rank order, scores
 // every client by the krum_k[P] smallest distances (fp64, ascending), keeps the krum_m[P] lowest (score, position)
@@ -216,7 +216,7 @@ struct FedAvgKrumArgs : FedAvgRobustArgs {
   uint8_t krum_k[B200_MAX_ROBUST_CLIENTS + 1];   // neighbours per score for P = 0 .. 32 (host-computed)
   uint8_t krum_m[B200_MAX_ROBUST_CLIENTS + 1];   // clients kept for P = 0 .. 32
 };
-// Server-optimizer round (the *_sopt kernels, any of the kinds above): the apply phase runs FedAvgM / FedAdagrad /
+// Server-optimizer round (ServerOptArgs<the round's struct>, any kind): the apply phase runs FedAvgM / FedAdagrad /
 // FedYogi / FedAdam (parallel/server_opt.py) on the parameter elements [0, n_param) instead of global += d, with
 // d = decode(wire) * apply_scale:  m = c0*m + d, x += c4*m (kind 0, avgm), or m = c0*m + c1*d, v by kind (1 adagrad:
 // v + d*d, 2 yogi: v - c3*(d*d)*sign(v - d*d), 3 adam: c2*v + c3*(d*d)), x += c4*m / (sqrt(v) + c5); every operation
@@ -231,22 +231,17 @@ struct ServerOptArgs : Base {
   int kind;                         // 0 avgm, 1 adagrad, 2 yogi, 3 adam
   float coef[6];                    // b1, 1 - b1, b2, 1 - b2, lr, tau
 };
+// One FedAvg round of the kind Args names: FedAvgArgs, FedAvgDPArgs, FedAvgScaffoldArgs, FedAvgRobustArgs,
+// FedAvgKrumArgs, FedAvgTopkArgs, or ServerOptArgs<one of them>.  Runs fedavg_round_kernel<WIRE, Args> (csrc/fedavg.cu)
+// cooperatively on at most n_ctas CTAs; -2 when the arguments do not fit the kind.
+template <class Args>
+int b200_fedavg_round(const Args* args, int n_ctas, cudaStream_t stream);
 }
-int b200_fedavg_allreduce_sopt(const ServerOptArgs<FedAvgArgs>* args, int n_ctas, cudaStream_t stream);
-int b200_fedavg_allreduce_dp_sopt(const ServerOptArgs<FedAvgDPArgs>* args, int n_ctas, cudaStream_t stream);
-int b200_fedavg_allreduce_scaffold_sopt(const ServerOptArgs<FedAvgScaffoldArgs>* args, int n_ctas, cudaStream_t stream);
-int b200_fedavg_allreduce_robust_sopt(const ServerOptArgs<FedAvgRobustArgs>* args, int n_ctas, cudaStream_t stream);
-int b200_fedavg_allreduce_krum_sopt(const ServerOptArgs<FedAvgKrumArgs>* args, int n_ctas, cudaStream_t stream);
-int b200_fedavg_allreduce(const FedAvgArgs* args, int n_ctas, cudaStream_t stream);
-int b200_fedavg_allreduce_robust(const FedAvgRobustArgs* args, int n_ctas, cudaStream_t stream);   // delta, peer loads
-int b200_fedavg_allreduce_krum(const FedAvgKrumArgs* args, int n_ctas, cudaStream_t stream);       // delta, peer loads
 // one logical client's upload: seg = cast(theta - global_w) in wire format wire_kind (fp8: scales behind the n payload
 // bytes), exactly the collective's own pack; reset != 0 also returns the replica to the global model (theta, bf16
 // shadow, momentum [0, n_mom)) as b200_fold_client does.  n % 8 == 0, 16-byte aligned fp32 arrays.
 int b200_pack_client(void* seg, float* theta, const float* global_w, void* w_bf16, float* mom, long long n_mom,
                      long long n, int wire_kind, int reset, cudaStream_t stream);
-int b200_fedavg_allreduce_dp(const FedAvgDPArgs* args, int n_ctas, cudaStream_t stream);   // delta mode, peer loads only
-int b200_fedavg_allreduce_scaffold(const FedAvgScaffoldArgs* args, int n_ctas, cudaStream_t stream);   // delta, peer loads
 // DP clip factor: s = min(1, clip / ||theta - global_w||_2) over [0, n), norm in fp64 (s = 0 when it is not finite), written to
 // s_out[0] (and s_copy[0] when given), the norm to norm_out[0]; a non-finite norm adds 1 to *nonfinite (optional).
 // Deterministic: fixed grid, per-block partials in work (int64 [B200_DP_WORK_WORDS], zero on first use), last-block finish.
@@ -257,11 +252,8 @@ int b200_dp_clip_factor(const float* theta, const float* global_w, long long n, 
 // clipped logical-client fold: acc (+)= s[0] * (theta - global) with s read from device memory, reset as b200_fold_client
 int b200_fold_client_scaled(float* acc, float* theta, const float* global_w, void* w_bf16, float* mom, long long n_mom,
                             long long n, const float* s, int first, int reset, cudaStream_t stream);
-int b200_flag_barrier(unsigned long long* const* pads, int rank, int world, uint32_t alive_mask, uint32_t epoch,
-                      int slot, cudaStream_t stream);
-// Top-k round (fedavg_allreduce_topk_kernel<WIRE>, fp32 / bf16 wire, delta mode, peer loads, no arrival flags): every
-// participant's upload is a sparse list in its wire half, written before the launch by b200_topk_pack /
-// b200_nonzero_pack (compress.cu): uint32 rowptr[n / 1024 + 1] at rowptr_off, uint16 off[cap] at off_off (the offset of
+// Top-k round (fp32 / bf16 wire, delta mode, peer loads, no arrival flags, prepacked): every participant's upload is a
+// sparse list in its wire half, written before the launch by b200_topk_pack / b200_nonzero_pack (compress.cu): uint32 rowptr[n / 1024 + 1] at rowptr_off, uint16 off[cap] at off_off (the offset of
 // an entry inside its 1024-element granule), values[cap] in the wire dtype at val_off, entries in index order.  The
 // owner of a tile adds w_k * value into an fp32 shared-memory tile, live ranks in order (fmaf from 0, skipping w_k == 0,
 // as the dense reduce), and stores the cast dense result into seg 0 of every live replica; pack phase: none; barriers,
@@ -271,8 +263,6 @@ struct FedAvgTopkArgs : FedAvgArgs {
   long long off_off;
   long long val_off;
 };
-int b200_fedavg_allreduce_topk(const FedAvgTopkArgs* args, int n_ctas, cudaStream_t stream);
-int b200_fedavg_allreduce_topk_sopt(const ServerOptArgs<FedAvgTopkArgs>* args, int n_ctas, cudaStream_t stream);
 
 // ---- compress.cu: top-k selection with error feedback (parallel/compress.py)
 // work: int32 [B200_TOPK_WORK_WORDS(n)] scratch; n % 1024 == 0, 1 <= k <= n, 16-byte aligned fp32 arrays.

@@ -16,7 +16,7 @@ sample-weighted mean of the clients' ``topk(u)``, cast through the session's wir
 
 This module holds the configuration, the per-client residuals and the host implementation of the rule:
 :func:`topk_select` / :func:`topk_ef_` (the oracle of the tests and the selection of :class:`NcclSession`) and
-:func:`topk_combine`, which reproduces the fused collective's reduce (``fedavg_allreduce_topk_kernel``).
+:func:`topk_combine`, which reproduces the fused collective's reduce (``fedavg_round_kernel<WIRE, FedAvgTopkArgs>``).
 """
 from __future__ import annotations
 

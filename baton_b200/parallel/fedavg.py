@@ -47,7 +47,7 @@ clients.  The optimizer-emitted upload is off: the selection needs all of ``u``.
 Both take ``server_opt=ServerOptConfig(...)`` (``parallel/server_opt.py``): FedAvgM, FedAdagrad, FedYogi or FedAdam
 applied to the round's aggregate, whatever computed it (mean, DP, SCAFFOLD, median, trimmed mean, Krum).  The session
 allocates the state ``arena.server_m`` / ``arena.server_v`` over the parameters, replicated on every rank; the fused
-session runs the ``*_sopt`` instantiation of the round's kernel, whose apply phase takes the step, and
+session runs the round's kernel on ``ServerOptArgs<...>`` of the round's arguments, whose apply phase takes the step, and
 :class:`NcclSession` calls :func:`server_step_` where it would add the aggregate.  :meth:`server_state` reads the state.
 """
 from __future__ import annotations
@@ -133,6 +133,19 @@ def _init_server_opt(arena: ParamArena, server_opt: Optional[ServerOptConfig], d
     return server_opt
 
 
+def _check_session(arena: ParamArena, wire_dtype: str, mode: str, dp: Optional[DPConfig], scaffold: bool,
+                   robust: Optional[RobustConfig], max_clients: int, tile_flags: bool,
+                   server_opt: Optional[ServerOptConfig], topk: Optional[TopKConfig]):
+    """Validate a session's combination of features (either kind of session: the same checks in the same order) and
+    allocate the server optimizer's state: ``(topk, server_opt, max_clients)``."""
+    delta = mode == "delta"
+    topk = _check_topk(topk, wire_dtype, dp, robust, scaffold, delta, tile_flags)
+    server_opt = _init_server_opt(arena, server_opt, delta)
+    _check_dp_mode(dp, delta)
+    _check_scaffold(scaffold, dp, delta)
+    return topk, server_opt, _check_robust(robust, dp, scaffold, delta, tile_flags, max_clients, topk)
+
+
 def _check_control(scaffold: bool, control) -> None:
     if scaffold and control is None:
         raise ValueError("a SCAFFOLD session needs control=(c, dc, n_clients) every round")
@@ -161,12 +174,9 @@ class FedAvgSession:
         from ..ops._ext import load
         self._C = load()
         assert wire_dtype in ("bf16", "fp32", "fp8") and mode in ("delta", "weights")
-        self.topk = _check_topk(topk, wire_dtype, dp, robust, scaffold, mode == "delta", tile_flags)
-        self.server_opt = _init_server_opt(arena, server_opt, mode == "delta")
+        self.topk, self.server_opt, self.max_clients = _check_session(arena, wire_dtype, mode, dp, scaffold, robust,
+                                                                      max_clients, tile_flags, server_opt, topk)
         self._sopt_coef = list(server_opt.coefficients()) if server_opt is not None else []
-        _check_dp_mode(dp, mode == "delta")
-        _check_scaffold(scaffold, dp, mode == "delta")
-        self.max_clients = _check_robust(robust, dp, scaffold, mode == "delta", tile_flags, max_clients, self.topk)
         self.robust = robust
         self.krum = robust is not None and robust.kind == "krum"
         self.scaffold = bool(scaffold)
@@ -561,81 +571,49 @@ class FedAvgSession:
                                    "before aggregate, with the same round index)")
             self._topk_sent = self._topk_end[1] if counts[self.rank] != 0.0 else None
             self._packed_epoch = None
-            with torch.cuda.stream(stream):
-                self._C.fedavg_allreduce_topk(
-                    self.symm.peer_ptrs(o_wire), self.symm.peer_ptrs(self.off_pads),
-                    a.theta, a.global_w, a.theta_bf16, a.momentum if self.reset_momentum else None,
-                    a.int_arena if a.n_int > 0 else None, self.symm.peer_ptrs(o_int) if a.n_int > 0 else [],
-                    self.loss_local, self.symm.peer_ptrs(o_loss), self.loss_out,
-                    counts, from_flags, mask, self.rank, world, self.wire_kind, self.epoch, tile, self.n_ctas,
-                    self.timeout_log2, self.status, self.phase_ns, self.topk_rowptr_off, self.topk_off_off,
-                    self.topk_val_off, *self._sopt_args())
-            self.epoch = (self.epoch + 3) & 0xFFFFFFFF
-            self.rounds += 1
-            self._side_pending = on_side_stream
-            return
-        if robust is not None and robust.kind == "krum":
-            o_dist = self.off_dist + par * self.half_dist
-            k_tab, m_tab = robust.krum_tables()
-            with torch.cuda.stream(stream):
-                self._C.fedavg_allreduce_krum(
-                    self.symm.peer_ptrs(o_wire), self.symm.peer_ptrs(self.off_pads),
-                    a.theta, a.global_w, a.theta_bf16, a.momentum if self.reset_momentum else None,
-                    a.int_arena if a.n_int > 0 else None, self.symm.peer_ptrs(o_int) if a.n_int > 0 else [],
-                    self.loss_local, self.symm.peer_ptrs(o_loss), self.loss_out,
-                    counts, from_flags, mask, self.rank, world, self.wire_kind, self.epoch, tile, self.n_ctas,
-                    self.timeout_log2, self.status, self.phase_ns, prepacked,
-                    self.symm.peer_ptrs(o_clip), m, self.seg_stride, self.symm.peer_ptrs(o_dist),
-                    self.krum_work, self.krum_sync, self.krum_report, k_tab, m_tab, *self._sopt_args())
-            self.epoch = (self.epoch + 3) & 0xFFFFFFFF
-            self.rounds += 1
-            self._side_pending = on_side_stream
-            return
-        if robust is not None:
-            with torch.cuda.stream(stream):
-                self._C.fedavg_allreduce_robust(
-                    self.symm.peer_ptrs(o_wire), self.symm.peer_ptrs(self.off_pads),
-                    a.theta, a.global_w, a.theta_bf16, a.momentum if self.reset_momentum else None,
-                    a.int_arena if a.n_int > 0 else None, self.symm.peer_ptrs(o_int) if a.n_int > 0 else [],
-                    self.loss_local, self.symm.peer_ptrs(o_loss), self.loss_out,
-                    counts, from_flags, mask, self.rank, world, self.wire_kind, self.epoch, tile, self.n_ctas,
-                    self.timeout_log2, self.status, self.phase_ns, prepacked,
-                    self.symm.peer_ptrs(o_clip), m, self.seg_stride, robust.kind_id, robust.trim_table(),
-                    *self._sopt_args())
-            self.epoch = (self.epoch + 3) & 0xFFFFFFFF
-            self.rounds += 1
-            self._side_pending = on_side_stream
-            return
+            prepacked = True        # the sparse lists are written before the launch: a top-k round has no pack phase
+        # the arguments every kind of round takes (csrc/bindings.cpp), then the kind's own
+        common = (self.symm.peer_ptrs(o_wire), self.symm.peer_ptrs(self.off_pads),
+                  self.symm.mc(o_wire) if nvls_now else 0,
+                  a.theta, a.global_w, a.theta_bf16, a.momentum if self.reset_momentum else None,
+                  a.int_arena if a.n_int > 0 else None, self.symm.peer_ptrs(o_int) if a.n_int > 0 else [],
+                  self.loss_local, self.symm.peer_ptrs(o_loss), self.loss_out,
+                  counts, from_flags, mask, self.rank, world, self.wire_kind, self.delta, nvls_now, self.epoch,
+                  self.tile_flags, flag_value, tile, self.n_ctas, self.timeout_log2, self.status, self.phase_ns,
+                  prepacked)
         with torch.cuda.stream(stream):
-            dp_args = ([], 0.0, 0, 0)
-            if dp is not None:
-                from ..ops import functional as F
-                page = self.symm.view(o_clip, 1, torch.float32)
-                if clipped:
-                    page.fill_(1.0)
-                    self.dp_s.fill_(1.0)
-                else:     # theta is final here: the norm pass runs right before the collective, on its stream
-                    F.dp_clip_factor(a.theta, a.global_w, dp.clip, self.dp_work, self.dp_s, self.dp_norm,
-                                     s_copy_ptr=page.data_ptr(), nonfinite=self.dp_nonfinite)
-                seed = dp.seed - (1 << 64) if dp.seed >= (1 << 63) else dp.seed      # int64 bit pattern of the key
-                dp_args = (self.symm.peer_ptrs(o_clip), dp.noise_std, seed, self.dp_round())
-            scaf_args = (None, None, 0, 0.0)
-            if control is not None:
-                c, dc, n_clients = control
-                n_p = self.arena.n_param
-                scaf_args = (dc[:n_p], c[:n_p], self.seg1_off, 1.0 / float(n_clients))
-            self._C.fedavg_allreduce(
-                self.symm.peer_ptrs(o_wire), self.symm.peer_ptrs(self.off_pads),
-                self.symm.mc(o_wire) if nvls_now else 0,
-                a.theta, a.global_w, a.theta_bf16,
-                a.momentum if self.reset_momentum else None,
-                a.int_arena if a.n_int > 0 else None,
-                self.symm.peer_ptrs(o_int) if a.n_int > 0 else [],
-                self.loss_local, self.symm.peer_ptrs(o_loss), self.loss_out,
-                counts, from_flags, mask, self.rank, world, self.wire_kind, self.delta,
-                nvls_now, self.epoch,
-                self.tile_flags, flag_value, tile, self.n_ctas, self.timeout_log2, self.status, self.phase_ns,
-                prepacked, *dp_args, *scaf_args, *self._sopt_args())
+            if self.topk is not None:
+                launch = self._C.fedavg_allreduce_topk
+                own = (self.topk_rowptr_off, self.topk_off_off, self.topk_val_off)
+            elif robust is not None and robust.kind == "krum":
+                launch = self._C.fedavg_allreduce_krum
+                own = (self.symm.peer_ptrs(o_clip), m, self.seg_stride,
+                       self.symm.peer_ptrs(self.off_dist + par * self.half_dist), self.krum_work, self.krum_sync,
+                       self.krum_report, *robust.krum_tables())
+            elif robust is not None:
+                launch = self._C.fedavg_allreduce_robust
+                own = (self.symm.peer_ptrs(o_clip), m, self.seg_stride, robust.kind_id, robust.trim_table())
+            else:
+                launch = self._C.fedavg_allreduce
+                dp_args = ([], 0.0, 0, 0)
+                if dp is not None:
+                    from ..ops import functional as F
+                    page = self.symm.view(o_clip, 1, torch.float32)
+                    if clipped:
+                        page.fill_(1.0)
+                        self.dp_s.fill_(1.0)
+                    else:     # theta is final here: the norm pass runs right before the collective, on its stream
+                        F.dp_clip_factor(a.theta, a.global_w, dp.clip, self.dp_work, self.dp_s, self.dp_norm,
+                                         s_copy_ptr=page.data_ptr(), nonfinite=self.dp_nonfinite)
+                    seed = dp.seed - (1 << 64) if dp.seed >= (1 << 63) else dp.seed      # int64 bit pattern of the key
+                    dp_args = (self.symm.peer_ptrs(o_clip), dp.noise_std, seed, self.dp_round())
+                scaf_args = (None, None, 0, 0.0)
+                if control is not None:
+                    c, dc, n_clients = control
+                    n_p = self.arena.n_param
+                    scaf_args = (dc[:n_p], c[:n_p], self.seg1_off, 1.0 / float(n_clients))
+                own = (*dp_args, *scaf_args)
+            launch(*common, *own, *self._sopt_args())
         self.epoch = (self.epoch + 3) & 0xFFFFFFFF     # uint32 wrap: the kernel compares signed differences
         self.rounds += 1
         self._side_pending = on_side_stream
@@ -760,11 +738,8 @@ class NcclSession:
                  robust: Optional[RobustConfig] = None, max_clients: int = 1, tile_flags: bool = False,
                  server_opt: Optional[ServerOptConfig] = None, topk: Optional[TopKConfig] = None, **_unused):
         import torch.distributed as dist
-        self.topk = _check_topk(topk, wire_dtype, dp, robust, scaffold, mode == "delta", tile_flags)
-        self.server_opt = _init_server_opt(arena, server_opt, mode == "delta")
-        _check_dp_mode(dp, mode == "delta")
-        _check_scaffold(scaffold, dp, mode == "delta")
-        self.max_clients = _check_robust(robust, dp, scaffold, mode == "delta", tile_flags, max_clients, self.topk)
+        self.topk, self.server_opt, self.max_clients = _check_session(arena, wire_dtype, mode, dp, scaffold, robust,
+                                                                      max_clients, tile_flags, server_opt, topk)
         # top-k: k, this rank's upload of the round as a dense fp32 vector (zeros off its support) and its entry count
         self.topk_k = self.topk.k(n_float(arena)) if self.topk is not None else 0
         self._topk_up = None

@@ -15,7 +15,7 @@ keep the max-over-participants policy, and the reported loss stays the sample-we
 
 At most ``MAX_ROBUST_CLIENTS`` = 32 participants per round: the fused collective's tile owner sorts every element's
 values in registers.  :func:`robust_combine` is the host implementation (the oracle of the tests and the CPU / gloo
-path); ``csrc/fedavg.cu`` (``fedavg_allreduce_robust_kernel``) computes the same bits on an fp32 wire.
+path); ``csrc/fedavg.cu`` (``fedavg_round_kernel<WIRE, FedAvgRobustArgs>``) computes the same bits on an fp32 wire.
 
 Multi-Krum (``kind="krum"``, ``krum_f`` = f Byzantine clients assumed, ``krum_m`` = m clients kept) works on whole
 updates instead of coordinates.  With ``D[i][j] = sum_e (d_i[e] - d_j[e])^2`` over the float arena (a non-finite
@@ -26,7 +26,7 @@ segment position)`` and the first ``m = clamp(krum_m or P - f, 1, P)`` are kept.
 ``krum_m = 1`` is classic Krum.  Blanchard's guarantee needs ``P > 2f + 2``: the engine and the configuration reject a
 planned participant count below ``2f + 3``, but a round that arrives with fewer participants still runs with the
 clamped ``k`` and ``m`` above.  :func:`krum_select` is the host selection; the fused collective
-(``fedavg_allreduce_krum_kernel``) computes ``D`` from fp32 partial sums per chunk, fp64 across chunks, so its scores
+(``fedavg_round_kernel<WIRE, FedAvgKrumArgs>``) computes ``D`` from fp32 partial sums per chunk, fp64 across chunks, so its scores
 agree with the host's to rounding and its kept mean is bitwise the host's for the same kept set.
 """
 from __future__ import annotations
