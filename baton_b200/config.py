@@ -57,10 +57,8 @@ class FederationConfig:
     seed: int = 0
 
     def __post_init__(self):
-        if not (0.0 <= float(self.prox_mu) < float("inf")):
-            raise ValueError("prox_mu must be a finite number >= 0, got {!r}".format(self.prox_mu))
-        from .train import check_adamw, check_optimizer
-        check_optimizer(self.optimizer, self.momentum, prox_mu=float(self.prox_mu))
+        from .train import check_adamw, check_prox_mu
+        check_prox_mu(self.prox_mu)
         check_adamw((self.adam_beta1, self.adam_beta2), self.adam_eps)
         from .parallel.dp import check_dp
         check_dp(self.dp_clip, self.dp_noise_multiplier)
@@ -68,19 +66,17 @@ class FederationConfig:
             raise ValueError("dp_delta must lie in (0, 1), got {!r}".format(self.dp_delta))
         from .parallel.robust import check_aggregator
         self.trim_ratio = check_aggregator(self.aggregator, self.trim_ratio)
-        if self.aggregator != "mean" and float(self.dp_clip) > 0.0:
-            raise ValueError("a robust aggregator with DP-FedAvg is not supported")
         if self.aggregator == "krum":
+            from .parallel.features import round_plan
             from .parallel.robust import check_krum, check_krum_participants
             check_krum(self.krum_f, self.krum_m)
-            population = self.logical_clients if self.logical_clients > self.clients else self.clients
-            check_krum_participants(min(self.sample_k, population) if self.sample_k else population, self.krum_f)
-
-        if self.server_opt != "none":
-            self.server_opt_config()          # validates kind, lr, betas and tau
-            if self.backend in ("fused", "nccl"):
-                from .parallel.dataplane import SEATED_SERVER_OPT
-                raise ValueError(SEATED_SERVER_OPT)
+            check_krum_participants(round_plan(self.clients, self.logical_clients, self.sample_k)[0], self.krum_f)
+        self.server_opt_config()          # validates kind, lr, betas and tau
+        from .parallel.features import check_features
+        check_features(dp=float(self.dp_clip) > 0.0, robust=self.aggregator != "mean",
+                       server_opt=self.server_opt != "none",
+                       plane="seated" if self.backend in ("fused", "nccl") else "http", optimizer=self.optimizer,
+                       momentum=self.momentum, prox_mu=float(self.prox_mu))
 
     def train_kwargs(self) -> dict:
         """Local-training keyword arguments of a worker (``FederatedModule.local_train``)."""

@@ -101,8 +101,6 @@ class Experiment:
         self.clock = clock
         self.client_manager = ClientManager(name, app, client_ttl, clock=clock, seed=seed)
         self.update_manager = UpdateManager(name)
-        if robust is not None and dp is not None:
-            raise ValueError("robust aggregation with DP-FedAvg is not supported")
         self.plane: ManagerPlane = make_manager_plane(dataplane, dp=dp, robust=robust, server_opt=server_opt)
         self.robust = robust
         self.server_opt = server_opt

@@ -128,22 +128,3 @@ def sparse_upload_bytes(n: int, entries: int, wire_dtype: str) -> int:
     """Bytes of one sparse upload: the row pointers, then a 16-bit offset and a value per entry."""
     vb = 4 if wire_dtype == "fp32" else 2
     return 4 * (int(n) // GRANULE + 1) + int(entries) * (2 + vb)
-
-
-def check_topk_exclusions(*, wire_dtype: str, dp, robust, scaffold: bool, delta: bool, tile_flags: bool) -> None:
-    """The combinations a top-k round cannot run: raises ``ValueError`` with the reason."""
-    if wire_dtype == "fp8":
-        raise ValueError("top-k uploads with the fp8 wire are not supported: its block scales have no meaning on a "
-                         "sparse list")
-    if dp is not None:
-        raise ValueError("top-k uploads with DP-FedAvg are not supported: the noise is calibrated to the dense clipped "
-                         "mean")
-    if robust is not None:
-        raise ValueError("top-k uploads with a robust aggregator are not supported: it needs every client's dense "
-                         "update")
-    if scaffold:
-        raise ValueError("top-k uploads with SCAFFOLD are not supported: its control-variate segment is dense")
-    if not delta:
-        raise ValueError("top-k uploads need mode='delta'")
-    if tile_flags:
-        raise ValueError("top-k uploads with tile_flags are not supported")

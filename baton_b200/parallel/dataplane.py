@@ -28,6 +28,7 @@ import torch
 
 from . import wire
 from .aggregate import dp_fedavg_into, fedavg_into, robust_into
+from .features import check_features
 from .server_opt import ServerOptConfig, server_step_
 
 log = logging.getLogger("baton_b200.dataplane")
@@ -70,8 +71,7 @@ class HttpManagerPlane(ManagerPlane):
     carries_tensors = True
 
     def __init__(self, int_policy: str = "max", dp=None, robust=None, server_opt=None):
-        if dp is not None and robust is not None:
-            raise ValueError("robust aggregation with DP-FedAvg is not supported")
+        check_features(dp=dp, robust=robust, server_opt=server_opt, plane="http")
         if server_opt is not None and not isinstance(server_opt, ServerOptConfig):
             raise TypeError("server_opt= takes a ServerOptConfig")
         self.int_policy = int_policy
@@ -181,8 +181,7 @@ class SeatedManagerPlane(ManagerPlane):
 
     def __init__(self, name: str = "fused", world_size: Optional[int] = None, distribute_initial: bool = True,
                  dp=None, robust=None):
-        if dp is not None and robust is not None:
-            raise ValueError("robust aggregation with DP-FedAvg is not supported")
+        check_features(dp=dp, robust=robust, plane="seated")
         # robust (a RobustConfig): the plan carries {"robust": RobustConfig.to_dict()}; every seat uploads one segment
         self.robust = robust
         self.name = name
@@ -346,14 +345,9 @@ class SeatedWorkerPlane(WorkerPlane):
             check()             # a peer that died mid-collective surfaces here as an error, not as a hang
 
 
-SEATED_SERVER_OPT = ("a server optimizer needs the http plane: on the seated planes its state would be replicated on "
-                     "the seats, an evicted seat would return with stale m and v, and the manager holds no copy to "
-                     "resend")
-
-
 def make_manager_plane(spec, dp=None, robust=None, server_opt=None) -> ManagerPlane:
-    if server_opt is not None and not (spec in (None, "http", "http_pickle") or isinstance(spec, HttpManagerPlane)):
-        raise ValueError(SEATED_SERVER_OPT)
+    http = spec in (None, "http", "http_pickle") or isinstance(spec, HttpManagerPlane)
+    check_features(dp=dp, robust=robust, server_opt=server_opt, plane="http" if http else "seated")
     if isinstance(spec, ManagerPlane):
         if server_opt is not None and getattr(spec, "server_opt", None) != server_opt:
             raise ValueError("a server-optimizer experiment needs a data plane built with the same server_opt=")
@@ -362,7 +356,7 @@ def make_manager_plane(spec, dp=None, robust=None, server_opt=None) -> ManagerPl
         if robust is not None and getattr(spec, "robust", None) is None:
             raise ValueError("a robust experiment needs a data plane built with the same robust=")
         return spec
-    if spec in (None, "http", "http_pickle"):
+    if http:
         return HttpManagerPlane(dp=dp, robust=robust, server_opt=server_opt)
     if spec in ("fused", "nccl"):
         return SeatedManagerPlane(spec, dp=dp, robust=robust)

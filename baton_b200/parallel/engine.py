@@ -26,10 +26,11 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from ..metrics import phase
-from ..train import GraphedLocalSGD, PortableLocalSGD, check_adamw, check_optimizer, check_prox_mu
+from ..train import GraphedLocalSGD, PortableLocalSGD, check_adamw, check_prox_mu
 from .arena import ParamArena
-from .compress import TopKConfig, TopKState, check_topk_exclusions
+from .compress import TopKConfig, TopKState
 from .dp import DPConfig, RDPAccountant, check_dp, clip_factor
+from .features import check_features, round_plan
 from .fedavg import FedAvgSession, NcclSession
 from .robust import RobustConfig, check_aggregator, check_krum_participants, check_participants
 from .server_opt import ServerOptConfig
@@ -124,50 +125,21 @@ class FederatedEngine:
         if compress not in (None, "topk"):
             raise ValueError("compress must be None or 'topk', got {!r}".format(compress))
         self.topk = TopKConfig(topk_ratio, error_feedback) if compress == "topk" else None
-        if self.topk is not None:
-            check_topk_exclusions(wire_dtype=wire_dtype, dp=dp_clip if dp_clip else None,
-                                  robust=aggregator if aggregator != "mean" else None, scaffold=scaffold,
-                                  delta=mode == "delta", tile_flags=tile_flags)
         sopt = None
         if server_opt is not None:
-            if mode != "delta":
-                raise ValueError("a server optimizer needs mode='delta': mode='weights' has no pseudo-gradient")
             b1, b2 = server_betas
             sopt = ServerOptConfig(server_opt, server_lr, b1, b2, server_tau)
         prox_mu = check_prox_mu(prox_mu)
-        adam = check_optimizer(optimizer, momentum, prox_mu=prox_mu)
+        adam = optimizer == "adamw"
         if adam:
-            if scaffold:
-                raise ValueError("AdamW with SCAFFOLD is not supported: option II's dc = (x - theta) / (K lr) - c "
-                                 "assumes SGD steps")
             betas, eps = check_adamw(betas, eps)
         dp_clip, dp_noise_multiplier = check_dp(dp_clip, dp_noise_multiplier)
-        if scaffold:
-            if dp_clip > 0.0:
-                raise ValueError("SCAFFOLD with DP-FedAvg is not supported: DP would also have to clip and noise dc")
-            if prox_mu > 0.0:
-                raise ValueError("SCAFFOLD and FedProx (prox_mu > 0) are exclusive")
-            if mode != "delta":
-                raise ValueError("SCAFFOLD needs mode='delta'")
-            if tile_flags:
-                raise ValueError("SCAFFOLD with tile_flags is not supported: the correction c - c_i reads c, which "
-                                 "the previous round's collective writes, so it cannot run ahead of the join")
         trim_ratio = check_aggregator(aggregator, trim_ratio)
         self.robust = RobustConfig(aggregator, trim_ratio, krum_f, krum_m) if aggregator != "mean" else None
-        if self.robust is not None:
-            if dp_clip > 0.0:
-                raise ValueError("a robust aggregator with DP-FedAvg is not supported: DP's noise is calibrated to the "
-                                 "clipped mean")
-            if scaffold:
-                raise ValueError("a robust aggregator with SCAFFOLD is not supported: its control-variate update is a "
-                                 "mean")
-            if mode != "delta":
-                raise ValueError("a robust aggregator needs mode='delta'")
-            if tile_flags:
-                raise ValueError("a robust aggregator with tile_flags is not supported")
         self.dp = DPConfig(dp_clip, dp_noise_multiplier, dp_seed) if dp_clip > 0.0 else None
-        if self.dp is not None and mode != "delta":
-            raise ValueError("DP-FedAvg needs mode='delta'")
+        check_features(wire_dtype=wire_dtype, mode=mode, dp=self.dp, scaffold=scaffold, robust=self.robust,
+                       topk=self.topk, server_opt=sopt, tile_flags=tile_flags, optimizer=optimizer, momentum=momentum,
+                       prox_mu=prox_mu)
         self.device = torch.device(device)
         self.model = model
         self.name = name
@@ -185,23 +157,18 @@ class FederatedEngine:
                                  "gloo on CPU) for CPU runs")
             self.trainer = PortableLocalSGD(model, self.arena, loss=loss)
         Session = {"fused": FedAvgSession, "nccl": NcclSession}[backend]
-        robust_kw = {}
-        if self.topk is not None:     # with logical clients the folded upload is the union of S clients' supports
-            world = self._group_size(group)
-            population = logical_clients if logical_clients and logical_clients > world else world
-            per_rank = -(-population // world) if population > world else 1
-            robust_kw = {"topk": self.topk, "max_clients": min(per_rank, sample_k or population)}
-        if self.robust is not None:
-            world = self._group_size(group)
-            population = logical_clients if logical_clients and logical_clients > world else world
-            planned = min(sample_k, population) if sample_k else population
-            check_participants(planned)
-            if self.robust.kind == "krum":
-                check_krum_participants(planned, self.robust.krum_f)
-            per_rank = -(-population // world) if population > world else 1
-            robust_kw = {"robust": self.robust, "max_clients": min(per_rank, sample_k or population)}
+        # robust: one segment per hosted client; top-k with logical clients: the folded upload is the union of their
+        # supports
+        max_clients = 1
+        if self.robust is not None or self.topk is not None:
+            planned, max_clients = round_plan(self._group_size(group), logical_clients, sample_k)
+            if self.robust is not None:
+                check_participants(planned)
+                if self.robust.kind == "krum":
+                    check_krum_participants(planned, self.robust.krum_f)
         self.session = Session(self.arena, group, wire_dtype=wire_dtype, mode=mode, n_ctas=n_ctas, nvls=nvls,
-                               tile_flags=tile_flags, dp=self.dp, scaffold=scaffold, server_opt=sopt, **robust_kw)
+                               tile_flags=tile_flags, dp=self.dp, scaffold=scaffold, server_opt=sopt,
+                               robust=self.robust, topk=self.topk, max_clients=max_clients)
         self.dp = self.session.dp                  # rank 0's noise key
         self.accountant = RDPAccountant(self.dp.noise_multiplier) if self.dp is not None else None
         self.backend = backend
@@ -310,26 +277,13 @@ class FederatedEngine:
                 total_n = X.shape[0]
                 if self.topk is not None:
                     self.session.pack_topk(self._residual(self.rank))
-        elif self.robust is not None:
-            # robust: every hosted participant uploads its own segment (a median of per-rank sums is not a median of
-            # clients); the next co-resident client starts from the global model
-            self.sync()
-            for j, cid in enumerate(mine):
-                X, y = shards(cid)
-                if not X.is_cuda:
-                    X, y = self.stage(X, y, slot=j)
-                ld = self._train_client(cid, X, y, n_epoch, first=(j == 0))
-                nk = X.shape[0]
-                losses_dev = ld * nk if losses_dev is None else losses_dev + ld * nk
-                total_n += nk
-                self.session.pack_client(j, reset=j + 1 < len(mine))
-            if losses_dev is not None and total_n:
-                losses_dev = losses_dev / total_n
         else:
             # time-sliced logical clients: fold n_k * (theta_k - global) locally, then upload the mean
-            # (DP: s_k * (theta_k - global) for every hosted client, even a single one, and the mean over clients)
+            # (DP: s_k * (theta_k - global) for every hosted client, even a single one, and the mean over clients;
+            # robust: every hosted client uploads its own segment -- a median of per-rank sums is not a median of
+            # clients)
             self.sync()
-            fold = len(mine) > 1 or (self.dp is not None and mine)
+            fold = self.robust is None and (len(mine) > 1 or (self.dp is not None and mine))
             if fold and self._acc is None:
                 self._acc = torch.zeros_like(a.theta)
             if fold and not a.theta.is_cuda:
@@ -344,18 +298,19 @@ class FederatedEngine:
                 nk = X.shape[0]
                 losses_dev = ld * nk if losses_dev is None else losses_dev + ld * nk
                 total_n += nk
-                if self.dp is not None:
-                    self._dp_fold(j, more=j + 1 < len(mine))
+                more = j + 1 < len(mine)               # the next co-resident client starts from the global model
+                if self.robust is not None:
+                    self.session.pack_client(j, reset=more)
+                elif self.dp is not None:
+                    self._dp_fold(j, more=more)
                 elif self.topk is not None:
                     # top-k: one hosted client uploads its own list; several fold n_k * topk(u_k), then upload the
                     # folded mean's non-zero entries
                     if len(mine) == 1:
                         self.session.pack_topk(self._residual(cid))
                     else:
-                        self.session.fold_topk(self._acc, self._residual(cid), nk, first=(j == 0),
-                                               reset=j + 1 < len(mine))
+                        self.session.fold_topk(self._acc, self._residual(cid), nk, first=(j == 0), reset=more)
                 elif len(mine) > 1:
-                    more = j + 1 < len(mine)           # the next co-resident client starts from the global model
                     if a.theta.is_cuda:
                         from ..ops import functional as F     # ONE kernel: fold the delta + reset the replica
                         F.fold_client(self._acc, a.theta, a.global_w, nk, first=(j == 0), reset=more,
@@ -524,48 +479,13 @@ class FederatedEngine:
         return self.accountant.get_privacy_spent(delta)
 
     def _aggregate(self, my_n: float, loss_dev, clipped: bool = False, n_clients: Optional[int] = None) -> None:
+        """The round's one ``aggregate``: the loss, upload and stream arguments every kind of round takes, then the
+        kind's own."""
         s = self.session
-        if self.robust is not None:    # n_clients: segments packed by pack_client (logical clients), else seg 0 as usual
-            kw = self._aggregate_kwargs(s, my_n, loss_dev)
-            if n_clients is not None:
-                kw["n_clients"] = n_clients
-            s.aggregate(my_n=my_n, **kw)
-            return
-        if self.scaf is not None:      # SCAFFOLD: c += (sum of the ranks' dc) / N in the same collective
-            s.aggregate(my_n=my_n, control=(self.scaf.c, self.scaf.up, self.logical_clients or self.world),
-                        **self._aggregate_kwargs(s, my_n, loss_dev))
-            return
-        if self.dp is not None:
-            kw = {"clipped": clipped}
-            if isinstance(s, FedAvgSession):
-                kw["on_side_stream"] = bool(self.overlap_collective)
-                kw["prepacked"] = bool(self.prepack and getattr(self.trainer, "emitted_wire", False) and my_n > 0
-                                       and not getattr(self.trainer, "last_had_tail_step", False))
-            if loss_dev is not None and hasattr(s, "loss_local"):
-                k = min(loss_dev.numel(), s.loss_local.numel())
-                s.loss_local.zero_()
-                s.loss_local[:k].copy_(loss_dev[:k])
-                s.aggregate(my_n=my_n, **kw)
-            else:
-                s.aggregate(my_n=my_n, loss_history=loss_dev.tolist() if loss_dev is not None else None, **kw)
-            return
-        side = bool(self.overlap_collective and isinstance(s, FedAvgSession))
-        if loss_dev is not None and hasattr(s, "loss_local"):
-            k = min(loss_dev.numel(), s.loss_local.numel())
-            s.loss_local.zero_()
-            s.loss_local[:k].copy_(loss_dev[:k])
-            pre = bool(self.prepack and getattr(self.trainer, "emitted_wire", False) and my_n > 0
-                       and not getattr(self.trainer, "last_had_tail_step", False))
-            s.aggregate(my_n=my_n, prepacked=pre, on_side_stream=side) if isinstance(s, FedAvgSession) else s.aggregate(my_n=my_n)
-        elif loss_dev is not None:
-            s.aggregate(my_n=my_n, loss_history=loss_dev.tolist())
-        else:
-            s.aggregate(my_n=my_n)
-
-    def _aggregate_kwargs(self, s, my_n: float, loss_dev) -> dict:
-        """Loss, upload and stream arguments of a round's ``aggregate`` (the plain round's choices)."""
         kw = {}
-        if isinstance(s, FedAvgSession):
+        plain = self.robust is None and self.scaf is None and self.dp is None
+        # a plain round of a rank that hosts no client (no loss) runs on the compute stream, with the kernel's own pack
+        if isinstance(s, FedAvgSession) and not (plain and loss_dev is None):
             kw["on_side_stream"] = bool(self.overlap_collective)
             kw["prepacked"] = bool(self.prepack and getattr(self.trainer, "emitted_wire", False) and my_n > 0
                                    and not getattr(self.trainer, "last_had_tail_step", False))
@@ -575,7 +495,14 @@ class FederatedEngine:
             s.loss_local[:k].copy_(loss_dev[:k])
         elif loss_dev is not None:
             kw["loss_history"] = loss_dev.tolist()
-        return kw
+        if self.robust is not None:    # n_clients: segments packed by pack_client (logical clients), else seg 0 as usual
+            if n_clients is not None:
+                kw["n_clients"] = n_clients
+        elif self.scaf is not None:    # SCAFFOLD: c += (sum of the ranks' dc) / N in the same collective
+            kw["control"] = (self.scaf.c, self.scaf.up, self.logical_clients or self.world)
+        elif self.dp is not None:
+            kw["clipped"] = clipped
+        s.aggregate(my_n=my_n, **kw)
 
     def global_loss(self, n_epoch: int) -> List[float]:
         return self.session.reduced_loss(n_epoch)

@@ -1,0 +1,79 @@
+"""Which federation features combine, in one place.
+
+Every entry point that builds or runs a round passes the features it has to :func:`check_features` and leaves the
+others at their defaults: :class:`~baton_b200.parallel.engine.FederatedEngine`, both sessions (at construction, and per
+round with the round's effective ``dp`` / ``robust``), :class:`~baton_b200.config.FederationConfig`, the manager planes
+and the local trainers.  The rules are checked in one fixed order, so a configuration that breaks two of them gets the
+same reason from every entry point.  A new feature adds its rules here.  Checks of one feature's own values stay with
+the feature (``check_dp``, ``check_robust``, ``TopKConfig``, ``ServerOptConfig``, ...).
+"""
+from __future__ import annotations
+
+from typing import Optional, Tuple
+
+OPTIMIZERS = ("sgd", "adamw")
+
+SEATED_SERVER_OPT = ("a server optimizer needs the http plane: on the seated planes its state would be replicated on "
+                     "the seats, an evicted seat would return with stale m and v, and the manager holds no copy to "
+                     "resend")
+
+
+def check_features(*, wire_dtype: str = "bf16", mode: str = "delta", dp=None, scaffold: bool = False, robust=None,
+                   topk=None, server_opt=None, tile_flags: bool = False, plane: Optional[str] = None,
+                   optimizer: str = "sgd", momentum: float = 0.0, nesterov: bool = False, prox_mu: float = 0.0) -> None:
+    """``ValueError`` with the reason if the features cannot run together.  ``dp``, ``robust``, ``topk`` and
+    ``server_opt`` are on unless they are None or False: the rules read only which features are on, so a caller may pass
+    the features' configurations or bools.  Whoever takes a configuration from outside checks its type.  ``plane``:
+    ``"http"`` or ``"seated"`` (the ``fused`` / ``nccl`` manager planes), None where no manager plane is involved."""
+    if optimizer not in OPTIMIZERS:
+        raise ValueError("optimizer must be one of {}, got {!r}".format(OPTIMIZERS, optimizer))
+    adamw = optimizer == "adamw"
+    dp, robust, topk, server_opt = (x is not None and x is not False for x in (dp, robust, topk, server_opt))
+    rules = (
+        (adamw and (momentum or nesterov), "momentum / nesterov are SGD options; AdamW keeps its own moments (betas)"),
+        (adamw and prox_mu > 0, "AdamW with FedProx (prox_mu > 0) is not supported"),
+        (adamw and scaffold, "AdamW with SCAFFOLD is not supported: option II's dc = (x - theta) / (K lr) - c assumes "
+                             "SGD steps"),
+        (scaffold and prox_mu > 0, "SCAFFOLD's correction and FedProx's proximal term are exclusive"),
+        (topk and wire_dtype == "fp8", "top-k uploads with the fp8 wire are not supported: its block scales have no "
+                                       "meaning on a sparse list"),
+        (topk and dp, "top-k uploads with DP-FedAvg are not supported: the noise is calibrated to the dense clipped "
+                      "mean"),
+        (topk and robust, "top-k uploads with a robust aggregator are not supported: it needs every client's dense "
+                          "update"),
+        (topk and scaffold, "top-k uploads with SCAFFOLD are not supported: its control-variate segment is dense"),
+        (topk and tile_flags, "top-k uploads with tile_flags are not supported"),
+        (server_opt and plane == "seated", SEATED_SERVER_OPT),
+        (scaffold and dp, "SCAFFOLD with DP-FedAvg is not supported: DP would also have to clip and noise dc"),
+        (scaffold and tile_flags, "SCAFFOLD with tile_flags is not supported: the correction c - c_i reads c, which "
+                                  "the previous round's collective writes, so it cannot run ahead of the join"),
+        (robust and dp, "a robust aggregator with DP-FedAvg is not supported: DP's noise is calibrated to the clipped "
+                        "mean"),
+        (robust and scaffold, "a robust aggregator with SCAFFOLD is not supported: its control-variate update is a "
+                              "mean"),
+        (robust and tile_flags, "a robust aggregator with tile_flags is not supported"),
+    )
+    for broken, reason in rules:
+        if broken:
+            raise ValueError(reason)
+    if mode != "delta":
+        for on, name in ((topk, "top-k uploads"), (server_opt, "a server optimizer"), (dp, "DP-FedAvg"),
+                         (scaffold, "SCAFFOLD"), (robust, "a robust aggregator")):
+            if on:
+                raise ValueError("{} needs mode='delta': it works on the update theta - global, which "
+                                 "mode='weights' does not upload".format(name))
+
+
+def peer_loads_only(*, wire_dtype: str, dp=None, scaffold: bool = False, robust=None, topk=None) -> bool:
+    """True when a round cannot use NVLS: the switch adds raw wire values, so block-scaled fp8, DP's per-rank clip
+    factors, SCAFFOLD's reader-side 1 / N, a selection (robust) and sparse lists (top-k) all need peer loads."""
+    return wire_dtype == "fp8" or any(x is not None and x is not False for x in (dp, scaffold, robust, topk))
+
+
+def round_plan(world: int, logical_clients: int = 0, sample_k: Optional[int] = None) -> Tuple[int, int]:
+    """``(planned, max_clients)``: the participants a round plans for (what Krum's ``2f + 3`` and the robust
+    aggregators' limit are checked against) and the client segments one rank may upload per round."""
+    population = logical_clients if logical_clients and logical_clients > world else world
+    planned = min(sample_k, population) if sample_k else population
+    per_rank = -(-population // world) if population > world > 0 else 1
+    return planned, min(per_rank, planned)

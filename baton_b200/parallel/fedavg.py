@@ -57,8 +57,9 @@ from typing import List, Optional, Sequence
 import torch
 
 from .arena import ParamArena
-from .compress import TopKConfig, check_topk_exclusions, n_float, sparse_upload_bytes, topk_ef_
+from .compress import TopKConfig, n_float, sparse_upload_bytes, topk_ef_
 from .dp import DPConfig, clip_factor, normals
+from .features import check_features, peer_loads_only
 from .robust import MAX_ROBUST_CLIENTS, RobustConfig, krum_select, robust_combine
 from .server_opt import ServerOptConfig, apply_update_
 from .symm import SymmetricBuffer
@@ -71,79 +72,33 @@ def _align(x: int, a: int) -> int:
     return (x + a - 1) // a * a
 
 
-def _check_dp_mode(dp: Optional[DPConfig], delta: bool) -> None:
-    if dp is not None and not delta:
-        raise ValueError("DP-FedAvg clips and noises the update theta - global: it needs mode='delta'")
+def _session_rules(features: dict, dp: Optional[DPConfig], robust: Optional[RobustConfig]) -> None:
+    """:func:`check_features` for a session's features with a round's ``dp`` / ``robust``, after ``TypeError`` for a
+    ``robust``, ``topk`` or ``server_opt`` that is not its configuration class."""
+    for x, cls, name in ((robust, RobustConfig, "robust"), (features["topk"], TopKConfig, "topk"),
+                         (features["server_opt"], ServerOptConfig, "server_opt")):
+        if x is not None and not isinstance(x, cls):
+            raise TypeError("{}= takes a {}".format(name, cls.__name__))
+    check_features(dp=dp, robust=robust, **features)
 
 
-def _check_scaffold(scaffold: bool, dp: Optional[DPConfig], delta: bool) -> None:
-    if scaffold and not delta:
-        raise ValueError("SCAFFOLD needs mode='delta'")
-    if scaffold and dp is not None:
-        raise ValueError("SCAFFOLD and DP-FedAvg are exclusive: DP would have to clip and noise dc too")
-
-
-def _check_robust(robust: Optional[RobustConfig], dp: Optional[DPConfig], scaffold: bool, delta: bool,
-                  tile_flags: bool, max_clients: int, topk: Optional[TopKConfig] = None) -> int:
-    if robust is None:
-        if topk is not None:      # the folded clients' union of supports sizes the sparse segment
-            if int(max_clients) < 1:
-                raise ValueError("max_clients must be >= 1, got {!r}".format(max_clients))
-            return int(max_clients)
-        if int(max_clients) != 1:
-            raise ValueError("max_clients > 1 needs a robust aggregator: plain rounds fold their clients into one upload")
-        return 1
-    if not isinstance(robust, RobustConfig):
-        raise TypeError("robust= takes a RobustConfig")
-    if not delta:
-        raise ValueError("robust aggregation combines the updates theta - global: it needs mode='delta'")
-    if dp is not None:
-        raise ValueError("robust aggregation with DP-FedAvg is not supported: DP's sensitivity bound assumes the clipped "
-                         "mean")
-    if scaffold:
-        raise ValueError("robust aggregation with SCAFFOLD is not supported: its control-variate update is a mean")
-    if tile_flags:
-        raise ValueError("robust aggregation with tile_flags is not supported")
-    if not (1 <= int(max_clients) <= MAX_ROBUST_CLIENTS):
-        raise ValueError("max_clients must be in 1..{}, got {!r}".format(MAX_ROBUST_CLIENTS, max_clients))
+def _init_session(arena: ParamArena, features: dict, dp: Optional[DPConfig], robust: Optional[RobustConfig],
+                  max_clients: int) -> int:
+    """Check a session's features (either kind of session), allocate the server optimizer's fresh state in the arena
+    (``m = 0``, ``v = tau^2``) and return the client segments per rank."""
+    _session_rules(features, dp, robust)
+    if robust is not None:
+        if not (1 <= int(max_clients) <= MAX_ROBUST_CLIENTS):
+            raise ValueError("max_clients must be in 1..{}, got {!r}".format(MAX_ROBUST_CLIENTS, max_clients))
+    elif features["topk"] is not None:      # the folded clients' union of supports sizes the sparse segment
+        if int(max_clients) < 1:
+            raise ValueError("max_clients must be >= 1, got {!r}".format(max_clients))
+    elif int(max_clients) != 1:
+        raise ValueError("max_clients > 1 needs a robust aggregator: plain rounds fold their clients into one upload")
+    server_opt = features["server_opt"]
+    if server_opt is not None:
+        arena.server_m, arena.server_v = server_opt.init_state(arena.n_param, arena.device)
     return int(max_clients)
-
-
-def _check_topk(topk: Optional[TopKConfig], wire_dtype: str, dp, robust, scaffold: bool, delta: bool,
-                tile_flags: bool) -> Optional[TopKConfig]:
-    if topk is None:
-        return None
-    if not isinstance(topk, TopKConfig):
-        raise TypeError("topk= takes a TopKConfig")
-    check_topk_exclusions(wire_dtype=wire_dtype, dp=dp, robust=robust, scaffold=scaffold, delta=delta,
-                          tile_flags=tile_flags)
-    return topk
-
-
-def _init_server_opt(arena: ParamArena, server_opt: Optional[ServerOptConfig], delta: bool) -> Optional[ServerOptConfig]:
-    """Validate a session's ``server_opt`` and allocate its fresh state in the arena (``m = 0``, ``v = tau^2``)."""
-    if server_opt is None:
-        return None
-    if not isinstance(server_opt, ServerOptConfig):
-        raise TypeError("server_opt= takes a ServerOptConfig")
-    if not delta:
-        raise ValueError("a server optimizer steps on the pseudo-gradient global - aggregate: it needs mode='delta' "
-                         "(mode='weights' has none)")
-    arena.server_m, arena.server_v = server_opt.init_state(arena.n_param, arena.device)
-    return server_opt
-
-
-def _check_session(arena: ParamArena, wire_dtype: str, mode: str, dp: Optional[DPConfig], scaffold: bool,
-                   robust: Optional[RobustConfig], max_clients: int, tile_flags: bool,
-                   server_opt: Optional[ServerOptConfig], topk: Optional[TopKConfig]):
-    """Validate a session's combination of features (either kind of session: the same checks in the same order) and
-    allocate the server optimizer's state: ``(topk, server_opt, max_clients)``."""
-    delta = mode == "delta"
-    topk = _check_topk(topk, wire_dtype, dp, robust, scaffold, delta, tile_flags)
-    server_opt = _init_server_opt(arena, server_opt, delta)
-    _check_dp_mode(dp, delta)
-    _check_scaffold(scaffold, dp, delta)
-    return topk, server_opt, _check_robust(robust, dp, scaffold, delta, tile_flags, max_clients, topk)
 
 
 def _check_control(scaffold: bool, control) -> None:
@@ -174,8 +129,10 @@ class FedAvgSession:
         from ..ops._ext import load
         self._C = load()
         assert wire_dtype in ("bf16", "fp32", "fp8") and mode in ("delta", "weights")
-        self.topk, self.server_opt, self.max_clients = _check_session(arena, wire_dtype, mode, dp, scaffold, robust,
-                                                                      max_clients, tile_flags, server_opt, topk)
+        self._features = dict(wire_dtype=wire_dtype, mode=mode, scaffold=scaffold, topk=topk, server_opt=server_opt,
+                             tile_flags=tile_flags)
+        self.max_clients = _init_session(arena, self._features, dp, robust, max_clients)
+        self.topk, self.server_opt = topk, server_opt
         self._sopt_coef = list(server_opt.coefficients()) if server_opt is not None else []
         self.robust = robust
         self.krum = robust is not None and robust.kind == "krum"
@@ -229,14 +186,11 @@ class FedAvgSession:
         self.symm = SymmetricBuffer(total, self.device, group)
         self.rank, self.world = self.symm.rank, self.symm.world
         assert self.world <= self._C.MAX_RANKS
-        self.use_nvls = self.symm.has_multicast if nvls == "auto" else (bool(nvls) and self.symm.has_multicast)
-        if self.wire_kind == 2:
-            self.use_nvls = False      # the switch adds raw elements; block scales need the P2P path
+        # nvls: True, False or "auto" (on where the box has multicast; autotuned below)
+        self.use_nvls = bool(nvls and self.symm.has_multicast
+                             and not peer_loads_only(wire_dtype=wire_dtype, dp=dp, scaffold=scaffold, robust=robust,
+                                                     topk=topk))
         self.dp = _agree_seed(dp, group)
-        if self.dp is not None or self.scaffold or self.robust is not None or self.topk is not None:
-            # the clip factors / the 1 / N of the control variates are applied by the readers, a selection is not
-            # a sum, and the switch cannot add sparse lists: peer loads only
-            self.use_nvls = False
         self._topk_work = None          # top-k: the selection's scratch, the residual-less u, the last upload's row end
         self._topk_u = None
         self._topk_end = None
@@ -487,15 +441,10 @@ class FedAvgSession:
         planes' plan carries it)."""
         world = self.world
         dp = dp if dp is not None else self.dp
-        _check_dp_mode(dp, self.delta)
-        _check_control(self.scaffold, control)
-        if control is not None and dp is not None:
-            raise ValueError("SCAFFOLD and DP-FedAvg are exclusive")
         robust = robust if robust is not None else self.robust
-        if self.topk is not None and (dp is not None or robust is not None):
-            raise ValueError("a top-k session runs top-k rounds only (no DP-FedAvg or robust rounds)")
-        if robust is not None and robust is not self.robust:
-            _check_robust(robust, dp, self.scaffold, self.delta, self.tile_flags is not None, 1)
+        if dp is not self.dp or robust is not self.robust:     # the session's own features were checked when built
+            _session_rules(self._features, dp, robust)
+        _check_control(self.scaffold, control)
         if robust is None and n_clients is not None:
             raise ValueError("n_clients= needs a robust session or robust=")
         if robust is not None and robust.kind == "krum" and not self.krum:
@@ -530,7 +479,9 @@ class FedAvgSession:
         a = self.arena
         # the optimizer's wire copy is only valid for the round / scale it was armed for and when the collective runs
         # the way arm_prepack assumed (NVLS needs every rank alive); otherwise the kernel packs itself (always correct)
-        nvls_now = bool(self.use_nvls and len(alive) == world and dp is None and robust is None)
+        nvls_now = bool(self.use_nvls and len(alive) == world
+                        and not peer_loads_only(wire_dtype=self.wire_dtype, dp=dp, scaffold=self.scaffold,
+                                                robust=robust, topk=self.topk))
         want_scale = (counts[self.rank] if not from_flags else float(my_n)) if (self.use_nvls and world > 1) else 1.0
         prepacked = bool(prepacked and self.wire_kind != 2 and self._armed_for == (self.epoch, float(want_scale))
                          and (nvls_now == bool(self.use_nvls and world > 1)))
@@ -738,8 +689,10 @@ class NcclSession:
                  robust: Optional[RobustConfig] = None, max_clients: int = 1, tile_flags: bool = False,
                  server_opt: Optional[ServerOptConfig] = None, topk: Optional[TopKConfig] = None, **_unused):
         import torch.distributed as dist
-        self.topk, self.server_opt, self.max_clients = _check_session(arena, wire_dtype, mode, dp, scaffold, robust,
-                                                                      max_clients, tile_flags, server_opt, topk)
+        self._features = dict(wire_dtype=wire_dtype, mode=mode, scaffold=scaffold, topk=topk, server_opt=server_opt,
+                             tile_flags=tile_flags)
+        self.max_clients = _init_session(arena, self._features, dp, robust, max_clients)
+        self.topk, self.server_opt = topk, server_opt
         # top-k: k, this rank's upload of the round as a dense fp32 vector (zeros off its support) and its entry count
         self.topk_k = self.topk.k(n_float(arena)) if self.topk is not None else 0
         self._topk_up = None
@@ -882,12 +835,14 @@ class NcclSession:
         manager's plan) sets the round counter, as it sets the fused session's barrier epoch.  ``control = (c, dc,
         n_clients)``: SCAFFOLD, as in :meth:`FedAvgSession.aggregate` -- all-reduce ``dc`` as a sum (a rank without
         participants contributes zeros), then ``c += sum / n_clients``."""
+        dp = dp if dp is not None else self.dp
+        robust = robust if robust is not None else self.robust
+        if dp is not self.dp or robust is not self.robust:     # the session's own features were checked when built
+            _session_rules(self._features, dp, robust)
         _check_control(self.scaffold, control)
         if round_index is not None:
             self.rounds = int(round_index)
         a, dist = self.arena, self.dist
-        dp = dp if dp is not None else self.dp
-        _check_dp_mode(dp, self.delta)
         if n_samples_by_rank is not None:
             counts = torch.tensor([float(x) for x in n_samples_by_rank][: self.world], device=self.device)
         else:
@@ -899,10 +854,7 @@ class NcclSession:
         total = counts.sum()
         w = counts[self.rank] / total
         src = (a.theta - a.global_w) if self.delta else a.theta
-        robust = robust if robust is not None else self.robust
         if self.topk is not None:
-            if dp is not None or robust is not None:
-                raise ValueError("a top-k session runs top-k rounds only (no DP-FedAvg or robust rounds)")
             mine = float(counts[self.rank]) != 0.0
             if mine and self._topk_up is None:
                 raise RuntimeError("a top-k round needs this rank's upload packed for it (pack_topk or pack_nonzero)")

@@ -60,9 +60,6 @@ def check_prox_mu(prox_mu: float) -> float:
     return mu
 
 
-OPTIMIZERS = ("sgd", "adamw")
-
-
 def check_adamw(betas, eps) -> Tuple[Tuple[float, float], float]:
     """AdamW's ``(betas, eps)`` as floats; ``ValueError`` unless both betas are in [0, 1) and ``eps > 0`` (finite)."""
     try:
@@ -80,19 +77,13 @@ def check_adamw(betas, eps) -> Tuple[Tuple[float, float], float]:
 
 def check_optimizer(optimizer: str, momentum: float = 0.0, nesterov: bool = False, prox_mu: float = 0.0,
                     corr=None) -> bool:
-    """True for ``"adamw"``, False for ``"sgd"``; ``ValueError`` for another name, or for AdamW together with
-    momentum, Nesterov, FedProx or SCAFFOLD (terms of the SGD step)."""
-    if optimizer not in OPTIMIZERS:
-        raise ValueError("optimizer must be one of {}, got {!r}".format(OPTIMIZERS, optimizer))
-    if optimizer != "adamw":
-        return False
-    if momentum or nesterov:
-        raise ValueError("momentum / nesterov are SGD options; AdamW keeps its own moments (betas)")
-    if prox_mu > 0:
-        raise ValueError("AdamW with FedProx (prox_mu > 0) is not supported")
-    if corr is not None:
-        raise ValueError("AdamW with SCAFFOLD is not supported: its control-variate update assumes SGD steps")
-    return True
+    """True for ``"adamw"``, False for ``"sgd"``; ``ValueError`` for another name, or for a local step that cannot
+    combine its terms (``parallel/features.py``: AdamW with momentum, Nesterov, FedProx or SCAFFOLD, and SCAFFOLD's
+    correction ``corr`` with FedProx)."""
+    from .parallel.features import check_features
+    check_features(optimizer=optimizer, momentum=momentum, nesterov=nesterov, prox_mu=prox_mu,
+                   scaffold=corr is not None)
+    return optimizer == "adamw"
 
 
 def _add_prox_term(params, anchors, prox_mu: float) -> None:
@@ -103,12 +94,8 @@ def _add_prox_term(params, anchors, prox_mu: float) -> None:
                 p.grad.add_(p.detach() - a, alpha=prox_mu)
 
 
-def _check_corr(corr, prox_mu: float, arena) -> None:
-    if corr is None:
-        return
-    if prox_mu > 0:
-        raise ValueError("SCAFFOLD's correction and FedProx's proximal term are exclusive")
-    if corr.dtype != torch.float32 or not corr.is_contiguous() or corr.numel() < arena.n_param:
+def _check_corr(corr, arena) -> None:
+    if corr is not None and (corr.dtype != torch.float32 or not corr.is_contiguous() or corr.numel() < arena.n_param):
         raise ValueError("corr must be a contiguous fp32 buffer covering the arena's parameters")
 
 
@@ -535,7 +522,7 @@ class GraphedLocalSGD:
         prox_mu = check_prox_mu(prox_mu)
         if prox_mu > 0 and self.arena.global_w is None:
             raise ValueError("prox_mu > 0 needs the arena's global copy (ParamArena(keep_global=True))")
-        _check_corr(corr, prox_mu, self.arena)
+        _check_corr(corr, self.arena)
         self.adam = check_optimizer(optimizer, momentum, self.nesterov, prox_mu, corr)
         if self.adam:
             betas, eps = check_adamw(betas, eps)
@@ -625,7 +612,7 @@ class PortableLocalSGD:
         ``optimizer="adamw"``: a fresh ``torch.optim.AdamW(lr, betas, eps, weight_decay)`` instead of SGD."""
         criterion = _loss_fn(self.loss_kind)
         prox_mu = check_prox_mu(prox_mu)
-        _check_corr(corr, prox_mu, self.arena)
+        _check_corr(corr, self.arena)
         adam = check_optimizer(optimizer, momentum, prox_mu=prox_mu, corr=corr)
         n = X.shape[0]
         batch_size = min(batch_size, n)
