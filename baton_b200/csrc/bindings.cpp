@@ -350,11 +350,6 @@ void quant_mx_cols(const at::Tensor& x, at::Tensor q, at::Tensor sf, int64_t R, 
   const c10::cuda::CUDAGuard guard(x.device());
   check(b200_quant_mx_cols(x.data_ptr(), q.data_ptr(), sf.data_ptr(), R, C, ld_in, Rp, cur_stream()), "quant_mx_cols");
 }
-void dequant_mx(const at::Tensor& q, const at::Tensor& sf, at::Tensor out, int64_t R, int64_t C, int64_t Cp) {
-  CHECK_CUDA(q);
-  const c10::cuda::CUDAGuard guard(q.device());
-  check(b200_dequant_mx(q.data_ptr(), sf.data_ptr(), out.data_ptr<float>(), R, C, Cp, cur_stream()), "dequant_mx");
-}
 
 void fused_sgd(at::Tensor w, at::Tensor g, const std::optional<at::Tensor>& mom, const std::optional<at::Tensor>& wb,
                const at::Tensor& hyper, bool zero_grad, bool nesterov, const std::optional<at::Tensor>& wire_slot,
@@ -1150,7 +1145,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("gemm_fp8", &gemm_fp8);
   m.def("quant_mx_rows", &quant_mx_rows);
   m.def("quant_mx_cols", &quant_mx_cols);
-  m.def("dequant_mx", &dequant_mx);
   m.def("fused_sgd", &fused_sgd);
   m.def("fused_sgd_segments", &fused_sgd_segments);
   m.def("weighted_sum", &weighted_sum);

@@ -80,7 +80,6 @@ int b200_gemm_fp8(const void* a, const void* b, void* d, const float* bias, cons
 int b200_quant_mx_rows(const void* x, void* q, void* sf, long long R, int C, long long ld_in, int Cp, cudaStream_t stream);
 int b200_quant_mx_cols(const void* x, void* q, void* sf, long long R, int C, long long ld_in, long long Rp,
                        cudaStream_t stream);
-int b200_dequant_mx(const void* q, const void* sf, float* out, long long R, int C, int Cp, cudaStream_t stream);
 int b200_gemm_simt(const void* a, const void* b, void* d, const float* bias, int M, int N, int K, long long lda,
                    long long ldb, long long ldd, int a_mn, int b_mn, int out_fp32, int act, int accumulate,
                    float alpha, cudaStream_t stream);

@@ -104,21 +104,6 @@ quant_mx_cols_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restrict__ 
   }
 }
 
-// reference dequantiser (tests): q[R, Cp] + atoms -> fp32 [R, C]
-__global__ void dequant_mx_kernel(const uint8_t* __restrict__ q, const uint8_t* __restrict__ sf, float* __restrict__ out,
-                                  long long R, int C, int Cp, int Cpad) {
-  const long long total = R * C;
-  const long long k_tiles = Cpad >> 7;
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const long long r = i / C;
-    const int c = static_cast<int>(i - r * C);
-    const __nv_fp8_e4m3 v = *reinterpret_cast<const __nv_fp8_e4m3*>(q + r * Cp + c);
-    const int e = static_cast<int>(sf[sf_offset(r, c, k_tiles)]) - 127;
-    out[i] = static_cast<float>(v) * exp2_int(e);
-  }
-}
-
 }  // namespace b200
 
 using namespace b200;
@@ -143,15 +128,6 @@ extern "C" int b200_quant_mx_cols(const void* x, void* q, void* sf, long long R,
   dim3 grid(Cpad / 128, static_cast<unsigned>(Rpad / 32));
   launch_pdl(quant_mx_cols_kernel, grid, 128, 0, stream, reinterpret_cast<const __nv_bfloat16*>(x),
              reinterpret_cast<uint8_t*>(q), reinterpret_cast<uint8_t*>(sf), R, C, ld_in, Rp, Rpad, Cpad);
-  return static_cast<int>(cudaGetLastError());
-}
-extern "C" int b200_dequant_mx(const void* q, const void* sf, float* out, long long R, int C, int Cp, cudaStream_t stream) {
-  if (R <= 0 || C <= 0) return 0;
-  const int Cpad = (C + 127) / 128 * 128;
-  long long blocks = (R * C + 255) / 256;
-  if (blocks > device_sm_count() * 8) blocks = device_sm_count() * 8;
-  dequant_mx_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
-      reinterpret_cast<const uint8_t*>(q), reinterpret_cast<const uint8_t*>(sf), out, R, C, Cp, Cpad);
   return static_cast<int>(cudaGetLastError());
 }
 

@@ -761,23 +761,20 @@ def quant_mx_cols(x2d: torch.Tensor):
     return q, sf
 
 
-def dequant_mx(q: torch.Tensor, sf: torch.Tensor, cols: int) -> torch.Tensor:
-    R, Cp = q.shape
-    out = torch.empty((R, cols), dtype=torch.float32, device=q.device)
-    load().dequant_mx(q, sf, out, R, cols, Cp)
-    return out
-
-
 def gemm_fp8(qa: torch.Tensor, sfa, qb: torch.Tensor, sfb, K: int, *, out: Optional[torch.Tensor] = None,
              out_dtype: torch.dtype = BF16, bias: Optional[torch.Tensor] = None, act: int = 0,
              accumulate: bool = False, alpha: float = 1.0, split_k: int = 1, n_valid: Optional[int] = None):
-    """``out[M,N] = act(alpha * (A*SFA) @ (B*SFB)^T + bias)`` with e4m3 operands ``qa [M,Kp]``, ``qb [N,Kp]``."""
+    """``out[M,N] = act(alpha * (A*SFA) @ (B*SFB)^T + bias)`` with e4m3 operands ``qa [M,Kp]``, ``qb [N,Kp]``.
+    ``accumulate`` adds onto ``out``.  With ``split_k > 1`` the K slices add their partial products into ``out`` with
+    atomics, so without ``accumulate`` the output is zeroed first."""
     M, N = qa.shape[0], qb.shape[0]
     if n_valid is not None:
         N = min(N, n_valid)
     if out is None:
-        out = torch.zeros((M, N), dtype=out_dtype, device=qa.device) if accumulate else \
+        out = torch.zeros((M, N), dtype=out_dtype, device=qa.device) if (accumulate or split_k > 1) else \
             torch.empty((M, N), dtype=out_dtype, device=qa.device)
+    elif split_k > 1 and not accumulate:
+        out.zero_()
     ldd = out.stride(0) if out.dim() == 2 else N
     load().gemm_fp8(qa, qb, out, bias, sfa, sfb, M, N, K, qa.stride(0), qb.stride(0), ldd, act, split_k, accumulate, alpha)
     return out

@@ -1,5 +1,6 @@
-"""MXFP8 tier: quantisers (rows / fused transpose) and the block-scaled wgmma GEMM against a
-dequantise-then-fp32-matmul reference (exact up to accumulation order)."""
+"""MXFP8 tier: the unscaled GEMM kind, the fp8 layers against their bf16 counterparts, and ResNet-18 training in
+MXFP8.  The quantisers and the block-scaled GEMM are checked byte for byte and element by element against the
+float64 reference in tests/test_gpu_mxfp8.py."""
 import pytest
 import torch
 
@@ -10,51 +11,6 @@ BF16 = torch.bfloat16
 def _rel(a, b):
     a, b = a.detach().float(), b.detach().float()
     return float((a - b).abs().max() / (b.abs().max() + 1e-6))
-
-
-@pytest.mark.parametrize("R,C", [(256, 512), (300, 200), (128, 4608), (1000, 72)])
-def test_quant_rows_and_cols_roundtrip(R, C):
-    from baton_b200.ops import functional as F
-    torch.manual_seed(R + C)
-    dev = torch.device("cuda:0")
-    x = (torch.randn(R, C, device=dev) * torch.logspace(-3, 2, C, device=dev)).to(BF16)
-    q, sf = F.quant_mx_rows(x)
-    back = F.dequant_mx(q, sf, C)
-    # e4m3 has 3 mantissa bits: relative error per element <= 2^-4 of the block maximum
-    blk = x.float().abs().reshape(R, -1)
-    err = (back - x.float()).abs()
-    tol = torch.zeros_like(err)
-    for c0 in range(0, C, 32):
-        tol[:, c0:c0 + 32] = x[:, c0:c0 + 32].float().abs().amax(1, keepdim=True) / 8 + 1e-30
-    assert bool((err <= tol).all()), float((err / tol).max())
-    assert _rel(back, x) < 0.07
-    qt, sft = F.quant_mx_cols(x)
-    assert qt.shape[0] == C
-    backt = F.dequant_mx(qt, sft, R)          # [C, R] == x^T
-    assert _rel(backt, x.float().t()) < 0.07
-
-
-@pytest.mark.parametrize("M,N,K", [(128, 128, 128), (256, 384, 512), (300, 200, 1000), (512, 64, 4608), (1000, 256, 72)])
-def test_gemm_mxfp8_matches_dequantised_reference(M, N, K):
-    from baton_b200.ops import functional as F
-    torch.manual_seed(M + N + K)
-    dev = torch.device("cuda:0")
-    A = (torch.randn(M, K, device=dev) * 3).to(BF16)
-    B = (torch.randn(N, K, device=dev) * 0.2).to(BF16)
-    qa, sa = F.quant_mx_rows(A)
-    qb, sb = F.quant_mx_rows(B)
-    ref = F.dequant_mx(qa, sa, K) @ F.dequant_mx(qb, sb, K).t()
-    out = F.gemm_fp8(qa, sa, qb, sb, K, out_dtype=torch.float32)
-    assert out.shape == (M, N)
-    assert _rel(out, ref) < 2e-3, _rel(out, ref)
-    # and it is a faithful fp8 approximation of the bf16 product
-    assert _rel(out, A.float() @ B.float().t()) < 0.08
-    bias = torch.randn(N, device=dev)
-    out2 = F.gemm_fp8(qa, sa, qb, sb, K, bias=bias, act=1)
-    assert _rel(out2, torch.relu(ref + bias)) < 1e-2
-    acc = torch.ones(M, N, device=dev)
-    F.gemm_fp8(qa, sa, qb, sb, K, out=acc, accumulate=True, split_k=3)
-    assert _rel(acc, ref + 1.0) < 2e-3
 
 
 def test_gemm_fp8_unscaled_kind():
@@ -120,7 +76,9 @@ def test_resnet18_trains_in_mxfp8_under_cuda_graph():
 
     def evidence(m, hist):
         """What a non-converging run looked like: loss history, non-finite parameters, and the fp8 GEMM of this
-        process at the ResNet-18 layer shapes against the dequantise-then-fp32 reference."""
+        process at the ResNet-18 layer shapes against the float64 reference of tests/mxref.py: whether the quantised
+        bytes match it, and the worst |error| / sum_kb sa * sb * sum |qa * qb| (about 2^-8 at most when correct)."""
+        import mxref
         from baton_b200.ops import functional as F
         bad = [n for n, p in m.named_parameters() if not bool(torch.isfinite(p).all())]
         errs = {}
@@ -130,9 +88,14 @@ def test_resnet18_trains_in_mxfp8_under_cuda_graph():
             b = torch.randn(N, K, device=dev, generator=g).to(BF16)
             qa, sa = F.quant_mx_rows(a)
             qb, sb = F.quant_mx_rows(b)
-            ref = F.dequant_mx(qa, sa, K) @ F.dequant_mx(qb, sb, K).t()
-            errs["{}x{}x{}".format(M, N, K)] = _rel(F.gemm_fp8(qa, sa, qb, sb, K, out_dtype=torch.float32), ref)
-        return "history {} non-finite parameters {} fp8 GEMM rel. error {}".format(hist, bad[:8], errs)
+            ra, rsa = mxref.quant_rows(a)
+            rb, rsb = mxref.quant_rows(b)
+            same = all(torch.equal(u, v) for u, v in ((qa, ra), (sa, rsa), (qb, rb), (sb, rsb)))
+            acc, mag = mxref.gemm(ra, rsa, rb, rsb, K)
+            out = F.gemm_fp8(qa, sa, qb, sb, K, out_dtype=torch.float32).double()
+            errs["{}x{}x{}".format(M, N, K)] = "bytes {} error/magnitude {:.3g}".format(
+                "match" if same else "DIFFER", float(((out - acc).abs() / mag.clamp_min(1e-300)).max()))
+        return "history {} non-finite parameters {} fp8 GEMM {}".format(hist, bad[:8], errs)
 
     # Typical history: 1.29, 0.07, 0.003, ...  An intermittent non-converging run inside the full suite is recorded in
     # DESIGN.md ("Known issue"); a failed attempt reports its evidence and is repeated once, and the assertion message
