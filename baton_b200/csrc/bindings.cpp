@@ -790,6 +790,43 @@ void fedavg_allreduce_topk(const std::vector<int64_t>& wire_ptrs, const std::vec
   launch_round(theta, a, n_ctas, "fedavg_allreduce_topk", sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
 }
 
+// personalized round (plain mean): the arena elements [local_lo, local_lo + local_len) are client-local and left alone;
+// the kernel works over the n - local_len shared elements (LocalArgs in launch.h)
+template <class Base>
+static void launch_local(const at::Tensor& theta, const Base& b, int64_t lo, int64_t len, int64_t n_ctas) {
+  LocalArgs<Base> l = {};
+  static_cast<Base&>(l) = b;
+  TORCH_CHECK(lo >= 0 && len > 0 && lo + len <= b.n, "local range outside the arena");
+  l.n = b.n - len;
+  l.lo = lo;
+  l.len = len;
+  const c10::cuda::CUDAGuard guard(theta.device());
+  check(b200_fedavg_round(&l, static_cast<int>(n_ctas), cur_stream()), "fedavg_allreduce_local");
+}
+
+void fedavg_allreduce_local(const std::vector<int64_t>& wire_ptrs, const std::vector<int64_t>& pad_ptrs,
+                            int64_t wire_mc, at::Tensor theta, const std::optional<at::Tensor>& global_w,
+                            const std::optional<at::Tensor>& theta_bf16, const std::optional<at::Tensor>& momentum,
+                            const std::optional<at::Tensor>& int_local, const std::vector<int64_t>& int_wire_ptrs,
+                            const std::optional<at::Tensor>& loss_local, const std::vector<int64_t>& loss_wire_ptrs,
+                            const std::optional<at::Tensor>& loss_out, const std::vector<double>& n_samples,
+                            bool counts_from_flags, int64_t alive_mask, int64_t rank, int64_t world, int64_t wire_kind,
+                            bool delta, bool use_nvls, int64_t epoch, const std::optional<at::Tensor>& tile_flags,
+                            int64_t flag_value, int64_t tile_elems, int64_t n_ctas, int64_t timeout_log2,
+                            const std::optional<at::Tensor>& status, const std::optional<at::Tensor>& phase_ns,
+                            bool prepacked, int64_t local_lo, int64_t local_len,
+                            const std::optional<at::Tensor>& sopt_m, const std::optional<at::Tensor>& sopt_v,
+                            int64_t sopt_n_param, int64_t sopt_kind, const std::vector<double>& sopt_coef) {
+  FedAvgArgs a = {};
+  fill_fedavg_args(a, wire_ptrs, pad_ptrs, wire_mc, theta, global_w, theta_bf16, momentum, int_local, int_wire_ptrs,
+                   loss_local, loss_wire_ptrs, loss_out, n_samples, counts_from_flags, alive_mask, rank, world, wire_kind,
+                   delta, use_nvls, epoch, tile_flags, flag_value, tile_elems, timeout_log2, status, phase_ns, prepacked);
+  if (sopt_m.has_value() && sopt_m->defined())      // the server state is checked against the physical arena
+    launch_local(theta, sopt_args(a, sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef), local_lo, local_len, n_ctas);
+  else
+    launch_local(theta, a, local_lo, local_len, n_ctas);
+}
+
 static void check_topk_io(const at::Tensor& theta, const at::Tensor& global_w, const at::Tensor& work) {
   CHECK_CUDA(theta); CHECK_CUDA(global_w); CHECK_CUDA(work);
   TORCH_CHECK(theta.scalar_type() == at::kFloat && global_w.scalar_type() == at::kFloat && theta.is_contiguous() &&
@@ -1167,6 +1204,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.attr("KRUM_PAIRS") = B200_KRUM_PAIRS;
   m.attr("KRUM_REPORT") = B200_KRUM_REPORT;
   m.def("fedavg_allreduce_topk", &fedavg_allreduce_topk);
+  m.def("fedavg_allreduce_local", &fedavg_allreduce_local);
   m.def("topk_pack", &topk_pack);
   m.def("topk_fold", &topk_fold);
   m.def("nonzero_pack", &nonzero_pack);

@@ -936,7 +936,16 @@ __device__ __forceinline__ float sopt_step(float x, float d, float& m, float& v,
 // would not fit under the 96-register cap).  Parameter vectors (n_param % 8 == 0: a vector never straddles it) take
 // the step, or keep the global model when the round had no weight (step == false); buffers take global += d as in the
 // plain loop.  Then theta, the bf16 shadow and the momentum reset, as there.
-template <int WIRE, typename Args>
+// Personalized rounds (LocalArgs): the shift from logical element e to its physical arena element, which skips the
+// local range [lo, lo + len); 0 in every other round, so their address arithmetic is unchanged.  e and e + VEC - 1 are
+// on the same side of lo (a multiple of 1024), so one shift serves a whole wire vector.
+template <bool LOCAL, typename Args>
+__device__ __forceinline__ long long local_shift(const Args& a, long long e) {
+  if constexpr (LOCAL) return e >= a.lo ? a.len : 0ll;
+  else return 0ll;
+}
+
+template <int WIRE, bool LOCAL, typename Args>
 __device__ __forceinline__ void sopt_apply_tile(const Args& a, const uint8_t* my_wire, long long base, int len,
                                                 float apply_scale, bool step) {
   using W = Wire<WIRE>;
@@ -944,12 +953,13 @@ __device__ __forceinline__ void sopt_apply_tile(const Args& a, const uint8_t* my
   constexpr size_t esz = W::VBYTES / VEC;
   const size_t sc_off = static_cast<size_t>(a.n);
   for (int i = threadIdx.x * VEC; i < len; i += FEDAVG_THREADS * VEC) {
-    const long long e = base + i;
-    const uint4 wv = W::ld(my_wire + e * esz);
+    const long long le = base + i;                    // logical: the wire
+    const uint4 wv = W::ld(my_wire + le * esz);
     float scale = 1.f;
-    if constexpr (W::SCALED) scale = exp2_int(static_cast<int>(ld_volatile_u8(my_wire + sc_off + (e >> 5))) - 127);
+    if constexpr (W::SCALED) scale = exp2_int(static_cast<int>(ld_volatile_u8(my_wire + sc_off + (le >> 5))) - 127);
     float f[VEC];
     W::unpack(wv, f, scale);
+    const long long e = le + local_shift<LOCAL>(a, le);   // physical: the replica and the server state
     const bool opt = e < a.n_param;
 #pragma unroll
     for (int j = 0; j < VEC; j += 4) {
@@ -987,7 +997,10 @@ __device__ __forceinline__ void sopt_apply_tile(const Args& a, const uint8_t* my
 // kind (and whether the apply phase runs the server optimizer): fedavg_round_kernel<WIRE, Args> is the round's kernel.
 enum class Agg { mean, dp, scaffold, robust, krum, topk };
 template <class Args> struct RoundOf;
-template <Agg K> struct RoundKind { static constexpr Agg kind = K; static constexpr bool sopt = false; };
+template <Agg K> struct RoundKind {
+  static constexpr Agg kind = K;
+  static constexpr bool sopt = false, local = false;
+};
 template <> struct RoundOf<FedAvgArgs> : RoundKind<Agg::mean> {};
 template <> struct RoundOf<FedAvgDPArgs> : RoundKind<Agg::dp> {};
 template <> struct RoundOf<FedAvgScaffoldArgs> : RoundKind<Agg::scaffold> {};
@@ -996,7 +1009,11 @@ template <> struct RoundOf<FedAvgKrumArgs> : RoundKind<Agg::krum> {};
 template <> struct RoundOf<FedAvgTopkArgs> : RoundKind<Agg::topk> {};
 template <class Base> struct RoundOf<ServerOptArgs<Base>> {
   static constexpr Agg kind = RoundOf<Base>::kind;
-  static constexpr bool sopt = true;
+  static constexpr bool sopt = true, local = false;
+};
+template <class Base> struct RoundOf<LocalArgs<Base>> {
+  static constexpr Agg kind = RoundOf<Base>::kind;
+  static constexpr bool sopt = RoundOf<Base>::sopt, local = true;
 };
 
 // K == Agg::mean: the weighted mean w_k = n_k / N.
@@ -1010,8 +1027,10 @@ template <class Base> struct RoundOf<ServerOptArgs<Base>> {
 // epoch + 3.
 // Agg::topk: a top-k round (topk_reduce above): no pack phase, the uploads are sparse lists written before the launch.
 // SOPT (with any kind): a server-optimizer round -- the apply phase runs sopt_apply_tile.
-// The whole round; Args is the kind's args struct (ServerOptArgs<that> when SOPT), see RoundOf.
-template <int WIRE, Agg K, bool SOPT, typename Args>
+// LOCAL (with the mean): a personalized round -- n is the logical element count, and the pack and apply phases address
+// the replica at the physical element local_shift gives (see LocalArgs in launch.h).
+// The whole round; Args is the kind's args struct (ServerOptArgs<that> when SOPT, LocalArgs<...> when LOCAL), see RoundOf.
+template <int WIRE, Agg K, bool SOPT, bool LOCAL, typename Args>
 __device__ __forceinline__ void fedavg_round(const Args& a) {
   constexpr bool DP = K == Agg::dp, SCAF = K == Agg::scaffold, KRUM = K == Agg::krum, TOPK = K == Agg::topk;
   constexpr bool ROBUST = K == Agg::robust || KRUM;
@@ -1072,10 +1091,11 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
           for (int u = 0; u < 2; ++u) {
             const int i = i0 + u * STEP;
             if (i < len) {
+              const long long sh = local_shift<LOCAL>(a, base + i);
 #pragma unroll
               for (int j = 0; j < VEC; j += 4) {
-                th[u][j >> 2] = __ldcs(reinterpret_cast<const float4*>(theta_r + base + i + j));
-                if (a.delta) gg[u][j >> 2] = __ldcs(reinterpret_cast<const float4*>(global_r + base + i + j));
+                th[u][j >> 2] = __ldcs(reinterpret_cast<const float4*>(theta_r + base + i + j + sh));
+                if (a.delta) gg[u][j >> 2] = __ldcs(reinterpret_cast<const float4*>(global_r + base + i + j + sh));
               }
             }
           }
@@ -1308,7 +1328,7 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
       const long long base = t * T;
       const int len = static_cast<int>((n - base) < T ? (n - base) : T);
       constexpr int STEP = FEDAVG_THREADS * VEC;
-      if constexpr (SOPT) sopt_apply_tile<WIRE>(a, my_wire, base, len, apply_scale, s_inv_total != 0.f);
+      if constexpr (SOPT) sopt_apply_tile<WIRE, LOCAL>(a, my_wire, base, len, apply_scale, s_inv_total != 0.f);
       else for (int i0 = threadIdx.x * VEC; i0 < len; i0 += 2 * STEP) {
         uint4 wv[2];
         uint32_t sc[2];
@@ -1320,8 +1340,10 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
             wv[u] = W::ld(my_wire + (base + i) * esz);
             if constexpr (SCALED) sc[u] = ld_volatile_u8(my_wire + sc_off + ((base + i) >> 5));
             if (a.delta) {
+              const long long sh = local_shift<LOCAL>(a, base + i);
 #pragma unroll
-              for (int j = 0; j < VEC; j += 4) gg[u][j >> 2] = *reinterpret_cast<const float4*>(a.global_w + base + i + j);
+              for (int j = 0; j < VEC; j += 4)
+                gg[u][j >> 2] = *reinterpret_cast<const float4*>(a.global_w + base + i + j + sh);
             }
           }
         }
@@ -1333,6 +1355,7 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
             float scale = 1.f;
             if constexpr (SCALED) scale = exp2_int(static_cast<int>(sc[u]) - 127);
             W::unpack(wv[u], f, scale);
+            const long long sh = local_shift<LOCAL>(a, base + i);
 #pragma unroll
             for (int j = 0; j < VEC; j += 4) {
               float4 nw = make_float4(f[j] * apply_scale, f[j + 1] * apply_scale, f[j + 2] * apply_scale,
@@ -1341,13 +1364,13 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
                 const float4 g = gg[u][j >> 2];
                 nw.x += g.x; nw.y += g.y; nw.z += g.z; nw.w += g.w;
               }
-              if (a.global_w != nullptr) *reinterpret_cast<float4*>(a.global_w + base + i + j) = nw;
-              *reinterpret_cast<float4*>(a.theta + base + i + j) = nw;
-              if (a.momentum != nullptr && base + i + j < a.n_momentum)
-                *reinterpret_cast<float4*>(a.momentum + base + i + j) = make_float4(0.f, 0.f, 0.f, 0.f);
+              if (a.global_w != nullptr) *reinterpret_cast<float4*>(a.global_w + base + i + j + sh) = nw;
+              *reinterpret_cast<float4*>(a.theta + base + i + j + sh) = nw;
+              if (a.momentum != nullptr && base + i + j + sh < a.n_momentum)
+                *reinterpret_cast<float4*>(a.momentum + base + i + j + sh) = make_float4(0.f, 0.f, 0.f, 0.f);
               if (a.theta_bf16 != nullptr) {
                 const uint2 o = make_uint2(pack_bf16x2(nw.x, nw.y), pack_bf16x2(nw.z, nw.w));
-                *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(a.theta_bf16) + (base + i + j) * 2) = o;
+                *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(a.theta_bf16) + (base + i + j + sh) * 2) = o;
               }
             }
           }
@@ -1395,7 +1418,7 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
 // Robust, Krum and top-k rounds also take dynamic shared memory (ROBUST_SMEM, KRUM_SMEM, TOPK_SMEM: see round_smem).
 template <int WIRE, typename Args>
 __global__ void __maxnreg__(96) fedavg_round_kernel(const __grid_constant__ Args a) {
-  fedavg_round<WIRE, RoundOf<Args>::kind, RoundOf<Args>::sopt>(a);
+  fedavg_round<WIRE, RoundOf<Args>::kind, RoundOf<Args>::sopt, RoundOf<Args>::local>(a);
 }
 
 // one logical client's upload into its wire segment: the phase-0 pack of fedavg_round (delta mode, scale 1) over the
@@ -1615,11 +1638,21 @@ static bool topk_args_ok(const FedAvgTopkArgs* args) {
 }
 
 // the server step needs the pseudo-gradient (delta mode), the global copy and the state over [0, n_param)
+// (n_phys: the physical arena elements, args->n except in a personalized round)
 template <class Base>
-static bool sopt_args_ok(const ServerOptArgs<Base>* args) {
+static bool sopt_args_ok(const ServerOptArgs<Base>* args, long long n_phys) {
   return args->delta && args->global_w != nullptr && args->m != nullptr && args->kind >= 0 && args->kind <= 3 &&
          (args->kind == 0 || args->v != nullptr) && args->n_param >= 0 && args->n_param % 8 == 0 &&
-         args->n_param <= args->n;
+         args->n_param <= n_phys;
+}
+
+// a personalized round: whole 1024-element granules on both edges of the local range (no wire vector or fp8 block
+// crosses one), the range inside the physical arena, the plain mean and no arrival flags (they index physical granules)
+template <class Args>
+static bool local_args_ok(const Args* args) {
+  using b200::FLAG_GRANULE;
+  return b200::RoundOf<Args>::kind == b200::Agg::mean && args->tile_flags == nullptr && args->lo >= 0 &&
+         args->len > 0 && args->lo % FLAG_GRANULE == 0 && args->len % FLAG_GRANULE == 0 && args->lo <= args->n;
 }
 
 template <class Args>
@@ -1630,8 +1663,13 @@ int b200_fedavg_round(const Args* args, int n_ctas, cudaStream_t stream) {
   if (args->tile_flags != nullptr && args->tile_elems % FLAG_GRANULE != 0) return -2;
   // block-scaled fp8 wire: 32-element blocks must not straddle tiles, and the switch cannot rescale
   if (args->wire_kind == 2 && (args->tile_elems % 32 != 0 || args->use_nvls)) return -2;
+  long long n_phys = args->n;
+  if constexpr (RoundOf<Args>::local) {
+    if (!local_args_ok(args)) return -2;
+    n_phys += args->len;
+  }
   if constexpr (RoundOf<Args>::sopt) {
-    if (!sopt_args_ok(args)) return -2;
+    if (!sopt_args_ok(args, n_phys)) return -2;
   }
   if constexpr (K == Agg::dp) {
     if (!dp_args_ok(args)) return -2;
@@ -1665,6 +1703,8 @@ template int b200_fedavg_round(const ServerOptArgs<FedAvgScaffoldArgs>*, int, cu
 template int b200_fedavg_round(const ServerOptArgs<FedAvgRobustArgs>*, int, cudaStream_t);
 template int b200_fedavg_round(const ServerOptArgs<FedAvgKrumArgs>*, int, cudaStream_t);
 template int b200_fedavg_round(const ServerOptArgs<FedAvgTopkArgs>*, int, cudaStream_t);
+template int b200_fedavg_round(const LocalArgs<FedAvgArgs>*, int, cudaStream_t);
+template int b200_fedavg_round(const LocalArgs<ServerOptArgs<FedAvgArgs>>*, int, cudaStream_t);
 
 extern "C" int b200_pack_client(void* seg, float* theta, const float* global_w, void* w_bf16, float* mom, long long n_mom,
                                 long long n, int wire_kind, int reset, cudaStream_t stream) {

@@ -230,8 +230,21 @@ struct ServerOptArgs : Base {
   int kind;                         // 0 avgm, 1 adagrad, 2 yogi, 3 adam
   float coef[6];                    // b1, 1 - b1, b2, 1 - b2, lr, tau
 };
+// Personalized round (LocalArgs<FedAvgArgs> or LocalArgs<ServerOptArgs<FedAvgArgs>>: plain weighted mean, no arrival
+// flags): the physical arena range [lo, lo + len) holds client-local entries that the round never reads or writes, in
+// any buffer.  Base::n is then the LOGICAL element count n_shared = physical n - len; the wire, its tiles, the reduce
+// and fp8 block scales work over [0, n_shared) exactly as a plain round over n_shared elements.  The phases that touch the
+// replica (pack: theta, global_w; apply: global_w, theta, bf16 shadow, momentum reset, server m / v) address logical
+// element e at physical e + (e >= lo ? len : 0).  lo and len are multiples of 1024, so no wire vector or fp8 block
+// crosses an edge of the range; n_momentum and the server optimizer's n_param stay physical.
+template <class Base>
+struct LocalArgs : Base {
+  long long lo;                     // first physical element of the local range (multiple of 1024)
+  long long len;                    // elements in the local range (multiple of 1024)
+};
 // One FedAvg round of the kind Args names: FedAvgArgs, FedAvgDPArgs, FedAvgScaffoldArgs, FedAvgRobustArgs,
-// FedAvgKrumArgs, FedAvgTopkArgs, or ServerOptArgs<one of them>.  Runs fedavg_round_kernel<WIRE, Args> (csrc/fedavg.cu)
+// FedAvgKrumArgs, FedAvgTopkArgs, ServerOptArgs<one of them>, or LocalArgs<FedAvgArgs / ServerOptArgs<FedAvgArgs>>.
+// Runs fedavg_round_kernel<WIRE, Args> (csrc/fedavg.cu)
 // cooperatively on at most n_ctas CTAs; -2 when the arguments do not fit the kind.
 template <class Args>
 int b200_fedavg_round(const Args* args, int n_ctas, cudaStream_t stream);

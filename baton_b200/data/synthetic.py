@@ -14,6 +14,10 @@ Held-out data for evaluating the global model: ``holdout_image_shard`` /
 ``holdout_token_shard`` draw IID, class-balanced samples of the same classes
 (the same image class means, the same vocabulary bands) from a random stream
 that no training client uses, so accuracy on them measures generalisation.
+
+Personalized FL (FedBN / FedPer): ``image_shard(..., shift > 0)`` gives each client its own per-channel contrast and
+brightness change (FedBN's feature-shift setting), and ``client_holdout_image_shard`` draws held-out samples from one
+client's own label distribution and shift, for the per-client accuracy those methods report.
 """
 from __future__ import annotations
 
@@ -92,6 +96,22 @@ def _stream(seed: int, mult: int, client: int) -> torch.Generator:
     return torch.Generator().manual_seed(seed * mult + 1000003 * (client + 1))
 
 
+# seed offsets of a client's feature shift and of its own held-out samples, on top of its training stream's seed; neither
+# equals another client's training stream, the global held-out stream or the other for any seed >= 0
+_SHIFT_OFFSET = 250013
+_CLIENT_HOLDOUT_OFFSET = 500009
+
+
+def _client_shift(seed: int, client: int, channels: int, shift: float):
+    """Client ``client``'s per-channel ``(contrast, brightness)``: ``exp(shift z1)`` and ``shift z2``, or None for
+    ``shift == 0``."""
+    if shift == 0.0:
+        return None
+    g = torch.Generator().manual_seed(seed * 7919 + 1000003 * (client + 1) + _SHIFT_OFFSET)
+    z = torch.randn(2, channels, generator=g)
+    return torch.exp(shift * z[0]), shift * z[1]
+
+
 def _holdout_stream(seed: int, mult: int) -> torch.Generator:
     """Sample generator of the held-out data: a stream no training client and no class-mean draw uses."""
     return torch.Generator().manual_seed(seed * mult + _HOLDOUT_OFFSET)
@@ -103,8 +123,10 @@ def class_means(num_classes: int, *, channels: int = 3, size: int = 32, seed: in
     return torch.randn(num_classes, size, size, channels, generator=gm) * 0.5
 
 
-def _images(means, y, g, noise, dtype, channels_last, pin):
+def _images(means, y, g, noise, dtype, channels_last, pin, affine=None):
     X = means[y] + noise * torch.randn(y.numel(), *means.shape[1:], generator=g)
+    if affine is not None:
+        X = X * affine[0] + affine[1]          # per channel (the last axis)
     if not channels_last:
         X = X.permute(0, 3, 1, 2).contiguous()
     X = X.to(dtype)
@@ -120,14 +142,27 @@ def _balanced_labels(num_classes: int, n: int, g: torch.Generator) -> torch.Tens
 
 def image_shard(spec: ShardSpec, *, channels: int = 3, size: int = 32, seed: int = 0,
                 dtype=torch.float32, channels_last: bool = True, pin: bool = False,
-                noise: float = 1.0) -> Tuple[torch.Tensor, torch.Tensor]:
+                noise: float = 1.0, shift: float = 0.0) -> Tuple[torch.Tensor, torch.Tensor]:
     """Class-conditional Gaussian images: each class has a fixed random mean
     pattern (shared across clients through ``seed``), samples are mean + noise.
-    Returned as NHWC when ``channels_last`` (the layout the conv kernels use)."""
+    Returned as NHWC when ``channels_last`` (the layout the conv kernels use).
+    ``shift > 0``: the client's images also get its own per-channel contrast ``exp(shift z1)`` and brightness
+    ``shift z2`` (``z`` standard normal from a client-seeded stream); 0 returns the unshifted images."""
     means = class_means(spec.class_probs.numel(), channels=channels, size=size, seed=seed)
     g = _stream(seed, 7919, spec.client)
     y = _labels_for(spec, g)
-    return _images(means, y, g, noise, dtype, channels_last, pin)
+    return _images(means, y, g, noise, dtype, channels_last, pin, _client_shift(seed, spec.client, channels, shift))
+
+
+def client_holdout_image_shard(spec: ShardSpec, n: int, *, channels: int = 3, size: int = 32, seed: int = 0,
+                               dtype=torch.float32, channels_last: bool = True, pin: bool = False,
+                               noise: float = 1.0, shift: float = 0.0) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``n`` held-out images of client ``spec.client``: its label distribution and (``shift``) its feature shift, the
+    class means of :func:`image_shard`, from a stream no training client and no global held-out set draws from."""
+    means = class_means(spec.class_probs.numel(), channels=channels, size=size, seed=seed)
+    g = torch.Generator().manual_seed(seed * 7919 + 1000003 * (spec.client + 1) + _CLIENT_HOLDOUT_OFFSET)
+    y = torch.multinomial(spec.class_probs, n, replacement=True, generator=g)
+    return _images(means, y, g, noise, dtype, channels_last, pin, _client_shift(seed, spec.client, channels, shift))
 
 
 def holdout_image_shard(num_classes: int, n: int, *, channels: int = 3, size: int = 32, seed: int = 0,

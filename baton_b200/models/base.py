@@ -32,6 +32,7 @@ class FederatedModule(nn.Module):
     default_weight_decay = 0.0
     default_prox_mu = 0.0          # FedProx coefficient (0: plain SGD)
     default_optimizer = "sgd"      # local optimizer: "sgd" or "adamw" (betas / eps: local_train keywords)
+    head = None                    # state_dict prefix of the classifier head (local_keys="head"), None: no head
 
     def signature(self):
         return tuple((k, *v.shape) for k, v in self.state_dict().items())

@@ -88,6 +88,7 @@ class BertForSequenceClassification(FederatedModule):
     loss_kind = "ce"
     default_lr = 0.01
     default_batch_size = 32
+    head = "classifier"
 
     def __init__(self, config: Optional[BertConfig] = None, name: Optional[str] = None):
         super().__init__()

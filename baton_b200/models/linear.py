@@ -15,6 +15,7 @@ from .base import FederatedModule
 class LinearModel(FederatedModule):
     name = "lineartest"
     loss_kind = "mse"
+    head = "fc1"                   # the whole model: it cannot be kept local
 
     def __init__(self, in_features: int = 10, out_features: int = 1):
         super().__init__()
@@ -27,6 +28,7 @@ class LinearModel(FederatedModule):
 class MLP2(FederatedModule):
     name = "mlp2"
     loss_kind = "mse"
+    head = "fc2"
     default_lr = 0.01
 
     def __init__(self, in_features: int = 10, hidden: int = 64, out_features: int = 1):

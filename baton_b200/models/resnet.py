@@ -171,6 +171,7 @@ class ResNet(FederatedModule):
     loss_kind = "ce"
     default_lr = 0.05
     default_batch_size = 128
+    head = "fc"
 
     def __init__(self, block: Type[nn.Module], layers: Sequence[int], num_classes: int = 1000,
                  in_channels: int = 3, name: Optional[str] = None):

@@ -15,6 +15,9 @@ the checkpoint layout are unchanged (reference: the global model is addressed by
   (``theta_bf16``) and the frozen global copy used for delta uploads
   (``global_w``) are parallel flat buffers with identical offsets on every rank.
 
+With client-local entries (FedBN / FedPer, ``parallel/personal.py``) the slots are reordered so that those entries
+form one 1024-aligned range ``local_range`` that the collective skips; see :class:`ParamArena`.
+
 Conv weights keep their logical ``[Cout, Cin, KH, KW]`` shape with channels_last
 strides, i.e. they are physically ``[Cout, KH, KW, Cin]`` in the arena.
 """
@@ -22,12 +25,13 @@ from __future__ import annotations
 
 from collections import OrderedDict
 from dataclasses import dataclass
-from typing import Dict, Optional, Tuple
+from typing import Dict, Iterable, Optional, Tuple
 
 import torch
 from torch import nn
 
 ALIGN = 8  # elements: 16 B for bf16, 32 B for fp32 -> every view satisfies TMA / vector alignment
+LOCAL_ALIGN = 1024  # edges of the client-local range: no wire vector, fp8 block or collective granule crosses one
 
 
 @dataclass
@@ -46,36 +50,60 @@ def _round_up(x: int, m: int) -> int:
 
 class ParamArena:
     def __init__(self, model: nn.Module, device=None, *, momentum: bool = False, bf16_shadow: bool = True,
-                 keep_global: bool = True, theta_storage: Optional[torch.Tensor] = None, total_align: int = 2048):
+                 keep_global: bool = True, theta_storage: Optional[torch.Tensor] = None, total_align: int = 2048,
+                 local: Iterable[str] = ()):
+        """``local``: names of float ``state_dict`` entries that stay with each client (``parallel/personal.py``).  They
+        are laid out as one contiguous range ``local_range = (lo, hi)`` of whole 1024-element granules that straddles
+        ``n_param``: ``[shared params | pad][local params | local float buffers | pad][shared float buffers]``.
+        Without them the layout is parameters, then float buffers, and ``local_range`` is None."""
         self.model = model
         params = [(n, p) for n, p in model.named_parameters()]
         device = torch.device(device) if device is not None else (params[0][1].device if params else torch.device("cpu"))
         self.device = device
         self.slots: "OrderedDict[str, Slot]" = OrderedDict()
         self.int_slots: "OrderedDict[str, Tuple[int, int]]" = OrderedDict()
-        off = 0
+        local = frozenset(local)
         seen = set()
+        uniq = []
         for name, p in params:
-            if id(p) in seen:
-                continue
-            seen.add(id(p))
-            cl = p.dim() == 4
-            self.slots[name] = Slot(name, off, p.numel(), tuple(p.shape), cl, True)
-            off = _round_up(off + p.numel(), ALIGN)
-        self.n_param = _round_up(off, ALIGN)
-        off = self.n_param
+            if id(p) not in seen:
+                seen.add(id(p))
+                uniq.append((name, p))
+        bufs = []
         ioff = 0
         for name, b in model.named_buffers():
             if name.split(".")[-1] in getattr(self._owner(name), "_non_persistent_buffers_set", ()):
                 continue
             if b.is_floating_point():
-                self.slots[name] = Slot(name, off, b.numel(), tuple(b.shape), False, False)
-                off = _round_up(off + b.numel(), ALIGN)
+                bufs.append((name, b))
             else:
                 self.int_slots[name] = (ioff, b.numel())
                 ioff += b.numel()
+        unknown = sorted(local - {n for n, _ in uniq} - {n for n, _ in bufs})
+        if unknown:
+            raise ValueError("local entries must be float state_dict entries of their own, got {}".format(unknown))
+
+        def place(items, off, is_param):
+            for name, t in items:
+                self.slots[name] = Slot(name, off, t.numel(), tuple(t.shape), is_param and t.dim() == 4, is_param)
+                off = _round_up(off + t.numel(), ALIGN)
+            return off
+
+        off = place([x for x in uniq if x[0] not in local], 0, True)
+        self.local_range: Optional[Tuple[int, int]] = None
+        if local:
+            lo = off = _round_up(off, LOCAL_ALIGN)
+            off = place([x for x in uniq if x[0] in local], off, True)
+        self.n_param = _round_up(off, ALIGN)
+        off = self.n_param
+        if local:
+            off = _round_up(place([x for x in bufs if x[0] in local], off, False), LOCAL_ALIGN)
+            self.local_range = (lo, off)
+        off = place([x for x in bufs if x[0] not in local], off, False)
         self.n = _round_up(max(off, ALIGN), total_align)   # padded so tiles / vectors never straddle the end
         self.n_int = ioff
+        if local and self.n % LOCAL_ALIGN:
+            raise ValueError("local entries need total_align to be a multiple of {}".format(LOCAL_ALIGN))
 
         if theta_storage is not None:
             assert theta_storage.numel() >= self.n and theta_storage.dtype == torch.float32
@@ -94,6 +122,14 @@ class ParamArena:
         self.global_w = torch.zeros(self.n, dtype=torch.float32, device=device) if keep_global else None
         self.int_arena = torch.zeros(max(self.n_int, 1), dtype=torch.int64, device=device)
         self._adopt()
+
+    @property
+    def n_shared(self) -> int:
+        """Elements the collective carries: ``n`` minus the client-local range (a multiple of 1024 when there is one)."""
+        if self.local_range is None:
+            return self.n
+        lo, hi = self.local_range
+        return self.n - (hi - lo)
 
     # ------------------------------------------------------------------
     def _owner(self, qualified: str) -> nn.Module:

@@ -21,7 +21,7 @@ from __future__ import annotations
 
 import random
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -32,6 +32,7 @@ from .compress import TopKConfig, TopKState
 from .dp import DPConfig, RDPAccountant, check_dp, clip_factor
 from .features import check_features, round_plan
 from .fedavg import FedAvgSession, NcclSession
+from .personal import LocalStore, resolve_local_keys
 from .robust import RobustConfig, check_aggregator, check_krum_participants, check_participants
 from .server_opt import ServerOptConfig
 from .scaffold import ScaffoldState
@@ -74,7 +75,8 @@ class FederatedEngine:
                  eps: float = 1e-8, aggregator: str = "mean", trim_ratio: float = 0.1, krum_f: int = 0,
                  krum_m: Optional[int] = None, server_opt: Optional[str] = None, server_lr: Optional[float] = None,
                  server_betas: Tuple[float, float] = (0.9, 0.99), server_tau: float = 1e-3,
-                 compress: Optional[str] = None, topk_ratio: float = 0.01, error_feedback: bool = True):
+                 compress: Optional[str] = None, topk_ratio: float = 0.01, error_feedback: bool = True,
+                 local_keys: "Optional[str | Sequence[str]]" = None):
         """``prox_mu > 0``: FedProx local training -- every step adds ``prox_mu * (theta - global_w)`` to the gradient,
         ``global_w`` being the global model the round started from (for logical clients too: each starts from it).
 
@@ -121,7 +123,19 @@ class FederatedEngine:
         sample-weighted mean of the sparse uploads; the downlink stays dense.  It cannot be combined with the fp8 wire,
         DP, a robust aggregator, SCAFFOLD, ``mode='weights'`` or ``tile_flags``; FedProx, AdamW, momentum, logical
         clients and every server optimizer combine freely.  :meth:`last_upload_bytes` reports the upload.  ``None``
-        (the default) runs exactly the plain engine."""
+        (the default) runs exactly the plain engine.
+
+        ``local_keys`` (``parallel/personal.py``): personalized FL -- the named float ``state_dict`` entries stay with
+        each client and out of the collective: ``"bn"`` (FedBN: every BatchNorm's weight, bias and running statistics),
+        ``"head"`` (FedPer: the model's ``head`` entries), ``state_dict`` keys or ``fnmatch`` patterns, or a sequence
+        mixing them.  Every client (logical clients included) starts from the model's values at construction the first
+        time it trains and keeps what its last training left; FedProx's anchor for a local entry is the client's own
+        value.  The shared entries follow the plain round (with a server optimizer if one is set); integer buffers stay
+        shared.  :meth:`client_state_dict` and :meth:`local_entries` read a hosted client's model and entries,
+        :meth:`evaluate` scores each hosted client's personalized model, and :meth:`state_dict` returns the local
+        entries at their initial values.  It cannot be combined with DP, SCAFFOLD, a robust aggregator or Krum, top-k
+        uploads or ``tile_flags``; the optimizer-emitted upload is off.  Each hosted client that has taken part costs
+        ``4 (hi - lo)`` bytes.  ``None`` (the default) runs exactly the plain engine."""
         if compress not in (None, "topk"):
             raise ValueError("compress must be None or 'topk', got {!r}".format(compress))
         self.topk = TopKConfig(topk_ratio, error_feedback) if compress == "topk" else None
@@ -137,13 +151,15 @@ class FederatedEngine:
         trim_ratio = check_aggregator(aggregator, trim_ratio)
         self.robust = RobustConfig(aggregator, trim_ratio, krum_f, krum_m) if aggregator != "mean" else None
         self.dp = DPConfig(dp_clip, dp_noise_multiplier, dp_seed) if dp_clip > 0.0 else None
+        keys = resolve_local_keys(model, local_keys) if local_keys is not None else None
         check_features(wire_dtype=wire_dtype, mode=mode, dp=self.dp, scaffold=scaffold, robust=self.robust,
                        topk=self.topk, server_opt=sopt, tile_flags=tile_flags, optimizer=optimizer, momentum=momentum,
-                       prox_mu=prox_mu)
+                       prox_mu=prox_mu, local=keys is not None)
         self.device = torch.device(device)
         self.model = model
         self.name = name
-        self.arena = ParamArena(model, self.device, momentum=momentum > 0)
+        self.arena = ParamArena(model, self.device, momentum=momentum > 0, local=keys or ())
+        self.personal = LocalStore(self.arena, keys) if keys is not None else None
         if hasattr(model, "build_workspace"):
             model.build_workspace(self.device)
         if self.device.type == "cuda":
@@ -168,7 +184,8 @@ class FederatedEngine:
                     check_krum_participants(planned, self.robust.krum_f)
         self.session = Session(self.arena, group, wire_dtype=wire_dtype, mode=mode, n_ctas=n_ctas, nvls=nvls,
                                tile_flags=tile_flags, dp=self.dp, scaffold=scaffold, server_opt=sopt,
-                               robust=self.robust, topk=self.topk, max_clients=max_clients)
+                               robust=self.robust, topk=self.topk, max_clients=max_clients,
+                               local=self.personal is not None)
         self.dp = self.session.dp                  # rank 0's noise key
         self.accountant = RDPAccountant(self.dp.noise_multiplier) if self.dp is not None else None
         self.backend = backend
@@ -176,7 +193,7 @@ class FederatedEngine:
         # K4: the last SGD step of the captured epoch writes the upload copy itself (no pack phase in the collective);
         # only for the plain one-client-per-GPU rounds -- logical clients fold their deltas after training
         self.prepack = (backend == "fused" and self.device.type == "cuda" and self.topk is None
-                        and not (logical_clients and logical_clients > self.world))
+                        and self.personal is None and not (logical_clients and logical_clients > self.world))
         if self.prepack and hasattr(self.session, "pack_spec"):
             self.trainer.pack = self.session.pack_spec()
         # the round-end collective runs on the session's high-priority side stream: the NEXT round's host->device shard
@@ -272,8 +289,12 @@ class FederatedEngine:
                     self.sync()              # the previous round's collective must have landed before training reads theta
                 if self.prepack and self.trainer.pack is not None:
                     self.session.arm_prepack(float(X.shape[0]))
+                if self.personal is not None:    # the replica holds its client's local entries across rounds
+                    self.personal.refresh()
                 with phase("baton.local_train", self.phase_s):
                     losses_dev = self._train_client(self.rank, X, y, n_epoch, first=True)
+                if self.personal is not None:
+                    self.personal.swap_out(self.rank)
                 total_n = X.shape[0]
                 if self.topk is not None:
                     self.session.pack_topk(self._residual(self.rank))
@@ -294,7 +315,11 @@ class FederatedEngine:
                 X, y = shards(cid)
                 if not X.is_cuda:
                     X, y = self.stage(X, y, slot=j)
+                if self.personal is not None:
+                    self.personal.swap_in(cid)
                 ld = self._train_client(cid, X, y, n_epoch, first=(j == 0))
+                if self.personal is not None:   # before the fold: it resets the replica, local range included
+                    self.personal.swap_out(cid)
                 nk = X.shape[0]
                 losses_dev = ld * nk if losses_dev is None else losses_dev + ld * nk
                 total_n += nk
@@ -514,26 +539,42 @@ class FederatedEngine:
         ``client_id -> (X, y)`` (every client this rank hosts is evaluated and the results are summed); ``None`` or
         an empty shard contributes nothing.  Host shards are staged into their own buffers, never the training ones.
         Nothing of the model, the arena or the training state changes.  Every rank must call it: the global numbers
-        come from one all-reduce of ``[loss sum, #correct, n]`` over the session's process group."""
+        come from one all-reduce of ``[loss sum, #correct, n]`` over the session's process group.
+
+        With ``local_keys``, each hosted client's shard is scored by that client's personalized model
+        (:meth:`client_state_dict`; initial local values for a client that has not trained yet)."""
         self.sync()          # the round-end collective may still be writing the arena on its side stream
         batch = int(batch_size or self.hp["batch_size"])
         if self.logical_clients:
             ids = [c for c in range(self.logical_clients) if self.hosted(c)]
-            pairs = [shards(c) for c in ids] if shards is not None else []
-        elif shards is None:
+        else:
+            ids = [self.rank]
+        if shards is None:
             pairs = []
+        elif self.logical_clients:
+            pairs = [shards(c) for c in ids]
         else:
             pairs = [shards(self.rank) if callable(shards) else shards]
+        saved = self._swap_for_eval() if self.personal is not None else None
         loss = correct = n = 0.0
-        for pair in pairs:
-            if pair is None or pair[0].shape[0] == 0:
-                continue
-            X, y = pair
-            if self.device.type == "cuda" and not X.is_cuda:
-                # one staging buffer per shape: a pass ends with a host read, so the next shard may overwrite it
-                X, y = self._copy_in(self._eval_stage, X, y, 0)
-            ls, c, k = self.trainer.evaluate(X, y, batch_size=batch)
-            loss, correct, n = loss + ls, correct + c, n + k
+        try:
+            for cid, pair in zip(ids, pairs):
+                if pair is None or pair[0].shape[0] == 0:
+                    continue
+                X, y = pair
+                if self.device.type == "cuda" and not X.is_cuda:
+                    # one staging buffer per shape: a pass ends with a host read, so the next shard may overwrite it
+                    X, y = self._copy_in(self._eval_stage, X, y, 0)
+                if saved is not None:
+                    self._load_local(self.personal.values(cid))
+                ls, c, k = self.trainer.evaluate(X, y, batch_size=batch)
+                loss, correct, n = loss + ls, correct + c, n + k
+        finally:
+            if saved is not None:
+                a, (lo, hi) = self.arena, self.arena.local_range
+                a.theta[lo:hi].copy_(saved[0])
+                if saved[1] is not None:
+                    a.theta_bf16[lo:hi].copy_(saved[1])
         tot = [loss, correct, n]
         group = getattr(self.session, "group", None)
         if self.world > 1 and torch.distributed.is_available() and torch.distributed.is_initialized():
@@ -543,6 +584,45 @@ class FederatedEngine:
         return EvalResult(loss=_mean(tot[0], tot[2]), accuracy=_mean(tot[1], tot[2]), n_samples=int(tot[2]),
                           local_loss=_mean(loss, n), local_accuracy=_mean(correct, n), local_n_samples=int(n))
 
-    def state_dict(self):
+    def _swap_for_eval(self):
+        a, (lo, hi) = self.arena, self.arena.local_range
+        return a.theta[lo:hi].clone(), a.theta_bf16[lo:hi].clone() if a.theta_bf16 is not None else None
+
+    @torch.no_grad()
+    def _load_local(self, v: torch.Tensor) -> None:
+        """Put one client's local entries into the replica's theta and bf16 shadow (evaluation only)."""
+        a, (lo, hi) = self.arena, self.arena.local_range
+        a.theta[lo:hi].copy_(v)
+        if a.theta_bf16 is not None:
+            a.theta_bf16[lo:hi].copy_(v)
+
+    def _check_hosted(self, cid: int) -> None:
+        if self.personal is None:
+            raise RuntimeError("client-local entries are off (local_keys=None)")
+        if not (0 <= int(cid) < (self.logical_clients or self.world)) or not self.hosted(int(cid)):
+            raise RuntimeError("client {} is not hosted by rank {}".format(cid, self.rank))
+
+    def local_entries(self, cid: int) -> Dict[str, torch.Tensor]:
+        """``{key: tensor}`` copies of hosted client ``cid``'s local entries (the initial values until it has trained)."""
+        self._check_hosted(cid)
         self.sync()
-        return self.model.state_dict()
+        return self.personal.entries(cid)
+
+    def client_state_dict(self, cid: int):
+        """The personalized model of hosted client ``cid`` (copies): the shared entries of the current global model and
+        the client's local entries."""
+        self._check_hosted(cid)
+        self.sync()
+        sd = self.model.state_dict()
+        mine = self.personal.entries(cid)
+        return type(sd)((k, mine[k] if k in mine else v.clone()) for k, v in sd.items())
+
+    def state_dict(self):
+        """The global model (live views of the arena).  With ``local_keys`` its local entries are copies of their
+        initial values: what a client that has not trained yet starts from."""
+        self.sync()
+        sd = self.model.state_dict()
+        if self.personal is None:
+            return sd
+        init = self.personal.initial_entries()
+        return type(sd)((k, init[k] if k in init else v) for k, v in sd.items())

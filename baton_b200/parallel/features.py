@@ -20,11 +20,13 @@ SEATED_SERVER_OPT = ("a server optimizer needs the http plane: on the seated pla
 
 def check_features(*, wire_dtype: str = "bf16", mode: str = "delta", dp=None, scaffold: bool = False, robust=None,
                    topk=None, server_opt=None, tile_flags: bool = False, plane: Optional[str] = None,
-                   optimizer: str = "sgd", momentum: float = 0.0, nesterov: bool = False, prox_mu: float = 0.0) -> None:
+                   optimizer: str = "sgd", momentum: float = 0.0, nesterov: bool = False, prox_mu: float = 0.0,
+                   local: bool = False) -> None:
     """``ValueError`` with the reason if the features cannot run together.  ``dp``, ``robust``, ``topk`` and
     ``server_opt`` are on unless they are None or False: the rules read only which features are on, so a caller may pass
     the features' configurations or bools.  Whoever takes a configuration from outside checks its type.  ``plane``:
-    ``"http"`` or ``"seated"`` (the ``fused`` / ``nccl`` manager planes), None where no manager plane is involved."""
+    ``"http"`` or ``"seated"`` (the ``fused`` / ``nccl`` manager planes), None where no manager plane is involved.
+    ``local``: client-local ``state_dict`` entries (FedBN / FedPer, ``parallel/personal.py``)."""
     if optimizer not in OPTIMIZERS:
         raise ValueError("optimizer must be one of {}, got {!r}".format(OPTIMIZERS, optimizer))
     adamw = optimizer == "adamw"
@@ -52,6 +54,18 @@ def check_features(*, wire_dtype: str = "bf16", mode: str = "delta", dp=None, sc
         (robust and scaffold, "a robust aggregator with SCAFFOLD is not supported: its control-variate update is a "
                               "mean"),
         (robust and tile_flags, "a robust aggregator with tile_flags is not supported"),
+        (local and dp, "client-local entries with DP-FedAvg are not supported: the clip norm and the noise would have "
+                       "to cover the shared entries only"),
+        (local and scaffold, "client-local entries with SCAFFOLD are not supported: c and dc span the whole parameter "
+                             "range"),
+        (local and robust, "client-local entries with a robust aggregator or Krum are not supported: the client "
+                           "segments span the whole arena"),
+        (local and topk, "client-local entries with top-k uploads are not supported: the selection spans the whole "
+                         "arena"),
+        (local and tile_flags, "client-local entries with tile_flags are not supported: the flags index physical "
+                               "granules, and the first layer may be local"),
+        (local and plane is not None, "client-local entries need the SPMD engine: a manager plane's payload is a whole "
+                                      "state_dict, and its seats would need per-client stores"),
     )
     for broken, reason in rules:
         if broken:

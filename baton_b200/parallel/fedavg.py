@@ -87,6 +87,8 @@ def _init_session(arena: ParamArena, features: dict, dp: Optional[DPConfig], rob
     """Check a session's features (either kind of session), allocate the server optimizer's fresh state in the arena
     (``m = 0``, ``v = tau^2``) and return the client segments per rank."""
     _session_rules(features, dp, robust)
+    if features["local"] != (arena.local_range is not None):
+        raise ValueError("local=True needs an arena built with local entries, and such an arena needs local=True")
     if robust is not None:
         if not (1 <= int(max_clients) <= MAX_ROBUST_CLIENTS):
             raise ValueError("max_clients must be in 1..{}, got {!r}".format(MAX_ROBUST_CLIENTS, max_clients))
@@ -125,13 +127,16 @@ class FedAvgSession:
                  nvls: "bool | str" = "auto", n_ctas: Optional[int] = None, tile_elems: int = 0, timeout_log2: int = 24,
                  reset_momentum: bool = True, tile_flags: bool = False, dp: Optional[DPConfig] = None,
                  scaffold: bool = False, robust: Optional[RobustConfig] = None, max_clients: int = 1,
-                 server_opt: Optional[ServerOptConfig] = None, topk: Optional[TopKConfig] = None):
+                 server_opt: Optional[ServerOptConfig] = None, topk: Optional[TopKConfig] = None,
+                 local: bool = False):
         from ..ops._ext import load
         self._C = load()
         assert wire_dtype in ("bf16", "fp32", "fp8") and mode in ("delta", "weights")
         self._features = dict(wire_dtype=wire_dtype, mode=mode, scaffold=scaffold, topk=topk, server_opt=server_opt,
-                             tile_flags=tile_flags)
+                             tile_flags=tile_flags, local=bool(local))
         self.max_clients = _init_session(arena, self._features, dp, robust, max_clients)
+        self.local_range = arena.local_range
+        self.n_wire = arena.n_shared           # elements on the wire: the arena minus its client-local range
         self.topk, self.server_opt = topk, server_opt
         self._sopt_coef = list(server_opt.coefficients()) if server_opt is not None else []
         self.robust = robust
@@ -298,7 +303,7 @@ class FedAvgSession:
     def pack_spec(self) -> Optional[dict]:
         """Arguments for ``ops.fused_sgd(pack=...)`` (stable device tensors: safe to capture), or None when the wire
         format needs the in-kernel pack (block-scaled fp8)."""
-        if self.wire_kind == 2 or self.device.type != "cuda" or self.topk is not None:
+        if self.wire_kind == 2 or self.device.type != "cuda" or self.topk is not None or self.local_range is not None:
             return None
         a = self.arena
         return {"wire_slot": self.wire_slot, "global_w": a.global_w if self.delta else None, "scale": self.pack_scale,
@@ -499,7 +504,7 @@ class FedAvgSession:
         if self.tile_elems:
             tile = self.tile_elems
         else:   # one tile per (live rank, CTA): n / (A * G), rounded up to a multiple of 8 elements
-            per = -(-a.n // (len(alive) * self.n_ctas))
+            per = -(-self.n_wire // (len(alive) * self.n_ctas))
             tile = max(self.min_tile, (per + 31) // 32 * 32)
         if self.tile_flags is not None or self.topk is not None:
             # arrival flags and sparse rows cover fixed 1024-element granules: tiles must not split one
@@ -544,6 +549,9 @@ class FedAvgSession:
             elif robust is not None:
                 launch = self._C.fedavg_allreduce_robust
                 own = (self.symm.peer_ptrs(o_clip), m, self.seg_stride, robust.kind_id, robust.trim_table())
+            elif self.local_range is not None:
+                launch = self._C.fedavg_allreduce_local
+                own = (self.local_range[0], self.local_range[1] - self.local_range[0])
             else:
                 launch = self._C.fedavg_allreduce
                 dp_args = ([], 0.0, 0, 0)
@@ -678,7 +686,7 @@ class FedAvgSession:
         SCAFFOLD, the model segment, its padding and the control-variate segment."""
         if self.scaffold:
             return self.seg1_off + self._seg_bytes(self.arena.n_param)
-        return self._seg_bytes(self.arena.n)
+        return self._seg_bytes(self.n_wire)
 
 
 class NcclSession:
@@ -687,11 +695,13 @@ class NcclSession:
     def __init__(self, arena: ParamArena, group=None, *, wire_dtype: str = "bf16", mode: str = "delta",
                  reset_momentum: bool = True, dp: Optional[DPConfig] = None, scaffold: bool = False,
                  robust: Optional[RobustConfig] = None, max_clients: int = 1, tile_flags: bool = False,
-                 server_opt: Optional[ServerOptConfig] = None, topk: Optional[TopKConfig] = None, **_unused):
+                 server_opt: Optional[ServerOptConfig] = None, topk: Optional[TopKConfig] = None,
+                 local: bool = False, **_unused):
         import torch.distributed as dist
         self._features = dict(wire_dtype=wire_dtype, mode=mode, scaffold=scaffold, topk=topk, server_opt=server_opt,
-                             tile_flags=tile_flags)
+                             tile_flags=tile_flags, local=bool(local))
         self.max_clients = _init_session(arena, self._features, dp, robust, max_clients)
+        self.local_range = arena.local_range
         self.topk, self.server_opt = topk, server_opt
         # top-k: k, this rank's upload of the round as a dense fp32 vector (zeros off its support) and its entry count
         self.topk_k = self.topk.k(n_float(arena)) if self.topk is not None else 0
@@ -712,7 +722,7 @@ class NcclSession:
         inited = dist.is_available() and dist.is_initialized()
         self.world = dist.get_world_size(group) if inited else 1
         self.rank = dist.get_rank(group) if inited else 0
-        self.wire = torch.zeros(arena.n, dtype=self.wire_dtype, device=self.device)
+        self.wire = torch.zeros(arena.n_shared, dtype=self.wire_dtype, device=self.device)
         # robust: this rank's client segments (wire format) and how many of them pack_client filled this round
         self.segs = (torch.zeros(self.max_clients, arena.n, dtype=self.wire_dtype, device=self.device)
                      if robust is not None else None)
@@ -853,7 +863,9 @@ class NcclSession:
             counts = self.counts
         total = counts.sum()
         w = counts[self.rank] / total
-        src = (a.theta - a.global_w) if self.delta else a.theta
+        # client-local entries: the round runs on the shared elements only, cat(x[:lo], x[hi:]), and writes them back
+        theta, global_w = self._shared(a.theta), self._shared(a.global_w)
+        src = (theta - global_w) if self.delta else theta
         if self.topk is not None:
             mine = float(counts[self.rank]) != 0.0
             if mine and self._topk_up is None:
@@ -899,19 +911,22 @@ class NcclSession:
         elif self.delta:
             d = self.wire.float()
         if d is None:
-            a.global_w.copy_(self.wire.float())
+            global_w.copy_(self.wire.float())
         elif self.server_opt is not None:
             if float(total) > 0.0:      # a round without weight leaves the model and the state unchanged
-                apply_update_(a.global_w, d, a.n_param, a.server_m, a.server_v, self.server_opt)
+                n_p = a.n_param if self.local_range is None else self.local_range[0]   # the shared parameters
+                apply_update_(global_w, d, n_p, a.server_m[:n_p], a.server_v[:n_p] if a.server_v is not None else None,
+                              self.server_opt)
         else:
-            a.global_w.add_(d)
-        a.theta.copy_(a.global_w)
+            global_w.add_(d)
+        self._put(a.global_w, global_w)
+        self._put(a.theta, global_w)
         if a.theta_bf16 is not None:
-            a.theta_bf16.copy_(a.theta.to(torch.bfloat16))
+            self._put(a.theta_bf16, global_w.to(torch.bfloat16))
         if a.n_int > 0 and self.world > 1:
             dist.all_reduce(a.int_arena, op=dist.ReduceOp.MAX, group=self.group)
         if self.reset_momentum and a.momentum is not None:
-            a.momentum.zero_()
+            a.momentum[: self.local_range[0] if self.local_range is not None else a.momentum.numel()].zero_()
         if control is not None:
             c, dc, n_clients = control
             n_p = a.n_param
@@ -920,6 +935,22 @@ class NcclSession:
                 dist.all_reduce(tot, group=self.group)
             c[:n_p].add_(tot / float(n_clients))
         self.rounds += 1
+
+    def _shared(self, x: torch.Tensor) -> torch.Tensor:
+        """The elements the collective carries, as a new tensor: ``x`` without the client-local range."""
+        if self.local_range is None:
+            return x.clone()
+        lo, hi = self.local_range
+        return torch.cat((x[:lo], x[hi:]))
+
+    def _put(self, dst: torch.Tensor, shared: torch.Tensor) -> None:
+        """Write the shared elements back into ``dst`` around the client-local range."""
+        if self.local_range is None:
+            dst.copy_(shared)
+            return
+        lo, hi = self.local_range
+        dst[:lo].copy_(shared[:lo])
+        dst[hi:].copy_(shared[lo:])
 
     def dp_round(self) -> int:
         return self.rounds & 0xFFFFFFFF
@@ -946,5 +977,5 @@ class NcclSession:
         pass
 
     def wire_bytes(self) -> int:
-        n = self.arena.n + (self.arena.n_param if self.scaffold else 0)
+        n = self.arena.n_shared + (self.arena.n_param if self.scaffold else 0)
         return n * (2 if self.wire_dtype == torch.bfloat16 else 4)
