@@ -34,8 +34,7 @@ from .base import FederatedModule
 def _conv_bn_fwd(conv: "bnn.Conv2d", bn: "bnn.BatchNorm2d", x, residual=None, after_conv=None):
     cc, cb = bnn.Ctx(), bnn.Ctx()
     stats = conv._fusable_stats(x)
-    z = bnn._ConvFn.forward(cc, x, conv.weight, conv._w_bf16(), conv.kernel_size, conv.kernel_size, conv.stride,
-                            conv.padding, None, stats, conv.flags_cfg)
+    z = bnn._ConvFn.forward(cc, x, conv.weight, conv._w_bf16(), conv.plan(x), None, stats, conv.flags_cfg)
     if after_conv is not None:
         after_conv()
     y = bnn._BNFn.forward(cb, z, residual, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.num_batches_tracked,
@@ -65,8 +64,7 @@ def _stem_fwd(conv, bn, pool, x, after_conv=None):
             or bnn._grad_target(bn.weight) is None or bnn._grad_target(bn.bias) is None):
         return None
     cc = bnn.Ctx()
-    z = bnn._ConvFn.forward(cc, x, conv.weight, conv._w_bf16(), conv.kernel_size, conv.kernel_size, conv.stride,
-                            conv.padding, None, stats, conv.flags_cfg)
+    z = bnn._ConvFn.forward(cc, x, conv.weight, conv._w_bf16(), conv.plan(x), None, stats, conv.flags_cfg)
     if after_conv is not None:
         after_conv()
     c = bn.num_features
@@ -96,27 +94,14 @@ def _stem_bwd(saved, bn, pool, dy_a, dy_b=None):
 # BatchNorm's ``eval_off`` -- plus the block's shortcut and the ReLU.  Where a GEMM declines the epilogue, the plain
 # GEMM and ``bn_apply(training=0)`` run instead.  The bf16 weights come from ``ResNet.prepare_eval`` (once per pass).
 def _conv_bn_eval(conv, bn, x, table, residual=None):
-    F = bnn.F
-    n, h, w, c = x.shape
-    k, s, p = conv.kernel_size, conv.stride, conv.padding
-    cout = conv.out_channels
-    ho, wo = F.conv_out_size(h, k, s, p), F.conv_out_size(w, k, s, p)
-    wt = conv.eval_weight
-    af = F.affine_epilogue_args(table, bn.eval_off, cout, bn.relu, residual)
-    centre = h == 1 and w == 1 and k % 2 == 1 and p == k // 2 and c % 8 == 0 and k > 1
-    if centre:                  # a k x k "same" convolution of a 1x1 map sees only its centre tap (see _ConvFn)
-        y = F.gemm(x.view(n, c), wt.view(cout, k * k, c)[:, (k // 2) * k + k // 2, :], affine=af)
-    elif k == 1 and s == 1 and p == 0 and c % 8 == 0:
-        y = F.gemm(x.view(n * h * w, c), wt, affine=af)
-    elif c % 64 == 0:
-        y = F.conv_igemm_fwd(x, wt, k, k, s, p, affine=af)
-    else:
-        y = F.gemm(F.im2col(x, k, k, s, p)[0], wt, affine=af)
+    plan, wt = conv.plan(x), conv.eval_weight
+    af = bnn.F.affine_epilogue_args(table, bn.eval_off, plan.cout, bn.relu, residual)
+    y = bnn.F.conv_fwd(x, wt, plan, affine=af)[0]
     if y is None:
-        z = bnn._ConvFn.forward(bnn.Ctx(), x, conv.weight, wt, k, k, s, p, None)
+        z = bnn._ConvFn.forward(bnn.Ctx(), x, conv.weight, wt, plan, None)
         y = bnn._BNFn.forward(bnn.Ctx(), z, residual, bn.weight, bn.bias, bn.running_mean, bn.running_var, None, bn.eps,
                               bn.momentum, bn.relu, False, None, None)
-    return y.view(n, ho, wo, cout)
+    return y.view(plan.n, plan.ho, plan.wo, plan.cout)
 
 
 class BasicBlock(nn.Module):

@@ -11,6 +11,8 @@ Conventions
 """
 from __future__ import annotations
 
+import collections
+import functools
 from typing import List, Optional, Sequence, Tuple
 
 import torch
@@ -424,14 +426,75 @@ def round_up(x: int, m: int) -> int:
     return (x + m - 1) // m * m
 
 
+def im2col_k(kh: int, kw: int, c: int) -> int:
+    """K of an explicit im2col GEMM: the ``kh*kw*C`` taps zero-padded to a multiple of 8 (16-byte TMA rows)."""
+    return round_up(kh * kw * c, 8)
+
+
 def im2col(x: torch.Tensor, kh: int, kw: int, stride: int, pad: int) -> Tuple[torch.Tensor, int, int, int]:
-    """NHWC ``x`` -> ``col[N*Ho*Wo, Kp]`` with ``Kp = round_up(kh*kw*C, 8)``."""
+    """NHWC ``x`` -> ``col[N*Ho*Wo, Kp]`` with ``Kp = im2col_k(kh, kw, C)``."""
     n, h, w, c = x.shape
     ho, wo = conv_out_size(h, kh, stride, pad), conv_out_size(w, kw, stride, pad)
-    kp = round_up(kh * kw * c, 8)
+    kp = im2col_k(kh, kw, c)
     col = torch.empty((n * ho * wo, kp), dtype=BF16, device=x.device)
     load().im2col(x, col, n, h, w, c, kh, kw, stride, pad, ho, wo, kp)
     return col, ho, wo, kp
+
+
+class ConvPlan(collections.namedtuple("ConvPlan", "n h w c cout kh kw stride pad form ho wo M K tap dgrad")):
+    """:func:`conv_plan` of one convolution: its geometry, the ``form`` of its forward GEMM, the output size, that
+    GEMM's ``M`` and ``K``, the ``tap`` index (``"centre"`` only, else ``None``) and the input gradient's ``dgrad``."""
+    __slots__ = ()
+
+    def weight(self, w2d: torch.Tensor) -> torch.Tensor:
+        """B operand of the forward and dgrad GEMMs: ``w2d [Cout, kh*kw*Cin]`` itself, or its centre-tap slice."""
+        return w2d.view(self.cout, self.kh * self.kw, self.c)[:, self.tap, :] if self.form == "centre" else w2d
+
+
+@functools.lru_cache(maxsize=None)      # pure: every call with one shape shares one plan
+def conv_plan(n: int, h: int, w: int, c: int, cout: int, kh: int, kw: int, stride: int, pad: int) -> ConvPlan:
+    """GEMM lowering of a convolution of NHWC ``[n, h, w, c]`` into ``cout`` channels, for training, its backward,
+    the fused BatchNorm statistics and evaluation alike.  ``form``:
+    * ``"centre"``: a k x k convolution (odd k > 1, "same" padding) over a 1x1 map only ever sees its centre tap --
+      every other tap multiplies zero padding.  Exact, and it turns the deepest ResNet stage (32x32 inputs: layer4 is
+      1x1) into plain ``[N, Cin] x [Cout, Cin]`` GEMMs on a strided weight view: no im2col / col2im, 9x less K.
+    * ``"pointwise"``: 1x1, stride 1, pad 0: a plain GEMM on ``x.view(-1, C)``.
+    * ``"implicit"`` (``C % 64 == 0``): A gathered from ``x`` inside the GEMM (:func:`conv_igemm_fwd`, which may
+      decline at run time: then ``"im2col"`` runs), no col buffer; the wgrad gathers ``im2col(x)`` on the fly.
+    * ``"im2col"``: explicit im2col / col2im + GEMM for the rest (the C = 3 stem, ``Cin % 64 != 0``).
+    ``dgrad``: ``"implicit"`` (:func:`conv_igemm_dgrad`, which may decline: then ``"col2im"``) for implicit
+    convolutions of stride 2 or of stride 1 and square k > 1; else the dgrad GEMM then ``"view"`` or ``"col2im"``."""
+    ho, wo = conv_out_size(h, kh, stride, pad), conv_out_size(w, kw, stride, pad)
+    tap = None
+    if h == 1 and w == 1 and kh == kw and kh % 2 == 1 and kh > 1 and pad == kh // 2 and c % 8 == 0:
+        form, K, tap = "centre", c, (kh // 2) * kw + kw // 2
+    elif kh == 1 and kw == 1 and stride == 1 and pad == 0 and c % 8 == 0:
+        form, K = "pointwise", c
+    elif c % 64 == 0:
+        form, K = "implicit", kh * kw * c
+    else:
+        form, K = "im2col", im2col_k(kh, kw, c)
+    dgrad = "view" if form in ("centre", "pointwise") else "col2im"
+    if form == "implicit" and (stride == 2 or (stride == 1 and kh == kw and kh > 1)):
+        dgrad = "implicit"
+    return ConvPlan(n, h, w, c, cout, kh, kw, stride, pad, form, ho, wo, n * ho * wo, K, tap, dgrad)
+
+
+def conv_fwd(x: torch.Tensor, w2d: torch.Tensor, plan: ConvPlan, form: Optional[str] = None,
+             col_stats: Optional[torch.Tensor] = None, gate: Optional[dict] = None,
+             affine: Optional[dict] = None) -> Tuple[Optional[torch.Tensor], torch.Tensor]:
+    """``plan``'s forward GEMM (or ``form``'s) on NHWC ``x`` and channels_last ``w2d``: ``(y [M, Cout] or None when it
+    declines, the A operand the wgrad reads)``.  ``col_stats`` / ``affine``: as in :func:`gemm`; ``gate`` (bcast_gemm,
+    pointwise and im2col forms): the TMA producer acquires the FedAvg arrival flags over ``w2d``."""
+    form = form or plan.form
+    if form == "implicit":
+        return conv_igemm_fwd(x, w2d, plan.kh, plan.kw, plan.stride, plan.pad, col_stats=col_stats, affine=affine), x
+    a = im2col(x, plan.kh, plan.kw, plan.stride, plan.pad)[0] if form == "im2col" else x.view(plan.M, plan.c)
+    gk = {}
+    if gate is not None and form != "centre":
+        gk = dict(flags=gate["flags"], flag_epoch_word=gate["epoch_word"], flag_elem_off=gate["elem_off"],
+                  flag_tile_elems=gate["tile_elems"], force_bn=pick_bn(a.shape[0], w2d.shape[0]))
+    return gemm(a, plan.weight(w2d), col_stats=col_stats, affine=affine, **gk), a
 
 
 HALO_BM = 64                      # output pixels of one halo-kernel tile (conv_halo.cu)

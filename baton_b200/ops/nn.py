@@ -345,119 +345,68 @@ class Linear(nn.Module):
 
 
 # ================================================================================ Conv2d (NHWC, implicit GEMM)
-# implicit-GEMM convolution (TMA im2col operands) wherever the shape allows it; explicit im2col / col2im + GEMM for
-# the shapes it declines (the C = 3 stem, Cin % 64 != 0, strides other than 1 and 2, stride-2 filters whose parity
-# classes need negative dy offsets or more than four taps, a kernel that reports "unsupported")
 class _ConvFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, weight, w_bf16, kh, kw, stride, pad, anchor, stats=None, gate=None):
-        """``gate``: bcast_gemm arrival-flag configuration of this layer's weights (first conv of the model only)."""
-        weight = _unwrap(weight)
-        n, h, w, c = x.shape
-        cout = w_bf16.shape[0]
-        # a k x k convolution (odd k, "same" padding) over a 1x1 feature map only ever sees its centre
-        # tap -- every other tap multiplies zero padding.  Exact, and it turns the deepest ResNet stage
-        # (32x32 inputs: layer4 is 1x1) into plain [N, Cin] x [Cout, Cin] GEMMs on a strided weight view:
-        # no im2col / col2im, 9x less K.
-        ctx.center = (h == 1 and w == 1 and kh == kw and kh % 2 == 1 and pad == kh // 2 and c % 8 == 0 and kh > 1)
-        if ctx.center:
-            col, ho, wo, kp = x.view(n, c), 1, 1, c
-            wc = w_bf16.view(cout, kh * kw, c)[:, (kh // 2) * kw + kw // 2, :]
-            y = F.gemm(col, wc, col_stats=stats)
-        else:
-            y = None
-            ctx.igemm = False
-            if kh == 1 and kw == 1 and stride == 1 and pad == 0 and c % 8 == 0:
-                col, ho, wo, kp = x.view(n * h * w, c), h, w, c
-            elif c % 64 == 0:
-                # A operand gathered by TMA im2col inside the GEMM, no col buffer (backward: implicit
-                # wgrad from x itself)
-                ho, wo, kp = F.conv_out_size(h, kh, stride, pad), F.conv_out_size(w, kw, stride, pad), kh * kw * c
-                y = F.conv_igemm_fwd(x, w_bf16, kh, kw, stride, pad, col_stats=stats)
-                col, ctx.igemm = x, y is not None
-            if y is None:
-                if not (kh == 1 and kw == 1 and stride == 1 and pad == 0 and c % 8 == 0):
-                    col, ho, wo, kp = F.im2col(x, kh, kw, stride, pad)
-                gk = {}
-                if gate is not None:     # the TMA producer acquires the arrival flags over this layer's weights
-                    gk = dict(flags=gate["flags"], flag_epoch_word=gate["epoch_word"], flag_elem_off=gate["elem_off"],
-                              flag_tile_elems=gate["tile_elems"], force_bn=F.pick_bn(col.shape[0], w_bf16.shape[0]))
-                y = F.gemm(col, w_bf16, col_stats=stats, **gk)
+    def forward(ctx, x, weight, w_bf16, plan, anchor, stats=None, gate=None):
+        """``plan``: GEMM lowering of this call (``F.conv_plan``).  ``gate``: bcast_gemm arrival-flag configuration of
+        this layer's weights (first conv of the model only)."""
+        y, col = F.conv_fwd(x, w_bf16, plan, col_stats=stats, gate=gate)
+        ctx.igemm = plan.form == "implicit" and y is not None      # col IS x: the wgrad gathers im2col(x) on the fly
+        if plan.form == "implicit" and y is None:                  # the kernel declined this shape: explicit im2col
+            y, col = F.conv_fwd(x, w_bf16, plan, form="im2col", col_stats=stats, gate=gate)
         ctx.save_for_backward(col, w_bf16)
-        ctx.weight = weight
-        ctx.geom = (n, h, w, c, kh, kw, stride, pad, ho, wo, kp)
+        ctx.weight, ctx.plan = _unwrap(weight), plan
         ctx.needs_dx = x.requires_grad
-        return y.view(n, ho, wo, cout)
+        return y.view(plan.n, plan.ho, plan.wo, plan.cout)
 
     @staticmethod
     def backward(ctx, dy):
         col, w_bf16 = ctx.saved_tensors
-        n, h, w, c, kh, kw, stride, pad, ho, wo, kp = ctx.geom
-        cout = w_bf16.shape[0]
-        dy2 = dy.reshape(n * ho * wo, cout)
+        p = ctx.plan
+        dy2 = dy.reshape(p.M, p.cout)
         if not dy2.is_contiguous():
             dy2 = dy2.contiguous()
-        weight = ctx.weight
-        k_true = kh * kw * c
-        gw = None
-        tgt = _grad_target(weight)
-        if ctx.center:
-            tap = (kh // 2) * kw + kw // 2
-            if tgt is None:
-                gw = torch.zeros((cout, kh, kw, c), dtype=torch.float32, device=dy.device)
-                g2d = gw.view(cout, kh * kw, c)[:, tap, :]
-                gw = gw.permute(0, 3, 1, 2)
-            else:
-                full = tgt.permute(0, 2, 3, 1).reshape(cout, kh * kw, c)
-                assert full.data_ptr() == tgt.data_ptr(), "conv weight grad must be channels_last in the arena"
-                g2d = full[:, tap, :]
-            if tgt is None:
-                F.gemm(dy2, col, a_mn=True, b_mn=True, out=g2d, accumulate=True)
-            tok = WGRAD.mark(dy2)
-            dx = None
-            if ctx.needs_dx:
-                wc = w_bf16.view(cout, kh * kw, c)[:, tap, :]
-                dx = F.gemm(dy2, wc, b_mn=True).view(n, 1, 1, c)
-            if tgt is not None:
-                # an optimizer epilogue rewrites the bf16 weights the dgrad above reads: it must start after it
-                WGRAD.run(lambda: _wgrad(lambda sgd: F.gemm(dy2, col, a_mn=True, b_mn=True, out=g2d, accumulate=True,
-                                                            sgd=sgd) is not None, g2d, nograd_of=tgt),
-                          dy2, col, after=None if SGD_EPI.active else tok)
-            return dx, gw, None, None, None, None, None, None, None, None
-        igemm = getattr(ctx, "igemm", False)          # col IS x: the weight gradient gathers im2col(x) on the fly
+        k_true = p.kh * p.kw * p.c
+        g2 = None
+        tgt = _grad_target(ctx.weight)
+        if p.form == "centre" and tgt is None:
+            # only the centre tap receives a gradient; the other taps of the full weight gradient stay zero
+            g2 = torch.zeros((p.cout, k_true), dtype=torch.float32, device=dy.device)
+            F.gemm(dy2, col, a_mn=True, b_mn=True, out=p.weight(g2), accumulate=True)
         tok = WGRAD.mark(dy2)      # the weight-gradient branch depends on what is enqueued so far, not on the dgrad below
         dx = None
         if ctx.needs_dx:
-            if kp == k_true and w_bf16.shape[1] == k_true and (stride == 2 or (stride == 1 and kh == kw and kh > 1)):
-                # implicit dgrad, no dcol buffer / col2im: stride 1 = flipped-filter convolution of dy, stride 2 = its
-                # four parity classes of dx pixels in one launch
-                dx = F.conv_igemm_dgrad(dy2.view(n, ho, wo, cout), w_bf16, (n, h, w, c), kh, kw, pad, stride=stride)
+            if p.dgrad == "implicit":
+                dx = F.conv_igemm_dgrad(dy2.view(p.n, p.ho, p.wo, p.cout), w_bf16, (p.n, p.h, p.w, p.c), p.kh, p.kw,
+                                        p.pad, stride=p.stride)
             if dx is None:
-                dcol = F.gemm(dy2, w_bf16, b_mn=True)  # [M, kp]
-                if kh == 1 and kw == 1 and stride == 1 and pad == 0 and c % 8 == 0:
-                    dx = dcol.view(n, h, w, c)
-                else:
-                    dx = F.col2im(dcol, (n, h, w, c), kh, kw, stride, pad, ho, wo)
+                dcol = F.gemm(dy2, p.weight(w_bf16), b_mn=True)  # [M, K]
+                dx = dcol.view(p.n, p.h, p.w, p.c) if p.dgrad == "view" else \
+                    F.col2im(dcol, (p.n, p.h, p.w, p.c), p.kh, p.kw, p.stride, p.pad, p.ho, p.wo)
         if tgt is not None:
             # the arena view is channels_last: physical [Cout, KH, KW, Cin] == [Cout, K]
-            out2d = tgt.permute(0, 2, 3, 1).reshape(cout, k_true) if tgt.dim() == 4 else tgt.view(cout, k_true)
+            out2d = tgt.permute(0, 2, 3, 1).reshape(p.cout, k_true) if tgt.dim() == 4 else tgt.view(p.cout, k_true)
             assert out2d.data_ptr() == tgt.data_ptr(), "conv weight grad must be channels_last in the arena"
-            if igemm:
-                # an optimizer epilogue rewrites the bf16 weights the dgrad above reads: it must start after it
-                WGRAD.run(lambda: _wgrad(lambda sgd: F.conv_igemm_wgrad_(dy2, col, out2d, kh, kw, stride, pad, sgd=sgd),
-                                         out2d),
+            # an optimizer epilogue rewrites the bf16 weights the dgrad above reads: it must start after it
+            if p.form == "centre":
+                g2d = p.weight(out2d)
+                WGRAD.run(lambda: _wgrad(lambda sgd: F.gemm(dy2, col, a_mn=True, b_mn=True, out=g2d, accumulate=True,
+                                                            sgd=sgd) is not None, g2d, nograd_of=tgt),
+                          dy2, col, after=None if SGD_EPI.active else tok)
+            elif ctx.igemm:
+                WGRAD.run(lambda: _wgrad(lambda sgd: F.conv_igemm_wgrad_(dy2, col, out2d, p.kh, p.kw, p.stride, p.pad,
+                                                                         sgd=sgd), out2d),
                           dy2, col, after=None if SGD_EPI.active else tok)
             else:
                 WGRAD.run(lambda: F.gemm(dy2, col, a_mn=True, b_mn=True, out=out2d, accumulate=True, n_valid=k_true),
                           dy2, col, after=tok)
-        elif igemm:
-            g2 = torch.zeros((cout, k_true), dtype=torch.float32, device=dy.device)
-            F.conv_igemm_wgrad_(dy2, col, g2, kh, kw, stride, pad)
-            gw = g2.view(cout, kh, kw, c).permute(0, 3, 1, 2)
-        else:
+        elif ctx.igemm:
+            g2 = torch.zeros((p.cout, k_true), dtype=torch.float32, device=dy.device)
+            F.conv_igemm_wgrad_(dy2, col, g2, p.kh, p.kw, p.stride, p.pad)
+        elif p.form != "centre":
             g2 = F.gemm(dy2, col, a_mn=True, b_mn=True, out_dtype=torch.float32, accumulate=True, n_valid=k_true)
-            gw = g2.view(cout, kh, kw, c).permute(0, 3, 1, 2)
-        return dx, gw, None, None, None, None, None, None, None, None
+        gw = None if g2 is None else g2.view(p.cout, p.kh, p.kw, p.c).permute(0, 3, 1, 2)
+        return dx, gw, None, None, None, None, None
 
 
 class Conv2d(nn.Module):
@@ -471,7 +420,7 @@ class Conv2d(nn.Module):
         nn.init.kaiming_normal_(w, mode="fan_out", nonlinearity="relu")
         self.weight = nn.Parameter(w.contiguous(memory_format=torch.channels_last))
         self.k_true = kernel_size * kernel_size * in_channels
-        self.kp = F.round_up(self.k_true, 8)
+        self.kp = F.im2col_k(kernel_size, kernel_size, in_channels)
         self.flags_cfg = None   # bcast_gemm: set by FedAvgSession.gate_first_conv for the first conv of the model
 
     def _w_bf16(self, gated: bool = True):
@@ -492,11 +441,16 @@ class Conv2d(nn.Module):
         if getattr(self, "fp8", False):
             return conv2d_fp8(x, self)
         stats = self._fusable_stats(x)
-        y = _ConvFn.apply(x, _wrap(self.weight, x), self._w_bf16(), self.kernel_size, self.kernel_size,
-                          self.stride, self.padding, _anchor(x, self.weight), stats, self.flags_cfg)
+        y = _ConvFn.apply(x, _wrap(self.weight, x), self._w_bf16(), self.plan(x), _anchor(x, self.weight), stats,
+                          self.flags_cfg)
         if stats is not None:
             y._bn_stats_ws = stats      # tells the BatchNorm that owns this workspace to skip its statistics pass
         return y
+
+    def plan(self, x) -> F.ConvPlan:
+        n, h, w, c = x.shape
+        return F.conv_plan(n, h, w, c, self.out_channels, self.kernel_size, self.kernel_size, self.stride,
+                           self.padding)
 
     def _fusable_stats(self, x):
         """The following BatchNorm's statistics workspace (``bn_ws``, linked by the model) if this call's GEMM
@@ -504,13 +458,8 @@ class Conv2d(nn.Module):
         ws = getattr(self, "bn_ws", None)
         if ws is None or not self.training or not torch.is_grad_enabled():
             return None
-        n, h, w, c = x.shape
-        k, s_, p_ = self.kernel_size, self.stride, self.padding
-        ho, wo = (h + 2 * p_ - k) // s_ + 1, (w + 2 * p_ - k) // s_ + 1
-        centre = h == 1 and w == 1 and k % 2 == 1 and p_ == k // 2 and c % 8 == 0 and k > 1
-        kdim = c if (centre or (k == 1 and c % 8 == 0)) else F.round_up(k * k * c, 8)
-        cout = self.weight.shape[0]
-        return ws[: 2 * cout] if F.gemm_stats_fusable(n * ho * wo, cout, kdim) else None
+        p = self.plan(x)
+        return ws[: 2 * p.cout] if F.gemm_stats_fusable(p.M, p.cout, p.K) else None
 
 
 # ================================================================================ BatchNorm (+residual +ReLU)
