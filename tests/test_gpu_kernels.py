@@ -51,7 +51,7 @@ def test_gemm_tcgen05_all_majors(F, a_mn, b_mn, M, N, K):
     assert out16.dtype == BF16 and _rel(out16, ref) < 1e-2
 
 
-@pytest.mark.parametrize("bn", [64, 128, 256])
+@pytest.mark.parametrize("bn", [64, 128])     # the host clamps a requested 256 to 128: no 256-wide kernel exists
 def test_gemm_tile_widths_bias_act(F, bn):
     torch.manual_seed(bn)
     dev = _dev()
