@@ -264,51 +264,29 @@ bool conv_igemm_dgrad(const at::Tensor& dy, const at::Tensor& w, at::Tensor dx, 
   check(rc, "conv_igemm_dgrad");
   return true;
 }
-// halo-tiled 3x3 stride-1 convolution: src [N, H, W, 64] (x forward, dy dgrad), w [Cout, 9*Cin], out [N*H*W, Nout]
+// halo-tiled 3x3 pad-1 convolution: src [N, H, W, C] (x forward, dy dgrad), w [Cout, 9*Cin], out [N*Ho*Wo, Nout]
 // (Nout = Cout forward, Cin dgrad); false = shape not supported by the kernel
-bool conv_halo(const at::Tensor& src, const at::Tensor& w, at::Tensor out, bool dgrad, int64_t mc,
+bool conv_halo(const at::Tensor& src, const at::Tensor& w, at::Tensor out, int64_t stride, bool dgrad, int64_t mc,
                const std::optional<at::Tensor>& col_stats) {
   CHECK_CUDA(src); CHECK_CUDA(w); CHECK_CUDA(out);
   TORCH_CHECK(src.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16 && out.scalar_type() == at::kBFloat16 &&
-              src.dim() == 4 && src.size(3) == 64 && src.is_contiguous() && w.is_contiguous() && out.is_contiguous());
-  const int64_t rows = src.size(0) * src.size(1) * src.size(2);
-  TORCH_CHECK(rows > 0 && out.numel() % rows == 0, "conv_halo: out must hold [N*H*W, Nout] elements");
+              src.dim() == 4 && src.is_contiguous() && w.is_contiguous() && out.is_contiguous());
+  TORCH_CHECK(stride == 1 || stride == 2, "conv_halo: stride 1 or 2");
+  const int64_t c = src.size(3);
+  const int64_t rows = src.size(0) * ((src.size(1) - 1) / stride + 1) * ((src.size(2) - 1) / stride + 1);
+  TORCH_CHECK(rows > 0 && out.numel() % rows == 0, "conv_halo: out must hold [N*Ho*Wo, Nout] elements");
   const int64_t nout = out.numel() / rows;
-  TORCH_CHECK(w.numel() == (dgrad ? 64 * 9 * nout : nout * 9 * 64), "conv_halo: w must be [Cout, 9*Cin]");
+  TORCH_CHECK(w.numel() == (dgrad ? c * 9 * nout : nout * 9 * c), "conv_halo: w must be [Cout, 9*Cin]");
   TORCH_CHECK(dgrad ? !col_stats.has_value()
                     : (!col_stats.has_value() || (col_stats->scalar_type() == at::kFloat && col_stats->numel() >= 2 * nout)),
               "conv_halo: col_stats is a [2 Cout] fp32 buffer of the forward");
   const c10::cuda::CUDAGuard guard(src.device());
   const int rc = b200_conv_halo(cptr(src), cptr(w), ptr(out), static_cast<int>(src.size(0)), static_cast<int>(src.size(1)),
-                                static_cast<int>(src.size(2)), static_cast<int>(nout), dgrad ? 1 : 0,
-                                static_cast<int>(mc), opt_ptr<float>(col_stats), cur_stream());
+                                static_cast<int>(src.size(2)), static_cast<int>(c), static_cast<int>(nout),
+                                static_cast<int>(stride), dgrad ? 1 : 0, static_cast<int>(mc), opt_ptr<float>(col_stats),
+                                cur_stream());
   if (rc == -2) return false;
   check(rc, "conv_halo");
-  return true;
-}
-// wide-channel halo-tiled 3x3 pad-1 convolution: src [N, H, W, C] (x forward, dy dgrad), w [Cout, 9*Cin], out
-// [N*Ho*Wo, Nout] (Nout = Cout forward, Cin dgrad); false = shape not supported by the kernel
-bool conv_halo_wide(const at::Tensor& src, const at::Tensor& w, at::Tensor out, int64_t stride, bool dgrad, int64_t mc,
-                    const std::optional<at::Tensor>& col_stats) {
-  CHECK_CUDA(src); CHECK_CUDA(w); CHECK_CUDA(out);
-  TORCH_CHECK(src.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16 && out.scalar_type() == at::kBFloat16 &&
-              src.dim() == 4 && src.is_contiguous() && w.is_contiguous() && out.is_contiguous());
-  TORCH_CHECK(stride == 1 || stride == 2, "conv_halo_wide: stride 1 or 2");
-  const int64_t c = src.size(3);
-  const int64_t rows = src.size(0) * ((src.size(1) - 1) / stride + 1) * ((src.size(2) - 1) / stride + 1);
-  TORCH_CHECK(rows > 0 && out.numel() % rows == 0, "conv_halo_wide: out must hold [N*Ho*Wo, Nout] elements");
-  const int64_t nout = out.numel() / rows;
-  TORCH_CHECK(w.numel() == (dgrad ? c * 9 * nout : nout * 9 * c), "conv_halo_wide: w must be [Cout, 9*Cin]");
-  TORCH_CHECK(dgrad ? !col_stats.has_value()
-                    : (!col_stats.has_value() || (col_stats->scalar_type() == at::kFloat && col_stats->numel() >= 2 * nout)),
-              "conv_halo_wide: col_stats is a [2 Cout] fp32 buffer of the forward");
-  const c10::cuda::CUDAGuard guard(src.device());
-  const int rc = b200_conv_halo_wide(cptr(src), cptr(w), ptr(out), static_cast<int>(src.size(0)),
-                                     static_cast<int>(src.size(1)), static_cast<int>(src.size(2)), static_cast<int>(c),
-                                     static_cast<int>(nout), static_cast<int>(stride), dgrad ? 1 : 0,
-                                     static_cast<int>(mc), opt_ptr<float>(col_stats), cur_stream());
-  if (rc == -2) return false;
-  check(rc, "conv_halo_wide");
   return true;
 }
 // stride 2: `ntaps` (4) taps per parity class, `taps` (4 x 4) packed tap words (ops/functional.py conv_s2_dgrad_taps)
@@ -1203,7 +1181,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("conv_igemm_dgrad", &conv_igemm_dgrad);
   m.def("conv_igemm_dgrad_s2", &conv_igemm_dgrad_s2);
   m.def("conv_halo", &conv_halo);
-  m.def("conv_halo_wide", &conv_halo_wide);
   m.def("gemm_batched", &gemm_batched);
   m.def("gemm_fp8", &gemm_fp8);
   m.def("quant_mx_rows", &quant_mx_rows);

@@ -67,12 +67,10 @@ int b200_conv_igemm_dgrad_s2(const void* dy, const void* w, void* dx, int N, int
 int b200_conv_igemm_wgrad(const void* dy, const void* x, float* dw, int N, int H, int W, int Cin, int Cout, int KH, int KW,
                           int stride, int pad, int Ho, int Wo, int split_k, int force_bn, const B200SgdEpilogue* sgd,
                           cudaStream_t stream);
-// ---- conv_halo.cu: 3x3 stride-1 pad-1 convolution over one 64-channel block, halo-tiled (dgrad != 0: input gradient)
-int b200_conv_halo(const void* src, const void* w, void* out, int N, int H, int W, int Nout, int dgrad, int mc,
-                   float* col_stats, cudaStream_t stream);
-// ---- conv_halo.cu: 3x3 pad-1 convolution over a gathered tensor of C = 128 (stride 1) or 64 (stride 2, forward)
-int b200_conv_halo_wide(const void* src, const void* w, void* out, int N, int H, int W, int C, int Nout, int stride,
-                        int dgrad, int mc, float* col_stats, cudaStream_t stream);
+// ---- conv_halo.cu: 3x3 pad-1 convolution, halo-tiled, over a gathered tensor of C = 64 or 128 channels (stride 1) or
+// C = 64 (stride 2, forward only); dgrad != 0: input gradient
+int b200_conv_halo(const void* src, const void* w, void* out, int N, int H, int W, int C, int Nout, int stride,
+                   int dgrad, int mc, float* col_stats, cudaStream_t stream);
 // ---- im2col_tma.cu (experimental: TMA im2col tensor maps, probe kernel only)
 int b200_im2col_tma_probe(const void* x, void* col, int N, int H, int W, int C, int KH, int KW, int stride, int pad,
                           int Ho, int Wo, cudaStream_t stream);

@@ -499,55 +499,39 @@ def conv_fwd(x: torch.Tensor, w2d: torch.Tensor, plan: ConvPlan, form: Optional[
 
 HALO_BM = 64                      # output pixels of one halo-kernel tile (conv_halo.cu)
 _HALO_MAX_SMEM = 227 * 1024       # shared memory one H100 block may use
+_HALO_FORMS = ((1, 64), (1, 128), (2, 64))   # (stride, gathered channels) conv_halo.cu instantiates; stride 2: forward
 
 
-def halo_smem_bytes(h: int, w: int) -> int:
-    """Shared memory of the halo kernel: the halo of ``64 / (h w)`` images (rounded up to 1 KB), nine 8 KB weight
-    slots, barriers, column statistics and the 1 KB realignment (conv_halo.cu halo_fixed_bytes)."""
-    halo = round_up((HALO_BM // (h * w)) * (h + 2) * (w + 2) * 128, 1024)
-    return halo + 9 * 8192 + 16 * 8 + 4 * 64 * 4 + 1024
+def halo_smem_bytes(h: int, w: int, c: int = 64, stride: int = 1) -> int:
+    """Shared memory of the halo kernel over an ``h x w`` input of ``c`` gathered channels at ``stride``: ``c / 64``
+    halo boxes of the ``64 / (ho wo)`` images (each rounded up to 1 KB), ``9 c / 64`` 8 KB weight slots, one mbarrier
+    per slot plus one for the halo (padded to a multiple of 16), column statistics and the 1 KB realignment
+    (conv_halo.cu halo_fixed_bytes)."""
+    ho, wo = conv_out_size(h, 3, stride, 1), conv_out_size(w, 3, stride, 1)
+    box = (HALO_BM // (ho * wo)) * (stride * (ho - 1) + 3) * (stride * (wo - 1) + 3) * 128
+    k_tiles = 9 * (c // 64)
+    return c // 64 * round_up(box, 1024) + k_tiles * 8192 + round_up(1 + k_tiles, 16) * 8 + 4 * 64 * 4 + 1024
 
 
-def halo_eligible(kh: int, kw: int, stride: int, pad: int, c: int, h: int, w: int, affine: Optional[dict] = None) -> bool:
-    """Whether the halo-tiled kernel takes a convolution: 3x3, stride 1, pad 1, the gathered tensor (``x`` forward,
-    ``dy`` dgrad) is one 64-channel block, a 64-row tile holds whole ``h x w`` images, the halo and the nine weight
-    slots fit in shared memory, and no eval-mode ``affine`` epilogue is asked for."""
-    return (kh == 3 and kw == 3 and stride == 1 and pad == 1 and c == 64 and h * w <= HALO_BM and
-            HALO_BM % (h * w) == 0 and affine is None and halo_smem_bytes(h, w) <= _HALO_MAX_SMEM)
+def halo_eligible(kh: int, kw: int, stride: int, pad: int, c: int, h: int, w: int,
+                  affine: Optional[dict] = None, dgrad: bool = False) -> bool:
+    """Whether the halo-tiled kernel takes a convolution over an ``h x w`` input: 3x3, pad 1, a (stride, gathered
+    channels) form of ``_HALO_FORMS`` -- stride 1 over 64 or 128 channels of the gathered tensor (``x`` forward, ``dy``
+    dgrad), or stride 2 over a 64-channel ``x`` (forward only) --, a 64-row tile holds whole output images, the halo
+    and the ``9 c / 64`` weight slots fit in shared memory, and no eval-mode ``affine`` epilogue is asked for."""
+    if kh != 3 or kw != 3 or pad != 1 or (stride, c) not in _HALO_FORMS or (dgrad and stride != 1):
+        return False
+    hw = conv_out_size(h, 3, stride, 1) * conv_out_size(w, 3, stride, 1)
+    return (hw <= HALO_BM and HALO_BM % hw == 0 and affine is None and
+            halo_smem_bytes(h, w, c, stride) <= _HALO_MAX_SMEM)
 
 
 def halo_cluster(m_rows: int) -> int:
     """CTAs of a halo-kernel cluster along M sharing the weight tiles: 4, or 2 / 1 when the tile count does not divide.
-    Both halo kernels use it.  For the wide kernel at the layer2 shapes (batch 128), clusters of 1, 2, 4 and 8 were
-    within 0.25 us of each other; 4 was fastest or tied for the stride-1 GEMMs (scripts/conv_halo_wide_bench.py, one
-    H100 80GB HBM3 at 700 W)."""
+    At the layer2 shapes (batch 128), clusters of 1, 2, 4 and 8 were within 0.25 us of each other; 4 was fastest or
+    tied for the stride-1 GEMMs (scripts/conv_halo_wide_bench.py, one H100 80GB HBM3 at 700 W)."""
     tiles = (m_rows + HALO_BM - 1) // HALO_BM
     return 4 if tiles % 4 == 0 else 2 if tiles % 2 == 0 else 1
-
-
-_HALO_WIDE_FORMS = ((1, 128), (2, 64))   # (stride, gathered channels) of the wide kernel's instantiations (conv_halo.cu)
-
-
-def halo_wide_smem_bytes(c: int, h: int, w: int, stride: int) -> int:
-    """Shared memory of the wide-channel halo kernel over an ``h x w`` input of ``c`` gathered channels: ``c / 64``
-    halo boxes of the ``64 / (ho wo)`` images (each rounded up to 1 KB), ``9 c / 64`` 8 KB weight slots, barriers,
-    column statistics and the 1 KB realignment (conv_halo.cu halo_wide_fixed_bytes)."""
-    ho, wo = conv_out_size(h, 3, stride, 1), conv_out_size(w, 3, stride, 1)
-    box = (HALO_BM // (ho * wo)) * (stride * (ho - 1) + 3) * (stride * (wo - 1) + 3) * 128
-    return c // 64 * (round_up(box, 1024) + 9 * 8192) + 32 * 8 + 4 * 64 * 4 + 1024
-
-
-def halo_wide_eligible(kh: int, kw: int, stride: int, pad: int, c: int, h: int, w: int,
-                       affine: Optional[dict] = None, dgrad: bool = False) -> bool:
-    """Whether the wide-channel halo kernel takes a convolution over an ``h x w`` input: 3x3, pad 1, and either stride
-    1 over a 128-channel gathered tensor (``x`` forward, ``dy`` dgrad) or stride 2 over a 64-channel ``x`` (forward
-    only); a 64-row tile holds whole output images, the halo and the ``9 c / 64`` weight slots fit in shared memory,
-    and no eval-mode ``affine`` epilogue is asked for.  Stride 1 over 64 channels is :func:`halo_eligible`'s."""
-    if kh != 3 or kw != 3 or pad != 1 or (stride, c) not in _HALO_WIDE_FORMS or (dgrad and stride != 1):
-        return False
-    hw = conv_out_size(h, 3, stride, 1) * conv_out_size(w, 3, stride, 1)
-    return (hw <= HALO_BM and HALO_BM % hw == 0 and affine is None and
-            halo_wide_smem_bytes(c, h, w, stride) <= _HALO_MAX_SMEM)
 
 
 def _conv_path(path: Optional[str], eligible: bool) -> str:
@@ -556,7 +540,7 @@ def _conv_path(path: Optional[str], eligible: bool) -> str:
     if path not in ("halo", "im2col"):
         raise ValueError("path must be None, 'halo' or 'im2col', not {!r}".format(path))
     if path == "halo" and not eligible:
-        raise ValueError("no halo kernel takes this convolution (see halo_eligible, halo_wide_eligible)")
+        raise ValueError("the halo kernel does not take this convolution (see halo_eligible)")
     return path
 
 
@@ -570,10 +554,10 @@ def conv_igemm_fwd(x: torch.Tensor, w2d: torch.Tensor, kh: int, kw: int, stride:
     BatchNorm epilogue as in :func:`gemm`.  ``out``: contiguous bf16 ``[N*Ho*Wo, Cout]`` to write.  Returns ``None``
     when the shape (or the epilogue) is not supported (Cin % 64 != 0).
 
-    ``path``: ``None`` takes a halo-tiled kernel whenever :func:`halo_eligible` or :func:`halo_wide_eligible` holds and
-    the im2col-mode kernel otherwise; ``"halo"`` / ``"im2col"`` force one (``"halo"`` on a shape neither halo kernel
-    takes raises).  ``mc``: cluster size of the halo kernel (default :func:`halo_cluster`);
-    ``cluster_k`` / ``force_bn`` apply to the im2col path."""
+    ``path``: ``None`` takes the halo-tiled kernel whenever :func:`halo_eligible` holds and the im2col-mode kernel
+    otherwise; ``"halo"`` / ``"im2col"`` force one (``"halo"`` on a shape the halo kernel does not take raises).
+    ``mc``: cluster size of the halo kernel (default :func:`halo_cluster`); ``cluster_k`` / ``force_bn`` apply to
+    the im2col path."""
     n, h, w, c = x.shape
     cout = w2d.shape[0]
     if c % 64 or w2d.shape[1] != kh * kw * c or not x.is_contiguous() or not w2d.is_contiguous():
@@ -581,13 +565,10 @@ def conv_igemm_fwd(x: torch.Tensor, w2d: torch.Tensor, kh: int, kw: int, stride:
     ho, wo = conv_out_size(h, kh, stride, pad), conv_out_size(w, kw, stride, pad)
     M, K = n * ho * wo, kh * kw * c
     halo = halo_eligible(kh, kw, stride, pad, c, h, w, affine) and cout % 8 == 0
-    wide = halo_wide_eligible(kh, kw, stride, pad, c, h, w, affine) and cout % 8 == 0
-    if _conv_path(path, halo or wide) == "halo":
+    if _conv_path(path, halo) == "halo":
         y = out if out is not None else torch.empty((M, cout), dtype=BF16, device=x.device)
-        if halo and not load().conv_halo(x, w2d, y, False, mc or halo_cluster(M), col_stats):
+        if not load().conv_halo(x, w2d, y, stride, False, mc or halo_cluster(M), col_stats):
             raise RuntimeError("conv_halo declined a convolution halo_eligible admits")
-        if wide and not load().conv_halo_wide(x, w2d, y, stride, False, mc or halo_cluster(M), col_stats):
-            raise RuntimeError("conv_halo_wide declined a convolution halo_wide_eligible admits")
         return y
     bn = force_bn or pick_bn(M, cout)
     if cluster_k is None:
@@ -640,20 +621,16 @@ def conv_igemm_dgrad(dy: torch.Tensor, w2d: torch.Tensor, in_shape, kh: int, kw:
     convolution of ``dy``.  Stride 2: one launch over the four parity classes of :func:`conv_s2_dgrad_taps`.
     ``out``: contiguous bf16 ``[N, H, W, Cin]`` to write (every element is written).  Returns ``None`` when the shape
     is not supported (channels not multiples of 64, other strides).  ``path`` / ``mc``: as in :func:`conv_igemm_fwd`
-    (the halo kernels gather ``dy``, so ``Cout`` is what their rules check).  ``cluster_k``: cluster split-K of the
+    (the halo kernel gathers ``dy``, so ``Cout`` is what its rule checks).  ``cluster_k``: cluster split-K of the
     stride-1 im2col path (default :func:`pick_cluster_k`)."""
     n, h, w, c = in_shape
     cout = dy.shape[-1]
     if c % 64 or cout % 64 or w2d.shape[1] != kh * kw * c or not dy.is_contiguous() or not w2d.is_contiguous():
         return None
-    halo = halo_eligible(kh, kw, stride, pad, cout, h, w)
-    wide = halo_wide_eligible(kh, kw, stride, pad, cout, h, w, dgrad=True)
-    if _conv_path(path, halo or wide) == "halo":
+    if _conv_path(path, halo_eligible(kh, kw, stride, pad, cout, h, w, dgrad=True)) == "halo":
         dx = out if out is not None else torch.empty((n, h, w, c), dtype=BF16, device=dy.device)
-        if halo and not load().conv_halo(dy, w2d, dx, True, mc or halo_cluster(n * h * w), None):
+        if not load().conv_halo(dy, w2d, dx, 1, True, mc or halo_cluster(n * h * w), None):
             raise RuntimeError("conv_halo declined a convolution halo_eligible admits")
-        if wide and not load().conv_halo_wide(dy, w2d, dx, 1, True, mc or halo_cluster(n * h * w), None):
-            raise RuntimeError("conv_halo_wide declined a convolution halo_wide_eligible admits")
         return dx
     if stride == 1:
         M, K = n * h * w, kh * kw * cout

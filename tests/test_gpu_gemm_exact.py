@@ -32,7 +32,7 @@ that explains its worst element that is not correctly rounded (``pytest -rP``). 
 700 W power limit:
 * fp32 rms ratio: 2^-23.4 to 2^-19.8, and 2^-18.6 for atomic split-K 7 at K = 16384;
 * bf16: 4.5 % to 18.8 % of the elements have a midpoint inside ``w``, and the worst implied error is
-  2^-22.5 sum|ab| (the stride-1 wide halo forward), well inside ``w``.
+  2^-22.5 sum|ab| (the stride-1 128-channel halo forward), well inside ``w``.
 
 Every output is written into a view of a larger buffer prefilled with a NaN bit pattern: extra rows after M, a row
 pitch ``ldd > N`` for GEMMs, a tail after the last element.  The guard elements must keep their bits, and an output
@@ -87,12 +87,8 @@ def persistent(bn, stages):
 SIMT = "simt"
 
 
-def halo(dgrad):
-    return "halo<{}>".format(int(dgrad))
-
-
-def halo_wide(dgrad, cb, stride):
-    return "halo_wide<{},{},{}>".format(int(dgrad), cb, stride)
+def halo(dgrad, cb, stride):
+    return "halo<{},{},{}>".format(int(dgrad), cb, stride)
 
 
 CASES = [
@@ -159,26 +155,26 @@ CASES = [
        kernels=[splitk(128, conv=1)]),
     _c("fwd_1x1_s2_shallow", "fwd", 126, 8, 8, 128, 128, 1, 2, 0, cluster_k=1, bn=128,
        kernels=[fixed(128, 3, conv=1)]),
-    # the layer1 halo kernel (64 channels, 8x8), cluster sizes 1 / 2 / 4, forward with statistics and input gradient
+    # the halo kernel, stride 1 over 64 channels (8x8), cluster sizes 1 / 2 / 4, forward with statistics and input
+    # gradient; then stride 1 over 128 channels (4x4) and stride 2 over 64 channels (8x8 -> 4x4)
     _c("halo_fwd_mc4_stats", "fwd", 128, 8, 8, 64, 64, 3, 1, 1, path="halo", mc=4, stats=True, fams="EF",
-       kernels=[halo(0)]),
-    _c("halo_fwd_mc2_stats", "fwd", 126, 8, 8, 64, 64, 3, 1, 1, path="halo", mc=2, stats=True, kernels=[halo(0)]),
-    _c("halo_fwd_mc1_stats", "fwd", 3, 8, 8, 64, 64, 3, 1, 1, path="halo", mc=1, stats=True, kernels=[halo(0)]),
-    _c("halo_dgrad_mc4", "dgrad", 128, 8, 8, 64, 64, 3, 1, 1, path="halo", mc=4, kernels=[halo(1)]),
-    _c("halo_dgrad_mc2", "dgrad", 126, 8, 8, 64, 64, 3, 1, 1, path="halo", mc=2, fams="EF", kernels=[halo(1)]),
-    _c("halo_dgrad_mc1", "dgrad", 1, 8, 8, 64, 64, 3, 1, 1, path="halo", mc=1, kernels=[halo(1)]),
-    # the wide halo kernel: stride 1 over 128 channels (4x4) and stride 2 over 64 channels (8x8 -> 4x4)
+       kernels=[halo(0, 1, 1)]),
+    _c("halo_fwd_mc2_stats", "fwd", 126, 8, 8, 64, 64, 3, 1, 1, path="halo", mc=2, stats=True, kernels=[halo(0, 1, 1)]),
+    _c("halo_fwd_mc1_stats", "fwd", 3, 8, 8, 64, 64, 3, 1, 1, path="halo", mc=1, stats=True, kernels=[halo(0, 1, 1)]),
+    _c("halo_dgrad_mc4", "dgrad", 128, 8, 8, 64, 64, 3, 1, 1, path="halo", mc=4, kernels=[halo(1, 1, 1)]),
+    _c("halo_dgrad_mc2", "dgrad", 126, 8, 8, 64, 64, 3, 1, 1, path="halo", mc=2, fams="EF", kernels=[halo(1, 1, 1)]),
+    _c("halo_dgrad_mc1", "dgrad", 1, 8, 8, 64, 64, 3, 1, 1, path="halo", mc=1, kernels=[halo(1, 1, 1)]),
     _c("wide_s1_fwd_mc8_stats", "fwd", 128, 4, 4, 128, 128, 3, 1, 1, path="halo", mc=8, stats=True, fams="EF",
-       kernels=[halo_wide(0, 2, 1)]),
-    _c("wide_s1_fwd_mc2", "fwd", 126, 4, 4, 128, 128, 3, 1, 1, path="halo", mc=2, kernels=[halo_wide(0, 2, 1)]),
-    _c("wide_s1_fwd_mc1", "fwd", 1, 4, 4, 128, 128, 3, 1, 1, path="halo", mc=1, kernels=[halo_wide(0, 2, 1)]),
+       kernels=[halo(0, 2, 1)]),
+    _c("wide_s1_fwd_mc2", "fwd", 126, 4, 4, 128, 128, 3, 1, 1, path="halo", mc=2, kernels=[halo(0, 2, 1)]),
+    _c("wide_s1_fwd_mc1", "fwd", 1, 4, 4, 128, 128, 3, 1, 1, path="halo", mc=1, kernels=[halo(0, 2, 1)]),
     _c("wide_s2_fwd_mc4_stats", "fwd", 128, 8, 8, 64, 128, 3, 2, 1, path="halo", mc=4, stats=True,
-       kernels=[halo_wide(0, 1, 2)]),
-    _c("wide_s2_fwd_mc1", "fwd", 3, 8, 8, 64, 128, 3, 2, 1, path="halo", mc=1, kernels=[halo_wide(0, 1, 2)]),
+       kernels=[halo(0, 1, 2)]),
+    _c("wide_s2_fwd_mc1", "fwd", 3, 8, 8, 64, 128, 3, 2, 1, path="halo", mc=1, kernels=[halo(0, 1, 2)]),
     _c("wide_dgrad_mc4", "dgrad", 128, 4, 4, 128, 128, 3, 1, 1, path="halo", mc=4, fams="EF",
-       kernels=[halo_wide(1, 2, 1)]),
-    _c("wide_dgrad_mc2", "dgrad", 6, 4, 4, 128, 128, 3, 1, 1, path="halo", mc=2, kernels=[halo_wide(1, 2, 1)]),
-    _c("wide_dgrad_mc1", "dgrad", 1, 4, 4, 128, 128, 3, 1, 1, path="halo", mc=1, kernels=[halo_wide(1, 2, 1)]),
+       kernels=[halo(1, 2, 1)]),
+    _c("wide_dgrad_mc2", "dgrad", 6, 4, 4, 128, 128, 3, 1, 1, path="halo", mc=2, kernels=[halo(1, 2, 1)]),
+    _c("wide_dgrad_mc1", "dgrad", 1, 4, 4, 128, 128, 3, 1, 1, path="halo", mc=1, kernels=[halo(1, 2, 1)]),
     # stride-1 implicit input gradient (im2col mode): cluster split-K 4 by default, and the single-pass kernel
     _c("dgrad_s1_im2col_cluster", "dgrad", 126, 2, 2, 256, 256, 3, 1, 1, path="im2col", kernels=[splitk(64, conv=3)]),
     _c("dgrad_s1_im2col_cluster1", "dgrad", 6, 8, 8, 64, 64, 3, 1, 1, path="im2col", cluster_k=1,
@@ -192,7 +188,7 @@ CASES = [
     _c("wgrad_s1", "wgrad", 6, 8, 8, 64, 64, 3, 1, 1, kernels=[fixed(64, 8, conv=2)]),
     _c("wgrad_s2", "wgrad", 3, 8, 8, 64, 128, 3, 2, 1, kernels=[fixed(64, 8, conv=2)]),
     _c("wgrad_split3", "wgrad", 128, 4, 4, 128, 128, 3, 1, 1, fams="EF", kernels=[fixed(64, 8, conv=2)]),
-    # eval-mode BatchNorm epilogue on the implicit forward (the halo kernels do not take it)
+    # eval-mode BatchNorm epilogue on the implicit forward (the halo kernel does not take it)
     _c("fwd_affine_cluster4", "fwd", 6, 4, 4, 128, 128, 3, 1, 1, affine="residual_relu",
        kernels=[splitk(64, conv=1, affine=1)]),
     _c("fwd_affine_single_pass", "fwd", 3, 8, 8, 64, 64, 3, 1, 1, affine="plain", cluster_k=1,
@@ -759,7 +755,7 @@ def test_full_mantissa_operands(case, dev):
 
 
 _KERNEL = re.compile(r"(gemm_bf16_fixed_kernel|gemm_bf16_persistent_kernel|gemm_bf16_splitk_kernel|gemm_simt_kernel|"
-                     r"conv_halo_wide_kernel|conv_halo_kernel)(?:<([^>]*)>)?")
+                     r"conv_halo_kernel)(?:<([^>]*)>)?")
 
 
 def _kernel_key(name):
@@ -777,9 +773,7 @@ def _kernel_key(name):
         return splitk(int(args[0]), int(args[2]), int(args[3]), int(args[1]))
     if base == "gemm_bf16_persistent_kernel":
         return persistent(int(args[0]), int(args[1]))
-    if base == "conv_halo_kernel":
-        return halo(int(args[0]))
-    return halo_wide(int(args[0]), int(args[1]), int(args[2]))
+    return halo(int(args[0]), int(args[1]), int(args[2]))
 
 
 def test_kernel_key_parses_demangled_names():
@@ -787,11 +781,11 @@ def test_kernel_key_parses_demangled_names():
                        "(CUtensorMap_st, CUtensorMap_st, b200::GemmParams)") == fixed(128, 6, 1, 1)
     assert _kernel_key("void b200::gemm_bf16_splitk_kernel<64, true, 3, false>(CUtensorMap_st, CUtensorMap_st, "
                        "b200::GemmParams)") == splitk(64, 3, 0)
-    assert _kernel_key("void b200::conv_halo_wide_kernel<(bool)1, 2, 1>(CUtensorMap_st, CUtensorMap_st, "
-                       "b200::HaloWideParams)") == halo_wide(1, 2, 1)
+    assert _kernel_key("void b200::conv_halo_kernel<(bool)1, 2, 1>(CUtensorMap_st, CUtensorMap_st, "
+                       "b200::HaloParams)") == halo(1, 2, 1)
     assert _kernel_key("b200::gemm_simt_kernel(__nv_bfloat16 const*, ...)") == SIMT
-    assert _kernel_key("void b200::conv_halo_kernel<false>(CUtensorMap_st, CUtensorMap_st, b200::HaloParams)") == \
-        halo(0)
+    assert _kernel_key("void b200::conv_halo_kernel<false, 1, 1>(CUtensorMap_st, CUtensorMap_st, b200::HaloParams)") \
+        == halo(0, 1, 1)
 
 
 @pytest.mark.gpu
@@ -808,4 +802,5 @@ def test_case_table_reaches_every_kernel_instantiation(dev):
     seen = {_kernel_key(e.name) for e in prof.events()} - {None}
     assert want <= seen, sorted(want - seen)
     assert {"fixed<64,4,0,0>", "fixed<64,8,0,0>", "fixed<128,3,0,0>", "fixed<128,6,0,0>", "persistent<128,3>",
-            "persistent<64,5>", "splitk<64,1,0,0>", "splitk<128,1,0,0>", SIMT, halo(0), halo(1)} <= want
+            "persistent<64,5>", "splitk<64,1,0,0>", "splitk<128,1,0,0>", SIMT, halo(0, 1, 1),
+            halo(1, 1, 1)} <= want
