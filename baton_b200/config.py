@@ -32,6 +32,8 @@ class FederationConfig:
     adam_beta1: float = 0.9            # AdamW betas and eps (read only with optimizer='adamw')
     adam_beta2: float = 0.999
     adam_eps: float = 1e-8
+    augment: str = "none"              # local-training augmentation: none | crop | flip | crop_flip (NHWC image shards)
+    augment_padding: int = 4           # zero padding of the random crop, pixels on each side
     dp_clip: float = 0.0               # DP-FedAvg: L2 clip norm of a client's update (0: DP off)
     dp_noise_multiplier: float = 0.0   # DP-FedAvg: noise std on the sum of clipped updates, in units of dp_clip
     dp_delta: float = 1e-5             # DP-FedAvg: delta of the (epsilon, delta) the manager reports
@@ -60,6 +62,8 @@ class FederationConfig:
         from .train import check_adamw, check_prox_mu
         check_prox_mu(self.prox_mu)
         check_adamw((self.adam_beta1, self.adam_beta2), self.adam_eps)
+        from .data.augment import check_augment
+        check_augment(self.augment, self.augment_padding)
         from .parallel.dp import check_dp
         check_dp(self.dp_clip, self.dp_noise_multiplier)
         if not (0.0 < float(self.dp_delta) < 1.0):
@@ -83,6 +87,8 @@ class FederationConfig:
         kw = {"lr": self.lr, "batch_size": self.batch_size, "prox_mu": self.prox_mu}
         if self.optimizer != "sgd":
             kw.update(optimizer=self.optimizer, betas=(self.adam_beta1, self.adam_beta2), eps=self.adam_eps)
+        if self.augment != "none":
+            kw.update(augment=self.augment, augment_padding=self.augment_padding)
         return kw
 
     def dp_config(self):

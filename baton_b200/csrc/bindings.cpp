@@ -477,6 +477,28 @@ void gather_rows(const at::Tensor& src, const at::Tensor& idx, at::Tensor dst) {
         "gather_rows");
 }
 
+void gather_augment(const at::Tensor& src, const at::Tensor& idx, at::Tensor dst, const at::Tensor& words,
+                    int64_t key, int64_t padding, bool crop, bool flip, int64_t s0) {
+  CHECK_CUDA(src);
+  CHECK_CUDA(idx);
+  CHECK_CUDA(dst);
+  CHECK_CUDA(words);
+  TORCH_CHECK(src.dim() == 4 && src.is_contiguous() && dst.is_contiguous() && dst.scalar_type() == src.scalar_type(),
+              "gather_augment: contiguous NHWC src and dst of one dtype");
+  TORCH_CHECK(idx.scalar_type() == at::kLong && idx.is_contiguous(), "gather_augment: contiguous int64 idx");
+  TORCH_CHECK(words.scalar_type() == at::kInt && words.is_contiguous() && words.numel() >= 3,
+              "gather_augment: words = int32 {epoch, stream_lo, stream_hi}");
+  TORCH_CHECK(dst.numel() == idx.numel() * (src.numel() / std::max<int64_t>(1, src.size(0))),
+              "gather_augment: dst holds one image per index");
+  const c10::cuda::CUDAGuard guard(src.device());
+  check(b200_gather_augment(src.data_ptr(), reinterpret_cast<const long long*>(idx.data_ptr<int64_t>()), dst.data_ptr(),
+                            reinterpret_cast<const unsigned*>(words.data_ptr<int32_t>()), idx.numel(), s0,
+                            static_cast<unsigned long long>(key), static_cast<int>(padding), crop ? 1 : 0, flip ? 1 : 0,
+                            static_cast<int>(src.size(1)), static_cast<int>(src.size(2)), static_cast<int>(src.size(3)),
+                            static_cast<int>(src.element_size()), cur_stream()),
+        "gather_augment");
+}
+
 void colsum(const at::Tensor& x, at::Tensor out, int64_t rows, int64_t cols, bool accumulate) {
   CHECK_CUDA(x);
   const c10::cuda::CUDAGuard guard(x.device());
@@ -1193,6 +1215,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("scaffold_dc", &scaffold_dc);
   m.def("cast", &cast);
   m.def("gather_rows", &gather_rows);
+  m.def("gather_augment", &gather_augment);
   m.def("colsum", &colsum);
   m.def("add_bf16", &add_bf16);
   m.def("relu_bwd", &relu_bwd);

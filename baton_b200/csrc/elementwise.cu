@@ -3,6 +3,7 @@
 // (bias gradients), ReLU / GELU pieces.  All use 16-byte vectors and grid-stride loops sized to
 // the device's SMs x a few resident CTAs.
 #define B200_TU_TAG 8
+#include "dp.cuh"
 #include "launch.h"
 #include "pdl.cuh"
 #include "ptx.cuh"
@@ -469,6 +470,87 @@ gather_rows_kernel(const uint4* __restrict__ src, const long long* __restrict__ 
     dst[i] = __ldg(src + idx[r] * row_vecs + c);
   }
 }
+// ------------------------------------------------------------------ augmenting batch gather (random crop + flip)
+// dst[s] = augment(src[idx[s]]) for NHWC images.  Output position p = s0 + s draws from ONE Philox4x32-10 output,
+// counter (p, epoch, stream_lo, stream_hi), key `key`: oy = x.x % (2 pad + 1), ox = x.y % (2 pad + 1) (0 without
+// crop), flip = x.z & 1 (0 without flip); out[h, w] = src[h + oy - pad, w' + ox - pad] (w' = W - 1 - w when flipped),
+// 0 outside the image.  The per-epoch words {epoch, stream_lo, stream_hi} are read from device memory so a replayed
+// graph picks up a new epoch without a recapture.
+//
+// One work item = a tile of up to `rows_per_tile` output rows of one image.  Its source rows are one contiguous byte
+// range (the crop shifts rows as a whole), which the CTA stages into shared memory with V-byte vector loads; each
+// thread then composes V output bytes from single-element shared-memory reads (the pixel order is reversed and
+// shifted by a non-vector amount) and writes them with one V-byte store.  Global traffic is V-byte vectors only.
+template <int N> struct AugVec;
+template <> struct AugVec<2> { using T = uint16_t; };
+template <> struct AugVec<4> { using T = uint32_t; };
+template <> struct AugVec<8> { using T = uint2; };
+template <> struct AugVec<16> { using T = uint4; };
+
+constexpr int AUG_THREADS = 256;
+constexpr int AUG_TILE_BYTES = 8192;    // shared memory per work item (more when one image row is larger)
+constexpr int AUG_MAX_ROW_BYTES = 48 * 1024;   // one image row must fit the default dynamic shared memory
+
+template <int ES, int V>
+__global__ void __launch_bounds__(AUG_THREADS)
+gather_augment_kernel(const uint8_t* __restrict__ src, const long long* __restrict__ idx, uint8_t* __restrict__ dst,
+                      const uint32_t* __restrict__ words, long long n_rows, long long s0, uint2 key, int pad,
+                      int crop, int flip, int H, int W, int C, int rows_per_tile) {
+  using E = typename AugVec<ES>::T;
+  using Vt = typename AugVec<V>::T;
+  constexpr int EPV = V / ES;
+  extern __shared__ uint4 aug_smem[];
+  const E* se = reinterpret_cast<const E*>(aug_smem);
+  griddep_launch_dependents();
+  griddep_wait();
+  const uint32_t epoch = words[0], st_lo = words[1], st_hi = words[2];
+  const int row_e = W * C;
+  const long long row_bytes = static_cast<long long>(row_e) * ES, img_bytes = row_bytes * H;
+  const int tiles = (H + rows_per_tile - 1) / rows_per_tile;
+  const int items = static_cast<int>(n_rows) * tiles;     // < 2^31 (checked at launch)
+  const uint32_t span = 2u * static_cast<uint32_t>(pad) + 1u;
+  for (int it = blockIdx.x; it < items; it += gridDim.x) {
+    const int s = it / tiles;
+    const int h0 = (it - s * tiles) * rows_per_tile;
+    const int hn = min(rows_per_tile, H - h0);
+    const uint4 x = philox4x32_10(make_uint4(static_cast<uint32_t>(s0 + s), epoch, st_lo, st_hi), key);
+    const int dy = crop ? static_cast<int>(x.x % span) - pad : 0;
+    const int dx = crop ? static_cast<int>(x.y % span) - pad : 0;
+    const bool fl = flip && (x.z & 1u);
+    const int lo = max(0, h0 + dy), hi = min(H, h0 + hn + dy);    // source rows this tile reads
+    if (hi > lo) {
+      const Vt* g = reinterpret_cast<const Vt*>(src + idx[s] * img_bytes + lo * row_bytes);
+      Vt* d = reinterpret_cast<Vt*>(aug_smem);
+      const int nv = static_cast<int>((hi - lo) * row_bytes / V);
+      for (int i = threadIdx.x; i < nv; i += AUG_THREADS) d[i] = __ldg(g + i);
+    }
+    __syncthreads();
+    Vt* out = reinterpret_cast<Vt*>(dst + static_cast<long long>(s) * img_bytes + h0 * row_bytes);
+    const int out_v = static_cast<int>(hn * row_bytes / V);
+    for (int i = threadIdx.x; i < out_v; i += AUG_THREADS) {
+      const int e = i * EPV;
+      int r = e / row_e;
+      int w = (e - r * row_e) / C;
+      int c = e - r * row_e - w * C;
+      uint32_t wd[(V + 3) / 4] = {};     // the output vector as 32-bit words (kept in registers)
+#pragma unroll
+      for (int k = 0; k < EPV; ++k) {
+        const int sh = h0 + r + dy, sw = (fl ? W - 1 - w : w) + dx;
+        const uint32_t val = (sh >= lo && sh < hi && sw >= 0 && sw < W) ? se[(sh - lo) * row_e + sw * C + c] : 0u;
+        wd[k * ES / 4] |= val << (8 * ((k * ES) & 3));
+        if (++c == C) {
+          c = 0;
+          if (++w == W) { w = 0; ++r; }
+        }
+      }
+      if constexpr (V == 16) out[i] = make_uint4(wd[0], wd[1], wd[2], wd[3]);
+      else if constexpr (V == 8) out[i] = make_uint2(wd[0], wd[1]);
+      else out[i] = static_cast<Vt>(wd[0]);
+    }
+    __syncthreads();
+  }
+}
+
 __global__ void gather_i64_kernel(const long long* __restrict__ src, const long long* __restrict__ idx,
                                   long long* __restrict__ dst, long long n) {
   griddep_launch_dependents();
@@ -800,6 +882,48 @@ extern "C" int b200_gather_rows(const void* src, const long long* idx, void* dst
   const int rv = static_cast<int>(row_bytes / 16);
   launch_pdl(gather_rows_kernel, ew_grid(n_rows * rv), EW_THREADS, 0, stream, reinterpret_cast<const uint4*>(src), idx,
                                                                       reinterpret_cast<uint4*>(dst), n_rows, rv);
+  RET_LAST();
+}
+template <int ES, int V>
+static void launch_gather_augment(const void* src, const long long* idx, void* dst, const uint32_t* words,
+                                  long long n_rows, long long s0, uint2 key, int pad, int crop, int flip, int H, int W,
+                                  int C, int rows_per_tile, cudaStream_t stream) {
+  const long long row_bytes = static_cast<long long>(W) * C * ES;
+  const size_t smem = static_cast<size_t>((rows_per_tile * row_bytes + 15) / 16 * 16);
+  const long long items = n_rows * ((H + rows_per_tile - 1) / rows_per_tile);
+  const int grid = static_cast<int>(items < device_sm_count() * 8LL ? items : device_sm_count() * 8LL);
+  launch_pdl(gather_augment_kernel<ES, V>, grid, AUG_THREADS, smem, stream, static_cast<const uint8_t*>(src), idx,
+             static_cast<uint8_t*>(dst), words, n_rows, s0, key, pad, crop, flip, H, W, C, rows_per_tile);
+}
+extern "C" int b200_gather_augment(const void* src, const long long* idx, void* dst, const unsigned* words,
+                                   long long n_rows, long long s0, unsigned long long key, int pad, int crop, int flip,
+                                   int H, int W, int C, int elem_bytes, cudaStream_t stream) {
+  if (n_rows <= 0) return 0;
+  if ((elem_bytes != 2 && elem_bytes != 4) || H < 1 || W < 1 || C < 1 || pad < 0) return -2;
+  const long long row_bytes = static_cast<long long>(W) * C * elem_bytes;
+  if (row_bytes > AUG_MAX_ROW_BYTES || n_rows * H >= (1LL << 31)) return -2;
+  // widest vector dividing the row pitch and both base addresses: every staged range and output tile starts on a row
+  int v = 16;
+  while (v > elem_bytes && (row_bytes % v || reinterpret_cast<uintptr_t>(src) % v || reinterpret_cast<uintptr_t>(dst) % v))
+    v >>= 1;
+  if (row_bytes % v || reinterpret_cast<uintptr_t>(src) % v || reinterpret_cast<uintptr_t>(dst) % v) return -2;
+  long long r = AUG_TILE_BYTES / row_bytes;
+  const int rows_per_tile = static_cast<int>(r < 1 ? 1 : (r > H ? H : r));
+  const uint2 k = make_uint2(static_cast<uint32_t>(key), static_cast<uint32_t>(key >> 32));
+  const uint32_t* w = reinterpret_cast<const uint32_t*>(words);
+#define B200_AUG(ES, V)                                                                                               \
+  launch_gather_augment<ES, V>(src, idx, dst, w, n_rows, s0, k, pad, crop, flip, H, W, C, rows_per_tile, stream)
+  if (elem_bytes == 2) {
+    if (v == 16) B200_AUG(2, 16);
+    else if (v == 8) B200_AUG(2, 8);
+    else if (v == 4) B200_AUG(2, 4);
+    else B200_AUG(2, 2);
+  } else {
+    if (v == 16) B200_AUG(4, 16);
+    else if (v == 8) B200_AUG(4, 8);
+    else B200_AUG(4, 4);
+  }
+#undef B200_AUG
   RET_LAST();
 }
 extern "C" int b200_gather_rows_i64(const long long* src, const long long* idx, long long* dst, long long n,

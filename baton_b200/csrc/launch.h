@@ -117,6 +117,12 @@ int b200_gather_rows(const void* src, const long long* idx, void* dst, long long
                      cudaStream_t stream);
 int b200_gather_rows_i64(const long long* src, const long long* idx, long long* dst, long long n,
                          cudaStream_t stream);
+// dst[s] = random crop (zero padding `pad`) + horizontal flip of the NHWC image src[idx[s]], s in [0, n_rows); the
+// draws of output position s0 + s come from Philox4x32-10 under `key` with counter (s0 + s, words[0..2]) where words =
+// {epoch, stream_lo, stream_hi} is read on the device.  elem_bytes 2 or 4; one image row at most 48 KB
+int b200_gather_augment(const void* src, const long long* idx, void* dst, const unsigned* words, long long n_rows,
+                        long long s0, unsigned long long key, int pad, int crop, int flip, int H, int W, int C,
+                        int elem_bytes, cudaStream_t stream);
 int b200_colsum(const void* x, float* out, long long rows, int cols, int accumulate, cudaStream_t stream);
 int b200_add_bf16(const void* a, const void* b, void* out, long long n, int relu, cudaStream_t stream);
 int b200_relu_bwd_bf16(const void* y, const void* dy, void* dx, long long n, cudaStream_t stream);

@@ -376,6 +376,38 @@ def gather_rows(src: torch.Tensor, idx: torch.Tensor, out: Optional[torch.Tensor
     return out
 
 
+AUGMENT_MAX_ROW_BYTES = 48 * 1024      # one image row of gather_augment fits the default dynamic shared memory
+
+
+def gather_augment(src: torch.Tensor, idx: torch.Tensor, words: torch.Tensor, key: int, padding: int, *,
+                   crop: bool = True, flip: bool = True, s0: int = 0,
+                   out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``augment(src[idx])`` for a resident NHWC image shard (bf16 / fp16 / fp32): a random crop of the zero-padded
+    image (``padding`` pixels each side) and a random horizontal flip, drawn for output position ``s0 + s`` from
+    Philox4x32-10 under the 64-bit ``key`` with counter ``(s0 + s, epoch, stream_lo, stream_hi)``.  ``words`` is a
+    device int32 tensor ``{epoch, stream_lo, stream_hi}`` read when the kernel runs (a captured graph follows its
+    contents).  ``data/augment.py: gather_augment_reference`` is the same function in torch."""
+    if src.dim() != 4 or not src.is_contiguous() or src.dtype not in (torch.bfloat16, torch.float16, torch.float32):
+        raise ValueError("gather_augment needs a contiguous NHWC bf16 / fp16 / fp32 shard, got {} {}".format(
+            tuple(src.shape), src.dtype))
+    H, W, C = src.shape[1:]
+    if W * C * src.element_size() > AUGMENT_MAX_ROW_BYTES:
+        raise ValueError("gather_augment: an image row is {} bytes, at most {} are supported".format(
+            W * C * src.element_size(), AUGMENT_MAX_ROW_BYTES))
+    if not 0 <= int(padding) < 1 << 15:
+        raise ValueError("gather_augment: padding must be in [0, 32768), got {!r}".format(padding))
+    if words.dtype != torch.int32 or words.numel() < 3 or words.device != src.device:
+        raise ValueError("gather_augment: words must be an int32 device tensor {epoch, stream_lo, stream_hi}")
+    if idx.dtype != torch.int64 or idx.device != src.device:
+        raise ValueError("gather_augment: idx must be an int64 tensor on the shard's device")
+    if out is None:
+        out = torch.empty((idx.numel(), H, W, C), dtype=src.dtype, device=src.device)
+    key = int(key) & 0xFFFFFFFFFFFFFFFF
+    load().gather_augment(src, idx.contiguous(), out, words, key - (1 << 64) if key >> 63 else key, int(padding),
+                          bool(crop), bool(flip), int(s0))
+    return out
+
+
 def colsum_(x2d: torch.Tensor, out: torch.Tensor, accumulate: bool = True) -> torch.Tensor:
     load().colsum(x2d, out, x2d.shape[0], x2d.shape[1], accumulate)
     return out

@@ -76,7 +76,8 @@ class FederatedEngine:
                  krum_m: Optional[int] = None, server_opt: Optional[str] = None, server_lr: Optional[float] = None,
                  server_betas: Tuple[float, float] = (0.9, 0.99), server_tau: float = 1e-3,
                  compress: Optional[str] = None, topk_ratio: float = 0.01, error_feedback: bool = True,
-                 local_keys: "Optional[str | Sequence[str]]" = None):
+                 local_keys: "Optional[str | Sequence[str]]" = None, augment: Optional[str] = None,
+                 augment_padding: int = 4):
         """``prox_mu > 0``: FedProx local training -- every step adds ``prox_mu * (theta - global_w)`` to the gradient,
         ``global_w`` being the global model the round started from (for logical clients too: each starts from it).
 
@@ -135,7 +136,16 @@ class FederatedEngine:
         :meth:`evaluate` scores each hosted client's personalized model, and :meth:`state_dict` returns the local
         entries at their initial values.  It cannot be combined with DP, SCAFFOLD, a robust aggregator or Krum, top-k
         uploads or ``tile_flags``; the optimizer-emitted upload is off.  Each hosted client that has taken part costs
-        ``4 (hi - lo)`` bytes.  ``None`` (the default) runs exactly the plain engine."""
+        ``4 (hi - lo)`` bytes.  ``None`` (the default) runs exactly the plain engine.
+
+        ``augment="crop"`` / ``"flip"`` / ``"crop_flip"`` (``data/augment.py``): every client's local epochs train on
+        random crops of the zero-padded images (``augment_padding`` pixels each side) and random horizontal flips,
+        drawn afresh per sample and epoch inside the batch gather.  The key is derived from ``seed`` (the same on every
+        rank) and each client's stream is ``(round_index << 32) | client_id``, so co-hosted clients and successive
+        rounds draw independently and a run is reproducible from its seed.  Shards must be NHWC images.  It is local to
+        each client and combines with every other option.  ``None`` (the default) runs exactly the plain engine."""
+        from ..data.augment import check_augment
+        aug = check_augment(augment, augment_padding)
         if compress not in (None, "topk"):
             raise ValueError("compress must be None or 'topk', got {!r}".format(compress))
         self.topk = TopKConfig(topk_ratio, error_feedback) if compress == "topk" else None
@@ -210,6 +220,8 @@ class FederatedEngine:
         self.hp = dict(lr=lr, batch_size=batch_size, momentum=momentum, weight_decay=weight_decay, prox_mu=prox_mu)
         if adam:
             self.hp.update(optimizer=optimizer, betas=betas, eps=eps)
+        self.aug_hp = (dict(augment=aug.kind, augment_padding=aug.padding, augment_seed=seed)
+                       if aug is not None else None)
         self.n_rounds = 0
         self._last_participants: Optional[List[int]] = None
         self.logical_clients = logical_clients if logical_clients and logical_clients > self.world else 0
@@ -416,11 +428,14 @@ class FederatedEngine:
 
     def _train_client(self, cid: int, X, y, n_epoch: int, first: bool):
         """Local training of client ``cid`` on the replica; with SCAFFOLD, its correction before and its control-variate
-        update after (before any fold resets the replica)."""
+        update after (before any fold resets the replica).  With augmentation, the client's stream of this round."""
+        hp = self.hp
+        if self.aug_hp is not None:
+            hp = dict(hp, augment_stream=(self.n_rounds << 32) | int(cid), **self.aug_hp)
         if self.scaf is None:
-            return self.trainer.run(X, y, n_epoch=n_epoch, return_device=True, **self.hp)
+            return self.trainer.run(X, y, n_epoch=n_epoch, return_device=True, **hp)
         self.scaf.begin_client(cid)
-        ld = self.trainer.run(X, y, n_epoch=n_epoch, return_device=True, corr=self.scaf.corr, **self.hp)
+        ld = self.trainer.run(X, y, n_epoch=n_epoch, return_device=True, corr=self.scaf.corr, **hp)
         self.scaf.end_client(cid, self.arena, n_epoch * self.trainer.last_steps, self.hp["lr"], first=first)
         return ld
 

@@ -28,6 +28,11 @@ steps are those of ``torch.optim.AdamW`` with one parameter group, created fresh
 each run -- the reference builds its optimizer inside every ``train()`` call.  The
 step count ``t`` runs across the epochs of one run.  AdamW takes no momentum,
 Nesterov, FedProx or SCAFFOLD term.
+
+Every trainer also takes ``augment="crop" | "flip" | "crop_flip"`` with ``augment_padding`` (``data/augment.py``):
+each epoch's batches are randomly cropped from the zero-padded image and flipped, fresh draws per sample and epoch.
+``GraphedLocalSGD`` does it inside the epoch's batch gather (``F.gather_augment``); the CPU trainers call the host
+reference per batch.  ``augment_seed`` / ``augment_stream`` pick the draws (``data/augment.py: AugmentStreams``).
 """
 from __future__ import annotations
 
@@ -39,6 +44,7 @@ from typing import Callable, List, Optional, Tuple
 import torch
 from torch import nn
 
+from .data.augment import AugmentStreams, check_augment, check_shard, gather_augment_reference
 from .utils.progress import EpochProgress
 
 
@@ -104,13 +110,18 @@ def run_local_sgd(model: nn.Module, X: torch.Tensor, y: torch.Tensor, *, n_epoch
                   weight_decay: float = 0.0, loss: "str | Callable" = "mse",
                   verbose: bool = False, reshuffle_each_epoch: bool = False,
                   generator: Optional[torch.Generator] = None, prox_mu: float = 0.0, optimizer: str = "sgd",
-                  betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8) -> List[float]:
+                  betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8, augment: Optional[str] = None,
+                  augment_padding: int = 4, augment_seed: Optional[int] = None,
+                  augment_stream: Optional[int] = None) -> List[float]:
     """Portable local SGD; returns the per-epoch mean loss.  ``prox_mu > 0``: FedProx, anchored on the parameters as
     they are on entry -- the global model the worker has just loaded.  ``optimizer="adamw"``: a fresh
-    ``torch.optim.AdamW(lr, betas, eps, weight_decay)`` instead of SGD."""
+    ``torch.optim.AdamW(lr, betas, eps, weight_decay)`` instead of SGD.  ``augment``: random crop / flip of every
+    batch; the model keeps the key and run counter (``AugmentStreams``) across calls."""
     criterion = _loss_fn(loss)
     prox_mu = check_prox_mu(prox_mu)
     adam = check_optimizer(optimizer, momentum, prox_mu=prox_mu)
+    aug = _augment_setup(model.__dict__.setdefault("_augment_streams", AugmentStreams()), X, augment,
+                         augment_padding, augment_seed, augment_stream)
     n = X.shape[0]
     nn.Module.train(model, True)
     params = list(model.parameters())
@@ -127,9 +138,9 @@ def run_local_sgd(model: nn.Module, X: torch.Tensor, y: torch.Tensor, *, n_epoch
         if reshuffle_each_epoch and epoch > 0:
             idxs = torch.randperm(n, generator=generator).to(X.device)
         batch_iter = EpochProgress(epoch, torch.split(idxs, batch_size), verbose=verbose)
-        for batch_idxs in batch_iter:
+        for b, batch_idxs in enumerate(batch_iter):
             optimizer.zero_grad(set_to_none=True)
-            output = model(X[batch_idxs])
+            output = model(_host_batch(X, batch_idxs, aug, epoch, b * batch_size))
             target = y[batch_idxs]
             if output.shape != target.shape and target.dtype.is_floating_point:
                 target = target.reshape(output.shape)  # (N,) vs (N,1) -- quirk 13
@@ -141,6 +152,23 @@ def run_local_sgd(model: nn.Module, X: torch.Tensor, y: torch.Tensor, *, n_epoch
             optimizer.step()
         loss_history.append(batch_iter.loss)
     return loss_history
+
+
+def _augment_setup(streams: AugmentStreams, X, augment, augment_padding, augment_seed, augment_stream):
+    """``(config, key, stream)`` of a run, or None when it does not augment; ``ValueError`` for a bad config or shard."""
+    cfg = check_augment(augment, augment_padding)
+    if cfg is None:
+        return None
+    check_shard(cfg, X)
+    return (cfg,) + streams.next(augment_seed, augment_stream)
+
+
+def _host_batch(X, idx, aug, epoch: int, s0: int):
+    """``X[idx]``, augmented (host reference) for epoch positions ``s0 ..`` when ``aug`` is set."""
+    if aug is None:
+        return X[idx]
+    cfg, key, stream = aug
+    return gather_augment_reference(X, idx, key, stream, epoch, cfg.padding, cfg.crop, cfg.flip, s0=s0)
 
 
 def bn_fold_table(model: nn.Module, arena):
@@ -220,6 +248,12 @@ class GraphedLocalSGD:
     epoch's replay, that epoch's rows are copied into the epoch graph's row buffer, and
     captured step ``s`` reads row ``s``.  The ragged eager step uses the buffer's last row.
 
+    ``run(augment=...)`` gathers the batches through ``F.gather_augment`` instead of ``F.gather_rows``.  Its per-epoch
+    words ``{epoch, stream_lo, stream_hi}`` follow the AdamW rows: one ``[n_epoch, 3]`` device table per run (written
+    on the device, see ``_aug_words``), and before each replay that epoch's row is copied into the graph's word
+    buffer.  The key is a launch argument, so
+    it is part of the epoch graph's key.
+
     ``model`` must already be adopted by a :class:`~baton_b200.parallel.arena.ParamArena`
     (``arena``); the engine is what ``FederatedModule.local_train`` dispatches to
     for CUDA shards (``model._graphed_trainer``).
@@ -250,6 +284,9 @@ class GraphedLocalSGD:
         self.corr = None              # SCAFFOLD: every SGD kernel of the step reads this correction c - c_i
         self.adam = False             # AdamW: every optimizer kernel of the step reads its step row and arena.adam_v
         self._adam_table = (None, None)   # (host key, device [n_epoch * steps, ADAMW_ROW] rows of the run)
+        self._aug = None              # augmentation of the current run: (AugmentConfig, key, stream) or None
+        self._aug_streams = AugmentStreams()
+        self._aug_table = None        # device [epochs, 3] per-epoch words of augmenting runs (see _aug_words)
         self.loss_acc = torch.zeros(2, dtype=torch.float32, device=dev)
         self._graphs = {}           # (n, batch, x_shape, y_shape) -> captured epoch
         self._hyper_host = None
@@ -268,19 +305,26 @@ class GraphedLocalSGD:
         loss = self.bnn.mse_loss(out, yb)
         return loss, torch.stack([loss.detach(), torch.zeros_like(loss.detach())])
 
-    def _gather(self, X, y, idx):
+    def _gather(self, X, y, idx, s0=0, words=None):
+        """``X[idx], y[idx]``; with augmentation on, ``X`` is gathered by ``F.gather_augment`` for epoch positions
+        ``s0 ..`` with the device words ``words``."""
         F = self.F
-        xb = F.gather_rows(X, idx)
+        if self._aug is not None:
+            cfg, key, _ = self._aug
+            xb = F.gather_augment(X, idx, words, key, cfg.padding, crop=cfg.crop, flip=cfg.flip, s0=s0)
+        else:
+            xb = F.gather_rows(X, idx)
         yb = F.gather_rows(y, idx) if y.dtype == torch.int64 and y.dim() == 1 else y.index_select(0, idx)
         return xb, yb
 
-    def _step(self, X, y, idx, batch=None, emit_wire=False, fuse_sgd=True, row=None):
+    def _step(self, X, y, idx, batch=None, emit_wire=False, fuse_sgd=True, row=None, s0=0, words=None):
         """One SGD step on ``X[idx], y[idx]`` (or on the already gathered ``batch``).  ``emit_wire``: last step of
         an epoch -- the optimizer kernel also writes the upload copy for the round-end collective (``self.pack``).
         ``fuse_sgd=False``: no optimizer epilogue in the weight-gradient GEMMs (one optimizer pass over the arena).
-        ``row``: with AdamW, the device row of this step's coefficients (``F.adamw_rows``)."""
+        ``row``: with AdamW, the device row of this step's coefficients (``F.adamw_rows``).  ``s0``, ``words``: the
+        epoch position of ``idx[0]`` and the device words of an augmenting gather."""
         F = self.F
-        xb, yb = batch if batch is not None else self._gather(X, y, idx)
+        xb, yb = batch if batch is not None else self._gather(X, y, idx, s0, words)
         ws = getattr(self.model, "stats_workspace", None)
         if ws is not None and not getattr(self.model, "zeroes_own_workspace", False):
             ws.zero_()
@@ -347,11 +391,25 @@ class GraphedLocalSGD:
             self._adam_table = (key, rows.to(self.device))
         return self._adam_table[1]
 
+    def _aug_words(self, stream: int, n_epoch: int):
+        """Device int32 ``[n_epoch, 3]`` per-epoch words ``{epoch, stream_lo, stream_hi}`` of an augmenting run.  The
+        table persists; a run rewrites the stream columns with two fills, so no host copy (and no host
+        synchronisation) is needed."""
+        t = self._aug_table
+        if t is None or t.shape[0] < n_epoch:
+            t = self._aug_table = torch.zeros(n_epoch, 3, dtype=torch.int32, device=self.device)
+            t[:, 0].copy_(torch.arange(n_epoch, dtype=torch.int32, device=self.device))
+        for col, word in ((1, stream & 0xFFFFFFFF), (2, (stream >> 32) & 0xFFFFFFFF)):
+            t[:, col].fill_(word - (1 << 32) if word >> 31 else word)
+        return t[:n_epoch]
+
     # -------------------------------------------------------------- epoch graph
     def _capture(self, X, y, n_steps, batch_size, rows=None):
         """``rows``: with AdamW, the device row buffer captured step ``s`` reads row ``s`` of (holding the first
-        epoch's rows, which the warm-up steps use too); kept in the returned entry."""
+        epoch's rows, which the warm-up steps use too); kept in the returned entry.  With augmentation on, the
+        gather reads the entry's word buffer ``words``."""
         perm = torch.zeros(n_steps * batch_size, dtype=torch.int64, device=self.device)
+        words = torch.zeros(3, dtype=torch.int32, device=self.device) if self._aug is not None else None
         perm.copy_(torch.arange(n_steps * batch_size, device=self.device) % X.shape[0])
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
@@ -361,7 +419,7 @@ class GraphedLocalSGD:
             snap_i = self.arena.int_arena.clone()
             snap_m = self.arena.momentum.clone() if self.arena.momentum is not None else None
             for _ in range(2):
-                self._step(X, y, perm[:batch_size], row=rows[0] if rows is not None else None)
+                self._step(X, y, perm[:batch_size], row=rows[0] if rows is not None else None, words=words)
         torch.cuda.current_stream(self.device).wait_stream(side)
         torch.cuda.synchronize(self.device)
         from .ops._ext import total_launches
@@ -372,7 +430,7 @@ class GraphedLocalSGD:
         def body():
             # the epoch's batches are gathered by ONE launch pair (a permuted copy of the shard, 25 MB for the
             # flagship config) instead of two latency-bound gathers at the head of every step
-            Xp, yp = self._gather(X, y, perm)
+            Xp, yp = self._gather(X, y, perm, 0, words)
             for s in range(n_steps):
                 self._step(X, y, None, batch=(Xp[s * batch_size:(s + 1) * batch_size],
                                               yp[s * batch_size:(s + 1) * batch_size]),
@@ -423,7 +481,7 @@ class GraphedLocalSGD:
         self.arena.grad.zero_()
         self.arena.sync_shadow()
         self.loss_acc.zero_()
-        return {"graph": graph, "graph2": graph2, "perm": perm, "X": X, "y": y, "rows": rows}
+        return {"graph": graph, "graph2": graph2, "perm": perm, "X": X, "y": y, "rows": rows, "words": words}
 
     # -------------------------------------------------------------- evaluation
     def _eval_pass(self, X, y, batch_size, explicit):
@@ -513,11 +571,15 @@ class GraphedLocalSGD:
     def run(self, X, y, n_epoch: int = 1, lr: float = 0.001, batch_size: int = 32, momentum: float = 0.0,
             weight_decay: float = 0.0, reshuffle_each_epoch: bool = False, return_device: bool = False,
             prox_mu: float = 0.0, corr: Optional[torch.Tensor] = None, optimizer: str = "sgd",
-            betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8, **_ignored):
+            betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8, augment: Optional[str] = None,
+            augment_padding: int = 4, augment_seed: Optional[int] = None, augment_stream: Optional[int] = None,
+            **_ignored):
         """``prox_mu > 0``: FedProx toward ``arena.global_w``, the global model the round started from.  ``corr``:
         SCAFFOLD's correction ``c - c_i`` (fp32 device buffer of ``arena.n_param`` elements), added to every step's
         gradient; it is read at replay, so the caller may rewrite it between runs.  ``optimizer="adamw"``: the steps of
-        a fresh ``torch.optim.AdamW(lr, betas, eps, weight_decay)`` instead of SGD."""
+        a fresh ``torch.optim.AdamW(lr, betas, eps, weight_decay)`` instead of SGD.  ``augment``: random crop / flip
+        in the batch gather (``data/augment.py``); ``augment_seed`` (None: a random key per trainer) and
+        ``augment_stream`` (None: this trainer's count of augmenting runs) pick the draws."""
         assert X.is_cuda, "GraphedLocalSGD needs a device-resident shard"
         prox_mu = check_prox_mu(prox_mu)
         if prox_mu > 0 and self.arena.global_w is None:
@@ -526,6 +588,7 @@ class GraphedLocalSGD:
         self.adam = check_optimizer(optimizer, momentum, self.nesterov, prox_mu, corr)
         if self.adam:
             betas, eps = check_adamw(betas, eps)
+        self._aug = _augment_setup(self._aug_streams, X, augment, augment_padding, augment_seed, augment_stream)
         nn.Module.train(self.model, True)
         n = X.shape[0]
         batch_size = min(batch_size, n)
@@ -541,10 +604,12 @@ class GraphedLocalSGD:
             self.arena.adam_v = torch.zeros_like(self.arena.grad)
         # every step of the run, t = 1 .. n_epoch * steps; the first ignores the stored moments (a fresh optimizer)
         table = self._adam_rows(lr, betas, eps, weight_decay, n_epoch, steps) if self.adam else None
+        aug_words = self._aug_words(self._aug[2], n_epoch) if self._aug is not None else None
+        aug_key = self._aug[:2] if self._aug is not None else None
         # the anchor and correction pointers are baked into the captured launches; the coefficient is read from `hyper`
         # at replay
         key = (n, batch_size, tuple(X.shape[1:]), tuple(y.shape[1:]), X.data_ptr(), y.data_ptr(), bool(momentum),
-               self.prox, corr.data_ptr() if corr is not None else None, self.adam)
+               self.prox, corr.data_ptr() if corr is not None else None, self.adam, aug_key)
         epoch_losses = torch.zeros(n_epoch, 2, dtype=torch.float32, device=self.device)
         if self.use_graph:
             ent = self._graphs.get(key)
@@ -558,6 +623,8 @@ class GraphedLocalSGD:
                 ent["perm"].copy_(perm_full[: n_steps * batch_size])
                 if self.adam:
                     ent["rows"].copy_(table[e * steps:(e + 1) * steps])
+                if aug_words is not None:
+                    ent["words"].copy_(aug_words[e])
                 self.loss_acc.zero_()
                 ent["graph"].replay()
                 if ent.get("graph2") is not None:
@@ -566,7 +633,8 @@ class GraphedLocalSGD:
                 if tail:
                     with torch.enable_grad():
                         self._step(X, y, perm_full[n_steps * batch_size:], fuse_sgd=False,
-                                   row=ent["rows"][n_steps] if self.adam else None)
+                                   row=ent["rows"][n_steps] if self.adam else None, s0=n_steps * batch_size,
+                                   words=ent["words"])
                 epoch_losses[e].copy_(self.loss_acc)
         else:
             perm_full = torch.randperm(n, device=self.device)
@@ -576,7 +644,8 @@ class GraphedLocalSGD:
                 self.loss_acc.zero_()
                 for s, idx in enumerate(torch.split(perm_full, batch_size)):
                     with torch.enable_grad():
-                        self._step(X, y, idx, row=table[e * steps + s] if self.adam else None)
+                        self._step(X, y, idx, row=table[e * steps + s] if self.adam else None, s0=s * batch_size,
+                                   words=aug_words[e] if aug_words is not None else None)
                 epoch_losses[e].copy_(self.loss_acc)
         self.last_steps = steps
         self.last_had_tail_step = bool(tail)        # a ragged eager step ran after the graph: its SGD did not emit the wire
@@ -602,18 +671,23 @@ class PortableLocalSGD:
         self.kernels_per_epoch = 0
         self.n_kernels_per_step = 0
         self.last_stats = {}
+        self._aug_streams = AugmentStreams()
 
     def run(self, X, y, n_epoch: int = 1, lr: float = 0.001, batch_size: int = 32, momentum: float = 0.0,
             weight_decay: float = 0.0, reshuffle_each_epoch: bool = False, return_device: bool = False,
             prox_mu: float = 0.0, corr: Optional[torch.Tensor] = None, optimizer: str = "sgd",
-            betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8, **_ignored):
+            betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8, augment: Optional[str] = None,
+            augment_padding: int = 4, augment_seed: Optional[int] = None, augment_stream: Optional[int] = None,
+            **_ignored):
         """``prox_mu > 0``: FedProx toward ``arena.global_w``, the global model the round started from.  ``corr``:
         SCAFFOLD's correction ``c - c_i`` (fp32, indexed like the arena's parameters), added to every gradient.
-        ``optimizer="adamw"``: a fresh ``torch.optim.AdamW(lr, betas, eps, weight_decay)`` instead of SGD."""
+        ``optimizer="adamw"``: a fresh ``torch.optim.AdamW(lr, betas, eps, weight_decay)`` instead of SGD.
+        ``augment``: as in :meth:`GraphedLocalSGD.run`, through the host reference."""
         criterion = _loss_fn(self.loss_kind)
         prox_mu = check_prox_mu(prox_mu)
         _check_corr(corr, self.arena)
         adam = check_optimizer(optimizer, momentum, prox_mu=prox_mu, corr=corr)
+        aug = _augment_setup(self._aug_streams, X, augment, augment_padding, augment_seed, augment_stream)
         n = X.shape[0]
         batch_size = min(batch_size, n)
         nn.Module.train(self.model, True)
@@ -638,9 +712,9 @@ class PortableLocalSGD:
                 perm = torch.randperm(n)
             batches = torch.split(perm, batch_size)
             steps = len(batches)
-            for idx in batches:
+            for b, idx in enumerate(batches):
                 opt.zero_grad(set_to_none=True)
-                pred = self.model(X[idx])
+                pred = self.model(_host_batch(X, idx, aug, e, b * batch_size))
                 tgt = y[idx]
                 if pred.shape != tgt.shape and tgt.dtype.is_floating_point:
                     tgt = tgt.reshape(pred.shape)
