@@ -34,6 +34,9 @@ class FederationConfig:
     adam_eps: float = 1e-8
     augment: str = "none"              # local-training augmentation: none | crop | flip | crop_flip (NHWC image shards)
     augment_padding: int = 4           # zero padding of the random crop, pixels on each side
+    mix: str = "none"                  # batch mixing: none | mixup | cutmix | mixup_cutmix (NHWC images, cross-entropy)
+    mix_alpha: float = 1.0             # lambda ~ Beta(mix_alpha, mix_alpha), one per batch
+    label_smoothing: float = 0.0       # soft-target smoothing eps in [0, 1) of the training cross-entropy
     dp_clip: float = 0.0               # DP-FedAvg: L2 clip norm of a client's update (0: DP off)
     dp_noise_multiplier: float = 0.0   # DP-FedAvg: noise std on the sum of clipped updates, in units of dp_clip
     dp_delta: float = 1e-5             # DP-FedAvg: delta of the (epsilon, delta) the manager reports
@@ -64,6 +67,8 @@ class FederationConfig:
         check_adamw((self.adam_beta1, self.adam_beta2), self.adam_eps)
         from .data.augment import check_augment
         check_augment(self.augment, self.augment_padding)
+        from .data.mix import check_mix
+        check_mix(self.mix, self.mix_alpha, self.label_smoothing)
         from .parallel.dp import check_dp
         check_dp(self.dp_clip, self.dp_noise_multiplier)
         if not (0.0 < float(self.dp_delta) < 1.0):
@@ -89,6 +94,10 @@ class FederationConfig:
             kw.update(optimizer=self.optimizer, betas=(self.adam_beta1, self.adam_beta2), eps=self.adam_eps)
         if self.augment != "none":
             kw.update(augment=self.augment, augment_padding=self.augment_padding)
+        if self.mix != "none":
+            kw.update(mix=self.mix, mix_alpha=self.mix_alpha)
+        if self.label_smoothing != 0.0:
+            kw.update(label_smoothing=self.label_smoothing)
         return kw
 
     def dp_config(self):

@@ -499,6 +499,35 @@ void gather_augment(const at::Tensor& src, const at::Tensor& idx, at::Tensor dst
         "gather_augment");
 }
 
+void gather_mix(const at::Tensor& src, const at::Tensor& idx, at::Tensor dst, const at::Tensor& words,
+                const at::Tensor& mix_rows, int64_t batch, int64_t key, int64_t padding, bool crop, bool flip,
+                int64_t s0) {
+  CHECK_CUDA(src);
+  CHECK_CUDA(idx);
+  CHECK_CUDA(dst);
+  CHECK_CUDA(words);
+  CHECK_CUDA(mix_rows);
+  TORCH_CHECK(src.dim() == 4 && src.is_contiguous() && dst.is_contiguous() && dst.scalar_type() == src.scalar_type(),
+              "gather_mix: contiguous NHWC src and dst of one dtype");
+  TORCH_CHECK(idx.scalar_type() == at::kLong && idx.is_contiguous(), "gather_mix: contiguous int64 idx");
+  TORCH_CHECK(words.scalar_type() == at::kInt && words.is_contiguous() && words.numel() >= 3,
+              "gather_mix: words = int32 {epoch, stream_lo, stream_hi}");
+  TORCH_CHECK(batch >= 1 && s0 >= 0 && s0 % batch == 0, "gather_mix: the call must start on a batch boundary");
+  TORCH_CHECK(mix_rows.scalar_type() == at::kInt && mix_rows.is_contiguous() &&
+                  mix_rows.numel() >= ((s0 + idx.numel() + batch - 1) / batch) * 8,
+              "gather_mix: mix_rows = int32 [n_batches, 8] covering every batch of the call");
+  TORCH_CHECK(dst.numel() == idx.numel() * (src.numel() / std::max<int64_t>(1, src.size(0))),
+              "gather_mix: dst holds one image per index");
+  const c10::cuda::CUDAGuard guard(src.device());
+  check(b200_gather_mix(src.data_ptr(), reinterpret_cast<const long long*>(idx.data_ptr<int64_t>()), dst.data_ptr(),
+                        reinterpret_cast<const unsigned*>(words.data_ptr<int32_t>()), mix_rows.data_ptr<int32_t>(),
+                        idx.numel(), s0, static_cast<int>(batch), static_cast<unsigned long long>(key),
+                        static_cast<int>(padding), crop ? 1 : 0, flip ? 1 : 0, static_cast<int>(src.size(1)),
+                        static_cast<int>(src.size(2)), static_cast<int>(src.size(3)),
+                        static_cast<int>(src.element_size()), src.scalar_type() == at::kHalf ? 1 : 0, cur_stream()),
+        "gather_mix");
+}
+
 void colsum(const at::Tensor& x, at::Tensor out, int64_t rows, int64_t cols, bool accumulate) {
   CHECK_CUDA(x);
   const c10::cuda::CUDAGuard guard(x.device());
@@ -1136,6 +1165,44 @@ void softmax_xent(const at::Tensor& logits, const at::Tensor& target, const std:
                           static_cast<float>(grad_scale), cur_stream()),
         "softmax_xent");
 }
+// soft targets: mix_row (nullable) is the step's int32 mix row, eps the label smoothing
+void softmax_xent_soft(const at::Tensor& logits, const at::Tensor& target, const std::optional<at::Tensor>& dlogits,
+                       at::Tensor loss_acc, int64_t rows, int64_t C, int64_t ld, double grad_scale,
+                       const std::optional<at::Tensor>& mix_row, double eps) {
+  CHECK_CUDA(logits);
+  TORCH_CHECK(target.scalar_type() == at::kLong && target.numel() >= rows && loss_acc.scalar_type() == at::kFloat &&
+              loss_acc.numel() >= 2);
+  TORCH_CHECK(!mix_row.has_value() || (mix_row->scalar_type() == at::kInt && mix_row->numel() >= 2));
+  const c10::cuda::CUDAGuard guard(logits.device());
+  const int in32 = logits.scalar_type() == at::kFloat;
+  const int out32 = dlogits.has_value() && dlogits->defined() && dlogits->scalar_type() == at::kFloat;
+  check(b200_softmax_xent_soft(logits.data_ptr(), in32, reinterpret_cast<const long long*>(target.data_ptr<int64_t>()),
+                               opt_ptr<void>(dlogits), out32, loss_acc.data_ptr<float>(), rows, C, ld,
+                               static_cast<float>(grad_scale), opt_ptr<const int>(mix_row), static_cast<float>(eps),
+                               cur_stream()),
+        "softmax_xent_soft");
+}
+bool linear_xent_head_soft(const at::Tensor& x, const at::Tensor& w, const std::optional<at::Tensor>& bias,
+                           const at::Tensor& target, const std::optional<at::Tensor>& dx, at::Tensor dw,
+                           const std::optional<at::Tensor>& db, at::Tensor loss_acc, double grad_scale,
+                           const std::optional<at::Tensor>& mix_row, double eps) {
+  CHECK_CUDA(x);
+  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16 && x.dim() == 2 && w.dim() == 2 &&
+              x.is_contiguous() && w.is_contiguous() && x.size(1) == w.size(1));
+  TORCH_CHECK(target.scalar_type() == at::kLong && target.numel() >= x.size(0) && dw.scalar_type() == at::kFloat &&
+              dw.is_contiguous() && dw.numel() == w.numel() && loss_acc.scalar_type() == at::kFloat &&
+              loss_acc.numel() >= 2);
+  TORCH_CHECK(!mix_row.has_value() || (mix_row->scalar_type() == at::kInt && mix_row->numel() >= 2));
+  const c10::cuda::CUDAGuard guard(x.device());
+  const int rc = b200_linear_xent_head_soft(
+      x.data_ptr(), w.data_ptr(), opt_ptr<const float>(bias), reinterpret_cast<const long long*>(target.data_ptr<int64_t>()),
+      opt_ptr<void>(dx), dw.data_ptr<float>(), opt_ptr<float>(db), loss_acc.data_ptr<float>(), static_cast<int>(x.size(0)),
+      static_cast<int>(x.size(1)), static_cast<int>(w.size(0)), static_cast<float>(grad_scale), opt_ptr<const int>(mix_row),
+      static_cast<float>(eps), cur_stream());
+  if (rc == -2) return false;
+  check(rc, "linear_xent_head_soft");
+  return true;
+}
 // False: shape not supported by the one-launch head (more than 32 classes, K % 8, ...)
 bool linear_xent_head(const at::Tensor& x, const at::Tensor& w, const std::optional<at::Tensor>& bias, const at::Tensor& target,
                       const std::optional<at::Tensor>& dx, at::Tensor dw, const std::optional<at::Tensor>& db,
@@ -1216,6 +1283,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("cast", &cast);
   m.def("gather_rows", &gather_rows);
   m.def("gather_augment", &gather_augment);
+  m.def("gather_mix", &gather_mix);
   m.def("colsum", &colsum);
   m.def("add_bf16", &add_bf16);
   m.def("relu_bwd", &relu_bwd);
@@ -1258,7 +1326,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("softmax_bwd", &softmax_bwd);
   m.def("softmax_xent", &softmax_xent);
   m.def("mse", &mse);
+  m.def("softmax_xent_soft", &softmax_xent_soft);
   m.def("linear_xent_head", &linear_xent_head);
+  m.def("linear_xent_head_soft", &linear_xent_head_soft);
   m.def("linear_xent_eval", &linear_xent_eval);
   m.def("bn_fold_eval", &bn_fold_eval);
 }

@@ -3,6 +3,8 @@
 // (bias gradients), ReLU / GELU pieces.  All use 16-byte vectors and grid-stride loops sized to
 // the device's SMs x a few resident CTAs.
 #define B200_TU_TAG 8
+#include <cuda_fp16.h>
+
 #include "dp.cuh"
 #include "launch.h"
 #include "pdl.cuh"
@@ -551,6 +553,134 @@ gather_augment_kernel(const uint8_t* __restrict__ src, const long long* __restri
   }
 }
 
+// ------------------------------------------------------------------ mixing batch gather (mixup / CutMix)
+// gather_augment_kernel, then each output image mixed with its batch partner (torchvision's batch.roll(1, 0)): within
+// the batch of `batch` positions holding s (the call covers whole batches, s0 % batch == 0; the last may be ragged, of L
+// rows), row j pairs with (j - 1 + L) % L.  Both images are augmented with their own draws first.  The batch's mix row
+// rows[(s0 + s) / batch] (data/mix.py) holds lam, lam1 (fp32 bits), the kind and the box y0, y1, x0, x1:
+//   mixup:  out = round(fp32(fp32(a lam) + fp32(b lam1)))   (mul_rn / add_rn: no contracted FMA)
+//   CutMix: out = b inside the box, a outside (data movement only)
+// A work item stages its own and its partner's source rows into two halves of shared memory (the partner's only when
+// the tile meets the box, for CutMix), then composes as gather_augment_kernel does.
+constexpr int MIX_ROW = 8;
+constexpr int MIX_CUTMIX = 1;
+
+// fp32 product and sum rounded to nearest, each on its own and without flushing subnormals (the build's fast-math flag
+// turns __fmul_rn / __fadd_rn into their .ftz forms; torch on the host keeps subnormals)
+__device__ __forceinline__ float mul_rn(float a, float b) {
+  float r;
+  asm("mul.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+__device__ __forceinline__ float add_rn(float a, float b) {
+  float r;
+  asm("add.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+template <int ES>
+__device__ __forceinline__ uint32_t mix_elem(uint32_t a, uint32_t b, float lam, float lam1, int fp16) {
+  if constexpr (ES == 4) {
+    return __float_as_uint(add_rn(mul_rn(__uint_as_float(a), lam), mul_rn(__uint_as_float(b), lam1)));
+  } else {
+    if (fp16) {
+      const float f = add_rn(mul_rn(__half2float(__ushort_as_half(static_cast<unsigned short>(a))), lam),
+                                mul_rn(__half2float(__ushort_as_half(static_cast<unsigned short>(b))), lam1));
+      return __half_as_ushort(__float2half_rn(f));
+    }
+    const float f = add_rn(mul_rn(__bfloat162float(__ushort_as_bfloat16(static_cast<unsigned short>(a))), lam),
+                              mul_rn(__bfloat162float(__ushort_as_bfloat16(static_cast<unsigned short>(b))), lam1));
+    return __bfloat16_as_ushort(__float2bfloat16_rn(f));
+  }
+}
+
+template <int ES, int V>
+__global__ void __launch_bounds__(AUG_THREADS)
+gather_mix_kernel(const uint8_t* __restrict__ src, const long long* __restrict__ idx, uint8_t* __restrict__ dst,
+                  const uint32_t* __restrict__ words, const int* __restrict__ mix_rows, long long n_rows, long long s0,
+                  int batch, uint2 key, int pad, int crop, int flip, int fp16, int H, int W, int C, int rows_per_tile,
+                  int half_bytes) {
+  using E = typename AugVec<ES>::T;
+  using Vt = typename AugVec<V>::T;
+  constexpr int EPV = V / ES;
+  extern __shared__ uint4 aug_smem[];
+  const E* sa = reinterpret_cast<const E*>(aug_smem);
+  const E* sb = reinterpret_cast<const E*>(reinterpret_cast<const uint8_t*>(aug_smem) + half_bytes);
+  griddep_launch_dependents();
+  griddep_wait();
+  const uint32_t epoch = words[0], st_lo = words[1], st_hi = words[2];
+  const int row_e = W * C;
+  const long long row_bytes = static_cast<long long>(row_e) * ES, img_bytes = row_bytes * H;
+  const int tiles = (H + rows_per_tile - 1) / rows_per_tile;
+  const int items = static_cast<int>(n_rows) * tiles;     // < 2^31 (checked at launch)
+  const uint32_t span = 2u * static_cast<uint32_t>(pad) + 1u;
+  for (int it = blockIdx.x; it < items; it += gridDim.x) {
+    const int s = it / tiles;
+    const int h0 = (it - s * tiles) * rows_per_tile;
+    const int hn = min(rows_per_tile, H - h0);
+    const int b0 = s / batch * batch;                       // first row of s's batch in this call
+    const int L = static_cast<int>(min(static_cast<long long>(batch), n_rows - b0));
+    const int sp = b0 + (s == b0 ? L - 1 : s - b0 - 1);     // the partner
+    const int* mr = mix_rows + (s0 + s) / batch * MIX_ROW;
+    const float lam = __int_as_float(mr[0]), lam1 = __int_as_float(mr[1]);
+    const bool cut = mr[2] == MIX_CUTMIX;
+    const int y0 = mr[3], y1 = mr[4], x0 = mr[5], x1 = mr[6];
+    const bool need_b = !cut || (y0 < h0 + hn && y1 > h0 && x1 > x0);
+    const uint4 x = philox4x32_10(make_uint4(static_cast<uint32_t>(s0 + s), epoch, st_lo, st_hi), key);
+    const uint4 xp = philox4x32_10(make_uint4(static_cast<uint32_t>(s0 + sp), epoch, st_lo, st_hi), key);
+    const int dy = crop ? static_cast<int>(x.x % span) - pad : 0;
+    const int dx = crop ? static_cast<int>(x.y % span) - pad : 0;
+    const bool fl = flip && (x.z & 1u);
+    const int dyb = crop ? static_cast<int>(xp.x % span) - pad : 0;
+    const int dxb = crop ? static_cast<int>(xp.y % span) - pad : 0;
+    const bool flb = flip && (xp.z & 1u);
+    const int lo = max(0, h0 + dy), hi = min(H, h0 + hn + dy);        // source rows of the own image
+    const int lob = max(0, h0 + dyb), hib = min(H, h0 + hn + dyb);    // and of the partner
+    if (hi > lo) {
+      const Vt* g = reinterpret_cast<const Vt*>(src + idx[s] * img_bytes + lo * row_bytes);
+      Vt* d = reinterpret_cast<Vt*>(aug_smem);
+      const int nv = static_cast<int>((hi - lo) * row_bytes / V);
+      for (int i = threadIdx.x; i < nv; i += AUG_THREADS) d[i] = __ldg(g + i);
+    }
+    if (need_b && hib > lob) {
+      const Vt* g = reinterpret_cast<const Vt*>(src + idx[sp] * img_bytes + lob * row_bytes);
+      Vt* d = reinterpret_cast<Vt*>(reinterpret_cast<uint8_t*>(aug_smem) + half_bytes);
+      const int nv = static_cast<int>((hib - lob) * row_bytes / V);
+      for (int i = threadIdx.x; i < nv; i += AUG_THREADS) d[i] = __ldg(g + i);
+    }
+    __syncthreads();
+    Vt* out = reinterpret_cast<Vt*>(dst + static_cast<long long>(s) * img_bytes + h0 * row_bytes);
+    const int out_v = static_cast<int>(hn * row_bytes / V);
+    for (int i = threadIdx.x; i < out_v; i += AUG_THREADS) {
+      const int e = i * EPV;
+      int r = e / row_e;
+      int w = (e - r * row_e) / C;
+      int c = e - r * row_e - w * C;
+      uint32_t wd[(V + 3) / 4] = {};
+#pragma unroll
+      for (int k = 0; k < EPV; ++k) {
+        const int oh = h0 + r;
+        const int sh = oh + dy, sw = (fl ? W - 1 - w : w) + dx;
+        uint32_t val = (sh >= lo && sh < hi && sw >= 0 && sw < W) ? static_cast<uint32_t>(sa[(sh - lo) * row_e + sw * C + c]) : 0u;
+        if (need_b && (!cut || (oh >= y0 && oh < y1 && w >= x0 && w < x1))) {
+          const int shb = oh + dyb, swb = (flb ? W - 1 - w : w) + dxb;
+          const uint32_t vb =
+              (shb >= lob && shb < hib && swb >= 0 && swb < W) ? static_cast<uint32_t>(sb[(shb - lob) * row_e + swb * C + c]) : 0u;
+          val = cut ? vb : mix_elem<ES>(val, vb, lam, lam1, fp16);
+        }
+        wd[k * ES / 4] |= val << (8 * ((k * ES) & 3));
+        if (++c == C) {
+          c = 0;
+          if (++w == W) { w = 0; ++r; }
+        }
+      }
+      if constexpr (V == 16) out[i] = make_uint4(wd[0], wd[1], wd[2], wd[3]);
+      else if constexpr (V == 8) out[i] = make_uint2(wd[0], wd[1]);
+      else out[i] = static_cast<Vt>(wd[0]);
+    }
+    __syncthreads();
+  }
+}
+
 __global__ void gather_i64_kernel(const long long* __restrict__ src, const long long* __restrict__ idx,
                                   long long* __restrict__ dst, long long n) {
   griddep_launch_dependents();
@@ -895,20 +1025,28 @@ static void launch_gather_augment(const void* src, const long long* idx, void* d
   launch_pdl(gather_augment_kernel<ES, V>, grid, AUG_THREADS, smem, stream, static_cast<const uint8_t*>(src), idx,
              static_cast<uint8_t*>(dst), words, n_rows, s0, key, pad, crop, flip, H, W, C, rows_per_tile);
 }
-extern "C" int b200_gather_augment(const void* src, const long long* idx, void* dst, const unsigned* words,
-                                   long long n_rows, long long s0, unsigned long long key, int pad, int crop, int flip,
-                                   int H, int W, int C, int elem_bytes, cudaStream_t stream) {
-  if (n_rows <= 0) return 0;
-  if ((elem_bytes != 2 && elem_bytes != 4) || H < 1 || W < 1 || C < 1 || pad < 0) return -2;
+// Vector width and rows per tile of an augmenting gather; false when the shape or the addresses are not supported.
+static bool gather_augment_plan(const void* src, const void* dst, long long n_rows, int H, int W, int C, int elem_bytes,
+                                int pad, int* vec, int* rows_per_tile) {
+  if ((elem_bytes != 2 && elem_bytes != 4) || H < 1 || W < 1 || C < 1 || pad < 0) return false;
   const long long row_bytes = static_cast<long long>(W) * C * elem_bytes;
-  if (row_bytes > AUG_MAX_ROW_BYTES || n_rows * H >= (1LL << 31)) return -2;
+  if (row_bytes > AUG_MAX_ROW_BYTES || n_rows * H >= (1LL << 31)) return false;
   // widest vector dividing the row pitch and both base addresses: every staged range and output tile starts on a row
   int v = 16;
   while (v > elem_bytes && (row_bytes % v || reinterpret_cast<uintptr_t>(src) % v || reinterpret_cast<uintptr_t>(dst) % v))
     v >>= 1;
-  if (row_bytes % v || reinterpret_cast<uintptr_t>(src) % v || reinterpret_cast<uintptr_t>(dst) % v) return -2;
+  if (row_bytes % v || reinterpret_cast<uintptr_t>(src) % v || reinterpret_cast<uintptr_t>(dst) % v) return false;
   long long r = AUG_TILE_BYTES / row_bytes;
-  const int rows_per_tile = static_cast<int>(r < 1 ? 1 : (r > H ? H : r));
+  *vec = v;
+  *rows_per_tile = static_cast<int>(r < 1 ? 1 : (r > H ? H : r));
+  return true;
+}
+extern "C" int b200_gather_augment(const void* src, const long long* idx, void* dst, const unsigned* words,
+                                   long long n_rows, long long s0, unsigned long long key, int pad, int crop, int flip,
+                                   int H, int W, int C, int elem_bytes, cudaStream_t stream) {
+  if (n_rows <= 0) return 0;
+  int v, rows_per_tile;
+  if (!gather_augment_plan(src, dst, n_rows, H, W, C, elem_bytes, pad, &v, &rows_per_tile)) return -2;
   const uint2 k = make_uint2(static_cast<uint32_t>(key), static_cast<uint32_t>(key >> 32));
   const uint32_t* w = reinterpret_cast<const uint32_t*>(words);
 #define B200_AUG(ES, V)                                                                                               \
@@ -924,6 +1062,54 @@ extern "C" int b200_gather_augment(const void* src, const long long* idx, void* 
     else B200_AUG(4, 4);
   }
 #undef B200_AUG
+  RET_LAST();
+}
+template <int ES, int V>
+static cudaError_t launch_gather_mix(const void* src, const long long* idx, void* dst, const uint32_t* words,
+                                     const int* rows, long long n_rows, long long s0, int batch, uint2 key, int pad,
+                                     int crop, int flip, int fp16, int H, int W, int C, int rows_per_tile,
+                                     cudaStream_t stream) {
+  const long long row_bytes = static_cast<long long>(W) * C * ES;
+  const int half = static_cast<int>((rows_per_tile * row_bytes + 15) / 16 * 16);
+  const size_t smem = 2 * static_cast<size_t>(half);
+  static size_t configured = 0;              // two images of up to AUG_MAX_ROW_BYTES rows may exceed the default 48 KB
+  if (smem > 48 * 1024 && smem > configured) {
+    const cudaError_t e = cudaFuncSetAttribute(gather_mix_kernel<ES, V>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               static_cast<int>(smem));
+    if (e != cudaSuccess) return e;
+    configured = smem;
+  }
+  const long long items = n_rows * ((H + rows_per_tile - 1) / rows_per_tile);
+  const int grid = static_cast<int>(items < device_sm_count() * 8LL ? items : device_sm_count() * 8LL);
+  return launch_pdl(gather_mix_kernel<ES, V>, grid, AUG_THREADS, smem, stream, static_cast<const uint8_t*>(src), idx,
+                    static_cast<uint8_t*>(dst), words, rows, n_rows, s0, batch, key, pad, crop, flip, fp16, H, W, C,
+                    rows_per_tile, half);
+}
+extern "C" int b200_gather_mix(const void* src, const long long* idx, void* dst, const unsigned* words, const int* rows,
+                               long long n_rows, long long s0, int batch, unsigned long long key, int pad, int crop,
+                               int flip, int H, int W, int C, int elem_bytes, int fp16, cudaStream_t stream) {
+  if (n_rows <= 0) return 0;
+  if (batch < 1 || s0 < 0 || s0 % batch) return -2;
+  int v, rows_per_tile;
+  if (!gather_augment_plan(src, dst, n_rows, H, W, C, elem_bytes, pad, &v, &rows_per_tile)) return -2;
+  const uint2 k = make_uint2(static_cast<uint32_t>(key), static_cast<uint32_t>(key >> 32));
+  const uint32_t* w = reinterpret_cast<const uint32_t*>(words);
+  cudaError_t e;
+#define B200_MIX(ES, V)                                                                                               \
+  e = launch_gather_mix<ES, V>(src, idx, dst, w, rows, n_rows, s0, batch, k, pad, crop, flip, fp16, H, W, C,           \
+                               rows_per_tile, stream)
+  if (elem_bytes == 2) {
+    if (v == 16) B200_MIX(2, 16);
+    else if (v == 8) B200_MIX(2, 8);
+    else if (v == 4) B200_MIX(2, 4);
+    else B200_MIX(2, 2);
+  } else {
+    if (v == 16) B200_MIX(4, 16);
+    else if (v == 8) B200_MIX(4, 8);
+    else B200_MIX(4, 4);
+  }
+#undef B200_MIX
+  if (e != cudaSuccess) return static_cast<int>(e);
   RET_LAST();
 }
 extern "C" int b200_gather_rows_i64(const long long* src, const long long* idx, long long* dst, long long n,

@@ -123,6 +123,13 @@ int b200_gather_rows_i64(const long long* src, const long long* idx, long long* 
 int b200_gather_augment(const void* src, const long long* idx, void* dst, const unsigned* words, long long n_rows,
                         long long s0, unsigned long long key, int pad, int crop, int flip, int H, int W, int C,
                         int elem_bytes, cudaStream_t stream);
+// gather_augment, then each image mixed with its batch partner: within every batch of `batch` positions (the last one
+// may be shorter), position j pairs with j - 1 (the first with the last); both are augmented with their own draws, then
+// mixed under the batch's mix row rows[(s0 + s) / batch] (8 int32: lam, lam1 as fp32 bits, kind 0 mixup / 1 CutMix,
+// box y0, y1, x0, x1).  s0 % batch == 0.  elem_bytes 2 (fp16 = 1 for half, else bf16) or 4 (fp32)
+int b200_gather_mix(const void* src, const long long* idx, void* dst, const unsigned* words, const int* rows,
+                    long long n_rows, long long s0, int batch, unsigned long long key, int pad, int crop, int flip,
+                    int H, int W, int C, int elem_bytes, int fp16, cudaStream_t stream);
 int b200_colsum(const void* x, float* out, long long rows, int cols, int accumulate, cudaStream_t stream);
 int b200_add_bf16(const void* a, const void* b, void* out, long long n, int relu, cudaStream_t stream);
 int b200_relu_bwd_bf16(const void* y, const void* dy, void* dx, long long n, cudaStream_t stream);
@@ -349,6 +356,14 @@ int b200_softmax_xent(const void* logits, int logits_fp32, const long long* targ
 int b200_linear_xent_head(const void* x, const void* w, const float* bias, const long long* target, void* dx, float* dw,
                           float* db, float* loss_acc, float* logits_out, int rows, int K, int NC, float grad_scale,
                           cudaStream_t stream);
+// soft-target forms (mixup / CutMix / label smoothing, data/mix.py): target of row r is (1 - eps)(lam 1[target[r]] +
+// lam1 1[target[r - 1 mod rows]]) + eps / C with lam, lam1 the fp32 words 0, 1 of mix_row (nullable: lam = 1, lam1 = 0)
+int b200_softmax_xent_soft(const void* logits, int logits_fp32, const long long* target, void* dlogits, int dl_fp32,
+                           float* loss_acc, long long rows, int C, long long ld, float grad_scale, const int* mix_row,
+                           float eps, cudaStream_t stream);
+int b200_linear_xent_head_soft(const void* x, const void* w, const float* bias, const long long* target, void* dx,
+                               float* dw, float* db, float* loss_acc, int rows, int K, int NC, float grad_scale,
+                               const int* mix_row, float eps, cudaStream_t stream);
 // forward-only head (evaluation): loss_acc[0] += sum of the row losses, loss_acc[1] += #correct
 int b200_linear_xent_eval(const void* x, const void* w, const float* bias, const long long* target, float* loss_acc,
                           float* logits_out, int rows, int K, int NC, cudaStream_t stream);

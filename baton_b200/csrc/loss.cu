@@ -27,12 +27,37 @@ __device__ __forceinline__ float load_logit(const void* p, long long i) {
     return __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p)[i]);
 }
 
+// Soft targets (mixup / CutMix / label smoothing): the target of row r is
+//   q = (1 - eps) (lam 1[a] + lam1 1[b]) + eps / C,   a = target[r], b = target[(r - 1 + rows) % rows]
+// (the partner of the batch rolled by one, as the mixing gather pairs the images), lam / lam1 the fp32 bit patterns in
+// words 0 / 1 of the step's mix row (data/mix.py); no mix row: lam = 1, lam1 = 0, b = a (plain label smoothing).
+// loss_row = logsumexp(z) - sum_c q_c z_c, dz = (softmax(z) - q) * grad_scale, #correct += lam [argmax = a] + lam1
+// [argmax = b].
+struct SoftTarget {
+  float wa, wb, u, lam, lam1;    // q = u + wa 1[a] + wb 1[b]
+  int b;
+};
+__device__ __forceinline__ SoftTarget soft_target(const long long* target, long long row, long long rows, int a,
+                                                  const int* mix_row, float eps, int C) {
+  SoftTarget q{0.f, 0.f, eps / static_cast<float>(C), 1.f, 0.f, a};
+  if (mix_row != nullptr) {
+    q.lam = __int_as_float(mix_row[0]);
+    q.lam1 = __int_as_float(mix_row[1]);
+    q.b = static_cast<int>(target[row == 0 ? rows - 1 : row - 1]);
+  }
+  q.wa = (1.f - eps) * q.lam;
+  q.wb = (1.f - eps) * q.lam1;
+  return q;
+}
+
 // one warp per row: loss_row = logsumexp(z) - z[target]; dz = (softmax(z) - onehot) * grad_scale
 // loss_acc[0] += sum(loss_row) * grad_scale ; loss_acc[1] += #correct (argmax == target)
-template <bool IN_FP32, bool OUT_FP32>
-__global__ void __launch_bounds__(256)
-softmax_xent_kernel(const void* __restrict__ logits, const long long* __restrict__ target, void* __restrict__ dlogits,
-                    float* __restrict__ loss_acc, long long rows, int C, long long ld, float grad_scale) {
+// SOFT: the soft target above instead of the one-hot
+template <bool IN_FP32, bool OUT_FP32, bool SOFT>
+__device__ __forceinline__ void
+softmax_xent_body(const void* __restrict__ logits, const long long* __restrict__ target, void* __restrict__ dlogits,
+                  float* __restrict__ loss_acc, long long rows, int C, long long ld, float grad_scale,
+                  const int* __restrict__ mix_row, float eps) {
   griddep_launch_dependents();
   griddep_wait();
   const int lane = threadIdx.x & 31;
@@ -59,9 +84,18 @@ softmax_xent_kernel(const void* __restrict__ logits, const long long* __restrict
     const float lse = m + __logf(s);
     const int t = static_cast<int>(target[row]);
     const float inv = 1.f / s;
+    SoftTarget q{};
+    float zsum = 0.f;
+    if constexpr (SOFT) q = soft_target(target, row, rows, t, mix_row, eps, C);
     for (int c = lane; c < C; c += 32) {
       const float z = load_logit<IN_FP32>(logits, base + c);
-      const float g = (__expf(z - m) * inv - (c == t ? 1.f : 0.f)) * grad_scale;
+      float g;
+      if constexpr (SOFT) {
+        zsum += z;
+        g = (__expf(z - m) * inv - (q.u + (c == t ? q.wa : 0.f) + (c == q.b ? q.wb : 0.f))) * grad_scale;
+      } else {
+        g = (__expf(z - m) * inv - (c == t ? 1.f : 0.f)) * grad_scale;
+      }
       if (dlogits != nullptr) {
         if constexpr (OUT_FP32)
           reinterpret_cast<float*>(dlogits)[base + c] = g;
@@ -69,7 +103,14 @@ softmax_xent_kernel(const void* __restrict__ logits, const long long* __restrict
           reinterpret_cast<__nv_bfloat16*>(dlogits)[base + c] = __float2bfloat16_rn(g);
       }
     }
-    if (lane == 0) {
+    if constexpr (SOFT) {
+      zsum = wsum(zsum);
+      if (lane == 0) {
+        const float zb = load_logit<IN_FP32>(logits, base + q.b);
+        my_loss = (lse - q.wa * load_logit<IN_FP32>(logits, base + t) - q.wb * zb - q.u * zsum) * grad_scale;
+        my_hit = (am == t ? q.lam : 0.f) + (am == q.b ? q.lam1 : 0.f);
+      }
+    } else if (lane == 0) {
       my_loss = (lse - load_logit<IN_FP32>(logits, base + t)) * grad_scale;
       my_hit = (am == t) ? 1.f : 0.f;
     }
@@ -84,6 +125,19 @@ softmax_xent_kernel(const void* __restrict__ logits, const long long* __restrict
     atomicAdd(loss_acc, a);
     atomicAdd(loss_acc + 1, b);
   }
+}
+template <bool IN_FP32, bool OUT_FP32>
+__global__ void __launch_bounds__(256)
+softmax_xent_kernel(const void* __restrict__ logits, const long long* __restrict__ target, void* __restrict__ dlogits,
+                    float* __restrict__ loss_acc, long long rows, int C, long long ld, float grad_scale) {
+  softmax_xent_body<IN_FP32, OUT_FP32, false>(logits, target, dlogits, loss_acc, rows, C, ld, grad_scale, nullptr, 0.f);
+}
+template <bool IN_FP32, bool OUT_FP32>
+__global__ void __launch_bounds__(256)
+softmax_xent_soft_kernel(const void* __restrict__ logits, const long long* __restrict__ target,
+                         void* __restrict__ dlogits, float* __restrict__ loss_acc, long long rows, int C, long long ld,
+                         float grad_scale, const int* __restrict__ mix_row, float eps) {
+  softmax_xent_body<IN_FP32, OUT_FP32, true>(logits, target, dlogits, loss_acc, rows, C, ld, grad_scale, mix_row, eps);
 }
 
 // MSE: loss_acc[0] += sum((p - t)^2) * grad_scale ; dp = 2 * (p - t) * grad_scale   (grad_scale = 1/numel)
@@ -125,13 +179,14 @@ mse_kernel(const void* __restrict__ pred, const float* __restrict__ target, void
 // It replaces six launches (GEMM 128x10x512, loss, cast, colsum, two SIMT GEMMs) for ~4 MFLOP of work.  One CTA handles HEAD_ROWS rows: warp w owns row w for the logits, the
 // 256 threads then share the dX / dW tiles.  x: bf16 [rows, K], W: bf16 [NC, K] (the arena's shadow), b: fp32.
 // BACKWARD = false: the evaluation instantiation -- logits, loss and #correct only (no dX / dW / db; grid.y = 1).
+// SOFT (training only): the soft target of softmax_xent_soft_kernel; z_b and sum(z) are one shuffle and one warp sum more.
 constexpr int HEAD_ROWS = 8;
-template <bool BACKWARD>
-__global__ void __launch_bounds__(256)
-linear_xent_head_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ w, const float* __restrict__ bias,
-                        const long long* __restrict__ target, __nv_bfloat16* __restrict__ dx, float* __restrict__ dw,
-                        float* __restrict__ db, float* __restrict__ loss_acc, float* __restrict__ logits_out, int rows,
-                        int K, int NC, float grad_scale) {
+template <bool BACKWARD, bool SOFT>
+__device__ __forceinline__ void
+linear_xent_head_body(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ w, const float* __restrict__ bias,
+                      const long long* __restrict__ target, __nv_bfloat16* __restrict__ dx, float* __restrict__ dw,
+                      float* __restrict__ db, float* __restrict__ loss_acc, float* __restrict__ logits_out, int rows,
+                      int K, int NC, float grad_scale, const int* __restrict__ mix_row, float eps) {
   griddep_launch_dependents();
   extern __shared__ __align__(16) unsigned char head_smem[];
   __nv_bfloat16* sw = reinterpret_cast<__nv_bfloat16*>(head_smem);                 // [NC][K]
@@ -190,9 +245,18 @@ linear_xent_head_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16
       const float ssum = wsum(e);
       const int t = static_cast<int>(target[row]);
       const float zt = __shfl_sync(0xffffffffu, mine, t & 31);
-      loss = (m + __logf(ssum)) - zt;
-      hit = (am == t) ? 1.f : 0.f;
-      dl = lane < NC ? (e / ssum - (lane == t ? 1.f : 0.f)) * grad_scale : 0.f;
+      if constexpr (SOFT) {
+        const SoftTarget q = soft_target(target, row, rows, t, mix_row, eps, NC);
+        const float zb = __shfl_sync(0xffffffffu, mine, q.b & 31);
+        const float zsum = wsum(lane < NC ? mine : 0.f);
+        loss = (m + __logf(ssum)) - q.wa * zt - q.wb * zb - q.u * zsum;
+        hit = (am == t ? q.lam : 0.f) + (am == q.b ? q.lam1 : 0.f);
+        dl = lane < NC ? (e / ssum - (q.u + (lane == t ? q.wa : 0.f) + (lane == q.b ? q.wb : 0.f))) * grad_scale : 0.f;
+      } else {
+        loss = (m + __logf(ssum)) - zt;
+        hit = (am == t) ? 1.f : 0.f;
+        dl = lane < NC ? (e / ssum - (lane == t ? 1.f : 0.f)) * grad_scale : 0.f;
+      }
     }
     sdl[warp * 32 + lane] = dl;
     if (lane == 0) { sred[warp * 2] = loss; sred[warp * 2 + 1] = hit; }
@@ -238,6 +302,24 @@ linear_xent_head_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16
     atomicAdd(db + threadIdx.x, a);
   }
 }
+template <bool BACKWARD>
+__global__ void __launch_bounds__(256)
+linear_xent_head_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ w, const float* __restrict__ bias,
+                        const long long* __restrict__ target, __nv_bfloat16* __restrict__ dx, float* __restrict__ dw,
+                        float* __restrict__ db, float* __restrict__ loss_acc, float* __restrict__ logits_out, int rows,
+                        int K, int NC, float grad_scale) {
+  linear_xent_head_body<BACKWARD, false>(x, w, bias, target, dx, dw, db, loss_acc, logits_out, rows, K, NC, grad_scale,
+                                         nullptr, 0.f);
+}
+__global__ void __launch_bounds__(256)
+linear_xent_head_soft_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ w,
+                             const float* __restrict__ bias, const long long* __restrict__ target,
+                             __nv_bfloat16* __restrict__ dx, float* __restrict__ dw, float* __restrict__ db,
+                             float* __restrict__ loss_acc, int rows, int K, int NC, float grad_scale,
+                             const int* __restrict__ mix_row, float eps) {
+  linear_xent_head_body<true, true>(x, w, bias, target, dx, dw, db, loss_acc, nullptr, rows, K, NC, grad_scale, mix_row,
+                                    eps);
+}
 
 }  // namespace b200
 
@@ -249,6 +331,20 @@ extern "C" int b200_softmax_xent(const void* logits, int logits_fp32, const long
   if (rows <= 0) return 0;
   const unsigned grid = static_cast<unsigned>((rows + 7) / 8);
 #define XENT(A, B) launch_pdl(softmax_xent_kernel<A, B>, grid, 256, 0, stream, logits, target, dlogits, loss_acc, rows, C, ld, grad_scale)
+  if (logits_fp32) { if (dl_fp32) XENT(true, true); else XENT(true, false); }
+  else             { if (dl_fp32) XENT(false, true); else XENT(false, false); }
+#undef XENT
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int b200_softmax_xent_soft(const void* logits, int logits_fp32, const long long* target, void* dlogits,
+                                      int dl_fp32, float* loss_acc, long long rows, int C, long long ld, float grad_scale,
+                                      const int* mix_row, float eps, cudaStream_t stream) {
+  if (rows <= 0) return 0;
+  const unsigned grid = static_cast<unsigned>((rows + 7) / 8);
+#define XENT(A, B)                                                                                                     \
+  launch_pdl(softmax_xent_soft_kernel<A, B>, grid, 256, 0, stream, logits, target, dlogits, loss_acc, rows, C, ld,     \
+             grad_scale, mix_row, eps)
   if (logits_fp32) { if (dl_fp32) XENT(true, true); else XENT(true, false); }
   else             { if (dl_fp32) XENT(false, true); else XENT(false, false); }
 #undef XENT
@@ -291,6 +387,33 @@ extern "C" int b200_linear_xent_head(const void* x, const void* w, const float* 
                               reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<const __nv_bfloat16*>(w), bias,
                               target, reinterpret_cast<__nv_bfloat16*>(dx), dw, db, loss_acc, logits_out, rows, K, NC,
                               grad_scale);
+  if (le != cudaSuccess) return static_cast<int>(le);
+  return static_cast<int>(cudaGetLastError());
+}
+
+// classifier head with soft targets (training): b200_linear_xent_head's shape limits, no logits output
+extern "C" int b200_linear_xent_head_soft(const void* x, const void* w, const float* bias, const long long* target,
+                                          void* dx, float* dw, float* db, float* loss_acc, int rows, int K, int NC,
+                                          float grad_scale, const int* mix_row, float eps, cudaStream_t stream) {
+  using namespace b200;
+  if (rows <= 0) return 0;
+  const size_t smem = static_cast<size_t>(K) * (NC + HEAD_ROWS) * 2 + HEAD_ROWS * 34 * 4;
+  if (NC < 1 || NC > 32 || (K % 8) || smem > 200 * 1024 || (reinterpret_cast<uintptr_t>(x) & 15) ||
+      (reinterpret_cast<uintptr_t>(w) & 15) || (reinterpret_cast<uintptr_t>(dx) & 3))
+    return -2;
+  static size_t configured = 0;
+  if (smem > 48 * 1024 && smem > configured) {
+    cudaError_t e = cudaFuncSetAttribute(linear_xent_head_soft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         static_cast<int>(smem));
+    if (e != cudaSuccess) return static_cast<int>(e);
+    configured = smem;
+  }
+  int ks = 8;
+  while (ks > 1 && (K % (ks * 8))) ks >>= 1;
+  cudaError_t le = launch_pdl(linear_xent_head_soft_kernel, dim3((rows + HEAD_ROWS - 1) / HEAD_ROWS, ks), dim3(256), smem,
+                              stream, reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<const __nv_bfloat16*>(w),
+                              bias, target, reinterpret_cast<__nv_bfloat16*>(dx), dw, db, loss_acc, rows, K, NC,
+                              grad_scale, mix_row, eps);
   if (le != cudaSuccess) return static_cast<int>(le);
   return static_cast<int>(cudaGetLastError());
 }

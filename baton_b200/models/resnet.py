@@ -243,12 +243,14 @@ class ResNet(FederatedModule):
             return [d, dx_ds]
         return [d, dres]
 
-    def explicit_step(self, x, target, loss_acc=None, after_first_gemm=None):
+    def explicit_step(self, x, target, loss_acc=None, after_first_gemm=None, mix=None):
         """Forward + loss + backward of one batch with parameter gradients accumulated into the arena (the same
         contract as ``loss.backward()`` on ``forward``); returns the device ``[mean loss, #correct]`` pair.
         CUDA + arena-adopted training mode only.
 
-        ``after_first_gemm`` (optional, from the trainer) is called right after the GEMM of the first convolution."""
+        ``after_first_gemm`` (optional, from the trainer) is called right after the GEMM of the first convolution.
+        ``mix = (mix_row, smoothing)``: the soft-target loss of ``data/mix.py`` in both head paths."""
+        soft = dict(mix_row=mix[0], smoothing=float(mix[1])) if mix is not None else {}
         F = bnn.F
         if self.stats_workspace is not None:
             self.stats_workspace.zero_()
@@ -276,7 +278,7 @@ class ResNet(FederatedModule):
         if fc.out_features <= 32 and tw is not None and (fc.bias is None or tb is not None) and fc.act == 0:
             # classifier head (linear + softmax cross-entropy, forward and backward) in ONE launch
             head = F.linear_xent_head(feat.contiguous(), bnn._shadow(fc, "weight", fc.weight), fc.bias, target, tw, tb,
-                                      acc=loss_acc)
+                                      acc=loss_acc, **soft)
         if head is not None:
             stats, d, _ = head
         else:
@@ -284,7 +286,7 @@ class ResNet(FederatedModule):
             logits = bnn._LinearFn.forward(cl, feat, fc.weight, fc.bias, bnn._shadow(fc, "weight", fc.weight), fc.act,
                                            fc.out_fp32, None, None)
             cl.needs_dx = True
-            stats, dlogits = F.softmax_xent(logits.contiguous(), target, want_grad=True, acc=loss_acc)
+            stats, dlogits = F.softmax_xent(logits.contiguous(), target, want_grad=True, acc=loss_acc, **soft)
             d = bnn._LinearFn.backward(cl, dlogits)[0]
         d = d.reshape(h.shape) if ca is None else bnn._AvgPoolFn.backward(ca, d)
         pieces = [d]

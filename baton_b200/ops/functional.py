@@ -380,13 +380,18 @@ AUGMENT_MAX_ROW_BYTES = 48 * 1024      # one image row of gather_augment fits th
 
 
 def gather_augment(src: torch.Tensor, idx: torch.Tensor, words: torch.Tensor, key: int, padding: int, *,
-                   crop: bool = True, flip: bool = True, s0: int = 0,
-                   out: Optional[torch.Tensor] = None) -> torch.Tensor:
+                   crop: bool = True, flip: bool = True, s0: int = 0, out: Optional[torch.Tensor] = None,
+                   mix_rows: Optional[torch.Tensor] = None, batch: Optional[int] = None) -> torch.Tensor:
     """``augment(src[idx])`` for a resident NHWC image shard (bf16 / fp16 / fp32): a random crop of the zero-padded
     image (``padding`` pixels each side) and a random horizontal flip, drawn for output position ``s0 + s`` from
     Philox4x32-10 under the 64-bit ``key`` with counter ``(s0 + s, epoch, stream_lo, stream_hi)``.  ``words`` is a
     device int32 tensor ``{epoch, stream_lo, stream_hi}`` read when the kernel runs (a captured graph follows its
-    contents).  ``data/augment.py: gather_augment_reference`` is the same function in torch."""
+    contents).  ``data/augment.py: gather_augment_reference`` is the same function in torch.
+
+    ``mix_rows`` (device int32 ``[n_batches, 8]``, read when the kernel runs) with ``batch``: mixup / CutMix
+    (``data/mix.py``).  Every image is then mixed with its partner in its batch of ``batch`` positions, under the mix
+    row ``mix_rows[(s0 + s) // batch]``.  The call must cover whole batches (``s0 % batch == 0``); only the last may be
+    short.  Each output is ``mix_batch_reference`` of the augmented batch."""
     if src.dim() != 4 or not src.is_contiguous() or src.dtype not in (torch.bfloat16, torch.float16, torch.float32):
         raise ValueError("gather_augment needs a contiguous NHWC bf16 / fp16 / fp32 shard, got {} {}".format(
             tuple(src.shape), src.dtype))
@@ -403,6 +408,14 @@ def gather_augment(src: torch.Tensor, idx: torch.Tensor, words: torch.Tensor, ke
     if out is None:
         out = torch.empty((idx.numel(), H, W, C), dtype=src.dtype, device=src.device)
     key = int(key) & 0xFFFFFFFFFFFFFFFF
+    if mix_rows is not None:
+        if batch is None or int(batch) < 1 or int(s0) % int(batch):
+            raise ValueError("gather_augment: mixing needs the batch size, and s0 = {} on a batch boundary".format(s0))
+        if mix_rows.dtype != torch.int32 or mix_rows.device != src.device or not mix_rows.is_contiguous():
+            raise ValueError("gather_augment: mix_rows must be a contiguous int32 tensor on the shard's device")
+        load().gather_mix(src, idx.contiguous(), out, words, mix_rows, int(batch),
+                          key - (1 << 64) if key >> 63 else key, int(padding), bool(crop), bool(flip), int(s0))
+        return out
     load().gather_augment(src, idx.contiguous(), out, words, key - (1 << 64) if key >> 63 else key, int(padding),
                           bool(crop), bool(flip), int(s0))
     return out
@@ -786,29 +799,44 @@ def avgpool_bwd(dy: torch.Tensor, in_shape) -> torch.Tensor:
 # ---------------------------------------------------------------------------- losses
 def softmax_xent(logits: torch.Tensor, target: torch.Tensor, want_grad: bool = True,
                  grad_dtype: Optional[torch.dtype] = None, acc: Optional[torch.Tensor] = None,
-                 loss_scale: Optional[float] = None):
+                 loss_scale: Optional[float] = None, mix_row: Optional[torch.Tensor] = None, smoothing: float = 0.0):
     """Fused softmax cross-entropy: returns ``(acc, dlogits)`` where ``acc[0]`` is the
     batch-mean loss and ``acc[1]`` the number of correct predictions.  ``acc`` (fp32 ``[2]``) may be supplied: the
     kernel ADDS into it (a device-side running sum over the steps of an epoch, no extra kernels).  ``loss_scale``
-    replaces the ``1 / rows`` that scales the loss and the gradient (1.0: the sum of the row losses)."""
+    replaces the ``1 / rows`` that scales the loss and the gradient (1.0: the sum of the row losses).
+
+    ``mix_row`` (the step's device int32 mix row) and ``smoothing``: the soft target of ``data/mix.py``, the partner
+    of row ``r`` being row ``r - 1`` (mod rows) of ``target``; ``acc[1]`` then adds the lam-weighted hits."""
     rows, c = logits.shape
     if acc is None:
         acc = torch.zeros(2, dtype=torch.float32, device=logits.device)
     dl = torch.empty_like(logits, dtype=grad_dtype or logits.dtype) if want_grad else None
-    load().softmax_xent(logits, target, dl, acc, rows, c, logits.stride(0), 1.0 / rows if loss_scale is None else loss_scale)
+    scale = 1.0 / rows if loss_scale is None else loss_scale
+    if mix_row is None and smoothing == 0.0:
+        load().softmax_xent(logits, target, dl, acc, rows, c, logits.stride(0), scale)
+    else:
+        load().softmax_xent_soft(logits, target, dl, acc, rows, c, logits.stride(0), scale, mix_row, float(smoothing))
     return acc, dl
 
 
 def linear_xent_head(x: torch.Tensor, w_bf16: torch.Tensor, bias: Optional[torch.Tensor], target: torch.Tensor,
                      dw: torch.Tensor, db: Optional[torch.Tensor], acc: Optional[torch.Tensor] = None,
-                     want_dx: bool = True, want_logits: bool = False):
+                     want_dx: bool = True, want_logits: bool = False, mix_row: Optional[torch.Tensor] = None,
+                     smoothing: float = 0.0):
     """Classifier head in one launch: ``logits = x w^T + b`` (<= 32 classes), softmax cross-entropy, and the head's whole
     backward -- ``dx`` (bf16), ``dw += dlogits^T x``, ``db += colsum(dlogits)`` (fp32, accumulated in place), the batch-mean
-    loss / #correct added into ``acc``.  Returns ``(acc, dx, logits)`` or ``None`` when the shape is not supported."""
+    loss / #correct added into ``acc``.  Returns ``(acc, dx, logits)`` or ``None`` when the shape is not supported.
+    ``mix_row`` / ``smoothing``: the soft target, as in :func:`softmax_xent` (no logits output)."""
     rows, K = x.shape
     if acc is None:
         acc = torch.zeros(2, dtype=torch.float32, device=x.device)
     dx = torch.empty((rows, K), dtype=BF16, device=x.device) if want_dx else None
+    if mix_row is not None or smoothing != 0.0:
+        if want_logits:
+            raise ValueError("linear_xent_head: the soft-target head has no logits output")
+        ok = load().linear_xent_head_soft(x, w_bf16, bias, target, dx, dw, db, acc, 1.0 / rows, mix_row,
+                                          float(smoothing))
+        return (acc, dx, None) if ok else None
     logits = torch.empty((rows, w_bf16.shape[0]), dtype=torch.float32, device=x.device) if want_logits else None
     ok = load().linear_xent_head(x, w_bf16, bias, target, dx, dw, db, acc, logits, 1.0 / rows)
     return (acc, dx, logits) if ok else None

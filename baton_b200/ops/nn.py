@@ -678,8 +678,8 @@ def softmax(x: torch.Tensor, scale: float = 1.0) -> torch.Tensor:
 # ================================================================================ losses
 class _XentFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, logits, target):
-        acc, dl = F.softmax_xent(logits, target, want_grad=True)
+    def forward(ctx, logits, target, mix_row=None, smoothing=0.0):
+        acc, dl = F.softmax_xent(logits, target, want_grad=True, mix_row=mix_row, smoothing=smoothing)
         ctx.save_for_backward(dl)
         ctx.mark_non_differentiable(acc)
         return acc[0].clone(), acc
@@ -687,16 +687,26 @@ class _XentFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g, _unused):
         (dl,) = ctx.saved_tensors
-        return dl * g.to(dl.dtype), None
+        return dl * g.to(dl.dtype), None, None, None
 
 
-def cross_entropy(logits: torch.Tensor, target: torch.Tensor):
+def cross_entropy(logits: torch.Tensor, target: torch.Tensor, mix=None):
     """Fused softmax + NLL + gradient.  Returns ``(loss, stats)`` with
-    ``stats = [mean loss, #correct]`` on the device."""
+    ``stats = [mean loss, #correct]`` on the device.  ``mix = (mix_row, smoothing)``: the soft target of
+    ``data/mix.py`` (``mix_row`` None: label smoothing only); the hits are then lam-weighted."""
     if not logits.is_cuda:
+        if mix is not None:
+            from ..data.mix import SoftTarget, decode_row, soft_cross_entropy, soft_hits
+            row, eps = mix
+            r = decode_row(row) if row is not None else None
+            t = SoftTarget(target, target.roll(1, 0) if r else target, r.lam if r else 1.0, r.lam1 if r else 0.0, eps)
+            loss = soft_cross_entropy(logits, t)
+            return loss, torch.stack([loss.detach(), soft_hits(logits, t)])
         loss = TF.cross_entropy(logits.float(), target)
         hits = (logits.argmax(-1) == target).sum().float()
         return loss, torch.stack([loss.detach(), hits])
+    if mix is not None:
+        return _XentFn.apply(logits.contiguous(), target, mix[0], float(mix[1]))
     return _XentFn.apply(logits.contiguous(), target)
 
 

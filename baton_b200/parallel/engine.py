@@ -77,7 +77,8 @@ class FederatedEngine:
                  server_betas: Tuple[float, float] = (0.9, 0.99), server_tau: float = 1e-3,
                  compress: Optional[str] = None, topk_ratio: float = 0.01, error_feedback: bool = True,
                  local_keys: "Optional[str | Sequence[str]]" = None, augment: Optional[str] = None,
-                 augment_padding: int = 4):
+                 augment_padding: int = 4, mix: Optional[str] = None, mix_alpha: float = 1.0,
+                 label_smoothing: float = 0.0):
         """``prox_mu > 0``: FedProx local training -- every step adds ``prox_mu * (theta - global_w)`` to the gradient,
         ``global_w`` being the global model the round started from (for logical clients too: each starts from it).
 
@@ -143,9 +144,19 @@ class FederatedEngine:
         drawn afresh per sample and epoch inside the batch gather.  The key is derived from ``seed`` (the same on every
         rank) and each client's stream is ``(round_index << 32) | client_id``, so co-hosted clients and successive
         rounds draw independently and a run is reproducible from its seed.  Shards must be NHWC images.  It is local to
-        each client and combines with every other option.  ``None`` (the default) runs exactly the plain engine."""
+        each client and combines with every other option.  ``None`` (the default) runs exactly the plain engine.
+
+        ``mix="mixup"`` / ``"cutmix"`` / ``"mixup_cutmix"`` (with ``mix_alpha``) and ``label_smoothing``
+        (``data/mix.py``): every client trains on batches mixed with themselves rolled by one, one lambda per batch, and
+        on the soft-target cross-entropy.  Mixing draws from the augmentation key and the client's stream of the round,
+        with or without ``augment``.  It needs the cross-entropy loss, and mixing needs NHWC image shards; both are
+        local to each client and combine with every other option.  Evaluation keeps hard labels.  ``None`` / ``0``
+        (the defaults) run exactly the plain engine."""
         from ..data.augment import check_augment
+        from ..data.mix import check_mix, check_mix_loss
         aug = check_augment(augment, augment_padding)
+        mixc = check_mix(mix, mix_alpha, label_smoothing)
+        check_mix_loss(mixc, loss)
         if compress not in (None, "topk"):
             raise ValueError("compress must be None or 'topk', got {!r}".format(compress))
         self.topk = TopKConfig(topk_ratio, error_feedback) if compress == "topk" else None
@@ -220,8 +231,12 @@ class FederatedEngine:
         self.hp = dict(lr=lr, batch_size=batch_size, momentum=momentum, weight_decay=weight_decay, prox_mu=prox_mu)
         if adam:
             self.hp.update(optimizer=optimizer, betas=betas, eps=eps)
-        self.aug_hp = (dict(augment=aug.kind, augment_padding=aug.padding, augment_seed=seed)
-                       if aug is not None else None)
+        aug_hp = {}
+        if aug is not None:
+            aug_hp.update(augment=aug.kind, augment_padding=aug.padding)
+        if mixc is not None:
+            aug_hp.update(mix=mixc.kind, mix_alpha=mixc.alpha, label_smoothing=mixc.smoothing)
+        self.aug_hp = dict(aug_hp, augment_seed=seed) if aug_hp else None
         self.n_rounds = 0
         self._last_participants: Optional[List[int]] = None
         self.logical_clients = logical_clients if logical_clients and logical_clients > self.world else 0
@@ -428,7 +443,8 @@ class FederatedEngine:
 
     def _train_client(self, cid: int, X, y, n_epoch: int, first: bool):
         """Local training of client ``cid`` on the replica; with SCAFFOLD, its correction before and its control-variate
-        update after (before any fold resets the replica).  With augmentation, the client's stream of this round."""
+        update after (before any fold resets the replica).  With augmentation or mixing, the client's stream of this
+        round."""
         hp = self.hp
         if self.aug_hp is not None:
             hp = dict(hp, augment_stream=(self.n_rounds << 32) | int(cid), **self.aug_hp)

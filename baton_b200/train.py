@@ -33,6 +33,12 @@ Every trainer also takes ``augment="crop" | "flip" | "crop_flip"`` with ``augmen
 each epoch's batches are randomly cropped from the zero-padded image and flipped, fresh draws per sample and epoch.
 ``GraphedLocalSGD`` does it inside the epoch's batch gather (``F.gather_augment``); the CPU trainers call the host
 reference per batch.  ``augment_seed`` / ``augment_stream`` pick the draws (``data/augment.py: AugmentStreams``).
+
+Cross-entropy trainers also take ``mix="mixup" | "cutmix" | "mixup_cutmix"`` with ``mix_alpha``, and
+``label_smoothing`` (``data/mix.py``): each batch is mixed with itself rolled by one under one lambda per batch, and
+the loss is the soft-target cross-entropy.  ``GraphedLocalSGD`` mixes inside the same batch gather and applies the soft
+target in the fused loss kernels; the CPU trainers call the host reference.  Mixing draws from the augmentation key
+and stream, so it takes the same ``augment_seed`` / ``augment_stream``.
 """
 from __future__ import annotations
 
@@ -45,6 +51,8 @@ import torch
 from torch import nn
 
 from .data.augment import AugmentStreams, check_augment, check_shard, gather_augment_reference
+from .data.mix import (MIX_ROW, check_mix, check_mix_loss, check_mix_shard, mix_batch_reference, mix_rows, mix_table,
+                       soft_cross_entropy, soft_hits)
 from .utils.progress import EpochProgress
 
 
@@ -112,16 +120,19 @@ def run_local_sgd(model: nn.Module, X: torch.Tensor, y: torch.Tensor, *, n_epoch
                   generator: Optional[torch.Generator] = None, prox_mu: float = 0.0, optimizer: str = "sgd",
                   betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8, augment: Optional[str] = None,
                   augment_padding: int = 4, augment_seed: Optional[int] = None,
-                  augment_stream: Optional[int] = None) -> List[float]:
+                  augment_stream: Optional[int] = None, mix: Optional[str] = None, mix_alpha: float = 1.0,
+                  label_smoothing: float = 0.0) -> List[float]:
     """Portable local SGD; returns the per-epoch mean loss.  ``prox_mu > 0``: FedProx, anchored on the parameters as
     they are on entry -- the global model the worker has just loaded.  ``optimizer="adamw"``: a fresh
     ``torch.optim.AdamW(lr, betas, eps, weight_decay)`` instead of SGD.  ``augment``: random crop / flip of every
-    batch; the model keeps the key and run counter (``AugmentStreams``) across calls."""
+    batch; the model keeps the key and run counter (``AugmentStreams``) across calls.  ``mix`` / ``label_smoothing``:
+    mixup / CutMix of every batch and the soft-target loss (``data/mix.py``)."""
     criterion = _loss_fn(loss)
     prox_mu = check_prox_mu(prox_mu)
     adam = check_optimizer(optimizer, momentum, prox_mu=prox_mu)
+    mixc = _mix_setup(mix, mix_alpha, label_smoothing, loss)
     aug = _augment_setup(model.__dict__.setdefault("_augment_streams", AugmentStreams()), X, augment,
-                         augment_padding, augment_seed, augment_stream)
+                         augment_padding, augment_seed, augment_stream, mixc)
     n = X.shape[0]
     nn.Module.train(model, True)
     params = list(model.parameters())
@@ -137,14 +148,19 @@ def run_local_sgd(model: nn.Module, X: torch.Tensor, y: torch.Tensor, *, n_epoch
     for epoch in range(n_epoch):
         if reshuffle_each_epoch and epoch > 0:
             idxs = torch.randperm(n, generator=generator).to(X.device)
-        batch_iter = EpochProgress(epoch, torch.split(idxs, batch_size), verbose=verbose)
+        batches = torch.split(idxs, batch_size)
+        rows = _host_mix_rows(mixc, aug, X, epoch, len(batches))
+        batch_iter = EpochProgress(epoch, batches, verbose=verbose)
         for b, batch_idxs in enumerate(batch_iter):
             optimizer.zero_grad(set_to_none=True)
-            output = model(_host_batch(X, batch_idxs, aug, epoch, b * batch_size))
+            xb = _host_batch(X, batch_idxs, aug, epoch, b * batch_size)
             target = y[batch_idxs]
+            if mixc is not None:
+                xb, soft = mix_batch_reference(xb, target, rows[b] if rows is not None else None, mixc.smoothing)
+            output = model(xb)
             if output.shape != target.shape and target.dtype.is_floating_point:
                 target = target.reshape(output.shape)  # (N,) vs (N,1) -- quirk 13
-            loss_batch = criterion(output, target)
+            loss_batch = criterion(output, target) if mixc is None else soft_cross_entropy(output, soft)
             batch_iter.update_loss(loss_batch)
             loss_batch.backward()
             if anchors is not None:
@@ -154,18 +170,38 @@ def run_local_sgd(model: nn.Module, X: torch.Tensor, y: torch.Tensor, *, n_epoch
     return loss_history
 
 
-def _augment_setup(streams: AugmentStreams, X, augment, augment_padding, augment_seed, augment_stream):
-    """``(config, key, stream)`` of a run, or None when it does not augment; ``ValueError`` for a bad config or shard."""
+def _augment_setup(streams: AugmentStreams, X, augment, augment_padding, augment_seed, augment_stream, mix=None):
+    """``(config, key, stream)`` of a run, or None when it neither augments nor mixes (``config`` is None when it only
+    mixes: mixing draws from the same key and stream); ``ValueError`` for a bad config or shard."""
     cfg = check_augment(augment, augment_padding)
-    if cfg is None:
+    mixing = mix is not None and mix.kind is not None
+    if cfg is None and not mixing:
         return None
-    check_shard(cfg, X)
+    if cfg is not None:
+        check_shard(cfg, X)
+    check_mix_shard(mix, X)
     return (cfg,) + streams.next(augment_seed, augment_stream)
 
 
+def _mix_setup(mix, mix_alpha, label_smoothing, loss):
+    """The run's :class:`~baton_b200.data.mix.MixConfig` (None: hard targets); ``ValueError`` for a bad config or a
+    loss that is not the cross-entropy."""
+    cfg = check_mix(mix, mix_alpha, label_smoothing)
+    check_mix_loss(cfg, loss)
+    return cfg
+
+
+def _host_mix_rows(mixc, aug, X, epoch: int, n_batches: int):
+    """The epoch's mix rows (``data/mix.py: mix_table``), or None when the run does not mix."""
+    if mixc is None or mixc.kind is None:
+        return None
+    _, key, stream = aug
+    return mix_table(key, stream, epoch, n_batches, mixc, X.shape[1], X.shape[2])
+
+
 def _host_batch(X, idx, aug, epoch: int, s0: int):
-    """``X[idx]``, augmented (host reference) for epoch positions ``s0 ..`` when ``aug`` is set."""
-    if aug is None:
+    """``X[idx]``, augmented (host reference) for epoch positions ``s0 ..`` when ``aug`` crops or flips."""
+    if aug is None or aug[0] is None:
         return X[idx]
     cfg, key, stream = aug
     return gather_augment_reference(X, idx, key, stream, epoch, cfg.padding, cfg.crop, cfg.flip, s0=s0)
@@ -254,6 +290,13 @@ class GraphedLocalSGD:
     buffer.  The key is a launch argument, so
     it is part of the epoch graph's key.
 
+    ``run(mix=...)`` gathers through the mixing form of the same kernel (``F.gather_augment(mix_rows=...)``) and
+    trains on the soft-target loss kernels (``label_smoothing`` alone needs only those).  The run's mix rows
+    (``data/mix.py: mix_rows``, ``[n_epoch, steps, 8]``) are built on the host in pinned memory and copied without a
+    host synchronisation; before each replay that epoch's rows are copied into the graph's ``[steps, 8]`` row buffer,
+    which the gather reads whole and captured step ``s`` passes row ``s`` of to the loss.  Whether the run mixes and
+    its smoothing (a launch argument) are part of the graph key; lambda and the boxes are not.
+
     ``model`` must already be adopted by a :class:`~baton_b200.parallel.arena.ParamArena`
     (``arena``); the engine is what ``FederatedModule.local_train`` dispatches to
     for CUDA shards (``model._graphed_trainer``).
@@ -287,6 +330,7 @@ class GraphedLocalSGD:
         self._aug = None              # augmentation of the current run: (AugmentConfig, key, stream) or None
         self._aug_streams = AugmentStreams()
         self._aug_table = None        # device [epochs, 3] per-epoch words of augmenting runs (see _aug_words)
+        self._mix = None              # MixConfig of the current run (mixing and / or label smoothing) or None
         self.loss_acc = torch.zeros(2, dtype=torch.float32, device=dev)
         self._graphs = {}           # (n, batch, x_shape, y_shape) -> captured epoch
         self._hyper_host = None
@@ -298,33 +342,41 @@ class GraphedLocalSGD:
         self.eval_launches = None     # Counter of the kernels in the last captured evaluation pass
 
     # -------------------------------------------------------------- one SGD step (capturable)
-    def _loss(self, out, yb):
+    def _loss(self, out, yb, mix=None):
         if self.loss_kind in ("ce", "cross_entropy"):
-            loss, stats = self.bnn.cross_entropy(out, yb)
+            loss, stats = self.bnn.cross_entropy(out, yb) if mix is None else self.bnn.cross_entropy(out, yb, mix=mix)
             return loss, stats
         loss = self.bnn.mse_loss(out, yb)
         return loss, torch.stack([loss.detach(), torch.zeros_like(loss.detach())])
 
-    def _gather(self, X, y, idx, s0=0, words=None):
-        """``X[idx], y[idx]``; with augmentation on, ``X`` is gathered by ``F.gather_augment`` for epoch positions
-        ``s0 ..`` with the device words ``words``."""
+    def _gather(self, X, y, idx, s0=0, words=None, mix_rows=None, bsz=None):
+        """``X[idx], y[idx]``; with augmentation or mixing on, ``X`` is gathered by ``F.gather_augment`` for epoch
+        positions ``s0 ..`` with the device words ``words`` (and the epoch's mix rows ``mix_rows``, batches of
+        ``bsz``)."""
         F = self.F
         if self._aug is not None:
             cfg, key, _ = self._aug
-            xb = F.gather_augment(X, idx, words, key, cfg.padding, crop=cfg.crop, flip=cfg.flip, s0=s0)
+            pad, crop, flip = (cfg.padding, cfg.crop, cfg.flip) if cfg is not None else (0, False, False)
+            xb = F.gather_augment(X, idx, words, key, pad, crop=crop, flip=flip, s0=s0, mix_rows=mix_rows, batch=bsz)
         else:
             xb = F.gather_rows(X, idx)
         yb = F.gather_rows(y, idx) if y.dtype == torch.int64 and y.dim() == 1 else y.index_select(0, idx)
         return xb, yb
 
-    def _step(self, X, y, idx, batch=None, emit_wire=False, fuse_sgd=True, row=None, s0=0, words=None):
+    def _step(self, X, y, idx, batch=None, emit_wire=False, fuse_sgd=True, row=None, s0=0, words=None, mix_rows=None,
+              bsz=None):
         """One SGD step on ``X[idx], y[idx]`` (or on the already gathered ``batch``).  ``emit_wire``: last step of
         an epoch -- the optimizer kernel also writes the upload copy for the round-end collective (``self.pack``).
         ``fuse_sgd=False``: no optimizer epilogue in the weight-gradient GEMMs (one optimizer pass over the arena).
         ``row``: with AdamW, the device row of this step's coefficients (``F.adamw_rows``).  ``s0``, ``words``: the
-        epoch position of ``idx[0]`` and the device words of an augmenting gather."""
+        epoch position of ``idx[0]`` and the device words of an augmenting gather.  ``mix_rows``, ``bsz``: the
+        epoch's device mix rows and the batch size of a mixing run; the loss reads row ``s0 // bsz``."""
         F = self.F
-        xb, yb = batch if batch is not None else self._gather(X, y, idx, s0, words)
+        xb, yb = batch if batch is not None else self._gather(X, y, idx, s0, words, mix_rows, bsz)
+        mix = None
+        if self._mix is not None:
+            mix = (mix_rows[s0 // bsz] if mix_rows is not None else None, self._mix.smoothing)
+        soft = {"mix": mix} if mix is not None else {}
         ws = getattr(self.model, "stats_workspace", None)
         if ws is not None and not getattr(self.model, "zeroes_own_workspace", False):
             ws.zero_()
@@ -343,17 +395,17 @@ class GraphedLocalSGD:
                 # the split-K = 1 convolution weight gradients apply SGD in their GEMM epilogue; one launch covers the rest
                 with self.bnn.SGD_EPI.open(a, hyper, self.nesterov, prox=self.prox, corr=self.corr,
                                            adam_v=adam_v) as epi:
-                    explicit(xb, yb, loss_acc=self.loss_acc, after_first_gemm=self._first_gemm_hook)
+                    explicit(xb, yb, loss_acc=self.loss_acc, after_first_gemm=self._first_gemm_hook, **soft)
                 F.fused_sgd_segments(a.theta, a.grad, hyper, self._segment_table(epi.fused, epi.nograd),
                                      a.momentum, bf, nesterov=self.nesterov, prox_anchor=anchor, corr=self.corr,
                                      adam_v=adam_v)
                 self.emitted_wire = False
                 return
-            explicit(xb, yb, loss_acc=self.loss_acc, after_first_gemm=self._first_gemm_hook)
+            explicit(xb, yb, loss_acc=self.loss_acc, after_first_gemm=self._first_gemm_hook, **soft)
             stats = None
         else:
             out = self.model(xb)
-            loss, stats = self._loss(out, yb)
+            loss, stats = self._loss(out, yb, mix)
             loss.backward()
             self.bnn.WGRAD.join()      # weight-gradient GEMMs run on a side stream; they must land before the step
         # one optimizer pass over the whole arena; the epoch's last step also emits the upload copy
@@ -403,13 +455,22 @@ class GraphedLocalSGD:
             t[:, col].fill_(word - (1 << 32) if word >> 31 else word)
         return t[:n_epoch]
 
+    def _mix_rows(self, n_epoch: int, steps: int, X):
+        """Device int32 ``[n_epoch, steps, 8]`` mix rows of a mixing run: built on the host in pinned memory and copied
+        asynchronously (no host synchronisation)."""
+        _, key, stream = self._aug
+        host = mix_rows(key, stream, n_epoch, steps, self._mix, X.shape[1], X.shape[2]).pin_memory()
+        return host.to(self.device, non_blocking=True)
+
     # -------------------------------------------------------------- epoch graph
-    def _capture(self, X, y, n_steps, batch_size, rows=None):
+    def _capture(self, X, y, n_steps, batch_size, rows=None, steps=None):
         """``rows``: with AdamW, the device row buffer captured step ``s`` reads row ``s`` of (holding the first
         epoch's rows, which the warm-up steps use too); kept in the returned entry.  With augmentation on, the
-        gather reads the entry's word buffer ``words``."""
+        gather reads the entry's word buffer ``words``; with mixing on, the entry's ``[steps, 8]`` mix rows ``mix``."""
         perm = torch.zeros(n_steps * batch_size, dtype=torch.int64, device=self.device)
         words = torch.zeros(3, dtype=torch.int32, device=self.device) if self._aug is not None else None
+        mixbuf = (torch.zeros(steps, MIX_ROW, dtype=torch.int32, device=self.device)
+                  if self._mix is not None and self._mix.kind is not None else None)
         perm.copy_(torch.arange(n_steps * batch_size, device=self.device) % X.shape[0])
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
@@ -419,7 +480,8 @@ class GraphedLocalSGD:
             snap_i = self.arena.int_arena.clone()
             snap_m = self.arena.momentum.clone() if self.arena.momentum is not None else None
             for _ in range(2):
-                self._step(X, y, perm[:batch_size], row=rows[0] if rows is not None else None, words=words)
+                self._step(X, y, perm[:batch_size], row=rows[0] if rows is not None else None, words=words,
+                           mix_rows=mixbuf, bsz=batch_size)
         torch.cuda.current_stream(self.device).wait_stream(side)
         torch.cuda.synchronize(self.device)
         from .ops._ext import total_launches
@@ -430,12 +492,13 @@ class GraphedLocalSGD:
         def body():
             # the epoch's batches are gathered by ONE launch pair (a permuted copy of the shard, 25 MB for the
             # flagship config) instead of two latency-bound gathers at the head of every step
-            Xp, yp = self._gather(X, y, perm, 0, words)
+            Xp, yp = self._gather(X, y, perm, 0, words, mixbuf, batch_size)
             for s in range(n_steps):
                 self._step(X, y, None, batch=(Xp[s * batch_size:(s + 1) * batch_size],
                                               yp[s * batch_size:(s + 1) * batch_size]),
                            emit_wire=(s == n_steps - 1 and self.pack is not None),
-                           row=rows[s] if rows is not None else None)
+                           row=rows[s] if rows is not None else None, s0=s * batch_size, mix_rows=mixbuf,
+                           bsz=batch_size)
             self.graph_emits_wire = self.pack is not None
 
         if (self.k3_join is not None and hasattr(self.model, "explicit_step")
@@ -481,7 +544,8 @@ class GraphedLocalSGD:
         self.arena.grad.zero_()
         self.arena.sync_shadow()
         self.loss_acc.zero_()
-        return {"graph": graph, "graph2": graph2, "perm": perm, "X": X, "y": y, "rows": rows, "words": words}
+        return {"graph": graph, "graph2": graph2, "perm": perm, "X": X, "y": y, "rows": rows, "words": words,
+                "mix": mixbuf}
 
     # -------------------------------------------------------------- evaluation
     def _eval_pass(self, X, y, batch_size, explicit):
@@ -573,13 +637,15 @@ class GraphedLocalSGD:
             prox_mu: float = 0.0, corr: Optional[torch.Tensor] = None, optimizer: str = "sgd",
             betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8, augment: Optional[str] = None,
             augment_padding: int = 4, augment_seed: Optional[int] = None, augment_stream: Optional[int] = None,
-            **_ignored):
+            mix: Optional[str] = None, mix_alpha: float = 1.0, label_smoothing: float = 0.0, **_ignored):
         """``prox_mu > 0``: FedProx toward ``arena.global_w``, the global model the round started from.  ``corr``:
         SCAFFOLD's correction ``c - c_i`` (fp32 device buffer of ``arena.n_param`` elements), added to every step's
         gradient; it is read at replay, so the caller may rewrite it between runs.  ``optimizer="adamw"``: the steps of
         a fresh ``torch.optim.AdamW(lr, betas, eps, weight_decay)`` instead of SGD.  ``augment``: random crop / flip
         in the batch gather (``data/augment.py``); ``augment_seed`` (None: a random key per trainer) and
-        ``augment_stream`` (None: this trainer's count of augmenting runs) pick the draws."""
+        ``augment_stream`` (None: this trainer's count of augmenting runs) pick the draws.  ``mix`` (with
+        ``mix_alpha``) and ``label_smoothing``: mixup / CutMix in the same gather and the soft-target loss
+        (``data/mix.py``), drawn from the same key and stream."""
         assert X.is_cuda, "GraphedLocalSGD needs a device-resident shard"
         prox_mu = check_prox_mu(prox_mu)
         if prox_mu > 0 and self.arena.global_w is None:
@@ -588,7 +654,9 @@ class GraphedLocalSGD:
         self.adam = check_optimizer(optimizer, momentum, self.nesterov, prox_mu, corr)
         if self.adam:
             betas, eps = check_adamw(betas, eps)
-        self._aug = _augment_setup(self._aug_streams, X, augment, augment_padding, augment_seed, augment_stream)
+        self._mix = _mix_setup(mix, mix_alpha, label_smoothing, self.loss_kind)
+        self._aug = _augment_setup(self._aug_streams, X, augment, augment_padding, augment_seed, augment_stream,
+                                   self._mix)
         nn.Module.train(self.model, True)
         n = X.shape[0]
         batch_size = min(batch_size, n)
@@ -606,16 +674,19 @@ class GraphedLocalSGD:
         table = self._adam_rows(lr, betas, eps, weight_decay, n_epoch, steps) if self.adam else None
         aug_words = self._aug_words(self._aug[2], n_epoch) if self._aug is not None else None
         aug_key = self._aug[:2] if self._aug is not None else None
+        mixing = self._mix is not None and self._mix.kind is not None
+        mix_table_dev = self._mix_rows(n_epoch, steps, X) if mixing else None
+        mix_key = (mixing, self._mix.smoothing) if self._mix is not None else None
         # the anchor and correction pointers are baked into the captured launches; the coefficient is read from `hyper`
         # at replay
         key = (n, batch_size, tuple(X.shape[1:]), tuple(y.shape[1:]), X.data_ptr(), y.data_ptr(), bool(momentum),
-               self.prox, corr.data_ptr() if corr is not None else None, self.adam, aug_key)
+               self.prox, corr.data_ptr() if corr is not None else None, self.adam, aug_key, mix_key)
         epoch_losses = torch.zeros(n_epoch, 2, dtype=torch.float32, device=self.device)
         if self.use_graph:
             ent = self._graphs.get(key)
             if ent is None:
                 rows = table[:steps].clone() if self.adam else None
-                ent = self._graphs[key] = self._capture(X, y, n_steps, batch_size, rows)
+                ent = self._graphs[key] = self._capture(X, y, n_steps, batch_size, rows, steps)
             perm_full = torch.randperm(n, device=self.device)
             for e in range(n_epoch):
                 if reshuffle_each_epoch and e > 0:
@@ -625,6 +696,8 @@ class GraphedLocalSGD:
                     ent["rows"].copy_(table[e * steps:(e + 1) * steps])
                 if aug_words is not None:
                     ent["words"].copy_(aug_words[e])
+                if mixing:
+                    ent["mix"].copy_(mix_table_dev[e])
                 self.loss_acc.zero_()
                 ent["graph"].replay()
                 if ent.get("graph2") is not None:
@@ -634,7 +707,7 @@ class GraphedLocalSGD:
                     with torch.enable_grad():
                         self._step(X, y, perm_full[n_steps * batch_size:], fuse_sgd=False,
                                    row=ent["rows"][n_steps] if self.adam else None, s0=n_steps * batch_size,
-                                   words=ent["words"])
+                                   words=ent["words"], mix_rows=ent["mix"], bsz=batch_size)
                 epoch_losses[e].copy_(self.loss_acc)
         else:
             perm_full = torch.randperm(n, device=self.device)
@@ -645,7 +718,8 @@ class GraphedLocalSGD:
                 for s, idx in enumerate(torch.split(perm_full, batch_size)):
                     with torch.enable_grad():
                         self._step(X, y, idx, row=table[e * steps + s] if self.adam else None, s0=s * batch_size,
-                                   words=aug_words[e] if aug_words is not None else None)
+                                   words=aug_words[e] if aug_words is not None else None,
+                                   mix_rows=mix_table_dev[e] if mixing else None, bsz=batch_size)
                 epoch_losses[e].copy_(self.loss_acc)
         self.last_steps = steps
         self.last_had_tail_step = bool(tail)        # a ragged eager step ran after the graph: its SGD did not emit the wire
@@ -678,16 +752,17 @@ class PortableLocalSGD:
             prox_mu: float = 0.0, corr: Optional[torch.Tensor] = None, optimizer: str = "sgd",
             betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8, augment: Optional[str] = None,
             augment_padding: int = 4, augment_seed: Optional[int] = None, augment_stream: Optional[int] = None,
-            **_ignored):
+            mix: Optional[str] = None, mix_alpha: float = 1.0, label_smoothing: float = 0.0, **_ignored):
         """``prox_mu > 0``: FedProx toward ``arena.global_w``, the global model the round started from.  ``corr``:
         SCAFFOLD's correction ``c - c_i`` (fp32, indexed like the arena's parameters), added to every gradient.
         ``optimizer="adamw"``: a fresh ``torch.optim.AdamW(lr, betas, eps, weight_decay)`` instead of SGD.
-        ``augment``: as in :meth:`GraphedLocalSGD.run`, through the host reference."""
+        ``augment``, ``mix``, ``label_smoothing``: as in :meth:`GraphedLocalSGD.run`, through the host references."""
         criterion = _loss_fn(self.loss_kind)
         prox_mu = check_prox_mu(prox_mu)
         _check_corr(corr, self.arena)
         adam = check_optimizer(optimizer, momentum, prox_mu=prox_mu, corr=corr)
-        aug = _augment_setup(self._aug_streams, X, augment, augment_padding, augment_seed, augment_stream)
+        mixc = _mix_setup(mix, mix_alpha, label_smoothing, self.loss_kind)
+        aug = _augment_setup(self._aug_streams, X, augment, augment_padding, augment_seed, augment_stream, mixc)
         n = X.shape[0]
         batch_size = min(batch_size, n)
         nn.Module.train(self.model, True)
@@ -712,13 +787,20 @@ class PortableLocalSGD:
                 perm = torch.randperm(n)
             batches = torch.split(perm, batch_size)
             steps = len(batches)
+            rows = _host_mix_rows(mixc, aug, X, e, steps)
             for b, idx in enumerate(batches):
                 opt.zero_grad(set_to_none=True)
-                pred = self.model(_host_batch(X, idx, aug, e, b * batch_size))
+                xb = _host_batch(X, idx, aug, e, b * batch_size)
                 tgt = y[idx]
+                if mixc is not None:
+                    xb, soft = mix_batch_reference(xb, tgt, rows[b] if rows is not None else None, mixc.smoothing)
+                pred = self.model(xb)
                 if pred.shape != tgt.shape and tgt.dtype.is_floating_point:
                     tgt = tgt.reshape(pred.shape)
-                loss = criterion(pred.float() if tgt.dtype.is_floating_point else pred, tgt)
+                if mixc is not None:
+                    loss = soft_cross_entropy(pred, soft)
+                else:
+                    loss = criterion(pred.float() if tgt.dtype.is_floating_point else pred, tgt)
                 loss.backward()
                 if prox_mu > 0:
                     _add_prox_term(params, anchors, prox_mu)
@@ -728,7 +810,9 @@ class PortableLocalSGD:
                             p.grad = cv.clone() if p.grad is None else p.grad.add_(cv)
                 opt.step()
                 out[e, 0] += float(loss.detach())
-                if not tgt.dtype.is_floating_point:
+                if mixc is not None:
+                    out[e, 1] += float(soft_hits(pred, soft))
+                elif not tgt.dtype.is_floating_point:
                     out[e, 1] += float((pred.argmax(-1) == tgt).sum())
         self.last_steps = steps
         if self.arena.theta_bf16 is not None:
