@@ -37,6 +37,7 @@ class FederationConfig:
     mix: str = "none"                  # batch mixing: none | mixup | cutmix | mixup_cutmix (NHWC images, cross-entropy)
     mix_alpha: float = 1.0             # lambda ~ Beta(mix_alpha, mix_alpha), one per batch
     label_smoothing: float = 0.0       # soft-target smoothing eps in [0, 1) of the training cross-entropy
+    max_grad_norm: float = 0.0         # clip_grad_norm_ of every local step's gradient to this 2-norm (0: off)
     dp_clip: float = 0.0               # DP-FedAvg: L2 clip norm of a client's update (0: DP off)
     dp_noise_multiplier: float = 0.0   # DP-FedAvg: noise std on the sum of clipped updates, in units of dp_clip
     dp_delta: float = 1e-5             # DP-FedAvg: delta of the (epsilon, delta) the manager reports
@@ -62,8 +63,9 @@ class FederationConfig:
     seed: int = 0
 
     def __post_init__(self):
-        from .train import check_adamw, check_prox_mu
+        from .train import check_adamw, check_max_grad_norm, check_prox_mu
         check_prox_mu(self.prox_mu)
+        check_max_grad_norm(self.max_grad_norm)
         check_adamw((self.adam_beta1, self.adam_beta2), self.adam_eps)
         from .data.augment import check_augment
         check_augment(self.augment, self.augment_padding)
@@ -98,6 +100,8 @@ class FederationConfig:
             kw.update(mix=self.mix, mix_alpha=self.mix_alpha)
         if self.label_smoothing != 0.0:
             kw.update(label_smoothing=self.label_smoothing)
+        if self.max_grad_norm > 0.0:
+            kw.update(max_grad_norm=self.max_grad_norm)
         return kw
 
     def dp_config(self):

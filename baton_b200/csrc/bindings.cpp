@@ -58,6 +58,12 @@ inline float* adam_v_ptr(const std::optional<at::Tensor>& v, int64_t numel, cons
   return v->data_ptr<float>();
 }
 
+// clipped optimizer step: the coefficient is hyper[5] of an SGD float[6], or row[9] of an AdamW step row
+inline void check_clip_hyper(bool clip, const at::Tensor& hyper, bool adam) {
+  TORCH_CHECK(!clip || hyper.numel() >= (adam ? 10 : 6),
+              "a clipped step reads its coefficient from hyper[5] (SGD, 6 floats) or row[9] (AdamW)");
+}
+
 // optimizer epilogue of a weight-gradient GEMM: theta / theta_bf16 / momentum / anchor / correction / second moment
 // start at the element of D[0, 0]
 inline std::optional<B200SgdEpilogue> sgd_epilogue(const std::optional<at::Tensor>& theta,
@@ -358,18 +364,20 @@ void fused_sgd(at::Tensor w, at::Tensor g, const std::optional<at::Tensor>& mom,
                const at::Tensor& hyper, bool zero_grad, bool nesterov, const std::optional<at::Tensor>& wire_slot,
                const std::optional<at::Tensor>& pack_global, const std::optional<at::Tensor>& pack_scale, int64_t n_pack,
                bool wire_fp32, const std::optional<at::Tensor>& prox_anchor_, const std::optional<at::Tensor>& corr,
-               const std::optional<at::Tensor>& adam_v) {
+               const std::optional<at::Tensor>& adam_v, bool clip) {
   CHECK_CUDA(w);
   TORCH_CHECK(w.scalar_type() == at::kFloat && g.scalar_type() == at::kFloat && hyper.scalar_type() == at::kFloat);
   TORCH_CHECK(w.is_contiguous() && g.is_contiguous() && w.numel() == g.numel());
   const c10::cuda::CUDAGuard guard(w.device());
   const float* anchor = prox_anchor(prox_anchor_, w.numel(), hyper);
   const float* c = scaf_corr(corr, w.numel(), anchor);
+  float* v = adam_v_ptr(adam_v, w.numel(), opt_ptr<float>(mom), hyper, anchor, c);
+  check_clip_hyper(clip, hyper, v != nullptr);
   check(b200_fused_sgd(w.data_ptr<float>(), g.data_ptr<float>(), opt_ptr<float>(mom), opt_ptr<void>(wb), w.numel(),
                        hyper.data_ptr<float>(), zero_grad, nesterov,
                        reinterpret_cast<const unsigned long long*>(opt_ptr<const int64_t>(wire_slot)),
                        opt_ptr<const float>(pack_global), opt_ptr<const float>(pack_scale), n_pack, wire_fp32, anchor,
-                       c, adam_v_ptr(adam_v, w.numel(), opt_ptr<float>(mom), hyper, anchor, c), cur_stream()),
+                       c, v, clip ? 1 : 0, cur_stream()),
         "fused_sgd");
 }
 
@@ -377,7 +385,7 @@ void fused_sgd(at::Tensor w, at::Tensor g, const std::optional<at::Tensor>& mom,
 void fused_sgd_segments(at::Tensor w, at::Tensor g, const std::optional<at::Tensor>& mom,
                         const std::optional<at::Tensor>& wb, const at::Tensor& segments, const at::Tensor& hyper,
                         bool nesterov, const std::optional<at::Tensor>& prox_anchor_,
-                        const std::optional<at::Tensor>& corr, const std::optional<at::Tensor>& adam_v) {
+                        const std::optional<at::Tensor>& corr, const std::optional<at::Tensor>& adam_v, bool clip) {
   CHECK_CUDA(w); CHECK_CUDA(segments);
   TORCH_CHECK(w.scalar_type() == at::kFloat && g.scalar_type() == at::kFloat && hyper.scalar_type() == at::kFloat);
   TORCH_CHECK(segments.scalar_type() == at::kLong && segments.dim() == 2 && segments.size(1) == 3 &&
@@ -385,11 +393,30 @@ void fused_sgd_segments(at::Tensor w, at::Tensor g, const std::optional<at::Tens
   const c10::cuda::CUDAGuard guard(w.device());
   const float* anchor = prox_anchor(prox_anchor_, w.numel(), hyper);
   const float* c = scaf_corr(corr, g.numel(), anchor);
+  float* v = adam_v_ptr(adam_v, g.numel(), opt_ptr<float>(mom), hyper, anchor, c);
+  check_clip_hyper(clip, hyper, v != nullptr);
   check(b200_fused_sgd_segments(w.data_ptr<float>(), g.data_ptr<float>(), opt_ptr<float>(mom), opt_ptr<void>(wb),
                                 reinterpret_cast<const long long*>(segments.data_ptr<int64_t>()),
-                                static_cast<int>(segments.size(0)), hyper.data_ptr<float>(), nesterov, anchor, c,
-                                adam_v_ptr(adam_v, g.numel(), opt_ptr<float>(mom), hyper, anchor, c), cur_stream()),
+                                static_cast<int>(segments.size(0)), hyper.data_ptr<float>(), nesterov, anchor, c, v,
+                                clip ? 1 : 0, cur_stream()),
         "fused_sgd_segments");
+}
+
+// gradient-norm clipping: the norm of g (fp32, contiguous, 16-byte aligned) and the clip coefficient of the fp32
+// threshold max_norm[0], written to norm_out[0] and coef_out[0]; work: int64 [GRAD_NORM_WORK_WORDS], zeroed once
+void grad_norm_clip(const at::Tensor& g, const at::Tensor& max_norm, at::Tensor work, at::Tensor norm_out,
+                    at::Tensor coef_out) {
+  CHECK_CUDA(g); CHECK_CUDA(max_norm); CHECK_CUDA(work); CHECK_CUDA(norm_out); CHECK_CUDA(coef_out);
+  TORCH_CHECK(g.scalar_type() == at::kFloat && g.is_contiguous(), "grad_norm_clip: contiguous fp32 gradient");
+  TORCH_CHECK(work.scalar_type() == at::kLong && work.numel() >= B200_GRAD_NORM_WORK_WORDS,
+              "grad_norm_clip: int64 work");
+  TORCH_CHECK(max_norm.scalar_type() == at::kFloat && norm_out.scalar_type() == at::kFloat &&
+              coef_out.scalar_type() == at::kFloat && max_norm.numel() >= 1 && norm_out.numel() >= 1 &&
+              coef_out.numel() >= 1, "grad_norm_clip: fp32 threshold and outputs");
+  const c10::cuda::CUDAGuard guard(g.device());
+  check(b200_grad_norm_clip(g.data_ptr<float>(), g.numel(), max_norm.data_ptr<float>(), work.data_ptr(),
+                            norm_out.data_ptr<float>(), coef_out.data_ptr<float>(), cur_stream()),
+        "grad_norm_clip");
 }
 
 // SCAFFOLD control variates over the parameters: every buffer fp32, contiguous, at least n elements
@@ -1276,6 +1303,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("quant_mx_cols", &quant_mx_cols);
   m.def("fused_sgd", &fused_sgd);
   m.def("fused_sgd_segments", &fused_sgd_segments);
+  m.def("grad_norm_clip", &grad_norm_clip);
+  m.attr("GRAD_NORM_WORK_WORDS") = B200_GRAD_NORM_WORK_WORDS;
   m.def("weighted_sum", &weighted_sum);
   m.def("fold_client", &fold_client);
   m.def("scaffold_corr", &scaffold_corr);

@@ -21,6 +21,24 @@ static inline int ew_grid(long long n_vec, int max_ctas = device_sm_count() * 8)
   return static_cast<int>(g);
 }
 
+// fp32 product and sum rounded to nearest, each on its own and without flushing subnormals (the build's fast-math flag
+// turns __fmul_rn / __fadd_rn into their .ftz forms; torch on the host keeps subnormals)
+__device__ __forceinline__ float mul_rn(float a, float b) {
+  float r;
+  asm("mul.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+__device__ __forceinline__ float add_rn(float a, float b) {
+  float r;
+  asm("add.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+__device__ __forceinline__ float rcp_rn(float a) {
+  float r;
+  asm("rcp.rn.f32 %0, %1;" : "=f"(r) : "f"(a));
+  return r;
+}
+
 // ------------------------------------------------------------------ fused SGD over the arena
 // One pass over {w, g, m}: the update of sgd.cuh ; g = 0 (so split-K wgrad GEMMs can red.add into it next step) ;
 // bf16 shadow = bf16(w).
@@ -49,11 +67,32 @@ __device__ __forceinline__ void sgd_pack4(const SgdPack& pk, uint8_t* wire, floa
   else reinterpret_cast<uint2*>(wire)[i] = make_uint2(pack_bf16x2(d.x, d.y), pack_bf16x2(d.z, d.w));
 }
 
+// The gradient of a clipped step, g' = fl32(g * coef) (clip_grad_norm_ multiplies even when coef is 1)
+__device__ __forceinline__ float4 clip4(float4 g, float c) {
+  return make_float4(mul_rn(g.x, c), mul_rn(g.y, c), mul_rn(g.z, c), mul_rn(g.w, c));
+}
+// The clip coefficient, written by the norm kernel this kernel waits on (programmatic dependent launch).  A plain load
+// through the `const __restrict__` hyper pointer may be issued as a read-only load ahead of griddep_wait(); this one
+// cannot move across it.
+__device__ __forceinline__ float load_clip_coef(const float* p) {
+  float r;
+  asm volatile("ld.relaxed.gpu.global.f32 %0, [%1];" : "=f"(r) : "l"(p) : "memory");
+  return r;
+}
+// float4 group i of the gradient, clipped when CLIP
+template <bool CLIP>
+__device__ __forceinline__ float4 load_grad4(float* g, long long i, float coef) {
+  if constexpr (CLIP) return clip4(reinterpret_cast<float4*>(g)[i], coef);
+  return reinterpret_cast<float4*>(g)[i];
+}
+
 // Body of the AdamW form of fused_sgd_kernel: the same passes (update + gradient zeroing + bf16 shadow + upload copy,
-// then the pack-only float buffers, then the scalar tail) with adamw_update in place of the SGD step.
+// then the pack-only float buffers, then the scalar tail) with adamw_update in place of the SGD step.  CLIP: the
+// gradient is multiplied by `coef` as it is loaded.
+template <bool CLIP>
 __device__ __forceinline__ void adamw_arena(float* __restrict__ w, float* __restrict__ g, float* __restrict__ m,
                                             float* __restrict__ v, __nv_bfloat16* __restrict__ wb, long long n,
-                                            const AdamHyper h, int zero_grad, const SgdPack& pk) {
+                                            const AdamHyper h, float coef, int zero_grad, const SgdPack& pk) {
   const long long nv = n >> 2;
   uint8_t* wire = nullptr;
   float pscale = 1.f;
@@ -64,8 +103,7 @@ __device__ __forceinline__ void adamw_arena(float* __restrict__ w, float* __rest
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < nv; i += stride) {
     float4 mv = reinterpret_cast<const float4*>(m)[i], vv = reinterpret_cast<const float4*>(v)[i];
-    const float4 wv = adamw_update4(h, reinterpret_cast<const float4*>(w)[i], reinterpret_cast<const float4*>(g)[i],
-                                    mv, vv);
+    const float4 wv = adamw_update4(h, reinterpret_cast<const float4*>(w)[i], load_grad4<CLIP>(g, i, coef), mv, vv);
     reinterpret_cast<float4*>(m)[i] = mv;
     reinterpret_cast<float4*>(v)[i] = vv;
     reinterpret_cast<float4*>(w)[i] = wv;
@@ -80,7 +118,7 @@ __device__ __forceinline__ void adamw_arena(float* __restrict__ w, float* __rest
   }
   if (blockIdx.x == 0) {
     for (long long i = (nv << 2) + threadIdx.x; i < n; i += blockDim.x) {
-      const float wv = adamw_update(h, w[i], g[i], m[i], v[i]);
+      const float wv = adamw_update(h, w[i], CLIP ? mul_rn(g[i], coef) : g[i], m[i], v[i]);
       w[i] = wv;
       if (zero_grad) g[i] = 0.f;
       if (wb != nullptr) wb[i] = __float2bfloat16_rn(wv);
@@ -94,7 +132,9 @@ __device__ __forceinline__ void adamw_arena(float* __restrict__ w, float* __rest
 // ADAM: the AdamW step of sgd.cuh instead of SGD.  `hyper` is then the step's AdamW row (ADAMW_ROW floats), `mom` the
 // first moment m and `aux` the second moment v, which this form also writes (each element is read once, by the thread
 // that writes it); `nesterov` is not read.
-template <bool PROX, bool SCAF = false, bool ADAM = false>
+// CLIP: gradient-norm clipping -- g is multiplied by the coefficient hyper[SGD_HYPER_CLIP] (AdamW: row[ADAMW_ROW_CLIP])
+// as it is loaded, before any other term; everything else is the unclipped form's.
+template <bool PROX, bool SCAF = false, bool ADAM = false, bool CLIP = false>
 __global__ void __launch_bounds__(EW_THREADS)
 fused_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict__ mom,
                  __nv_bfloat16* __restrict__ wb, long long n, const float* __restrict__ hyper, int zero_grad,
@@ -104,10 +144,12 @@ fused_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict
   griddep_launch_dependents();
   griddep_wait();
   if constexpr (ADAM) {
-    adamw_arena(w, g, mom, const_cast<float*>(aux), wb, n, load_adam_hyper(hyper), zero_grad, pk);
+    adamw_arena<CLIP>(w, g, mom, const_cast<float*>(aux), wb, n, load_adam_hyper(hyper),
+                      CLIP ? load_clip_coef(hyper + ADAMW_ROW_CLIP) : 1.f, zero_grad, pk);
     return;
   }
   const SgdHyper h = PROX ? load_sgd_hyper_prox(hyper) : load_sgd_hyper(hyper);
+  const float coef = CLIP ? load_clip_coef(hyper + SGD_HYPER_CLIP) : 1.f;
   const long long nv = n >> 2;
   uint8_t* wire = nullptr;
   float pscale = 1.f;
@@ -124,13 +166,13 @@ fused_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict
     float4 wv;
     if constexpr (PROX) {
       av = reinterpret_cast<const float4*>(aux)[i];
-      wv = sgd_update4_prox(h, reinterpret_cast<float4*>(w)[i], reinterpret_cast<float4*>(g)[i], av, mv,
+      wv = sgd_update4_prox(h, reinterpret_cast<float4*>(w)[i], load_grad4<CLIP>(g, i, coef), av, mv,
                             mom != nullptr, nesterov);
     } else if constexpr (SCAF) {
-      wv = sgd_update4_scaf(h, reinterpret_cast<float4*>(w)[i], reinterpret_cast<float4*>(g)[i],
+      wv = sgd_update4_scaf(h, reinterpret_cast<float4*>(w)[i], load_grad4<CLIP>(g, i, coef),
                             reinterpret_cast<const float4*>(aux)[i], mv, mom != nullptr, nesterov);
     } else {
-      wv = sgd_update4(h, reinterpret_cast<float4*>(w)[i], reinterpret_cast<float4*>(g)[i], mv, mom != nullptr,
+      wv = sgd_update4(h, reinterpret_cast<float4*>(w)[i], load_grad4<CLIP>(g, i, coef), mv, mom != nullptr,
                        nesterov);
     }
     if (mom != nullptr) reinterpret_cast<float4*>(mom)[i] = mv;
@@ -166,9 +208,11 @@ fused_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict
   if (blockIdx.x == 0) {
     for (long long i = (nv << 2) + threadIdx.x; i < n; i += blockDim.x) {
       float mv = mom != nullptr ? mom[i] : 0.f;
-      const float wv = PROX ? sgd_update_prox(h, w[i], g[i], aux[i], mv, mom != nullptr, nesterov)
-                       : SCAF ? sgd_update_scaf(h, w[i], g[i], aux[i], mv, mom != nullptr, nesterov)
-                              : sgd_update(h, w[i], g[i], mv, mom != nullptr, nesterov);
+      const float wv = PROX ? sgd_update_prox(h, w[i], CLIP ? mul_rn(g[i], coef) : g[i], aux[i], mv, mom != nullptr,
+                                              nesterov)
+                       : SCAF ? sgd_update_scaf(h, w[i], CLIP ? mul_rn(g[i], coef) : g[i], aux[i], mv, mom != nullptr,
+                                                nesterov)
+                              : sgd_update(h, w[i], CLIP ? mul_rn(g[i], coef) : g[i], mv, mom != nullptr, nesterov);
       if (mom != nullptr) mom[i] = mv;
       w[i] = wv;
       if (zero_grad) g[i] = 0.f;
@@ -188,9 +232,12 @@ __device__ __forceinline__ bool same_bits4(float4 a, float4 b) {
 // at the first step, where they are processed once so that their stored m and v really are 0 for the whole-arena
 // steps of the run (the momentum buffer may hold an earlier SGD run's momentum).  The skip is decided from the step
 // row in device memory, so a captured epoch stays exact.  Kind-1 weights are stored only where their bits change.
+// CLIP: kind-0 gradients are multiplied by `coef` as they are loaded.
+template <bool CLIP>
 __device__ __forceinline__ void adamw_segments(float* __restrict__ w, float* __restrict__ g, float* __restrict__ m,
                                                float* __restrict__ v, __nv_bfloat16* __restrict__ wb,
-                                               const long long* __restrict__ seg, int n_seg, const AdamHyper h) {
+                                               const long long* __restrict__ seg, int n_seg, const AdamHyper h,
+                                               float coef) {
   const bool nograd_is_identity = h.decay == 1.f && !h.first;
   for (int s = blockIdx.x; s < n_seg; s += gridDim.x) {
     const long long off = seg[3 * s], len = seg[3 * s + 1];
@@ -202,7 +249,8 @@ __device__ __forceinline__ void adamw_segments(float* __restrict__ w, float* __r
       for (long long i = threadIdx.x; i < nv; i += blockDim.x) {
         const long long e = off + (i << 2);
         float4 mv = *reinterpret_cast<const float4*>(m + e), vv = *reinterpret_cast<const float4*>(v + e);
-        const float4 gv = has_grad ? *reinterpret_cast<const float4*>(g + e) : make_float4(0.f, 0.f, 0.f, 0.f);
+        float4 gv = has_grad ? *reinterpret_cast<const float4*>(g + e) : make_float4(0.f, 0.f, 0.f, 0.f);
+        if constexpr (CLIP) gv = has_grad ? clip4(gv, coef) : gv;
         const float4 w0 = *reinterpret_cast<const float4*>(w + e);
         const float4 wv = adamw_update4(h, w0, gv, mv, vv);
         *reinterpret_cast<float4*>(m + e) = mv;
@@ -217,7 +265,7 @@ __device__ __forceinline__ void adamw_segments(float* __restrict__ w, float* __r
     for (long long i = done + threadIdx.x; i < len; i += blockDim.x) {
       const long long e = off + i;
       const float w0 = w[e];
-      const float wv = adamw_update(h, w0, has_grad ? g[e] : 0.f, m[e], v[e]);
+      const float wv = adamw_update(h, w0, has_grad ? (CLIP ? mul_rn(g[e], coef) : g[e]) : 0.f, m[e], v[e]);
       if (!has_grad && __float_as_uint(w0) == __float_as_uint(wv)) continue;
       w[e] = wv;
       if (has_grad) g[e] = 0.f;
@@ -239,7 +287,9 @@ __device__ __forceinline__ void adamw_segments(float* __restrict__ w, float* __r
 // SCAF (`aux` = the correction c - c_i, as in fused_sgd_kernel): a kind-1 element moves by -lr * (corr [+ wd*w]), so
 // kind-1 chunks are never skipped; they use the same sparse store (a zero correction writes nothing).
 // ADAM (`hyper` = the AdamW step row, `mom` = m, `aux` = v, as in fused_sgd_kernel): see adamw_segments.
-template <bool PROX, bool SCAF = false, bool ADAM = false>
+// CLIP (as in fused_sgd_kernel): kind-0 gradients are multiplied by the clip coefficient as they are loaded; a kind-1
+// gradient is 0 and stays 0, so kind-1 chunks are skipped (or not) exactly as without clipping.
+template <bool PROX, bool SCAF = false, bool ADAM = false, bool CLIP = false>
 __global__ void __launch_bounds__(EW_THREADS)
 fused_sgd_segments_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict__ mom,
                           __nv_bfloat16* __restrict__ wb, const long long* __restrict__ seg, int n_seg,
@@ -249,10 +299,12 @@ fused_sgd_segments_kernel(float* __restrict__ w, float* __restrict__ g, float* _
   griddep_launch_dependents();
   griddep_wait();
   if constexpr (ADAM) {
-    adamw_segments(w, g, mom, const_cast<float*>(aux), wb, seg, n_seg, load_adam_hyper(hyper));
+    adamw_segments<CLIP>(w, g, mom, const_cast<float*>(aux), wb, seg, n_seg, load_adam_hyper(hyper),
+                         CLIP ? load_clip_coef(hyper + ADAMW_ROW_CLIP) : 1.f);
     return;
   }
   const SgdHyper h = PROX ? load_sgd_hyper_prox(hyper) : load_sgd_hyper(hyper);
+  const float coef = CLIP ? load_clip_coef(hyper + SGD_HYPER_CLIP) : 1.f;
   const bool has_mom = mom != nullptr;
   const bool nograd_is_identity = !SCAF && h.prox == 0.f && h.wd == 0.f && !has_mom;
   for (int s = blockIdx.x; s < n_seg; s += gridDim.x) {
@@ -266,7 +318,8 @@ fused_sgd_segments_kernel(float* __restrict__ w, float* __restrict__ g, float* _
       for (long long i = threadIdx.x; i < nv; i += blockDim.x) {
         const long long e = off + (i << 2);
         float4 mv = has_mom ? *reinterpret_cast<float4*>(mom + e) : make_float4(0.f, 0.f, 0.f, 0.f);
-        const float4 gv = has_grad ? *reinterpret_cast<float4*>(g + e) : make_float4(0.f, 0.f, 0.f, 0.f);
+        float4 gv = has_grad ? *reinterpret_cast<float4*>(g + e) : make_float4(0.f, 0.f, 0.f, 0.f);
+        if constexpr (CLIP) gv = has_grad ? clip4(gv, coef) : gv;
         const float4 w0 = *reinterpret_cast<float4*>(w + e);
         const float4 wv = PROX ? sgd_update4_prox(h, w0, gv, *reinterpret_cast<const float4*>(aux + e), mv, has_mom,
                                                   nesterov)
@@ -284,7 +337,7 @@ fused_sgd_segments_kernel(float* __restrict__ w, float* __restrict__ g, float* _
     for (long long i = done + threadIdx.x; i < len; i += blockDim.x) {
       const long long e = off + i;
       float mv = has_mom ? mom[e] : 0.f;
-      const float gv = has_grad ? g[e] : 0.f;
+      const float gv = has_grad ? (CLIP ? mul_rn(g[e], coef) : g[e]) : 0.f;
       const float w0 = w[e];
       const float wv = PROX ? sgd_update_prox(h, w0, gv, aux[e], mv, has_mom, nesterov)
                        : SCAF ? sgd_update_scaf(h, w0, gv, aux[e], mv, has_mom, nesterov)
@@ -296,6 +349,65 @@ fused_sgd_segments_kernel(float* __restrict__ w, float* __restrict__ g, float* _
       if (wb != nullptr) wb[e] = __float2bfloat16_rn(wv);
     }
   }
+}
+
+// ------------------------------------------------------------------ gradient-norm clipping (clip_grad_norm_)
+// norm = ||g[0, n)|| over a FIXED grid of B200_GRAD_NORM_BLOCKS CTAs (independent of the SM count): squares and sums in
+// fp64, one fp64 partial per CTA in work[0, B), and the last CTA to arrive (counter work[B], reset by it) sums them in
+// index order -- dp_clip_factor_kernel's pattern, so the norm is a pure function of the gradient's values and n, graph
+// or eager.  work[B + 1] keeps the fp64 sum of squares.  Then, as torch computes it from its fp32 norm,
+//     coef = clamp(fl32(fl32(1 / fl32(norm + 1e-6)) * max_norm), max = 1)
+// with IEEE-rounded, non-flushing operations (a NaN norm gives NaN, an infinite one 0).  `max_norm` is read from device
+// memory so a captured step follows a new threshold; norm and coef are written to device memory.
+constexpr int GRAD_NORM_THREADS = 256;
+__device__ __forceinline__ double add_squares4(float4 a, double d) {
+  const double x = a.x, y = a.y, z = a.z, w = a.w;
+  return fma(w, w, fma(z, z, fma(y, y, fma(x, x, d))));
+}
+__global__ void __launch_bounds__(GRAD_NORM_THREADS)
+grad_norm_clip_kernel(const float* __restrict__ g, long long n, const float* __restrict__ max_norm,
+                      unsigned long long* __restrict__ work, float* __restrict__ norm_out, float* __restrict__ coef_out) {
+  __shared__ double red[GRAD_NORM_THREADS / 32];
+  __shared__ bool last;
+  griddep_launch_dependents();
+  griddep_wait();
+  const long long nv = n >> 2;
+  const long long stride = static_cast<long long>(B200_GRAD_NORM_BLOCKS) * GRAD_NORM_THREADS;
+  double d0 = 0.0, d1 = 0.0;        // two loads in flight per thread
+  long long i = blockIdx.x * static_cast<long long>(GRAD_NORM_THREADS) + threadIdx.x;
+  for (; i + stride < nv; i += 2 * stride) {
+    const float4 a = reinterpret_cast<const float4*>(g)[i], b = reinterpret_cast<const float4*>(g)[i + stride];
+    d0 = add_squares4(a, d0);
+    d1 = add_squares4(b, d1);
+  }
+  if (i < nv) d0 = add_squares4(reinterpret_cast<const float4*>(g)[i], d0);
+  if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {     // scalar tail
+    const double t = g[(nv << 2) + threadIdx.x];
+    d1 = fma(t, t, d1);
+  }
+  double d = d0 + d1;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = d;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double b = 0.0;
+    for (int w = 0; w < GRAD_NORM_THREADS / 32; ++w) b += red[w];
+    reinterpret_cast<double*>(work)[blockIdx.x] = b;
+    __threadfence();
+    last = atomicAdd(work + B200_GRAD_NORM_BLOCKS, 1ull) == B200_GRAD_NORM_BLOCKS - 1;
+  }
+  __syncthreads();
+  if (!last || threadIdx.x != 0) return;
+  __threadfence();
+  double sq = 0.0;
+  for (int b = 0; b < B200_GRAD_NORM_BLOCKS; ++b) sq += reinterpret_cast<const volatile double*>(work)[b];
+  work[B200_GRAD_NORM_BLOCKS] = 0ull;
+  reinterpret_cast<double*>(work)[B200_GRAD_NORM_BLOCKS + 1] = sq;
+  const float norm = static_cast<float>(sqrt(sq));
+  const float c = mul_rn(rcp_rn(add_rn(norm, 1e-6f)), *max_norm);
+  norm_out[0] = norm;
+  coef_out[0] = c > 1.f ? 1.f : c;
 }
 
 // ------------------------------------------------------------------ logical-client fold (time-sliced clients on one GPU)
@@ -565,18 +677,6 @@ gather_augment_kernel(const uint8_t* __restrict__ src, const long long* __restri
 constexpr int MIX_ROW = 8;
 constexpr int MIX_CUTMIX = 1;
 
-// fp32 product and sum rounded to nearest, each on its own and without flushing subnormals (the build's fast-math flag
-// turns __fmul_rn / __fadd_rn into their .ftz forms; torch on the host keeps subnormals)
-__device__ __forceinline__ float mul_rn(float a, float b) {
-  float r;
-  asm("mul.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
-  return r;
-}
-__device__ __forceinline__ float add_rn(float a, float b) {
-  float r;
-  asm("add.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
-  return r;
-}
 template <int ES>
 __device__ __forceinline__ uint32_t mix_elem(uint32_t a, uint32_t b, float lam, float lam1, int fp16) {
   if constexpr (ES == 4) {
@@ -916,7 +1016,8 @@ using namespace b200;
 extern "C" int b200_fused_sgd(float* w, float* g, float* mom, void* w_bf16, long long n, const float* hyper,
                               int zero_grad, int nesterov, const unsigned long long* wire_slot,
                               const float* pack_global, const float* pack_scale, long long n_pack, int wire_fp32,
-                              const float* prox_anchor, const float* corr, float* adam_v, cudaStream_t stream) {
+                              const float* prox_anchor, const float* corr, float* adam_v, int clip,
+                              cudaStream_t stream) {
   if (n <= 0) return 0;
   SgdPack pk;
   pk.wire_slot = wire_slot; pk.global_w = pack_global; pk.scale = pack_scale;
@@ -928,10 +1029,14 @@ extern "C" int b200_fused_sgd(float* w, float* g, float* mom, void* w_bf16, long
   if ((reinterpret_cast<uintptr_t>(prox_anchor) | reinterpret_cast<uintptr_t>(corr) |
        reinterpret_cast<uintptr_t>(adam_v)) & 15)
     return -2;
-  auto kernel = adam_v != nullptr      ? fused_sgd_kernel<false, false, true>
-                : prox_anchor != nullptr ? fused_sgd_kernel<true>
-                : corr != nullptr      ? fused_sgd_kernel<false, true>
-                                       : fused_sgd_kernel<false>;
+  auto kernel = clip ? (adam_v != nullptr        ? fused_sgd_kernel<false, false, true, true>
+                       : prox_anchor != nullptr ? fused_sgd_kernel<true, false, false, true>
+                       : corr != nullptr        ? fused_sgd_kernel<false, true, false, true>
+                                                : fused_sgd_kernel<false, false, false, true>)
+                     : (adam_v != nullptr        ? fused_sgd_kernel<false, false, true>
+                       : prox_anchor != nullptr ? fused_sgd_kernel<true>
+                       : corr != nullptr        ? fused_sgd_kernel<false, true>
+                                                : fused_sgd_kernel<false>);
   launch_pdl(kernel, ew_grid(n >> 2), EW_THREADS, 0, stream, w, g, mom, reinterpret_cast<__nv_bfloat16*>(w_bf16), n,
              hyper, zero_grad, nesterov, pk,
              adam_v != nullptr ? adam_v : prox_anchor != nullptr ? prox_anchor : corr);
@@ -939,7 +1044,7 @@ extern "C" int b200_fused_sgd(float* w, float* g, float* mom, void* w_bf16, long
 }
 extern "C" int b200_fused_sgd_segments(float* w, float* g, float* mom, void* w_bf16, const long long* segments, int n_seg,
                                        const float* hyper, int nesterov, const float* prox_anchor, const float* corr,
-                                       float* adam_v, cudaStream_t stream) {
+                                       float* adam_v, int clip, cudaStream_t stream) {
   if (n_seg <= 0) return 0;
   if ((reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(mom) |
        reinterpret_cast<uintptr_t>(prox_anchor) | reinterpret_cast<uintptr_t>(corr) |
@@ -948,13 +1053,25 @@ extern "C" int b200_fused_sgd_segments(float* w, float* g, float* mom, void* w_b
     return -2;
   if (prox_anchor != nullptr && corr != nullptr) return -2;
   if (adam_v != nullptr && (prox_anchor != nullptr || corr != nullptr || mom == nullptr)) return -2;
-  auto kernel = adam_v != nullptr        ? fused_sgd_segments_kernel<false, false, true>
-                : prox_anchor != nullptr ? fused_sgd_segments_kernel<true>
-                : corr != nullptr      ? fused_sgd_segments_kernel<false, true>
-                                       : fused_sgd_segments_kernel<false>;
+  auto kernel = clip ? (adam_v != nullptr        ? fused_sgd_segments_kernel<false, false, true, true>
+                       : prox_anchor != nullptr ? fused_sgd_segments_kernel<true, false, false, true>
+                       : corr != nullptr        ? fused_sgd_segments_kernel<false, true, false, true>
+                                                : fused_sgd_segments_kernel<false, false, false, true>)
+                     : (adam_v != nullptr        ? fused_sgd_segments_kernel<false, false, true>
+                       : prox_anchor != nullptr ? fused_sgd_segments_kernel<true>
+                       : corr != nullptr        ? fused_sgd_segments_kernel<false, true>
+                                                : fused_sgd_segments_kernel<false>);
   launch_pdl(kernel, ew_grid(n_seg * static_cast<long long>(EW_THREADS)), EW_THREADS, 0, stream, w, g, mom,
              reinterpret_cast<__nv_bfloat16*>(w_bf16), segments, n_seg, hyper, nesterov,
              adam_v != nullptr ? adam_v : prox_anchor != nullptr ? prox_anchor : corr);
+  RET_LAST();
+}
+extern "C" int b200_grad_norm_clip(const float* g, long long n, const float* max_norm, void* work, float* norm_out,
+                                   float* coef_out, cudaStream_t stream) {
+  if (n < 0 || max_norm == nullptr || work == nullptr || norm_out == nullptr || coef_out == nullptr) return -2;
+  if (reinterpret_cast<uintptr_t>(g) & 15) return -2;
+  launch_pdl(grad_norm_clip_kernel, B200_GRAD_NORM_BLOCKS, GRAD_NORM_THREADS, 0, stream, g, n, max_norm,
+             static_cast<unsigned long long*>(work), norm_out, coef_out);
   RET_LAST();
 }
 extern "C" int b200_scaffold_corr(float* corr, const float* c, const float* ci, long long n, cudaStream_t stream) {

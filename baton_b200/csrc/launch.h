@@ -95,12 +95,21 @@ int b200_gemm_simt(const void* a, const void* b, void* d, const float* bias, int
 int b200_fused_sgd(float* w, float* g, float* mom, void* w_bf16, long long n, const float* hyper, int zero_grad,
                    int nesterov, const unsigned long long* wire_slot, const float* pack_global,
                    const float* pack_scale, long long n_pack, int wire_fp32, const float* prox_anchor,
-                   const float* corr, float* adam_v, cudaStream_t stream);
+                   const float* corr, float* adam_v, int clip, cudaStream_t stream);
 // the same step over a device table of n_seg arena chunks {offset, length, kind} (int64 [n_seg][3]); kind 0: with a
 // gradient (zeroed afterwards), kind 1: gradient identically zero (never read)
 int b200_fused_sgd_segments(float* w, float* g, float* mom, void* w_bf16, const long long* segments, int n_seg,
                             const float* hyper, int nesterov, const float* prox_anchor, const float* corr,
-                            float* adam_v, cudaStream_t stream);
+                            float* adam_v, int clip, cudaStream_t stream);
+// Gradient-norm clipping (clip_grad_norm_): norm_out[0] = ||g[0, n)|| (fp32; accumulated in fp64 with a fixed grid and
+// summation order) and coef_out[0] = min(max_norm[0] / (norm + 1e-6), 1) as torch rounds it.  work: int64
+// [B200_GRAD_NORM_WORK_WORDS], zero on first use (partials, arrival counter, fp64 sum of squares); g 16-byte aligned.
+// clip != 0 in the two calls above selects their clipped forms, which multiply g by hyper[5] (SGD: hyper is then
+// float[6]) or by row[9] (AdamW) as they load it.
+#define B200_GRAD_NORM_BLOCKS 528
+#define B200_GRAD_NORM_WORK_WORDS (B200_GRAD_NORM_BLOCKS + 2)
+int b200_grad_norm_clip(const float* g, long long n, const float* max_norm, void* work, float* norm_out,
+                        float* coef_out, cudaStream_t stream);
 // SCAFFOLD control variates over n parameters (n % 4 == 0, 16-byte aligned): corr = c - c_i before a client trains;
 // after it trained, dc = (global_w - theta) * inv_k_eta - c, c_i += dc, up = dc (first != 0) or up += dc
 int b200_scaffold_corr(float* corr, const float* c, const float* ci, long long n, cudaStream_t stream);

@@ -21,6 +21,10 @@ __device__ __forceinline__ SgdHyper load_sgd_hyper(const float* h) { return SgdH
 __device__ __forceinline__ SgdHyper load_sgd_hyper_prox(const float* h) {
   return SgdHyper{h[0], h[1], h[2], h[3], h[4]};
 }
+// Gradient-norm clipping: the coefficient g is multiplied by before the step (clip_grad_norm_), written on the device by
+// the norm kernel into a spare float of the step's hyper-parameters -- hyper[SGD_HYPER_CLIP] of the SGD float[6], or
+// [ADAMW_ROW_CLIP] of the AdamW row.  Only the CLIP instantiations of the arena kernels read it.
+constexpr int SGD_HYPER_CLIP = 5;
 
 // momentum and learning rate on the full gradient g' (weight decay and proximal term already added)
 __device__ __forceinline__ float sgd_apply(const SgdHyper& h, float w, float g, float& m, bool has_mom, bool nesterov) {
@@ -86,6 +90,7 @@ __device__ __forceinline__ float4 sgd_update4_scaf(const SgdHyper& h, float4 w, 
 // captured warm-up steps need no reset pass.  The operations are the IEEE-rounded intrinsics so that fast-math builds
 // cannot contract them differently at the three sites.
 constexpr int ADAMW_ROW = 12;   // floats per step row (48 B): the fields of AdamHyper, then padding
+constexpr int ADAMW_ROW_CLIP = 9;   // the clip coefficient of a clipped step (padding otherwise)
 
 struct AdamHyper {
   float decay;          // 1 - lr*wd

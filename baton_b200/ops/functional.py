@@ -171,8 +171,12 @@ def gemm_stats_fusable(M: int, N: int, K: int) -> bool:
 def fused_sgd(w: torch.Tensor, g: torch.Tensor, hyper: torch.Tensor, momentum_buf: Optional[torch.Tensor] = None,
               w_bf16: Optional[torch.Tensor] = None, zero_grad: bool = True, nesterov: bool = False,
               pack: Optional[dict] = None, prox_anchor: Optional[torch.Tensor] = None,
-              corr: Optional[torch.Tensor] = None, adam_v: Optional[torch.Tensor] = None) -> None:
+              corr: Optional[torch.Tensor] = None, adam_v: Optional[torch.Tensor] = None, clip: bool = False) -> None:
     """One kernel over the whole flat arena (reference: ``optimizer.step()``, demo.py:47).
+
+    ``clip`` (gradient-norm clipping): the gradient is multiplied by the coefficient :func:`grad_norm_clip` wrote, as it
+    is loaded and before any other term -- ``hyper[SGD_HYPER_CLIP]`` (``hyper`` then holds 6 floats) or, with AdamW,
+    ``hyper[ADAMW_ROW_CLIP]`` of the step's row.
 
     ``adam_v`` (AdamW, exclusive with ``prox_anchor`` and ``corr``): fp32 second moment indexed like ``w``; the step is
     then AdamW's, ``momentum_buf`` (required) is the first moment and ``hyper`` the step's row of :func:`adamw_rows`.
@@ -191,10 +195,22 @@ def fused_sgd(w: torch.Tensor, g: torch.Tensor, hyper: torch.Tensor, momentum_bu
     pk = pack or {}
     load().fused_sgd(w, g, momentum_buf, w_bf16, hyper, zero_grad, nesterov, pk.get("wire_slot"),
                      pk.get("global_w"), pk.get("scale"), int(pk.get("n_pack", 0)), bool(pk.get("wire_fp32", False)),
-                     prox_anchor, corr, adam_v)
+                     prox_anchor, corr, adam_v, bool(clip))
 
 
 ADAMW_ROW = 12         # floats per AdamW step row (csrc/sgd.cuh: ADAMW_ROW / AdamHyper)
+SGD_HYPER_CLIP = 5     # the clip coefficient's float in the SGD hyper-parameters (csrc/sgd.cuh)
+ADAMW_ROW_CLIP = 9     # ... and in an AdamW step row
+
+
+def grad_norm_clip(g: torch.Tensor, max_norm: torch.Tensor, work: torch.Tensor, norm_out: torch.Tensor,
+                   coef_out: torch.Tensor) -> None:
+    """``clip_grad_norm_``'s norm and coefficient on the device: ``norm_out[0] = ||g||`` (fp32, accumulated in fp64 with
+    a fixed grid and summation order: the same bits on every launch) and ``coef_out[0] = min(max_norm[0] / (norm +
+    1e-6), 1)`` rounded as torch rounds it from the fp32 norm.  ``max_norm``: fp32 device scalar.  ``work``: int64
+    ``[GRAD_NORM_WORK_WORDS]`` of zeros, reusable by launches on the same stream; its last word holds the fp64 sum of
+    squares afterwards."""
+    load().grad_norm_clip(g, max_norm, work, norm_out, coef_out)
 
 
 def adamw_rows(lr: float, betas: Tuple[float, float], eps: float, weight_decay: float, t0: int, count: int,
@@ -266,12 +282,14 @@ def sgd_segments(n: int, fused: Sequence[Tuple[int, int, int, int]], nograd: Seq
 def fused_sgd_segments(w: torch.Tensor, g: torch.Tensor, hyper: torch.Tensor, segments: torch.Tensor,
                        momentum_buf: Optional[torch.Tensor] = None, w_bf16: Optional[torch.Tensor] = None,
                        nesterov: bool = False, prox_anchor: Optional[torch.Tensor] = None,
-                       corr: Optional[torch.Tensor] = None, adam_v: Optional[torch.Tensor] = None) -> None:
+                       corr: Optional[torch.Tensor] = None, adam_v: Optional[torch.Tensor] = None,
+                       clip: bool = False) -> None:
     """The step of :func:`fused_sgd` over the arena chunks of ``segments`` (device int64 ``[S, 3]`` from
-    :func:`sgd_segments`); chunks of kind 1 never read the gradient.  ``prox_anchor``, ``corr`` and ``adam_v`` as in
-    :func:`fused_sgd`; a kind-1 element without a momentum buffer (or with AdamW) is then written only where the step
-    changes it."""
-    load().fused_sgd_segments(w, g, momentum_buf, w_bf16, segments, hyper, nesterov, prox_anchor, corr, adam_v)
+    :func:`sgd_segments`); chunks of kind 1 never read the gradient.  ``prox_anchor``, ``corr``, ``adam_v`` and
+    ``clip`` as in :func:`fused_sgd`; a kind-1 element without a momentum buffer (or with AdamW) is then written only
+    where the step changes it."""
+    load().fused_sgd_segments(w, g, momentum_buf, w_bf16, segments, hyper, nesterov, prox_anchor, corr, adam_v,
+                              bool(clip))
 
 
 def scaffold_corr(corr: torch.Tensor, c: torch.Tensor, c_i: torch.Tensor) -> None:

@@ -182,14 +182,17 @@ class _SgdEpilogue:
     arena (``F.sgd_segments``).  The gradient of a fused block is never written, so it stays zero for unfused steps.
     ``prox``: FedProx step anchored on ``arena.global_w`` (``hyper`` then holds the coefficient as its fifth float).
     ``corr``: SCAFFOLD step with the correction ``c - c_i`` (fp32, indexed like the parameters).
-    ``adam_v``: AdamW step with this second moment (``arena.momentum`` is the first, ``hyper`` the step's AdamW row)."""
+    ``adam_v``: AdamW step with this second moment (``arena.momentum`` is the first, ``hyper`` the step's AdamW row).
+    ``fuse=False`` (a gradient-clipped step, whose coefficient needs the whole gradient): no GEMM applies the step;
+    only the ``nograd`` ranges are recorded -- the centre-tap weights minus their centre tap."""
 
     def __init__(self):
         self.arena = None
+        self.fuse = True
 
     @contextlib.contextmanager
-    def open(self, arena, hyper, nesterov, prox=False, corr=None, adam_v=None):
-        self.arena, self.hyper, self.nesterov = arena, hyper, nesterov
+    def open(self, arena, hyper, nesterov, prox=False, corr=None, adam_v=None, fuse=True):
+        self.arena, self.hyper, self.nesterov, self.fuse = arena, hyper, nesterov, fuse
         self.anchor = arena.global_w if prox else None
         self.corr = corr
         self.adam_v = adam_v
@@ -201,12 +204,18 @@ class _SgdEpilogue:
 
     @property
     def active(self):
-        return self.arena is not None
+        """True while wgrad GEMMs apply the optimizer step in their epilogue."""
+        return self.arena is not None and self.fuse
+
+    @property
+    def recording(self):
+        """True while an unfused step records its no-gradient ranges."""
+        return self.arena is not None and not self.fuse
 
     def args(self, out2d):
-        """``sgd=`` argument for a wgrad GEMM writing the arena gradient view ``out2d``, or None when closed."""
+        """``sgd=`` argument for a wgrad GEMM writing the arena gradient view ``out2d``, or None when not fusing."""
         a = self.arena
-        if a is None:
+        if not self.active:
             return None
         return F.sgd_epilogue_args(a.theta, a.grad, out2d, self.hyper, a.momentum, a.theta_bf16, self.nesterov,
                                    self.anchor, self.corr, self.adam_v)
@@ -216,6 +225,21 @@ class _SgdEpilogue:
         self.fused.append((off, out2d.shape[0], out2d.shape[1], out2d.stride(0)))
         if nograd_of is not None:
             self.nograd.append(((nograd_of.data_ptr() - self.arena.grad.data_ptr()) // 4, nograd_of.numel()))
+
+    def record_nograd(self, out2d, nograd_of):
+        """Unfused step: the ranges of the weight gradient ``nograd_of`` outside the block ``out2d`` (the centre tap,
+        which the GEMM accumulated into the arena) as ``nograd`` ranges."""
+        g0 = self.arena.grad.data_ptr()
+        pos = (nograd_of.data_ptr() - g0) // 4
+        end = pos + nograd_of.numel()
+        off, ld, cols = (out2d.data_ptr() - g0) // 4, out2d.stride(0), out2d.shape[1]
+        for r in range(out2d.shape[0]):
+            s = off + r * ld
+            if s > pos:
+                self.nograd.append((pos, s - pos))
+            pos = s + cols
+        if pos < end:
+            self.nograd.append((pos, end - pos))
 
 
 SGD_EPI = _SgdEpilogue()
@@ -229,6 +253,8 @@ def _wgrad(fn, out2d, nograd_of=None):
         SGD_EPI.record(out2d, nograd_of)
     else:
         fn(None)
+        if nograd_of is not None and SGD_EPI.recording:
+            SGD_EPI.record_nograd(out2d, nograd_of)
 
 
 def _grad_target(p: Optional[torch.Tensor]):

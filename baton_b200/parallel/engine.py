@@ -26,7 +26,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import torch
 
 from ..metrics import phase
-from ..train import GraphedLocalSGD, PortableLocalSGD, check_adamw, check_prox_mu
+from ..train import GraphedLocalSGD, PortableLocalSGD, check_adamw, check_max_grad_norm, check_prox_mu
 from .arena import ParamArena
 from .compress import TopKConfig, TopKState
 from .dp import DPConfig, RDPAccountant, check_dp, clip_factor
@@ -78,7 +78,7 @@ class FederatedEngine:
                  compress: Optional[str] = None, topk_ratio: float = 0.01, error_feedback: bool = True,
                  local_keys: "Optional[str | Sequence[str]]" = None, augment: Optional[str] = None,
                  augment_padding: int = 4, mix: Optional[str] = None, mix_alpha: float = 1.0,
-                 label_smoothing: float = 0.0):
+                 label_smoothing: float = 0.0, max_grad_norm: float = 0.0):
         """``prox_mu > 0``: FedProx local training -- every step adds ``prox_mu * (theta - global_w)`` to the gradient,
         ``global_w`` being the global model the round started from (for logical clients too: each starts from it).
 
@@ -151,7 +151,14 @@ class FederatedEngine:
         on the soft-target cross-entropy.  Mixing draws from the augmentation key and the client's stream of the round,
         with or without ``augment``.  It needs the cross-entropy loss, and mixing needs NHWC image shards; both are
         local to each client and combine with every other option.  Evaluation keeps hard labels.  ``None`` / ``0``
-        (the defaults) run exactly the plain engine."""
+        (the defaults) run exactly the plain engine.
+
+        ``max_grad_norm > 0``: every local step clips the gradient of the loss to this 2-norm, as
+        ``torch.nn.utils.clip_grad_norm_(model.parameters(), max_grad_norm)`` right after backward and before weight
+        decay, FedProx, SCAFFOLD, momentum or AdamW act.  The norm covers every trained parameter, client-local ones
+        included.  It is local to each client and combines with every other option; it is not DP (``dp_clip`` clips
+        client updates).  :meth:`last_grad_norms` reports the pre-clip norms.  ``0`` (the default) runs exactly the
+        plain engine."""
         from ..data.augment import check_augment
         from ..data.mix import check_mix, check_mix_loss
         aug = check_augment(augment, augment_padding)
@@ -165,6 +172,7 @@ class FederatedEngine:
             b1, b2 = server_betas
             sopt = ServerOptConfig(server_opt, server_lr, b1, b2, server_tau)
         prox_mu = check_prox_mu(prox_mu)
+        max_grad_norm = check_max_grad_norm(max_grad_norm)
         adam = optimizer == "adamw"
         if adam:
             betas, eps = check_adamw(betas, eps)
@@ -231,6 +239,9 @@ class FederatedEngine:
         self.hp = dict(lr=lr, batch_size=batch_size, momentum=momentum, weight_decay=weight_decay, prox_mu=prox_mu)
         if adam:
             self.hp.update(optimizer=optimizer, betas=betas, eps=eps)
+        if max_grad_norm > 0:
+            self.hp.update(max_grad_norm=max_grad_norm)
+        self._grad_norms: Dict[int, torch.Tensor] = {}     # client id -> [n_epoch, steps] norms of the last round
         aug_hp = {}
         if aug is not None:
             aug_hp.update(augment=aug.kind, augment_padding=aug.padding)
@@ -302,6 +313,7 @@ class FederatedEngine:
         update_name = "update_{}_{:05d}".format(self.name, self.n_rounds)
         participants = self.draw_participants()
         self._last_participants = participants
+        self._grad_norms = {}
         mine = [c for c in participants if self.hosted(c)]
         a = self.arena
         total_n = 0
@@ -449,11 +461,19 @@ class FederatedEngine:
         if self.aug_hp is not None:
             hp = dict(hp, augment_stream=(self.n_rounds << 32) | int(cid), **self.aug_hp)
         if self.scaf is None:
-            return self.trainer.run(X, y, n_epoch=n_epoch, return_device=True, **hp)
-        self.scaf.begin_client(cid)
-        ld = self.trainer.run(X, y, n_epoch=n_epoch, return_device=True, corr=self.scaf.corr, **hp)
-        self.scaf.end_client(cid, self.arena, n_epoch * self.trainer.last_steps, self.hp["lr"], first=first)
+            ld = self.trainer.run(X, y, n_epoch=n_epoch, return_device=True, **hp)
+        else:
+            self.scaf.begin_client(cid)
+            ld = self.trainer.run(X, y, n_epoch=n_epoch, return_device=True, corr=self.scaf.corr, **hp)
+            self.scaf.end_client(cid, self.arena, n_epoch * self.trainer.last_steps, self.hp["lr"], first=first)
+        if self.trainer.grad_norms is not None:
+            self._grad_norms[int(cid)] = self.trainer.grad_norms      # a fresh buffer per run: no copy
         return ld
+
+    def last_grad_norms(self) -> Dict[int, List[List[float]]]:
+        """``{client_id: [[norm per step] per epoch]}``: the pre-clip gradient norms of the clients this rank trained
+        in the last round, logical clients included (a host read; empty when ``max_grad_norm`` is 0)."""
+        return {c: t.tolist() for c, t in self._grad_norms.items()}
 
     def control_variates(self):
         """SCAFFOLD's ``(c, {client_id: c_i})``: the server control variate and those of the clients this rank hosts

@@ -39,6 +39,11 @@ Cross-entropy trainers also take ``mix="mixup" | "cutmix" | "mixup_cutmix"`` wit
 the loss is the soft-target cross-entropy.  ``GraphedLocalSGD`` mixes inside the same batch gather and applies the soft
 target in the fused loss kernels; the CPU trainers call the host reference.  Mixing draws from the augmentation key
 and stream, so it takes the same ``augment_seed`` / ``augment_stream``.
+
+Every trainer also takes ``max_grad_norm`` (``C > 0``): ``torch.nn.utils.clip_grad_norm_(parameters, C)`` of every
+step's gradient right after backward, before weight decay and the FedProx, SCAFFOLD, momentum or AdamW terms act.
+``GraphedLocalSGD`` runs one norm kernel per step (``F.grad_norm_clip``) and the clipped optimizer kernels; the CPU
+trainers call ``clip_grad_norm_``.  ``last_grad_norms()`` returns the pre-clip norms of the last run.
 """
 from __future__ import annotations
 
@@ -47,6 +52,7 @@ import gc
 from collections import OrderedDict
 from typing import Callable, List, Optional, Tuple
 
+import numpy as np
 import torch
 from torch import nn
 
@@ -72,6 +78,33 @@ def check_prox_mu(prox_mu: float) -> float:
     if not (0.0 <= mu < float("inf")):
         raise ValueError("prox_mu must be a finite number >= 0, got {!r}".format(prox_mu))
     return mu
+
+
+def check_max_grad_norm(max_grad_norm: float) -> float:
+    """The gradient-norm clip threshold as a float; ``ValueError`` unless it is a finite number >= 0 (0: no clipping)."""
+    try:
+        c = float(max_grad_norm)
+    except (TypeError, ValueError):
+        raise ValueError("max_grad_norm must be a finite number >= 0, got {!r}".format(max_grad_norm)) from None
+    if not (0.0 <= c < float("inf")):
+        raise ValueError("max_grad_norm must be a finite number >= 0, got {!r}".format(max_grad_norm))
+    return c
+
+
+def clip_coefficient(norm, max_grad_norm: float) -> np.ndarray:
+    """The coefficient ``clip_grad_norm_`` multiplies the gradients by, as the device kernel computes it from its fp32
+    norm: ``min(fl32(fl32(1 / fl32(norm + 1e-6)) * C), 1)`` with ``C`` rounded to fp32 and every operation rounded to
+    fp32.  That is torch's ``clamp(reciprocal(norm + 1e-6) * C, max=1)`` bit for bit; a NaN norm gives NaN, an
+    infinite one 0."""
+    n = np.asarray(norm, dtype=np.float32)
+    with np.errstate(divide="ignore", over="ignore", invalid="ignore"):
+        c = (np.float32(1.0) / (n + np.float32(1e-6))) * np.float32(max_grad_norm)
+    return np.where(c > np.float32(1.0), np.float32(1.0), c).astype(np.float32)
+
+
+def _clip_grads(params, max_grad_norm: float):
+    """``clip_grad_norm_`` of the step's gradients (2-norm, non-finite norms allowed); returns the pre-clip norm."""
+    return nn.utils.clip_grad_norm_(params, max_grad_norm, error_if_nonfinite=False).detach()
 
 
 def check_adamw(betas, eps) -> Tuple[Tuple[float, float], float]:
@@ -121,14 +154,16 @@ def run_local_sgd(model: nn.Module, X: torch.Tensor, y: torch.Tensor, *, n_epoch
                   betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8, augment: Optional[str] = None,
                   augment_padding: int = 4, augment_seed: Optional[int] = None,
                   augment_stream: Optional[int] = None, mix: Optional[str] = None, mix_alpha: float = 1.0,
-                  label_smoothing: float = 0.0) -> List[float]:
+                  label_smoothing: float = 0.0, max_grad_norm: float = 0.0) -> List[float]:
     """Portable local SGD; returns the per-epoch mean loss.  ``prox_mu > 0``: FedProx, anchored on the parameters as
     they are on entry -- the global model the worker has just loaded.  ``optimizer="adamw"``: a fresh
     ``torch.optim.AdamW(lr, betas, eps, weight_decay)`` instead of SGD.  ``augment``: random crop / flip of every
     batch; the model keeps the key and run counter (``AugmentStreams``) across calls.  ``mix`` / ``label_smoothing``:
-    mixup / CutMix of every batch and the soft-target loss (``data/mix.py``)."""
+    mixup / CutMix of every batch and the soft-target loss (``data/mix.py``).  ``max_grad_norm > 0``:
+    ``clip_grad_norm_(parameters, max_grad_norm)`` right after every backward, before the FedProx term."""
     criterion = _loss_fn(loss)
     prox_mu = check_prox_mu(prox_mu)
+    max_grad_norm = check_max_grad_norm(max_grad_norm)
     adam = check_optimizer(optimizer, momentum, prox_mu=prox_mu)
     mixc = _mix_setup(mix, mix_alpha, label_smoothing, loss)
     aug = _augment_setup(model.__dict__.setdefault("_augment_streams", AugmentStreams()), X, augment,
@@ -163,6 +198,8 @@ def run_local_sgd(model: nn.Module, X: torch.Tensor, y: torch.Tensor, *, n_epoch
             loss_batch = criterion(output, target) if mixc is None else soft_cross_entropy(output, soft)
             batch_iter.update_loss(loss_batch)
             loss_batch.backward()
+            if max_grad_norm > 0:
+                _clip_grads(params, max_grad_norm)
             if anchors is not None:
                 _add_prox_term(params, anchors, prox_mu)
             optimizer.step()
@@ -322,7 +359,8 @@ class GraphedLocalSGD:
         self.graph_emits_wire = False
         dev = arena.device
         self.device = dev
-        self.hyper = torch.zeros(5, dtype=torch.float32, device=dev)   # [lr, momentum, wd, dampening, prox_mu]
+        # [lr, momentum, wd, dampening, prox_mu, clip coefficient]; the last is written on the device by a clipped step
+        self.hyper = torch.zeros(6, dtype=torch.float32, device=dev)
         self.prox = False             # FedProx: every SGD kernel of the step reads the anchor arena.global_w
         self.corr = None              # SCAFFOLD: every SGD kernel of the step reads this correction c - c_i
         self.adam = False             # AdamW: every optimizer kernel of the step reads its step row and arena.adam_v
@@ -331,6 +369,11 @@ class GraphedLocalSGD:
         self._aug_streams = AugmentStreams()
         self._aug_table = None        # device [epochs, 3] per-epoch words of augmenting runs (see _aug_words)
         self._mix = None              # MixConfig of the current run (mixing and / or label smoothing) or None
+        self.clip = False             # gradient-norm clipping: each step runs the norm kernel, then a clipped optimizer
+        self.max_norm = torch.zeros(1, dtype=torch.float32, device=dev)   # its threshold, read by the norm kernel
+        self._max_norm_host = None
+        self._norm_work = None        # the norm kernel's partials and arrival counter
+        self.grad_norms = None        # device [n_epoch, steps] pre-clip norms of the last run (None: no clipping)
         self.loss_acc = torch.zeros(2, dtype=torch.float32, device=dev)
         self._graphs = {}           # (n, batch, x_shape, y_shape) -> captured epoch
         self._hyper_host = None
@@ -364,13 +407,14 @@ class GraphedLocalSGD:
         return xb, yb
 
     def _step(self, X, y, idx, batch=None, emit_wire=False, fuse_sgd=True, row=None, s0=0, words=None, mix_rows=None,
-              bsz=None):
+              bsz=None, norm=None):
         """One SGD step on ``X[idx], y[idx]`` (or on the already gathered ``batch``).  ``emit_wire``: last step of
         an epoch -- the optimizer kernel also writes the upload copy for the round-end collective (``self.pack``).
         ``fuse_sgd=False``: no optimizer epilogue in the weight-gradient GEMMs (one optimizer pass over the arena).
         ``row``: with AdamW, the device row of this step's coefficients (``F.adamw_rows``).  ``s0``, ``words``: the
         epoch position of ``idx[0]`` and the device words of an augmenting gather.  ``mix_rows``, ``bsz``: the
-        epoch's device mix rows and the batch size of a mixing run; the loss reads row ``s0 // bsz``."""
+        epoch's device mix rows and the batch size of a mixing run; the loss reads row ``s0 // bsz``.  ``norm``: with
+        clipping on, the device scalar this step writes its pre-clip gradient norm to."""
         F = self.F
         xb, yb = batch if batch is not None else self._gather(X, y, idx, s0, words, mix_rows, bsz)
         mix = None
@@ -392,13 +436,17 @@ class GraphedLocalSGD:
             # hand-scheduled forward + loss + backward (no autograd engine): two-piece block gradients, parallel shortcut
             # branch; the loss kernel accumulates straight into the epoch's running sums
             if fuse_sgd and not emit_wire:
-                # the split-K = 1 convolution weight gradients apply SGD in their GEMM epilogue; one launch covers the rest
+                # the split-K = 1 convolution weight gradients apply SGD in their GEMM epilogue; one launch covers the rest.
+                # A clipped step cannot: its coefficient needs the last gradient.  Its GEMMs only record the no-gradient
+                # taps, which the leftover pass (then over the whole arena) still skips.
                 with self.bnn.SGD_EPI.open(a, hyper, self.nesterov, prox=self.prox, corr=self.corr,
-                                           adam_v=adam_v) as epi:
+                                           adam_v=adam_v, fuse=not self.clip) as epi:
                     explicit(xb, yb, loss_acc=self.loss_acc, after_first_gemm=self._first_gemm_hook, **soft)
+                if self.clip:
+                    self._grad_norm(norm, hyper)
                 F.fused_sgd_segments(a.theta, a.grad, hyper, self._segment_table(epi.fused, epi.nograd),
                                      a.momentum, bf, nesterov=self.nesterov, prox_anchor=anchor, corr=self.corr,
-                                     adam_v=adam_v)
+                                     adam_v=adam_v, clip=self.clip)
                 self.emitted_wire = False
                 return
             explicit(xb, yb, loss_acc=self.loss_acc, after_first_gemm=self._first_gemm_hook, **soft)
@@ -410,13 +458,23 @@ class GraphedLocalSGD:
             self.bnn.WGRAD.join()      # weight-gradient GEMMs run on a side stream; they must land before the step
         # one optimizer pass over the whole arena; the epoch's last step also emits the upload copy
         pack = self.pack if emit_wire else None
+        if self.clip:
+            self._grad_norm(norm, hyper)
         F.fused_sgd(a.theta[: a.n_param], a.grad, hyper, a.momentum,
                     bf[: a.n_param] if bf is not None else None, zero_grad=True, nesterov=self.nesterov, pack=pack,
                     prox_anchor=anchor[: a.n_param] if anchor is not None else None,
-                    corr=self.corr[: a.n_param] if self.corr is not None else None, adam_v=adam_v)
+                    corr=self.corr[: a.n_param] if self.corr is not None else None, adam_v=adam_v, clip=self.clip)
         self.emitted_wire = pack is not None
         if stats is not None:
             self.loss_acc.add_(stats)
+
+    def _grad_norm(self, norm, hyper):
+        """The norm kernel of a clipped step: ``||grad[0:n_param]||`` into ``norm`` and the clip coefficient into the
+        slot of ``hyper`` (the SGD hyper-parameters or the step's AdamW row) the clipped optimizer kernels read."""
+        F = self.F
+        slot = F.ADAMW_ROW_CLIP if self.adam else F.SGD_HYPER_CLIP
+        F.grad_norm_clip(self.arena.grad[: self.arena.n_param], self.max_norm, self._norm_work, norm,
+                         hyper[slot: slot + 1])
 
     def _segment_table(self, fused, nograd):
         """Device chunk table of the leftover optimizer pass, built once per set of epilogue-updated ranges (they only
@@ -431,8 +489,15 @@ class GraphedLocalSGD:
     def _set_hyper(self, lr, momentum, weight_decay, dampening=0.0, prox_mu=0.0):
         vals = (float(lr), float(momentum), float(weight_decay), float(dampening), float(prox_mu))
         if vals != self._hyper_host:
-            self.hyper.copy_(torch.tensor(vals, dtype=torch.float32))
+            self.hyper[:5].copy_(torch.tensor(vals, dtype=torch.float32))
             self._hyper_host = vals
+
+    def _set_max_norm(self, max_grad_norm: float):
+        if max_grad_norm != self._max_norm_host:
+            self.max_norm.fill_(max_grad_norm)
+            self._max_norm_host = max_grad_norm
+        if self._norm_work is None:
+            self._norm_work = torch.zeros(self.F.load().GRAD_NORM_WORK_WORDS, dtype=torch.int64, device=self.device)
 
     def _adam_rows(self, lr, betas, eps, weight_decay, n_epoch, steps):
         """Device ``[n_epoch * steps, ADAMW_ROW]`` AdamW coefficients of every local step of a run (step ``t`` counts
@@ -466,11 +531,13 @@ class GraphedLocalSGD:
     def _capture(self, X, y, n_steps, batch_size, rows=None, steps=None):
         """``rows``: with AdamW, the device row buffer captured step ``s`` reads row ``s`` of (holding the first
         epoch's rows, which the warm-up steps use too); kept in the returned entry.  With augmentation on, the
-        gather reads the entry's word buffer ``words``; with mixing on, the entry's ``[steps, 8]`` mix rows ``mix``."""
+        gather reads the entry's word buffer ``words``; with mixing on, the entry's ``[steps, 8]`` mix rows ``mix``.
+        With clipping on, captured step ``s`` writes its gradient norm to ``norms[s]`` of the entry."""
         perm = torch.zeros(n_steps * batch_size, dtype=torch.int64, device=self.device)
         words = torch.zeros(3, dtype=torch.int32, device=self.device) if self._aug is not None else None
         mixbuf = (torch.zeros(steps, MIX_ROW, dtype=torch.int32, device=self.device)
                   if self._mix is not None and self._mix.kind is not None else None)
+        norms = torch.zeros(steps, dtype=torch.float32, device=self.device) if self.clip else None
         perm.copy_(torch.arange(n_steps * batch_size, device=self.device) % X.shape[0])
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
@@ -481,7 +548,7 @@ class GraphedLocalSGD:
             snap_m = self.arena.momentum.clone() if self.arena.momentum is not None else None
             for _ in range(2):
                 self._step(X, y, perm[:batch_size], row=rows[0] if rows is not None else None, words=words,
-                           mix_rows=mixbuf, bsz=batch_size)
+                           mix_rows=mixbuf, bsz=batch_size, norm=norms[0:1] if norms is not None else None)
         torch.cuda.current_stream(self.device).wait_stream(side)
         torch.cuda.synchronize(self.device)
         from .ops._ext import total_launches
@@ -498,7 +565,7 @@ class GraphedLocalSGD:
                                               yp[s * batch_size:(s + 1) * batch_size]),
                            emit_wire=(s == n_steps - 1 and self.pack is not None),
                            row=rows[s] if rows is not None else None, s0=s * batch_size, mix_rows=mixbuf,
-                           bsz=batch_size)
+                           bsz=batch_size, norm=norms[s:s + 1] if norms is not None else None)
             self.graph_emits_wire = self.pack is not None
 
         if (self.k3_join is not None and hasattr(self.model, "explicit_step")
@@ -545,7 +612,7 @@ class GraphedLocalSGD:
         self.arena.sync_shadow()
         self.loss_acc.zero_()
         return {"graph": graph, "graph2": graph2, "perm": perm, "X": X, "y": y, "rows": rows, "words": words,
-                "mix": mixbuf}
+                "mix": mixbuf, "norms": norms}
 
     # -------------------------------------------------------------- evaluation
     def _eval_pass(self, X, y, batch_size, explicit):
@@ -637,7 +704,8 @@ class GraphedLocalSGD:
             prox_mu: float = 0.0, corr: Optional[torch.Tensor] = None, optimizer: str = "sgd",
             betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8, augment: Optional[str] = None,
             augment_padding: int = 4, augment_seed: Optional[int] = None, augment_stream: Optional[int] = None,
-            mix: Optional[str] = None, mix_alpha: float = 1.0, label_smoothing: float = 0.0, **_ignored):
+            mix: Optional[str] = None, mix_alpha: float = 1.0, label_smoothing: float = 0.0,
+            max_grad_norm: float = 0.0, **_ignored):
         """``prox_mu > 0``: FedProx toward ``arena.global_w``, the global model the round started from.  ``corr``:
         SCAFFOLD's correction ``c - c_i`` (fp32 device buffer of ``arena.n_param`` elements), added to every step's
         gradient; it is read at replay, so the caller may rewrite it between runs.  ``optimizer="adamw"``: the steps of
@@ -645,9 +713,12 @@ class GraphedLocalSGD:
         in the batch gather (``data/augment.py``); ``augment_seed`` (None: a random key per trainer) and
         ``augment_stream`` (None: this trainer's count of augmenting runs) pick the draws.  ``mix`` (with
         ``mix_alpha``) and ``label_smoothing``: mixup / CutMix in the same gather and the soft-target loss
-        (``data/mix.py``), drawn from the same key and stream."""
+        (``data/mix.py``), drawn from the same key and stream.  ``max_grad_norm > 0``: ``clip_grad_norm_`` of every
+        step's gradient before the optimizer's terms are added (the norm kernel, then the clipped optimizer kernels);
+        the threshold is read from device memory, so a new one replays the same graph."""
         assert X.is_cuda, "GraphedLocalSGD needs a device-resident shard"
         prox_mu = check_prox_mu(prox_mu)
+        max_grad_norm = check_max_grad_norm(max_grad_norm)
         if prox_mu > 0 and self.arena.global_w is None:
             raise ValueError("prox_mu > 0 needs the arena's global copy (ParamArena(keep_global=True))")
         _check_corr(corr, self.arena)
@@ -666,6 +737,9 @@ class GraphedLocalSGD:
         self._set_hyper(lr, momentum, weight_decay, prox_mu=prox_mu)
         self.prox = prox_mu > 0
         self.corr = corr
+        self.clip = max_grad_norm > 0
+        if self.clip:
+            self._set_max_norm(max_grad_norm)
         if (momentum or self.adam) and self.arena.momentum is None:
             self.arena.momentum = torch.zeros_like(self.arena.grad)
         if self.adam and self.arena.adam_v is None:
@@ -680,8 +754,9 @@ class GraphedLocalSGD:
         # the anchor and correction pointers are baked into the captured launches; the coefficient is read from `hyper`
         # at replay
         key = (n, batch_size, tuple(X.shape[1:]), tuple(y.shape[1:]), X.data_ptr(), y.data_ptr(), bool(momentum),
-               self.prox, corr.data_ptr() if corr is not None else None, self.adam, aug_key, mix_key)
+               self.prox, corr.data_ptr() if corr is not None else None, self.adam, aug_key, mix_key, self.clip)
         epoch_losses = torch.zeros(n_epoch, 2, dtype=torch.float32, device=self.device)
+        grad_norms = torch.zeros(n_epoch, steps, dtype=torch.float32, device=self.device) if self.clip else None
         if self.use_graph:
             ent = self._graphs.get(key)
             if ent is None:
@@ -707,8 +782,11 @@ class GraphedLocalSGD:
                     with torch.enable_grad():
                         self._step(X, y, perm_full[n_steps * batch_size:], fuse_sgd=False,
                                    row=ent["rows"][n_steps] if self.adam else None, s0=n_steps * batch_size,
-                                   words=ent["words"], mix_rows=ent["mix"], bsz=batch_size)
+                                   words=ent["words"], mix_rows=ent["mix"], bsz=batch_size,
+                                   norm=ent["norms"][n_steps:] if self.clip else None)
                 epoch_losses[e].copy_(self.loss_acc)
+                if self.clip:
+                    grad_norms[e].copy_(ent["norms"])
         else:
             perm_full = torch.randperm(n, device=self.device)
             for e in range(n_epoch):
@@ -719,9 +797,11 @@ class GraphedLocalSGD:
                     with torch.enable_grad():
                         self._step(X, y, idx, row=table[e * steps + s] if self.adam else None, s0=s * batch_size,
                                    words=aug_words[e] if aug_words is not None else None,
-                                   mix_rows=mix_table_dev[e] if mixing else None, bsz=batch_size)
+                                   mix_rows=mix_table_dev[e] if mixing else None, bsz=batch_size,
+                                   norm=grad_norms[e, s:s + 1] if self.clip else None)
                 epoch_losses[e].copy_(self.loss_acc)
         self.last_steps = steps
+        self.grad_norms = grad_norms
         self.last_had_tail_step = bool(tail)        # a ragged eager step ran after the graph: its SGD did not emit the wire
         if self.use_graph:
             self.emitted_wire = bool(self.graph_emits_wire and not tail)
@@ -730,6 +810,12 @@ class GraphedLocalSGD:
         host = epoch_losses.tolist()          # the ONLY host read of the round
         self.last_stats = {"accuracy": [h[1] / n for h in host], "steps_per_epoch": steps}
         return [h[0] / steps for h in host]
+
+
+    def last_grad_norms(self) -> Optional[List[List[float]]]:
+        """The pre-clip gradient norm of every step of the last run, ``[n_epoch][steps]`` (a host read); None when it
+        did not clip."""
+        return self.grad_norms.tolist() if self.grad_norms is not None else None
 
 
 class PortableLocalSGD:
@@ -746,19 +832,24 @@ class PortableLocalSGD:
         self.n_kernels_per_step = 0
         self.last_stats = {}
         self._aug_streams = AugmentStreams()
+        self.grad_norms = None        # [n_epoch, steps] pre-clip gradient norms of the last run (None: no clipping)
 
     def run(self, X, y, n_epoch: int = 1, lr: float = 0.001, batch_size: int = 32, momentum: float = 0.0,
             weight_decay: float = 0.0, reshuffle_each_epoch: bool = False, return_device: bool = False,
             prox_mu: float = 0.0, corr: Optional[torch.Tensor] = None, optimizer: str = "sgd",
             betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8, augment: Optional[str] = None,
             augment_padding: int = 4, augment_seed: Optional[int] = None, augment_stream: Optional[int] = None,
-            mix: Optional[str] = None, mix_alpha: float = 1.0, label_smoothing: float = 0.0, **_ignored):
+            mix: Optional[str] = None, mix_alpha: float = 1.0, label_smoothing: float = 0.0,
+            max_grad_norm: float = 0.0, **_ignored):
         """``prox_mu > 0``: FedProx toward ``arena.global_w``, the global model the round started from.  ``corr``:
         SCAFFOLD's correction ``c - c_i`` (fp32, indexed like the arena's parameters), added to every gradient.
         ``optimizer="adamw"``: a fresh ``torch.optim.AdamW(lr, betas, eps, weight_decay)`` instead of SGD.
-        ``augment``, ``mix``, ``label_smoothing``: as in :meth:`GraphedLocalSGD.run`, through the host references."""
+        ``augment``, ``mix``, ``label_smoothing``: as in :meth:`GraphedLocalSGD.run`, through the host references.
+        ``max_grad_norm > 0``: ``clip_grad_norm_(parameters, max_grad_norm)`` right after every backward, before the
+        FedProx and SCAFFOLD terms are added."""
         criterion = _loss_fn(self.loss_kind)
         prox_mu = check_prox_mu(prox_mu)
+        max_grad_norm = check_max_grad_norm(max_grad_norm)
         _check_corr(corr, self.arena)
         adam = check_optimizer(optimizer, momentum, prox_mu=prox_mu, corr=corr)
         mixc = _mix_setup(mix, mix_alpha, label_smoothing, self.loss_kind)
@@ -781,6 +872,7 @@ class PortableLocalSGD:
             opt = torch.optim.SGD(params, lr=lr, momentum=momentum, weight_decay=weight_decay)
         perm = torch.randperm(n)
         out = torch.zeros(n_epoch, 2, dtype=torch.float32)
+        norms = torch.zeros(n_epoch, -(-n // batch_size), dtype=torch.float32) if max_grad_norm > 0 else None
         steps = 1
         for e in range(n_epoch):
             if reshuffle_each_epoch and e > 0:
@@ -802,6 +894,8 @@ class PortableLocalSGD:
                 else:
                     loss = criterion(pred.float() if tgt.dtype.is_floating_point else pred, tgt)
                 loss.backward()
+                if norms is not None:
+                    norms[e, b] = _clip_grads(params, max_grad_norm)
                 if prox_mu > 0:
                     _add_prox_term(params, anchors, prox_mu)
                 if corr is not None:
@@ -815,6 +909,7 @@ class PortableLocalSGD:
                 elif not tgt.dtype.is_floating_point:
                     out[e, 1] += float((pred.argmax(-1) == tgt).sum())
         self.last_steps = steps
+        self.grad_norms = norms
         if self.arena.theta_bf16 is not None:
             self.arena.sync_shadow()
         if return_device:
@@ -822,6 +917,10 @@ class PortableLocalSGD:
         host = out.tolist()
         self.last_stats = {"accuracy": [h[1] / n for h in host], "steps_per_epoch": steps}
         return [h[0] / steps for h in host]
+
+    def last_grad_norms(self) -> Optional[List[List[float]]]:
+        """The pre-clip gradient norm of every step of the last run, ``[n_epoch][steps]``; None when it did not clip."""
+        return self.grad_norms.tolist() if self.grad_norms is not None else None
 
     def evaluate(self, X, y, batch_size: int = 512):
         """Same contract as :meth:`GraphedLocalSGD.evaluate` on plain PyTorch ops."""
