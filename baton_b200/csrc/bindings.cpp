@@ -871,6 +871,73 @@ void fedavg_allreduce_topk(const std::vector<int64_t>& wire_ptrs, const std::vec
   launch_round(theta, a, n_ctas, "fedavg_allreduce_topk", sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
 }
 
+// secure-aggregation round: key_words = world x 8 uint32 words (row j: the key shared with rank j; this rank's row is
+// not read), R and f = 30 - ceil(log2 R), saturated = this rank's int64 counter of clamped / non-finite elements
+void fedavg_allreduce_secagg(const std::vector<int64_t>& wire_ptrs, const std::vector<int64_t>& pad_ptrs,
+                             int64_t wire_mc, at::Tensor theta, const std::optional<at::Tensor>& global_w,
+                             const std::optional<at::Tensor>& theta_bf16, const std::optional<at::Tensor>& momentum,
+                             const std::optional<at::Tensor>& int_local, const std::vector<int64_t>& int_wire_ptrs,
+                             const std::optional<at::Tensor>& loss_local, const std::vector<int64_t>& loss_wire_ptrs,
+                             const std::optional<at::Tensor>& loss_out, const std::vector<double>& n_samples,
+                             bool counts_from_flags, int64_t alive_mask, int64_t rank, int64_t world, int64_t wire_kind,
+                             bool delta, bool use_nvls, int64_t epoch, const std::optional<at::Tensor>& tile_flags,
+                             int64_t flag_value, int64_t tile_elems, int64_t n_ctas, int64_t timeout_log2,
+                             const std::optional<at::Tensor>& status, const std::optional<at::Tensor>& phase_ns,
+                             bool prepacked, const std::vector<int64_t>& key_words, double range, int64_t frac_bits,
+                             at::Tensor saturated,
+                             const std::optional<at::Tensor>& sopt_m, const std::optional<at::Tensor>& sopt_v,
+                             int64_t sopt_n_param, int64_t sopt_kind, const std::vector<double>& sopt_coef) {
+  FedAvgSecAggArgs a = {};
+  fill_fedavg_args(a, wire_ptrs, pad_ptrs, wire_mc, theta, global_w, theta_bf16, momentum, int_local, int_wire_ptrs,
+                   loss_local, loss_wire_ptrs, loss_out, n_samples, counts_from_flags, alive_mask, rank, world, wire_kind,
+                   delta, use_nvls, epoch, tile_flags, flag_value, tile_elems, timeout_log2, status, phase_ns, prepacked);
+  TORCH_CHECK(static_cast<int64_t>(key_words.size()) == world * 8, "secagg: 8 key words per rank");
+  TORCH_CHECK(frac_bits >= 10 && frac_bits <= 50, "secagg: f in 10..50");
+  CHECK_CUDA(saturated);
+  TORCH_CHECK(saturated.scalar_type() == at::kLong && saturated.numel() >= 1, "secagg: saturated = int64[1]");
+  for (int64_t k = 0; k < world; ++k)
+    for (int j = 0; j < 8; ++j) a.keys[k][j] = static_cast<uint32_t>(key_words[k * 8 + j]);
+  a.range = static_cast<float>(range);
+  a.frac_bits = static_cast<int>(frac_bits);
+  a.two_f = std::ldexp(1.f, a.frac_bits);
+  a.inv_two_f = std::ldexp(1.f, -a.frac_bits);
+  a.saturated = reinterpret_cast<unsigned long long*>(saturated.data_ptr<int64_t>());
+  launch_round(theta, a, n_ctas, "fedavg_allreduce_secagg", sopt_m, sopt_v, sopt_n_param, sopt_kind, sopt_coef);
+}
+
+// the standalone encode + mask of a secure round (b200_secagg_encode): key_words = n_peers x 8 uint32 words, signs
+// +1 / -1 per peer, nonce = 3 words; out = int32[n] (the uint32 ring values), saturated = int64[1] (added to)
+void secagg_encode(const at::Tensor& theta, const std::optional<at::Tensor>& global_w, double w, double range,
+                   int64_t frac_bits, const std::vector<int64_t>& key_words, const std::vector<int64_t>& signs,
+                   const std::vector<int64_t>& nonce, int64_t counter0, at::Tensor out, at::Tensor saturated) {
+  CHECK_CUDA(theta); CHECK_CUDA(out); CHECK_CUDA(saturated);
+  TORCH_CHECK(theta.scalar_type() == at::kFloat && theta.is_contiguous(), "secagg_encode: contiguous fp32 theta");
+  if (global_w.has_value() && global_w->defined())
+    TORCH_CHECK(global_w->scalar_type() == at::kFloat && global_w->is_contiguous() && global_w->numel() == theta.numel(),
+                "secagg_encode: fp32 global_w of theta's size");
+  TORCH_CHECK(out.scalar_type() == at::kInt && out.is_contiguous() && out.numel() == theta.numel(),
+              "secagg_encode: out = int32 of theta's size");
+  TORCH_CHECK(saturated.scalar_type() == at::kLong && saturated.numel() >= 1, "secagg_encode: saturated = int64[1]");
+  const int64_t n_peers = static_cast<int64_t>(signs.size());
+  TORCH_CHECK(n_peers < B200_MAX_RANKS && static_cast<int64_t>(key_words.size()) == n_peers * 8,
+              "secagg_encode: at most MAX_RANKS - 1 peers, 8 key words each");
+  TORCH_CHECK(nonce.size() == 3 && counter0 >= 0 && counter0 <= 0xFFFFFFFFll, "secagg_encode: 3 nonce words, 32-bit counter");
+  B200SecAggPeers peers = {};
+  peers.n = static_cast<int>(n_peers);
+  for (int64_t p = 0; p < n_peers; ++p) {
+    TORCH_CHECK(signs[p] == 1 || signs[p] == -1, "secagg_encode: signs are +1 or -1");
+    peers.sign[p] = static_cast<int>(signs[p]);
+    for (int j = 0; j < 8; ++j) peers.key[p][j] = static_cast<uint32_t>(key_words[p * 8 + j]);
+  }
+  const uint32_t nw[3] = {static_cast<uint32_t>(nonce[0]), static_cast<uint32_t>(nonce[1]), static_cast<uint32_t>(nonce[2])};
+  const c10::cuda::CUDAGuard guard(theta.device());
+  check(b200_secagg_encode(theta.data_ptr<float>(), opt_ptr<float>(global_w), theta.numel(), static_cast<float>(w),
+                           static_cast<float>(range), static_cast<int>(frac_bits), &peers, nw,
+                           static_cast<uint32_t>(counter0), reinterpret_cast<uint32_t*>(out.data_ptr<int>()),
+                           reinterpret_cast<unsigned long long*>(saturated.data_ptr<int64_t>()), cur_stream()),
+        "secagg_encode");
+}
+
 // personalized round (plain mean): the arena elements [local_lo, local_lo + local_len) are client-local and left alone;
 // the kernel works over the n - local_len shared elements (LocalArgs in launch.h)
 template <class Base>
@@ -1328,6 +1395,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.attr("KRUM_REPORT") = B200_KRUM_REPORT;
   m.def("fedavg_allreduce_topk", &fedavg_allreduce_topk);
   m.def("fedavg_allreduce_local", &fedavg_allreduce_local);
+  m.def("fedavg_allreduce_secagg", &fedavg_allreduce_secagg);
+  m.def("secagg_encode", &secagg_encode);
   m.def("topk_pack", &topk_pack);
   m.def("topk_fold", &topk_fold);
   m.def("nonzero_pack", &nonzero_pack);

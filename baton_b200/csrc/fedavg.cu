@@ -39,6 +39,7 @@
 #include "launch.h"
 #include "mx.cuh"
 #include "dp.cuh"
+#include "secagg.cuh"
 
 namespace b200 {
 
@@ -162,6 +163,22 @@ struct Wire<2> {
   __device__ static void st(void* p, const uint4& v) { *reinterpret_cast<uint2*>(p) = make_uint2(v.x, v.y); }
   __device__ static void st_na(void* p, const uint4& v) { st_na_v2(p, make_uint2(v.x, v.y)); }
   __device__ static uint4 mc_reduce(const void*) { return make_uint4(0, 0, 0, 0); }   // the switch cannot apply block scales
+};
+// WIRE 3: the int32 ring of a secure-aggregation round, 4 per 16 B.  Its pack (encode + masks) and reduce (wrapping
+// integer adds) are secagg_pack / secagg_reduce; the apply phase reads fp32(int32) and scales it by 2^-f.
+template <>
+struct Wire<3> {
+  static constexpr int VEC = 4, VBYTES = 16;
+  static constexpr bool SCALED = false;
+  __device__ static void unpack(const uint4& u, float (&f)[4], float) {
+    f[0] = __int2float_rn(static_cast<int>(u.x)); f[1] = __int2float_rn(static_cast<int>(u.y));
+    f[2] = __int2float_rn(static_cast<int>(u.z)); f[3] = __int2float_rn(static_cast<int>(u.w));
+  }
+  __device__ static uint4 ld(const void* p) { return ld_volatile_v4(p); }
+  __device__ static void st_na(void* p, const uint4& v) { st_na_v4(p, v); }
+  // the generic reduce loop names these, but a secure round never runs it
+  __device__ static uint4 pack(const float (&)[4], float) { return make_uint4(0, 0, 0, 0); }
+  __device__ static uint4 mc_reduce(const void*) { return make_uint4(0, 0, 0, 0); }   // ptxas has no .v4.u32 ld_reduce
 };
 
 // shared exponent of the 32-element block owned by a quad of adjacent lanes (8 elements each);
@@ -912,6 +929,81 @@ __device__ __forceinline__ void topk_reduce(const FedAvgTopkArgs& a, uint8_t* co
   }
 }
 
+// ---------------------------------------------------------------- secure aggregation (see launch.h / parallel/secagg.py)
+// phase 0 of a secure round, after the count barrier: this participant's masked upload over the tiles this CTA packs,
+// one 16-element ChaCha20 block per thread and trip (tile_elems % 16 == 0, so a block never straddles a tile).  keys[p] /
+// add[p]: the n_peers other participants' pair keys and signs (+ for a higher rank); w: this rank's weight.
+__device__ __forceinline__ void secagg_pack(const FedAvgSecAggArgs& a, uint8_t* my_wire, const uint32_t (*keys)[8],
+                                            const int* add, int n_peers, float w, int A, int G) {
+  const long long n = a.n;
+  const int T = a.tile_elems;
+  const long long n_tiles = (n + T - 1) / T;
+  int sat = 0;
+  for (long long q = blockIdx.x; q * A < n_tiles; q += G) {
+    for (int r = 0; r < A; ++r) {
+      const long long t = q * A + r;
+      if (t >= n_tiles) break;
+      const long long base = t * T;
+      const int len = static_cast<int>((n - base) < T ? (n - base) : T);
+      for (int i = threadIdx.x * 16; i < len; i += FEDAVG_THREADS * 16) {
+        const int valid = len - i < 16 ? len - i : 16;     // a multiple of 4 (n % 8 == 0)
+        float x[16];
+#pragma unroll
+        for (int j = 0; j < 16; j += 4) {
+          float4 d = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (j < valid) {
+            const float4 th = __ldcs(reinterpret_cast<const float4*>(a.theta + base + i + j));
+            const float4 g = __ldcs(reinterpret_cast<const float4*>(a.global_w + base + i + j));
+            d = make_float4(__fsub_rn(th.x, g.x), __fsub_rn(th.y, g.y), __fsub_rn(th.z, g.z), __fsub_rn(th.w, g.w));
+          }
+          x[j] = d.x; x[j + 1] = d.y; x[j + 2] = d.z; x[j + 3] = d.w;
+        }
+        uint32_t u[16];
+        sat += secagg_encode_block(x, valid, w, a.range, a.two_f, n_peers, [&](int p) { return keys[p]; },
+                                   [&](int p) { return add[p] != 0; }, static_cast<uint32_t>((base + i) >> 4), a.epoch,
+                                   0u, 0u, u);
+#pragma unroll
+        for (int j = 0; j < 16; j += 4)
+          if (j < valid) *reinterpret_cast<uint4*>(my_wire + (base + i + j) * 4) = make_uint4(u[j], u[j + 1], u[j + 2], u[j + 3]);
+      }
+    }
+  }
+  if (sat != 0 && a.saturated != nullptr) atomicAdd(a.saturated, static_cast<unsigned long long>(sat));
+}
+
+// phase 1 of a secure round: the owner of a tile adds the participants' (part[k] > 0) uploads as uint32 with
+// wrap-around, in rank order, eight peer loads in flight, and stores the sum into that tile of every live replica
+__device__ __forceinline__ void secagg_reduce(const FedAvgSecAggArgs& a, uint8_t* const* s_wire, const float* part, int A,
+                                              int my_pos) {
+  constexpr int KG = 8;
+  const int G = gridDim.x;
+  const long long n = a.n;
+  const int T = a.tile_elems;
+  const long long n_tiles = (n + T - 1) / T;
+  for (long long t = my_pos + static_cast<long long>(blockIdx.x) * A; t < n_tiles; t += static_cast<long long>(G) * A) {
+    const long long base = t * T;
+    const int len = static_cast<int>((n - base) < T ? (n - base) : T);
+    for (int i = threadIdx.x * 4; i < len; i += FEDAVG_THREADS * 4) {
+      const size_t off = (base + i) * 4;
+      uint4 acc = make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll 1
+      for (int k0 = 0; k0 < A; k0 += KG) {
+        uint4 v[KG];
+#pragma unroll
+        for (int k = 0; k < KG; ++k)
+          if (k0 + k < A && part[k0 + k] > 0.f) v[k] = ld_volatile_v4(s_wire[k0 + k] + off);
+#pragma unroll
+        for (int k = 0; k < KG; ++k)
+          if (k0 + k < A && part[k0 + k] > 0.f) {
+            acc.x += v[k].x; acc.y += v[k].y; acc.z += v[k].z; acc.w += v[k].w;
+          }
+      }
+#pragma unroll 1
+      for (int k = 0; k < A; ++k) st_na_v4(s_wire[k] + off, acc);
+    }
+  }
+}
+
 // ---------------------------------------------------------------- server optimizer (see launch.h / parallel/server_opt.py)
 // one element: the state update, then the model update, each operation rounded separately (no FMA contraction)
 __device__ __forceinline__ float sopt_step(float x, float d, float& m, float& v, int kind, const float* c) {
@@ -995,7 +1087,7 @@ __device__ __forceinline__ void sopt_apply_tile(const Args& a, const uint8_t* my
 
 // The kind of aggregation a round runs.  Every kind is one args struct of launch.h, and RoundOf maps the struct to its
 // kind (and whether the apply phase runs the server optimizer): fedavg_round_kernel<WIRE, Args> is the round's kernel.
-enum class Agg { mean, dp, scaffold, robust, krum, topk };
+enum class Agg { mean, dp, scaffold, robust, krum, topk, secagg };
 template <class Args> struct RoundOf;
 template <Agg K> struct RoundKind {
   static constexpr Agg kind = K;
@@ -1007,6 +1099,7 @@ template <> struct RoundOf<FedAvgScaffoldArgs> : RoundKind<Agg::scaffold> {};
 template <> struct RoundOf<FedAvgRobustArgs> : RoundKind<Agg::robust> {};
 template <> struct RoundOf<FedAvgKrumArgs> : RoundKind<Agg::krum> {};
 template <> struct RoundOf<FedAvgTopkArgs> : RoundKind<Agg::topk> {};
+template <> struct RoundOf<FedAvgSecAggArgs> : RoundKind<Agg::secagg> {};
 template <class Base> struct RoundOf<ServerOptArgs<Base>> {
   static constexpr Agg kind = RoundOf<Base>::kind;
   static constexpr bool sopt = true, local = false;
@@ -1026,6 +1119,8 @@ template <class Base> struct RoundOf<LocalArgs<Base>> {
 // Agg::krum: a Multi-Krum round (krum_reduce above), a robust round whose exchange barrier takes epoch + 2 and barrier 2
 // epoch + 3.
 // Agg::topk: a top-k round (topk_reduce above): no pack phase, the uploads are sparse lists written before the launch.
+// Agg::secagg: a secure-aggregation round (WIRE 3, see launch.h): the count barrier (epoch + 1) comes before the pack
+// (secagg_pack above), barrier 1 takes epoch + 2, the reduce is secagg_reduce, barrier 2 takes epoch + 3.
 // SOPT (with any kind): a server-optimizer round -- the apply phase runs sopt_apply_tile.
 // LOCAL (with the mean): a personalized round -- n is the logical element count, and the pack and apply phases address
 // the replica at the physical element local_shift gives (see LocalArgs in launch.h).
@@ -1034,6 +1129,7 @@ template <int WIRE, Agg K, bool SOPT, bool LOCAL, typename Args>
 __device__ __forceinline__ void fedavg_round(const Args& a) {
   constexpr bool DP = K == Agg::dp, SCAF = K == Agg::scaffold, KRUM = K == Agg::krum, TOPK = K == Agg::topk;
   constexpr bool ROBUST = K == Agg::robust || KRUM;
+  constexpr bool SECAGG = K == Agg::secagg;
   using W = Wire<WIRE>;
   constexpr int VEC = W::VEC;
   constexpr bool SCALED = W::SCALED;
@@ -1045,7 +1141,11 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
   __shared__ float s_w[B200_MAX_RANKS];
   __shared__ uint32_t s_payload[B200_MAX_RANKS];  // indexed by rank
   __shared__ float s_inv_total;
-  __shared__ float s_part[DP ? B200_MAX_RANKS : 1];   // DP: participation weights n_k / N (loss, integer arena)
+  __shared__ float s_part[DP || SECAGG ? B200_MAX_RANKS : 1];   // DP: participation weights n_k / N (loss, integer
+                                                                 // arena); secure rounds: the counts n_k
+  __shared__ uint32_t s_key[SECAGG ? B200_MAX_RANKS : 1][8];     // secure rounds: the other participants' pair keys
+  __shared__ int s_add[SECAGG ? B200_MAX_RANKS : 1];             // ... and signs (1: a higher rank, added)
+  __shared__ int s_npeer;
   int A = 0, my_pos = -1;
   for (int k = 0; k < a.world; ++k)
     if ((a.alive_mask >> k) & 1u) {
@@ -1076,7 +1176,32 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
   // Loop bounds are warp-uniform (first lane's element) so the block-scale shuffles are legal.
   const float pack_scale = a.use_nvls ? my_n * a.nvls_prescale : 1.0f;
   phase_stamp(a, 0);                                   // start
-  if (!TOPK && (my_n != 0.f || a.use_nvls) && !a.prepacked) {
+  if constexpr (SECAGG) {
+    // the count barrier: every rank learns the counts, hence the participants and the weights, before anyone packs
+    if (!cta_barrier_all_ranks(a, a.epoch + 1, __float_as_uint(my_n), s_payload)) return;
+    if (threadIdx.x == 0) {          // IEEE-rounded operations: the weights are bit-equal to the host reference's
+      float total = 0.f;
+      for (int k = 0; k < A; ++k) {
+        const float nk = a.counts_from_flags ? __uint_as_float(s_payload[s_rank[k]]) : a.n_samples[s_rank[k]];
+        s_part[k] = nk;
+        total = __fadd_rn(total, nk);
+      }
+      const float inv = total > 0.f ? __fdiv_rn(1.f, total) : 0.f;
+      int np = 0;
+      for (int k = 0; k < A; ++k) {
+        s_w[k] = __fmul_rn(s_part[k], inv);
+        if (k != my_pos && s_part[k] > 0.f) {
+          s_add[np] = s_rank[k] > a.rank ? 1 : 0;
+          for (int j = 0; j < 8; ++j) s_key[np][j] = a.keys[s_rank[k]][j];
+          ++np;
+        }
+      }
+      s_npeer = np;
+      s_inv_total = inv;
+    }
+    __syncthreads();
+    if (s_part[my_pos] > 0.f) secagg_pack(a, my_wire, s_key, s_add, s_npeer, s_w[my_pos], A, G);
+  } else if (!TOPK && (my_n != 0.f || a.use_nvls) && !a.prepacked) {
     for (long long q = blockIdx.x; q * A < n_tiles; q += G) {
       for (int r = 0; r < A; ++r) {
         const long long t = q * A + r;
@@ -1145,11 +1270,11 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
     if (threadIdx.x == 0) *reinterpret_cast<volatile uint32_t*>(a.seg_page[a.rank]) = a.my_segs;
   }
   phase_stamp(a, 1);                                   // pack done
-  if (!cta_barrier_all_ranks(a, a.epoch + 1, __float_as_uint(my_n), s_payload)) return;
+  if (!cta_barrier_all_ranks(a, a.epoch + (SECAGG ? 2 : 1), __float_as_uint(my_n), s_payload)) return;
   phase_stamp(a, 2);                                   // barrier 1 passed
 
   // weights w_k = n_k / N from the counts that rode on the barrier flags (or the host's plan)
-  if (threadIdx.x == 0) {
+  if (!SECAGG && threadIdx.x == 0) {
     float total = 0.f;
     for (int k = 0; k < A; ++k) {
       const float nk = a.counts_from_flags ? __uint_as_float(s_payload[s_rank[k]]) : a.n_samples[s_rank[k]];
@@ -1285,6 +1410,8 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
     if (!krum_reduce<WIRE>(a, s_wire, s_rank, A, my_pos)) return;
   } else if constexpr (TOPK) {
     topk_reduce<WIRE>(a, s_wire, s_w, A, my_pos);
+  } else if constexpr (SECAGG) {
+    secagg_reduce(a, s_wire, s_part, A, my_pos);
   } else if constexpr (ROBUST) {
     robust_reduce<WIRE>(a, s_wire, s_rank, A, my_pos);
   } else if constexpr (SCAF) {
@@ -1315,12 +1442,13 @@ __device__ __forceinline__ void fedavg_round(const Args& a) {
     }
   }
   phase_stamp(a, 3);                                   // reduce + broadcast done
-  if (!cta_barrier_all_ranks(a, a.epoch + (KRUM ? 3 : 2), 0u, nullptr)) return;
+  if (!cta_barrier_all_ranks(a, a.epoch + (KRUM || SECAGG ? 3 : 2), 0u, nullptr)) return;
   phase_stamp(a, 4);                                   // barrier 2 passed
 
   // ---------------------------------------------------------------- phase 2: running-mean apply
   // CTA b applies exactly the tiles CTA b of the owners produced: (t / A) % G == b
-  const float apply_scale = a.use_nvls ? s_inv_total / a.nvls_prescale : 1.0f;
+  float apply_scale = a.use_nvls ? s_inv_total / a.nvls_prescale : 1.0f;
+  if constexpr (SECAGG) apply_scale = a.inv_two_f;
   for (long long q = blockIdx.x; q * A < n_tiles; q += G) {
     for (int r = 0; r < A; ++r) {
       const long long t = q * A + r;
@@ -1550,6 +1678,40 @@ fold_client_scaled_kernel(float* __restrict__ acc, float* __restrict__ theta, co
   }
 }
 
+// the standalone encode + mask (b200_secagg_encode): one 16-element block per thread and trip, the peers' keys in
+// shared memory; the same secagg_encode_block as the collective's pack
+constexpr int SECAGG_THREADS = 256;
+__global__ void __launch_bounds__(SECAGG_THREADS)
+secagg_encode_kernel(const float* __restrict__ theta, const float* __restrict__ global_w, long long n, float w, float R,
+                     float two_f, const __grid_constant__ B200SecAggPeers peers, uint32_t n0, uint32_t n1, uint32_t n2,
+                     uint32_t counter0, uint32_t* __restrict__ out, unsigned long long* saturated) {
+  __shared__ uint32_t s_key[B200_MAX_RANKS][8];
+  __shared__ int s_add[B200_MAX_RANKS];
+  for (int i = threadIdx.x; i < peers.n * 8; i += SECAGG_THREADS) s_key[i >> 3][i & 7] = peers.key[i >> 3][i & 7];
+  if (static_cast<int>(threadIdx.x) < peers.n) s_add[threadIdx.x] = peers.sign[threadIdx.x] > 0;
+  __syncthreads();
+  const long long nb = (n + 15) >> 4;
+  int sat = 0;
+  for (long long b = blockIdx.x * static_cast<long long>(SECAGG_THREADS) + threadIdx.x; b < nb;
+       b += static_cast<long long>(gridDim.x) * SECAGG_THREADS) {
+    const long long e0 = b << 4;
+    const int valid = n - e0 < 16 ? static_cast<int>(n - e0) : 16;
+    float x[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      x[j] = 0.f;
+      if (j < valid) x[j] = global_w != nullptr ? __fsub_rn(theta[e0 + j], global_w[e0 + j]) : theta[e0 + j];
+    }
+    uint32_t u[16];
+    sat += secagg_encode_block(x, valid, w, R, two_f, peers.n, [&](int p) { return s_key[p]; },
+                               [&](int p) { return s_add[p] != 0; }, counter0 + static_cast<uint32_t>(b), n0, n1, n2, u);
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+      if (j < valid) out[e0 + j] = u[j];
+  }
+  if (sat != 0 && saturated != nullptr) atomicAdd(saturated, static_cast<unsigned long long>(sat));
+}
+
 }  // namespace b200
 
 // The kernel spins on cross-GPU flags per CTA, so every CTA of the grid must be resident at the same time or the ranks
@@ -1637,6 +1799,17 @@ static bool topk_args_ok(const FedAvgTopkArgs* args) {
            args->val_off % 4 != 0 || (args->wire_kind != 0 && args->wire_kind != 1));
 }
 
+// a ring sum needs peer loads (on sm_90a the switch adds u32 only in scalar form), the delta, the fp32-sized wire, the
+// kernel's own pack after the count barrier, 16-element blocks inside a tile, a block counter that cannot wrap, and
+// f, 2^f, 2^-f consistent with R
+static bool secagg_args_ok(const FedAvgSecAggArgs* args) {
+  return !(args->use_nvls || !args->delta || args->prepacked || args->tile_flags != nullptr || args->wire_kind != 0 ||
+           args->global_w == nullptr || args->tile_elems <= 0 || args->tile_elems % 16 != 0 ||
+           args->n >= B200_SECAGG_MAX_ELEMS || !(args->range >= 0x1p-20f && args->range <= 0x1p20f) ||
+           args->frac_bits < 10 || args->frac_bits > 50 || args->two_f != ldexpf(1.f, args->frac_bits) ||
+           args->inv_two_f != ldexpf(1.f, -args->frac_bits) || args->world > B200_MAX_RANKS);
+}
+
 // the server step needs the pseudo-gradient (delta mode), the global copy and the state over [0, n_param)
 // (n_phys: the physical arena elements, args->n except in a personalized round)
 template <class Base>
@@ -1682,13 +1855,19 @@ int b200_fedavg_round(const Args* args, int n_ctas, cudaStream_t stream) {
     if (n_ctas > B200_KRUM_MAX_CTAS) n_ctas = B200_KRUM_MAX_CTAS;
   } else if constexpr (K == Agg::topk) {
     if (!topk_args_ok(args)) return -2;
+  } else if constexpr (K == Agg::secagg) {
+    if (!secagg_args_ok(args)) return -2;
   }
   if (n_ctas < 1) n_ctas = 1;
-  if constexpr (K != Agg::topk) {   // top-k rounds carry fp32 or bf16 values only
-    if (args->wire_kind == 2) return launch_round_kernel<2>(args, n_ctas, stream);
+  if constexpr (K == Agg::secagg) {   // the int32 ring
+    return launch_round_kernel<3>(args, n_ctas, stream);
+  } else {
+    if constexpr (K != Agg::topk) {   // top-k rounds carry fp32 or bf16 values only
+      if (args->wire_kind == 2) return launch_round_kernel<2>(args, n_ctas, stream);
+    }
+    if (args->wire_kind == 1) return launch_round_kernel<1>(args, n_ctas, stream);
+    return launch_round_kernel<0>(args, n_ctas, stream);
   }
-  if (args->wire_kind == 1) return launch_round_kernel<1>(args, n_ctas, stream);
-  return launch_round_kernel<0>(args, n_ctas, stream);
 }
 
 template int b200_fedavg_round(const FedAvgArgs*, int, cudaStream_t);
@@ -1703,6 +1882,8 @@ template int b200_fedavg_round(const ServerOptArgs<FedAvgScaffoldArgs>*, int, cu
 template int b200_fedavg_round(const ServerOptArgs<FedAvgRobustArgs>*, int, cudaStream_t);
 template int b200_fedavg_round(const ServerOptArgs<FedAvgKrumArgs>*, int, cudaStream_t);
 template int b200_fedavg_round(const ServerOptArgs<FedAvgTopkArgs>*, int, cudaStream_t);
+template int b200_fedavg_round(const FedAvgSecAggArgs*, int, cudaStream_t);
+template int b200_fedavg_round(const ServerOptArgs<FedAvgSecAggArgs>*, int, cudaStream_t);
 template int b200_fedavg_round(const LocalArgs<FedAvgArgs>*, int, cudaStream_t);
 template int b200_fedavg_round(const LocalArgs<ServerOptArgs<FedAvgArgs>>*, int, cudaStream_t);
 
@@ -1749,6 +1930,23 @@ extern "C" int b200_fold_client_scaled(float* acc, float* theta, const float* gl
   if (g > cap) g = cap;
   fold_client_scaled_kernel<<<static_cast<unsigned>(g), DP_NORM_THREADS, 0, stream>>>(
       acc, theta, global_w, reinterpret_cast<__nv_bfloat16*>(w_bf16), mom, n_mom, n, s, first, reset);
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int b200_secagg_encode(const float* theta, const float* global_w, long long n, float w, float range,
+                                  int frac_bits, const B200SecAggPeers* peers, const uint32_t* nonce, uint32_t counter0,
+                                  uint32_t* out, unsigned long long* saturated, cudaStream_t stream) {
+  using namespace b200;
+  if (n <= 0) return 0;
+  if (peers == nullptr || nonce == nullptr || peers->n < 0 || peers->n >= B200_MAX_RANKS || frac_bits < 10 ||
+      frac_bits > 50 || !(range >= 0x1p-20f && range <= 0x1p20f) ||
+      static_cast<unsigned long long>(counter0) + static_cast<unsigned long long>((n + 15) >> 4) > (1ull << 32))
+    return -2;
+  long long g = ((n + 15) / 16 + SECAGG_THREADS - 1) / SECAGG_THREADS;
+  const long long cap = 8ll * device_sm_count();
+  if (g > cap) g = cap;
+  secagg_encode_kernel<<<static_cast<unsigned>(g), SECAGG_THREADS, 0, stream>>>(
+      theta, global_w, n, w, range, ldexpf(1.f, frac_bits), *peers, nonce[0], nonce[1], nonce[2], counter0, out, saturated);
   return static_cast<int>(cudaGetLastError());
 }
 

@@ -266,7 +266,8 @@ struct LocalArgs : Base {
   long long len;                    // elements in the local range (multiple of 1024)
 };
 // One FedAvg round of the kind Args names: FedAvgArgs, FedAvgDPArgs, FedAvgScaffoldArgs, FedAvgRobustArgs,
-// FedAvgKrumArgs, FedAvgTopkArgs, ServerOptArgs<one of them>, or LocalArgs<FedAvgArgs / ServerOptArgs<FedAvgArgs>>.
+// FedAvgKrumArgs, FedAvgTopkArgs, FedAvgSecAggArgs (declared below), ServerOptArgs<one of them>, or
+// LocalArgs<FedAvgArgs / ServerOptArgs<FedAvgArgs>>.
 // Runs fedavg_round_kernel<WIRE, Args> (csrc/fedavg.cu)
 // cooperatively on at most n_ctas CTAs; -2 when the arguments do not fit the kind.
 template <class Args>
@@ -298,6 +299,32 @@ struct FedAvgTopkArgs : FedAvgArgs {
   long long off_off;
   long long val_off;
 };
+
+// Secure-aggregation round (parallel/secagg.py; fp32-sized wire, delta mode, peer loads, no arrival flags, not prepacked):
+// a count barrier at epoch + 1 (payload n_k) fixes the participants (live ranks with n_k > 0) and the weights
+// w_k = n_k * (1 / N) before the pack; each participant packs u = encode(theta - global) + its pairwise ChaCha20 masks
+// (csrc/secagg.cuh) as uint32, 4 per 16 B; barrier at epoch + 2; the owner of a tile adds the participants' u as
+// uint32 with wrap-around (the masks cancel) and stores the sum into every live replica; barrier at epoch + 3; the apply
+// phase adds fp32(int32(sum)) * 2^-f (or takes the server step on it).  Loss and integer arena: as in the plain round.
+struct FedAvgSecAggArgs : FedAvgArgs {
+  uint32_t keys[B200_MAX_RANKS][8]; // keys[j]: the ChaCha20 key this rank shares with rank j (unused for j == rank)
+  float range;                      // R: the clamp of every update element
+  int frac_bits;                    // f = 30 - ceil(log2 R)
+  float two_f, inv_two_f;           // 2^f, 2^-f
+  unsigned long long* saturated;    // local device counter: elements this rank clamped (or found non-finite)
+};
+#define B200_SECAGG_MAX_ELEMS (1ll << 36)   // the 32-bit block counter e / 16
+// Standalone encode + mask (the pack of a secure round, for NcclSession and tests): out[e] = encode(theta[e] - global_w[e])
+// + sum over the n_peers peers of sign[p] * S(keys[p], block counter0 + e / 16, nonce)  (mod 2^32), e in [0, n);
+// *saturated += the clamped / non-finite elements.  global_w may be nullptr (x = theta).
+struct B200SecAggPeers {
+  uint32_t key[B200_MAX_RANKS][8];
+  int sign[B200_MAX_RANKS];         // +1 or -1
+  int n;
+};
+int b200_secagg_encode(const float* theta, const float* global_w, long long n, float w, float range, int frac_bits,
+                       const B200SecAggPeers* peers, const uint32_t* nonce, uint32_t counter0, uint32_t* out,
+                       unsigned long long* saturated, cudaStream_t stream);
 
 // ---- compress.cu: top-k selection with error feedback (parallel/compress.py)
 // work: int32 [B200_TOPK_WORK_WORDS(n)] scratch; n % 1024 == 0, 1 <= k <= n, 16-byte aligned fp32 arrays.

@@ -362,6 +362,18 @@ def nonzero_pack(theta: torch.Tensor, global_w: torch.Tensor, work: torch.Tensor
     load().nonzero_pack(theta, global_w, work, int(rowptr), int(off), int(val), 0 if wire_fp32 else 1, int(cap))
 
 
+def secagg_encode(theta: torch.Tensor, global_w: Optional[torch.Tensor], w: float, range_: float, frac_bits: int,
+                  keys: Sequence[Sequence[int]], signs: Sequence[int], nonce: Sequence[int], counter0: int,
+                  out: torch.Tensor, saturated: torch.Tensor) -> None:
+    """The masked upload of a secure-aggregation round (``parallel/secagg.py``): ``out[e] = encode(theta[e] -
+    global_w[e]) + sum_p signs[p] * ChaCha20(keys[p], counter0 + e / 16, nonce)[e % 16]  (mod 2^32)`` as int32 bits,
+    ``saturated[0] +=`` the clamped or non-finite elements.  ``global_w`` None: ``x = theta``.  ``keys``: eight uint32
+    words per peer; ``signs``: +1 / -1 per peer."""
+    words = [int(k) & 0xFFFFFFFF for key in keys for k in key]
+    load().secagg_encode(theta, global_w, float(w), float(range_), int(frac_bits), words, [int(s) for s in signs],
+                         [int(x) & 0xFFFFFFFF for x in nonce], int(counter0), out, saturated)
+
+
 def dp_clip_factor(theta: torch.Tensor, global_w: torch.Tensor, clip: float, work: torch.Tensor, s_out: torch.Tensor,
                    norm_out: torch.Tensor, *, s_copy_ptr: int = 0, nonfinite: Optional[torch.Tensor] = None) -> None:
     """DP-FedAvg clip factor: ``s_out[0] = min(1, clip / ||theta - global_w||)`` (0 for a non-finite norm, which also

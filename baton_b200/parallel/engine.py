@@ -36,6 +36,7 @@ from .personal import LocalStore, resolve_local_keys
 from .robust import RobustConfig, check_aggregator, check_krum_participants, check_participants
 from .server_opt import ServerOptConfig
 from .scaffold import ScaffoldState
+from .secagg import SecAggConfig
 
 
 @dataclass
@@ -78,7 +79,8 @@ class FederatedEngine:
                  compress: Optional[str] = None, topk_ratio: float = 0.01, error_feedback: bool = True,
                  local_keys: "Optional[str | Sequence[str]]" = None, augment: Optional[str] = None,
                  augment_padding: int = 4, mix: Optional[str] = None, mix_alpha: float = 1.0,
-                 label_smoothing: float = 0.0, max_grad_norm: float = 0.0):
+                 label_smoothing: float = 0.0, max_grad_norm: float = 0.0, secure_agg: bool = False,
+                 secagg_range: float = 64.0):
         """``prox_mu > 0``: FedProx local training -- every step adds ``prox_mu * (theta - global_w)`` to the gradient,
         ``global_w`` being the global model the round started from (for logical clients too: each starts from it).
 
@@ -158,6 +160,17 @@ class FederatedEngine:
         decay, FedProx, SCAFFOLD, momentum or AdamW act.  The norm covers every trained parameter, client-local ones
         included.  It is local to each client and combines with every other option; it is not DP (``dp_clip`` clips
         client updates).  :meth:`last_grad_norms` reports the pre-clip norms.  ``0`` (the default) runs exactly the
+        plain engine.
+
+        ``secure_agg=True`` (``parallel/secagg.py``): secure aggregation -- every rank clamps its update to
+        ``[-secagg_range, secagg_range]``, encodes its weighted share in fixed point and uploads it under pairwise ChaCha20
+        masks that cancel in the ring sum, so no rank's upload is readable in the clear through the symmetric mapping.
+        The rank is the party: logical clients it hosts are folded before the upload and are not hidden from each
+        other.  The counts, the losses and integer buffers are not masked.  It needs ``wire_dtype='fp32'`` and
+        ``mode='delta'``; it cannot be combined with DP, a robust aggregator or Krum, top-k uploads, SCAFFOLD,
+        client-local entries or ``tile_flags``; every server optimizer, FedProx, AdamW, momentum, augmentation, mixing,
+        gradient clipping, logical clients and sampling combine.  The optimizer-emitted upload is off.
+        :meth:`last_secagg_saturation` reports this rank's clamped elements.  ``False`` (the default) runs exactly the
         plain engine."""
         from ..data.augment import check_augment
         from ..data.mix import check_mix, check_mix_loss
@@ -181,9 +194,12 @@ class FederatedEngine:
         self.robust = RobustConfig(aggregator, trim_ratio, krum_f, krum_m) if aggregator != "mean" else None
         self.dp = DPConfig(dp_clip, dp_noise_multiplier, dp_seed) if dp_clip > 0.0 else None
         keys = resolve_local_keys(model, local_keys) if local_keys is not None else None
+        if not isinstance(secure_agg, bool):
+            raise TypeError("secure_agg must be a bool, got {!r}".format(secure_agg))
+        self.secagg = SecAggConfig(secagg_range) if secure_agg else None
         check_features(wire_dtype=wire_dtype, mode=mode, dp=self.dp, scaffold=scaffold, robust=self.robust,
                        topk=self.topk, server_opt=sopt, tile_flags=tile_flags, optimizer=optimizer, momentum=momentum,
-                       prox_mu=prox_mu, local=keys is not None)
+                       prox_mu=prox_mu, local=keys is not None, secure_agg=secure_agg)
         self.device = torch.device(device)
         self.model = model
         self.name = name
@@ -214,7 +230,7 @@ class FederatedEngine:
         self.session = Session(self.arena, group, wire_dtype=wire_dtype, mode=mode, n_ctas=n_ctas, nvls=nvls,
                                tile_flags=tile_flags, dp=self.dp, scaffold=scaffold, server_opt=sopt,
                                robust=self.robust, topk=self.topk, max_clients=max_clients,
-                               local=self.personal is not None)
+                               local=self.personal is not None, secagg=self.secagg)
         self.dp = self.session.dp                  # rank 0's noise key
         self.accountant = RDPAccountant(self.dp.noise_multiplier) if self.dp is not None else None
         self.backend = backend
@@ -222,7 +238,8 @@ class FederatedEngine:
         # K4: the last SGD step of the captured epoch writes the upload copy itself (no pack phase in the collective);
         # only for the plain one-client-per-GPU rounds -- logical clients fold their deltas after training
         self.prepack = (backend == "fused" and self.device.type == "cuda" and self.topk is None
-                        and self.personal is None and not (logical_clients and logical_clients > self.world))
+                        and self.personal is None and self.secagg is None
+                        and not (logical_clients and logical_clients > self.world))
         if self.prepack and hasattr(self.session, "pack_spec"):
             self.trainer.pack = self.session.pack_spec()
         # the round-end collective runs on the session's high-priority side stream: the NEXT round's host->device shard
@@ -446,6 +463,14 @@ class FederatedEngine:
         if len(order) != len(scores):
             raise RuntimeError("the session reports {} clients, the round had {}".format(len(scores), len(order)))
         return {c: (float(scores[i]), bool(kept[i])) for i, c in enumerate(order)}
+
+    def last_secagg_saturation(self) -> int:
+        """Elements of this rank's upload that the last secure round clamped to ``[-secagg_range, secagg_range]`` or
+        found non-finite (a device read, made only when asked)."""
+        if self.secagg is None:
+            raise RuntimeError("secure aggregation is off (secure_agg=False)")
+        self.sync()
+        return self.session.last_secagg_saturation()
 
     def server_state(self):
         """``(m, v)``: the server optimizer's state over the parameters (live fp32 tensors on the engine's device, equal

@@ -21,12 +21,13 @@ SEATED_SERVER_OPT = ("a server optimizer needs the http plane: on the seated pla
 def check_features(*, wire_dtype: str = "bf16", mode: str = "delta", dp=None, scaffold: bool = False, robust=None,
                    topk=None, server_opt=None, tile_flags: bool = False, plane: Optional[str] = None,
                    optimizer: str = "sgd", momentum: float = 0.0, nesterov: bool = False, prox_mu: float = 0.0,
-                   local: bool = False) -> None:
+                   local: bool = False, secure_agg: bool = False) -> None:
     """``ValueError`` with the reason if the features cannot run together.  ``dp``, ``robust``, ``topk`` and
     ``server_opt`` are on unless they are None or False: the rules read only which features are on, so a caller may pass
     the features' configurations or bools.  Whoever takes a configuration from outside checks its type.  ``plane``:
     ``"http"`` or ``"seated"`` (the ``fused`` / ``nccl`` manager planes), None where no manager plane is involved.
-    ``local``: client-local ``state_dict`` entries (FedBN / FedPer, ``parallel/personal.py``)."""
+    ``local``: client-local ``state_dict`` entries (FedBN / FedPer, ``parallel/personal.py``).  ``secure_agg``: secure
+    aggregation (``parallel/secagg.py``)."""
     if optimizer not in OPTIMIZERS:
         raise ValueError("optimizer must be one of {}, got {!r}".format(OPTIMIZERS, optimizer))
     adamw = optimizer == "adamw"
@@ -66,22 +67,40 @@ def check_features(*, wire_dtype: str = "bf16", mode: str = "delta", dp=None, sc
                                "granules, and the first layer may be local"),
         (local and plane is not None, "client-local entries need the SPMD engine: a manager plane's payload is a whole "
                                       "state_dict, and its seats would need per-client stores"),
+        (secure_agg and wire_dtype != "fp32", "secure aggregation needs wire_dtype='fp32': its ring elements are 4 "
+                                              "bytes, and the symmetric buffer is sized from the wire dtype"),
+        (secure_agg and dp, "secure aggregation with DP-FedAvg is not supported: the reader-side clip factors and the "
+                            "owner's noise sit outside the ring"),
+        (secure_agg and robust, "secure aggregation with a robust aggregator or Krum is not supported: they need every "
+                                "client's individual update"),
+        (secure_agg and topk, "secure aggregation with top-k uploads is not supported: the sparse supports reveal "
+                              "positions"),
+        (secure_agg and scaffold, "secure aggregation with SCAFFOLD is not supported: its control-variate segment would "
+                                  "need its own masks"),
+        (secure_agg and local, "secure aggregation with client-local entries is not supported"),
+        (secure_agg and tile_flags, "secure aggregation with tile_flags is not supported: the ring sum is decoded in "
+                                    "the apply phase, not published tile by tile"),
+        (secure_agg and plane is not None, "secure aggregation needs the SPMD engine: the manager planes have no key "
+                                           "exchange, and their payload is a pickled state_dict"),
     )
     for broken, reason in rules:
         if broken:
             raise ValueError(reason)
     if mode != "delta":
         for on, name in ((topk, "top-k uploads"), (server_opt, "a server optimizer"), (dp, "DP-FedAvg"),
-                         (scaffold, "SCAFFOLD"), (robust, "a robust aggregator")):
+                         (scaffold, "SCAFFOLD"), (robust, "a robust aggregator"), (secure_agg, "secure aggregation")):
             if on:
                 raise ValueError("{} needs mode='delta': it works on the update theta - global, which "
                                  "mode='weights' does not upload".format(name))
 
 
-def peer_loads_only(*, wire_dtype: str, dp=None, scaffold: bool = False, robust=None, topk=None) -> bool:
+def peer_loads_only(*, wire_dtype: str, dp=None, scaffold: bool = False, robust=None, topk=None,
+                    secure_agg: bool = False) -> bool:
     """True when a round cannot use NVLS: the switch adds raw wire values, so block-scaled fp8, DP's per-rank clip
-    factors, SCAFFOLD's reader-side 1 / N, a selection (robust) and sparse lists (top-k) all need peer loads."""
-    return wire_dtype == "fp8" or any(x is not None and x is not False for x in (dp, scaffold, robust, topk))
+    factors, SCAFFOLD's reader-side 1 / N, a selection (robust) and sparse lists (top-k) all need peer loads.  A secure
+    round's ring sum would need ``multimem.ld_reduce.add.u32``, which sm_90a has in scalar form only (four times the
+    switch operations of the float path, not measured)."""
+    return wire_dtype == "fp8" or any(x is not None and x is not False for x in (dp, scaffold, robust, topk, secure_agg))
 
 
 def round_plan(world: int, logical_clients: int = 0, sample_k: Optional[int] = None) -> Tuple[int, int]:

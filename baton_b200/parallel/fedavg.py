@@ -49,11 +49,20 @@ applied to the round's aggregate, whatever computed it (mean, DP, SCAFFOLD, medi
 allocates the state ``arena.server_m`` / ``arena.server_v`` over the parameters, replicated on every rank; the fused
 session runs the round's kernel on ``ServerOptArgs<...>`` of the round's arguments, whose apply phase takes the step, and
 :class:`NcclSession` calls :func:`server_step_` where it would add the aggregate.  :meth:`server_state` reads the state.
+
+Both take ``secagg=SecAggConfig(range)`` (``parallel/secagg.py``): secure aggregation over the fp32-sized wire in delta
+mode.  The ranks agree on pairwise ChaCha20 keys with one X25519 exchange at construction; every round each participant
+uploads its fixed-point update plus its pairwise masks, which cancel in the uint32 sum.  The fused session runs the
+``Agg::secagg`` kernel (count barrier, masked pack, wrapping reduce, decode in the apply phase), always on peer loads and
+never prepacked; :class:`NcclSession` encodes with the same kernel (the numpy reference on the CPU), all-reduces the
+masked words as int64 and keeps the low 32 bits.  :meth:`last_secagg_saturation` reads this rank's clamped elements of
+the last round.
 """
 from __future__ import annotations
 
 from typing import List, Optional, Sequence
 
+import numpy as np
 import torch
 
 from .arena import ParamArena
@@ -61,6 +70,8 @@ from .compress import TopKConfig, n_float, sparse_upload_bytes, topk_ef_
 from .dp import DPConfig, clip_factor, normals
 from .features import check_features, peer_loads_only
 from .robust import MAX_ROBUST_CLIENTS, RobustConfig, krum_select, robust_combine
+from . import secagg as sa
+from .secagg import SecAggConfig
 from .server_opt import ServerOptConfig, apply_update_
 from .symm import SymmetricBuffer
 
@@ -76,10 +87,12 @@ def _session_rules(features: dict, dp: Optional[DPConfig], robust: Optional[Robu
     """:func:`check_features` for a session's features with a round's ``dp`` / ``robust``, after ``TypeError`` for a
     ``robust``, ``topk`` or ``server_opt`` that is not its configuration class."""
     for x, cls, name in ((robust, RobustConfig, "robust"), (features["topk"], TopKConfig, "topk"),
-                         (features["server_opt"], ServerOptConfig, "server_opt")):
+                         (features["server_opt"], ServerOptConfig, "server_opt"), (features["secagg"], SecAggConfig,
+                                                                                   "secagg")):
         if x is not None and not isinstance(x, cls):
             raise TypeError("{}= takes a {}".format(name, cls.__name__))
-    check_features(dp=dp, robust=robust, **features)
+    f = dict(features)
+    check_features(dp=dp, robust=robust, secure_agg=f.pop("secagg") is not None, **f)
 
 
 def _init_session(arena: ParamArena, features: dict, dp: Optional[DPConfig], robust: Optional[RobustConfig],
@@ -110,6 +123,13 @@ def _check_control(scaffold: bool, control) -> None:
         raise ValueError("control= needs a session built with scaffold=True")
 
 
+def _secagg_keys(secagg: Optional[SecAggConfig], group) -> dict:
+    """``{peer rank: eight uint32 key words}`` of a secure session (one X25519 exchange over ``group``), else ``{}``."""
+    if secagg is None:
+        return {}
+    return {j: sa.key_words(k) for j, k in sa.agree_keys(group).items()}
+
+
 def _agree_seed(dp: Optional[DPConfig], group) -> Optional[DPConfig]:
     """Every rank must draw the same noise: take rank 0's Philox key (a DPConfig built with seed=None differs per
     process)."""
@@ -128,12 +148,12 @@ class FedAvgSession:
                  reset_momentum: bool = True, tile_flags: bool = False, dp: Optional[DPConfig] = None,
                  scaffold: bool = False, robust: Optional[RobustConfig] = None, max_clients: int = 1,
                  server_opt: Optional[ServerOptConfig] = None, topk: Optional[TopKConfig] = None,
-                 local: bool = False):
+                 local: bool = False, secagg: Optional[SecAggConfig] = None):
         from ..ops._ext import load
         self._C = load()
         assert wire_dtype in ("bf16", "fp32", "fp8") and mode in ("delta", "weights")
         self._features = dict(wire_dtype=wire_dtype, mode=mode, scaffold=scaffold, topk=topk, server_opt=server_opt,
-                             tile_flags=tile_flags, local=bool(local))
+                             tile_flags=tile_flags, local=bool(local), secagg=secagg)
         self.max_clients = _init_session(arena, self._features, dp, robust, max_clients)
         self.local_range = arena.local_range
         self.n_wire = arena.n_shared           # elements on the wire: the arena minus its client-local range
@@ -194,8 +214,16 @@ class FedAvgSession:
         # nvls: True, False or "auto" (on where the box has multicast; autotuned below)
         self.use_nvls = bool(nvls and self.symm.has_multicast
                              and not peer_loads_only(wire_dtype=wire_dtype, dp=dp, scaffold=scaffold, robust=robust,
-                                                     topk=topk))
+                                                     topk=topk, secure_agg=secagg is not None))
         self.dp = _agree_seed(dp, group)
+        # secure aggregation: the pair keys (host memory and this rank's kernel arguments only) and the saturation count
+        self.secagg = secagg
+        if secagg is not None:
+            if arena.n >= sa.MAX_ARENA:
+                raise ValueError("secure aggregation needs an arena of fewer than 2^36 elements")
+            keys = _secagg_keys(secagg, group)
+            self._secagg_words = [w for r in range(self.world) for w in keys.get(r, [0] * 8)]
+            self.secagg_sat = torch.zeros(1, dtype=torch.int64, device=self.device)
         self._topk_work = None          # top-k: the selection's scratch, the residual-less u, the last upload's row end
         self._topk_u = None
         self._topk_end = None
@@ -303,7 +331,8 @@ class FedAvgSession:
     def pack_spec(self) -> Optional[dict]:
         """Arguments for ``ops.fused_sgd(pack=...)`` (stable device tensors: safe to capture), or None when the wire
         format needs the in-kernel pack (block-scaled fp8)."""
-        if self.wire_kind == 2 or self.device.type != "cuda" or self.topk is not None or self.local_range is not None:
+        if (self.wire_kind == 2 or self.device.type != "cuda" or self.topk is not None or self.local_range is not None
+                or self.secagg is not None):
             return None
         a = self.arena
         return {"wire_slot": self.wire_slot, "global_w": a.global_w if self.delta else None, "scale": self.pack_scale,
@@ -489,7 +518,7 @@ class FedAvgSession:
                                                 robust=robust, topk=self.topk))
         want_scale = (counts[self.rank] if not from_flags else float(my_n)) if (self.use_nvls and world > 1) else 1.0
         prepacked = bool(prepacked and self.wire_kind != 2 and self._armed_for == (self.epoch, float(want_scale))
-                         and (nvls_now == bool(self.use_nvls and world > 1)))
+                         and (nvls_now == bool(self.use_nvls and world > 1)) and self.secagg is None)
         if robust is not None:
             m = (1 if counts[self.rank] != 0.0 else 0) if n_clients is None else int(n_clients)
             if not (0 <= m <= self.max_clients):
@@ -541,6 +570,10 @@ class FedAvgSession:
             if self.topk is not None:
                 launch = self._C.fedavg_allreduce_topk
                 own = (self.topk_rowptr_off, self.topk_off_off, self.topk_val_off)
+            elif self.secagg is not None:
+                launch = self._C.fedavg_allreduce_secagg
+                self.secagg_sat.zero_()
+                own = (self._secagg_words, self.secagg.range, self.secagg.frac_bits, self.secagg_sat)
             elif robust is not None and robust.kind == "krum":
                 launch = self._C.fedavg_allreduce_krum
                 own = (self.symm.peer_ptrs(o_clip), m, self.seg_stride,
@@ -590,6 +623,13 @@ class FedAvgSession:
             raise RuntimeError("server_state needs a session built with server_opt=")
         self.join()
         return self.arena.server_m, self.arena.server_v
+
+    def last_secagg_saturation(self) -> int:
+        """Elements this rank clamped to ``[-R, R]`` (or found non-finite) in the last secure round (a host read)."""
+        if self.secagg is None:
+            raise RuntimeError("last_secagg_saturation needs a session built with secagg=")
+        self.join()
+        return int(self.secagg_sat.item())
 
     def last_krum(self):
         """``(D, scores, kept)`` of the last Krum round, in segment order (a host read): the fp64 ``[P, P]`` squared
@@ -696,10 +736,10 @@ class NcclSession:
                  reset_momentum: bool = True, dp: Optional[DPConfig] = None, scaffold: bool = False,
                  robust: Optional[RobustConfig] = None, max_clients: int = 1, tile_flags: bool = False,
                  server_opt: Optional[ServerOptConfig] = None, topk: Optional[TopKConfig] = None,
-                 local: bool = False, **_unused):
+                 local: bool = False, secagg: Optional[SecAggConfig] = None, **_unused):
         import torch.distributed as dist
         self._features = dict(wire_dtype=wire_dtype, mode=mode, scaffold=scaffold, topk=topk, server_opt=server_opt,
-                             tile_flags=tile_flags, local=bool(local))
+                             tile_flags=tile_flags, local=bool(local), secagg=secagg)
         self.max_clients = _init_session(arena, self._features, dp, robust, max_clients)
         self.local_range = arena.local_range
         self.topk, self.server_opt = topk, server_opt
@@ -727,6 +767,9 @@ class NcclSession:
         self.segs = (torch.zeros(self.max_clients, arena.n, dtype=self.wire_dtype, device=self.device)
                      if robust is not None else None)
         self.counts = torch.zeros(self.world, dtype=torch.float32, device=self.device)
+        self.secagg = secagg
+        self._secagg_keys = _secagg_keys(secagg, group)
+        self.secagg_saturated = 0
         self.loss_buf = torch.zeros(MAX_LOSS, dtype=torch.float32, device=self.device)
         self.loss_out = torch.zeros(MAX_LOSS, dtype=torch.float32, device=self.device)
         self.rounds = 0
@@ -828,6 +871,42 @@ class NcclSession:
             robust = RobustConfig("trimmed_mean", 0.0)
         return robust_combine(stacked, robust).to(self.wire_dtype).float()
 
+    def _secagg_update(self, counts: torch.Tensor, src: torch.Tensor) -> torch.Tensor:
+        """The secure round's aggregate ``d``: this rank's masked upload (the encode kernel on CUDA, the numpy reference
+        on the CPU; zeros when it does not participate), the int64 all-reduce of the uint32 words, the low 32 bits,
+        decoded.  The nonce is the round counter."""
+        cfg, f = self.secagg, self.secagg.frac_bits
+        c = counts.tolist()
+        w, _ = sa.weights(c)
+        parts = [k for k, x in enumerate(c) if x > 0]
+        nonce = (self.rounds & 0xFFFFFFFF, 0, 0)
+        self.secagg_saturated = 0
+        u = torch.zeros(src.numel(), dtype=torch.int64, device=self.device)
+        if self.rank in parts:
+            peers = sa.peer_list(self.rank, parts, self._secagg_keys)
+            if src.is_cuda:
+                from ..ops import functional as F
+                out = torch.empty(src.numel(), dtype=torch.int32, device=self.device)
+                sat = torch.zeros(1, dtype=torch.int64, device=self.device)
+                F.secagg_encode(src.contiguous(), None, float(w[self.rank]), cfg.range, f, [k for k, _ in peers],
+                                [s for _, s in peers], nonce, 0, out, sat)
+                u = out.to(torch.int64) & 0xFFFFFFFF
+                self.secagg_saturated = int(sat.item())
+            else:
+                q, self.secagg_saturated = sa.encode(src.numpy(), float(w[self.rank]), cfg.range, f)
+                u = torch.from_numpy(sa.mask(q, peers, nonce).astype(np.int64))
+        if self.world > 1:
+            self.dist.all_reduce(u, group=self.group)
+        u = u & 0xFFFFFFFF
+        ring = torch.where(u >= 1 << 31, u - (1 << 32), u).to(torch.int32)     # int32(sum mod 2^32)
+        return ring.float() * (2.0 ** -f)
+
+    def last_secagg_saturation(self) -> int:
+        """Elements this rank clamped (or found non-finite) in the last secure round."""
+        if self.secagg is None:
+            raise RuntimeError("last_secagg_saturation needs a session built with secagg=")
+        return self.secagg_saturated
+
     def last_krum(self):
         """``(D, scores, kept)`` of the last Krum round in segment order, as :meth:`FedAvgSession.last_krum` (here the
         host oracle's fp64 values)."""
@@ -876,6 +955,8 @@ class NcclSession:
         if robust is not None:
             upd = self._robust_update(counts, n_clients, robust)
             w = w if float(total) > 0.0 else torch.zeros_like(w)
+        elif self.secagg is not None:
+            upd = self._secagg_update(counts, src)
         elif n_clients is not None:
             raise ValueError("n_clients= needs a session built with robust=")
         elif dp is not None:
@@ -890,7 +971,7 @@ class NcclSession:
             self.wire.copy_((src * wd).to(self.wire_dtype))
         else:
             self.wire.copy_((src * w).to(self.wire_dtype))
-        if self.world > 1 and robust is None:
+        if self.world > 1 and robust is None and self.secagg is None:
             dist.all_reduce(self.wire, group=self.group)
         # every rank joins the loss reduce every round -- a rank that hosts no sampled client this round
         # contributes zeros (weight 0); skipping the call there would desynchronise the collectives
@@ -902,7 +983,7 @@ class NcclSession:
             dist.all_reduce(self.loss_buf, group=self.group)
         self.loss_out.copy_(self.loss_buf)
         d = None                        # the round's aggregate (delta mode)
-        if robust is not None:
+        if robust is not None or self.secagg is not None:
             d = upd
         elif dp is not None and dp.noise_std > 0.0 and float(total) > 0.0:
             z = torch.from_numpy(normals(dp.seed, self.rounds & 0xFFFFFFFF, a.n)).to(device=self.device,
