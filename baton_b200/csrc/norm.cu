@@ -828,10 +828,11 @@ bn_bwd_cluster_kernel(const uint4* __restrict__ x, const uint4* __restrict__ y, 
   const int r_begin = static_cast<int>(me) * rows_per_cta;
   int r_end = r_begin + rows_per_cta;
   if (r_end > rows) r_end = rows;
+  // mean / rstd come from the forward pass, but only the wait is transitive: the grid that wrote them may still run
+  griddep_wait();
   float m[8], rs[8];
 #pragma unroll
-  for (int j = 0; j < 8; ++j) { m[j] = mean[c0 + j]; rs[j] = rstd[c0 + j]; }    // written two kernels ago at the latest
-  griddep_wait();
+  for (int j = 0; j < 8; ++j) { m[j] = mean[c0 + j]; rs[j] = rstd[c0 + j]; }
   constexpr int NC = ITER > 0 ? ITER : 1;          // ITER == 0: rows are NOT cached (any row count): second pass re-reads
   float xh[NC][8], g[NC][8];
   float sg[8], sgx[8];
@@ -884,11 +885,12 @@ bn_bwd_cluster_kernel(const uint4* __restrict__ x, const uint4* __restrict__ y, 
       }
     }
   }
-  // warp reduce over the 16 row lanes that share this chunk (lane bit 0 = chunk)
+  // warp reduce over the 16 row lanes that share this chunk (lane bit 0 = chunk); the 16 chains are independent, so
+  // each round issues all of them before the next round needs their results
 #pragma unroll
-  for (int j = 0; j < 8; ++j) {
+  for (int o = 2; o < 32; o <<= 1) {
 #pragma unroll
-    for (int o = 2; o < 32; o <<= 1) {
+    for (int j = 0; j < 8; ++j) {
       sg[j] += __shfl_xor_sync(0xffffffffu, sg[j], o);
       sgx[j] += __shfl_xor_sync(0xffffffffu, sgx[j], o);
     }
@@ -1286,7 +1288,9 @@ extern "C" int b200_bn_bwd_apply(const void* x, const void* y, const void* dy, v
                                  float* dbeta, long long rows, int C, int relu, cudaStream_t stream) {
   if (rows <= 0) return 0;
   if (C % 8) return -2;
-  launch_pdl(bn_bwd_apply_kernel, stream_grid(rows * (C / 8)), 256, 4 * C * sizeof(float), stream, 
+  const size_t smem = 4 * C * sizeof(float);     // above the 48 KB default from C = 3080 (shapes the cluster kernel declines)
+  if (smem > 48 * 1024) cudaFuncSetAttribute(bn_bwd_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  launch_pdl(bn_bwd_apply_kernel, stream_grid(rows * (C / 8)), 256, smem, stream,
       reinterpret_cast<const uint4*>(x), reinterpret_cast<const uint4*>(y), reinterpret_cast<const uint4*>(dy),
       reinterpret_cast<uint4*>(dx), reinterpret_cast<uint4*>(dres), gamma, save_mean, save_rstd, sums, dgamma, dbeta,
       rows, C, relu);
