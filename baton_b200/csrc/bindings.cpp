@@ -1204,6 +1204,66 @@ bool bn_bwd_cluster(const at::Tensor& x, const at::Tensor& y, const at::Tensor& 
   check(rc, "bn_bwd_cluster");
   return true;
 }
+// GroupNorm forward / backward over NHWC bf16 [N, H, W, C] (csrc/norm.cu).  `work`: fp32 [G + 2 N C] whose first G
+// words the forward zeroes (optional there) and the backward needs zero; dgamma / dbeta are accumulated.
+static void gn_check(const at::Tensor& z, int64_t G, const char* what) {
+  CHECK_CUDA(z);
+  TORCH_CHECK(z.dim() == 4 && z.scalar_type() == at::kBFloat16 && z.is_contiguous(), what, ": contiguous bf16 NHWC input");
+  TORCH_CHECK(G > 0 && z.size(3) % G == 0, what, ": num_groups must divide the channels");
+}
+// an activation-shaped argument: contiguous bf16 of z's shape on z's device
+static void gn_like(const at::Tensor& t, const at::Tensor& z, const char* what, const char* name) {
+  TORCH_CHECK(t.device() == z.device() && t.scalar_type() == at::kBFloat16 && t.sizes() == z.sizes() && t.is_contiguous(),
+              what, ": ", name, " must be a contiguous bf16 tensor shaped like the input");
+}
+// an fp32 vector of at least n elements on z's device
+static void gn_f32(const at::Tensor& t, const at::Tensor& z, int64_t n, const char* what, const char* name) {
+  TORCH_CHECK(t.device() == z.device() && t.scalar_type() == at::kFloat && t.is_contiguous() && t.numel() >= n, what,
+              ": ", name, " must be a contiguous fp32 tensor of at least ", n, " elements");
+}
+void gn_fwd(const at::Tensor& z, const std::optional<at::Tensor>& res, at::Tensor y, const at::Tensor& gamma,
+            const at::Tensor& beta, at::Tensor mean, at::Tensor rstd, int64_t G, double eps, bool relu,
+            const std::optional<at::Tensor>& work) {
+  gn_check(z, G, "gn_fwd");
+  const int64_t N = z.size(0), C = z.size(3);
+  if (res) gn_like(*res, z, "gn_fwd", "residual");
+  gn_like(y, z, "gn_fwd", "y");
+  gn_f32(gamma, z, C, "gn_fwd", "gamma");
+  gn_f32(beta, z, C, "gn_fwd", "beta");
+  gn_f32(mean, z, N * G, "gn_fwd", "mean");
+  gn_f32(rstd, z, N * G, "gn_fwd", "rstd");
+  if (work) gn_f32(*work, z, G, "gn_fwd", "work");
+  const c10::cuda::CUDAGuard guard(z.device());
+  check(b200_gn_fwd(z.data_ptr(), opt_ptr<const void>(res), y.data_ptr(), gamma.data_ptr<float>(), beta.data_ptr<float>(),
+                    mean.data_ptr<float>(), rstd.data_ptr<float>(), opt_ptr<float>(work), z.size(0),
+                    z.size(1) * z.size(2), static_cast<int>(z.size(3)), static_cast<int>(G), static_cast<float>(eps), relu,
+                    cur_stream()),
+        "gn_fwd");
+}
+void gn_bwd(const at::Tensor& z, const at::Tensor& y, const at::Tensor& dy_a, const std::optional<at::Tensor>& dy_b,
+            at::Tensor dz, const std::optional<at::Tensor>& dres, const at::Tensor& gamma, const at::Tensor& mean,
+            const at::Tensor& rstd, const std::optional<at::Tensor>& dgamma, const std::optional<at::Tensor>& dbeta,
+            int64_t G, bool relu, at::Tensor work) {
+  gn_check(z, G, "gn_bwd");
+  const int64_t N = z.size(0), C = z.size(3);
+  gn_like(y, z, "gn_bwd", "y");
+  gn_like(dy_a, z, "gn_bwd", "dy_a");
+  if (dy_b) gn_like(*dy_b, z, "gn_bwd", "dy_b");
+  gn_like(dz, z, "gn_bwd", "dz");
+  if (dres) gn_like(*dres, z, "gn_bwd", "dres");
+  gn_f32(gamma, z, C, "gn_bwd", "gamma");
+  gn_f32(mean, z, N * G, "gn_bwd", "mean");
+  gn_f32(rstd, z, N * G, "gn_bwd", "rstd");
+  if (dgamma) gn_f32(*dgamma, z, C, "gn_bwd", "dgamma");
+  if (dbeta) gn_f32(*dbeta, z, C, "gn_bwd", "dbeta");
+  gn_f32(work, z, G + 2 * N * C, "gn_bwd", "work");
+  const c10::cuda::CUDAGuard guard(z.device());
+  check(b200_gn_bwd(z.data_ptr(), y.data_ptr(), dy_a.data_ptr(), opt_ptr<const void>(dy_b), dz.data_ptr(),
+                    opt_ptr<void>(dres), gamma.data_ptr<float>(), mean.data_ptr<float>(), rstd.data_ptr<float>(),
+                    opt_ptr<float>(dgamma), opt_ptr<float>(dbeta), work.data_ptr<float>(), z.size(0),
+                    z.size(1) * z.size(2), static_cast<int>(z.size(3)), static_cast<int>(G), relu, cur_stream()),
+        "gn_bwd");
+}
 // eval-mode BatchNorm folding of every BatchNorm in `table` (int64 [n_bn, 7], see launch.h) into `out`
 void bn_fold_eval(const at::Tensor& arena, const at::Tensor& table, at::Tensor out) {
   CHECK_CUDA(arena); CHECK_CUDA(table); CHECK_CUDA(out);
@@ -1358,6 +1418,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("attention_fwd", &attention_fwd);
   m.def("attention_bwd", &attention_bwd);
   m.def("bn_bwd_cluster", &bn_bwd_cluster);
+  m.def("gn_fwd", &gn_fwd);
+  m.def("gn_bwd", &gn_bwd);
   m.def("im2col_tma_probe", &im2col_tma_probe);
   m.def("conv_igemm_fwd", &conv_igemm_fwd);
   m.def("conv_igemm_wgrad", &conv_igemm_wgrad);

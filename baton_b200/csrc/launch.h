@@ -374,6 +374,15 @@ int b200_bn_maxpool_bwd(const void* z, const void* p, const void* argmax, const 
 int b200_bn_bwd_cluster(const void* x, const void* y, const void* dy_a, const void* dy_b, void* dx, void* dres,
                         const float* gamma, const float* save_mean, const float* save_rstd, float* dgamma, float* dbeta,
                         long long rows, int C, int relu, int max_cluster, cudaStream_t stream);
+// GroupNorm over NHWC bf16 [N, HW, C], G groups of C / G channels (csrc/norm.cu).  Forward: y = relu?(gamma * (z -
+// mean) * rstd + beta + residual?), mean / rstd fp32 [N, G]; `work` (or nullptr): the backward's buffer, whose G
+// counters it zeroes.  Backward: dz, dres = dy' (or nullptr), dgamma / dbeta ACCUMULATED (fixed summation order);
+// work: fp32 [G + 2 N C], first G words zero.  Both return -2 when G does not divide C.
+int b200_gn_fwd(const void* z, const void* residual, void* y, const float* gamma, const float* beta, float* mean,
+                float* rstd, float* work, long long N, long long HW, int C, int G, float eps, int relu, cudaStream_t stream);
+int b200_gn_bwd(const void* z, const void* y, const void* dy_a, const void* dy_b, void* dz, void* dres, const float* gamma,
+                const float* mean, const float* rstd, float* dgamma, float* dbeta, float* work, long long N, long long HW,
+                int C, int G, int relu, cudaStream_t stream);
 // eval-mode BatchNorm folding: one block per BatchNorm; table = int64 [n_bn][7] {gamma, beta, running_mean,
 // running_var (element offsets into arena; gamma / beta -1 = none), output offset, C, eps as float bits}
 int b200_bn_fold_eval(const float* arena, const long long* table, int n_bn, float* out, cudaStream_t stream);

@@ -2,6 +2,8 @@
 // [rows, C] bf16 matrix (fused residual add + ReLU, running-stat update), LayerNorm forward /
 // backward (fused residual add) and row softmax for attention.  Statistics and gradients in fp32.
 #define B200_TU_TAG 10
+#include <atomic>
+
 #include "launch.h"
 #include "pdl.cuh"
 #include "ptx.cuh"
@@ -1225,6 +1227,252 @@ bn_fold_eval_kernel(const float* __restrict__ arena, const long long* __restrict
   }
 }
 
+// ------------------------------------------------------------------ GroupNorm (+residual +ReLU)
+// NHWC bf16 [N, HW, C] with G groups of Cg = C / G contiguous channels: group (n, g) is the HW x Cg block of sample n,
+// M = HW * Cg elements.  One CTA per (n, g), blockIdx.x = n * G + g.  Statistics in fp32: the mean, then the biased
+// variance from centred values (post-ReLU inputs have large means, so E[x^2] - E[x]^2 would cancel).
+//   forward : y = relu?(gamma_c * (z - mean) * rstd + beta_c + residual?), saves mean / rstd [N, G]
+//   backward: dy' = (dy_a + dy_b?) * (y > 0 if relu), dres = dy',
+//             dz = rstd * (gamma_c dy' - mean(gamma dy') - xhat * mean(gamma dy' xhat)),
+//             dgamma_c += sum_{n,hw} dy' xhat, dbeta_c += sum_{n,hw} dy'.
+// CACHE: the (n, g) block is kept in shared memory (z as bf16, and dy' as fp32 in the backward), so global memory is read
+// once and written once; otherwise (ResNet stems of large images) every pass re-reads global memory.  Every sum has a
+// fixed order for a given shape: shuffle trees, warp partials in index order, and for the per-channel parameter
+// gradients (which cross samples) per-CTA partials that the last CTA of each group adds in sample order -- the same bits
+// on every launch, with no float atomics.  work: fp32 [G + 2 N C]; words [0, G) are per-group arrival counters that the
+// forward zeroes and the backward leaves zero, then the [N][C][2] partials.
+constexpr int GN_THREADS = 256;
+constexpr long long GN_CACHE_ELEMS = 16384;      // one (n, g) block on chip: 32 KB forward, 96 KB backward
+
+template <int W>
+__device__ __forceinline__ void gn_ld(const __nv_bfloat16* p, float (&f)[W]) {
+  if constexpr (W == 8) {
+    unpack8_bn(*reinterpret_cast<const uint4*>(p), f);
+  } else {
+#pragma unroll
+    for (int j = 0; j < W; ++j) f[j] = __bfloat162float(p[j]);
+  }
+}
+template <int W>
+__device__ __forceinline__ void gn_st(__nv_bfloat16* p, const float (&f)[W]) {
+  if constexpr (W == 8) {
+    *reinterpret_cast<uint4*>(p) = make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]),
+                                              pack_bf16x2(f[6], f[7]));
+  } else {
+#pragma unroll
+    for (int j = 0; j < W; ++j) p[j] = __float2bfloat16_rn(f[j]);
+  }
+}
+// x and the masked gradient dy' of W consecutive channels at element offset o
+template <int W>
+__device__ __forceinline__ void gn_grad(long long o, const __nv_bfloat16* __restrict__ z, const __nv_bfloat16* __restrict__ y,
+                                        const __nv_bfloat16* __restrict__ dy_a, const __nv_bfloat16* __restrict__ dy_b,
+                                        int relu, float (&xf)[W], float (&gf)[W]) {
+  gn_ld<W>(z + o, xf);
+  gn_ld<W>(dy_a + o, gf);
+  if (dy_b != nullptr) {
+    float t[W];
+    gn_ld<W>(dy_b + o, t);
+#pragma unroll
+    for (int j = 0; j < W; ++j) gf[j] += t[j];
+  }
+  if (relu) {
+    float yf[W];
+    gn_ld<W>(y + o, yf);
+#pragma unroll
+    for (int j = 0; j < W; ++j)
+      if (!(yf[j] > 0.f)) gf[j] = 0.f;
+  }
+}
+// CTA-wide sum in a fixed order; every thread receives it.  `red`: GN_THREADS / 32 floats of shared memory.
+__device__ __forceinline__ float gn_cta_sum(float v, float* red) {
+  v = warp_sum(v);
+  __syncthreads();                 // a previous call may still be reading red
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float t = 0.f;
+#pragma unroll
+  for (int w = 0; w < GN_THREADS / 32; ++w) t += red[w];
+  return t;
+}
+
+template <int VEC, bool CACHE>
+__global__ void __launch_bounds__(GN_THREADS)
+gn_fwd_kernel(const __nv_bfloat16* __restrict__ z, const __nv_bfloat16* __restrict__ res, __nv_bfloat16* __restrict__ y,
+              const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ mean_out,
+              float* __restrict__ rstd_out, unsigned* __restrict__ counters, long long HW, int C, int G, float eps,
+              int relu) {
+  griddep_launch_dependents();
+  extern __shared__ __align__(16) unsigned char gn_smem[];
+  __nv_bfloat16* zc = reinterpret_cast<__nv_bfloat16*>(gn_smem);    // [M] when CACHE
+  __shared__ float red[GN_THREADS / 32];
+  const int g = static_cast<int>(blockIdx.x % G);
+  const long long n = blockIdx.x / G;
+  const int Cg = C / G, CgV = Cg / VEC;
+  const long long M = HW * Cg, MV = M / VEC;
+  const long long base = n * HW * C + static_cast<long long>(g) * Cg;
+  griddep_wait();
+  float s = 0.f;
+  for (long long v = threadIdx.x; v < MV; v += GN_THREADS) {
+    float f[VEC];
+    gn_ld<VEC>(z + base + (v / CgV) * C + (v % CgV) * VEC, f);
+    if constexpr (CACHE) gn_st<VEC>(zc + v * VEC, f);
+#pragma unroll
+    for (int j = 0; j < VEC; ++j) s += f[j];
+  }
+  const float fm = static_cast<float>(M);
+  const float mean = __fdiv_rn(gn_cta_sum(s, red), fm);
+  float q = 0.f;
+  for (long long v = threadIdx.x; v < MV; v += GN_THREADS) {
+    float f[VEC];
+    gn_ld<VEC>(CACHE ? zc + v * VEC : z + base + (v / CgV) * C + (v % CgV) * VEC, f);
+#pragma unroll
+    for (int j = 0; j < VEC; ++j) {
+      const float d = f[j] - mean;
+      q = fmaf(d, d, q);
+    }
+  }
+  const float var = __fdiv_rn(gn_cta_sum(q, red), fm);
+  const float rstd = rsqrtf(var + eps);
+  if (threadIdx.x == 0) {
+    mean_out[blockIdx.x] = mean;
+    rstd_out[blockIdx.x] = rstd;
+    if (counters != nullptr && n == 0) counters[g] = 0u;
+  }
+  for (long long v = threadIdx.x; v < MV; v += GN_THREADS) {
+    const long long o = base + (v / CgV) * C + (v % CgV) * VEC;
+    const int c0 = g * Cg + static_cast<int>(v % CgV) * VEC;
+    float f[VEC], r[VEC];
+    gn_ld<VEC>(CACHE ? zc + v * VEC : z + o, f);
+    if (res != nullptr) {
+      gn_ld<VEC>(res + o, r);
+    } else {
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) r[j] = 0.f;
+    }
+#pragma unroll
+    for (int j = 0; j < VEC; ++j) {
+      float u = fmaf(gamma[c0 + j], (f[j] - mean) * rstd, beta[c0 + j]) + r[j];
+      if (relu) u = fmaxf(u, 0.f);
+      f[j] = u;
+    }
+    gn_st<VEC>(y + o, f);
+  }
+}
+
+template <int VEC, bool CACHE>
+__global__ void __launch_bounds__(GN_THREADS)
+gn_bwd_kernel(const __nv_bfloat16* __restrict__ z, const __nv_bfloat16* __restrict__ y,
+              const __nv_bfloat16* __restrict__ dy_a, const __nv_bfloat16* __restrict__ dy_b, __nv_bfloat16* __restrict__ dz,
+              __nv_bfloat16* __restrict__ dres, const float* __restrict__ gamma, const float* __restrict__ mean_in,
+              const float* __restrict__ rstd_in, float* __restrict__ dgamma, float* __restrict__ dbeta,
+              float* __restrict__ work, long long HW, int C, int G, int relu) {
+  griddep_launch_dependents();
+  extern __shared__ __align__(16) unsigned char gn_smem[];
+  const int g = static_cast<int>(blockIdx.x % G);
+  const long long n = blockIdx.x / G;
+  const int N = static_cast<int>(gridDim.x / G);
+  const int Cg = C / G, CgV = Cg / VEC;
+  const long long M = HW * Cg, MV = M / VEC;
+  float* gc = reinterpret_cast<float*>(gn_smem);                               // [M] dy' when CACHE
+  __nv_bfloat16* zc = reinterpret_cast<__nv_bfloat16*>(gn_smem + M * 4);     // [M] z when CACHE
+  __shared__ float red[GN_THREADS / 32];
+  __shared__ float part[2][GN_THREADS];
+  __shared__ bool last;
+  const long long base = n * HW * C + static_cast<long long>(g) * Cg;
+  unsigned* counters = reinterpret_cast<unsigned*>(work);
+  float* partials = work + G;                                                   // [N][C][2]: sum dy', sum dy' xhat
+  griddep_wait();
+  const float mean = mean_in[blockIdx.x], rstd = rstd_in[blockIdx.x];
+  // pass 1: dy' -> dres, and the on-chip copy
+  if (CACHE || dres != nullptr) {
+    for (long long v = threadIdx.x; v < MV; v += GN_THREADS) {
+      const long long o = base + (v / CgV) * C + (v % CgV) * VEC;
+      float xf[VEC], gf[VEC];
+      gn_grad<VEC>(o, z, y, dy_a, dy_b, relu, xf, gf);
+      if (dres != nullptr) gn_st<VEC>(dres + o, gf);
+      if constexpr (CACHE) {
+        gn_st<VEC>(zc + v * VEC, xf);
+#pragma unroll
+        for (int j = 0; j < VEC; ++j) gc[v * VEC + j] = gf[j];
+      }
+    }
+    if constexpr (CACHE) __syncthreads();
+  }
+  // per-channel sums over the HW positions of this sample: `span` channels at a time, each summed by `ns` threads over
+  // interleaved positions, then the ns partials in slice order.  Their gamma-weighted totals are mean(gamma dy') etc.
+  float ga = 0.f, gb = 0.f;
+  for (int cb = 0; cb < Cg; cb += GN_THREADS) {
+    const int span = min(Cg - cb, GN_THREADS), ns = GN_THREADS / span;
+    const int cl = cb + static_cast<int>(threadIdx.x) % span, sl = static_cast<int>(threadIdx.x) / span;
+    float sg = 0.f, sgx = 0.f;
+    if (sl < ns) {
+      for (long long p = sl; p < HW; p += ns) {
+        float xf[1], gf[1];
+        if constexpr (CACHE) {
+          xf[0] = __bfloat162float(zc[p * Cg + cl]);
+          gf[0] = gc[p * Cg + cl];
+        } else {
+          gn_grad<1>(base + p * C + cl, z, y, dy_a, dy_b, relu, xf, gf);
+        }
+        sg += gf[0];
+        sgx = fmaf(gf[0], (xf[0] - mean) * rstd, sgx);
+      }
+    }
+    __syncthreads();               // the previous block of channels may still be reading part
+    part[0][threadIdx.x] = sg;
+    part[1][threadIdx.x] = sgx;
+    __syncthreads();
+    if (static_cast<int>(threadIdx.x) < span) {
+      float a = 0.f, b = 0.f;
+      for (int k = 0; k < ns; ++k) {
+        a += part[0][k * span + threadIdx.x];
+        b += part[1][k * span + threadIdx.x];
+      }
+      const int c = g * Cg + cb + static_cast<int>(threadIdx.x);
+      partials[(n * C + c) * 2] = a;
+      partials[(n * C + c) * 2 + 1] = b;
+      ga = fmaf(gamma[c], a, ga);
+      gb = fmaf(gamma[c], b, gb);
+    }
+  }
+  const float fm = static_cast<float>(M);
+  const float ka = __fdiv_rn(gn_cta_sum(ga, red), fm), kb = __fdiv_rn(gn_cta_sum(gb, red), fm);
+  // pass 2: dz
+  for (long long v = threadIdx.x; v < MV; v += GN_THREADS) {
+    const long long o = base + (v / CgV) * C + (v % CgV) * VEC;
+    const int c0 = g * Cg + static_cast<int>(v % CgV) * VEC;
+    float xf[VEC], gf[VEC];
+    if constexpr (CACHE) {
+      gn_ld<VEC>(zc + v * VEC, xf);
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) gf[j] = gc[v * VEC + j];
+    } else {
+      gn_grad<VEC>(o, z, y, dy_a, dy_b, relu, xf, gf);
+    }
+#pragma unroll
+    for (int j = 0; j < VEC; ++j) xf[j] = rstd * (gamma[c0 + j] * gf[j] - ka - (xf[j] - mean) * rstd * kb);
+    gn_st<VEC>(dz + o, xf);
+  }
+  // dgamma / dbeta: the last CTA of group g to arrive adds the N partials of each of its channels in sample order
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) last = atomicAdd(counters + g, 1u) == static_cast<unsigned>(N - 1);
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  for (int c = g * Cg + static_cast<int>(threadIdx.x); c < (g + 1) * Cg; c += GN_THREADS) {
+    float a = 0.f, b = 0.f;
+    for (int k = 0; k < N; ++k) {
+      a += __ldcg(partials + (static_cast<long long>(k) * C + c) * 2);
+      b += __ldcg(partials + (static_cast<long long>(k) * C + c) * 2 + 1);
+    }
+    if (dbeta != nullptr) dbeta[c] += a;
+    if (dgamma != nullptr) dgamma[c] += b;
+  }
+  if (threadIdx.x == 0) counters[g] = 0u;
+}
+
 static inline int stream_grid(long long nvec) {
   long long g = (nvec + 255) / 256;
   if (g < 1) g = 1;
@@ -1486,6 +1734,87 @@ extern "C" int b200_bn_maxpool_bwd(const void* z, const void* p, const void* arg
              reinterpret_cast<const uint4*>(z), reinterpret_cast<const uint4*>(p), reinterpret_cast<const uint2*>(argmax),
              reinterpret_cast<const uint4*>(dy_a), reinterpret_cast<const uint4*>(dy_b), reinterpret_cast<uint4*>(dz), gamma,
              save_mean, save_rstd, sums, dgamma, dbeta, N, H, W, C, k, stride, pad, Ho, Wo);
+  RET_LAST();
+}
+
+// ---- GroupNorm.  Returns -2 for an unsupported shape (G not dividing C).  16-byte vectors when Cg % 8 == 0 and every
+// tensor is 16-byte aligned; the (n, g) block stays on chip when it holds at most GN_CACHE_ELEMS elements.
+// The cached backward keeps up to GN_CACHE_ELEMS * 6 bytes of dynamic shared memory, above the 48 KB default: opt each
+// cached instantiation in to that maximum once per device (the same value from every thread, so concurrent first
+// launches set the same attribute).  Returns the attribute's error code.
+constexpr int GN_MAX_DEVICES = 64;
+template <int V>
+static int gn_bwd_cache_optin() {
+  static std::atomic<int> done[GN_MAX_DEVICES] = {};
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return static_cast<int>(e);
+  if (dev < GN_MAX_DEVICES && done[dev].load(std::memory_order_acquire)) return 0;
+  e = cudaFuncSetAttribute(gn_bwd_kernel<V, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           static_cast<int>(GN_CACHE_ELEMS * 6));
+  if (e != cudaSuccess) return static_cast<int>(e);
+  if (dev < GN_MAX_DEVICES) done[dev].store(1, std::memory_order_release);
+  return 0;
+}
+static inline bool gn_vec_ok(int C, int G, std::initializer_list<const void*> ptrs) {
+  if ((C / G) % 8) return false;
+  uintptr_t al = 0;
+  for (const void* p : ptrs) al |= reinterpret_cast<uintptr_t>(p);
+  return (al & 15) == 0;
+}
+
+extern "C" int b200_gn_fwd(const void* z, const void* residual, void* y, const float* gamma, const float* beta,
+                           float* mean, float* rstd, float* work, long long N, long long HW, int C, int G, float eps,
+                           int relu, cudaStream_t stream) {
+  if (G <= 0 || C % G) return -2;
+  if (N <= 0 || HW <= 0) return 0;
+  const unsigned grid = static_cast<unsigned>(N * G);
+  const long long M = HW * (C / G);
+  const bool cache = M <= GN_CACHE_ELEMS;
+  const size_t smem = cache ? static_cast<size_t>(M) * 2 : 0;
+  unsigned* counters = reinterpret_cast<unsigned*>(work);
+  const auto* zp = reinterpret_cast<const __nv_bfloat16*>(z);
+  const auto* rp = reinterpret_cast<const __nv_bfloat16*>(residual);
+  auto* yp = reinterpret_cast<__nv_bfloat16*>(y);
+#define GN_FWD(V, CA) launch_pdl(gn_fwd_kernel<V, CA>, grid, GN_THREADS, smem, stream, zp, rp, yp, gamma, beta, mean, rstd, \
+                                 counters, HW, C, G, eps, relu)
+  if (gn_vec_ok(C, G, {z, residual, y})) {
+    if (cache) GN_FWD(8, true); else GN_FWD(8, false);
+  } else {
+    if (cache) GN_FWD(1, true); else GN_FWD(1, false);
+  }
+#undef GN_FWD
+  RET_LAST();
+}
+
+extern "C" int b200_gn_bwd(const void* z, const void* y, const void* dy_a, const void* dy_b, void* dz, void* dres,
+                           const float* gamma, const float* mean, const float* rstd, float* dgamma, float* dbeta,
+                           float* work, long long N, long long HW, int C, int G, int relu, cudaStream_t stream) {
+  if (G <= 0 || C % G || work == nullptr) return -2;
+  if (N <= 0 || HW <= 0) return 0;
+  const unsigned grid = static_cast<unsigned>(N * G);
+  const long long M = HW * (C / G);
+  const bool cache = M <= GN_CACHE_ELEMS;
+  const size_t smem = cache ? static_cast<size_t>(M) * 6 : 0;
+  const auto* zp = reinterpret_cast<const __nv_bfloat16*>(z);
+  const auto* yp = reinterpret_cast<const __nv_bfloat16*>(y);
+  const auto* ap = reinterpret_cast<const __nv_bfloat16*>(dy_a);
+  const auto* bp = reinterpret_cast<const __nv_bfloat16*>(dy_b);
+  auto* dzp = reinterpret_cast<__nv_bfloat16*>(dz);
+  auto* drp = reinterpret_cast<__nv_bfloat16*>(dres);
+  const bool vec = gn_vec_ok(C, G, {z, relu ? y : z, dy_a, dy_b, dz, dres});
+  if (cache) {
+    const int rc = vec ? gn_bwd_cache_optin<8>() : gn_bwd_cache_optin<1>();
+    if (rc != 0) return rc;
+  }
+#define GN_BWD(V, CA) launch_pdl(gn_bwd_kernel<V, CA>, grid, GN_THREADS, smem, stream, zp, yp, ap, bp, dzp, drp, gamma, \
+                                 mean, rstd, dgamma, dbeta, work, HW, C, G, relu)
+  if (vec) {
+    if (cache) GN_BWD(8, true); else GN_BWD(8, false);
+  } else {
+    if (cache) GN_BWD(1, true); else GN_BWD(1, false);
+  }
+#undef GN_BWD
   RET_LAST();
 }
 

@@ -36,6 +36,12 @@ def build_model(kind: str):
     if kind == "resnet50":
         from .models import resnet50
         return resnet50(num_classes=1000)
+    if kind == "resnet18_gn":     # GroupNorm(2, C) in place of BatchNorm (Hsieh et al. 2020; Reddi et al. 2021)
+        from .models import resnet18
+        return resnet18(num_classes=10, norm="group", groups=2)
+    if kind == "resnet50_gn":
+        from .models import resnet50
+        return resnet50(num_classes=1000, norm="group", groups=2)
     if kind == "bert_base":
         from .models import bert_base
         return bert_base()

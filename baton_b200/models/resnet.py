@@ -52,6 +52,27 @@ def _conv_bn_bwd(ctxs, dy_a, dy_b=None, needs_dx=True):
     return dx, dres
 
 
+# The same pair for GroupNorm: the conv GEMM takes no statistics (they are per sample, computed by gn_fwd itself).
+def _conv_gn_fwd(conv: "bnn.Conv2d", gn: "bnn.GroupNorm", x, residual=None, after_conv=None):
+    cc, cg = bnn.Ctx(), bnn.Ctx()
+    z = bnn._ConvFn.forward(cc, x, conv.weight, conv._w_bf16(), conv.plan(x), None, None, conv.flags_cfg)
+    if after_conv is not None:
+        after_conv()
+    y = bnn._GNFn.forward(cg, z, residual, gn.weight, gn.bias, gn.num_groups, gn.eps, gn.relu, True, None)
+    return y, (cc, cg)
+
+
+def _conv_gn_bwd(ctxs, dy_a, dy_b=None, needs_dx=True):
+    cc, cg = ctxs
+    cc.needs_dx = needs_dx
+    dz, dres = bnn._GNFn.backward(cg, dy_a, dy_b)[:2]
+    dx = bnn._ConvFn.backward(cc, dz)[0]
+    return dx, dres
+
+
+_CONV_NORM = {"batch": (_conv_bn_fwd, _conv_bn_bwd), "group": (_conv_gn_fwd, _conv_gn_bwd)}
+
+
 # The stem (conv1 -> bn1 -> relu -> maxpool): BatchNorm + ReLU + max-pool are ONE kernel forward and two backward (the
 # normalised 16x16 activation is never written: the pooled output carries the ReLU mask, BatchNorm's backward sums run
 # over the pooled gradient -- csrc/norm.cu, "ResNet stem").  Where _stem_fwd declines, the separate kernels run.
@@ -104,15 +125,24 @@ def _conv_bn_eval(conv, bn, x, table, residual=None):
     return y.view(plan.n, plan.ho, plan.wo, plan.cout)
 
 
+def _batch_norm(c: int, relu: bool) -> nn.Module:
+    return bnn.BatchNorm2d(c, relu=relu)
+
+
+def _group_norm(groups: int):
+    return lambda c, relu: bnn.GroupNorm(groups, c, relu=relu)
+
+
 class BasicBlock(nn.Module):
     expansion = 1
 
-    def __init__(self, inplanes: int, planes: int, stride: int = 1, downsample: Optional[nn.Module] = None):
+    def __init__(self, inplanes: int, planes: int, stride: int = 1, downsample: Optional[nn.Module] = None,
+                 norm=_batch_norm):
         super().__init__()
         self.conv1 = bnn.Conv2d(inplanes, planes, 3, stride, 1)
-        self.bn1 = bnn.BatchNorm2d(planes, relu=True)
+        self.bn1 = norm(planes, True)
         self.conv2 = bnn.Conv2d(planes, planes, 3, 1, 1)
-        self.bn2 = bnn.BatchNorm2d(planes, relu=True)      # relu(bn2(.) + identity), fused
+        self.bn2 = norm(planes, True)                       # relu(bn2(.) + identity), fused
         self.downsample = downsample
 
     def forward(self, x):
@@ -126,14 +156,15 @@ class BasicBlock(nn.Module):
 class Bottleneck(nn.Module):
     expansion = 4
 
-    def __init__(self, inplanes: int, planes: int, stride: int = 1, downsample: Optional[nn.Module] = None):
+    def __init__(self, inplanes: int, planes: int, stride: int = 1, downsample: Optional[nn.Module] = None,
+                 norm=_batch_norm):
         super().__init__()
         self.conv1 = bnn.Conv2d(inplanes, planes, 1, 1, 0)
-        self.bn1 = bnn.BatchNorm2d(planes, relu=True)
+        self.bn1 = norm(planes, True)
         self.conv2 = bnn.Conv2d(planes, planes, 3, stride, 1)
-        self.bn2 = bnn.BatchNorm2d(planes, relu=True)
+        self.bn2 = norm(planes, True)
         self.conv3 = bnn.Conv2d(planes, planes * 4, 1, 1, 0)
-        self.bn3 = bnn.BatchNorm2d(planes * 4, relu=True)
+        self.bn3 = norm(planes * 4, True)
         self.downsample = downsample
 
     def forward(self, x):
@@ -146,10 +177,10 @@ class Bottleneck(nn.Module):
 
 
 class _Downsample(nn.Sequential):
-    """``0`` = 1x1 strided conv, ``1`` = BatchNorm (same indices as the stock model)."""
+    """``0`` = 1x1 strided conv, ``1`` = BatchNorm or GroupNorm (same indices as the stock model)."""
 
-    def __init__(self, inplanes: int, outplanes: int, stride: int):
-        super().__init__(bnn.Conv2d(inplanes, outplanes, 1, stride, 0), bnn.BatchNorm2d(outplanes, relu=False))
+    def __init__(self, inplanes: int, outplanes: int, stride: int, norm=_batch_norm):
+        super().__init__(bnn.Conv2d(inplanes, outplanes, 1, stride, 0), norm(outplanes, False))
 
 
 class ResNet(FederatedModule):
@@ -159,18 +190,24 @@ class ResNet(FederatedModule):
     head = "fc"
 
     def __init__(self, block: Type[nn.Module], layers: Sequence[int], num_classes: int = 1000,
-                 in_channels: int = 3, name: Optional[str] = None):
+                 in_channels: int = 3, name: Optional[str] = None, norm: str = "batch", groups: int = 2):
+        """``norm="group"``: every BatchNorm becomes a ``GroupNorm(groups, C)`` under the same name (torchvision's model
+        built with ``norm_layer=lambda c: nn.GroupNorm(groups, c)``), so the model has no buffers."""
         super().__init__()
+        if norm not in _CONV_NORM:
+            raise ValueError("ResNet: norm must be 'batch' or 'group', got {!r}".format(norm))
         if name:
             self.name = name
+        self.norm = norm
+        norm_layer = _batch_norm if norm == "batch" else _group_norm(groups)
         self.inplanes = 64
         self.conv1 = bnn.Conv2d(in_channels, 64, 7, 2, 3)
-        self.bn1 = bnn.BatchNorm2d(64, relu=True)
+        self.bn1 = norm_layer(64, True)
         self.maxpool = bnn.MaxPool2d(3, 2, 1)
-        self.layer1 = self._make_layer(block, 64, layers[0], 1)
-        self.layer2 = self._make_layer(block, 128, layers[1], 2)
-        self.layer3 = self._make_layer(block, 256, layers[2], 2)
-        self.layer4 = self._make_layer(block, 512, layers[3], 2)
+        self.layer1 = self._make_layer(block, 64, layers[0], 1, norm_layer)
+        self.layer2 = self._make_layer(block, 128, layers[1], 2, norm_layer)
+        self.layer3 = self._make_layer(block, 256, layers[2], 2, norm_layer)
+        self.layer4 = self._make_layer(block, 512, layers[3], 2, norm_layer)
         self.avgpool = bnn.GlobalAvgPool()
         self.fc = bnn.Linear(512 * block.expansion, num_classes, out_fp32=True)
         self.stats_workspace = None
@@ -181,14 +218,14 @@ class ResNet(FederatedModule):
             elif isinstance(m, Bottleneck):
                 nn.init.zeros_(m.bn3.weight)
 
-    def _make_layer(self, block, planes: int, blocks: int, stride: int) -> nn.Sequential:
+    def _make_layer(self, block, planes: int, blocks: int, stride: int, norm_layer) -> nn.Sequential:
         downsample = None
         if stride != 1 or self.inplanes != planes * block.expansion:
-            downsample = _Downsample(self.inplanes, planes * block.expansion, stride)
-        layers: List[nn.Module] = [block(self.inplanes, planes, stride, downsample)]
+            downsample = _Downsample(self.inplanes, planes * block.expansion, stride, norm_layer)
+        layers: List[nn.Module] = [block(self.inplanes, planes, stride, downsample, norm_layer)]
         self.inplanes = planes * block.expansion
         for _ in range(1, blocks):
-            layers.append(block(self.inplanes, planes))
+            layers.append(block(self.inplanes, planes, norm=norm_layer))
         return nn.Sequential(*layers)
 
     def set_precision(self, dtype: str = "bf16") -> "ResNet":
@@ -215,7 +252,7 @@ class ResNet(FederatedModule):
         identity = x
         if blk.downsample is not None:
             with bnn.BRANCH.fork(x):                      # parallel graph branch: 1x1 conv + BN of the shortcut
-                identity, ds_ctx = _conv_bn_fwd(blk.downsample[0], blk.downsample[1], x)
+                identity, ds_ctx = _CONV_NORM[self.norm][0](blk.downsample[0], blk.downsample[1], x)
         out = x
         ctxs = []
         n = len(blk.units)
@@ -223,7 +260,7 @@ class ResNet(FederatedModule):
             last = i == n - 1
             if last:
                 bnn.BRANCH.join()                         # the shortcut must have landed before the residual add
-            out, c = _conv_bn_fwd(getattr(blk, cn), getattr(blk, bnn_), out, identity if last else None)
+            out, c = _CONV_NORM[self.norm][0](getattr(blk, cn), getattr(blk, bnn_), out, identity if last else None)
             ctxs.append(c)
         tape.append((ctxs, ds_ctx))
         return out
@@ -231,13 +268,14 @@ class ResNet(FederatedModule):
     def _block_bwd(self, entry, pieces):
         """``pieces``: 1-2 tensors whose sum is the gradient of the block output -> pieces of the block-input gradient"""
         ctxs, ds_ctx = entry
-        d, dres = _conv_bn_bwd(ctxs[-1], pieces[0], pieces[1] if len(pieces) > 1 else None)
+        bwd = _CONV_NORM[self.norm][1]
+        d, dres = bwd(ctxs[-1], pieces[0], pieces[1] if len(pieces) > 1 else None)
         dx_ds = None
         if ds_ctx is not None:
             with bnn.BRANCH.fork(dres):                   # shortcut backward in parallel with the main branch
-                dx_ds, _ = _conv_bn_bwd(ds_ctx, dres)
+                dx_ds, _ = bwd(ds_ctx, dres)
         for c in reversed(ctxs[:-1]):
-            d, _ = _conv_bn_bwd(c, d)
+            d, _ = bwd(c, d)
         if ds_ctx is not None:
             bnn.BRANCH.join()
             return [d, dx_ds]
@@ -255,11 +293,12 @@ class ResNet(FederatedModule):
         if self.stats_workspace is not None:
             self.stats_workspace.zero_()
         stem = cp = None
-        fused_stem = _stem_fwd(self.conv1, self.bn1, self.maxpool, x, after_first_gemm)
+        fwd, bwd = _CONV_NORM[self.norm]
+        fused_stem = _stem_fwd(self.conv1, self.bn1, self.maxpool, x, after_first_gemm) if self.norm == "batch" else None
         if fused_stem is not None:
             h = fused_stem[0]
         else:
-            h, stem = _conv_bn_fwd(self.conv1, self.bn1, x, after_conv=after_first_gemm)
+            h, stem = fwd(self.conv1, self.bn1, x, after_conv=after_first_gemm)
             cp = bnn.Ctx()
             h = bnn._MaxPoolFn.forward(cp, h, self.maxpool.k, self.maxpool.stride, self.maxpool.pad)
         tape = []
@@ -296,7 +335,7 @@ class ResNet(FederatedModule):
             _stem_bwd(fused_stem, self.bn1, self.maxpool, pieces[0], pieces[1] if len(pieces) > 1 else None)
         else:
             d = bnn._MaxPoolFn.backward(cp, pieces[0], pieces[1] if len(pieces) > 1 else None)[0]
-            _conv_bn_bwd(stem, d, needs_dx=False)
+            bwd(stem, d, needs_dx=False)
         bnn.WGRAD.join()
         return stats
 
@@ -358,7 +397,7 @@ class ResNet(FederatedModule):
         for m in bns:
             m.workspace = ws[off: off + 4 * m.num_features]
             off += 4 * m.num_features
-        self.stats_workspace = ws
+        self.stats_workspace = ws if bns else None      # a GroupNorm model has no batch statistics
         # convolution -> BatchNorm pairs: the conv GEMM's epilogue accumulates the batch statistics straight
         # into the BatchNorm's workspace, so the separate statistics pass over the activation disappears
         for parent in self.modules():
@@ -366,16 +405,17 @@ class ResNet(FederatedModule):
                 conv, bn = getattr(parent, conv_name, None), getattr(parent, bn_name, None)
                 if isinstance(conv, bnn.Conv2d) and isinstance(bn, bnn.BatchNorm2d):
                     conv.bn_ws = bn.workspace
-            if isinstance(parent, _Downsample):
+            if isinstance(parent, _Downsample) and isinstance(parent[1], bnn.BatchNorm2d):
                 parent[0].bn_ws = parent[1].workspace
         return ws
 
 
 def resnet18(num_classes: int = 10, **kw) -> ResNet:
-    kw.setdefault("name", "resnet18")
+    """``norm="group", groups=G``: GroupNorm(G, C) in place of every BatchNorm."""
+    kw.setdefault("name", "resnet18" if kw.get("norm", "batch") == "batch" else "resnet18_gn")
     return ResNet(BasicBlock, [2, 2, 2, 2], num_classes=num_classes, **kw)
 
 
 def resnet50(num_classes: int = 1000, **kw) -> ResNet:
-    kw.setdefault("name", "resnet50")
+    kw.setdefault("name", "resnet50" if kw.get("norm", "batch") == "batch" else "resnet50_gn")
     return ResNet(Bottleneck, [3, 4, 6, 3], num_classes=num_classes, **kw)

@@ -812,6 +812,44 @@ def bn_maxpool_bwd(z: torch.Tensor, p: torch.Tensor, arg: torch.Tensor, dy_a: to
     return dz
 
 
+def gn_work(n: int, c: int, groups: int, device) -> torch.Tensor:
+    """Scratch of :func:`gn_bwd`: fp32 ``[G + 2 N C]``, per-group arrival counters then per-sample channel partials.  The
+    counters must be zero when the backward starts: :func:`gn_fwd` zeroes them when it is given the buffer, and the
+    backward leaves them zero, so one buffer serves any number of launches on one stream."""
+    return torch.empty(groups + 2 * n * c, dtype=torch.float32, device=device)
+
+
+def gn_fwd(z: torch.Tensor, residual: Optional[torch.Tensor], gamma: torch.Tensor, beta: torch.Tensor, groups: int,
+           eps: float = 1e-5, relu: bool = False, work: Optional[torch.Tensor] = None):
+    """GroupNorm of NHWC bf16 ``z`` with ``groups`` contiguous channel blocks, plus the residual and the ReLU:
+    ``y = relu(gamma_c * (z - mean_ng) * rstd_ng + beta_c + residual)``, biased variance, statistics in fp32.
+    -> ``(y, mean, rstd)`` with fp32 ``[N, G]`` statistics.  ``work``: the backward's :func:`gn_work` buffer, if any."""
+    n = z.shape[0]
+    y = torch.empty_like(z)
+    mean = torch.empty((n, groups), dtype=torch.float32, device=z.device)
+    rstd = torch.empty((n, groups), dtype=torch.float32, device=z.device)
+    load().gn_fwd(z, None if residual is None else residual.contiguous(), y, gamma, beta, mean, rstd, int(groups),
+                  float(eps), bool(relu), work)
+    return y, mean, rstd
+
+
+def gn_bwd(z: torch.Tensor, y: torch.Tensor, dy_a: torch.Tensor, dy_b: Optional[torch.Tensor], gamma: torch.Tensor,
+           mean: torch.Tensor, rstd: torch.Tensor, dgamma: Optional[torch.Tensor], dbeta: Optional[torch.Tensor],
+           groups: int, relu: bool = False, want_dres: bool = False, work: Optional[torch.Tensor] = None):
+    """Backward of :func:`gn_fwd` from the gradient ``dy_a (+ dy_b)`` of ``y``: -> ``(dz, dres)`` where ``dres`` (the
+    residual's gradient, ``dy'`` after the ReLU mask) is ``None`` unless ``want_dres``.  ``dgamma`` / ``dbeta`` (fp32
+    ``[C]``) are ACCUMULATED, in a fixed summation order.  ``work``: a :func:`gn_work` buffer with zero counters (a
+    fresh zeroed one when ``None``)."""
+    n, c = z.shape[0], z.shape[3]
+    if work is None:
+        work = torch.zeros(groups + 2 * n * c, dtype=torch.float32, device=z.device)
+    dz = torch.empty_like(z)
+    dres = torch.empty_like(z) if want_dres else None
+    load().gn_bwd(z, y, dy_a.contiguous(), None if dy_b is None else dy_b.contiguous(), dz, dres, gamma, mean, rstd,
+                  dgamma, dbeta, int(groups), bool(relu), work)
+    return dz, dres
+
+
 def avgpool(x: torch.Tensor) -> torch.Tensor:
     n, h, w, c = x.shape
     y = torch.empty((n, c), dtype=BF16, device=x.device)

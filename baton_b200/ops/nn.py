@@ -575,6 +575,61 @@ class BatchNorm2d(nn.Module):
                            self.momentum, self.relu, self.training, ws, _anchor(x, self.weight), ready)
 
 
+# ================================================================================ GroupNorm (+residual +ReLU)
+class _GNFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, residual, gamma, beta, groups, eps, relu, need_bwd, anchor):
+        """``need_bwd``: allocate the backward's scratch (``F.gn_work``), whose counters the forward kernel zeroes."""
+        gamma, beta = _unwrap(gamma), _unwrap(beta)
+        work = F.gn_work(x.shape[0], x.shape[3], groups, x.device) if need_bwd else None
+        y, mean, rstd = F.gn_fwd(x, residual, gamma, beta, groups, eps, relu, work)
+        ctx.save_for_backward(x, y, mean, rstd, work)
+        ctx.gamma, ctx.beta = gamma, beta
+        ctx.groups, ctx.relu, ctx.has_res = groups, relu, residual is not None
+        return y
+
+    @staticmethod
+    def backward(ctx, dy, dy_b=None):
+        """``dy_b``: optional second piece of the incoming gradient, summed inside the kernel (hand-scheduled step only)."""
+        x, y, mean, rstd, work = ctx.saved_tensors
+        gamma, beta = ctx.gamma, ctx.beta
+        tg, tb = _grad_target(gamma), _grad_target(beta)
+        gg = gb = None
+        if tg is None:
+            gg = tg = torch.zeros(x.shape[3], dtype=torch.float32, device=x.device)
+        if tb is None:
+            gb = tb = torch.zeros(x.shape[3], dtype=torch.float32, device=x.device)
+        dx, dres = F.gn_bwd(x, y, dy, dy_b, gamma, mean, rstd, tg, tb, ctx.groups, ctx.relu, want_dres=ctx.has_res,
+                            work=work)
+        return dx, dres, gg, gb, None, None, None, None, None
+
+
+class GroupNorm(nn.Module):
+    """GroupNorm over ``num_groups`` contiguous channel blocks of an NHWC tensor (``torch.nn.GroupNorm``'s grouping and
+    ``weight`` / ``bias``, no buffers), with the residual add and ReLU of a ResNet block fused into the same pass:
+    ``relu(gn(x) + residual)``.  Statistics are per sample, so training and evaluation compute the same thing."""
+
+    def __init__(self, num_groups: int, num_channels: int, eps: float = 1e-5, relu: bool = False):
+        super().__init__()
+        if (isinstance(num_groups, bool) or not isinstance(num_groups, int) or num_groups <= 0
+                or num_channels % num_groups):
+            raise ValueError("GroupNorm: num_groups must be a positive int dividing num_channels, got {!r} for {} "
+                             "channels".format(num_groups, num_channels))
+        self.num_groups, self.num_channels, self.eps, self.relu = num_groups, num_channels, eps, relu
+        self.weight = nn.Parameter(torch.ones(num_channels))
+        self.bias = nn.Parameter(torch.zeros(num_channels))
+
+    def forward(self, x, residual=None):
+        if not x.is_cuda:
+            y = TF.group_norm(x.permute(0, 3, 1, 2), self.num_groups, self.weight, self.bias,
+                              self.eps).permute(0, 2, 3, 1)
+            if residual is not None:
+                y = y + residual
+            return TF.relu(y) if self.relu else y
+        return _GNFn.apply(x.contiguous(), residual, _wrap(self.weight, x), _wrap(self.bias, x), self.num_groups,
+                           self.eps, self.relu, torch.is_grad_enabled(), _anchor(x, self.weight))
+
+
 # ================================================================================ pooling / misc
 class _MaxPoolFn(torch.autograd.Function):
     @staticmethod

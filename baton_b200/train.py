@@ -651,12 +651,14 @@ class GraphedLocalSGD:
         if explicit and self._fold is None:
             fold = bn_fold_table(self.model, self.arena)
             if fold is None:
-                explicit = False
+                self._fold = False        # no BatchNorm to fold (a GroupNorm ResNet): the generic eval forward, every call
             else:
                 table, size = fold
                 out = torch.zeros(size, dtype=torch.float32, device=self.device)
                 self._fold = (table, out)
                 self.model.eval_bn_table = out
+        if self._fold is False:
+            explicit = False
         was_training = self.model.training
         nn.Module.train(self.model, False)
         try:
