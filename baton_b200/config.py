@@ -38,6 +38,7 @@ class FederationConfig:
     mix_alpha: float = 1.0             # lambda ~ Beta(mix_alpha, mix_alpha), one per batch
     label_smoothing: float = 0.0       # soft-target smoothing eps in [0, 1) of the training cross-entropy
     max_grad_norm: float = 0.0         # clip_grad_norm_ of every local step's gradient to this 2-norm (0: off)
+    dropout: float = 0.0               # BERT: hidden and attention-probability dropout (the classifier follows hidden)
     dp_clip: float = 0.0               # DP-FedAvg: L2 clip norm of a client's update (0: DP off)
     dp_noise_multiplier: float = 0.0   # DP-FedAvg: noise std on the sum of clipped updates, in units of dp_clip
     dp_delta: float = 1e-5             # DP-FedAvg: delta of the (epsilon, delta) the manager reports
@@ -71,6 +72,10 @@ class FederationConfig:
         check_augment(self.augment, self.augment_padding)
         from .data.mix import check_mix
         check_mix(self.mix, self.mix_alpha, self.label_smoothing)
+        from .data.dropout import check_dropout
+        check_dropout(self.dropout, "dropout")
+        if self.dropout > 0.0 and self.model != "bert_base":
+            raise ValueError("dropout applies to the BERT models only, not {!r}".format(self.model))
         from .parallel.dp import check_dp
         check_dp(self.dp_clip, self.dp_noise_multiplier)
         if not (0.0 < float(self.dp_delta) < 1.0):

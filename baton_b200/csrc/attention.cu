@@ -13,6 +13,7 @@
 // writes P, reads P).  It runs whenever S = 128, d_head = 64 and there is no mask; tests/test_gpu_bert.py checks it
 // against the multi-kernel path and an fp32 reference.
 #define B200_TU_TAG 4
+#include "dropout.cuh"
 #include "launch.h"
 #include "pdl.cuh"
 #include "ptx.cuh"
@@ -41,9 +42,12 @@ struct AttnParams {
   float scale_log2e;       // softmax scale * log2(e)
 };
 
+// DROP: dropout on the probabilities.  Pass B zeroes the dropped entries of P~ before MMA 2 and the epilogue scales by
+// inv * s; the saved probs stay the undropped P.  Element i of the mask is the index into probs.
+template <bool DROP>
 __global__ void __launch_bounds__(AT_THREADS, 1)
 attention_fwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                          const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
+                          const __grid_constant__ CUtensorMap tmV, const AttnParams p, const DropArgs da) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
@@ -102,6 +106,8 @@ attention_fwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
     const float* srow = sS + r * AT_SP;
     float mb = 0.f, inv = 0.f;
     if (ew < 4) {
+      DropCtr dc;
+      if constexpr (DROP) dc = drop_ctr(da);
       // pass A: row maximum
       float m = -INFINITY;
 #pragma unroll 1
@@ -124,6 +130,15 @@ attention_fwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
         for (int j = 0; j < 32; ++j) {
           e[j] = exp2f(fmaf(__uint_as_float(x[j]), p.scale_log2e, -mb));
           sum += e[j];
+        }
+        if constexpr (DROP) {
+          const unsigned long long i0 = (static_cast<unsigned long long>(bh) * AT_S + r) * AT_S + c;
+#pragma unroll
+          for (int j = 0; j < 32; j += 8) {
+            const uint32_t bits = drop_keep8(dc, i0 + j);
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) e[j + jj] = kept(bits, jj, e[j + jj], 1.f);
+          }
         }
         uint8_t* tile = prow + (c >> 6) * 16384;                     // 64-key k-tile
 #pragma unroll
@@ -173,7 +188,8 @@ attention_fwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
               make_uint4(pack_bf16x2(e[j], e[j + 1]), pack_bf16x2(e[j + 2], e[j + 3]), pack_bf16x2(e[j + 4], e[j + 5]),
                          pack_bf16x2(e[j + 6], e[j + 7]));
       }
-      // epilogue: O = O~ / rowsum
+      // epilogue: O = O~ / rowsum (times s with dropout)
+      if constexpr (DROP) inv *= da.scale;
       __nv_bfloat16* orow = p.out + (static_cast<size_t>(b) * AT_S + r) * p.D + h * AT_D;
 #pragma unroll 1
       for (int c = 0; c < AT_D; c += 32) {
@@ -205,14 +221,19 @@ attention_fwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
 // HBM); here P is read once and nothing S x S is written.  It runs wherever the fused forward did.
 struct AttnBwdParams {
   __nv_bfloat16* dqkv;     // [B*S, 3*D]
+  const __nv_bfloat16* probs;   // [B*H*S, S]: re-read by the row pass of the dropout form
   int H, D;
   float scale;
 };
 
+// DROP: with M the mask and s the scale, dV = (P o M s)^T dO, dP = M s o (dO V^T), delta = rowsum(P o dP),
+// dS = P o (dP - delta).  Before the first MMAs each row owner turns its row of the P tile into bf16(P o M s) in place
+// and keeps its 128 keep bits in registers; the row pass then re-reads the undropped P row from global memory (L2).
+template <bool DROP>
 __global__ void __launch_bounds__(AT_THREADS, 1)
 attention_bwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                           const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
-                          const __grid_constant__ CUtensorMap tmP, const AttnBwdParams p) {
+                          const __grid_constant__ CUtensorMap tmP, const AttnBwdParams p, const DropArgs da) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
@@ -251,6 +272,37 @@ attention_bwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
     const int ew = warp - 4, g = ew >> 2;
     const uint32_t q = smem_u32(sQ), k = smem_u32(sK), v = smem_u32(sV), d_o = smem_u32(sdO), pp = smem_u32(sP);
     mbar_wait(bar_load, 0);
+    uint32_t keep[AT_S / 32];     // DROP: keep bits of this thread's row (warpgroup 1)
+    if constexpr (DROP) {
+      if (ew < 4) {
+        const DropCtr dc = drop_ctr(da);
+        const int rr = (ew & 3) * 32 + static_cast<int>(lane_id());
+        const unsigned long long i0 = (static_cast<unsigned long long>(bh) * AT_S + rr) * AT_S;
+        uint8_t* prow = sP + rr * 128;
+#pragma unroll
+        for (int c = 0; c < AT_S; c += 32) {
+          uint32_t bits = 0;
+#pragma unroll
+          for (int j = 0; j < 32; j += 8) bits |= drop_keep8(dc, i0 + c + j) << j;
+          keep[c >> 5] = bits;
+          uint8_t* tile = prow + (c >> 6) * 16384;
+#pragma unroll
+          for (int j = 0; j < 32; j += 8) {
+            uint4* slot = reinterpret_cast<uint4*>(tile + (((((c & 63) + j) >> 3) ^ (rr & 7)) << 4));
+            float f[8];
+            const uint4 pv = *slot;
+            const float2 p0 = unpack_bf16x2(pv.x), p1 = unpack_bf16x2(pv.y), p2 = unpack_bf16x2(pv.z), p3 = unpack_bf16x2(pv.w);
+            f[0] = p0.x; f[1] = p0.y; f[2] = p1.x; f[3] = p1.y; f[4] = p2.x; f[5] = p2.y; f[6] = p3.x; f[7] = p3.y;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) f[jj] = kept(bits, j + jj, f[jj], da.scale);
+            *slot = make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]),
+                               pack_bf16x2(f[6], f[7]));
+          }
+        }
+        fence_proxy_async();        // the dropped tile (generic-proxy writes) -> visible to the tensor core
+      }
+      named_bar_sync(1, AT_CONSUMERS);
+    }
     {
       // dV[key, d] = sum_q P[q, key] dO[q, d]: both operands MN-major, reduction over the 128 query rows;
       // warpgroup g owns keys 64 g .. 64 g + 63 = the g-th 64-key half of P
@@ -283,17 +335,24 @@ attention_bwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
     if (ew < 4) {
       uint8_t* prow = sP + r * 128;
       const float* wrow = sW + r * AT_SP;
+      const __nv_bfloat16* gprow = p.probs + (static_cast<size_t>(bh) * AT_S + r) * AT_S;   // DROP: undropped P
       // pass 1: delta = sum_key P[r, key] * dP[r, key]
       float delta = 0.f;
 #pragma unroll 1
       for (int c = 0; c < AT_S; c += 32) {
         uint32_t x[32];
         acc_ld_row32(wrow + c, x);
+        if constexpr (DROP) {
+          const uint32_t kb = c == 0 ? keep[0] : c == 32 ? keep[1] : c == 64 ? keep[2] : keep[3];   // static indices
+#pragma unroll
+          for (int j = 0; j < 32; ++j) x[j] = __float_as_uint(kept(kb, j, __uint_as_float(x[j]), da.scale));
+        }
         const uint8_t* tile = prow + (c >> 6) * 16384;
 #pragma unroll
         for (int j = 0; j < 32; j += 8) {
           const int chunk = ((c & 63) + j) >> 3;
-          const uint4 pv = *reinterpret_cast<const uint4*>(tile + ((chunk ^ (r & 7)) << 4));
+          const uint4 pv = DROP ? *reinterpret_cast<const uint4*>(gprow + c + j)
+                                : *reinterpret_cast<const uint4*>(tile + ((chunk ^ (r & 7)) << 4));
           const float2 p0 = unpack_bf16x2(pv.x), p1 = unpack_bf16x2(pv.y), p2 = unpack_bf16x2(pv.z), p3 = unpack_bf16x2(pv.w);
           delta = fmaf(p0.x, __uint_as_float(x[j]), delta);     delta = fmaf(p0.y, __uint_as_float(x[j + 1]), delta);
           delta = fmaf(p1.x, __uint_as_float(x[j + 2]), delta); delta = fmaf(p1.y, __uint_as_float(x[j + 3]), delta);
@@ -306,12 +365,17 @@ attention_bwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
       for (int c = 0; c < AT_S; c += 32) {
         uint32_t x[32];
         acc_ld_row32(wrow + c, x);
+        if constexpr (DROP) {
+          const uint32_t kb = c == 0 ? keep[0] : c == 32 ? keep[1] : c == 64 ? keep[2] : keep[3];   // static indices
+#pragma unroll
+          for (int j = 0; j < 32; ++j) x[j] = __float_as_uint(kept(kb, j, __uint_as_float(x[j]), da.scale));
+        }
         uint8_t* tile = prow + (c >> 6) * 16384;
 #pragma unroll
         for (int j = 0; j < 32; j += 8) {
           const int chunk = ((c & 63) + j) >> 3;
           uint4* slot = reinterpret_cast<uint4*>(tile + ((chunk ^ (r & 7)) << 4));
-          const uint4 pv = *slot;
+          const uint4 pv = DROP ? *reinterpret_cast<const uint4*>(gprow + c + j) : *slot;
           const float2 p0 = unpack_bf16x2(pv.x), p1 = unpack_bf16x2(pv.y), p2 = unpack_bf16x2(pv.z), p3 = unpack_bf16x2(pv.w);
           *slot = make_uint4(pack_bf16x2(p0.x * (__uint_as_float(x[j]) - delta), p0.y * (__uint_as_float(x[j + 1]) - delta)),
                              pack_bf16x2(p1.x * (__uint_as_float(x[j + 2]) - delta), p1.y * (__uint_as_float(x[j + 3]) - delta)),
@@ -385,8 +449,9 @@ attention_bwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
 using namespace b200;
 
 // qkv: packed [B*S, 3*H*64] bf16; out [B*S, H*64]; probs [B*H*S, S].  Returns -2 for unsupported shapes.
-extern "C" int b200_attention_fwd(const void* qkv, void* out, void* probs, int B, int S, int H, int dh, float scale,
-                                  cudaStream_t stream) {
+template <bool DROP>
+static int attention_fwd_launch(const void* qkv, void* out, void* probs, int B, int S, int H, int dh, float scale,
+                                const DropArgs& da, cudaStream_t stream) {
   if (B <= 0) return 0;
   if (S != AT_S || dh != AT_D) return -2;
   const long long D = static_cast<long long>(H) * dh;
@@ -406,11 +471,12 @@ extern "C" int b200_attention_fwd(const void* qkv, void* out, void* probs, int B
   constexpr int smem = 3 * AT_Q_BYTES + AT_P_BYTES + AT_WIDE_BYTES + AT_NARROW_BYTES + 8 + 1024;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(attention_fwd_s128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e = cudaFuncSetAttribute(attention_fwd_s128_kernel<DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return static_cast<int>(e);
     configured = true;
   }
-  cudaError_t le = launch_pdl(attention_fwd_s128_kernel, dim3(static_cast<unsigned>(B) * H), AT_THREADS, smem, stream, tq, tk, tv, p);
+  cudaError_t le = launch_pdl(attention_fwd_s128_kernel<DROP>, dim3(static_cast<unsigned>(B) * H), AT_THREADS, smem, stream,
+                              tq, tk, tv, p, da);
   if (le != cudaSuccess) return static_cast<int>(le);
   return static_cast<int>(cudaGetLastError());
 }
@@ -419,8 +485,9 @@ extern "C" int b200_encode_map2_bf16(void* map, const void* base, long long rows
                                      int box_cols, int box_rows);
 
 // qkv [B*S, 3D], dout [B*S, D], probs [B*H*S, S] (saved by the forward) -> dqkv [B*S, 3D]
-extern "C" int b200_attention_bwd(const void* qkv, const void* dout, const void* probs, void* dqkv, int B, int S, int H,
-                                  int dh, float scale, cudaStream_t stream) {
+template <bool DROP>
+static int attention_bwd_launch(const void* qkv, const void* dout, const void* probs, void* dqkv, int B, int S, int H,
+                                int dh, float scale, const DropArgs& da, cudaStream_t stream) {
   if (B <= 0) return 0;
   if (S != AT_S || dh != AT_D) return -2;
   const long long D = static_cast<long long>(H) * dh;
@@ -438,20 +505,39 @@ extern "C" int b200_attention_bwd(const void* qkv, const void* dout, const void*
   if (rc) return rc;
   AttnBwdParams p;
   p.dqkv = reinterpret_cast<__nv_bfloat16*>(dqkv);
+  p.probs = reinterpret_cast<const __nv_bfloat16*>(probs);
   p.H = H;
   p.D = static_cast<int>(D);
   p.scale = scale;
   constexpr int smem = 4 * AT_Q_BYTES + AT_P_BYTES + AT_WIDE_BYTES + AT_NARROW_BYTES + 8 + 1024;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(attention_bwd_s128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e = cudaFuncSetAttribute(attention_bwd_s128_kernel<DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return static_cast<int>(e);
     configured = true;
   }
-  cudaError_t le = launch_pdl(attention_bwd_s128_kernel, dim3(static_cast<unsigned>(B) * H), AT_THREADS, smem, stream, tq,
-                              tk, tv, tdo, tp, p);
+  cudaError_t le = launch_pdl(attention_bwd_s128_kernel<DROP>, dim3(static_cast<unsigned>(B) * H), AT_THREADS, smem, stream,
+                              tq, tk, tv, tdo, tp, p, da);
   if (le != cudaSuccess) return static_cast<int>(le);
   return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int b200_attention_fwd(const void* qkv, void* out, void* probs, int B, int S, int H, int dh, float scale,
+                                  cudaStream_t stream) {
+  return attention_fwd_launch<false>(qkv, out, probs, B, S, H, dh, scale, DropArgs{}, stream);
+}
+extern "C" int b200_attention_bwd(const void* qkv, const void* dout, const void* probs, void* dqkv, int B, int S, int H,
+                                  int dh, float scale, cudaStream_t stream) {
+  return attention_bwd_launch<false>(qkv, dout, probs, dqkv, B, S, H, dh, scale, DropArgs{}, stream);
+}
+
+extern "C" int b200_attention_drop_fwd(const void* qkv, void* out, void* probs, int B, int S, int H, int dh, float scale,
+                                       const B200Dropout* drop, cudaStream_t stream) {
+  return attention_fwd_launch<true>(qkv, out, probs, B, S, H, dh, scale, drop_args(drop), stream);
+}
+extern "C" int b200_attention_drop_bwd(const void* qkv, const void* dout, const void* probs, void* dqkv, int B, int S,
+                                       int H, int dh, float scale, const B200Dropout* drop, cudaStream_t stream) {
+  return attention_bwd_launch<true>(qkv, dout, probs, dqkv, B, S, H, dh, scale, drop_args(drop), stream);
 }
 
 B200_TRACE_REGISTER(attention)

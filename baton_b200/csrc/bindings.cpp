@@ -113,7 +113,7 @@ inline std::optional<B200AffineEpilogue> affine_epilogue(const std::optional<at:
 // ---- in-graph kernel timeline (pdl.cuh): every translation unit owns a copy of the trace pointer
 extern "C" {
 #define B200_TRACE_TUS(X) X(gemm_wgmma) X(gemm_fp8) X(quant) X(attention) X(im2col_tma) X(gemm_simt) X(fedavg) \
-  X(elementwise) X(conv) X(norm) X(loss) X(conv_halo)
+  X(elementwise) X(conv) X(norm) X(loss) X(conv_halo) X(dropout)
 #define B200_DECL(tu) int b200_trace_set_##tu(unsigned long long* p);
 B200_TRACE_TUS(B200_DECL)
 #undef B200_DECL
@@ -1306,6 +1306,107 @@ void softmax_bwd(const at::Tensor& y, const at::Tensor& dy, at::Tensor dx, int64
         "softmax_bwd");
 }
 
+// ---- dropout forms (csrc/dropout.cu, csrc/attention.cu) ---------------------------------------------
+// words: device int32 {epoch, stream_lo, stream_hi}; key: the 64-bit Philox key as a signed int64; the rest as in
+// B200Dropout (launch.h)
+#define DROP_ARGS const at::Tensor &words, int64_t key, int64_t site, int64_t step, int64_t steps, int64_t thresh, double scale
+inline B200Dropout make_drop(const at::Tensor& words, int64_t key, int64_t site, int64_t step, int64_t steps,
+                             int64_t thresh, double scale) {
+  CHECK_CUDA(words);
+  TORCH_CHECK(words.scalar_type() == at::kInt && words.is_contiguous() && words.numel() >= 3,
+              "dropout words: contiguous int32 {epoch, stream_lo, stream_hi}");
+  TORCH_CHECK(site >= 0 && site < 512 && step >= 0 && steps > 0 && step < (1 << 22) && steps < (1 << 22) &&
+                  thresh >= 0 && thresh < (1ll << 32),
+              "dropout: site < 512, 0 <= step, 0 < steps < 2^22, 0 <= thresh < 2^32");
+  return B200Dropout{words.data_ptr<int>(), static_cast<unsigned long long>(key), static_cast<uint32_t>(site),
+                     static_cast<uint32_t>(step), static_cast<uint32_t>(steps), static_cast<uint32_t>(thresh),
+                     static_cast<float>(scale)};
+}
+#define DROP_PASS words, key, site, step, steps, thresh, scale
+inline void check_bf16(std::initializer_list<const at::Tensor*> ts, const char* what) {
+  for (const at::Tensor* t : ts) {
+    CHECK_CUDA(*t);
+    TORCH_CHECK(t->scalar_type() == at::kBFloat16 && t->is_contiguous(), what, ": contiguous bf16 tensors");
+  }
+}
+void layernorm_drop_fwd(const at::Tensor& x, const std::optional<at::Tensor>& res, at::Tensor y,
+                        const std::optional<at::Tensor>& pre, const at::Tensor& gamma, const at::Tensor& beta,
+                        at::Tensor mean, at::Tensor rstd, int64_t rows, int64_t C, double eps, int64_t mode, DROP_ARGS) {
+  check_bf16({&x, &y}, "layernorm_drop_fwd");
+  TORCH_CHECK(x.numel() == rows * C && y.numel() == rows * C, "layernorm_drop_fwd: x, y must hold rows * C elements");
+  const B200Dropout d = make_drop(DROP_PASS);
+  const c10::cuda::CUDAGuard guard(x.device());
+  check(b200_layernorm_drop_fwd(x.data_ptr(), opt_ptr<const void>(res), y.data_ptr(), opt_ptr<void>(pre),
+                                gamma.data_ptr<float>(), beta.data_ptr<float>(), mean.data_ptr<float>(),
+                                rstd.data_ptr<float>(), rows, C, static_cast<float>(eps), static_cast<int>(mode), &d,
+                                cur_stream()),
+        "layernorm_drop_fwd");
+}
+void layernorm_drop_bwd(const at::Tensor& x, const at::Tensor& dy, at::Tensor dx, const std::optional<at::Tensor>& dxd,
+                        const at::Tensor& gamma, const at::Tensor& mean, const at::Tensor& rstd, at::Tensor dgamma,
+                        at::Tensor dbeta, int64_t rows, int64_t C, int64_t mode, DROP_ARGS) {
+  check_bf16({&x, &dy, &dx}, "layernorm_drop_bwd");
+  TORCH_CHECK(x.numel() == rows * C && dy.numel() == rows * C && dx.numel() == rows * C,
+              "layernorm_drop_bwd: x, dy, dx must hold rows * C elements");
+  const B200Dropout d = make_drop(DROP_PASS);
+  const c10::cuda::CUDAGuard guard(x.device());
+  check(b200_layernorm_drop_bwd(x.data_ptr(), dy.data_ptr(), dx.data_ptr(), opt_ptr<void>(dxd), gamma.data_ptr<float>(),
+                                mean.data_ptr<float>(), rstd.data_ptr<float>(), dgamma.data_ptr<float>(),
+                                dbeta.data_ptr<float>(), rows, C, static_cast<int>(mode), &d, cur_stream()),
+        "layernorm_drop_bwd");
+}
+void softmax_drop_fwd(const at::Tensor& x, at::Tensor y, at::Tensor yd, int64_t rows, int64_t C, double sm_scale,
+                      DROP_ARGS) {
+  check_bf16({&x, &y, &yd}, "softmax_drop_fwd");
+  const B200Dropout d = make_drop(DROP_PASS);
+  const c10::cuda::CUDAGuard guard(x.device());
+  check(b200_softmax_drop_fwd(x.data_ptr(), y.data_ptr(), yd.data_ptr(), rows, C, static_cast<float>(sm_scale), &d,
+                              cur_stream()),
+        "softmax_drop_fwd");
+}
+void softmax_drop_bwd(const at::Tensor& y, const at::Tensor& dy, at::Tensor dx, int64_t rows, int64_t C, double sm_scale,
+                      DROP_ARGS) {
+  check_bf16({&y, &dy, &dx}, "softmax_drop_bwd");
+  const B200Dropout d = make_drop(DROP_PASS);
+  const c10::cuda::CUDAGuard guard(y.device());
+  check(b200_softmax_drop_bwd(y.data_ptr(), dy.data_ptr(), dx.data_ptr(), rows, C, static_cast<float>(sm_scale), &d,
+                              cur_stream()),
+        "softmax_drop_bwd");
+}
+void dropout(const at::Tensor& x, at::Tensor y, DROP_ARGS) {
+  check_bf16({&x, &y}, "dropout");
+  TORCH_CHECK(x.numel() == y.numel(), "dropout: x and y differ in size");
+  const B200Dropout d = make_drop(DROP_PASS);
+  const c10::cuda::CUDAGuard guard(x.device());
+  check(b200_dropout(x.data_ptr(), y.data_ptr(), x.numel(), &d, cur_stream()), "dropout");
+}
+bool attention_drop_fwd(const at::Tensor& qkv, at::Tensor out, at::Tensor probs, int64_t B, int64_t S, int64_t H,
+                        int64_t dh, double sm_scale, DROP_ARGS) {
+  check_bf16({&qkv, &out, &probs}, "attention_drop_fwd");
+  const B200Dropout d = make_drop(DROP_PASS);
+  const c10::cuda::CUDAGuard guard(qkv.device());
+  const int rc = b200_attention_drop_fwd(cptr(qkv), ptr(out), ptr(probs), static_cast<int>(B), static_cast<int>(S),
+                                         static_cast<int>(H), static_cast<int>(dh), static_cast<float>(sm_scale), &d,
+                                         cur_stream());
+  if (rc == -2) return false;
+  check(rc, "attention_drop_fwd");
+  return true;
+}
+bool attention_drop_bwd(const at::Tensor& qkv, const at::Tensor& dout, const at::Tensor& probs, at::Tensor dqkv,
+                        int64_t B, int64_t S, int64_t H, int64_t dh, double sm_scale, DROP_ARGS) {
+  check_bf16({&qkv, &dout, &probs, &dqkv}, "attention_drop_bwd");
+  const B200Dropout d = make_drop(DROP_PASS);
+  const c10::cuda::CUDAGuard guard(qkv.device());
+  const int rc = b200_attention_drop_bwd(cptr(qkv), cptr(dout), cptr(probs), ptr(dqkv), static_cast<int>(B),
+                                         static_cast<int>(S), static_cast<int>(H), static_cast<int>(dh),
+                                         static_cast<float>(sm_scale), &d, cur_stream());
+  if (rc == -2) return false;
+  check(rc, "attention_drop_bwd");
+  return true;
+}
+#undef DROP_ARGS
+#undef DROP_PASS
+
 // ---- losses ------------------------------------------------------------------------------------------
 void softmax_xent(const at::Tensor& logits, const at::Tensor& target, const std::optional<at::Tensor>& dlogits,
                   at::Tensor loss_acc, int64_t rows, int64_t C, int64_t ld, double grad_scale) {
@@ -1481,6 +1582,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("bn_relu_maxpool", &bn_relu_maxpool);
   m.def("bn_maxpool_bwd", &bn_maxpool_bwd);
   m.def("layernorm_fwd", &layernorm_fwd);
+  m.def("layernorm_drop_fwd", &layernorm_drop_fwd);
+  m.def("layernorm_drop_bwd", &layernorm_drop_bwd);
+  m.def("softmax_drop_fwd", &softmax_drop_fwd);
+  m.def("softmax_drop_bwd", &softmax_drop_bwd);
+  m.def("dropout", &dropout);
+  m.def("attention_drop_fwd", &attention_drop_fwd);
+  m.def("attention_drop_bwd", &attention_drop_bwd);
   m.def("layernorm_bwd", &layernorm_bwd);
   m.def("softmax_fwd", &softmax_fwd);
   m.def("softmax_bwd", &softmax_bwd);

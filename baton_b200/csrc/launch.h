@@ -56,6 +56,13 @@ int b200_attention_fwd(const void* qkv, void* out, void* probs, int B, int S, in
                        cudaStream_t stream);
 int b200_attention_bwd(const void* qkv, const void* dout, const void* probs, void* dqkv, int B, int S, int H, int dh,
                        float scale, cudaStream_t stream);
+// the same with dropout on the probabilities (struct B200Dropout below; element i = the index into probs): the
+// forward's probs stay the undropped P, out = (P o M s) V; the backward regenerates the mask
+struct B200Dropout;
+int b200_attention_drop_fwd(const void* qkv, void* out, void* probs, int B, int S, int H, int dh, float scale,
+                            const B200Dropout* drop, cudaStream_t stream);
+int b200_attention_drop_bwd(const void* qkv, const void* dout, const void* probs, void* dqkv, int B, int S, int H, int dh,
+                            float scale, const B200Dropout* drop, cudaStream_t stream);
 // ---- implicit-GEMM convolution (experimental: gemm_wgmma.cu CONV modes fed by TMA im2col maps)
 int b200_conv_igemm_fwd(const void* x, const void* w, void* y, int N, int H, int W, int Cin, int Cout, int KH, int KW,
                         int stride, int pad, int Ho, int Wo, int cluster_k, int force_bn, float* col_stats,
@@ -393,6 +400,34 @@ int b200_layernorm_bwd(const void* x, const void* dy, void* dx, const float* gam
 int b200_softmax_fwd(const void* x, void* y, long long rows, int C, float scale, cudaStream_t stream);
 int b200_softmax_bwd(const void* y, const void* dy, void* dx, long long rows, int C, float scale,
                      cudaStream_t stream);
+
+// ---- dropout.cu (and the dropout forms of the fused attention): the mask of one dropout site (csrc/dropout.cuh,
+// baton_b200/data/dropout.py).  words: device int32 {epoch, stream_lo, stream_hi}; the run's local step is
+// t = epoch * steps + step.  Element i is kept iff word i & 3 of philox4x32_10((i >> 2, 0x80000000 | site << 22 | t,
+// stream_lo, stream_hi), key) >= thresh; a kept value is multiplied by scale.  site < 512, t < 2^22.
+struct B200Dropout {
+  const int* words;
+  unsigned long long key;
+  uint32_t site, step, steps;
+  uint32_t thresh;                  // floor(p * 2^32)
+  float scale;                      // fp32(1 / (1 - p))
+};
+// LayerNorm with dropout: mode 1 (input dropout) pre = drop(x) + residual?, y = LN(pre) (pre written, bf16); mode 2
+// (output dropout) y = drop(LN(x + residual?)).  Backward: x = the pre-norm input; mode 1 writes dx = dpre and
+// dxd = M s dpre, mode 2 applies M s to dy as it loads it (dxd unused).  dgamma / dbeta ACCUMULATED.
+int b200_layernorm_drop_fwd(const void* x, const void* residual, void* y, void* pre, const float* gamma,
+                            const float* beta, float* mean, float* rstd, long long rows, int C, float eps, int mode,
+                            const B200Dropout* drop, cudaStream_t stream);
+int b200_layernorm_drop_bwd(const void* x, const void* dy, void* dx, void* dxd, const float* gamma, const float* mean,
+                            const float* rstd, float* dgamma, float* dbeta, long long rows, int C, int mode,
+                            const B200Dropout* drop, cudaStream_t stream);
+// softmax with dropout: y = softmax(scale x) (saved), yd = drop(y); backward dx = scale y (g - sum(g y)), g = M s dy
+int b200_softmax_drop_fwd(const void* x, void* y, void* yd, long long rows, int C, float scale, const B200Dropout* drop,
+                          cudaStream_t stream);
+int b200_softmax_drop_bwd(const void* y, const void* dy, void* dx, long long rows, int C, float scale,
+                          const B200Dropout* drop, cudaStream_t stream);
+// y = drop(x) over n bf16 elements (forward and backward of an elementwise dropout)
+int b200_dropout(const void* x, void* y, long long n, const B200Dropout* drop, cudaStream_t stream);
 
 // ---- loss.cu
 int b200_softmax_xent(const void* logits, int logits_fp32, const long long* target, void* dlogits, int dl_fp32,

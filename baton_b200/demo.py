@@ -25,7 +25,11 @@ from .data import linear_regression_shard
 from .models import MLP2, LinearModel
 
 
-def build_model(kind: str):
+def build_model(kind: str, dropout: float = 0.0):
+    """The model ``kind``; ``dropout``: the hidden and attention-probability dropout of the BERT models (``ValueError``
+    for a model without dropout sites)."""
+    if dropout and kind != "bert_base":
+        raise ValueError("dropout applies to the BERT models only, not {!r}".format(kind))
     if kind in ("lineartest", "linear"):
         return LinearModel()
     if kind == "mlp2":
@@ -44,7 +48,7 @@ def build_model(kind: str):
         return resnet50(num_classes=1000, norm="group", groups=2)
     if kind == "bert_base":
         from .models import bert_base
-        return bert_base()
+        return bert_base(hidden_dropout_prob=dropout, attention_probs_dropout_prob=dropout)
     raise SystemExit("unknown model {!r}".format(kind))
 
 
@@ -91,7 +95,7 @@ def make_gpu_worker(app, model, host: str, port: int, cfg: FederationConfig):
 def make_app(role: str, host: str, port: int, cfg: Optional[FederationConfig] = None) -> web.Application:
     cfg = cfg or FederationConfig()
     app = web.Application(client_max_size=1 << 34)
-    model = build_model(cfg.model)
+    model = build_model(cfg.model, cfg.dropout)
     if role == "manager":
         manager = Manager(app)
         manager.register_experiment(

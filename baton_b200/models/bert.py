@@ -8,8 +8,11 @@ the usual parameter names (``bert.embeddings.word_embeddings.weight``,
 Hugging-Face ``BertForSequenceClassification`` state_dict onto it and back, so HF checkpoints load and our
 checkpoints stay loadable by HF -- tests/test_bert_hf_compat.py).  Every matmul is the wgmma
 GEMM (GELU fused in the epilogue), attention is four strided-batched GEMMs + the softmax kernel on
-the packed QKV buffer, LayerNorm fuses the residual add.  Dropout is omitted (p = 0): the
-reference has none and synthetic-shard benchmarking does not want the noise.
+the packed QKV buffer, LayerNorm fuses the residual add.  Dropout follows Hugging-Face's five positions with its
+config names (``hidden_dropout_prob``, ``attention_probs_dropout_prob``, ``classifier_dropout``); the defaults are 0,
+which runs exactly the kernels of a model without dropout.  The masks come from a counter (``data/dropout.py``), drawn
+inside the fused attention, LayerNorm and softmax kernels; the trainers set the model's ``dropout_run`` before every
+step, and nothing is dropped outside a training run or in eval mode.
 """
 from __future__ import annotations
 
@@ -19,6 +22,7 @@ from typing import Optional
 import torch
 from torch import nn
 
+from ..data.dropout import DropoutRun, check_dropout
 from ..ops import nn as bnn
 from .base import FederatedModule
 
@@ -34,11 +38,31 @@ class BertConfig:
     type_vocab_size: int = 2
     layer_norm_eps: float = 1e-12
     num_labels: int = 2
+    hidden_dropout_prob: float = 0.0
+    attention_probs_dropout_prob: float = 0.0
+    classifier_dropout: Optional[float] = None     # None: hidden_dropout_prob
+
+    def __post_init__(self):
+        check_dropout(self.hidden_dropout_prob, "hidden_dropout_prob")
+        check_dropout(self.attention_probs_dropout_prob, "attention_probs_dropout_prob")
+        if self.classifier_dropout is not None:
+            check_dropout(self.classifier_dropout, "classifier_dropout")
+
+    @property
+    def classifier_p(self) -> float:
+        return float(self.hidden_dropout_prob if self.classifier_dropout is None else self.classifier_dropout)
+
+
+def _site(module: nn.Module, site: int, p: float):
+    """``(run, site, p)`` when dropout site ``site`` drops in this call, else None."""
+    run = module.dropout_run
+    return (run, site, p) if p > 0.0 and module.training and run.active else None
 
 
 class BertEmbeddings(nn.Module):
-    def __init__(self, c: BertConfig):
+    def __init__(self, c: BertConfig, run: DropoutRun):
         super().__init__()
+        self.dropout_run, self.p = run, float(c.hidden_dropout_prob)
         self.word_embeddings = bnn.Embedding(c.vocab_size, c.hidden_size)
         self.position_embeddings = bnn.Embedding(c.max_position_embeddings, c.hidden_size)
         self.token_type_embeddings = bnn.Embedding(c.type_vocab_size, c.hidden_size)
@@ -48,11 +72,13 @@ class BertEmbeddings(nn.Module):
         w = self.word_embeddings(ids)
         p = self.position_embeddings(pos_ids)
         t = self.token_type_embeddings(type_ids)
+        drop = _site(self, 0, self.p)
+        if drop is not None:
+            drop = drop + (2,)                 # output dropout
         if w.is_cuda:
-            from ..ops import functional as F
             pt = _Add.apply(p, t)
-            return self.LayerNorm(w, pt)
-        return self.LayerNorm(w + p + t)
+            return self.LayerNorm(w, pt) if drop is None else self.LayerNorm(w, pt, drop=drop)
+        return self.LayerNorm(w + p + t) if drop is None else self.LayerNorm(w + p + t, drop=drop)
 
 
 class _Add(torch.autograd.Function):
@@ -67,8 +93,10 @@ class _Add(torch.autograd.Function):
 
 
 class BertLayer(nn.Module):
-    def __init__(self, c: BertConfig):
+    def __init__(self, c: BertConfig, run: DropoutRun, index: int):
         super().__init__()
+        self.dropout_run, self.site = run, 1 + 3 * index        # sites: probabilities, attn_out, ffn_out
+        self.p_attn, self.p_hidden = float(c.attention_probs_dropout_prob), float(c.hidden_dropout_prob)
         self.H, self.dh = c.num_attention_heads, c.hidden_size // c.num_attention_heads
         self.qkv = bnn.Linear(c.hidden_size, 3 * c.hidden_size)
         self.attn_out = bnn.Linear(c.hidden_size, c.hidden_size)
@@ -78,9 +106,19 @@ class BertLayer(nn.Module):
         self.ffn_ln = bnn.LayerNorm(c.hidden_size, c.layer_norm_eps)
 
     def forward(self, x, B, S, mask_bias=None):
-        a = bnn.attention(self.qkv(x), B, S, self.H, self.dh, mask_bias=mask_bias)
-        x = self.attn_ln(self.attn_out(a), x)
-        return self.ffn_ln(self.ffn_out(self.ffn_in(x)), x)
+        d_attn = _site(self, self.site, self.p_attn)
+        if d_attn is None:
+            a = bnn.attention(self.qkv(x), B, S, self.H, self.dh, mask_bias=mask_bias)
+        else:
+            a = bnn.attention(self.qkv(x), B, S, self.H, self.dh, mask_bias=mask_bias, drop=d_attn)
+        d_out, d_ffn = _site(self, self.site + 1, self.p_hidden), _site(self, self.site + 2, self.p_hidden)
+        if d_out is None:
+            x = self.attn_ln(self.attn_out(a), x)
+        else:
+            x = self.attn_ln(self.attn_out(a), x, drop=d_out + (1,))        # input dropout
+        if d_ffn is None:
+            return self.ffn_ln(self.ffn_out(self.ffn_in(x)), x)
+        return self.ffn_ln(self.ffn_out(self.ffn_in(x)), x, drop=d_ffn + (1,))
 
 
 class BertForSequenceClassification(FederatedModule):
@@ -95,8 +133,9 @@ class BertForSequenceClassification(FederatedModule):
         self.config = c = config or BertConfig()
         if name:
             self.name = name
-        self.embeddings = BertEmbeddings(c)
-        self.layers = nn.ModuleList([BertLayer(c) for _ in range(c.num_hidden_layers)])
+        self.dropout_run = DropoutRun()      # set by the trainers before every step (data/dropout.py)
+        self.embeddings = BertEmbeddings(c, self.dropout_run)
+        self.layers = nn.ModuleList([BertLayer(c, self.dropout_run, i) for i in range(c.num_hidden_layers)])
         self.pooler = bnn.Linear(c.hidden_size, c.hidden_size)
         self.classifier = bnn.Linear(c.hidden_size, c.num_labels, out_fp32=True)
         self._static = {}
@@ -105,6 +144,16 @@ class BertForSequenceClassification(FederatedModule):
                 nn.init.normal_(m.weight, std=0.02)
                 if m.bias is not None:
                     nn.init.zeros_(m.bias)
+
+    @property
+    def n_dropout_sites(self) -> int:
+        return 2 + 3 * self.config.num_hidden_layers
+
+    @property
+    def has_dropout(self) -> bool:
+        """True when some dropout probability is nonzero."""
+        c = self.config
+        return max(c.hidden_dropout_prob, c.attention_probs_dropout_prob, c.classifier_p) > 0.0
 
     def _ids(self, B, S, device):
         key = (B, S, str(device))
@@ -131,6 +180,9 @@ class BertForSequenceClassification(FederatedModule):
         pooled = torch.tanh(self.pooler(first).float())
         if pooled.is_cuda:
             pooled = pooled.to(torch.bfloat16)
+        drop = _site(self, self.n_dropout_sites - 1, self.config.classifier_p)
+        if drop is not None:
+            pooled = bnn.dropout(pooled, *drop)
         return self.classifier(pooled)
 
 

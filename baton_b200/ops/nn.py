@@ -712,8 +712,50 @@ class _LNFn(torch.autograd.Function):
         return dx, (dx if ctx.has_res else None), gg, gb, None, None
 
 
+class _LNDropFn(torch.autograd.Function):
+    """LayerNorm with dropout (csrc/dropout.cu).  mode 1, input dropout: ``LN(drop(x) + residual)``, the kernel writes
+    the pre-norm sum; backward writes its gradient (the residual's) and ``M s`` times it (x's) in one launch.  mode 2,
+    output dropout: ``drop(LN(x + residual))``; backward masks ``dy`` as it loads it.  ``dargs``: the dropout arguments
+    of the kernel entry points (``DropoutRun.kernel_args``)."""
+
+    @staticmethod
+    def forward(ctx, x, residual, gamma, beta, eps, mode, dargs, anchor):
+        gamma, beta = _unwrap(gamma), _unwrap(beta)
+        c = x.shape[-1]
+        rows = x.numel() // c
+        y = torch.empty_like(x)
+        mean = torch.empty(rows, dtype=torch.float32, device=x.device)
+        rstd = torch.empty(rows, dtype=torch.float32, device=x.device)
+        pre = torch.empty_like(x) if mode == 1 else None
+        load().layernorm_drop_fwd(x, residual, y, pre, gamma, beta, mean, rstd, rows, c, eps, mode, *dargs)
+        if mode == 2:
+            pre = x if residual is None else F.add(x, residual)
+        ctx.save_for_backward(pre, mean, rstd)
+        ctx.gamma, ctx.beta, ctx.has_res, ctx.rows, ctx.c = gamma, beta, residual is not None, rows, c
+        ctx.mode, ctx.dargs = mode, dargs
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        pre, mean, rstd = ctx.saved_tensors
+        dy = dy.contiguous()
+        dpre = torch.empty_like(pre)
+        dx = torch.empty_like(pre) if ctx.mode == 1 else None
+        tg, tb = _grad_target(ctx.gamma), _grad_target(ctx.beta)
+        gg = gb = None
+        if tg is None:
+            gg = tg = torch.zeros(ctx.c, dtype=torch.float32, device=dy.device)
+        if tb is None:
+            gb = tb = torch.zeros(ctx.c, dtype=torch.float32, device=dy.device)
+        load().layernorm_drop_bwd(pre, dy, dpre, dx, ctx.gamma, mean, rstd, tg, tb, ctx.rows, ctx.c, ctx.mode, *ctx.dargs)
+        if ctx.mode == 2:
+            dx = dpre
+        return dx, (dpre if ctx.has_res else None), gg, gb, None, None, None, None
+
+
 class LayerNorm(nn.Module):
-    """``LN(x + residual)`` over the last axis (residual optional)."""
+    """``LN(x + residual)`` over the last axis (residual optional).  ``drop = (run, site, p, mode)``: the dropout form
+    (``data/dropout.py``), mode 1 ``LN(drop(x) + residual)``, mode 2 ``drop(LN(x + residual))``."""
 
     def __init__(self, normalized_shape: int, eps: float = 1e-12):
         super().__init__()
@@ -721,7 +763,17 @@ class LayerNorm(nn.Module):
         self.weight = nn.Parameter(torch.ones(normalized_shape))
         self.bias = nn.Parameter(torch.zeros(normalized_shape))
 
-    def forward(self, x, residual=None):
+    def forward(self, x, residual=None, drop=None):
+        if drop is not None:
+            run, site, p, mode = drop
+            if not x.is_cuda:
+                if mode == 1:
+                    x = run.apply(x, site, p)
+                y = self.forward(x, residual)
+                return run.apply(y, site, p) if mode == 2 else y
+            return _LNDropFn.apply(x.contiguous(), None if residual is None else residual.contiguous(),
+                                   _wrap(self.weight, x), _wrap(self.bias, x), self.eps, mode,
+                                   run.kernel_args(site, p), _anchor(x, self.weight))
         if not x.is_cuda:
             if residual is not None:
                 x = x + residual
@@ -817,14 +869,17 @@ class _AttnFn(torch.autograd.Function):
     gradients are addressed in place through 4-D TMA maps (no head split / merge copies)."""
 
     @staticmethod
-    def forward(ctx, qkv, B, S, H, dh, mask_bias=None):
+    def forward(ctx, qkv, B, S, H, dh, mask_bias=None, dargs=None):
         D = H * dh
+        ctx.dargs = dargs
         if S == 128 and dh == 64 and mask_bias is None:
             # single-kernel forward (csrc/attention.cu): scores stay in shared memory, P is written once
             probs = torch.empty((B * H * S, S), dtype=BF16, device=qkv.device)
             out = torch.empty((B * S, D), dtype=BF16, device=qkv.device)
-            if load().attention_fwd(qkv, out, probs, B, S, H, dh, 1.0 / math.sqrt(dh)):
-                ctx.save_for_backward(qkv, probs)
+            ok = (load().attention_fwd(qkv, out, probs, B, S, H, dh, 1.0 / math.sqrt(dh)) if dargs is None else
+                  load().attention_drop_fwd(qkv, out, probs, B, S, H, dh, 1.0 / math.sqrt(dh), *dargs))
+            if ok:
+                ctx.save_for_backward(qkv, probs, None)
                 ctx.dims = (B, S, H, dh)
                 return out
         q, k, v = qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:]
@@ -835,52 +890,65 @@ class _AttnFn(torch.autograd.Function):
         if mask_bias is not None:        # additive key-padding mask [B, S] (0 / large negative), broadcast over heads and queries
             scores.view(B, H, S, S).add_(mask_bias.to(scores.dtype).view(B, 1, 1, S))
         probs = torch.empty_like(scores)
-        load().softmax_fwd(scores, probs, B * H * S, S, 1.0)
+        pdrop = None
+        if dargs is None:
+            load().softmax_fwd(scores, probs, B * H * S, S, 1.0)
+        else:        # P is saved for backward, the dropped P (the one extra S x S buffer) feeds the PV GEMM and dV
+            pdrop = torch.empty_like(scores)
+            load().softmax_drop_fwd(scores, probs, pdrop, B * H * S, S, 1.0, *dargs)
         out = torch.empty((B * S, D), dtype=BF16, device=qkv.device)
-        F.gemm_batched(probs, v, out, M=S, N=dh, K=S, lda=S, ldb=3 * D, ldd=D, a_mn=False, b_mn=True,
+        F.gemm_batched(probs if pdrop is None else pdrop, v, out, M=S, N=dh, K=S, lda=S, ldb=3 * D, ldd=D, a_mn=False, b_mn=True,
                        n_outer=B, n_inner=H, a_strides=(H * S * S, S * S), b_strides=(S * 3 * D, dh),
                        d_strides=(S * D, dh))
-        ctx.save_for_backward(qkv, probs)
+        ctx.save_for_backward(qkv, probs, pdrop)
         ctx.dims = (B, S, H, dh)
         ctx.masked = mask_bias is not None
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        qkv, probs = ctx.saved_tensors
+        qkv, probs, pdrop = ctx.saved_tensors
         B, S, H, dh = ctx.dims
         D = H * dh
+        dargs = ctx.dargs
         dout = dout.contiguous()
         dqkv = torch.empty_like(qkv)
         if S == 128 and dh == 64 and not getattr(ctx, "masked", False):
             # single-kernel backward (csrc/attention.cu): dP / dS never leave the SM
-            if load().attention_bwd(qkv, dout, probs, dqkv, B, S, H, dh, 1.0 / math.sqrt(dh)):
-                return dqkv, None, None, None, None, None
+            ok = (load().attention_bwd(qkv, dout, probs, dqkv, B, S, H, dh, 1.0 / math.sqrt(dh)) if dargs is None else
+                  load().attention_drop_bwd(qkv, dout, probs, dqkv, B, S, H, dh, 1.0 / math.sqrt(dh), *dargs))
+            if ok:
+                return dqkv, None, None, None, None, None, None
         q, k, v = qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:]
         dq, dk, dv = dqkv[:, :D], dqkv[:, D:2 * D], dqkv[:, 2 * D:]
         bh = (H * S * S, S * S)
         pk = (S * 3 * D, dh)
-        # dV = P^T dO
-        F.gemm_batched(probs, dout, dv, M=S, N=dh, K=S, lda=S, ldb=D, ldd=3 * D, a_mn=True, b_mn=True,
+        # dV = P^T dO (the dropped P with dropout)
+        F.gemm_batched(probs if pdrop is None else pdrop, dout, dv, M=S, N=dh, K=S, lda=S, ldb=D, ldd=3 * D, a_mn=True, b_mn=True,
                        n_outer=B, n_inner=H, a_strides=bh, b_strides=(S * D, dh), d_strides=pk)
         # dP = dO V^T
         dprobs = torch.empty_like(probs)
         F.gemm_batched(dout, v, dprobs, M=S, N=S, K=dh, lda=D, ldb=3 * D, ldd=S, a_mn=False, b_mn=False,
                        n_outer=B, n_inner=H, a_strides=(S * D, dh), b_strides=pk, d_strides=bh)
         dscores = torch.empty_like(probs)
-        load().softmax_bwd(probs, dprobs, dscores, B * H * S, S, 1.0)
+        if dargs is None:
+            load().softmax_bwd(probs, dprobs, dscores, B * H * S, S, 1.0)
+        else:
+            load().softmax_drop_bwd(probs, dprobs, dscores, B * H * S, S, 1.0, *dargs)
         alpha = 1.0 / math.sqrt(dh)
         # dQ = alpha dS K ; dK = alpha dS^T Q
         F.gemm_batched(dscores, k, dq, M=S, N=dh, K=S, lda=S, ldb=3 * D, ldd=3 * D, a_mn=False, b_mn=True,
                        n_outer=B, n_inner=H, a_strides=bh, b_strides=pk, d_strides=pk, alpha=alpha)
         F.gemm_batched(dscores, q, dk, M=S, N=dh, K=S, lda=S, ldb=3 * D, ldd=3 * D, a_mn=True, b_mn=True,
                        n_outer=B, n_inner=H, a_strides=bh, b_strides=pk, d_strides=pk, alpha=alpha)
-        return dqkv, None, None, None, None, None
+        return dqkv, None, None, None, None, None, None
 
 
-def attention(qkv: torch.Tensor, B: int, S: int, H: int, dh: int, mask_bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+def attention(qkv: torch.Tensor, B: int, S: int, H: int, dh: int, mask_bias: Optional[torch.Tensor] = None,
+              drop=None) -> torch.Tensor:
     """``softmax(Q K^T / sqrt(dh) + mask_bias) V`` for packed ``qkv [B*S, 3*H*dh]`` -> ``[B*S, H*dh]``.
-    ``mask_bias``: optional additive key mask ``[B, S]`` (0 = attend, large negative = padding)."""
+    ``mask_bias``: optional additive key mask ``[B, S]`` (0 = attend, large negative = padding).  ``drop = (run, site,
+    p)``: dropout on the probabilities (``data/dropout.py``), element i the index into ``[B*H*S, S]``."""
     if not qkv.is_cuda:
         D = H * dh
         q, k, v = (t.reshape(B, S, H, dh).transpose(1, 2) for t in qkv.split(D, dim=-1))
@@ -888,8 +956,38 @@ def attention(qkv: torch.Tensor, B: int, S: int, H: int, dh: int, mask_bias: Opt
         if mask_bias is not None:
             sc = sc + mask_bias.to(sc.dtype).view(B, 1, 1, S)
         p = torch.softmax(sc, dim=-1)
+        if drop is not None:
+            run, site, pr = drop
+            p = run.apply(p.contiguous(), site, pr)
         return (p @ v).transpose(1, 2).reshape(B * S, D)
-    return _AttnFn.apply(qkv.contiguous(), B, S, H, dh, mask_bias)
+    dargs = drop[0].kernel_args(drop[1], drop[2]) if drop is not None else None
+    return _AttnFn.apply(qkv.contiguous(), B, S, H, dh, mask_bias, dargs)
+
+
+class _DropFn(torch.autograd.Function):
+    """Elementwise dropout of a bf16 tensor (``csrc/dropout.cu``): forward and backward apply the same mask."""
+
+    @staticmethod
+    def forward(ctx, x, dargs):
+        y = torch.empty_like(x)
+        load().dropout(x, y, *dargs)
+        ctx.dargs = dargs
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        dx = torch.empty_like(dy, memory_format=torch.contiguous_format)
+        load().dropout(dy.contiguous(), dx, *ctx.dargs)
+        return dx, None
+
+
+def dropout(x: torch.Tensor, run, site: int, p: float) -> torch.Tensor:
+    """``x`` with the mask of dropout ``site`` at ``run``'s current step (``data/dropout.py``)."""
+    if not x.is_cuda:
+        return run.apply(x, site, p)
+    if x.dtype != BF16:
+        x = F.cast(x.contiguous(), BF16)
+    return _DropFn.apply(x.contiguous(), run.kernel_args(site, p))
 
 
 class _EmbedFn(torch.autograd.Function):

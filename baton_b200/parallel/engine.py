@@ -264,7 +264,8 @@ class FederatedEngine:
             aug_hp.update(augment=aug.kind, augment_padding=aug.padding)
         if mixc is not None:
             aug_hp.update(mix=mixc.kind, mix_alpha=mixc.alpha, label_smoothing=mixc.smoothing)
-        self.aug_hp = dict(aug_hp, augment_seed=seed) if aug_hp else None
+        # dropout (a BERT model with a nonzero probability) draws from the same key and per-client stream
+        self.aug_hp = dict(aug_hp, augment_seed=seed) if aug_hp or getattr(model, "has_dropout", False) else None
         self.n_rounds = 0
         self._last_participants: Optional[List[int]] = None
         self.logical_clients = logical_clients if logical_clients and logical_clients > self.world else 0
@@ -480,8 +481,8 @@ class FederatedEngine:
 
     def _train_client(self, cid: int, X, y, n_epoch: int, first: bool):
         """Local training of client ``cid`` on the replica; with SCAFFOLD, its correction before and its control-variate
-        update after (before any fold resets the replica).  With augmentation or mixing, the client's stream of this
-        round."""
+        update after (before any fold resets the replica).  With augmentation, mixing or dropout, the client's stream of
+        this round."""
         hp = self.hp
         if self.aug_hp is not None:
             hp = dict(hp, augment_stream=(self.n_rounds << 32) | int(cid), **self.aug_hp)

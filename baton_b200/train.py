@@ -166,8 +166,23 @@ def run_local_sgd(model: nn.Module, X: torch.Tensor, y: torch.Tensor, *, n_epoch
     max_grad_norm = check_max_grad_norm(max_grad_norm)
     adam = check_optimizer(optimizer, momentum, prox_mu=prox_mu)
     mixc = _mix_setup(mix, mix_alpha, label_smoothing, loss)
-    aug = _augment_setup(model.__dict__.setdefault("_augment_streams", AugmentStreams()), X, augment,
-                         augment_padding, augment_seed, augment_stream, mixc)
+    streams = model.__dict__.setdefault("_augment_streams", AugmentStreams())
+    aug = _augment_setup(streams, X, augment, augment_padding, augment_seed, augment_stream, mixc)
+    drop = _dropout_setup(model, streams, aug, augment_seed, augment_stream)
+    n = X.shape[0]
+    if drop is not None:
+        drop[0].begin(drop[1], drop[2], -(-n // batch_size), n_epoch, model.n_dropout_sites)
+    try:
+        return _run_local_sgd(model, X, y, n_epoch, lr, batch_size, momentum, weight_decay, verbose,
+                              reshuffle_each_epoch, generator, prox_mu, adam, betas, eps, mixc, aug, max_grad_norm,
+                              criterion, drop)
+    finally:
+        if drop is not None:
+            drop[0].end()
+
+
+def _run_local_sgd(model, X, y, n_epoch, lr, batch_size, momentum, weight_decay, verbose, reshuffle_each_epoch,
+                   generator, prox_mu, adam, betas, eps, mixc, aug, max_grad_norm, criterion, drop):
     n = X.shape[0]
     nn.Module.train(model, True)
     params = list(model.parameters())
@@ -188,6 +203,8 @@ def run_local_sgd(model: nn.Module, X: torch.Tensor, y: torch.Tensor, *, n_epoch
         batch_iter = EpochProgress(epoch, batches, verbose=verbose)
         for b, batch_idxs in enumerate(batch_iter):
             optimizer.zero_grad(set_to_none=True)
+            if drop is not None:
+                drop[0].at(epoch, b)
             xb = _host_batch(X, batch_idxs, aug, epoch, b * batch_size)
             target = y[batch_idxs]
             if mixc is not None:
@@ -218,6 +235,17 @@ def _augment_setup(streams: AugmentStreams, X, augment, augment_padding, augment
         check_shard(cfg, X)
     check_mix_shard(mix, X)
     return (cfg,) + streams.next(augment_seed, augment_stream)
+
+
+def _dropout_setup(model, streams: AugmentStreams, aug, augment_seed, augment_stream):
+    """``(run, key, stream)`` of a run of a model with a nonzero dropout probability (``data/dropout.py``), or None.
+    Dropout draws from the augmentation key and stream: those of ``aug`` when the run augments or mixes, else the
+    next of ``streams``."""
+    run = getattr(model, "dropout_run", None)
+    if run is None or not getattr(model, "has_dropout", False):
+        return None
+    key, stream = aug[1:] if aug is not None else streams.next(augment_seed, augment_stream)
+    return run, key, stream
 
 
 def _mix_setup(mix, mix_alpha, label_smoothing, loss):
@@ -369,6 +397,7 @@ class GraphedLocalSGD:
         self._aug_streams = AugmentStreams()
         self._aug_table = None        # device [epochs, 3] per-epoch words of augmenting runs (see _aug_words)
         self._mix = None              # MixConfig of the current run (mixing and / or label smoothing) or None
+        self._drop = None             # dropout of the current run: (DropoutRun, key, stream) or None
         self.clip = False             # gradient-norm clipping: each step runs the norm kernel, then a clipped optimizer
         self.max_norm = torch.zeros(1, dtype=torch.float32, device=dev)   # its threshold, read by the norm kernel
         self._max_norm_host = None
@@ -417,6 +446,8 @@ class GraphedLocalSGD:
         clipping on, the device scalar this step writes its pre-clip gradient norm to."""
         F = self.F
         xb, yb = batch if batch is not None else self._gather(X, y, idx, s0, words, mix_rows, bsz)
+        if self._drop is not None:
+            self._drop[0].at(0, s0 // bsz, words)       # the kernels read the epoch from `words`
         mix = None
         if self._mix is not None:
             mix = (mix_rows[s0 // bsz] if mix_rows is not None else None, self._mix.smoothing)
@@ -534,7 +565,8 @@ class GraphedLocalSGD:
         gather reads the entry's word buffer ``words``; with mixing on, the entry's ``[steps, 8]`` mix rows ``mix``.
         With clipping on, captured step ``s`` writes its gradient norm to ``norms[s]`` of the entry."""
         perm = torch.zeros(n_steps * batch_size, dtype=torch.int64, device=self.device)
-        words = torch.zeros(3, dtype=torch.int32, device=self.device) if self._aug is not None else None
+        words = (torch.zeros(3, dtype=torch.int32, device=self.device)
+                 if self._aug is not None or self._drop is not None else None)
         mixbuf = (torch.zeros(steps, MIX_ROW, dtype=torch.int32, device=self.device)
                   if self._mix is not None and self._mix.kind is not None else None)
         norms = torch.zeros(steps, dtype=torch.float32, device=self.device) if self.clip else None
@@ -564,7 +596,7 @@ class GraphedLocalSGD:
                 self._step(X, y, None, batch=(Xp[s * batch_size:(s + 1) * batch_size],
                                               yp[s * batch_size:(s + 1) * batch_size]),
                            emit_wire=(s == n_steps - 1 and self.pack is not None),
-                           row=rows[s] if rows is not None else None, s0=s * batch_size, mix_rows=mixbuf,
+                           row=rows[s] if rows is not None else None, s0=s * batch_size, words=words, mix_rows=mixbuf,
                            bsz=batch_size, norm=norms[s:s + 1] if norms is not None else None)
             self.graph_emits_wire = self.pack is not None
 
@@ -730,12 +762,26 @@ class GraphedLocalSGD:
         self._mix = _mix_setup(mix, mix_alpha, label_smoothing, self.loss_kind)
         self._aug = _augment_setup(self._aug_streams, X, augment, augment_padding, augment_seed, augment_stream,
                                    self._mix)
-        nn.Module.train(self.model, True)
+        self._drop = _dropout_setup(self.model, self._aug_streams, self._aug, augment_seed, augment_stream)
         n = X.shape[0]
         batch_size = min(batch_size, n)
         n_steps = n // batch_size
         tail = n - n_steps * batch_size
         steps = n_steps + (1 if tail else 0)
+        if self._drop is None:
+            return self._run(X, y, n_epoch, lr, batch_size, momentum, weight_decay, reshuffle_each_epoch, return_device,
+                             prox_mu, corr, betas, eps, max_grad_norm, n, n_steps, tail, steps)
+        run, key, stream = self._drop
+        run.begin(key, stream, steps, n_epoch, self.model.n_dropout_sites)
+        try:
+            return self._run(X, y, n_epoch, lr, batch_size, momentum, weight_decay, reshuffle_each_epoch, return_device,
+                             prox_mu, corr, betas, eps, max_grad_norm, n, n_steps, tail, steps)
+        finally:
+            run.end()
+
+    def _run(self, X, y, n_epoch, lr, batch_size, momentum, weight_decay, reshuffle_each_epoch, return_device, prox_mu,
+             corr, betas, eps, max_grad_norm, n, n_steps, tail, steps):
+        nn.Module.train(self.model, True)
         self._set_hyper(lr, momentum, weight_decay, prox_mu=prox_mu)
         self.prox = prox_mu > 0
         self.corr = corr
@@ -748,15 +794,17 @@ class GraphedLocalSGD:
             self.arena.adam_v = torch.zeros_like(self.arena.grad)
         # every step of the run, t = 1 .. n_epoch * steps; the first ignores the stored moments (a fresh optimizer)
         table = self._adam_rows(lr, betas, eps, weight_decay, n_epoch, steps) if self.adam else None
-        aug_words = self._aug_words(self._aug[2], n_epoch) if self._aug is not None else None
+        stream = self._aug[2] if self._aug is not None else (self._drop[2] if self._drop is not None else None)
+        aug_words = self._aug_words(stream, n_epoch) if stream is not None else None
         aug_key = self._aug[:2] if self._aug is not None else None
+        drop_key = self._drop[1] if self._drop is not None else None      # baked into the captured dropout kernels
         mixing = self._mix is not None and self._mix.kind is not None
         mix_table_dev = self._mix_rows(n_epoch, steps, X) if mixing else None
         mix_key = (mixing, self._mix.smoothing) if self._mix is not None else None
         # the anchor and correction pointers are baked into the captured launches; the coefficient is read from `hyper`
         # at replay
         key = (n, batch_size, tuple(X.shape[1:]), tuple(y.shape[1:]), X.data_ptr(), y.data_ptr(), bool(momentum),
-               self.prox, corr.data_ptr() if corr is not None else None, self.adam, aug_key, mix_key, self.clip)
+               self.prox, corr.data_ptr() if corr is not None else None, self.adam, aug_key, mix_key, self.clip, drop_key)
         epoch_losses = torch.zeros(n_epoch, 2, dtype=torch.float32, device=self.device)
         grad_norms = torch.zeros(n_epoch, steps, dtype=torch.float32, device=self.device) if self.clip else None
         if self.use_graph:
@@ -856,8 +904,21 @@ class PortableLocalSGD:
         adam = check_optimizer(optimizer, momentum, prox_mu=prox_mu, corr=corr)
         mixc = _mix_setup(mix, mix_alpha, label_smoothing, self.loss_kind)
         aug = _augment_setup(self._aug_streams, X, augment, augment_padding, augment_seed, augment_stream, mixc)
+        drop = _dropout_setup(self.model, self._aug_streams, aug, augment_seed, augment_stream)
         n = X.shape[0]
         batch_size = min(batch_size, n)
+        if drop is not None:
+            drop[0].begin(drop[1], drop[2], -(-n // batch_size), n_epoch, self.model.n_dropout_sites)
+        try:
+            return self._run(X, y, n_epoch, lr, batch_size, momentum, weight_decay, reshuffle_each_epoch,
+                             return_device, prox_mu, corr, betas, eps, max_grad_norm, criterion, adam, mixc, aug, drop)
+        finally:
+            if drop is not None:
+                drop[0].end()
+
+    def _run(self, X, y, n_epoch, lr, batch_size, momentum, weight_decay, reshuffle_each_epoch, return_device, prox_mu,
+             corr, betas, eps, max_grad_norm, criterion, adam, mixc, aug, drop):
+        n = X.shape[0]
         nn.Module.train(self.model, True)
         a = self.arena
         if prox_mu > 0 and a.global_w is None:
@@ -884,6 +945,8 @@ class PortableLocalSGD:
             rows = _host_mix_rows(mixc, aug, X, e, steps)
             for b, idx in enumerate(batches):
                 opt.zero_grad(set_to_none=True)
+                if drop is not None:
+                    drop[0].at(e, b)
                 xb = _host_batch(X, idx, aug, e, b * batch_size)
                 tgt = y[idx]
                 if mixc is not None:

@@ -23,7 +23,7 @@ from typing import Callable, Dict, List, Tuple
 import torch
 
 _TUS = ["?", "gemm_wgmma", "gemm_fp8", "quant", "attention", "im2col_tma", "gemm_simt", "fedavg", "elementwise",
-        "conv", "norm", "loss", "conv_halo"]
+        "conv", "norm", "loss", "conv_halo", "dropout"]
 _CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "csrc")
 _NAME_CACHE: Dict[int, str] = {}
 
