@@ -295,6 +295,31 @@ bool conv_halo(const at::Tensor& src, const at::Tensor& w, at::Tensor out, int64
   check(rc, "conv_halo");
   return true;
 }
+// the same convolution from whole small images in shared memory (layer3 of ResNet-18 at 32x32: 2x2 maps), `bn` = 32
+// or 64 output columns per CTA; false = shape not supported by the kernel
+bool conv_smallmap(const at::Tensor& src, const at::Tensor& w, at::Tensor out, int64_t stride, bool dgrad, int64_t mc,
+                   int64_t bn, const std::optional<at::Tensor>& col_stats) {
+  CHECK_CUDA(src); CHECK_CUDA(w); CHECK_CUDA(out);
+  TORCH_CHECK(src.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16 && out.scalar_type() == at::kBFloat16 &&
+              src.dim() == 4 && src.is_contiguous() && w.is_contiguous() && out.is_contiguous());
+  TORCH_CHECK(stride == 1 || stride == 2, "conv_smallmap: stride 1 or 2");
+  const int64_t c = src.size(3);
+  const int64_t rows = src.size(0) * ((src.size(1) - 1) / stride + 1) * ((src.size(2) - 1) / stride + 1);
+  TORCH_CHECK(rows > 0 && out.numel() % rows == 0, "conv_smallmap: out must hold [N*Ho*Wo, Nout] elements");
+  const int64_t nout = out.numel() / rows;
+  TORCH_CHECK(w.numel() == (dgrad ? c * 9 * nout : nout * 9 * c), "conv_smallmap: w must be [Cout, 9*Cin]");
+  TORCH_CHECK(dgrad ? !col_stats.has_value()
+                    : (!col_stats.has_value() || (col_stats->scalar_type() == at::kFloat && col_stats->numel() >= 2 * nout)),
+              "conv_smallmap: col_stats is a [2 Cout] fp32 buffer of the forward");
+  const c10::cuda::CUDAGuard guard(src.device());
+  const int rc = b200_conv_smallmap(cptr(src), cptr(w), ptr(out), static_cast<int>(src.size(0)),
+                                    static_cast<int>(src.size(1)), static_cast<int>(src.size(2)), static_cast<int>(c),
+                                    static_cast<int>(nout), static_cast<int>(stride), dgrad ? 1 : 0, static_cast<int>(mc),
+                                    static_cast<int>(bn), opt_ptr<float>(col_stats), cur_stream());
+  if (rc == -2) return false;
+  check(rc, "conv_smallmap");
+  return true;
+}
 // stride 2: `ntaps` (4) taps per parity class, `taps` (4 x 4) packed tap words (ops/functional.py conv_s2_dgrad_taps)
 bool conv_igemm_dgrad_s2(const at::Tensor& dy, const at::Tensor& w, at::Tensor dx, int64_t kh, int64_t kw,
                          const std::vector<int64_t>& ntaps, const std::vector<int64_t>& taps, int64_t force_bn) {
@@ -1527,6 +1552,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("conv_igemm_dgrad", &conv_igemm_dgrad);
   m.def("conv_igemm_dgrad_s2", &conv_igemm_dgrad_s2);
   m.def("conv_halo", &conv_halo);
+  m.def("conv_smallmap", &conv_smallmap);
   m.def("gemm_batched", &gemm_batched);
   m.def("gemm_fp8", &gemm_fp8);
   m.def("quant_mx_rows", &quant_mx_rows);

@@ -1126,9 +1126,10 @@ static EncodeTiledFn get_encode_fn() {
 }
 
 // 2-D bf16 tensor map over a row-major [rows, cols] matrix with row pitch `ld` elements;
-// box = [box_cols (inner), box_rows], 128B swizzle (box_cols must be 64).
+// box = [box_cols (inner), box_rows], 128B swizzle (box_cols must be 64) unless `swizzle` is another mode (its span
+// bounds box_cols).
 static int make_map(CUtensorMap* map, const void* base, long long rows, long long cols, long long ld, int box_cols,
-                    int box_rows) {
+                    int box_rows, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   EncodeTiledFn fn = get_encode_fn();
   if (fn == nullptr) return -1;
   cuuint64_t gdim[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
@@ -1136,7 +1137,7 @@ static int make_map(CUtensorMap* map, const void* base, long long rows, long lon
   cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstr, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : static_cast<int>(r);
 }
@@ -1296,6 +1297,12 @@ static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const GemmPa
 extern "C" int b200_encode_map2_bf16(void* map, const void* base, long long rows, long long cols, long long ld,
                                      int box_cols, int box_rows) {
   return b200::make_map(reinterpret_cast<CUtensorMap*>(map), base, rows, cols, ld, box_cols, box_rows);
+}
+// the same with a 64-byte swizzle (conv_halo.cu: the MN-major [64 cout] x [32 cin] weight slab of a 32-column tile)
+extern "C" int b200_encode_map2_sw64_bf16(void* map, const void* base, long long rows, long long cols, long long ld,
+                                          int box_cols, int box_rows) {
+  return b200::make_map(reinterpret_cast<CUtensorMap*>(map), base, rows, cols, ld, box_cols, box_rows,
+                        CU_TENSOR_MAP_SWIZZLE_64B);
 }
 extern "C" int b200_encode_map4_bf16(void* map, const void* base, long long rows, long long cols, long long ld,
                                      long long inner, long long s_inner, long long outer, long long s_outer,

@@ -78,6 +78,10 @@ int b200_conv_igemm_wgrad(const void* dy, const void* x, float* dw, int N, int H
 // C = 64 (stride 2, forward only); dgrad != 0: input gradient
 int b200_conv_halo(const void* src, const void* w, void* out, int N, int H, int W, int C, int Nout, int stride,
                    int dgrad, int mc, float* col_stats, cudaStream_t stream);
+// the same kernel from whole small images in shared memory (no halo), bn = 32 or 64 output columns per CTA, over
+// C = 256 (stride 1) or C = 128 (stride 2, forward only) gathered channels
+int b200_conv_smallmap(const void* src, const void* w, void* out, int N, int H, int W, int C, int Nout, int stride,
+                       int dgrad, int mc, int bn, float* col_stats, cudaStream_t stream);
 // ---- im2col_tma.cu (experimental: TMA im2col tensor maps, probe kernel only)
 int b200_im2col_tma_probe(const void* x, void* col, int N, int H, int W, int C, int KH, int KW, int stride, int pad,
                           int Ho, int Wo, cudaStream_t stream);

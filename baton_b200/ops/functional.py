@@ -609,13 +609,45 @@ def halo_cluster(m_rows: int) -> int:
     return 4 if tiles % 4 == 0 else 2 if tiles % 2 == 0 else 1
 
 
-def _conv_path(path: Optional[str], eligible: bool) -> str:
+_SMALLMAP_FORMS = ((1, 256), (2, 128))   # (stride, gathered channels) of conv_smallmap; stride 2: forward only
+SMALLMAP_BN = 32                          # output columns of one image-tile CTA: all 36 weight k-tiles fit
+
+
+def smallmap_smem_bytes(h: int, w: int, c: int = 256, stride: int = 1, bn: int = SMALLMAP_BN) -> int:
+    """Shared memory of the image-tile kernel over an ``h x w`` input of ``c`` gathered channels at ``stride``:
+    ``c / 64`` boxes of the ``64 / (ho wo)`` whole input images (no halo; each rounded up to 1 KB), ``9 c / 64``
+    weight slots of ``bn x 64`` bf16, one mbarrier per slot plus one for the images (padded to a multiple of 16),
+    column statistics, the 128-byte zero line of the out-of-image taps and the 1 KB realignment (conv_halo.cu
+    halo_fixed_bytes)."""
+    ho, wo = conv_out_size(h, 3, stride, 1), conv_out_size(w, 3, stride, 1)
+    box = (HALO_BM // (ho * wo)) * h * w * 128
+    k_tiles = 9 * (c // 64)
+    return (c // 64 * round_up(box, 1024) + k_tiles * bn * 128 + round_up(1 + k_tiles, 16) * 8 + 4 * bn * 4 + 128
+            + 1024)
+
+
+def smallmap_eligible(kh: int, kw: int, stride: int, pad: int, c: int, h: int, w: int,
+                      affine: Optional[dict] = None, dgrad: bool = False) -> bool:
+    """Whether the image-tile kernel (``conv_smallmap``) takes a convolution over an ``h x w`` input: 3x3, pad 1, a
+    (stride, gathered channels) form of ``_SMALLMAP_FORMS`` -- stride 1 over 256 channels of the gathered tensor
+    (``x`` forward, ``dy`` dgrad) or stride 2 over a 128-channel ``x`` (forward only) --, a 64-row tile holds whole
+    output images, the images and the weight slots fit in shared memory, and no eval-mode ``affine`` epilogue."""
+    if kh != 3 or kw != 3 or pad != 1 or (stride, c) not in _SMALLMAP_FORMS or (dgrad and stride != 1):
+        return False
+    hw = conv_out_size(h, 3, stride, 1) * conv_out_size(w, 3, stride, 1)
+    return (hw <= HALO_BM and HALO_BM % hw == 0 and affine is None and
+            smallmap_smem_bytes(h, w, c, stride) <= _HALO_MAX_SMEM)
+
+
+def _conv_path(path: Optional[str], eligible: bool, smallmap: bool = False) -> str:
     if path is None:
-        return "halo" if eligible else "im2col"
-    if path not in ("halo", "im2col"):
-        raise ValueError("path must be None, 'halo' or 'im2col', not {!r}".format(path))
+        return "halo" if eligible else "smallmap" if smallmap else "im2col"
+    if path not in ("halo", "smallmap", "im2col"):
+        raise ValueError("path must be None, 'halo', 'smallmap' or 'im2col', not {!r}".format(path))
     if path == "halo" and not eligible:
         raise ValueError("the halo kernel does not take this convolution (see halo_eligible)")
+    if path == "smallmap" and not smallmap:
+        raise ValueError("the image-tile kernel does not take this convolution (see smallmap_eligible)")
     return path
 
 
@@ -623,16 +655,17 @@ def conv_igemm_fwd(x: torch.Tensor, w2d: torch.Tensor, kh: int, kw: int, stride:
                    col_stats: Optional[torch.Tensor] = None, affine: Optional[dict] = None,
                    cluster_k: Optional[int] = None, force_bn: int = 0,
                    out: Optional[torch.Tensor] = None, path: Optional[str] = None,
-                   mc: Optional[int] = None) -> Optional[torch.Tensor]:
+                   mc: Optional[int] = None, bn: int = SMALLMAP_BN) -> Optional[torch.Tensor]:
     """Implicit-GEMM convolution forward: ``y[N*Ho*Wo, Cout]`` straight from NHWC ``x`` through TMA
     im2col loads (no ``col`` buffer).  ``w2d``: ``[Cout, kh*kw*Cin]`` channels_last weights.  ``affine``: eval-mode
     BatchNorm epilogue as in :func:`gemm`.  ``out``: contiguous bf16 ``[N*Ho*Wo, Cout]`` to write.  Returns ``None``
     when the shape (or the epilogue) is not supported (Cin % 64 != 0).
 
-    ``path``: ``None`` takes the halo-tiled kernel whenever :func:`halo_eligible` holds and the im2col-mode kernel
-    otherwise; ``"halo"`` / ``"im2col"`` force one (``"halo"`` on a shape the halo kernel does not take raises).
-    ``mc``: cluster size of the halo kernel (default :func:`halo_cluster`); ``cluster_k`` / ``force_bn`` apply to
-    the im2col path."""
+    ``path``: ``None`` takes the halo-tiled kernel whenever :func:`halo_eligible` holds, else the image-tile kernel
+    whenever :func:`smallmap_eligible` holds, else the im2col-mode kernel; ``"halo"`` / ``"smallmap"`` /
+    ``"im2col"`` force one (``"halo"`` or ``"smallmap"`` on a shape that kernel does not take raises).
+    ``mc``: cluster size of the halo and image-tile kernels (default :func:`halo_cluster`); ``bn``: output columns
+    per image-tile CTA (32, or 64 at the stride-2 form); ``cluster_k`` / ``force_bn`` apply to the im2col path."""
     n, h, w, c = x.shape
     cout = w2d.shape[0]
     if c % 64 or w2d.shape[1] != kh * kw * c or not x.is_contiguous() or not w2d.is_contiguous():
@@ -640,10 +673,17 @@ def conv_igemm_fwd(x: torch.Tensor, w2d: torch.Tensor, kh: int, kw: int, stride:
     ho, wo = conv_out_size(h, kh, stride, pad), conv_out_size(w, kw, stride, pad)
     M, K = n * ho * wo, kh * kw * c
     halo = halo_eligible(kh, kw, stride, pad, c, h, w, affine) and cout % 8 == 0
-    if _conv_path(path, halo) == "halo":
+    small = smallmap_eligible(kh, kw, stride, pad, c, h, w, affine) and cout % bn == 0
+    kind = _conv_path(path, halo, small)
+    if kind == "halo":
         y = out if out is not None else torch.empty((M, cout), dtype=BF16, device=x.device)
         if not load().conv_halo(x, w2d, y, stride, False, mc or halo_cluster(M), col_stats):
             raise RuntimeError("conv_halo declined a convolution halo_eligible admits")
+        return y
+    if kind == "smallmap":
+        y = out if out is not None else torch.empty((M, cout), dtype=BF16, device=x.device)
+        if not load().conv_smallmap(x, w2d, y, stride, False, mc or halo_cluster(M), bn, col_stats):
+            raise RuntimeError("conv_smallmap declined a convolution smallmap_eligible admits")
         return y
     bn = force_bn or pick_bn(M, cout)
     if cluster_k is None:
@@ -696,16 +736,23 @@ def conv_igemm_dgrad(dy: torch.Tensor, w2d: torch.Tensor, in_shape, kh: int, kw:
     convolution of ``dy``.  Stride 2: one launch over the four parity classes of :func:`conv_s2_dgrad_taps`.
     ``out``: contiguous bf16 ``[N, H, W, Cin]`` to write (every element is written).  Returns ``None`` when the shape
     is not supported (channels not multiples of 64, other strides).  ``path`` / ``mc``: as in :func:`conv_igemm_fwd`
-    (the halo kernel gathers ``dy``, so ``Cout`` is what its rule checks).  ``cluster_k``: cluster split-K of the
-    stride-1 im2col path (default :func:`pick_cluster_k`)."""
+    (the halo and image-tile kernels gather ``dy``, so ``Cout`` is what their rules check).  ``cluster_k``: cluster
+    split-K of the stride-1 im2col path (default :func:`pick_cluster_k`)."""
     n, h, w, c = in_shape
     cout = dy.shape[-1]
     if c % 64 or cout % 64 or w2d.shape[1] != kh * kw * c or not dy.is_contiguous() or not w2d.is_contiguous():
         return None
-    if _conv_path(path, halo_eligible(kh, kw, stride, pad, cout, h, w, dgrad=True)) == "halo":
+    kind = _conv_path(path, halo_eligible(kh, kw, stride, pad, cout, h, w, dgrad=True),
+                      smallmap_eligible(kh, kw, stride, pad, cout, h, w, dgrad=True) and c % SMALLMAP_BN == 0)
+    if kind == "halo":
         dx = out if out is not None else torch.empty((n, h, w, c), dtype=BF16, device=dy.device)
         if not load().conv_halo(dy, w2d, dx, 1, True, mc or halo_cluster(n * h * w), None):
             raise RuntimeError("conv_halo declined a convolution halo_eligible admits")
+        return dx
+    if kind == "smallmap":
+        dx = out if out is not None else torch.empty((n, h, w, c), dtype=BF16, device=dy.device)
+        if not load().conv_smallmap(dy, w2d, dx, 1, True, mc or halo_cluster(n * h * w), SMALLMAP_BN, None):
+            raise RuntimeError("conv_smallmap declined a convolution smallmap_eligible admits")
         return dx
     if stride == 1:
         M, K = n * h * w, kh * kw * cout
