@@ -39,6 +39,10 @@ class FederationConfig:
     label_smoothing: float = 0.0       # soft-target smoothing eps in [0, 1) of the training cross-entropy
     max_grad_norm: float = 0.0         # clip_grad_norm_ of every local step's gradient to this 2-norm (0: off)
     dropout: float = 0.0               # BERT: hidden and attention-probability dropout (the classifier follows hidden)
+    lora_r: int = 0                    # BERT: LoRA rank, 8 | 16 | 32 | 64 (0: full fine-tuning)
+    lora_alpha: float = 16.0           # LoRA scale alpha / r
+    lora_targets: str = "query,value"  # comma-separated subset of query, key, value, attn_out, ffn_in, ffn_out
+    lora_freeze_a: bool = False        # FFA-LoRA: A stays frozen, only B and the classifier train
     dp_clip: float = 0.0               # DP-FedAvg: L2 clip norm of a client's update (0: DP off)
     dp_noise_multiplier: float = 0.0   # DP-FedAvg: noise std on the sum of clipped updates, in units of dp_clip
     dp_delta: float = 1e-5             # DP-FedAvg: delta of the (epsilon, delta) the manager reports
@@ -76,6 +80,10 @@ class FederationConfig:
         check_dropout(self.dropout, "dropout")
         if self.dropout > 0.0 and self.model != "bert_base":
             raise ValueError("dropout applies to the BERT models only, not {!r}".format(self.model))
+        if self.lora_r:
+            if self.model != "bert_base":
+                raise ValueError("LoRA applies to bert_base only, not {!r}".format(self.model))
+            self.lora_config()
         from .parallel.dp import check_dp
         check_dp(self.dp_clip, self.dp_noise_multiplier)
         if not (0.0 < float(self.dp_delta) < 1.0):
@@ -92,7 +100,15 @@ class FederationConfig:
         check_features(dp=float(self.dp_clip) > 0.0, robust=self.aggregator != "mean",
                        server_opt=self.server_opt != "none",
                        plane="seated" if self.backend in ("fused", "nccl") else "http", optimizer=self.optimizer,
-                       momentum=self.momentum, prox_mu=float(self.prox_mu))
+                       momentum=self.momentum, prox_mu=float(self.prox_mu), frozen=bool(self.lora_r))
+
+    def lora_config(self):
+        """The :class:`~baton_b200.models.bert.LoraConfig` of these fields, or None (``lora_r == 0``)."""
+        if not self.lora_r:
+            return None
+        from .models.bert import LoraConfig
+        return LoraConfig(self.lora_r, self.lora_alpha, tuple(t.strip() for t in self.lora_targets.split(",")),
+                          self.lora_freeze_a)
 
     def train_kwargs(self) -> dict:
         """Local-training keyword arguments of a worker (``FederatedModule.local_train``)."""
@@ -154,6 +170,8 @@ class FederationConfig:
                 typ = float
             if f.name in ("checkpoint_dir",):
                 typ = str
+            if typ is bool:
+                typ = lambda v: v.lower() in ("1", "true", "yes")    # noqa: E731
             parser.add_argument(flag, dest=f.name, type=typ, default=default)
 
     @classmethod

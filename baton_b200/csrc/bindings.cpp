@@ -1534,12 +1534,69 @@ void mse(const at::Tensor& pred, const at::Tensor& target, const std::optional<a
         "mse");
 }
 
+// ---- LoRA (csrc/lora.cu, the LoRA epilogue of csrc/gemm_wgmma.cu): shapes, strides and offsets come from ops/functional.py
+static void check_bf16(const at::Tensor& t, const char* what) {
+  CHECK_CUDA(t);
+  TORCH_CHECK(t.scalar_type() == at::kBFloat16, what, " must be bf16");
+}
+
+void gemm_lora(const at::Tensor& a, const at::Tensor& b, at::Tensor d, const std::optional<at::Tensor>& bias, int64_t M,
+               int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldd, bool a_mn, bool b_mn, int64_t act,
+               double alpha, const at::Tensor& u, int64_t ldu, const at::Tensor& f, int64_t fs_n, int64_t fs_j, int64_t R,
+               int64_t rs, int64_t ds, const std::vector<int64_t>& slot, double s) {
+  check_bf16(a, "gemm_lora a"); check_bf16(b, "gemm_lora b"); check_bf16(u, "gemm_lora u"); check_bf16(f, "gemm_lora f");
+  CHECK_CUDA(d);
+  TORCH_CHECK(d.scalar_type() == at::kBFloat16 || d.scalar_type() == at::kFloat, "gemm_lora output must be bf16/fp32");
+  TORCH_CHECK(slot.size() == 3, "gemm_lora: three slice slots");
+  const c10::cuda::CUDAGuard guard(a.device());
+  B200LoraEpilogue l = {};
+  l.u = u.data_ptr(); l.ldu = ldu; l.f = f.data_ptr(); l.fs_n = fs_n; l.fs_j = fs_j;
+  l.R = static_cast<int>(R); l.rs = static_cast<int>(rs); l.ds = static_cast<int>(ds);
+  for (int i = 0; i < 3; ++i) l.slot[i] = static_cast<int>(slot[i]);
+  l.s = static_cast<float>(s);
+  check(b200_gemm_bf16_lora(cptr(a), cptr(b), ptr(d), opt_ptr<const float>(bias), M, N, K, lda, ldb, ldd, a_mn, b_mn,
+                            d.scalar_type() == at::kFloat, static_cast<int>(act), static_cast<float>(alpha), &l,
+                            cur_stream()),
+        "gemm_bf16_lora");
+}
+
+void lora_down(const at::Tensor& x, int64_t ldx, const at::Tensor& w, int64_t w_ts, int64_t wsj, int64_t wsk,
+               at::Tensor u, int64_t ldu, int64_t M, int64_t T, int64_t rs, int64_t kt, const std::vector<int64_t>& xoff) {
+  check_bf16(x, "lora_down x"); check_bf16(w, "lora_down w"); check_bf16(u, "lora_down u");
+  TORCH_CHECK(static_cast<int64_t>(xoff.size()) == T, "lora_down: one x offset per slice");
+  const c10::cuda::CUDAGuard guard(x.device());
+  std::vector<long long> xo(xoff.begin(), xoff.end());
+  check(b200_lora_down(cptr(x), ldx, cptr(w), w_ts, wsj, wsk, ptr(u), ldu, M, T, rs, kt, xo.data(), cur_stream()),
+        "lora_down");
+}
+
+void lora_grad(const at::Tensor& l, int64_t ldl, const at::Tensor& q, int64_t ldq, at::Tensor out, int64_t osa,
+               int64_t osb, int64_t out_ts, int64_t M, int64_t NA, int64_t NB, int64_t T, const std::vector<int64_t>& lo,
+               const std::vector<int64_t>& qo, double s, at::Tensor work) {
+  check_bf16(l, "lora_grad l"); check_bf16(q, "lora_grad q");
+  CHECK_CUDA(out); CHECK_CUDA(work);
+  TORCH_CHECK(out.scalar_type() == at::kFloat && work.scalar_type() == at::kFloat, "lora_grad: fp32 out and work");
+  TORCH_CHECK(static_cast<int64_t>(lo.size()) == T && static_cast<int64_t>(qo.size()) == T, "lora_grad: offsets per slice");
+  const int64_t splits = (M + B200_LORA_SPLIT_ROWS - 1) / B200_LORA_SPLIT_ROWS;
+  TORCH_CHECK(work.numel() >= T * splits * NA * NB, "lora_grad: work holds T * splits * NA * NB floats");
+  const c10::cuda::CUDAGuard guard(l.device());
+  std::vector<long long> lo_(lo.begin(), lo.end()), qo_(qo.begin(), qo.end());
+  check(b200_lora_grad(cptr(l), ldl, cptr(q), ldq, out.data_ptr<float>(), osa, osb, out_ts, M, NA, NB, T, lo_.data(),
+                       qo_.data(), static_cast<float>(s), work.data_ptr<float>(), cur_stream()),
+        "lora_grad");
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "baton_b200 sm_90a kernels";
   m.attr("MAX_RANKS") = B200_MAX_RANKS;
   m.def("gemm", &gemm);
+  m.def("gemm_lora", &gemm_lora);
+  m.def("lora_down", &lora_down);
+  m.def("lora_grad", &lora_grad);
+  m.attr("LORA_MAX_R") = B200_LORA_MAX_R;
+  m.attr("LORA_SPLIT_ROWS") = B200_LORA_SPLIT_ROWS;
   m.def("trace_set", &trace_set);
   m.def("attention_fwd", &attention_fwd);
   m.def("attention_bwd", &attention_bwd);

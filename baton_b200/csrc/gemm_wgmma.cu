@@ -101,6 +101,15 @@ struct GemmParams {
   // AdamW second moment of the optimizer epilogue, indexed like sgd_theta (sgd_mom is then the first moment and
   // sgd_hyper the step's AdamW row); nullptr: SGD
   float* sgd_v = nullptr;
+  // rank-R LoRA term of the LORA instantiation (see lora_chunk), added to the fp32 accumulator before alpha / bias / act
+  const __nv_bfloat16* lora_u = nullptr;     // [M, lora_ldu]: the down projection, ranks [0, lora_R)
+  const __nv_bfloat16* lora_f = nullptr;     // the up factor, element (row, j) at row * lora_fs_n + j * lora_fs_j
+  long long lora_ldu = 0, lora_fs_n = 0, lora_fs_j = 0;
+  int lora_R = 0;                            // ranks of U (multiple of 8, <= B200_LORA_MAX_R)
+  int lora_rs = 0;                           // ranks per slice (multiple of 8)
+  int lora_ds = 0;                           // columns per slice (multiple of 32)
+  int lora_slot[3] = {-1, -1, -1};           // slice -> its rank block t (U columns [t rs, t rs + rs)), -1: no term
+  float lora_s = 0.f;
 };
 
 // Wait until every arrival flag covering arena elements [e0, e1] has reached `need` (published by the FedAvg kernel with
@@ -460,6 +469,71 @@ __device__ __forceinline__ void s2_load_ktile(const CUtensorMap* tmA, const CUte
   for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * 8192, tmB, bar, wcol + j * 64, cb * 64);
 }
 
+// ---- LoRA epilogue (the LORA instantiation of the fixed-depth kernel) ----
+// Column n of slice sl = n / lora_ds with rank block t = lora_slot[sl] >= 0 receives
+//     lora_s * sum_{j < rs} U[m, t rs + j] * F(t ds + n - sl ds, j)
+// in fp32, j ascending, added to the accumulator (one fmaf) before alpha, bias and activation; the output is then
+// rounded once.  The CTA stages its 128 U rows ([128][R + 8] bf16) and the factor rows of its BN columns ([BN][rs + 8]
+// bf16, zero for columns of an untargeted slice or past N) behind the column-statistics area.
+__device__ __forceinline__ int lora_slot(const GemmParams& p, int sl) {
+  return sl == 0 ? p.lora_slot[0] : (sl == 1 ? p.lora_slot[1] : (sl == 2 ? p.lora_slot[2] : -1));
+}
+
+template <int BN>
+__device__ __forceinline__ void lora_stage(const GemmParams& p, __nv_bfloat16* us, __nv_bfloat16* fs, int m0, int n0) {
+  const int tid = static_cast<int>(threadIdx.x) - 128;
+  const int R = p.lora_R, up = R + 8, rs = p.lora_rs, fp = rs + 8;
+  const int vr = R / 8;      // 16-byte vectors per U row (host: R % 8 == 0, ldu % 8 == 0, 16-byte aligned U)
+  for (int i = tid; i < BM * vr; i += CONSUMER_THREADS) {
+    const int r = i / vr, c = (i - r * vr) * 8;
+    uint4 v = make_uint4(0u, 0u, 0u, 0u);
+    if (m0 + r < p.M) v = __ldg(reinterpret_cast<const uint4*>(p.lora_u + static_cast<size_t>(m0 + r) * p.lora_ldu + c));
+    *reinterpret_cast<uint4*>(us + r * up + c) = v;
+  }
+  for (int i = tid; i < BN * rs; i += CONSUMER_THREADS) {
+    const int j = i / BN, c = i - j * BN, n = n0 + c;
+    __nv_bfloat16 v = __float2bfloat16_rn(0.f);
+    if (n < p.N) {
+      const int sl = n / p.lora_ds, t = lora_slot(p, sl);
+      if (t >= 0)
+        v = p.lora_f[static_cast<long long>(t * p.lora_ds + n - sl * p.lora_ds) * p.lora_fs_n +
+                     static_cast<long long>(j) * p.lora_fs_j];
+    }
+    fs[c * fp + j] = v;
+  }
+}
+
+// the rank term of one 32-column row chunk: local row lrow, local columns [c, c + 32); lora_ds % 32 == 0, so the chunk
+// lies in one slice
+__device__ __forceinline__ void lora_chunk(const GemmParams& p, const __nv_bfloat16* us, const __nv_bfloat16* fs,
+                                           int lrow, int c, int col0, float (&v)[32]) {
+  const int t = lora_slot(p, col0 / p.lora_ds);      // warp-uniform
+  if (t < 0) return;
+  const int rs = p.lora_rs, fp = rs + 8;
+  const __nv_bfloat16* urow = us + lrow * (p.lora_R + 8) + t * rs;
+  float acc[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+#pragma unroll 1
+  for (int j = 0; j < rs; j += 8) {
+    const uint4 uv = *reinterpret_cast<const uint4*>(urow + j);
+    const float2 u0 = unpack_bf16x2(uv.x), u1 = unpack_bf16x2(uv.y), u2 = unpack_bf16x2(uv.z), u3 = unpack_bf16x2(uv.w);
+    const float u[8] = {u0.x, u0.y, u1.x, u1.y, u2.x, u2.y, u3.x, u3.y};
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {       // every lane reads the same factor row: one broadcast request
+      const uint4 fv = *reinterpret_cast<const uint4*>(fs + (c + i) * fp + j);
+      const float2 f0 = unpack_bf16x2(fv.x), f1 = unpack_bf16x2(fv.y), f2 = unpack_bf16x2(fv.z), f3 = unpack_bf16x2(fv.w);
+      float a = acc[i];
+      a = fmaf(u[0], f0.x, a); a = fmaf(u[1], f0.y, a); a = fmaf(u[2], f1.x, a); a = fmaf(u[3], f1.y, a);
+      a = fmaf(u[4], f2.x, a); a = fmaf(u[5], f2.y, a); a = fmaf(u[6], f3.x, a); a = fmaf(u[7], f3.y, a);
+      acc[i] = a;
+    }
+  }
+  const float s = p.lora_s;
+#pragma unroll
+  for (int i = 0; i < 32; ++i) v[i] = fmaf(s, acc[i], v[i]);
+}
+
 // ---- fixed-depth pipeline: the default path ----
 // CONV: 0 = plain GEMM; 1 = implicit-GEMM conv forward (A = im2col(x) gathered by TMA im2col, k-tile = one filter
 // tap x 64 input channels); 2 = implicit wgrad (B = im2col(x) MN-major, k-tile = 64 output pixels, every 64-wide
@@ -472,8 +546,9 @@ __device__ __forceinline__ void s2_load_ktile(const CUtensorMap* tmA, const CUte
 // PROX (with SGD): the FedProx form of that epilogue.  SCAF (with SGD): its SCAFFOLD form.  ADAM (with SGD): its
 // AdamW form (adamw_epilogue_chunk).
 // AFFINE: eval-mode BatchNorm epilogue instantiation (affine_chunk, forward convolutions in evaluation).
+// LORA: the rank-R LoRA term in the epilogue (lora_chunk; plain GEMM, single K pass).
 template <int BN, int STAGES, int CONV = 0, bool SGD = false, bool AFFINE = false, bool PROX = false, bool SCAF = false,
-          bool ADAM = false>
+          bool ADAM = false, bool LORA = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                          const GemmParams p) {
@@ -609,6 +684,9 @@ gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   } else if (warp >= 4) {
     // ===================== consumers: two warpgroups of wgmma, then the epilogue =====================
     const int ew = warp - 4;                    // 0..7
+    __nv_bfloat16* lora_us = reinterpret_cast<__nv_bfloat16*>(cstat + 8 * BN);
+    __nv_bfloat16* lora_fs = lora_us + BM * (p.lora_R + 8);
+    if constexpr (LORA) lora_stage<BN>(p, lora_us, lora_fs, m0, n0);   // read after the barriers below
     float acc[BN / 2];
     int s = 0;
     uint32_t ph = 0;
@@ -653,6 +731,7 @@ gemm_bf16_fixed_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
         if (want_stats) { sstat[c + lane_id()] = 0.f; sstat[BN + c + lane_id()] = 0.f; }
         continue;
       }
+      if constexpr (LORA) lora_chunk(p, lora_us, lora_fs, lrow, c, col0, v);
       if constexpr (AFFINE) {
         if (!row_ok) continue;
         affine_chunk<32>(p, row, col0, v);
@@ -1213,6 +1292,27 @@ static int launch_fixed_sgd(const CUtensorMap& ta, const CUtensorMap& tb, const 
                                  : launch_fixed<BN, STAGES, CONV, true>(ta, tb, p, grid, stream);
 }
 
+// the LoRA instantiation: its dynamic shared memory grows with the staged U and factor rows (lora_stage)
+template <int BN, int STAGES>
+static int launch_fixed_lora(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, dim3 grid,
+                             cudaStream_t stream) {
+  constexpr int base = STAGES * SmemLayout<BN>::STAGE_BYTES + 2 * STAGES * 8 + 8 * BN * 4 + 1024;
+  constexpr int cap = base + (BM + BN) * (B200_LORA_MAX_R + 8) * 2;
+  static_assert(cap <= 227 * 1024, "LoRA GEMM exceeds the 227 KB of shared memory a block may use");
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_fixed_kernel<BN, STAGES, 0, false, false, false, false, false, true>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
+    if (e != cudaSuccess) return static_cast<int>(e);
+    configured = true;
+  }
+  const int smem = base + (BM * (p.lora_R + 8) + BN * (p.lora_rs + 8)) * 2;
+  cudaError_t le = launch_pdl(gemm_bf16_fixed_kernel<BN, STAGES, 0, false, false, false, false, false, true>, grid,
+                              GEMM_THREADS, smem, stream, ta, tb, p);
+  if (le != cudaSuccess) return static_cast<int>(le);
+  return static_cast<int>(cudaGetLastError());
+}
+
 template <int BN, int STAGES>
 static int launch_persistent(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, int num_tiles,
                              cudaStream_t stream) {
@@ -1426,6 +1526,44 @@ extern "C" int b200_gemm_bf16(const void* a, const void* b, void* d, const float
   }
   if (bn == 128) return shallow ? launch_fixed<128, 3>(ta, tb, p, grid, stream) : launch_fixed<128, 6>(ta, tb, p, grid, stream);
   return shallow ? launch_fixed<64, 4>(ta, tb, p, grid, stream) : launch_fixed<64, 8>(ta, tb, p, grid, stream);
+}
+
+// D = act(alpha * (A B^T + s U F^T) + bias) with the LoRA term of B200LoraEpilogue (csrc/launch.h) in the epilogue of
+// the fixed-depth kernel, one K pass per CTA.  Operand conventions as b200_gemm_bf16; D is written, not accumulated.
+extern "C" int b200_gemm_bf16_lora(const void* a, const void* b, void* d, const float* bias, int M, int N, int K,
+                                   long long lda, long long ldb, long long ldd, int a_mn, int b_mn, int out_fp32,
+                                   int act, float alpha, const B200LoraEpilogue* lora, cudaStream_t stream) {
+  using namespace b200;
+  if (M <= 0 || N <= 0 || K <= 0) return 0;
+  if (lora == nullptr || lora->u == nullptr || lora->f == nullptr) return -3;
+  const B200LoraEpilogue& l = *lora;
+  if (l.R < 8 || l.R > B200_LORA_MAX_R || l.R % 8 || l.rs < 8 || l.rs % 8 || l.rs > l.R || l.ds < 32 || l.ds % 32 ||
+      N > 3 * l.ds || l.ldu < l.R || l.ldu % 8 || (reinterpret_cast<uintptr_t>(l.u) & 15))
+    return -3;
+  for (int i = 0; i < 3; ++i)
+    if (l.slot[i] < -1 || (l.slot[i] + 1) * l.rs > l.R) return -3;
+  if ((lda % 8) || (ldb % 8) || (reinterpret_cast<uintptr_t>(a) & 15) || (reinterpret_cast<uintptr_t>(b) & 15))
+    return -2;
+  const int bn = N > 64 ? 128 : 64;
+  CUtensorMap ta, tb;
+  int rc = !a_mn ? make_map(&ta, a, M, K, lda, BK, BM) : make_map(&ta, a, K, M, lda, 64, BK);
+  if (rc) return rc;
+  rc = !b_mn ? make_map(&tb, b, N, K, ldb, BK, bn) : make_map(&tb, b, K, N, ldb, 64, BK);
+  if (rc) return rc;
+  GemmParams p;
+  p.M = M; p.N = N; p.K = K; p.D = d; p.ldd = ldd; p.bias = bias; p.out_fp32 = out_fp32; p.act = act;
+  p.col_stats = nullptr; p.a_mn = a_mn; p.b_mn = b_mn; p.k_tiles_per_split = (K + BK - 1) / BK;
+  p.atomic_out = 0; p.cluster_k = 1; p.tile_flags = nullptr; p.flag_epoch = 0; p.flag_elem_off = 0;
+  p.flag_tile_elems = 0; p.flag_bias_off = -1; p.ldb = ldb; p.alpha = alpha; p.flag_epoch_ptr = nullptr;
+  p.batched = 0; p.batch_inner = 1; p.batch_count = 1; p.d_outer = 0; p.d_inner = 0;
+  p.lora_u = reinterpret_cast<const __nv_bfloat16*>(l.u); p.lora_f = reinterpret_cast<const __nv_bfloat16*>(l.f);
+  p.lora_ldu = l.ldu; p.lora_fs_n = l.fs_n; p.lora_fs_j = l.fs_j; p.lora_R = l.R; p.lora_rs = l.rs; p.lora_ds = l.ds;
+  for (int i = 0; i < 3; ++i) p.lora_slot[i] = l.slot[i];
+  p.lora_s = l.s;
+  dim3 grid((N + bn - 1) / bn, (M + BM - 1) / BM, 1);
+  if (bn == 128) { p.stages = 3; return launch_fixed_lora<128, 3>(ta, tb, p, grid, stream); }
+  p.stages = 4;
+  return launch_fixed_lora<64, 4>(ta, tb, p, grid, stream);
 }
 
 // Strided-batched GEMM (attention): for z = outer * n_inner + inner

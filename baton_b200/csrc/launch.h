@@ -39,6 +39,40 @@ struct B200AffineEpilogue {
 };
 #define B200_AFFINE_EPILOGUE_DECLINED (-7)
 
+// LoRA term of a bf16 GEMM (b200_gemm_bf16_lora, csrc/lora.cu): D = act(alpha * (A B^T + s T) + bias) with
+//     T[m, n] = sum_{j < rs} U[m, t rs + j] * F(t ds + n - sl ds, j),   sl = n / ds, t = slot[sl] (-1: T = 0),
+// F(row, j) = f[row * fs_n + j * fs_j].  The forward passes U = X A^T and F = the stacked B of the targeted slices
+// (fs_n = rs, fs_j = 1); the data gradient U = V = dY' B and F = A^T (one slice, rs = R, fs_n = 1, fs_j = K).
+// R = columns of U in use (multiple of 8, <= B200_LORA_MAX_R), ldu % 8 == 0, U 16-byte aligned, ds % 32 == 0,
+// N <= 3 ds; -3 otherwise.
+#define B200_LORA_MAX_R 192
+struct B200LoraEpilogue {
+  const void* u;                    // bf16 [M, ldu]
+  long long ldu;
+  const void* f;                    // bf16 up factor
+  long long fs_n, fs_j;
+  int R, rs, ds;
+  int slot[3];
+  float s;
+};
+int b200_gemm_bf16_lora(const void* a, const void* b, void* d, const float* bias, int M, int N, int K, long long lda,
+                        long long ldb, long long ldd, int a_mn, int b_mn, int out_fp32, int act, float alpha,
+                        const B200LoraEpilogue* lora, cudaStream_t stream);
+// LoRA down projection (csrc/lora.cu): for each of the T <= 3 slices t and j < rs, k over [0, kt)
+//     U[m, t rs + j] = bf16( sum_k X[m, xoff[t] + k] * W[t w_ts + j wsj + k wsk] )      (fp32 accumulation, k ascending)
+// forward: T = 1, W = A [R, K] (wsj = K, wsk = 1); backward V = dY' B: xoff[t] = the slice's first column, kt = its width,
+// W = the stacked B [T ds, r] (w_ts = ds r, wsj = 1, wsk = r).  rs % 8 == 0, T rs <= B200_LORA_MAX_R.
+int b200_lora_down(const void* x, long long ldx, const void* w, long long w_ts, long long wsj, long long wsk, void* u,
+                   long long ldu, int M, int T, int rs, int kt, const long long* xoff, cudaStream_t stream);
+// LoRA adapter gradient (csrc/lora.cu): for each slice t < T, a < NA, b < NB
+//     out[t out_ts + a osa + b osb] += s * sum_m L[m, lo[t] + a] * Q[m, qo[t] + b]
+// over M in a fixed split of B200_LORA_SPLIT_ROWS rows per partial (work: T * ceil(M / rows) * NA * NB floats), the
+// partials summed in split order by a second kernel: the bits depend on the shapes only.
+#define B200_LORA_SPLIT_ROWS 256
+int b200_lora_grad(const void* l, long long ldl, const void* q, long long ldq, float* out, long long osa, long long osb,
+                   long long out_ts, int M, int NA, int NB, int T, const long long* lo, const long long* qo, float s,
+                   float* work, cudaStream_t stream);
+
 // ---- gemm_wgmma.cu
 // sgd != nullptr: optimizer epilogue (accumulate, fp32 D, MN-major operands, single K pass on the fixed-depth kernel)
 // affine != nullptr: eval-mode BatchNorm epilogue (bf16 D, act 0, no bias / split-K partials; fixed or cluster kernel)

@@ -8,7 +8,7 @@ def __getattr__(name):
     if name in ("ResNet", "resnet18", "resnet50"):
         from . import resnet
         return getattr(resnet, name)
-    if name in ("BertConfig", "BertForSequenceClassification", "bert_base", "bert_tiny"):
+    if name in ("BertConfig", "BertForSequenceClassification", "LoraConfig", "bert_base", "bert_tiny"):
         from . import bert
         return getattr(bert, name)
     raise AttributeError(name)

@@ -27,6 +27,42 @@ from ..ops import nn as bnn
 from .base import FederatedModule
 
 
+LORA_TARGETS = ("query", "key", "value", "attn_out", "ffn_in", "ffn_out")
+LORA_RANKS = (8, 16, 32, 64)
+# Hugging-Face module of each single-slice target, under bert.encoder.layer.N.
+_LORA_HF = {"query": "attention.self.query", "key": "attention.self.key", "value": "attention.self.value",
+            "attn_out": "attention.output.dense", "ffn_in": "intermediate.dense", "ffn_out": "output.dense"}
+
+
+@dataclass(frozen=True)
+class LoraConfig:
+    """LoRA fine-tuning (PEFT's semantics): every targeted projection computes ``x W^T + b + s (x A^T) B^T`` with
+    ``s = alpha / r``, ``A`` ``[r, in]`` from ``kaiming_uniform_(a=sqrt(5))`` and ``B`` ``[out, r]`` zero, so a fresh
+    model computes what the base model does.  The base weights are frozen; the adapters and the classifier train.
+    ``freeze_a``: FFA-LoRA -- ``A`` stays at its shared initial value, so the clients' mean of ``B`` is the mean of their
+    products ``B A``."""
+    r: int = 8
+    alpha: float = 16.0
+    targets: tuple = ("query", "value")
+    freeze_a: bool = False
+
+    def __post_init__(self):
+        if isinstance(self.r, bool) or self.r not in LORA_RANKS:
+            raise ValueError("LoRA: r must be one of {}, got {!r}".format(LORA_RANKS, self.r))
+        if isinstance(self.alpha, bool) or not isinstance(self.alpha, (int, float)) or not self.alpha > 0:
+            raise ValueError("LoRA: alpha must be a number > 0, got {!r}".format(self.alpha))
+        t = (self.targets,) if isinstance(self.targets, str) else tuple(self.targets)
+        if not t or len(set(t)) != len(t) or any(x not in LORA_TARGETS for x in t):
+            raise ValueError("LoRA: targets must be distinct names from {}, got {!r}".format(LORA_TARGETS, self.targets))
+        object.__setattr__(self, "targets", tuple(x for x in LORA_TARGETS if x in t))
+        if not isinstance(self.freeze_a, bool):
+            raise ValueError("LoRA: freeze_a must be a bool, got {!r}".format(self.freeze_a))
+
+    @property
+    def scale(self) -> float:
+        return float(self.alpha) / self.r
+
+
 @dataclass
 class BertConfig:
     vocab_size: int = 30522
@@ -128,8 +164,11 @@ class BertForSequenceClassification(FederatedModule):
     default_batch_size = 32
     head = "classifier"
 
-    def __init__(self, config: Optional[BertConfig] = None, name: Optional[str] = None):
+    def __init__(self, config: Optional[BertConfig] = None, name: Optional[str] = None,
+                 lora: Optional[LoraConfig] = None):
         super().__init__()
+        if lora is not None and not isinstance(lora, LoraConfig):
+            raise TypeError("lora= takes a LoraConfig, got {!r}".format(lora))
         self.config = c = config or BertConfig()
         if name:
             self.name = name
@@ -144,6 +183,23 @@ class BertForSequenceClassification(FederatedModule):
                 nn.init.normal_(m.weight, std=0.02)
                 if m.bias is not None:
                     nn.init.zeros_(m.bias)
+        self.lora = lora
+        if lora is not None:
+            self._add_lora(lora)
+
+    def _add_lora(self, lora: LoraConfig) -> None:
+        """Adapters on the targeted projections of every layer, then everything but the adapters and the classifier
+        frozen (``A`` too with ``freeze_a``)."""
+        t = set(lora.targets)
+        for layer in self.layers:
+            if t & {"query", "key", "value"}:
+                layer.qkv.add_lora(lora.r, lora.scale, tuple(n in t for n in ("query", "key", "value")))
+            for name in ("attn_out", "ffn_in", "ffn_out"):
+                if name in t:
+                    getattr(layer, name).add_lora(lora.r, lora.scale, (True,))
+        for n, p in self.named_parameters():
+            train = n.startswith("classifier.") or n.endswith(".lora_B") or (n.endswith(".lora_A") and not lora.freeze_a)
+            p.requires_grad_(train)
 
     @property
     def n_dropout_sites(self) -> int:
@@ -215,7 +271,10 @@ class BertForSequenceClassification(FederatedModule):
         sd.pop("bert.embeddings.token_type_ids", None)
         if strict and sd:
             raise KeyError("unexpected Hugging-Face keys: {}".format(sorted(sd)[:5]))
-        self.load_state_dict(own, strict=strict)
+        missing, unexpected = self.load_state_dict(own, strict=False)     # a LoRA model keeps its adapters
+        missing = [k for k in missing if not k.endswith((".lora_A", ".lora_B"))]
+        if strict and (missing or unexpected):
+            raise KeyError("state_dict mismatch: missing {}, unexpected {}".format(missing[:5], unexpected[:5]))
         arena = getattr(self, "_arena", None)
         if arena is not None:
             arena.commit_global()
@@ -243,12 +302,79 @@ class BertForSequenceClassification(FederatedModule):
         return out
 
 
-def bert_base(num_labels: int = 2, **kw) -> BertForSequenceClassification:
-    return BertForSequenceClassification(BertConfig(num_labels=num_labels, **kw))
+    # ------------------------------------------------------------------ LoRA adapters under Hugging-Face names
+    def _lora_modules(self):
+        """``(HF module prefix, layer, rank block, slice)`` of every adapter: the packed ``qkv`` layer holds one rank
+        block per targeted slice."""
+        if self.lora is None:
+            raise RuntimeError("this model has no LoRA adapters (build it with lora=LoraConfig(...))")
+        out = []
+        for i, layer in enumerate(self.layers):
+            hf = "bert.encoder.layer.{}.".format(i)
+            for mod, names in ((layer.qkv, ("query", "key", "value")), (layer.attn_out, ("attn_out",)),
+                               (layer.ffn_in, ("ffn_in",)), (layer.ffn_out, ("ffn_out",))):
+                if getattr(mod, "lora_cfg", None) is None:
+                    continue
+                slot = mod.lora_cfg[2]
+                for j, n in enumerate(names):
+                    if slot[j] >= 0:
+                        out.append((hf + _LORA_HF[n], mod, slot[j], j))
+        return out
+
+    @torch.no_grad()
+    def lora_state_dict(self) -> dict:
+        """The trainable entries -- every adapter's ``lora_A.weight`` ``[r, in]`` and ``lora_B.weight`` ``[out, r]``
+        under its Hugging-Face module name, and ``classifier.weight`` / ``.bias`` -- as fp32 copies."""
+        r = self.lora.r
+        out = {}
+        for name, mod, t, _ in self._lora_modules():
+            ds = mod.lora_cfg[3]
+            out[name + ".lora_A.weight"] = mod.lora_A[t * r:(t + 1) * r].detach().clone()
+            out[name + ".lora_B.weight"] = mod.lora_B[t * ds:(t + 1) * ds].detach().clone()
+        for p in ("weight", "bias"):
+            out["classifier." + p] = getattr(self.classifier, p).detach().clone()
+        return out
+
+    @torch.no_grad()
+    def load_lora_state_dict(self, state: dict) -> None:
+        """Inverse of :meth:`lora_state_dict`; every key must be present and no other."""
+        own = self.lora_state_dict()
+        if set(state) != set(own):
+            raise KeyError("LoRA state_dict keys differ: missing {}, unexpected {}".format(
+                sorted(set(own) - set(state))[:5], sorted(set(state) - set(own))[:5]))
+        r = self.lora.r
+        for name, mod, t, _ in self._lora_modules():
+            ds = mod.lora_cfg[3]
+            mod.lora_A[t * r:(t + 1) * r].copy_(state[name + ".lora_A.weight"])
+            mod.lora_B[t * ds:(t + 1) * ds].copy_(state[name + ".lora_B.weight"])
+        for p in ("weight", "bias"):
+            getattr(self.classifier, p).copy_(state["classifier." + p])
+        arena = getattr(self, "_arena", None)
+        if arena is not None:
+            arena.commit_global()
+
+    @torch.no_grad()
+    def merged_hf_state_dict(self) -> dict:
+        """A stock Hugging-Face ``state_dict`` (as :meth:`hf_state_dict`) with every adapter merged, ``W + s B A``
+        computed in float64 and rounded to fp32 once: it loads with ``strict=True`` into a model without LoRA."""
+        out = self.hf_state_dict()
+        s, r = self.lora.scale, self.lora.r
+        for name, mod, t, _ in self._lora_modules():
+            ds = mod.lora_cfg[3]
+            a = mod.lora_A[t * r:(t + 1) * r].double()
+            b = mod.lora_B[t * ds:(t + 1) * ds].double()
+            w = out[name + ".weight"]
+            out[name + ".weight"] = (w.double() + s * (b @ a).to(w.device)).float()
+        return out
 
 
-def bert_tiny(num_labels: int = 2) -> BertForSequenceClassification:
+def bert_base(num_labels: int = 2, lora: Optional[LoraConfig] = None, **kw) -> BertForSequenceClassification:
+    return BertForSequenceClassification(BertConfig(num_labels=num_labels, **kw), lora=lora)
+
+
+def bert_tiny(num_labels: int = 2, lora: Optional[LoraConfig] = None) -> BertForSequenceClassification:
     """2-layer, 128-wide model for tests."""
     return BertForSequenceClassification(BertConfig(vocab_size=1024, hidden_size=128, num_hidden_layers=2,
                                                     num_attention_heads=2, intermediate_size=512,
-                                                    max_position_embeddings=128, num_labels=num_labels), name="bert_tiny")
+                                                    max_position_embeddings=128, num_labels=num_labels), name="bert_tiny",
+                                         lora=lora)

@@ -188,6 +188,10 @@ class ResNet(FederatedModule):
     default_lr = 0.05
     default_batch_size = 128
     head = "fc"
+    # read by ParamArena: the hand-scheduled step applies the optimizer in the convolution weight-gradient epilogues
+    frozen_params_unsupported = ("ResNets do not support frozen parameters: their hand-scheduled training step "
+                                 "(explicit_step) computes and applies a gradient for every convolution, BatchNorm and "
+                                 "fc parameter")
 
     def __init__(self, block: Type[nn.Module], layers: Sequence[int], num_classes: int = 1000,
                  in_channels: int = 3, name: Optional[str] = None, norm: str = "batch", groups: int = 2):

@@ -142,6 +142,44 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
     return out
 
 
+def lora_down(x: torch.Tensor, w: torch.Tensor, *, T: int, rs: int, kt: int, xoff: Sequence[int], w_ts: int, wsj: int,
+              wsk: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """LoRA down projection ``U[m, t rs + j] = bf16(sum_k x[m, xoff[t] + k] * w[t w_ts + j wsj + k wsk])`` for ``T``
+    slices, ``k < kt`` (csrc/lora.cu): ``U = X A^T`` in the forward, ``V = dY' B`` per targeted slice in the backward.
+    Returns ``[M, T rs]`` bf16 (``out`` when given)."""
+    M = x.shape[0]
+    u = torch.empty((M, T * rs), dtype=BF16, device=x.device) if out is None else out
+    load().lora_down(x, _pitch(x), w, w_ts, wsj, wsk, u, _pitch(u), M, T, rs, kt, list(xoff))
+    return u
+
+
+def gemm_lora(a: torch.Tensor, b: torch.Tensor, lora: dict, *, b_mn: bool = False, bias: Optional[torch.Tensor] = None,
+              act: int = 0, out_dtype: torch.dtype = BF16, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``act(A @ B^T + s T + bias)`` with the rank term ``T`` of ``lora`` in the GEMM epilogue (``B200LoraEpilogue`` in
+    csrc/launch.h): keys ``u`` (bf16 ``[M, R]``), ``f``, ``fs_n``, ``fs_j``, ``rs``, ``ds``, ``slot`` (three entries) and
+    ``s``.  ``A`` is K-major ``[M, K]``; ``B`` is ``[N, K]``, or ``[K, N]`` with ``b_mn``."""
+    M, K = a.shape
+    N = b.shape[1] if b_mn else b.shape[0]
+    if out is None:
+        out = torch.empty((M, N), dtype=out_dtype, device=a.device)
+    u = lora["u"]
+    load().gemm_lora(a, b, out, bias, M, N, K, _pitch(a), _pitch(b), _pitch(out), False, b_mn, act, 1.0, u, _pitch(u), lora["f"],
+                     lora["fs_n"], lora["fs_j"], u.shape[1], lora["rs"], lora["ds"], list(lora["slot"]), lora["s"])
+    return out
+
+
+def lora_grad_(l: torch.Tensor, q: torch.Tensor, out: torch.Tensor, *, NA: int, NB: int, lo: Sequence[int],
+               qo: Sequence[int], osa: int, osb: int, out_ts: int, s: float) -> None:
+    """Adapter gradient ``out[t out_ts + a osa + b osb] += s * sum_m l[m, lo[t] + a] * q[m, qo[t] + b]`` (csrc/lora.cu):
+    ``dA = s V^T X`` and ``dB = s dY'^T U``.  A fixed split over M, summed in a fixed order: the bits do not depend on
+    the device, the run or graph capture."""
+    C = load()
+    M, T = l.shape[0], len(lo)
+    splits = -(-M // C.LORA_SPLIT_ROWS)
+    work = torch.empty(T * splits * NA * NB, dtype=torch.float32, device=l.device)
+    C.lora_grad(l, _pitch(l), q, _pitch(q), out, osa, osb, out_ts, M, NA, NB, T, list(lo), list(qo), s, work)
+
+
 def affine_epilogue_args(table: torch.Tensor, offset: int, channels: int, relu: bool,
                          residual: Optional[torch.Tensor] = None) -> dict:
     """``affine=`` argument of :func:`gemm` / :func:`conv_igemm_fwd` for the BatchNorm whose eval scale / shift

@@ -20,7 +20,7 @@ from __future__ import annotations
 
 import contextlib
 import math
-from typing import Optional
+from typing import Optional, Tuple
 
 import torch
 from torch import nn
@@ -312,8 +312,37 @@ class _LinearFn(torch.autograd.Function):
             dy2 = F.relu_bwd(aux, dy2)
         elif ctx.act == 2:
             dy2 = F.gelu_bwd(aux, dy2)
-        weight, bias = ctx.weight, ctx.bias
-        gw = gb = None
+        gw, gb = _linear_param_grads(dy2, x2, ctx.weight, ctx.bias)
+        dx = None
+        if ctx.needs_dx:
+            # dgrad: dX[M, K] = dY[M, N] W[N, K]   (B = W is MN-major for this product)
+            dx = F.gemm(dy2, w_bf16, b_mn=True).view(ctx.x_shape)
+        return dx, gw, gb, None, None, None, None, None
+
+
+def _act_bwd(ctx, dy, aux):
+    """``dY'``: the bf16 gradient of a Linear's pre-activation output."""
+    dy2 = dy.reshape(-1, dy.shape[-1])
+    if dy2.dtype != BF16:
+        dy2 = F.cast(dy2.contiguous(), BF16)
+    elif not dy2.is_contiguous():
+        dy2 = dy2.contiguous()
+    if ctx.act == 1:
+        dy2 = F.relu_bwd(aux, dy2)
+    elif ctx.act == 2:
+        dy2 = F.gelu_bwd(aux, dy2)
+    return dy2
+
+
+def _frozen(p) -> bool:
+    return p is None or not p.requires_grad
+
+
+def _linear_param_grads(dy2, x2, weight, bias):
+    """Weight and bias gradients of a Linear: accumulated into the arena views (returns None, None) or returned to
+    autograd.  A frozen weight runs no weight-gradient GEMM, a frozen bias no column sum."""
+    gw = gb = None
+    if not _frozen(weight):
         # wgrad: dW[N, K] += dY^T[N, M] X[M, K]   (both operands MN-major, no transposes)
         tgt = _grad_target(weight)
         if tgt is not None:
@@ -321,17 +350,74 @@ class _LinearFn(torch.autograd.Function):
             WGRAD.run(lambda: F.gemm(dy2, x2, a_mn=True, b_mn=True, out=out2d, accumulate=True), dy2, x2)
         else:
             gw = F.gemm(dy2, x2, a_mn=True, b_mn=True, out_dtype=torch.float32, accumulate=True).view_as(weight)
-        if bias is not None:
-            tb = _grad_target(bias)
-            if tb is not None:
-                F.colsum_(dy2, tb, accumulate=True)
-            else:
-                gb = F.colsum_(dy2, torch.zeros_like(bias, dtype=torch.float32), accumulate=True)
+    if not _frozen(bias):
+        tb = _grad_target(bias)
+        if tb is not None:
+            F.colsum_(dy2, tb, accumulate=True)
+        else:
+            gb = F.colsum_(dy2, torch.zeros_like(bias, dtype=torch.float32), accumulate=True)
+    return gw, gb
+
+
+def _grad_or_scratch(p):
+    """(buffer to accumulate into, gradient to return to autograd) of a trainable parameter."""
+    tgt = _grad_target(p)
+    if tgt is not None:
+        return tgt, None
+    g = torch.zeros_like(p, dtype=torch.float32)
+    return g, g
+
+
+class _LoraLinearFn(torch.autograd.Function):
+    """``y = act(x W^T + b + s (x A^T) B^T)`` with the rank term per targeted output slice (``Linear.add_lora``):
+    the down projection ``U = x A^T`` is one launch for every slice, the up projection runs in the epilogue of the
+    base GEMM, and the output is rounded once.  Backward: ``V = dY' B`` (one launch), ``dx = dY' W + s V A`` (the
+    same epilogue form), ``dB = s dY'^T U`` and ``dA = s V^T x`` as fixed-order reductions over the rows."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, w_bf16, lora_a, lora_b, a_bf16, b_bf16, cfg, act, out_fp32, anchor):
+        weight, bias, lora_a, lora_b = _unwrap(weight), _unwrap(bias), _unwrap(lora_a), _unwrap(lora_b)
+        x2 = x.reshape(-1, x.shape[-1])
+        r, s, slot, ds = cfg
+        R, K = a_bf16.shape
+        u = F.lora_down(x2, a_bf16, T=1, rs=R, kt=K, xoff=(0,), w_ts=0, wsj=K, wsk=1)
+        y = F.gemm_lora(x2, w_bf16, dict(u=u, f=b_bf16, fs_n=r, fs_j=1, rs=r, ds=ds, slot=slot, s=s), bias=bias,
+                        act=act if act != 2 else 0, out_dtype=torch.float32 if out_fp32 else BF16)
+        pre = None
+        if act == 2:
+            pre = y
+            y = F.gelu(pre)
+        ctx.save_for_backward(x2, w_bf16, u, a_bf16, b_bf16, y if act == 1 else pre)
+        ctx.act, ctx.cfg = act, cfg
+        ctx.weight, ctx.bias, ctx.lora_a, ctx.lora_b = weight, bias, lora_a, lora_b
+        ctx.x_shape = x.shape
+        ctx.needs_dx = x.requires_grad
+        return y.view(*x.shape[:-1], w_bf16.shape[0])
+
+    @staticmethod
+    def backward(ctx, dy):
+        x2, w_bf16, u, a_bf16, b_bf16, aux = ctx.saved_tensors
+        dy2 = _act_bwd(ctx, dy, aux)
+        r, s, slot, ds = ctx.cfg
+        R, K = a_bf16.shape
+        gw, gb = _linear_param_grads(dy2, x2, ctx.weight, ctx.bias)
+        sl = [i for i in range(3) if slot[i] >= 0]          # targeted slices in rank-block order
+        sl.sort(key=lambda i: slot[i])
+        lo = [i * ds for i in sl]
+        v = F.lora_down(dy2, b_bf16, T=len(sl), rs=r, kt=ds, xoff=lo, w_ts=ds * r, wsj=1, wsk=r)
+        ga = gbb = None
+        if not _frozen(ctx.lora_b):
+            tgt, gbb = _grad_or_scratch(ctx.lora_b)
+            F.lora_grad_(dy2, u, tgt, NA=ds, NB=r, lo=lo, qo=[slot[i] * r for i in sl], osa=r, osb=1, out_ts=ds * r,
+                         s=s)
+        if not _frozen(ctx.lora_a):
+            tgt, ga = _grad_or_scratch(ctx.lora_a)
+            F.lora_grad_(x2, v, tgt, NA=K, NB=R, lo=(0,), qo=(0,), osa=1, osb=K, out_ts=0, s=s)
         dx = None
         if ctx.needs_dx:
-            # dgrad: dX[M, K] = dY[M, N] W[N, K]   (B = W is MN-major for this product)
-            dx = F.gemm(dy2, w_bf16, b_mn=True).view(ctx.x_shape)
-        return dx, gw, gb, None, None, None, None, None
+            dx = F.gemm_lora(dy2, w_bf16, dict(u=v, f=a_bf16, fs_n=1, fs_j=K, rs=R, ds=K, slot=(0, -1, -1), s=s),
+                             b_mn=True).view(ctx.x_shape)
+        return dx, gw, gb, None, ga, gbb, None, None, None, None, None, None
 
 
 class Linear(nn.Module):
@@ -354,12 +440,55 @@ class Linear(nn.Module):
             bound = 1 / math.sqrt(self.in_features)
             nn.init.uniform_(self.bias, -bound, bound)
 
+    def add_lora(self, r: int, s: float, targets: Tuple[bool, ...]) -> None:
+        """Low-rank adapters on the output slices ``targets`` (the output splits into ``len(targets)`` equal slices, at
+        most three: the packed q / k / v projection): ``lora_A`` ``[T r, in]`` stacks the targeted slices' ``A`` in slice
+        order, ``lora_B`` ``[T ds, r]`` their ``B``.  ``A`` starts as ``kaiming_uniform_(a=sqrt(5))``, ``B`` at zero, so
+        the layer computes what it did.  Called before the arena adopts the model."""
+        n = len(targets)
+        if not 1 <= n <= 3 or self.out_features % n or not any(targets):
+            raise ValueError("LoRA: one to three equal output slices with at least one target, got {}".format(targets))
+        ds = self.out_features // n
+        if ds % 32 or self.in_features % 32:
+            raise ValueError("LoRA needs slice widths and in_features that are multiples of 32")
+        slot, t = [-1, -1, -1], 0
+        for i, on in enumerate(targets):
+            if on:
+                slot[i], t = t, t + 1
+        a = torch.empty(t * r, self.in_features)
+        for i in range(t):
+            nn.init.kaiming_uniform_(a[i * r:(i + 1) * r], a=math.sqrt(5))
+        self.lora_A = nn.Parameter(a)
+        self.lora_B = nn.Parameter(torch.zeros(t * ds, r))
+        self.lora_cfg = (int(r), float(s), tuple(slot), ds)
+
+    def _lora_term(self, x):
+        """CPU form of the adapter term, ``s (x A_t^T) B_t^T`` in the targeted slices and zero elsewhere."""
+        r, s, slot, ds = self.lora_cfg
+        u = x @ self.lora_A.to(x.dtype).t()
+        parts = []
+        for t in slot:
+            if t < 0:
+                parts.append(x.new_zeros(*x.shape[:-1], ds))
+            else:
+                parts.append(s * (u[..., t * r:(t + 1) * r] @ self.lora_B[t * ds:(t + 1) * ds].to(x.dtype).t()))
+        return torch.cat(parts[: self.out_features // ds], dim=-1)
+
     def forward(self, x):
+        lora = getattr(self, "lora_cfg", None)
         if not x.is_cuda:
             y = TF.linear(x, self.weight.to(x.dtype), None if self.bias is None else self.bias.to(x.dtype))
+            if lora is not None:
+                y = y + self._lora_term(x)
             return TF.relu(y) if self.act == 1 else (TF.gelu(y, approximate="tanh") if self.act == 2 else y)
         if x.dtype != BF16:
             x = F.cast(x.contiguous(), BF16)
+        if lora is not None:
+            y = _LoraLinearFn.apply(x, _wrap(self.weight, x), _wrap(self.bias, x), _shadow(self, "weight", self.weight),
+                                    _wrap(self.lora_A, x), _wrap(self.lora_B, x), _shadow(self, "lora_A", self.lora_A),
+                                    _shadow(self, "lora_B", self.lora_B), lora, self.act, self.out_fp32,
+                                    _anchor(x, self.lora_A, self.lora_B))
+            return y
         if getattr(self, "fp8", False) and self.act == 0 and self.bias is None and not self.out_fp32:
             y = matmul_fp8(x.reshape(-1, x.shape[-1]), self, _shadow(self, "weight", self.weight), self.in_features)
             return y.view(*x.shape[:-1], self.out_features)
@@ -367,7 +496,7 @@ class Linear(nn.Module):
         if cfg is not None and cfg.get("epoch_word") is None:
             self.flags_cfg = None  # launch-constant epoch: one-shot, only the first GEMM after a round is gated
         return _LinearFn.apply(x, _wrap(self.weight, x), _wrap(self.bias, x), _shadow(self, "weight", self.weight),
-                               self.act, self.out_fp32, cfg, _anchor(x, self.weight))
+                               self.act, self.out_fp32, cfg, _anchor(x, self.weight, self.bias))
 
 
 # ================================================================================ Conv2d (NHWC, implicit GEMM)
@@ -1002,6 +1131,8 @@ class _EmbedFn(torch.autograd.Function):
     def backward(ctx, dy):
         (ids,) = ctx.saved_tensors
         table = ctx.table
+        if _frozen(table):
+            return None, None, None, None
         tgt = _grad_target(table)
         g = None
         if tgt is None:

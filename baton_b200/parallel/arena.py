@@ -16,7 +16,9 @@ the checkpoint layout are unchanged (reference: the global model is addressed by
   (``global_w``) are parallel flat buffers with identical offsets on every rank.
 
 With client-local entries (FedBN / FedPer, ``parallel/personal.py``) the slots are reordered so that those entries
-form one 1024-aligned range ``local_range`` that the collective skips; see :class:`ParamArena`.
+form one 1024-aligned range ``local_range`` that the collective skips; see :class:`ParamArena`.  Frozen parameters
+(``requires_grad=False``, e.g. the base weights of a LoRA model) form the 1024-aligned range ``frozen_range`` right
+after the trainable ones: they have no gradient or optimizer state, and the collective skips them too.
 
 Conv weights keep their logical ``[Cout, Cin, KH, KW]`` shape with channels_last
 strides, i.e. they are physically ``[Cout, KH, KW, Cin]`` in the arena.
@@ -55,7 +57,12 @@ class ParamArena:
         """``local``: names of float ``state_dict`` entries that stay with each client (``parallel/personal.py``).  They
         are laid out as one contiguous range ``local_range = (lo, hi)`` of whole 1024-element granules that straddles
         ``n_param``: ``[shared params | pad][local params | local float buffers | pad][shared float buffers]``.
-        Without them the layout is parameters, then float buffers, and ``local_range`` is None."""
+        Without them the layout is parameters, then float buffers, and ``local_range`` is None.
+
+        Parameters with ``requires_grad=False`` are laid out as ``frozen_range = (lo, hi)`` of whole 1024-element
+        granules: ``[trainable params | pad][frozen params | pad][float buffers]`` with ``n_param = lo``, so the gradient,
+        momentum, AdamW and server-optimizer state cover the trainable parameters only while ``theta``, ``global_w`` and
+        the bf16 shadow hold everything.  Without frozen parameters ``frozen_range`` is None and the layout unchanged."""
         self.model = model
         params = [(n, p) for n, p in model.named_parameters()]
         device = torch.device(device) if device is not None else (params[0][1].device if params else torch.device("cpu"))
@@ -89,21 +96,37 @@ class ParamArena:
                 off = _round_up(off + t.numel(), ALIGN)
             return off
 
+        frozen = [x for x in uniq if not x[1].requires_grad]
+        if frozen:
+            reason = getattr(model, "frozen_params_unsupported", None)
+            if reason:
+                raise ValueError(reason)
+            if local:
+                raise ValueError("frozen parameters with client-local entries are not supported: the collective skips "
+                                 "one range")
+            uniq = [x for x in uniq if x[1].requires_grad]
         off = place([x for x in uniq if x[0] not in local], 0, True)
         self.local_range: Optional[Tuple[int, int]] = None
+        self.frozen_range: Optional[Tuple[int, int]] = None
         if local:
             lo = off = _round_up(off, LOCAL_ALIGN)
             off = place([x for x in uniq if x[0] in local], off, True)
-        self.n_param = _round_up(off, ALIGN)
-        off = self.n_param
+        if frozen:
+            self.n_param = lo = _round_up(off, LOCAL_ALIGN)
+            off = _round_up(place(frozen, lo, True), LOCAL_ALIGN)
+            self.frozen_range = (lo, off)
+        else:
+            self.n_param = _round_up(off, ALIGN)
+            off = self.n_param
         if local:
             off = _round_up(place([x for x in bufs if x[0] in local], off, False), LOCAL_ALIGN)
             self.local_range = (lo, off)
         off = place([x for x in bufs if x[0] not in local], off, False)
         self.n = _round_up(max(off, ALIGN), total_align)   # padded so tiles / vectors never straddle the end
         self.n_int = ioff
-        if local and self.n % LOCAL_ALIGN:
-            raise ValueError("local entries need total_align to be a multiple of {}".format(LOCAL_ALIGN))
+        if (local or frozen) and self.n % LOCAL_ALIGN:
+            raise ValueError("local entries and frozen parameters need total_align to be a multiple of {}".format(
+                LOCAL_ALIGN))
 
         if theta_storage is not None:
             assert theta_storage.numel() >= self.n and theta_storage.dtype == torch.float32
@@ -124,11 +147,16 @@ class ParamArena:
         self._adopt()
 
     @property
+    def skip_range(self) -> Optional[Tuple[int, int]]:
+        """The one range the collective skips: the client-local range or the frozen range (never both), or None."""
+        return self.local_range if self.local_range is not None else self.frozen_range
+
+    @property
     def n_shared(self) -> int:
-        """Elements the collective carries: ``n`` minus the client-local range (a multiple of 1024 when there is one)."""
-        if self.local_range is None:
+        """Elements the collective carries: ``n`` minus the skipped range (a multiple of 1024 when there is one)."""
+        if self.skip_range is None:
             return self.n
-        lo, hi = self.local_range
+        lo, hi = self.skip_range
         return self.n - (hi - lo)
 
     # ------------------------------------------------------------------
@@ -156,7 +184,7 @@ class ParamArena:
                 p = getattr(owner, leaf)
                 view.copy_(p.detach().to(self.device))
                 p.data = view
-                p.grad = self._view(self.grad, slot)
+                p.grad = self._view(self.grad, slot) if slot.offset < self.n_param else None
                 if self.theta_bf16 is not None:
                     sh = self.theta_bf16[slot.offset: slot.offset + slot.numel]
                     sh = sh.view(slot.shape[0], -1) if len(slot.shape) >= 2 else sh.view(slot.shape)

@@ -199,7 +199,8 @@ class FederatedEngine:
         self.secagg = SecAggConfig(secagg_range) if secure_agg else None
         check_features(wire_dtype=wire_dtype, mode=mode, dp=self.dp, scaffold=scaffold, robust=self.robust,
                        topk=self.topk, server_opt=sopt, tile_flags=tile_flags, optimizer=optimizer, momentum=momentum,
-                       prox_mu=prox_mu, local=keys is not None, secure_agg=secure_agg)
+                       prox_mu=prox_mu, local=keys is not None, secure_agg=secure_agg,
+                       frozen=any(not p.requires_grad for p in model.parameters()))
         self.device = torch.device(device)
         self.model = model
         self.name = name
@@ -231,6 +232,8 @@ class FederatedEngine:
                                tile_flags=tile_flags, dp=self.dp, scaffold=scaffold, server_opt=sopt,
                                robust=self.robust, topk=self.topk, max_clients=max_clients,
                                local=self.personal is not None, secagg=self.secagg)
+        if self.arena.frozen_range is not None:
+            self._check_frozen_agree(group)
         self.dp = self.session.dp                  # rank 0's noise key
         self.accountant = RDPAccountant(self.dp.noise_multiplier) if self.dp is not None else None
         self.backend = backend
@@ -284,6 +287,32 @@ class FederatedEngine:
         self.last_losses_dev = None
         self.samples_trained = 0          # samples this rank pushed through local SGD (per epoch)
         self.phase_s: Dict[str, float] = {}   # host seconds per NVTX phase (launch cost; device time is in bench.py)
+
+    def _check_frozen_agree(self, group) -> None:
+        """The collective never carries the frozen range, so every rank must start from the same frozen weights: one
+        hash of the range, all-reduced as (max, -min), and a ``ValueError`` on every rank when they differ."""
+        import hashlib
+        import torch.distributed as dist
+        if not (dist.is_available() and dist.is_initialized()) or self._group_size(group) == 1:
+            return
+        lo, hi = self.arena.frozen_range
+        digest = hashlib.sha256(self.arena.theta[lo:hi].cpu().numpy().tobytes()).digest()
+        h = int.from_bytes(digest[:7], "little")           # fits an int64 with its negation
+        t = torch.tensor([h, -h], dtype=torch.int64, device=self.device)
+        dist.all_reduce(t, op=dist.ReduceOp.MAX, group=group)
+        if int(t[0]) != -int(t[1]):
+            raise ValueError("the frozen parameters differ between ranks: every client must start from the same base "
+                             "weights, which the collective never carries")
+
+    def lora_state_dict(self) -> dict:
+        """The model's adapter and classifier entries under Hugging-Face names (``models/bert.py``)."""
+        self.sync()
+        return self.model.lora_state_dict()
+
+    def merged_hf_state_dict(self) -> dict:
+        """A stock Hugging-Face ``state_dict`` with the adapters merged into the base weights (``models/bert.py``)."""
+        self.sync()
+        return self.model.merged_hf_state_dict()
 
     @staticmethod
     def _group_size(group) -> int:

@@ -21,13 +21,14 @@ SEATED_SERVER_OPT = ("a server optimizer needs the http plane: on the seated pla
 def check_features(*, wire_dtype: str = "bf16", mode: str = "delta", dp=None, scaffold: bool = False, robust=None,
                    topk=None, server_opt=None, tile_flags: bool = False, plane: Optional[str] = None,
                    optimizer: str = "sgd", momentum: float = 0.0, nesterov: bool = False, prox_mu: float = 0.0,
-                   local: bool = False, secure_agg: bool = False) -> None:
+                   local: bool = False, secure_agg: bool = False, frozen: bool = False) -> None:
     """``ValueError`` with the reason if the features cannot run together.  ``dp``, ``robust``, ``topk`` and
     ``server_opt`` are on unless they are None or False: the rules read only which features are on, so a caller may pass
     the features' configurations or bools.  Whoever takes a configuration from outside checks its type.  ``plane``:
     ``"http"`` or ``"seated"`` (the ``fused`` / ``nccl`` manager planes), None where no manager plane is involved.
     ``local``: client-local ``state_dict`` entries (FedBN / FedPer, ``parallel/personal.py``).  ``secure_agg``: secure
-    aggregation (``parallel/secagg.py``)."""
+    aggregation (``parallel/secagg.py``).  ``frozen``: a model with frozen parameters (LoRA fine-tuning), whose
+    arena range the collective skips."""
     if optimizer not in OPTIMIZERS:
         raise ValueError("optimizer must be one of {}, got {!r}".format(OPTIMIZERS, optimizer))
     adamw = optimizer == "adamw"
@@ -82,6 +83,20 @@ def check_features(*, wire_dtype: str = "bf16", mode: str = "delta", dp=None, sc
                                     "the apply phase, not published tile by tile"),
         (secure_agg and plane is not None, "secure aggregation needs the SPMD engine: the manager planes have no key "
                                            "exchange, and their payload is a pickled state_dict"),
+        (frozen and dp, "frozen parameters with DP-FedAvg are not supported: its round has no skipped range, so the "
+                        "clip norm and the noise would cover the frozen weights"),
+        (frozen and scaffold, "frozen parameters with SCAFFOLD are not supported: its round has no skipped range"),
+        (frozen and robust, "frozen parameters with a robust aggregator or Krum are not supported: the client segments "
+                            "span the whole arena"),
+        (frozen and topk, "frozen parameters with top-k uploads are not supported: the selection spans the whole arena"),
+        (frozen and secure_agg, "frozen parameters with secure aggregation are not supported: its ring has no skipped "
+                                "range"),
+        (frozen and tile_flags, "frozen parameters with tile_flags are not supported: the flags index physical "
+                                "granules, and the skipped range has none"),
+        (frozen and local, "frozen parameters with client-local entries are not supported: the collective skips one "
+                           "range"),
+        (frozen and plane is not None, "frozen parameters need the SPMD engine: a manager plane's payload is a whole "
+                                       "state_dict"),
     )
     for broken, reason in rules:
         if broken:

@@ -153,10 +153,11 @@ class FedAvgSession:
         self._C = load()
         assert wire_dtype in ("bf16", "fp32", "fp8") and mode in ("delta", "weights")
         self._features = dict(wire_dtype=wire_dtype, mode=mode, scaffold=scaffold, topk=topk, server_opt=server_opt,
-                             tile_flags=tile_flags, local=bool(local), secagg=secagg)
+                             tile_flags=tile_flags, local=bool(local), secagg=secagg,
+                              frozen=arena.frozen_range is not None)
         self.max_clients = _init_session(arena, self._features, dp, robust, max_clients)
-        self.local_range = arena.local_range
-        self.n_wire = arena.n_shared           # elements on the wire: the arena minus its client-local range
+        self.local_range = arena.skip_range    # client-local or frozen: the range the round never touches
+        self.n_wire = arena.n_shared           # elements on the wire: the arena minus that range
         self.topk, self.server_opt = topk, server_opt
         self._sopt_coef = list(server_opt.coefficients()) if server_opt is not None else []
         self.robust = robust
@@ -739,9 +740,10 @@ class NcclSession:
                  local: bool = False, secagg: Optional[SecAggConfig] = None, **_unused):
         import torch.distributed as dist
         self._features = dict(wire_dtype=wire_dtype, mode=mode, scaffold=scaffold, topk=topk, server_opt=server_opt,
-                             tile_flags=tile_flags, local=bool(local), secagg=secagg)
+                             tile_flags=tile_flags, local=bool(local), secagg=secagg,
+                              frozen=arena.frozen_range is not None)
         self.max_clients = _init_session(arena, self._features, dp, robust, max_clients)
-        self.local_range = arena.local_range
+        self.local_range = arena.skip_range
         self.topk, self.server_opt = topk, server_opt
         # top-k: k, this rank's upload of the round as a dense fp32 vector (zeros off its support) and its entry count
         self.topk_k = self.topk.k(n_float(arena)) if self.topk is not None else 0
