@@ -27,7 +27,8 @@ if TRACE:
     BUILD = os.path.join(HERE, "csrc", "build_trace")
 TARGET = os.path.join(HERE, "_C_trace.so" if TRACE else "_C.so")
 
-CU_SOURCES = ["gemm_wgmma.cu", "gemm_fp8.cu", "quant.cu", "attention.cu", "im2col_tma.cu", "gemm_simt.cu", "fedavg.cu", "elementwise.cu", "conv.cu", "norm.cu", "loss.cu", "conv_halo.cu", "compress.cu", "dropout.cu", "lora.cu"]
+CU_SOURCES = ["gemm_wgmma.cu", "gemm_fp8.cu", "quant.cu", "attention.cu", "im2col_tma.cu", "gemm_simt.cu", "fedavg.cu", "elementwise.cu", "conv.cu", "norm.cu", "loss.cu", "conv_halo.cu", "compress.cu", "dropout.cu", "lora.cu",
+              "vit.cu"]
 HEADERS = ["ptx.cuh", "launch.h", "pdl.cuh", "mx.cuh", "sgd.cuh", "dp.cuh", "epilogue.cuh", "secagg.cuh", "rows.cuh", "dropout.cuh"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math", "-Xptxas", "-v"]

@@ -16,7 +16,8 @@ from typing import Optional
 
 @dataclass
 class FederationConfig:
-    model: str = "lineartest"          # lineartest | mlp2 | resnet18 | resnet50 | resnet18_gn | resnet50_gn | bert_base
+    model: str = "lineartest"          # lineartest | mlp2 | resnet18 | resnet50 | resnet18_gn | resnet50_gn | bert_base |
+    #                                    vit_tiny | vit_small
     dtype: str = "fp32"                # fp32 | bf16 | fp8 (block-scaled mxfp8 GEMMs)
     backend: str = "http"              # http | fused | nccl
     clients: int = 2                   # physical clients (GPUs)

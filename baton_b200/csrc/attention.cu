@@ -12,6 +12,13 @@
 // The S x S scores never touch HBM and P is written exactly once (the unfused path writes S, reads S,
 // writes P, reads P).  It runs whenever S = 128, d_head = 64 and there is no mask; tests/test_gpu_bert.py checks it
 // against the multi-kernel path and an fp32 reference.
+//
+// PAD: the same tiles for a runtime S < 128 (ViT sequence lengths such as 8 x 8 patches + a class token = 65), no
+// mask, no dropout.  The TMA maps carry the tensor dimension S, so query / key / value / dO rows >= S arrive as zeros.
+// Key columns >= S are left out of the row max and the row sum and get P~ = 0; no row >= S of out or dqkv is written
+// (the next image's tokens live there).  probs is [B*H, S, Sp] with Sp = round_up(S, 8), columns S..Sp-1 written as 0;
+// the backward loads its P tile through a 3-D map, so rows >= S and columns >= Sp arrive as zeros and every product
+// that reaches a padded row or column multiplies finite values.
 #define B200_TU_TAG 4
 #include "dropout.cuh"
 #include "launch.h"
@@ -37,14 +44,15 @@ constexpr int AT_NARROW_BYTES = AT_S * AT_OP * 4;
 
 struct AttnParams {
   __nv_bfloat16* out;      // [B*S, D]
-  __nv_bfloat16* probs;    // [B*H*S, S]
+  __nv_bfloat16* probs;    // [B*H*S, S]; PAD: [B*H, S, Sp]
   int H, D;                // heads, model width (H * 64)
   float scale_log2e;       // softmax scale * log2(e)
+  int S;                   // PAD: sequence length (< 128); probs row pitch Sp = round_up(S, 8)
 };
 
 // DROP: dropout on the probabilities.  Pass B zeroes the dropped entries of P~ before MMA 2 and the epilogue scales by
 // inv * s; the saved probs stay the undropped P.  Element i of the mask is the index into probs.
-template <bool DROP>
+template <bool DROP, bool PAD = false>
 __global__ void __launch_bounds__(AT_THREADS, 1)
 attention_fwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                           const __grid_constant__ CUtensorMap tmV, const AttnParams p, const DropArgs da) {
@@ -115,7 +123,7 @@ attention_fwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
         uint32_t x[32];
         acc_ld_row32(srow + c, x);
 #pragma unroll
-        for (int j = 0; j < 32; ++j) m = fmaxf(m, __uint_as_float(x[j]));
+        for (int j = 0; j < 32; ++j) m = fmaxf(m, PAD && c + j >= p.S ? -INFINITY : __uint_as_float(x[j]));
       }
       mb = m * p.scale_log2e;
       // pass B: P~ = exp2(scale*log2e*x - mb) -> bf16 -> swizzled shared memory (K-major A operand); row sum
@@ -128,7 +136,7 @@ attention_fwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
         float e[32];
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
-          e[j] = exp2f(fmaf(__uint_as_float(x[j]), p.scale_log2e, -mb));
+          e[j] = PAD && c + j >= p.S ? 0.f : exp2f(fmaf(__uint_as_float(x[j]), p.scale_log2e, -mb));
           sum += e[j];
         }
         if constexpr (DROP) {
@@ -172,25 +180,28 @@ attention_fwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
       wg_store_acc<64>(acc, sO, AT_OP, 64 * g);
     }
     named_bar_sync(1, AT_CONSUMERS);
-    if (ew < 4) {
+    const int S = PAD ? p.S : AT_S, Sp = PAD ? (p.S + 7) & ~7 : AT_S;
+    if (ew < 4 && (!PAD || r < S)) {
       // normalised probabilities to global memory (saved for backward)
-      __nv_bfloat16* grow = p.probs + (static_cast<size_t>(bh) * AT_S + r) * AT_S;
+      __nv_bfloat16* grow = p.probs + (static_cast<size_t>(bh) * S + r) * Sp;
 #pragma unroll 1
-      for (int c = 0; c < AT_S; c += 32) {
+      for (int c = 0; c < Sp; c += 32) {
         uint32_t x[32];
         acc_ld_row32(srow + c, x);
         float e[32];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) e[j] = exp2f(fmaf(__uint_as_float(x[j]), p.scale_log2e, -mb)) * inv;
+        for (int j = 0; j < 32; ++j)
+          e[j] = PAD && c + j >= S ? 0.f : exp2f(fmaf(__uint_as_float(x[j]), p.scale_log2e, -mb)) * inv;
 #pragma unroll
         for (int j = 0; j < 32; j += 8)
-          *reinterpret_cast<uint4*>(grow + c + j) =
-              make_uint4(pack_bf16x2(e[j], e[j + 1]), pack_bf16x2(e[j + 2], e[j + 3]), pack_bf16x2(e[j + 4], e[j + 5]),
-                         pack_bf16x2(e[j + 6], e[j + 7]));
+          if (!PAD || c + j < Sp)
+            *reinterpret_cast<uint4*>(grow + c + j) =
+                make_uint4(pack_bf16x2(e[j], e[j + 1]), pack_bf16x2(e[j + 2], e[j + 3]), pack_bf16x2(e[j + 4], e[j + 5]),
+                           pack_bf16x2(e[j + 6], e[j + 7]));
       }
       // epilogue: O = O~ / rowsum (times s with dropout)
       if constexpr (DROP) inv *= da.scale;
-      __nv_bfloat16* orow = p.out + (static_cast<size_t>(b) * AT_S + r) * p.D + h * AT_D;
+      __nv_bfloat16* orow = p.out + (static_cast<size_t>(b) * S + r) * p.D + h * AT_D;
 #pragma unroll 1
       for (int c = 0; c < AT_D; c += 32) {
         uint32_t x[32];
@@ -224,12 +235,13 @@ struct AttnBwdParams {
   const __nv_bfloat16* probs;   // [B*H*S, S]: re-read by the row pass of the dropout form
   int H, D;
   float scale;
+  int S;                   // PAD: sequence length (< 128)
 };
 
 // DROP: with M the mask and s the scale, dV = (P o M s)^T dO, dP = M s o (dO V^T), delta = rowsum(P o dP),
 // dS = P o (dP - delta).  Before the first MMAs each row owner turns its row of the P tile into bf16(P o M s) in place
 // and keeps its 128 keep bits in registers; the row pass then re-reads the undropped P row from global memory (L2).
-template <bool DROP>
+template <bool DROP, bool PAD = false>
 __global__ void __launch_bounds__(AT_THREADS, 1)
 attention_bwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                           const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
@@ -265,8 +277,13 @@ attention_bwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
       tma_load_4d(sK, &tmK, bar_load, 0, 0, h, b);
       tma_load_4d(sV, &tmV, bar_load, 0, 0, h, b);
       tma_load_4d(sdO, &tmdO, bar_load, 0, 0, h, b);
-      tma_load_2d(sP, &tmP, bar_load, 0, bh * AT_S);                 // keys 0..63   x 128 query rows
-      tma_load_2d(sP + 16384, &tmP, bar_load, 64, bh * AT_S);        // keys 64..127
+      if constexpr (PAD) {
+        tma_load_4d(sP, &tmP, bar_load, 0, 0, bh, 0);                // [B*H][S][Sp] map: rows >= S, keys >= Sp -> 0
+        tma_load_4d(sP + 16384, &tmP, bar_load, 64, 0, bh, 0);
+      } else {
+        tma_load_2d(sP, &tmP, bar_load, 0, bh * AT_S);               // keys 0..63   x 128 query rows
+        tma_load_2d(sP + 16384, &tmP, bar_load, 64, bh * AT_S);      // keys 64..127
+      }
     }
   } else if (warp >= 4) {
     const int ew = warp - 4, g = ew >> 2;
@@ -331,7 +348,8 @@ attention_bwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
     named_bar_sync(1, AT_CONSUMERS);
     const int lane = static_cast<int>(lane_id());
     const int r = (ew & 3) * 32 + lane;                            // query row (dP, dQ) / key row (dV, dK)
-    __nv_bfloat16* grow = p.dqkv + (static_cast<size_t>(b) * AT_S + r) * (3 * static_cast<size_t>(p.D)) + h * AT_D;
+    const int S = PAD ? p.S : AT_S;
+    __nv_bfloat16* grow = p.dqkv + (static_cast<size_t>(b) * S + r) * (3 * static_cast<size_t>(p.D)) + h * AT_D;
     if (ew < 4) {
       uint8_t* prow = sP + r * 128;
       const float* wrow = sW + r * AT_SP;
@@ -384,7 +402,7 @@ attention_bwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
         }
       }
       fence_proxy_async();            // dS (generic-proxy writes) -> visible to the tensor core
-    } else {
+    } else if (!PAD || r < S) {
       // dV row r (= key index) is complete: the second warpgroup stores it while the first computes dS
 #pragma unroll 1
       for (int c = 0; c < AT_D; c += 32) {
@@ -429,7 +447,7 @@ attention_bwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
     // the two warpgroups take one half each
     const int c = (ew < 4 ? 0 : AT_D);
 #pragma unroll 1
-    for (int cc = c; cc < c + AT_D; cc += 32) {
+    for (int cc = c; cc < (PAD && r >= S ? c : c + AT_D); cc += 32) {
       uint32_t x[32];
       acc_ld_row32(sW + r * AT_SP + cc, x);
       __nv_bfloat16* dst = grow + (cc < AT_D ? cc : p.D + (cc - AT_D));
@@ -448,12 +466,13 @@ attention_bwd_s128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
 
 using namespace b200;
 
-// qkv: packed [B*S, 3*H*64] bf16; out [B*S, H*64]; probs [B*H*S, S].  Returns -2 for unsupported shapes.
-template <bool DROP>
+// qkv: packed [B*S, 3*H*64] bf16; out [B*S, H*64]; probs [B*H*S, S] (PAD: [B*H, S, round_up(S, 8)]).  Returns -2
+// for unsupported shapes.
+template <bool DROP, bool PAD = false>
 static int attention_fwd_launch(const void* qkv, void* out, void* probs, int B, int S, int H, int dh, float scale,
                                 const DropArgs& da, cudaStream_t stream) {
   if (B <= 0) return 0;
-  if (S != AT_S || dh != AT_D) return -2;
+  if ((PAD ? S <= 0 || S >= AT_S : S != AT_S) || dh != AT_D) return -2;
   const long long D = static_cast<long long>(H) * dh;
   if ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(probs)) & 15) return -2;
   const __nv_bfloat16* base = reinterpret_cast<const __nv_bfloat16*>(qkv);
@@ -468,15 +487,17 @@ static int attention_fwd_launch(const void* qkv, void* out, void* probs, int B, 
   p.H = H;
   p.D = static_cast<int>(D);
   p.scale_log2e = scale * 1.4426950408889634f;
+  p.S = S;
   constexpr int smem = 3 * AT_Q_BYTES + AT_P_BYTES + AT_WIDE_BYTES + AT_NARROW_BYTES + 8 + 1024;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(attention_fwd_s128_kernel<DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e = cudaFuncSetAttribute(attention_fwd_s128_kernel<DROP, PAD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         smem);
     if (e != cudaSuccess) return static_cast<int>(e);
     configured = true;
   }
-  cudaError_t le = launch_pdl(attention_fwd_s128_kernel<DROP>, dim3(static_cast<unsigned>(B) * H), AT_THREADS, smem, stream,
-                              tq, tk, tv, p, da);
+  cudaError_t le = launch_pdl(attention_fwd_s128_kernel<DROP, PAD>, dim3(static_cast<unsigned>(B) * H), AT_THREADS, smem,
+                              stream, tq, tk, tv, p, da);
   if (le != cudaSuccess) return static_cast<int>(le);
   return static_cast<int>(cudaGetLastError());
 }
@@ -484,12 +505,12 @@ static int attention_fwd_launch(const void* qkv, void* out, void* probs, int B, 
 extern "C" int b200_encode_map2_bf16(void* map, const void* base, long long rows, long long cols, long long ld,
                                      int box_cols, int box_rows);
 
-// qkv [B*S, 3D], dout [B*S, D], probs [B*H*S, S] (saved by the forward) -> dqkv [B*S, 3D]
-template <bool DROP>
+// qkv [B*S, 3D], dout [B*S, D], probs [B*H*S, S] (PAD: [B*H, S, round_up(S, 8)]; saved by the forward) -> dqkv [B*S, 3D]
+template <bool DROP, bool PAD = false>
 static int attention_bwd_launch(const void* qkv, const void* dout, const void* probs, void* dqkv, int B, int S, int H,
                                 int dh, float scale, const DropArgs& da, cudaStream_t stream) {
   if (B <= 0) return 0;
-  if (S != AT_S || dh != AT_D) return -2;
+  if ((PAD ? S <= 0 || S >= AT_S : S != AT_S) || dh != AT_D) return -2;
   const long long D = static_cast<long long>(H) * dh;
   if ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(dout) | reinterpret_cast<uintptr_t>(probs) |
        reinterpret_cast<uintptr_t>(dqkv)) & 15)
@@ -501,7 +522,12 @@ static int attention_bwd_launch(const void* qkv, const void* dout, const void* p
   if (rc == 0) rc = b200_encode_map4_bf16(&tk, base + D, S, dh, 3 * D, H, dh, B, so, 64, 128);
   if (rc == 0) rc = b200_encode_map4_bf16(&tv, base + 2 * D, S, dh, 3 * D, H, dh, B, so, 64, 128);
   if (rc == 0) rc = b200_encode_map4_bf16(&tdo, dout, S, dh, D, H, dh, B, static_cast<long long>(S) * D, 64, 128);
-  if (rc == 0) rc = b200_encode_map2_bf16(&tp, probs, static_cast<long long>(B) * H * S, S, S, 64, 128);
+  if (PAD) {
+    const long long sp = (S + 7) & ~7, bh = static_cast<long long>(B) * H;
+    if (rc == 0) rc = b200_encode_map4_bf16(&tp, probs, S, sp, sp, bh, S * sp, 1, bh * S * sp, 64, 128);
+  } else if (rc == 0) {
+    rc = b200_encode_map2_bf16(&tp, probs, static_cast<long long>(B) * H * S, S, S, 64, 128);
+  }
   if (rc) return rc;
   AttnBwdParams p;
   p.dqkv = reinterpret_cast<__nv_bfloat16*>(dqkv);
@@ -509,15 +535,17 @@ static int attention_bwd_launch(const void* qkv, const void* dout, const void* p
   p.H = H;
   p.D = static_cast<int>(D);
   p.scale = scale;
+  p.S = S;
   constexpr int smem = 4 * AT_Q_BYTES + AT_P_BYTES + AT_WIDE_BYTES + AT_NARROW_BYTES + 8 + 1024;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(attention_bwd_s128_kernel<DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e = cudaFuncSetAttribute(attention_bwd_s128_kernel<DROP, PAD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         smem);
     if (e != cudaSuccess) return static_cast<int>(e);
     configured = true;
   }
-  cudaError_t le = launch_pdl(attention_bwd_s128_kernel<DROP>, dim3(static_cast<unsigned>(B) * H), AT_THREADS, smem, stream,
-                              tq, tk, tv, tdo, tp, p, da);
+  cudaError_t le = launch_pdl(attention_bwd_s128_kernel<DROP, PAD>, dim3(static_cast<unsigned>(B) * H), AT_THREADS, smem,
+                              stream, tq, tk, tv, tdo, tp, p, da);
   if (le != cudaSuccess) return static_cast<int>(le);
   return static_cast<int>(cudaGetLastError());
 }
@@ -538,6 +566,16 @@ extern "C" int b200_attention_drop_fwd(const void* qkv, void* out, void* probs, 
 extern "C" int b200_attention_drop_bwd(const void* qkv, const void* dout, const void* probs, void* dqkv, int B, int S,
                                        int H, int dh, float scale, const B200Dropout* drop, cudaStream_t stream) {
   return attention_bwd_launch<true>(qkv, dout, probs, dqkv, B, S, H, dh, scale, drop_args(drop), stream);
+}
+
+// S < 128 (not a multiple of 8 in practice: other lengths take the multi-kernel path), d_head = 64, no mask, no dropout
+extern "C" int b200_attention_short_fwd(const void* qkv, void* out, void* probs, int B, int S, int H, int dh, float scale,
+                                        cudaStream_t stream) {
+  return attention_fwd_launch<false, true>(qkv, out, probs, B, S, H, dh, scale, DropArgs{}, stream);
+}
+extern "C" int b200_attention_short_bwd(const void* qkv, const void* dout, const void* probs, void* dqkv, int B, int S,
+                                        int H, int dh, float scale, cudaStream_t stream) {
+  return attention_bwd_launch<false, true>(qkv, dout, probs, dqkv, B, S, H, dh, scale, DropArgs{}, stream);
 }
 
 B200_TRACE_REGISTER(attention)

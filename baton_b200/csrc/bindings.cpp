@@ -232,6 +232,37 @@ bool attention_bwd(const at::Tensor& qkv, const at::Tensor& dout, const at::Tens
   return true;
 }
 
+// fused attention at 0 < S < 128, d_head = 64, no mask (ViT): probs [B*H, S, round_up(S, 8)]
+static void check_short_attention(const at::Tensor& qkv, const at::Tensor& rows_d, const at::Tensor& probs, int64_t B,
+                                  int64_t S, int64_t H, int64_t dh, const char* what) {
+  TORCH_CHECK(qkv.numel() == B * S * 3 * H * dh && rows_d.numel() == B * S * H * dh &&
+                  probs.numel() == B * H * S * ((S + 7) / 8 * 8),
+              what, ": qkv [B*S, 3*H*dh], out / dout [B*S, H*dh] and probs [B*H, S, round_up(S, 8)] expected");
+}
+void attention_short_fwd(const at::Tensor& qkv, at::Tensor out, at::Tensor probs, int64_t B, int64_t S, int64_t H,
+                         int64_t dh, double scale) {
+  CHECK_CUDA(qkv); CHECK_CUDA(out); CHECK_CUDA(probs);
+  TORCH_CHECK(qkv.scalar_type() == at::kBFloat16 && out.scalar_type() == at::kBFloat16 &&
+              probs.scalar_type() == at::kBFloat16 && qkv.is_contiguous() && out.is_contiguous() && probs.is_contiguous());
+  check_short_attention(qkv, out, probs, B, S, H, dh, "attention_short_fwd");
+  const c10::cuda::CUDAGuard guard(qkv.device());
+  check(b200_attention_short_fwd(cptr(qkv), ptr(out), ptr(probs), static_cast<int>(B), static_cast<int>(S),
+                                 static_cast<int>(H), static_cast<int>(dh), static_cast<float>(scale), cur_stream()),
+        "attention_short_fwd");
+}
+void attention_short_bwd(const at::Tensor& qkv, const at::Tensor& dout, const at::Tensor& probs, at::Tensor dqkv,
+                         int64_t B, int64_t S, int64_t H, int64_t dh, double scale) {
+  CHECK_CUDA(qkv); CHECK_CUDA(dout); CHECK_CUDA(probs); CHECK_CUDA(dqkv);
+  TORCH_CHECK(qkv.scalar_type() == at::kBFloat16 && dout.scalar_type() == at::kBFloat16 &&
+              probs.scalar_type() == at::kBFloat16 && dqkv.scalar_type() == at::kBFloat16 && qkv.is_contiguous() &&
+              dout.is_contiguous() && probs.is_contiguous() && dqkv.is_contiguous() && dqkv.numel() == qkv.numel());
+  check_short_attention(qkv, dout, probs, B, S, H, dh, "attention_short_bwd");
+  const c10::cuda::CUDAGuard guard(qkv.device());
+  check(b200_attention_short_bwd(cptr(qkv), cptr(dout), cptr(probs), ptr(dqkv), static_cast<int>(B), static_cast<int>(S),
+                                 static_cast<int>(H), static_cast<int>(dh), static_cast<float>(scale), cur_stream()),
+        "attention_short_bwd");
+}
+
 // implicit-GEMM convolution; false = shape not supported (caller falls back to im2col + GEMM)
 bool conv_igemm_fwd(const at::Tensor& x, const at::Tensor& w, at::Tensor y, int64_t kh, int64_t kw, int64_t stride,
                     int64_t pad, int64_t ho, int64_t wo, int64_t cluster_k, int64_t force_bn,
@@ -604,6 +635,48 @@ void gelu_bwd(const at::Tensor& x, const at::Tensor& dy, at::Tensor dx) {
   CHECK_CUDA(x);
   const c10::cuda::CUDAGuard guard(x.device());
   check(b200_gelu_bwd_bf16(x.data_ptr(), dy.data_ptr(), dx.data_ptr(), x.numel(), cur_stream()), "gelu_bwd");
+}
+void gelu_erf(const at::Tensor& x, at::Tensor y) {
+  CHECK_CUDA(x);
+  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && y.scalar_type() == at::kBFloat16 && y.numel() == x.numel());
+  const c10::cuda::CUDAGuard guard(x.device());
+  check(b200_gelu_erf_bf16(x.data_ptr(), y.data_ptr(), x.numel(), cur_stream()), "gelu_erf");
+}
+void gelu_erf_bwd(const at::Tensor& x, const at::Tensor& dy, at::Tensor dx) {
+  CHECK_CUDA(x);
+  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && dy.scalar_type() == at::kBFloat16 && dx.scalar_type() == at::kBFloat16 &&
+              dy.numel() == x.numel() && dx.numel() == x.numel());
+  const c10::cuda::CUDAGuard guard(x.device());
+  check(b200_gelu_erf_bwd_bf16(x.data_ptr(), dy.data_ptr(), dx.data_ptr(), x.numel(), cur_stream()), "gelu_erf_bwd");
+}
+// ViT tokens: z [B, S-1, D] bf16 (patch embeddings), cls [D], bias [D], pos [S, D] fp32 -> tok [B, S, D] bf16
+void vit_tokens_fwd(const at::Tensor& z, const at::Tensor& cls, const at::Tensor& bias, const at::Tensor& pos,
+                    at::Tensor tok, int64_t B, int64_t S, int64_t D) {
+  CHECK_CUDA(z); CHECK_CUDA(tok);
+  TORCH_CHECK(z.scalar_type() == at::kBFloat16 && tok.scalar_type() == at::kBFloat16 && cls.scalar_type() == at::kFloat &&
+                  bias.scalar_type() == at::kFloat && pos.scalar_type() == at::kFloat && z.numel() == B * (S - 1) * D &&
+                  tok.numel() == B * S * D && cls.numel() == D && bias.numel() == D && pos.numel() == S * D &&
+                  z.is_contiguous() && tok.is_contiguous() && pos.is_contiguous(),
+              "vit_tokens_fwd: z [B, S-1, D] / tok [B, S, D] bf16, cls / bias [D], pos [S, D] fp32");
+  const c10::cuda::CUDAGuard guard(z.device());
+  check(b200_vit_tokens_fwd(z.data_ptr(), cls.data_ptr<float>(), bias.data_ptr<float>(), pos.data_ptr<float>(),
+                            tok.data_ptr(), static_cast<int>(B), static_cast<int>(S), static_cast<int>(D), cur_stream()),
+        "vit_tokens_fwd");
+}
+// dtok [B, S, D] -> dz [B, S-1, D] (written); dcls, dbias [D] and dpos [S, D] fp32 accumulated in a fixed order
+void vit_tokens_bwd(const at::Tensor& dtok, at::Tensor dz, at::Tensor dcls, at::Tensor dbias, at::Tensor dpos, int64_t B,
+                    int64_t S, int64_t D) {
+  CHECK_CUDA(dtok); CHECK_CUDA(dz);
+  TORCH_CHECK(dtok.scalar_type() == at::kBFloat16 && dz.scalar_type() == at::kBFloat16 &&
+                  dcls.scalar_type() == at::kFloat && dbias.scalar_type() == at::kFloat && dpos.scalar_type() == at::kFloat &&
+                  dtok.numel() == B * S * D && dz.numel() == B * (S - 1) * D && dcls.numel() == D && dbias.numel() == D &&
+                  dpos.numel() == S * D && dtok.is_contiguous() && dz.is_contiguous() && dpos.is_contiguous(),
+              "vit_tokens_bwd: dtok [B, S, D] / dz [B, S-1, D] bf16, dcls / dbias [D], dpos [S, D] fp32");
+  const c10::cuda::CUDAGuard guard(dtok.device());
+  check(b200_vit_tokens_bwd(dtok.data_ptr(), dz.data_ptr(), dcls.data_ptr<float>(), dbias.data_ptr<float>(),
+                            dpos.data_ptr<float>(), static_cast<int>(B), static_cast<int>(S), static_cast<int>(D),
+                            cur_stream()),
+        "vit_tokens_bwd");
 }
 void embedding_bwd(const at::Tensor& dy, const at::Tensor& idx, at::Tensor grad) {
   CHECK_CUDA(dy);
@@ -1319,6 +1392,30 @@ void layernorm_bwd(const at::Tensor& x, const at::Tensor& dy, at::Tensor dx, con
                            cur_stream()),
         "layernorm_bwd");
 }
+// pre-LN blocks: s = x + res and y = LN(s), both written; backward dsum = LN_bwd(dy) + ds
+void layernorm_sum_fwd(const at::Tensor& x, const at::Tensor& res, at::Tensor y, at::Tensor s, const at::Tensor& gamma,
+                       const at::Tensor& beta, at::Tensor mean, at::Tensor rstd, int64_t rows, int64_t C, double eps) {
+  CHECK_CUDA(x);
+  TORCH_CHECK(x.numel() == rows * C && res.numel() == rows * C && y.numel() == rows * C && s.numel() == rows * C &&
+              mean.numel() == rows && rstd.numel() == rows, "layernorm_sum_fwd: [rows, C] operands expected");
+  const c10::cuda::CUDAGuard guard(x.device());
+  check(b200_layernorm_sum_fwd(x.data_ptr(), res.data_ptr(), y.data_ptr(), s.data_ptr(), gamma.data_ptr<float>(),
+                               beta.data_ptr<float>(), mean.data_ptr<float>(), rstd.data_ptr<float>(), rows, C,
+                               static_cast<float>(eps), cur_stream()),
+        "layernorm_sum_fwd");
+}
+void layernorm_sum_bwd(const at::Tensor& s, const at::Tensor& dy, const at::Tensor& ds, at::Tensor dsum,
+                       const at::Tensor& gamma, const at::Tensor& mean, const at::Tensor& rstd, at::Tensor dgamma,
+                       at::Tensor dbeta, int64_t rows, int64_t C) {
+  CHECK_CUDA(s);
+  TORCH_CHECK(s.numel() == rows * C && dy.numel() == rows * C && ds.numel() == rows * C && dsum.numel() == rows * C,
+              "layernorm_sum_bwd: [rows, C] operands expected");
+  const c10::cuda::CUDAGuard guard(s.device());
+  check(b200_layernorm_sum_bwd(s.data_ptr(), dy.data_ptr(), ds.data_ptr(), dsum.data_ptr(), gamma.data_ptr<float>(),
+                               mean.data_ptr<float>(), rstd.data_ptr<float>(), dgamma.data_ptr<float>(),
+                               dbeta.data_ptr<float>(), rows, C, cur_stream()),
+        "layernorm_sum_bwd");
+}
 void softmax_fwd(const at::Tensor& x, at::Tensor y, int64_t rows, int64_t C, double scale) {
   CHECK_CUDA(x);
   const c10::cuda::CUDAGuard guard(x.device());
@@ -1600,6 +1697,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("trace_set", &trace_set);
   m.def("attention_fwd", &attention_fwd);
   m.def("attention_bwd", &attention_bwd);
+  m.def("attention_short_fwd", &attention_short_fwd);
+  m.def("attention_short_bwd", &attention_short_bwd);
   m.def("bn_bwd_cluster", &bn_bwd_cluster);
   m.def("gn_fwd", &gn_fwd);
   m.def("gn_bwd", &gn_bwd);
@@ -1631,6 +1730,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("relu_bwd", &relu_bwd);
   m.def("gelu", &gelu);
   m.def("gelu_bwd", &gelu_bwd);
+  m.def("gelu_erf", &gelu_erf);
+  m.def("gelu_erf_bwd", &gelu_erf_bwd);
+  m.def("vit_tokens_fwd", &vit_tokens_fwd);
+  m.def("vit_tokens_bwd", &vit_tokens_bwd);
   m.def("pad_rows", &pad_rows);
   m.def("embedding_bwd", &embedding_bwd);
   m.def("fedavg_allreduce", &fedavg_allreduce);
@@ -1665,6 +1768,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("bn_relu_maxpool", &bn_relu_maxpool);
   m.def("bn_maxpool_bwd", &bn_maxpool_bwd);
   m.def("layernorm_fwd", &layernorm_fwd);
+  m.def("layernorm_sum_fwd", &layernorm_sum_fwd);
+  m.def("layernorm_sum_bwd", &layernorm_sum_bwd);
   m.def("layernorm_drop_fwd", &layernorm_drop_fwd);
   m.def("layernorm_drop_bwd", &layernorm_drop_bwd);
   m.def("softmax_drop_fwd", &softmax_drop_fwd);

@@ -9,6 +9,7 @@
 #include "launch.h"
 #include "pdl.cuh"
 #include "ptx.cuh"
+#include "rows.cuh"
 #include "sgd.cuh"
 
 namespace b200 {
@@ -959,6 +960,39 @@ gelu_bwd_vec_kernel(const uint4* __restrict__ x, const uint4* __restrict__ dy, u
     dx[i] = make_uint4(o[0], o[1], o[2], o[3]);
   }
 }
+// exact GELU, x Phi(x) (torch.nn.GELU() / approximate="none"), and its derivative Phi(x) + x phi(x)
+__device__ __forceinline__ float gelu_erf_f(float v) { return 0.5f * v * (1.f + erff(v * 0.7071067811865476f)); }
+__device__ __forceinline__ float gelu_erf_grad_f(float v) {
+  return 0.5f * (1.f + erff(v * 0.7071067811865476f)) + v * 0.3989422804014327f * expf(-0.5f * v * v);
+}
+__global__ void __launch_bounds__(EW_THREADS)
+gelu_erf_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, long long nv) {
+  griddep_launch_dependents();
+  griddep_wait();
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < nv;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    float v[8];
+    unpack8(__ldcs(x + i), v);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = gelu_erf_f(v[j]);
+    y[i] = pack8(v);
+  }
+}
+__global__ void __launch_bounds__(EW_THREADS)
+gelu_erf_bwd_kernel(const uint4* __restrict__ x, const uint4* __restrict__ dy, uint4* __restrict__ dx, long long nv) {
+  griddep_launch_dependents();
+  griddep_wait();
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < nv;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    float v[8], g[8];
+    unpack8(__ldcs(x + i), v);
+    unpack8(__ldcs(dy + i), g);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) g[j] *= gelu_erf_grad_f(v[j]);
+    dx[i] = pack8(g);
+  }
+}
+
 // dst[r, 0:kp] = src[r, 0:k] zero padded (weights whose K is not a multiple of 8, e.g. 7x7x3 = 147)
 __global__ void __launch_bounds__(EW_THREADS)
 pad_rows_kernel(const __nv_bfloat16* __restrict__ s, __nv_bfloat16* __restrict__ d, long long rows, int k, int kp,
@@ -1294,6 +1328,21 @@ extern "C" int b200_gelu_bwd_bf16(const void* x, const void* dy, void* dx, long 
   launch_pdl(gelu_bwd_kernel, ew_grid(n), EW_THREADS, 0, stream, reinterpret_cast<const __nv_bfloat16*>(x),
                                                          reinterpret_cast<const __nv_bfloat16*>(dy),
                                                          reinterpret_cast<__nv_bfloat16*>(dx), n);
+  RET_LAST();
+}
+extern "C" int b200_gelu_erf_bf16(const void* x, void* y, long long n, cudaStream_t stream) {
+  if (n <= 0) return 0;
+  if (n % 8 || ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15)) return -2;
+  launch_pdl(gelu_erf_kernel, ew_grid(n / 8), EW_THREADS, 0, stream, reinterpret_cast<const uint4*>(x),
+             reinterpret_cast<uint4*>(y), n / 8);
+  RET_LAST();
+}
+extern "C" int b200_gelu_erf_bwd_bf16(const void* x, const void* dy, void* dx, long long n, cudaStream_t stream) {
+  if (n <= 0) return 0;
+  if (n % 8 || ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx)) & 15))
+    return -2;
+  launch_pdl(gelu_erf_bwd_kernel, ew_grid(n / 8), EW_THREADS, 0, stream, reinterpret_cast<const uint4*>(x),
+             reinterpret_cast<const uint4*>(dy), reinterpret_cast<uint4*>(dx), n / 8);
   RET_LAST();
 }
 extern "C" int b200_pad_rows_bf16(const void* src, void* dst, long long rows, int k, int kp, const uint32_t* flags,

@@ -97,6 +97,12 @@ int b200_attention_drop_fwd(const void* qkv, void* out, void* probs, int B, int 
                             const B200Dropout* drop, cudaStream_t stream);
 int b200_attention_drop_bwd(const void* qkv, const void* dout, const void* probs, void* dqkv, int B, int S, int H, int dh,
                             float scale, const B200Dropout* drop, cudaStream_t stream);
+// the same tiles at 0 < S < 128 (ViT: patches + class token), d_head = 64, no mask or dropout; probs is
+// [B*H, S, round_up(S, 8)] with the pad columns written as 0, and no row >= S of out / dqkv is written
+int b200_attention_short_fwd(const void* qkv, void* out, void* probs, int B, int S, int H, int dh, float scale,
+                             cudaStream_t stream);
+int b200_attention_short_bwd(const void* qkv, const void* dout, const void* probs, void* dqkv, int B, int S, int H, int dh,
+                             float scale, cudaStream_t stream);
 // ---- implicit-GEMM convolution (experimental: gemm_wgmma.cu CONV modes fed by TMA im2col maps)
 int b200_conv_igemm_fwd(const void* x, const void* w, void* y, int N, int H, int W, int Cin, int Cout, int KH, int KW,
                         int stride, int pad, int Ho, int Wo, int cluster_k, int force_bn, float* col_stats,
@@ -189,6 +195,12 @@ int b200_add_bf16(const void* a, const void* b, void* out, long long n, int relu
 int b200_relu_bwd_bf16(const void* y, const void* dy, void* dx, long long n, cudaStream_t stream);
 int b200_gelu_bf16(const void* x, void* y, long long n, cudaStream_t stream);
 int b200_gelu_bwd_bf16(const void* x, const void* dy, void* dx, long long n, cudaStream_t stream);
+int b200_gelu_erf_bf16(const void* x, void* y, long long n, cudaStream_t stream);
+int b200_gelu_erf_bwd_bf16(const void* x, const void* dy, void* dx, long long n, cudaStream_t stream);
+int b200_vit_tokens_fwd(const void* z, const float* cls, const float* bias, const float* pos, void* tok, int B, int S,
+                        int D, cudaStream_t stream);
+int b200_vit_tokens_bwd(const void* dtok, void* dz, float* dcls, float* dbias, float* dpos, int B, int S, int D,
+                        cudaStream_t stream);
 int b200_embedding_bwd(const void* dy, const long long* idx, float* grad, long long n_rows, int width,
                        cudaStream_t stream);
 // flags != nullptr: wait (bounded) until the arrival flags covering arena elements [elem_off, elem_off + rows * k) have
@@ -435,6 +447,12 @@ int b200_layernorm_fwd(const void* x, const void* residual, void* y, const float
                        float* mean, float* rstd, long long rows, int C, float eps, cudaStream_t stream);
 int b200_layernorm_bwd(const void* x, const void* dy, void* dx, const float* gamma, const float* mean,
                        const float* rstd, float* dgamma, float* dbeta, long long rows, int C, cudaStream_t stream);
+int b200_layernorm_sum_fwd(const void* x, const void* residual, void* y, void* sum, const float* gamma,
+                           const float* beta, float* mean, float* rstd, long long rows, int C, float eps,
+                           cudaStream_t stream);
+int b200_layernorm_sum_bwd(const void* s, const void* dy, const void* ds, void* dsum, const float* gamma,
+                           const float* mean, const float* rstd, float* dgamma, float* dbeta, long long rows, int C,
+                           cudaStream_t stream);
 int b200_softmax_fwd(const void* x, void* y, long long rows, int C, float scale, cudaStream_t stream);
 int b200_softmax_bwd(const void* y, const void* dy, void* dx, long long rows, int C, float scale,
                      cudaStream_t stream);

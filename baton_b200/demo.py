@@ -49,6 +49,9 @@ def build_model(kind: str, dropout: float = 0.0):
     if kind == "bert_base":
         from .models import bert_base
         return bert_base(hidden_dropout_prob=dropout, attention_probs_dropout_prob=dropout)
+    if kind in ("vit_tiny", "vit_small"):     # patch 4 on 32x32 images: 65 tokens
+        from .models import vit
+        return getattr(vit, kind)(num_classes=10)
     raise SystemExit("unknown model {!r}".format(kind))
 
 

@@ -518,6 +518,20 @@ def gelu_bwd(x: torch.Tensor, dy: torch.Tensor) -> torch.Tensor:
     return dx
 
 
+def gelu_erf(x: torch.Tensor) -> torch.Tensor:
+    """Exact GELU ``x Phi(x)`` of a bf16 tensor (``torch.nn.GELU()``)."""
+    y = torch.empty_like(x)
+    load().gelu_erf(x, y)
+    return y
+
+
+def gelu_erf_bwd(x: torch.Tensor, dy: torch.Tensor) -> torch.Tensor:
+    """``dy (Phi(x) + x phi(x))``, the gradient of :func:`gelu_erf` at ``x``."""
+    dx = torch.empty_like(x)
+    load().gelu_erf_bwd(x, dy, dx)
+    return dx
+
+
 def pad_rows(src2d: torch.Tensor, kp: int, out: Optional[torch.Tensor] = None, gate: Optional[dict] = None) -> torch.Tensor:
     """``gate`` (bcast_gemm): ``{"flags", "epoch_word", "elem_off", "tile_elems"}`` -- wait for the FedAvg collective's
     arrival flags over the source slice of the bf16 arena before reading it."""

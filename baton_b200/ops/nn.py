@@ -287,13 +287,13 @@ class _LinearFn(torch.autograd.Function):
             kw = dict(flags=flags_cfg["flags"], flag_epoch=flags_cfg.get("epoch", 0), flag_elem_off=flags_cfg["elem_off"],
                       flag_tile_elems=flags_cfg["tile_elems"], flag_bias_off=flags_cfg.get("bias_off", -1),
                       force_bn=128, flag_epoch_word=flags_cfg.get("epoch_word"))
-        y = F.gemm(x2, w_bf16, bias=bias, act=act if act != 2 else 0,
+        y = F.gemm(x2, w_bf16, bias=bias, act=act if act == 1 else 0,
                    out_dtype=torch.float32 if out_fp32 else BF16, **kw)
         ctx.act = act
         pre = None
-        if act == 2:  # GELU needs the pre-activation for backward
+        if act in (2, 3):  # GELU needs the pre-activation for backward
             pre = y
-            y = F.gelu(pre)
+            y = F.gelu(pre) if act == 2 else F.gelu_erf(pre)
         ctx.save_for_backward(x2, w_bf16, y if act == 1 else pre)
         ctx.weight, ctx.bias = weight, bias
         ctx.x_shape = x.shape
@@ -312,6 +312,8 @@ class _LinearFn(torch.autograd.Function):
             dy2 = F.relu_bwd(aux, dy2)
         elif ctx.act == 2:
             dy2 = F.gelu_bwd(aux, dy2)
+        elif ctx.act == 3:
+            dy2 = F.gelu_erf_bwd(aux, dy2)
         gw, gb = _linear_param_grads(dy2, x2, ctx.weight, ctx.bias)
         dx = None
         if ctx.needs_dx:
@@ -421,13 +423,14 @@ class _LoraLinearFn(torch.autograd.Function):
 
 
 class Linear(nn.Module):
-    """``y = act(x W^T + b)``; ``act`` in {None, 'relu', 'gelu'} is fused into the GEMM epilogue."""
+    """``y = act(x W^T + b)``; ``act`` in {None, 'relu', 'gelu', 'gelu_erf'}: ReLU is fused into the GEMM epilogue,
+    the tanh GELU ('gelu') and the exact one ('gelu_erf', ``torch.nn.GELU()``) run as an elementwise kernel after it."""
 
     def __init__(self, in_features: int, out_features: int, bias: bool = True, act: Optional[str] = None,
                  out_fp32: bool = False):
         super().__init__()
         self.in_features, self.out_features = in_features, out_features
-        self.act = {None: 0, "relu": 1, "gelu": 2}[act]
+        self.act = {None: 0, "relu": 1, "gelu": 2, "gelu_erf": 3}[act]
         self.out_fp32 = out_fp32
         self.weight = nn.Parameter(torch.empty(out_features, in_features))
         self.bias = nn.Parameter(torch.empty(out_features)) if bias else None
@@ -480,10 +483,14 @@ class Linear(nn.Module):
             y = TF.linear(x, self.weight.to(x.dtype), None if self.bias is None else self.bias.to(x.dtype))
             if lora is not None:
                 y = y + self._lora_term(x)
+            if self.act == 3:
+                return TF.gelu(y, approximate="none")
             return TF.relu(y) if self.act == 1 else (TF.gelu(y, approximate="tanh") if self.act == 2 else y)
         if x.dtype != BF16:
             x = F.cast(x.contiguous(), BF16)
         if lora is not None:
+            if self.act == 3:
+                raise ValueError("LoRA adapters on a Linear with act='gelu_erf' are not supported")
             y = _LoraLinearFn.apply(x, _wrap(self.weight, x), _wrap(self.bias, x), _shadow(self, "weight", self.weight),
                                     _wrap(self.lora_A, x), _wrap(self.lora_B, x), _shadow(self, "lora_A", self.lora_A),
                                     _shadow(self, "lora_B", self.lora_B), lora, self.act, self.out_fp32,
@@ -497,6 +504,18 @@ class Linear(nn.Module):
             self.flags_cfg = None  # launch-constant epoch: one-shot, only the first GEMM after a round is gated
         return _LinearFn.apply(x, _wrap(self.weight, x), _wrap(self.bias, x), _shadow(self, "weight", self.weight),
                                self.act, self.out_fp32, cfg, _anchor(x, self.weight, self.bias))
+
+
+def linear(x: torch.Tensor, owner: nn.Module, weight: str, bias: str) -> torch.Tensor:
+    """``x W^T + b`` with ``W = owner.<weight>`` and ``b = owner.<bias>``: the GEMM of :class:`Linear` for a module
+    that keeps its projection under other ``state_dict`` names (torchvision's packed ``in_proj_weight`` /
+    ``in_proj_bias``).  The arena's bf16 shadow is ``owner.<weight>_bf16``."""
+    w, b = getattr(owner, weight), getattr(owner, bias)
+    if not x.is_cuda:
+        return TF.linear(x, w.to(x.dtype), b.to(x.dtype))
+    if x.dtype != BF16:
+        x = F.cast(x.contiguous(), BF16)
+    return _LinearFn.apply(x, _wrap(w, x), _wrap(b, x), _shadow(owner, weight, w), 0, False, None, _anchor(x, w, b))
 
 
 # ================================================================================ Conv2d (NHWC, implicit GEMM)
@@ -841,6 +860,45 @@ class _LNFn(torch.autograd.Function):
         return dx, (dx if ctx.has_res else None), gg, gb, None, None
 
 
+class _AddLNFn(torch.autograd.Function):
+    """Pre-LN residual step: ``s = x + residual`` and ``y = LN(s)``, both returned.  Backward takes ``dy`` and the skip
+    gradient ``ds`` and writes ``dsum = LN_bwd(dy) + ds`` once, the gradient of both summands (no separate add)."""
+
+    @staticmethod
+    def forward(ctx, x, residual, gamma, beta, eps, anchor):
+        gamma, beta = _unwrap(gamma), _unwrap(beta)
+        c = x.shape[-1]
+        rows = x.numel() // c
+        y = torch.empty_like(x)
+        s = torch.empty_like(x)
+        mean = torch.empty(rows, dtype=torch.float32, device=x.device)
+        rstd = torch.empty(rows, dtype=torch.float32, device=x.device)
+        load().layernorm_sum_fwd(x, residual, y, s, gamma, beta, mean, rstd, rows, c, eps)
+        ctx.save_for_backward(s, mean, rstd)
+        ctx.set_materialize_grads(False)
+        ctx.gamma, ctx.beta, ctx.rows, ctx.c = gamma, beta, rows, c
+        return y, s
+
+    @staticmethod
+    def backward(ctx, dy, ds):
+        s, mean, rstd = ctx.saved_tensors
+        if dy is None:
+            return ds, ds, None, None, None, None
+        dy = dy.contiguous()
+        dsum = torch.empty_like(s)
+        tg, tb = _grad_target(ctx.gamma), _grad_target(ctx.beta)
+        gg = gb = None
+        if tg is None:
+            gg = tg = torch.zeros(ctx.c, dtype=torch.float32, device=dy.device)
+        if tb is None:
+            gb = tb = torch.zeros(ctx.c, dtype=torch.float32, device=dy.device)
+        if ds is None:       # the sum feeds nothing else (the last block's)
+            load().layernorm_bwd(s, dy, dsum, ctx.gamma, mean, rstd, tg, tb, ctx.rows, ctx.c)
+        else:
+            load().layernorm_sum_bwd(s, dy, ds.contiguous(), dsum, ctx.gamma, mean, rstd, tg, tb, ctx.rows, ctx.c)
+        return dsum, dsum, gg, gb, None, None
+
+
 class _LNDropFn(torch.autograd.Function):
     """LayerNorm with dropout (csrc/dropout.cu).  mode 1, input dropout: ``LN(drop(x) + residual)``, the kernel writes
     the pre-norm sum; backward writes its gradient (the residual's) and ``M s`` times it (x's) in one launch.  mode 2,
@@ -909,6 +967,15 @@ class LayerNorm(nn.Module):
             return TF.layer_norm(x, (self.c,), self.weight.to(x.dtype), self.bias.to(x.dtype), self.eps)
         return _LNFn.apply(x.contiguous(), None if residual is None else residual.contiguous(),
                            _wrap(self.weight, x), _wrap(self.bias, x), self.eps, _anchor(x, self.weight))
+
+    def add_norm(self, x, residual):
+        """``(LN(s), s)`` with ``s = x + residual``: the residual step of a pre-LN transformer block, which needs the sum
+        as the next skip input.  On CUDA ``s`` is rounded to bf16 once and normalised as stored."""
+        if not x.is_cuda:
+            s = x + residual
+            return TF.layer_norm(s, (self.c,), self.weight.to(s.dtype), self.bias.to(s.dtype), self.eps), s
+        return _AddLNFn.apply(x.contiguous(), residual.contiguous(), _wrap(self.weight, x), _wrap(self.bias, x),
+                              self.eps, _anchor(x, self.weight))
 
 
 class _SoftmaxFn(torch.autograd.Function):
@@ -1001,6 +1068,21 @@ class _AttnFn(torch.autograd.Function):
     def forward(ctx, qkv, B, S, H, dh, mask_bias=None, dargs=None):
         D = H * dh
         ctx.dargs = dargs
+        ctx.short = S % 8 != 0
+        if ctx.short:
+            # S < 128 and not a multiple of 8 (ViT: patches + class token): the fused kernels with the tensor dimension S,
+            # probs [B*H, S, round_up(S, 8)]
+            if not (S < 128 and dh == 64 and mask_bias is None and dargs is None):
+                raise ValueError("attention: S = {} is not a multiple of 8, which only the fused kernel for S < 128, "
+                                 "d_head = 64 without mask or dropout runs (got d_head = {}{}{})".format(
+                                     S, dh, ", a mask" if mask_bias is not None else "",
+                                     ", dropout" if dargs is not None else ""))
+            probs = torch.empty((B * H, S, (S + 7) // 8 * 8), dtype=BF16, device=qkv.device)
+            out = torch.empty((B * S, D), dtype=BF16, device=qkv.device)
+            load().attention_short_fwd(qkv, out, probs, B, S, H, dh, 1.0 / math.sqrt(dh))
+            ctx.save_for_backward(qkv, probs, None)
+            ctx.dims = (B, S, H, dh)
+            return out
         if S == 128 and dh == 64 and mask_bias is None:
             # single-kernel forward (csrc/attention.cu): scores stay in shared memory, P is written once
             probs = torch.empty((B * H * S, S), dtype=BF16, device=qkv.device)
@@ -1042,6 +1124,9 @@ class _AttnFn(torch.autograd.Function):
         dargs = ctx.dargs
         dout = dout.contiguous()
         dqkv = torch.empty_like(qkv)
+        if ctx.short:
+            load().attention_short_bwd(qkv, dout, probs, dqkv, B, S, H, dh, 1.0 / math.sqrt(dh))
+            return dqkv, None, None, None, None, None, None
         if S == 128 and dh == 64 and not getattr(ctx, "masked", False):
             # single-kernel backward (csrc/attention.cu): dP / dS never leave the SM
             ok = (load().attention_bwd(qkv, dout, probs, dqkv, B, S, H, dh, 1.0 / math.sqrt(dh)) if dargs is None else
@@ -1091,6 +1176,45 @@ def attention(qkv: torch.Tensor, B: int, S: int, H: int, dh: int, mask_bias: Opt
         return (p @ v).transpose(1, 2).reshape(B * S, D)
     dargs = drop[0].kernel_args(drop[1], drop[2]) if drop is not None else None
     return _AttnFn.apply(qkv.contiguous(), B, S, H, dh, mask_bias, dargs)
+
+
+class _TokensFn(torch.autograd.Function):
+    """ViT token assembly (csrc/elementwise.cu): forward one launch, backward one launch that writes the patch gradient
+    and accumulates the class-token, bias and position-embedding gradients in a fixed order."""
+
+    @staticmethod
+    def forward(ctx, z, cls, bias, pos, anchor):
+        cls, bias, pos = _unwrap(cls), _unwrap(bias), _unwrap(pos)
+        B, N, D = z.shape
+        tok = torch.empty((B, N + 1, D), dtype=BF16, device=z.device)
+        load().vit_tokens_fwd(z, cls.detach(), bias.detach(), pos.detach(), tok, B, N + 1, D)
+        ctx.params = (cls, bias, pos)
+        return tok
+
+    @staticmethod
+    def backward(ctx, dtok):
+        B, S, D = dtok.shape
+        tgts, grads = [], []
+        for p in ctx.params:
+            t = _grad_target(p)
+            g = None
+            if t is None:
+                g = t = torch.zeros_like(p, dtype=torch.float32)
+            tgts.append(t)
+            grads.append(g)
+        dz = torch.empty((B, S - 1, D), dtype=BF16, device=dtok.device)
+        load().vit_tokens_bwd(dtok.contiguous(), dz, *tgts, B, S, D)
+        return (dz, *grads, None)
+
+
+def vit_tokens(z: torch.Tensor, cls: torch.Tensor, bias: torch.Tensor, pos: torch.Tensor) -> torch.Tensor:
+    """``[cls; z + bias] + pos``: the token sequence ``[B, 1 + N, D]`` of a Vision Transformer from its patch embeddings
+    ``z [B, N, D]`` (without the projection bias), the class token ``[1, 1, D]``, the projection bias ``[D]`` and the
+    position embedding ``[1, 1 + N, D]``.  On CUDA each token is summed in fp32 and rounded to bf16 once."""
+    if not z.is_cuda:
+        B = z.shape[0]
+        return torch.cat([cls.to(z.dtype).expand(B, -1, -1), z + bias.to(z.dtype)], dim=1) + pos.to(z.dtype)
+    return _TokensFn.apply(z.contiguous(), _wrap(cls, z), _wrap(bias, z), _wrap(pos, z), _anchor(z, cls, bias, pos))
 
 
 class _DropFn(torch.autograd.Function):

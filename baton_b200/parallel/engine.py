@@ -200,7 +200,8 @@ class FederatedEngine:
         check_features(wire_dtype=wire_dtype, mode=mode, dp=self.dp, scaffold=scaffold, robust=self.robust,
                        topk=self.topk, server_opt=sopt, tile_flags=tile_flags, optimizer=optimizer, momentum=momentum,
                        prox_mu=prox_mu, local=keys is not None, secure_agg=secure_agg,
-                       frozen=any(not p.requires_grad for p in model.parameters()))
+                       frozen=any(not p.requires_grad for p in model.parameters()),
+                       vit=getattr(model, "is_vit", False))
         self.device = torch.device(device)
         self.model = model
         self.name = name

@@ -21,14 +21,14 @@ SEATED_SERVER_OPT = ("a server optimizer needs the http plane: on the seated pla
 def check_features(*, wire_dtype: str = "bf16", mode: str = "delta", dp=None, scaffold: bool = False, robust=None,
                    topk=None, server_opt=None, tile_flags: bool = False, plane: Optional[str] = None,
                    optimizer: str = "sgd", momentum: float = 0.0, nesterov: bool = False, prox_mu: float = 0.0,
-                   local: bool = False, secure_agg: bool = False, frozen: bool = False) -> None:
+                   local: bool = False, secure_agg: bool = False, frozen: bool = False, vit: bool = False) -> None:
     """``ValueError`` with the reason if the features cannot run together.  ``dp``, ``robust``, ``topk`` and
     ``server_opt`` are on unless they are None or False: the rules read only which features are on, so a caller may pass
     the features' configurations or bools.  Whoever takes a configuration from outside checks its type.  ``plane``:
     ``"http"`` or ``"seated"`` (the ``fused`` / ``nccl`` manager planes), None where no manager plane is involved.
     ``local``: client-local ``state_dict`` entries (FedBN / FedPer, ``parallel/personal.py``).  ``secure_agg``: secure
     aggregation (``parallel/secagg.py``).  ``frozen``: a model with frozen parameters (LoRA fine-tuning), whose
-    arena range the collective skips."""
+    arena range the collective skips.  ``vit``: a Vision Transformer (``models/vit.py``)."""
     if optimizer not in OPTIMIZERS:
         raise ValueError("optimizer must be one of {}, got {!r}".format(OPTIMIZERS, optimizer))
     adamw = optimizer == "adamw"
@@ -97,6 +97,8 @@ def check_features(*, wire_dtype: str = "bf16", mode: str = "delta", dp=None, sc
                            "range"),
         (frozen and plane is not None, "frozen parameters need the SPMD engine: a manager plane's payload is a whole "
                                        "state_dict"),
+        (vit and tile_flags, "a Vision Transformer with tile_flags is not supported: its token kernel reads class_token "
+                             "and pos_embedding, which the first GEMM's arrival flags do not cover"),
     )
     for broken, reason in rules:
         if broken:
